@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the k-diffusion sampling hot path on B200.
+"""bench.py -- images/sec of the k-diffusion sampling hot path on H100.
 
 One "step" = one complete sampler call over one batch of synthetic latents per GPU on the image_transformer_v2 denoiser.
 `--config` selects the BASELINE.json workload (default cfg2 = configs[1], the one the headline metric is quoted on):
@@ -11,6 +11,7 @@ One "step" = one complete sampler call over one batch of synthetic latents per G
 
     python bench.py [--config cfgN] [--gpus N] [--steps K] [--warmup W]   # N>1: launched by torch.distributed.run
     python bench.py --impl reference ...                                  # the reference algorithm's CPU port (oracle/)
+    python bench.py --dump-outputs DIR ...                                # also save the last timed step's samples as DIR/samples.npy
 
 Weak scaling: every rank samples its own batch.  Prints ONE JSON line on rank 0 (contract: task statement / DESIGN.md section 6).
 """
@@ -71,7 +72,11 @@ def parse():
     ap.add_argument("--no-extras", action="store_true", help="skip the roofline, parity and cpu_baseline legs")
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--parity-seconds", type=float, default=25.0, help="CPU budget of the parity leg (oracle run of one image)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
+    if args.steps is not None and args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.wl = CONFIGS[args.config]
     if args.batch is None:
         args.batch = args.wl["batch"]
@@ -93,7 +98,7 @@ def workload_config(args, n_gpus):
                         f"weights, Karras schedule rho=7 sigma [{SIGMA_MIN}, {SIGMA_MAX}], batch {batch} per GPU",
             "baseline_config": args.config, "sampler": wl["sampler"], "sampler_steps": wl["steps"], "nfe_per_image": nfe, "resolution": wl["res"],
             "per_gpu_batch": batch, "global_batch": batch * n_gpus, "parallelism": f"dp{n_gpus} (batch shards, no per-step collective)",
-            "l2": "256 MiB buffer rewritten between timed steps; per-step activation working set also exceeds the 126 MB L2"}
+            "l2": "256 MiB buffer rewritten between timed steps; per-step activation working set also exceeds the 50 MB L2"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -224,7 +229,7 @@ def run_reference(args, rank, world):
             "dtype": "fp32", "data": "synthetic", "impl": "reference", "config": workload_config(args, args.gpus),
             "cpu_baseline": {"value": v, "unit": UNIT, "cores": cores, "kind": "port",
                              "sample": "per step: " + sample + "; CPU torch fp32 port of the reference algorithm (oracle/kdiff_oracle.py); "
-                                       "the reference itself is Python and /root/reference does not travel to the GPU box"},
+                                       "the reference itself is Python and is not needed to run the benchmark"},
             "e2e": {"value": v, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
 
@@ -232,12 +237,31 @@ def run_reference(args, rank, world):
 # ------------------------------------------------------------------------------------------------
 # per-kernel device times of the graph-replayed step (CUPTI activity records through torch.profiler)
 # ------------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """{name: tensor} -> out_dir/<name>.npy in float32.  An array over its share of DUMP_LIMIT_BYTES keeps a fixed, seeded sample of
+    its leading index (images), in increasing order; the indices kept go to out_dir/<name>_index.npy (float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > share:
+            keep = max(1, share // (a[0].nbytes if a.ndim > 1 else 4))
+            idx = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+            a = a[idx]
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def kernel_family(name):
     """Kernel name (as CUPTI reports it) -> the family names of kdb_launch_breakdown."""
     name = name.replace("(int)", "").replace(" ", "")
-    if "gemm_tc_kernel<64,5>" in name:
+    if "gemm_wg_kernel<64,5>" in name:
         return "patch_out"
-    for key, fam in (("ffn_fused", "gemm_tc"), ("gemm_tc", "gemm_tc"), ("gemm_simt", "gemm_simt"), ("attn_", "attn_tc"), ("patch_in", "patch_in"), ("patch_out", "patch_out"),
+    for key, fam in (("ffn_fused", "gemm_tc"), ("gemm_wg", "gemm_tc"), ("gemm_simt", "gemm_simt"), ("attn_", "attn_tc"), ("patch_in", "patch_in"), ("patch_out", "patch_out"),
                      ("fold_norm", "fused_norm"), ("ew_kernel", "solver"), ("precond", "precond"), ("noise_", "noise"),
                      ("conditioning", "cond"), ("rmsnorm", "rmsnorm"), ("qknorm", "qknorm_rope"), ("geglu_kernel", "geglu")):
         if key in name:
@@ -267,9 +291,9 @@ def graph_kernel_times(fn):
             out.append((kernel_family(name), name, float(e.time_range.start), float(e.time_range.elapsed_us()) / 1000.0))
         out.sort(key=lambda r: r[2])
         # Under programmatic dependent launch a kernel is resident (prologue, then parked in griddepcontrol.wait) while its
-        # predecessor still runs, and CUPTI's duration includes that wait: the raw durations of one evaluation summed to 2.11 ms
-        # against a 1.69 ms span (profiles/r2_bench_cfg2_first.json).  Attribute to each kernel only the time after the previous
-        # kernel ENDED (one stream, in-order completion): the exclusive durations sum to the span exactly.
+        # predecessor still runs, and CUPTI's duration includes that wait, so raw durations over-count the span.  Attribute to each
+        # kernel only the time after the previous kernel ENDED (one stream, in-order completion): the exclusive durations sum to the
+        # span exactly.
         excl, prev_end = [], None
         for fam, name, start, dur in out:
             end = start + dur * 1000.0
@@ -362,18 +386,22 @@ def main():
         n0 = S.total_kernel_launches()
         t0 = time.time()
         e0.record()
+        last = None
         for i in range(k):
-            fn(i)
+            last = fn(i)
         e1.record()
         barrier()
         t1 = time.time()
-        return max_over_ranks(e0.elapsed_time(e1)), S.total_kernel_launches() - n0, t0, t1
+        return max_over_ranks(e0.elapsed_time(e1)), S.total_kernel_launches() - n0, t0, t1, last
 
     clocks = ClockSampler(local) if rank == 0 else None
     time.sleep(0.3)
-    ms, launches, t0, t1 = timed(step_device, args.steps, args.warmup)
+    ms, launches, t0, t1, last = timed(step_device, args.steps, args.warmup)
     clk = clocks.stop(t0, t1) if clocks else None
-    ms_e2e, _, _, _ = timed(step_e2e, args.steps, 1)
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, {"samples": last})      # the denoised images of the last timed step (this rank's batch)
+    del last
+    ms_e2e, _, _, _, _ = timed(step_e2e, args.steps, 1)
     out = step_device(0)
     finite = bool(torch.isfinite(out).all())
     value = world * B * args.steps / (ms / 1000.0)
@@ -413,7 +441,7 @@ def main():
         total = sum(t for _, t in prof.by_family.values())
         breakdown = {f: {"launches": c, "ms": round(t, 3), "share": round(t / total, 4)} for f, (c, t) in
                      sorted(prof.by_family.items(), key=lambda kv: -kv[1][1])}
-        # dominant kernel = the tcgen05 GEMM behind every nn.Linear on the token stream (94 % of the model's MACs).
+        # dominant kernel = the wgmma GEMM behind every nn.Linear on the token stream (94 % of the model's MACs).
         # Launches are matched to shapes by execution order (k_diffusion.models.flops.linear_layers).
         gemm_fams = [f for f in prof.by_family if f.startswith("gemm")]
         g_times = [t for f, t in prof.launches if f.startswith("gemm")]
@@ -434,7 +462,7 @@ def main():
         if peaks_file.exists():
             peak, which = json.loads(peaks_file.read_text())["bf16_tflops_sustained"], "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
         else:
-            peak, which = 1400.0, "fallback (B200_PROFILING.md sustained 1.4 PFLOP/s)"
+            peak, which = 989.0, "fallback (H100 SXM data sheet, dense BF16 at 700 W: 989 TFLOP/s)"
         ach = flops / (g_ms / 1000.0) / 1e12
         shapes = []
         for (kind, M_, N_, K_, macs_), (c, tot) in sorted(per_shape.items(), key=lambda kv: -kv[1][1])[:8]:
@@ -450,21 +478,8 @@ def main():
             a_fl = 2.0 * K.models.flops.attention_macs(cfg["model"], B) * prof_evals
             attn = {"launches": len(a_times), "ms_per_eval": round(sum(a_times) / prof_evals, 4),
                     "achieved_tflops": round(a_fl / (sum(a_times) / 1000.0) / 1e12, 1), "share_of_step": round(sum(a_times) / total, 4)}
-        ncu_file = ROOT / "profiles" / "r2_ncu_full_summary.json"
-        traffic, traffic_note = None, "no ncu capture committed for this build"
-        if ncu_file.exists():
-            try:
-                first = json.loads(ncu_file.read_text())["roofline_kernel"]
-                unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-                traffic = 0.0
-                for key, val in first.items():          # ncu picks the unit per value: "dram__bytes_read.sum [Mbyte]", "... [Kbyte]"
-                    if key.startswith("dram__bytes_read.sum [") or key.startswith("dram__bytes_write.sum ["):
-                        traffic += float(val) * unit[key[key.index("[") + 1:-1]]
-                traffic_note = ("dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the heaviest shape (" + first["launch"] +
-                                "), from the committed ncu --set full capture profiles/r2_ncu_full_summary.json")
-            except (KeyError, ValueError, StopIteration):
-                pass
-        roofline = {"bound": "tensor", "kernel": "gemm_tc_persist / gemm_tc_kernel (tcgen05 GEMM, all token-stream Linear layers: " +
+        traffic, traffic_note = None, "not measured (no DRAM counter capture in this run)"
+        roofline = {"bound": "tensor", "kernel": "gemm_wg_kernel / ffn_fused_kernel (wgmma GEMM, all token-stream Linear layers: " +
                                                  "+".join(sorted(gemm_fams)) + ")",
                     "achieved": round(ach, 2), "peak": peak, "unit": "TFLOP/s", "frac": round(ach / peak, 4), "peak_source": which,
                     "avg_launch_us": round(1000.0 * g_ms / max(g_launch, 1), 2), "launches": g_launch,

@@ -1,4 +1,4 @@
-/* kdiffusion_b200.h -- C ABI of libkdb200.so, the B200 (sm_100a) native library behind the
+/* kdiffusion_b200.h -- C ABI of libkdb200.so, the H100 (sm_90a) native library behind the
  * k_diffusion sampling hot path.
  *
  * The reference (crowsonkb/k-diffusion) is pure Python and has no FFI layer of its own
@@ -205,7 +205,7 @@ int64_t kdb_model_tap_count(const KdbModel* m);
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)
  * ------------------------------------------------------------------------------------------ */
 
-/* C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulate in TMEM (tcgen05.mma), bf16 out. */
+/* C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulate (wgmma), bf16 out. */
 int kdb_gemm_bf16(const void* a_bf16, const void* w_bf16, void* c_bf16, int M, int N, int K, void* stream);
 
 /* out[M,N2/2] = value * gelu(gate) of A[M,K] * W_il[N2,K]^T: up_proj with the GEGLU fused in the epilogue

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libkdb200 (sm_100a only).
+// common.cuh -- shared helpers for libkdb200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -69,12 +69,12 @@ __device__ __forceinline__ void karras_scalings(float sigma, float sd, float& c_
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;   // H100 SXM; the launchers query the device where it matters
 
 }  // namespace kdb
 
 // Programmatic dependent launch: let the CTAs of the next kernel in the stream (if it was launched with the programmatic
-// attribute -- the persistent GEMM is) be scheduled as soon as every CTA of this grid has passed this point or exited.
+// attribute -- attention and the fused feed-forward kernel are) be scheduled as soon as every CTA of this grid has passed this point or exited.
 // The caller must itself be past any dependency on ITS predecessor, i.e. ordinary (fully serialised) launches call it first thing.
 #define KDB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 

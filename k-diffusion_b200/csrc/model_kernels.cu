@@ -2,7 +2,7 @@
 // forward pass (reference: k_diffusion/models/image_transformer_v2.py).  With T = float this is the
 // fp32-exact path behind the rtol 1e-3 / atol 1e-5 parity gate: all reductions accumulate in fp32,
 // transcendental functions are the accurate (non fast-math) variants.  With T = bf16 the same
-// kernels serve as the fallback for shapes the tcgen05 kernels do not cover.
+// kernels serve as the fallback for shapes the tensor-core (wgmma) kernels do not cover.
 #include <cmath>
 
 #include "model_kernels.cuh"

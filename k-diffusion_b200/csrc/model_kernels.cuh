@@ -20,7 +20,7 @@ struct GemmEpi {
   // TokenMerge folded into the A-operand load (tensor-core path only): A = fine tokens [B, 2*mhc, 2*mwc, mC], K = 4*mC in
   // (nh nw e) order, M = B*mhc*mwc.  mC == 0 -> A is a plain [M, K] matrix.
   int mhc = 0, mwc = 0, mC = 0;
-  // fused RMSNorm (tensor-core persistent kernel only).  Consumer (EPI_STORE / EPI_QKV_ROPE): A is the raw residual stream, W
+  // fused RMSNorm (tensor-core kernel only).  Consumer (EPI_STORE / EPI_QKV_ROPE): A is the raw residual stream, W
   // already carries the channel scale, ss_in [M, 8] holds sum(x^2) per 128-channel block of every row and the epilogue scales
   // the accumulator by 1/rms (q/k thirds of EPI_QKV_ROPE are scale invariant).  Producer (EPI_RESID / EPI_SPLIT_LERP): ss_out
   // receives those sums for the rows written.

@@ -1,4 +1,4 @@
-// tc_attention.cu -- bf16 attention on tcgen05 for the two attention types of the bench configuration:
+// tc_attention.cu -- bf16 attention on the sm_90a tensor core (wgmma) for the attention types of the model configurations:
 //   * shifted-window attention, 8x8 windows, d_head 64 (reference image_transformer_v2.py:253-337,446-476)
 //   * global attention, sequence a multiple of 128, d_head 64 (:355-396)
 // q and k arrive already cosine-normalised and rotated (qknorm_rope kernel); softmax scale is 1.0.
@@ -14,9 +14,10 @@
 //            borders, always 49 keys).  Rows = an 8x16 query block of one head; its keys all lie in the clamped 14x22 halo,
 //            streamed as three TMA boxes of 5 halo rows (110 keys per 128-row tile, the tail rows are masked / zero);
 //            the per-query 7x7 window is a mask on S.  Same two-pass softmax as GLOBAL.
-// Pipeline per key block: TMA (SWIZZLE_128B) -> S = Q K^T (tcgen05.mma, fp32 in TMEM) -> tcgen05.ld, softmax in
-// registers (one thread per row) -> P (bf16) written to shared memory in the UMMA K-major SW128 layout ->
-// O += P V (V consumed as an MN-major operand straight from the TMA tile) -> tcgen05.ld, 1/l scaling, store.
+// Roles: warp 4 = TMA producer, warps 0-3 = the warpgroup that issues the MMAs and runs the softmax.  Per key block: TMA
+// (SWIZZLE_128B) -> S = Q K^T (wgmma, two M = 64 halves) -> fp32 S tile in shared memory -> softmax (one thread per row) ->
+// P (bf16) written to shared memory in the K-major SW128 layout -> O += P V (V consumed as an MN-major operand straight from
+// the TMA tile, O in registers across key blocks) -> fp32 O tile, 1/l scaling, store.
 #include "tc_common.cuh"
 #include "tc_kernels.cuh"
 
@@ -26,6 +27,7 @@ namespace {
 constexpr int ROWS = 128, DH = 64;
 constexpr int TILE_BYTES = ROWS * DH * 2;    // 16 KiB: 128 rows x 128 B
 constexpr float LOG2E = 1.4426950408889634f;
+constexpr int S_LD = ROWS + 4;               // row pitch (floats) of the fp32 S / O tile
 
 enum { MODE_WINDOW = 0, MODE_GLOBAL = 1, MODE_NA = 2 };
 
@@ -44,8 +46,7 @@ struct AttnParams {
 };
 
 struct Bars {
-  uint64_t q, kv, s, sc, p, o;
-  uint32_t tmem;
+  uint64_t q, kv, kv_free;
 };
 
 __device__ __forceinline__ uint32_t p_offset(int row, int chunk16) {   // byte offset of 16-byte chunk `chunk16` (0..7) of `row` in a K-major SW128 tile
@@ -53,17 +54,18 @@ __device__ __forceinline__ uint32_t p_offset(int row, int chunk16) {   // byte o
 }
 
 template <int MODE, bool BOUNDED>
-__global__ void __launch_bounds__(160, MODE == MODE_WINDOW ? 4 : 2) attn_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
-                                                                                      const AttnParams p) {
+__global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
+                                                         const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = base;
   uint8_t* sK = base + TILE_BYTES;
   uint8_t* sV = base + 2 * TILE_BYTES;
   // P (two K-blocks of 64 keys, 32 KiB).  WINDOW has a single key block: Q and K are dead once S = Q K^T has completed, so
-  // P overwrites them (48 KiB per CTA -> 3-4 CTAs per SM); GLOBAL re-uses Q for every key block and keeps P separate.
+  // P overwrites them; GLOBAL re-uses Q for every key block and keeps P separate.
   uint8_t* sP = (MODE == MODE_WINDOW) ? sQ : base + 3 * TILE_BYTES;
-  Bars* bars = reinterpret_cast<Bars*>(base + (MODE == MODE_WINDOW ? 3 : 5) * TILE_BYTES);
+  float* sS = reinterpret_cast<float*>(base + (MODE == MODE_WINDOW ? 3 : 5) * TILE_BYTES);   // fp32 S (then O) tile, row pitch S_LD
+  Bars* bars = reinterpret_cast<Bars*>(sS + ROWS * S_LD);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nh = p.nh;
@@ -89,15 +91,13 @@ __global__ void __launch_bounds__(160, MODE == MODE_WINDOW ? 4 : 2) attn_tc_kern
   const int nblk = (MODE == MODE_WINDOW) ? 1 : p.nblk;
   constexpr bool bounded = BOUNDED;
   const bool two_pass = nblk > 1 && !bounded;
+  const int n_iter = two_pass ? 2 * nblk : nblk;
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmap);
     tc::mbar_init(&bars->q, 1);
     tc::mbar_init(&bars->kv, 1);
-    tc::mbar_init(&bars->s, 1);
-    tc::mbar_init(&bars->sc, 128);
-    tc::mbar_init(&bars->p, 128);
-    tc::mbar_init(&bars->o, 1);
+    tc::mbar_init(&bars->kv_free, 4);          // lane 0 of each warp of the warpgroup
     tc::fence_barrier_init();
   }
   if constexpr (MODE == MODE_NA) {   // rows 110..127 of the V tile are never written by TMA: they must be finite (P there is exactly 0)
@@ -105,20 +105,13 @@ __global__ void __launch_bounds__(160, MODE == MODE_WINDOW ? 4 : 2) attn_tc_kern
       *reinterpret_cast<uint4*>(sV + NA_BLK_KEYS * 128 + i * 16) = make_uint4(0u, 0u, 0u, 0u);
     tc::fence_proxy_async();
   }
-  constexpr uint32_t TMEM_COLS = (MODE == MODE_WINDOW) ? 128 : 256;
-  if (warp == 4) tc::tmem_alloc(&bars->tmem, TMEM_COLS);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
   tc::pdl_wait();                              // programmatic launch: the qkv projection before us must be complete from here on
   tc::pdl_launch_dependents();
-  const uint32_t tmem_s = bars->tmem;          // columns [0,128): S
-  // O: 64 columns.  WINDOW: P V is only issued after every thread has read S (bar_p), so O re-uses S's first columns.
-  const uint32_t tmem_o = bars->tmem + (MODE == MODE_WINDOW ? 0 : 128);
 
   if (warp == 4) {
     if (tc::elect_one()) {
-      // ------------------------------------------------ loads of Q (and window K,V)
+      // ------------------------------------------------ loads of Q and of each key block (K, and V in the P V pass)
       auto load_window_tile = [&](uint8_t* dst, int t, uint64_t* bar) {
         if (p.shift == 0) {   // unshifted window: one 8x8 box per head, rows in (lr, lc) order (tensor map box = 64 x 8 x 8)
 #pragma unroll
@@ -141,233 +134,222 @@ __global__ void __launch_bounds__(160, MODE == MODE_WINDOW ? 4 : 2) attn_tc_kern
         tc::tma_load_4d(sQ, &tmap, &bars->q, head0 * DH, qj0, qi0, b);
       else
         tc::tma_load_3d(sQ, &tmap, &bars->q, head0 * DH, mtile * ROWS, b);
-
-      const uint64_t qdesc = tc::smem_desc_k_sw128(tc::smem_u32(sQ));
-      const uint64_t kdesc = tc::smem_desc_k_sw128(tc::smem_u32(sK));
-      const uint64_t pdesc = tc::smem_desc_k_sw128(tc::smem_u32(sP));
-      const uint64_t vdesc = tc::smem_desc_mn_sw128(tc::smem_u32(sV), 1024, 1024);
-      constexpr uint32_t IDESC_S = tc::idesc_bf16(ROWS, 128);
-      constexpr uint32_t IDESC_O = tc::idesc_bf16(ROWS, DH, 0, 1);
-
-      uint32_t it = 0, ph_sc = 0, ph_p = 0, ph_o = 0;
-      bool prev_pass_a = false;
-      for (int pass = two_pass ? 0 : 1; pass < 2; ++pass) {
-        for (int j = 0; j < nblk; ++j, ++it) {
-          const bool with_v = pass == 1;
-          constexpr uint32_t KV_BYTES = (MODE == MODE_NA) ? NA_BLK_KEYS * 128 : TILE_BYTES;
-          tc::mbar_arrive_expect_tx(&bars->kv, with_v ? 2 * KV_BYTES : KV_BYTES);
-          if constexpr (MODE == MODE_WINDOW) {
-            load_window_tile(sK, 1, &bars->kv);
-            load_window_tile(sV, 2, &bars->kv);
-          } else if constexpr (MODE == MODE_NA) {
-            tc::tma_load_4d(sK, &tmap_kv, &bars->kv, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
-            if (with_v) tc::tma_load_4d(sV, &tmap_kv, &bars->kv, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
-          } else {
-            tc::tma_load_3d(sK, &tmap, &bars->kv, (nh + head0) * DH, j * ROWS, b);
-            if (with_v) tc::tma_load_3d(sV, &tmap, &bars->kv, (2 * nh + head0) * DH, j * ROWS, b);
-          }
-          if (it == 0) tc::mbar_wait(&bars->q, 0);
-          tc::mbar_wait(&bars->kv, it & 1u);
-          if (it > 0 && prev_pass_a) {           // S of the previous block fully read by the softmax threads?
-            tc::mbar_wait(&bars->sc, ph_sc);
-            ph_sc ^= 1u;
-          }
-          tc::tc_fence_after();
-#pragma unroll
-          for (int k = 0; k < DH / 16; ++k) tc::umma_bf16(tmem_s, qdesc + 2ull * k, kdesc + 2ull * k, IDESC_S, (uint32_t)(k != 0));
-          tc::umma_commit(&bars->s);
-          if (pass == 1) {
-            tc::mbar_wait(&bars->p, ph_p);       // P written (and S consumed)
-            ph_p ^= 1u;
-            tc::tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < ROWS / 16; ++k) {
-              const uint64_t ad = pdesc + (uint64_t)((k >> 2) * (TILE_BYTES >> 4)) + 2ull * (k & 3);
-              const uint64_t bd = vdesc + (uint64_t)(k * ((16 * 128) >> 4));
-              tc::umma_bf16(tmem_o, ad, bd, IDESC_O, (uint32_t)((j | k) != 0));
-            }
-            tc::umma_commit(&bars->o);
-            tc::mbar_wait(&bars->o, ph_o);       // K, V, P buffers free again
-            ph_o ^= 1u;
-            prev_pass_a = false;
-          } else {
-            tc::mbar_wait(&bars->s, it & 1u);    // K buffer free again
-            prev_pass_a = true;
-          }
-        }
-      }
-    }
-  } else {
-    // ---------------------------------------------------- softmax / epilogue: thread = row
-    const int row = warp * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    float m = -INFINITY, l = 0.f;
-    uint32_t it = 0;
-    // window geometry of this row
-    const int hd = row >> 6, quad = (row & 63) >> 4;
-    const bool seam_r = MODE == MODE_WINDOW && p.shift > 0 && wi == 0;
-    const bool seam_c = MODE == MODE_WINDOW && p.shift > 0 && wj == 0;
-    // NA: this row's query and the origin of its clamped 7x7 window
-    const int na_qi = qi0 + (row >> 4), na_qj = qj0 + (row & 15);
-    const int na_rs = min(max(na_qi - 3, 0), p.h - 7), na_cs = min(max(na_qj - 3, 0), p.w - 7);
-    auto key_ok = [&](int j, int t) -> bool {      // is tile column t of key block j inside this row's neighbourhood?
-      if constexpr (MODE != MODE_NA) return true;
-      const int dr = (t * 745) >> 14;               // t / 22 for t < 128
-      const int kr = r0 + j * NA_BLK_ROWS + dr, kc = c0 + (t - dr * NA_KW);
-      return t < NA_BLK_KEYS && (unsigned)(kr - na_rs) < 7u && (unsigned)(kc - na_cs) < 7u;
-    };
-    for (int pass = two_pass ? 0 : 1; pass < 2; ++pass) {
-      for (int j = 0; j < nblk; ++j, ++it) {
-        tc::mbar_wait(&bars->s, it & 1u);
-        tc::tc_fence_after();
-        if (pass == 0) {
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            float v[32];
-            tc::tmem_ld32(tmem_s + lane_base + c * 32, v);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) m = fmaxf(m, key_ok(j, c * 32 + i) ? v[i] : -INFINITY);
-          }
-          tc::tc_fence_before();
-          tc::mbar_arrive(&bars->sc);
-        } else if constexpr (MODE != MODE_WINDOW) {
-          if constexpr (bounded) m = __ldg(p.bound + head0);
-          const float mb = m * LOG2E;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            float v[32];
-            tc::tmem_ld32(tmem_s + lane_base + c * 32, v);
-            if (!two_pass && !bounded && c == 0) {   // single block: the row maximum comes from this very tile (two more reads are cheap)
-              float mm = -INFINITY;
-#pragma unroll 1
-              for (int c2 = 0; c2 < 4; ++c2) {
-                float u[32];
-                tc::tmem_ld32(tmem_s + lane_base + c2 * 32, u);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) mm = fmaxf(mm, u[i]);
-              }
-              m = mm;
-            }
-            const float mbb = (two_pass || bounded) ? mb : m * LOG2E;
-            uint32_t pk[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float p0 = key_ok(j, c * 32 + 2 * i) ? exp2f(fmaf(v[2 * i], LOG2E, -mbb)) : 0.f;
-              const float p1 = key_ok(j, c * 32 + 2 * i + 1) ? exp2f(fmaf(v[2 * i + 1], LOG2E, -mbb)) : 0.f;
-              pk[i] = tc::pack_bf16x2(p0, p1);
-              float q0, q1;
-              tc::unpack_bf16x2(pk[i], q0, q1);     // l accumulates exactly what the P V MMA sees
-              l += q0 + q1;
-            }
-            uint8_t* pt = sP + (c >> 1) * TILE_BYTES;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj)
-              *reinterpret_cast<uint4*>(pt + p_offset(row, (c & 1) * 4 + jj)) = make_uint4(pk[jj * 4], pk[jj * 4 + 1], pk[jj * 4 + 2], pk[jj * 4 + 3]);
-          }
-          tc::fence_proxy_async();
-          tc::tc_fence_before();
-          tc::mbar_arrive(&bars->p);
+      for (int it = 0; it < n_iter; ++it) {
+        const int j = it % nblk;
+        const bool with_v = !two_pass || it >= nblk;
+        if (it > 0) tc::mbar_wait(&bars->kv_free, (uint32_t)(it - 1) & 1u);
+        constexpr uint32_t KV_BYTES = (MODE == MODE_NA) ? NA_BLK_KEYS * 128 : TILE_BYTES;
+        tc::mbar_arrive_expect_tx(&bars->kv, with_v ? 2 * KV_BYTES : KV_BYTES);
+        if constexpr (MODE == MODE_WINDOW) {
+          load_window_tile(sK, 1, &bars->kv);
+          load_window_tile(sV, 2, &bars->kv);
+        } else if constexpr (MODE == MODE_NA) {
+          tc::tma_load_4d(sK, &tmap_kv, &bars->kv, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
+          if (with_v) tc::tma_load_4d(sV, &tmap_kv, &bars->kv, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
         } else {
-          // WINDOW: own head's 64 key columns live at [64*hd, 64*hd+64); the other head's block is garbage -> zeros in P
-          float v[64];
-          {
-            float t0[32], t1[32];
-            tc::tmem_ld32(tmem_s + lane_base + hd * 64, t0);
-            tc::tmem_ld32(tmem_s + lane_base + hd * 64 + 32, t1);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
-          }
-          if constexpr (!bounded) {
-#pragma unroll
-            for (int i = 0; i < 64; ++i) {
-              const int kq = i >> 4;
-              const bool ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-              v[i] = ok ? v[i] : -INFINITY;
-              m = fmaxf(m, v[i]);
-            }
-          } else {
-            m = __ldg(p.bound + head0 + hd);          // fixed shift: no maximum scan; masked keys get p = 0 below
-          }
-          const float mb = m * LOG2E;
-          uint8_t* own = sP + hd * TILE_BYTES;
-          uint8_t* other = sP + (1 - hd) * TILE_BYTES;
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            uint32_t pk[4];
-            bool ok = true;                        // (bounded) seam mask of this 8-key group: zero probability instead of -inf logit
-            if constexpr (bounded) {
-              const int kq = jj >> 1;
-              ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-            }
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              float p0 = exp2f(fmaf(v[jj * 8 + 2 * t], LOG2E, -mb)), p1 = exp2f(fmaf(v[jj * 8 + 2 * t + 1], LOG2E, -mb));
-              if constexpr (bounded) {
-                p0 = ok ? p0 : 0.f;
-                p1 = ok ? p1 : 0.f;
-              }
-              pk[t] = tc::pack_bf16x2(p0, p1);
-              float q0, q1;
-              tc::unpack_bf16x2(pk[t], q0, q1);
-              l += q0 + q1;
-            }
-            *reinterpret_cast<uint4*>(own + p_offset(row, jj)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            *reinterpret_cast<uint4*>(other + p_offset(row, jj)) = make_uint4(0u, 0u, 0u, 0u);
-          }
-          tc::fence_proxy_async();
-          tc::tc_fence_before();
-          tc::mbar_arrive(&bars->p);
+          tc::tma_load_3d(sK, &tmap, &bars->kv, (nh + head0) * DH, j * ROWS, b);
+          if (with_v) tc::tma_load_3d(sV, &tmap, &bars->kv, (2 * nh + head0) * DH, j * ROWS, b);
         }
       }
     }
-    // ------------------------------------------------------ O / l -> out
-    tc::mbar_wait(&bars->o, (uint32_t)((nblk - 1) & 1));
-    tc::tc_fence_after();
-    const float inv = 1.f / l;
-    int64_t token;
-    int head;
-    if constexpr (MODE == MODE_WINDOW) {
-      int oi, oj;
-      if (p.shift == 0) {
-        oi = wi * 8 + ((row & 63) >> 3);
-        oj = wj * 8 + (row & 7);
-      } else {
-        const int lr = (row & 15) >> 2, lc = row & 3;
-        oi = (wi * 8 + (quad >> 1) * 4 + lr - p.shift + p.h) % p.h;
-        oj = (wj * 8 + (quad & 1) * 4 + lc - p.shift + p.w) % p.w;
-      }
-      token = (int64_t)oi * p.w + oj;
-      head = head0 + hd;
-    } else if constexpr (MODE == MODE_NA) {
-      token = (int64_t)na_qi * p.w + na_qj;
-      head = head0;
-    } else {
-      token = (int64_t)mtile * ROWS + row;
-      head = head0;
-    }
-    uint4* dst = reinterpret_cast<uint4*>(p.out + (((int64_t)b * p.h * p.w + token) * nh + head) * DH);
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      float v[32];
-      tc::tmem_ld32(tmem_o + lane_base + c * 32, v);
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj)
-        dst[c * 4 + jj] = make_uint4(tc::pack_bf16x2(v[jj * 8 + 0] * inv, v[jj * 8 + 1] * inv), tc::pack_bf16x2(v[jj * 8 + 2] * inv, v[jj * 8 + 3] * inv),
-                                     tc::pack_bf16x2(v[jj * 8 + 4] * inv, v[jj * 8 + 5] * inv), tc::pack_bf16x2(v[jj * 8 + 6] * inv, v[jj * 8 + 7] * inv));
-    }
+    return;
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(bars->tmem, TMEM_COLS);
+
+  // ---------------------------------------------------- warpgroup: S = Q K^T (wgmma) -> softmax, thread = row -> O += P V (wgmma)
+  const int row = warp * 32 + lane;
+  float m = -INFINITY, l = 0.f;
+  // window geometry of this row
+  const int hd = row >> 6, quad = (row & 63) >> 4;
+  const bool seam_r = MODE == MODE_WINDOW && p.shift > 0 && wi == 0;
+  const bool seam_c = MODE == MODE_WINDOW && p.shift > 0 && wj == 0;
+  // NA: this row's query and the origin of its clamped 7x7 window
+  const int na_qi = qi0 + (row >> 4), na_qj = qj0 + (row & 15);
+  const int na_rs = min(max(na_qi - 3, 0), p.h - 7), na_cs = min(max(na_qj - 3, 0), p.w - 7);
+  auto key_ok = [&](int j, int t) -> bool {      // is tile column t of key block j inside this row's neighbourhood?
+    if constexpr (MODE != MODE_NA) return true;
+    const int dr = (t * 745) >> 14;               // t / 22 for t < 128
+    const int kr = r0 + j * NA_BLK_ROWS + dr, kc = c0 + (t - dr * NA_KW);
+    return t < NA_BLK_KEYS && (unsigned)(kr - na_rs) < 7u && (unsigned)(kc - na_cs) < 7u;
+  };
+  const uint32_t q_addr = tc::smem_u32(sQ), k_addr = tc::smem_u32(sK), p_addr = tc::smem_u32(sP);
+  const uint64_t vdesc = tc::smem_desc_mn_sw128(tc::smem_u32(sV), 1024, 1024);
+  float o0[32], o1[32];                        // O rows 0-63 / 64-127, accumulated over the key blocks of the P V pass
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o0[i] = o1[i] = 0.f;
+  tc::mbar_wait(&bars->q, 0);
+  for (int it = 0; it < n_iter; ++it) {
+    const int j = it % nblk;
+    const int pass = (two_pass && it < nblk) ? 0 : 1;
+    tc::mbar_wait(&bars->kv, (uint32_t)it & 1u);
+    // S = Q K^T, one M = 64 half at a time -> fp32 tile
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      float s[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) s[i] = 0.f;
+      const uint64_t qd = tc::smem_desc_k_sw128(q_addr + (uint32_t)h * 8192u), kd = tc::smem_desc_k_sw128(k_addr);
+      tc::wg_fence_acc(s);
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < DH / 16; ++k) tc::wgmma_128(s, qd + 2ull * k, kd + 2ull * k, 1u);
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(s);
+      tc::acc_store(sS, S_LD, 64 * h, s);
+    }
+    tc::named_barrier_sync(1, 128);            // S complete; every read of Q and K is done (WINDOW: P may overwrite them)
+    if (pass == 0) {
+#pragma unroll 1
+      for (int c = 0; c < 4; ++c) {
+        float v[32];
+        tc::acc_ld32(sS, S_LD, row, c * 32, v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) m = fmaxf(m, key_ok(j, c * 32 + i) ? v[i] : -INFINITY);
+      }
+    } else if constexpr (MODE != MODE_WINDOW) {
+      if constexpr (bounded) m = __ldg(p.bound + head0);
+      if (!two_pass && !bounded) {             // single block: the row maximum comes from this very tile
+        float mm = -INFINITY;
+#pragma unroll 1
+        for (int c2 = 0; c2 < 4; ++c2) {
+          float u[32];
+          tc::acc_ld32(sS, S_LD, row, c2 * 32, u);
+#pragma unroll
+          for (int i = 0; i < 32; ++i) mm = fmaxf(mm, u[i]);
+        }
+        m = mm;
+      }
+      const float mb = m * LOG2E;
+#pragma unroll 1
+      for (int c = 0; c < 4; ++c) {
+        float v[32];
+        tc::acc_ld32(sS, S_LD, row, c * 32, v);
+        uint32_t pk[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const float p0 = key_ok(j, c * 32 + 2 * i) ? exp2f(fmaf(v[2 * i], LOG2E, -mb)) : 0.f;
+          const float p1 = key_ok(j, c * 32 + 2 * i + 1) ? exp2f(fmaf(v[2 * i + 1], LOG2E, -mb)) : 0.f;
+          pk[i] = tc::pack_bf16x2(p0, p1);
+          float q0, q1;
+          tc::unpack_bf16x2(pk[i], q0, q1);     // l accumulates exactly what the P V MMA sees
+          l += q0 + q1;
+        }
+        uint8_t* pt = sP + (c >> 1) * TILE_BYTES;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj)
+          *reinterpret_cast<uint4*>(pt + p_offset(row, (c & 1) * 4 + jj)) = make_uint4(pk[jj * 4], pk[jj * 4 + 1], pk[jj * 4 + 2], pk[jj * 4 + 3]);
+      }
+    } else {
+      // WINDOW: own head's 64 key columns live at [64*hd, 64*hd+64); the other head's block is garbage -> zeros in P
+      float v[64];
+      {
+        float t0[32], t1[32];
+        tc::acc_ld32(sS, S_LD, row, hd * 64, t0);
+        tc::acc_ld32(sS, S_LD, row, hd * 64 + 32, t1);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
+      }
+      if constexpr (!bounded) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int kq = i >> 4;
+          const bool ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
+          v[i] = ok ? v[i] : -INFINITY;
+          m = fmaxf(m, v[i]);
+        }
+      } else {
+        m = __ldg(p.bound + head0 + hd);          // fixed shift: no maximum scan; masked keys get p = 0 below
+      }
+      const float mb = m * LOG2E;
+      uint8_t* own = sP + hd * TILE_BYTES;
+      uint8_t* other = sP + (1 - hd) * TILE_BYTES;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        uint32_t pk[4];
+        bool ok = true;                        // (bounded) seam mask of this 8-key group: zero probability instead of -inf logit
+        if constexpr (bounded) {
+          const int kq = jj >> 1;
+          ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
+        }
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          float p0 = exp2f(fmaf(v[jj * 8 + 2 * t], LOG2E, -mb)), p1 = exp2f(fmaf(v[jj * 8 + 2 * t + 1], LOG2E, -mb));
+          if constexpr (bounded) {
+            p0 = ok ? p0 : 0.f;
+            p1 = ok ? p1 : 0.f;
+          }
+          pk[t] = tc::pack_bf16x2(p0, p1);
+          float q0, q1;
+          tc::unpack_bf16x2(pk[t], q0, q1);
+          l += q0 + q1;
+        }
+        *reinterpret_cast<uint4*>(own + p_offset(row, jj)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+        *reinterpret_cast<uint4*>(other + p_offset(row, jj)) = make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+    if (pass == 1) {
+      tc::fence_proxy_async();                 // P (generic-proxy writes) -> visible to the tensor core
+      tc::named_barrier_sync(1, 128);
+      tc::wg_fence_acc(o0);
+      tc::wg_fence_acc(o1);
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < ROWS / 16; ++k) {    // 16 keys per step: K-block k / 4 of P, rows 16 k.. of V (two 8-row groups)
+        const uint32_t pa = p_addr + (uint32_t)((k >> 2) * TILE_BYTES);
+        const uint64_t bd = vdesc + (uint64_t)(k * ((16 * 128) >> 4));
+        tc::wgmma_64<1>(o0, tc::smem_desc_k_sw128(pa) + 2ull * (k & 3), bd, 1u);
+        tc::wgmma_64<1>(o1, tc::smem_desc_k_sw128(pa + 8192u) + 2ull * (k & 3), bd, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(o0);
+      tc::wg_fence_acc(o1);
+    }
+    tc::named_barrier_sync(1, 128);            // S, K, V and P are free for the next key block
+    if (lane == 0 && it + 1 < n_iter) tc::mbar_arrive(&bars->kv_free);
+  }
+  // ------------------------------------------------------ O / l -> out
+  tc::acc_store(sS, S_LD, 0, o0);
+  tc::acc_store(sS, S_LD, 64, o1);
+  tc::named_barrier_sync(1, 128);
+  const float inv = 1.f / l;
+  int64_t token;
+  int head;
+  if constexpr (MODE == MODE_WINDOW) {
+    int oi, oj;
+    if (p.shift == 0) {
+      oi = wi * 8 + ((row & 63) >> 3);
+      oj = wj * 8 + (row & 7);
+    } else {
+      const int lr = (row & 15) >> 2, lc = row & 3;
+      oi = (wi * 8 + (quad >> 1) * 4 + lr - p.shift + p.h) % p.h;
+      oj = (wj * 8 + (quad & 1) * 4 + lc - p.shift + p.w) % p.w;
+    }
+    token = (int64_t)oi * p.w + oj;
+    head = head0 + hd;
+  } else if constexpr (MODE == MODE_NA) {
+    token = (int64_t)na_qi * p.w + na_qj;
+    head = head0;
+  } else {
+    token = (int64_t)mtile * ROWS + row;
+    head = head0;
+  }
+  uint4* dst = reinterpret_cast<uint4*>(p.out + (((int64_t)b * p.h * p.w + token) * nh + head) * DH);
+#pragma unroll 1
+  for (int c = 0; c < 2; ++c) {
+    float v[32];
+    tc::acc_ld32(sS, S_LD, row, c * 32, v);
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+      dst[c * 4 + jj] = make_uint4(tc::pack_bf16x2(v[jj * 8 + 0] * inv, v[jj * 8 + 1] * inv), tc::pack_bf16x2(v[jj * 8 + 2] * inv, v[jj * 8 + 3] * inv),
+                                   tc::pack_bf16x2(v[jj * 8 + 4] * inv, v[jj * 8 + 5] * inv), tc::pack_bf16x2(v[jj * 8 + 6] * inv, v[jj * 8 + 7] * inv));
   }
 }
 
-#include "tc_attention_pipe.cuh"
 
-constexpr size_t ATTN_SMEM = 5 * TILE_BYTES + 1024 + 128;          // GLOBAL
-constexpr size_t ATTN_SMEM_WINDOW = 3 * TILE_BYTES + 1024 + 128;   // WINDOW (P aliases Q,K)
+constexpr size_t ATTN_S_BYTES = (size_t)ROWS * S_LD * 4;
+constexpr size_t ATTN_SMEM = 5 * TILE_BYTES + ATTN_S_BYTES + 1024 + 128;          // GLOBAL, NA
+constexpr size_t ATTN_SMEM_WINDOW = 3 * TILE_BYTES + ATTN_S_BYTES + 1024 + 128;   // WINDOW (P aliases Q,K)
 
 }  // namespace
 
@@ -385,7 +367,7 @@ bool tc_attention_supported(int h, int w, int nh, int e, int attn_type, int attn
   return false;
 }
 
-// programmatic dependent launch: barrier init / TMEM allocation overlap the tail of the qkv projection (KDB200_NO_PDL=1 disables)
+// programmatic dependent launch: barrier init overlaps the tail of the qkv projection (KDB200_NO_PDL=1 disables)
 template <int MODE>
 static cudaError_t set_attn_smem(size_t smem) {
   cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel<MODE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -423,16 +405,6 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
   p.out = out;
   p.B = B; p.h = h; p.w = w; p.nh = nh; p.shift = shift;
   p.bound = logit_bound;
-  // persistent pipelined kernels (tc_attention_pipe.cuh) need the logit bound; KDB200_ATTN_ONESHOT=1 keeps the one-shot kernels (A/B)
-  static const bool oneshot = [] {
-    const char* e_ = getenv("KDB200_ATTN_ONESHOT");
-    return e_ != nullptr && e_[0] == '1';
-  }();
-  const bool use_pipe = logit_bound != nullptr && !oneshot;
-  PipeAttnParams pp{};
-  pp.out = out;
-  pp.bound = logit_bound;
-  pp.B = B; pp.h = h; pp.w = w; pp.nh = nh; pp.shift = shift;
   CUtensorMap tm;
   static bool attr_w = false, attr_g = false;
   if (attn_type == KDB_ATTN_SHIFTED_WINDOW) {
@@ -447,14 +419,6 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
       attr_w = true;
     }
     p.nblk = 1;
-    if (use_pipe && (((int64_t)B * (h / 8) * (w / 8) * (nh / 2)) & 1) == 0) {
-      pp.nb = 1;
-      pp.n_pairs = (int)(((int64_t)B * (h / 8) * (w / 8) * (nh / 2)) / 2);
-      int prc = launch_attn_pipe<MODE_WINDOW>(tm, tm, pp, st);
-      if (prc) return prc;
-      KDB_LAUNCH_CHECK(F_ATTN_TC, st);
-      return 0;
-    }
     dim3 grid((unsigned)((h / 8) * (w / 8)), (unsigned)(nh / 2), (unsigned)B);
     KDB_CUDA(launch_attn<MODE_WINDOW>(grid, ATTN_SMEM_WINDOW, st, tm, tm, p));
   } else if (attn_type == KDB_ATTN_NEIGHBORHOOD) {
@@ -470,14 +434,6 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
       KDB_CUDA(set_attn_smem<MODE_NA>(ATTN_SMEM));
       attr_n = true;
     }
-    if (use_pipe && (((int64_t)B * nh * (h / NA_QH) * (w / NA_QW)) & 1) == 0) {
-      pp.nb = 3;
-      pp.n_pairs = (int)(((int64_t)B * nh * (h / NA_QH) * (w / NA_QW)) / 2);
-      int prc = launch_attn_pipe<MODE_NA>(tm, tkv, pp, st);
-      if (prc) return prc;
-      KDB_LAUNCH_CHECK(F_ATTN_TC, st);
-      return 0;
-    }
     p.nblk = 3;      // 14 halo rows = 5 + 5 + 4
     dim3 grid((unsigned)((h / NA_QH) * (w / NA_QW)), (unsigned)nh, (unsigned)B);
     KDB_CUDA(launch_attn<MODE_NA>(grid, ATTN_SMEM, st, tm, tkv, p));
@@ -491,14 +447,6 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
     if (!attr_g) {
       KDB_CUDA(set_attn_smem<MODE_GLOBAL>(ATTN_SMEM));
       attr_g = true;
-    }
-    if (use_pipe && T % 256 == 0) {
-      pp.nb = (int)(T / ROWS);
-      pp.n_pairs = B * nh * (int)(T / 256);
-      int prc = launch_attn_pipe<MODE_GLOBAL>(tm, tm, pp, st);
-      if (prc) return prc;
-      KDB_LAUNCH_CHECK(F_ATTN_TC, st);
-      return 0;
     }
     p.nblk = (int)(T / ROWS);
     dim3 grid((unsigned)(T / ROWS), (unsigned)nh, (unsigned)B);

@@ -1,7 +1,6 @@
-// tc_common.cuh -- sm_100a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld), UMMA shared-memory and instruction descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix descriptors" (also mirrored in CUTLASS
-// cute/arch/mma_sm100_desc.hpp, which was used to cross-check the field positions).
+// tc_common.cuh -- sm_90a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA) and its shared-memory descriptors.
+// Bit layouts follow the PTX ISA "asynchronous warpgroup level matrix shared memory layout / matrix descriptor".
 #pragma once
 #include <cuda.h>
 
@@ -35,7 +34,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 // One probe of the phase.  The suspend-time hint lets the hardware park the thread until the phase completes (or the hint
 // expires) instead of returning after ~100 cycles: warps that wait no longer burn issue slots their scheduler's working warps
-// (epilogue arithmetic, the tcgen05.mma issuer) need.
+// (epilogue arithmetic, the MMA warpgroup) need.
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -68,7 +67,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // Wait of a SINGLE-THREAD role (TMA producer, MMA issuer): the parked wait above goes to sleep (NANOSLEEP.SYNCS) when the phase is not
 // complete yet and pays the wake-up on the hand-off's critical path; a lone thread that polls costs no other warp an issue slot worth
 // having.  KDB_SPIN_ROLES: 0 = parked waits everywhere (default), 1 = the single-thread roles poll, 2 = also the epilogue groups'
-// accumulator waits.  Measured on one box (cfg2): 209.7 / 208.7 / 208.4 img/s for 0 / 1 / 2 -- the wake-up is not what the hand-offs cost.
+// accumulator waits.
 // Bounded like mbar_wait.
 #ifndef KDB_SPIN_ROLES
 #define KDB_SPIN_ROLES 0
@@ -154,101 +153,83 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk16) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk16 ^ (row & 7)) << 4));
 }
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {   // whole warp, cols = power of two >= 32
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {     // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (bf16 operands, fp32 accumulate); issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every tcgen05.mma issued so far by this thread has completed (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (32*(warp%4) + i), registers = columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// Issued by all 128 threads of a warpgroup; the fp32 accumulator lives in their registers.  Fragment of m64nNk16: thread t of
+// the warpgroup holds, for every 8-column block j, d[4j], d[4j+1] = (row 16 (t / 32) + (t % 32) / 4, columns 8j + 2 (t % 4) + {0, 1})
+// and d[4j+2], d[4j+3] = the same columns of row + 8.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// ties the accumulator registers to a point in the instruction stream (no read or write of them is moved across it)
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(uint32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-// same load without the wait: issue several, then tmem_ld_wait() once
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows = TMEM lanes, K along the columns, two bf16 per 32-bit column with the
-// even k in the low half) is read from tensor memory -- how P of attention reaches the P V MMA without a shared-memory round trip.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[smem, K-major] * B[smem, K-major]^T, bf16 in, fp32 accumulate
+__device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// 32 lanes x 16 consecutive 32-bit columns, registers -> TMEM (thread i of the warp writes lane 32 * (warp % 4) + i)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+// D[64 x 64] (+)= A[smem, K-major] * B[smem]; TB = 1: B is MN-major (N contiguous), as a V tile of attention is
+template <int TB>
+__device__ __forceinline__ void wgmma_64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-      "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
-// 32 lanes x 8 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]),
-               "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
+// D[64 x 128] (+)= A[registers: m64k16 bf16 fragment, 4 x bf16x2] * B[smem, K-major]^T
+__device__ __forceinline__ void wgmma_128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// The same wait, with the destination registers of an earlier tmem_ld32_nowait tied to it as read-write operands: the compiler
-// then sees the values as PRODUCED here and cannot schedule their consumers above the wait (software-pipelined loops that keep
-// one load in flight while working on the previous chunk).
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]),
-                 "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]),
-                 "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]),
-                 "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
+// Accumulator fragment of rows [row0, row0 + 64) -> fp32 shared-memory tile, row-major with `ld` floats per row: the row-per-thread
+// epilogues then read whole rows (acc_ld32).
+template <int R>
+__device__ __forceinline__ void acc_store(float* s, int ld, int row0, const float (&d)[R]) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(s + (size_t)r * ld + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(s + (size_t)(r + 8) * ld + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
+// 32 consecutive fp32 columns of one row of such a tile
+__device__ __forceinline__ void acc_ld32(const float* s, int ld, int row, int col0, float (&v)[32]) {
+  const float4* src = reinterpret_cast<const float4*>(s + (size_t)row * ld + col0);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 q = src[i];
+    v[4 * i] = q.x;
+    v[4 * i + 1] = q.y;
+    v[4 * i + 2] = q.z;
+    v[4 * i + 3] = q.w;
+  }
+}
+
 // 2^x on the MUFU unit, flush-to-zero: for softmax terms (x <= ~0; results below 2^-126 are irrelevant)
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -278,26 +259,19 @@ __device__ __forceinline__ float rowss_sum(const float4 s0, const float4 s1, con
   return acc;
 }
 
-// ---------------------------------------------------------------- packed fp32 (sm_100 FFMA2 / FMUL2: two lanes per issue slot)
-// The GEMM epilogues are bound by instruction issue, not by the fp32 datapath: pairing neighbouring columns halves the
-// number of multiply / fma instructions.  Results are bit-identical to the scalar .rn operations.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
+// ---------------------------------------------------------------- fp32 pairs
+// The epilogues work on neighbouring columns in pairs; every operation is the scalar .rn one.
+struct f32x2 {
+  float x, y;
+};
+__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return f32x2{lo, hi}; }
+__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
+  lo = v.x;
+  hi = v.y;
 }
-__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return f32x2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
+__device__ __forceinline__ f32x2 neg2(f32x2 a) { return f32x2{-a.x, -a.y}; }
 // (2 * half_val) * gelu_fast(gate) for two (value, gate) pairs; `half_val` = 0.5 * value (the caller folds the 0.5 into the
 // row scale it applies anyway):  val * gate * (0.5 + 0.5 t) = w + w t  with w = half_val * gate  -> 5 packed instructions + 2 MUFU
 __device__ __forceinline__ f32x2 geglu2(f32x2 half_val, f32x2 gate) {
@@ -311,21 +285,15 @@ __device__ __forceinline__ f32x2 geglu2(f32x2 half_val, f32x2 gate) {
 }
 
 // ---------------------------------------------------------------- descriptors
-// K-major operand tile whose rows are 128 bytes (64 bf16) wide, 128B-swizzled, 8-row groups 1024 B apart.
-// bits [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=64) | [46,48) version=1 | [61,64) layout=2 (SW128)
+// wgmma shared-memory matrix descriptor, 128B swizzle: bits [0,14) start >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [62,64) layout = 1 (SW128).
+// K-major operand tile whose rows are 128 bytes (64 bf16) wide, 8-row groups 1024 B apart (LBO unused).  A K step of 16 bf16 = 32 B
+// inside the swizzle atom is +2 on the descriptor.
 __device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// MN-major operand tile (rows of the *K* index are 128 B = 64 bf16 of the MN index), 128B-swizzled:
-// canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units -> 64-element MN atoms LBO apart, 8-row K groups SBO apart.
+// MN-major operand tile (rows of the *K* index are 128 B = 64 bf16 of the MN index): 64-element MN atoms LBO apart, 8-row K groups SBO apart.
 __device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// instruction descriptor, kind::f16: c=F32 (1<<4), a=b=BF16 (1<<7, 1<<10), majors (bit 15 / 16: 1 = MN-major), N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 62);
 }
 
 __device__ __forceinline__ bool elect_one() {

@@ -2,61 +2,45 @@
 //
 //   x <- x + down_proj( value(x_n) * gelu(gate(x_n)) ),   x_n = AdaRMSNorm(x)            (reference image_transformer_v2.py:479-493, :89-95)
 //
-// Unfused this is two launches: up_proj + GEGLU writes the [M, d_ff] hidden to HBM (100 MB at level 0 of the 256x256 model, batch 32) and
-// down_proj reads it back (profiles/r2_ncu_full_summary.json: 54.6 + 33.3 us; 147 MB of DRAM traffic in the second kernel alone).  Here
-// the hidden never leaves the SM: per 128-token tile the CTA walks d_ff in chunks of 64 hidden features,
+// Unfused this is two launches: up_proj + GEGLU writes the [M, d_ff] hidden to HBM and down_proj reads it back.  Here the hidden never
+// leaves the registers: per 128-token tile the CTA walks d_ff in chunks of 64 hidden features,
 //
-//   M1(c):  acc1[b]  = X[128 x C] . Wup_c^T          128 accumulator columns = 8 x (8 value | 8 gate) features, K = C      (SS MMA)
-//   G(c):   H_c      = value * gelu(gate) * ...      epilogue group b: tcgen05.ld -> fp32 math -> bf16 pairs -> tcgen05.st INTO acc1[b]
-//   M2(c):  acc2    += H_c[128 x 64] . Wdown_c^T     A operand read from TENSOR MEMORY (columns of acc1[b]), K = 64         (TS MMA)
+//   M1(c):  acc1     = X[64 x C] . Wup_c^T           128 accumulator columns = 8 x (8 value | 8 gate) features, K = C      (wgmma, A and B in smem)
+//   G(c):   H_c      = value * gelu(gate) * ...      in registers: a value column and its gate column sit in the same thread
+//   M2(c):  acc2    += H_c[64 x 64] . Wdown_c^T      H_c is the A operand straight from registers (the accumulator fragment of
+//                                                    two 8-column blocks is the bf16 A fragment of one k16 step), K = 64
 //
-// and after the last chunk one group adds the residual (the X tile is still in shared memory), leaves sum(x^2) for the next fused
-// RMSNorm, and stores the tile by TMA from the X buffer itself.  AdaRMSNorm is fused as in the stand-alone GEMMs: Wup carries the
-// channel scale for this evaluation (fold kernel), 1/rms of the row comes from the statistics its producer left (TcParams::ss_in).
+// and after the last chunk the residual is added (the X tile is still in shared memory), sum(x^2) is left for the next fused RMSNorm,
+// and the tile is stored by TMA from the X buffer itself.  AdaRMSNorm is fused as in the stand-alone GEMMs: Wup carries the channel scale
+// for this evaluation (fold kernel), 1/rms of the row comes from the statistics its producer left.
 //
-// Roles (480 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...):
-//   warps 0-11  three epilogue groups; group g owns acc1[g] and the chunks q = tile * nc + c with q % 3 == g; the group with
-//               tile % 3 == g also does the tile's final epilogue (after its own last chunk of that tile)
-//   warp 12     TMA producer: X tiles (2 buffers), Wup chunks (3 x 32 KiB ring), Wdown chunks (3 x 16 KiB ring) -- the weights stream
-//               from L2 once per tile (294 KiB; all CTAs walk the same chunks at about the same time)
-//   warp 13     M1 issuer, warp 14  M2 issuer: two threads, because the tensor pipe queues almost nothing behind the executing MMA
-//               (tools/mma_dual_issue_bench.cu) and each stream has its own waits; their MMAs interleave in the pipe
-// TMEM (512 columns): acc2 [0,128)  acc1[0..2] [128,512).  Shared memory: X 2 x 32 KiB, Wup 3 x 32 KiB, Wdown 3 x 16 KiB = 208 KiB.
-// Every mbarrier has ONE waiter role that observes all of its phases in order (a parity wait must never be two phases behind): the
-// final epilogue rotates over the groups, so acc2_full exists once per group.
+// Roles (288 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...):
+//   warpgroups 0, 1   rows [0, 64) / [64, 128) of every tile: M1, GEGLU, M2, final epilogue; both read the same weight chunks
+//   warp 8            TMA producer: X tiles (2 buffers), Wup chunks (3 x 32 KiB ring), Wdown chunks (3 x 16 KiB ring) -- the weights
+//                     stream from L2 once per tile (all CTAs walk the same chunks at about the same time)
+// Shared memory: X 2 x 32 KiB, Wup 3 x 32 KiB, Wdown 3 x 16 KiB = 208 KiB.
 #pragma once
 
 constexpr int FF_C = 128;                  // level width this kernel is built for
 constexpr int FF_CH = 64;                  // hidden features per chunk
-constexpr int FF_XBUF = 2, FF_WU = 3, FF_WD = 3, FF_NG = 3;
+constexpr int FF_XBUF = 2, FF_WU = 3, FF_WD = 3;
 constexpr int FF_X_BYTES = 2 * A_STAGE_BYTES;       // [128 x 128] bf16 = two SW128 k-block tiles
 constexpr int FF_WU_BYTES = 2 * A_STAGE_BYTES;      // [128 rows x 128 K]
 constexpr int FF_WD_BYTES = A_STAGE_BYTES;          // [128 rows x 64 K]
-constexpr int FF_THREADS = 128 * FF_NG + 96;
+constexpr int FF_THREADS = 256 + 32;
 
 struct FfnBars {
   uint64_t x_full[FF_XBUF], x_empty[FF_XBUF];
   uint64_t wu_full[FF_WU], wu_empty[FF_WU];
   uint64_t wd_full[FF_WD], wd_empty[FF_WD];
-  uint64_t acc1_full[FF_NG], h_ready[FF_NG], acc1_free[FF_NG];
-  uint64_t acc2_full[FF_NG], acc2_free;     // acc2_full[i % 3]: each final-epilogue group waits on its own barrier and sees all of its phases
-  uint32_t tmem;
 };
 constexpr size_t FF_SMEM = (size_t)FF_XBUF * FF_X_BYTES + (size_t)FF_WU * FF_WU_BYTES + (size_t)FF_WD * FF_WD_BYTES + sizeof(FfnBars) + 1024;
-
-constexpr int FF_TRACE_Q = 30;
-#define FF_TRACE(q_, slot_)                                                                         \
-  do {                                                                                             \
-    if (p.trace != nullptr && blockIdx.x == 0 && (q_) < FF_TRACE_Q) p.trace[(q_) * 8 + (slot_)] = clock64(); \
-  } while (0)
 
 struct FfnParams {
   const float* ss_in;      // [M, SS_PARTS] sum(x^2) of the input rows (slot 0 = the 128 channels)
   float* ss_out;           // same for the output rows, or nullptr
   int64_t M;               // tokens, multiple of 128
-  int nc;                  // d_ff / 64 chunks, >= 3
-  long long* trace;        // KDB200_FFN_TRACE=1: clock64 stamps of CTA 0, [FF_TRACE_Q chunks][8 slots], else nullptr
-  int dbg;                 // experiments (KDB200_FFN_DBG, tools/ffn_probe.py; results are garbage): 1 = weights are loaded for the first tile only, 2 = no GEGLU arithmetic
+  int nc;                  // d_ff / 64 chunks
 };
 
 __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmwu,
@@ -80,288 +64,169 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
     tc::tma_prefetch_desc(&tmo);
     for (int i = 0; i < FF_XBUF; ++i) {
       tc::mbar_init(&bars->x_full[i], 1);
-      tc::mbar_init(&bars->x_empty[i], 1);
+      tc::mbar_init(&bars->x_empty[i], 2);     // one store-drained arrival per warpgroup
     }
     for (int i = 0; i < FF_WU; ++i) {
       tc::mbar_init(&bars->wu_full[i], 1);
-      tc::mbar_init(&bars->wu_empty[i], 1);
+      tc::mbar_init(&bars->wu_empty[i], 8);    // lane 0 of each of the eight MMA warps
     }
     for (int i = 0; i < FF_WD; ++i) {
       tc::mbar_init(&bars->wd_full[i], 1);
-      tc::mbar_init(&bars->wd_empty[i], 1);
+      tc::mbar_init(&bars->wd_empty[i], 8);
     }
-    for (int i = 0; i < FF_NG; ++i) {
-      tc::mbar_init(&bars->acc1_full[i], 1);
-      tc::mbar_init(&bars->h_ready[i], 128);
-      tc::mbar_init(&bars->acc1_free[i], 1);
-    }
-    for (int i = 0; i < FF_NG; ++i) tc::mbar_init(&bars->acc2_full[i], 1);
-    tc::mbar_init(&bars->acc2_free, 128);
     tc::fence_barrier_init();
   }
-  if (pwarp == 13) tc::tmem_alloc(&bars->tmem, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = bars->tmem;
-  const uint32_t tm_acc2 = tmem, tm_acc1 = tmem + 128u;
   tc::pdl_wait();                    // x (and its row statistics) come from the kernel before us
   tc::pdl_launch_dependents();
 
-  if (pwarp == 12) {
+  if (pwarp == 8) {
     // ------------------------------------------------------------------ TMA producer
     if (tc::elect_one()) {
       uint32_t su = 0, pu = 0, sd = 0, pd = 0;        // ring slot / phase of the next Wup / Wdown chunk
-      auto load_x = [&](int i) {
+      for (int i = 0; i < n_local; ++i) {
         const int buf = i & 1;
-        tc::mbar_wait_role(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
+        tc::mbar_wait(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
         tc::mbar_arrive_expect_tx(&bars->x_full[buf], FF_X_BYTES);
         const int m0 = ((int)blockIdx.x + i * (int)gridDim.x) * BM;
         tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES, &tmx, &bars->x_full[buf], 0, m0);
         tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES + A_STAGE_BYTES, &tmx, &bars->x_full[buf], BK, m0);
-      };
-      if (n_local > 0) load_x(0);
-      for (int i = 0; i < n_local; ++i) {
         for (int c = 0; c < nc; ++c) {
-          tc::mbar_wait_role(&bars->wu_empty[su], pu ^ 1u);
-          if ((p.dbg & 1) && i > 0) {
-            tc::mbar_arrive(&bars->wu_full[su]);
-          } else {
-            tc::mbar_arrive_expect_tx(&bars->wu_full[su], FF_WU_BYTES);
-            tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES, &tmwu, &bars->wu_full[su], 0, c * 128);
-            tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES + A_STAGE_BYTES, &tmwu, &bars->wu_full[su], BK, c * 128);
-          }
+          tc::mbar_wait(&bars->wu_empty[su], pu ^ 1u);
+          tc::mbar_arrive_expect_tx(&bars->wu_full[su], FF_WU_BYTES);
+          tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES, &tmwu, &bars->wu_full[su], 0, c * 128);
+          tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES + A_STAGE_BYTES, &tmwu, &bars->wu_full[su], BK, c * 128);
           if (++su == FF_WU) {
             su = 0;
             pu ^= 1u;
           }
-          tc::mbar_wait_role(&bars->wd_empty[sd], pd ^ 1u);
-          if ((p.dbg & 1) && i > 0) {
-            tc::mbar_arrive(&bars->wd_full[sd]);
-          } else {
-            tc::mbar_arrive_expect_tx(&bars->wd_full[sd], FF_WD_BYTES);
-            tc::tma_load_2d(sWD + (size_t)sd * FF_WD_BYTES, &tmwd, &bars->wd_full[sd], c * FF_CH, 0);
-          }
+          tc::mbar_wait(&bars->wd_empty[sd], pd ^ 1u);
+          tc::mbar_arrive_expect_tx(&bars->wd_full[sd], FF_WD_BYTES);
+          tc::tma_load_2d(sWD + (size_t)sd * FF_WD_BYTES, &tmwd, &bars->wd_full[sd], c * FF_CH, 0);
           if (++sd == FF_WD) {
             sd = 0;
             pd ^= 1u;
           }
         }
-        // the next tile's X goes into the buffer of tile i - 1, whose final epilogue ended while this tile's weights streamed
-        if (i + 1 < n_local) load_x(i + 1);
       }
     }
-  } else if (pwarp == 13) {
-    // ------------------------------------------------------------------ M1 issuer: acc1[b] = X . Wup_c^T
-    if (tc::elect_one()) {
-      constexpr uint32_t IDESC = tc::idesc_bf16(BM, 128);
-      const uint32_t x_base = tc::smem_u32(sX), wu_base = tc::smem_u32(sWU);
-      uint32_t su = 0, pu = 0;
-      uint32_t b = 0, u_par = 1;       // acc1 buffer of the next chunk (q % 3) and the parity of its "free" wait: ((q / 3) & 1) ^ 1
-      for (int i = 0; i < n_local; ++i) {
-        const int buf = i & 1;
-        tc::mbar_wait_role(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
-        const uint32_t xa = x_base + (uint32_t)(buf * FF_X_BYTES);
-        for (int c = 0; c < nc; ++c) {
-          tc::mbar_wait_role(&bars->acc1_free[b], u_par);          // M2 of the chunk that used this buffer before has completed (first use: passes)
-          tc::mbar_wait_role(&bars->wu_full[su], pu);
-          tc::tc_fence_after();
-          FF_TRACE(i * nc + c, 0);
-          const uint32_t d = tm_acc1 + b * 128u;
-          const uint32_t wa = wu_base + su * (uint32_t)FF_WU_BYTES;
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb) {
-            const uint64_t ad = tc::smem_desc_k_sw128(xa + (uint32_t)(kb * A_STAGE_BYTES)), bd = tc::smem_desc_k_sw128(wa + (uint32_t)(kb * A_STAGE_BYTES));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_bf16(d, ad + 2ull * k, bd + 2ull * k, IDESC, (uint32_t)((kb | k) != 0));
-          }
-          tc::umma_commit(&bars->acc1_full[b]);
-          tc::umma_commit(&bars->wu_empty[su]);
-          FF_TRACE(i * nc + c, 1);
-          if (++su == FF_WU) {
-            su = 0;
-            pu ^= 1u;
-          }
-          if (++b == FF_NG) {
-            b = 0;
-            u_par ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (pwarp == 14) {
-    // ------------------------------------------------------------------ M2 issuer: acc2 += H_c . Wdown_c^T, H_c in tensor memory
-    if (tc::elect_one()) {
-      constexpr uint32_t IDESC = tc::idesc_bf16(BM, FF_C);
-      const uint32_t wd_base = tc::smem_u32(sWD);
-      uint32_t sd = 0, pd = 0;
-      uint32_t b = 0, u_par = 0;       // h_ready[b] parity of the next chunk: (q / 3) & 1
-      for (int i = 0; i < n_local; ++i) {
-        tc::mbar_wait_role(&bars->acc2_free, (uint32_t)((i & 1) ^ 1));        // the previous tile's final epilogue has read acc2 (first tile: passes)
-        for (int c = 0; c < nc; ++c) {
-          tc::mbar_wait_role(&bars->wd_full[sd], pd);
-          tc::mbar_wait_role(&bars->h_ready[b], u_par);
-          tc::tc_fence_after();
-          FF_TRACE(i * nc + c, 2);
-          const uint64_t bd = tc::smem_desc_k_sw128(wd_base + sd * (uint32_t)FF_WD_BYTES);
-          const uint32_t a = tm_acc1 + b * 128u;                         // H_c: 32 columns of packed bf16 pairs
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_bf16_ts(tm_acc2, a + (uint32_t)(k * 8), bd + 2ull * k, IDESC, (uint32_t)((c | k) != 0));
-          tc::umma_commit(&bars->acc1_free[b]);
-          tc::umma_commit(&bars->wd_empty[sd]);
-          FF_TRACE(i * nc + c, 3);
-          if (++sd == FF_WD) {
-            sd = 0;
-            pd ^= 1u;
-          }
-          if (++b == FF_NG) {
-            b = 0;
-            u_par ^= 1u;
-          }
-        }
-        tc::umma_commit(&bars->acc2_full[i % FF_NG]);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue groups
-    const int grp = pwarp >> 2, q4 = pwarp & 3;
-    const int row = q4 * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(q4 * 32) << 16;
-    const uint32_t tm_mine = tm_acc1 + (uint32_t)grp * 128u + lane_base;
-    const bool issuer = (pwarp & 3) == 0 && lane == 0;
-    // chunks of this group: q = grp, grp + 3, ...; (i, c) carried incrementally
-    int i = 0, c = grp;
-    while (c >= nc) {
-      c -= nc;
-      ++i;
-    }
-    uint32_t use = 0;                        // uses of acc1[grp] so far = q / 3
-    float rstd = 1.f;
-    int rstd_tile = -1;
-    while (i < n_local) {
-      const int64_t m = ((int64_t)blockIdx.x + (int64_t)i * gridDim.x) * BM + row;
-      if (rstd_tile != i) {                  // 1/rms of this thread's row: once per tile (two chunks per tile and group at d_ff = 384)
-        rstd = rsqrtf(__ldg(p.ss_in + m * SS_PARTS) / (float)FF_C + 1e-6f);
-        rstd_tile = i;
-      }
-      tc::mbar_wait_group(&bars->acc1_full[grp], use & 1u);
-      tc::tc_fence_after();
-      ++use;
-      if (row == 0) FF_TRACE(i * nc + c, 4);
-      const tc::f32x2 r2 = tc::pk2(rstd, rstd), rh = tc::pk2(0.5f * rstd, 0.5f * rstd);     // the GELU's 0.5 rides on the value's row scale
-      // four sub-passes of 32 accumulator columns = two [8 value | 8 gate] groups = 16 hidden features = 8 packed H columns.  The loads
-      // are double buffered in registers: tcgen05.wait::ld waits for every outstanding load, so the load of sub-pass s + 1 is issued right
-      // after the wait for sub-pass s and streams in behind its arithmetic (a load + wait costs ~250 cycles when nothing hides it).
-      uint32_t rr[2][32];
-      tc::tmem_ld32_nowait(tm_mine, rr[0]);
-#pragma unroll
-      for (int sp = 0; sp < 4; ++sp) {
-        tc::tmem_ld_wait(rr[sp & 1]);
-        if (sp < 3) tc::tmem_ld32_nowait(tm_mine + (uint32_t)((sp + 1) * 32), rr[(sp + 1) & 1]);
-        const uint32_t* v = rr[sp & 1];
-        uint32_t pk[8];
-#pragma unroll
-        for (int gg = 0; gg < 2; ++gg) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            tc::f32x2 val = tc::pk2(__uint_as_float(v[gg * 16 + 2 * j]), __uint_as_float(v[gg * 16 + 2 * j + 1]));
-            tc::f32x2 gate = tc::pk2(__uint_as_float(v[gg * 16 + 8 + 2 * j]), __uint_as_float(v[gg * 16 + 8 + 2 * j + 1]));
-            val = tc::mul2(val, rh);
-            gate = tc::mul2(gate, r2);
-            float o0, o1;
-            tc::upk2((p.dbg & 2) ? val : tc::geglu2(val, gate), o0, o1);
-            pk[gg * 4 + j] = tc::pack_bf16x2(o0, o1);
-          }
-        }
-        // H columns [8 sp, 8 sp + 8) overwrite accumulator columns this thread has already read (sub-pass s covers columns up to 32 s + 31)
-        tc::tmem_st8(tm_mine + (uint32_t)(sp * 8), pk);
-      }
-      tc::tmem_st_wait();
-      tc::tc_fence_before();
-      tc::mbar_arrive(&bars->h_ready[grp]);
-      if (row == 0) FF_TRACE(i * nc + c, 5);
-
-      const bool last_of_tile = c + FF_NG >= nc;
-      if (last_of_tile && (i % FF_NG) == grp) {
-        // ---- final epilogue of tile i: out = acc2 + x (residual from the X tile in shared memory), in place, then TMA store
-        const int buf = i & 1;
-        uint8_t* xt = sX + (size_t)buf * FF_X_BYTES;
-        tc::mbar_wait_group(&bars->acc2_full[grp], (uint32_t)((i / FF_NG) & 1));
-        tc::tc_fence_after();
-        if (row == 0) FF_TRACE(i * nc + c, 6);
-        tc::mbar_wait_group(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));     // long complete (the MMAs consumed the tile): acquire for the residual reads below
-
-        float ssq[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          float v[64];
-          {
-            uint32_t r0[32], r1[32];
-            tc::tmem_ld32_nowait(tm_acc2 + lane_base + (uint32_t)(g * 64), r0);
-            tc::tmem_ld32_nowait(tm_acc2 + lane_base + (uint32_t)(g * 64 + 32), r1);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int t = 0; t < 32; ++t) { v[t] = __uint_as_float(r0[t]); v[32 + t] = __uint_as_float(r1[t]); }
-          }
-          if (g == 1) {                      // acc2 is in registers: the next tile's M2 chain may start
-            tc::tc_fence_before();
-            tc::mbar_arrive(&bars->acc2_free);
-          }
-          uint8_t* rt = xt + g * SUB_TILE_BYTES;     // this thread reads and then overwrites only its own row
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint4 r4 = *reinterpret_cast<const uint4*>(rt + tc::sw128_offset(row, j));
-            const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              v[j * 8 + t * 2] += __uint_as_float(rw[t] << 16);
-              v[j * 8 + t * 2 + 1] += __uint_as_float(rw[t] & 0xffff0000u);
-            }
-          }
-#pragma unroll
-          for (int t = 0; t < 64; t += 4) {
-            ssq[0] = fmaf(v[t], v[t], ssq[0]);
-            ssq[1] = fmaf(v[t + 1], v[t + 1], ssq[1]);
-            ssq[2] = fmaf(v[t + 2], v[t + 2], ssq[2]);
-            ssq[3] = fmaf(v[t + 3], v[t + 3], ssq[3]);
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(rt + tc::sw128_offset(row, j)) =
-                make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
-                           tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
-        }
-        if (p.ss_out != nullptr) p.ss_out[m * SS_PARTS] = (ssq[0] + ssq[1]) + (ssq[2] + ssq[3]);
-        tc::fence_proxy_async();
-        tc::named_barrier_sync(1 + grp, 128);
-        if (issuer) {
-          const int m0 = ((int)blockIdx.x + i * (int)gridDim.x) * BM;
-          tc::tma_store_2d(&tmo, xt, 0, m0);
-          tc::tma_store_2d(&tmo, xt + SUB_TILE_BYTES, 64, m0);
-          tc::tma_store_commit();
-          tc::tma_store_wait_read();         // the X buffer may be refilled (tile i + 2)
-          tc::mbar_arrive(&bars->x_empty[buf]);
-          FF_TRACE(i * nc + c, 7);
-        }
-      }
-      c += FF_NG;
-      while (c >= nc) {
-        c -= nc;
-        ++i;
-      }
-    }
+    return;
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (pwarp == 13) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 512);
+
+  // ------------------------------------------------------------------ warpgroups: rows [64 wg, 64 wg + 64) of every tile
+  const int wg = pwarp >> 2, t = threadIdx.x & 127;
+  const int r0 = 64 * wg + 16 * (t >> 5) + (lane >> 2);      // this thread's two accumulator rows: r0 and r0 + 8
+  const int cq = 2 * (lane & 3);                             // and its column pair inside every 8-column block
+  const uint32_t wu_base = tc::smem_u32(sWU), wd_base = tc::smem_u32(sWD);
+  uint32_t su = 0, pu = 0, sd = 0, pd = 0;
+  for (int i = 0; i < n_local; ++i) {
+    const int buf = i & 1;
+    const int64_t m0 = ((int64_t)blockIdx.x + (int64_t)i * gridDim.x) * BM;
+    const float rstd0 = rsqrtf(__ldg(p.ss_in + (m0 + r0) * SS_PARTS) / (float)FF_C + 1e-6f);
+    const float rstd1 = rsqrtf(__ldg(p.ss_in + (m0 + r0 + 8) * SS_PARTS) / (float)FF_C + 1e-6f);
+    // the GELU's 0.5 rides on the value's row scale
+    const tc::f32x2 g0 = tc::pk2(rstd0, rstd0), g1 = tc::pk2(rstd1, rstd1), h0 = tc::pk2(0.5f * rstd0, 0.5f * rstd0), h1 = tc::pk2(0.5f * rstd1, 0.5f * rstd1);
+    tc::mbar_wait(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
+    const uint32_t xa = tc::smem_u32(sX + (size_t)buf * FF_X_BYTES) + (uint32_t)wg * 8192u;   // rows 64 wg.. of both k-block tiles
+    float acc2[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc2[j] = 0.f;
+    for (int c = 0; c < nc; ++c) {
+      // ---- M1: acc1 = X . Wup_c^T
+      float acc1[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc1[j] = 0.f;
+      tc::mbar_wait(&bars->wu_full[su], pu);
+      const uint32_t wa = wu_base + su * (uint32_t)FF_WU_BYTES;
+      tc::wg_fence_acc(acc1);
+      tc::wg_fence();
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb) {
+        const uint64_t ad = tc::smem_desc_k_sw128(xa + (uint32_t)(kb * A_STAGE_BYTES)), bd = tc::smem_desc_k_sw128(wa + (uint32_t)(kb * A_STAGE_BYTES));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_128(acc1, ad + 2ull * k, bd + 2ull * k, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(acc1);
+      if (lane == 0) tc::mbar_arrive(&bars->wu_empty[su]);
+      if (++su == FF_WU) {
+        su = 0;
+        pu ^= 1u;
+      }
+      // ---- GEGLU: 8-column block 2q = 8 value features, block 2q + 1 = their gates -> hidden block q (rows r0, r0 + 8)
+      uint32_t hreg[16];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const tc::f32x2 v0 = tc::mul2(tc::pk2(acc1[8 * q], acc1[8 * q + 1]), h0), v1 = tc::mul2(tc::pk2(acc1[8 * q + 2], acc1[8 * q + 3]), h1);
+        const tc::f32x2 q0 = tc::mul2(tc::pk2(acc1[8 * q + 4], acc1[8 * q + 5]), g0), q1 = tc::mul2(tc::pk2(acc1[8 * q + 6], acc1[8 * q + 7]), g1);
+        float o0, o1, o2, o3;
+        tc::upk2(tc::geglu2(v0, q0), o0, o1);
+        tc::upk2(tc::geglu2(v1, q1), o2, o3);
+        // A fragment of k16 step q / 2: {block 2kk row r0, block 2kk row r0 + 8, block 2kk + 1 row r0, block 2kk + 1 row r0 + 8}
+        hreg[(q >> 1) * 4 + (q & 1) * 2 + 0] = tc::pack_bf16x2(o0, o1);
+        hreg[(q >> 1) * 4 + (q & 1) * 2 + 1] = tc::pack_bf16x2(o2, o3);
+      }
+      // ---- M2: acc2 += H_c . Wdown_c^T
+      tc::mbar_wait(&bars->wd_full[sd], pd);
+      const uint64_t bd = tc::smem_desc_k_sw128(wd_base + sd * (uint32_t)FF_WD_BYTES);
+      tc::wg_fence_acc(acc2);
+      tc::wg_fence_acc(hreg);
+      tc::wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint32_t a[4] = {hreg[4 * kk], hreg[4 * kk + 1], hreg[4 * kk + 2], hreg[4 * kk + 3]};
+        tc::wgmma_128_rs(acc2, a, bd + 2ull * kk, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(acc2);
+      if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
+      if (++sd == FF_WD) {
+        sd = 0;
+        pd ^= 1u;
+      }
+    }
+    // ---- final epilogue: out = acc2 + x (residual from the X tile in shared memory), in place, then TMA store of this half
+    uint8_t* xt = sX + (size_t)buf * FF_X_BYTES;
+    float ss0 = 0.f, ss1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      uint8_t* sub = xt + (j >> 3) * SUB_TILE_BYTES;
+      const uint32_t in16 = (uint32_t)(cq * 2);              // byte offset of the column pair inside its 16-byte chunk
+      uint32_t* p0 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0, j & 7) + in16);
+      uint32_t* p1 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0 + 8, j & 7) + in16);
+      const uint32_t x0 = *p0, x1 = *p1;
+      const float a0 = acc2[4 * j] + __uint_as_float(x0 << 16), a1 = acc2[4 * j + 1] + __uint_as_float(x0 & 0xffff0000u);
+      const float b0 = acc2[4 * j + 2] + __uint_as_float(x1 << 16), b1 = acc2[4 * j + 3] + __uint_as_float(x1 & 0xffff0000u);
+      ss0 = fmaf(a0, a0, fmaf(a1, a1, ss0));
+      ss1 = fmaf(b0, b0, fmaf(b1, b1, ss1));
+      *p0 = tc::pack_bf16x2(a0, a1);
+      *p1 = tc::pack_bf16x2(b0, b1);
+    }
+    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
+    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
+    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
+    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+    if (p.ss_out != nullptr && (lane & 3) == 0) {
+      p.ss_out[(m0 + r0) * SS_PARTS] = ss0;
+      p.ss_out[(m0 + r0 + 8) * SS_PARTS] = ss1;
+    }
+    tc::fence_proxy_async();
+    tc::named_barrier_sync(1 + wg, 128);
+    if (t == 0) {
+      tc::tma_store_2d(&tmo, xt + wg * 8192, 0, (int)m0 + 64 * wg);
+      tc::tma_store_2d(&tmo, xt + SUB_TILE_BYTES + wg * 8192, 64, (int)m0 + 64 * wg);
+      tc::tma_store_commit();
+      tc::tma_store_wait_read();         // the X buffer may be refilled (tile i + 2)
+      tc::mbar_arrive(&bars->x_empty[buf]);
+    }
   }
 }
 
 // x [M, 128] bf16 (raw residual stream, updated IN PLACE), w_up_il [2 d_ff, 128] (value / gate rows interleaved, AdaRMSNorm scale folded in),
 // w_down [128, d_ff], ss_in / ss_out [M, SS_PARTS] row statistics
-inline bool ffn_fused_supported(int64_t M, int C, int dff) { return C == FF_C && M > 0 && M % BM == 0 && dff % FF_CH == 0 && dff / FF_CH >= FF_NG; }
+inline bool ffn_fused_supported(int64_t M, int C, int dff) { return C == FF_C && M > 0 && M % BM == 0 && dff % FF_CH == 0 && dff / FF_CH >= 3; }
 
 int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int64_t M, int dff, const float* ss_in, float* ss_out, cudaStream_t st) {
   CUtensorMap tx, twu, twd, to;
@@ -369,7 +234,7 @@ int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int6
   if ((rc = tmap_2d(&tx, x, FF_C, (uint64_t)M, BK, BM))) return rc;
   if ((rc = tmap_2d(&twu, w_up_il, FF_C, (uint64_t)2 * dff, BK, 128))) return rc;
   if ((rc = tmap_2d(&twd, w_down, (uint64_t)dff, FF_C, BK, FF_C))) return rc;
-  if ((rc = tmap_2d(&to, x, FF_C, (uint64_t)M, 64, BM))) return rc;
+  if ((rc = tmap_2d(&to, x, FF_C, (uint64_t)M, 64, BM / 2))) return rc;     // each warpgroup stores its 64 rows
   static bool attr_set = false;
   if (!attr_set) {
     KDB_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
@@ -379,18 +244,7 @@ int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int6
     const char* e = getenv("KDB200_NO_PDL");
     return e != nullptr && e[0] == '1';
   }();
-  const char* dbg_env = getenv("KDB200_FFN_DBG");      // read per launch: tools/ffn_probe.py flips it between timed runs
-  FfnParams p{ss_in, ss_out, M, dff / FF_CH, nullptr, dbg_env != nullptr ? atoi(dbg_env) : 0};
-  static const bool trace_on = [] {
-    const char* e = getenv("KDB200_FFN_TRACE");
-    return e != nullptr && e[0] == '1';
-  }();
-  static long long* trace_buf = nullptr;
-  if (trace_on) {
-    if (trace_buf == nullptr) KDB_CUDA(cudaMalloc(&trace_buf, FF_TRACE_Q * 8 * sizeof(long long)));
-    KDB_CUDA(cudaMemsetAsync(trace_buf, 0, FF_TRACE_Q * 8 * sizeof(long long), st));
-    p.trace = trace_buf;
-  }
+  FfnParams p{ss_in, ss_out, M, dff / FF_CH};
   const int64_t m_tiles = M / BM;
   cudaLaunchConfig_t lc{};
   lc.gridDim = dim3((unsigned)(m_tiles < num_sms() ? m_tiles : num_sms()));
@@ -404,18 +258,5 @@ int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int6
   lc.numAttrs = no_pdl ? 0 : 1;
   KDB_CUDA(cudaLaunchKernelEx(&lc, ffn_fused_kernel, tx, twu, twd, to, p));
   KDB_LAUNCH_CHECK(F_GEMM_TC, st);
-  if (trace_on) {
-    static long long h[FF_TRACE_Q * 8];
-    KDB_CUDA(cudaMemcpyAsync(h, trace_buf, sizeof(h), cudaMemcpyDeviceToHost, st));
-    KDB_CUDA(cudaStreamSynchronize(st));
-    fprintf(stderr, "FFN trace M=%lld nc=%d grid=%u (CTA 0, cycles since M1 of chunk 0 was ready to issue): q: M1 waits done / M1 issued+committed | M2 waits done / M2 issued | group saw acc1_full / arrived h_ready | final epilogue saw acc2_full / store drained\n",
-            (long long)M, p.nc, lc.gridDim.x);
-    const long long t0 = h[0];
-    for (int q = 0; q < FF_TRACE_Q; ++q) {
-      fprintf(stderr, " q %2d:", q);
-      for (int k = 0; k < 8; ++k) fprintf(stderr, " %lld", h[q * 8 + k] ? h[q * 8 + k] - t0 : -1);
-      fprintf(stderr, "\n");
-    }
-  }
   return 0;
 }

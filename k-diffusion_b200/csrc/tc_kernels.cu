@@ -1,16 +1,15 @@
-// tc_kernels.cu -- bf16 tensor-core GEMM for sm_100a: TMA (SWIZZLE_128B tiles) -> shared memory ->
-// tcgen05.mma (fp32 accumulators in TMEM) -> tcgen05.ld -> fused epilogue -> swizzled shared tile -> TMA store.
+// tc_kernels.cu -- bf16 tensor-core GEMM for sm_90a: TMA (SWIZZLE_128B tiles) -> shared memory -> wgmma (fp32 accumulators in
+// registers) -> fp32 shared-memory tile -> fused epilogue (thread = output row) -> swizzled shared tile -> TMA store.
 //
 // C[M,N] = A[M,K] W[N,K]^T for every nn.Linear on the token stream (reference image_transformer_v2.py:126-139).
 // Epilogues: plain store; +residual (out_proj / down_proj, :396,:493; residual tile prefetched by TMA while the main loop
 // runs); GEGLU (:89-95; rows of W interleaved 8 value / 8 gate); cosine-sim scaling + axial RoPE of q and k fused into the
 // qkv projection (:106-114,187-199,245-248; cos/sin from a per-layer table); TokenSplit scatter + lerp (:618-621).
 //
-// Warp roles in a 192-thread CTA: warp 0 = TMA producer (one elected lane), warp 1 = TMEM allocator + MMA issuer (one
-// elected lane), warps 2-5 = epilogue (warp w owns TMEM lanes 32*(w%4)..+31, one accumulator row per thread).
-// One 128 x BN output tile per CTA; 2-3 CTAs are co-resident per SM so one tile's epilogue overlaps the next tile's main loop.
-// Output rows are written to a SWIZZLE_128B staging tile (the freed pipeline stage 0) and leave through one TMA store per
-// 64 columns: fully coalesced, clipped at the M edge by the tensor map.
+// Warp roles in a 160-thread CTA: warps 0-3 = the warpgroup that issues wgmma and then runs the epilogue (one accumulator row
+// per thread), warp 4 = TMA producer (one elected lane).  One 128 x BN output tile per CTA; two CTAs are co-resident per SM so
+// one tile's epilogue overlaps the other's main loop.  Output rows are written to a SWIZZLE_128B staging tile and leave through
+// one TMA store per 64 columns: fully coalesced, clipped at the M edge by the tensor map.
 #include "tc_common.cuh"
 #include "tc_kernels.cuh"
 
@@ -62,6 +61,7 @@ constexpr int BM = 128, BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KiB
 constexpr int SUB_TILE_BYTES = BM * 128;     // one [128 x 64] bf16 output sub-tile
 constexpr int MAX_STAGES = 4;
+constexpr int GEMM_THREADS = 160;            // warps 0-3: MMA + epilogue warpgroup, warp 4: TMA producer
 
 enum TcEpi { TCE_STORE = 0, TCE_RESID = 1, TCE_GEGLU = 2, TCE_SPLIT = 3, TCE_QKV = 4, TCE_PATCHOUT = 5 };
 
@@ -83,25 +83,10 @@ struct TcParams {
   float sd;
   int H, Wimg, th, tw;
   const float* ss_in;    // fused RMSNorm (consumer): A = raw x, W carries the channel scale; [M, SS_PARTS] sums of squares of x
-  float* ss_out;         // RESID / SPLIT (producer): sums of squares of the rows written, for the next fused RMSNorm
+  float* ss_out;         // RESID / SPLIT / STORE (producer): sums of squares of the rows written, for the next fused RMSNorm
   int a_merge, mwc, mC;  // A operand gathered from fine tokens (TokenMerge): coarse grid width, fine channels
-  int box_w, box_h;      // 5-D TMA boxes of merge / split: 128 rows = box_h x box_w coarse tokens
-  long long* trace;      // debug: per-tile clock64 stamps of CTA 0 (KDB200_GEMM_TRACE=1), else nullptr
-  int dbg;               // experiments only (KDB200_GEMM_DBG bit mask, tools/gemm_probe.py): 8 = the MMA issuers do not wait for the accumulator, 16 = nor for A / B, 32 = no TMA loads
-                         // (bits 1 / 2 / 4 switched parts of the epilogue off for profiles/r2_gemm_probe_epilogue_knockout.txt and were removed again)
+  int box_w, box_h;      // 5-D TMA box of the merge gather: 128 rows = box_h x box_w coarse tokens
 };
-
-// fast erf-GELU: erf via Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7, far below bf16 resolution)
-__device__ __forceinline__ float gelu_erf_fast(float x) {
-  const float z = fabsf(x) * 0.70710678118654752440f;
-  const float t = __fdividef(1.f, fmaf(0.3275911f, z, 1.f));
-  float poly = fmaf(1.061405429f, t, -1.453152027f);
-  poly = fmaf(poly, t, 1.421413741f);
-  poly = fmaf(poly, t, -0.284496736f);
-  poly = fmaf(poly, t, 0.254829592f);
-  const float erf_abs = 1.f - poly * t * __expf(-z * z);
-  return 0.5f * x * (1.f + copysignf(erf_abs, x));
-}
 
 __device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
@@ -113,8 +98,8 @@ int tmap_2d(CUtensorMap* t, const void* base, uint64_t inner, uint64_t outer, ui
 }
 
 // 5-D view of a fine token tensor X[B, 2*hc, 2*wc, C] as (e, nw, wx, nh, b*hc+hy): one (nh, nw) quadrant of `box_h x box_w`
-// coarse tokens x 64 channels is a [128 x 64] SWIZZLE_128B tile in coarse-token order -- TokenMerge's gather and TokenSplit's
-// scatter become TMA coordinates (reference image_transformer_v2.py:594,607,620).
+// coarse tokens x 64 channels is a [128 x 64] SWIZZLE_128B tile in coarse-token order -- TokenMerge's gather becomes TMA
+// coordinates (reference image_transformer_v2.py:594,607).
 int tmap_quad(CUtensorMap* t, const void* base, int C, int wc, uint64_t bhc, int box_w, int box_h) {
   const uint64_t dims[5] = {(uint64_t)C, 2, (uint64_t)wc, 2, bhc};
   const uint64_t strides[4] = {(uint64_t)C * 2, (uint64_t)C * 4, (uint64_t)wc * C * 4, (uint64_t)wc * C * 8};
@@ -136,24 +121,40 @@ bool quad_box(int wc, int* box_w, int* box_h) {
   return true;
 }
 
+// Shared memory of one GEMM CTA: the TMA ring, which the fp32 accumulator tile re-uses once the main loop is done, then the bf16
+// output staging tile (RESID: the residual tile is loaded into it and the epilogue adds in place), then the barriers.
+template <int BN> constexpr int acc_ld() { return BN + 4; }   // fp32 accumulator row pitch (+4: rows start on different banks)
+template <int BN, int EPI> constexpr int out_bytes() {
+  return EPI == TCE_GEGLU ? SUB_TILE_BYTES : (EPI == TCE_SPLIT || EPI == TCE_PATCHOUT) ? 0 : (BN / 64) * SUB_TILE_BYTES;
+}
+template <int BN>
+__host__ __device__ inline size_t gemm_region0(int stages) {
+  const size_t ring = (size_t)stages * (A_STAGE_BYTES + BN * BK * 2), acc = (size_t)BM * acc_ld<BN>() * 4;
+  return ((ring > acc ? ring : acc) + 1023) & ~(size_t)1023;
+}
+template <int BN, int EPI> inline size_t gemm_smem(int stages) { return 1024 + gemm_region0<BN>(stages) + out_bytes<BN, EPI>() + 128; }
+
+// C[M,N] tile of 128 x BN per CTA.  Warp 4 (one elected lane) streams A / W k-blocks through a ring of SWIZZLE_128B stages; the
+// warpgroup of warps 0-3 issues wgmma (two M = 64 halves per k-step) with the accumulators in registers, keeps one k-block in
+// flight while it releases the previous stage, then writes the accumulators to an fp32 tile in shared memory so that each thread
+// owns one output row for the fused epilogue (fp32 arithmetic, one rounding to bf16 at the pack, one TMA store per 64 columns).
 template <int BN, int EPI>
-__global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
-                                                      const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
-                                                      const TcParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
+                                                               const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
+                                                               const TcParams p) {
   KDB_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   constexpr int B_STAGE_BYTES = BN * BK * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr int NSUB = BN / 64;              // 64-column groups per tile
-  constexpr uint32_t IDESC = tc::idesc_bf16(BM, BN);
+  constexpr int NSUB = BN / 64;
+  constexpr int LD = acc_ld<BN>();
+  constexpr bool RES = EPI == TCE_RESID;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sC = base;                                            // staging tile = pipeline stage 0 once the main loop is done
-  uint8_t* sR = base + (size_t)p.stages * STAGE_BYTES;           // residual tile (RESID only)
-  uint64_t* full = reinterpret_cast<uint64_t*>(sR + (EPI == TCE_RESID ? NSUB * SUB_TILE_BYTES : 0));
+  float* sAcc = reinterpret_cast<float*>(base);
+  uint8_t* sC = base + gemm_region0<BN>(p.stages);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sC + out_bytes<BN, EPI>());
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tmem_full = empty + MAX_STAGES;
-  uint64_t* resid_full = tmem_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(resid_full + 1);
+  uint64_t* resid_full = empty + MAX_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t m0 = (int64_t)blockIdx.y * BM;
@@ -163,27 +164,21 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tma);
     tc::tma_prefetch_desc(&tmb);
-    if constexpr (EPI != TCE_SPLIT && EPI != TCE_PATCHOUT) tc::tma_prefetch_desc(&tmc);
     for (int s = 0; s < p.stages; ++s) {
       tc::mbar_init(&full[s], 1);
-      tc::mbar_init(&empty[s], 1);
+      tc::mbar_init(&empty[s], 4);       // lane 0 of each MMA warp
     }
-    tc::mbar_init(tmem_full, 1);
     tc::mbar_init(resid_full, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, BN);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (tc::elect_one()) {
-      if constexpr (EPI == TCE_RESID) {
+      if constexpr (RES) {
         tc::mbar_arrive_expect_tx(resid_full, NSUB * SUB_TILE_BYTES);
 #pragma unroll
-        for (int g = 0; g < NSUB; ++g) tc::tma_load_2d(sR + g * SUB_TILE_BYTES, &tmr, resid_full, n0 + g * 64, (int)m0);
+        for (int g = 0; g < NSUB; ++g) tc::tma_load_2d(sC + g * SUB_TILE_BYTES, &tmr, resid_full, n0 + g * 64, (int)m0);
       }
       for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb % p.stages;
@@ -191,220 +186,294 @@ __global__ void __launch_bounds__(192) gemm_tc_kernel(const __grid_constant__ CU
         tc::mbar_wait(&empty[s], ph ^ 1u);
         tc::mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
         uint8_t* a = base + (size_t)s * STAGE_BYTES;
-        tc::tma_load_2d(a, &tma, &full[s], kb * BK, (int)m0);
+        if (p.a_merge) {   // TokenMerge: k-block kb lives in quadrant (nh, nw) of the fine grid, channels e0..e0+63
+          const int qd = (kb * BK) / p.mC, e0 = kb * BK - qd * p.mC;
+          tc::tma_load_5d(a, &tma, &full[s], e0, qd & 1, p.box_h == 1 ? (int)(m0 % p.mwc) : 0, qd >> 1, (int)(m0 / p.mwc));
+        } else {
+          tc::tma_load_2d(a, &tma, &full[s], kb * BK, (int)m0);
+        }
         tc::tma_load_2d(a + A_STAGE_BYTES, &tmb, &full[s], kb * BK, n0);
       }
     }
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % p.stages;
-        const uint32_t ph = (uint32_t)(kb / p.stages) & 1u;
-        tc::mbar_wait(&full[s], ph);
-        tc::tc_fence_after();
-        const uint32_t a_addr = tc::smem_u32(base + (size_t)s * STAGE_BYTES);
-        const uint64_t adesc = tc::smem_desc_k_sw128(a_addr);
-        const uint64_t bdesc = tc::smem_desc_k_sw128(a_addr + A_STAGE_BYTES);
+    return;
+  }
+
+  // ---------------- main loop: warpgroup MMA, accumulators in registers
+  {
+    float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)   // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
-          tc::umma_bf16(tmem, adesc + 2ull * k, bdesc + 2ull * k, IDESC, (uint32_t)((kb | k) != 0));
-        tc::umma_commit(&empty[s]);
+    for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int s = kb % p.stages;
+      tc::mbar_wait(&full[s], (uint32_t)(kb / p.stages) & 1u);
+      const uint32_t a_addr = tc::smem_u32(base + (size_t)s * STAGE_BYTES);
+      const uint64_t ad0 = tc::smem_desc_k_sw128(a_addr), ad1 = tc::smem_desc_k_sw128(a_addr + 8 * 1024);   // rows 0-63 / 64-127
+      const uint64_t bd = tc::smem_desc_k_sw128(a_addr + A_STAGE_BYTES);
+      tc::wg_fence_acc(acc0);
+      tc::wg_fence_acc(acc1);
+      tc::wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {   // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
+        if constexpr (BN == 128) {
+          tc::wgmma_128(acc0, ad0 + 2ull * k, bd + 2ull * k, 1u);
+          tc::wgmma_128(acc1, ad1 + 2ull * k, bd + 2ull * k, 1u);
+        } else {
+          tc::wgmma_64<0>(acc0, ad0 + 2ull * k, bd + 2ull * k, 1u);
+          tc::wgmma_64<0>(acc1, ad1 + 2ull * k, bd + 2ull * k, 1u);
+        }
       }
-      tc::umma_commit(tmem_full);
+      tc::wg_commit();
+      tc::wg_wait<1>();                  // k-block kb - 1 has completed: its stage may be refilled
+      tc::wg_fence_acc(acc0);
+      tc::wg_fence_acc(acc1);
+      if (kb > 0 && lane == 0) tc::mbar_arrive(&empty[(kb - 1) % p.stages]);
     }
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(acc0);
+    tc::wg_fence_acc(acc1);
+    tc::named_barrier_sync(1, 128);      // every read of the ring is done: the accumulator tile may overwrite it
+    tc::acc_store(sAcc, LD, 0, acc0);
+    tc::acc_store(sAcc, LD, 64, acc1);
+  }
+  tc::named_barrier_sync(1, 128);
+
+  // ---------------- epilogue: thread = output row
+  const int row = threadIdx.x;
+  const int64_t m = m0 + row;
+  float rstd = 1.f;
+  if (p.ss_in != nullptr) {   // fused RMSNorm (consumer side): the producer of x left sum(x^2) of every token, one slot per 128 channels
+    const float4* sp = reinterpret_cast<const float4*>(p.ss_in + (m < p.M ? m : 0) * SS_PARTS);
+    rstd = rsqrtf(tc::rowss_sum(__ldg(sp), __ldg(sp + 1), p.K >> 7) / (float)p.K + 1e-6f);
+  }
+  if constexpr (EPI == TCE_PATCHOUT) {
+    // TokenSplitWithoutSkip 4x4 + NCHW + Denoiser combine (reference :598-607,:758-760, layers.py:88-90).  Row m = token
+    // (b, ty, tx); column n = (nh*4 + nw)*3 + c.  For fixed (c, nh) the 4 nw pixels are one float4.
+    float v[64];
+    {
+      float t0[32], t1[32];
+      tc::acc_ld32(sAcc, LD, row, 0, t0);
+      tc::acc_ld32(sAcc, LD, row, 32, t1);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
+    }
+    if (m < p.M) {
+      if (p.ss_in != nullptr) {   // fused out_norm: A is the raw residual stream, W carries the channel scale
+#pragma unroll
+        for (int i = 0; i < 48; ++i) v[i] *= rstd;
+      }
+      const int per = p.th * p.tw;
+      const int b = (int)(m / per);
+      const int r = (int)(m - (int64_t)b * per);
+      const int ty = r / p.tw, tx = r - ty * p.tw;
+      float c_skip = 0.f, c_out = 1.f, c_in;
+      if (p.sd > 0.f) karras_scalings(__ldg(p.sigma + b), p.sd, c_skip, c_out, c_in);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+#pragma unroll
+        for (int nh = 0; nh < 4; ++nh) {
+          const int64_t o = (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.Wimg + tx * 4;
+          float4 y = make_float4(bf16_round(v[(nh * 4 + 0) * 3 + c]), bf16_round(v[(nh * 4 + 1) * 3 + c]), bf16_round(v[(nh * 4 + 2) * 3 + c]),
+                                 bf16_round(v[(nh * 4 + 3) * 3 + c]));
+          if (p.sd > 0.f) {
+            const float4 xi = __ldg(reinterpret_cast<const float4*>(p.x_in + o));
+            y = make_float4(y.x * c_out + xi.x * c_skip, y.y * c_out + xi.y * c_skip, y.z * c_out + xi.z * c_skip, y.w * c_out + xi.w * c_skip);
+          }
+          *reinterpret_cast<float4*>(p.fout + o) = y;
+        }
+    }
+  } else if constexpr (EPI == TCE_SPLIT) {
+    // TokenSplit + torch.lerp(skip, x, fac) (reference :618-621): row m = (b, hy, wx) on the coarse grid; 32 columns inside one
+    // (nh, nw) quadrant (Cf % 32 == 0), scattered to the fine token
+    const bool live = m < p.M;
+    const float facv = __ldg(p.fac);
+    float ss = 0.f;
+    int64_t fine = 0;
+#pragma unroll 1
+    for (int c = 0; c < BN / 32; ++c) {
+      float v[32];
+      tc::acc_ld32(sAcc, LD, row, c * 32, v);
+      if (!live) continue;
+      const int n = n0 + c * 32;
+      const int64_t b = m / ((int64_t)p.hc * p.wc);
+      const int r = (int)(m - b * p.hc * p.wc);
+      const int hy = r / p.wc, wx = r - hy * p.wc;
+      const int qd = n / p.Cf, e = n - qd * p.Cf;
+      fine = (b * (2 * p.hc) + (2 * hy + (qd >> 1))) * (2 * p.wc) + (2 * wx + (qd & 1));
+      const int64_t off = fine * p.Cf + e;
+      const uint4* sk = reinterpret_cast<const uint4*>(p.resid + off);
+      uint4* dst = reinterpret_cast<uint4*>(p.out + off);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint4 r4 = sk[j];
+        const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
+        uint32_t ow[4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const float lo = __uint_as_float(rw[t] << 16), hi = __uint_as_float(rw[t] & 0xffff0000u);   // bf16 -> fp32 is a shift / mask
+          const float e0 = v[j * 8 + t * 2], e1 = v[j * 8 + t * 2 + 1];
+          const float d0 = e0 - lo, d1 = e1 - hi;
+          const float o0 = (facv < 0.5f) ? fmaf(facv, d0, lo) : e0 - d0 * (1.f - facv);
+          const float o1 = (facv < 0.5f) ? fmaf(facv, d1, hi) : e1 - d1 * (1.f - facv);
+          ss = fmaf(o0, o0, fmaf(o1, o1, ss));
+          ow[t] = tc::pack_bf16x2(o0, o1);
+        }
+        dst[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      }
+    }
+    // statistics of the new residual stream for the next fused RMSNorm (BN = 128 inside one quadrant: Cf % 128 == 0)
+    if (p.ss_out != nullptr && live) p.ss_out[fine * SS_PARTS + ((n0 % p.Cf) >> 7)] = ss;
   } else {
-    // ---------------- epilogue: TMEM -> registers -> (swizzled smem -> TMA store | direct scatter)
-    tc::mbar_wait(tmem_full, 0);
-    tc::tc_fence_after();
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int64_t m = m0 + row;
-    const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);
-    if constexpr (EPI == TCE_PATCHOUT) {
-      // TokenSplitWithoutSkip 4x4 + NCHW + Denoiser combine (reference :598-607,:758-760, layers.py:88-90).  Row m = token
-      // (b, ty, tx); column n = (nh*4 + nw)*3 + c.  For fixed (c, nh) the 4 nw pixels are one float4, and consecutive lanes are
-      // consecutive tokens of a row -> every warp-wide load / store is 512 contiguous bytes.
+    if constexpr (RES) tc::mbar_wait(resid_full, 0);
+    float ss_acc[4] = {0.f, 0.f, 0.f, 0.f};   // producer side: sum of squares of the row this thread writes
+#pragma unroll 1
+    for (int g = 0; g < NSUB; ++g) {
       float v[64];
       {
         float t0[32], t1[32];
-        tc::tmem_ld32(taddr, t0);
-        tc::tmem_ld32(taddr + 32, t1);
+        tc::acc_ld32(sAcc, LD, row, g * 64, t0);
+        tc::acc_ld32(sAcc, LD, row, g * 64 + 32, t1);
 #pragma unroll
         for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
       }
-      if (m < p.M) {
-        if (p.ss_in != nullptr) {   // fused out_norm: A is the raw residual stream, W carries the channel scale
-          const float4* sp = reinterpret_cast<const float4*>(p.ss_in + m * SS_PARTS);
-          const float rstd = rsqrtf(tc::rowss_sum(__ldg(sp), __ldg(sp + 1), p.K >> 7) / (float)p.K + 1e-6f);
+      if (EPI != TCE_GEGLU && p.ss_in != nullptr) {
+        // fused RMSNorm row scale.  q and k are cosine-normalised afterwards (scale invariant): only v needs it.
+        bool apply = true;
+        if constexpr (EPI == TCE_QKV) apply = (n0 + g * 64) >= 2 * p.C;
+        if (apply) {
 #pragma unroll
-          for (int i = 0; i < 48; ++i) v[i] *= rstd;
-        }
-        const int per = p.th * p.tw;
-        const int b = (int)(m / per);
-        const int r = (int)(m - (int64_t)b * per);
-        const int ty = r / p.tw, tx = r - ty * p.tw;
-        float c_skip = 0.f, c_out = 1.f, c_in;
-        if (p.sd > 0.f) karras_scalings(__ldg(p.sigma + b), p.sd, c_skip, c_out, c_in);
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-#pragma unroll
-          for (int nh = 0; nh < 4; ++nh) {
-            const int64_t o = (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.Wimg + tx * 4;
-            float4 y = make_float4(bf16_round(v[(nh * 4 + 0) * 3 + c]), bf16_round(v[(nh * 4 + 1) * 3 + c]), bf16_round(v[(nh * 4 + 2) * 3 + c]),
-                                   bf16_round(v[(nh * 4 + 3) * 3 + c]));
-            if (p.sd > 0.f) {
-              const float4 xi = __ldg(reinterpret_cast<const float4*>(p.x_in + o));
-              y = make_float4(y.x * c_out + xi.x * c_skip, y.y * c_out + xi.y * c_skip, y.z * c_out + xi.z * c_skip, y.w * c_out + xi.w * c_skip);
-            }
-            *reinterpret_cast<float4*>(p.fout + o) = y;
-          }
-      }
-    } else if constexpr (EPI == TCE_SPLIT) {
-      // TokenSplit: row m = (b, hy, wx) on the coarse grid; 32 columns inside one (nh, nw) quadrant (Cf % 32 == 0)
-      const bool live = m < p.M;
-      const float facv = __ldg(p.fac);
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tc::tmem_ld32(taddr + (uint32_t)(c * 32), v);
-        if (!live) continue;
-        const int n = n0 + c * 32;
-        const int64_t b = m / ((int64_t)p.hc * p.wc);
-        const int r = (int)(m - b * p.hc * p.wc);
-        const int hy = r / p.wc, wx = r - hy * p.wc;
-        const int qd = n / p.Cf, e = n - qd * p.Cf;
-        const int64_t off = ((b * (2 * p.hc) + (2 * hy + (qd >> 1))) * (2 * p.wc) + (2 * wx + (qd & 1))) * p.Cf + e;
-        const uint4* sk = reinterpret_cast<const uint4*>(p.resid + off);
-        uint4* dst = reinterpret_cast<uint4*>(p.out + off);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint4 r4 = sk[j];
-          const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
-          uint32_t ow[4];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            float lo, hi;
-            tc::unpack_bf16x2(rw[t], lo, hi);
-            const float e0 = bf16_round(v[j * 8 + t * 2]), e1 = bf16_round(v[j * 8 + t * 2 + 1]);
-            const float d0 = e0 - lo, d1 = e1 - hi;
-            const float o0 = (facv < 0.5f) ? fmaf(facv, d0, lo) : e0 - d0 * (1.f - facv);
-            const float o1 = (facv < 0.5f) ? fmaf(facv, d1, hi) : e1 - d1 * (1.f - facv);
-            ow[t] = tc::pack_bf16x2(o0, o1);
-          }
-          dst[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+          for (int i = 0; i < 64; ++i) v[i] *= rstd;
         }
       }
-    } else {
-      if constexpr (EPI == TCE_RESID) tc::mbar_wait(resid_full, 0);
-#pragma unroll 1
-      for (int g = 0; g < NSUB; ++g) {
-        float v[64];
-        {
-          float t0[32], t1[32];
-          tc::tmem_ld32(taddr + (uint32_t)(g * 64), t0);
-          tc::tmem_ld32(taddr + (uint32_t)(g * 64 + 32), t1);
+      if constexpr (EPI == TCE_GEGLU) {
+        // columns come as [8 value | 8 gate] groups (interleaved up_proj rows) -> 32 outputs = chunks 4g..4g+3 of the output sub-tile
+        const tc::f32x2 r2 = tc::pk2(rstd, rstd), rh = tc::pk2(0.5f * rstd, 0.5f * rstd);     // the GELU's 0.5 rides on the value's row scale
 #pragma unroll
-          for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
-        }
-        if constexpr (EPI == TCE_GEGLU) {
-          // 64 columns = 4 groups of (8 value, 8 gate) -> 32 outputs = chunks 4g..4g+3 of the single output sub-tile
+        for (int gg = 0; gg < 4; ++gg) {
+          uint32_t o[4];
 #pragma unroll
-          for (int gg = 0; gg < 4; ++gg) {
-            float o[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = bf16_round(v[gg * 16 + j]) * bf16_round(gelu_erf_fast(bf16_round(v[gg * 16 + 8 + j])));
-            *reinterpret_cast<uint4*>(sC + tc::sw128_offset(row, g * 4 + gg)) =
-                make_uint4(tc::pack_bf16x2(o[0], o[1]), tc::pack_bf16x2(o[2], o[3]), tc::pack_bf16x2(o[4], o[5]), tc::pack_bf16x2(o[6], o[7]));
+          for (int j = 0; j < 4; ++j) {
+            tc::f32x2 val = tc::pk2(v[gg * 16 + 2 * j], v[gg * 16 + 2 * j + 1]);
+            tc::f32x2 gate = tc::pk2(v[gg * 16 + 8 + 2 * j], v[gg * 16 + 8 + 2 * j + 1]);
+            val = tc::mul2(val, rh);
+            if (p.ss_in != nullptr) gate = tc::mul2(gate, r2);
+            float o0, o1;
+            tc::upk2(tc::geglu2(val, gate), o0, o1);
+            o[j] = tc::pack_bf16x2(o0, o1);
           }
-        } else {
-          if constexpr (EPI == TCE_RESID) {
-            const uint8_t* rt = sR + g * SUB_TILE_BYTES;
+          *reinterpret_cast<uint4*>(sC + tc::sw128_offset(row, g * 4 + gg)) = make_uint4(o[0], o[1], o[2], o[3]);
+        }
+      } else {
+        uint8_t* cg = sC + g * SUB_TILE_BYTES;
+        if constexpr (RES) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint4 r4 = *reinterpret_cast<const uint4*>(rt + tc::sw128_offset(row, j));
-              const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
+          for (int j = 0; j < 8; ++j) {      // this thread reads and then overwrites only its own row
+            const uint4 r4 = *reinterpret_cast<const uint4*>(cg + tc::sw128_offset(row, j));
+            const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                float lo, hi;
-                tc::unpack_bf16x2(rw[t], lo, hi);
-                v[j * 8 + t * 2] += lo;
-                v[j * 8 + t * 2 + 1] += hi;
-              }
+            for (int t = 0; t < 4; ++t) {
+              v[j * 8 + t * 2] += __uint_as_float(rw[t] << 16);
+              v[j * 8 + t * 2 + 1] += __uint_as_float(rw[t] & 0xffff0000u);
             }
           }
-          if constexpr (EPI == TCE_QKV) {
-            // this 64-column group is one head of q, k or v (feature order (t nh e), d_head 64)
-            const int n = n0 + g * 64;
-            const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
-            if (t3 < 2) {
-              float ss = 0.f;
+        }
+        if constexpr (RES || EPI == TCE_STORE) {
+          if (p.ss_out != nullptr) {
 #pragma unroll
-              for (int i = 0; i < 64; ++i) {
-                v[i] = bf16_round(v[i]);
-                ss = fmaf(v[i], v[i], ss);
-              }
-              const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(ss + 1e-6f);
-#pragma unroll
-              for (int i = 0; i < 64; ++i) v[i] = bf16_round(v[i] * sc);
-              const int64_t tok = (m < p.M ? m : 0) % p.T;
-              const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T + tok;   // [head][i][token]
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 cs = __ldg(tb + (int64_t)i * p.T);      // (cos t_2i, cos t_2i+1, sin t_2i, sin t_2i+1)
-                const float x1a = v[2 * i], x2a = v[16 + 2 * i], x1b = v[2 * i + 1], x2b = v[17 + 2 * i];
-                v[2 * i] = x1a * cs.x - x2a * cs.z;
-                v[16 + 2 * i] = x2a * cs.x + x1a * cs.z;
-                v[2 * i + 1] = x1b * cs.y - x2b * cs.w;
-                v[17 + 2 * i] = x2b * cs.y + x1b * cs.w;
-              }
+            for (int i = 0; i < 64; i += 4) {
+              ss_acc[0] = fmaf(v[i], v[i], ss_acc[0]);
+              ss_acc[1] = fmaf(v[i + 1], v[i + 1], ss_acc[1]);
+              ss_acc[2] = fmaf(v[i + 2], v[i + 2], ss_acc[2]);
+              ss_acc[3] = fmaf(v[i + 3], v[i + 3], ss_acc[3]);
             }
           }
-          uint8_t* ct = sC + g * SUB_TILE_BYTES;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(ct + tc::sw128_offset(row, j)) =
-                make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
-                           tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
         }
-      }
-      tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
-      tc::named_barrier_sync(1, 128);          // the four epilogue warps only
-      if (warp == 2 && tc::elect_one()) {
-        if constexpr (EPI == TCE_GEGLU) {
-          tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
-        } else {
+        if constexpr (EPI == TCE_QKV) {
+          const int n = n0 + g * 64;               // one head of q, k or v (feature order (t nh e), d_head 64)
+          const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
+          if (t3 < 2) {
+            // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248).  Columns (2i, 2i+1) pair with (16+2i, 17+2i); the
+            // table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4.
+            const int64_t tok = (m < p.M ? m : 0) % p.T;
+            const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T + tok;   // [head][i][token]
+            tc::f32x2 P[32];
 #pragma unroll
-          for (int g = 0; g < NSUB; ++g) tc::tma_store_2d(&tmc, sC + g * SUB_TILE_BYTES, n0 + g * 64, (int)m0);
+            for (int i = 0; i < 32; ++i) P[i] = tc::pk2(v[2 * i], v[2 * i + 1]);
+            tc::f32x2 q0 = tc::mul2(P[0], P[0]), q1 = tc::mul2(P[1], P[1]), q2 = tc::mul2(P[2], P[2]), q3 = tc::mul2(P[3], P[3]);
+#pragma unroll
+            for (int i = 4; i < 32; i += 4) {
+              q0 = tc::fma2(P[i], P[i], q0);
+              q1 = tc::fma2(P[i + 1], P[i + 1], q1);
+              q2 = tc::fma2(P[i + 2], P[i + 2], q2);
+              q3 = tc::fma2(P[i + 3], P[i + 3], q3);
+            }
+            const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y)) + 1e-6f);
+            const tc::f32x2 sc2 = tc::pk2(sc, sc);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const float4 cs = __ldg(tb + (int64_t)i * p.T);
+              const tc::f32x2 C = tc::pk2(cs.x, cs.y), S = tc::pk2(cs.z, cs.w);
+              const tc::f32x2 X1 = P[i], X2 = P[8 + i];
+              P[i] = tc::mul2(tc::fma2(X2, tc::neg2(S), tc::mul2(X1, C)), sc2);
+              P[8 + i] = tc::mul2(tc::fma2(X1, S, tc::mul2(X2, C)), sc2);
+            }
+#pragma unroll
+            for (int i = 16; i < 32; ++i) P[i] = tc::mul2(P[i], sc2);
+#pragma unroll
+            for (int i = 0; i < 32; ++i) tc::upk2(P[i], v[2 * i], v[2 * i + 1]);
+          }
         }
-        tc::tma_store_commit();
-        tc::tma_store_wait_read();             // smem must stay alive until the bulk store has read it
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j)) =
+              make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
+                         tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, BN);
+    if constexpr (RES || EPI == TCE_STORE) {
+      if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = (ss_acc[0] + ss_acc[1]) + (ss_acc[2] + ss_acc[3]);
+    }
+    tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
+    tc::named_barrier_sync(1, 128);
+    if (threadIdx.x == 0) {
+      if constexpr (EPI == TCE_GEGLU) {
+        tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
+      } else {
+#pragma unroll
+        for (int g = 0; g < NSUB; ++g) tc::tma_store_2d(&tmc, sC + g * SUB_TILE_BYTES, n0 + g * 64, (int)m0);
+      }
+      tc::tma_store_commit();
+      tc::tma_store_wait_read();             // smem must stay alive until the bulk store has read it
+    }
   }
 }
 
-#include "tc_gemm_persist.cuh"
+inline int num_sms() {
+  static int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kNumSMs;
+    return v;
+  }();
+  return n;
+}
+
 #include "tc_ffn_fused.cuh"
 
-bool use_persistent(const TcParams& p) {
-  static const bool off = [] {
-    const char* e = getenv("KDB200_GEMM_SIMPLE");
-    return e != nullptr && e[0] == '1';
-  }();
-  return !off && p.N % P_BN == 0;
+// Ring depth: two CTAs stay co-resident per SM (one CTA's epilogue overlaps the other's main loop), so a 128-wide tile keeps two
+// stages (the fp32 accumulator tile re-uses them) and a 64-wide tile up to four.
+int pick_stages(int K, int BN) {
+  const int nkb = K / BK, want = BN == 128 ? 2 : 4;
+  return nkb < want ? (nkb < 1 ? 1 : nkb) : want;
 }
 
 template <int BN, int EPI>
-int launch_tc(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) {
+int launch_tc(const bf16* A, const bf16* W, TcParams p, cudaStream_t st) {
   CUtensorMap ta, tb, tcm, tr;
   int rc;
-  if ((rc = tmap_2d(&ta, A, (uint64_t)p.K, (uint64_t)p.M, BK, BM))) return rc;
+  if (p.a_merge) {
+    if ((rc = tmap_quad(&ta, A, p.mC, p.mwc, (uint64_t)p.M / p.mwc, p.box_w, p.box_h))) return rc;
+  } else {
+    if ((rc = tmap_2d(&ta, A, (uint64_t)p.K, (uint64_t)p.M, BK, BM))) return rc;
+  }
   if ((rc = tmap_2d(&tb, W, (uint64_t)p.K, (uint64_t)p.N, BK, BN))) return rc;
   const uint64_t n_out = EPI == TCE_GEGLU ? (uint64_t)p.N / 2 : (uint64_t)p.N;
   if (EPI != TCE_SPLIT && EPI != TCE_PATCHOUT) {
@@ -417,26 +486,22 @@ int launch_tc(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) 
   } else {
     tr = ta;
   }
-  const size_t smem = (size_t)p.stages * (A_STAGE_BYTES + BN * BK * 2) + (EPI == TCE_RESID ? (BN / 64) * SUB_TILE_BYTES : 0) + 1024 + 256;
+  p.stages = pick_stages(p.K, BN);
+  const size_t smem = gemm_smem<BN, EPI>(p.stages);
   static bool attr_set = false;
   if (!attr_set) {
-    KDB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    KDB_CUDA(cudaFuncSetAttribute(gemm_wg_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem<BN, EPI>(MAX_STAGES)));
     attr_set = true;
   }
   dim3 grid((unsigned)(p.N / BN), (unsigned)ceil_div(p.M, BM));
-  gemm_tc_kernel<BN, EPI><<<grid, 192, smem, st>>>(ta, tb, tcm, tr, p);
+  gemm_wg_kernel<BN, EPI><<<grid, GEMM_THREADS, smem, st>>>(ta, tb, tcm, tr, p);
   KDB_LAUNCH_CHECK(EPI == TCE_PATCHOUT ? F_PATCH_OUT : F_GEMM_TC, st);   // (the profiler's per-family bookkeeping only)
   return 0;
 }
 
+// 128-wide tiles whenever N allows: they emit the per-128-channel row statistics of the fused RMSNorm
 template <int EPI>
 int dispatch_bn(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) {
-  if constexpr (EPI != TCE_SPLIT) {
-    if (use_persistent(p)) return launch_persist<EPI>(A, W, p, st);
-  } else {
-    TcParams q = p;
-    if (use_persistent(p) && p.Cf % P_BN == 0 && p.M % p.wc == 0 && quad_box(p.wc, &q.box_w, &q.box_h)) return launch_persist<EPI>(A, W, q, st);
-  }
   if (p.N % 128 == 0) return launch_tc<128, EPI>(A, W, p, st);
   return launch_tc<64, EPI>(A, W, p, st);
 }
@@ -445,24 +510,16 @@ bool shape_ok(int64_t M, int N, int K) {
   return M > 0 && M < (65535LL * BM) && N >= 64 && N % 64 == 0 && K >= 64 && K % 64 == 0;
 }
 
-// stage 0 doubles as the output staging tile, so >= 2 stages keep the tile inside it; the residual variant keeps the CTA
-// under ~100 KB so two CTAs stay co-resident per SM
-int pick_stages(int K, bool resid) {
-  const int nkb = K / BK;
-  const int want = resid ? 2 : 3;
-  return nkb < want ? (nkb < 1 ? 1 : nkb) : want;
-}
-
 }  // namespace
 
 namespace {
 // ------------------------------------------------------------------------------------------------
 // patch_in on the tensor core (reference image_transformer_v2.py:586-595,723-724): tokens = TokenMerge 4x4 of c_in * x, then
-// Linear(48 -> C0).  The A tile [128 tokens x 64] is not a TMA box of the NCHW fp32 latent, so the four epilogue warps build
-// it: thread = token, 12 coalesced float4 loads (3 channels x 4 patch rows: consecutive tokens are consecutive 16-byte
-// pieces of an image row), * c_in, bf16, six 16-byte swizzled shared-memory stores.  K is ordered (c, nh, nw) -- the weight
-// copy made at finalize has its columns permuted to match and is zero-padded from 48 to 64.  One tcgen05.mma k-block, then
-// the usual TMEM -> bf16 staging tile -> TMA store epilogue, which also leaves sum(x^2) per row for the fused RMSNorm.
+// Linear(48 -> C0).  The A tile [128 tokens x 64] is not a TMA box of the NCHW fp32 latent, so the warpgroup builds it: thread =
+// token, 12 coalesced float4 loads (3 channels x 4 patch rows: consecutive tokens are consecutive 16-byte pieces of an image row),
+// * c_in, bf16, six 16-byte swizzled shared-memory stores.  K is ordered (c, nh, nw) -- the weight copy made at finalize has its
+// columns permuted to match and is zero-padded from 48 to 64.  One wgmma k-block, then the usual accumulator tile -> bf16 staging
+// tile -> TMA store epilogue, which also leaves sum(x^2) per row for the fused RMSNorm.
 // ------------------------------------------------------------------------------------------------
 struct PatchInParams {
   const float* x;
@@ -473,132 +530,129 @@ struct PatchInParams {
   float* ss_out;
 };
 
-__global__ void __launch_bounds__(192) patch_in_tc_kernel(const __grid_constant__ CUtensorMap tmw, const __grid_constant__ CUtensorMap tmc,
-                                                          const PatchInParams p) {
+constexpr size_t PATCH_IN_SMEM = 1024 + 2 * A_STAGE_BYTES + (size_t)BM * acc_ld<128>() * 4 + 2 * SUB_TILE_BYTES + 64;
+
+__global__ void __launch_bounds__(GEMM_THREADS) patch_in_tc_kernel(const __grid_constant__ CUtensorMap tmw, const __grid_constant__ CUtensorMap tmc,
+                                                                   const PatchInParams p) {
   KDB_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
-  constexpr uint32_t IDESC = tc::idesc_bf16(BM, 128);
+  constexpr int LD = acc_ld<128>();
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = base;                       // [128 tokens x 64] bf16, SWIZZLE_128B
   uint8_t* sW = base + A_STAGE_BYTES;       // [128 outputs x 64]
   uint8_t* sC = sW + A_STAGE_BYTES;         // staging tile, two 64-column halves
-  uint64_t* w_full = reinterpret_cast<uint64_t*>(sC + 2 * SUB_TILE_BYTES);
-  uint64_t* a_full = w_full + 1;
-  uint64_t* tmem_full = w_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 3);
+  float* sAcc = reinterpret_cast<float*>(sC + 2 * SUB_TILE_BYTES);
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(sAcc + BM * LD);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int64_t m0 = (int64_t)blockIdx.x * BM;
   const int n0 = blockIdx.y * 128;
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmw);
     tc::tma_prefetch_desc(&tmc);
     tc::mbar_init(w_full, 1);
-    tc::mbar_init(a_full, 128);
-    tc::mbar_init(tmem_full, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 128);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (tc::elect_one()) {
       tc::mbar_arrive_expect_tx(w_full, A_STAGE_BYTES);
       tc::tma_load_2d(sW, &tmw, w_full, 0, n0);
     }
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      tc::mbar_wait(w_full, 0);
-      tc::mbar_wait(a_full, 0);
-      tc::tc_fence_after();
-      const uint64_t adesc = tc::smem_desc_k_sw128(tc::smem_u32(sA)), bdesc = tc::smem_desc_k_sw128(tc::smem_u32(sW));
+    return;
+  }
+  const int row = threadIdx.x;
+  const int64_t m = m0 + row;
+  // ---- gather: the token's 4x4x3 pixels
+  uint4 chunk[6];
+  if (m < p.M) {
+    const int per = p.th * p.tw;
+    const int b = (int)(m / per);
+    const int r = (int)(m - (int64_t)b * per);
+    const int ty = r / p.tw, tx = r - ty * p.tw;
+    float c_in = 1.f;
+    if (p.sd > 0.f) {
+      const float sg = __ldg(p.sigma + b);
+      c_in = rsqrtf(fmaf(sg, sg, p.sd * p.sd));
+    }
+    float4 px[12];
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) tc::umma_bf16(tmem, adesc + 2ull * k, bdesc + 2ull * k, IDESC, (uint32_t)(k != 0));
-      tc::umma_commit(tmem_full);
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int nh = 0; nh < 4; ++nh)
+        px[c * 4 + nh] = __ldg(reinterpret_cast<const float4*>(p.x + (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.Wimg + tx * 4));
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {          // chunk j = K columns 8j .. 8j+7 = (c = j / 2, nh = 2 (j & 1) and 2 (j & 1) + 1)
+      const float4 a = px[2 * j], bq = px[2 * j + 1];
+      chunk[j] = make_uint4(tc::pack_bf16x2(a.x * c_in, a.y * c_in), tc::pack_bf16x2(a.z * c_in, a.w * c_in), tc::pack_bf16x2(bq.x * c_in, bq.y * c_in),
+                            tc::pack_bf16x2(bq.z * c_in, bq.w * c_in));
     }
   } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int64_t m = m0 + row;
-    // ---- gather: the token's 4x4x3 pixels
-    uint4 chunk[6];
-    if (m < p.M) {
-      const int per = p.th * p.tw;
-      const int b = (int)(m / per);
-      const int r = (int)(m - (int64_t)b * per);
-      const int ty = r / p.tw, tx = r - ty * p.tw;
-      float c_in = 1.f;
-      if (p.sd > 0.f) {
-        const float sg = __ldg(p.sigma + b);
-        c_in = rsqrtf(fmaf(sg, sg, p.sd * p.sd));
-      }
-      float4 px[12];
 #pragma unroll
-      for (int c = 0; c < 3; ++c)
-#pragma unroll
-        for (int nh = 0; nh < 4; ++nh)
-          px[c * 4 + nh] = __ldg(reinterpret_cast<const float4*>(p.x + (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.Wimg + tx * 4));
-#pragma unroll
-      for (int j = 0; j < 6; ++j) {          // chunk j = K columns 8j .. 8j+7 = (c = j / 2, nh = 2 (j & 1) and 2 (j & 1) + 1)
-        const float4 a = px[2 * j], bq = px[2 * j + 1];
-        chunk[j] = make_uint4(tc::pack_bf16x2(a.x * c_in, a.y * c_in), tc::pack_bf16x2(a.z * c_in, a.w * c_in), tc::pack_bf16x2(bq.x * c_in, bq.y * c_in),
-                              tc::pack_bf16x2(bq.z * c_in, bq.w * c_in));
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 6; ++j) chunk[j] = make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int j = 0; j < 6; ++j) *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, j)) = chunk[j];
-    *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, 6)) = make_uint4(0u, 0u, 0u, 0u);     // K 48..63: zero padding
-    *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, 7)) = make_uint4(0u, 0u, 0u, 0u);
-    tc::fence_proxy_async();                 // generic-proxy writes -> visible to the tensor core's shared-memory reads
-    tc::mbar_arrive(a_full);
-    // ---- epilogue
-    tc::mbar_wait(tmem_full, 0);
-    tc::tc_fence_after();
-    float ss0 = 0.f, ss1 = 0.f;
-#pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      float v[64];
-      {
-        float t0[32], t1[32];
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(g * 64);
-        tc::tmem_ld32(taddr, t0);
-        tc::tmem_ld32(taddr + 32, t1);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
-      }
-#pragma unroll
-      for (int i = 0; i < 64; i += 2) {
-        ss0 = fmaf(v[i], v[i], ss0);
-        ss1 = fmaf(v[i + 1], v[i + 1], ss1);
-      }
-      uint8_t* cg = sC + g * SUB_TILE_BYTES;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j)) =
-            make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
-                       tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
-    }
-    if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = ss0 + ss1;
-    tc::fence_proxy_async();
-    tc::named_barrier_sync(1, 128);
-    if (warp == 2 && tc::elect_one()) {
-      tc::tma_store_2d(&tmc, sC, n0, (int)m0);
-      tc::tma_store_2d(&tmc, sC + SUB_TILE_BYTES, n0 + 64, (int)m0);
-      tc::tma_store_commit();
-      tc::tma_store_wait_read();
-    }
+    for (int j = 0; j < 6; ++j) chunk[j] = make_uint4(0u, 0u, 0u, 0u);
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 128);
+#pragma unroll
+  for (int j = 0; j < 6; ++j) *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, j)) = chunk[j];
+  *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, 6)) = make_uint4(0u, 0u, 0u, 0u);     // K 48..63: zero padding
+  *reinterpret_cast<uint4*>(sA + tc::sw128_offset(row, 7)) = make_uint4(0u, 0u, 0u, 0u);
+  tc::fence_proxy_async();                 // generic-proxy writes -> visible to the tensor core's shared-memory reads
+  tc::named_barrier_sync(1, 128);
+  tc::mbar_wait(w_full, 0);
+  {
+    float acc0[64], acc1[64];
+    const uint32_t a_addr = tc::smem_u32(sA);
+    const uint64_t ad0 = tc::smem_desc_k_sw128(a_addr), ad1 = tc::smem_desc_k_sw128(a_addr + 8 * 1024), bd = tc::smem_desc_k_sw128(tc::smem_u32(sW));
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
+    tc::wg_fence_acc(acc0);
+    tc::wg_fence_acc(acc1);
+    tc::wg_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      tc::wgmma_128(acc0, ad0 + 2ull * k, bd + 2ull * k, 1u);
+      tc::wgmma_128(acc1, ad1 + 2ull * k, bd + 2ull * k, 1u);
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(acc0);
+    tc::wg_fence_acc(acc1);
+    tc::acc_store(sAcc, LD, 0, acc0);
+    tc::acc_store(sAcc, LD, 64, acc1);
+  }
+  tc::named_barrier_sync(1, 128);
+  // ---- epilogue
+  float ss0 = 0.f, ss1 = 0.f;
+#pragma unroll
+  for (int g = 0; g < 2; ++g) {
+    float v[64];
+    {
+      float t0[32], t1[32];
+      tc::acc_ld32(sAcc, LD, row, g * 64, t0);
+      tc::acc_ld32(sAcc, LD, row, g * 64 + 32, t1);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
+    }
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      ss0 = fmaf(v[i], v[i], ss0);
+      ss1 = fmaf(v[i + 1], v[i + 1], ss1);
+    }
+    uint8_t* cg = sC + g * SUB_TILE_BYTES;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j)) =
+          make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
+                     tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
+  }
+  if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = ss0 + ss1;
+  tc::fence_proxy_async();
+  tc::named_barrier_sync(1, 128);
+  if (threadIdx.x == 0) {
+    tc::tma_store_2d(&tmc, sC, n0, (int)m0);
+    tc::tma_store_2d(&tmc, sC + SUB_TILE_BYTES, n0 + 64, (int)m0);
+    tc::tma_store_commit();
+    tc::tma_store_wait_read();
   }
 }
 
@@ -626,7 +680,7 @@ bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi) {
   if (g_tc_disabled || !shape_ok(M, N, K)) return false;
   if (epi.ss_in != nullptr && (N % 128 != 0 || K % 128 != 0 || K > 128 * SS_PARTS || (epi.mode != EPI_STORE && epi.mode != EPI_QKV_ROPE) || epi.mC > 0))
     return false;
-  if (epi.mC > 0) {   // TokenMerge gather folded into the A loads: persistent kernel only, plain store epilogue
+  if (epi.mC > 0) {   // TokenMerge gather folded into the A loads: 128-wide tiles, plain store epilogue
     int bw, bh;
     if (epi.mode != EPI_STORE || N % 128 != 0 || epi.mC % 64 != 0 || K != 4 * epi.mC || M % epi.mwc != 0 || !quad_box(epi.mwc, &bw, &bh)) return false;
   }
@@ -635,17 +689,12 @@ bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi) {
   return epi.mode == EPI_STORE || epi.mode == EPI_RESID;
 }
 
-// true when the RESID / SPLIT GEMM of this shape runs on the persistent kernel, which can leave sum(x^2) of every row it writes
+// true when the RESID / SPLIT / STORE GEMM of this shape runs on 128-wide tiles, which leave sum(x^2) of every row they write
 bool tc_gemm_emits_rowss(int64_t M, int N, int K, const GemmEpi& epi) {
   if (!tc_gemm_supported(M, N, K, epi)) return false;
-  TcParams p{};
-  p.N = N;
-  if (!use_persistent(p)) return false;
+  if (N % 128 != 0) return false;
   if (epi.mode == EPI_RESID || epi.mode == EPI_STORE) return N <= 128 * SS_PARTS;   // (STORE: the TokenMerge projection)
-  if (epi.mode == EPI_SPLIT_LERP) {
-    int bw, bh;
-    return epi.C % P_BN == 0 && epi.C <= 128 * SS_PARTS && M % epi.wc == 0 && quad_box(epi.wc, &bw, &bh);
-  }
+  if (epi.mode == EPI_SPLIT_LERP) return epi.C % 128 == 0 && epi.C <= 128 * SS_PARTS;
   return false;
 }
 
@@ -658,7 +707,6 @@ int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int 
   p.M = M;
   p.N = N;
   p.K = K;
-  p.stages = pick_stages(K, epi.mode == EPI_RESID);
   p.ss_in = epi.ss_in;
   p.ss_out = epi.ss_out;
   KDB_REQUIRE(epi.ss_in == nullptr || tc_gemm_supported(M, N, K, epi), KDB_ERR_UNSUPPORTED, "gemm_tc: fused-norm geometry not supported");
@@ -669,7 +717,7 @@ int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int 
     p.mC = epi.mC;
     p.mwc = epi.mwc;
     quad_box(epi.mwc, &p.box_w, &p.box_h);
-    return launch_persist<TCE_STORE>(A, W, p, st);
+    return launch_tc<128, TCE_STORE>(A, W, p, st);
   }
   switch (epi.mode) {
     case EPI_STORE:
@@ -709,7 +757,6 @@ int launch_patch_out_tc(const bf16* xn, const bf16* W_pad, const float* x_in, co
   p.M = (int64_t)B * (H / 4) * (Wimg / 4);
   p.N = 64;
   p.K = C0;
-  p.stages = pick_stages(C0, false);
   p.fout = out;
   p.x_in = x_in;
   p.sigma = sigma;
@@ -750,13 +797,13 @@ int launch_patch_in_tc(const float* x, const float* sigma, float sigma_data, con
   int rc;
   if ((rc = tmap_2d(&tw, W_perm, 64, (uint64_t)C0, 64, 128))) return rc;
   if ((rc = tmap_2d(&tcm, out, (uint64_t)C0, (uint64_t)p.M, 64, BM))) return rc;
-  const size_t smem = 2 * A_STAGE_BYTES + 2 * SUB_TILE_BYTES + 1024 + 256;
+  const size_t smem = PATCH_IN_SMEM;
   static bool attr_set = false;
   if (!attr_set) {
     KDB_CUDA(cudaFuncSetAttribute(patch_in_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  patch_in_tc_kernel<<<dim3((unsigned)ceil_div(p.M, BM), (unsigned)(C0 / 128)), 192, smem, st>>>(tw, tcm, p);
+  patch_in_tc_kernel<<<dim3((unsigned)ceil_div(p.M, BM), (unsigned)(C0 / 128)), GEMM_THREADS, smem, st>>>(tw, tcm, p);
   KDB_LAUNCH_CHECK(F_PATCH_IN, st);
   return 0;
 }
@@ -800,8 +847,6 @@ int launch_gemm_tc_geglu(const bf16* A, const bf16* W_il, bf16* out, int64_t M, 
   p.M = M;
   p.N = N2;
   p.K = K;
-  p.stages = pick_stages(K, false);
-  if (use_persistent(p)) return launch_persist<TCE_GEGLU>(A, W_il, p, st);
   return launch_tc<128, TCE_GEGLU>(A, W_il, p, st);
 }
 

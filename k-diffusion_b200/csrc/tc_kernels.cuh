@@ -1,12 +1,12 @@
-// tc_kernels.cuh -- tcgen05 / TMEM / TMA kernels for the bf16 fast path (sm_100a).
+// tc_kernels.cuh -- wgmma / TMA kernels for the bf16 fast path (sm_90a).
 #pragma once
 #include "model_kernels.cuh"
 
 namespace kdb {
 
-// C[M,N] = A[M,K] W[N,K]^T (+ epilogue), bf16 operands staged by TMA, fp32 accumulators in TMEM.
+// C[M,N] = A[M,K] W[N,K]^T (+ epilogue), bf16 operands staged by TMA, fp32 accumulators in registers (wgmma).
 bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi);
-// Fused RMSNorm: a RESID / SPLIT_LERP GEMM can leave sum(x^2) of every row it writes ([rows, SS_PARTS] fp32, one slot per 128
+// Fused RMSNorm: a RESID / SPLIT_LERP GEMM with N % 128 == 0 can leave sum(x^2) of every row it writes ([rows, SS_PARTS] fp32, one slot per 128
 // channels) and a STORE / QKV_ROPE / GEGLU GEMM whose A operand is that x can apply 1/rms in its epilogue (GemmEpi::ss_out / ss_in).
 constexpr int SS_PARTS = 8;
 bool tc_gemm_emits_rowss(int64_t M, int N, int K, const GemmEpi& epi);

@@ -1,4 +1,4 @@
-"""k_diffusion -- B200-native drop-in for the sampling hot path of crowsonkb/k-diffusion.
+"""k_diffusion -- H100-native drop-in for the sampling hot path of crowsonkb/k-diffusion.
 
 Same import surface as the reference for the path in scope (`sampling`, `layers.Denoiser`,
 `external.DiscreteSchedule`, `config.load_config / make_model / make_denoiser_wrapper`,

@@ -107,7 +107,7 @@ def check(rc):
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("k_diffusion (B200-native) operates on CUDA tensors only; there is no CPU fallback "
+            raise RuntimeError("k_diffusion (H100-native) operates on CUDA tensors only; there is no CPU fallback "
                                f"(got a {t.device} tensor)")
 
 
@@ -431,7 +431,7 @@ class Engine:
 
 @_on_device_of_first
 def gemm_bf16(a, w):
-    """a [M,K] bf16, w [N,K] bf16 -> [M,N] bf16 on the tcgen05 kernel (N % 64 == 0, K % 64 == 0)."""
+    """a [M,K] bf16, w [N,K] bf16 -> [M,N] bf16 on the wgmma kernel (N % 64 == 0, K % 64 == 0)."""
     require_cuda(a, w)
     assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.is_contiguous() and w.is_contiguous()
     M, K = a.shape
@@ -451,7 +451,7 @@ def interleave_geglu_rows(w_up):
 
 @_on_device_of_first
 def gemm_bf16_geglu(a, w_up, ss_in=None):
-    """a [M,K] bf16, w_up [2F,K] bf16 (reference row order) -> value * gelu(gate) [M,F] bf16 on the persistent tcgen05 kernel."""
+    """a [M,K] bf16, w_up [2F,K] bf16 (reference row order) -> value * gelu(gate) [M,F] bf16 on the wgmma kernel."""
     require_cuda(a, w_up, ss_in)
     assert a.dtype == torch.bfloat16 and w_up.dtype == torch.bfloat16 and a.is_contiguous()
     M, K = a.shape

@@ -46,7 +46,7 @@ def load_config(path_or_dict):
     config = _read(path_or_dict)
     kind = config['model']['type']
     if kind != 'image_transformer_v2':
-        raise ValueError(f'model type {kind!r} is out of scope for the B200 sampling path (only image_transformer_v2)')
+        raise ValueError(f'model type {kind!r} is out of scope for the H100 sampling path (only image_transformer_v2)')
     config = _overlay({'model': _V2_MODEL_DEFAULTS, 'optimizer': _V2_OPT_DEFAULTS}, config)
     m = config['model']
     n = len(m['widths'])

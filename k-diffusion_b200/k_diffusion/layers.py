@@ -37,7 +37,7 @@ class Denoiser(nn.Module):
         return self.sigma_data ** 2 / var, sigma * self.sigma_data / var ** 0.5, 1 / var ** 0.5
 
     def loss(self, *args, **kwargs):
-        raise NotImplementedError('training losses are out of scope for the B200 sampling path')
+        raise NotImplementedError('training losses are out of scope for the H100 sampling path')
 
     def is_native(self):
         return hasattr(self.inner_model, 'denoise') and hasattr(self.inner_model, 'engine')

@@ -211,7 +211,7 @@ class ImageTransformerDenoiserModelV2(nn.Module):
         return _native.PREC_BF16 if p == "bf16" else _native.PREC_FP32
 
     def param_groups(self, *args, **kwargs):
-        raise NotImplementedError("training is out of scope for the B200 sampling path")
+        raise NotImplementedError("training is out of scope for the H100 sampling path")
 
     # ------------------------------------------------------------------ forward
     def _check_cond(self, class_cond, mapping_cond):

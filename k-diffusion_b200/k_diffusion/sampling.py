@@ -1,4 +1,4 @@
-"""Sigma schedules, noise samplers and the Karras ODE/SDE solver loops on B200-native kernels.
+"""Sigma schedules, noise samplers and the Karras ODE/SDE solver loops on H100-native kernels.
 
 Drop-in for the functions of reference `k_diffusion/sampling.py` that are on the north-star path:
 schedules (:17-43), `to_d` (:46), `get_ancestral_step` (:51), noise samplers (:61-114),
@@ -454,7 +454,7 @@ class CFGDenoiser:
         out = self.inner_model(x_in, sigma_in, class_cond=cc)
         out_uncond, out_cond = out.chunk(2)
         if not out.is_cuda:
-            raise RuntimeError("k_diffusion (B200-native) operates on CUDA tensors only; there is no CPU fallback")
+            raise RuntimeError("k_diffusion (H100-native) operates on CUDA tensors only; there is no CPU fallback")
         return _native.cfg_combine(_native.f32c(out_uncond), _native.f32c(out_cond), self.cfg_scale)
 
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Draw images from a k-diffusion checkpoint on the B200-native engine.
+"""Draw images from a k-diffusion checkpoint on the H100-native engine.
 
 Command line of the reference's sample.py (same flags, same `<prefix>_<index>.png` files), plus three optional ones:
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Generate tests/golden/* by running the REAL reference (imported from /root/reference).
+"""Generate tests/golden/* by running the REAL reference (imported from the checkout named by $K_DIFFUSION_REFERENCE).
 
-Run in the build container only (the GPU box has no /root/reference):
+Run by hand on a machine with a reference checkout (nothing else needs it):
 
     python oracle/make_golden.py
 
@@ -23,7 +23,7 @@ from pathlib import Path
 
 os.environ["K_DIFFUSION_USE_COMPILE"] = "0"
 ROOT = Path(__file__).resolve().parents[1]
-REF = Path("/root/reference")
+REF = Path(os.environ.get("K_DIFFUSION_REFERENCE", "k-diffusion"))     # a checkout of crowsonkb/k-diffusion
 OUT = ROOT / "tests" / "golden"
 
 import numpy as np

@@ -4,7 +4,7 @@
     python oracle/make_golden_cfg.py        # -> tests/golden/cfg1_cfg.npz
 
 `make_cfg_model_fn` is a closure inside train.py's main() (train.py:333-344) and cannot be imported, so this script cuts its
-source lines out of /root/reference/train.py AT RUN TIME (nothing is copied into the repo) and executes them with the two
+source lines out of the reference's train.py ($K_DIFFUSION_REFERENCE) AT RUN TIME (nothing is copied into the repo) and executes them with the two
 free variables it reads (`cfg_scale`, `num_classes`) bound.  The recorded run is the reference's own demo() recipe
 (train.py:363: sample_dpmpp_2m_sde, eta=0, solver_type='heun') on the cfg1 MNIST model (10 classes + unconditional token)."""
 import json

@@ -14,7 +14,7 @@ for p in (str(ROOT), str(ROOT / "k-diffusion_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

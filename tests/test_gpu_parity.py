@@ -138,7 +138,7 @@ def test_neighborhood_model_vs_oracle():
 
 
 def test_neighborhood_model_bf16_tensor_core_path():
-    """128x128 input -> 32x32 tokens at level 0: the tcgen05 neighbourhood kernel (level 1 = 16x16 stays on the generic one)."""
+    """128x128 input -> 32x32 tokens at level 0: the tensor-core neighbourhood kernel (level 1 = 16x16 stays on the generic one)."""
     raw = {"model": dict(NA_CFG["model"], input_size=[128, 128], depths=[1, 1, 1])}
     cfg, sd, inner, model, _ = build(raw, precision="bf16")
     g = torch.Generator().manual_seed(8)

@@ -269,63 +269,6 @@ def test_shard_helpers():
     assert P.sample_seeds(7, 4, 9) == full[4:9] and P.sample_seeds(8, 0, 16) != full
 
 
-def _protocol_sim():
-    import importlib.util
-    from conftest import ROOT
-    spec = importlib.util.spec_from_file_location("mma_protocol_sim", ROOT / "tools" / "mma_protocol_sim.py")
-    sim = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(sim)
-    return sim
-
-
-def test_attention_pipeline_barrier_protocol_model():
-    """tools/mma_protocol_sim.py attn(): randomised interleavings of attn_pipe_kernel's mbarrier protocol (producer, MMA issuer, two
-    softmax groups, asynchronous TMA / MMA completion, try_wait.parity semantics) must never alias a phase, deadlock, overwrite a
-    live buffer or hand a consumer the wrong tile -- for shared K/V (global) and per-tile K/V (window nb = 1, neighbourhood nb = 3),
-    with the 5-stage (P in tensor memory) and the 3-stage ring."""
-    sim = _protocol_sim()
-    for shared, nb in ((True, 2), (True, 8), (False, 1), (False, 3)):
-        for n_local in (0, 1, 2, 3, 7):
-            for seed in range(12):
-                assert sim.attn(n_local, nb, shared, seed)
-                assert sim.attn(n_local, nb, shared, seed, stages=3)
-    # the rejected one-issuer-per-tile variant: fine with shared K/V, flagged with per-tile K/V on the 3-stage ring (an issuer that
-    # visits every second ring position can be a phase behind a stage the other tile used last)
-    assert all(sim.attn(5, 3, True, seed, issuers=2) for seed in range(20))
-    with pytest.raises(AssertionError, match="parity aliasing"):
-        for seed in range(200):
-            sim.attn(5, 3, False, seed, stages=3, issuers=2)
-
-
-def test_gemm_two_issuer_protocol_model():
-    """gemm_tc_persist with one or two MMA-issuing threads (tools/mma_protocol_sim.py gemm()): weight-resident mode with 1-3 n-blocks
-    per A tile, streaming mode with more k-blocks than ring stages, 2 and 3 epilogue groups.  The turn token is what makes two issuers
-    legal: without it the model reports the parity aliasing that deadlocked the first GPU run."""
-    sim = _protocol_sim()
-    for seed in range(8):
-        for nb, nkb, stages, ng in ((3, 2, 4, 2), (3, 2, 4, 3), (1, 2, 6, 2), (1, 4, 6, 3), (2, 2, 6, 2), (1, 6, 6, 2)):
-            for issuers in (1, 2):
-                for n_tiles in (0, 1, 2, 3, 7):
-                    assert sim.gemm(n_tiles * nb, nb, nkb, stages, ng, issuers, seed)
-        for nkb, stages, ng in ((8, 4, 2), (32, 4, 3), (12, 4, 2)):
-            for issuers in (1, 2):
-                for n_local in (1, 2, 5):
-                    assert sim.gemm(n_local, 1, nkb, stages, ng, issuers, seed, b_res=False)
-    with pytest.raises(AssertionError, match="parity aliasing"):
-        for seed in range(20):
-            sim.gemm(9, 1, 8, 4, 3, 2, seed, b_res=False, token=False)
-
-
-def test_fused_feed_forward_protocol_model():
-    """ffn_fused_kernel (tools/mma_protocol_sim.py ffn()): producer, M1 issuer, M2 issuer, three epilogue groups with the rotating
-    final epilogue; d_ff = 192 .. 512 (3 .. 8 chunks), 0 .. 7 tiles per CTA."""
-    sim = _protocol_sim()
-    for seed in range(10):
-        for nc in (3, 4, 5, 6, 8):
-            for n_local in (0, 1, 2, 3, 7):
-                assert sim.ffn(n_local, nc, seed)
-
-
 def test_dpm_solver_plans_and_entry_points_with_stubbed_kernels(monkeypatch):
     """SURVEY 8(f) row 4: sample_dpm_fast (an op plan like the other fixed-schedule samplers) and sample_dpm_adaptive (host PID loop
     around the same lincomb / evaluation / error-norm primitives) against outputs recorded from the reference

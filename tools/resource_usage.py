@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """(CPU) Registers / stack / static shared memory of every kernel of libkdb200.so (cuobjdump --dump-resource-usage):
 
-    python tools/resource_usage.py > profiles/rN_resource_usage.txt
+    python tools/resource_usage.py > resource_usage.txt
 """
 import re
 import subprocess
@@ -23,9 +23,9 @@ def main():
             rows.append((name,) + tuple(int(v) for v in m.groups()))
             name = None
     names = subprocess.run(["c++filt"], input="\n".join(r[0] for r in rows), capture_output=True, text=True).stdout.split("\n")
-    print("cuobjdump --dump-resource-usage libkdb200.so (sm_100a): registers per thread, stack bytes (spills / local arrays), static shared bytes.")
+    print("cuobjdump --dump-resource-usage libkdb200.so (sm_90a): registers per thread, stack bytes (spills / local arrays), static shared bytes.")
     print("Dynamic shared memory (the TMA-staged tiles of the tensor-core kernels) is requested at launch and is not listed here; SHARED = 1024 is the")
-    print("1 KiB the CUDA 12.9 runtime reserves per CTA on sm_100.  STACK is the frame size (by-value parameter structs, trap paths of the mbarrier")
+    print("1 KiB the CUDA 12.9 runtime reserves per CTA on sm_90.  STACK is the frame size (by-value parameter structs, trap paths of the mbarrier")
     print("time-outs, small local arrays), not a spill count.  `-Xptxas -v` (round 2 build) reports spills for 7 of the 101 kernels only:")
     print("gemm_tc_kernel<64,3> 8 B; ffn_fused_kernel 48 B stores / 116 B loads; attn_pipe_kernel variants 28-140 B stores / 108-176 B loads")
     print("(register cap 168 at 320 threads per CTA); every other kernel 0 bytes.  In ffn_fused_kernel no local load / store lies between the")
