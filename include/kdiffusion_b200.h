@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 7
+#define KDB_ABI_VERSION 8
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -221,6 +221,19 @@ int kdb_gemm_bf16_geglu(const void* a_bf16, const void* w_il_bf16, void* c_bf16,
  * sum(x_new^2).  Needs M % 128 == 0, d_ff % 64 == 0, d_ff >= 192.  The [M,d_ff] hidden never leaves the SM. */
 int kdb_ffn_fused_bf16(void* x_bf16, const void* w_up_il_bf16, const void* w_down_bf16, int M, int d_ff, const float* ss_in, float* ss_out,
                        void* stream);
+
+/* The whole self-attention block of a 128-wide shifted-window level in one kernel, IN PLACE on the raw residual stream
+ * x[batch,h,w,128] (bf16), two heads of d_head 64, window 8:
+ *   x <- x + out_proj( window_attn( rope(cos_sim(q)), rope(cos_sim(k)), v ) ),  [q k v] = x_n . w_qkv^T,  x_n = x / rms(x)
+ * (image_transformer_v2.py:253-337, :106-114, :187-199, :245-248, :396; the AdaRMSNorm channel scale is expected folded into w_qkv's
+ * columns).  w_qkv [384,128] (feature order (t nh e)), w_out [128,128]; qk_scale [2] fp32 = the layer's `scale`; shift 0 or 4 (the
+ * roll of the odd layers, :523).  rope: fp32 [2][8][h*w][4] = (cos t_2i, cos t_2i+1, sin t_2i, sin t_2i+1) of head n, pair i < 8 and
+ * token y*w+x, where t_j (j < 16) is the RoPE angle of column j of a head (:245-248: pos_y * freqs[n][j] for j < 8, pos_x *
+ * freqs[n][j-8] otherwise); column j < 16 of q and k rotates with column 16+j.  ss_in [batch*h*w,8] fp32 with sum(x^2) of each row
+ * in slot 0 (required); ss_out (required, may alias ss_in) receives sum(x_new^2) in slot 0, slots 1..7 untouched.  Needs
+ * h % 8 == 0 and w % 8 == 0.  q, k, v and the attention output never leave the SM. */
+int kdb_attn_block_bf16(void* x_bf16, const void* w_qkv_bf16, const void* w_out_bf16, const float* rope, const float* qk_scale, int batch, int h,
+                        int w, int shift, const float* ss_in, float* ss_out, void* stream);
 
 /* out[B,h,w,nh*e] = attention(qkv[B,h,w,3*nh*e]) on fp32 or bf16 token tensors, feature order
  * (t nh e) as produced by qkv_proj (image_transformer_v2.py:377,386,422,431,467). q/k must already be

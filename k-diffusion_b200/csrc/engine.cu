@@ -361,7 +361,17 @@ int run_layer(KdbModel* m, const LayerPlan& L, T* x, int B, int h, int w, const 
   // that produced x left its row statistics in ws.rowss
   const bool emit = std::is_same<T, bf16>::value && m->fuse_norm && C % 128 == 0;
   const bool fold = emit && cond_bs == 0 && m->fold_descs != nullptr;
-  if (L.attn_type != KDB_ATTN_NONE) {
+  // fused attention block (128-wide shifted-window levels): q, k, v and the attention output never leave the SM.  Not when one of
+  // them is being tapped.
+  const bool tapped_inside = m->tap_out != nullptr && (m->tap_name == tag + ".qkv" || m->tap_name == tag + ".ao");
+  if (fold && m->ss_valid && L.qkv_wf != nullptr && pt->rope[L.exec_index] != nullptr && !tapped_inside &&
+      tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift)) {
+    if ((rc = launch_attn_block(reinterpret_cast<bf16*>(x), L.qkv_wf, L.out_wb, pt->rope[L.exec_index], L.scale, B, h, w, L.shift, ws.rowss, ws.rowss,
+                                st)))
+      return rc;
+    m->ss_valid = true;
+    if ((rc = tap<T>(m, tag + ".attn", x, M * C, st))) return rc;
+  } else if (L.attn_type != KDB_ATTN_NONE) {
     GemmEpi qe;
     qe.mode = (L.e == 64 && pt->rope[L.exec_index] != nullptr) ? EPI_QKV_ROPE : EPI_STORE;
     qe.C = C;

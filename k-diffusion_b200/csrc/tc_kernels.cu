@@ -457,6 +457,7 @@ inline int num_sms() {
 }
 
 #include "tc_ffn_fused.cuh"
+#include "tc_attn_block.cuh"
 
 // Ring depth: two CTAs stay co-resident per SM (one CTA's epilogue overlaps the other's main loop), so a 128-wide tile keeps two
 // stages (the fp32 accumulator tile re-uses them) and a 64-wide tile up to four.
@@ -863,6 +864,18 @@ int launch_ffn_fused(bf16* x, const bf16* w_up_il, const bf16* w_down, int64_t M
   return launch_ffn_fused_impl(x, w_up_il, w_down, M, dff, ss_in, ss_out, st);
 }
 
+bool tc_attn_block_supported(int h, int w, int C, int nh, int e, int attn_type, int attn_param, int shift) {
+  return !g_tc_disabled && attn_block_supported(h, w, C, nh, e, attn_type, attn_param, shift);
+}
+
+int launch_attn_block(bf16* x, const bf16* w_qkv, const bf16* w_out, const float2* rope, const float* qk_scale, int B, int h, int w, int shift,
+                      const float* ss_in, float* ss_out, cudaStream_t st) {
+  KDB_REQUIRE(B > 0 && attn_block_supported(h, w, AB_C, 2, 64, KDB_ATTN_SHIFTED_WINDOW, 8, shift), KDB_ERR_BAD_SHAPE,
+              "attn_block: unsupported shape (needs C = 128, two heads of 64, window 8, shift 0 or 4, h %% 8 == 0, w %% 8 == 0; got B=%d h=%d w=%d shift=%d)",
+              B, h, w, shift);
+  return launch_attn_block_impl(x, w_qkv, w_out, rope, qk_scale, B, h, w, shift, ss_in, ss_out, st);
+}
+
 }  // namespace kdb
 
 extern "C" int kdb_gemm_bf16(const void* a, const void* w, void* c, int M, int N, int K, void* stream) {
@@ -886,4 +899,12 @@ extern "C" int kdb_ffn_fused_bf16(void* x, const void* w_up_il, const void* w_do
   KDB_REQUIRE(x && w_up_il && w_down && ss_in, KDB_ERR_BAD_ARG, "ffn_fused_bf16: NULL operand");
   return launch_ffn_fused(static_cast<bf16*>(x), static_cast<const bf16*>(w_up_il), static_cast<const bf16*>(w_down), M, 128, d_ff, ss_in, ss_out,
                           (cudaStream_t)stream);
+}
+
+extern "C" int kdb_attn_block_bf16(void* x, const void* w_qkv, const void* w_out, const float* rope, const float* qk_scale, int batch, int h, int w,
+                                   int shift, const float* ss_in, float* ss_out, void* stream) {
+  using namespace kdb;
+  KDB_REQUIRE(x && w_qkv && w_out && rope && qk_scale && ss_in && ss_out, KDB_ERR_BAD_ARG, "attn_block_bf16: NULL operand");
+  return launch_attn_block(static_cast<bf16*>(x), static_cast<const bf16*>(w_qkv), static_cast<const bf16*>(w_out), reinterpret_cast<const float2*>(rope),
+                           qk_scale, batch, h, w, shift, ss_in, ss_out, (cudaStream_t)stream);
 }

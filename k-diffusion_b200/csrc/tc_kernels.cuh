@@ -22,6 +22,13 @@ int launch_gemm_tc_geglu(const bf16* A, const bf16* W_il, bf16* out, int64_t M, 
 bool tc_ffn_fused_supported(int64_t M, int C, int dff);
 int launch_ffn_fused(bf16* x, const bf16* w_up_il, const bf16* w_down, int64_t M, int C, int dff, const float* ss_in, float* ss_out, cudaStream_t st);
 
+// The whole attention block of a 128-wide shifted-window level in one kernel (tc_attn_block.cuh): x <- x + out_proj(window_attn(qkv(x_n))),
+// in place on x [B, h, w, 128].  w_qkv carries the AdaRMSNorm channel scale (fold kernel); rope = the layer's launch_rope_table output;
+// ss_in = row statistics of x (required), ss_out = where to leave sum(x_new^2) per row (may alias ss_in).
+bool tc_attn_block_supported(int h, int w, int C, int nh, int e, int attn_type, int attn_param, int shift);
+int launch_attn_block(bf16* x, const bf16* w_qkv, const bf16* w_out, const float2* rope, const float* qk_scale, int B, int h, int w, int shift,
+                      const float* ss_in, float* ss_out, cudaStream_t st);
+
 // W'[n,k] = W[n,k] * g[k] for a table of weight matrices (AdaRMSNorm channel scale folded into the consumer weights)
 struct FoldDesc {
   const bf16* src;

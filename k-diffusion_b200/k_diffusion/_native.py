@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -67,6 +67,7 @@ SIGNATURES = {
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16_geglu": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "kdb_attn_block_bf16": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "kdb_attention": (_i32, [_i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
 }
 
@@ -471,6 +472,23 @@ def ffn_fused_bf16(x, w_up, w_down, ss_in, ss_out=None):
     M, F = x.shape[0], w_down.shape[1]
     w_il = interleave_geglu_rows(w_up)
     check(lib().kdb_ffn_fused_bf16(ptr(x), ptr(w_il), ptr(w_down), M, F, ptr(ss_in), ptr(ss_out), stream()))
+    return x
+
+
+@_on_device_of_first
+def attn_block_bf16(x, w_qkv, w_out, theta, scale, shift, ss_in, ss_out):
+    """x [B,h,w,128] bf16 (updated IN PLACE and returned), w_qkv [384,128] and w_out [128,128] bf16, theta [h,w,2,16] fp32 RoPE angles as
+    the reference's AxialRoPE makes them (pos * freqs, y then x), scale [2] fp32, shift 0 or 4, ss_in / ss_out [B*h*w,8] fp32 (sum(x^2)
+    per row in slot 0): x <- x + out_proj(shifted_window_attn(qkv(x / rms(x)))) in one kernel (tc_attn_block.cuh)."""
+    require_cuda(x, w_qkv, w_out, theta, scale, ss_in, ss_out)
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and w_qkv.is_contiguous() and w_out.is_contiguous()
+    assert ss_in.dtype == torch.float32 and ss_out.dtype == torch.float32 and scale.dtype == torch.float32
+    B, h, w, _ = x.shape
+    # [h,w,2,16] -> [2][8][h*w] x (cos t_2i, cos t_2i+1, sin t_2i, sin t_2i+1)
+    th = theta.float().reshape(h * w, 2, 8, 2).permute(1, 2, 0, 3)
+    table = torch.cat([th.cos(), th.sin()], dim=-1).contiguous()
+    check(lib().kdb_attn_block_bf16(ptr(x), ptr(w_qkv), ptr(w_out), ptr(table), ptr(scale.contiguous()), B, h, w, shift, ptr(ss_in), ptr(ss_out),
+                                    stream()))
     return x
 
 
