@@ -523,7 +523,10 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     if ((rc = tap<T>(m, "L" + std::to_string(l) + ".up", up, (int64_t)B * h * w * c.width[l], st))) return rc;
     cur = up;
   }
-  if (std::is_same<T, bf16>::value && m->patch_out_wb != nullptr &&
+  // the tensor-core epilogue reads x and writes out as float4: a view that starts inside a 16-byte granule (a storage offset, a
+  // caller's out= buffer) takes the scalar kernels instead
+  const bool po_aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sd <= 0.f || (reinterpret_cast<uintptr_t>(x) & 15) == 0);
+  if (std::is_same<T, bf16>::value && m->patch_out_wb != nullptr && po_aligned &&
       tc_patch_out_supported(c.width[0], c.out_channels, c.patch_h, c.patch_w, W)) {
     // out_norm as a row kernel, then the projection on the tensor core with un-patch + Karras combine in its epilogue
     if (m->ss_valid && m->patch_out_wf != nullptr && c.width[0] % 128 == 0 && c.width[0] <= 128 * SS_PARTS)

@@ -753,6 +753,8 @@ bool tc_patch_out_supported(int C0, int Cout, int ph, int pw, int Wimg) {
 int launch_patch_out_tc(const bf16* xn, const bf16* W_pad, const float* x_in, const float* sigma, float sigma_data, float* out, int B, int H,
                         int Wimg, int C0, cudaStream_t st, const float* ss_in) {
   KDB_REQUIRE(ss_in == nullptr || (C0 % 128 == 0 && C0 <= 128 * SS_PARTS), KDB_ERR_UNSUPPORTED, "patch_out_tc: fused norm needs C0 %% 128 == 0");
+  KDB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sigma_data <= 0.f || (reinterpret_cast<uintptr_t>(x_in) & 15) == 0), KDB_ERR_BAD_ARG,
+              "patch_out_tc: x and out must be 16-byte aligned (float4 epilogue)");
   TcParams p{};
   p.ss_in = ss_in;
   p.M = (int64_t)B * (H / 4) * (Wimg / 4);
