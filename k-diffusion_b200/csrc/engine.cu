@@ -7,6 +7,7 @@
 #include <cmath>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -29,14 +30,13 @@ struct LayerPlan {
   const float *ff_norm_w = nullptr, *up_w = nullptr, *down_w = nullptr;
   bf16 *qkv_wb = nullptr, *out_wb = nullptr, *up_wb = nullptr, *down_wb = nullptr;
   bf16* up_wb_il = nullptr;          // up_proj rows interleaved (value/gate) for the fused GEGLU epilogue
-  int exec_index = 0;                // position in execution order (indexes PosTables::rope)
   bool bounded = false;              // every scale[h] in (0, KDB_ATTN_MAX_BOUND]: the scale is the attention kernels' fixed softmax shift
   bf16 *qkv_wf = nullptr, *up_wf = nullptr;   // per-evaluation copies with the AdaRMSNorm channel scale folded in (fused norm)
 };
 
 struct PosTables {
   std::vector<float*> pos;          // per level: [T_l, 2] (y, x)
-  std::vector<float2*> rope;        // per layer (execution order): [T_l, nh, 16] (cos, sin) of the RoPE angles, or nullptr
+  std::vector<float2*> rope;        // per layer (KdbModel::layers): [T_l, nh, 16] (cos, sin) of the RoPE angles, or nullptr
 };
 
 }  // namespace kdb
@@ -47,16 +47,17 @@ struct KdbModel {
   KdbModelConfig cfg{};
   std::unordered_map<std::string, TensorRef> tensors;
   bool finalized = false;
-  std::vector<std::vector<LayerPlan>> down, up;
-  std::vector<LayerPlan> mid;
+  // execution order, which is also the order of the conditioning row: down levels, mid, up levels (outermost last).  Level l < n-1
+  // has depth[l] layers on the way down and as many on the way up.
+  std::vector<LayerPlan> layers;
   std::vector<const float*> merge_w, split_w, split_fac;
+  const float *patch_in_w = nullptr, *out_norm = nullptr, *patch_out_w = nullptr;
   std::vector<bf16*> merge_wb, split_wb;
   std::vector<void*> owned;
   float* ada_cat = nullptr;
   FoldDesc* fold_descs = nullptr;   // device table for launch_fold_norm_weights
   int n_fold = 0;
   bool fuse_norm = true;
-  bool ss_valid = false;            // ws.rowss describes the current residual stream (set by the GEMM that produced it)
   bf16* patch_out_wb = nullptr;     // patch_out.proj.weight zero-padded to 64 rows (tensor-core patch-out)
   bf16* patch_out_wf = nullptr;     // the same with out_norm.scale folded in (fused out_norm)
   bf16* patch_in_wb = nullptr;      // patch_in.proj.weight, columns permuted to (c, nh, nw) and padded to 64 (tensor-core patch-in)
@@ -67,8 +68,6 @@ struct KdbModel {
   std::string tap_name;
   float* tap_out = nullptr;
   int64_t tap_cap = 0, tap_count = 0;
-  int layer_counter = 0;
-  int n_layers = 0;
 };
 
 namespace {
@@ -230,31 +229,16 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
     }
   }
   // per-layer RoPE tables (freqs are per-layer buffers of the checkpoint)
-  pt.rope.assign(m->n_layers, nullptr);
-  {
-    auto build = [&](const LayerPlan& L, int hl, int wl) -> int {
-      if (L.attn_type == KDB_ATTN_NONE || L.e != 64) return 0;
-      float2* tab = nullptr;
-      int rc = dev_alloc(m, &tab, (size_t)hl * wl * L.nh * 16);
-      if (rc) return rc;
-      rc = launch_rope_table(pt.pos[L.level], L.freqs, tab, hl * wl, L.nh, L.e / 8, st);
-      if (rc) return rc;
-      pt.rope[L.exec_index] = tab;
-      return 0;
-    };
-    const int nl = m->cfg.n_levels;
-    for (int l = 0; l < nl; ++l) {
-      const int hl = h0 >> l, wl = w0 >> l;
-      int rc;
-      if (l < nl - 1) {
-        for (auto& L : m->down[l]) if ((rc = build(L, hl, wl))) return rc;
-        for (auto& L : m->up[l]) if ((rc = build(L, hl, wl))) return rc;
-      } else {
-        for (auto& L : m->mid) if ((rc = build(L, hl, wl))) return rc;
-      }
-    }
-    KDB_CUDA(cudaStreamSynchronize(st));
+  pt.rope.assign(m->layers.size(), nullptr);
+  for (size_t k = 0; k < m->layers.size(); ++k) {
+    const LayerPlan& L = m->layers[k];
+    if (L.attn_type == KDB_ATTN_NONE || L.e != 64) continue;
+    const int T_l = (h0 >> L.level) * (w0 >> L.level);
+    int rc = dev_alloc(m, &pt.rope[k], (size_t)T_l * L.nh * 16);
+    if (rc) return rc;
+    if ((rc = launch_rope_table(pt.pos[L.level], L.freqs, pt.rope[k], T_l, L.nh, L.e / 8, st))) return rc;
   }
+  KDB_CUDA(cudaStreamSynchronize(st));
   auto ins = m->pos_cache.emplace(key, std::move(pt));
   *out = &ins.first->second;
   return 0;
@@ -344,164 +328,206 @@ int linear<bf16>(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int K,
   return launch_gemm_simt<bf16, bf16>(A, W, C, M, N, K, epi, st);
 }
 
+// One forward's state: its workspace, stream and conditioning rows, and what the fused RMSNorm may use.
+struct Fwd {
+  int B;
+  Workspace& ws;
+  cudaStream_t st;
+  const float* cond;
+  int64_t cond_bs;          // conditioning row stride over the batch; 0: one row for every image
+  const PosTables* pt;
+  bool emit;                // bf16 with fused RMSNorm: producers leave the row statistics of what they write where their shape allows
+  bool fold;                // emit, one shared conditioning row and a fold table: consumers take the weights with the norm scale folded in
+  bool stats;               // ws.rowss holds the row statistics of the current residual stream
+
+  // a RESID / SPLIT_LERP / merge GEMM is about to write the residual stream: it leaves its row statistics if it can
+  void produce(GemmEpi& e, int64_t M, int N, int K) {
+    stats = emit && tc_gemm_emits_rowss(M, N, K, e);
+    e.ss_out = stats ? ws.rowss : nullptr;
+  }
+};
+
 template <typename T>
-int run_layer(KdbModel* m, const LayerPlan& L, T* x, int B, int h, int w, const PosTables* pt, const float* cond, int64_t cond_bs,
-              Workspace& ws, cudaStream_t st) {
-  const float* pos = pt->pos[L.level];
-  const int64_t Ttok = (int64_t)h * w, M = (int64_t)B * Ttok;
+int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
+  const LayerPlan& L = m->layers[k];
+  const float* pos = f.pt->pos[L.level];
+  const float2* rope = f.pt->rope[k];
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok;
   const int C = L.C;
-  T* xn = reinterpret_cast<T*>(ws.xn);
-  T* qkv = reinterpret_cast<T*>(ws.qkv);
-  T* ao = reinterpret_cast<T*>(ws.ao);
-  T* hb = reinterpret_cast<T*>(ws.hbuf);
-  T* gb = reinterpret_cast<T*>(ws.gbuf);
-  const std::string tag = "layer" + std::to_string(m->layer_counter++);
-  int rc;
-  // fused RMSNorm: possible when the whole batch shares one conditioning row (folded weights are per evaluation) and the GEMM
-  // that produced x left its row statistics in ws.rowss
-  const bool emit = std::is_same<T, bf16>::value && m->fuse_norm && C % 128 == 0;
-  const bool fold = emit && cond_bs == 0 && m->fold_descs != nullptr;
-  // fused attention block (128-wide shifted-window levels): q, k, v and the attention output never leave the SM.  Not when one of
-  // them is being tapped.
-  const bool tapped_inside = m->tap_out != nullptr && (m->tap_name == tag + ".qkv" || m->tap_name == tag + ".ao");
-  if (fold && m->ss_valid && L.qkv_wf != nullptr && pt->rope[L.exec_index] != nullptr && !tapped_inside &&
-      tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift)) {
-    if ((rc = launch_attn_block(reinterpret_cast<bf16*>(x), L.qkv_wf, L.out_wb, pt->rope[L.exec_index], L.scale, B, h, w, L.shift, ws.rowss, ws.rowss,
-                                st)))
-      return rc;
-    m->ss_valid = true;
-    if ((rc = tap<T>(m, tag + ".attn", x, M * C, st))) return rc;
-  } else if (L.attn_type != KDB_ATTN_NONE) {
+  T* xn = reinterpret_cast<T*>(f.ws.xn);
+  T* qkv = reinterpret_cast<T*>(f.ws.qkv);
+  T* ao = reinterpret_cast<T*>(f.ws.ao);
+  T* hb = reinterpret_cast<T*>(f.ws.hbuf);
+  T* gb = reinterpret_cast<T*>(f.ws.gbuf);
+  const std::string tag = "layer" + std::to_string(k);
+  auto tapped = [&](const char* part) { return m->tap_out != nullptr && m->tap_name == tag + part; };
+  int rc = 0;
+  if (L.attn_type != KDB_ATTN_NONE) {
     GemmEpi qe;
-    qe.mode = (L.e == 64 && pt->rope[L.exec_index] != nullptr) ? EPI_QKV_ROPE : EPI_STORE;
+    qe.mode = (L.e == 64 && rope != nullptr) ? EPI_QKV_ROPE : EPI_STORE;
     qe.C = C;
     qe.nh = L.nh;
     qe.T_tokens = (int)Ttok;
-    qe.rope = pt->rope[L.exec_index];
+    qe.rope = rope;
     qe.qk_scale = L.scale;
     GemmEpi qf = qe;
-    qf.ss_in = ws.rowss;
-    if (fold && m->ss_valid && L.qkv_wf != nullptr && tc_gemm_supported(M, 3 * C, C, qf)) {
-      if ((rc = launch_gemm_tc(reinterpret_cast<const bf16*>(x), L.qkv_wf, reinterpret_cast<bf16*>(qkv), M, 3 * C, C, qf, st))) return rc;
-      if (qf.mode == EPI_STORE && (rc = launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
-    } else {
-      if ((rc = launch_rmsnorm<T>(x, xn, cond + L.ada_attn, cond_bs, Ttok, M, C, st))) return rc;
-      if ((rc = tap<T>(m, tag + ".xn1", xn, M * C, st))) return rc;
-      if (std::is_same<T, bf16>::value && qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
-        // cosine-sim scaling + RoPE fused into the qkv projection's epilogue
-        if ((rc = launch_gemm_tc(reinterpret_cast<const bf16*>(xn), L.qkv_wb, reinterpret_cast<bf16*>(qkv), M, 3 * C, C, qe, st))) return rc;
+    qf.ss_in = f.ws.rowss;
+    auto norm = [&] {
+      int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
+      return r ? r : tap<T>(m, tag + ".xn1", xn, M * C, f.st);
+    };
+    auto unfused = [&] {
+      int r = norm();
+      if (!r) r = linear<T>(xn, WSel<T>::qkv(L), qkv, M, 3 * C, C, GemmEpi{}, f.st);
+      return r ? r : launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+    };
+    // attention, routes in priority order (fp32 has only the last):
+    //   attn_block: the whole half in one kernel (128-wide shifted-window levels; not while .qkv or .ao is tapped)
+    //   folded qkv GEMM: 1/rms from the row statistics, the AdaRMSNorm scale folded into the weight
+    //   RMSNorm + QKV_ROPE GEMM
+    //   RMSNorm + linear + qknorm_rope
+    // then, after all but attn_block, attention and out_proj
+    const bool block = f.fold && f.stats && rope != nullptr && !tapped(".qkv") && !tapped(".ao") &&
+                       tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift);
+    if constexpr (std::is_same_v<T, bf16>) {
+      if (block) {
+        rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st);
+        f.stats = true;
+      } else if (f.fold && f.stats && tc_gemm_supported(M, 3 * C, C, qf)) {
+        rc = launch_gemm_tc(x, L.qkv_wf, qkv, M, 3 * C, C, qf, f.st);
+        if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+      } else if (qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
+        if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv_wb, qkv, M, 3 * C, C, qe, f.st);
       } else {
-        if ((rc = linear<T>(xn, WSel<T>::qkv(L), qkv, M, 3 * C, C, GemmEpi{}, st))) return rc;
-        if ((rc = launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
+        rc = unfused();
       }
+    } else {
+      rc = unfused();
     }
-    if ((rc = tap<T>(m, tag + ".qkv", qkv, M * 3 * C, st))) return rc;
-    // the bound holds for q, k normalised by the fused QKV epilogue or by qknorm_rope (both paths above)
-    if ((rc = attention_dispatch<T>(qkv, ao, B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st, L.bounded ? L.scale : nullptr))) return rc;
-    if ((rc = tap<T>(m, tag + ".ao", ao, M * C, st))) return rc;
+    if (rc) return rc;
+    if (!block) {
+      if ((rc = tap<T>(m, tag + ".qkv", qkv, M * 3 * C, f.st))) return rc;
+      // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
+      if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
+        return rc;
+      if ((rc = tap<T>(m, tag + ".ao", ao, M * C, f.st))) return rc;
+      GemmEpi e;
+      e.mode = EPI_RESID;
+      e.resid = x;
+      f.produce(e, M, C, C);
+      if ((rc = linear<T>(ao, WSel<T>::out(L), x, M, C, C, e, f.st))) return rc;
+    }
+    if ((rc = tap<T>(m, tag + ".attn", x, M * C, f.st))) return rc;
+  }
+  auto unfused = [&] {
+    int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
+    if (!r) r = linear<T>(xn, WSel<T>::up(L), hb, M, 2 * L.dff, C, GemmEpi{}, f.st);
+    return r ? r : launch_geglu<T>(hb, gb, M, L.dff, f.st);
+  };
+  // feed-forward, routes in priority order (fp32 has only the last):
+  //   ffn_fused: the whole half in one kernel (128-wide levels; not while .geglu is tapped)
+  //   folded GEGLU GEMM: 1/rms from the row statistics, the AdaRMSNorm scale folded into the weight
+  //   RMSNorm + GEGLU GEMM
+  //   RMSNorm + linear + geglu
+  // then, after all but ffn_fused, down_proj
+  const bool ffn = f.fold && f.stats && L.up_wf != nullptr && tc_ffn_fused_supported(M, C, L.dff) && !tapped(".geglu");
+  if constexpr (std::is_same_v<T, bf16>) {
+    if (ffn) {
+      rc = launch_ffn_fused(x, L.up_wf, L.down_wb, M, C, L.dff, f.ws.rowss, f.ws.rowss, f.st);
+      f.stats = true;
+    } else if (f.fold && f.stats && L.up_wf != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C, true)) {
+      rc = launch_gemm_tc_geglu(x, L.up_wf, gb, M, 2 * L.dff, C, f.st, f.ws.rowss);
+    } else if (L.up_wb_il != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C)) {
+      rc = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
+      if (!rc) rc = launch_gemm_tc_geglu(xn, L.up_wb_il, gb, M, 2 * L.dff, C, f.st);
+    } else {
+      rc = unfused();
+    }
+  } else {
+    rc = unfused();
+  }
+  if (rc) return rc;
+  if (!ffn) {
+    if ((rc = tap<T>(m, tag + ".geglu", gb, M * L.dff, f.st))) return rc;
     GemmEpi e;
     e.mode = EPI_RESID;
     e.resid = x;
-    m->ss_valid = emit && tc_gemm_emits_rowss(M, C, C, e);
-    if (m->ss_valid) e.ss_out = ws.rowss;
-    if ((rc = linear<T>(ao, WSel<T>::out(L), x, M, C, C, e, st))) return rc;
-    if ((rc = tap<T>(m, tag + ".attn", x, M * C, st))) return rc;
+    f.produce(e, M, C, L.dff);
+    if ((rc = linear<T>(gb, WSel<T>::down(L), x, M, C, L.dff, e, f.st))) return rc;
   }
-  // fused feed-forward (128-wide levels): the hidden never leaves the SM.  Not when the hidden itself is being tapped.
-  if (fold && m->ss_valid && L.up_wf != nullptr && L.down_wb != nullptr && tc_ffn_fused_supported(M, C, L.dff) &&
-      !(m->tap_out != nullptr && m->tap_name == tag + ".geglu")) {
-    if ((rc = launch_ffn_fused(reinterpret_cast<bf16*>(x), L.up_wf, L.down_wb, M, C, L.dff, ws.rowss, ws.rowss, st))) return rc;
-    m->ss_valid = true;
-    return tap<T>(m, tag + ".ff", x, M * C, st);
-  }
-  bool fused_geglu = false;
-  if (fold && m->ss_valid && L.up_wf != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C, true)) {
-    if ((rc = launch_gemm_tc_geglu(reinterpret_cast<const bf16*>(x), L.up_wf, reinterpret_cast<bf16*>(gb), M, 2 * L.dff, C, st, ws.rowss))) return rc;
-    fused_geglu = true;
-  } else if ((rc = launch_rmsnorm<T>(x, xn, cond + L.ada_ff, cond_bs, Ttok, M, C, st))) {
-    return rc;
-  }
-  if (!fused_geglu && std::is_same<T, bf16>::value && L.up_wb_il != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C)) {
-    if ((rc = launch_gemm_tc_geglu(reinterpret_cast<const bf16*>(xn), L.up_wb_il, reinterpret_cast<bf16*>(gb), M, 2 * L.dff, C, st)))
-      return rc;
-    fused_geglu = true;
-  }
-  if (!fused_geglu) {
-    if ((rc = linear<T>(xn, WSel<T>::up(L), hb, M, 2 * L.dff, C, GemmEpi{}, st))) return rc;
-    if ((rc = launch_geglu<T>(hb, gb, M, L.dff, st))) return rc;
-  }
-  if ((rc = tap<T>(m, tag + ".geglu", gb, M * L.dff, st))) return rc;
-  GemmEpi e;
-  e.mode = EPI_RESID;
-  e.resid = x;
-  m->ss_valid = emit && tc_gemm_emits_rowss(M, C, L.dff, e);
-  if (m->ss_valid) e.ss_out = ws.rowss;
-  if ((rc = linear<T>(gb, WSel<T>::down(L), x, M, C, L.dff, e, st))) return rc;
-  return tap<T>(m, tag + ".ff", x, M * C, st);
+  return tap<T>(m, tag + ".ff", x, M * C, f.st);
 }
 
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cond_bs,
                  float* out, Workspace& ws, cudaStream_t st) {
+  constexpr bool kBf16 = std::is_same_v<T, bf16>;
   const KdbModelConfig& c = m->cfg;
-  const int n = c.n_levels;
+  const int n = c.n_levels, C0 = c.width[0];
   const int h0 = H / c.patch_h, w0 = W / c.patch_w;
   PosTables* pt = nullptr;
   int rc = ensure_pos(m, h0, w0, st, &pt);
   if (rc) return rc;
-  m->layer_counter = 0;
   m->tap_count = 0;
-  const float* patch_in_w = nullptr;
-  const float *out_norm = nullptr, *patch_out_w = nullptr;
-  GET("patch_in.proj.weight", &patch_in_w, c.width[0], (int64_t)c.patch_h * c.patch_w * c.in_channels);
-  GET("out_norm.scale", &out_norm, c.width[0]);
-  GET("patch_out.proj.weight", &patch_out_w, (int64_t)c.patch_h * c.patch_w * c.out_channels, c.width[0]);
+  Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false};
+  f.fold = f.emit && cond_bs == 0 && m->fold_descs != nullptr;
+  if (f.fold && (rc = launch_fold_norm_weights(m->fold_descs, m->n_fold, cond, st))) return rc;
 
-  if (std::is_same<T, bf16>::value && m->fuse_norm && cond_bs == 0 && m->fold_descs != nullptr)
-    if ((rc = launch_fold_norm_weights(m->fold_descs, m->n_fold, cond, st))) return rc;
-  m->ss_valid = false;
   T* cur = reinterpret_cast<T*>(ws.xs[0]);
-  if (std::is_same<T, bf16>::value && m->patch_in_wb != nullptr && tc_patch_in_supported(c.in_channels, c.patch_h, c.patch_w, c.width[0], W) &&
-      (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-    m->ss_valid = m->fuse_norm;
-    if ((rc = launch_patch_in_tc(x, sigma, sd, m->patch_in_wb, reinterpret_cast<bf16*>(cur), B, H, W, c.width[0], m->ss_valid ? ws.rowss : nullptr, st)))
-      return rc;
-  } else if ((rc = launch_patch_in<T>(x, sigma, sd, patch_in_w, cur, B, c.in_channels, H, W, c.patch_h, c.patch_w, c.width[0], st))) {
-    return rc;
+  auto patch_in = [&] {
+    return launch_patch_in<T>(x, sigma, sd, m->patch_in_w, cur, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
+  };
+  // patch_in: on the tensor core, which leaves the row statistics for the first fused RMSNorm, or the scalar kernel
+  if constexpr (kBf16) {
+    if (m->patch_in_wb != nullptr && tc_patch_in_supported(c.in_channels, c.patch_h, c.patch_w, C0, W) &&
+        (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+      f.stats = f.emit;
+      rc = launch_patch_in_tc(x, sigma, sd, m->patch_in_wb, cur, B, H, W, C0, f.stats ? ws.rowss : nullptr, st);
+    } else {
+      rc = patch_in();
+    }
+  } else {
+    rc = patch_in();
   }
-  if ((rc = tap<T>(m, "patch_in", cur, (int64_t)B * h0 * w0 * c.width[0], st))) return rc;
+  if (rc || (rc = tap<T>(m, "patch_in", cur, (int64_t)B * h0 * w0 * C0, st))) return rc;
 
-  int h = h0, w = w0;
+  int k = 0, h = h0, w = w0;
   for (int l = 0; l < n - 1; ++l) {
-    for (const LayerPlan& L : m->down[l])
-      if ((rc = run_layer<T>(m, L, cur, B, h, w, pt, cond, cond_bs, ws, st))) return rc;
+    for (int i = 0; i < c.depth[l]; ++i)
+      if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
     if ((rc = tap<T>(m, "L" + std::to_string(l) + ".down", cur, (int64_t)B * h * w * c.width[l], st))) return rc;
     T* nxt = reinterpret_cast<T*>(ws.xs[l + 1]);
-    GemmEpi me;                      // TokenMerge: the 2x2 gather rides on the GEMM's TMA loads when the geometry allows
-    me.mC = c.width[l];
-    me.mhc = h / 2;
-    me.mwc = w / 2;
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
-    bool merge_ss = false;
-    if (std::is_same<T, bf16>::value && tc_gemm_supported(Mc, c.width[l + 1], 4 * c.width[l], me)) {
-      merge_ss = m->fuse_norm && c.width[l + 1] % 128 == 0 && tc_gemm_emits_rowss(Mc, c.width[l + 1], 4 * c.width[l], me);
-      if (merge_ss) me.ss_out = ws.rowss;      // row statistics of the merged tokens for the next level's first fused RMSNorm
-      if ((rc = launch_gemm_tc(reinterpret_cast<const bf16*>(cur), m->merge_wb[l], reinterpret_cast<bf16*>(nxt), Mc, c.width[l + 1], 4 * c.width[l],
-                               me, st)))
-        return rc;
-    } else {
+    const int N = c.width[l + 1], K = 4 * c.width[l];
+    auto merge = [&] {
       T* mg = reinterpret_cast<T*>(ws.mg);
-      if ((rc = launch_merge_gather<T>(cur, mg, B, h, w, c.width[l], st))) return rc;
-      if ((rc = linear<T>(mg, WSel<T>::merge(m, l), nxt, Mc, c.width[l + 1], 4 * c.width[l], GemmEpi{}, st))) return rc;
+      f.stats = false;
+      int r = launch_merge_gather<T>(cur, mg, B, h, w, c.width[l], st);
+      return r ? r : linear<T>(mg, WSel<T>::merge(m, l), nxt, Mc, N, K, GemmEpi{}, st);
+    };
+    // TokenMerge: the 2x2 gather rides on the GEMM's TMA loads when the geometry allows, else a gather kernel and a plain GEMM
+    if constexpr (kBf16) {
+      GemmEpi me;
+      me.mC = c.width[l];
+      me.mhc = h / 2;
+      me.mwc = w / 2;
+      if (tc_gemm_supported(Mc, N, K, me)) {
+        f.produce(me, Mc, N, K);
+        rc = launch_gemm_tc(cur, m->merge_wb[l], nxt, Mc, N, K, me, st);
+      } else {
+        rc = merge();
+      }
+    } else {
+      rc = merge();
     }
-    m->ss_valid = merge_ss;
+    if (rc) return rc;
     h /= 2;
     w /= 2;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".merge", nxt, (int64_t)B * h * w * c.width[l + 1], st))) return rc;
+    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".merge", nxt, (int64_t)B * h * w * N, st))) return rc;
     cur = nxt;
   }
-  for (const LayerPlan& L : m->mid)
-    if ((rc = run_layer<T>(m, L, cur, B, h, w, pt, cond, cond_bs, ws, st))) return rc;
+  for (int i = 0; i < c.depth[n - 1]; ++i)
+    if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
   if ((rc = tap<T>(m, "mid", cur, (int64_t)B * h * w * c.width[n - 1], st))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     T* up = reinterpret_cast<T*>(ws.xup[l]);
@@ -512,31 +538,34 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     e.hc = h;
     e.wc = w;
     e.C = c.width[l];
-    m->ss_valid = std::is_same<T, bf16>::value && m->fuse_norm && tc_gemm_emits_rowss((int64_t)B * h * w, 4 * c.width[l], c.width[l + 1], e);
-    if (m->ss_valid) e.ss_out = ws.rowss;
+    f.produce(e, (int64_t)B * h * w, 4 * c.width[l], c.width[l + 1]);
     if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)B * h * w, 4 * c.width[l], c.width[l + 1], e, st))) return rc;
     h *= 2;
     w *= 2;
     if ((rc = tap<T>(m, "L" + std::to_string(l) + ".split", up, (int64_t)B * h * w * c.width[l], st))) return rc;
-    for (const LayerPlan& L : m->up[l])
-      if ((rc = run_layer<T>(m, L, up, B, h, w, pt, cond, cond_bs, ws, st))) return rc;
+    for (int i = 0; i < c.depth[l]; ++i)
+      if ((rc = run_layer<T>(m, f, k++, up, h, w))) return rc;
     if ((rc = tap<T>(m, "L" + std::to_string(l) + ".up", up, (int64_t)B * h * w * c.width[l], st))) return rc;
     cur = up;
   }
-  // the tensor-core epilogue reads x and writes out as float4: a view that starts inside a 16-byte granule (a storage offset, a
-  // caller's out= buffer) takes the scalar kernels instead
-  const bool po_aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sd <= 0.f || (reinterpret_cast<uintptr_t>(x) & 15) == 0);
-  if (std::is_same<T, bf16>::value && m->patch_out_wb != nullptr && po_aligned &&
-      tc_patch_out_supported(c.width[0], c.out_channels, c.patch_h, c.patch_w, W)) {
-    // out_norm as a row kernel, then the projection on the tensor core with un-patch + Karras combine in its epilogue
-    if (m->ss_valid && m->patch_out_wf != nullptr && c.width[0] % 128 == 0 && c.width[0] <= 128 * SS_PARTS)
-      return launch_patch_out_tc(reinterpret_cast<const bf16*>(cur), m->patch_out_wf, x, sigma, sd, out, B, H, W, c.width[0], st, ws.rowss);
-    T* xn = reinterpret_cast<T*>(ws.xn);
-    const int64_t M0 = (int64_t)B * h0 * w0;
-    if ((rc = launch_rmsnorm<T>(cur, xn, out_norm, 0, M0, M0, c.width[0], st))) return rc;
-    return launch_patch_out_tc(reinterpret_cast<const bf16*>(xn), m->patch_out_wb, x, sigma, sd, out, B, H, W, c.width[0], st);
+  // patch_out, routes in priority order (fp32 has only the last):
+  //   out_norm folded into the tensor-core projection, 1/rms from the row statistics
+  //   out_norm as a row kernel, then the tensor-core projection
+  //   the scalar kernel
+  // The tensor-core epilogue un-patches and applies the Karras combine; it reads x and writes out as float4, so a view that starts
+  // inside a 16-byte granule (a storage offset, a caller's out= buffer) takes the scalar kernel.
+  if constexpr (kBf16) {
+    const bool aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sd <= 0.f || (reinterpret_cast<uintptr_t>(x) & 15) == 0);
+    if (m->patch_out_wb != nullptr && aligned && tc_patch_out_supported(C0, c.out_channels, c.patch_h, c.patch_w, W)) {
+      if (f.stats && m->patch_out_wf != nullptr && C0 % 128 == 0 && C0 <= 128 * SS_PARTS)
+        return launch_patch_out_tc(cur, m->patch_out_wf, x, sigma, sd, out, B, H, W, C0, st, ws.rowss);
+      bf16* xn = reinterpret_cast<bf16*>(ws.xn);
+      const int64_t M0 = (int64_t)B * h0 * w0;
+      if ((rc = launch_rmsnorm<bf16>(cur, xn, m->out_norm, 0, M0, M0, C0, st))) return rc;
+      return launch_patch_out_tc(xn, m->patch_out_wb, x, sigma, sd, out, B, H, W, C0, st);
+    }
   }
-  return launch_patch_out<T>(cur, out_norm, patch_out_w, x, sigma, sd, out, B, c.out_channels, H, W, c.patch_h, c.patch_w, c.width[0], st);
+  return launch_patch_out<T>(cur, m->out_norm, m->patch_out_w, x, sigma, sd, out, B, c.out_channels, H, W, c.patch_h, c.patch_w, C0, st);
 }
 
 }  // namespace
@@ -583,56 +612,33 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->finalized = false;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, mw = c.mapping_width;
-  m->down.assign(n, {});
-  m->up.assign(n, {});
-  m->mid.clear();
+  m->layers.clear();
   m->merge_w.assign(n, nullptr);
   m->split_w.assign(n, nullptr);
   m->split_fac.assign(n, nullptr);
   m->merge_wb.assign(n, nullptr);
   m->split_wb.assign(n, nullptr);
-  int ada = 0, rc;
-  // conditioning row order == execution order: down levels, mid, up levels (outermost last)
-  for (int l = 0; l < n - 1; ++l) {
-    m->down[l].resize(c.depth[l]);
-    for (int i = 0; i < c.depth[l]; ++i) {
-      rc = plan_layer(m, m->down[l][i], "down_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i, &ada, st);
-      if (rc) return rc;
-    }
-  }
-  m->mid.resize(c.depth[n - 1]);
-  for (int i = 0; i < c.depth[n - 1]; ++i) {
-    rc = plan_layer(m, m->mid[i], "mid_level." + std::to_string(i) + ".", n - 1, i, &ada, st);
-    if (rc) return rc;
-  }
-  for (int l = n - 2; l >= 0; --l) {
-    m->up[l].resize(c.depth[l]);
-    for (int i = 0; i < c.depth[l]; ++i) {   // image_transformer_v2.py:697: up-level layer index continues after the down level
-      rc = plan_layer(m, m->up[l][i], "up_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i + c.depth[l], &ada, st);
-      if (rc) return rc;
-    }
-  }
+  int ada = 0, rc = 0;
+  // execution order; the layer index picks the shift (image_transformer_v2.py:697: an up level's index continues after its down level)
+  auto plan = [&](const std::string& prefix, int level, int index) {
+    m->layers.emplace_back();
+    return plan_layer(m, m->layers.back(), prefix, level, index, &ada, st);
+  };
+  for (int l = 0; l < n - 1; ++l)
+    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = plan("down_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i);
+  for (int i = 0; i < c.depth[n - 1] && rc == 0; ++i) rc = plan("mid_level." + std::to_string(i) + ".", n - 1, i);
+  for (int l = n - 2; l >= 0; --l)
+    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = plan("up_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i + c.depth[l]);
+  if (rc) return rc;
   m->ada_total = ada;
   {
-    int k = 0;
-    for (int l = 0; l < n - 1; ++l)
-      for (auto& L : m->down[l]) L.exec_index = k++;
-    for (auto& L : m->mid) L.exec_index = k++;
-    for (int l = n - 2; l >= 0; --l)
-      for (auto& L : m->up[l]) L.exec_index = k++;
-    m->n_layers = k;
     // table of (weights -> folded copy) pairs for the fused RMSNorm path
     std::vector<FoldDesc> descs;
-    auto add = [&](const LayerPlan& L) {
-      if (L.C % 8 != 0) return;
+    for (const LayerPlan& L : m->layers) {
+      if (L.C % 8 != 0) continue;
       if (L.qkv_wf != nullptr && L.ada_attn >= 0) descs.push_back(FoldDesc{L.qkv_wb, L.qkv_wf, 3 * L.C, L.C, L.ada_attn});
       if (L.up_wf != nullptr && L.up_wb_il != nullptr) descs.push_back(FoldDesc{L.up_wb_il, L.up_wf, 2 * L.dff, L.C, L.ada_ff});
-    };
-    for (int l = 0; l < n - 1; ++l)
-      for (auto& L : m->down[l]) add(L);
-    for (auto& L : m->mid) add(L);
-    for (int l = n - 2; l >= 0; --l)
-      for (auto& L : m->up[l]) add(L);
+    }
     m->n_fold = (int)descs.size();
     m->fold_descs = nullptr;
     if (!descs.empty()) {
@@ -650,37 +656,30 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     if ((rc = make_bf16(m, m->merge_w[l], 4LL * c.width[l] * c.width[l + 1], &m->merge_wb[l], st))) return rc;
     if ((rc = make_bf16(m, m->split_w[l], 4LL * c.width[l] * c.width[l + 1], &m->split_wb[l], st))) return rc;
   }
-  const float* tmp = nullptr;
-  GET("patch_in.proj.weight", &tmp, c.width[0], (int64_t)c.patch_h * c.patch_w * c.in_channels);
-  GET("out_norm.scale", &tmp, c.width[0]);
-  GET("patch_out.proj.weight", &tmp, (int64_t)c.patch_h * c.patch_w * c.out_channels, c.width[0]);
+  const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels;
+  GET("patch_in.proj.weight", &m->patch_in_w, C0, (int64_t)c.patch_h * c.patch_w * c.in_channels);
+  GET("out_norm.scale", &m->out_norm, C0);
+  GET("patch_out.proj.weight", &m->patch_out_w, Np, C0);
 
   m->patch_in_wb = nullptr;
-  if (c.in_channels == 3 && c.patch_h == 4 && c.patch_w == 4 && c.width[0] % 128 == 0) {
-    const float* piw = nullptr;
-    GET("patch_in.proj.weight", &piw, c.width[0], (int64_t)48);
-    if ((rc = dev_alloc(m, &m->patch_in_wb, (size_t)c.width[0] * 64))) return rc;
-    if ((rc = prepare_patch_in_weight(piw, m->patch_in_wb, c.width[0], st))) return rc;
+  if (c.in_channels == 3 && c.patch_h == 4 && c.patch_w == 4 && C0 % 128 == 0) {
+    if ((rc = dev_alloc(m, &m->patch_in_wb, (size_t)C0 * 64))) return rc;
+    if ((rc = prepare_patch_in_weight(m->patch_in_w, m->patch_in_wb, C0, st))) return rc;
   }
-  {   // zero-padded bf16 patch_out weight [64, C0]
-    const int Np = c.patch_h * c.patch_w * c.out_channels, C0 = c.width[0];
-    m->patch_out_wb = nullptr;
-    if (Np <= 64) {
-      if ((rc = dev_alloc(m, &m->patch_out_wb, (size_t)64 * C0))) return rc;
-      KDB_CUDA(cudaMemsetAsync(m->patch_out_wb, 0, (size_t)64 * C0 * sizeof(bf16), st));
-      if ((rc = launch_f32_to_bf16(tmp, m->patch_out_wb, (int64_t)Np * C0, st))) return rc;
-      m->patch_out_wf = nullptr;
-      if (C0 % 8 == 0) {   // out_norm.scale is a plain parameter: fold it once
-        const float* out_scale = nullptr;
-        GET("out_norm.scale", &out_scale, C0);
-        FoldDesc* d1 = nullptr;
-        if ((rc = dev_alloc(m, &m->patch_out_wf, (size_t)64 * C0))) return rc;
-        if ((rc = dev_alloc(m, &d1, 1))) return rc;
-        const FoldDesc hd{m->patch_out_wb, m->patch_out_wf, 64, C0, 0};
-        KDB_CUDA(cudaMemcpyAsync(d1, &hd, sizeof(FoldDesc), cudaMemcpyHostToDevice, st));
-        if ((rc = launch_fold_norm_weights(d1, 1, out_scale, st))) return rc;
-        KDB_CUDA(cudaStreamSynchronize(st));
-      }
+  m->patch_out_wb = nullptr;
+  m->patch_out_wf = nullptr;
+  if (Np <= 64) {   // zero-padded bf16 patch_out weight [64, C0]
+    if ((rc = dev_alloc(m, &m->patch_out_wb, (size_t)64 * C0))) return rc;
+    KDB_CUDA(cudaMemsetAsync(m->patch_out_wb, 0, (size_t)64 * C0 * sizeof(bf16), st));
+    if ((rc = launch_f32_to_bf16(m->patch_out_w, m->patch_out_wb, (int64_t)Np * C0, st))) return rc;
+    if (C0 % 8 == 0) {   // out_norm.scale is a plain parameter: fold it once
+      FoldDesc* d1 = nullptr;
+      if ((rc = dev_alloc(m, &m->patch_out_wf, (size_t)64 * C0))) return rc;
+      if ((rc = dev_alloc(m, &d1, 1))) return rc;
+      const FoldDesc hd{m->patch_out_wb, m->patch_out_wf, 64, C0, 0};
+      KDB_CUDA(cudaMemcpyAsync(d1, &hd, sizeof(FoldDesc), cudaMemcpyHostToDevice, st));
+      if ((rc = launch_fold_norm_weights(d1, 1, m->out_norm, st))) return rc;
+      KDB_CUDA(cudaStreamSynchronize(st));
     }
   }
   // conditioning weights
@@ -708,20 +707,11 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   }
   // concatenated AdaRMSNorm projection [ada_total, mw]
   if ((rc = dev_alloc(m, &m->ada_cat, (size_t)ada * mw))) return rc;
-  auto put = [&](const LayerPlan& L) -> int {
+  for (const LayerPlan& L : m->layers) {
     if (L.ada_attn >= 0)
       KDB_CUDA(cudaMemcpyAsync(m->ada_cat + (size_t)L.ada_attn * mw, L.attn_norm_w, sizeof(float) * L.C * mw, cudaMemcpyDeviceToDevice, st));
     KDB_CUDA(cudaMemcpyAsync(m->ada_cat + (size_t)L.ada_ff * mw, L.ff_norm_w, sizeof(float) * L.C * mw, cudaMemcpyDeviceToDevice, st));
-    return 0;
-  };
-  for (auto& lv : m->down)
-    for (auto& L : lv)
-      if ((rc = put(L))) return rc;
-  for (auto& L : m->mid)
-    if ((rc = put(L))) return rc;
-  for (auto& lv : m->up)
-    for (auto& L : lv)
-      if ((rc = put(L))) return rc;
+  }
   w.ada_cat = m->ada_cat;
   KDB_CUDA(cudaStreamSynchronize(st));
   m->finalized = true;

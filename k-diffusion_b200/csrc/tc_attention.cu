@@ -49,10 +49,6 @@ struct Bars {
   uint64_t q, kv, kv_free;
 };
 
-__device__ __forceinline__ uint32_t p_offset(int row, int chunk16) {   // byte offset of 16-byte chunk `chunk16` (0..7) of `row` in a K-major SW128 tile
-  return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk16 ^ (row & 7)) << 4));
-}
-
 template <int MODE, bool BOUNDED>
 __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
                                                          const AttnParams p) {
@@ -237,7 +233,7 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
         uint8_t* pt = sP + (c >> 1) * TILE_BYTES;
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj)
-          *reinterpret_cast<uint4*>(pt + p_offset(row, (c & 1) * 4 + jj)) = make_uint4(pk[jj * 4], pk[jj * 4 + 1], pk[jj * 4 + 2], pk[jj * 4 + 3]);
+          *reinterpret_cast<uint4*>(pt + tc::sw128_offset(row, (c & 1) * 4 + jj)) = make_uint4(pk[jj * 4], pk[jj * 4 + 1], pk[jj * 4 + 2], pk[jj * 4 + 3]);
       }
     } else {
       // WINDOW: own head's 64 key columns live at [64*hd, 64*hd+64); the other head's block is garbage -> zeros in P
@@ -283,8 +279,8 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
           tc::unpack_bf16x2(pk[t], q0, q1);
           l += q0 + q1;
         }
-        *reinterpret_cast<uint4*>(own + p_offset(row, jj)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        *reinterpret_cast<uint4*>(other + p_offset(row, jj)) = make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(own + tc::sw128_offset(row, jj)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+        *reinterpret_cast<uint4*>(other + tc::sw128_offset(row, jj)) = make_uint4(0u, 0u, 0u, 0u);
       }
     }
     if (pass == 1) {
@@ -367,7 +363,6 @@ bool tc_attention_supported(int h, int w, int nh, int e, int attn_type, int attn
   return false;
 }
 
-// programmatic dependent launch: barrier init overlaps the tail of the qkv projection (KDB200_NO_PDL=1 disables)
 template <int MODE>
 static cudaError_t set_attn_smem(size_t smem) {
   cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel<MODE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -375,24 +370,11 @@ static cudaError_t set_attn_smem(size_t smem) {
   return cudaFuncSetAttribute(attn_tc_kernel<MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 }
 
+// programmatic dependent launch: barrier init overlaps the tail of the qkv projection
 template <int MODE>
 static cudaError_t launch_attn(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tkv, const AttnParams& p) {
-  static const bool no_pdl = [] {
-    const char* e = getenv("KDB200_NO_PDL");
-    return e != nullptr && e[0] == '1';
-  }();
-  cudaLaunchConfig_t lc{};
-  lc.gridDim = grid;
-  lc.blockDim = dim3(160);
-  lc.dynamicSmemBytes = smem;
-  lc.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = attr;
-  lc.numAttrs = no_pdl ? 0 : 1;
-  if (p.bound != nullptr) return cudaLaunchKernelEx(&lc, attn_tc_kernel<MODE, true>, tq, tkv, p);
-  return cudaLaunchKernelEx(&lc, attn_tc_kernel<MODE, false>, tq, tkv, p);
+  if (p.bound != nullptr) return launch_pdl(attn_tc_kernel<MODE, true>, grid, dim3(160), smem, st, tq, tkv, p);
+  return launch_pdl(attn_tc_kernel<MODE, false>, grid, dim3(160), smem, st, tq, tkv, p);
 }
 
 int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh, int e, int attn_type, int attn_param, int shift,

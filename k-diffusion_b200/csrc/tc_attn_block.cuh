@@ -424,23 +424,10 @@ int launch_attn_block_impl(bf16* x, const bf16* w_qkv, const bf16* w_out, const 
     KDB_CUDA(cudaFuncSetAttribute(gemm_wg_attn_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AB_SMEM));
     attr_set = true;
   }
-  static const bool no_pdl = [] {
-    const char* e = getenv("KDB200_NO_PDL");
-    return e != nullptr && e[0] == '1';
-  }();
   AttnBlockParams p{ss_in, ss_out, reinterpret_cast<const float4*>(rope), qk_scale, h, w, shift, B * (h / 8) * (w / 8)};
   const int n_tiles = (p.nwin + 1) / 2;
-  cudaLaunchConfig_t lc{};
-  lc.gridDim = dim3((unsigned)(n_tiles < num_sms() ? n_tiles : num_sms()));
-  lc.blockDim = dim3(AB_THREADS);
-  lc.dynamicSmemBytes = AB_SMEM;
-  lc.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = attr;
-  lc.numAttrs = no_pdl ? 0 : 1;
-  KDB_CUDA(cudaLaunchKernelEx(&lc, gemm_wg_attn_block_kernel, tx, twq, two, p));
+  KDB_CUDA(launch_pdl(gemm_wg_attn_block_kernel, dim3((unsigned)(n_tiles < num_sms() ? n_tiles : num_sms())), dim3(AB_THREADS), AB_SMEM, st,
+                      tx, twq, two, p));
   KDB_LAUNCH_CHECK(F_GEMM_TC, st);
   return 0;
 }

@@ -74,45 +74,6 @@ __device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity)
     if ((++spins & 63u) == 0 && globaltimer_ns() - t0 > 2000000000ull) __trap();
 }
 
-// Wait of a SINGLE-THREAD role (TMA producer, MMA issuer): the parked wait above goes to sleep (NANOSLEEP.SYNCS) when the phase is not
-// complete yet and pays the wake-up on the hand-off's critical path; a lone thread that polls costs no other warp an issue slot worth
-// having.  KDB_SPIN_ROLES: 0 = parked waits everywhere (default), 1 = the single-thread roles poll, 2 = also the epilogue groups'
-// accumulator waits.
-// Bounded like mbar_wait.
-#ifndef KDB_SPIN_ROLES
-#define KDB_SPIN_ROLES 0
-#endif
-__device__ __forceinline__ bool mbar_try_wait_nohint(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait_nohint(bar, parity)) return;
-  const uint64_t t0 = globaltimer_ns();
-  uint32_t spins = 0;
-  while (!mbar_try_wait_nohint(bar, parity)) {
-    if ((++spins & 1023u) == 0 && globaltimer_ns() - t0 > 2000000000ull) {
-      printf("libkdb200: mbarrier wait timed out (block %d,%d,%d thread %d parity %u)\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void mbar_wait_role(uint64_t* bar, uint32_t parity) {
-  if (KDB_SPIN_ROLES >= 1) mbar_wait_spin(bar, parity);
-  else mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void mbar_wait_group(uint64_t* bar, uint32_t parity) {
-  if (KDB_SPIN_ROLES >= 2) mbar_wait_spin(bar, parity);
-  else mbar_wait(bar, parity);
-}
-
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -142,11 +103,6 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
                "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
                : "memory");
 }
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
@@ -160,7 +116,6 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read_le1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // byte offset of 16-byte chunk `chunk16` (0..7) of `row` inside a [rows x 128 B] SWIZZLE_128B tile (what TMA / UMMA expect)
@@ -257,23 +212,10 @@ __device__ __forceinline__ void acc_ld32(const float* s, int ld, int row, int co
   }
 }
 
-// 2^x on the MUFU unit, flush-to-zero: for softmax terms (x <= ~0; results below 2^-126 are irrelevant)
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-// GELU in the tanh form on the MUFU tanh unit (6 instructions).  |gelu_tanh - gelu_erf| <= 5e-4 absolute, i.e. below one
-// bf16 ulp wherever the output magnitude exceeds 0.07 -- used only on the bf16 fast path; the fp32 path keeps erff.
-__device__ __forceinline__ float gelu_fast(float x) {
-  const float u = x * fmaf(0.0356774081f, x * x, 0.7978845608f);     // sqrt(2/pi) (x + 0.044715 x^3)
-  return x * fmaf(0.5f, tanh_approx(u), 0.5f);
 }
 
 // fused RMSNorm: sum of the first `parts` (1..8) per-128-channel slots of one row-statistics record.  Exactly `parts` slots are
@@ -299,8 +241,9 @@ __device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
 __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return f32x2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
 __device__ __forceinline__ f32x2 neg2(f32x2 a) { return f32x2{-a.x, -a.y}; }
-// (2 * half_val) * gelu_fast(gate) for two (value, gate) pairs; `half_val` = 0.5 * value (the caller folds the 0.5 into the
-// row scale it applies anyway):  val * gate * (0.5 + 0.5 t) = w + w t  with w = half_val * gate  -> 5 packed instructions + 2 MUFU
+// (2 * half_val) * gelu_tanh(gate) for two (value, gate) pairs, GELU in the tanh form on the MUFU tanh unit: |gelu_tanh - gelu_erf|
+// <= 5e-4 absolute, below one bf16 ulp wherever the output magnitude exceeds 0.07 -- used only on the bf16 fast path; the fp32
+// path keeps erff.  `half_val` = 0.5 * value (the caller folds the 0.5 into the row scale it applies anyway):  val * gate * (0.5 + 0.5 t) = w + w t  with w = half_val * gate  -> 5 packed instructions + 2 MUFU
 __device__ __forceinline__ f32x2 geglu2(f32x2 half_val, f32x2 gate) {
   const f32x2 c1 = pk2(0.0356774081f, 0.0356774081f), c0 = pk2(0.7978845608f, 0.7978845608f);
   const f32x2 u = mul2(gate, fma2(c1, mul2(gate, gate), c0));
@@ -349,5 +292,24 @@ __device__ __forceinline__ void unpack_bf16x2(uint32_t v, float& lo, float& hi) 
 // 2-D..4-D bf16 tensor map with 128B swizzle; dims/strides innermost first (strides in bytes, for dims 1..rank-1).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box);
+
+// ---------------------------------------------------------------- host: programmatic dependent launch
+// Launches `kernel` with programmatic stream serialization, so that its prologue overlaps the tail of the previous kernel in the
+// stream (the kernel calls pdl_wait() before it reads that kernel's output).  In plain stream order when pdl_enabled() is false.
+bool pdl_enabled();
+template <typename... Params, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t lc{};
+  lc.gridDim = grid;
+  lc.blockDim = block;
+  lc.dynamicSmemBytes = smem;
+  lc.stream = st;
+  lc.attrs = attr;
+  lc.numAttrs = pdl_enabled() ? 1 : 0;
+  return cudaLaunchKernelEx(&lc, kernel, args...);
+}
 
 }  // namespace kdb

@@ -240,23 +240,10 @@ int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int6
     KDB_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
     attr_set = true;
   }
-  static const bool no_pdl = [] {
-    const char* e = getenv("KDB200_NO_PDL");
-    return e != nullptr && e[0] == '1';
-  }();
   FfnParams p{ss_in, ss_out, M, dff / FF_CH};
   const int64_t m_tiles = M / BM;
-  cudaLaunchConfig_t lc{};
-  lc.gridDim = dim3((unsigned)(m_tiles < num_sms() ? m_tiles : num_sms()));
-  lc.blockDim = dim3(FF_THREADS);
-  lc.dynamicSmemBytes = FF_SMEM;
-  lc.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = attr;
-  lc.numAttrs = no_pdl ? 0 : 1;
-  KDB_CUDA(cudaLaunchKernelEx(&lc, ffn_fused_kernel, tx, twu, twd, to, p));
+  KDB_CUDA(launch_pdl(ffn_fused_kernel, dim3((unsigned)(m_tiles < num_sms() ? m_tiles : num_sms())), dim3(FF_THREADS), FF_SMEM, st, tx, twu,
+                      twd, to, p));
   KDB_LAUNCH_CHECK(F_GEMM_TC, st);
   return 0;
 }

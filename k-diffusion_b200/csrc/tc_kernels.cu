@@ -52,6 +52,15 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return 0;
 }
 
+// programmatic dependent launch for every kernel launched with launch_pdl, unless the switch below is 1 (read once, at the first launch)
+bool pdl_enabled() {
+  static const bool enabled = [] {
+    const char* e = getenv("KDB200_NO_PDL");
+    return !(e != nullptr && e[0] == '1');
+  }();
+  return enabled;
+}
+
 // ------------------------------------------------------------------------------------------------
 // GEMM
 // ------------------------------------------------------------------------------------------------

@@ -61,7 +61,7 @@ def bf(t):
 
 
 def gelu_tanh(x):
-    """the tanh form of GELU that the tensor-core GEGLU epilogues evaluate (tc_common.cuh gelu_fast)"""
+    """the tanh form of GELU that the tensor-core GEGLU epilogues evaluate (tc_common.cuh geglu2)"""
     return 0.5 * x * (1.0 + torch.tanh(0.7978845608 * (x + 0.044715 * x ** 3)))
 
 

@@ -10,6 +10,7 @@ GEMMs (fold kernel + row statistics), launches enqueued behind a gate kernel so 
 """
 import argparse
 import json
+import os
 import sys
 from pathlib import Path
 
@@ -22,34 +23,6 @@ import torch
 
 import k_diffusion as K
 from k_diffusion import _native
-
-
-def gemm_sequence(mcfg, B):
-    """(label, M, N, K) of every Linear in execution order (matches engine.cu run order)."""
-    widths, depths, d_ffs, attns = mcfg["widths"], mcfg["depths"], mcfg["d_ffs"], mcfg["self_attns"]
-    t0 = (mcfg["input_size"][0] // mcfg["patch_size"][0]) * (mcfg["input_size"][1] // mcfg["patch_size"][1])
-    n = len(widths)
-    seq = []
-
-    def layer(l, tag):
-        M, C, F = B * (t0 >> (2 * l)), widths[l], d_ffs[l]
-        if attns[l]["type"] != "none":
-            seq.append((f"{tag} qkv", M, 3 * C, C))
-            seq.append((f"{tag} out+res", M, C, C))
-        seq.append((f"{tag} up+geglu", M, 2 * F, C))
-        seq.append((f"{tag} down+res", M, C, F))
-
-    for l in range(n - 1):
-        for i in range(depths[l]):
-            layer(l, f"L{l}.down{i}")
-        seq.append((f"merge{l}", B * (t0 >> (2 * l + 2)), widths[l + 1], 4 * widths[l]))
-    for i in range(depths[-1]):
-        layer(n - 1, f"mid{i}")
-    for l in reversed(range(n - 1)):
-        seq.append((f"split{l}", B * (t0 >> (2 * l + 2)), 4 * widths[l], widths[l + 1]))
-        for i in range(depths[l]):
-            layer(l, f"L{l}.up{i}")
-    return seq
 
 
 def main():
@@ -87,17 +60,15 @@ def main():
     with _native.profile(gate_ms=10.0 * args.repeat) as prof:
         for _ in range(args.repeat):
             evaluate()
-    import os
-    seq = [(lab, M, N, Kd) for lab, M, N, Kd, _ in K.models.flops.launch_layers(cfg["model"], args.batch, os.environ.get("KDB200_NO_FFN_FUSE", "0") != "1")]
-    macs = {i: m for i, (_, _, _, _, m) in enumerate(K.models.flops.launch_layers(cfg["model"], args.batch, os.environ.get("KDB200_NO_FFN_FUSE", "0") != "1"))}
+    seq = K.models.flops.launch_layers(cfg["model"], args.batch, os.environ.get("KDB200_NO_FFN_FUSE", "0") != "1")
     gi = 0
     rows = []
     peak = 1396.9
     for fam, ms in prof.launches:
         note = ""
         if fam.startswith("gemm"):
-            label, M, N, Kd = seq[gi % len(seq)]
-            tf = 2.0 * macs[gi % len(seq)] / (ms * 1e-3) / 1e12
+            label, M, N, Kd, macs = seq[gi % len(seq)]
+            tf = 2.0 * macs / (ms * 1e-3) / 1e12
             gi += 1
             gb = 2.0 * (M * Kd + N * Kd + M * (N if "geglu" not in label else N // 2) + (M * N if "res" in label else 0)) / (ms * 1e-3) / 1e9
             note = f"{label:18s} M={M:6d} N={N:5d} K={Kd:5d}  {tf:7.1f} TFLOP/s ({tf / peak:5.1%})  min-traffic {gb:7.0f} GB/s"
