@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 8
+#define KDB_ABI_VERSION 9
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -192,6 +192,18 @@ int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int wid
                       const float* x, const float* sigma, float sigma_data,
                       const float* cond, int64_t cond_batch_stride, float* out,
                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* Forward-mode derivative (JVP) of the same evaluation along v [B, C_in, H, W]: out = D(x, sigma) as kdb_model_forward computes it at
+ * KDB_PREC_FP32 (bit for bit), out_tangent = J_D(x) v = c_skip v + c_out J_F(c_in x) c_in v (sigma_data > 0) or J_F(x) v (sigma_data <= 0).
+ * The derivative is taken with respect to x only (sigma and the conditioning are held fixed).  fp32 only: any other precision returns
+ * KDB_ERR_UNSUPPORTED.  The tangent rides through the engine as images [B, 2B) of every token buffer, so the workspace must hold
+ * kdb_model_workspace_bytes(m, KDB_PREC_FP32, 2 * batch, height, width) bytes.  cond / cond_batch_stride as for kdb_model_forward:
+ * tangent image b uses the conditioning row of image b.  Armed debug taps receive the primal rows followed by the tangent rows.  Same
+ * stream, allocation and CUDA-graph rules as kdb_model_forward. */
+int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int width,
+                          const float* x, const float* v, const float* sigma, float sigma_data,
+                          const float* cond, int64_t cond_batch_stride, float* out, float* out_tangent,
+                          void* workspace, size_t workspace_bytes, void* stream);
 
 /* Debug/parity tap: arm a copy of one intermediate of the NEXT forward into `out` (fp32, device).
  * name: "patch_in", "L<l>.down", "L<l>.merge", "mid", "L<l>.split", "L<l>.up", "layer<k>.xn1",

@@ -339,6 +339,10 @@ struct Fwd {
   bool emit;                // bf16 with fused RMSNorm: producers leave the row statistics of what they write where their shape allows
   bool fold;                // emit, one shared conditioning row and a fold table: consumers take the weights with the norm scale folded in
   bool stats;               // ws.rowss holds the row statistics of the current residual stream
+  bool jvp;                 // fp32 forward-mode derivative: images [B, 2B) of every token buffer carry the tangent of images [0, B)
+
+  // images held by the token buffers: linear launches and taps cover them all, nonlinear primal launches the first B
+  int images() const { return jvp ? 2 * B : B; }
 
   // a RESID / SPLIT_LERP / merge GEMM is about to write the residual stream: it leaves its row statistics if it can
   void produce(GemmEpi& e, int64_t M, int N, int K) {
@@ -352,7 +356,8 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   const LayerPlan& L = m->layers[k];
   const float* pos = f.pt->pos[L.level];
   const float2* rope = f.pt->rope[k];
-  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok;
+  // M: primal token rows; Ma: every row of the token buffers (the tangent rows [M, 2M) follow on a JVP forward)
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok, Ma = (int64_t)f.images() * Ttok;
   const int C = L.C;
   T* xn = reinterpret_cast<T*>(f.ws.xn);
   T* qkv = reinterpret_cast<T*>(f.ws.qkv);
@@ -374,11 +379,16 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     qf.ss_in = f.ws.rowss;
     auto norm = [&] {
       int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
-      return r ? r : tap<T>(m, tag + ".xn1", xn, M * C, f.st);
+      if constexpr (std::is_same_v<T, float>)
+        if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
+      return r ? r : tap<T>(m, tag + ".xn1", xn, Ma * C, f.st);
     };
     auto unfused = [&] {
       int r = norm();
-      if (!r) r = linear<T>(xn, WSel<T>::qkv(L), qkv, M, 3 * C, C, GemmEpi{}, f.st);
+      if (!r) r = linear<T>(xn, WSel<T>::qkv(L), qkv, Ma, 3 * C, C, GemmEpi{}, f.st);
+      // the tangent reads the un-normalised primal q and k, so it runs before the in-place primal launch
+      if constexpr (std::is_same_v<T, float>)
+        if (!r && f.jvp) r = launch_qknorm_rope_jvp(qkv, qkv + M * 3 * C, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
       return r ? r : launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
     };
     // attention, routes in priority order (fp32 has only the last):
@@ -406,23 +416,31 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     }
     if (rc) return rc;
     if (!block) {
-      if ((rc = tap<T>(m, tag + ".qkv", qkv, M * 3 * C, f.st))) return rc;
+      if ((rc = tap<T>(m, tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
       // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
       if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
         return rc;
-      if ((rc = tap<T>(m, tag + ".ao", ao, M * C, f.st))) return rc;
+      if constexpr (std::is_same_v<T, float>)
+        if (f.jvp && (rc = launch_attention_jvp(qkv, qkv + M * 3 * C, ao + M * C, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st)))
+          return rc;
+      if ((rc = tap<T>(m, tag + ".ao", ao, Ma * C, f.st))) return rc;
       GemmEpi e;
       e.mode = EPI_RESID;
       e.resid = x;
-      f.produce(e, M, C, C);
-      if ((rc = linear<T>(ao, WSel<T>::out(L), x, M, C, C, e, f.st))) return rc;
+      f.produce(e, Ma, C, C);
+      if ((rc = linear<T>(ao, WSel<T>::out(L), x, Ma, C, C, e, f.st))) return rc;
     }
-    if ((rc = tap<T>(m, tag + ".attn", x, M * C, f.st))) return rc;
+    if ((rc = tap<T>(m, tag + ".attn", x, Ma * C, f.st))) return rc;
   }
   auto unfused = [&] {
     int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-    if (!r) r = linear<T>(xn, WSel<T>::up(L), hb, M, 2 * L.dff, C, GemmEpi{}, f.st);
-    return r ? r : launch_geglu<T>(hb, gb, M, L.dff, f.st);
+    if constexpr (std::is_same_v<T, float>)
+      if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
+    if (!r) r = linear<T>(xn, WSel<T>::up(L), hb, Ma, 2 * L.dff, C, GemmEpi{}, f.st);
+    if (!r) r = launch_geglu<T>(hb, gb, M, L.dff, f.st);
+    if constexpr (std::is_same_v<T, float>)
+      if (!r && f.jvp) r = launch_geglu_jvp(hb, hb + M * 2 * L.dff, gb + M * L.dff, M, L.dff, f.st);
+    return r;
   };
   // feed-forward, routes in priority order (fp32 has only the last):
   //   ffn_fused: the whole half in one kernel (128-wide levels; not while .geglu is tapped)
@@ -448,19 +466,22 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   }
   if (rc) return rc;
   if (!ffn) {
-    if ((rc = tap<T>(m, tag + ".geglu", gb, M * L.dff, f.st))) return rc;
+    if ((rc = tap<T>(m, tag + ".geglu", gb, Ma * L.dff, f.st))) return rc;
     GemmEpi e;
     e.mode = EPI_RESID;
     e.resid = x;
-    f.produce(e, M, C, L.dff);
-    if ((rc = linear<T>(gb, WSel<T>::down(L), x, M, C, L.dff, e, f.st))) return rc;
+    f.produce(e, Ma, C, L.dff);
+    if ((rc = linear<T>(gb, WSel<T>::down(L), x, Ma, C, L.dff, e, f.st))) return rc;
   }
-  return tap<T>(m, tag + ".ff", x, M * C, f.st);
+  return tap<T>(m, tag + ".ff", x, Ma * C, f.st);
 }
 
+// v != nullptr (fp32 only): forward-mode derivative along v, the tangent D'(x) v goes to out_t.  The primal launches are those of a
+// plain forward of B images; the linear ones run over the tangent images as well (the SIMT GEMM's per-row arithmetic does not depend
+// on M), each nonlinear one is followed by its tangent kernel.
 template <typename T>
-int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cond_bs,
-                 float* out, Workspace& ws, cudaStream_t st) {
+int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
+                 int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st) {
   constexpr bool kBf16 = std::is_same_v<T, bf16>;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
@@ -469,13 +490,18 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   int rc = ensure_pos(m, h0, w0, st, &pt);
   if (rc) return rc;
   m->tap_count = 0;
-  Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false};
+  Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false, !kBf16 && v != nullptr};
   f.fold = f.emit && cond_bs == 0 && m->fold_descs != nullptr;
   if (f.fold && (rc = launch_fold_norm_weights(m->fold_descs, m->n_fold, cond, st))) return rc;
+  const int Bt = f.images();
 
   T* cur = reinterpret_cast<T*>(ws.xs[0]);
   auto patch_in = [&] {
-    return launch_patch_in<T>(x, sigma, sd, m->patch_in_w, cur, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
+    int r = launch_patch_in<T>(x, sigma, sd, m->patch_in_w, cur, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
+    // c_in x is linear in x: the tangent images are patch_in of v with the same sigma
+    if (!r && f.jvp)
+      r = launch_patch_in<T>(v, sigma, sd, m->patch_in_w, cur + (int64_t)B * h0 * w0 * C0, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
+    return r;
   };
   // patch_in: on the tensor core, which leaves the row statistics for the first fused RMSNorm, or the scalar kernel
   if constexpr (kBf16) {
@@ -489,20 +515,20 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   } else {
     rc = patch_in();
   }
-  if (rc || (rc = tap<T>(m, "patch_in", cur, (int64_t)B * h0 * w0 * C0, st))) return rc;
+  if (rc || (rc = tap<T>(m, "patch_in", cur, (int64_t)Bt * h0 * w0 * C0, st))) return rc;
 
   int k = 0, h = h0, w = w0;
   for (int l = 0; l < n - 1; ++l) {
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".down", cur, (int64_t)B * h * w * c.width[l], st))) return rc;
+    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".down", cur, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     T* nxt = reinterpret_cast<T*>(ws.xs[l + 1]);
-    const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
+    const int64_t Mc = (int64_t)Bt * (h / 2) * (w / 2);
     const int N = c.width[l + 1], K = 4 * c.width[l];
     auto merge = [&] {
       T* mg = reinterpret_cast<T*>(ws.mg);
       f.stats = false;
-      int r = launch_merge_gather<T>(cur, mg, B, h, w, c.width[l], st);
+      int r = launch_merge_gather<T>(cur, mg, Bt, h, w, c.width[l], st);
       return r ? r : linear<T>(mg, WSel<T>::merge(m, l), nxt, Mc, N, K, GemmEpi{}, st);
     };
     // TokenMerge: the 2x2 gather rides on the GEMM's TMA loads when the geometry allows, else a gather kernel and a plain GEMM
@@ -523,12 +549,12 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     if (rc) return rc;
     h /= 2;
     w /= 2;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".merge", nxt, (int64_t)B * h * w * N, st))) return rc;
+    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".merge", nxt, (int64_t)Bt * h * w * N, st))) return rc;
     cur = nxt;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
     if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
-  if ((rc = tap<T>(m, "mid", cur, (int64_t)B * h * w * c.width[n - 1], st))) return rc;
+  if ((rc = tap<T>(m, "mid", cur, (int64_t)Bt * h * w * c.width[n - 1], st))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     T* up = reinterpret_cast<T*>(ws.xup[l]);
     GemmEpi e;
@@ -538,14 +564,14 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     e.hc = h;
     e.wc = w;
     e.C = c.width[l];
-    f.produce(e, (int64_t)B * h * w, 4 * c.width[l], c.width[l + 1]);
-    if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)B * h * w, 4 * c.width[l], c.width[l + 1], e, st))) return rc;
+    f.produce(e, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1]);
+    if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], e, st))) return rc;
     h *= 2;
     w *= 2;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".split", up, (int64_t)B * h * w * c.width[l], st))) return rc;
+    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".split", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = run_layer<T>(m, f, k++, up, h, w))) return rc;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".up", up, (int64_t)B * h * w * c.width[l], st))) return rc;
+    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".up", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     cur = up;
   }
   // patch_out, routes in priority order (fp32 has only the last):
@@ -565,7 +591,12 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       return launch_patch_out_tc(xn, m->patch_out_wb, x, sigma, sd, out, B, H, W, C0, st);
     }
   }
-  return launch_patch_out<T>(cur, m->out_norm, m->patch_out_w, x, sigma, sd, out, B, c.out_channels, H, W, c.patch_h, c.patch_w, C0, st);
+  rc = launch_patch_out<T>(cur, m->out_norm, m->patch_out_w, x, sigma, sd, out, B, c.out_channels, H, W, c.patch_h, c.patch_w, C0, st);
+  if constexpr (!kBf16)
+    if (!rc && f.jvp)
+      rc = launch_patch_out_jvp(cur, cur + (int64_t)B * h0 * w0 * C0, m->out_norm, m->patch_out_w, v, sigma, sd, out_t, B, c.out_channels, H, W,
+                                c.patch_h, c.patch_w, C0, st);
+  return rc;
 }
 
 }  // namespace
@@ -742,27 +773,68 @@ size_t kdb_model_workspace_bytes(const KdbModel* m, int precision, int batch, in
   return ws.total;
 }
 
+}  // extern "C"
+
+namespace {
+
+// image geometry and preconditioning checks shared by the forward entry points
+int check_image(const KdbModel* m, const char* what, int height, int width, float sigma_data) {
+  const KdbModelConfig& c = m->cfg;
+  KDB_REQUIRE(height % c.patch_h == 0 && width % c.patch_w == 0, KDB_ERR_BAD_SHAPE, "%s: %dx%d not divisible by the patch size", what, height,
+              width);
+  const int div = 1 << (c.n_levels - 1);
+  KDB_REQUIRE((height / c.patch_h) % div == 0 && (width / c.patch_w) % div == 0, KDB_ERR_BAD_SHAPE,
+              "%s: token grid %dx%d not divisible by 2^(levels-1)", what, height / c.patch_h, width / c.patch_w);
+  KDB_REQUIRE(!(sigma_data > 0.f && c.in_channels != c.out_channels), KDB_ERR_BAD_ARG, "%s: preconditioning needs C_in == C_out", what);
+  return 0;
+}
+
+// carve a workspace of `images` token-stream images out of the caller's buffer
+int carve_checked(const KdbModel* m, const char* what, int precision, int images, int height, int width, void* workspace, size_t workspace_bytes,
+                  Workspace& ws) {
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 1024));
+  carve(m->cfg, precision, images, height, width, base, ws);
+  KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "%s: workspace %zu < required %zu", what, workspace_bytes, ws.total);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
 int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
                       float sigma_data, const float* cond, int64_t cond_batch_stride, float* out, void* workspace,
                       size_t workspace_bytes, void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward: model not finalized");
   KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward: NULL argument");
   KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_BF16, KDB_ERR_BAD_ARG, "forward: bad precision %d", precision);
-  const KdbModelConfig& c = m->cfg;
-  KDB_REQUIRE(height % c.patch_h == 0 && width % c.patch_w == 0, KDB_ERR_BAD_SHAPE, "forward: %dx%d not divisible by the patch size", height, width);
-  const int div = 1 << (c.n_levels - 1);
-  KDB_REQUIRE((height / c.patch_h) % div == 0 && (width / c.patch_w) % div == 0, KDB_ERR_BAD_SHAPE,
-              "forward: token grid %dx%d not divisible by 2^(levels-1)", height / c.patch_h, width / c.patch_w);
-  KDB_REQUIRE(!(sigma_data > 0.f && c.in_channels != c.out_channels), KDB_ERR_BAD_ARG, "forward: preconditioning needs C_in == C_out");
+  int rc = check_image(m, "forward", height, width, sigma_data);
+  if (rc) return rc;
   Workspace ws;
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 1024));
-  carve(c, precision, batch, height, width, base, ws);
-  KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward: workspace %zu < required %zu", workspace_bytes, ws.total);
-  int rc;
+  if ((rc = carve_checked(m, "forward", precision, batch, height, width, workspace, workspace_bytes, ws))) return rc;
   if (precision == KDB_PREC_FP32)
-    rc = forward_impl<float>(m, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream);
+    rc = forward_impl<float>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
+                             (cudaStream_t)stream);
   else
-    rc = forward_impl<bf16>(m, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream);
+    rc = forward_impl<bf16>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
+                            (cudaStream_t)stream);
+  m->tap_out = nullptr;
+  m->tap_name.clear();
+  return rc;
+}
+
+int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* v, const float* sigma,
+                          float sigma_data, const float* cond, int64_t cond_batch_stride, float* out, float* out_tangent, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward_jvp: model not finalized");
+  KDB_REQUIRE(x && v && sigma && cond && out && out_tangent && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_jvp: NULL argument");
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "forward_jvp: the derivative is built for the fp32 path only (precision %d)",
+              precision);
+  int rc = check_image(m, "forward_jvp", height, width, sigma_data);
+  if (rc) return rc;
+  Workspace ws;
+  if ((rc = carve_checked(m, "forward_jvp", precision, 2 * batch, height, width, workspace, workspace_bytes, ws))) return rc;
+  rc = forward_impl<float>(m, batch, height, width, x, v, sigma, sigma_data, cond, cond_batch_stride, out, out_tangent, ws, (cudaStream_t)stream);
   m->tap_out = nullptr;
   m->tap_name.clear();
   return rc;

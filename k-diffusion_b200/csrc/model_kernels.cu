@@ -651,6 +651,275 @@ template int launch_patch_out<bf16>(const bf16*, const float*, const float*, con
                                     int, int, int, int, cudaStream_t);
 
 // ------------------------------------------------------------------------------------------------
+// Tangent kernels of the forward-mode derivative (JVP), fp32.  Each reads the primal input of one nonlinear op and its tangent
+// and writes the tangent of the op's output; the primal launch is left as it is.  Every tangent output is linear in the input
+// tangent and uses only products with it, so scaling the tangent by a power of two scales the result exactly.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) rmsnorm_jvp_kernel(const float* __restrict__ x, const float* __restrict__ dx, float* __restrict__ dy,
+                                                          const float* __restrict__ scale, int64_t scale_bstride, int64_t rows_per_batch,
+                                                          int64_t rows, int C) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const float* xr = x + row * C;
+  const float* dr = dx + row * C;
+  float ss = 0.f, sd = 0.f;
+  for (int c = lane; c < C; c += 32) {
+    const float v = xr[c];
+    ss = fmaf(v, v, ss);
+    sd = fmaf(v, dr[c], sd);
+  }
+  ss = warp_sum(ss);
+  sd = warp_sum(sd);
+  const float r = rsqrtf(ss / (float)C + kEps);   // the primal kernel's 1/rms
+  const float r3m = r * r * r * (sd / (float)C);
+  const float* sc = scale + (row / rows_per_batch) * scale_bstride;
+  float* yr = dy + row * C;
+  for (int c = lane; c < C; c += 32) yr[c] = __ldg(sc + c) * (r * dr[c] - xr[c] * r3m);
+}
+
+int launch_rmsnorm_jvp(const float* x, const float* dx, float* dy, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
+                       int64_t rows, int C, cudaStream_t st) {
+  rmsnorm_jvp_kernel<<<(unsigned)ceil_div(rows, 8), 256, 0, st>>>(x, dx, dy, scale, scale_bstride, rows_per_batch, rows, C);
+  KDB_LAUNCH_CHECK(F_RMSNORM, st);
+  return 0;
+}
+
+// One warp per (token row, head) of the tangent rows; reads the un-normalised primal q, k of the same row.
+__global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __restrict__ qkv, float* __restrict__ dqkv,
+                                                              const float* __restrict__ pos, const float* __restrict__ freqs,
+                                                              const float* __restrict__ scale, int64_t rows, int Ttok, int nh, int e) {
+  extern __shared__ float sm[];   // [warps][2][e]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+  if (item >= rows * nh) return;
+  const int64_t row = item / nh;
+  const int h = (int)(item - row * nh);
+  float* buf = sm + (size_t)warp * 2 * e;
+  const int dr = e / 4, nf = e / 8;
+  const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
+  const float sqs = sqrtf(scale[h]);
+#pragma unroll
+  for (int t = 0; t < 2; ++t) {
+    const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
+    const float* v = qkv + off;
+    float* dv = dqkv + off;
+    float ss = 0.f, sd = 0.f;
+    for (int d = lane; d < e; d += 32) {
+      ss = fmaf(v[d], v[d], ss);
+      sd = fmaf(v[d], dv[d], sd);
+    }
+    ss = warp_sum(ss);
+    sd = warp_sum(sd);
+    const float rho = rsqrtf(ss + kEps);
+    const float r3s = rho * rho * rho * sd;
+    // d(q rho) = rho dq - q rho^3 (q . dq), then the primal's rotation
+    for (int d = lane; d < e; d += 32) buf[t * e + d] = sqs * (rho * dv[d] - v[d] * r3s);
+    __syncwarp();
+    for (int d = lane; d < e; d += 32) {
+      float o;
+      if (d < 2 * dr) {
+        const int j = d < dr ? d : d - dr;
+        const float theta = (j < nf ? py : px) * freqs[h * nf + (j < nf ? j : j - nf)];
+        float s, c;
+        sincosf(theta, &s, &c);
+        const float x1 = buf[t * e + j], x2 = buf[t * e + j + dr];
+        o = d < dr ? x1 * c - x2 * s : x2 * c + x1 * s;
+      } else {
+        o = buf[t * e + d];
+      }
+      dv[d] = o;
+    }
+    __syncwarp();
+  }
+}
+
+int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
+                           int nh, int e, cudaStream_t st) {
+  KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope_jvp: d_head %d must be a multiple of 8", e);
+  const size_t smem = sizeof(float) * 4 * 2 * e;
+  qknorm_rope_jvp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, freqs, scale, rows, T_tokens, nh, e);
+  KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
+  return 0;
+}
+
+// Attention tangent, one warp per (batch, head, query), the key set of attn_generic_kernel:
+//   do_i = sum_j P_ij dv_j + sum_j P_ij dS_ij (v_j - o_i),   dS_ij = dq_i . k_j + q_i . dk_j
+__global__ void __launch_bounds__(128) attn_jvp_kernel(const float* __restrict__ qkv, const float* __restrict__ dqkv, float* __restrict__ dout,
+                                                       int h, int w, int nh, int e, int type, int param, int shift, int maxkeys) {
+  extern __shared__ float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int Ttok = h * w;
+  const int q = blockIdx.x * 4 + warp;
+  const int head = blockIdx.y;
+  const int64_t b = blockIdx.z;
+  float* qv = sm + (size_t)warp * (2 * e + 3 * maxkeys);
+  float* dqv = qv + e;
+  float* sc = dqv + e;
+  float* dsc = sc + maxkeys;
+  int* toks = reinterpret_cast<int*>(dsc + maxkeys);
+  if (q >= Ttok) return;
+  const int64_t rs = 3LL * nh * e;
+  const float* base = qkv + b * Ttok * rs;
+  const float* dbase = dqkv + b * Ttok * rs;
+  for (int d = lane; d < e; d += 32) {
+    qv[d] = base[(int64_t)q * rs + (int64_t)head * e + d];
+    dqv[d] = dbase[(int64_t)q * rs + (int64_t)head * e + d];
+  }
+  __syncwarp();
+  KeySet ks;
+  ks.init(type, h, w, param, shift, q);
+  const int nk = ks.count();
+  float mx = -INFINITY;
+  for (int j0 = 0; j0 < nk; j0 += 32) {
+    const int j = j0 + lane;
+    if (j < nk) {
+      const int tok = ks.token(j);
+      float s = -INFINITY, ds = 0.f;
+      if (tok >= 0) {
+        const float* kp = base + (int64_t)tok * rs + (int64_t)(nh + head) * e;
+        const float* dkp = dbase + (int64_t)tok * rs + (int64_t)(nh + head) * e;
+        s = 0.f;
+        for (int d = 0; d < e; ++d) {
+          s = fmaf(qv[d], kp[d], s);
+          ds = fmaf(dqv[d], kp[d], fmaf(qv[d], dkp[d], ds));
+        }
+      }
+      sc[j] = s;
+      dsc[j] = ds;
+      toks[j] = tok;
+      mx = fmaxf(mx, s);
+    }
+  }
+  mx = warp_max(mx);
+  float sum = 0.f, sds = 0.f;
+  __syncwarp();
+  for (int j = lane; j < nk; j += 32) {
+    const float p = (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
+    sc[j] = p;
+    sum += p;
+    sds = fmaf(p, dsc[j], sds);
+  }
+  sum = warp_sum(sum);
+  sds = warp_sum(sds);
+  __syncwarp();
+  const float inv = 1.f / sum;
+  const float psd = sds * inv;   // sum_j P_j dS_j
+  float* op = dout + (b * Ttok + q) * (int64_t)nh * e + (int64_t)head * e;
+  for (int d = lane; d < e; d += 32) {
+    float o = 0.f, t = 0.f;
+    for (int j = 0; j < nk; ++j) {
+      const int tok = toks[j];
+      if (tok >= 0) {
+        const int64_t vo = (int64_t)tok * rs + (int64_t)(2 * nh + head) * e + d;
+        const float vv = base[vo];
+        o = fmaf(sc[j], vv, o);
+        t = fmaf(sc[j], fmaf(dsc[j], vv, dbase[vo]), t);
+      }
+    }
+    op[d] = t * inv - (o * inv) * psd;
+  }
+}
+
+int launch_attention_jvp(const float* qkv, const float* dqkv, float* dout, int B, int h, int w, int nh, int e, int attn_type, int attn_param,
+                         int shift, cudaStream_t st) {
+  int maxkeys;
+  if (attn_type == KDB_ATTN_GLOBAL) {
+    maxkeys = h * w;
+  } else if (attn_type == KDB_ATTN_NEIGHBORHOOD || attn_type == KDB_ATTN_SHIFTED_WINDOW) {
+    maxkeys = attn_param * attn_param;   // geometry checked by the primal launch
+  } else {
+    KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "attention_jvp: bad type %d", attn_type);
+  }
+  const size_t smem = sizeof(float) * 4 * (size_t)(2 * e + 3 * maxkeys);
+  KDB_REQUIRE(smem <= 200 * 1024, KDB_ERR_UNSUPPORTED, "attention_jvp: %d keys exceed the shared-memory budget", maxkeys);
+  static bool attr = false;
+  if (!attr) {
+    KDB_CUDA(cudaFuncSetAttribute(attn_jvp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr = true;
+  }
+  dim3 grid((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B);
+  attn_jvp_kernel<<<grid, 128, smem, st>>>(qkv, dqkv, dout, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
+  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
+  return 0;
+}
+
+// d(a gelu(g)) = da gelu(g) + a (Phi(g) + g phi(g)) dg, erf form
+__global__ void __launch_bounds__(256) geglu_jvp_kernel(const float* __restrict__ hp, const float* __restrict__ dh, float* __restrict__ dout,
+                                                        int64_t M, int F) {
+  const int64_t total = M * F;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int64_t m = i / F;
+    const int f = (int)(i - m * F);
+    const float a = hp[m * 2 * F + f], g = hp[m * 2 * F + F + f];
+    const float Phi = 0.5f * (1.f + erff(g * 0.70710678118654752440f));
+    const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
+    dout[i] = dh[m * 2 * F + f] * (g * Phi) + (a * fmaf(g, phi, Phi)) * dh[m * 2 * F + F + f];
+  }
+}
+
+int launch_geglu_jvp(const float* h, const float* dh, float* dout, int64_t M, int F, cudaStream_t st) {
+  int64_t blocks = ceil_div(M * F, 256);
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  geglu_jvp_kernel<<<(unsigned)blocks, 256, 0, st>>>(h, dh, dout, M, F);
+  KDB_LAUNCH_CHECK(F_GEGLU, st);
+  return 0;
+}
+
+// out_norm tangent + patch_out projection + un-patch + the tangent of the Karras combine (c_skip v + c_out dF).  One warp per token.
+__global__ void __launch_bounds__(128) patch_out_jvp_kernel(const float* __restrict__ tokens, const float* __restrict__ dtokens,
+                                                            const float* __restrict__ nscale, const float* __restrict__ W,
+                                                            const float* __restrict__ v_in, const float* __restrict__ sigma, float sd,
+                                                            float* __restrict__ out, int Cout, int H, int Wd, int ph, int pw, int C0,
+                                                            int64_t tokens_total) {
+  extern __shared__ float sm[];   // [warps][C0]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t tok = (int64_t)blockIdx.x * 4 + warp;
+  if (tok >= tokens_total) return;
+  float* dn = sm + (size_t)warp * C0;
+  const float* xr = tokens + tok * C0;
+  const float* dr = dtokens + tok * C0;
+  float ss = 0.f, sdot = 0.f;
+  for (int c = lane; c < C0; c += 32) {
+    ss = fmaf(xr[c], xr[c], ss);
+    sdot = fmaf(xr[c], dr[c], sdot);
+  }
+  ss = warp_sum(ss);
+  sdot = warp_sum(sdot);
+  const float r = rsqrtf(ss / (float)C0 + kEps);
+  const float r3m = r * r * r * (sdot / (float)C0);
+  for (int c = lane; c < C0; c += 32) dn[c] = __ldg(nscale + c) * (r * dr[c] - xr[c] * r3m);
+  __syncwarp();
+  const int th_n = H / ph, tw_n = Wd / pw;
+  const int64_t b = tok / ((int64_t)th_n * tw_n);
+  const int rr = (int)(tok - b * th_n * tw_n);
+  const int ty = rr / tw_n, tx = rr - ty * tw_n;
+  float c_skip = 0.f, c_out = 1.f, c_in;
+  if (sd > 0.f) karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
+  const int N = ph * pw * Cout;
+  for (int n = lane; n < N; n += 32) {
+    const float* wr = W + (int64_t)n * C0;
+    float acc = 0.f;
+    for (int k = 0; k < C0; ++k) acc = fmaf(dn[k], __ldg(wr + k), acc);
+    const int q = n / Cout, c = n - q * Cout;
+    const int nh = q / pw, nw = q - nh * pw;
+    const int64_t o = ((b * Cout + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw);
+    out[o] = (sd > 0.f) ? acc * c_out + v_in[o] * c_skip : acc;
+  }
+}
+
+int launch_patch_out_jvp(const float* tokens, const float* dtokens, const float* norm_scale, const float* W, const float* v_in, const float* sigma,
+                         float sigma_data, float* out, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st) {
+  const int64_t tok = (int64_t)B * (H / ph) * (Wd / pw);
+  const size_t smem = sizeof(float) * 4 * C0;
+  KDB_REQUIRE(smem <= 48 * 1024, KDB_ERR_UNSUPPORTED, "patch_out_jvp: width %d too large", C0);
+  patch_out_jvp_kernel<<<(unsigned)ceil_div(tok, 4), 128, smem, st>>>(tokens, dtokens, norm_scale, W, v_in, sigma, sigma_data, out, Cout, H,
+                                                                      Wd, ph, pw, C0, tok);
+  KDB_LAUNCH_CHECK(F_PATCH_OUT, st);
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Conditioning: FourierFeatures -> in-proj -> MappingNetwork -> concatenated AdaRMSNorm projections.
 // One CTA (8 warps) per row; warp-per-output matvecs, weights streamed from L2.
 // ------------------------------------------------------------------------------------------------

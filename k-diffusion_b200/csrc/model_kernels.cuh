@@ -68,6 +68,23 @@ template <typename T>
 int launch_patch_out(const T* tokens, const float* norm_scale, const float* W, const float* x_in, const float* sigma,
                      float sigma_data, float* out, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st);
 
+// Tangent kernels of the forward-mode derivative (fp32).  Each takes the primal input of one nonlinear op and its tangent and
+// writes the tangent of the output; the primal op is launched separately, unchanged.
+// RMSNorm: dy = s (r dx - x r^3 mean(x dx)), r = rsqrt(mean(x^2) + eps); scale rows as launch_rmsnorm
+int launch_rmsnorm_jvp(const float* x, const float* dx, float* dy, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
+                       int64_t rows, int C, cudaStream_t st);
+// cosine-sim scale + RoPE of the tangent q, k (in place on dqkv [rows, 3, nh, e]); qkv holds the primal q, k BEFORE launch_qknorm_rope
+int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
+                           int nh, int e, cudaStream_t st);
+// attention tangent over the key set of launch_attention_generic; qkv = the normalised, rotated primal, dqkv its tangent
+int launch_attention_jvp(const float* qkv, const float* dqkv, float* dout, int B, int h, int w, int nh, int e, int attn_type, int attn_param,
+                         int shift, cudaStream_t st);
+// GEGLU tangent: dout = da gelu(g) + a gelu'(g) dg over h / dh [M, 2F]
+int launch_geglu_jvp(const float* h, const float* dh, float* dout, int64_t M, int F, cudaStream_t st);
+// out_norm tangent + patch_out + un-patch; sigma_data > 0: out = c_skip v + c_out dF, else dF
+int launch_patch_out_jvp(const float* tokens, const float* dtokens, const float* norm_scale, const float* W, const float* v_in, const float* sigma,
+                         float sigma_data, float* out, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st);
+
 // tiled fast variants (patch_kernels.cu); return false when the shape is outside their envelope
 template <typename T>
 bool launch_patch_in_tiled(const float* x, const float* sigma, float sigma_data, const float* W, T* out, int B, int C, int H, int Wd, int ph,

@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -62,6 +62,7 @@ SIGNATURES = {
     "kdb_model_conditioning": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "kdb_model_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
     "kdb_model_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
+    "kdb_model_forward_jvp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_model_tap_count": (_i64, [_vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
@@ -416,6 +417,21 @@ class Engine:
             check(lib().kdb_model_forward(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
                                           ptr(out), ptr(ws), ws.numel(), stream()))
         return out
+
+    def forward_jvp(self, x, v, sigma, cond, cond_batch_stride, sigma_data, out=None, out_tangent=None):
+        """Forward-mode derivative on the fp32 path: -> (out, tangent), out as forward() at fp32, tangent = J(x) v.
+        x, v [B,C,H,W] fp32 contiguous; the workspace holds 2B images (the tangent rides as the second half of the batch)."""
+        B, _, H, W = x.shape
+        if v.shape != x.shape:
+            raise ValueError(f"tangent shape {tuple(v.shape)} != x shape {tuple(x.shape)}")
+        shape = (B, self.cfg.out_channels, H, W)
+        out = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
+        out_tangent = torch.empty(shape, device=x.device, dtype=torch.float32) if out_tangent is None else out_tangent
+        ws = self._workspace(PREC_FP32, 2 * B, H, W, x.device)
+        with device_of(x):
+            check(lib().kdb_model_forward_jvp(self._h, PREC_FP32, B, H, W, ptr(x), ptr(v), ptr(sigma), float(sigma_data), ptr(cond),
+                                              cond_batch_stride, ptr(out), ptr(out_tangent), ptr(ws), ws.numel(), stream()))
+        return out, out_tangent
 
     def arm_tap(self, name, capacity, device):
         buf = torch.empty(capacity, dtype=torch.float32, device=device)

@@ -51,6 +51,21 @@ class Denoiser(nn.Module):
         f = self.inner_model(_native.precond_scale_in(x, sig, float(self.sigma_data)), sigma, **kwargs)
         return _native.precond_combine(_native.f32c(f), x, sig, float(self.sigma_data))
 
+    def jvp(self, input, sigma, tangent, **kwargs):
+        """(D(x, sigma), J_D(x) tangent): the denoiser and its forward-mode derivative with respect to `input` along `tangent`.
+
+        A native inner model computes both in one fp32 engine call.  Any other inner model goes through `torch.func.jvp` of
+        inner(c_in x); the combine c_skip x + c_out f is linear, so one combine kernel serves the primal and the tangent."""
+        _native.require_cuda(input, sigma, tangent)
+        if self.is_native():
+            return self.inner_model.denoise_jvp(input, sigma, tangent, self.sigma_data, **kwargs)
+        x, t = _native.f32c(input), _native.f32c(tangent)
+        sig = _native.f32c(sigma).expand(x.shape[0]).contiguous()
+        sd = float(self.sigma_data)
+        c_in = (1 / (sig * sig + sd * sd).sqrt()).view(-1, *([1] * (x.ndim - 1)))
+        f, df = torch.func.jvp(lambda xx: self.inner_model(xx * c_in, sigma, **kwargs), (x,), (t,))
+        return _native.precond_combine(_native.f32c(f), x, sig, sd), _native.precond_combine(_native.f32c(df), t, sig, sd)
+
 
 class DenoiserWithVariance(Denoiser):
     """reference layers.py:93-101: differs from Denoiser in `loss` only (training, out of scope); sampling is identical."""

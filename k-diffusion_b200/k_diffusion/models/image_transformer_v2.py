@@ -226,8 +226,8 @@ class ImageTransformerDenoiserModelV2(nn.Module):
         return self.engine().conditioning(sigma, aug_cond, class_cond if self.class_emb is not None else None,
                                           mapping_cond if self.mapping_cond_in_proj is not None else None)
 
-    def _run(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out=None):
-        _native.require_cuda(x, sigma)
+    def _run(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out=None, tangent=None):
+        _native.require_cuda(x, sigma, tangent)
         if x.ndim != 4:
             raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
         if self.training and any(s.dropout > 0 for s in self.levels):
@@ -243,7 +243,14 @@ class ImageTransformerDenoiserModelV2(nn.Module):
                 eng.check_class_range(class_cond)           # nn.Embedding raises on out-of-range labels (reference :735)
             cond = eng.conditioning(sig, aug_cond, class_cond if self.class_emb is not None else None,
                                     mapping_cond if self.mapping_cond_in_proj is not None else None)
-            res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
+            if tangent is None:
+                res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
+            else:
+                if tangent.shape != x.shape:
+                    raise ValueError(f"tangent must have the shape of x {tuple(x.shape)}, got {tuple(tangent.shape)}")
+                res = eng.forward_jvp(xin, _native.f32c(tangent), sig, cond, eng.cond_stride, sigma_data)
+        if tangent is not None:
+            return res if x.dtype == torch.float32 else tuple(r.to(x.dtype) for r in res)
         return res if x.dtype == torch.float32 else res.to(x.dtype)
 
     def forward(self, x, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
@@ -253,3 +260,13 @@ class ImageTransformerDenoiserModelV2(nn.Module):
     def denoise(self, x, sigma, sigma_data, aug_cond=None, class_cond=None, mapping_cond=None, out=None):
         """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
         return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, out=out)
+
+    def jvp(self, x, sigma, v, aug_cond=None, class_cond=None, mapping_cond=None):
+        """(F(x, sigma), J_F(x) v): the raw inner model and its forward-mode derivative along `v` with respect to x, in one engine call.
+        Always runs on the exact fp32 path, whatever `set_precision` selected (the tangent kernels are fp32 only)."""
+        return self._run(x, sigma, 0.0, aug_cond, class_cond, mapping_cond, tangent=v)
+
+    def denoise_jvp(self, x, sigma, v, sigma_data, aug_cond=None, class_cond=None, mapping_cond=None):
+        """(D(x, sigma), J_D(x) v) of the Karras-preconditioned evaluation, J_D v = c_skip v + c_out J_F(c_in x) c_in v, in one engine
+        call.  Always runs on the exact fp32 path, whatever `set_precision` selected."""
+        return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, tangent=v)
