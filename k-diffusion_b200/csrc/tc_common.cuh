@@ -117,6 +117,13 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// arrive without waiting: the other `threads - 32 k` threads of the barrier wait on it with named_barrier_sync
+__device__ __forceinline__ void named_barrier_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
+// Hand registers between warpgroups (every warp of the warpgroup executes it): a producer warpgroup gives up what its MMA
+// warpgroups then take, within the CTA's allocation at launch.
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // byte offset of 16-byte chunk `chunk16` (0..7) of `row` inside a [rows x 128 B] SWIZZLE_128B tile (what TMA / UMMA expect)
 __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk16) {
