@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 9
+#define KDB_ABI_VERSION 10
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -203,6 +203,23 @@ int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int wid
 int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int width,
                           const float* x, const float* v, const float* sigma, float sigma_data,
                           const float* cond, int64_t cond_batch_stride, float* out, float* out_tangent,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
+/* Reverse-mode derivative (VJP) of the same evaluation for a cotangent u [B, C_out, H, W]: out = D(x, sigma) as kdb_model_forward computes it
+ * at KDB_PREC_FP32 (bit for bit), grad_x = u^T J_D(x) = c_skip u + c_in J_F(c_in x)^T (c_out u) (sigma_data > 0) or J_F(x)^T u
+ * (sigma_data <= 0), shape of x.  The derivative is taken with respect to x only (sigma and the conditioning are held fixed).  fp32 only:
+ * any other precision returns KDB_ERR_UNSUPPORTED.  The forward keeps the fp32 residual stream entering every attention half, every
+ * feed-forward half and out_norm on a tape; the backward walks the layers in reverse, recomputes each half's activations from its tape
+ * entry with the forward's own launches and runs the backward kernels.  The workspace holds one fp32 forward workspace of `batch` images,
+ * the tape and the gradient buffers: kdb_model_vjp_workspace_bytes returns its size in bytes (or a negative KDB_ERR_* for a NULL model
+ * or a non-positive size; kdb_model_workspace_bytes is unchanged), a shorter one returns KDB_ERR_WORKSPACE.  cond / cond_batch_stride
+ * as for kdb_model_forward.  No atomics: two calls on the same inputs return the same bits.  Same stream, allocation and CUDA-graph
+ * rules as kdb_model_forward. */
+int64_t kdb_model_vjp_workspace_bytes(const KdbModel* m, int batch, int height, int width);
+int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int width,
+                          const float* x, const float* sigma, float sigma_data,
+                          const float* cond, int64_t cond_batch_stride,
+                          const float* cotangent, float* out, float* grad_x,
                           void* workspace, size_t workspace_bytes, void* stream);
 
 /* Debug/parity tap: arm a copy of one intermediate of the NEXT forward into `out` (fp32, device).

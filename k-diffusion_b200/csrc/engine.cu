@@ -340,6 +340,7 @@ struct Fwd {
   bool fold;                // emit, one shared conditioning row and a fold table: consumers take the weights with the norm scale folded in
   bool stats;               // ws.rowss holds the row statistics of the current residual stream
   bool jvp;                 // fp32 forward-mode derivative: images [B, 2B) of every token buffer carry the tangent of images [0, B)
+  float* const* tape = nullptr;   // fp32 reverse mode: slot 2k / 2k+1 keep the residual stream entering layer k's attention / feed-forward half
 
   // images held by the token buffers: linear launches and taps cover them all, nonlinear primal launches the first B
   int images() const { return jvp ? 2 * B : B; }
@@ -368,6 +369,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   auto tapped = [&](const char* part) { return m->tap_out != nullptr && m->tap_name == tag + part; };
   int rc = 0;
   if (L.attn_type != KDB_ATTN_NONE) {
+    if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
     GemmEpi qe;
     qe.mode = (L.e == 64 && rope != nullptr) ? EPI_QKV_ROPE : EPI_STORE;
     qe.C = C;
@@ -432,6 +434,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     }
     if ((rc = tap<T>(m, tag + ".attn", x, Ma * C, f.st))) return rc;
   }
+  if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k + 1], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
   auto unfused = [&] {
     int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
     if constexpr (std::is_same_v<T, float>)
@@ -479,9 +482,11 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
 // v != nullptr (fp32 only): forward-mode derivative along v, the tangent D'(x) v goes to out_t.  The primal launches are those of a
 // plain forward of B images; the linear ones run over the tangent images as well (the SIMT GEMM's per-row arithmetic does not depend
 // on M), each nonlinear one is followed by its tangent kernel.
+// tape != nullptr (fp32 only): the residual stream entering every attention / feed-forward half and out_norm is copied to the tape
+// (slots 2k, 2k+1 of layer k, slot 2 * layers for out_norm) for the reverse walk of kdb_model_forward_vjp; the launches are unchanged.
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
-                 int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st) {
+                 int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st, float* const* tape = nullptr) {
   constexpr bool kBf16 = std::is_same_v<T, bf16>;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
@@ -492,6 +497,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   m->tap_count = 0;
   Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false, !kBf16 && v != nullptr};
   f.fold = f.emit && cond_bs == 0 && m->fold_descs != nullptr;
+  f.tape = tape;
   if (f.fold && (rc = launch_fold_norm_weights(m->fold_descs, m->n_fold, cond, st))) return rc;
   const int Bt = f.images();
 
@@ -591,12 +597,156 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       return launch_patch_out_tc(xn, m->patch_out_wb, x, sigma, sd, out, B, H, W, C0, st);
     }
   }
+  if (tape)
+    KDB_CUDA(cudaMemcpyAsync(tape[2 * m->layers.size()], cur, sizeof(T) * B * h0 * w0 * C0, cudaMemcpyDeviceToDevice, st));
   rc = launch_patch_out<T>(cur, m->out_norm, m->patch_out_w, x, sigma, sd, out, B, c.out_channels, H, W, c.patch_h, c.patch_w, C0, st);
   if constexpr (!kBf16)
     if (!rc && f.jvp)
       rc = launch_patch_out_jvp(cur, cur + (int64_t)B * h0 * w0 * C0, m->out_norm, m->patch_out_w, v, sigma, sd, out_t, B, c.out_channels, H, W,
                                 c.patch_h, c.patch_w, C0, st);
   return rc;
+}
+
+// Reverse mode.  The workspace of kdb_model_forward_vjp is one fp32 forward workspace of B images followed by the tape (the residual
+// stream entering every attention half, every feed-forward half and out_norm) and the gradient buffers.  The backward walk reuses the
+// forward workspace's xn / qkv / ao / hbuf / mg buffers for the recomputed activations and as scratch.
+struct VjpSpace {
+  std::vector<float*> tape;   // 2 per layer (KdbModel::layers order; nullptr for the attention half of a layer without one) + out_norm
+  std::vector<float*> g;      // per level: gradient of the residual stream [B, T_l, C_l]
+  float *qkv_raw = nullptr;   // the qkv projection before launch_qknorm_rope normalises it in place
+  float *dqkv = nullptr, *dbuf = nullptr, *dh = nullptr, *stats = nullptr;
+  size_t total = 0;
+};
+
+void carve_vjp(const KdbModelConfig& c, int B, int H, int W, char* base, Workspace& ws, VjpSpace& vs) {
+  carve(c, KDB_PREC_FP32, B, H, W, base, ws);
+  size_t off = align_up(ws.total, 1024);
+  auto take = [&](size_t floats) {
+    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+    off += align_up(floats * sizeof(float), 1024);
+    return p;
+  };
+  const int n = c.n_levels;
+  const int64_t T0 = (int64_t)(H / c.patch_h) * (W / c.patch_w);
+  auto stream_floats = [&](int l) { return (size_t)B * (T0 >> (2 * l)) * c.width[l]; };
+  // layer levels in execution order (as kdb_model_finalize plans them)
+  std::vector<int> lv;
+  for (int l = 0; l < n - 1; ++l) lv.insert(lv.end(), c.depth[l], l);
+  lv.insert(lv.end(), c.depth[n - 1], n - 1);
+  for (int l = n - 2; l >= 0; --l) lv.insert(lv.end(), c.depth[l], l);
+  vs.tape.clear();
+  for (int l : lv) {
+    vs.tape.push_back(c.attn_type[l] != KDB_ATTN_NONE ? take(stream_floats(l)) : nullptr);
+    vs.tape.push_back(take(stream_floats(l)));
+  }
+  vs.tape.push_back(take(stream_floats(0)));
+  vs.g.assign(n, nullptr);
+  size_t mqkv = 0, md = 0, mh = 0, mst = 0;
+  for (int l = 0; l < n; ++l) {
+    vs.g[l] = take(stream_floats(l));
+    const size_t toks = (size_t)B * (T0 >> (2 * l));
+    md = std::max(md, toks * std::max(c.width[l], c.d_ff[l]));
+    mh = std::max(mh, toks * 2 * c.d_ff[l]);
+    if (c.attn_type[l] != KDB_ATTN_NONE) {
+      mqkv = std::max(mqkv, 3 * stream_floats(l));
+      mst = std::max(mst, toks * (c.width[l] / std::max(c.d_head[l], 1)) * 3);
+    }
+  }
+  vs.qkv_raw = take(mqkv);
+  vs.dqkv = take(mqkv);
+  vs.dbuf = take(md);
+  vs.dh = take(mh);
+  vs.stats = take(mst);
+  vs.total = off + 1024;
+}
+
+struct Bwd {
+  int B;
+  Workspace& ws;
+  VjpSpace& vs;
+  cudaStream_t st;
+  const float* cond;
+  int64_t cond_bs;
+  const PosTables* pt;
+};
+
+// Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
+// its activations from the tape with the forward's own launches, runs the backward kernels and adds the branch gradient to g.
+int vjp_layer(KdbModel* m, Bwd& b, int k, float* g, int h, int w) {
+  const LayerPlan& L = m->layers[k];
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)b.B * Ttok;
+  const int C = L.C, F = L.dff;
+  float* xn = reinterpret_cast<float*>(b.ws.xn);
+  float* qkv = reinterpret_cast<float*>(b.ws.qkv);
+  float* ao = reinterpret_cast<float*>(b.ws.ao);
+  float* hb = reinterpret_cast<float*>(b.ws.hbuf);
+  cudaStream_t st = b.st;
+  int rc;
+  // feed-forward half: x + down(geglu(up(norm(x))))
+  const float* x = b.vs.tape[2 * k + 1];
+  if ((rc = launch_rmsnorm<float>(x, xn, b.cond + L.ada_ff, b.cond_bs, Ttok, M, C, st))) return rc;
+  if ((rc = launch_gemm_simt<float, float>(xn, L.up_w, hb, M, 2 * F, C, GemmEpi{}, st))) return rc;
+  if ((rc = launch_gemm_vjp(g, L.down_w, b.vs.dbuf, M, C, F, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_geglu_vjp(hb, b.vs.dbuf, b.vs.dh, M, F, st))) return rc;
+  if ((rc = launch_gemm_vjp(b.vs.dh, L.up_w, xn, M, 2 * F, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_rmsnorm_vjp(x, xn, g, b.cond + L.ada_ff, b.cond_bs, Ttok, M, C, st))) return rc;
+  if (L.attn_type == KDB_ATTN_NONE) return 0;
+  // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
+  x = b.vs.tape[2 * k];
+  const float* pos = b.pt->pos[L.level];
+  if ((rc = launch_rmsnorm<float>(x, xn, b.cond + L.ada_attn, b.cond_bs, Ttok, M, C, st))) return rc;
+  if ((rc = launch_gemm_simt<float, float>(xn, L.qkv_w, b.vs.qkv_raw, M, 3 * C, C, GemmEpi{}, st))) return rc;
+  KDB_CUDA(cudaMemcpyAsync(qkv, b.vs.qkv_raw, sizeof(float) * M * 3 * C, cudaMemcpyDeviceToDevice, st));
+  if ((rc = launch_qknorm_rope<float>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
+  if ((rc = launch_attention_generic<float>(qkv, ao, b.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st))) return rc;
+  if ((rc = launch_gemm_vjp(g, L.out_w, b.vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_attention_vjp(qkv, ao, b.vs.dbuf, b.vs.dqkv, b.vs.stats, b.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
+    return rc;
+  if ((rc = launch_qknorm_rope_vjp(b.vs.qkv_raw, b.vs.dqkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
+  if ((rc = launch_gemm_vjp(b.vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  return launch_rmsnorm_vjp(x, xn, g, b.cond + L.ada_attn, b.cond_bs, Ttok, M, C, st);
+}
+
+// out = the fp32 forward (bit for bit: the same launches, plus the tape copies), then grad_x = u^T J(x) by a walk of the forward in
+// reverse: patch_out + out_norm + combine; each up level's layers then its split-lerp; the mid layers; each down level (innermost
+// first) its merge then its layers; patch_in.
+int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, const float* sigma, float sd, const float* cond, int64_t cond_bs,
+             float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st) {
+  int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data());
+  if (rc) return rc;
+  const KdbModelConfig& c = m->cfg;
+  const int n = c.n_levels, C0 = c.width[0];
+  const int h0 = H / c.patch_h, w0 = W / c.patch_w;
+  PosTables* pt = nullptr;
+  if ((rc = ensure_pos(m, h0, w0, st, &pt))) return rc;
+  Bwd b{B, ws, vs, st, cond, cond_bs, pt};
+  if ((rc = launch_patch_out_vjp(vs.tape.back(), m->out_norm, m->patch_out_w, u, sigma, sd, vs.g[0], B, c.out_channels, H, W, c.patch_h,
+                                 c.patch_w, C0, st)))
+    return rc;
+  int k = (int)m->layers.size();
+  float* mg = reinterpret_cast<float*>(ws.mg);
+  for (int l = 0; l < n - 1; ++l) {
+    const int h = h0 >> l, w = w0 >> l;
+    for (int i = 0; i < c.depth[l]; ++i)
+      if ((rc = vjp_layer(m, b, --k, vs.g[l], h, w))) return rc;
+    // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
+    if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
+    if ((rc = launch_gemm_vjp(mg, m->split_w[l], vs.g[l + 1], (int64_t)B * (h / 2) * (w / 2), 4 * c.width[l], c.width[l + 1], VJP_STORE, 0, 0, 0,
+                              st)))
+      return rc;
+  }
+  for (int i = 0; i < c.depth[n - 1]; ++i)
+    if ((rc = vjp_layer(m, b, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1)))) return rc;
+  for (int l = n - 2; l >= 0; --l) {
+    const int h = h0 >> l, w = w0 >> l;
+    // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added
+    if ((rc = launch_gemm_vjp(vs.g[l + 1], m->merge_w[l], vs.g[l], (int64_t)B * (h / 2) * (w / 2), c.width[l + 1], 4 * c.width[l],
+                              VJP_UNPATCH_ACC, h / 2, w / 2, c.width[l], st)))
+      return rc;
+    for (int i = 0; i < c.depth[l]; ++i)
+      if ((rc = vjp_layer(m, b, --k, vs.g[l], h, w))) return rc;
+  }
+  return launch_patch_in_vjp(vs.g[0], m->patch_in_w, u, sigma, sd, grad_x, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
 }
 
 }  // namespace
@@ -835,6 +985,34 @@ int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int
   Workspace ws;
   if ((rc = carve_checked(m, "forward_jvp", precision, 2 * batch, height, width, workspace, workspace_bytes, ws))) return rc;
   rc = forward_impl<float>(m, batch, height, width, x, v, sigma, sigma_data, cond, cond_batch_stride, out, out_tangent, ws, (cudaStream_t)stream);
+  m->tap_out = nullptr;
+  m->tap_name.clear();
+  return rc;
+}
+
+int64_t kdb_model_vjp_workspace_bytes(const KdbModel* m, int batch, int height, int width) {
+  KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "vjp_workspace_bytes: bad argument");
+  Workspace ws;
+  VjpSpace vs;
+  carve_vjp(m->cfg, batch, height, width, nullptr, ws, vs);
+  return (int64_t)vs.total;
+}
+
+int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                          const float* cond, int64_t cond_batch_stride, const float* cotangent, float* out, float* grad_x, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward_vjp: model not finalized");
+  KDB_REQUIRE(x && sigma && cond && cotangent && out && grad_x && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_vjp: NULL argument");
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "forward_vjp: the derivative is built for the fp32 path only (precision %d)",
+              precision);
+  int rc = check_image(m, "forward_vjp", height, width, sigma_data);
+  if (rc) return rc;
+  Workspace ws;
+  VjpSpace vs;
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 1024));
+  carve_vjp(m->cfg, batch, height, width, base, ws, vs);
+  KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_vjp: workspace %zu < required %zu", workspace_bytes, vs.total);
+  rc = vjp_impl(m, batch, height, width, x, cotangent, sigma, sigma_data, cond, cond_batch_stride, out, grad_x, ws, vs, (cudaStream_t)stream);
   m->tap_out = nullptr;
   m->tap_name.clear();
   return rc;

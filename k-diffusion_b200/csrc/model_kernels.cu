@@ -3,6 +3,7 @@
 // fp32-exact path behind the rtol 1e-3 / atol 1e-5 parity gate: all reductions accumulate in fp32,
 // transcendental functions are the accurate (non fast-math) variants.  With T = bf16 the same
 // kernels serve as the fallback for shapes the tensor-core (wgmma) kernels do not cover.
+#include <algorithm>
 #include <cmath>
 
 #include "model_kernels.cuh"
@@ -434,6 +435,62 @@ struct KeySet {
     if (shift > 0) {   // seam mask (:300-315): only the first window row/col contains wrapped tokens
       if (wi == 0 && ((lqi < shift) != (a < shift))) return -1;
       if (wj == 0 && ((lqj < shift) != (b < shift))) return -1;
+    }
+    const int oi = (wi * param + a - shift + h) % h, oj = (wj * param + b - shift + w) % w;
+    return oi * w + oj;
+  }
+};
+
+// The inverse of KeySet: the queries whose key set contains key token `kt` (the key-centric pass of the attention VJP).
+//   global: every query.
+//   shifted window: the queries of the key's rolled window on the key's side of the seam (the seam mask is symmetric).
+//   neighbourhood: per axis the queries with s(i) <= a < s(i) + k, s(i) = clamp(i - k/2, 0, n - k); s is monotone, so they form one
+//   contiguous range: k queries inside the grid, up to 3 (k/2) + 1 near a border.
+struct QuerySet {
+  int type, h, w, param, shift;
+  int i0, j0, ni, nj;   // neighbourhood: query row/column ranges [i0, i0+ni) x [j0, j0+nj)
+  int wi, wj, la, lb;   // shifted-window: the key's window and local coords (rolled frame)
+  __device__ static int max_count(int type, int h, int w, int param) {
+    if (type == KDB_ATTN_GLOBAL) return h * w;
+    if (type == KDB_ATTN_NEIGHBORHOOD) return (3 * (param / 2) + 1) * (3 * (param / 2) + 1);
+    return param * param;
+  }
+  __device__ static void range(int a, int n, int k, int& lo, int& cnt) {
+    lo = n;
+    int hi = -1;
+    for (int i = max(0, a - 2 * k); i <= min(n - 1, a + 2 * k); ++i) {
+      const int s = min(max(i - k / 2, 0), n - k);
+      if (s <= a && a < s + k) {
+        lo = min(lo, i);
+        hi = max(hi, i);
+      }
+    }
+    cnt = hi - lo + 1;
+  }
+  __device__ int count() const {
+    if (type == KDB_ATTN_GLOBAL) return h * w;
+    if (type == KDB_ATTN_NEIGHBORHOOD) return ni * nj;
+    return param * param;
+  }
+  __device__ void init(int type_, int h_, int w_, int param_, int shift_, int kt) {
+    type = type_; h = h_; w = w_; param = param_; shift = shift_;
+    const int ki = kt / w, kj = kt - (kt / w) * w;
+    if (type == KDB_ATTN_NEIGHBORHOOD) {
+      range(ki, h, param, i0, ni);
+      range(kj, w, param, j0, nj);
+    } else if (type == KDB_ATTN_SHIFTED_WINDOW) {
+      const int ri = (ki + shift) % h, rj = (kj + shift) % w;
+      wi = ri / param; wj = rj / param; la = ri - wi * param; lb = rj - wj * param;
+    }
+  }
+  // token index of query t, or -1 if the seam mask hides the key from it
+  __device__ int token(int t) const {
+    if (type == KDB_ATTN_GLOBAL) return t;
+    if (type == KDB_ATTN_NEIGHBORHOOD) return (i0 + t / nj) * w + (j0 + t % nj);
+    const int a = t / param, b = t - a * param;   // the query's local coords in the key's window
+    if (shift > 0) {
+      if (wi == 0 && ((a < shift) != (la < shift))) return -1;
+      if (wj == 0 && ((b < shift) != (lb < shift))) return -1;
     }
     const int oi = (wi * param + a - shift + h) % h, oj = (wj * param + b - shift + w) % w;
     return oi * w + oj;
@@ -916,6 +973,502 @@ int launch_patch_out_jvp(const float* tokens, const float* dtokens, const float*
   patch_out_jvp_kernel<<<(unsigned)ceil_div(tok, 4), 128, smem, st>>>(tokens, dtokens, norm_scale, W, v_in, sigma, sigma_data, out, Cout, H,
                                                                       Wd, ph, pw, C0, tok);
   KDB_LAUNCH_CHECK(F_PATCH_OUT, st);
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Backward kernels of the reverse-mode derivative (VJP), fp32.  Each reads the primal input of one op (recomputed from the tape) and
+// the gradient of its output, and writes or adds the gradient of its input.  One writer per output element, no atomics, fixed
+// reduction orders: two calls on the same inputs give the same bits, and every gradient is linear in the cotangent using only
+// products with it, so scaling the cotangent by a power of two scales the result exactly.
+// ------------------------------------------------------------------------------------------------
+
+// dA[M,K] = dC[M,N] W[N,K] (the input gradient of C = A W^T): W is read along N, so no transposed copy exists.  64x64x16 tiles over
+// (M, K), 256 threads, 4x4 micro-tile per thread, like gemm_simt_kernel.  VJP_UNPATCH_ACC: row m is a coarse token (b, hy, wx) and
+// column k = (nh, nw, e); the result is added to the fine token (2hy+nh, 2wx+nw), channel e of out [B, 2hc, 2wc, Cf] -- the inverse
+// of the TokenMerge gather, a bijection, so each element still has one writer.
+template <int EPI>
+__global__ void __launch_bounds__(256) gemm_vjp_kernel(const float* __restrict__ dC, const float* __restrict__ W, float* __restrict__ out,
+                                                       int64_t M, int N, int K, int hc, int wc, int Cf) {
+  __shared__ __align__(16) float As[GBK][GBM + GPAD];
+  __shared__ __align__(16) float Ws[GBK][GBN + GPAD];
+  const int tid = threadIdx.x;
+  const int64_t m0 = (int64_t)blockIdx.y * GBM;
+  const int k0 = blockIdx.x * GBN;
+  const int lr = tid >> 2, lk = (tid & 3) * 4;    // dC loader: row 0..63, reduction offset 0,4,8,12
+  const int wr = tid >> 4, wc4 = (tid & 15) * 4;  // W loader: reduction row 0..15, column offset 0..60
+  const int ty = tid >> 4, tx = tid & 15;
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+
+  for (int n0 = 0; n0 < N; n0 += GBK) {
+    float av[4], wv[4];
+    load4<float>(dC + (m0 + lr) * N + n0 + lk, (m0 + lr) < M && (n0 + lk) < N, av);
+    load4<float>(W + (int64_t)(n0 + wr) * K + k0 + wc4, (n0 + wr) < N && (k0 + wc4) < K, wv);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) As[lk + i][lr] = av[i];
+    *reinterpret_cast<float4*>(&Ws[wr][wc4]) = make_float4(wv[0], wv[1], wv[2], wv[3]);
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < GBK; ++kk) {
+      const float4 a = *reinterpret_cast<const float4*>(&As[kk][ty * 4]);
+      const float4 b = *reinterpret_cast<const float4*>(&Ws[kk][tx * 4]);
+      const float aa[4] = {a.x, a.y, a.z, a.w}, bb[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int64_t m = m0 + ty * 4 + i;
+    if (m >= M) continue;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = k0 + tx * 4 + j;
+      if (k >= K) continue;
+      if constexpr (EPI == VJP_STORE) {
+        out[m * K + k] = acc[i][j];
+      } else {
+        const int64_t b = m / ((int64_t)hc * wc);
+        const int r = (int)(m - b * hc * wc);
+        const int hy = r / wc, wx = r - hy * wc;
+        const int q = k / Cf, e = k - q * Cf;
+        const int64_t dst = ((b * (2 * hc) + (2 * hy + (q >> 1))) * (2 * wc) + (2 * wx + (q & 1))) * Cf + e;
+        out[dst] += acc[i][j];
+      }
+    }
+  }
+}
+
+int launch_gemm_vjp(const float* dC, const float* W, float* out, int64_t M, int N, int K, int epi, int hc, int wc, int Cf, cudaStream_t st) {
+  KDB_REQUIRE(N % 4 == 0 && K % 4 == 0, KDB_ERR_BAD_SHAPE, "gemm_vjp: N=%d and K=%d must be multiples of 4", N, K);
+  KDB_REQUIRE(M > 0, KDB_ERR_BAD_SHAPE, "gemm_vjp: empty problem");
+  KDB_REQUIRE(epi == VJP_STORE || (K == 4 * Cf && M % ((int64_t)hc * wc) == 0), KDB_ERR_BAD_SHAPE, "gemm_vjp: bad un-patch geometry");
+  const int64_t chunk = 65535LL * GBM;   // split M so gridDim.y stays legal (whole images per chunk for the un-patch epilogue)
+  const int64_t step = epi == VJP_STORE ? chunk : std::max<int64_t>(chunk / ((int64_t)hc * wc), 1) * hc * wc;
+  for (int64_t mo = 0; mo < M; mo += step) {
+    const int64_t Mi = std::min(step, M - mo);
+    dim3 grid((unsigned)ceil_div(K, GBN), (unsigned)ceil_div(Mi, GBM));
+    KDB_REQUIRE(grid.y <= 65535u, KDB_ERR_BAD_SHAPE, "gemm_vjp: image too large");
+    if (epi == VJP_STORE)
+      gemm_vjp_kernel<VJP_STORE><<<grid, 256, 0, st>>>(dC + mo * N, W, out + mo * K, Mi, N, K, 0, 0, 0);
+    else
+      gemm_vjp_kernel<VJP_UNPATCH_ACC><<<grid, 256, 0, st>>>(dC + mo * N, W, out + mo * K, Mi, N, K, hc, wc, Cf);
+    KDB_LAUNCH_CHECK(F_GEMM_SIMT, st);
+  }
+  return 0;
+}
+
+// dx += r (s dy) - x r^3 mean(x s dy), r = rsqrt(mean(x^2) + eps): the input gradient of (Ada)RMSNorm added to dx.  One warp per row.
+__global__ void __launch_bounds__(256) rmsnorm_vjp_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx,
+                                                          const float* __restrict__ scale, int64_t scale_bstride, int64_t rows_per_batch,
+                                                          int64_t rows, int C) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const float* xr = x + row * C;
+  const float* gr = dy + row * C;
+  const float* sc = scale + (row / rows_per_batch) * scale_bstride;
+  float ss = 0.f, sd = 0.f;
+  for (int c = lane; c < C; c += 32) {
+    ss = fmaf(xr[c], xr[c], ss);
+    sd = fmaf(xr[c], __ldg(sc + c) * gr[c], sd);
+  }
+  ss = warp_sum(ss);
+  sd = warp_sum(sd);
+  const float r = rsqrtf(ss / (float)C + kEps);
+  const float r3m = r * r * r * (sd / (float)C);
+  float* dr = dx + row * C;
+  for (int c = lane; c < C; c += 32) dr[c] += r * (__ldg(sc + c) * gr[c]) - xr[c] * r3m;
+}
+
+int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
+                       int64_t rows, int C, cudaStream_t st) {
+  rmsnorm_vjp_kernel<<<(unsigned)ceil_div(rows, 8), 256, 0, st>>>(x, dy, dx, scale, scale_bstride, rows_per_batch, rows, C);
+  KDB_LAUNCH_CHECK(F_RMSNORM, st);
+  return 0;
+}
+
+// In place on the q and k thirds of dqkv: g = R(theta)^T dq^ (rotate by -theta on the primal's column pairs), then
+// dq = sqrt(scale) (rho g - q rho^3 (q . g)), rho = rsqrt(sum q^2 + eps) of the un-normalised primal q in qkv.  One warp per
+// (token row, head).
+__global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __restrict__ qkv, float* __restrict__ dqkv,
+                                                              const float* __restrict__ pos, const float* __restrict__ freqs,
+                                                              const float* __restrict__ scale, int64_t rows, int Ttok, int nh, int e) {
+  extern __shared__ float sm[];   // [warps][e]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
+  if (item >= rows * nh) return;
+  const int64_t row = item / nh;
+  const int h = (int)(item - row * nh);
+  float* buf = sm + (size_t)warp * e;
+  const int dr = e / 4, nf = e / 8;
+  const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
+  const float sqs = sqrtf(scale[h]);
+#pragma unroll
+  for (int t = 0; t < 2; ++t) {
+    const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
+    const float* v = qkv + off;
+    float* dv = dqkv + off;
+    for (int d = lane; d < e; d += 32) {
+      float g;
+      if (d < 2 * dr) {
+        const int j = d < dr ? d : d - dr;
+        const float theta = (j < nf ? py : px) * freqs[h * nf + (j < nf ? j : j - nf)];
+        float s, c;
+        sincosf(theta, &s, &c);
+        const float g1 = dv[j], g2 = dv[j + dr];
+        g = d < dr ? g1 * c + g2 * s : g2 * c - g1 * s;
+      } else {
+        g = dv[d];
+      }
+      buf[d] = g;
+    }
+    __syncwarp();
+    float ss = 0.f, sg = 0.f;
+    for (int d = lane; d < e; d += 32) {
+      ss = fmaf(v[d], v[d], ss);
+      sg = fmaf(v[d], buf[d], sg);
+    }
+    ss = warp_sum(ss);
+    sg = warp_sum(sg);
+    const float rho = rsqrtf(ss + kEps);
+    const float r3s = rho * rho * rho * sg;
+    for (int d = lane; d < e; d += 32) dv[d] = sqs * (rho * buf[d] - v[d] * r3s);
+    __syncwarp();
+  }
+}
+
+int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
+                           int nh, int e, cudaStream_t st) {
+  KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope_vjp: d_head %d must be a multiple of 8", e);
+  const size_t smem = sizeof(float) * 4 * e;
+  qknorm_rope_vjp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, freqs, scale, rows, T_tokens, nh, e);
+  KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
+  return 0;
+}
+
+// Attention VJP, query-centric pass: one warp per (batch, head, query i) over the key set of attn_generic_kernel.
+//   Delta_i = dO_i . O_i,  dS_ij = P_ij (dO_i . v_j - Delta_i),  dq_i = sum_j dS_ij k_j
+// It also leaves (row maximum, 1 / row sum, Delta_i) of query i in stats [B, nh, T, 3] for the key-centric pass.
+__global__ void __launch_bounds__(128) attn_vjp_q_kernel(const float* __restrict__ qkv, const float* __restrict__ o, const float* __restrict__ dout,
+                                                         float* __restrict__ dqkv, float* __restrict__ stats, int h, int w, int nh, int e,
+                                                         int type, int param, int shift, int maxkeys) {
+  extern __shared__ float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int Ttok = h * w;
+  const int q = blockIdx.x * 4 + warp;
+  const int head = blockIdx.y;
+  const int64_t b = blockIdx.z;
+  float* qv = sm + (size_t)warp * (2 * e + 2 * maxkeys);
+  float* dov = qv + e;
+  float* sc = dov + e;
+  int* toks = reinterpret_cast<int*>(sc + maxkeys);
+  if (q >= Ttok) return;
+  const int64_t rs = 3LL * nh * e;
+  const float* base = qkv + b * Ttok * rs;
+  const int64_t orow = (b * Ttok + q) * (int64_t)nh * e + (int64_t)head * e;
+  float delta = 0.f;
+  for (int d = lane; d < e; d += 32) {
+    qv[d] = base[(int64_t)q * rs + (int64_t)head * e + d];
+    dov[d] = dout[orow + d];
+    delta = fmaf(dov[d], o[orow + d], delta);
+  }
+  delta = warp_sum(delta);
+  __syncwarp();
+  KeySet ks;
+  ks.init(type, h, w, param, shift, q);
+  const int nk = ks.count();
+  float mx = -INFINITY;
+  for (int j = lane; j < nk; j += 32) {
+    const int tok = ks.token(j);
+    float s = -INFINITY;
+    if (tok >= 0) {
+      const float* kp = base + (int64_t)tok * rs + (int64_t)(nh + head) * e;
+      s = 0.f;
+      for (int d = 0; d < e; ++d) s = fmaf(qv[d], kp[d], s);
+    }
+    sc[j] = s;
+    toks[j] = tok;
+    mx = fmaxf(mx, s);
+  }
+  mx = warp_max(mx);
+  float sum = 0.f;
+  for (int j = lane; j < nk; j += 32) sum += (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
+  sum = warp_sum(sum);
+  const float inv = 1.f / sum;
+  for (int j = lane; j < nk; j += 32) {
+    const int tok = toks[j];
+    float ds = 0.f;
+    if (tok >= 0) {
+      const float* vp = base + (int64_t)tok * rs + (int64_t)(2 * nh + head) * e;
+      float dp = 0.f;
+      for (int d = 0; d < e; ++d) dp = fmaf(dov[d], vp[d], dp);
+      ds = expf(sc[j] - mx) * inv * (dp - delta);
+    }
+    sc[j] = ds;
+  }
+  __syncwarp();
+  float* dq = dqkv + (b * Ttok + q) * rs + (int64_t)head * e;
+  for (int d = lane; d < e; d += 32) {
+    float acc = 0.f;
+    for (int j = 0; j < nk; ++j) {
+      const int tok = toks[j];
+      if (tok >= 0) acc = fmaf(sc[j], base[(int64_t)tok * rs + (int64_t)(nh + head) * e + d], acc);
+    }
+    dq[d] = acc;
+  }
+  if (lane == 0) {
+    float* st = stats + ((b * nh + head) * Ttok + q) * 3;
+    st[0] = mx;
+    st[1] = inv;
+    st[2] = delta;
+  }
+}
+
+// Attention VJP, key-centric pass: one warp per (batch, head, key j) over the queries that see key j (QuerySet).
+//   dk_j = sum_i dS_ij q_i,  dv_j = sum_i P_ij dO_i
+__global__ void __launch_bounds__(128) attn_vjp_kv_kernel(const float* __restrict__ qkv, const float* __restrict__ dout, const float* __restrict__ stats,
+                                                          float* __restrict__ dqkv, int h, int w, int nh, int e, int type, int param, int shift,
+                                                          int maxq) {
+  extern __shared__ float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int Ttok = h * w;
+  const int kt = blockIdx.x * 4 + warp;
+  const int head = blockIdx.y;
+  const int64_t b = blockIdx.z;
+  float* kv = sm + (size_t)warp * (2 * e + 3 * maxq);
+  float* vv = kv + e;
+  float* pv = vv + e;
+  float* dsv = pv + maxq;
+  int* toks = reinterpret_cast<int*>(dsv + maxq);
+  if (kt >= Ttok) return;
+  const int64_t rs = 3LL * nh * e;
+  const float* base = qkv + b * Ttok * rs;
+  for (int d = lane; d < e; d += 32) {
+    kv[d] = base[(int64_t)kt * rs + (int64_t)(nh + head) * e + d];
+    vv[d] = base[(int64_t)kt * rs + (int64_t)(2 * nh + head) * e + d];
+  }
+  __syncwarp();
+  QuerySet qs;
+  qs.init(type, h, w, param, shift, kt);
+  const int nq = qs.count();
+  const float* sb = stats + (b * nh + head) * (int64_t)Ttok * 3;
+  for (int t = lane; t < nq; t += 32) {
+    const int tok = qs.token(t);
+    float p = 0.f, ds = 0.f;
+    if (tok >= 0) {
+      const float* qp = base + (int64_t)tok * rs + (int64_t)head * e;
+      const float* dop = dout + (b * Ttok + tok) * (int64_t)nh * e + (int64_t)head * e;
+      float s = 0.f, dp = 0.f;
+      for (int d = 0; d < e; ++d) {
+        s = fmaf(qp[d], kv[d], s);
+        dp = fmaf(dop[d], vv[d], dp);
+      }
+      p = expf(s - sb[tok * 3 + 0]) * sb[tok * 3 + 1];
+      ds = p * (dp - sb[tok * 3 + 2]);
+    }
+    pv[t] = p;
+    dsv[t] = ds;
+    toks[t] = tok;
+  }
+  __syncwarp();
+  float* dk = dqkv + (b * Ttok + kt) * rs + (int64_t)(nh + head) * e;
+  float* dvv = dk + (int64_t)nh * e;
+  for (int d = lane; d < e; d += 32) {
+    float ak = 0.f, av = 0.f;
+    for (int t = 0; t < nq; ++t) {
+      const int tok = toks[t];
+      if (tok >= 0) {
+        ak = fmaf(dsv[t], base[(int64_t)tok * rs + (int64_t)head * e + d], ak);
+        av = fmaf(pv[t], dout[(b * Ttok + tok) * (int64_t)nh * e + (int64_t)head * e + d], av);
+      }
+    }
+    dk[d] = ak;
+    dvv[d] = av;
+  }
+}
+
+int launch_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int B, int h, int w, int nh, int e,
+                         int attn_type, int attn_param, int shift, cudaStream_t st) {
+  int maxkeys, maxq;
+  if (attn_type == KDB_ATTN_GLOBAL) {
+    maxkeys = maxq = h * w;
+  } else if (attn_type == KDB_ATTN_NEIGHBORHOOD || attn_type == KDB_ATTN_SHIFTED_WINDOW) {
+    maxkeys = attn_param * attn_param;   // geometry checked by the primal launch
+    maxq = attn_type == KDB_ATTN_NEIGHBORHOOD ? (3 * (attn_param / 2) + 1) * (3 * (attn_param / 2) + 1) : maxkeys;
+  } else {
+    KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "attention_vjp: bad type %d", attn_type);
+  }
+  const size_t smem_q = sizeof(float) * 4 * (size_t)(2 * e + 2 * maxkeys);
+  const size_t smem_kv = sizeof(float) * 4 * (size_t)(2 * e + 3 * maxq);
+  KDB_REQUIRE(smem_q <= 200 * 1024 && smem_kv <= 200 * 1024, KDB_ERR_UNSUPPORTED, "attention_vjp: %d keys exceed the shared-memory budget",
+              maxkeys);
+  static bool attr = false;
+  if (!attr) {
+    KDB_CUDA(cudaFuncSetAttribute(attn_vjp_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    KDB_CUDA(cudaFuncSetAttribute(attn_vjp_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr = true;
+  }
+  dim3 grid((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B);
+  attn_vjp_q_kernel<<<grid, 128, smem_q, st>>>(qkv, out, dout, dqkv, stats, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
+  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
+  attn_vjp_kv_kernel<<<grid, 128, smem_kv, st>>>(qkv, dout, stats, dqkv, h, w, nh, e, attn_type, attn_param, shift, maxq);
+  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
+  return 0;
+}
+
+// da = dy gelu(g), dg = dy a (Phi(g) + g phi(g)), erf form; h [M, 2F] the primal up_proj output, dh [M, 2F]
+__global__ void __launch_bounds__(256) geglu_vjp_kernel(const float* __restrict__ hp, const float* __restrict__ dy, float* __restrict__ dh,
+                                                        int64_t M, int F) {
+  const int64_t total = M * F;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int64_t m = i / F;
+    const int f = (int)(i - m * F);
+    const float a = hp[m * 2 * F + f], g = hp[m * 2 * F + F + f];
+    const float Phi = 0.5f * (1.f + erff(g * 0.70710678118654752440f));
+    const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
+    dh[m * 2 * F + f] = dy[i] * (g * Phi);
+    dh[m * 2 * F + F + f] = dy[i] * (a * fmaf(g, phi, Phi));
+  }
+}
+
+int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int F, cudaStream_t st) {
+  int64_t blocks = ceil_div(M * F, 256);
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  geglu_vjp_kernel<<<(unsigned)blocks, 256, 0, st>>>(h, dy, dh, M, F);
+  KDB_LAUNCH_CHECK(F_GEGLU, st);
+  return 0;
+}
+
+// TokenSplit VJP, elementwise part: dcur_patched = patch2x2(fac dup) -> out [B, H/2, W/2, (nh nw e)] (the TokenMerge gather order), and
+// dup <- (1 - fac) dup in place (the gradient the skip connection receives).  Same derivative on both branches of lerp_like_torch.
+__global__ void __launch_bounds__(256) split_vjp_gather_kernel(float* __restrict__ dup, float* __restrict__ out, const float* __restrict__ fac,
+                                                               int H, int Wd, int C, int64_t total) {
+  const int hc = H / 2, wc = Wd / 2;
+  const float f = __ldg(fac), g = 1.f - f;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int e = (int)(i % C);
+    int64_t r = i / C;
+    const int q = (int)(r & 3);
+    r >>= 2;
+    const int wx = (int)(r % wc);
+    r /= wc;
+    const int hy = (int)(r % hc);
+    const int64_t b = r / hc;
+    const int64_t src = ((b * H + (2 * hy + (q >> 1))) * Wd + (2 * wx + (q & 1))) * C + e;
+    const float d = dup[src];
+    out[i] = f * d;
+    dup[src] = g * d;
+  }
+}
+
+int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int H, int Wd, int C, cudaStream_t st) {
+  KDB_REQUIRE(H % 2 == 0 && Wd % 2 == 0, KDB_ERR_BAD_SHAPE, "token split vjp: grid %dx%d not even", H, Wd);
+  const int64_t total = (int64_t)B * H * Wd * C;
+  int64_t blocks = ceil_div(total, 256);
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  split_vjp_gather_kernel<<<(unsigned)blocks, 256, 0, st>>>(dup, out, fac, H, Wd, C, total);
+  KDB_LAUNCH_CHECK(F_MERGE_GATHER, st);
+  return 0;
+}
+
+// patch_out + out_norm VJP: per token, dy = patch(c_out u) (c_out = 1 for the raw model), dxn = dy W_po, dt = RMSNorm_vjp(tokens, dxn)
+// written to dtokens.  One warp per token.
+__global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restrict__ tokens, const float* __restrict__ nscale,
+                                                            const float* __restrict__ W, const float* __restrict__ u, const float* __restrict__ sigma,
+                                                            float sd, float* __restrict__ dtokens, int Cout, int H, int Wd, int ph, int pw,
+                                                            int C0, int64_t tokens_total) {
+  extern __shared__ float sm[];   // [warps][C0 + N]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t tok = (int64_t)blockIdx.x * 4 + warp;
+  if (tok >= tokens_total) return;
+  const int N = ph * pw * Cout;
+  float* dn = sm + (size_t)warp * (C0 + N);
+  float* dy = dn + C0;
+  const int th_n = H / ph, tw_n = Wd / pw;
+  const int64_t b = tok / ((int64_t)th_n * tw_n);
+  const int rr = (int)(tok - b * th_n * tw_n);
+  const int ty = rr / tw_n, tx = rr - ty * tw_n;
+  float c_skip, c_out = 1.f, c_in;
+  if (sd > 0.f) karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
+  for (int n = lane; n < N; n += 32) {
+    const int q = n / Cout, c = n - q * Cout;
+    const int nh = q / pw, nw = q - nh * pw;
+    dy[n] = c_out * u[((b * Cout + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw)];
+  }
+  __syncwarp();
+  for (int k = lane; k < C0; k += 32) {
+    float acc = 0.f;
+    for (int n = 0; n < N; ++n) acc = fmaf(dy[n], __ldg(W + (int64_t)n * C0 + k), acc);
+    dn[k] = acc;
+  }
+  __syncwarp();
+  const float* xr = tokens + tok * C0;
+  float ss = 0.f, sdot = 0.f;
+  for (int c = lane; c < C0; c += 32) {
+    ss = fmaf(xr[c], xr[c], ss);
+    sdot = fmaf(xr[c], __ldg(nscale + c) * dn[c], sdot);
+  }
+  ss = warp_sum(ss);
+  sdot = warp_sum(sdot);
+  const float r = rsqrtf(ss / (float)C0 + kEps);
+  const float r3m = r * r * r * (sdot / (float)C0);
+  float* dr = dtokens + tok * C0;
+  for (int c = lane; c < C0; c += 32) dr[c] = r * (__ldg(nscale + c) * dn[c]) - xr[c] * r3m;
+}
+
+int launch_patch_out_vjp(const float* tokens, const float* norm_scale, const float* W, const float* u, const float* sigma, float sigma_data,
+                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st) {
+  const int64_t tok = (int64_t)B * (H / ph) * (Wd / pw);
+  const size_t smem = sizeof(float) * 4 * (size_t)(C0 + ph * pw * Cout);
+  KDB_REQUIRE(smem <= 48 * 1024, KDB_ERR_UNSUPPORTED, "patch_out_vjp: width %d too large", C0);
+  patch_out_vjp_kernel<<<(unsigned)ceil_div(tok, 4), 128, smem, st>>>(tokens, norm_scale, W, u, sigma, sigma_data, dtokens, Cout, H, Wd, ph, pw,
+                                                                      C0, tok);
+  KDB_LAUNCH_CHECK(F_PATCH_OUT, st);
+  return 0;
+}
+
+// patch_in VJP with the Karras combine's skip term: grad_x = c_skip u + c_in unpatch(dt0 W_pi) (sigma_data > 0), else unpatch(dt0 W_pi).
+// One thread per input element; W_pi [N, K] with K = (nh, nw, c).
+__global__ void __launch_bounds__(256) patch_in_vjp_kernel(const float* __restrict__ dtok, const float* __restrict__ W, const float* __restrict__ u,
+                                                           const float* __restrict__ sigma, float sd, float* __restrict__ grad, int C, int H, int Wd,
+                                                           int ph, int pw, int N, int64_t total) {
+  const int K = ph * pw * C;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int xx = (int)(i % Wd);
+    int64_t r = i / Wd;
+    const int y = (int)(r % H);
+    r /= H;
+    const int c = (int)(r % C);
+    const int64_t b = r / C;
+    const int64_t tok = (b * (H / ph) + y / ph) * (Wd / pw) + xx / pw;
+    const int k = ((y % ph) * pw + (xx % pw)) * C + c;
+    const float* dr = dtok + tok * N;
+    float acc = 0.f;
+    for (int n = 0; n < N; ++n) acc = fmaf(dr[n], __ldg(W + (int64_t)n * K + k), acc);
+    if (sd > 0.f) {
+      float c_skip, c_out, c_in;
+      karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
+      acc = c_skip * u[i] + c_in * acc;
+    }
+    grad[i] = acc;
+  }
+}
+
+int launch_patch_in_vjp(const float* dtokens, const float* W, const float* u, const float* sigma, float sigma_data, float* grad_x, int B, int C,
+                        int H, int Wd, int ph, int pw, int N, cudaStream_t st) {
+  const int64_t total = (int64_t)B * C * H * Wd;
+  int64_t blocks = ceil_div(total, 256);
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  patch_in_vjp_kernel<<<(unsigned)blocks, 256, 0, st>>>(dtokens, W, u, sigma, sigma_data, grad_x, C, H, Wd, ph, pw, N, total);
+  KDB_LAUNCH_CHECK(F_PATCH_IN, st);
   return 0;
 }
 

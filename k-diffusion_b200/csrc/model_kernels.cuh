@@ -85,6 +85,34 @@ int launch_geglu_jvp(const float* h, const float* dh, float* dout, int64_t M, in
 int launch_patch_out_jvp(const float* tokens, const float* dtokens, const float* norm_scale, const float* W, const float* v_in, const float* sigma,
                          float sigma_data, float* out, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st);
 
+// Backward kernels of the reverse-mode derivative (fp32).  Each takes the primal input of one op (recomputed from the tape by the op's
+// forward launch) and the gradient of its output, and writes (or, where named, adds) the gradient of its input.  No atomics.
+enum GemmVjpEpilogue { VJP_STORE = 0, VJP_UNPATCH_ACC = 1 };
+// dA[M,K] = dC[M,N] W[N,K], the input gradient of C = A W^T, W read along N (no transposed copy).  VJP_UNPATCH_ACC: rows are coarse
+// tokens of [B, hc, wc], columns (nh nw e) with e < Cf; the result is ADDED to the fine tokens out [B, 2hc, 2wc, Cf] (TokenMerge VJP)
+int launch_gemm_vjp(const float* dC, const float* W, float* out, int64_t M, int N, int K, int epi, int hc, int wc, int Cf, cudaStream_t st);
+// RMSNorm: dx += r (s dy) - x r^3 mean(x s dy), r = rsqrt(mean(x^2) + eps); scale rows as launch_rmsnorm
+int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
+                       int64_t rows, int C, cudaStream_t st);
+// cosine-sim scale + RoPE, in place on the q, k thirds of dqkv [rows, 3, nh, e] (v passes through); qkv = the primal BEFORE launch_qknorm_rope
+int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
+                           int nh, int e, cudaStream_t st);
+// attention over the key set of launch_attention_generic: qkv the normalised, rotated primal, out its output, dout the output gradient
+// -> dqkv [B, T, 3, nh, e].  stats: scratch of B * nh * T * 3 floats (per-query softmax statistics handed from the query-centric pass
+// to the key-centric one)
+int launch_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int B, int h, int w, int nh, int e,
+                         int attn_type, int attn_param, int shift, cudaStream_t st);
+// GEGLU: h [M, 2F] primal up_proj output, dy [M, F] -> dh [M, 2F]
+int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int F, cudaStream_t st);
+// TokenSplit lerp: out [B, H/2, W/2, 4C] = patch2x2(fac dup) (then launch_gemm_vjp with the split weight), dup *= (1 - fac) in place
+int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int H, int Wd, int C, cudaStream_t st);
+// out_norm + patch_out + un-patch: dtokens = RMSNorm_vjp(tokens, patch(c_out u) W_po)  (c_out = 1 when sigma_data <= 0)
+int launch_patch_out_vjp(const float* tokens, const float* norm_scale, const float* W, const float* u, const float* sigma, float sigma_data,
+                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st);
+// patch_in: grad_x = c_skip u + c_in unpatch(dtokens W_pi) (sigma_data > 0), else unpatch(dtokens W_pi)
+int launch_patch_in_vjp(const float* dtokens, const float* W, const float* u, const float* sigma, float sigma_data, float* grad_x, int B, int C,
+                        int H, int Wd, int ph, int pw, int N, cudaStream_t st);
+
 // tiled fast variants (patch_kernels.cu); return false when the shape is outside their envelope
 template <typename T>
 bool launch_patch_in_tiled(const float* x, const float* sigma, float sigma_data, const float* W, T* out, int B, int C, int H, int Wd, int ph,

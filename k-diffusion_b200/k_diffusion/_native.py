@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -63,6 +63,8 @@ SIGNATURES = {
     "kdb_model_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
     "kdb_model_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_model_forward_jvp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_model_vjp_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
+    "kdb_model_forward_vjp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_model_tap_count": (_i64, [_vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
@@ -432,6 +434,27 @@ class Engine:
             check(lib().kdb_model_forward_jvp(self._h, PREC_FP32, B, H, W, ptr(x), ptr(v), ptr(sigma), float(sigma_data), ptr(cond),
                                               cond_batch_stride, ptr(out), ptr(out_tangent), ptr(ws), ws.numel(), stream()))
         return out, out_tangent
+
+    def forward_vjp(self, x, u, sigma, cond, cond_batch_stride, sigma_data, out=None, out_grad=None):
+        """Reverse-mode derivative on the fp32 path: -> (out, grad_x), out as forward() at fp32, grad_x = u^T J(x).
+        x [B,C_in,H,W] and u [B,C_out,H,W] fp32 contiguous; the workspace holds the forward's tape (kdb_model_vjp_workspace_bytes)."""
+        B, _, H, W = x.shape
+        shape = (B, self.cfg.out_channels, H, W)
+        if tuple(u.shape) != shape:
+            raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {shape}")
+        out = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
+        out_grad = torch.empty_like(x) if out_grad is None else out_grad
+        need = int(lib().kdb_model_vjp_workspace_bytes(self._h, B, H, W))
+        if need < 0:
+            check(need)
+        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
+            self._ws = None
+            self._ws = torch.empty(need, dtype=torch.uint8, device=x.device)
+        ws = self._ws
+        with device_of(x):
+            check(lib().kdb_model_forward_vjp(self._h, PREC_FP32, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
+                                              ptr(u), ptr(out), ptr(out_grad), ptr(ws), ws.numel(), stream()))
+        return out, out_grad
 
     def arm_tap(self, name, capacity, device):
         buf = torch.empty(capacity, dtype=torch.float32, device=device)

@@ -66,6 +66,23 @@ class Denoiser(nn.Module):
         f, df = torch.func.jvp(lambda xx: self.inner_model(xx * c_in, sigma, **kwargs), (x,), (t,))
         return _native.precond_combine(_native.f32c(f), x, sig, sd), _native.precond_combine(_native.f32c(df), t, sig, sd)
 
+    def vjp(self, input, sigma, cotangent, **kwargs):
+        """(D(x, sigma), cotangent^T J_D(x)): the denoiser and its reverse-mode derivative with respect to `input`.
+
+        A native inner model computes both in one fp32 engine call.  Any other inner model goes through `torch.func.vjp` of
+        inner(c_in x), whose gradient g = c_in J_F^T u is linear in u, so c_skip u + c_in J_F^T (c_out u) = c_out g + c_skip u is
+        one combine kernel, as in `jvp`."""
+        _native.require_cuda(input, sigma, cotangent)
+        if self.is_native():
+            return self.inner_model.denoise_vjp(input, sigma, cotangent, self.sigma_data, **kwargs)
+        x, u = _native.f32c(input), _native.f32c(cotangent)
+        sig = _native.f32c(sigma).expand(x.shape[0]).contiguous()
+        sd = float(self.sigma_data)
+        c_in = (1 / (sig * sig + sd * sd).sqrt()).view(-1, *([1] * (x.ndim - 1)))
+        f, pull = torch.func.vjp(lambda xx: self.inner_model(xx * c_in, sigma, **kwargs), x)
+        (g,) = pull(u.to(f.dtype))
+        return _native.precond_combine(_native.f32c(f), x, sig, sd), _native.precond_combine(_native.f32c(g), u, sig, sd)
+
 
 class DenoiserWithVariance(Denoiser):
     """reference layers.py:93-101: differs from Denoiser in `loss` only (training, out of scope); sampling is identical."""

@@ -226,30 +226,39 @@ class ImageTransformerDenoiserModelV2(nn.Module):
         return self.engine().conditioning(sigma, aug_cond, class_cond if self.class_emb is not None else None,
                                           mapping_cond if self.mapping_cond_in_proj is not None else None)
 
-    def _run(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out=None, tangent=None):
-        _native.require_cuda(x, sigma, tangent)
+    def _inputs(self, x, sigma, aug_cond, class_cond, mapping_cond):
+        """(engine, fp32 x, sigma [B], conditioning rows) of one evaluation; the caller has made x's device current."""
+        xin = _native.f32c(x)
+        sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
+        if sig.shape != (x.shape[0],):
+            raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
+        eng = self.engine()
+        if self.class_emb is not None and not torch.cuda.is_current_stream_capturing():
+            eng.check_class_range(class_cond)           # nn.Embedding raises on out-of-range labels (reference :735)
+        cond = eng.conditioning(sig, aug_cond, class_cond if self.class_emb is not None else None,
+                                mapping_cond if self.mapping_cond_in_proj is not None else None)
+        return eng, xin, sig, cond
+
+    def _run(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out=None, tangent=None, cotangent=None):
+        _native.require_cuda(x, sigma, tangent, cotangent)
         if x.ndim != 4:
             raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
         if self.training and any(s.dropout > 0 for s in self.levels):
             raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
         self._check_cond(class_cond, mapping_cond)
+        if tangent is None and cotangent is None and torch.is_grad_enabled() and x.requires_grad:
+            return _autograd_eval(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out)
         with torch.cuda.device(x.device):
-            xin = _native.f32c(x)
-            sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
-            if sig.shape != (x.shape[0],):
-                raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
-            eng = self.engine()
-            if self.class_emb is not None and not torch.cuda.is_current_stream_capturing():
-                eng.check_class_range(class_cond)           # nn.Embedding raises on out-of-range labels (reference :735)
-            cond = eng.conditioning(sig, aug_cond, class_cond if self.class_emb is not None else None,
-                                    mapping_cond if self.mapping_cond_in_proj is not None else None)
-            if tangent is None:
-                res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
-            else:
+            eng, xin, sig, cond = self._inputs(x, sigma, aug_cond, class_cond, mapping_cond)
+            if tangent is not None:
                 if tangent.shape != x.shape:
                     raise ValueError(f"tangent must have the shape of x {tuple(x.shape)}, got {tuple(tangent.shape)}")
                 res = eng.forward_jvp(xin, _native.f32c(tangent), sig, cond, eng.cond_stride, sigma_data)
-        if tangent is not None:
+            elif cotangent is not None:
+                res = eng.forward_vjp(xin, _native.f32c(cotangent), sig, cond, eng.cond_stride, sigma_data)
+            else:
+                res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
+        if tangent is not None or cotangent is not None:
             return res if x.dtype == torch.float32 else tuple(r.to(x.dtype) for r in res)
         return res if x.dtype == torch.float32 else res.to(x.dtype)
 
@@ -270,3 +279,47 @@ class ImageTransformerDenoiserModelV2(nn.Module):
         """(D(x, sigma), J_D(x) v) of the Karras-preconditioned evaluation, J_D v = c_skip v + c_out J_F(c_in x) c_in v, in one engine
         call.  Always runs on the exact fp32 path, whatever `set_precision` selected."""
         return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, tangent=v)
+
+    def vjp(self, x, sigma, u, aug_cond=None, class_cond=None, mapping_cond=None):
+        """(F(x, sigma), u^T J_F(x)): the raw inner model and its reverse-mode derivative for the cotangent `u` with respect to x, in one
+        engine call.  Always runs on the exact fp32 path, whatever `set_precision` selected (the backward kernels are fp32 only)."""
+        return self._run(x, sigma, 0.0, aug_cond, class_cond, mapping_cond, cotangent=u)
+
+    def denoise_vjp(self, x, sigma, u, sigma_data, aug_cond=None, class_cond=None, mapping_cond=None):
+        """(D(x, sigma), u^T J_D(x)) of the Karras-preconditioned evaluation, u^T J_D = c_skip u + c_in J_F(c_in x)^T (c_out u), in one
+        engine call.  Always runs on the exact fp32 path, whatever `set_precision` selected."""
+        return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, cotangent=u)
+
+
+class _NativeEval(torch.autograd.Function):
+    """torch.autograd through the native engine with respect to x.  The forward is the ordinary engine call at the model's precision (its
+    value is bit-identical to a call without grad); the backward is one fp32 forward_vjp at the saved x, sigma and conditioning rows.  At
+    bf16 the gradient is therefore that of the fp32 function."""
+
+    @staticmethod
+    def forward(ctx, x, model, sigma, sigma_data, aug_cond, class_cond, mapping_cond):
+        with torch.cuda.device(x.device):
+            eng, xin, sig, cond = model._inputs(x, sigma, aug_cond, class_cond, mapping_cond)
+            res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, model.resolved_precision())
+        ctx.model, ctx.sigma_data, ctx.dtype = model, sigma_data, x.dtype
+        ctx.save_for_backward(xin, sig, cond)
+        return res if x.dtype == torch.float32 else res.to(x.dtype)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        xin, sig, cond = ctx.saved_tensors
+        with torch.cuda.device(xin.device):
+            eng = ctx.model.engine()
+            _, gx = eng.forward_vjp(xin, _native.f32c(grad_out), sig, cond, eng.cond_stride, ctx.sigma_data)
+        return gx.to(ctx.dtype), None, None, None, None, None, None
+
+
+def _autograd_eval(model, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out):
+    """An evaluation whose x requires grad: the gradient reaches x only, so other inputs that require grad are refused, not ignored."""
+    for name, t in (("sigma", sigma), ("aug_cond", aug_cond), ("mapping_cond", mapping_cond)):
+        if t is not None and t.requires_grad:
+            raise RuntimeError(f"the native model is differentiable with respect to x only, but {name} requires grad")
+    if out is not None:
+        raise RuntimeError("out= cannot be used when x requires grad (the result must carry a grad_fn)")
+    return _NativeEval.apply(x, model, sigma, sigma_data, aug_cond, class_cond, mapping_cond)

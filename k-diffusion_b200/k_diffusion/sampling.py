@@ -568,6 +568,11 @@ class _Evaluator:
         cond, stride = self._rows(k)
         return self.eng.forward_jvp(x, v, self.sigma_rows[k], cond, stride, self.sigma_data)
 
+    def vjp(self, k, x, u):
+        """(D(x, sigma_k), u^T J_D(x)): one reverse-mode engine call on the fp32 path (native, without CFG)"""
+        cond, stride = self._rows(k)
+        return self.eng.forward_vjp(x, u, self.sigma_rows[k], cond, stride, self.sigma_data)
+
 
 def _prepare(x, sigmas, extra_args):
     _native.require_cuda(x)
