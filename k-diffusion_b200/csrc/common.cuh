@@ -66,10 +66,33 @@ __device__ __forceinline__ void karras_scalings(float sigma, float sd, float& c_
   c_in = 1.0f / rs;
 }
 
+// Patch addressing: token tok of a [B, th, tw] token grid is token (ty, tx) of image b; pixel (y, x) of channel c of image b sits
+// at nchw_offset in an NCHW [B, C, H, W] image.
+__device__ __forceinline__ void token_coords(int64_t tok, int th, int tw, int& b, int& ty, int& tx) {
+  const int64_t per = (int64_t)th * tw;
+  b = (int)(tok / per);
+  const int r = (int)(tok - (int64_t)b * per);
+  ty = r / tw;
+  tx = r - ty * tw;
+}
+__device__ __forceinline__ int64_t nchw_offset(int b, int c, int y, int x, int C, int H, int W) {
+  return (((int64_t)b * C + c) * H + y) * W + x;
+}
+
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 constexpr int kNumSMs = 132;   // H100 SXM; the launchers query the device where it matters
+
+// Opens `kernel` to `bytes` of dynamic shared memory on its first launch (flag: one static per kernel).
+template <typename K>
+int set_smem_once(K kernel, bool& flag, int bytes) {
+  if (!flag) {
+    KDB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    flag = true;
+  }
+  return 0;
+}
 
 }  // namespace kdb
 

@@ -47,9 +47,7 @@ struct KdbModel {
   KdbModelConfig cfg{};
   std::unordered_map<std::string, TensorRef> tensors;
   bool finalized = false;
-  // execution order, which is also the order of the conditioning row: down levels, mid, up levels (outermost last).  Level l < n-1
-  // has depth[l] layers on the way down and as many on the way up.
-  std::vector<LayerPlan> layers;
+  std::vector<LayerPlan> layers;   // in execution order (for_each_layer)
   std::vector<const float*> merge_w, split_w, split_fac;
   const float *patch_in_w = nullptr, *out_norm = nullptr, *patch_out_w = nullptr;
   std::vector<bf16*> merge_wb, split_wb;
@@ -129,6 +127,22 @@ __global__ void interleave_geglu_rows_kernel(const float* __restrict__ w, bf16* 
     const int64_t src_row = (j < 8) ? (g * 8 + j) : ((int64_t)F + g * 8 + (j - 8));
     out[i] = __float2bfloat16_rn(w[src_row * C + c]);
   }
+}
+
+// The layers in execution order, which is also the order of KdbModel::layers and of the conditioning row: down levels, mid, up levels
+// (outermost last); level l < n-1 has depth[l] layers on the way down and as many on the way up.  f(prefix, level, index) receives
+// each layer's state-dict prefix, level and index within the level, which picks the shift (image_transformer_v2.py:697: an up level's
+// index continues after its down level).  Stops at the first nonzero return.
+template <typename F>
+int for_each_layer(const KdbModelConfig& c, F&& f) {
+  const int n = c.n_levels;
+  int rc = 0;
+  for (int l = 0; l < n - 1; ++l)
+    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = f("down_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i);
+  for (int i = 0; i < c.depth[n - 1] && rc == 0; ++i) rc = f("mid_level." + std::to_string(i) + ".", n - 1, i);
+  for (int l = n - 2; l >= 0; --l)
+    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = f("up_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i + c.depth[l]);
+  return rc;
 }
 
 int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, int index, int* ada_off, cudaStream_t st) {
@@ -352,8 +366,15 @@ struct Fwd {
   }
 };
 
+// The attention half's activations from the residual stream x, up to the attention output in ws.ao: the qkv projection goes to raw,
+// the cosine-normalised and rotated q, k (with v) to ws.qkv.  The forward passes raw = ws.qkv and cosine-sim + RoPE runs in place (so
+// on a JVP forward, where the tangent of q, k reads the projection, the raw tangent rows are in ws.qkv too); the reverse walk passes a
+// buffer of its own, which keeps the projection for the cosine-sim VJP.  Routes in priority order (fp32 has only the last):
+//   folded qkv GEMM: 1/rms from the row statistics, the AdaRMSNorm scale folded into the weight
+//   RMSNorm + QKV_ROPE GEMM
+//   RMSNorm + linear + qknorm_rope
 template <typename T>
-int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
+int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* raw) {
   const LayerPlan& L = m->layers[k];
   const float* pos = f.pt->pos[L.level];
   const float2* rope = f.pt->rope[k];
@@ -363,13 +384,23 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   T* xn = reinterpret_cast<T*>(f.ws.xn);
   T* qkv = reinterpret_cast<T*>(f.ws.qkv);
   T* ao = reinterpret_cast<T*>(f.ws.ao);
-  T* hb = reinterpret_cast<T*>(f.ws.hbuf);
-  T* gb = reinterpret_cast<T*>(f.ws.gbuf);
   const std::string tag = "layer" + std::to_string(k);
-  auto tapped = [&](const char* part) { return m->tap_out != nullptr && m->tap_name == tag + part; };
-  int rc = 0;
-  if (L.attn_type != KDB_ATTN_NONE) {
-    if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
+  auto norm = [&] {
+    int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
+    if constexpr (std::is_same_v<T, float>)
+      if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
+    return r ? r : tap<T>(m, tag + ".xn1", xn, Ma * C, f.st);
+  };
+  auto unfused = [&] {
+    int r = norm();
+    if (!r) r = linear<T>(xn, WSel<T>::qkv(L), raw, Ma, 3 * C, C, GemmEpi{}, f.st);
+    // the tangent reads the un-normalised primal q and k, so it runs before the primal launch
+    if constexpr (std::is_same_v<T, float>)
+      if (!r && f.jvp) r = launch_qknorm_rope_jvp(raw, raw + M * 3 * C, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+    return r ? r : launch_qknorm_rope<T>(raw, qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+  };
+  int rc;
+  if constexpr (std::is_same_v<T, bf16>) {
     GemmEpi qe;
     qe.mode = (L.e == 64 && rope != nullptr) ? EPI_QKV_ROPE : EPI_STORE;
     qe.C = C;
@@ -379,67 +410,77 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     qe.qk_scale = L.scale;
     GemmEpi qf = qe;
     qf.ss_in = f.ws.rowss;
-    auto norm = [&] {
-      int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
-      if constexpr (std::is_same_v<T, float>)
-        if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
-      return r ? r : tap<T>(m, tag + ".xn1", xn, Ma * C, f.st);
-    };
-    auto unfused = [&] {
-      int r = norm();
-      if (!r) r = linear<T>(xn, WSel<T>::qkv(L), qkv, Ma, 3 * C, C, GemmEpi{}, f.st);
-      // the tangent reads the un-normalised primal q and k, so it runs before the in-place primal launch
-      if constexpr (std::is_same_v<T, float>)
-        if (!r && f.jvp) r = launch_qknorm_rope_jvp(qkv, qkv + M * 3 * C, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
-      return r ? r : launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
-    };
-    // attention, routes in priority order (fp32 has only the last):
-    //   attn_block: the whole half in one kernel (128-wide shifted-window levels; not while .qkv or .ao is tapped)
-    //   folded qkv GEMM: 1/rms from the row statistics, the AdaRMSNorm scale folded into the weight
-    //   RMSNorm + QKV_ROPE GEMM
-    //   RMSNorm + linear + qknorm_rope
-    // then, after all but attn_block, attention and out_proj
+    if (f.fold && f.stats && tc_gemm_supported(M, 3 * C, C, qf)) {
+      rc = launch_gemm_tc(x, L.qkv_wf, qkv, M, 3 * C, C, qf, f.st);
+      if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+    } else if (qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
+      if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv_wb, qkv, M, 3 * C, C, qe, f.st);
+    } else {
+      rc = unfused();
+    }
+  } else {
+    rc = unfused();
+  }
+  if (rc || (rc = tap<T>(m, tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
+  // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
+  if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
+    return rc;
+  if constexpr (std::is_same_v<T, float>)
+    if (f.jvp && (rc = launch_attention_jvp(qkv, qkv + M * 3 * C, ao + M * C, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st)))
+      return rc;
+  return tap<T>(m, tag + ".ao", ao, Ma * C, f.st);
+}
+
+// The feed-forward half's up projection from the residual stream x: RMSNorm into ws.xn, up_proj into ws.hbuf.  The forward's unfused
+// route and the reverse walk's recompute.
+template <typename T>
+int ff_up(KdbModel* m, Fwd& f, int k, const T* x, int h, int w) {
+  const LayerPlan& L = m->layers[k];
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok;
+  const int C = L.C;
+  T* xn = reinterpret_cast<T*>(f.ws.xn);
+  int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
+  if constexpr (std::is_same_v<T, float>)
+    if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
+  return r ? r : linear<T>(xn, WSel<T>::up(L), reinterpret_cast<T*>(f.ws.hbuf), f.images() * Ttok, 2 * L.dff, C, GemmEpi{}, f.st);
+}
+
+template <typename T>
+int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
+  const LayerPlan& L = m->layers[k];
+  const float2* rope = f.pt->rope[k];
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok, Ma = (int64_t)f.images() * Ttok;
+  const int C = L.C;
+  T* hb = reinterpret_cast<T*>(f.ws.hbuf);
+  T* gb = reinterpret_cast<T*>(f.ws.gbuf);
+  const std::string tag = "layer" + std::to_string(k);
+  auto tapped = [&](const char* part) { return m->tap_out != nullptr && m->tap_name == tag + part; };
+  int rc = 0;
+  if (L.attn_type != KDB_ATTN_NONE) {
+    if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
+    // attention: the whole half in one kernel (attn_block: 128-wide shifted-window levels; not while .qkv or .ao is tapped), or its
+    // activations (attn_activations) and out_proj
     const bool block = f.fold && f.stats && rope != nullptr && !tapped(".qkv") && !tapped(".ao") &&
                        tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift);
     if constexpr (std::is_same_v<T, bf16>) {
       if (block) {
-        rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st);
+        if ((rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st))) return rc;
         f.stats = true;
-      } else if (f.fold && f.stats && tc_gemm_supported(M, 3 * C, C, qf)) {
-        rc = launch_gemm_tc(x, L.qkv_wf, qkv, M, 3 * C, C, qf, f.st);
-        if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
-      } else if (qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
-        if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv_wb, qkv, M, 3 * C, C, qe, f.st);
-      } else {
-        rc = unfused();
       }
-    } else {
-      rc = unfused();
     }
-    if (rc) return rc;
     if (!block) {
-      if ((rc = tap<T>(m, tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
-      // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
-      if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
-        return rc;
-      if constexpr (std::is_same_v<T, float>)
-        if (f.jvp && (rc = launch_attention_jvp(qkv, qkv + M * 3 * C, ao + M * C, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st)))
-          return rc;
-      if ((rc = tap<T>(m, tag + ".ao", ao, Ma * C, f.st))) return rc;
+      if ((rc = attn_activations<T>(m, f, k, x, h, w, reinterpret_cast<T*>(f.ws.qkv)))) return rc;
       GemmEpi e;
       e.mode = EPI_RESID;
       e.resid = x;
       f.produce(e, Ma, C, C);
-      if ((rc = linear<T>(ao, WSel<T>::out(L), x, Ma, C, C, e, f.st))) return rc;
+      if ((rc = linear<T>(reinterpret_cast<T*>(f.ws.ao), WSel<T>::out(L), x, Ma, C, C, e, f.st))) return rc;
     }
     if ((rc = tap<T>(m, tag + ".attn", x, Ma * C, f.st))) return rc;
   }
   if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k + 1], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
   auto unfused = [&] {
-    int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-    if constexpr (std::is_same_v<T, float>)
-      if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-    if (!r) r = linear<T>(xn, WSel<T>::up(L), hb, Ma, 2 * L.dff, C, GemmEpi{}, f.st);
+    int r = ff_up<T>(m, f, k, x, h, w);
     if (!r) r = launch_geglu<T>(hb, gb, M, L.dff, f.st);
     if constexpr (std::is_same_v<T, float>)
       if (!r && f.jvp) r = launch_geglu_jvp(hb, hb + M * 2 * L.dff, gb + M * L.dff, M, L.dff, f.st);
@@ -453,6 +494,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   // then, after all but ffn_fused, down_proj
   const bool ffn = f.fold && f.stats && L.up_wf != nullptr && tc_ffn_fused_supported(M, C, L.dff) && !tapped(".geglu");
   if constexpr (std::is_same_v<T, bf16>) {
+    T* xn = reinterpret_cast<T*>(f.ws.xn);
     if (ffn) {
       rc = launch_ffn_fused(x, L.up_wf, L.down_wb, M, C, L.dff, f.ws.rowss, f.ws.rowss, f.st);
       f.stats = true;
@@ -484,9 +526,11 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
 // on M), each nonlinear one is followed by its tangent kernel.
 // tape != nullptr (fp32 only): the residual stream entering every attention / feed-forward half and out_norm is copied to the tape
 // (slots 2k, 2k+1 of layer k, slot 2 * layers for out_norm) for the reverse walk of kdb_model_forward_vjp; the launches are unchanged.
+// pos_tables != nullptr: receives the position tables of this token grid.
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
-                 int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st, float* const* tape = nullptr) {
+                 int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st, float* const* tape = nullptr,
+                 const PosTables** pos_tables = nullptr) {
   constexpr bool kBf16 = std::is_same_v<T, bf16>;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
@@ -494,6 +538,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   PosTables* pt = nullptr;
   int rc = ensure_pos(m, h0, w0, st, &pt);
   if (rc) return rc;
+  if (pos_tables) *pos_tables = pt;
   m->tap_count = 0;
   Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false, !kBf16 && v != nullptr};
   f.fold = f.emit && cond_bs == 0 && m->fold_descs != nullptr;
@@ -613,7 +658,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
 struct VjpSpace {
   std::vector<float*> tape;   // 2 per layer (KdbModel::layers order; nullptr for the attention half of a layer without one) + out_norm
   std::vector<float*> g;      // per level: gradient of the residual stream [B, T_l, C_l]
-  float *qkv_raw = nullptr;   // the qkv projection before launch_qknorm_rope normalises it in place
+  float *qkv_raw = nullptr;   // the qkv projection of the half being differentiated, before cosine-sim + RoPE
   float *dqkv = nullptr, *dbuf = nullptr, *dh = nullptr, *stats = nullptr;
   size_t total = 0;
 };
@@ -629,16 +674,12 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, char* base, Workspa
   const int n = c.n_levels;
   const int64_t T0 = (int64_t)(H / c.patch_h) * (W / c.patch_w);
   auto stream_floats = [&](int l) { return (size_t)B * (T0 >> (2 * l)) * c.width[l]; };
-  // layer levels in execution order (as kdb_model_finalize plans them)
-  std::vector<int> lv;
-  for (int l = 0; l < n - 1; ++l) lv.insert(lv.end(), c.depth[l], l);
-  lv.insert(lv.end(), c.depth[n - 1], n - 1);
-  for (int l = n - 2; l >= 0; --l) lv.insert(lv.end(), c.depth[l], l);
   vs.tape.clear();
-  for (int l : lv) {
+  for_each_layer(c, [&](const std::string&, int l, int) {
     vs.tape.push_back(c.attn_type[l] != KDB_ATTN_NONE ? take(stream_floats(l)) : nullptr);
     vs.tape.push_back(take(stream_floats(l)));
-  }
+    return 0;
+  });
   vs.tape.push_back(take(stream_floats(0)));
   vs.g.assign(n, nullptr);
   size_t mqkv = 0, md = 0, mh = 0, mst = 0;
@@ -660,51 +701,36 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, char* base, Workspa
   vs.total = off + 1024;
 }
 
-struct Bwd {
-  int B;
-  Workspace& ws;
-  VjpSpace& vs;
-  cudaStream_t st;
-  const float* cond;
-  int64_t cond_bs;
-  const PosTables* pt;
-};
-
 // Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
-// its activations from the tape with the forward's own launches, runs the backward kernels and adds the branch gradient to g.
-int vjp_layer(KdbModel* m, Bwd& b, int k, float* g, int h, int w) {
+// its activations from the tape with the forward's functions (ff_up, attn_activations; f is an fp32 forward of B images), runs the
+// backward kernels and adds the branch gradient to g.
+int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w) {
   const LayerPlan& L = m->layers[k];
-  const int64_t Ttok = (int64_t)h * w, M = (int64_t)b.B * Ttok;
+  const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok;
   const int C = L.C, F = L.dff;
-  float* xn = reinterpret_cast<float*>(b.ws.xn);
-  float* qkv = reinterpret_cast<float*>(b.ws.qkv);
-  float* ao = reinterpret_cast<float*>(b.ws.ao);
-  float* hb = reinterpret_cast<float*>(b.ws.hbuf);
-  cudaStream_t st = b.st;
+  float* xn = reinterpret_cast<float*>(f.ws.xn);
+  float* qkv = reinterpret_cast<float*>(f.ws.qkv);
+  float* ao = reinterpret_cast<float*>(f.ws.ao);
+  float* hb = reinterpret_cast<float*>(f.ws.hbuf);
+  cudaStream_t st = f.st;
   int rc;
   // feed-forward half: x + down(geglu(up(norm(x))))
-  const float* x = b.vs.tape[2 * k + 1];
-  if ((rc = launch_rmsnorm<float>(x, xn, b.cond + L.ada_ff, b.cond_bs, Ttok, M, C, st))) return rc;
-  if ((rc = launch_gemm_simt<float, float>(xn, L.up_w, hb, M, 2 * F, C, GemmEpi{}, st))) return rc;
-  if ((rc = launch_gemm_vjp(g, L.down_w, b.vs.dbuf, M, C, F, VJP_STORE, 0, 0, 0, st))) return rc;
-  if ((rc = launch_geglu_vjp(hb, b.vs.dbuf, b.vs.dh, M, F, st))) return rc;
-  if ((rc = launch_gemm_vjp(b.vs.dh, L.up_w, xn, M, 2 * F, C, VJP_STORE, 0, 0, 0, st))) return rc;
-  if ((rc = launch_rmsnorm_vjp(x, xn, g, b.cond + L.ada_ff, b.cond_bs, Ttok, M, C, st))) return rc;
+  const float* x = vs.tape[2 * k + 1];
+  if ((rc = ff_up<float>(m, f, k, x, h, w))) return rc;
+  if ((rc = launch_gemm_vjp(g, L.down_w, vs.dbuf, M, C, F, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_geglu_vjp(hb, vs.dbuf, vs.dh, M, F, st))) return rc;
+  if ((rc = launch_gemm_vjp(vs.dh, L.up_w, xn, M, 2 * F, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, st))) return rc;
   if (L.attn_type == KDB_ATTN_NONE) return 0;
   // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
-  x = b.vs.tape[2 * k];
-  const float* pos = b.pt->pos[L.level];
-  if ((rc = launch_rmsnorm<float>(x, xn, b.cond + L.ada_attn, b.cond_bs, Ttok, M, C, st))) return rc;
-  if ((rc = launch_gemm_simt<float, float>(xn, L.qkv_w, b.vs.qkv_raw, M, 3 * C, C, GemmEpi{}, st))) return rc;
-  KDB_CUDA(cudaMemcpyAsync(qkv, b.vs.qkv_raw, sizeof(float) * M * 3 * C, cudaMemcpyDeviceToDevice, st));
-  if ((rc = launch_qknorm_rope<float>(qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
-  if ((rc = launch_attention_generic<float>(qkv, ao, b.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st))) return rc;
-  if ((rc = launch_gemm_vjp(g, L.out_w, b.vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
-  if ((rc = launch_attention_vjp(qkv, ao, b.vs.dbuf, b.vs.dqkv, b.vs.stats, b.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
+  x = vs.tape[2 * k];
+  if ((rc = attn_activations<float>(m, f, k, x, h, w, vs.qkv_raw))) return rc;
+  if ((rc = launch_gemm_vjp(g, L.out_w, vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
-  if ((rc = launch_qknorm_rope_vjp(b.vs.qkv_raw, b.vs.dqkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
-  if ((rc = launch_gemm_vjp(b.vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
-  return launch_rmsnorm_vjp(x, xn, g, b.cond + L.ada_attn, b.cond_bs, Ttok, M, C, st);
+  if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
+  if ((rc = launch_gemm_vjp(vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  return launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, st);
 }
 
 // out = the fp32 forward (bit for bit: the same launches, plus the tape copies), then grad_x = u^T J(x) by a walk of the forward in
@@ -712,14 +738,13 @@ int vjp_layer(KdbModel* m, Bwd& b, int k, float* g, int h, int w) {
 // first) its merge then its layers; patch_in.
 int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, const float* sigma, float sd, const float* cond, int64_t cond_bs,
              float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st) {
-  int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data());
+  const PosTables* pt = nullptr;
+  int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data(), &pt);
   if (rc) return rc;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
   const int h0 = H / c.patch_h, w0 = W / c.patch_w;
-  PosTables* pt = nullptr;
-  if ((rc = ensure_pos(m, h0, w0, st, &pt))) return rc;
-  Bwd b{B, ws, vs, st, cond, cond_bs, pt};
+  Fwd f{B, ws, st, cond, cond_bs, pt, false, false, false, false};
   if ((rc = launch_patch_out_vjp(vs.tape.back(), m->out_norm, m->patch_out_w, u, sigma, sd, vs.g[0], B, c.out_channels, H, W, c.patch_h,
                                  c.patch_w, C0, st)))
     return rc;
@@ -728,7 +753,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
   for (int l = 0; l < n - 1; ++l) {
     const int h = h0 >> l, w = w0 >> l;
     for (int i = 0; i < c.depth[l]; ++i)
-      if ((rc = vjp_layer(m, b, --k, vs.g[l], h, w))) return rc;
+      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w))) return rc;
     // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
     if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
     if ((rc = launch_gemm_vjp(mg, m->split_w[l], vs.g[l + 1], (int64_t)B * (h / 2) * (w / 2), 4 * c.width[l], c.width[l + 1], VJP_STORE, 0, 0, 0,
@@ -736,7 +761,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
       return rc;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
-    if ((rc = vjp_layer(m, b, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1)))) return rc;
+    if ((rc = vjp_layer(m, f, vs, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1)))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     const int h = h0 >> l, w = w0 >> l;
     // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added
@@ -744,7 +769,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
                               VJP_UNPATCH_ACC, h / 2, w / 2, c.width[l], st)))
       return rc;
     for (int i = 0; i < c.depth[l]; ++i)
-      if ((rc = vjp_layer(m, b, --k, vs.g[l], h, w))) return rc;
+      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w))) return rc;
   }
   return launch_patch_in_vjp(vs.g[0], m->patch_in_w, u, sigma, sd, grad_x, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
 }
@@ -799,17 +824,11 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->split_fac.assign(n, nullptr);
   m->merge_wb.assign(n, nullptr);
   m->split_wb.assign(n, nullptr);
-  int ada = 0, rc = 0;
-  // execution order; the layer index picks the shift (image_transformer_v2.py:697: an up level's index continues after its down level)
-  auto plan = [&](const std::string& prefix, int level, int index) {
+  int ada = 0;
+  int rc = for_each_layer(c, [&](const std::string& prefix, int level, int index) {
     m->layers.emplace_back();
     return plan_layer(m, m->layers.back(), prefix, level, index, &ada, st);
-  };
-  for (int l = 0; l < n - 1; ++l)
-    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = plan("down_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i);
-  for (int i = 0; i < c.depth[n - 1] && rc == 0; ++i) rc = plan("mid_level." + std::to_string(i) + ".", n - 1, i);
-  for (int l = n - 2; l >= 0; --l)
-    for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = plan("up_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i + c.depth[l]);
+  });
   if (rc) return rc;
   m->ada_total = ada;
   {

@@ -11,6 +11,72 @@
 namespace kdb {
 
 constexpr float kEps = 1e-6f;   // RMSNorm / cosine-sim eps (image_transformer_v2.py:143,378)
+constexpr float kRsqrt2 = 0.70710678118654752440f;
+
+// grid of a grid-stride kernel of 256 threads over n elements
+static unsigned grid_stride_blocks(int64_t n) { return (unsigned)std::min<int64_t>(ceil_div(n, 256), kNumSMs * 16); }
+
+// NCHW offset of patch column n = (nh, nw, c) of token (ty, tx) of image b: channel c of pixel (ty ph + nh, tx pw + nw)
+__device__ __forceinline__ int64_t patch_pixel(int b, int ty, int tx, int n, int C, int H, int W, int ph, int pw) {
+  const int q = n / C, c = n - q * C;
+  const int nh = q / pw, nw = q - nh * pw;
+  return nchw_offset(b, c, ty * ph + nh, tx * pw + nw, C, H, W);
+}
+
+// TokenMerge / TokenSplit 2x2 order (image_transformer_v2.py:594,618): channel e of quadrant q = 2 nh + nw of coarse token (hy, wx)
+// of image b is channel e of fine token (2 hy + nh, 2 wx + nw) of [B, 2 hc, 2 wc, Cf]
+__device__ __forceinline__ int64_t fine_offset(int64_t b, int hy, int wx, int q, int e, int hc, int wc, int Cf) {
+  return ((b * (2 * hc) + (2 * hy + (q >> 1))) * (2 * wc) + (2 * wx + (q & 1))) * Cf + e;
+}
+// element i of a coarse [B, hc, wc, 4 Cf] tensor in that order -> offset of its fine element
+__device__ __forceinline__ int64_t merge_source(int64_t i, int hc, int wc, int Cf) {
+  const int e = (int)(i % Cf);
+  int64_t r = i / Cf;
+  const int q = (int)(r & 3);
+  r >>= 2;
+  const int wx = (int)(r % wc);
+  r /= wc;
+  const int hy = (int)(r % hc);
+  return fine_offset(r / hc, hy, wx, q, e, hc, wc, Cf);
+}
+
+// Tangent of a row norm y = x r, r = rsqrt(ss / n + eps), ss = sum x^2 (RMSNorm: n = row width; cosine-sim: n = 1), along u with
+// sd = x . u: dy = r u - x r^3 sd / n.  The row sums are the caller's.
+struct NormTangent {
+  float r, r3m;
+  __device__ NormTangent(float ss, float sd, float n) : r(rsqrtf(ss / n + kEps)), r3m(r * r * r * (sd / n)) {}
+  __device__ float operator()(float x, float u) const { return r * u - x * r3m; }
+};
+
+// Axial RoPE of a head of e columns (AxialRoPE(d_head // 2)): column j < e/4 pairs with column j + e/4 and both turn by
+// theta_j = pos_y f_j (j < nf) or pos_x f_(j - nf), nf = e/8, f = the head's freqs; columns from e/2 on pass through.
+__device__ __forceinline__ void rope_sincos(float py, float px, const float* f, int j, int nf, float& s, float& c) {
+  sincosf((j < nf ? py : px) * f[j < nf ? j : j - nf], &s, &c);
+}
+// column d of the rotated head v; INV: rotated by -theta (the transpose)
+template <bool INV>
+__device__ __forceinline__ float rope_rotate(const float* v, int d, int e, float py, float px, const float* f) {
+  const int dr = e / 4;
+  if (d >= 2 * dr) return v[d];
+  const int j = d < dr ? d : d - dr;
+  float s, c;
+  rope_sincos(py, px, f, j, e / 8, s, c);
+  const float x1 = v[j], x2 = v[j + dr];
+  if constexpr (INV)
+    return d < dr ? x1 * c + x2 * s : x2 * c - x1 * s;
+  else
+    return d < dr ? x1 * c - x2 * s : x2 * c + x1 * s;
+}
+
+// erf GELU (image_transformer_v2.py:89-95) in the reference's association, 0.5 g (1 + erf(g / sqrt 2))
+__device__ __forceinline__ float gelu_erf(float g) { return 0.5f * g * (1.f + erff(g * kRsqrt2)); }
+// the derivatives' form: gelu = g Phi(g) and slope = Phi(g) + g phi(g)
+__device__ __forceinline__ void gelu_erf_slope(float g, float& gelu, float& slope) {
+  const float Phi = 0.5f * (1.f + erff(g * kRsqrt2));
+  const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
+  gelu = g * Phi;
+  slope = fmaf(g, phi, Phi);
+}
 
 // ------------------------------------------------------------------------------------------------
 // patch_in: pixel-unshuffle + Linear (K = ph*pw*C is tiny: 16 or 48)
@@ -30,16 +96,14 @@ __global__ void __launch_bounds__(128) patch_in_kernel(const float* __restrict__
     const int64_t tok = tok0 + t;
     float v = 0.f;
     if (tok < tokens_total) {
-      const int b = (int)(tok / ((int64_t)th_n * tw_n));
-      const int r = (int)(tok - (int64_t)b * th_n * tw_n);
-      const int ty = r / tw_n, tx = r - ty * tw_n;
-      const int nh = k / (pw * C), nw = (k / C) % pw, c = k % C;
+      int b, ty, tx;
+      token_coords(tok, th_n, tw_n, b, ty, tx);
       float c_in = 1.f;
       if (sd > 0.f) {
         float cs, co;
         karras_scalings(sigma[b], sd, cs, co, c_in);
       }
-      v = x[(((int64_t)b * C + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw)] * c_in;
+      v = x[patch_pixel(b, ty, tx, k, C, H, Wd, ph, pw)] * c_in;
     }
     patch[idx] = v;
   }
@@ -269,12 +333,10 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const T* __restrict__ A,
         Cout[m * N + n] = from_f<T>(acc[i][j] + to_f(resid[m * N + n]));
       } else {
         // TokenSplit: row m = (b, hy, wx) on the coarse grid, column n = (nh, nw, e)
-        const int64_t b = m / ((int64_t)hc * wc);
-        const int r = (int)(m - b * hc * wc);
-        const int hy = r / wc, wx = r - hy * wc;
+        int b, hy, wx;
+        token_coords(m, hc, wc, b, hy, wx);
         const int q = n / Cf, e = n - q * Cf;
-        const int nh = q >> 1, nw = q & 1;
-        const int64_t dst = ((b * (2 * hc) + (2 * hy + nh)) * (2 * wc) + (2 * wx + nw)) * Cf + e;
+        const int64_t dst = fine_offset(b, hy, wx, q, e, hc, wc, Cf);
         Cout[dst] = from_f<T>(lerp_like_torch(to_f(resid[dst]), acc[i][j], facv));
       }
     }
@@ -320,10 +382,11 @@ template int launch_gemm_simt<float, float>(const float*, const float*, float*, 
 template int launch_gemm_simt<bf16, bf16>(const bf16*, const bf16*, bf16*, int64_t, int, int, const GemmEpi&, cudaStream_t);
 
 // ------------------------------------------------------------------------------------------------
-// cosine-sim scaling + axial RoPE, in place on q and k.  One warp per (token row, head).
+// cosine-sim scaling + axial RoPE of q and k from src to dst (src == dst: in place; else v is copied through).  One warp per (token row,
+// head).
 // ------------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(128) qknorm_rope_kernel(T* __restrict__ qkv, const float* __restrict__ pos,
+__global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, const float* __restrict__ pos,
                                                           const float* __restrict__ freqs, const float* __restrict__ scale,
                                                           int64_t rows, int Ttok, int nh, int e) {
   extern __shared__ float sm[];   // [warps][2][e]
@@ -333,13 +396,12 @@ __global__ void __launch_bounds__(128) qknorm_rope_kernel(T* __restrict__ qkv, c
   const int64_t row = item / nh;
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * 2 * e;
-  const int dr = e / 4;        // rotated pair width: theta has 2 * (e/8) entries (AxialRoPE(d_head // 2))
-  const int nf = e / 8;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
   const float sqs = sqrtf(scale[h]);
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
-    T* v = qkv + (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
+    const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
+    const T* v = src + off;
     float ss = 0.f;
     for (int d = lane; d < e; d += 32) {
       const float f = to_f(v[d]);
@@ -350,35 +412,26 @@ __global__ void __launch_bounds__(128) qknorm_rope_kernel(T* __restrict__ qkv, c
     // the reference rounds the scaled q/k back to the activation dtype before RoPE (:114)
     for (int d = lane; d < e; d += 32) buf[t * e + d] = to_f(from_f<T>(to_f(v[d]) * sc));
     __syncwarp();
-    for (int d = lane; d < e; d += 32) {
-      float o;
-      if (d < 2 * dr) {
-        const int j = d < dr ? d : d - dr;
-        const float theta = (j < nf ? py : px) * freqs[h * nf + (j < nf ? j : j - nf)];
-        float s, c;
-        sincosf(theta, &s, &c);
-        const float x1 = buf[t * e + j], x2 = buf[t * e + j + dr];
-        o = d < dr ? x1 * c - x2 * s : x2 * c + x1 * s;
-      } else {
-        o = buf[t * e + d];
-      }
-      v[d] = from_f<T>(o);
-    }
+    for (int d = lane; d < e; d += 32) dst[off + d] = from_f<T>(rope_rotate<false>(buf + t * e, d, e, py, px, freqs + h * (e / 8)));
     __syncwarp();
+  }
+  if (src != dst) {
+    const int64_t off = (row * 3 + 2) * (int64_t)nh * e + (int64_t)h * e;
+    for (int d = lane; d < e; d += 32) dst[off + d] = src[off + d];
   }
 }
 
 template <typename T>
-int launch_qknorm_rope(T* qkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh, int e,
+int launch_qknorm_rope(const T* src, T* dst, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh, int e,
                        cudaStream_t st) {
   KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope: d_head %d must be a multiple of 8", e);
   const size_t smem = sizeof(float) * 4 * 2 * e;
-  qknorm_rope_kernel<T><<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, pos, freqs, scale, rows, T_tokens, nh, e);
+  qknorm_rope_kernel<T><<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(src, dst, pos, freqs, scale, rows, T_tokens, nh, e);
   KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
   return 0;
 }
-template int launch_qknorm_rope<float>(float*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
-template int launch_qknorm_rope<bf16>(bf16*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
+template int launch_qknorm_rope<float>(const float*, float*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
+template int launch_qknorm_rope<bf16>(const bf16*, bf16*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
 
 // RoPE table for the QKV epilogue: float4 [(head * nf + i) * T + token] = (cos t_2i, cos t_2i+1, sin t_2i, sin t_2i+1), i < nf.
 // Token-minor, so the 32 threads of an epilogue warp (32 consecutive tokens) read 512 contiguous bytes per load, and the
@@ -391,9 +444,8 @@ __global__ void __launch_bounds__(256) rope_table_kernel(const float* __restrict
     const int t = i % T_tokens;
     const int j = (i / T_tokens) % (2 * nf);
     const int h = i / (T_tokens * 2 * nf);
-    const float theta = (j < nf ? pos[t * 2] : pos[t * 2 + 1]) * freqs[h * nf + (j < nf ? j : j - nf)];
     float s, c;
-    sincosf(theta, &s, &c);
+    rope_sincos(pos[t * 2], pos[t * 2 + 1], freqs + h * nf, j, nf, s, c);
     const int64_t base = (((int64_t)h * nf + (j >> 1)) * T_tokens + t) * 4;
     o[base + (j & 1)] = c;
     o[base + 2 + (j & 1)] = s;
@@ -415,7 +467,8 @@ struct KeySet {
   int qi, qj;           // query coordinates
   int r0, c0;           // neighbourhood origin
   int wi, wj, lqi, lqj; // shifted-window: window index and local query coords (rolled frame)
-  __device__ int count() const { return type == KDB_ATTN_GLOBAL ? h * w : param * param; }
+  __host__ __device__ static int count(int type, int h, int w, int param) { return type == KDB_ATTN_GLOBAL ? h * w : param * param; }
+  __device__ int count() const { return count(type, h, w, param); }
   __device__ void init(int type_, int h_, int w_, int param_, int shift_, int q) {
     type = type_; h = h_; w = w_; param = param_; shift = shift_;
     qi = q / w; qj = q - qi * w;
@@ -450,7 +503,7 @@ struct QuerySet {
   int type, h, w, param, shift;
   int i0, j0, ni, nj;   // neighbourhood: query row/column ranges [i0, i0+ni) x [j0, j0+nj)
   int wi, wj, la, lb;   // shifted-window: the key's window and local coords (rolled frame)
-  __device__ static int max_count(int type, int h, int w, int param) {
+  __host__ __device__ static int max_count(int type, int h, int w, int param) {
     if (type == KDB_ATTN_GLOBAL) return h * w;
     if (type == KDB_ATTN_NEIGHBORHOOD) return (3 * (param / 2) + 1) * (3 * (param / 2) + 1);
     return param * param;
@@ -556,33 +609,41 @@ __global__ void __launch_bounds__(128) attn_generic_kernel(const T* __restrict__
   }
 }
 
+// Launch geometry of the warp-per-query (or per-key) attention kernels: a grid of (query blocks of 4 warps, heads, images), the key set's
+// geometry checked, and per_warp floats of dynamic shared memory per warp within the budget the kernel is opened to on its first launch.
+constexpr int kAttnSmemMax = 200 * 1024;
+
+int check_attn_geometry(int h, int w, int type, int param) {
+  if (type == KDB_ATTN_NEIGHBORHOOD) {
+    KDB_REQUIRE(param >= 1 && h >= param && w >= param, KDB_ERR_BAD_SHAPE, "neighborhood attention: grid %dx%d smaller than kernel %d", h, w,
+                param);
+  } else if (type == KDB_ATTN_SHIFTED_WINDOW) {
+    KDB_REQUIRE(param >= 1 && h % param == 0 && w % param == 0, KDB_ERR_BAD_SHAPE,
+                "shifted-window attention: grid %dx%d not divisible by window %d", h, w, param);
+  } else {
+    KDB_REQUIRE(type == KDB_ATTN_GLOBAL, KDB_ERR_BAD_ARG, "attention: bad type %d", type);
+  }
+  return 0;
+}
+
+template <typename K>
+int attn_smem(K kernel, bool& opened, const char* what, int keys, size_t per_warp, size_t* smem) {
+  *smem = sizeof(float) * 4 * per_warp;
+  KDB_REQUIRE(*smem <= kAttnSmemMax, KDB_ERR_UNSUPPORTED, "%s: %d keys exceed the shared-memory budget", what, keys);
+  return set_smem_once(kernel, opened, kAttnSmemMax);
+}
+
+dim3 attn_grid(int B, int h, int w, int nh) { return dim3((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B); }
+
 template <typename T>
 int launch_attention_generic(const T* qkv, T* out, int B, int h, int w, int nh, int e, int attn_type, int attn_param, int shift,
                              cudaStream_t st) {
-  int maxkeys;
-  if (attn_type == KDB_ATTN_GLOBAL) {
-    maxkeys = h * w;
-  } else if (attn_type == KDB_ATTN_NEIGHBORHOOD) {
-    KDB_REQUIRE(attn_param >= 1 && h >= attn_param && w >= attn_param, KDB_ERR_BAD_SHAPE,
-                "neighborhood attention: grid %dx%d smaller than kernel %d", h, w, attn_param);
-    maxkeys = attn_param * attn_param;
-  } else if (attn_type == KDB_ATTN_SHIFTED_WINDOW) {
-    KDB_REQUIRE(attn_param >= 1 && h % attn_param == 0 && w % attn_param == 0, KDB_ERR_BAD_SHAPE,
-                "shifted-window attention: grid %dx%d not divisible by window %d", h, w, attn_param);
-    maxkeys = attn_param * attn_param;
-  } else {
-    KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "attention: bad type %d", attn_type);
-  }
-  const size_t smem = sizeof(float) * 4 * (size_t)(e + 2 * maxkeys);
-  KDB_REQUIRE(smem <= 200 * 1024, KDB_ERR_UNSUPPORTED, "attention_generic: %d keys exceed the shared-memory budget", maxkeys);
-  static bool attr_f = false, attr_b = false;
-  bool& attr = std::is_same<T, float>::value ? attr_f : attr_b;
-  if (!attr) {
-    KDB_CUDA(cudaFuncSetAttribute(attn_generic_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
-  dim3 grid((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B);
-  attn_generic_kernel<T><<<grid, 128, smem, st>>>(qkv, out, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
+  const int maxkeys = KeySet::count(attn_type, h, w, attn_param);
+  static bool opened = false;
+  size_t smem;
+  int rc = check_attn_geometry(h, w, attn_type, attn_param);
+  if (rc || (rc = attn_smem(attn_generic_kernel<T>, opened, "attention_generic", maxkeys, e + 2 * maxkeys, &smem))) return rc;
+  attn_generic_kernel<T><<<attn_grid(B, h, w, nh), 128, smem, st>>>(qkv, out, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
   KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
   return 0;
 }
@@ -599,16 +660,13 @@ __global__ void __launch_bounds__(256) geglu_kernel(const T* __restrict__ h, T* 
     const int64_t m = i / F;
     const int f = (int)(i - m * F);
     const float a = to_f(h[m * 2 * F + f]), g = to_f(h[m * 2 * F + F + f]);
-    const float gelu = 0.5f * g * (1.f + erff(g * 0.70710678118654752440f));
-    out[i] = from_f<T>(a * to_f(from_f<T>(gelu)));
+    out[i] = from_f<T>(a * to_f(from_f<T>(gelu_erf(g))));
   }
 }
 
 template <typename T>
 int launch_geglu(const T* h, T* out, int64_t M, int F, cudaStream_t st) {
-  int64_t blocks = ceil_div(M * F, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  geglu_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(h, out, M, F);
+  geglu_kernel<T><<<grid_stride_blocks(M * F), 256, 0, st>>>(h, out, M, F);
   KDB_LAUNCH_CHECK(F_GEGLU, st);
   return 0;
 }
@@ -618,27 +676,15 @@ template int launch_geglu<bf16>(const bf16*, bf16*, int64_t, int, cudaStream_t);
 template <typename T>
 __global__ void __launch_bounds__(256) merge_gather_kernel(const T* __restrict__ x, T* __restrict__ out, int H, int Wd, int C,
                                                            int64_t total) {
-  const int hc = H / 2, wc = Wd / 2;
-  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
-    const int e = (int)(i % C);
-    int64_t r = i / C;
-    const int q = (int)(r & 3);
-    r >>= 2;
-    const int wx = (int)(r % wc);
-    r /= wc;
-    const int hy = (int)(r % hc);
-    const int64_t b = r / hc;
-    out[i] = x[((b * H + (2 * hy + (q >> 1))) * Wd + (2 * wx + (q & 1))) * C + e];
-  }
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256)
+    out[i] = x[merge_source(i, H / 2, Wd / 2, C)];
 }
 
 template <typename T>
 int launch_merge_gather(const T* x, T* out, int B, int H, int Wd, int C, cudaStream_t st) {
   KDB_REQUIRE(H % 2 == 0 && Wd % 2 == 0, KDB_ERR_BAD_SHAPE, "token merge: grid %dx%d not even", H, Wd);
   const int64_t total = (int64_t)B * H * Wd * C;
-  int64_t blocks = ceil_div(total, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  merge_gather_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(x, out, H, Wd, C, total);
+  merge_gather_kernel<T><<<grid_stride_blocks(total), 256, 0, st>>>(x, out, H, Wd, C, total);
   KDB_LAUNCH_CHECK(F_MERGE_GATHER, st);
   return 0;
 }
@@ -668,10 +714,8 @@ __global__ void __launch_bounds__(128) patch_out_kernel(const T* __restrict__ to
   const float rstd = rsqrtf(ss / (float)C0 + kEps);
   for (int c = lane; c < C0; c += 32) xn[c] = to_f(from_f<T>(to_f(xr[c]) * (__ldg(nscale + c) * rstd)));
   __syncwarp();
-  const int th_n = H / ph, tw_n = Wd / pw;
-  const int64_t b = tok / ((int64_t)th_n * tw_n);
-  const int r = (int)(tok - b * th_n * tw_n);
-  const int ty = r / tw_n, tx = r - ty * tw_n;
+  int b, ty, tx;
+  token_coords(tok, H / ph, Wd / pw, b, ty, tx);
   float c_skip = 0.f, c_out = 1.f, c_in;
   if (sd > 0.f) karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
   const int N = ph * pw * Cout;
@@ -680,9 +724,7 @@ __global__ void __launch_bounds__(128) patch_out_kernel(const T* __restrict__ to
     float acc = 0.f;
     for (int k = 0; k < C0; ++k) acc = fmaf(xn[k], __ldg(wr + k), acc);
     acc = to_f(from_f<T>(acc));
-    const int q = n / Cout, c = n - q * Cout;
-    const int nh = q / pw, nw = q - nh * pw;
-    const int64_t o = ((b * Cout + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw);
+    const int64_t o = patch_pixel(b, ty, tx, n, Cout, H, Wd, ph, pw);
     out[o] = (sd > 0.f) ? acc * c_out + x_in[o] * c_skip : acc;
   }
 }
@@ -726,13 +768,10 @@ __global__ void __launch_bounds__(256) rmsnorm_jvp_kernel(const float* __restric
     ss = fmaf(v, v, ss);
     sd = fmaf(v, dr[c], sd);
   }
-  ss = warp_sum(ss);
-  sd = warp_sum(sd);
-  const float r = rsqrtf(ss / (float)C + kEps);   // the primal kernel's 1/rms
-  const float r3m = r * r * r * (sd / (float)C);
+  const NormTangent nt(warp_sum(ss), warp_sum(sd), (float)C);
   const float* sc = scale + (row / rows_per_batch) * scale_bstride;
   float* yr = dy + row * C;
-  for (int c = lane; c < C; c += 32) yr[c] = __ldg(sc + c) * (r * dr[c] - xr[c] * r3m);
+  for (int c = lane; c < C; c += 32) yr[c] = __ldg(sc + c) * nt(xr[c], dr[c]);
 }
 
 int launch_rmsnorm_jvp(const float* x, const float* dx, float* dy, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
@@ -753,7 +792,6 @@ __global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __res
   const int64_t row = item / nh;
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * 2 * e;
-  const int dr = e / 4, nf = e / 8;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
   const float sqs = sqrtf(scale[h]);
 #pragma unroll
@@ -766,27 +804,11 @@ __global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __res
       ss = fmaf(v[d], v[d], ss);
       sd = fmaf(v[d], dv[d], sd);
     }
-    ss = warp_sum(ss);
-    sd = warp_sum(sd);
-    const float rho = rsqrtf(ss + kEps);
-    const float r3s = rho * rho * rho * sd;
-    // d(q rho) = rho dq - q rho^3 (q . dq), then the primal's rotation
-    for (int d = lane; d < e; d += 32) buf[t * e + d] = sqs * (rho * dv[d] - v[d] * r3s);
+    // the tangent of the cosine-sim scaling, then the primal's rotation
+    const NormTangent nt(warp_sum(ss), warp_sum(sd), 1.f);
+    for (int d = lane; d < e; d += 32) buf[t * e + d] = sqs * nt(v[d], dv[d]);
     __syncwarp();
-    for (int d = lane; d < e; d += 32) {
-      float o;
-      if (d < 2 * dr) {
-        const int j = d < dr ? d : d - dr;
-        const float theta = (j < nf ? py : px) * freqs[h * nf + (j < nf ? j : j - nf)];
-        float s, c;
-        sincosf(theta, &s, &c);
-        const float x1 = buf[t * e + j], x2 = buf[t * e + j + dr];
-        o = d < dr ? x1 * c - x2 * s : x2 * c + x1 * s;
-      } else {
-        o = buf[t * e + d];
-      }
-      dv[d] = o;
-    }
+    for (int d = lane; d < e; d += 32) dv[d] = rope_rotate<false>(buf + t * e, d, e, py, px, freqs + h * (e / 8));
     __syncwarp();
   }
 }
@@ -880,23 +902,12 @@ __global__ void __launch_bounds__(128) attn_jvp_kernel(const float* __restrict__
 
 int launch_attention_jvp(const float* qkv, const float* dqkv, float* dout, int B, int h, int w, int nh, int e, int attn_type, int attn_param,
                          int shift, cudaStream_t st) {
-  int maxkeys;
-  if (attn_type == KDB_ATTN_GLOBAL) {
-    maxkeys = h * w;
-  } else if (attn_type == KDB_ATTN_NEIGHBORHOOD || attn_type == KDB_ATTN_SHIFTED_WINDOW) {
-    maxkeys = attn_param * attn_param;   // geometry checked by the primal launch
-  } else {
-    KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "attention_jvp: bad type %d", attn_type);
-  }
-  const size_t smem = sizeof(float) * 4 * (size_t)(2 * e + 3 * maxkeys);
-  KDB_REQUIRE(smem <= 200 * 1024, KDB_ERR_UNSUPPORTED, "attention_jvp: %d keys exceed the shared-memory budget", maxkeys);
-  static bool attr = false;
-  if (!attr) {
-    KDB_CUDA(cudaFuncSetAttribute(attn_jvp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
-  dim3 grid((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B);
-  attn_jvp_kernel<<<grid, 128, smem, st>>>(qkv, dqkv, dout, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
+  const int maxkeys = KeySet::count(attn_type, h, w, attn_param);
+  static bool opened = false;
+  size_t smem;
+  int rc = check_attn_geometry(h, w, attn_type, attn_param);
+  if (rc || (rc = attn_smem(attn_jvp_kernel, opened, "attention_jvp", maxkeys, 2 * e + 3 * maxkeys, &smem))) return rc;
+  attn_jvp_kernel<<<attn_grid(B, h, w, nh), 128, smem, st>>>(qkv, dqkv, dout, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
   KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
   return 0;
 }
@@ -909,16 +920,14 @@ __global__ void __launch_bounds__(256) geglu_jvp_kernel(const float* __restrict_
     const int64_t m = i / F;
     const int f = (int)(i - m * F);
     const float a = hp[m * 2 * F + f], g = hp[m * 2 * F + F + f];
-    const float Phi = 0.5f * (1.f + erff(g * 0.70710678118654752440f));
-    const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
-    dout[i] = dh[m * 2 * F + f] * (g * Phi) + (a * fmaf(g, phi, Phi)) * dh[m * 2 * F + F + f];
+    float gelu, slope;
+    gelu_erf_slope(g, gelu, slope);
+    dout[i] = dh[m * 2 * F + f] * gelu + (a * slope) * dh[m * 2 * F + F + f];
   }
 }
 
 int launch_geglu_jvp(const float* h, const float* dh, float* dout, int64_t M, int F, cudaStream_t st) {
-  int64_t blocks = ceil_div(M * F, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  geglu_jvp_kernel<<<(unsigned)blocks, 256, 0, st>>>(h, dh, dout, M, F);
+  geglu_jvp_kernel<<<grid_stride_blocks(M * F), 256, 0, st>>>(h, dh, dout, M, F);
   KDB_LAUNCH_CHECK(F_GEGLU, st);
   return 0;
 }
@@ -941,16 +950,11 @@ __global__ void __launch_bounds__(128) patch_out_jvp_kernel(const float* __restr
     ss = fmaf(xr[c], xr[c], ss);
     sdot = fmaf(xr[c], dr[c], sdot);
   }
-  ss = warp_sum(ss);
-  sdot = warp_sum(sdot);
-  const float r = rsqrtf(ss / (float)C0 + kEps);
-  const float r3m = r * r * r * (sdot / (float)C0);
-  for (int c = lane; c < C0; c += 32) dn[c] = __ldg(nscale + c) * (r * dr[c] - xr[c] * r3m);
+  const NormTangent nt(warp_sum(ss), warp_sum(sdot), (float)C0);
+  for (int c = lane; c < C0; c += 32) dn[c] = __ldg(nscale + c) * nt(xr[c], dr[c]);
   __syncwarp();
-  const int th_n = H / ph, tw_n = Wd / pw;
-  const int64_t b = tok / ((int64_t)th_n * tw_n);
-  const int rr = (int)(tok - b * th_n * tw_n);
-  const int ty = rr / tw_n, tx = rr - ty * tw_n;
+  int b, ty, tx;
+  token_coords(tok, H / ph, Wd / pw, b, ty, tx);
   float c_skip = 0.f, c_out = 1.f, c_in;
   if (sd > 0.f) karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
   const int N = ph * pw * Cout;
@@ -958,9 +962,7 @@ __global__ void __launch_bounds__(128) patch_out_jvp_kernel(const float* __restr
     const float* wr = W + (int64_t)n * C0;
     float acc = 0.f;
     for (int k = 0; k < C0; ++k) acc = fmaf(dn[k], __ldg(wr + k), acc);
-    const int q = n / Cout, c = n - q * Cout;
-    const int nh = q / pw, nw = q - nh * pw;
-    const int64_t o = ((b * Cout + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw);
+    const int64_t o = patch_pixel(b, ty, tx, n, Cout, H, Wd, ph, pw);
     out[o] = (sd > 0.f) ? acc * c_out + v_in[o] * c_skip : acc;
   }
 }
@@ -1035,12 +1037,10 @@ __global__ void __launch_bounds__(256) gemm_vjp_kernel(const float* __restrict__
       if constexpr (EPI == VJP_STORE) {
         out[m * K + k] = acc[i][j];
       } else {
-        const int64_t b = m / ((int64_t)hc * wc);
-        const int r = (int)(m - b * hc * wc);
-        const int hy = r / wc, wx = r - hy * wc;
+        int b, hy, wx;
+        token_coords(m, hc, wc, b, hy, wx);
         const int q = k / Cf, e = k - q * Cf;
-        const int64_t dst = ((b * (2 * hc) + (2 * hy + (q >> 1))) * (2 * wc) + (2 * wx + (q & 1))) * Cf + e;
-        out[dst] += acc[i][j];
+        out[fine_offset(b, hy, wx, q, e, hc, wc, Cf)] += acc[i][j];
       }
     }
   }
@@ -1080,12 +1080,9 @@ __global__ void __launch_bounds__(256) rmsnorm_vjp_kernel(const float* __restric
     ss = fmaf(xr[c], xr[c], ss);
     sd = fmaf(xr[c], __ldg(sc + c) * gr[c], sd);
   }
-  ss = warp_sum(ss);
-  sd = warp_sum(sd);
-  const float r = rsqrtf(ss / (float)C + kEps);
-  const float r3m = r * r * r * (sd / (float)C);
+  const NormTangent nt(warp_sum(ss), warp_sum(sd), (float)C);
   float* dr = dx + row * C;
-  for (int c = lane; c < C; c += 32) dr[c] += r * (__ldg(sc + c) * gr[c]) - xr[c] * r3m;
+  for (int c = lane; c < C; c += 32) dr[c] += nt(xr[c], __ldg(sc + c) * gr[c]);
 }
 
 int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
@@ -1108,7 +1105,6 @@ __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __res
   const int64_t row = item / nh;
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * e;
-  const int dr = e / 4, nf = e / 8;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
   const float sqs = sqrtf(scale[h]);
 #pragma unroll
@@ -1116,31 +1112,15 @@ __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __res
     const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
     const float* v = qkv + off;
     float* dv = dqkv + off;
-    for (int d = lane; d < e; d += 32) {
-      float g;
-      if (d < 2 * dr) {
-        const int j = d < dr ? d : d - dr;
-        const float theta = (j < nf ? py : px) * freqs[h * nf + (j < nf ? j : j - nf)];
-        float s, c;
-        sincosf(theta, &s, &c);
-        const float g1 = dv[j], g2 = dv[j + dr];
-        g = d < dr ? g1 * c + g2 * s : g2 * c - g1 * s;
-      } else {
-        g = dv[d];
-      }
-      buf[d] = g;
-    }
+    for (int d = lane; d < e; d += 32) buf[d] = rope_rotate<true>(dv, d, e, py, px, freqs + h * (e / 8));
     __syncwarp();
     float ss = 0.f, sg = 0.f;
     for (int d = lane; d < e; d += 32) {
       ss = fmaf(v[d], v[d], ss);
       sg = fmaf(v[d], buf[d], sg);
     }
-    ss = warp_sum(ss);
-    sg = warp_sum(sg);
-    const float rho = rsqrtf(ss + kEps);
-    const float r3s = rho * rho * rho * sg;
-    for (int d = lane; d < e; d += 32) dv[d] = sqs * (rho * buf[d] - v[d] * r3s);
+    const NormTangent nt(warp_sum(ss), warp_sum(sg), 1.f);
+    for (int d = lane; d < e; d += 32) dv[d] = sqs * nt(v[d], buf[d]);
     __syncwarp();
   }
 }
@@ -1297,26 +1277,14 @@ __global__ void __launch_bounds__(128) attn_vjp_kv_kernel(const float* __restric
 
 int launch_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int B, int h, int w, int nh, int e,
                          int attn_type, int attn_param, int shift, cudaStream_t st) {
-  int maxkeys, maxq;
-  if (attn_type == KDB_ATTN_GLOBAL) {
-    maxkeys = maxq = h * w;
-  } else if (attn_type == KDB_ATTN_NEIGHBORHOOD || attn_type == KDB_ATTN_SHIFTED_WINDOW) {
-    maxkeys = attn_param * attn_param;   // geometry checked by the primal launch
-    maxq = attn_type == KDB_ATTN_NEIGHBORHOOD ? (3 * (attn_param / 2) + 1) * (3 * (attn_param / 2) + 1) : maxkeys;
-  } else {
-    KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "attention_vjp: bad type %d", attn_type);
-  }
-  const size_t smem_q = sizeof(float) * 4 * (size_t)(2 * e + 2 * maxkeys);
-  const size_t smem_kv = sizeof(float) * 4 * (size_t)(2 * e + 3 * maxq);
-  KDB_REQUIRE(smem_q <= 200 * 1024 && smem_kv <= 200 * 1024, KDB_ERR_UNSUPPORTED, "attention_vjp: %d keys exceed the shared-memory budget",
-              maxkeys);
-  static bool attr = false;
-  if (!attr) {
-    KDB_CUDA(cudaFuncSetAttribute(attn_vjp_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    KDB_CUDA(cudaFuncSetAttribute(attn_vjp_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
-  dim3 grid((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B);
+  const int maxkeys = KeySet::count(attn_type, h, w, attn_param), maxq = QuerySet::max_count(attn_type, h, w, attn_param);
+  static bool opened_q = false, opened_kv = false;
+  size_t smem_q, smem_kv;
+  int rc = check_attn_geometry(h, w, attn_type, attn_param);
+  if (rc || (rc = attn_smem(attn_vjp_q_kernel, opened_q, "attention_vjp", maxkeys, 2 * e + 2 * maxkeys, &smem_q)) ||
+      (rc = attn_smem(attn_vjp_kv_kernel, opened_kv, "attention_vjp", maxq, 2 * e + 3 * maxq, &smem_kv)))
+    return rc;
+  const dim3 grid = attn_grid(B, h, w, nh);
   attn_vjp_q_kernel<<<grid, 128, smem_q, st>>>(qkv, out, dout, dqkv, stats, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
   KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
   attn_vjp_kv_kernel<<<grid, 128, smem_kv, st>>>(qkv, dout, stats, dqkv, h, w, nh, e, attn_type, attn_param, shift, maxq);
@@ -1332,17 +1300,15 @@ __global__ void __launch_bounds__(256) geglu_vjp_kernel(const float* __restrict_
     const int64_t m = i / F;
     const int f = (int)(i - m * F);
     const float a = hp[m * 2 * F + f], g = hp[m * 2 * F + F + f];
-    const float Phi = 0.5f * (1.f + erff(g * 0.70710678118654752440f));
-    const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
-    dh[m * 2 * F + f] = dy[i] * (g * Phi);
-    dh[m * 2 * F + F + f] = dy[i] * (a * fmaf(g, phi, Phi));
+    float gelu, slope;
+    gelu_erf_slope(g, gelu, slope);
+    dh[m * 2 * F + f] = dy[i] * gelu;
+    dh[m * 2 * F + F + f] = dy[i] * (a * slope);
   }
 }
 
 int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int F, cudaStream_t st) {
-  int64_t blocks = ceil_div(M * F, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  geglu_vjp_kernel<<<(unsigned)blocks, 256, 0, st>>>(h, dy, dh, M, F);
+  geglu_vjp_kernel<<<grid_stride_blocks(M * F), 256, 0, st>>>(h, dy, dh, M, F);
   KDB_LAUNCH_CHECK(F_GEGLU, st);
   return 0;
 }
@@ -1351,18 +1317,9 @@ int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int 
 // dup <- (1 - fac) dup in place (the gradient the skip connection receives).  Same derivative on both branches of lerp_like_torch.
 __global__ void __launch_bounds__(256) split_vjp_gather_kernel(float* __restrict__ dup, float* __restrict__ out, const float* __restrict__ fac,
                                                                int H, int Wd, int C, int64_t total) {
-  const int hc = H / 2, wc = Wd / 2;
   const float f = __ldg(fac), g = 1.f - f;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
-    const int e = (int)(i % C);
-    int64_t r = i / C;
-    const int q = (int)(r & 3);
-    r >>= 2;
-    const int wx = (int)(r % wc);
-    r /= wc;
-    const int hy = (int)(r % hc);
-    const int64_t b = r / hc;
-    const int64_t src = ((b * H + (2 * hy + (q >> 1))) * Wd + (2 * wx + (q & 1))) * C + e;
+    const int64_t src = merge_source(i, H / 2, Wd / 2, C);
     const float d = dup[src];
     out[i] = f * d;
     dup[src] = g * d;
@@ -1372,9 +1329,7 @@ __global__ void __launch_bounds__(256) split_vjp_gather_kernel(float* __restrict
 int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int H, int Wd, int C, cudaStream_t st) {
   KDB_REQUIRE(H % 2 == 0 && Wd % 2 == 0, KDB_ERR_BAD_SHAPE, "token split vjp: grid %dx%d not even", H, Wd);
   const int64_t total = (int64_t)B * H * Wd * C;
-  int64_t blocks = ceil_div(total, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  split_vjp_gather_kernel<<<(unsigned)blocks, 256, 0, st>>>(dup, out, fac, H, Wd, C, total);
+  split_vjp_gather_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(dup, out, fac, H, Wd, C, total);
   KDB_LAUNCH_CHECK(F_MERGE_GATHER, st);
   return 0;
 }
@@ -1392,17 +1347,11 @@ __global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restr
   const int N = ph * pw * Cout;
   float* dn = sm + (size_t)warp * (C0 + N);
   float* dy = dn + C0;
-  const int th_n = H / ph, tw_n = Wd / pw;
-  const int64_t b = tok / ((int64_t)th_n * tw_n);
-  const int rr = (int)(tok - b * th_n * tw_n);
-  const int ty = rr / tw_n, tx = rr - ty * tw_n;
+  int b, ty, tx;
+  token_coords(tok, H / ph, Wd / pw, b, ty, tx);
   float c_skip, c_out = 1.f, c_in;
   if (sd > 0.f) karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
-  for (int n = lane; n < N; n += 32) {
-    const int q = n / Cout, c = n - q * Cout;
-    const int nh = q / pw, nw = q - nh * pw;
-    dy[n] = c_out * u[((b * Cout + c) * H + (ty * ph + nh)) * Wd + (tx * pw + nw)];
-  }
+  for (int n = lane; n < N; n += 32) dy[n] = c_out * u[patch_pixel(b, ty, tx, n, Cout, H, Wd, ph, pw)];
   __syncwarp();
   for (int k = lane; k < C0; k += 32) {
     float acc = 0.f;
@@ -1416,12 +1365,9 @@ __global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restr
     ss = fmaf(xr[c], xr[c], ss);
     sdot = fmaf(xr[c], __ldg(nscale + c) * dn[c], sdot);
   }
-  ss = warp_sum(ss);
-  sdot = warp_sum(sdot);
-  const float r = rsqrtf(ss / (float)C0 + kEps);
-  const float r3m = r * r * r * (sdot / (float)C0);
+  const NormTangent nt(warp_sum(ss), warp_sum(sdot), (float)C0);
   float* dr = dtokens + tok * C0;
-  for (int c = lane; c < C0; c += 32) dr[c] = r * (__ldg(nscale + c) * dn[c]) - xr[c] * r3m;
+  for (int c = lane; c < C0; c += 32) dr[c] = nt(xr[c], __ldg(nscale + c) * dn[c]);
 }
 
 int launch_patch_out_vjp(const float* tokens, const float* norm_scale, const float* W, const float* u, const float* sigma, float sigma_data,
@@ -1465,9 +1411,7 @@ __global__ void __launch_bounds__(256) patch_in_vjp_kernel(const float* __restri
 int launch_patch_in_vjp(const float* dtokens, const float* W, const float* u, const float* sigma, float sigma_data, float* grad_x, int B, int C,
                         int H, int Wd, int ph, int pw, int N, cudaStream_t st) {
   const int64_t total = (int64_t)B * C * H * Wd;
-  int64_t blocks = ceil_div(total, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  patch_in_vjp_kernel<<<(unsigned)blocks, 256, 0, st>>>(dtokens, W, u, sigma, sigma_data, grad_x, C, H, Wd, ph, pw, N, total);
+  patch_in_vjp_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(dtokens, W, u, sigma, sigma_data, grad_x, C, H, Wd, ph, pw, N, total);
   KDB_LAUNCH_CHECK(F_PATCH_IN, st);
   return 0;
 }
@@ -1595,10 +1539,7 @@ __global__ void __launch_bounds__(256) conditioning_kernel(const CondWeights w, 
     block_rmsnorm(emb, xn, w.blk_norm[l], mw, red);
     block_matvec(w.blk_up[l], xn, up, 0, 2 * dff, mw, false);
     __syncthreads();
-    for (int i = threadIdx.x; i < dff; i += blockDim.x) {
-      const float g = up[dff + i];
-      up[i] = up[i] * (0.5f * g * (1.f + erff(g * 0.70710678118654752440f)));
-    }
+    for (int i = threadIdx.x; i < dff; i += blockDim.x) up[i] = up[i] * gelu_erf(up[dff + i]);
     __syncthreads();
     block_matvec(w.blk_down[l], up, emb, 0, mw, dff, true);
     __syncthreads();
@@ -1632,9 +1573,7 @@ __global__ void __launch_bounds__(256) f32_to_bf16_kernel(const float* __restric
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) out[i] = __float2bfloat16_rn(in[i]);
 }
 int launch_f32_to_bf16(const float* in, bf16* out, int64_t n, cudaStream_t st) {
-  int64_t blocks = ceil_div(n, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  f32_to_bf16_kernel<<<(unsigned)blocks, 256, 0, st>>>(in, out, n);
+  f32_to_bf16_kernel<<<grid_stride_blocks(n), 256, 0, st>>>(in, out, n);
   KDB_LAUNCH_CHECK(F_CONVERT, st);
   return 0;
 }
@@ -1645,9 +1584,7 @@ __global__ void __launch_bounds__(256) to_f32_kernel(const T* __restrict__ in, f
 }
 template <typename T>
 int launch_to_f32(const T* in, float* out, int64_t n, cudaStream_t st) {
-  int64_t blocks = ceil_div(n, 256);
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-  to_f32_kernel<T><<<(unsigned)blocks, 256, 0, st>>>(in, out, n);
+  to_f32_kernel<T><<<grid_stride_blocks(n), 256, 0, st>>>(in, out, n);
   KDB_LAUNCH_CHECK(F_CONVERT, st);
   return 0;
 }

@@ -43,11 +43,11 @@ int launch_rmsnorm(const T* x, T* y, const float* scale, int64_t scale_bstride, 
 template <typename T, typename TW>
 int launch_gemm_simt(const T* A, const TW* W, T* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st);
 
-// in-place cosine-sim scaling of q,k and axial RoPE on qkv [rows, 3, nh, e]  (image_transformer_v2.py:106-114,187-199,245-248)
-// pos [T,2] (y,x) for the level, freqs [nh, e/8], scale [nh]; rows = B*T
+// cosine-sim scaling of q,k and axial RoPE, qkv [rows, 3, nh, e] src -> dst (src == dst: in place; else v is copied through)
+// (image_transformer_v2.py:106-114,187-199,245-248).  pos [T,2] (y,x) for the level, freqs [nh, e/8], scale [nh]; rows = B*T
 template <typename T>
-int launch_qknorm_rope(T* qkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh, int e,
-                       cudaStream_t st);
+int launch_qknorm_rope(const T* src, T* dst, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh,
+                       int e, cudaStream_t st);
 
 // softmax(q k^T) v over the key set of attn_type (scale 1.0); qkv [B,h,w,3,nh,e] -> out [B,h,w,nh,e]
 template <typename T>

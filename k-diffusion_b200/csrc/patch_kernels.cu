@@ -21,13 +21,6 @@ struct PatchGeom {
   int64_t tokens;
 };
 
-__device__ __forceinline__ void tok_coords(const PatchGeom& g, int64_t tok, int& b, int& ty, int& tx) {
-  const int64_t per = (int64_t)g.th * g.tw;
-  b = (int)(tok / per);
-  const int r = (int)(tok - (int64_t)b * per);
-  ty = r / g.tw;
-  tx = r - ty * g.tw;
-}
 // coordinates of token (tile origin + t) from the tile origin's coordinates, without 64-bit division
 __device__ __forceinline__ void tok_step(const PatchGeom& g, int b0, int ty0, int tx0, int t, int& b, int& ty, int& tx) {
   b = b0; ty = ty0; tx = tx0 + t;
@@ -68,7 +61,7 @@ __global__ void __launch_bounds__(256) patch_in_tiled(const float* __restrict__ 
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t tok0 = tile * TOK;
     int b0, ty0, tx0;
-    tok_coords(g, tok0, b0, ty0, tx0);
+    token_coords(tok0, g.th, g.tw, b0, ty0, tx0);
     __syncthreads();                      // previous tile's patch fully consumed (and Ws visible on the first pass)
     // gather pixels, pixel-contiguous order: idx = ((c*PH + nh)*TOK + t)*PW + nw.  All loads of a thread are issued
     // before any is consumed (the kernel is latency-bound otherwise).
@@ -86,7 +79,7 @@ __global__ void __launch_bounds__(256) patch_in_tiled(const float* __restrict__ 
         if (tok0 + t < g.tokens) {
           int b, ty, tx;
           tok_step(g, b0, ty0, tx0, t, b, ty, tx);
-          gv[it] = __ldg(x + (((int64_t)b * g.C + c) * g.H + (ty * PH + nh)) * g.W + (tx * PW + nw));
+          gv[it] = __ldg(x + nchw_offset(b, c, ty * PH + nh, tx * PW + nw, g.C, g.H, g.W));
         }
       }
     }
@@ -166,7 +159,7 @@ __global__ void __launch_bounds__(256) patch_out_tiled(const T* __restrict__ tok
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t tok0 = tile * TOK;
     int b0, ty0, tx0;
-    tok_coords(g, tok0, b0, ty0, tx0);
+    token_coords(tok0, g.th, g.tw, b0, ty0, tx0);
     __syncthreads();                       // previous tile's xn / ys consumed
     // RMSNorm: warp per token (8 tokens per warp), normalised row written transposed.  For C0 <= 256 the 8 rows are
     // fetched into registers up front (8 x C0/32 independent loads per lane) so the loads overlap.
@@ -250,7 +243,7 @@ __global__ void __launch_bounds__(256) patch_out_tiled(const T* __restrict__ tok
         if (tok0 + tt < g.tokens) {
           int b, ty, tx;
           tok_step(g, b0, ty0, tx0, tt, b, ty, tx);
-          ov[it] = (((int64_t)b * Cout + c) * g.H + (ty * PH + nh)) * g.W + (tx * PW + nw);
+          ov[it] = nchw_offset(b, c, ty * PH + nh, tx * PW + nw, Cout, g.H, g.W);
           if (sd > 0.f) xv[it] = __ldg(x_in + ov[it]);
         }
       }
@@ -278,19 +271,12 @@ __global__ void __launch_bounds__(256) patch_out_tiled(const T* __restrict__ tok
   }
 }
 
-template <typename K>
-int set_smem_once(K kernel, bool& flag) {
-  if (!flag) {
-    KDB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    flag = true;
-  }
-  return 0;
-}
+constexpr int kSmemMax = 160 * 1024;
 
 template <typename T, int PH, int PW, int TT>
 int run_patch_in(const float* x, const float* sigma, float sd, const float* W, T* out, const PatchGeom& g, size_t smem, cudaStream_t st) {
   static bool attr = false;
-  int rc = set_smem_once(patch_in_tiled<T, PH, PW, TT>, attr);
+  int rc = set_smem_once(patch_in_tiled<T, PH, PW, TT>, attr, kSmemMax);
   if (rc) return rc;
   patch_in_tiled<T, PH, PW, TT><<<(unsigned)std::min<int64_t>(ceil_div(g.tokens, TOK), kNumSMs * 2), 256, smem, st>>>(x, sigma, sd, W, out, g);
   KDB_LAUNCH_CHECK(F_PATCH_IN, st);
@@ -301,7 +287,7 @@ template <typename T, int PH, int PW>
 int run_patch_out(const T* tokens, const float* ns, const float* W, const float* x_in, const float* sigma, float sd, float* out,
                   const PatchGeom& g, int C0, size_t smem, cudaStream_t st) {
   static bool attr = false;
-  int rc = set_smem_once(patch_out_tiled<T, PH, PW>, attr);
+  int rc = set_smem_once(patch_out_tiled<T, PH, PW>, attr, kSmemMax);
   if (rc) return rc;
   patch_out_tiled<T, PH, PW><<<(unsigned)std::min<int64_t>(ceil_div(g.tokens, TOK), kNumSMs * 2), 256, smem, st>>>(tokens, ns, W, x_in, sigma, sd,
                                                                                                                   out, g, C0);
@@ -316,7 +302,7 @@ bool launch_patch_in_tiled(const float* x, const float* sigma, float sigma_data,
                            int pw, int N, cudaStream_t st, int* rc) {
   const int K = ph * pw * C;
   const size_t smem = sizeof(float) * ((size_t)K * TOK + (size_t)K * N);
-  if (smem > 160 * 1024 || (N != 64 && N != 128 && N != 256) || !((ph == 4 && pw == 4) || (ph == 2 && pw == 2))) return false;
+  if (smem > kSmemMax || (N != 64 && N != 128 && N != 256) || !((ph == 4 && pw == 4) || (ph == 2 && pw == 2))) return false;
   PatchGeom g{C, H, Wd, H / ph, Wd / pw, (int64_t)B * (H / ph) * (Wd / pw)};
 #define KDB_PI(PH_, PW_)                                                                                   \
   switch (N) {                                                                                             \
@@ -336,7 +322,7 @@ bool launch_patch_out_tiled(const T* tokens, const float* norm_scale, const floa
                             float* out, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st, int* rc) {
   const int N = ph * pw * Cout;
   const size_t smem = sizeof(float) * ((size_t)C0 * (TOK + 4) + (size_t)C0 * N + (size_t)N * (TOK + 4));
-  if (N > 64 || N % 4 != 0 || smem > 160 * 1024 || !((ph == 4 && pw == 4) || (ph == 2 && pw == 2))) return false;
+  if (N > 64 || N % 4 != 0 || smem > kSmemMax || !((ph == 4 && pw == 4) || (ph == 2 && pw == 2))) return false;
   PatchGeom g{Cout, H, Wd, H / ph, Wd / pw, (int64_t)B * (H / ph) * (Wd / pw)};
   if (ph == 4)
     *rc = run_patch_out<T, 4, 4>(tokens, norm_scale, W, x_in, sigma, sigma_data, out, g, C0, smem, st);

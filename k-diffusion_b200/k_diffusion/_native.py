@@ -403,7 +403,14 @@ class Engine:
             raise IndexError(f"class_cond values must lie in [0, {n}) (class_emb has {n} rows), got [{lo}, {hi}]")
 
     def _workspace(self, precision, B, H, W, device):
-        need = int(lib().kdb_model_workspace_bytes(self._h, precision, B, H, W))
+        """The workspace of a forward of B images (kdb_model_workspace_bytes)."""
+        return self._reserve(lib().kdb_model_workspace_bytes(self._h, precision, B, H, W), device)
+
+    def _reserve(self, need, device):
+        """The engine's workspace of at least `need` bytes on `device`, grown and reused across calls."""
+        need = int(need)
+        if need < 0:
+            check(need)
         if self._ws is None or self._ws.numel() < need or self._ws.device != device:
             self._ws = None
             self._ws = torch.empty(need, dtype=torch.uint8, device=device)
@@ -444,13 +451,7 @@ class Engine:
             raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {shape}")
         out = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
         out_grad = torch.empty_like(x) if out_grad is None else out_grad
-        need = int(lib().kdb_model_vjp_workspace_bytes(self._h, B, H, W))
-        if need < 0:
-            check(need)
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = None
-            self._ws = torch.empty(need, dtype=torch.uint8, device=x.device)
-        ws = self._ws
+        ws = self._reserve(lib().kdb_model_vjp_workspace_bytes(self._h, B, H, W), x.device)
         with device_of(x):
             check(lib().kdb_model_forward_vjp(self._h, PREC_FP32, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
                                               ptr(u), ptr(out), ptr(out_grad), ptr(ws), ws.numel(), stream()))
