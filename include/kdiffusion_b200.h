@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 10
+#define KDB_ABI_VERSION 11
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -272,6 +272,17 @@ int kdb_attn_block_bf16(void* x_bf16, const void* w_qkv_bf16, const void* w_out_
  * softmax's fixed shift (one pass over the keys, no row maximum); NULL keeps the exact two-pass row-maximum kernels. */
 int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch, int h, int w, int n_heads, int d_head,
                   int attn_type, int attn_param, int shift, const float* logit_bound, void* stream);
+
+/* Derivatives of the fp32 kdb_attention (precision KDB_PREC_FP32, fast 0), the kernels the model's forward_jvp / forward_vjp launch.
+ * qkv as for kdb_attention.
+ *   kdb_attention_jvp: dout[B,h,w,nh*e] = the tangent of the attention output along dqkv (same layout as qkv).
+ *   kdb_attention_vjp: out = kdb_attention's output on qkv, dout its gradient [B,h,w,nh*e] -> dqkv [B,h,w,3*nh*e], every element written.
+ *                      stats: caller scratch of batch * n_heads * h * w * 3 floats (per-query softmax statistics).
+ * A key set (query set for the VJP's per-key pass) too large for the kernels' shared memory returns KDB_ERR_UNSUPPORTED before any launch. */
+int kdb_attention_jvp(const float* qkv, const float* dqkv, float* dout, int batch, int h, int w, int n_heads, int d_head,
+                      int attn_type, int attn_param, int shift, void* stream);
+int kdb_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int batch, int h, int w,
+                      int n_heads, int d_head, int attn_type, int attn_param, int shift, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1067,4 +1067,18 @@ int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch
                                         attn_param, shift, st);
 }
 
+int kdb_attention_jvp(const float* qkv, const float* dqkv, float* dout, int batch, int h, int w, int n_heads, int d_head, int attn_type,
+                      int attn_param, int shift, void* stream) {
+  KDB_REQUIRE(qkv && dqkv && dout && batch > 0 && h > 0 && w > 0 && n_heads > 0 && d_head > 0, KDB_ERR_BAD_ARG,
+              "attention_jvp: bad argument");
+  return launch_attention_jvp(qkv, dqkv, dout, batch, h, w, n_heads, d_head, attn_type, attn_param, shift, (cudaStream_t)stream);
+}
+
+int kdb_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int batch, int h, int w, int n_heads,
+                      int d_head, int attn_type, int attn_param, int shift, void* stream) {
+  KDB_REQUIRE(qkv && out && dout && dqkv && stats && batch > 0 && h > 0 && w > 0 && n_heads > 0 && d_head > 0, KDB_ERR_BAD_ARG,
+              "attention_vjp: bad argument");
+  return launch_attention_vjp(qkv, out, dout, dqkv, stats, batch, h, w, n_heads, d_head, attn_type, attn_param, shift, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -72,6 +72,8 @@ SIGNATURES = {
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "kdb_attn_block_bf16": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "kdb_attention": (_i32, [_i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_attention_jvp": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_attention_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
 }
 
 _lib = None
@@ -544,3 +546,38 @@ def attention(qkv, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, fast
     check(lib().kdb_attention(prec, 1 if fast else 0, ptr(qkv.contiguous()), ptr(out), B, h, w, n_heads, d_head, code, attn_param, shift,
                                ptr(logit_bound), stream()))
     return out
+
+
+def _fp32_attention_args(tensors, numels):
+    for t, n in zip(tensors, numels):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n:
+            raise ValueError(f"the attention derivatives take contiguous fp32 tensors of the attention's shape (got {t.dtype} {tuple(t.shape)})")
+
+
+@_on_device_of_first
+def attention_jvp(qkv, dqkv, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, out=None):
+    """Tangent of the fp32 attention(qkv) along dqkv (both [B, h*w, 3*n_heads*d_head]) -> [B, h*w, n_heads*d_head]."""
+    require_cuda(qkv, dqkv, out)
+    B = qkv.shape[0]
+    out = torch.empty(B, h * w, n_heads * d_head, dtype=torch.float32, device=qkv.device) if out is None else out
+    T = B * h * w * n_heads * d_head
+    _fp32_attention_args((qkv, dqkv, out), (3 * T, 3 * T, T))
+    code = _ATTN_CODE[attn_type] if isinstance(attn_type, str) else attn_type
+    check(lib().kdb_attention_jvp(ptr(qkv), ptr(dqkv), ptr(out), B, h, w, n_heads, d_head, code, attn_param, shift, stream()))
+    return out
+
+
+@_on_device_of_first
+def attention_vjp(qkv, out, dout, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, dqkv=None, stats=None):
+    """Gradient of the fp32 attention(qkv) for the output gradient dout: qkv [B, h*w, 3*n_heads*d_head], out = attention(qkv) and dout
+    [B, h*w, n_heads*d_head] -> dqkv like qkv.  stats: optional scratch [B, n_heads, h*w, 3] fp32 (the per-query softmax statistics)."""
+    require_cuda(qkv, out, dout, dqkv, stats)
+    B = qkv.shape[0]
+    dqkv = torch.empty_like(qkv) if dqkv is None else dqkv
+    stats = torch.empty(B, n_heads, h * w, 3, dtype=torch.float32, device=qkv.device) if stats is None else stats
+    T = B * h * w * n_heads * d_head
+    _fp32_attention_args((qkv, out, dout, dqkv, stats), (3 * T, T, T, 3 * T, B * n_heads * h * w * 3))
+    code = _ATTN_CODE[attn_type] if isinstance(attn_type, str) else attn_type
+    check(lib().kdb_attention_vjp(ptr(qkv), ptr(out), ptr(dout), ptr(dqkv), ptr(stats), B, h, w, n_heads, d_head, code, attn_param, shift,
+                                   stream()))
+    return dqkv

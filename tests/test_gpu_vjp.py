@@ -27,6 +27,8 @@ DEV = "cuda"
 
 NA3_64x96 = copy.deepcopy(NA3)
 NA3_64x96["model"]["input_size"] = [64, 96]
+NA3_48 = copy.deepcopy(NA3)
+NA3_48["model"]["input_size"] = [48, 48]          # a 12x12 neighbourhood level: a middle key is seen by all 12 queries of each axis
 
 
 def cotangent(shape, seed):
@@ -58,12 +60,13 @@ def test_cfg1_per_sample_rows_vs_oracle(aug):
     check_tangent(g, want_g, "cfg1 u^T J_D")
 
 
-@pytest.mark.parametrize("name", ["sw64", "na3", "na3_64x96", "nonsquare"])
+@pytest.mark.parametrize("name", ["sw64", "na3", "na3_64x96", "na3_48", "nonsquare"])
 def test_models_vs_oracle_both_routes(name):
-    """sw64 (shift 0 and 4 at every level), [neighbourhood, none, global] at 64x64 and on the non-square 16x24 token grid (the inverse
-    neighbourhood ranges at the borders), and a non-square model with mapping / class / aug conditioning, patch 2x4 and window 4.  The
-    per-sample route through Denoiser.vjp; without conditioning also the shared-row route (cond_batch_stride 0) through the evaluator."""
-    raw = {"sw64": "sw64", "na3": NA3, "na3_64x96": NA3_64x96, "nonsquare": NONSQUARE}[name]
+    """sw64 (shift 0 and 4 at every level), [neighbourhood, none, global] at 64x64, on the non-square 16x24 token grid (the inverse
+    neighbourhood ranges at the borders) and at 48x48 (12x12 tokens with k = 7, where the clamped windows of the two borders overlap), and
+    a non-square model with mapping / class / aug conditioning, patch 2x4 and window 4.  The per-sample route through Denoiser.vjp; without
+    conditioning also the shared-row route (cond_batch_stride 0) through the evaluator."""
+    raw = {"sw64": "sw64", "na3": NA3, "na3_64x96": NA3_64x96, "na3_48": NA3_48, "nonsquare": NONSQUARE}[name]
     cfg, sd, inner, model, _ = build(raw)
     mcfg = cfg["model"]
     C, (H, W) = mcfg["input_channels"], mcfg["input_size"]
