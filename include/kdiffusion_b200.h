@@ -119,7 +119,10 @@ int kdb_noise_normal(float* out, const int64_t* seeds, uint64_t stream_id, int b
 /* Virtual Brownian bridge increment W(t1) - W(t0), normalised by sqrt(|t1 - t0|), per sample.
  * Replaces BatchedBrownianTree / BrownianTreeNoiseSampler (sampling.py:65-114): dyadic Brownian-bridge
  * tree on [t_min, t_max] of `depth` levels evaluated from (seed[b], node, element) counters.
- * Parity with torchsde is UNPINNED (torchsde absent); contract = determinism, additivity, unit variance. */
+ * Parity with torchsde is UNPINNED (torchsde absent).  The values are pinned instead: oracle/counter_noise.py restates the counter
+ * stream in float64 and tests/test_gpu_noise.py holds this kernel to it element by element.
+ * t0 and t1 are clamped to [t_min, t_max], but the norm is the UNCLAMPED sqrt(|t1 - t0|): a call reaching outside the interval
+ * returns increments of variance |clamped span| / |t1 - t0| < 1.  The samplers never make such a call. */
 int kdb_noise_brownian(float* out, const int64_t* seeds, int batch, int64_t per_sample,
                        double t_min, double t_max, double t0, double t1, int depth, void* stream);
 

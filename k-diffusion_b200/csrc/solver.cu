@@ -261,7 +261,10 @@ __global__ void __launch_bounds__(256) noise_normal_kernel(float* __restrict__ o
 }
 
 // Box-Muller on the MUFU unit (lg2, sqrt, sin, cos: ~8 MUFU + 12 FP32 instructions for four normals instead of ~150 with the
-// accurate logf / sincospif): the Brownian tree draws 25-50 of these per output group, absolute error ~1e-6.
+// accurate logf / sincospif): the Brownian tree draws 25-50 of these per output group.  Absolute error, measured on an H100 80GB HBM3
+// against float64 Box-Muller of the same uniforms (tests/test_gpu_noise.py): 1.4e-6 at the largest radius (u = 2^-25, r = 5.9), but
+// 1.2e-4 at u = 1 - 2^-23, where r is only 4.9e-4 and the absolute error of __log2f near 1 (2^-22 in the CUDA guide) dominates; the
+// guide's bounds allow up to 5.8e-4 there.  u = 1.0f gives exactly 0.
 __device__ __forceinline__ float4 normal4_fast(uint4 r) {
   constexpr float kNeg2Ln2 = -1.3862943611198906f, kTwoPi = 6.283185307179586f;
   const float r0 = __fsqrt_rn(kNeg2Ln2 * __log2f(u01(r.x)));
