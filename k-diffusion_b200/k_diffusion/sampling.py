@@ -181,31 +181,55 @@ def host_sigmas(sigmas):
     return [float(v) for v in sigmas.detach().to(torch.float32).cpu().tolist()]
 
 
-def _churn(sig, i, s_churn, s_tmin, s_tmax):
+# Every fixed-schedule sampler is a plan: a list of steps, each a short list of ops over named buffers ('x' is the state):
+#     ('eval',  out, src)                 out = D(src, sigma_k)      k-th entry of the step's 'evals'
+#     ('lin',   out, [(name, coef), ...]) out = sum coef * name      one kdb_solver_lincomb launch
+#     ('noise', out, sigma_from, sigma_to) out = noise_sampler(sigma_from, sigma_to)
+#     ('randn', out)                      out = torch.randn_like(x)  torch's global generator (Karras churn): never captured
+#     ('keep',  out, src)                 out aliases src (history of multistep methods; evals always write fresh buffers)
+#     ('euler', out, x, den, r, noise, cn)          out = x + (x - den) r [+ noise cn]       one kdb_solver_euler_step launch
+#     ('heun',  out, x, den, x2, den2, a1, a2)      out = x + (x - den) a1 + (x2 - den2) a2  one kdb_solver_heun_correct launch
+#     ('dpmpp_2m', out, x, den, old, a, b, k1, k0)  out = a x - b (k1 den + k0 old)          one kdb_solver_dpmpp_2m_step launch
+# In 'euler' noise = None drops the noise term; in 'dpmpp_2m' old is not read when k0 == 0 (the first step has no history).
+# The fused kinds serve Euler, Heun, Euler-ancestral and DPM++(2M).  Every update of the other samplers is a linear combination,
+# with host-computable scalar coefficients, of at most five image tensors: they stay on 'lin' (a fused kind would change their rounding).
+# Plans are pure host math (verified on the CPU against reference trajectories in tests/test_host_logic.py); `_sample_ops` runs them.
+
+def _churn(sig, i, s_churn, s_tmin, s_tmax, s_noise):
+    """(gamma, sigma_hat, ops) of step i's Karras churn: the noise is drawn only on steps with gamma > 0 (DESIGN.md quirk Q1)."""
     n = len(sig) - 1
     gamma = min(s_churn / n, 2 ** 0.5 - 1) if s_tmin <= sig[i] <= s_tmax else 0.
     sigma_hat = float(f32(sig[i]) * f32(gamma + 1))
-    coef = float(np.sqrt(f32(sigma_hat) ** 2 - f32(sig[i]) ** 2)) if gamma > 0 else 0.
-    return gamma, sigma_hat, coef
+    if not gamma > 0:
+        return gamma, sigma_hat, []
+    coef = float(np.sqrt(f32(sigma_hat) ** 2 - f32(sig[i]) ** 2))
+    return gamma, sigma_hat, [('randn', 'n'), ('lin', 'x', [('x', 1.), ('n', s_noise * coef)])]
 
 
-def plan_euler(sig, s_churn=0., s_tmin=0., s_tmax=float('inf')):
+def plan_euler(sig, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
     steps = []
     for i in range(len(sig) - 1):
-        gamma, sigma_hat, coef = _churn(sig, i, s_churn, s_tmin, s_tmax)
-        dt = float(f32(sig[i + 1]) - f32(sigma_hat))
-        steps.append(dict(i=i, gamma=gamma, sigma_hat=sigma_hat, churn=coef, r=dt / sigma_hat, evals=[sigma_hat]))
+        gamma, sigma_hat, ops = _churn(sig, i, s_churn, s_tmin, s_tmax, s_noise)
+        r = float(f32(sig[i + 1]) - f32(sigma_hat)) / sigma_hat
+        ops += [('eval', 'den', 'x'), ('euler', 'x', 'x', 'den', r, None, 0.)]
+        steps.append(dict(i=i, gamma=gamma, sigma_hat=sigma_hat, ops=ops, evals=[sigma_hat]))
     return steps
 
 
-def plan_heun(sig, s_churn=0., s_tmin=0., s_tmax=float('inf')):
-    steps = plan_euler(sig, s_churn, s_tmin, s_tmax)
-    for st in steps:
-        nxt = sig[st['i'] + 1]
-        dt = float(f32(nxt) - f32(st['sigma_hat']))
-        st['last'] = nxt == 0
-        if not st['last']:
-            st.update(sigma_next=nxt, a1=dt / (2 * st['sigma_hat']), a2=dt / (2 * nxt), evals=[st['sigma_hat'], nxt])
+def plan_heun(sig, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
+    steps = []
+    for i in range(len(sig) - 1):
+        gamma, sigma_hat, ops = _churn(sig, i, s_churn, s_tmin, s_tmax, s_noise)
+        nxt = sig[i + 1]
+        dt = float(f32(nxt) - f32(sigma_hat))
+        if nxt == 0:                                      # the final step to sigma = 0 is Euler
+            ops += [('eval', 'den', 'x'), ('euler', 'x', 'x', 'den', dt / sigma_hat, None, 0.)]
+            evals = [sigma_hat]
+        else:                                             # Euler predictor, trapezoidal corrector
+            ops += [('eval', 'den', 'x'), ('euler', 'x2', 'x', 'den', dt / sigma_hat, None, 0.), ('eval', 'den2', 'x2'),
+                    ('heun', 'x', 'x', 'den', 'x2', 'den2', dt / (2 * sigma_hat), dt / (2 * nxt))]
+            evals = [sigma_hat, nxt]
+        steps.append(dict(i=i, gamma=gamma, sigma_hat=sigma_hat, ops=ops, evals=evals))
     return steps
 
 
@@ -213,8 +237,9 @@ def plan_euler_ancestral(sig, eta=1., s_noise=1.):
     steps = []
     for i in range(len(sig) - 1):
         down, up = get_ancestral_step(sig[i], sig[i + 1], eta=eta)
-        steps.append(dict(i=i, sigma=sig[i], sigma_next=sig[i + 1], r=(down - sig[i]) / sig[i], cn=s_noise * up,
-                          noise=sig[i + 1] > 0, evals=[sig[i]]))
+        noise = [('noise', 'n', sig[i], sig[i + 1])] if sig[i + 1] > 0 else []
+        ops = [('eval', 'den', 'x')] + noise + [('euler', 'x', 'x', 'den', (down - sig[i]) / sig[i], 'n' if noise else None, s_noise * up)]
+        steps.append(dict(i=i, sigma_hat=sig[i], ops=ops, evals=[sig[i]]))
     return steps
 
 
@@ -232,20 +257,10 @@ def plan_dpmpp_2m(sig):
         else:
             r = (math.log(sig[i - 1]) - math.log(s)) / h
             k1, k0 = 1 + 1 / (2 * r), -1 / (2 * r)
-        steps.append(dict(i=i, sigma=s, a=a, b=b, k1=k1, k0=k0, evals=[s]))
+        ops = [('eval', 'den', 'x'), ('dpmpp_2m', 'x', 'x', 'den', 'old', a, b, k1, k0), ('keep', 'old', 'den')]
+        steps.append(dict(i=i, sigma_hat=s, ops=ops, evals=[s]))
     return steps
 
-
-# --------------------------------------------------------------------------------------------
-# Generic step plans (SURVEY 8f.1: the remaining fixed-schedule samplers).  Every update of these solvers is a linear
-# combination, with host-computable scalar coefficients, of at most five image tensors, so a step is a short list of ops
-# over named buffers:
-#     ('eval',  out, src)                 out = D(src, sigma_k)      k-th entry of the step's 'evals'
-#     ('lin',   out, [(name, coef), ...]) out = sum coef * name      one kdb_solver_lincomb launch
-#     ('noise', out, sigma_from, sigma_to) out = noise_sampler(sigma_from, sigma_to)
-#     ('keep',  out, src)                 out aliases src (history of multistep methods; evals always write fresh buffers)
-# Plans are pure host math (verified on the CPU against reference trajectories in tests/test_host_logic.py).
-# --------------------------------------------------------------------------------------------
 
 def _log_mid(a, b):
     return math.exp(0.5 * (math.log(a) + math.log(b)))
@@ -267,12 +282,12 @@ def _dpm2_ops(sigma, target):
             ('lin', 'x', [('x', 1.), ('x2', c2), ('den2', -c2)])], [sigma, mid]
 
 
-def plan_dpm_2(sig, s_churn=0., s_tmin=0., s_tmax=float('inf')):
+def plan_dpm_2(sig, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
     steps = []
     for i in range(len(sig) - 1):
-        gamma, sigma_hat, coef = _churn(sig, i, s_churn, s_tmin, s_tmax)
+        gamma, sigma_hat, churn = _churn(sig, i, s_churn, s_tmin, s_tmax, s_noise)
         ops, evals = _dpm2_ops(sigma_hat, sig[i + 1])
-        steps.append(dict(i=i, gamma=gamma, sigma_hat=sigma_hat, churn=coef, ops=ops, evals=evals))
+        steps.append(dict(i=i, gamma=gamma, sigma_hat=sigma_hat, ops=churn + ops, evals=evals))
     return steps
 
 
@@ -585,7 +600,8 @@ def _finish(x_work, x):
 
 
 def _scalar_like(sigmas, v):
-    return torch.as_tensor(v, dtype=sigmas.dtype, device=sigmas.device)
+    """0-d tensor of v on sigmas' device, filled there: a host-to-device copy would synchronise the eager loop every step"""
+    return torch.full((), v, dtype=sigmas.dtype, device=sigmas.device)
 
 
 _graph_cache = {}
@@ -712,131 +728,20 @@ def _on_x_device(fn):
     return wrapper
 
 
-@_on_x_device
-@torch.no_grad()
-def sample_euler(model, x, sigmas, extra_args=None, callback=None, disable=None, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
-    """Algorithm 2 (Euler steps) from Karras et al. (2022)."""
-    xw, sig, extra_args = _prepare(x, sigmas, extra_args)
-    plan = plan_euler(sig, s_churn, s_tmin, s_tmax)
-    ev = _Evaluator(model, xw, extra_args, [s for st in plan for s in st['evals']])
-
-    def body(xc):
-        for k, st in enumerate(_progress(plan, disable)):
-            if st['gamma'] > 0:
-                xc = _native.lincomb([xc, torch.randn_like(xc)], [1., s_noise * st['churn']])
-            den = ev(k, xc)
-            if callback is not None:
-                callback({'x': xc, 'i': st['i'], 'sigma': sigmas[st['i']], 'sigma_hat': _scalar_like(sigmas, st['sigma_hat']), 'denoised': den})
-            xc = _native.euler_step(xc, den, st['r'])
-        return xc
-
-    out = _run('euler', body, ev, xw, sig, (s_churn, s_tmin, s_tmax, s_noise), callback, noise_sampler=_GLOBAL_RNG if any(st['gamma'] > 0 for st in plan) else None)
-    return _finish(out, x)
-
-
-@_on_x_device
-@torch.no_grad()
-def sample_euler_ancestral(model, x, sigmas, extra_args=None, callback=None, disable=None, eta=1., s_noise=1., noise_sampler=None):
-    """Ancestral sampling with Euler method steps."""
-    xw, sig, extra_args = _prepare(x, sigmas, extra_args)
-    ours = isinstance(noise_sampler, (BrownianTreeNoiseSampler, PhiloxNoiseSampler))
-    noise_sampler = default_noise_sampler(xw) if noise_sampler is None else noise_sampler
-    plan = plan_euler_ancestral(sig, eta, s_noise)
-    ev = _Evaluator(model, xw, extra_args, [s for st in plan for s in st['evals']])
-
-    def body(xc):
-        for k, st in enumerate(_progress(plan, disable)):
-            den = ev(k, xc)
-            if callback is not None:
-                callback({'x': xc, 'i': st['i'], 'sigma': sigmas[st['i']], 'sigma_hat': sigmas[st['i']], 'denoised': den})
-            noise = None
-            if st['noise']:      # our samplers take host floats (no sync); foreign callables get tensors like the reference
-                args = (st['sigma'], st['sigma_next']) if ours else (sigmas[st['i']], sigmas[st['i'] + 1])
-                noise = _native.f32c(noise_sampler(*args))
-            xc = _native.euler_step(xc, den, st['r'], noise=noise, cn=st['cn'])
-        return xc
-
-    # a graph replays the same noise kernels every call: only legal for the Brownian tree (a pure function of seeds and sigma)
-    out = _run('euler_a', body, ev, xw, sig, (eta, s_noise), callback, noise_sampler=noise_sampler if any(st['noise'] for st in plan) else None)
-    return _finish(out, x)
-
-
-@_on_x_device
-@torch.no_grad()
-def sample_heun(model, x, sigmas, extra_args=None, callback=None, disable=None, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
-    """Algorithm 2 (Heun steps) from Karras et al. (2022)."""
-    xw, sig, extra_args = _prepare(x, sigmas, extra_args)
-    plan = plan_heun(sig, s_churn, s_tmin, s_tmax)
-    ev = _Evaluator(model, xw, extra_args, [s for st in plan for s in st['evals']])
-
-    def body(xc):
-        k = 0
-        for st in _progress(plan, disable):
-            if st['gamma'] > 0:
-                xc = _native.lincomb([xc, torch.randn_like(xc)], [1., s_noise * st['churn']])
-            den = ev(k, xc)
-            k += 1
-            if callback is not None:
-                callback({'x': xc, 'i': st['i'], 'sigma': sigmas[st['i']], 'sigma_hat': _scalar_like(sigmas, st['sigma_hat']), 'denoised': den})
-            if st['last']:
-                xc = _native.euler_step(xc, den, st['r'])                               # final step to sigma = 0 is Euler
-            else:
-                x_2 = _native.euler_step(xc, den, st['r'])                              # predictor
-                den_2 = ev(k, x_2)
-                k += 1
-                xc = _native.heun_correct(xc, den, x_2, den_2, st['a1'], st['a2'])      # trapezoidal corrector
-        return xc
-
-    out = _run('heun', body, ev, xw, sig, (s_churn, s_tmin, s_tmax, s_noise), callback, noise_sampler=_GLOBAL_RNG if any(st['gamma'] > 0 for st in plan) else None)
-    return _finish(out, x)
-
-
-@_on_x_device
-@torch.no_grad()
-def sample_dpmpp_2m(model, x, sigmas, extra_args=None, callback=None, disable=None):
-    """DPM-Solver++(2M)."""
-    xw, sig, extra_args = _prepare(x, sigmas, extra_args)
-    plan = plan_dpmpp_2m(sig)
-    ev = _Evaluator(model, xw, extra_args, [s for st in plan for s in st['evals']])
-
-    def body(xc):
-        old = None
-        for k, st in enumerate(_progress(plan, disable)):
-            den = ev(k, xc)
-            if callback is not None:
-                callback({'x': xc, 'i': st['i'], 'sigma': sigmas[st['i']], 'sigma_hat': sigmas[st['i']], 'denoised': den})
-            xc = _native.dpmpp_2m_step(xc, den, old if st['k0'] != 0 else None, st['a'], st['b'], st['k1'], st['k0'])
-            old = den
-        return xc
-
-    out = _run('dpmpp_2m', body, ev, xw, sig, (), callback)
-    return _finish(out, x)
-
-
-# --------------------------------------------------------------------------------------------
-# SURVEY 8f.1: the remaining fixed-schedule samplers, on the generic op plans.  Same evaluator, same graph runner and the
-# same kernels (`kdb_solver_lincomb`, the noise kernels) as the four samplers above; the plans are verified on the CPU
-# against reference trajectories (tests/test_host_logic.py).  GPU parity tests for these entry points land with round 2.
-# --------------------------------------------------------------------------------------------
-
-def _sample_ops(name, model, x, sigmas, plan_fn, extra_args, callback, disable, params, noise_sampler=None, churn_noise=0., callback_extra=None,
-                on_eval=None):
-    """Run a generic op plan.  `plan_fn(sig)` builds it from the host copy of `sigmas` (or is the plan itself, a list);
+def _sample_ops(name, model, x, sigmas, plan_fn, extra_args, callback, disable, params, noise_sampler=None, callback_extra=None, on_eval=None):
+    """Run an op plan.  `plan_fn(sig)` builds it from the host copy of `sigmas` (or is the plan itself, a list);
     `callback_extra(st)` may add keys to the callback payload of a step; `on_eval()` runs after every model evaluation (like `callback`
     it keeps the loop out of a CUDA graph)."""
     xw, sig, extra_args = _prepare(x, sigmas, extra_args)
     plan = plan_fn if isinstance(plan_fn, list) else plan_fn(sig)
-    needs_noise = any(op[0] == 'noise' for st in plan for op in st['ops'])
+    kinds = {op[0] for st in plan for op in st['ops']}
     ours = isinstance(noise_sampler, (BrownianTreeNoiseSampler, PhiloxNoiseSampler))
-    churned = any(st.get('gamma', 0) > 0 for st in plan)
     ev = _Evaluator(model, xw, extra_args, [s_ for st in plan for s_ in st['evals']])
 
     def body(xc):
         T = {'x': xc}
         k = 0
         for st in _progress(plan, disable):
-            if st.get('gamma', 0) > 0:
-                T['x'] = _native.lincomb([T['x'], torch.randn_like(T['x'])], [1., churn_noise * st['churn']])
             first = True
             for op in st['ops']:
                 kind = op[0]
@@ -851,17 +756,57 @@ def _sample_ops(name, model, x, sigmas, plan_fn, extra_args, callback, disable, 
                     first = False
                 elif kind == 'lin':
                     T[op[1]] = _lin_x([(T[n], c) for n, c in op[2]], keep_zero=True)
+                elif kind == 'euler':
+                    T[op[1]] = _native.euler_step(T[op[2]], T[op[3]], op[4], noise=None if op[5] is None else T[op[5]], cn=op[6])
+                elif kind == 'heun':
+                    T[op[1]] = _native.heun_correct(T[op[2]], T[op[3]], T[op[4]], T[op[5]], op[6], op[7])
+                elif kind == 'dpmpp_2m':
+                    T[op[1]] = _native.dpmpp_2m_step(T[op[2]], T[op[3]], T[op[4]] if op[8] != 0 else None, *op[5:])
                 elif kind == 'noise':    # our samplers take host floats (no sync); foreign callables get tensors like the reference
                     args = (op[2], op[3]) if ours else (_scalar_like(sigmas, op[2]), _scalar_like(sigmas, op[3]))
                     T[op[1]] = _native.f32c(noise_sampler(*args))
+                elif kind == 'randn':
+                    T[op[1]] = torch.randn_like(T['x'])
                 else:                    # 'keep': alias, evaluations always write fresh buffers
                     T[op[1]] = T[op[2]]
         return T['x']
 
     # a graph replays the same noise kernels every call: only legal without noise or with the Brownian tree
     out = _run(name, body, ev, xw, sig, params, callback if callback is not None else on_eval,
-               noise_sampler=_GLOBAL_RNG if churned else (noise_sampler if needs_noise else None))
+               noise_sampler=_GLOBAL_RNG if 'randn' in kinds else (noise_sampler if 'noise' in kinds else None))
     return _finish(out, x)
+
+
+@_on_x_device
+@torch.no_grad()
+def sample_euler(model, x, sigmas, extra_args=None, callback=None, disable=None, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
+    """Algorithm 2 (Euler steps) from Karras et al. (2022)."""
+    return _sample_ops('euler', model, x, sigmas, lambda sig: plan_euler(sig, s_churn, s_tmin, s_tmax, s_noise), extra_args, callback, disable,
+                       (s_churn, s_tmin, s_tmax, s_noise))
+
+
+@_on_x_device
+@torch.no_grad()
+def sample_euler_ancestral(model, x, sigmas, extra_args=None, callback=None, disable=None, eta=1., s_noise=1., noise_sampler=None):
+    """Ancestral sampling with Euler method steps."""
+    noise_sampler = default_noise_sampler(_native.f32c(x)) if noise_sampler is None else noise_sampler
+    return _sample_ops('euler_a', model, x, sigmas, lambda sig: plan_euler_ancestral(sig, eta, s_noise), extra_args, callback, disable,
+                       (eta, s_noise), noise_sampler)
+
+
+@_on_x_device
+@torch.no_grad()
+def sample_heun(model, x, sigmas, extra_args=None, callback=None, disable=None, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
+    """Algorithm 2 (Heun steps) from Karras et al. (2022)."""
+    return _sample_ops('heun', model, x, sigmas, lambda sig: plan_heun(sig, s_churn, s_tmin, s_tmax, s_noise), extra_args, callback, disable,
+                       (s_churn, s_tmin, s_tmax, s_noise))
+
+
+@_on_x_device
+@torch.no_grad()
+def sample_dpmpp_2m(model, x, sigmas, extra_args=None, callback=None, disable=None):
+    """DPM-Solver++(2M)."""
+    return _sample_ops('dpmpp_2m', model, x, sigmas, plan_dpmpp_2m, extra_args, callback, disable, ())
 
 
 def _default_brownian(x, sigmas):
@@ -873,8 +818,8 @@ def _default_brownian(x, sigmas):
 @torch.no_grad()
 def sample_dpm_2(model, x, sigmas, extra_args=None, callback=None, disable=None, s_churn=0., s_tmin=0., s_tmax=float('inf'), s_noise=1.):
     """A sampler inspired by DPM-Solver-2 and Algorithm 2 from Karras et al. (2022)  (reference sampling.py:187-214)."""
-    return _sample_ops('dpm_2', model, x, sigmas, lambda sig: plan_dpm_2(sig, s_churn, s_tmin, s_tmax), extra_args, callback, disable,
-                       (s_churn, s_tmin, s_tmax, s_noise), churn_noise=s_noise)
+    return _sample_ops('dpm_2', model, x, sigmas, lambda sig: plan_dpm_2(sig, s_churn, s_tmin, s_tmax, s_noise), extra_args, callback, disable,
+                       (s_churn, s_tmin, s_tmax, s_noise))
 
 
 @_on_x_device

@@ -46,47 +46,9 @@ def test_ancestral_step_and_scalings(kat):
         assert_close(got, unhex(want), rtol=2e-7, atol=0)
 
 
-def _exec_plan(kind, plan, model, x, noise=None):
-    """numpy executor of a step plan: what the fused kernels compute, on the CPU, for plan verification only."""
-    x = x.clone()
-    B = x.shape[0]
-    old = None
-    for st in plan:
-        if kind in ("euler", "heun"):
-            den = model(x, torch.full([B], st["sigma_hat"]))
-            if kind == "euler" or st["last"]:
-                x = x + (x - den) * np.float32(st["r"])
-            else:
-                x2 = x + (x - den) * np.float32(st["r"])
-                den2 = model(x2, torch.full([B], st["sigma_next"]))
-                x = x + ((x - den) * np.float32(st["a1"]) + (x2 - den2) * np.float32(st["a2"]))
-        elif kind == "euler_a":
-            den = model(x, torch.full([B], st["sigma"]))
-            x = x + (x - den) * np.float32(st["r"])
-            if st["noise"]:
-                x = x + noise[st["i"]] * np.float32(st["cn"])
-        else:
-            den = model(x, torch.full([B], st["sigma"]))
-            x = np.float32(st["a"]) * x - np.float32(st["b"]) * (np.float32(st["k1"]) * den + (np.float32(st["k0"]) * old if old is not None else 0))
-            old = den
-    return x
-
-
-def test_step_plans_reproduce_reference_trajectories():
-    z = load_npz("toy_samplers.npz")
-    toy2 = lambda x, s, **kw: x / (1 + s[:, None, None, None] ** 2) + 0.1 * torch.tanh(x)
-    sig = S.host_sigmas(z["sigmas"])
-    cases = [("euler", S.plan_euler(sig), "sample_euler"), ("heun", S.plan_heun(sig), "sample_heun"),
-             ("dpmpp", S.plan_dpmpp_2m(sig), "sample_dpmpp_2m")]
-    for kind, plan, key in cases:
-        assert_close(_exec_plan(kind, plan, toy2, z["x"]), z[key], rtol=1e-4, atol=1e-5, what=key)
-    assert_close(_exec_plan("euler_a", S.plan_euler_ancestral(sig), toy2, z["x"], z["noise"]), z["sample_euler_ancestral"], rtol=1e-4, atol=1e-5)
-    assert_close(_exec_plan("euler_a", S.plan_euler_ancestral(sig, eta=0.5, s_noise=0.9), toy2, z["x"], z["noise"]),
-                 z["sample_euler_ancestral_eta05"], rtol=1e-4, atol=1e-5)
-
-
 def _exec_ops(plan, model, x, noise=None):
-    """CPU interpreter of the generic op plans (what the lincomb kernel and the evaluator do), for plan verification only."""
+    """CPU interpreter of the op plans (what the solver kernels and the evaluator do), for plan verification only."""
+    f = np.float32
     T = {"x": x.clone()}
     B = x.shape[0]
     it = iter(noise) if noise is not None else None
@@ -97,7 +59,16 @@ def _exec_ops(plan, model, x, noise=None):
                 T[op[1]] = model(T[op[2]], torch.full([B], st["evals"][k]))
                 k += 1
             elif op[0] == "lin":
-                T[op[1]] = sum(np.float32(c) * T[n] for n, c in op[2])
+                T[op[1]] = sum(f(c) * T[n] for n, c in op[2])
+            elif op[0] == "euler":
+                _, out, xn, dn, r, nn, cn = op
+                T[out] = T[xn] + (T[xn] - T[dn]) * f(r) + (0 if nn is None else T[nn] * f(cn))
+            elif op[0] == "heun":
+                _, out, xn, dn, x2, d2, a1, a2 = op
+                T[out] = T[xn] + ((T[xn] - T[dn]) * f(a1) + (T[x2] - T[d2]) * f(a2))
+            elif op[0] == "dpmpp_2m":
+                _, out, xn, dn, old, a, b, k1, k0 = op
+                T[out] = f(a) * T[xn] - f(b) * (f(k1) * T[dn] + (f(k0) * T[old] if k0 != 0 else 0))
             elif op[0] == "noise":
                 T[op[1]] = next(it)
             elif op[0] == "keep":
@@ -106,6 +77,19 @@ def _exec_ops(plan, model, x, noise=None):
                 raise AssertionError(op)
         assert k == len(st["evals"])
     return T["x"]
+
+
+def test_fused_step_plans_reproduce_reference_trajectories():
+    """Euler / Heun / DPM++(2M) / Euler-ancestral op plans (fused step kinds) vs trajectories recorded from the reference
+    (oracle/make_golden.py), through the same op interpreter as the other samplers' plans."""
+    toy2 = lambda x, s, **kw: x / (1 + s[:, None, None, None] ** 2) + 0.1 * torch.tanh(x)
+    z = load_npz("toy_samplers.npz")
+    sig = S.host_sigmas(z["sigmas"])
+    for key, plan, noise in [("sample_euler", S.plan_euler(sig), None), ("sample_heun", S.plan_heun(sig), None),
+                             ("sample_dpmpp_2m", S.plan_dpmpp_2m(sig), None),
+                             ("sample_euler_ancestral", S.plan_euler_ancestral(sig), z["noise"]),
+                             ("sample_euler_ancestral_eta05", S.plan_euler_ancestral(sig, eta=0.5, s_noise=0.9), z["noise"])]:
+        assert_close(_exec_ops(plan, toy2, z["x"], noise), z[key], rtol=1e-4, atol=1e-5, what=key)
 
 
 def test_generic_op_plans_reproduce_reference_trajectories():
@@ -185,19 +169,21 @@ def test_generic_sampler_entry_points_with_stubbed_kernels(monkeypatch):
         S.sample_dpmpp_2m_sde(toy2, x, sig, solver_type="euler")
 
 
-def test_plan_details():
+def test_op_plan_details():
     sig = S.host_sigmas(S.get_sigmas_karras(50, 1e-2, 160))
+    kinds = lambda st: [op[0] for op in st["ops"]]
     heun = S.plan_heun(sig)
     assert sum(len(st["evals"]) for st in heun) == 99                       # NFE of Heun-50 (SURVEY 3.2)
-    assert heun[-1]["last"] and heun[-1]["r"] == -1.0                       # final Euler step lands on denoised
+    assert kinds(heun[-1]) == ["eval", "euler"] and heun[-1]["ops"][-1][4] == -1.0      # final Euler step lands on denoised
     assert sum(len(st["evals"]) for st in S.plan_dpmpp_2m(S.host_sigmas(S.get_sigmas_karras(25, 1e-2, 160)))) == 25
-    d = S.plan_dpmpp_2m(sig)
-    assert d[0]["k0"] == 0 and d[-1]["a"] == 0 and d[-1]["b"] == -1 and d[-1]["k0"] == 0
+    d = [[op for op in st["ops"] if op[0] == "dpmpp_2m"][0] for st in S.plan_dpmpp_2m(sig)]     # (kind, out, x, den, old, a, b, k1, k0)
+    assert d[0][8] == 0 and d[-1][5] == 0 and d[-1][6] == -1 and d[-1][8] == 0
     ch = S.plan_heun(sig, s_churn=40, s_tmin=0.05, s_tmax=50)
     on = [st for st in ch if st["gamma"] > 0]
     assert on and all(0.05 <= sig[st["i"]] <= 50 for st in on) and all(abs(st["gamma"] - (2 ** 0.5 - 1)) < 1e-12 for st in on)
+    assert all(kinds(st)[:3] == ["randn", "lin", "eval"] if st["gamma"] > 0 else "randn" not in kinds(st) for st in ch)   # draw before the step
     ea = S.plan_euler_ancestral(sig)
-    assert not ea[-1]["noise"] and ea[-1]["r"] == -1.0 and all(st["noise"] for st in ea[:-1])
+    assert "noise" not in kinds(ea[-1]) and ea[-1]["ops"][-1][4] == -1.0 and all("noise" in kinds(st) for st in ea[:-1])
     with pytest.raises(ValueError):
         S.host_sigmas(torch.zeros(1))
 
