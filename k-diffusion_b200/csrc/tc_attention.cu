@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
       for (int it = 0; it < n_iter; ++it) {
         const int j = it % nblk;
         const bool with_v = !two_pass || it >= nblk;
-        if (it > 0) tc::mbar_wait(&bars->kv_free, (uint32_t)(it - 1) & 1u);
+        if (it > 0) tc::mbar_wait_nocall(&bars->kv_free, (uint32_t)(it - 1) & 1u);
         constexpr uint32_t KV_BYTES = (MODE == MODE_NA) ? NA_BLK_KEYS * 128 : TILE_BYTES;
         tc::mbar_arrive_expect_tx(&bars->kv, with_v ? 2 * KV_BYTES : KV_BYTES);
         if constexpr (MODE == MODE_WINDOW) {
@@ -172,11 +172,11 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
   float o0[32], o1[32];                        // O rows 0-63 / 64-127, accumulated over the key blocks of the P V pass
 #pragma unroll
   for (int i = 0; i < 32; ++i) o0[i] = o1[i] = 0.f;
-  tc::mbar_wait(&bars->q, 0);
+  tc::mbar_wait_nocall(&bars->q, 0);
   for (int it = 0; it < n_iter; ++it) {
     const int j = it % nblk;
     const int pass = (two_pass && it < nblk) ? 0 : 1;
-    tc::mbar_wait(&bars->kv, (uint32_t)it & 1u);
+    tc::mbar_wait_nocall(&bars->kv, (uint32_t)it & 1u);
     // S = Q K^T, one M = 64 half at a time -> fp32 tile
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {

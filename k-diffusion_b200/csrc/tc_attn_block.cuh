@@ -8,7 +8,8 @@
 // (x -> qkv -> attention output -> x: ~11 bytes moved per byte of x).  Here every 8x8 window is read once and written once; q, k, v and
 // the attention output never leave the SM.  Per window (64 tokens) and head h (d_head 64, two heads), all m64 wgmma:
 //
-//   V, K, Q   = X . Wqkv_h^T          64 x 64 accumulators, A = the X window in shared memory; Q's MMAs overlap the k epilogue
+//   V, K, Q   = X . Wqkv_h^T          64 x 64 accumulators, A = the X window in shared memory; issued together, the
+//                                    v and k epilogues overlap the K and Q MMAs
 //   v         : x 1/rms (the row statistics the producer of x left); bf16 -> shared memory (B operand of P V)
 //   k, q      : cosine-normalised in registers (a row's 64 columns sit in the 4 threads of a quad: two shfl_xor), x sqrt(scale_h),
 //               RoPE from the per-layer table (columns 2i, 2i+1 pair with 16+2i, 17+2i: same thread); k -> shared memory, q stays in
@@ -24,9 +25,11 @@
 // roll of the shifted layers (:274) is the quadrants' coordinates; shift 0 uses the same row order.  Rows of a window: quadrant-major,
 // then (row, column) inside the quadrant -- the seam-mask regions (:300-315) are whole quadrants.
 //
-// Roles (288 threads, one CTA per SM, tiles of two windows blockIdx.x, + gridDim.x, ...):
-//   warpgroups 0, 1   window 2 tile + wg; the second warpgroup of the last tile idles when the number of windows is odd
-//   warp 8            TMA producer: the weights once per CTA, then the X tiles (2 buffers)
+// Roles (384 threads, one CTA per SM, tiles of two windows blockIdx.x, + gridDim.x, ...):
+//   warpgroups 0, 1   window 2 tile + wg; the second warpgroup of the last tile idles when the number of windows is odd.  232 registers
+//                     each: the V, K and Q accumulators of a head are live together, and the RoPE table entries load under the MMAs
+//   warpgroup 2       producer (40 registers): one elected lane of warp 8 loads by TMA the weights once per CTA, then the X tiles
+//                     (2 buffers)
 // Shared memory: X 2 x 32 KiB, Wqkv 96 KiB, Wout 32 KiB, K and V per warpgroup 4 x 8 KiB = 224 KiB.
 #pragma once
 
@@ -36,7 +39,7 @@ constexpr int AB_X_BYTES = 2 * A_STAGE_BYTES;      // two windows x 128 channels
 constexpr int AB_WQKV_KB = 3 * AB_C * 128;         // one k-block of Wqkv: [384 rows x 64] bf16 = 48 KiB
 constexpr int AB_WO_BYTES = 2 * A_STAGE_BYTES;     // Wout [128 x 128]: k-block h = the input channels of head h
 constexpr int AB_KV_BYTES = 64 * 128;              // one [64 tokens x 64] bf16 SW128 tile
-constexpr int AB_THREADS = 256 + 32;
+constexpr int AB_THREADS = 256 + 128;
 
 struct AttnBlockBars {
   uint64_t w_full, x_full[AB_XBUF], x_empty[AB_XBUF];
@@ -96,9 +99,10 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   tc::pdl_wait();
   tc::pdl_launch_dependents();
 
-  if (pwarp == 8) {
+  if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    if (tc::elect_one()) {
+    tc::setmaxnreg_dec<40>();
+    if (pwarp == 8 && tc::elect_one()) {
       tc::mbar_arrive_expect_tx(&bars->w_full, 2 * AB_WQKV_KB + AB_WO_BYTES);
 #pragma unroll
       for (int kb = 0; kb < 2; ++kb) {
@@ -130,6 +134,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   }
 
   // ------------------------------------------------------------------ warpgroups: one window each
+  tc::setmaxnreg_inc<232>();
   const int wg = pwarp >> 2, t = threadIdx.x & 127;
   const int rw = 16 * (t >> 5) + (lane >> 2);                // this thread's two window rows: rw and rw + 8 (same quadrant)
   const int r0 = 64 * wg + rw;                               // ... as rows of the X tile
@@ -152,16 +157,10 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
       *reinterpret_cast<uint32_t*>(dst + tc::sw128_offset(rw + 8, j) + cq * 2) = tc::pack_bf16x2(a[4 * j + 2], a[4 * j + 3]);
     }
   };
-  // q, k: cosine-sim scale (:106-114) + axial RoPE (:187-199) of head hd, rows = image tokens tok0, tok1.  The RoPE table entries (the
-  // same for q and k: window attention's keys are its queries) are loaded at each use rather than kept live across the K / Q MMAs.
-  auto qk_norm_rope = [&](float (&a)[32], int hd, int tok0, int tok1) {
-    float4 cs[2][2];                           // column pair 8 jj + cq of row rw + 8 rr
-#pragma unroll
-    for (int jj = 0; jj < 2; ++jj) {
-      const float4* tb = p.rope + (int64_t)(hd * 8 + 4 * jj + (lane & 3)) * T;
-      cs[0][jj] = __ldg(tb + tok0);
-      cs[1][jj] = __ldg(tb + tok1);
-    }
+  // q, k: cosine-sim scale (:106-114) + axial RoPE (:187-199) of head hd, rows = image tokens tok0, tok1.  cs[rr][jj] = the RoPE table
+  // entry of column pair 8 jj + cq of row rw + 8 rr, the same for q and k (window attention's keys are its queries): loaded once per
+  // head, while the projections run.
+  auto qk_norm_rope = [&](float (&a)[32], int hd, const float4 (&cs)[2][2]) {
     const float sq = sqs[hd];
     float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -218,12 +217,13 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     uint32_t of[2][16];                        // O_h / l of both heads: bf16 A fragments of the out projection
 #pragma unroll 1
     for (int hd = 0; hd < 2; ++hd) {
-      // ---- V, K, Q = X . Wqkv_h^T, three commit groups
+      // ---- V, K, Q = X . Wqkv_h^T, three commit groups issued together
       float va[32], ka[32], qa[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) va[j] = ka[j] = qa[j] = 0.f;
       tc::wg_fence_acc(va);
       tc::wg_fence_acc(ka);
+      tc::wg_fence_acc(qa);
       tc::wg_fence();
       auto project = [&](float (&d)[32], int third) {      // third: 0 = q, 1 = k, 2 = v (feature order (t nh e))
 #pragma unroll
@@ -235,11 +235,18 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
         }
         tc::wg_commit();
       };
-      // (Q is issued once V is retired: three live 64 x 64 accumulators would crowd the 168 registers a thread has at 288 threads)
       project(va, 2);
       project(ka, 1);
+      project(qa, 0);
+      float4 cs[2][2];
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const float4* tb = p.rope + (int64_t)(hd * 8 + 4 * jj + (lane & 3)) * T;
+        cs[0][jj] = __ldg(tb + tok0);
+        cs[1][jj] = __ldg(tb + tok1);
+      }
       if (hd == 1) tc::named_barrier_sync(1 + wg, 128);     // head 0's S and P V MMAs (all four warps) are done with K and V
-      tc::wg_wait<1>();
+      tc::wg_wait<2>();
       tc::wg_fence_acc(va);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -249,16 +256,13 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
         va[4 * j + 3] *= rstd1;
       }
       store_tile(sV, va);
-      tc::wg_fence_acc(qa);
-      tc::wg_fence();
-      project(qa, 0);
       tc::wg_wait<1>();
       tc::wg_fence_acc(ka);
-      qk_norm_rope(ka, hd, tok0, tok1);
+      qk_norm_rope(ka, hd, cs);
       store_tile(sK, ka);
       tc::wg_wait<0>();
       tc::wg_fence_acc(qa);
-      qk_norm_rope(qa, hd, tok0, tok1);
+      qk_norm_rope(qa, hd, cs);
       uint32_t qf[16];
       to_afrag(qa, qf);
       tc::fence_proxy_async();                 // K, V (generic-proxy writes) -> visible to the tensor core

@@ -14,11 +14,19 @@
 // and the tile is stored by TMA from the X buffer itself.  AdaRMSNorm is fused as in the stand-alone GEMMs: Wup carries the channel scale
 // for this evaluation (fold kernel), 1/rms of the row comes from the statistics its producer left.
 //
-// Roles (288 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...):
+// Roles (384 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...):
 //   warpgroups 0, 1   rows [0, 64) / [64, 128) of every tile: M1, GEGLU, M2, final epilogue; both read the same weight chunks
-//   warp 8            TMA producer: X tiles (2 buffers), Wup chunks (3 x 32 KiB ring), Wdown chunks (3 x 16 KiB ring) -- the weights
-//                     stream from L2 once per tile (all CTAs walk the same chunks at about the same time)
+//   warpgroup 2       producer (40 registers, the MMA warpgroups take 232): one elected lane of warp 8 streams by TMA the X tiles
+//                     (2 buffers), Wup chunks (3 x 32 KiB ring), Wdown chunks (3 x 16 KiB ring) -- the weights stream from L2 once per
+//                     tile (all CTAs walk the same chunks at about the same time)
 // Shared memory: X 2 x 32 KiB, Wup 3 x 32 KiB, Wdown 3 x 16 KiB = 208 KiB.
+//
+// Schedule: a warpgroup issues its MMAs in blocks -- M1(0) of a tile, then after each GEGLU(c) the block M2(c), M1(c + 1) -- and the two
+// warpgroups take turns to issue (named barriers 3 and 4), so that one warpgroup's GEGLU and wait latencies run while the tensor cores
+// work through the other's block.  Issued together both would finish together, and the tensor cores would idle during every GEGLU.  A
+// warpgroup is at most one block ahead of the other, which the 3-deep weight rings cover.  Every accumulator sees the same wgmma
+// sequence as in a serial M1 -> GEGLU -> M2 order: the schedule changes no result bit.  The waits are mbar_wait_nocall: a call in the
+// kernel body would make ptxas serialise every wgmma.
 #pragma once
 
 constexpr int FF_C = 128;                  // level width this kernel is built for
@@ -27,7 +35,7 @@ constexpr int FF_XBUF = 2, FF_WU = 3, FF_WD = 3;
 constexpr int FF_X_BYTES = 2 * A_STAGE_BYTES;       // [128 x 128] bf16 = two SW128 k-block tiles
 constexpr int FF_WU_BYTES = 2 * A_STAGE_BYTES;      // [128 rows x 128 K]
 constexpr int FF_WD_BYTES = A_STAGE_BYTES;          // [128 rows x 64 K]
-constexpr int FF_THREADS = 256 + 32;
+constexpr int FF_THREADS = 256 + 128;
 
 struct FfnBars {
   uint64_t x_full[FF_XBUF], x_empty[FF_XBUF];
@@ -80,19 +88,20 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
   tc::pdl_wait();                    // x (and its row statistics) come from the kernel before us
   tc::pdl_launch_dependents();
 
-  if (pwarp == 8) {
+  if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    if (tc::elect_one()) {
+    tc::setmaxnreg_dec<40>();
+    if (pwarp == 8 && tc::elect_one()) {
       uint32_t su = 0, pu = 0, sd = 0, pd = 0;        // ring slot / phase of the next Wup / Wdown chunk
       for (int i = 0; i < n_local; ++i) {
         const int buf = i & 1;
-        tc::mbar_wait(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
+        tc::mbar_wait_nocall(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
         tc::mbar_arrive_expect_tx(&bars->x_full[buf], FF_X_BYTES);
         const int m0 = ((int)blockIdx.x + i * (int)gridDim.x) * BM;
         tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES, &tmx, &bars->x_full[buf], 0, m0);
         tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES + A_STAGE_BYTES, &tmx, &bars->x_full[buf], BK, m0);
         for (int c = 0; c < nc; ++c) {
-          tc::mbar_wait(&bars->wu_empty[su], pu ^ 1u);
+          tc::mbar_wait_nocall(&bars->wu_empty[su], pu ^ 1u);
           tc::mbar_arrive_expect_tx(&bars->wu_full[su], FF_WU_BYTES);
           tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES, &tmwu, &bars->wu_full[su], 0, c * 128);
           tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES + A_STAGE_BYTES, &tmwu, &bars->wu_full[su], BK, c * 128);
@@ -100,7 +109,7 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
             su = 0;
             pu ^= 1u;
           }
-          tc::mbar_wait(&bars->wd_empty[sd], pd ^ 1u);
+          tc::mbar_wait_nocall(&bars->wd_empty[sd], pd ^ 1u);
           tc::mbar_arrive_expect_tx(&bars->wd_full[sd], FF_WD_BYTES);
           tc::tma_load_2d(sWD + (size_t)sd * FF_WD_BYTES, &tmwd, &bars->wd_full[sd], c * FF_CH, 0);
           if (++sd == FF_WD) {
@@ -114,11 +123,17 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
   }
 
   // ------------------------------------------------------------------ warpgroups: rows [64 wg, 64 wg + 64) of every tile
+  tc::setmaxnreg_inc<232>();
   const int wg = pwarp >> 2, t = threadIdx.x & 127;
   const int r0 = 64 * wg + 16 * (t >> 5) + (lane >> 2);      // this thread's two accumulator rows: r0 and r0 + 8
   const int cq = 2 * (lane & 3);                             // and its column pair inside every 8-column block
   const uint32_t wu_base = tc::smem_u32(sWU), wd_base = tc::smem_u32(sWD);
   uint32_t su = 0, pu = 0, sd = 0, pd = 0;
+  // Issue turns: warpgroup 0 issues block k after warpgroup 1 has issued block k - 1 (barrier 3), warpgroup 1 issues block k after
+  // warpgroup 0 has issued block k (barrier 4).  Both issue nc + 1 blocks per tile; the arrivals match the syncs one for one.
+  bool first_block = true;
+  float acc1[64], acc2[64];
+  uint32_t hreg[16];
   for (int i = 0; i < n_local; ++i) {
     const int buf = i & 1;
     const int64_t m0 = ((int64_t)blockIdx.x + (int64_t)i * gridDim.x) * BM;
@@ -126,66 +141,89 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
     const float rstd1 = rsqrtf(__ldg(p.ss_in + (m0 + r0 + 8) * SS_PARTS) / (float)FF_C + 1e-6f);
     // the GELU's 0.5 rides on the value's row scale
     const tc::f32x2 g0 = tc::pk2(rstd0, rstd0), g1 = tc::pk2(rstd1, rstd1), h0 = tc::pk2(0.5f * rstd0, 0.5f * rstd0), h1 = tc::pk2(0.5f * rstd1, 0.5f * rstd1);
-    tc::mbar_wait(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
+    tc::mbar_wait_nocall(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
     const uint32_t xa = tc::smem_u32(sX + (size_t)buf * FF_X_BYTES) + (uint32_t)wg * 8192u;   // rows 64 wg.. of both k-block tiles
-    float acc2[64];
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc2[j] = 0.f;
-    for (int c = 0; c < nc; ++c) {
-      // ---- M1: acc1 = X . Wup_c^T
-      float acc1[64];
+    // block c: M2(c - 1) for c > 0, M1(c) for c < nc.  One program point per wgmma: accumulators carried into the loop from a second
+    // issue site would take register moves inside the in-flight stage, and ptxas would serialise the wgmmas.
+    for (int c = 0; c <= nc; ++c) {
+      if (c > 0) {
+        // M1(c - 1) and, from c = 2 on, M2(c - 2) were this warpgroup's last block
+        tc::wg_wait<0>();
+        tc::wg_fence_acc(acc1);
+        tc::wg_fence_acc(acc2);
+        tc::wg_fence_acc(hreg);
+        if (lane == 0) tc::mbar_arrive(&bars->wu_empty[su]);
+        if (++su == FF_WU) {
+          su = 0;
+          pu ^= 1u;
+        }
+        if (c > 1) {
+          if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
+          if (++sd == FF_WD) {
+            sd = 0;
+            pd ^= 1u;
+          }
+        }
+        // ---- GEGLU(c - 1): 8-column block 2q = 8 value features, block 2q + 1 = their gates -> hidden block q (rows r0, r0 + 8)
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const tc::f32x2 v0 = tc::mul2(tc::pk2(acc1[8 * q], acc1[8 * q + 1]), h0), v1 = tc::mul2(tc::pk2(acc1[8 * q + 2], acc1[8 * q + 3]), h1);
+          const tc::f32x2 q0 = tc::mul2(tc::pk2(acc1[8 * q + 4], acc1[8 * q + 5]), g0), q1 = tc::mul2(tc::pk2(acc1[8 * q + 6], acc1[8 * q + 7]), g1);
+          float o0, o1, o2, o3;
+          tc::upk2(tc::geglu2(v0, q0), o0, o1);
+          tc::upk2(tc::geglu2(v1, q1), o2, o3);
+          // A fragment of k16 step q / 2: {block 2kk row r0, block 2kk row r0 + 8, block 2kk + 1 row r0, block 2kk + 1 row r0 + 8}
+          hreg[(q >> 1) * 4 + (q & 1) * 2 + 0] = tc::pack_bf16x2(o0, o1);
+          hreg[(q >> 1) * 4 + (q & 1) * 2 + 1] = tc::pack_bf16x2(o2, o3);
+        }
+      }
 #pragma unroll
       for (int j = 0; j < 64; ++j) acc1[j] = 0.f;
-      tc::mbar_wait(&bars->wu_full[su], pu);
-      const uint32_t wa = wu_base + su * (uint32_t)FF_WU_BYTES;
-      tc::wg_fence_acc(acc1);
-      tc::wg_fence();
+      tc::wg_fence_acc(acc1);          // the zeros are written before this turn's first wgmma
+      // ---- this warpgroup's turn to issue
+      if (wg == 1) tc::named_barrier_sync(4, 256);
+      else if (!first_block) tc::named_barrier_sync(3, 256);
+      first_block = false;
+      if (c > 0) {
+        // ---- M2(c - 1): acc2 += H . Wdown^T
+        tc::mbar_wait_nocall(&bars->wd_full[sd], pd);
+        const uint64_t bd = tc::smem_desc_k_sw128(wd_base + sd * (uint32_t)FF_WD_BYTES);
+        tc::wg_fence_acc(acc2);
+        tc::wg_fence_acc(hreg);
+        tc::wg_fence();
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb) {
-        const uint64_t ad = tc::smem_desc_k_sw128(xa + (uint32_t)(kb * A_STAGE_BYTES)), bd = tc::smem_desc_k_sw128(wa + (uint32_t)(kb * A_STAGE_BYTES));
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint32_t a[4] = {hreg[4 * kk], hreg[4 * kk + 1], hreg[4 * kk + 2], hreg[4 * kk + 3]};
+          tc::wgmma_128_rs(acc2, a, bd + 2ull * kk, 1u);
+        }
+        tc::wg_commit();
+      }
+      if (c < nc) {
+        // ---- M1(c): acc1 = X . Wup^T
+        tc::mbar_wait_nocall(&bars->wu_full[su], pu);
+        const uint32_t wa = wu_base + su * (uint32_t)FF_WU_BYTES;
+        tc::wg_fence_acc(acc1);
+        tc::wg_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc::wgmma_128(acc1, ad + 2ull * k, bd + 2ull * k, 1u);
-      }
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(acc1);
-      if (lane == 0) tc::mbar_arrive(&bars->wu_empty[su]);
-      if (++su == FF_WU) {
-        su = 0;
-        pu ^= 1u;
-      }
-      // ---- GEGLU: 8-column block 2q = 8 value features, block 2q + 1 = their gates -> hidden block q (rows r0, r0 + 8)
-      uint32_t hreg[16];
+        for (int kb = 0; kb < 2; ++kb) {
+          const uint64_t ad = tc::smem_desc_k_sw128(xa + (uint32_t)(kb * A_STAGE_BYTES)), bd = tc::smem_desc_k_sw128(wa + (uint32_t)(kb * A_STAGE_BYTES));
 #pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const tc::f32x2 v0 = tc::mul2(tc::pk2(acc1[8 * q], acc1[8 * q + 1]), h0), v1 = tc::mul2(tc::pk2(acc1[8 * q + 2], acc1[8 * q + 3]), h1);
-        const tc::f32x2 q0 = tc::mul2(tc::pk2(acc1[8 * q + 4], acc1[8 * q + 5]), g0), q1 = tc::mul2(tc::pk2(acc1[8 * q + 6], acc1[8 * q + 7]), g1);
-        float o0, o1, o2, o3;
-        tc::upk2(tc::geglu2(v0, q0), o0, o1);
-        tc::upk2(tc::geglu2(v1, q1), o2, o3);
-        // A fragment of k16 step q / 2: {block 2kk row r0, block 2kk row r0 + 8, block 2kk + 1 row r0, block 2kk + 1 row r0 + 8}
-        hreg[(q >> 1) * 4 + (q & 1) * 2 + 0] = tc::pack_bf16x2(o0, o1);
-        hreg[(q >> 1) * 4 + (q & 1) * 2 + 1] = tc::pack_bf16x2(o2, o3);
+          for (int k = 0; k < 4; ++k) tc::wgmma_128(acc1, ad + 2ull * k, bd + 2ull * k, 1u);
+        }
+        tc::wg_commit();
       }
-      // ---- M2: acc2 += H_c . Wdown_c^T
-      tc::mbar_wait(&bars->wd_full[sd], pd);
-      const uint64_t bd = tc::smem_desc_k_sw128(wd_base + sd * (uint32_t)FF_WD_BYTES);
-      tc::wg_fence_acc(acc2);
-      tc::wg_fence_acc(hreg);
-      tc::wg_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t a[4] = {hreg[4 * kk], hreg[4 * kk + 1], hreg[4 * kk + 2], hreg[4 * kk + 3]};
-        tc::wgmma_128_rs(acc2, a, bd + 2ull * kk, 1u);
-      }
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(acc2);
-      if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
-      if (++sd == FF_WD) {
-        sd = 0;
-        pd ^= 1u;
-      }
+      if (wg == 0) tc::named_barrier_arrive(4, 256);
+      else if (c < nc || i + 1 < n_local) tc::named_barrier_arrive(3, 256);
+    }
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(acc2);
+    tc::wg_fence_acc(hreg);
+    if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
+    if (++sd == FF_WD) {
+      sd = 0;
+      pd ^= 1u;
     }
     // ---- final epilogue: out = acc2 + x (residual from the X tile in shared memory), in place, then TMA store of this half
     uint8_t* xt = sX + (size_t)buf * FF_X_BYTES;
