@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 11
+#define KDB_ABI_VERSION 12
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -232,6 +232,67 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
  * <0 = capacity too small).  The tap disarms itself after one forward. */
 int     kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity);
 int64_t kdb_model_tap_count(const KdbModel* m);
+
+/* ------------------------------------------------------------------------------------------
+ * image_v1 U-Net denoiser engine, exact fp32 path (models/image_v1.py, layers.py:116-313, augmentation.py:92-104)
+ * ------------------------------------------------------------------------------------------
+ * A separate handle with the same life cycle as KdbModel: create, bind every state-dict entry, finalize, then fill a
+ * conditioning table once per sampler call and run forwards.  Activations are token-major [B, H, W, C] fp32 inside the
+ * workspace.  Every entry point returns a negative KDB_ERR_* for a NULL handle before any CUDA call. */
+
+typedef struct KdbUNetConfig {
+  int32_t n_levels;                       /* len(depths)                                               (image_v1.py:107-115) */
+  int32_t in_channels;                    /* input_channels = c_in                                                           */
+  int32_t patch_size;                     /* pixel_unshuffle / pixel_shuffle factor                    (:146-154)            */
+  int32_t mapping_out;                    /* feats_in of the mapping net and every AdaGN mapper        (:97-100)             */
+  int32_t mapping_cond_dim;               /* in-features of the mapping_cond Linear, 0 = none; 9 more with the augment wrapper */
+  int32_t augment_wrapper;                /* 1: KarrasAugmentWrapper, mapping_cond = cat(aug_cond or zeros(9), mapping_cond)  */
+  int32_t skip_stages;
+  int32_t has_variance;                   /* proj_out has one extra (dropped) output channel           (:151-152)            */
+  int32_t depth[KDB_MAX_LEVELS];          /* ResConvBlocks per DBlock / UBlock                                               */
+  int32_t channels[KDB_MAX_LEVELS];       /* multiples of 4                                                                  */
+  int32_t self_attn[KDB_MAX_LEVELS];      /* self_attn_depths                                                                */
+} KdbUNetConfig;
+
+typedef struct KdbUNet KdbUNet;
+
+int kdb_unet_create(const KdbUNetConfig* cfg, KdbUNet** out);
+int kdb_unet_destroy(KdbUNet* m);
+
+/* Bind one state-dict entry of ImageDenoiserModelV1 (fp32, contiguous, device) by its reference key name, e.g.
+ * "u_net.d_blocks.1.2.main.2.weight"; a KarrasAugmentWrapper's "inner_model." prefix is not part of the name.  Borrowed until
+ * the next finalize or destroy. */
+int kdb_unet_set_tensor(KdbUNet* m, const char* key, const float* data, const int64_t* shape, int ndim);
+
+/* Validate every required key and build the derived tables: tap-major convolution weights, qkv_proj with 1/sqrt(d_head) folded
+ * into its q rows and bias, the concatenated AdaGN mappers.  Synchronises `stream`. */
+int kdb_unet_finalize(KdbUNet* m, void* stream);
+
+/* Floats per conditioning row: the (weight, bias) pair of every AdaGN in execution order, then the mapping net's output. */
+int64_t kdb_unet_cond_stride(const KdbUNet* m);
+
+/* Fourier features of log(sigma)/4, the mapping_cond Linear, the mapping net and every AdaGN mapper for `rows` tuples
+ * (image_v1.py:136-139, layers.py:173).  aug_cond [rows, 9] (augment wrapper only; NULL = zeros) and mapping_cond
+ * [rows, mapping_cond_dim minus the wrapper's 9] may be NULL where the reference allows None. */
+int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, float* cond_out,
+                          void* stream);
+
+/* Workspace of one forward in bytes; KDB_ERR_UNSUPPORTED for a precision other than KDB_PREC_FP32. */
+int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int height, int width);
+
+/* One evaluation on x [B, in_channels, H, W] -> out of the same shape, as kdb_model_forward: sigma_data > 0 gives the
+ * Karras-preconditioned denoiser, sigma_data <= 0 the raw inner model; cond rows with cond_batch_stride (0 = one shared row).
+ * KDB_PREC_FP32 only (any other precision: KDB_ERR_UNSUPPORTED).  Every level but the innermost needs an even grid and every
+ * level at least 2x2.  Allocates nothing and synchronises nothing, so it can be captured into a CUDA graph; a workspace shorter
+ * than kdb_unet_workspace_bytes returns KDB_ERR_WORKSPACE.  Deterministic (no atomics). */
+int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                     const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Debug/parity tap of the NEXT forward, token-major [B, h, w, C] fp32: "patch_in", "d<l>.down", "d<l>.<i>", "u<l>.<i>",
+ * "u<l>.up" -- level l, i the module index inside the reference's DBlock (1..) / UBlock (0..), i.e. the output of that
+ * ResConvBlock or SelfAttention2d.  kdb_unet_tap_count: floats written (0 = not hit, < 0 = capacity too small). */
+int     kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity);
+int64_t kdb_unet_tap_count(const KdbUNet* m);
 
 /* ------------------------------------------------------------------------------------------
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)

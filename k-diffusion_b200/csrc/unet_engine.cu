@@ -1,0 +1,491 @@
+// unet_engine.cu -- host-side execution plan of the image_v1 U-Net denoiser on the exact fp32 path
+// (reference: k_diffusion/models/image_v1.py, layers.py:116-313, augmentation.py:92-104).
+//
+// Like the transformer engine, it owns no activations: the caller passes one workspace and the forward carves it.  Weights are
+// borrowed device pointers keyed by the state-dict names of ImageDenoiserModelV1; kdb_unet_finalize builds the derived tables
+// (tap-major convolution weights, the attention scale folded into qkv_proj's q rows, the concatenated AdaGN mappers).
+#include <algorithm>
+#include <cmath>
+#include <string>
+#include <unordered_map>
+#include <vector>
+
+#include "model_kernels.cuh"
+#include "unet_kernels.cuh"
+
+namespace {
+
+enum ModKind { M_RES = 0, M_ATTN, M_DOWN, M_UP, M_CONCAT };
+
+// One module of the U-Net in execution order.  M_CONCAT starts a UBlock that receives the matching skip.
+struct UMod {
+  int kind = M_RES, level = 0;
+  std::string tap;
+  int c_in = 0, c_mid = 0, c_out = 0;
+  int groups1 = 1, groups2 = 1, ada1 = 0, ada2 = 0;
+  const float *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr, *skip_w = nullptr;   // derived (owned) weights
+  const float *mapper1_w = nullptr, *mapper1_b = nullptr, *mapper2_w = nullptr, *mapper2_b = nullptr;
+  bool to_skip = false;           // the last module of a DBlock writes the level's skip buffer
+};
+
+struct TensorRefU {
+  const float* p = nullptr;
+  std::vector<int64_t> shape;
+};
+
+}  // namespace
+
+struct KdbUNet {
+  KdbUNetConfig cfg{};
+  std::unordered_map<std::string, TensorRefU> tensors;
+  bool finalized = false;
+  std::vector<UMod> mods;
+  std::vector<void*> owned;
+  const float *proj_in_w = nullptr, *proj_in_b = nullptr, *proj_out_w = nullptr, *proj_out_b = nullptr;
+  int ada_total = 0;
+  kdb::UNetCondWeights cw{};
+  std::string tap_name;
+  float* tap_out = nullptr;
+  int64_t tap_cap = 0, tap_count = 0;
+};
+
+using namespace kdb;
+
+namespace {
+
+int uget(KdbUNet* m, const std::string& key, std::vector<int64_t> want, const float** out) {
+  auto it = m->tensors.find(key);
+  if (it == m->tensors.end()) {
+    set_error("missing state-dict entry '%s'", key.c_str());
+    return KDB_ERR_MISSING_KEY;
+  }
+  if (it->second.shape != want) {
+    std::string got, exp;
+    for (auto v : it->second.shape) got += std::to_string(v) + ",";
+    for (auto v : want) exp += std::to_string(v) + ",";
+    set_error("shape mismatch for '%s': got [%s] expected [%s]", key.c_str(), got.c_str(), exp.c_str());
+    return KDB_ERR_BAD_SHAPE;
+  }
+  *out = it->second.p;
+  return 0;
+}
+
+#define UGET(key, out, ...)                                      \
+  do {                                                           \
+    int rc__ = uget(m, (key), {__VA_ARGS__}, (out));             \
+    if (rc__) return rc__;                                       \
+  } while (0)
+
+int ualloc(KdbUNet* m, float** p, size_t count) {
+  void* q = nullptr;
+  KDB_CUDA(cudaMalloc(&q, count * sizeof(float) + 256));
+  m->owned.push_back(q);
+  *p = reinterpret_cast<float*>(q);
+  return 0;
+}
+
+void ufree(KdbUNet* m) {
+  for (void* p : m->owned) cudaFree(p);
+  m->owned.clear();
+}
+
+// owned tap-major copy of a conv weight [N, C, ks, ks]; the first scaled_rows output rows times scale
+int conv_weight(KdbUNet* m, const std::string& key, int N, int C, int ks, const float** out, cudaStream_t st, int scaled_rows = 0,
+                float scale = 1.f) {
+  const float* src;
+  UGET(key, &src, N, C, ks, ks);
+  float* dst = nullptr;
+  int rc = ualloc(m, &dst, (size_t)N * C * ks * ks);
+  if (rc || (rc = launch_unet_reorder_conv_weight(src, dst, N, C, ks, scaled_rows, scale, st))) return rc;
+  *out = dst;
+  return 0;
+}
+
+int bias_copy(KdbUNet* m, const std::string& key, int N, const float** out, cudaStream_t st, int scaled_rows = 0, float scale = 1.f) {
+  const float* src;
+  UGET(key, &src, N);
+  float* dst = nullptr;
+  int rc = ualloc(m, &dst, (size_t)N);
+  if (rc || (rc = launch_unet_reorder_conv_weight(src, dst, N, 1, 1, scaled_rows, scale, st))) return rc;
+  *out = dst;
+  return 0;
+}
+
+// AdaGN mapper of `prefix` (Linear feats_in -> 2C with bias): bound and given the next offset of the conditioning row
+int mapper(KdbUNet* m, const std::string& prefix, int C, const float** w, const float** b, int* off) {
+  const int mw = m->cfg.mapping_out;
+  UGET(prefix + "mapper.weight", w, 2 * C, mw);
+  UGET(prefix + "mapper.bias", b, 2 * C);
+  *off = m->ada_total;
+  m->ada_total += 2 * C;
+  return 0;
+}
+
+int plan_res(KdbUNet* m, const std::string& p, UMod& u, cudaStream_t st) {
+  int rc;
+  if ((rc = mapper(m, p + "main.0.", u.c_in, &u.mapper1_w, &u.mapper1_b, &u.ada1))) return rc;
+  if ((rc = conv_weight(m, p + "main.2.weight", u.c_mid, u.c_in, 3, &u.w1, st))) return rc;
+  if ((rc = bias_copy(m, p + "main.2.bias", u.c_mid, &u.b1, st))) return rc;
+  if ((rc = mapper(m, p + "main.4.", u.c_mid, &u.mapper2_w, &u.mapper2_b, &u.ada2))) return rc;
+  if ((rc = conv_weight(m, p + "main.6.weight", u.c_out, u.c_mid, 3, &u.w2, st))) return rc;
+  if ((rc = bias_copy(m, p + "main.6.bias", u.c_out, &u.b2, st))) return rc;
+  if (u.c_in != u.c_out && (rc = conv_weight(m, p + "skip.weight", u.c_out, u.c_in, 1, &u.skip_w, st))) return rc;
+  u.groups1 = std::max(1, u.c_in / 32);
+  u.groups2 = std::max(1, u.c_mid / 32);
+  return 0;
+}
+
+// SelfAttention2d: softmax's 1/sqrt(d_head) is folded into the q rows of qkv_proj (weight and bias)
+int plan_attn(KdbUNet* m, const std::string& p, UMod& u, cudaStream_t st) {
+  int rc;
+  const int C = u.c_out, nh = std::max(1, C / 64);
+  const float scale = 1.f / std::sqrt((float)(C / nh));
+  if ((rc = mapper(m, p + "norm_in.", C, &u.mapper1_w, &u.mapper1_b, &u.ada1))) return rc;
+  if ((rc = conv_weight(m, p + "qkv_proj.weight", 3 * C, C, 1, &u.w1, st, C, scale))) return rc;
+  if ((rc = bias_copy(m, p + "qkv_proj.bias", 3 * C, &u.b1, st, C, scale))) return rc;
+  if ((rc = conv_weight(m, p + "out_proj.weight", C, C, 1, &u.w2, st))) return rc;
+  if ((rc = bias_copy(m, p + "out_proj.bias", C, &u.b2, st))) return rc;
+  u.groups1 = std::max(1, C / 32);
+  return 0;
+}
+
+// DBlock / UBlock modules (image_v1.py:33-68): ResConvBlock [+ SelfAttention2d] per layer
+int plan_block(KdbUNet* m, const std::string& p, int level, const char* tag, int depth, int c_in, int c_mid, int c_out, bool attn, int first,
+               cudaStream_t st) {
+  int idx = first, rc;
+  for (int i = 0; i < depth; ++i) {
+    UMod r;
+    r.kind = M_RES;
+    r.level = level;
+    r.c_in = i == 0 ? c_in : c_mid;
+    r.c_mid = c_mid;
+    r.c_out = i < depth - 1 ? c_mid : c_out;
+    r.tap = std::string(tag) + std::to_string(level) + "." + std::to_string(idx);
+    if ((rc = plan_res(m, p + std::to_string(idx) + ".", r, st))) return rc;
+    m->mods.push_back(r);
+    ++idx;
+    if (attn) {
+      UMod a;
+      a.kind = M_ATTN;
+      a.level = level;
+      a.c_in = a.c_mid = a.c_out = r.c_out;
+      a.tap = std::string(tag) + std::to_string(level) + "." + std::to_string(idx);
+      if ((rc = plan_attn(m, p + std::to_string(idx) + ".", a, st))) return rc;
+      m->mods.push_back(a);
+      ++idx;
+    }
+  }
+  return 0;
+}
+
+int tap(KdbUNet* m, const std::string& name, const float* p, int64_t n, cudaStream_t st) {
+  if (m->tap_out == nullptr || m->tap_name != name) return 0;
+  if (n > m->tap_cap) {
+    m->tap_count = -n;
+    return 0;
+  }
+  m->tap_count = n;
+  KDB_CUDA(cudaMemcpyAsync(m->tap_out, p, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+// Workspace: the skip buffer of every level, then seven working buffers of `elems` floats each (two for the block stream, the
+// AdaGN output, the first conv's output, the skip conv's output, qkv and the attention output).
+struct UWs {
+  float* skip[KDB_MAX_LEVELS] = {};
+  float *x[2] = {}, *n1 = nullptr, *n2 = nullptr, *s = nullptr, *qkv = nullptr, *ao = nullptr;
+  size_t total = 0;
+};
+
+void level_dims(const KdbUNetConfig& c, int H, int W, int l, int* h, int* w) {
+  *h = H / c.patch_size;
+  *w = W / c.patch_size;
+  for (int i = c.skip_stages; i < l; ++i) {
+    *h /= 2;
+    *w /= 2;
+  }
+}
+
+void ucarve(const KdbUNetConfig& c, int B, int H, int W, char* base, UWs& ws) {
+  size_t off = 0;
+  auto take = [&](size_t floats) {
+    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+    off += align_up(floats * sizeof(float), 256);
+    return p;
+  };
+  size_t elems = 0;
+  for (int l = c.skip_stages; l < c.n_levels; ++l) {
+    int h, w;
+    level_dims(c, H, W, l, &h, &w);
+    const size_t px = (size_t)B * h * w;
+    ws.skip[l] = take(px * c.channels[l]);
+    const size_t wide = std::max({3 * c.channels[l], 2 * c.channels[l], c.channels[std::max(0, l - 1)]});
+    elems = std::max(elems, px * wide);
+  }
+  ws.x[0] = take(elems);
+  ws.x[1] = take(elems);
+  ws.n1 = take(elems);
+  ws.n2 = take(elems);
+  ws.s = take(elems);
+  ws.qkv = take(elems);
+  ws.ao = take(elems);
+  ws.total = off + 256;
+}
+
+// the block input: one tensor, or a tensor and the matching skip (the UBlock concat)
+struct Src {
+  const float* p1 = nullptr;
+  int c1 = 0;
+  const float* p2 = nullptr;
+  int c2 = 0;
+};
+
+int run_res(KdbUNet* m, const UMod& u, const Src& in, float* out, UWs& ws, int B, int h, int w, const float* cond, int64_t cbs, cudaStream_t st) {
+  int rc;
+  if ((rc = launch_unet_adagn(in.p1, in.c1, in.p2, in.c2, ws.n1, cond, cbs, u.ada1, u.groups1, true, B, h * w, st))) return rc;
+  ConvArgs a;
+  a.B = B, a.H = h, a.W = w;
+  a.in1 = ws.n1, a.c1 = u.c_in, a.w = u.w1, a.bias = u.b1, a.out = ws.n2, a.N = u.c_mid;
+  if ((rc = launch_unet_conv(a, 3, st))) return rc;
+  if ((rc = launch_unet_adagn(ws.n2, u.c_mid, nullptr, 0, ws.n1, cond, cbs, u.ada2, u.groups2, true, B, h * w, st))) return rc;
+  ConvArgs c2;
+  c2.B = B, c2.H = h, c2.W = w;
+  if (u.skip_w != nullptr) {
+    ConvArgs s;
+    s.B = B, s.H = h, s.W = w;
+    s.in1 = in.p1, s.c1 = in.c1, s.in2 = in.p2, s.c2 = in.c2, s.w = u.skip_w, s.out = ws.s, s.N = u.c_out;
+    if ((rc = launch_unet_conv(s, 1, st))) return rc;
+    c2.r1 = ws.s, c2.rc1 = u.c_out;
+  } else {
+    c2.r1 = in.p1, c2.rc1 = in.c1, c2.r2 = in.p2;
+  }
+  c2.in1 = ws.n1, c2.c1 = u.c_mid, c2.w = u.w2, c2.bias = u.b2, c2.out = out, c2.N = u.c_out;
+  return launch_unet_conv(c2, 3, st);
+}
+
+int run_attn(KdbUNet* m, const UMod& u, const float* x, float* out, UWs& ws, int B, int h, int w, const float* cond, int64_t cbs, cudaStream_t st) {
+  int rc;
+  const int C = u.c_out, nh = std::max(1, C / 64);
+  if ((rc = launch_unet_adagn(x, C, nullptr, 0, ws.n1, cond, cbs, u.ada1, u.groups1, false, B, h * w, st))) return rc;
+  ConvArgs q;
+  q.B = B, q.H = h, q.W = w;
+  q.in1 = ws.n1, q.c1 = C, q.w = u.w1, q.bias = u.b1, q.out = ws.qkv, q.N = 3 * C;
+  if ((rc = launch_unet_conv(q, 1, st))) return rc;
+  if ((rc = launch_attention_generic<float>(ws.qkv, ws.ao, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st))) return rc;
+  ConvArgs o;
+  o.B = B, o.H = h, o.W = w;
+  o.in1 = ws.ao, o.c1 = C, o.w = u.w2, o.bias = u.b2, o.r1 = x, o.rc1 = C, o.out = out, o.N = C;
+  return launch_unet_conv(o, 1, st);
+}
+
+int unet_forward(KdbUNet* m, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cbs, float* out,
+                 UWs& ws, cudaStream_t st) {
+  const KdbUNetConfig& c = m->cfg;
+  const int s0 = c.skip_stages, C0 = c.channels[std::max(0, s0 - 1)];
+  int h, w, rc;
+  level_dims(c, H, W, s0, &h, &w);
+  if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, ws.x[0], B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
+  if ((rc = tap(m, "patch_in", ws.x[0], (int64_t)B * h * w * C0, st))) return rc;
+  Src cur{ws.x[0], C0, nullptr, 0};
+  int cur_buf = 0;                         // index of the ping-pong buffer holding cur (-1: a skip buffer)
+  for (const UMod& u : m->mods) {
+    const int nb = cur_buf == 0 ? 1 : 0;
+    float* dst = u.to_skip ? ws.skip[u.level] : ws.x[nb];
+    int C = u.c_out;
+    switch (u.kind) {
+      case M_DOWN:
+        if ((rc = launch_unet_resample(cur.p1, dst, B, h, w, cur.c1, false, st))) return rc;
+        h /= 2, w /= 2, C = cur.c1;
+        break;
+      case M_UP:
+        if ((rc = launch_unet_resample(cur.p1, dst, B, h, w, cur.c1, true, st))) return rc;
+        h *= 2, w *= 2, C = cur.c1;
+        break;
+      case M_CONCAT:
+        cur.p2 = ws.skip[u.level], cur.c2 = c.channels[u.level];
+        continue;
+      case M_RES:
+        if ((rc = run_res(m, u, cur, dst, ws, B, h, w, cond, cbs, st))) return rc;
+        break;
+      default:
+        if ((rc = run_attn(m, u, cur.p1, dst, ws, B, h, w, cond, cbs, st))) return rc;
+    }
+    if ((rc = tap(m, u.tap, dst, (int64_t)B * h * w * C, st))) return rc;
+    cur = Src{dst, C, nullptr, 0};
+    cur_buf = u.to_skip ? -1 : nb;
+  }
+  return launch_unet_patch_out(cur.p1, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, cur.c1, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+int kdb_unet_create(const KdbUNetConfig* cfg, KdbUNet** out) {
+  KDB_REQUIRE(cfg && out, KDB_ERR_BAD_ARG, "unet_create: NULL argument");
+  KDB_REQUIRE(cfg->n_levels >= 1 && cfg->n_levels <= KDB_MAX_LEVELS, KDB_ERR_BAD_ARG, "unet_create: n_levels %d", cfg->n_levels);
+  KDB_REQUIRE(cfg->in_channels >= 1 && cfg->patch_size >= 1 && cfg->mapping_out >= 2 && cfg->mapping_out % 2 == 0, KDB_ERR_BAD_ARG,
+              "unet_create: bad channels / patch size / mapping_out");
+  KDB_REQUIRE(cfg->skip_stages >= 0 && cfg->skip_stages < cfg->n_levels, KDB_ERR_BAD_ARG, "unet_create: skip_stages %d", cfg->skip_stages);
+  KDB_REQUIRE(cfg->mapping_cond_dim >= (cfg->augment_wrapper ? 9 : 0), KDB_ERR_BAD_ARG,
+              "unet_create: the augment wrapper needs mapping_cond_dim >= 9");
+  for (int l = 0; l < cfg->n_levels; ++l)
+    KDB_REQUIRE(cfg->depth[l] >= 1 && cfg->channels[l] >= 4 && cfg->channels[l] % 4 == 0, KDB_ERR_UNSUPPORTED,
+                "unet_create: level %d needs depth >= 1 and a channel count that is a multiple of 4", l);
+  KdbUNet* m = new KdbUNet();
+  m->cfg = *cfg;
+  *out = m;
+  return 0;
+}
+
+int kdb_unet_destroy(KdbUNet* m) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_destroy: NULL handle");
+  ufree(m);
+  delete m;
+  return 0;
+}
+
+int kdb_unet_set_tensor(KdbUNet* m, const char* key, const float* data, const int64_t* shape, int ndim) {
+  KDB_REQUIRE(m && key && data && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "unet_set_tensor: bad argument");
+  TensorRefU t;
+  t.p = data;
+  t.shape.assign(shape, shape + ndim);
+  m->tensors[key] = t;
+  m->finalized = false;
+  return 0;
+}
+
+int kdb_unet_finalize(KdbUNet* m, void* stream) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_finalize: NULL handle");
+  cudaStream_t st = (cudaStream_t)stream;
+  ufree(m);
+  m->finalized = false;
+  m->mods.clear();
+  m->ada_total = 0;
+  const KdbUNetConfig& c = m->cfg;
+  const int n = c.n_levels, s0 = c.skip_stages, mw = c.mapping_out, C0 = c.channels[std::max(0, s0 - 1)];
+  int rc;
+  for (int l = s0; l < n; ++l) {          // DBlocks (image_v1.py:108-110); module 0 downsamples when l > skip_stages
+    if (l > s0) {
+      UMod d;
+      d.kind = M_DOWN, d.level = l, d.tap = "d" + std::to_string(l) + ".down";
+      m->mods.push_back(d);
+    }
+    if ((rc = plan_block(m, "u_net.d_blocks." + std::to_string(l) + ".", l, "d", c.depth[l], c.channels[std::max(0, l - 1)], c.channels[l],
+                         c.channels[l], c.self_attn[l] != 0, 1, st)))
+      return rc;
+    m->mods.back().to_skip = true;
+  }
+  for (int l = n - 1; l >= s0; --l) {     // UBlocks innermost first (layers.py:310-311); u_net.u_blocks.k holds level n-1-k
+    if (l < n - 1) {
+      UMod cc;
+      cc.kind = M_CONCAT, cc.level = l;
+      m->mods.push_back(cc);
+    }
+    const int c_in = l < n - 1 ? 2 * c.channels[l] : c.channels[l];
+    if ((rc = plan_block(m, "u_net.u_blocks." + std::to_string(n - 1 - l) + ".", l, "u", c.depth[l], c_in, c.channels[l],
+                         c.channels[std::max(0, l - 1)], c.self_attn[l] != 0, 0, st)))
+      return rc;
+    if (l > s0) {
+      UMod up;
+      up.kind = M_UP, up.level = l, up.tap = "u" + std::to_string(l) + ".up";
+      m->mods.push_back(up);
+    }
+  }
+  const int Kin = c.in_channels * c.patch_size * c.patch_size, Kout = Kin + (c.has_variance ? 1 : 0);
+  UGET("proj_in.weight", &m->proj_in_w, C0, Kin, 1, 1);
+  UGET("proj_in.bias", &m->proj_in_b, C0);
+  UGET("proj_out.weight", &m->proj_out_w, Kout, C0, 1, 1);
+  UGET("proj_out.bias", &m->proj_out_b, Kout);
+  // conditioning weights and the concatenated AdaGN mappers
+  UNetCondWeights& w = m->cw;
+  w = UNetCondWeights{};
+  w.mw = mw, w.mcond_dim = c.mapping_cond_dim, w.augment = c.augment_wrapper, w.ada_total = m->ada_total;
+  UGET("timestep_embed.weight", &w.time_emb, mw / 2, 1);
+  if (c.mapping_cond_dim > 0) UGET("mapping_cond.weight", &w.mcond_w, mw, c.mapping_cond_dim);
+  UGET("mapping.0.weight", &w.map_w0, mw, mw);
+  UGET("mapping.0.bias", &w.map_b0, mw);
+  UGET("mapping.2.weight", &w.map_w1, mw, mw);
+  UGET("mapping.2.bias", &w.map_b1, mw);
+  float *aw, *ab;
+  if ((rc = ualloc(m, &aw, (size_t)m->ada_total * mw)) || (rc = ualloc(m, &ab, (size_t)m->ada_total))) return rc;
+  for (const UMod& u : m->mods) {
+    const int n_ada = u.kind == M_RES ? 2 : (u.kind == M_ATTN ? 1 : 0);
+    for (int i = 0; i < n_ada; ++i) {
+      const int off = i ? u.ada2 : u.ada1, C = i ? u.c_mid : (u.kind == M_RES ? u.c_in : u.c_out);
+      KDB_CUDA(cudaMemcpyAsync(aw + (size_t)off * mw, i ? u.mapper2_w : u.mapper1_w, sizeof(float) * 2 * C * mw, cudaMemcpyDeviceToDevice, st));
+      KDB_CUDA(cudaMemcpyAsync(ab + off, i ? u.mapper2_b : u.mapper1_b, sizeof(float) * 2 * C, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  w.ada_w = aw, w.ada_b = ab;
+  KDB_CUDA(cudaStreamSynchronize(st));
+  m->finalized = true;
+  return 0;
+}
+
+int64_t kdb_unet_cond_stride(const KdbUNet* m) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_cond_stride: model NULL or not finalized");
+  return (int64_t)align_up((size_t)(m->ada_total + m->cfg.mapping_out), 4);
+}
+
+int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, float* cond_out,
+                          void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_conditioning: model NULL or not finalized");
+  KDB_REQUIRE(rows > 0 && sigma && cond_out, KDB_ERR_BAD_ARG, "unet_conditioning: bad arguments");
+  const KdbUNetConfig& c = m->cfg;
+  KDB_REQUIRE(!(aug_cond && !c.augment_wrapper), KDB_ERR_BAD_ARG, "unet_conditioning: aug_cond needs the augment wrapper");
+  KDB_REQUIRE(!(c.augment_wrapper && c.mapping_cond_dim > 9 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
+              "unet_conditioning: mapping_cond must be given (mapping_cond_dim %d)", c.mapping_cond_dim - 9);
+  KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG,
+              "unet_conditioning: the model takes no mapping_cond");
+  return launch_unet_conditioning(m->cw, rows, sigma, aug_cond, mapping_cond, cond_out, kdb_unet_cond_stride(m), (cudaStream_t)stream);
+}
+
+int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int height, int width) {
+  KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "unet_workspace_bytes: bad argument");
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "unet_workspace_bytes: only the fp32 path is built (precision %d)", precision);
+  UWs ws;
+  ucarve(m->cfg, batch, height, width, nullptr, ws);
+  return (int64_t)ws.total;
+}
+
+int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                     const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_forward: model NULL or not finalized");
+  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward: NULL argument");
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "unet_forward: only the fp32 path is built (precision %d)", precision);
+  const KdbUNetConfig& c = m->cfg;
+  KDB_REQUIRE(height > 0 && width > 0 && height % c.patch_size == 0 && width % c.patch_size == 0, KDB_ERR_BAD_SHAPE,
+              "unet_forward: %dx%d not divisible by the patch size %d", height, width, c.patch_size);
+  for (int l = c.skip_stages; l < c.n_levels; ++l) {
+    int h, w;
+    level_dims(c, height, width, l, &h, &w);
+    const bool down_from = l < c.n_levels - 1;        // this grid is downsampled, and the upsample must restore it
+    KDB_REQUIRE(h >= 2 && w >= 2 && (!down_from || (h % 2 == 0 && w % 2 == 0)), KDB_ERR_BAD_SHAPE,
+                "unet_forward: level %d grid %dx%d (every level but the innermost needs an even grid, every level >= 2x2)", l, h, w);
+  }
+  UWs ws;
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 256));
+  ucarve(c, batch, height, width, base, ws);
+  KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward: workspace %zu < required %zu", workspace_bytes, ws.total);
+  const int rc = unet_forward(m, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream);
+  m->tap_out = nullptr;
+  m->tap_name.clear();
+  return rc;
+}
+
+int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) {
+  KDB_REQUIRE(m && name && out && capacity > 0, KDB_ERR_BAD_ARG, "unet_debug_tap: bad argument");
+  m->tap_name = name;
+  m->tap_out = out;
+  m->tap_cap = capacity;
+  m->tap_count = 0;
+  return 0;
+}
+
+int64_t kdb_unet_tap_count(const KdbUNet* m) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_tap_count: NULL handle");
+  return m->tap_count;
+}
+
+}  // extern "C"

@@ -1,0 +1,65 @@
+// unet_kernels.cuh -- launchers of the fp32 image_v1 U-Net kernels (reference models/image_v1.py, layers.py:116-313).
+// Activations are token-major: [B, H, W, C] fp32, channels contiguous (DESIGN.md section 3).  Every kernel is deterministic:
+// fixed reduction orders, no atomics.
+#pragma once
+#include "common.cuh"
+
+namespace kdb {
+
+// out[m, n] = bias[n] + sum_{tap, c} w[n, tap, c] * in(pixel m shifted by tap, c) + resid[m, n]
+// A ks x ks convolution (ks = 1 or 3, zero padding ks / 2, stride 1) run as an implicit GEMM.  The input is the channel
+// concatenation of in1 [B,H,W,c1] and in2 [B,H,W,c2] (c2 = 0: one source), so a UBlock's torch.cat is never materialised.
+// w is tap-major [N, ks*ks, c1 + c2]; bias and the residual may be NULL.  The residual is [B,H,W,N] read as the concatenation of
+// r1 (rc1 channels) and r2 (N - rc1 channels).  c1, c2 and rc1 must be multiples of 4.
+struct ConvArgs {
+  const float* in1 = nullptr;
+  const float* in2 = nullptr;
+  int c1 = 0, c2 = 0;
+  const float* w = nullptr;
+  const float* bias = nullptr;
+  const float* r1 = nullptr;
+  const float* r2 = nullptr;
+  int rc1 = 0;
+  float* out = nullptr;
+  int B = 0, H = 0, W = 0, N = 0;
+};
+int launch_unet_conv(const ConvArgs& a, int ks, cudaStream_t st);
+
+// AdaGN (layers.py:172-175), optionally followed by the erf GELU: out = [gelu](group_norm(x) * (1 + weight) + bias) with the
+// (weight, bias) pair read from the conditioning row of image b at cond + b * cond_bs + ada_off (C weights, then C biases).
+// x is the concatenation of in1 (c1 channels) and in2 (c2 channels, may be 0); out is [B, HW, c1 + c2].  One CTA per
+// (group, image) reduces the group's mean and variance in a fixed order, then normalises the group.
+int launch_unet_adagn(const float* in1, int c1, const float* in2, int c2, float* out, const float* cond, int64_t cond_bs, int ada_off,
+                      int groups, bool gelu, int B, int HW, cudaStream_t st);
+
+// Downsample2d / Upsample2d (layers.py:251-280): depthwise [1,3,3,1]/8 filter, reflect padding 1, stride 2.
+// in [B, H, W, C] -> out [B, H/2, W/2, C] (up = false) or [B, 2H, 2W, C] (up = true).  H, W >= 2.
+int launch_unet_resample(const float* in, float* out, int B, int H, int W, int C, bool up, cudaStream_t st);
+
+// pixel_unshuffle(c_in(sigma) x, p) then proj_in (1x1 conv with bias): x [B, Cin, H, W] NCHW -> out [B, H/p, W/p, N]
+// (image_v1.py:146-148, layers.py:88-90).  sigma_data <= 0: no c_in scaling.  w [N, Cin*p*p].
+int launch_unet_patch_in(const float* x, const float* sigma, float sigma_data, const float* w, const float* bias, float* out, int B, int Cin,
+                         int H, int W, int p, int N, cudaStream_t st);
+
+// proj_out (1x1 conv with bias) then pixel_shuffle, the variance channel (has_variance) skipped, then (sigma_data > 0) the
+// Karras combine out = c_out F + c_skip x_in (image_v1.py:150-154, layers.py:88-90).  tokens [B, H/p, W/p, K], w [>= Cout*p*p, K],
+// out [B, Cout, H, W] NCHW.
+int launch_unet_patch_out(const float* tokens, const float* w, const float* bias, const float* x_in, const float* sigma, float sigma_data,
+                          float* out, int B, int Cout, int H, int W, int p, int K, cudaStream_t st);
+
+// Conditioning (image_v1.py:136-139, augmentation.py:97-104, and every AdaGN mapper, layers.py:173): per row
+//   cond = MappingNet(FourierFeatures(log(sigma) / 4) + mapping_cond_linear(v)),  v = [aug_cond or zeros(9), mapping_cond] with the
+//   augment wrapper, mapping_cond otherwise (NULL: no term);  out[row] = [ada_w cond + ada_b (ada_total floats), cond (mw floats)].
+struct UNetCondWeights {
+  int mw = 0, mcond_dim = 0, augment = 0, ada_total = 0;
+  const float *time_emb = nullptr, *mcond_w = nullptr;
+  const float *map_w0 = nullptr, *map_b0 = nullptr, *map_w1 = nullptr, *map_b1 = nullptr;
+  const float *ada_w = nullptr, *ada_b = nullptr;   // [ada_total, mw], [ada_total]
+};
+int launch_unet_conditioning(const UNetCondWeights& w, int rows, const float* sigma, const float* aug, const float* mcond, float* out,
+                             int64_t out_stride, cudaStream_t st);
+
+// torch conv weight [N, C, k, k] -> tap-major [N, k*k, C], times `scale` for rows n < scaled_rows (the folded attention scale)
+int launch_unet_reorder_conv_weight(const float* src, float* dst, int N, int C, int ks, int scaled_rows, float scale, cudaStream_t st);
+
+}  // namespace kdb

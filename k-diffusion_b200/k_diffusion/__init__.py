@@ -2,9 +2,9 @@
 
 Same import surface as the reference for the path in scope (`sampling`, `layers.Denoiser`,
 `external.DiscreteSchedule`, `config.load_config / make_model / make_denoiser_wrapper`,
-`models.ImageTransformerDenoiserModelV2`); everything on the latent runs in libkdb200.so.
+`models.ImageTransformerDenoiserModelV2`, `models.ImageDenoiserModelV1`, `augmentation.KarrasAugmentWrapper`); everything on the latent runs in libkdb200.so.
 """
-from . import config, evaluation, external, layers, models, parallel, sampling, synth, utils
+from . import augmentation, config, evaluation, external, layers, models, parallel, sampling, synth, utils
 from .layers import Denoiser
 
-__all__ = ["config", "evaluation", "external", "layers", "models", "parallel", "sampling", "synth", "utils", "Denoiser"]
+__all__ = ["augmentation", "config", "evaluation", "external", "layers", "models", "parallel", "sampling", "synth", "utils", "Denoiser"]

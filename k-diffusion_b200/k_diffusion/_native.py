@@ -18,7 +18,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -30,6 +30,14 @@ class KdbModelConfig(ctypes.Structure):
         ("mapping_width", _i32), ("mapping_depth", _i32), ("mapping_d_ff", _i32), ("num_classes", _i32), ("mapping_cond_dim", _i32),
         ("width", _i32 * MAX_LEVELS), ("depth", _i32 * MAX_LEVELS), ("d_ff", _i32 * MAX_LEVELS), ("attn_type", _i32 * MAX_LEVELS),
         ("d_head", _i32 * MAX_LEVELS), ("attn_param", _i32 * MAX_LEVELS),
+    ]
+
+
+class KdbUNetConfig(ctypes.Structure):
+    _fields_ = [
+        ("n_levels", _i32), ("in_channels", _i32), ("patch_size", _i32), ("mapping_out", _i32), ("mapping_cond_dim", _i32),
+        ("augment_wrapper", _i32), ("skip_stages", _i32), ("has_variance", _i32),
+        ("depth", _i32 * MAX_LEVELS), ("channels", _i32 * MAX_LEVELS), ("self_attn", _i32 * MAX_LEVELS),
     ]
 
 
@@ -67,6 +75,16 @@ SIGNATURES = {
     "kdb_model_forward_vjp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_model_tap_count": (_i64, [_vp]),
+    "kdb_unet_create": (_i32, [ctypes.POINTER(KdbUNetConfig), ctypes.POINTER(_vp)]),
+    "kdb_unet_destroy": (_i32, [_vp]),
+    "kdb_unet_set_tensor": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
+    "kdb_unet_finalize": (_i32, [_vp, _vp]),
+    "kdb_unet_cond_stride": (_i64, [_vp]),
+    "kdb_unet_conditioning": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "kdb_unet_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32, _i32]),
+    "kdb_unet_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
+    "kdb_unet_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
+    "kdb_unet_tap_count": (_i64, [_vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16_geglu": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
@@ -323,6 +341,11 @@ _ATTN_CODE = {"none": ATTN_NONE, "global": ATTN_GLOBAL, "neighborhood": ATTN_NEI
 class Engine:
     """Owns one KdbModel handle for one ImageTransformerDenoiserModelV2 instance on one device."""
 
+    _api = "model"          # kdb_<api>_set_tensor / _finalize / _cond_stride / _debug_tap / _tap_count
+
+    def _fn(self, name):
+        return getattr(lib(), f"kdb_{self._api}_{name}")
+
     def __init__(self, spec):
         cfg = KdbModelConfig()
         levels = spec["levels"]
@@ -371,11 +394,11 @@ class Engine:
                 t32 = f32c(t.detach())
                 held[k] = t32
                 shape = (_i64 * t32.ndim)(*t32.shape)
-                check(lib().kdb_model_set_tensor(self._h, k.encode(), ptr(t32), shape, t32.ndim))
-            check(lib().kdb_model_finalize(self._h, stream()))
+                check(self._fn("set_tensor")(self._h, k.encode(), ptr(t32), shape, t32.ndim))
+            check(self._fn("finalize")(self._h, stream()))
         self._held = held
         self._sig = sig
-        self._stride = int(lib().kdb_model_cond_stride(self._h))
+        self._stride = int(self._fn("cond_stride")(self._h))
 
     @property
     def cond_stride(self):
@@ -461,11 +484,80 @@ class Engine:
 
     def arm_tap(self, name, capacity, device):
         buf = torch.empty(capacity, dtype=torch.float32, device=device)
-        check(lib().kdb_model_debug_tap(self._h, name.encode(), ptr(buf), capacity))
+        check(self._fn("debug_tap")(self._h, name.encode(), ptr(buf), capacity))
         return buf
 
     def tap_count(self):
-        return int(lib().kdb_model_tap_count(self._h))
+        return int(self._fn("tap_count")(self._h))
+
+
+class UNetEngine(Engine):
+    """Owns one KdbUNet handle (the image_v1 U-Net on the exact fp32 path) for one ImageDenoiserModelV1 on one device.
+
+    Same interface as Engine where the sampler executor calls it (bind, cond_stride, conditioning, forward, taps); the
+    derivative entry points do not exist for the U-Net."""
+
+    _api = "unet"
+
+    def __init__(self, spec):
+        cfg = KdbUNetConfig()
+        n = len(spec["depths"])
+        if n > MAX_LEVELS:
+            raise ValueError(f"at most {MAX_LEVELS} levels supported")
+        cfg.n_levels, cfg.in_channels, cfg.patch_size, cfg.mapping_out = n, spec["c_in"], spec["patch_size"], spec["feats_in"]
+        cfg.mapping_cond_dim, cfg.augment_wrapper = spec["mapping_cond_dim"], int(spec["augment"])
+        cfg.skip_stages, cfg.has_variance = spec["skip_stages"], int(spec["has_variance"])
+        for i in range(n):
+            cfg.depth[i], cfg.channels[i], cfg.self_attn[i] = spec["depths"][i], spec["channels"][i], int(bool(spec["self_attn_depths"][i]))
+        self.cfg = cfg
+        self._h = _vp()
+        check(lib().kdb_unet_create(ctypes.byref(cfg), ctypes.byref(self._h)))
+        self._sig, self._held, self._ws, self._stride, self.device = None, {}, None, None, None
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and _lib is not None:
+                _lib.kdb_unet_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def conditioning(self, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
+        """-> [rows, cond_stride] fp32 table (mapping net + every AdaGN's (weight, bias))."""
+        if class_cond is not None:
+            raise TypeError("the image_v1 U-Net takes no class_cond")
+        require_cuda(sigma, aug_cond, mapping_cond)
+        sigma = f32c(sigma)
+        rows = sigma.numel()
+        aug_cond = None if aug_cond is None else f32c(aug_cond)
+        mapping_cond = None if mapping_cond is None else f32c(mapping_cond)
+        out = torch.empty(rows, self._stride, device=sigma.device, dtype=torch.float32)
+        with device_of(sigma):
+            check(lib().kdb_unet_conditioning(self._h, rows, ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(out), stream()))
+        return out
+
+    def workspace_bytes(self, precision, B, H, W):
+        need = int(lib().kdb_unet_workspace_bytes(self._h, precision, B, H, W))
+        if need < 0:
+            check(need)
+        return need
+
+    def forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
+        """x [B,C,H,W] fp32; sigma [B]; cond rows; sigma_data <= 0 -> raw inner model."""
+        B, C, H, W = x.shape
+        if out is None:
+            out = torch.empty(B, C, H, W, device=x.device, dtype=torch.float32)
+        ws = self._reserve(self.workspace_bytes(precision, B, H, W), x.device)
+        with device_of(x):
+            check(lib().kdb_unet_forward(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
+                                         ptr(out), ptr(ws), ws.numel(), stream()))
+        return out
+
+    def forward_jvp(self, *args, **kwargs):
+        raise NotImplementedError("the image_v1 U-Net engine has no forward-mode derivative (only its fp32 forward is built)")
+
+    def forward_vjp(self, *args, **kwargs):
+        raise NotImplementedError("the image_v1 U-Net engine has no reverse-mode derivative (only its fp32 forward is built)")
 
 
 # ---------------------------------------------------------------------------------------------

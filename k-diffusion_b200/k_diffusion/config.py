@@ -1,16 +1,21 @@
 """Config loading / model factory for the path in scope (reference: k_diffusion/config.py:23-231).
 
 Accepts the reference's JSON files, dicts, and `.safetensors` checkpoints carrying the config in
-their metadata.  Only `image_transformer_v2` can be built; the other model families are out of scope.
+their metadata.  `image_transformer_v2` and `image_v1` can be built; `image_transformer_v1` is out of scope.
 """
 import json
 from functools import partial
 from pathlib import Path
 
-from . import layers, models
+from . import augmentation, layers, models
 
 _V2_MODEL_DEFAULTS = dict(mapping_width=256, mapping_depth=2, mapping_d_ff=None, mapping_cond_dim=0, mapping_dropout_rate=0.,
                           d_ffs=None, self_attns=None, dropout_rate=None, augment_wrapper=False, skip_stages=0, has_variance=False)
+_V1_MODEL_DEFAULTS = dict(patch_size=1, augment_wrapper=True, mapping_cond_dim=0, unet_cond_dim=0, cross_cond_dim=0, cross_attn_depths=None,
+                          skip_stages=0, has_variance=False)
+_V1_OPT_DEFAULTS = dict(type='adamw', lr=1e-4, betas=[0.95, 0.999], eps=1e-6, weight_decay=1e-3)
+# keys make_model needs that have no default: the reference fails on them later, in make_model (KeyError)
+_V1_REQUIRED = ('input_channels', 'input_size', 'mapping_out', 'depths', 'channels', 'self_attn_depths')
 _V2_OPT_DEFAULTS = dict(type='adamw', lr=5e-4, betas=[0.9, 0.99], eps=1e-8, weight_decay=1e-4)
 _COMMON_DEFAULTS = {
     'model': dict(sigma_data=1., dropout_rate=0., augment_prob=0., loss_config='karras', loss_weighting='karras', loss_scales=1),
@@ -45,8 +50,13 @@ def _read(path_or_dict):
 def load_config(path_or_dict):
     config = _read(path_or_dict)
     kind = config['model']['type']
+    if kind == 'image_v1':
+        missing = [k for k in _V1_REQUIRED if k not in config['model']]
+        if missing:
+            raise ValueError(f'image_v1 config lacks {missing} (make_model needs them and they have no default)')
+        return _overlay(_COMMON_DEFAULTS, _overlay({'model': _V1_MODEL_DEFAULTS, 'optimizer': _V1_OPT_DEFAULTS}, config))
     if kind != 'image_transformer_v2':
-        raise ValueError(f'model type {kind!r} is out of scope for the H100 sampling path (only image_transformer_v2)')
+        raise ValueError(f'model type {kind!r} is out of scope for the H100 sampling path (image_transformer_v2 and image_v1 only)')
     config = _overlay({'model': _V2_MODEL_DEFAULTS, 'optimizer': _V2_OPT_DEFAULTS}, config)
     m = config['model']
     n = len(m['widths'])
@@ -79,6 +89,14 @@ def _attn_spec(a):
 def make_model(config):
     num_classes = config['dataset']['num_classes']
     m = config['model']
+    if m['type'] == 'image_v1':
+        if m['unet_cond_dim'] > 0 or m['cross_cond_dim'] > 0:
+            raise NotImplementedError('unet_cond_dim / cross_cond_dim > 0: the native image_v1 engine has no U-Net or cross-attention conditioning')
+        model = models.ImageDenoiserModelV1(
+            m['input_channels'], m['mapping_out'], m['depths'], m['channels'], m['self_attn_depths'], m['cross_attn_depths'],
+            patch_size=m['patch_size'], dropout_rate=m['dropout_rate'], mapping_cond_dim=m['mapping_cond_dim'] + (9 if m['augment_wrapper'] else 0),
+            unet_cond_dim=m['unet_cond_dim'], cross_cond_dim=m['cross_cond_dim'], skip_stages=m['skip_stages'], has_variance=m['has_variance'])
+        return augmentation.KarrasAugmentWrapper(model) if m['augment_wrapper'] else model
     if m['type'] != 'image_transformer_v2':
         raise ValueError(f'unsupported model type {m["type"]}')
     v2 = models.image_transformer_v2

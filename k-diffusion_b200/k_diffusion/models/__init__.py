@@ -1,2 +1,3 @@
-from . import flags, flops, image_transformer_v2
+from . import flags, flops, image_transformer_v2, image_v1
 from .image_transformer_v2 import ImageTransformerDenoiserModelV2
+from .image_v1 import ImageDenoiserModelV1

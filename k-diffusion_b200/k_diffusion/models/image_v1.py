@@ -1,0 +1,251 @@
+"""image_v1 U-Net denoiser -- parameter container + native forward on the exact fp32 path.
+
+Constructor, forward signature and `state_dict()` layout follow the reference (k_diffusion/models/image_v1.py, layers.py:116-313),
+so reference checkpoints load unchanged; the forward pass itself is executed by libkdb200.so (kdb_unet_*).  The torch modules
+below only hold named parameters and buffers: none of their forward methods runs.  Inference only; fp32 only (a tensor-core
+route for the U-Net is not built).
+"""
+from types import SimpleNamespace
+
+import torch
+from torch import nn
+
+from .. import _native
+from ..layers import FourierFeatures
+from . import flags
+
+
+def orthogonal_(module):
+    nn.init.orthogonal_(module.weight)
+    return module
+
+
+class AdaGN(nn.Module):
+    """layers.py:162-175"""
+
+    def __init__(self, feats_in, c_out, num_groups, eps=1e-5, cond_key='cond'):
+        super().__init__()
+        self.num_groups, self.eps, self.cond_key = num_groups, eps, cond_key
+        self.mapper = nn.Linear(feats_in, c_out * 2)
+        nn.init.zeros_(self.mapper.weight)
+        nn.init.zeros_(self.mapper.bias)
+
+
+class ResConvBlock(nn.Module):
+    """image_v1.py:15-29 (ConditionedResidualBlock, layers.py:151-159): main.{0..7} and skip"""
+
+    def __init__(self, feats_in, c_in, c_mid, c_out, group_size=32, dropout_rate=0.):
+        super().__init__()
+        self.main = nn.Sequential(
+            AdaGN(feats_in, c_in, max(1, c_in // group_size)), nn.GELU(), nn.Conv2d(c_in, c_mid, 3, padding=1), nn.Dropout2d(dropout_rate),
+            AdaGN(feats_in, c_mid, max(1, c_mid // group_size)), nn.GELU(), nn.Conv2d(c_mid, c_out, 3, padding=1), nn.Dropout2d(dropout_rate))
+        self.skip = nn.Identity() if c_in == c_out else orthogonal_(nn.Conv2d(c_in, c_out, 1, bias=False))
+        nn.init.zeros_(self.main[-2].weight)
+        nn.init.zeros_(self.main[-2].bias)
+
+
+class SelfAttention2d(nn.Module):
+    """layers.py:181-200"""
+
+    def __init__(self, c_in, n_head, norm, dropout_rate=0.):
+        super().__init__()
+        assert c_in % n_head == 0
+        self.norm_in = norm(c_in)
+        self.n_head = n_head
+        self.qkv_proj = nn.Conv2d(c_in, c_in * 3, 1)
+        self.out_proj = nn.Conv2d(c_in, c_in, 1)
+        self.dropout = nn.Dropout(dropout_rate)
+        nn.init.zeros_(self.out_proj.weight)
+        nn.init.zeros_(self.out_proj.bias)
+
+
+class Downsample2d(nn.Module):
+    """layers.py:251-257 ('linear' filter, reflect padding)"""
+
+    def __init__(self):
+        super().__init__()
+        k1 = torch.tensor([[1 / 8, 3 / 8, 3 / 8, 1 / 8]])
+        self.register_buffer('kernel', k1.T @ k1)
+
+
+class Upsample2d(nn.Module):
+    """layers.py:267-273"""
+
+    def __init__(self):
+        super().__init__()
+        k1 = torch.tensor([[1 / 8, 3 / 8, 3 / 8, 1 / 8]]) * 2
+        self.register_buffer('kernel', k1.T @ k1)
+
+
+def _block(n_layers, feats_in, c_in, c_mid, c_out, self_attn, dropout_rate, group_size=32, head_size=64):
+    mods = []
+    for i in range(n_layers):
+        my_c_in = c_in if i == 0 else c_mid
+        my_c_out = c_mid if i < n_layers - 1 else c_out
+        mods.append(ResConvBlock(feats_in, my_c_in, c_mid, my_c_out, group_size, dropout_rate))
+        if self_attn:
+            norm = lambda c, g=max(1, my_c_out // group_size): AdaGN(feats_in, c, g)
+            mods.append(SelfAttention2d(my_c_out, max(1, my_c_out // head_size), norm, dropout_rate))
+    return mods
+
+
+def DBlock(n_layers, feats_in, c_in, c_mid, c_out, dropout_rate=0., downsample=False, self_attn=False):
+    """image_v1.py:32-50: [Downsample2d | Identity, (ResConvBlock, [SelfAttention2d]) * n_layers]"""
+    return nn.Sequential(Downsample2d() if downsample else nn.Identity(), *_block(n_layers, feats_in, c_in, c_mid, c_out, self_attn, dropout_rate))
+
+
+def UBlock(n_layers, feats_in, c_in, c_mid, c_out, dropout_rate=0., upsample=False, self_attn=False):
+    """image_v1.py:53-77: [(ResConvBlock, [SelfAttention2d]) * n_layers, Upsample2d | Identity]"""
+    return nn.Sequential(*_block(n_layers, feats_in, c_in, c_mid, c_out, self_attn, dropout_rate), Upsample2d() if upsample else nn.Identity())
+
+
+class UNet(nn.Module):
+    """layers.py:298-303 (u_blocks innermost first)"""
+
+    def __init__(self, d_blocks, u_blocks, skip_stages=0):
+        super().__init__()
+        self.d_blocks = nn.ModuleList(d_blocks)
+        self.u_blocks = nn.ModuleList(u_blocks)
+        self.skip_stages = skip_stages
+
+
+class ImageDenoiserModelV1(nn.Module):
+    def __init__(self, c_in, feats_in, depths, channels, self_attn_depths, cross_attn_depths=None, mapping_cond_dim=0, unet_cond_dim=0,
+                 cross_cond_dim=0, dropout_rate=0., patch_size=1, skip_stages=0, has_variance=False):
+        super().__init__()
+        if unet_cond_dim > 0 or cross_cond_dim > 0:
+            raise NotImplementedError('unet_cond and cross-attention conditioning are not supported by the native image_v1 engine')
+        self.c_in, self.channels, self.unet_cond_dim, self.patch_size, self.has_variance = c_in, channels, unet_cond_dim, patch_size, has_variance
+        self.feats_in, self.depths, self.self_attn_depths, self.mapping_cond_dim = feats_in, list(depths), list(self_attn_depths), mapping_cond_dim
+        self.dropout_rate = dropout_rate
+        self.timestep_embed = FourierFeatures(1, feats_in)
+        if mapping_cond_dim > 0:
+            self.mapping_cond = nn.Linear(mapping_cond_dim, feats_in, bias=False)
+        self.mapping = nn.Sequential(orthogonal_(nn.Linear(feats_in, feats_in)), nn.GELU(), orthogonal_(nn.Linear(feats_in, feats_in)), nn.GELU())
+        self.proj_in = nn.Conv2d((c_in + unet_cond_dim) * patch_size ** 2, channels[max(0, skip_stages - 1)], 1)
+        self.proj_out = nn.Conv2d(channels[max(0, skip_stages - 1)], c_in * patch_size ** 2 + (1 if has_variance else 0), 1)
+        nn.init.zeros_(self.proj_out.weight)
+        nn.init.zeros_(self.proj_out.bias)
+        d_blocks, u_blocks = [], []
+        for i in range(len(depths)):
+            d_blocks.append(DBlock(depths[i], feats_in, channels[max(0, i - 1)], channels[i], channels[i], dropout_rate, i > skip_stages,
+                                   self_attn_depths[i]))
+        for i in range(len(depths)):
+            my_c_in = channels[i] * 2 if i < len(depths) - 1 else channels[i]
+            u_blocks.append(UBlock(depths[i], feats_in, my_c_in, channels[i], channels[max(0, i - 1)], dropout_rate, i > skip_stages,
+                                   self_attn_depths[i]))
+        self.u_net = UNet(d_blocks, reversed(u_blocks), skip_stages=skip_stages)
+        self.precision = None
+        self._engines = {}
+
+    # ------------------------------------------------------------------ engine plumbing
+    def __getstate__(self):
+        state = self.__dict__.copy()
+        state["_engines"] = {}
+        return state
+
+    def __deepcopy__(self, memo):
+        import copy
+        engines, self._engines = self._engines, {}
+        try:
+            new = self.__class__.__new__(self.__class__)
+            memo[id(self)] = new
+            new.__dict__ = copy.deepcopy(self.__dict__, memo)
+        finally:
+            self._engines = engines
+        return new
+
+    @property
+    def levels(self):
+        """per-level dropout (what the sampler executor checks before running the inference-only engine)"""
+        return [SimpleNamespace(dropout=self.dropout_rate)] * len(self.depths)
+
+    def engine(self, augment=False):
+        """Native engine with the current parameters bound; `augment`: conditioning as KarrasAugmentWrapper forms it."""
+        eng = self._engines.get(augment)
+        if eng is None:
+            eng = self._engines[augment] = _native.UNetEngine(dict(
+                c_in=self.c_in, feats_in=self.feats_in, depths=self.depths, channels=self.channels, self_attn_depths=self.self_attn_depths,
+                mapping_cond_dim=self.mapping_cond_dim, augment=augment, patch_size=self.patch_size, skip_stages=self.u_net.skip_stages,
+                has_variance=self.has_variance))
+        eng.bind(dict(self.state_dict(keep_vars=True)))
+        return eng
+
+    def set_precision(self, precision):
+        """'fp32' or None/'auto' (both the exact fp32 path); the U-Net has no bf16 route."""
+        if precision not in (None, "auto", "fp32", "float32"):
+            raise ValueError(f"the image_v1 U-Net runs on the exact fp32 path only (got precision {precision!r})")
+        self.precision = None if precision in (None, "auto") else "fp32"
+        return self
+
+    def resolved_precision(self):
+        p = flags.resolve_precision(self.precision, torch.float32)
+        if p != "fp32":
+            raise ValueError(f"the image_v1 U-Net runs on the exact fp32 path only (resolved precision {p!r})")
+        return _native.PREC_FP32
+
+    def param_groups(self, *args, **kwargs):
+        raise NotImplementedError("training is out of scope for the H100 sampling path")
+
+    # ------------------------------------------------------------------ native interface of the bare model (no augment wrapper)
+    class_emb = None
+
+    @property
+    def mapping_cond_in_proj(self):
+        return True if self.mapping_cond_dim > 0 else None
+
+    def _check_cond(self, class_cond, mapping_cond):
+        self.check_cond(False, class_cond, mapping_cond)
+
+    def denoise(self, x, sigma, sigma_data, mapping_cond=None, out=None):
+        """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
+        return self.run(x, sigma, float(sigma_data), False, mapping_cond=mapping_cond, out=out)
+
+    def denoise_jvp(self, *args, **kwargs):
+        raise NotImplementedError("the image_v1 U-Net engine has no forward-mode derivative (only its fp32 forward is built)")
+
+    def denoise_vjp(self, *args, **kwargs):
+        raise NotImplementedError("the image_v1 U-Net engine has no reverse-mode derivative (only its fp32 forward is built)")
+
+    # ------------------------------------------------------------------ forward
+    def user_mapping_cond_dim(self, augment):
+        return self.mapping_cond_dim - (9 if augment else 0)
+
+    def check_cond(self, augment, class_cond, mapping_cond):
+        if class_cond is not None:
+            raise TypeError("the image_v1 U-Net takes no class_cond")
+        if mapping_cond is not None and self.user_mapping_cond_dim(augment) <= 0:
+            raise ValueError("this model takes no mapping_cond")
+        if mapping_cond is None and augment and self.user_mapping_cond_dim(augment) > 0:
+            raise ValueError("mapping_cond must be specified if mapping_cond_dim > 0")
+
+    def run(self, x, sigma, sigma_data, augment, aug_cond=None, mapping_cond=None, out=None):
+        """One native evaluation: the raw model (sigma_data <= 0) or the Karras-preconditioned denoiser."""
+        _native.require_cuda(x, sigma)
+        if x.ndim != 4:
+            raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
+        if self.training and self.dropout_rate > 0:
+            raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
+        if torch.is_grad_enabled() and x.requires_grad:
+            raise NotImplementedError("the image_v1 U-Net engine has no derivative: only its fp32 forward is built, so autograd cannot "
+                                      "reach x")
+        if aug_cond is not None and not augment:
+            raise TypeError("aug_cond needs the KarrasAugmentWrapper")
+        self.check_cond(augment, None, mapping_cond)
+        with torch.cuda.device(x.device):
+            xin = _native.f32c(x)
+            sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
+            if sig.shape != (x.shape[0],):
+                raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
+            eng = self.engine(augment)
+            cond = eng.conditioning(sig, aug_cond, None, mapping_cond)
+            res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
+        return res if x.dtype == torch.float32 else res.to(x.dtype)
+
+    def forward(self, input, sigma, mapping_cond=None, unet_cond=None, cross_cond=None, cross_cond_padding=None, return_variance=False):
+        """reference image_v1.py:135-157"""
+        if unet_cond is not None or cross_cond is not None:
+            raise NotImplementedError('unet_cond and cross-attention conditioning are not supported by the native image_v1 engine')
+        if return_variance:
+            raise NotImplementedError('the variance output is a training quantity; the native engine returns the denoised channels only')
+        return self.run(input, sigma, 0.0, False, mapping_cond=mapping_cond)

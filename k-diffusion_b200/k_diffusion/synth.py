@@ -41,6 +41,16 @@ def synth_tensor(key, shape, seed=0):
         return 1.0 + 0.1 * torch.randn(shape, generator=g)          # RMSNorm scale, init 1
     if key in ("time_emb.weight", "aug_emb.weight", "class_emb.weight"):
         return torch.randn(shape, generator=g)                      # FourierFeatures buffers / nn.Embedding
+    # image_v1 U-Net (reference models/image_v1.py, layers.py:162-280)
+    if key.endswith(".kernel") and shape == (4, 4):                 # Downsample2d / Upsample2d filter buffers
+        k1 = torch.tensor([[1 / 8, 3 / 8, 3 / 8, 1 / 8]]) * (2 if ".u_blocks." in key else 1)
+        return k1.T @ k1
+    if key.endswith("timestep_embed.weight"):
+        return torch.randn(shape, generator=g)                      # FourierFeatures buffer
+    if key.endswith(("mapper.weight", "main.6.weight", "proj_out.weight")) or key.endswith(".bias"):
+        return torch.randn(shape, generator=g) * ZERO_INIT_STD      # zero-initialised in the reference; biases small
+    if key.endswith(".weight") and len(shape) == 4:
+        return torch.randn(shape, generator=g) / math.sqrt(3.0 * math.prod(shape[1:]))
     if key.endswith(".weight") and len(shape) == 2:
         return torch.randn(shape, generator=g) / math.sqrt(3.0 * shape[1])   # variance of nn.Linear's default
     raise KeyError(f"synth_tensor: no recipe for {key} {shape}")
