@@ -57,6 +57,21 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// sum of v over the CTA, in the same order on every thread; red: shared scratch of one float per warp
+__device__ __forceinline__ float block_sum(float v, float* red) {
+  v = warp_sum(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float t = 0.f;
+  for (int i = 0; i < nw; ++i) t += red[i];
+  return t;
+}
+
+constexpr float kRsqrt2 = 0.70710678118654752440f;
+// erf GELU (image_transformer_v2.py:89-95, layers.py of image_v1) in the reference's association, 0.5 g (1 + erf(g / sqrt 2))
+__device__ __forceinline__ float gelu_erf(float g) { return 0.5f * g * (1.f + erff(g * kRsqrt2)); }
 
 // Karras preconditioner scalings (reference layers.py:70-74), fp32 like the reference.
 __device__ __forceinline__ void karras_scalings(float sigma, float sd, float& c_skip, float& c_out, float& c_in) {

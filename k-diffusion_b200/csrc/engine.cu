@@ -8,18 +8,12 @@
 #include <map>
 #include <string>
 #include <type_traits>
-#include <unordered_map>
 #include <vector>
 
-#include "model_kernels.cuh"
+#include "model_core.cuh"
 #include "tc_kernels.cuh"
 
 namespace kdb {
-
-struct TensorRef {
-  const float* p = nullptr;
-  std::vector<int64_t> shape;
-};
 
 struct LayerPlan {
   std::string prefix;
@@ -43,15 +37,12 @@ struct PosTables {
 
 using namespace kdb;
 
-struct KdbModel {
+struct KdbModel : ModelCore {
   KdbModelConfig cfg{};
-  std::unordered_map<std::string, TensorRef> tensors;
-  bool finalized = false;
   std::vector<LayerPlan> layers;   // in execution order (for_each_layer)
   std::vector<const float*> merge_w, split_w, split_fac;
   const float *patch_in_w = nullptr, *out_norm = nullptr, *patch_out_w = nullptr;
   std::vector<bf16*> merge_wb, split_wb;
-  std::vector<void*> owned;
   float* ada_cat = nullptr;
   FoldDesc* fold_descs = nullptr;   // device table for launch_fold_norm_weights
   int n_fold = 0;
@@ -61,56 +52,13 @@ struct KdbModel {
   bf16* patch_in_wb = nullptr;      // patch_in.proj.weight, columns permuted to (c, nh, nw) and padded to 64 (tensor-core patch-in)
   int ada_total = 0;
   CondWeights cw{};
-  std::map<std::pair<int, int>, PosTables> pos_cache;
-  // tap
-  std::string tap_name;
-  float* tap_out = nullptr;
-  int64_t tap_cap = 0, tap_count = 0;
+  std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
 };
 
 namespace {
 
-int get(KdbModel* m, const std::string& key, std::initializer_list<int64_t> shape, const float** out) {
-  auto it = m->tensors.find(key);
-  if (it == m->tensors.end()) {
-    set_error("missing state-dict entry '%s'", key.c_str());
-    return KDB_ERR_MISSING_KEY;
-  }
-  const std::vector<int64_t> want(shape);
-  if (it->second.shape != want) {
-    std::string got, exp;
-    for (auto v : it->second.shape) got += std::to_string(v) + ",";
-    for (auto v : want) exp += std::to_string(v) + ",";
-    set_error("shape mismatch for '%s': got [%s] expected [%s]", key.c_str(), got.c_str(), exp.c_str());
-    return KDB_ERR_BAD_SHAPE;
-  }
-  *out = it->second.p;
-  return 0;
-}
-
-#define GET(key, out, ...)                                        \
-  do {                                                            \
-    int rc__ = get(m, (key), {__VA_ARGS__}, (out));               \
-    if (rc__) return rc__;                                        \
-  } while (0)
-
-template <typename T>
-int dev_alloc(KdbModel* m, T** p, size_t count) {
-  void* q = nullptr;
-  KDB_CUDA(cudaMalloc(&q, count * sizeof(T) + 1024));
-  m->owned.push_back(q);
-  *p = reinterpret_cast<T*>(q);
-  return 0;
-}
-
-void free_owned(KdbModel* m) {
-  for (void* p : m->owned) cudaFree(p);
-  m->owned.clear();
-  m->pos_cache.clear();
-}
-
 int make_bf16(KdbModel* m, const float* src, int64_t n, bf16** dst, cudaStream_t st) {
-  int rc = dev_alloc(m, dst, (size_t)n);
+  int rc = m->alloc(dst, (size_t)n);
   if (rc) return rc;
   return launch_f32_to_bf16(src, *dst, n, st);
 }
@@ -178,7 +126,7 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
     int rc;
     if ((rc = make_bf16(m, L.qkv_w, 3LL * L.C * L.C, &L.qkv_wb, st))) return rc;
     if ((rc = make_bf16(m, L.out_w, (int64_t)L.C * L.C, &L.out_wb, st))) return rc;
-    if ((rc = dev_alloc(m, &L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
+    if ((rc = m->alloc(&L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
   }
   const std::string f = prefix + "ff.";
   GET(f + "norm.linear.weight", &L.ff_norm_w, L.C, mw);
@@ -190,10 +138,10 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
   if ((rc = make_bf16(m, L.up_w, 2LL * L.dff * L.C, &L.up_wb, st))) return rc;
   if ((rc = make_bf16(m, L.down_w, (int64_t)L.C * L.dff, &L.down_wb, st))) return rc;
   if (L.dff % 8 == 0) {
-    if ((rc = dev_alloc(m, &L.up_wb_il, (size_t)2 * L.dff * L.C))) return rc;
+    if ((rc = m->alloc(&L.up_wb_il, (size_t)2 * L.dff * L.C))) return rc;
     interleave_geglu_rows_kernel<<<kNumSMs * 4, 256, 0, st>>>(L.up_w, L.up_wb_il, L.dff, L.C);
     KDB_LAUNCH_CHECK(F_CONVERT, st);
-    if ((rc = dev_alloc(m, &L.up_wf, (size_t)2 * L.dff * L.C))) return rc;
+    if ((rc = m->alloc(&L.up_wf, (size_t)2 * L.dff * L.C))) return rc;
   }
   return 0;
 }
@@ -223,7 +171,7 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
   for (int l = 0; l < m->cfg.n_levels; ++l) {
     std::vector<float> f(cur.begin(), cur.end());
     float* d = nullptr;
-    int rc = dev_alloc(m, &d, f.size());
+    int rc = m->alloc(&d, f.size());
     if (rc) return rc;
     KDB_CUDA(cudaMemcpyAsync(d, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice, st));
     KDB_CUDA(cudaStreamSynchronize(st));
@@ -248,7 +196,7 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
     const LayerPlan& L = m->layers[k];
     if (L.attn_type == KDB_ATTN_NONE || L.e != 64) continue;
     const int T_l = (h0 >> L.level) * (w0 >> L.level);
-    int rc = dev_alloc(m, &pt.rope[k], (size_t)T_l * L.nh * 16);
+    int rc = m->alloc(&pt.rope[k], (size_t)T_l * L.nh * 16);
     if (rc) return rc;
     if ((rc = launch_rope_table(pt.pos[L.level], L.freqs, pt.rope[k], T_l, L.nh, L.e / 8, st))) return rc;
   }
@@ -265,14 +213,8 @@ struct Workspace {
   size_t total = 0;
 };
 
-void carve(const KdbModelConfig& c, int prec, int B, int H, int W, char* base, Workspace& ws) {
+void carve(const KdbModelConfig& c, int prec, int B, int H, int W, Carver& cv, Workspace& ws) {
   const size_t s = prec == KDB_PREC_BF16 ? 2 : 4;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    char* p = base ? base + off : nullptr;
-    off += align_up(bytes, 1024);
-    return p;
-  };
   const int n = c.n_levels;
   int64_t T = (int64_t)(H / c.patch_h) * (W / c.patch_w);
   size_t mx = 0, mqkv = 0, mh = 0, mg = 0;
@@ -280,33 +222,22 @@ void carve(const KdbModelConfig& c, int prec, int B, int H, int W, char* base, W
   ws.xup.assign(n, nullptr);
   for (int l = 0; l < n; ++l) {
     const size_t xb = (size_t)B * T * c.width[l] * s;
-    ws.xs[l] = take(xb);
-    if (l < n - 1) ws.xup[l] = take(xb);
+    ws.xs[l] = cv.take(xb);
+    if (l < n - 1) ws.xup[l] = cv.take(xb);
     mx = std::max(mx, xb);
     if (c.attn_type[l] != KDB_ATTN_NONE) mqkv = std::max(mqkv, 3 * xb);
     mh = std::max(mh, (size_t)B * T * 2 * c.d_ff[l] * s);
     if (l < n - 1) mg = std::max(mg, xb);
     T /= 4;
   }
-  ws.xn = take(mx);
-  ws.qkv = take(mqkv);
-  ws.ao = take(mx);
-  ws.hbuf = take(mh);
-  ws.gbuf = take(mh / 2);
-  ws.mg = take(mg);
-  ws.rowss = reinterpret_cast<float*>(take((size_t)B * (H / c.patch_h) * (W / c.patch_w) * SS_PARTS * sizeof(float)));
-  ws.total = off + 1024;
-}
-
-template <typename T>
-int tap(KdbModel* m, const std::string& name, const T* p, int64_t n, cudaStream_t st) {
-  if (m->tap_out == nullptr || m->tap_name != name) return 0;
-  if (n > m->tap_cap) {
-    m->tap_count = -n;
-    return 0;
-  }
-  m->tap_count = n;
-  return launch_to_f32<T>(p, m->tap_out, n, st);
+  ws.xn = cv.take(mx);
+  ws.qkv = cv.take(mqkv);
+  ws.ao = cv.take(mx);
+  ws.hbuf = cv.take(mh);
+  ws.gbuf = cv.take(mh / 2);
+  ws.mg = cv.take(mg);
+  ws.rowss = cv.take<float>((size_t)B * (H / c.patch_h) * (W / c.patch_w) * SS_PARTS * sizeof(float));
+  ws.total = cv.total();
 }
 
 template <typename T> struct WSel;
@@ -389,7 +320,7 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
     int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
     if constexpr (std::is_same_v<T, float>)
       if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, f.st);
-    return r ? r : tap<T>(m, tag + ".xn1", xn, Ma * C, f.st);
+    return r ? r : m->tap<T>(tag + ".xn1", xn, Ma * C, f.st);
   };
   auto unfused = [&] {
     int r = norm();
@@ -421,14 +352,14 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
   } else {
     rc = unfused();
   }
-  if (rc || (rc = tap<T>(m, tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
+  if (rc || (rc = m->tap<T>(tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
   // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
   if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
     return rc;
   if constexpr (std::is_same_v<T, float>)
     if (f.jvp && (rc = launch_attention_jvp(qkv, qkv + M * 3 * C, ao + M * C, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st)))
       return rc;
-  return tap<T>(m, tag + ".ao", ao, Ma * C, f.st);
+  return m->tap<T>(tag + ".ao", ao, Ma * C, f.st);
 }
 
 // The feed-forward half's up projection from the residual stream x: RMSNorm into ws.xn, up_proj into ws.hbuf.  The forward's unfused
@@ -454,13 +385,12 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   T* hb = reinterpret_cast<T*>(f.ws.hbuf);
   T* gb = reinterpret_cast<T*>(f.ws.gbuf);
   const std::string tag = "layer" + std::to_string(k);
-  auto tapped = [&](const char* part) { return m->tap_out != nullptr && m->tap_name == tag + part; };
   int rc = 0;
   if (L.attn_type != KDB_ATTN_NONE) {
     if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
     // attention: the whole half in one kernel (attn_block: 128-wide shifted-window levels; not while .qkv or .ao is tapped), or its
     // activations (attn_activations) and out_proj
-    const bool block = f.fold && f.stats && rope != nullptr && !tapped(".qkv") && !tapped(".ao") &&
+    const bool block = f.fold && f.stats && rope != nullptr && !m->tapped(tag + ".qkv") && !m->tapped(tag + ".ao") &&
                        tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift);
     if constexpr (std::is_same_v<T, bf16>) {
       if (block) {
@@ -476,7 +406,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
       f.produce(e, Ma, C, C);
       if ((rc = linear<T>(reinterpret_cast<T*>(f.ws.ao), WSel<T>::out(L), x, Ma, C, C, e, f.st))) return rc;
     }
-    if ((rc = tap<T>(m, tag + ".attn", x, Ma * C, f.st))) return rc;
+    if ((rc = m->tap<T>(tag + ".attn", x, Ma * C, f.st))) return rc;
   }
   if (f.tape) KDB_CUDA(cudaMemcpyAsync(f.tape[2 * k + 1], x, sizeof(T) * M * C, cudaMemcpyDeviceToDevice, f.st));
   auto unfused = [&] {
@@ -492,7 +422,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   //   RMSNorm + GEGLU GEMM
   //   RMSNorm + linear + geglu
   // then, after all but ffn_fused, down_proj
-  const bool ffn = f.fold && f.stats && L.up_wf != nullptr && tc_ffn_fused_supported(M, C, L.dff) && !tapped(".geglu");
+  const bool ffn = f.fold && f.stats && L.up_wf != nullptr && tc_ffn_fused_supported(M, C, L.dff) && !m->tapped(tag + ".geglu");
   if constexpr (std::is_same_v<T, bf16>) {
     T* xn = reinterpret_cast<T*>(f.ws.xn);
     if (ffn) {
@@ -511,14 +441,14 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   }
   if (rc) return rc;
   if (!ffn) {
-    if ((rc = tap<T>(m, tag + ".geglu", gb, Ma * L.dff, f.st))) return rc;
+    if ((rc = m->tap<T>(tag + ".geglu", gb, Ma * L.dff, f.st))) return rc;
     GemmEpi e;
     e.mode = EPI_RESID;
     e.resid = x;
     f.produce(e, Ma, C, L.dff);
     if ((rc = linear<T>(gb, WSel<T>::down(L), x, Ma, C, L.dff, e, f.st))) return rc;
   }
-  return tap<T>(m, tag + ".ff", x, Ma * C, f.st);
+  return m->tap<T>(tag + ".ff", x, Ma * C, f.st);
 }
 
 // v != nullptr (fp32 only): forward-mode derivative along v, the tangent D'(x) v goes to out_t.  The primal launches are those of a
@@ -566,13 +496,13 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   } else {
     rc = patch_in();
   }
-  if (rc || (rc = tap<T>(m, "patch_in", cur, (int64_t)Bt * h0 * w0 * C0, st))) return rc;
+  if (rc || (rc = m->tap<T>("patch_in", cur, (int64_t)Bt * h0 * w0 * C0, st))) return rc;
 
   int k = 0, h = h0, w = w0;
   for (int l = 0; l < n - 1; ++l) {
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".down", cur, (int64_t)Bt * h * w * c.width[l], st))) return rc;
+    if ((rc = m->tap<T>("L" + std::to_string(l) + ".down", cur, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     T* nxt = reinterpret_cast<T*>(ws.xs[l + 1]);
     const int64_t Mc = (int64_t)Bt * (h / 2) * (w / 2);
     const int N = c.width[l + 1], K = 4 * c.width[l];
@@ -600,12 +530,12 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     if (rc) return rc;
     h /= 2;
     w /= 2;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".merge", nxt, (int64_t)Bt * h * w * N, st))) return rc;
+    if ((rc = m->tap<T>("L" + std::to_string(l) + ".merge", nxt, (int64_t)Bt * h * w * N, st))) return rc;
     cur = nxt;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
     if ((rc = run_layer<T>(m, f, k++, cur, h, w))) return rc;
-  if ((rc = tap<T>(m, "mid", cur, (int64_t)Bt * h * w * c.width[n - 1], st))) return rc;
+  if ((rc = m->tap<T>("mid", cur, (int64_t)Bt * h * w * c.width[n - 1], st))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     T* up = reinterpret_cast<T*>(ws.xup[l]);
     GemmEpi e;
@@ -619,10 +549,10 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], e, st))) return rc;
     h *= 2;
     w *= 2;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".split", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
+    if ((rc = m->tap<T>("L" + std::to_string(l) + ".split", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = run_layer<T>(m, f, k++, up, h, w))) return rc;
-    if ((rc = tap<T>(m, "L" + std::to_string(l) + ".up", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
+    if ((rc = m->tap<T>("L" + std::to_string(l) + ".up", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
     cur = up;
   }
   // patch_out, routes in priority order (fp32 has only the last):
@@ -663,14 +593,11 @@ struct VjpSpace {
   size_t total = 0;
 };
 
-void carve_vjp(const KdbModelConfig& c, int B, int H, int W, char* base, Workspace& ws, VjpSpace& vs) {
-  carve(c, KDB_PREC_FP32, B, H, W, base, ws);
-  size_t off = align_up(ws.total, 1024);
-  auto take = [&](size_t floats) {
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += align_up(floats * sizeof(float), 1024);
-    return p;
-  };
+void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Workspace& ws, VjpSpace& vs) {
+  Carver cv(workspace, 1024);
+  carve(c, KDB_PREC_FP32, B, H, W, cv, ws);
+  cv.off = ws.total;
+  auto take = [&](size_t floats) { return cv.take<float>(floats * sizeof(float)); };
   const int n = c.n_levels;
   const int64_t T0 = (int64_t)(H / c.patch_h) * (W / c.patch_w);
   auto stream_floats = [&](int l) { return (size_t)B * (T0 >> (2 * l)) * c.width[l]; };
@@ -698,7 +625,7 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, char* base, Workspa
   vs.dbuf = take(md);
   vs.dh = take(mh);
   vs.stats = take(mst);
-  vs.total = off + 1024;
+  vs.total = cv.total();
 }
 
 // Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
@@ -795,26 +722,17 @@ int kdb_model_create(const KdbModelConfig* cfg, KdbModel** out) {
   return 0;
 }
 
-void kdb_model_destroy(KdbModel* m) {
-  if (!m) return;
-  free_owned(m);
-  delete m;
-}
+void kdb_model_destroy(KdbModel* m) { delete m; }
 
 int kdb_model_set_tensor(KdbModel* m, const char* key, const float* data, const int64_t* shape, int ndim) {
-  KDB_REQUIRE(m && key && data && ndim >= 0 && ndim <= 4, KDB_ERR_BAD_ARG, "set_tensor: bad argument");
-  TensorRef t;
-  t.p = data;
-  t.shape.assign(shape, shape + ndim);
-  m->tensors[key] = t;
-  m->finalized = false;
-  return 0;
+  return set_tensor(m, key, data, shape, ndim);
 }
 
 int kdb_model_finalize(KdbModel* m, void* stream) {
   KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "finalize: NULL model");
   cudaStream_t st = (cudaStream_t)stream;
-  free_owned(m);
+  m->free_all();
+  m->pos_cache.clear();
   m->finalized = false;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, mw = c.mapping_width;
@@ -842,7 +760,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     m->n_fold = (int)descs.size();
     m->fold_descs = nullptr;
     if (!descs.empty()) {
-      if ((rc = dev_alloc(m, &m->fold_descs, descs.size()))) return rc;
+      if ((rc = m->alloc(&m->fold_descs, descs.size()))) return rc;
       KDB_CUDA(cudaMemcpyAsync(m->fold_descs, descs.data(), descs.size() * sizeof(FoldDesc), cudaMemcpyHostToDevice, st));
       KDB_CUDA(cudaStreamSynchronize(st));
     }
@@ -863,19 +781,19 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
 
   m->patch_in_wb = nullptr;
   if (c.in_channels == 3 && c.patch_h == 4 && c.patch_w == 4 && C0 % 128 == 0) {
-    if ((rc = dev_alloc(m, &m->patch_in_wb, (size_t)C0 * 64))) return rc;
+    if ((rc = m->alloc(&m->patch_in_wb, (size_t)C0 * 64))) return rc;
     if ((rc = prepare_patch_in_weight(m->patch_in_w, m->patch_in_wb, C0, st))) return rc;
   }
   m->patch_out_wb = nullptr;
   m->patch_out_wf = nullptr;
   if (Np <= 64) {   // zero-padded bf16 patch_out weight [64, C0]
-    if ((rc = dev_alloc(m, &m->patch_out_wb, (size_t)64 * C0))) return rc;
+    if ((rc = m->alloc(&m->patch_out_wb, (size_t)64 * C0))) return rc;
     KDB_CUDA(cudaMemsetAsync(m->patch_out_wb, 0, (size_t)64 * C0 * sizeof(bf16), st));
     if ((rc = launch_f32_to_bf16(m->patch_out_w, m->patch_out_wb, (int64_t)Np * C0, st))) return rc;
     if (C0 % 8 == 0) {   // out_norm.scale is a plain parameter: fold it once
       FoldDesc* d1 = nullptr;
-      if ((rc = dev_alloc(m, &m->patch_out_wf, (size_t)64 * C0))) return rc;
-      if ((rc = dev_alloc(m, &d1, 1))) return rc;
+      if ((rc = m->alloc(&m->patch_out_wf, (size_t)64 * C0))) return rc;
+      if ((rc = m->alloc(&d1, 1))) return rc;
       const FoldDesc hd{m->patch_out_wb, m->patch_out_wf, 64, C0, 0};
       KDB_CUDA(cudaMemcpyAsync(d1, &hd, sizeof(FoldDesc), cudaMemcpyHostToDevice, st));
       if ((rc = launch_fold_norm_weights(d1, 1, m->out_norm, st))) return rc;
@@ -906,7 +824,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     GET(p + "down_proj.weight", &w.blk_down[i], mw, c.mapping_d_ff);
   }
   // concatenated AdaRMSNorm projection [ada_total, mw]
-  if ((rc = dev_alloc(m, &m->ada_cat, (size_t)ada * mw))) return rc;
+  if ((rc = m->alloc(&m->ada_cat, (size_t)ada * mw))) return rc;
   for (const LayerPlan& L : m->layers) {
     if (L.ada_attn >= 0)
       KDB_CUDA(cudaMemcpyAsync(m->ada_cat + (size_t)L.ada_attn * mw, L.attn_norm_w, sizeof(float) * L.C * mw, cudaMemcpyDeviceToDevice, st));
@@ -938,7 +856,8 @@ int kdb_model_conditioning(KdbModel* m, int rows, const float* sigma, const floa
 size_t kdb_model_workspace_bytes(const KdbModel* m, int precision, int batch, int height, int width) {
   if (!m || batch <= 0 || height <= 0 || width <= 0) return 0;
   Workspace ws;
-  carve(m->cfg, precision, batch, height, width, nullptr, ws);
+  Carver cv(nullptr, 1024);
+  carve(m->cfg, precision, batch, height, width, cv, ws);
   return ws.total;
 }
 
@@ -961,8 +880,8 @@ int check_image(const KdbModel* m, const char* what, int height, int width, floa
 // carve a workspace of `images` token-stream images out of the caller's buffer
 int carve_checked(const KdbModel* m, const char* what, int precision, int images, int height, int width, void* workspace, size_t workspace_bytes,
                   Workspace& ws) {
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 1024));
-  carve(m->cfg, precision, images, height, width, base, ws);
+  Carver cv(workspace, 1024);
+  carve(m->cfg, precision, images, height, width, cv, ws);
   KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "%s: workspace %zu < required %zu", what, workspace_bytes, ws.total);
   return 0;
 }
@@ -982,14 +901,10 @@ int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int wid
   Workspace ws;
   if ((rc = carve_checked(m, "forward", precision, batch, height, width, workspace, workspace_bytes, ws))) return rc;
   if (precision == KDB_PREC_FP32)
-    rc = forward_impl<float>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
-                             (cudaStream_t)stream);
-  else
-    rc = forward_impl<bf16>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
-                            (cudaStream_t)stream);
-  m->tap_out = nullptr;
-  m->tap_name.clear();
-  return rc;
+    return m->disarm_tap(forward_impl<float>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr,
+                                             ws, (cudaStream_t)stream));
+  return m->disarm_tap(forward_impl<bf16>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
+                                          (cudaStream_t)stream));
 }
 
 int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* v, const float* sigma,
@@ -1003,10 +918,8 @@ int kdb_model_forward_jvp(KdbModel* m, int precision, int batch, int height, int
   if (rc) return rc;
   Workspace ws;
   if ((rc = carve_checked(m, "forward_jvp", precision, 2 * batch, height, width, workspace, workspace_bytes, ws))) return rc;
-  rc = forward_impl<float>(m, batch, height, width, x, v, sigma, sigma_data, cond, cond_batch_stride, out, out_tangent, ws, (cudaStream_t)stream);
-  m->tap_out = nullptr;
-  m->tap_name.clear();
-  return rc;
+  return m->disarm_tap(
+      forward_impl<float>(m, batch, height, width, x, v, sigma, sigma_data, cond, cond_batch_stride, out, out_tangent, ws, (cudaStream_t)stream));
 }
 
 int64_t kdb_model_vjp_workspace_bytes(const KdbModel* m, int batch, int height, int width) {
@@ -1028,23 +941,13 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
   if (rc) return rc;
   Workspace ws;
   VjpSpace vs;
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 1024));
-  carve_vjp(m->cfg, batch, height, width, base, ws, vs);
+  carve_vjp(m->cfg, batch, height, width, workspace, ws, vs);
   KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_vjp: workspace %zu < required %zu", workspace_bytes, vs.total);
-  rc = vjp_impl(m, batch, height, width, x, cotangent, sigma, sigma_data, cond, cond_batch_stride, out, grad_x, ws, vs, (cudaStream_t)stream);
-  m->tap_out = nullptr;
-  m->tap_name.clear();
-  return rc;
+  return m->disarm_tap(
+      vjp_impl(m, batch, height, width, x, cotangent, sigma, sigma_data, cond, cond_batch_stride, out, grad_x, ws, vs, (cudaStream_t)stream));
 }
 
-int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) {
-  KDB_REQUIRE(m && name && out && capacity > 0, KDB_ERR_BAD_ARG, "debug_tap: bad argument");
-  m->tap_name = name;
-  m->tap_out = out;
-  m->tap_cap = capacity;
-  m->tap_count = 0;
-  return 0;
-}
+int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }
 
 int64_t kdb_model_tap_count(const KdbModel* m) { return m ? m->tap_count : 0; }
 

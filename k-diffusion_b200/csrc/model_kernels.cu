@@ -8,11 +8,11 @@
 
 #include "attn_sets.cuh"
 #include "model_kernels.cuh"
+#include "simt_tile.cuh"
 
 namespace kdb {
 
 constexpr float kEps = 1e-6f;   // RMSNorm / cosine-sim eps (image_transformer_v2.py:143,378)
-constexpr float kRsqrt2 = 0.70710678118654752440f;
 
 // grid of a grid-stride kernel of 256 threads over n elements
 static unsigned grid_stride_blocks(int64_t n) { return (unsigned)std::min<int64_t>(ceil_div(n, 256), kNumSMs * 16); }
@@ -69,9 +69,7 @@ __device__ __forceinline__ float rope_rotate(const float* v, int d, int e, float
     return d < dr ? x1 * c - x2 * s : x2 * c + x1 * s;
 }
 
-// erf GELU (image_transformer_v2.py:89-95) in the reference's association, 0.5 g (1 + erf(g / sqrt 2))
-__device__ __forceinline__ float gelu_erf(float g) { return 0.5f * g * (1.f + erff(g * kRsqrt2)); }
-// the derivatives' form: gelu = g Phi(g) and slope = Phi(g) + g phi(g)
+// the erf GELU's derivatives' form: gelu = g Phi(g) and slope = Phi(g) + g phi(g)
 __device__ __forceinline__ void gelu_erf_slope(float g, float& gelu, float& slope) {
   const float Phi = 0.5f * (1.f + erff(g * kRsqrt2));
   const float phi = 0.39894228040143267794f * expf(-0.5f * g * g);
@@ -249,9 +247,8 @@ template int launch_rmsnorm<float>(const float*, float*, const float*, int64_t, 
 template int launch_rmsnorm<bf16>(const bf16*, bf16*, const float*, int64_t, int64_t, int64_t, int, cudaStream_t);
 
 // ------------------------------------------------------------------------------------------------
-// SIMT GEMM, C = A W^T, fp32 accumulate.  64x64x16 tiles, 256 threads, 4x4 micro-tile per thread.
+// SIMT GEMM, C = A W^T, fp32 accumulate, on the tile loop of simt_tile.cuh.
 // ------------------------------------------------------------------------------------------------
-constexpr int GBM = 64, GBN = 64, GBK = 16, GPAD = 4;
 
 template <typename T>
 __device__ __forceinline__ void load4(const T* p, bool ok, float (&v)[4]);
@@ -282,20 +279,11 @@ template <typename T, typename TW, int EPI>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(const T* __restrict__ A, const TW* __restrict__ W, T* __restrict__ Cout,
                                                         int64_t M, int N, int K, const T* __restrict__ resid,
                                                         const float* __restrict__ fac, int hc, int wc, int Cf) {
-  __shared__ __align__(16) float As[GBK][GBM + GPAD];
-  __shared__ __align__(16) float Ws[GBK][GBN + GPAD];
+  const int64_t m0 = (int64_t)blockIdx.y * kTileM;
+  const int n0 = blockIdx.x * kTileN;
   const int tid = threadIdx.x;
-  const int64_t m0 = (int64_t)blockIdx.y * GBM;
-  const int n0 = blockIdx.x * GBN;
   const int lr = tid >> 2, lk = (tid & 3) * 4;   // loader: row 0..63, k offset 0,4,8,12
-  const int ty = tid >> 4, tx = tid & 15;
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  for (int k0 = 0; k0 < K; k0 += GBK) {
+  auto fill = [&](int k0, TileSmem& As, TileSmem& Ws) {
     float av[4], wv[4];
     load4<T>(A + (m0 + lr) * K + k0 + lk, (m0 + lr) < M && (k0 + lk) < K, av);
     load4<TW>(W + (int64_t)(n0 + lr) * K + k0 + lk, (n0 + lr) < N && (k0 + lk) < K, wv);
@@ -304,54 +292,31 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const T* __restrict__ A,
       As[lk + i][lr] = av[i];
       Ws[lk + i][lr] = wv[i];
     }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GBK; ++kk) {
-      const float4 a = *reinterpret_cast<const float4*>(&As[kk][ty * 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&Ws[kk][tx * 4]);
-      const float aa[4] = {a.x, a.y, a.z, a.w}, bb[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
+  };
+  simt_tile(m0, n0, M, N, K, fill, [&](int64_t m, int n, float acc) {
+    if constexpr (EPI == EPI_STORE) {
+      Cout[m * N + n] = from_f<T>(acc);
+    } else if constexpr (EPI == EPI_RESID) {
+      Cout[m * N + n] = from_f<T>(acc + to_f(resid[m * N + n]));
+    } else {
+      // TokenSplit: row m = (b, hy, wx) on the coarse grid, column n = (nh, nw, e)
+      int b, hy, wx;
+      token_coords(m, hc, wc, b, hy, wx);
+      const int q = n / Cf, e = n - q * Cf;
+      const int64_t dst = fine_offset(b, hy, wx, q, e, hc, wc, Cf);
+      Cout[dst] = from_f<T>(lerp_like_torch(to_f(resid[dst]), acc, __ldg(fac)));
     }
-    __syncthreads();
-  }
-
-  float facv = 0.f;
-  if constexpr (EPI == EPI_SPLIT_LERP) facv = __ldg(fac);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx * 4 + j;
-      if (n >= N) continue;
-      if constexpr (EPI == EPI_STORE) {
-        Cout[m * N + n] = from_f<T>(acc[i][j]);
-      } else if constexpr (EPI == EPI_RESID) {
-        Cout[m * N + n] = from_f<T>(acc[i][j] + to_f(resid[m * N + n]));
-      } else {
-        // TokenSplit: row m = (b, hy, wx) on the coarse grid, column n = (nh, nw, e)
-        int b, hy, wx;
-        token_coords(m, hc, wc, b, hy, wx);
-        const int q = n / Cf, e = n - q * Cf;
-        const int64_t dst = fine_offset(b, hy, wx, q, e, hc, wc, Cf);
-        Cout[dst] = from_f<T>(lerp_like_torch(to_f(resid[dst]), acc[i][j], facv));
-      }
-    }
-  }
+  });
 }
 
 template <typename T, typename TW>
 int launch_gemm_simt(const T* A, const TW* W, T* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st) {
   KDB_REQUIRE(K % 4 == 0, KDB_ERR_BAD_SHAPE, "gemm_simt: K=%d must be a multiple of 4", K);
   KDB_REQUIRE(M > 0 && N > 0, KDB_ERR_BAD_SHAPE, "gemm_simt: empty problem");
-  dim3 grid((unsigned)ceil_div(N, GBN), (unsigned)ceil_div(M, GBM));
+  dim3 grid((unsigned)ceil_div(N, kTileN), (unsigned)ceil_div(M, kTileM));
   KDB_REQUIRE(grid.y <= 65535u * 16u, KDB_ERR_BAD_SHAPE, "gemm_simt: M too large");
   if (grid.y > 65535u) {   // split M so gridDim.y stays legal
-    const int64_t chunk = 65535LL * GBM;
+    const int64_t chunk = 65535LL * kTileM;
     for (int64_t mo = 0; mo < M; mo += chunk) {
       GemmEpi e2 = epi;
       KDB_REQUIRE(epi.mode != EPI_SPLIT_LERP, KDB_ERR_UNSUPPORTED, "gemm_simt: split-lerp with M > 4M rows");
@@ -898,76 +863,47 @@ int launch_patch_out_jvp(const float* tokens, const float* dtokens, const float*
 // products with it, so scaling the cotangent by a power of two scales the result exactly.
 // ------------------------------------------------------------------------------------------------
 
-// dA[M,K] = dC[M,N] W[N,K] (the input gradient of C = A W^T): W is read along N, so no transposed copy exists.  64x64x16 tiles over
-// (M, K), 256 threads, 4x4 micro-tile per thread, like gemm_simt_kernel.  VJP_UNPATCH_ACC: row m is a coarse token (b, hy, wx) and
+// dA[M,K] = dC[M,N] W[N,K] (the input gradient of C = A W^T): W is read along N, so no transposed copy exists.  The tile loop of
+// simt_tile.cuh over (M, K), reducing over N.  VJP_UNPATCH_ACC: row m is a coarse token (b, hy, wx) and
 // column k = (nh, nw, e); the result is added to the fine token (2hy+nh, 2wx+nw), channel e of out [B, 2hc, 2wc, Cf] -- the inverse
 // of the TokenMerge gather, a bijection, so each element still has one writer.
 template <int EPI>
 __global__ void __launch_bounds__(256) gemm_vjp_kernel(const float* __restrict__ dC, const float* __restrict__ W, float* __restrict__ out,
                                                        int64_t M, int N, int K, int hc, int wc, int Cf) {
-  __shared__ __align__(16) float As[GBK][GBM + GPAD];
-  __shared__ __align__(16) float Ws[GBK][GBN + GPAD];
+  const int64_t m0 = (int64_t)blockIdx.y * kTileM;
+  const int k0 = blockIdx.x * kTileN;
   const int tid = threadIdx.x;
-  const int64_t m0 = (int64_t)blockIdx.y * GBM;
-  const int k0 = blockIdx.x * GBN;
   const int lr = tid >> 2, lk = (tid & 3) * 4;    // dC loader: row 0..63, reduction offset 0,4,8,12
   const int wr = tid >> 4, wc4 = (tid & 15) * 4;  // W loader: reduction row 0..15, column offset 0..60
-  const int ty = tid >> 4, tx = tid & 15;
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  for (int n0 = 0; n0 < N; n0 += GBK) {
+  auto fill = [&](int n0, TileSmem& As, TileSmem& Ws) {
     float av[4], wv[4];
     load4<float>(dC + (m0 + lr) * N + n0 + lk, (m0 + lr) < M && (n0 + lk) < N, av);
     load4<float>(W + (int64_t)(n0 + wr) * K + k0 + wc4, (n0 + wr) < N && (k0 + wc4) < K, wv);
 #pragma unroll
     for (int i = 0; i < 4; ++i) As[lk + i][lr] = av[i];
     *reinterpret_cast<float4*>(&Ws[wr][wc4]) = make_float4(wv[0], wv[1], wv[2], wv[3]);
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < GBK; ++kk) {
-      const float4 a = *reinterpret_cast<const float4*>(&As[kk][ty * 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&Ws[kk][tx * 4]);
-      const float aa[4] = {a.x, a.y, a.z, a.w}, bb[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
+  };
+  simt_tile(m0, k0, M, K, N, fill, [&](int64_t m, int k, float acc) {
+    if constexpr (EPI == VJP_STORE) {
+      out[m * K + k] = acc;
+    } else {
+      int b, hy, wx;
+      token_coords(m, hc, wc, b, hy, wx);
+      const int q = k / Cf, e = k - q * Cf;
+      out[fine_offset(b, hy, wx, q, e, hc, wc, Cf)] += acc;
     }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int k = k0 + tx * 4 + j;
-      if (k >= K) continue;
-      if constexpr (EPI == VJP_STORE) {
-        out[m * K + k] = acc[i][j];
-      } else {
-        int b, hy, wx;
-        token_coords(m, hc, wc, b, hy, wx);
-        const int q = k / Cf, e = k - q * Cf;
-        out[fine_offset(b, hy, wx, q, e, hc, wc, Cf)] += acc[i][j];
-      }
-    }
-  }
+  });
 }
 
 int launch_gemm_vjp(const float* dC, const float* W, float* out, int64_t M, int N, int K, int epi, int hc, int wc, int Cf, cudaStream_t st) {
   KDB_REQUIRE(N % 4 == 0 && K % 4 == 0, KDB_ERR_BAD_SHAPE, "gemm_vjp: N=%d and K=%d must be multiples of 4", N, K);
   KDB_REQUIRE(M > 0, KDB_ERR_BAD_SHAPE, "gemm_vjp: empty problem");
   KDB_REQUIRE(epi == VJP_STORE || (K == 4 * Cf && M % ((int64_t)hc * wc) == 0), KDB_ERR_BAD_SHAPE, "gemm_vjp: bad un-patch geometry");
-  const int64_t chunk = 65535LL * GBM;   // split M so gridDim.y stays legal (whole images per chunk for the un-patch epilogue)
+  const int64_t chunk = 65535LL * kTileM;   // split M so gridDim.y stays legal (whole images per chunk for the un-patch epilogue)
   const int64_t step = epi == VJP_STORE ? chunk : std::max<int64_t>(chunk / ((int64_t)hc * wc), 1) * hc * wc;
   for (int64_t mo = 0; mo < M; mo += step) {
     const int64_t Mi = std::min(step, M - mo);
-    dim3 grid((unsigned)ceil_div(K, GBN), (unsigned)ceil_div(Mi, GBM));
+    dim3 grid((unsigned)ceil_div(K, kTileN), (unsigned)ceil_div(Mi, kTileM));
     KDB_REQUIRE(grid.y <= 65535u, KDB_ERR_BAD_SHAPE, "gemm_vjp: image too large");
     if (epi == VJP_STORE)
       gemm_vjp_kernel<VJP_STORE><<<grid, 256, 0, st>>>(dC + mo * N, W, out + mo * K, Mi, N, K, 0, 0, 0);
@@ -1371,17 +1307,6 @@ __device__ __forceinline__ void block_matvec(const float* __restrict__ W, const 
       if (lane == 0 && oo < o_end) vout[oo] = (accumulate ? vout[oo] : 0.f) + bias + t;
     }
   }
-}
-
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int i = 0; i < nw; ++i) t += red[i];
-  return t;
 }
 
 // y = x * scale * rsqrt(mean(x^2) + eps), vectors in shared memory

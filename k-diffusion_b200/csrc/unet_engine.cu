@@ -7,10 +7,9 @@
 #include <algorithm>
 #include <cmath>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
-#include "model_kernels.cuh"
+#include "model_core.cuh"
 #include "unet_kernels.cuh"
 
 namespace {
@@ -28,74 +27,27 @@ struct UMod {
   bool to_skip = false;           // the last module of a DBlock writes the level's skip buffer
 };
 
-struct TensorRefU {
-  const float* p = nullptr;
-  std::vector<int64_t> shape;
-};
-
 }  // namespace
 
-struct KdbUNet {
+struct KdbUNet : kdb::ModelCore {
   KdbUNetConfig cfg{};
-  std::unordered_map<std::string, TensorRefU> tensors;
-  bool finalized = false;
   std::vector<UMod> mods;
-  std::vector<void*> owned;
   const float *proj_in_w = nullptr, *proj_in_b = nullptr, *proj_out_w = nullptr, *proj_out_b = nullptr;
   int ada_total = 0;
   kdb::UNetCondWeights cw{};
-  std::string tap_name;
-  float* tap_out = nullptr;
-  int64_t tap_cap = 0, tap_count = 0;
 };
 
 using namespace kdb;
 
 namespace {
 
-int uget(KdbUNet* m, const std::string& key, std::vector<int64_t> want, const float** out) {
-  auto it = m->tensors.find(key);
-  if (it == m->tensors.end()) {
-    set_error("missing state-dict entry '%s'", key.c_str());
-    return KDB_ERR_MISSING_KEY;
-  }
-  if (it->second.shape != want) {
-    std::string got, exp;
-    for (auto v : it->second.shape) got += std::to_string(v) + ",";
-    for (auto v : want) exp += std::to_string(v) + ",";
-    set_error("shape mismatch for '%s': got [%s] expected [%s]", key.c_str(), got.c_str(), exp.c_str());
-    return KDB_ERR_BAD_SHAPE;
-  }
-  *out = it->second.p;
-  return 0;
-}
-
-#define UGET(key, out, ...)                                      \
-  do {                                                           \
-    int rc__ = uget(m, (key), {__VA_ARGS__}, (out));             \
-    if (rc__) return rc__;                                       \
-  } while (0)
-
-int ualloc(KdbUNet* m, float** p, size_t count) {
-  void* q = nullptr;
-  KDB_CUDA(cudaMalloc(&q, count * sizeof(float) + 256));
-  m->owned.push_back(q);
-  *p = reinterpret_cast<float*>(q);
-  return 0;
-}
-
-void ufree(KdbUNet* m) {
-  for (void* p : m->owned) cudaFree(p);
-  m->owned.clear();
-}
-
 // owned tap-major copy of a conv weight [N, C, ks, ks]; the first scaled_rows output rows times scale
 int conv_weight(KdbUNet* m, const std::string& key, int N, int C, int ks, const float** out, cudaStream_t st, int scaled_rows = 0,
                 float scale = 1.f) {
   const float* src;
-  UGET(key, &src, N, C, ks, ks);
+  GET(key, &src, N, C, ks, ks);
   float* dst = nullptr;
-  int rc = ualloc(m, &dst, (size_t)N * C * ks * ks);
+  int rc = m->alloc(&dst, (size_t)N * C * ks * ks);
   if (rc || (rc = launch_unet_reorder_conv_weight(src, dst, N, C, ks, scaled_rows, scale, st))) return rc;
   *out = dst;
   return 0;
@@ -103,9 +55,9 @@ int conv_weight(KdbUNet* m, const std::string& key, int N, int C, int ks, const 
 
 int bias_copy(KdbUNet* m, const std::string& key, int N, const float** out, cudaStream_t st, int scaled_rows = 0, float scale = 1.f) {
   const float* src;
-  UGET(key, &src, N);
+  GET(key, &src, N);
   float* dst = nullptr;
-  int rc = ualloc(m, &dst, (size_t)N);
+  int rc = m->alloc(&dst, (size_t)N);
   if (rc || (rc = launch_unet_reorder_conv_weight(src, dst, N, 1, 1, scaled_rows, scale, st))) return rc;
   *out = dst;
   return 0;
@@ -114,8 +66,8 @@ int bias_copy(KdbUNet* m, const std::string& key, int N, const float** out, cuda
 // AdaGN mapper of `prefix` (Linear feats_in -> 2C with bias): bound and given the next offset of the conditioning row
 int mapper(KdbUNet* m, const std::string& prefix, int C, const float** w, const float** b, int* off) {
   const int mw = m->cfg.mapping_out;
-  UGET(prefix + "mapper.weight", w, 2 * C, mw);
-  UGET(prefix + "mapper.bias", b, 2 * C);
+  GET(prefix + "mapper.weight", w, 2 * C, mw);
+  GET(prefix + "mapper.bias", b, 2 * C);
   *off = m->ada_total;
   m->ada_total += 2 * C;
   return 0;
@@ -178,17 +130,6 @@ int plan_block(KdbUNet* m, const std::string& p, int level, const char* tag, int
   return 0;
 }
 
-int tap(KdbUNet* m, const std::string& name, const float* p, int64_t n, cudaStream_t st) {
-  if (m->tap_out == nullptr || m->tap_name != name) return 0;
-  if (n > m->tap_cap) {
-    m->tap_count = -n;
-    return 0;
-  }
-  m->tap_count = n;
-  KDB_CUDA(cudaMemcpyAsync(m->tap_out, p, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
-
 // Workspace: the skip buffer of every level, then seven working buffers of `elems` floats each (two for the block stream, the
 // AdaGN output, the first conv's output, the skip conv's output, qkv and the attention output).
 struct UWs {
@@ -206,13 +147,9 @@ void level_dims(const KdbUNetConfig& c, int H, int W, int l, int* h, int* w) {
   }
 }
 
-void ucarve(const KdbUNetConfig& c, int B, int H, int W, char* base, UWs& ws) {
-  size_t off = 0;
-  auto take = [&](size_t floats) {
-    float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-    off += align_up(floats * sizeof(float), 256);
-    return p;
-  };
+void carve(const KdbUNetConfig& c, int B, int H, int W, void* workspace, UWs& ws) {
+  Carver cv(workspace, 256);
+  auto take = [&](size_t floats) { return cv.take<float>(floats * sizeof(float)); };
   size_t elems = 0;
   for (int l = c.skip_stages; l < c.n_levels; ++l) {
     int h, w;
@@ -229,7 +166,7 @@ void ucarve(const KdbUNetConfig& c, int B, int H, int W, char* base, UWs& ws) {
   ws.s = take(elems);
   ws.qkv = take(elems);
   ws.ao = take(elems);
-  ws.total = off + 256;
+  ws.total = cv.total();
 }
 
 // the block input: one tensor, or a tensor and the matching skip (the UBlock concat)
@@ -285,7 +222,7 @@ int unet_forward(KdbUNet* m, int B, int H, int W, const float* x, const float* s
   int h, w, rc;
   level_dims(c, H, W, s0, &h, &w);
   if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, ws.x[0], B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
-  if ((rc = tap(m, "patch_in", ws.x[0], (int64_t)B * h * w * C0, st))) return rc;
+  if ((rc = m->tap("patch_in", ws.x[0], (int64_t)B * h * w * C0, st))) return rc;
   Src cur{ws.x[0], C0, nullptr, 0};
   int cur_buf = 0;                         // index of the ping-pong buffer holding cur (-1: a skip buffer)
   for (const UMod& u : m->mods) {
@@ -310,7 +247,7 @@ int unet_forward(KdbUNet* m, int B, int H, int W, const float* x, const float* s
       default:
         if ((rc = run_attn(m, u, cur.p1, dst, ws, B, h, w, cond, cbs, st))) return rc;
     }
-    if ((rc = tap(m, u.tap, dst, (int64_t)B * h * w * C, st))) return rc;
+    if ((rc = m->tap(u.tap, dst, (int64_t)B * h * w * C, st))) return rc;
     cur = Src{dst, C, nullptr, 0};
     cur_buf = u.to_skip ? -1 : nb;
   }
@@ -340,25 +277,18 @@ int kdb_unet_create(const KdbUNetConfig* cfg, KdbUNet** out) {
 
 int kdb_unet_destroy(KdbUNet* m) {
   KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_destroy: NULL handle");
-  ufree(m);
   delete m;
   return 0;
 }
 
 int kdb_unet_set_tensor(KdbUNet* m, const char* key, const float* data, const int64_t* shape, int ndim) {
-  KDB_REQUIRE(m && key && data && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "unet_set_tensor: bad argument");
-  TensorRefU t;
-  t.p = data;
-  t.shape.assign(shape, shape + ndim);
-  m->tensors[key] = t;
-  m->finalized = false;
-  return 0;
+  return set_tensor(m, key, data, shape, ndim);
 }
 
 int kdb_unet_finalize(KdbUNet* m, void* stream) {
   KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_finalize: NULL handle");
   cudaStream_t st = (cudaStream_t)stream;
-  ufree(m);
+  m->free_all();
   m->finalized = false;
   m->mods.clear();
   m->ada_total = 0;
@@ -393,22 +323,22 @@ int kdb_unet_finalize(KdbUNet* m, void* stream) {
     }
   }
   const int Kin = c.in_channels * c.patch_size * c.patch_size, Kout = Kin + (c.has_variance ? 1 : 0);
-  UGET("proj_in.weight", &m->proj_in_w, C0, Kin, 1, 1);
-  UGET("proj_in.bias", &m->proj_in_b, C0);
-  UGET("proj_out.weight", &m->proj_out_w, Kout, C0, 1, 1);
-  UGET("proj_out.bias", &m->proj_out_b, Kout);
+  GET("proj_in.weight", &m->proj_in_w, C0, Kin, 1, 1);
+  GET("proj_in.bias", &m->proj_in_b, C0);
+  GET("proj_out.weight", &m->proj_out_w, Kout, C0, 1, 1);
+  GET("proj_out.bias", &m->proj_out_b, Kout);
   // conditioning weights and the concatenated AdaGN mappers
   UNetCondWeights& w = m->cw;
   w = UNetCondWeights{};
   w.mw = mw, w.mcond_dim = c.mapping_cond_dim, w.augment = c.augment_wrapper, w.ada_total = m->ada_total;
-  UGET("timestep_embed.weight", &w.time_emb, mw / 2, 1);
-  if (c.mapping_cond_dim > 0) UGET("mapping_cond.weight", &w.mcond_w, mw, c.mapping_cond_dim);
-  UGET("mapping.0.weight", &w.map_w0, mw, mw);
-  UGET("mapping.0.bias", &w.map_b0, mw);
-  UGET("mapping.2.weight", &w.map_w1, mw, mw);
-  UGET("mapping.2.bias", &w.map_b1, mw);
+  GET("timestep_embed.weight", &w.time_emb, mw / 2, 1);
+  if (c.mapping_cond_dim > 0) GET("mapping_cond.weight", &w.mcond_w, mw, c.mapping_cond_dim);
+  GET("mapping.0.weight", &w.map_w0, mw, mw);
+  GET("mapping.0.bias", &w.map_b0, mw);
+  GET("mapping.2.weight", &w.map_w1, mw, mw);
+  GET("mapping.2.bias", &w.map_b1, mw);
   float *aw, *ab;
-  if ((rc = ualloc(m, &aw, (size_t)m->ada_total * mw)) || (rc = ualloc(m, &ab, (size_t)m->ada_total))) return rc;
+  if ((rc = m->alloc(&aw, (size_t)m->ada_total * mw)) || (rc = m->alloc(&ab, (size_t)m->ada_total))) return rc;
   for (const UMod& u : m->mods) {
     const int n_ada = u.kind == M_RES ? 2 : (u.kind == M_ATTN ? 1 : 0);
     for (int i = 0; i < n_ada; ++i) {
@@ -445,7 +375,7 @@ int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int
   KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "unet_workspace_bytes: bad argument");
   KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "unet_workspace_bytes: only the fp32 path is built (precision %d)", precision);
   UWs ws;
-  ucarve(m->cfg, batch, height, width, nullptr, ws);
+  carve(m->cfg, batch, height, width, nullptr, ws);
   return (int64_t)ws.total;
 }
 
@@ -465,23 +395,12 @@ int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width
                 "unet_forward: level %d grid %dx%d (every level but the innermost needs an even grid, every level >= 2x2)", l, h, w);
   }
   UWs ws;
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace), 256));
-  ucarve(c, batch, height, width, base, ws);
+  carve(c, batch, height, width, workspace, ws);
   KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward: workspace %zu < required %zu", workspace_bytes, ws.total);
-  const int rc = unet_forward(m, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream);
-  m->tap_out = nullptr;
-  m->tap_name.clear();
-  return rc;
+  return m->disarm_tap(unet_forward(m, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream));
 }
 
-int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) {
-  KDB_REQUIRE(m && name && out && capacity > 0, KDB_ERR_BAD_ARG, "unet_debug_tap: bad argument");
-  m->tap_name = name;
-  m->tap_out = out;
-  m->tap_cap = capacity;
-  m->tap_count = 0;
-  return 0;
-}
+int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }
 
 int64_t kdb_unet_tap_count(const KdbUNet* m) {
   KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_tap_count: NULL handle");

@@ -1,6 +1,7 @@
 // unet_kernels.cu -- fp32 kernels of the image_v1 U-Net engine (unet_engine.cu).  Token-major activations [B, H, W, C].
 #include <cmath>
 
+#include "simt_tile.cuh"
 #include "unet_kernels.cuh"
 
 namespace kdb {
@@ -8,26 +9,18 @@ namespace kdb {
 namespace {
 
 constexpr float kGnEps = 1e-5f;                 // AdaGN eps (layers.py:163)
-constexpr float kRsqrt2U = 0.70710678118654752f;
-
-__device__ __forceinline__ float gelu_erf_u(float g) { return 0.5f * g * (1.f + erff(g * kRsqrt2U)); }
 
 // ------------------------------------------------------------------------------------------------
-// implicit-GEMM convolution: 64x64x16 tiles, 256 threads, 4x4 micro-tile per thread (the SIMT GEMM's tiling)
+// implicit-GEMM convolution on the SIMT GEMM's tile loop (simt_tile.cuh), A gathered per tap
 // ------------------------------------------------------------------------------------------------
-constexpr int CBM = 64, CBN = 64, CBK = 16, CPAD = 4;
-
 template <int KS>
 __global__ void __launch_bounds__(256) unet_conv_kernel(const ConvArgs a) {
-  __shared__ __align__(16) float As[CBK][CBM + CPAD];
-  __shared__ __align__(16) float Ws[CBK][CBN + CPAD];
-  const int tid = threadIdx.x;
   const int64_t M = (int64_t)a.B * a.H * a.W;
   const int Ct = a.c1 + a.c2, K = KS * KS * Ct, N = a.N;
-  const int64_t m0 = (int64_t)blockIdx.y * CBM;
-  const int n0 = blockIdx.x * CBN;
+  const int64_t m0 = (int64_t)blockIdx.y * kTileM;
+  const int n0 = blockIdx.x * kTileN;
+  const int tid = threadIdx.x;
   const int lr = tid >> 2, lk = (tid & 3) * 4;   // loader: row 0..63, k offset 0,4,8,12
-  const int ty = tid >> 4, tx = tid & 15;
   // pixel of the A row this thread loads
   const int64_t am = m0 + lr;
   const bool arow = am < M;
@@ -37,13 +30,7 @@ __global__ void __launch_bounds__(256) unet_conv_kernel(const ConvArgs a) {
     ay = r / a.W;
     ax = r - ay * a.W;
   }
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  for (int k0 = 0; k0 < K; k0 += CBK) {
+  auto fill = [&](int k0, TileSmem& As, TileSmem& Ws) {
     const int k = k0 + lk;
     float4 av = make_float4(0.f, 0.f, 0.f, 0.f), wv = make_float4(0.f, 0.f, 0.f, 0.f);
     if (arow && k < K) {
@@ -58,50 +45,17 @@ __global__ void __launch_bounds__(256) unet_conv_kernel(const ConvArgs a) {
     if (n0 + lr < N && k < K) wv = __ldg(reinterpret_cast<const float4*>(a.w + (int64_t)(n0 + lr) * K + k));
     As[lk + 0][lr] = av.x; As[lk + 1][lr] = av.y; As[lk + 2][lr] = av.z; As[lk + 3][lr] = av.w;
     Ws[lk + 0][lr] = wv.x; Ws[lk + 1][lr] = wv.y; Ws[lk + 2][lr] = wv.z; Ws[lk + 3][lr] = wv.w;
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < CBK; ++kk) {
-      const float4 x = *reinterpret_cast<const float4*>(&As[kk][ty * 4]);
-      const float4 y = *reinterpret_cast<const float4*>(&Ws[kk][tx * 4]);
-      const float aa[4] = {x.x, x.y, x.z, x.w}, bb[4] = {y.x, y.y, y.z, y.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(aa[i], bb[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx * 4 + j;
-      if (n >= N) continue;
-      float v = acc[i][j];
-      if (a.bias != nullptr) v += __ldg(a.bias + n);
-      if (a.r1 != nullptr) v += n < a.rc1 ? a.r1[m * a.rc1 + n] : a.r2[m * (N - a.rc1) + (n - a.rc1)];
-      a.out[m * N + n] = v;
-    }
-  }
+  };
+  simt_tile(m0, n0, M, N, K, fill, [&](int64_t m, int n, float v) {
+    if (a.bias != nullptr) v += __ldg(a.bias + n);
+    if (a.r1 != nullptr) v += n < a.rc1 ? a.r1[m * a.rc1 + n] : a.r2[m * (N - a.rc1) + (n - a.rc1)];
+    a.out[m * N + n] = v;
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
 // AdaGN (+ GELU): one CTA per (group, image)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float block_sum_u(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = 0.f;
-  for (int i = 0; i < nw; ++i) t += red[i];
-  return t;
-}
-
 __global__ void __launch_bounds__(256) unet_adagn_kernel(const float* __restrict__ in1, int c1, const float* __restrict__ in2, int c2,
                                                          float* __restrict__ out, const float* __restrict__ cond, int64_t cond_bs, int ada_off,
                                                          int groups, int gelu, int HW) {
@@ -122,7 +76,7 @@ __global__ void __launch_bounds__(256) unet_adagn_kernel(const float* __restrict
     int64_t pix;
     s += load(i, c, pix);
   }
-  const float mean = block_sum_u(s, red) / (float)n;
+  const float mean = block_sum(s, red) / (float)n;
   float q = 0.f;
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
     int c;
@@ -130,14 +84,14 @@ __global__ void __launch_bounds__(256) unet_adagn_kernel(const float* __restrict
     const float d = load(i, c, pix) - mean;
     q = fmaf(d, d, q);
   }
-  const float rstd = rsqrtf(block_sum_u(q, red) / (float)n + kGnEps);
+  const float rstd = rsqrtf(block_sum(q, red) / (float)n + kGnEps);
   const float* row = cond + (int64_t)b * cond_bs + ada_off;
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
     int c;
     int64_t pix;
     const float v = (load(i, c, pix) - mean) * rstd;
     float y = fmaf(v, __ldg(row + c) + 1.f, __ldg(row + C + c));
-    if (gelu) y = gelu_erf_u(y);
+    if (gelu) y = gelu_erf(y);
     out[pix * C + c] = y;
   }
 }
@@ -259,7 +213,7 @@ __device__ __forceinline__ void warp_matvec(const float* __restrict__ W, const f
     s = warp_sum(s);
     if (lane == 0) {
       float v = s + (bias ? __ldg(bias + o) : 0.f);
-      vout[o] = gelu ? gelu_erf_u(v) : v;
+      vout[o] = gelu ? gelu_erf(v) : v;
     }
   }
 }
@@ -328,7 +282,7 @@ int launch_unet_conv(const ConvArgs& a, int ks, cudaStream_t st) {
               "unet_conv: channel counts %d + %d must be multiples of 4", a.c1, a.c2);
   KDB_REQUIRE(!a.r1 || a.rc1 == a.N || (a.r2 && a.rc1 < a.N), KDB_ERR_BAD_ARG, "unet_conv: bad residual split");
   const int64_t M = (int64_t)a.B * a.H * a.W;
-  dim3 grid((unsigned)ceil_div(a.N, CBN), (unsigned)ceil_div(M, CBM));
+  dim3 grid((unsigned)ceil_div(a.N, kTileN), (unsigned)ceil_div(M, kTileM));
   KDB_REQUIRE(grid.y <= 65535u, KDB_ERR_BAD_SHAPE, "unet_conv: %lld pixels exceed the grid", (long long)M);
   if (ks == 3)
     unet_conv_kernel<3><<<grid, 256, 0, st>>>(a);

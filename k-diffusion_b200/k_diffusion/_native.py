@@ -4,6 +4,7 @@ There is deliberately NO fallback: if the shared library is missing or a tensor 
 device the call raises.  PyTorch is used only for device memory, streams and views.
 """
 import contextlib
+import copy
 import ctypes
 import math
 import functools
@@ -338,15 +339,52 @@ def noise_brownian(like, seeds, t_min, t_max, t0, t1, depth=24, out=None):
 _ATTN_CODE = {"none": ATTN_NONE, "global": ATTN_GLOBAL, "neighborhood": ATTN_NEIGHBORHOOD, "shifted-window": ATTN_SHIFTED_WINDOW}
 
 
-class Engine:
-    """Owns one KdbModel handle for one ImageTransformerDenoiserModelV2 instance on one device."""
+UNET_NO_DERIVATIVE = "the image_v1 U-Net engine has no derivative: only its fp32 forward is built (no JVP, VJP or autograd through x)"
 
-    _api = "model"          # kdb_<api>_set_tensor / _finalize / _cond_stride / _debug_tap / _tap_count
+
+def unet_has_no_derivative(*args, **kwargs):
+    """What every derivative entry point of the U-Net does (the engine, the model and the augment wrapper's view of it)."""
+    raise NotImplementedError(UNET_NO_DERIVATIVE)
+
+
+class EngineCache:
+    """Base of the model classes that keep their native engines in self._engines ({key: Engine}).  An engine holds device pointers into
+    the model's own tensors, so a pickled or deep-copied model starts without engines and builds its own on first use."""
+
+    def __getstate__(self):
+        state = self.__dict__.copy()
+        state["_engines"] = {}
+        return state
+
+    def __deepcopy__(self, memo):
+        engines, self._engines = self._engines, {}
+        try:
+            new = self.__class__.__new__(self.__class__)
+            memo[id(self)] = new
+            new.__dict__ = copy.deepcopy(self.__dict__, memo)
+        finally:
+            self._engines = engines
+        return new
+
+
+class Engine:
+    """Owns one native model handle on one device: a KdbModel for an ImageTransformerDenoiserModelV2 (`_api` "model"), or, in the
+    UNetEngine subclass, a KdbUNet for an ImageDenoiserModelV1 (`_api` "unet").  Both handles take the same calls (create, destroy,
+    set_tensor, finalize, cond_stride, workspace_bytes, forward, debug_tap, tap_count) under kdb_<api>_*."""
+
+    _api = "model"
 
     def _fn(self, name):
         return getattr(lib(), f"kdb_{self._api}_{name}")
 
     def __init__(self, spec):
+        self.cfg = self._config(spec)
+        self._h = _vp()
+        check(self._fn("create")(ctypes.byref(self.cfg), ctypes.byref(self._h)))
+        self._sig, self._held, self._ws, self._stride, self.device = None, {}, None, None, None
+
+    @staticmethod
+    def _config(spec):
         cfg = KdbModelConfig()
         levels = spec["levels"]
         if len(levels) > MAX_LEVELS:
@@ -361,19 +399,15 @@ class Engine:
             cfg.attn_type[i] = _ATTN_CODE[lv["attn"]]
             cfg.d_head[i] = lv.get("d_head", 0)
             cfg.attn_param[i] = lv.get("attn_param", 0)
-        self.cfg = cfg
-        self._h = _vp()
-        check(lib().kdb_model_create(ctypes.byref(cfg), ctypes.byref(self._h)))
-        self._sig = None
-        self._held = {}
-        self._ws = None
-        self._stride = None
-        self.device = None
+        return cfg
+
+    def _out_channels(self, x):
+        return self.cfg.out_channels
 
     def __del__(self):
         try:
             if getattr(self, "_h", None) and _lib is not None:
-                _lib.kdb_model_destroy(self._h)
+                getattr(_lib, f"kdb_{self._api}_destroy")(self._h)
                 self._h = None
         except Exception:
             pass
@@ -427,9 +461,15 @@ class Engine:
         if lo < 0 or hi >= n:
             raise IndexError(f"class_cond values must lie in [0, {n}) (class_emb has {n} rows), got [{lo}, {hi}]")
 
+    def workspace_bytes(self, precision, B, H, W):
+        """kdb_<api>_workspace_bytes: the workspace of a forward of B images"""
+        need = int(self._fn("workspace_bytes")(self._h, precision, B, H, W))
+        if need < 0:
+            check(need)
+        return need
+
     def _workspace(self, precision, B, H, W, device):
-        """The workspace of a forward of B images (kdb_model_workspace_bytes)."""
-        return self._reserve(lib().kdb_model_workspace_bytes(self._h, precision, B, H, W), device)
+        return self._reserve(self.workspace_bytes(precision, B, H, W), device)
 
     def _reserve(self, need, device):
         """The engine's workspace of at least `need` bytes on `device`, grown and reused across calls."""
@@ -445,11 +485,11 @@ class Engine:
         """x [B,C,H,W] fp32; sigma [B]; cond rows; sigma_data <= 0 -> raw inner model."""
         B, _, H, W = x.shape
         if out is None:
-            out = torch.empty(B, self.cfg.out_channels, H, W, device=x.device, dtype=torch.float32)
+            out = torch.empty(B, self._out_channels(x), H, W, device=x.device, dtype=torch.float32)
         ws = self._workspace(precision, B, H, W, x.device)
         with device_of(x):
-            check(lib().kdb_model_forward(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
-                                          ptr(out), ptr(ws), ws.numel(), stream()))
+            check(self._fn("forward")(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
+                                      ptr(out), ptr(ws), ws.numel(), stream()))
         return out
 
     def forward_jvp(self, x, v, sigma, cond, cond_batch_stride, sigma_data, out=None, out_tangent=None):
@@ -492,14 +532,12 @@ class Engine:
 
 
 class UNetEngine(Engine):
-    """Owns one KdbUNet handle (the image_v1 U-Net on the exact fp32 path) for one ImageDenoiserModelV1 on one device.
-
-    Same interface as Engine where the sampler executor calls it (bind, cond_stride, conditioning, forward, taps); the
-    derivative entry points do not exist for the U-Net."""
+    """The image_v1 U-Net on the exact fp32 path: the Engine calls where the sampler executor makes them; no derivatives."""
 
     _api = "unet"
 
-    def __init__(self, spec):
+    @staticmethod
+    def _config(spec):
         cfg = KdbUNetConfig()
         n = len(spec["depths"])
         if n > MAX_LEVELS:
@@ -509,18 +547,10 @@ class UNetEngine(Engine):
         cfg.skip_stages, cfg.has_variance = spec["skip_stages"], int(spec["has_variance"])
         for i in range(n):
             cfg.depth[i], cfg.channels[i], cfg.self_attn[i] = spec["depths"][i], spec["channels"][i], int(bool(spec["self_attn_depths"][i]))
-        self.cfg = cfg
-        self._h = _vp()
-        check(lib().kdb_unet_create(ctypes.byref(cfg), ctypes.byref(self._h)))
-        self._sig, self._held, self._ws, self._stride, self.device = None, {}, None, None, None
+        return cfg
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None) and _lib is not None:
-                _lib.kdb_unet_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+    def _out_channels(self, x):
+        return x.shape[1]
 
     def conditioning(self, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
         """-> [rows, cond_stride] fp32 table (mapping net + every AdaGN's (weight, bias))."""
@@ -536,28 +566,7 @@ class UNetEngine(Engine):
             check(lib().kdb_unet_conditioning(self._h, rows, ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(out), stream()))
         return out
 
-    def workspace_bytes(self, precision, B, H, W):
-        need = int(lib().kdb_unet_workspace_bytes(self._h, precision, B, H, W))
-        if need < 0:
-            check(need)
-        return need
-
-    def forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
-        """x [B,C,H,W] fp32; sigma [B]; cond rows; sigma_data <= 0 -> raw inner model."""
-        B, C, H, W = x.shape
-        if out is None:
-            out = torch.empty(B, C, H, W, device=x.device, dtype=torch.float32)
-        ws = self._reserve(self.workspace_bytes(precision, B, H, W), x.device)
-        with device_of(x):
-            check(lib().kdb_unet_forward(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
-                                         ptr(out), ptr(ws), ws.numel(), stream()))
-        return out
-
-    def forward_jvp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no forward-mode derivative (only its fp32 forward is built)")
-
-    def forward_vjp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no reverse-mode derivative (only its fp32 forward is built)")
+    forward_jvp = forward_vjp = unet_has_no_derivative
 
 
 # ---------------------------------------------------------------------------------------------

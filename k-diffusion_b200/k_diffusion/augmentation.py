@@ -2,6 +2,7 @@
 import torch
 from torch import nn
 
+from . import _native
 from .models.image_v1 import ImageDenoiserModelV1
 
 
@@ -74,8 +75,4 @@ class _UNetView:
     def denoise(self, x, sigma, sigma_data, aug_cond=None, mapping_cond=None, out=None):
         return self.unet.run(x, sigma, float(sigma_data), True, aug_cond, mapping_cond, out=out)
 
-    def denoise_jvp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no forward-mode derivative (only its fp32 forward is built)")
-
-    def denoise_vjp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no reverse-mode derivative (only its fp32 forward is built)")
+    denoise_jvp = denoise_vjp = _native.unet_has_no_derivative

@@ -127,7 +127,7 @@ def _level(spec, cond_width):
     return nn.ModuleList([_layer(spec, cond_width) for _ in range(spec.depth)])
 
 
-class ImageTransformerDenoiserModelV2(nn.Module):
+class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
     def __init__(self, levels, mapping, in_channels, out_channels, patch_size, num_classes=0, mapping_cond_dim=0):
         super().__init__()
         levels = list(levels)
@@ -164,26 +164,9 @@ class ImageTransformerDenoiserModelV2(nn.Module):
         self.patch_out = _Node(proj=_linear(out_channels * n_patch, w0, zero=True))
 
         self.precision = None        # None -> flags.resolve_precision ("auto" unless KDB200_PRECISION is set)
-        self._engine_obj = None
+        self._engines = {}
 
     # ------------------------------------------------------------------ engine plumbing
-    def __getstate__(self):
-        state = self.__dict__.copy()
-        state["_engine_obj"] = None
-        return state
-
-    def __deepcopy__(self, memo):
-        import copy
-        eng, self._engine_obj = self._engine_obj, None
-        try:
-            cls = self.__class__
-            new = cls.__new__(cls)
-            memo[id(self)] = new
-            new.__dict__ = copy.deepcopy(self.__dict__, memo)
-        finally:
-            self._engine_obj = eng
-        return new
-
     def engine_spec(self):
         lv = []
         for s in self.levels:
@@ -195,11 +178,11 @@ class ImageTransformerDenoiserModelV2(nn.Module):
 
     def engine(self):
         """Native engine with the current parameters bound (rebinds only after the parameters changed)."""
-        if self._engine_obj is None:
-            self._engine_obj = _native.Engine(self.engine_spec())
-        tensors = dict(self.state_dict(keep_vars=True))
-        self._engine_obj.bind(tensors)
-        return self._engine_obj
+        eng = self._engines.get(None)
+        if eng is None:
+            eng = self._engines[None] = _native.Engine(self.engine_spec())
+        eng.bind(dict(self.state_dict(keep_vars=True)))
+        return eng
 
     def set_precision(self, precision):
         """'fp32' (exact path, parity gate), 'bf16' (tensor-core path) or None/'auto'."""

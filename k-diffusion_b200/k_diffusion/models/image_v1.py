@@ -109,7 +109,7 @@ class UNet(nn.Module):
         self.skip_stages = skip_stages
 
 
-class ImageDenoiserModelV1(nn.Module):
+class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
     def __init__(self, c_in, feats_in, depths, channels, self_attn_depths, cross_attn_depths=None, mapping_cond_dim=0, unet_cond_dim=0,
                  cross_cond_dim=0, dropout_rate=0., patch_size=1, skip_stages=0, has_variance=False):
         super().__init__()
@@ -139,35 +139,21 @@ class ImageDenoiserModelV1(nn.Module):
         self._engines = {}
 
     # ------------------------------------------------------------------ engine plumbing
-    def __getstate__(self):
-        state = self.__dict__.copy()
-        state["_engines"] = {}
-        return state
-
-    def __deepcopy__(self, memo):
-        import copy
-        engines, self._engines = self._engines, {}
-        try:
-            new = self.__class__.__new__(self.__class__)
-            memo[id(self)] = new
-            new.__dict__ = copy.deepcopy(self.__dict__, memo)
-        finally:
-            self._engines = engines
-        return new
-
     @property
     def levels(self):
         """per-level dropout (what the sampler executor checks before running the inference-only engine)"""
         return [SimpleNamespace(dropout=self.dropout_rate)] * len(self.depths)
 
+    def engine_spec(self, augment):
+        return dict(c_in=self.c_in, feats_in=self.feats_in, depths=self.depths, channels=self.channels, self_attn_depths=self.self_attn_depths,
+                    mapping_cond_dim=self.mapping_cond_dim, augment=augment, patch_size=self.patch_size, skip_stages=self.u_net.skip_stages,
+                    has_variance=self.has_variance)
+
     def engine(self, augment=False):
         """Native engine with the current parameters bound; `augment`: conditioning as KarrasAugmentWrapper forms it."""
         eng = self._engines.get(augment)
         if eng is None:
-            eng = self._engines[augment] = _native.UNetEngine(dict(
-                c_in=self.c_in, feats_in=self.feats_in, depths=self.depths, channels=self.channels, self_attn_depths=self.self_attn_depths,
-                mapping_cond_dim=self.mapping_cond_dim, augment=augment, patch_size=self.patch_size, skip_stages=self.u_net.skip_stages,
-                has_variance=self.has_variance))
+            eng = self._engines[augment] = _native.UNetEngine(self.engine_spec(augment))
         eng.bind(dict(self.state_dict(keep_vars=True)))
         return eng
 
@@ -201,11 +187,7 @@ class ImageDenoiserModelV1(nn.Module):
         """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
         return self.run(x, sigma, float(sigma_data), False, mapping_cond=mapping_cond, out=out)
 
-    def denoise_jvp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no forward-mode derivative (only its fp32 forward is built)")
-
-    def denoise_vjp(self, *args, **kwargs):
-        raise NotImplementedError("the image_v1 U-Net engine has no reverse-mode derivative (only its fp32 forward is built)")
+    denoise_jvp = denoise_vjp = _native.unet_has_no_derivative
 
     # ------------------------------------------------------------------ forward
     def user_mapping_cond_dim(self, augment):
@@ -227,8 +209,7 @@ class ImageDenoiserModelV1(nn.Module):
         if self.training and self.dropout_rate > 0:
             raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
         if torch.is_grad_enabled() and x.requires_grad:
-            raise NotImplementedError("the image_v1 U-Net engine has no derivative: only its fp32 forward is built, so autograd cannot "
-                                      "reach x")
+            _native.unet_has_no_derivative()
         if aug_cond is not None and not augment:
             raise TypeError("aug_cond needs the KarrasAugmentWrapper")
         self.check_cond(augment, None, mapping_cond)

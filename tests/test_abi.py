@@ -66,6 +66,80 @@ def test_every_entry_point_rejects_null_arguments_without_touching_the_gpu():
     assert checked >= 24
 
 
+def _engines():
+    """(name, native engine, image sizes) of cfg1, the cfg2 model and the four image_v1 U-Net configs; creating an engine needs no GPU"""
+    import json
+    import k_diffusion as K
+    from k_diffusion import _native
+    golden = ROOT / "tests" / "golden"
+    for stem, sizes in (("cfg1_mnist", [(28, 28)]), ("cfg2_sw256", [(64, 64), (256, 256)])):
+        cfg = json.loads((golden / f"{stem}_shapes.json").read_text())["config"]
+        yield stem, _native.Engine(K.config.make_model(K.config.load_config(cfg)).engine_spec()), sizes
+    for name, meta in sorted(json.loads((golden / "unet_configs.json").read_text()).items()):
+        cfg = K.config.load_config(meta["config"])
+        model = K.config.make_model(cfg)
+        augment = isinstance(model, K.augmentation.KarrasAugmentWrapper)
+        spec = (model.inner_model if augment else model).engine_spec(augment)
+        yield f"unet {name}", _native.UNetEngine(spec), [tuple(cfg["model"]["input_size"])]
+
+
+# byte counts of kdb_*_workspace_bytes: a change moves every caller's workspace
+WORKSPACE_BYTES = {
+    "cfg1_mnist 28x28 B1 prec0": 755712,
+    "cfg1_mnist 28x28 B1 prec1": 381952,
+    "cfg1_mnist 28x28 B1 vjp": 2415616,
+    "cfg1_mnist 28x28 B3 prec0": 2264064,
+    "cfg1_mnist 28x28 B3 prec1": 1137664,
+    "cfg1_mnist 28x28 B3 vjp": 7239680,
+    "cfg2_sw256 64x64 B1 prec0": 2401280,
+    "cfg2_sw256 64x64 B1 prec1": 1205248,
+    "cfg2_sw256 64x64 B1 vjp": 6569984,
+    "cfg2_sw256 64x64 B3 prec0": 7201792,
+    "cfg2_sw256 64x64 B3 prec1": 3613696,
+    "cfg2_sw256 64x64 B3 vjp": 19705856,
+    "cfg2_sw256 256x256 B1 prec0": 38405120,
+    "cfg2_sw256 256x256 B1 prec1": 19268608,
+    "cfg2_sw256 256x256 B1 vjp": 105089024,
+    "cfg2_sw256 256x256 B3 prec0": 115213312,
+    "cfg2_sw256 256x256 B3 prec1": 57803776,
+    "cfg2_sw256 256x256 B3 vjp": 315262976,
+    "unet 32x32_small 32x32 B1": 11927808,
+    "unet 32x32_small 32x32 B3": 35782912,
+    "unet 32x32_small_butterflies 32x32 B1": 11927808,
+    "unet 32x32_small_butterflies 32x32 B3": 35782912,
+    "unet cifar10 32x32 B1": 11927808,
+    "unet cifar10 32x32 B3": 35782912,
+    "unet mnist 28x28 B1": 8981760,
+    "unet mnist 28x28 B3": 26944768,
+}
+
+
+def test_workspace_bytes_of_every_engine():
+    from k_diffusion import _native
+    L = _native.lib()
+    got = {}
+    for name, eng, sizes in _engines():
+        for (H, W) in sizes:
+            for B in (1, 3):
+                if name.startswith("unet"):
+                    got[f"{name} {H}x{W} B{B}"] = int(L.kdb_unet_workspace_bytes(eng._h, _native.PREC_FP32, B, H, W))
+                else:
+                    for prec in (_native.PREC_FP32, _native.PREC_BF16):
+                        got[f"{name} {H}x{W} B{B} prec{prec}"] = int(L.kdb_model_workspace_bytes(eng._h, prec, B, H, W))
+                    got[f"{name} {H}x{W} B{B} vjp"] = int(L.kdb_model_vjp_workspace_bytes(eng._h, B, H, W))
+    assert got == WORKSPACE_BYTES
+
+
+def test_set_tensor_rejects_a_null_shape():
+    from k_diffusion import _native
+    L = _native.lib()
+    data = ctypes.c_void_p(256)       # never dereferenced: set_tensor only records the pointer
+    for name, eng, _ in _engines():
+        set_tensor = L.kdb_unet_set_tensor if name.startswith("unet") else L.kdb_model_set_tensor
+        assert set_tensor(eng._h, b"k", data, None, 2) == -1, name
+        assert b"set_tensor" in L.kdb_last_error(), name
+
+
 def test_header_is_plain_c_and_a_c_program_links(tmp_path):
     """The boundary is a C ABI, not a C++ one: the header compiles as pedantic C99 and a C program that calls into the
     library links against libkdb200.so and runs without a GPU (kdb_abi_version, kdb_last_error, an argument-validation failure)."""
