@@ -1,23 +1,32 @@
 // tc_attention.cu -- bf16 attention on the sm_90a tensor core (wgmma) for the attention types of the model configurations:
 //   * shifted-window attention, 8x8 windows, d_head 64 (reference image_transformer_v2.py:253-337,446-476)
 //   * global attention, sequence a multiple of 128, d_head 64 (:355-396)
+//   * 7x7 neighbourhood attention, d_head 64 (:399-443)
 // q and k arrive already cosine-normalised and rotated (qknorm_rope kernel); softmax scale is 1.0.
 //
-// One CTA = one 128-row S tile:
-//   WINDOW : rows = 2 heads x 64 tokens of one window; S = [Q_h0;Q_h1][K_h0;K_h1]^T is computed as one 128x128
-//            MMA and only the two 64x64 diagonal blocks are used (attention is ~2 % of the model's MACs: the
-//            wasted half is cheaper than half-rate M=64 MMAs).  The roll (:274) is pure index arithmetic: the window
-//            is fetched as four 4x4-token TMA boxes (quadrants), which are exactly the seam-mask regions (:300-315).
-//   GLOBAL : rows = 128 queries of one head; keys streamed in blocks of 128; exact two-pass softmax
-//            (pass A: row maxima, pass B: exp / P V) so no accumulator rescaling is needed.
-//   NA     : 7x7 neighbourhood attention (reference :399-443 via natten; NATTEN definition: window clamped inward at the
-//            borders, always 49 keys).  Rows = an 8x16 query block of one head; its keys all lie in the clamped 14x22 halo,
-//            streamed as three TMA boxes of 5 halo rows (110 keys per 128-row tile, the tail rows are masked / zero);
-//            the per-query 7x7 window is a mask on S.  Same two-pass softmax as GLOBAL.
-// Roles: warp 4 = TMA producer, warps 0-3 = the warpgroup that issues the MMAs and runs the softmax.  Per key block: TMA
-// (SWIZZLE_128B) -> S = Q K^T (wgmma, two M = 64 halves) -> fp32 S tile in shared memory -> softmax (one thread per row) ->
-// P (bf16) written to shared memory in the K-major SW128 layout -> O += P V (V consumed as an MN-major operand straight from
-// the TMA tile, O in registers across key blocks) -> fp32 O tile, 1/l scaling, store.
+// WINDOW and GLOBAL: attn_ws_kernel, persistent and warp-specialized (384 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...).
+//   A tile is 128 query rows, 64 per MMA warpgroup, and a sequence of key blocks:
+//   WINDOW : the tile is two work items (image, window, head) -- heads 2k and 2k + 1 of one window, one per warpgroup; each warpgroup
+//            computes its own 64x64 S with m64n64k16 against its head's 64 keys, one key block.  The roll (:274) is pure index
+//            arithmetic: a window is fetched as four 4x4-token TMA boxes (quadrants), which are exactly the seam-mask regions (:300-315);
+//            rows of a window are quadrant-major, then (row, column) inside the quadrant.
+//   GLOBAL : the tile is 128 queries of one (image, head); keys and values are streamed in blocks of 128 through a ring of stages that
+//            both warpgroups read (S = 64 x 128 per warpgroup, m64n128k16).
+//   Roles: warpgroup 2 is the producer (40 registers): one elected lane loads by TMA the Q tile of every tile (WS_QBUF buffers) and its
+//   key blocks (WS_KV_STAGES stages of K and V), so the next tile loads while the current one computes.  Warpgroups 0 and 1 (232
+//   registers): S = Q K^T into registers, softmax in registers (a row's columns sit in the 4 threads of a quad: max and sum by two
+//   shuffles), P rounded to bf16 is the register A operand of O += P V (V an MN-major operand straight from the TMA tile), O stays in
+//   registers across the key blocks and is scaled by 1/l once; the bf16 output is staged in shared memory and leaves by TMA (the
+//   quadrant boxes for windows).
+//   Softmax: with the bound (below) a single pass with the fixed shift exp(s - bound); without it the row maximum: GLOBAL keeps a running
+//   maximum and rescales O and l when it grows (exact: the result is that of the final maximum), WINDOW has one key block.
+// NA: attn_na_kernel, one CTA = one 128-query block of one head (160 threads).  7x7 neighbourhood (NATTEN definition: window clamped
+//   inward at the borders, always 49 keys).  Rows = an 8x16 query block; its keys all lie in the clamped 14x22 halo, streamed as three
+//   TMA boxes of 5 halo rows (110 keys per 128-row tile, the tail rows are masked / zero); the per-query 7x7 window is a mask on S.
+//   Roles: warp 4 = TMA producer, warps 0-3 = the warpgroup that issues the MMAs and runs the softmax.  Per key block: TMA (SWIZZLE_128B)
+//   -> S = Q K^T (wgmma, two M = 64 halves) -> fp32 S tile in shared memory -> softmax (one thread per row) -> P (bf16) written to shared
+//   memory in the K-major SW128 layout -> O += P V -> fp32 O tile, 1/l scaling, store.  Without the bound an exact two-pass softmax
+//   (pass A: row maxima, pass B: exp / P V).
 #include "tc_common.cuh"
 #include "tc_kernels.cuh"
 
@@ -26,10 +35,11 @@ namespace {
 
 constexpr int ROWS = 128, DH = 64;
 constexpr int TILE_BYTES = ROWS * DH * 2;    // 16 KiB: 128 rows x 128 B
+constexpr int HALF_BYTES = TILE_BYTES / 2;   // 64 rows: one warpgroup's share, one window of one head
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr int S_LD = ROWS + 4;               // row pitch (floats) of the fp32 S / O tile
 
-enum { MODE_WINDOW = 0, MODE_GLOBAL = 1, MODE_NA = 2 };
+enum { MODE_WINDOW = 0, MODE_GLOBAL = 1 };
 
 constexpr int NA_QH = 8, NA_QW = 16;          // query block of one CTA (128 queries of one head)
 constexpr int NA_KH = 14, NA_KW = 22;         // its clamped key halo for a 7x7 neighbourhood
@@ -40,51 +50,295 @@ struct AttnParams {
   bf16* out;
   // [nh] or nullptr: upper bound of |q . k| per head.  q and k are cosine-normalised (|q| = |k| = sqrt(scale_h), reference
   // :106-114, RoPE is a rotation), so the layer's scale IS that bound and softmax can use it as a FIXED shift: exp(s - bound)
-  // needs no row maximum -> GLOBAL / NA run ONE pass over the key blocks instead of two, WINDOW skips its max scan.
+  // needs no row maximum -> one pass over the key blocks, no maximum scan.
   const float* bound;
   int B, h, w, nh, shift, nblk;
+  int n_tiles;                                 // attn_ws_kernel: WINDOW B (h / 8) (w / 8) nh / 2, GLOBAL B nh (h w / 128)
 };
 
+// ================================================================ WINDOW, GLOBAL
+constexpr int WS_THREADS = 384;
+// Loads are the bound (a window tile is ~0.5 us of MMA and softmax against 48 KiB in, 16 KiB out): four tiles in flight per SM keep
+// enough bytes outstanding to cover the latency of HBM at its bandwidth share of one SM
+constexpr int WS_QBUF = 4, WS_KV_STAGES = 4;
+
+struct WsBars {
+  uint64_t q_full[WS_QBUF], q_empty[WS_QBUF], kv_full[WS_KV_STAGES], kv_empty[WS_KV_STAGES];
+};
+// Q buffers, K and V stages, one output staging tile per warpgroup
+constexpr size_t WS_SMEM = (size_t)WS_QBUF * TILE_BYTES + (size_t)WS_KV_STAGES * 2 * TILE_BYTES + 2 * HALF_BYTES + sizeof(WsBars) + 1024;
+
+// tile -> image b, window (wi, wj), first head of the pair
+__device__ __forceinline__ void ws_window(const AttnParams& p, int tile, int& b, int& wi, int& wj, int& head0) {
+  const int hp = p.nh >> 1, nww = p.w >> 3, per_img = (p.h >> 3) * nww * hp;
+  b = tile / per_img;
+  int rem = tile - b * per_img;
+  const int win = rem / hp;
+  head0 = 2 * (rem - win * hp);
+  wi = win / nww;
+  wj = win - wi * nww;
+}
+// origin of quadrant q of window (wi, wj) in original coordinates (:274)
+__device__ __forceinline__ void ws_quad(const AttnParams& p, int wi, int wj, int q, int& r, int& c) {
+  r = (wi * 8 + (q >> 1) * 4 - p.shift + p.h) % p.h;
+  c = (wj * 8 + (q & 1) * 4 - p.shift + p.w) % p.w;
+}
+// tile -> image b, head, 128-query tile m (GLOBAL)
+__device__ __forceinline__ void ws_global(const AttnParams& p, int tile, int& b, int& head, int& m) {
+  b = tile / (p.nh * p.nblk);
+  const int rem = tile - b * p.nh * p.nblk;
+  head = rem / p.nblk;
+  m = rem - head * p.nblk;
+}
+
+template <int MODE, bool BOUNDED>
+__global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_out,
+                                                                const AttnParams p) {
+  constexpr int NK = MODE == MODE_WINDOW ? 64 : 128;   // keys per block seen by one warpgroup
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* sQ = base;
+  uint8_t* sKV = sQ + WS_QBUF * TILE_BYTES;                    // stage s: K at 2 s TILE_BYTES, V after it
+  uint8_t* sO = sKV + WS_KV_STAGES * 2 * TILE_BYTES;
+  WsBars* bars = reinterpret_cast<WsBars*>(sO + 2 * HALF_BYTES);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nblk = MODE == MODE_WINDOW ? 1 : p.nblk;
+  const int n_local = (int)blockIdx.x < p.n_tiles ? (p.n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+
+  if (threadIdx.x == 0) {
+    tc::tma_prefetch_desc(&tm_in);
+    tc::tma_prefetch_desc(&tm_out);
+    for (int i = 0; i < WS_QBUF; ++i) {
+      tc::mbar_init(&bars->q_full[i], 1);
+      tc::mbar_init(&bars->q_empty[i], 8);    // lane 0 of every MMA warp
+    }
+    for (int i = 0; i < WS_KV_STAGES; ++i) {
+      tc::mbar_init(&bars->kv_full[i], 1);
+      tc::mbar_init(&bars->kv_empty[i], 8);
+    }
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  tc::pdl_wait();                              // programmatic launch: the qkv projection before us must be complete from here on
+  tc::pdl_launch_dependents();
+
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ TMA producer
+    tc::setmaxnreg_dec<40>();
+    if (warp == 8 && tc::elect_one()) {
+      // the window of heads head0, head0 + 1, third t of qkv (0 q, 1 k, 2 v): two 64-row halves of four quadrant boxes
+      auto load_window = [&](uint8_t* dst, int t, uint64_t* bar, int b, int wi, int wj, int head0) {
+#pragma unroll
+        for (int hd = 0; hd < 2; ++hd)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            int r, c;
+            ws_quad(p, wi, wj, q, r, c);
+            tc::tma_load_4d(dst + hd * HALF_BYTES + q * 2048, &tm_in, bar, (t * p.nh + head0 + hd) * DH, c, r, b);
+          }
+      };
+      int kv = 0;
+      for (int i = 0; i < n_local; ++i) {
+        const int tile = (int)blockIdx.x + i * (int)gridDim.x, qb = i % WS_QBUF;
+        tc::mbar_wait_nocall(&bars->q_empty[qb], (uint32_t)(((i / WS_QBUF) & 1) ^ 1));
+        tc::mbar_arrive_expect_tx(&bars->q_full[qb], TILE_BYTES);
+        uint8_t* q_dst = sQ + qb * TILE_BYTES;
+        if constexpr (MODE == MODE_WINDOW) {
+          int b, wi, wj, head0;
+          ws_window(p, tile, b, wi, wj, head0);
+          load_window(q_dst, 0, &bars->q_full[qb], b, wi, wj, head0);
+          const int st = kv % WS_KV_STAGES;
+          tc::mbar_wait_nocall(&bars->kv_empty[st], (uint32_t)(((kv / WS_KV_STAGES) & 1) ^ 1));
+          tc::mbar_arrive_expect_tx(&bars->kv_full[st], 2 * TILE_BYTES);
+          load_window(sKV + st * 2 * TILE_BYTES, 1, &bars->kv_full[st], b, wi, wj, head0);
+          load_window(sKV + st * 2 * TILE_BYTES + TILE_BYTES, 2, &bars->kv_full[st], b, wi, wj, head0);
+          ++kv;
+        } else {
+          int b, head, m;
+          ws_global(p, tile, b, head, m);
+          tc::tma_load_3d(q_dst, &tm_in, &bars->q_full[qb], head * DH, m * ROWS, b);
+          for (int j = 0; j < nblk; ++j, ++kv) {
+            const int st = kv % WS_KV_STAGES;
+            tc::mbar_wait_nocall(&bars->kv_empty[st], (uint32_t)(((kv / WS_KV_STAGES) & 1) ^ 1));
+            tc::mbar_arrive_expect_tx(&bars->kv_full[st], 2 * TILE_BYTES);
+            tc::tma_load_3d(sKV + st * 2 * TILE_BYTES, &tm_in, &bars->kv_full[st], (p.nh + head) * DH, j * ROWS, b);
+            tc::tma_load_3d(sKV + st * 2 * TILE_BYTES + TILE_BYTES, &tm_in, &bars->kv_full[st], (2 * p.nh + head) * DH, j * ROWS, b);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------------ MMA warpgroups: 64 query rows each
+  tc::setmaxnreg_inc<232>();
+  const int wg = warp >> 2, t = threadIdx.x & 127;
+  const int rw = 16 * (t >> 5) + (lane >> 2);                // this thread's two rows of the warpgroup's 64: rw and rw + 8
+  const int cq = 2 * (lane & 3);                             // and its column pair inside every 8-column block
+  const int quad = rw >> 4;                                  // WINDOW: the quadrant of both rows
+  uint8_t* sOw = sO + wg * HALF_BYTES;
+  int kv = 0;
+  for (int i = 0; i < n_local; ++i) {
+    const int tile = (int)blockIdx.x + i * (int)gridDim.x, qb = i % WS_QBUF;
+    int b, head, wi = 0, wj = 0, m = 0;
+    if constexpr (MODE == MODE_WINDOW) {
+      ws_window(p, tile, b, wi, wj, head);
+      head += wg;
+    } else {
+      ws_global(p, tile, b, head, m);
+    }
+    const bool seam_r = MODE == MODE_WINDOW && p.shift > 0 && wi == 0;
+    const bool seam_c = MODE == MODE_WINDOW && p.shift > 0 && wj == 0;
+    float mx0 = -INFINITY, mx1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running row maxima (or the bound) and partial row sums
+    if constexpr (BOUNDED) mx0 = mx1 = __ldg(p.bound + head);
+    float o[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) o[j] = 0.f;
+    const uint64_t qdesc = tc::smem_desc_k_sw128(tc::smem_u32(sQ + qb * TILE_BYTES + wg * HALF_BYTES));
+    tc::mbar_wait_nocall(&bars->q_full[qb], (uint32_t)((i / WS_QBUF) & 1));
+    for (int j = 0; j < nblk; ++j, ++kv) {
+      const int st = kv % WS_KV_STAGES;
+      const uint32_t k_addr = tc::smem_u32(sKV + st * 2 * TILE_BYTES) + (MODE == MODE_WINDOW ? wg * HALF_BYTES : 0);
+      const uint32_t v_addr = k_addr + TILE_BYTES;
+      tc::mbar_wait_nocall(&bars->kv_full[st], (uint32_t)((kv / WS_KV_STAGES) & 1));
+      // ---- S = Q K^T
+      float s[NK / 2];
+#pragma unroll
+      for (int c = 0; c < NK / 2; ++c) s[c] = 0.f;
+      tc::wg_fence_acc(s);
+      tc::wg_fence();
+      const uint64_t kdesc = tc::smem_desc_k_sw128(k_addr);
+#pragma unroll
+      for (int k = 0; k < DH / 16; ++k) {
+        if constexpr (NK == 64)
+          tc::wgmma_64<0>(s, qdesc + 2ull * k, kdesc + 2ull * k, 1u);
+        else
+          tc::wgmma_128(s, qdesc + 2ull * k, kdesc + 2ull * k, 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(s);
+      if (j == nblk - 1 && lane == 0) tc::mbar_arrive(&bars->q_empty[qb]);   // every read of this Q tile is done
+      // ---- softmax in registers.  Key column 8 c + cq (+1); WINDOW: it lies in quadrant c / 2, and the seam mask keeps a query to keys
+      // on its own side of the wrapped row / column of the top / left windows.
+      auto key_ok = [&](int c) -> bool {
+        const int kq = c >> 1;
+        return (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
+      };
+      if constexpr (!BOUNDED) {
+        float n0 = mx0, n1 = mx1;
+#pragma unroll
+        for (int c = 0; c < NK / 8; ++c) {
+          if (MODE == MODE_WINDOW && !key_ok(c)) s[4 * c] = s[4 * c + 1] = s[4 * c + 2] = s[4 * c + 3] = -INFINITY;
+          n0 = fmaxf(n0, fmaxf(s[4 * c], s[4 * c + 1]));
+          n1 = fmaxf(n1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
+        }
+        n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 1));
+        n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 2));
+        n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 1));
+        n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 2));
+        if (j > 0) {                           // the maximum grew: rescale what was accumulated against the old one
+          const float a0 = exp2f((mx0 - n0) * LOG2E), a1 = exp2f((mx1 - n1) * LOG2E);
+          l0 *= a0;
+          l1 *= a1;
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            o[4 * c] *= a0;
+            o[4 * c + 1] *= a0;
+            o[4 * c + 2] *= a1;
+            o[4 * c + 3] *= a1;
+          }
+        }
+        mx0 = n0;
+        mx1 = n1;
+      }
+      const float mb0 = mx0 * LOG2E, mb1 = mx1 * LOG2E;
+      uint32_t pf[NK / 4];
+#pragma unroll
+      for (int i2 = 0; i2 < NK / 4; ++i2) {
+        const float mb = (i2 & 1) ? mb1 : mb0;
+        float p0 = exp2f(fmaf(s[2 * i2], LOG2E, -mb)), p1 = exp2f(fmaf(s[2 * i2 + 1], LOG2E, -mb));
+        if (BOUNDED && MODE == MODE_WINDOW && !key_ok(i2 >> 1)) p0 = p1 = 0.f;   // (bounded) zero probability instead of a -inf logit
+        pf[i2] = tc::pack_bf16x2(p0, p1);
+        float e0, e1;
+        tc::unpack_bf16x2(pf[i2], e0, e1);     // l accumulates exactly what the P V MMA sees
+        if (i2 & 1) l1 += e0 + e1;
+        else l0 += e0 + e1;
+      }
+      // ---- O += P V, 16 keys per step: rows 16 kk.. of V
+      tc::wg_fence_acc(o);
+      tc::wg_fence_acc(pf);
+      tc::wg_fence();
+      const uint64_t vdesc = tc::smem_desc_mn_sw128(v_addr, 1024, 1024);
+#pragma unroll
+      for (int kk = 0; kk < NK / 16; ++kk) {
+        const uint32_t a[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
+        tc::wgmma_64_rs<1>(o, a, vdesc + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(o);
+      if (lane == 0) tc::mbar_arrive(&bars->kv_empty[st]);
+    }
+    // ---- O / l -> bf16 staging tile (rows = this warpgroup's 64 queries) -> TMA store
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+    if (t == 0) tc::tma_store_wait_read();    // the previous tile's store has read the staging tile
+    tc::named_barrier_sync(1 + wg, 128);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw, c) + cq * 2) = tc::pack_bf16x2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
+      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw + 8, c) + cq * 2) = tc::pack_bf16x2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
+    }
+    tc::fence_proxy_async();                   // staging tile (generic-proxy writes) -> visible to the TMA engine
+    tc::named_barrier_sync(1 + wg, 128);
+    if (t == 0) {
+      if constexpr (MODE == MODE_WINDOW) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          int r, c;
+          ws_quad(p, wi, wj, q, r, c);
+          tc::tma_store_4d(&tm_out, sOw + q * 2048, head * DH, c, r, b);
+        }
+      } else {
+        tc::tma_store_3d(&tm_out, sOw, head * DH, m * ROWS + wg * 64, b);
+      }
+      tc::tma_store_commit();
+    }
+  }
+  if (t == 0) tc::tma_store_wait_read();      // shared memory stays alive until the last store has read it
+}
+
+// ================================================================ NA
 struct Bars {
   uint64_t q, kv, kv_free;
 };
 
-template <int MODE, bool BOUNDED>
-__global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
+template <bool BOUNDED>
+__global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
                                                          const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sQ = base;
   uint8_t* sK = base + TILE_BYTES;
   uint8_t* sV = base + 2 * TILE_BYTES;
-  // P (two K-blocks of 64 keys, 32 KiB).  WINDOW has a single key block: Q and K are dead once S = Q K^T has completed, so
-  // P overwrites them; GLOBAL re-uses Q for every key block and keeps P separate.
-  uint8_t* sP = (MODE == MODE_WINDOW) ? sQ : base + 3 * TILE_BYTES;
-  float* sS = reinterpret_cast<float*>(base + (MODE == MODE_WINDOW ? 3 : 5) * TILE_BYTES);   // fp32 S (then O) tile, row pitch S_LD
+  uint8_t* sP = base + 3 * TILE_BYTES;         // P: two K-blocks of 64 keys, 32 KiB
+  float* sS = reinterpret_cast<float*>(base + 5 * TILE_BYTES);   // fp32 S (then O) tile, row pitch S_LD
   Bars* bars = reinterpret_cast<Bars*>(sS + ROWS * S_LD);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nh = p.nh;
-  // work decomposition
-  int b = blockIdx.z, head0, wi = 0, wj = 0, mtile = 0;
-  if constexpr (MODE == MODE_WINDOW) {
-    const int nww = p.w / 8;
-    wi = blockIdx.x / nww;
-    wj = blockIdx.x - wi * nww;
-    head0 = blockIdx.y * 2;
-  } else {
-    mtile = blockIdx.x;
-    head0 = blockIdx.y;
-  }
-  int qi0 = 0, qj0 = 0, r0 = 0, c0 = 0;      // NA: query block origin and clamped halo origin
-  if constexpr (MODE == MODE_NA) {
-    const int nbw = p.w / NA_QW;
-    qi0 = (blockIdx.x / nbw) * NA_QH;
-    qj0 = (blockIdx.x % nbw) * NA_QW;
-    r0 = min(max(qi0 - 3, 0), p.h - NA_KH);
-    c0 = min(max(qj0 - 3, 0), p.w - NA_KW);
-  }
-  const int nblk = (MODE == MODE_WINDOW) ? 1 : p.nblk;
+  // work decomposition: query block origin and clamped halo origin
+  const int b = blockIdx.z, head0 = blockIdx.y;
+  const int nbw = p.w / NA_QW;
+  const int qi0 = (blockIdx.x / nbw) * NA_QH;
+  const int qj0 = (blockIdx.x % nbw) * NA_QW;
+  const int r0 = min(max(qi0 - 3, 0), p.h - NA_KH);
+  const int c0 = min(max(qj0 - 3, 0), p.w - NA_KW);
+  const int nblk = p.nblk;
   constexpr bool bounded = BOUNDED;
   const bool two_pass = nblk > 1 && !bounded;
   const int n_iter = two_pass ? 2 * nblk : nblk;
@@ -96,11 +350,10 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
     tc::mbar_init(&bars->kv_free, 4);          // lane 0 of each warp of the warpgroup
     tc::fence_barrier_init();
   }
-  if constexpr (MODE == MODE_NA) {   // rows 110..127 of the V tile are never written by TMA: they must be finite (P there is exactly 0)
-    for (int i = threadIdx.x; i < (ROWS - NA_BLK_KEYS) * 8; i += blockDim.x)
-      *reinterpret_cast<uint4*>(sV + NA_BLK_KEYS * 128 + i * 16) = make_uint4(0u, 0u, 0u, 0u);
-    tc::fence_proxy_async();
-  }
+  // rows 110..127 of the V tile are never written by TMA: they must be finite (P there is exactly 0)
+  for (int i = threadIdx.x; i < (ROWS - NA_BLK_KEYS) * 8; i += blockDim.x)
+    *reinterpret_cast<uint4*>(sV + NA_BLK_KEYS * 128 + i * 16) = make_uint4(0u, 0u, 0u, 0u);
+  tc::fence_proxy_async();
   __syncthreads();
   tc::pdl_wait();                              // programmatic launch: the qkv projection before us must be complete from here on
   tc::pdl_launch_dependents();
@@ -108,44 +361,16 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
   if (warp == 4) {
     if (tc::elect_one()) {
       // ------------------------------------------------ loads of Q and of each key block (K, and V in the P V pass)
-      auto load_window_tile = [&](uint8_t* dst, int t, uint64_t* bar) {
-        if (p.shift == 0) {   // unshifted window: one 8x8 box per head, rows in (lr, lc) order (tensor map box = 64 x 8 x 8)
-#pragma unroll
-          for (int hd = 0; hd < 2; ++hd) tc::tma_load_4d(dst + hd * 64 * 128, &tmap, bar, (t * nh + head0 + hd) * DH, wj * 8, wi * 8, b);
-          return;
-        }
-#pragma unroll
-        for (int hd = 0; hd < 2; ++hd)
-#pragma unroll
-          for (int quad = 0; quad < 4; ++quad) {
-            const int r0 = (wi * 8 + (quad >> 1) * 4 - p.shift + p.h) % p.h;   // rolled -> original coordinates (:274)
-            const int c0 = (wj * 8 + (quad & 1) * 4 - p.shift + p.w) % p.w;
-            tc::tma_load_4d(dst + (hd * 64 + quad * 16) * 128, &tmap, bar, (t * nh + head0 + hd) * DH, c0, r0, b);
-          }
-      };
       tc::mbar_arrive_expect_tx(&bars->q, TILE_BYTES);
-      if constexpr (MODE == MODE_WINDOW)
-        load_window_tile(sQ, 0, &bars->q);
-      else if constexpr (MODE == MODE_NA)
-        tc::tma_load_4d(sQ, &tmap, &bars->q, head0 * DH, qj0, qi0, b);
-      else
-        tc::tma_load_3d(sQ, &tmap, &bars->q, head0 * DH, mtile * ROWS, b);
+      tc::tma_load_4d(sQ, &tmap, &bars->q, head0 * DH, qj0, qi0, b);
       for (int it = 0; it < n_iter; ++it) {
         const int j = it % nblk;
         const bool with_v = !two_pass || it >= nblk;
         if (it > 0) tc::mbar_wait_nocall(&bars->kv_free, (uint32_t)(it - 1) & 1u);
-        constexpr uint32_t KV_BYTES = (MODE == MODE_NA) ? NA_BLK_KEYS * 128 : TILE_BYTES;
+        constexpr uint32_t KV_BYTES = NA_BLK_KEYS * 128;
         tc::mbar_arrive_expect_tx(&bars->kv, with_v ? 2 * KV_BYTES : KV_BYTES);
-        if constexpr (MODE == MODE_WINDOW) {
-          load_window_tile(sK, 1, &bars->kv);
-          load_window_tile(sV, 2, &bars->kv);
-        } else if constexpr (MODE == MODE_NA) {
-          tc::tma_load_4d(sK, &tmap_kv, &bars->kv, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
-          if (with_v) tc::tma_load_4d(sV, &tmap_kv, &bars->kv, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
-        } else {
-          tc::tma_load_3d(sK, &tmap, &bars->kv, (nh + head0) * DH, j * ROWS, b);
-          if (with_v) tc::tma_load_3d(sV, &tmap, &bars->kv, (2 * nh + head0) * DH, j * ROWS, b);
-        }
+        tc::tma_load_4d(sK, &tmap_kv, &bars->kv, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
+        if (with_v) tc::tma_load_4d(sV, &tmap_kv, &bars->kv, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
       }
     }
     return;
@@ -154,15 +379,10 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
   // ---------------------------------------------------- warpgroup: S = Q K^T (wgmma) -> softmax, thread = row -> O += P V (wgmma)
   const int row = warp * 32 + lane;
   float m = -INFINITY, l = 0.f;
-  // window geometry of this row
-  const int hd = row >> 6, quad = (row & 63) >> 4;
-  const bool seam_r = MODE == MODE_WINDOW && p.shift > 0 && wi == 0;
-  const bool seam_c = MODE == MODE_WINDOW && p.shift > 0 && wj == 0;
-  // NA: this row's query and the origin of its clamped 7x7 window
+  // this row's query and the origin of its clamped 7x7 window
   const int na_qi = qi0 + (row >> 4), na_qj = qj0 + (row & 15);
   const int na_rs = min(max(na_qi - 3, 0), p.h - 7), na_cs = min(max(na_qj - 3, 0), p.w - 7);
   auto key_ok = [&](int j, int t) -> bool {      // is tile column t of key block j inside this row's neighbourhood?
-    if constexpr (MODE != MODE_NA) return true;
     const int dr = (t * 745) >> 14;               // t / 22 for t < 128
     const int kr = r0 + j * NA_BLK_ROWS + dr, kc = c0 + (t - dr * NA_KW);
     return t < NA_BLK_KEYS && (unsigned)(kr - na_rs) < 7u && (unsigned)(kc - na_cs) < 7u;
@@ -193,7 +413,7 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
       tc::wg_fence_acc(s);
       tc::acc_store(sS, S_LD, 64 * h, s);
     }
-    tc::named_barrier_sync(1, 128);            // S complete; every read of Q and K is done (WINDOW: P may overwrite them)
+    tc::named_barrier_sync(1, 128);            // S complete; every read of Q and K is done
     if (pass == 0) {
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
@@ -202,7 +422,7 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
 #pragma unroll
         for (int i = 0; i < 32; ++i) m = fmaxf(m, key_ok(j, c * 32 + i) ? v[i] : -INFINITY);
       }
-    } else if constexpr (MODE != MODE_WINDOW) {
+    } else {
       if constexpr (bounded) m = __ldg(p.bound + head0);
       if (!two_pass && !bounded) {             // single block: the row maximum comes from this very tile
         float mm = -INFINITY;
@@ -235,53 +455,6 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
         for (int jj = 0; jj < 4; ++jj)
           *reinterpret_cast<uint4*>(pt + tc::sw128_offset(row, (c & 1) * 4 + jj)) = make_uint4(pk[jj * 4], pk[jj * 4 + 1], pk[jj * 4 + 2], pk[jj * 4 + 3]);
       }
-    } else {
-      // WINDOW: own head's 64 key columns live at [64*hd, 64*hd+64); the other head's block is garbage -> zeros in P
-      float v[64];
-      {
-        float t0[32], t1[32];
-        tc::acc_ld32(sS, S_LD, row, hd * 64, t0);
-        tc::acc_ld32(sS, S_LD, row, hd * 64 + 32, t1);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) { v[i] = t0[i]; v[32 + i] = t1[i]; }
-      }
-      if constexpr (!bounded) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          const int kq = i >> 4;
-          const bool ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-          v[i] = ok ? v[i] : -INFINITY;
-          m = fmaxf(m, v[i]);
-        }
-      } else {
-        m = __ldg(p.bound + head0 + hd);          // fixed shift: no maximum scan; masked keys get p = 0 below
-      }
-      const float mb = m * LOG2E;
-      uint8_t* own = sP + hd * TILE_BYTES;
-      uint8_t* other = sP + (1 - hd) * TILE_BYTES;
-#pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
-        uint32_t pk[4];
-        bool ok = true;                        // (bounded) seam mask of this 8-key group: zero probability instead of -inf logit
-        if constexpr (bounded) {
-          const int kq = jj >> 1;
-          ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-        }
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          float p0 = exp2f(fmaf(v[jj * 8 + 2 * t], LOG2E, -mb)), p1 = exp2f(fmaf(v[jj * 8 + 2 * t + 1], LOG2E, -mb));
-          if constexpr (bounded) {
-            p0 = ok ? p0 : 0.f;
-            p1 = ok ? p1 : 0.f;
-          }
-          pk[t] = tc::pack_bf16x2(p0, p1);
-          float q0, q1;
-          tc::unpack_bf16x2(pk[t], q0, q1);
-          l += q0 + q1;
-        }
-        *reinterpret_cast<uint4*>(own + tc::sw128_offset(row, jj)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        *reinterpret_cast<uint4*>(other + tc::sw128_offset(row, jj)) = make_uint4(0u, 0u, 0u, 0u);
-      }
     }
     if (pass == 1) {
       tc::fence_proxy_async();                 // P (generic-proxy writes) -> visible to the tensor core
@@ -309,28 +482,8 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
   tc::acc_store(sS, S_LD, 64, o1);
   tc::named_barrier_sync(1, 128);
   const float inv = 1.f / l;
-  int64_t token;
-  int head;
-  if constexpr (MODE == MODE_WINDOW) {
-    int oi, oj;
-    if (p.shift == 0) {
-      oi = wi * 8 + ((row & 63) >> 3);
-      oj = wj * 8 + (row & 7);
-    } else {
-      const int lr = (row & 15) >> 2, lc = row & 3;
-      oi = (wi * 8 + (quad >> 1) * 4 + lr - p.shift + p.h) % p.h;
-      oj = (wj * 8 + (quad & 1) * 4 + lc - p.shift + p.w) % p.w;
-    }
-    token = (int64_t)oi * p.w + oj;
-    head = head0 + hd;
-  } else if constexpr (MODE == MODE_NA) {
-    token = (int64_t)na_qi * p.w + na_qj;
-    head = head0;
-  } else {
-    token = (int64_t)mtile * ROWS + row;
-    head = head0;
-  }
-  uint4* dst = reinterpret_cast<uint4*>(p.out + (((int64_t)b * p.h * p.w + token) * nh + head) * DH);
+  const int64_t token = (int64_t)na_qi * p.w + na_qj;
+  uint4* dst = reinterpret_cast<uint4*>(p.out + (((int64_t)b * p.h * p.w + token) * nh + head0) * DH);
 #pragma unroll 1
   for (int c = 0; c < 2; ++c) {
     float v[32];
@@ -342,10 +495,7 @@ __global__ void __launch_bounds__(160, 1) attn_tc_kernel(const __grid_constant__
   }
 }
 
-
-constexpr size_t ATTN_S_BYTES = (size_t)ROWS * S_LD * 4;
-constexpr size_t ATTN_SMEM = 5 * TILE_BYTES + ATTN_S_BYTES + 1024 + 128;          // GLOBAL, NA
-constexpr size_t ATTN_SMEM_WINDOW = 3 * TILE_BYTES + ATTN_S_BYTES + 1024 + 128;   // WINDOW (P aliases Q,K)
+constexpr size_t ATTN_NA_SMEM = 5 * TILE_BYTES + (size_t)ROWS * S_LD * 4 + 1024 + 128;
 
 }  // namespace
 
@@ -363,18 +513,25 @@ bool tc_attention_supported(int h, int w, int nh, int e, int attn_type, int attn
   return false;
 }
 
-template <int MODE>
-static cudaError_t set_attn_smem(size_t smem) {
-  cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel<MODE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(attn_tc_kernel<MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <typename K>
+static cudaError_t set_smem(K kernel, size_t smem) {
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 }
 
-// programmatic dependent launch: barrier init overlaps the tail of the qkv projection
+// persistent WINDOW / GLOBAL launch: min(tiles, SMs) CTAs; programmatic dependent launch, so that barrier init overlaps the tail of the
+// qkv projection
 template <int MODE>
-static cudaError_t launch_attn(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tq, const CUtensorMap& tkv, const AttnParams& p) {
-  if (p.bound != nullptr) return launch_pdl(attn_tc_kernel<MODE, true>, grid, dim3(160), smem, st, tq, tkv, p);
-  return launch_pdl(attn_tc_kernel<MODE, false>, grid, dim3(160), smem, st, tq, tkv, p);
+static cudaError_t launch_ws(cudaStream_t st, const CUtensorMap& tin, const CUtensorMap& tout, const AttnParams& p) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = set_smem(attn_ws_kernel<MODE, false>, WS_SMEM);
+    if (e == cudaSuccess) e = set_smem(attn_ws_kernel<MODE, true>, WS_SMEM);
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  const dim3 grid((unsigned)(p.n_tiles < num_sms() ? p.n_tiles : num_sms()));
+  if (p.bound != nullptr) return launch_pdl(attn_ws_kernel<MODE, true>, grid, dim3(WS_THREADS), WS_SMEM, st, tin, tout, p);
+  return launch_pdl(attn_ws_kernel<MODE, false>, grid, dim3(WS_THREADS), WS_SMEM, st, tin, tout, p);
 }
 
 int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh, int e, int attn_type, int attn_param, int shift,
@@ -382,57 +539,50 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
   KDB_REQUIRE(tc_attention_supported(h, w, nh, e, attn_type, attn_param), KDB_ERR_UNSUPPORTED, "attention_tc: unsupported shape");
   KDB_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, KDB_ERR_BAD_ARG,
               "attention_tc: operands must be 16-byte aligned");
-  const uint64_t F = 3ull * nh * e;
+  const uint64_t F = 3ull * nh * e, C = (uint64_t)nh * e;
   AttnParams p{};
   p.out = out;
   p.B = B; p.h = h; p.w = w; p.nh = nh; p.shift = shift;
   p.bound = logit_bound;
-  CUtensorMap tm;
-  static bool attr_w = false, attr_g = false;
+  CUtensorMap tm, to;
+  int rc;
   if (attn_type == KDB_ATTN_SHIFTED_WINDOW) {
     KDB_REQUIRE(shift == 0 || shift == 4, KDB_ERR_UNSUPPORTED, "attention_tc: window shift must be 0 or window/2");
-    const uint64_t dims[4] = {F, (uint64_t)w, (uint64_t)h, (uint64_t)B};
-    const uint64_t strides[3] = {F * 2, F * 2 * w, F * 2 * w * h};
-    const uint32_t box_q[4] = {DH, 4, 4, 1}, box_f[4] = {DH, 8, 8, 1};
-    int rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, shift == 0 ? box_f : box_q);
-    if (rc) return rc;
-    if (!attr_w) {
-      KDB_CUDA(set_attn_smem<MODE_WINDOW>(ATTN_SMEM_WINDOW));
-      attr_w = true;
-    }
+    const uint64_t dims[4] = {F, (uint64_t)w, (uint64_t)h, (uint64_t)B}, dims_o[4] = {C, (uint64_t)w, (uint64_t)h, (uint64_t)B};
+    const uint64_t strides[3] = {F * 2, F * 2 * w, F * 2 * w * h}, strides_o[3] = {C * 2, C * 2 * w, C * 2 * w * h};
+    const uint32_t box[4] = {DH, 4, 4, 1};    // one quadrant of a window
+    if ((rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, box))) return rc;
+    if ((rc = make_tmap_bf16(&to, out, 4, dims_o, strides_o, box))) return rc;
     p.nblk = 1;
-    dim3 grid((unsigned)((h / 8) * (w / 8)), (unsigned)(nh / 2), (unsigned)B);
-    KDB_CUDA(launch_attn<MODE_WINDOW>(grid, ATTN_SMEM_WINDOW, st, tm, tm, p));
+    p.n_tiles = B * (h / 8) * (w / 8) * (nh / 2);
+    KDB_CUDA(launch_ws<MODE_WINDOW>(st, tm, to, p));
   } else if (attn_type == KDB_ATTN_NEIGHBORHOOD) {
     static bool attr_n = false;
-    CUtensorMap tkv;
     const uint64_t dims[4] = {F, (uint64_t)w, (uint64_t)h, (uint64_t)B};
     const uint64_t strides[3] = {F * 2, F * 2 * w, F * 2 * w * h};
     const uint32_t box_q[4] = {DH, NA_QW, NA_QH, 1}, box_kv[4] = {DH, NA_KW, NA_BLK_ROWS, 1};
-    int rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, box_q);
-    if (rc) return rc;
+    if ((rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, box_q))) return rc;
+    CUtensorMap tkv;
     if ((rc = make_tmap_bf16(&tkv, qkv, 4, dims, strides, box_kv))) return rc;
     if (!attr_n) {
-      KDB_CUDA(set_attn_smem<MODE_NA>(ATTN_SMEM));
+      KDB_CUDA(set_smem(attn_na_kernel<false>, ATTN_NA_SMEM));
+      KDB_CUDA(set_smem(attn_na_kernel<true>, ATTN_NA_SMEM));
       attr_n = true;
     }
     p.nblk = 3;      // 14 halo rows = 5 + 5 + 4
     dim3 grid((unsigned)((h / NA_QH) * (w / NA_QW)), (unsigned)nh, (unsigned)B);
-    KDB_CUDA(launch_attn<MODE_NA>(grid, ATTN_SMEM, st, tm, tkv, p));
+    if (p.bound != nullptr) KDB_CUDA(launch_pdl(attn_na_kernel<true>, grid, dim3(160), ATTN_NA_SMEM, st, tm, tkv, p));
+    else KDB_CUDA(launch_pdl(attn_na_kernel<false>, grid, dim3(160), ATTN_NA_SMEM, st, tm, tkv, p));
   } else {
     const uint64_t T = (uint64_t)h * w;
-    const uint64_t dims[3] = {F, T, (uint64_t)B};
-    const uint64_t strides[2] = {F * 2, F * 2 * T};
-    const uint32_t box[3] = {DH, ROWS, 1};
-    int rc = make_tmap_bf16(&tm, qkv, 3, dims, strides, box);
-    if (rc) return rc;
-    if (!attr_g) {
-      KDB_CUDA(set_attn_smem<MODE_GLOBAL>(ATTN_SMEM));
-      attr_g = true;
-    }
+    const uint64_t dims[3] = {F, T, (uint64_t)B}, dims_o[3] = {C, T, (uint64_t)B};
+    const uint64_t strides[2] = {F * 2, F * 2 * T}, strides_o[2] = {C * 2, C * 2 * T};
+    const uint32_t box[3] = {DH, ROWS, 1}, box_o[3] = {DH, 64, 1};
+    if ((rc = make_tmap_bf16(&tm, qkv, 3, dims, strides, box))) return rc;
+    if ((rc = make_tmap_bf16(&to, out, 3, dims_o, strides_o, box_o))) return rc;
     p.nblk = (int)(T / ROWS);
-    dim3 grid((unsigned)(T / ROWS), (unsigned)nh, (unsigned)B);
-    KDB_CUDA(launch_attn<MODE_GLOBAL>(grid, ATTN_SMEM, st, tm, tm, p));
+    p.n_tiles = B * nh * p.nblk;
+    KDB_CUDA(launch_ws<MODE_GLOBAL>(st, tm, to, p));
   }
   KDB_LAUNCH_CHECK(F_ATTN_TC, st);
   return 0;

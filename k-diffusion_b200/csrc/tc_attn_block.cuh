@@ -14,7 +14,7 @@
 //   k, q      : cosine-normalised in registers (a row's 64 columns sit in the 4 threads of a quad: two shfl_xor), x sqrt(scale_h),
 //               RoPE from the per-layer table (columns 2i, 2i+1 pair with 16+2i, 17+2i: same thread); k -> shared memory, q stays in
 //               registers as the A fragment of S = Q K^T (the accumulator fragment of two 8-column blocks is the A fragment of one k16 step)
-//   S = Q K^T : softmax in registers (row max and sum by quad shuffles), seam mask by quadrant as attn_tc_kernel; P is the A operand of
+//   S = Q K^T : softmax in registers (row max and sum by quad shuffles), seam mask by quadrant as attn_ws_kernel; P is the A operand of
 //   O = P V   : O / l -> bf16 A fragment, kept in registers
 //
 // and after both heads acc = sum_h O_h . Wout[:, 64h:64h+64]^T (wgmma, A from registers), the residual is added from the X tile still in shared memory, sum(x_new^2) is left for the fused RMSNorm of the

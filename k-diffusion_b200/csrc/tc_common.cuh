@@ -108,6 +108,11 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void*
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 // store: shared (SWIZZLE_128B tile) -> global, bulk-group completion
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
@@ -299,6 +304,16 @@ __device__ __forceinline__ void unpack_bf16x2(uint32_t v, float& lo, float& hi) 
 // 2-D..4-D bf16 tensor map with 128B swizzle; dims/strides innermost first (strides in bytes, for dims 1..rank-1).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box);
+
+// SM count of the current device: the grid of the persistent kernels
+inline int num_sms() {
+  static int n = [] {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kNumSMs;
+    return v;
+  }();
+  return n;
+}
 
 // ---------------------------------------------------------------- host: programmatic dependent launch
 // Launches `kernel` with programmatic stream serialization, so that its prologue overlaps the tail of the previous kernel in the

@@ -509,14 +509,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
   }
 }
 
-inline int num_sms() {
-  static int n = [] {
-    int dev = 0, v = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = kNumSMs;
-    return v;
-  }();
-  return n;
-}
 
 #include "tc_ffn_fused.cuh"
 #include "tc_attn_block.cuh"

@@ -82,7 +82,7 @@ def linear_macs(mcfg, batch=1):
 
 
 def attention_macs(mcfg, batch=1):
-    """q k^T and a v MACs of the attention that runs in the stand-alone attention kernels (attn_tc_kernel), i.e. of every level except
+    """q k^T and a v MACs of the attention that runs in the stand-alone attention kernels (attn_ws_kernel, attn_na_kernel), i.e. of every level except
     the `fused_attention_levels`, whose attention runs inside the fused attention-block kernel."""
     widths, depths, attns = mcfg["widths"], mcfg["depths"], mcfg["self_attns"]
     h, w = token_grid(mcfg)
