@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 12
+#define KDB_ABI_VERSION 13
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -347,6 +347,16 @@ int kdb_attention_jvp(const float* qkv, const float* dqkv, float* dout, int batc
                       int attn_type, int attn_param, int shift, void* stream);
 int kdb_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int batch, int h, int w,
                       int n_heads, int d_head, int attn_type, int attn_param, int shift, void* stream);
+
+/* The U-Net engine's fp32 convolution (ksize 1 or 3, zero padding ksize / 2, stride 1) as an implicit GEMM:
+ *   out[m, n] = bias[n] + sum_{tap, c} w[n, tap, c] * in(pixel m shifted by tap, c) + resid[m, n]
+ * Activations are token-major: in1 [batch, h, w, c1], in2 [batch, h, w, c2] (c2 = 0: one source; the input is the channel
+ * concatenation of the two), out [batch, h, w, n_out].  w_tapmajor is [n_out, ksize*ksize, c1 + c2], the layout
+ * kdb_unet_finalize derives from a torch weight [n_out, c1 + c2, ksize, ksize].  bias [n_out] may be NULL.  The residual
+ * [batch, h, w, n_out] is the concatenation of r1 (rc1 channels) and r2 (n_out - rc1 channels): r1 NULL = none, rc1 = n_out
+ * with r2 NULL = r1 alone.  c1, c2 and rc1 must be multiples of 4; batch * h * w is at most 65535 * 64 (KDB_ERR_BAD_SHAPE). */
+int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1, int rc1,
+                  const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
 
 #ifdef __cplusplus
 }

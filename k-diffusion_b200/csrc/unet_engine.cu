@@ -266,9 +266,14 @@ int kdb_unet_create(const KdbUNetConfig* cfg, KdbUNet** out) {
   KDB_REQUIRE(cfg->skip_stages >= 0 && cfg->skip_stages < cfg->n_levels, KDB_ERR_BAD_ARG, "unet_create: skip_stages %d", cfg->skip_stages);
   KDB_REQUIRE(cfg->mapping_cond_dim >= (cfg->augment_wrapper ? 9 : 0), KDB_ERR_BAD_ARG,
               "unet_create: the augment wrapper needs mapping_cond_dim >= 9");
-  for (int l = 0; l < cfg->n_levels; ++l)
+  for (int l = 0; l < cfg->n_levels; ++l) {
     KDB_REQUIRE(cfg->depth[l] >= 1 && cfg->channels[l] >= 4 && cfg->channels[l] % 4 == 0, KDB_ERR_UNSUPPORTED,
                 "unet_create: level %d needs depth >= 1 and a channel count that is a multiple of 4", l);
+    // a self-attention level attends at channels[l] and, in its UBlock's last layer, at channels[l - 1] (layers.py:184 asserts both)
+    for (int C : {cfg->channels[l], cfg->channels[std::max(0, l - 1)]})
+      KDB_REQUIRE(!cfg->self_attn[l] || C % std::max(1, C / 64) == 0, KDB_ERR_BAD_ARG,
+                  "unet_create: level %d self-attention width %d is not divisible by its %d heads", l, C, std::max(1, C / 64));
+  }
   KdbUNet* m = new KdbUNet();
   m->cfg = *cfg;
   *out = m;
@@ -405,6 +410,14 @@ int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacit
 int64_t kdb_unet_tap_count(const KdbUNet* m) {
   KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_tap_count: NULL handle");
   return m->tap_count;
+}
+
+int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1, int rc1,
+                  const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream) {
+  ConvArgs a;
+  a.in1 = in1, a.c1 = c1, a.in2 = in2, a.c2 = c2, a.w = w_tapmajor, a.bias = bias, a.r1 = r1, a.rc1 = rc1, a.r2 = r2, a.out = out;
+  a.B = batch, a.H = h, a.W = w, a.N = n_out;
+  return launch_unet_conv(a, ksize, (cudaStream_t)stream);
 }
 
 }  // extern "C"

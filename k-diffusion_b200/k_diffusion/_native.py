@@ -19,7 +19,7 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 PREC_FP32, PREC_BF16 = 0, 1
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -93,6 +93,7 @@ SIGNATURES = {
     "kdb_attention": (_i32, [_i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_attention_jvp": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_attention_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_unet_conv": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
 }
 
 _lib = None
@@ -646,6 +647,23 @@ def attention(qkv, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, fast
     code = _ATTN_CODE[attn_type] if isinstance(attn_type, str) else attn_type
     check(lib().kdb_attention(prec, 1 if fast else 0, ptr(qkv.contiguous()), ptr(out), B, h, w, n_heads, d_head, code, attn_param, shift,
                                ptr(logit_bound), stream()))
+    return out
+
+
+@_on_device_of_first
+def unet_conv(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
+    """The U-Net engine's convolution (kdb_unet_conv): x1 [B,h,w,c1] and x2 [B,h,w,c2] token-major fp32 (their channel concatenation is
+    the input), w the tap-major weight [N, ksize*ksize, c1 + c2], bias [N], the residual [B,h,w,N] given as r1 (the first rc1 channels,
+    all N without r2) and r2 (the rest) -> out [B,h,w,N]."""
+    require_cuda(x1, w, x2, bias, r1, r2, out)
+    B, h, wd, c1 = x1.shape
+    N = w.shape[0]
+    c2 = 0 if x2 is None else x2.shape[-1]
+    rc1 = 0 if r1 is None else r1.shape[-1]
+    if out is None:
+        out = torch.empty(B, h, wd, N, dtype=torch.float32, device=x1.device)
+    x1, x2, w, bias, r1, r2 = (None if t is None else f32c(t) for t in (x1, x2, w, bias, r1, r2))
+    check(lib().kdb_unet_conv(ptr(x1), c1, ptr(x2), c2, ptr(w), ptr(bias), ptr(r1), rc1, ptr(r2), ptr(out), B, h, wd, N, ksize, stream()))
     return out
 
 

@@ -110,6 +110,53 @@ def block_modules(depth, c_in, c_mid, c_out, attn, first):
     return mods, idx
 
 
+def stage_plan(mcfg):
+    """The native engine's debug taps after patch_in, in execution order: tap name -> (tap of its input, op, tap of the DBlock output
+    concatenated to the input by a UBlock or None, level whose grid the output is on).  op is ("res" | "attn", state-dict prefix, c_in,
+    c_mid, c_out), "down" or "up"; stage_op applies it."""
+    depths, channels, attn, n = mcfg["depths"], mcfg["channels"], mcfg["self_attn_depths"], len(mcfg["depths"])
+    s0 = mcfg.get("skip_stages", 0)
+    stages, skips, prev = {}, {}, "patch_in"
+    for i in range(s0, n):
+        if i > s0:
+            stages[f"d{i}.down"] = (prev, "down", None, i)
+            prev = f"d{i}.down"
+        mods, _ = block_modules(depths[i], channels[max(0, i - 1)], channels[i], channels[i], attn[i], 1)
+        for idx, kind, ci, cm, co in mods:
+            stages[f"d{i}.{idx}"] = (prev, (kind, f"u_net.d_blocks.{i}.{idx}.", ci, cm, co), None, i)
+            prev = f"d{i}.{idx}"
+        skips[i] = prev
+    for i in range(n - 1, s0 - 1, -1):
+        k = n - 1 - i                                          # u_net.u_blocks holds the UBlocks innermost first
+        c_in = channels[i] * 2 if i < n - 1 else channels[i]
+        mods, _ = block_modules(depths[i], c_in, channels[i], channels[max(0, i - 1)], attn[i], 0)
+        for j, (idx, kind, ci, cm, co) in enumerate(mods):
+            stages[f"u{i}.{idx}"] = (prev, (kind, f"u_net.u_blocks.{k}.{idx}.", ci, cm, co), skips[i] if (j == 0 and i < n - 1) else None, i)
+            prev = f"u{i}.{idx}"
+        if i > s0:
+            stages[f"u{i}.up"] = (prev, "up", None, i - 1)
+            prev = f"u{i}.up"
+    return stages
+
+
+def stage_op(sd, op, x, cond):
+    """one stage of stage_plan applied to its (concatenated) input"""
+    if op == "down":
+        return downsample(x)
+    if op == "up":
+        return upsample(x)
+    kind, p, c_in, c_mid, c_out = op
+    return res_conv_block(sd, p, x, cond, c_in, c_mid, c_out) if kind == "res" else self_attention(sd, p, x, cond)
+
+
+def level_hw(mcfg, H, W, level):
+    """token grid of `level` for an H x W input (patch_size, then one halving per level past skip_stages)"""
+    h, w = H // mcfg["patch_size"], W // mcfg["patch_size"]
+    for _ in range(mcfg.get("skip_stages", 0), level):
+        h, w = h // 2, w // 2
+    return h, w
+
+
 def model_forward(sd, mcfg, x, sigma, mapping_cond=None, taps=None):
     """image_v1.py:135-157 and layers.py:305-312 (UNet.forward)"""
     depths, channels, attn = mcfg["depths"], mcfg["channels"], mcfg["self_attn_depths"]

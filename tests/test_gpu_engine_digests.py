@@ -38,7 +38,8 @@ def _nan_workspace(eng, need):
 def unet_digests(name):
     from conftest import load_npz
     from k_diffusion import _native
-    from test_gpu_unet import _stage_inputs, build
+    from oracle.unet_oracle import stage_plan
+    from test_gpu_unet import build
     cfg, _, model, den = build(name)
     eng = model.engine()
     z = load_npz(f"unet_{name}.npz")
@@ -54,7 +55,7 @@ def unet_digests(name):
     rec["cond"] = _digest(eng.conditioning(sig))
     rec["cond aug"] = _digest(eng.conditioning(sig, aug))
     cond = eng.conditioning(sig, aug)
-    for tap in ["patch_in", *_stage_inputs(cfg["model"])]:
+    for tap in ["patch_in", *stage_plan(cfg["model"])]:
         _nan_workspace(eng, need)
         buf = eng.arm_tap(tap, 1 << 24, x.device)
         eng.forward(x, sig, cond, eng.cond_stride, 0.0, _native.PREC_FP32)

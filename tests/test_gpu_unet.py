@@ -19,9 +19,9 @@ META = json.loads((GOLDEN / "unet_configs.json").read_text())
 DEV = "cuda"
 
 
-def build(name):
-    cfg = K.config.load_config(META[name]["config"])
-    sd = synth_sd(META[name]["shapes"], 1)
+def build(name, meta=META):
+    cfg = K.config.load_config(meta[name]["config"])
+    sd = synth_sd(meta[name]["shapes"], 1)
     model = K.config.make_model(cfg).eval().requires_grad_(False)
     model.load_state_dict(sd)
     model = model.to(DEV)
@@ -41,86 +41,70 @@ def test_forward_matches_reference_and_oracle(name):
     assert_close(got_aug, want, what=f"{name} aug_cond vs oracle")
 
 
-def _stage_inputs(mcfg):
-    """tap name -> (tap name of its input, oracle function of (input NCHW float64, cond float64), skip tap for the UBlock concat)"""
-    depths, channels, attn, n = mcfg["depths"], mcfg["channels"], mcfg["self_attn_depths"], len(mcfg["depths"])
-    stages, prev = {}, "patch_in"
-    for i in range(n):
-        if i > 0:
-            stages[f"d{i}.down"] = (prev, lambda x, c: U.downsample(x), None)
-            prev = f"d{i}.down"
-        mods, _ = U.block_modules(depths[i], channels[max(0, i - 1)], channels[i], channels[i], attn[i], 1)
-        for idx, kind, ci, cm, co in mods:
-            stages[f"d{i}.{idx}"] = (prev, (kind, f"u_net.d_blocks.{i}.{idx}.", ci, cm, co), None)
-            prev = f"d{i}.{idx}"
-    skips = [f"d{i}.{U.block_modules(depths[i], 0, 0, 0, attn[i], 1)[1] - 1}" for i in range(n)]
-    for k in range(n):
-        i = n - 1 - k
-        c_in = channels[i] * 2 if i < n - 1 else channels[i]
-        mods, _ = U.block_modules(depths[i], c_in, channels[i], channels[max(0, i - 1)], attn[i], 0)
-        for j, (idx, kind, ci, cm, co) in enumerate(mods):
-            stages[f"u{i}.{idx}"] = (prev, (kind, f"u_net.u_blocks.{k}.{idx}.", ci, cm, co), skips[i] if (j == 0 and k > 0) else None)
-            prev = f"u{i}.{idx}"
-        if i > 0:
-            stages[f"u{i}.up"] = (prev, lambda x, c: U.upsample(x), None)
-            prev = f"u{i}.up"
-    return stages
+def unet_engine(model, mcfg):
+    """the native engine of a make_model result, with the conditioning its config's wrapper forms"""
+    augment = mcfg["augment_wrapper"]
+    return (model.inner_model if augment else model).engine(augment=augment)
 
 
-@pytest.mark.parametrize("name", ["mnist", "cifar10"])
-def test_every_stage_against_the_oracle(name):
-    """Each tap is checked against the oracle's restatement of its stage applied (in float64) to the engine's own tapped input, after
-    the workspace was filled with NaN: conv3x3 at borders on 28/14/7 and 32/16/8 grids, the skip conv with c_in != c_out on the
-    two-source concat, AdaGN, attention, down- and upsampling, patch-in."""
-    cfg, sd, model, _ = build(name)
+def oracle_mapping_cond(mcfg, B, aug=None, mc=None):
+    """the mapping_cond the bare model sees (augmentation.py:97-104): [aug_cond or zeros(9), mapping_cond] with the wrapper"""
+    if not mcfg["augment_wrapper"]:
+        return mc
+    a = torch.zeros(B, 9, dtype=torch.float64) if aug is None else aug
+    return a if mc is None else torch.cat([a, mc], dim=1)
+
+
+def check_every_stage(name, cfg, sd, model, x, sig, aug=None, mc=None):
+    """Each tap against the oracle's restatement of its stage applied (in float64) to the engine's own tapped input, after the workspace
+    was filled with NaN; every tap holds exactly B * h * w * C floats, with (h, w) the grid of its level."""
     mcfg = cfg["model"]
-    unet = model.inner_model
-    B, (H, W) = 2, mcfg["input_size"]
-    g = torch.Generator().manual_seed(5)
-    x = torch.randn(B, mcfg["input_channels"], H, W, generator=g).to(DEV)
-    sig = torch.tensor([0.7, 9.0], device=DEV)
-    aug = (torch.randn(B, 9, generator=g) * 0.5).to(DEV)
-    eng = unet.engine(augment=True)
-    cond = eng.conditioning(sig, aug)
+    eng = unet_engine(model, mcfg)
+    B, _, H, W = x.shape
+    cond = eng.conditioning(sig, aug, mapping_cond=mc)
     sd64 = {k: v.double() for k, v in sd.items()}
-    cond_want = U.mapping(sd64, sig.cpu().double(), aug.cpu().double())
-    assert_close(cond[:, -mcfg["mapping_out"]:], cond_want, rtol=1e-4, atol=1e-5, what="conditioning: mapping net")
-    c64 = cond_want
+    c64 = U.mapping(sd64, sig.cpu().double(), oracle_mapping_cond(mcfg, B, *(None if t is None else t.cpu().double() for t in (aug, mc))))
+    assert_close(cond[:, -mcfg["mapping_out"]:], c64, rtol=1e-4, atol=1e-5, what=f"{name} conditioning: mapping net")
 
-    def run_tap(tap):
+    def run_tap(tap, level, c):
         need = eng.workspace_bytes(K._native.PREC_FP32, B, H, W)
         ws = eng._reserve(need, x.device)
         ws.view(torch.uint8)[: need - need % 4].view(torch.float32).fill_(float("nan"))
         buf = eng.arm_tap(tap, 1 << 24, x.device)
         eng.forward(x, sig, cond, eng.cond_stride, 0.0, K._native.PREC_FP32)
-        n = eng.tap_count()
-        assert n > 0, tap
-        return buf[:n]
-
-    def nchw(t, c):
-        h = int(round((t.numel() / (B * c)) ** 0.5))
-        return t.view(B, h, -1, c).permute(0, 3, 1, 2).cpu().double()
-
-    stages = _stage_inputs(mcfg)
-    got_pin = nchw(run_tap("patch_in"), mcfg["channels"][0])
-    want_pin = F.conv2d(x.cpu().double(), sd64["proj_in.weight"], sd64["proj_in.bias"])
-    assert_close(got_pin, want_pin, rtol=1e-4, atol=1e-5, what="patch_in")
-    outs = {"patch_in": got_pin}
-    for tap, (src, op, skip) in stages.items():
-        inp = outs[src]
-        if skip is not None:
-            inp = torch.cat([inp, outs[skip]], dim=1)
-        if isinstance(op, tuple):
-            kind, p, ci, cm, co = op
-            want = U.res_conv_block(sd64, p, inp, c64, ci, cm, co) if kind == "res" else U.self_attention(sd64, p, inp, c64)
-            c_out = co
-        else:
-            want = op(inp, c64)
-            c_out = inp.shape[1]
-        got = nchw(run_tap(tap), c_out)
+        h, w = U.level_hw(mcfg, H, W, level)
+        assert eng.tap_count() == B * h * w * c, (tap, eng.tap_count(), (B, h, w, c))
+        got = buf[: B * h * w * c].view(B, h, w, c).permute(0, 3, 1, 2).cpu().double()
         assert torch.isfinite(got).all(), tap
+        return got
+
+    s0, p = mcfg.get("skip_stages", 0), mcfg["patch_size"]
+    got_pin = run_tap("patch_in", s0, mcfg["channels"][max(0, s0 - 1)])
+    x64 = x.cpu().double()
+    want_pin = F.conv2d(F.pixel_unshuffle(x64, p) if p > 1 else x64, sd64["proj_in.weight"], sd64["proj_in.bias"])
+    assert_close(got_pin, want_pin, rtol=1e-4, atol=1e-5, what=f"{name} patch_in")
+    outs = {"patch_in": got_pin}
+    for tap, (src, op, skip, level) in U.stage_plan(mcfg).items():
+        inp = outs[src] if skip is None else torch.cat([outs[src], outs[skip]], dim=1)
+        want = U.stage_op(sd64, op, inp, c64)
+        got = run_tap(tap, level, want.shape[1])
         assert_close(got, want, rtol=1e-3, atol=1e-4, what=f"{name} stage {tap}")
         outs[tap] = got
+    return len(outs)
+
+
+@pytest.mark.parametrize("name", ["mnist", "cifar10"])
+def test_every_stage_against_the_oracle(name):
+    """conv3x3 at borders on 28/14/7 and 32/16/8 grids, the skip conv with c_in != c_out on the two-source concat, AdaGN, attention,
+    down- and upsampling, patch-in"""
+    cfg, sd, model, _ = build(name)
+    mcfg = cfg["model"]
+    B, (H, W) = 2, mcfg["input_size"]
+    g = torch.Generator().manual_seed(5)
+    x = torch.randn(B, mcfg["input_channels"], H, W, generator=g).to(DEV)
+    sig = torch.tensor([0.7, 9.0], device=DEV)
+    aug = (torch.randn(B, 9, generator=g) * 0.5).to(DEV)
+    check_every_stage(name, cfg, sd, model, x, sig, aug)
 
 
 def test_samplers_through_the_graph_executor_match_the_oracle():
