@@ -12,12 +12,11 @@
 //            rows of a window are quadrant-major, then (row, column) inside the quadrant.
 //   GLOBAL : the tile is 128 queries of one (image, head); keys and values are streamed in blocks of 128 through a ring of stages that
 //            both warpgroups read (S = 64 x 128 per warpgroup, m64n128k16).
-//   Roles: warpgroup 2 is the producer (40 registers): one elected lane loads by TMA the Q tile of every tile (WS_QBUF buffers) and its
-//   key blocks (WS_KV_STAGES stages of K and V), so the next tile loads while the current one computes.  Warpgroups 0 and 1 (232
-//   registers): S = Q K^T into registers, softmax in registers (a row's columns sit in the 4 threads of a quad: max and sum by two
-//   shuffles), P rounded to bf16 is the register A operand of O += P V (V an MN-major operand straight from the TMA tile), O stays in
-//   registers across the key blocks and is scaled by 1/l once; the bf16 output is staged in shared memory and leaves by TMA (the
-//   quadrant boxes for windows).
+//   Roles: warpgroup 2 is the producer: one elected lane loads by TMA the Q tile of every tile (WS_QBUF buffers) and its key blocks
+//   (WS_KV_STAGES stages of K and V), so the next tile loads while the current one computes.  Warpgroups 0 and 1: S = Q K^T into
+//   registers, softmax in registers (a row's columns sit in the 4 threads of a quad: max and sum by two shuffles), P rounded to bf16
+//   is the register A operand of O += P V (V an MN-major operand straight from the TMA tile), O stays in registers across the key
+//   blocks and is scaled by 1/l once; the bf16 output is staged in shared memory and leaves by TMA (the quadrant boxes for windows).
 //   Softmax: with the bound (below) a single pass with the fixed shift exp(s - bound); without it the row maximum: GLOBAL keeps a running
 //   maximum and rescales O and l when it grows (exact: the result is that of the final maximum), WINDOW has one key block.
 // NA: attn_na_kernel, one CTA = one 128-query block of one head (160 threads).  7x7 neighbourhood (NATTEN definition: window clamped
@@ -63,7 +62,8 @@ constexpr int WS_THREADS = 384;
 constexpr int WS_QBUF = 4, WS_KV_STAGES = 4;
 
 struct WsBars {
-  uint64_t q_full[WS_QBUF], q_empty[WS_QBUF], kv_full[WS_KV_STAGES], kv_empty[WS_KV_STAGES];
+  tc::TmaRing<WS_QBUF> q;
+  tc::TmaRing<WS_KV_STAGES> kv;
 };
 // Q buffers, K and V stages, one output staging tile per warpgroup
 constexpr size_t WS_SMEM = (size_t)WS_QBUF * TILE_BYTES + (size_t)WS_KV_STAGES * 2 * TILE_BYTES + 2 * HALF_BYTES + sizeof(WsBars) + 1024;
@@ -108,14 +108,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tm_in);
     tc::tma_prefetch_desc(&tm_out);
-    for (int i = 0; i < WS_QBUF; ++i) {
-      tc::mbar_init(&bars->q_full[i], 1);
-      tc::mbar_init(&bars->q_empty[i], 8);    // lane 0 of every MMA warp
-    }
-    for (int i = 0; i < WS_KV_STAGES; ++i) {
-      tc::mbar_init(&bars->kv_full[i], 1);
-      tc::mbar_init(&bars->kv_empty[i], 8);
-    }
+    bars->q.init(tc::REL_WARPS_2WG);
+    bars->kv.init(tc::REL_WARPS_2WG);
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -124,7 +118,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    tc::setmaxnreg_dec<40>();
+    tc::setmaxnreg_dec<tc::PRODUCER_REGS>();
     if (warp == 8 && tc::elect_one()) {
       // the window of heads head0, head0 + 1, third t of qkv (0 q, 1 k, 2 v): two 64-row halves of four quadrant boxes
       auto load_window = [&](uint8_t* dst, int t, uint64_t* bar, int b, int wi, int wj, int head0) {
@@ -137,32 +131,25 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
             tc::tma_load_4d(dst + hd * HALF_BYTES + q * 2048, &tm_in, bar, (t * p.nh + head0 + hd) * DH, c, r, b);
           }
       };
-      int kv = 0;
-      for (int i = 0; i < n_local; ++i) {
-        const int tile = (int)blockIdx.x + i * (int)gridDim.x, qb = i % WS_QBUF;
-        tc::mbar_wait_nocall(&bars->q_empty[qb], (uint32_t)(((i / WS_QBUF) & 1) ^ 1));
-        tc::mbar_arrive_expect_tx(&bars->q_full[qb], TILE_BYTES);
-        uint8_t* q_dst = sQ + qb * TILE_BYTES;
-        if constexpr (MODE == MODE_WINDOW) {
-          int b, wi, wj, head0;
-          ws_window(p, tile, b, wi, wj, head0);
-          load_window(q_dst, 0, &bars->q_full[qb], b, wi, wj, head0);
-          const int st = kv % WS_KV_STAGES;
-          tc::mbar_wait_nocall(&bars->kv_empty[st], (uint32_t)(((kv / WS_KV_STAGES) & 1) ^ 1));
-          tc::mbar_arrive_expect_tx(&bars->kv_full[st], 2 * TILE_BYTES);
-          load_window(sKV + st * 2 * TILE_BYTES, 1, &bars->kv_full[st], b, wi, wj, head0);
-          load_window(sKV + st * 2 * TILE_BYTES + TILE_BYTES, 2, &bars->kv_full[st], b, wi, wj, head0);
-          ++kv;
-        } else {
-          int b, head, m;
-          ws_global(p, tile, b, head, m);
-          tc::tma_load_3d(q_dst, &tm_in, &bars->q_full[qb], head * DH, m * ROWS, b);
-          for (int j = 0; j < nblk; ++j, ++kv) {
-            const int st = kv % WS_KV_STAGES;
-            tc::mbar_wait_nocall(&bars->kv_empty[st], (uint32_t)(((kv / WS_KV_STAGES) & 1) ^ 1));
-            tc::mbar_arrive_expect_tx(&bars->kv_full[st], 2 * TILE_BYTES);
-            tc::tma_load_3d(sKV + st * 2 * TILE_BYTES, &tm_in, &bars->kv_full[st], (p.nh + head) * DH, j * ROWS, b);
-            tc::tma_load_3d(sKV + st * 2 * TILE_BYTES + TILE_BYTES, &tm_in, &bars->kv_full[st], (2 * p.nh + head) * DH, j * ROWS, b);
+      PipeState<WS_QBUF> qs{};
+      PipeState<WS_KV_STAGES> ks{};
+      for (int i = 0; i < n_local; ++i, qs.advance()) {
+        const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+        int b, head, wi = 0, wj = 0, m = 0;
+        if constexpr (MODE == MODE_WINDOW) ws_window(p, tile, b, wi, wj, head);
+        else ws_global(p, tile, b, head, m);
+        uint64_t* bar = bars->q.acquire(qs, TILE_BYTES);
+        if constexpr (MODE == MODE_WINDOW) load_window(sQ + qs.slot * TILE_BYTES, 0, bar, b, wi, wj, head);
+        else tc::tma_load_3d(sQ + qs.slot * TILE_BYTES, &tm_in, bar, head * DH, m * ROWS, b);
+        for (int j = 0; j < nblk; ++j, ks.advance()) {     // WINDOW: one key block
+          bar = bars->kv.acquire(ks, 2 * TILE_BYTES);
+          uint8_t* k_dst = sKV + ks.slot * 2 * TILE_BYTES;
+          if constexpr (MODE == MODE_WINDOW) {
+            load_window(k_dst, 1, bar, b, wi, wj, head);
+            load_window(k_dst + TILE_BYTES, 2, bar, b, wi, wj, head);
+          } else {
+            tc::tma_load_3d(k_dst, &tm_in, bar, (p.nh + head) * DH, j * ROWS, b);
+            tc::tma_load_3d(k_dst + TILE_BYTES, &tm_in, bar, (2 * p.nh + head) * DH, j * ROWS, b);
           }
         }
       }
@@ -171,15 +158,16 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
   }
 
   // ------------------------------------------------------------------ MMA warpgroups: 64 query rows each
-  tc::setmaxnreg_inc<232>();
+  tc::setmaxnreg_inc<tc::MMA_REGS>();
   const int wg = warp >> 2, t = threadIdx.x & 127;
   const int rw = 16 * (t >> 5) + (lane >> 2);                // this thread's two rows of the warpgroup's 64: rw and rw + 8
   const int cq = 2 * (lane & 3);                             // and its column pair inside every 8-column block
   const int quad = rw >> 4;                                  // WINDOW: the quadrant of both rows
   uint8_t* sOw = sO + wg * HALF_BYTES;
-  int kv = 0;
-  for (int i = 0; i < n_local; ++i) {
-    const int tile = (int)blockIdx.x + i * (int)gridDim.x, qb = i % WS_QBUF;
+  PipeState<WS_QBUF> qs{};
+  PipeState<WS_KV_STAGES> ks{};
+  for (int i = 0; i < n_local; ++i, qs.advance()) {
+    const int tile = (int)blockIdx.x + i * (int)gridDim.x;
     int b, head, wi = 0, wj = 0, m = 0;
     if constexpr (MODE == MODE_WINDOW) {
       ws_window(p, tile, b, wi, wj, head);
@@ -194,13 +182,12 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
     float o[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) o[j] = 0.f;
-    const uint64_t qdesc = tc::smem_desc_k_sw128(tc::smem_u32(sQ + qb * TILE_BYTES + wg * HALF_BYTES));
-    tc::mbar_wait_nocall(&bars->q_full[qb], (uint32_t)((i / WS_QBUF) & 1));
-    for (int j = 0; j < nblk; ++j, ++kv) {
-      const int st = kv % WS_KV_STAGES;
-      const uint32_t k_addr = tc::smem_u32(sKV + st * 2 * TILE_BYTES) + (MODE == MODE_WINDOW ? wg * HALF_BYTES : 0);
+    const uint64_t qdesc = tc::smem_desc_k_sw128(tc::smem_u32(sQ + qs.slot * TILE_BYTES + wg * HALF_BYTES));
+    bars->q.wait(qs);
+    for (int j = 0; j < nblk; ++j, ks.advance()) {
+      const uint32_t k_addr = tc::smem_u32(sKV + ks.slot * 2 * TILE_BYTES) + (MODE == MODE_WINDOW ? wg * HALF_BYTES : 0);
       const uint32_t v_addr = k_addr + TILE_BYTES;
-      tc::mbar_wait_nocall(&bars->kv_full[st], (uint32_t)((kv / WS_KV_STAGES) & 1));
+      bars->kv.wait(ks);
       // ---- S = Q K^T
       float s[NK / 2];
 #pragma unroll
@@ -218,7 +205,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
       tc::wg_commit();
       tc::wg_wait<0>();
       tc::wg_fence_acc(s);
-      if (j == nblk - 1 && lane == 0) tc::mbar_arrive(&bars->q_empty[qb]);   // every read of this Q tile is done
+      if (j == nblk - 1 && lane == 0) bars->q.release(qs);   // every read of this Q tile is done
       // ---- softmax in registers.  Key column 8 c + cq (+1); WINDOW: it lies in quadrant c / 2, and the seam mask keeps a query to keys
       // on its own side of the wrapped row / column of the top / left windows.
       auto key_ok = [&](int c) -> bool {
@@ -278,7 +265,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
       tc::wg_commit();
       tc::wg_wait<0>();
       tc::wg_fence_acc(o);
-      if (lane == 0) tc::mbar_arrive(&bars->kv_empty[st]);
+      if (lane == 0) bars->kv.release(ks);
     }
     // ---- O / l -> bf16 staging tile (rows = this warpgroup's 64 queries) -> TMA store
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
@@ -287,14 +274,14 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
     l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
     const float inv0 = 1.f / l0, inv1 = 1.f / l1;
     if (t == 0) tc::tma_store_wait_read();    // the previous tile's store has read the staging tile
-    tc::named_barrier_sync(1 + wg, 128);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
       *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw, c) + cq * 2) = tc::pack_bf16x2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
       *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw + 8, c) + cq * 2) = tc::pack_bf16x2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
     }
     tc::fence_proxy_async();                   // staging tile (generic-proxy writes) -> visible to the TMA engine
-    tc::named_barrier_sync(1 + wg, 128);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
     if (t == 0) {
       if constexpr (MODE == MODE_WINDOW) {
 #pragma unroll
@@ -314,7 +301,8 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
 
 // ================================================================ NA
 struct Bars {
-  uint64_t q, kv, kv_free;
+  uint64_t q;
+  tc::TmaRing<1> kv;
 };
 
 template <bool BOUNDED>
@@ -346,8 +334,7 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmap);
     tc::mbar_init(&bars->q, 1);
-    tc::mbar_init(&bars->kv, 1);
-    tc::mbar_init(&bars->kv_free, 4);          // lane 0 of each warp of the warpgroup
+    bars->kv.init(tc::REL_WARPS);
     tc::fence_barrier_init();
   }
   // rows 110..127 of the V tile are never written by TMA: they must be finite (P there is exactly 0)
@@ -366,11 +353,10 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
       for (int it = 0; it < n_iter; ++it) {
         const int j = it % nblk;
         const bool with_v = !two_pass || it >= nblk;
-        if (it > 0) tc::mbar_wait_nocall(&bars->kv_free, (uint32_t)(it - 1) & 1u);
         constexpr uint32_t KV_BYTES = NA_BLK_KEYS * 128;
-        tc::mbar_arrive_expect_tx(&bars->kv, with_v ? 2 * KV_BYTES : KV_BYTES);
-        tc::tma_load_4d(sK, &tmap_kv, &bars->kv, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
-        if (with_v) tc::tma_load_4d(sV, &tmap_kv, &bars->kv, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
+        uint64_t* bar = bars->kv.acquire(PipeState<1>::at(it), with_v ? 2 * KV_BYTES : KV_BYTES);
+        tc::tma_load_4d(sK, &tmap_kv, bar, (nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
+        if (with_v) tc::tma_load_4d(sV, &tmap_kv, bar, (2 * nh + head0) * DH, c0, r0 + j * NA_BLK_ROWS, b);
       }
     }
     return;
@@ -396,7 +382,7 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
   for (int it = 0; it < n_iter; ++it) {
     const int j = it % nblk;
     const int pass = (two_pass && it < nblk) ? 0 : 1;
-    tc::mbar_wait_nocall(&bars->kv, (uint32_t)it & 1u);
+    bars->kv.wait(PipeState<1>::at(it));
     // S = Q K^T, one M = 64 half at a time -> fp32 tile
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
@@ -413,7 +399,7 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
       tc::wg_fence_acc(s);
       tc::acc_store(sS, S_LD, 64 * h, s);
     }
-    tc::named_barrier_sync(1, 128);            // S complete; every read of Q and K is done
+    tc::named_barrier_sync(tc::BAR_WG, 128);            // S complete; every read of Q and K is done
     if (pass == 0) {
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
@@ -458,7 +444,7 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
     }
     if (pass == 1) {
       tc::fence_proxy_async();                 // P (generic-proxy writes) -> visible to the tensor core
-      tc::named_barrier_sync(1, 128);
+      tc::named_barrier_sync(tc::BAR_WG, 128);
       tc::wg_fence_acc(o0);
       tc::wg_fence_acc(o1);
       tc::wg_fence();
@@ -474,13 +460,13 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
       tc::wg_fence_acc(o0);
       tc::wg_fence_acc(o1);
     }
-    tc::named_barrier_sync(1, 128);            // S, K, V and P are free for the next key block
-    if (lane == 0 && it + 1 < n_iter) tc::mbar_arrive(&bars->kv_free);
+    tc::named_barrier_sync(tc::BAR_WG, 128);            // S, K, V and P are free for the next key block
+    if (lane == 0 && it + 1 < n_iter) bars->kv.release(PipeState<1>::at(it));   // none after the last block: its phase is never waited for
   }
   // ------------------------------------------------------ O / l -> out
   tc::acc_store(sS, S_LD, 0, o0);
   tc::acc_store(sS, S_LD, 64, o1);
-  tc::named_barrier_sync(1, 128);
+  tc::named_barrier_sync(tc::BAR_WG, 128);
   const float inv = 1.f / l;
   const int64_t token = (int64_t)na_qi * p.w + na_qj;
   uint4* dst = reinterpret_cast<uint4*>(p.out + (((int64_t)b * p.h * p.w + token) * nh + head0) * DH);

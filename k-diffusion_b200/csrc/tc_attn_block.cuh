@@ -26,10 +26,9 @@
 // then (row, column) inside the quadrant -- the seam-mask regions (:300-315) are whole quadrants.
 //
 // Roles (384 threads, one CTA per SM, tiles of two windows blockIdx.x, + gridDim.x, ...):
-//   warpgroups 0, 1   window 2 tile + wg; the second warpgroup of the last tile idles when the number of windows is odd.  232 registers
-//                     each: the V, K and Q accumulators of a head are live together, and the RoPE table entries load under the MMAs
-//   warpgroup 2       producer (40 registers): one elected lane of warp 8 loads by TMA the weights once per CTA, then the X tiles
-//                     (2 buffers)
+//   warpgroups 0, 1   window 2 tile + wg; the second warpgroup of the last tile idles when the number of windows is odd.  The V, K
+//                     and Q accumulators of a head are live together, and the RoPE table entries load under the MMAs
+//   warpgroup 2       producer: one elected lane of warp 8 loads by TMA the weights once per CTA, then the X tiles (2 buffers)
 // Shared memory: X 2 x 32 KiB, Wqkv 96 KiB, Wout 32 KiB, K and V per warpgroup 4 x 8 KiB = 224 KiB.
 #pragma once
 
@@ -42,7 +41,8 @@ constexpr int AB_KV_BYTES = 64 * 128;              // one [64 tokens x 64] bf16 
 constexpr int AB_THREADS = 256 + 128;
 
 struct AttnBlockBars {
-  uint64_t w_full, x_full[AB_XBUF], x_empty[AB_XBUF];
+  uint64_t w_full;
+  tc::TmaRing<AB_XBUF> x;
 };
 constexpr size_t AB_SMEM = (size_t)AB_XBUF * AB_X_BYTES + 2 * AB_WQKV_KB + AB_WO_BYTES + 4 * AB_KV_BYTES + sizeof(AttnBlockBars) + 1024;
 
@@ -87,10 +87,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     tc::tma_prefetch_desc(&tmwq);
     tc::tma_prefetch_desc(&tmwo);
     tc::mbar_init(&bars->w_full, 1);
-    for (int i = 0; i < AB_XBUF; ++i) {
-      tc::mbar_init(&bars->x_full[i], 1);
-      tc::mbar_init(&bars->x_empty[i], 2);     // one store-drained arrival per warpgroup
-    }
+    bars->x.init(tc::REL_THREAD_2WG);          // once its store has read the window
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -101,7 +98,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
 
   if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    tc::setmaxnreg_dec<40>();
+    tc::setmaxnreg_dec<tc::PRODUCER_REGS>();
     if (pwarp == 8 && tc::elect_one()) {
       tc::mbar_arrive_expect_tx(&bars->w_full, 2 * AB_WQKV_KB + AB_WO_BYTES);
 #pragma unroll
@@ -110,12 +107,11 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
         tc::tma_load_2d(sWQ + kb * AB_WQKV_KB + 192 * 128, &tmwq, &bars->w_full, kb * BK, 192);
         tc::tma_load_2d(sWO + kb * A_STAGE_BYTES, &tmwo, &bars->w_full, kb * BK, 0);
       }
-      for (int i = 0; i < n_local; ++i) {
-        const int buf = i & 1;
+      PipeState<AB_XBUF> xs{};
+      for (int i = 0; i < n_local; ++i, xs.advance()) {
         const int win0 = 2 * ((int)blockIdx.x + i * (int)gridDim.x);
         const int nw = p.nwin - win0 < 2 ? 1 : 2;
-        tc::mbar_wait_nocall(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
-        tc::mbar_arrive_expect_tx(&bars->x_full[buf], (uint32_t)nw * 2u * AB_KV_BYTES);
+        uint64_t* bar = bars->x.acquire(xs, (uint32_t)nw * 2u * AB_KV_BYTES);
         for (int s = 0; s < nw; ++s) {
           int b, wi, wj;
           ab_window(p, win0 + s, b, wi, wj);
@@ -125,7 +121,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
             ab_quad(p, wi, wj, q, r, c);
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb)
-              tc::tma_load_4d(sX + (size_t)buf * AB_X_BYTES + kb * A_STAGE_BYTES + s * AB_KV_BYTES + q * 2048, &tmx, &bars->x_full[buf], kb * BK, c, r, b);
+              tc::tma_load_4d(sX + (size_t)xs.slot * AB_X_BYTES + kb * A_STAGE_BYTES + s * AB_KV_BYTES + q * 2048, &tmx, bar, kb * BK, c, r, b);
           }
         }
       }
@@ -134,7 +130,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   }
 
   // ------------------------------------------------------------------ warpgroups: one window each
-  tc::setmaxnreg_inc<232>();
+  tc::setmaxnreg_inc<tc::MMA_REGS>();
   const int wg = pwarp >> 2, t = threadIdx.x & 127;
   const int rw = 16 * (t >> 5) + (lane >> 2);                // this thread's two window rows: rw and rw + 8 (same quadrant)
   const int r0 = 64 * wg + rw;                               // ... as rows of the X tile
@@ -200,8 +196,8 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   };
 
   tc::mbar_wait_nocall(&bars->w_full, 0);
-  for (int i = 0; i < n_local; ++i) {
-    const int buf = i & 1;
+  PipeState<AB_XBUF> xs{};
+  for (int i = 0; i < n_local; ++i, xs.advance()) {
     const int win = 2 * ((int)blockIdx.x + i * (int)gridDim.x) + wg;
     if (win >= p.nwin) continue;
     int b, wi, wj, qr, qc;
@@ -212,8 +208,8 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     const float rstd0 = rsqrtf(__ldg(p.ss_in + m0 * SS_PARTS) / (float)AB_C + 1e-6f);
     const float rstd1 = rsqrtf(__ldg(p.ss_in + m1 * SS_PARTS) / (float)AB_C + 1e-6f);
     const bool seam_r = p.shift > 0 && wi == 0, seam_c = p.shift > 0 && wj == 0;
-    tc::mbar_wait_nocall(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
-    const uint32_t xa = tc::smem_u32(sX + (size_t)buf * AB_X_BYTES) + (uint32_t)wg * AB_KV_BYTES;   // this window's rows of both k-blocks
+    bars->x.wait(xs);
+    const uint32_t xa = tc::smem_u32(sX + (size_t)xs.slot * AB_X_BYTES) + (uint32_t)wg * AB_KV_BYTES;   // this window's rows of both k-blocks
     uint32_t of[2][16];                        // O_h / l of both heads: bf16 A fragments of the out projection
 #pragma unroll 1
     for (int hd = 0; hd < 2; ++hd) {
@@ -245,7 +241,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
         cs[0][jj] = __ldg(tb + tok0);
         cs[1][jj] = __ldg(tb + tok1);
       }
-      if (hd == 1) tc::named_barrier_sync(1 + wg, 128);     // head 0's S and P V MMAs (all four warps) are done with K and V
+      if (hd == 1) tc::named_barrier_sync(tc::BAR_WG + wg, 128);     // head 0's S and P V MMAs (all four warps) are done with K and V
       tc::wg_wait<2>();
       tc::wg_fence_acc(va);
 #pragma unroll
@@ -266,7 +262,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
       uint32_t qf[16];
       to_afrag(qa, qf);
       tc::fence_proxy_async();                 // K, V (generic-proxy writes) -> visible to the tensor core
-      tc::named_barrier_sync(1 + wg, 128);
+      tc::named_barrier_sync(tc::BAR_WG + wg, 128);
       // ---- S = Q K^T
       float s[32];
 #pragma unroll
@@ -366,7 +362,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     tc::wg_wait<0>();
     tc::wg_fence_acc(acc);
     // ---- epilogue: x_new = acc + x (residual from the X tile in shared memory), in place, then TMA store of this window
-    uint8_t* xt = sX + (size_t)buf * AB_X_BYTES;
+    uint8_t* xt = sX + (size_t)xs.slot * AB_X_BYTES;
     float ss0 = 0.f, ss1 = 0.f;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -390,7 +386,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
       p.ss_out[m1 * SS_PARTS] = ss1;
     }
     tc::fence_proxy_async();
-    tc::named_barrier_sync(1 + wg, 128);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
     if (t == 0) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
@@ -401,7 +397,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
       }
       tc::tma_store_commit();
       tc::tma_store_wait_read();         // the X buffer may be refilled (tile i + 2)
-      tc::mbar_arrive(&bars->x_empty[buf]);
+      bars->x.release(xs);
     }
   }
 }

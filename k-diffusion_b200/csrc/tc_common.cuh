@@ -5,6 +5,7 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "pipe_state.cuh"
 
 namespace kdb {
 namespace tc {
@@ -126,9 +127,39 @@ __device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm vo
 __device__ __forceinline__ void named_barrier_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // Hand registers between warpgroups (every warp of the warpgroup executes it): a producer warpgroup gives up what its MMA
-// warpgroups then take, within the CTA's allocation at launch.
+// warpgroups then take, within the CTA's allocation at launch (168 per thread for the 384-thread kernels: 128 x 40 + 256 x 232).
 template <uint32_t R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <uint32_t R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+constexpr uint32_t PRODUCER_REGS = 40, MMA_REGS = 232;
+
+// ---------------------------------------------------------------- warp-specialized kernels
+// Named barriers; id 0 is __syncthreads.  BAR_WG + wg: the 128 threads of MMA warpgroup wg.  BAR_TURN + wg: both MMA warpgroups,
+// warpgroup wg may issue its next block of MMAs.  BAR_ACC + wg: both MMA warpgroups, wg may write the GEMM's fp32 accumulator tile.
+enum : int { BAR_WG = 1, BAR_TURN = 3, BAR_ACC = 5 };
+// Who releases a ring slot: the arrival count of its `empty` barrier
+constexpr uint32_t REL_WARPS = 4;                  // lane 0 of each warp of one warpgroup
+constexpr uint32_t REL_WARPS_2WG = 2 * REL_WARPS;  // ... of both MMA warpgroups
+constexpr uint32_t REL_THREAD_2WG = 2;             // one thread of each MMA warpgroup
+
+// N buffers filled by TMA from one producer thread.  full[s] completes when slot s has landed, empty[s] when it is released.
+template <int N>
+struct TmaRing {
+  uint64_t full[N], empty[N];
+  __device__ __forceinline__ void init(uint32_t releasers) {   // by one thread, before fence_barrier_init
+    for (int s = 0; s < N; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], releasers);
+    }
+  }
+  // producer: wait for the slot's releases, arm `full` for `bytes` and return it for the slot's TMA loads
+  __device__ __forceinline__ uint64_t* acquire(PipeState<N> ps, uint32_t bytes) {
+    mbar_wait_nocall(&empty[ps.slot], ps.producer_parity());
+    mbar_arrive_expect_tx(&full[ps.slot], bytes);
+    return &full[ps.slot];
+  }
+  __device__ __forceinline__ void wait(PipeState<N> ps) { mbar_wait_nocall(&full[ps.slot], ps.consumer_parity()); }
+  __device__ __forceinline__ void release(PipeState<N> ps) { mbar_arrive(&empty[ps.slot]); }
+};
 
 // byte offset of 16-byte chunk `chunk16` (0..7) of `row` inside a [rows x 128 B] SWIZZLE_128B tile (what TMA / UMMA expect)
 __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk16) {

@@ -16,17 +16,15 @@
 //
 // Roles (384 threads, one CTA per SM, tiles blockIdx.x, + gridDim.x, ...):
 //   warpgroups 0, 1   rows [0, 64) / [64, 128) of every tile: M1, GEGLU, M2, final epilogue; both read the same weight chunks
-//   warpgroup 2       producer (40 registers, the MMA warpgroups take 232): one elected lane of warp 8 streams by TMA the X tiles
-//                     (2 buffers), Wup chunks (3 x 32 KiB ring), Wdown chunks (3 x 16 KiB ring) -- the weights stream from L2 once per
-//                     tile (all CTAs walk the same chunks at about the same time)
+//   warpgroup 2       producer: one elected lane of warp 8 streams by TMA the X tiles (2 buffers), Wup chunks (3 x 32 KiB ring),
+//                     Wdown chunks (3 x 16 KiB ring) -- the weights from L2 once per tile (all CTAs walk the same chunks together)
 // Shared memory: X 2 x 32 KiB, Wup 3 x 32 KiB, Wdown 3 x 16 KiB = 208 KiB.
 //
 // Schedule: a warpgroup issues its MMAs in blocks -- M1(0) of a tile, then after each GEGLU(c) the block M2(c), M1(c + 1) -- and the two
-// warpgroups take turns to issue (named barriers 3 and 4), so that one warpgroup's GEGLU and wait latencies run while the tensor cores
+// warpgroups take turns to issue (BAR_TURN), so that one warpgroup's GEGLU and wait latencies run while the tensor cores
 // work through the other's block.  Issued together both would finish together, and the tensor cores would idle during every GEGLU.  A
 // warpgroup is at most one block ahead of the other, which the 3-deep weight rings cover.  Every accumulator sees the same wgmma
-// sequence as in a serial M1 -> GEGLU -> M2 order: the schedule changes no result bit.  The waits are mbar_wait_nocall: a call in the
-// kernel body would make ptxas serialise every wgmma.
+// sequence as in a serial M1 -> GEGLU -> M2 order: the schedule changes no result bit.
 #pragma once
 
 constexpr int FF_C = 128;                  // level width this kernel is built for
@@ -38,9 +36,9 @@ constexpr int FF_WD_BYTES = A_STAGE_BYTES;          // [128 rows x 64 K]
 constexpr int FF_THREADS = 256 + 128;
 
 struct FfnBars {
-  uint64_t x_full[FF_XBUF], x_empty[FF_XBUF];
-  uint64_t wu_full[FF_WU], wu_empty[FF_WU];
-  uint64_t wd_full[FF_WD], wd_empty[FF_WD];
+  tc::TmaRing<FF_XBUF> x;
+  tc::TmaRing<FF_WU> wu;
+  tc::TmaRing<FF_WD> wd;
 };
 constexpr size_t FF_SMEM = (size_t)FF_XBUF * FF_X_BYTES + (size_t)FF_WU * FF_WU_BYTES + (size_t)FF_WD * FF_WD_BYTES + sizeof(FfnBars) + 1024;
 
@@ -70,18 +68,9 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
     tc::tma_prefetch_desc(&tmwu);
     tc::tma_prefetch_desc(&tmwd);
     tc::tma_prefetch_desc(&tmo);
-    for (int i = 0; i < FF_XBUF; ++i) {
-      tc::mbar_init(&bars->x_full[i], 1);
-      tc::mbar_init(&bars->x_empty[i], 2);     // one store-drained arrival per warpgroup
-    }
-    for (int i = 0; i < FF_WU; ++i) {
-      tc::mbar_init(&bars->wu_full[i], 1);
-      tc::mbar_init(&bars->wu_empty[i], 8);    // lane 0 of each of the eight MMA warps
-    }
-    for (int i = 0; i < FF_WD; ++i) {
-      tc::mbar_init(&bars->wd_full[i], 1);
-      tc::mbar_init(&bars->wd_empty[i], 8);
-    }
+    bars->x.init(tc::REL_THREAD_2WG);          // once its store has read the tile
+    bars->wu.init(tc::REL_WARPS_2WG);
+    bars->wd.init(tc::REL_WARPS_2WG);
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -90,32 +79,22 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
 
   if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
-    tc::setmaxnreg_dec<40>();
+    tc::setmaxnreg_dec<tc::PRODUCER_REGS>();
     if (pwarp == 8 && tc::elect_one()) {
-      uint32_t su = 0, pu = 0, sd = 0, pd = 0;        // ring slot / phase of the next Wup / Wdown chunk
-      for (int i = 0; i < n_local; ++i) {
-        const int buf = i & 1;
-        tc::mbar_wait_nocall(&bars->x_empty[buf], (uint32_t)(((i >> 1) & 1) ^ 1));
-        tc::mbar_arrive_expect_tx(&bars->x_full[buf], FF_X_BYTES);
+      PipeState<FF_XBUF> xs{};
+      PipeState<FF_WU> us{};
+      PipeState<FF_WD> ds{};
+      for (int i = 0; i < n_local; ++i, xs.advance()) {
+        uint64_t* bar = bars->x.acquire(xs, FF_X_BYTES);
         const int m0 = ((int)blockIdx.x + i * (int)gridDim.x) * BM;
-        tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES, &tmx, &bars->x_full[buf], 0, m0);
-        tc::tma_load_2d(sX + (size_t)buf * FF_X_BYTES + A_STAGE_BYTES, &tmx, &bars->x_full[buf], BK, m0);
-        for (int c = 0; c < nc; ++c) {
-          tc::mbar_wait_nocall(&bars->wu_empty[su], pu ^ 1u);
-          tc::mbar_arrive_expect_tx(&bars->wu_full[su], FF_WU_BYTES);
-          tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES, &tmwu, &bars->wu_full[su], 0, c * 128);
-          tc::tma_load_2d(sWU + (size_t)su * FF_WU_BYTES + A_STAGE_BYTES, &tmwu, &bars->wu_full[su], BK, c * 128);
-          if (++su == FF_WU) {
-            su = 0;
-            pu ^= 1u;
-          }
-          tc::mbar_wait_nocall(&bars->wd_empty[sd], pd ^ 1u);
-          tc::mbar_arrive_expect_tx(&bars->wd_full[sd], FF_WD_BYTES);
-          tc::tma_load_2d(sWD + (size_t)sd * FF_WD_BYTES, &tmwd, &bars->wd_full[sd], c * FF_CH, 0);
-          if (++sd == FF_WD) {
-            sd = 0;
-            pd ^= 1u;
-          }
+        tc::tma_load_2d(sX + (size_t)xs.slot * FF_X_BYTES, &tmx, bar, 0, m0);
+        tc::tma_load_2d(sX + (size_t)xs.slot * FF_X_BYTES + A_STAGE_BYTES, &tmx, bar, BK, m0);
+        for (int c = 0; c < nc; ++c, us.advance(), ds.advance()) {
+          bar = bars->wu.acquire(us, FF_WU_BYTES);
+          tc::tma_load_2d(sWU + (size_t)us.slot * FF_WU_BYTES, &tmwu, bar, 0, c * 128);
+          tc::tma_load_2d(sWU + (size_t)us.slot * FF_WU_BYTES + A_STAGE_BYTES, &tmwu, bar, BK, c * 128);
+          bar = bars->wd.acquire(ds, FF_WD_BYTES);
+          tc::tma_load_2d(sWD + (size_t)ds.slot * FF_WD_BYTES, &tmwd, bar, c * FF_CH, 0);
         }
       }
     }
@@ -123,26 +102,27 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
   }
 
   // ------------------------------------------------------------------ warpgroups: rows [64 wg, 64 wg + 64) of every tile
-  tc::setmaxnreg_inc<232>();
+  tc::setmaxnreg_inc<tc::MMA_REGS>();
   const int wg = pwarp >> 2, t = threadIdx.x & 127;
   const int r0 = 64 * wg + 16 * (t >> 5) + (lane >> 2);      // this thread's two accumulator rows: r0 and r0 + 8
   const int cq = 2 * (lane & 3);                             // and its column pair inside every 8-column block
   const uint32_t wu_base = tc::smem_u32(sWU), wd_base = tc::smem_u32(sWD);
-  uint32_t su = 0, pu = 0, sd = 0, pd = 0;
-  // Issue turns: warpgroup 0 issues block k after warpgroup 1 has issued block k - 1 (barrier 3), warpgroup 1 issues block k after
-  // warpgroup 0 has issued block k (barrier 4).  Both issue nc + 1 blocks per tile; the arrivals match the syncs one for one.
+  PipeState<FF_XBUF> xs{};
+  PipeState<FF_WU> us{};
+  PipeState<FF_WD> ds{};
+  // Issue turns: warpgroup 0 issues block k after warpgroup 1 has issued block k - 1 (BAR_TURN), warpgroup 1 issues block k after
+  // warpgroup 0 has issued block k (BAR_TURN + 1).  Both issue nc + 1 blocks per tile; the arrivals match the syncs one for one.
   bool first_block = true;
   float acc1[64], acc2[64];
   uint32_t hreg[16];
-  for (int i = 0; i < n_local; ++i) {
-    const int buf = i & 1;
+  for (int i = 0; i < n_local; ++i, xs.advance()) {
     const int64_t m0 = ((int64_t)blockIdx.x + (int64_t)i * gridDim.x) * BM;
     const float rstd0 = rsqrtf(__ldg(p.ss_in + (m0 + r0) * SS_PARTS) / (float)FF_C + 1e-6f);
     const float rstd1 = rsqrtf(__ldg(p.ss_in + (m0 + r0 + 8) * SS_PARTS) / (float)FF_C + 1e-6f);
     // the GELU's 0.5 rides on the value's row scale
     const tc::f32x2 g0 = tc::pk2(rstd0, rstd0), g1 = tc::pk2(rstd1, rstd1), h0 = tc::pk2(0.5f * rstd0, 0.5f * rstd0), h1 = tc::pk2(0.5f * rstd1, 0.5f * rstd1);
-    tc::mbar_wait_nocall(&bars->x_full[buf], (uint32_t)((i >> 1) & 1));
-    const uint32_t xa = tc::smem_u32(sX + (size_t)buf * FF_X_BYTES) + (uint32_t)wg * 8192u;   // rows 64 wg.. of both k-block tiles
+    bars->x.wait(xs);
+    const uint32_t xa = tc::smem_u32(sX + (size_t)xs.slot * FF_X_BYTES) + (uint32_t)wg * 8192u;   // rows 64 wg.. of both k-block tiles
 #pragma unroll
     for (int j = 0; j < 64; ++j) acc2[j] = 0.f;
     // block c: M2(c - 1) for c > 0, M1(c) for c < nc.  One program point per wgmma: accumulators carried into the loop from a second
@@ -154,17 +134,11 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
         tc::wg_fence_acc(acc1);
         tc::wg_fence_acc(acc2);
         tc::wg_fence_acc(hreg);
-        if (lane == 0) tc::mbar_arrive(&bars->wu_empty[su]);
-        if (++su == FF_WU) {
-          su = 0;
-          pu ^= 1u;
-        }
+        if (lane == 0) bars->wu.release(us);
+        us.advance();
         if (c > 1) {
-          if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
-          if (++sd == FF_WD) {
-            sd = 0;
-            pd ^= 1u;
-          }
+          if (lane == 0) bars->wd.release(ds);
+          ds.advance();
         }
         // ---- GEGLU(c - 1): 8-column block 2q = 8 value features, block 2q + 1 = their gates -> hidden block q (rows r0, r0 + 8)
 #pragma unroll
@@ -183,13 +157,13 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
       for (int j = 0; j < 64; ++j) acc1[j] = 0.f;
       tc::wg_fence_acc(acc1);          // the zeros are written before this turn's first wgmma
       // ---- this warpgroup's turn to issue
-      if (wg == 1) tc::named_barrier_sync(4, 256);
-      else if (!first_block) tc::named_barrier_sync(3, 256);
+      if (wg == 1) tc::named_barrier_sync(tc::BAR_TURN + 1, 256);
+      else if (!first_block) tc::named_barrier_sync(tc::BAR_TURN, 256);
       first_block = false;
       if (c > 0) {
         // ---- M2(c - 1): acc2 += H . Wdown^T
-        tc::mbar_wait_nocall(&bars->wd_full[sd], pd);
-        const uint64_t bd = tc::smem_desc_k_sw128(wd_base + sd * (uint32_t)FF_WD_BYTES);
+        bars->wd.wait(ds);
+        const uint64_t bd = tc::smem_desc_k_sw128(wd_base + ds.slot * (uint32_t)FF_WD_BYTES);
         tc::wg_fence_acc(acc2);
         tc::wg_fence_acc(hreg);
         tc::wg_fence();
@@ -202,8 +176,8 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
       }
       if (c < nc) {
         // ---- M1(c): acc1 = X . Wup^T
-        tc::mbar_wait_nocall(&bars->wu_full[su], pu);
-        const uint32_t wa = wu_base + su * (uint32_t)FF_WU_BYTES;
+        bars->wu.wait(us);
+        const uint32_t wa = wu_base + us.slot * (uint32_t)FF_WU_BYTES;
         tc::wg_fence_acc(acc1);
         tc::wg_fence();
 #pragma unroll
@@ -214,19 +188,16 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
         }
         tc::wg_commit();
       }
-      if (wg == 0) tc::named_barrier_arrive(4, 256);
-      else if (c < nc || i + 1 < n_local) tc::named_barrier_arrive(3, 256);
+      if (wg == 0) tc::named_barrier_arrive(tc::BAR_TURN + 1, 256);
+      else if (c < nc || i + 1 < n_local) tc::named_barrier_arrive(tc::BAR_TURN, 256);
     }
     tc::wg_wait<0>();
     tc::wg_fence_acc(acc2);
     tc::wg_fence_acc(hreg);
-    if (lane == 0) tc::mbar_arrive(&bars->wd_empty[sd]);
-    if (++sd == FF_WD) {
-      sd = 0;
-      pd ^= 1u;
-    }
+    if (lane == 0) bars->wd.release(ds);
+    ds.advance();
     // ---- final epilogue: out = acc2 + x (residual from the X tile in shared memory), in place, then TMA store of this half
-    uint8_t* xt = sX + (size_t)buf * FF_X_BYTES;
+    uint8_t* xt = sX + (size_t)xs.slot * FF_X_BYTES;
     float ss0 = 0.f, ss1 = 0.f;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -251,13 +222,13 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
       p.ss_out[(m0 + r0 + 8) * SS_PARTS] = ss1;
     }
     tc::fence_proxy_async();
-    tc::named_barrier_sync(1 + wg, 128);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
     if (t == 0) {
       tc::tma_store_2d(&tmo, xt + wg * 8192, 0, (int)m0 + 64 * wg);
       tc::tma_store_2d(&tmo, xt + SUB_TILE_BYTES + wg * 8192, 64, (int)m0 + 64 * wg);
       tc::tma_store_commit();
       tc::tma_store_wait_read();         // the X buffer may be refilled (tile i + 2)
-      tc::mbar_arrive(&bars->x_empty[buf]);
+      bars->x.release(xs);
     }
   }
 }

@@ -1,15 +1,11 @@
 // tc_kernels.cu -- bf16 tensor-core GEMM for sm_90a: TMA (SWIZZLE_128B tiles) -> shared memory -> wgmma (fp32 accumulators in
-// registers) -> fp32 shared-memory tile -> fused epilogue (thread = output row) -> swizzled shared tile -> TMA store.
+// registers) -> fp32 shared-memory tile -> fused epilogue (thread = output row) -> swizzled shared tile -> TMA store (clipped at the
+// M edge by the tensor map).
 //
 // C[M,N] = A[M,K] W[N,K]^T for every nn.Linear on the token stream (reference image_transformer_v2.py:126-139).
 // Epilogues: plain store; +residual (out_proj / down_proj, :396,:493; residual tile prefetched by TMA while the main loop
 // runs); GEGLU (:89-95; rows of W interleaved 8 value / 8 gate); cosine-sim scaling + axial RoPE of q and k fused into the
 // qkv projection (:106-114,187-199,245-248; cos/sin from a per-layer table); TokenSplit scatter + lerp (:618-621).
-//
-// Persistent: one 384-thread CTA per SM walks 128 x BN output tiles.  Warp 8 = TMA producer (one elected lane) streaming the
-// k-blocks of every tile through one ring; warpgroups 0 and 1 take alternate tiles and hand the MMA issue to each other, so one
-// warpgroup's main loop runs while the other runs its epilogue (one accumulator row per thread).  Output rows are written to a
-// SWIZZLE_128B staging tile and leave through one TMA store per 64 columns: fully coalesced, clipped at the M edge by the tensor map.
 #include "tc_common.cuh"
 #include "tc_kernels.cuh"
 
@@ -169,10 +165,10 @@ __device__ __forceinline__ void stage_ld32(const float* s, int row, int col0, fl
 // b + 2 grid, ... and its warpgroup w the odd / even ones of those.  Warp 8 (one elected lane) streams the A / W k-blocks of the
 // CTA's tiles, in tile order, through one ring of SWIZZLE_128B stages, so the next tile's k-blocks load during an epilogue.  A
 // warpgroup issues wgmma (two M = 64 halves per k-step) with the accumulators in registers, keeps one k-block in flight while it
-// releases the previous stage, and hands the MMA issue to the other warpgroup once its last k-block is issued (named barriers 3 and
-// 4: the two main loops never interleave, which also keeps each ring stage at most one phase ahead of its waiter).  Its epilogue then
+// releases the previous stage, and hands the MMA issue to the other warpgroup once its last k-block is issued (BAR_TURN: the two
+// main loops never interleave, which also keeps each ring stage at most one phase ahead of its waiter).  Its epilogue then
 // writes the accumulators to the fp32 tile in shared memory so that each thread owns one output row (fp32 arithmetic, one rounding
-// to bf16 at the pack, one TMA store per 64 columns), and hands the fp32 tile on once its rows are read (named barriers 5 and 6).
+// to bf16 at the pack, one TMA store per 64 columns), and hands the fp32 tile on once its rows are read (BAR_ACC).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
                                                                   const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
@@ -186,9 +182,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
   constexpr bool RES = EPI == TCE_RESID;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* sAcc = reinterpret_cast<float*>(base + GEMM_RING_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>());
-  uint64_t* empty = full + STAGES;
-  uint64_t* resid_full = empty + STAGES;   // one per warpgroup
+  auto* ring = reinterpret_cast<tc::TmaRing<STAGES>*>(base + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>());
+  uint64_t* resid_full = reinterpret_cast<uint64_t*>(ring + 1);   // one per warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = p.K / BK;
@@ -199,10 +194,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tma);
     tc::tma_prefetch_desc(&tmb);
-    for (int s = 0; s < STAGES; ++s) {
-      tc::mbar_init(&full[s], 1);
-      tc::mbar_init(&empty[s], 4);       // lane 0 of each warp of the consuming warpgroup
-    }
+    ring->init(tc::REL_WARPS);           // by the warpgroup that consumes the k-block
     tc::mbar_init(&resid_full[0], 1);
     tc::mbar_init(&resid_full[1], 1);
     tc::fence_barrier_init();
@@ -210,9 +202,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
   __syncthreads();
   tc::pdl_wait();   // A, the residual, the row statistics and W (folded for this evaluation) are written by the kernels before us
 
-  // 168 registers per thread at launch: the producer warpgroup needs few, the MMA warpgroups take what it gives up
   if (warp >= 8) {
-    tc::setmaxnreg_dec<40>();
+    tc::setmaxnreg_dec<tc::PRODUCER_REGS>();
     if (warp == 8 && tc::elect_one()) {
       int it = 0;                        // ring position of the next k-block
       for (int i = 0; i < n_local; ++i) {
@@ -220,28 +211,26 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
         const int64_t m0 = (int64_t)(t / n_tiles) * BM;
         const int n0 = (t % n_tiles) * BN;
         for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          tc::mbar_wait_nocall(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
-          tc::mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
-          uint8_t* a = base + (size_t)s * STAGE_BYTES;
+          const auto ps = PipeState<STAGES>::at(it);
+          uint64_t* bar = ring->acquire(ps, STAGE_BYTES);
+          uint8_t* a = base + (size_t)ps.slot * STAGE_BYTES;
           if (p.a_merge) {   // TokenMerge: k-block kb lives in quadrant (nh, nw) of the fine grid, channels e0..e0+63
             const int qd = (kb * BK) / p.mC, e0 = kb * BK - qd * p.mC;
-            tc::tma_load_5d(a, &tma, &full[s], e0, qd & 1, p.box_h == 1 ? (int)(m0 % p.mwc) : 0, qd >> 1, (int)(m0 / p.mwc));
+            tc::tma_load_5d(a, &tma, bar, e0, qd & 1, p.box_h == 1 ? (int)(m0 % p.mwc) : 0, qd >> 1, (int)(m0 / p.mwc));
           } else {
-            tc::tma_load_2d(a, &tma, &full[s], kb * BK, (int)m0);
+            tc::tma_load_2d(a, &tma, bar, kb * BK, (int)m0);
           }
-          tc::tma_load_2d(a + A_STAGE_BYTES, &tmb, &full[s], kb * BK, n0);
+          tc::tma_load_2d(a + A_STAGE_BYTES, &tmb, bar, kb * BK, n0);
         }
       }
     }
     return;
   }
-  tc::setmaxnreg_inc<232>();
+  tc::setmaxnreg_inc<tc::MMA_REGS>();
 
   const int wg = warp >> 2;
   const int row = threadIdx.x & 127;
   uint8_t* sC = base + GEMM_RING_BYTES + BM * BN * 4 + wg * out_bytes<BN, EPI>();
-  const int ebar = 1 + wg;               // named barrier of this warpgroup's 128 threads
   for (int i = wg; i < n_local; i += 2) {
     const int t = (int)blockIdx.x + i * (int)gridDim.x;
     const int64_t m0 = (int64_t)(t / n_tiles) * BM;
@@ -258,12 +247,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
     float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
     for (int k = 0; k < BN / 2; ++k) acc0[k] = acc1[k] = 0.f;
-    if (i > 0) tc::named_barrier_sync(3 + wg, 256);   // the other warpgroup has issued the main loop of tile i - 1
+    if (i > 0) tc::named_barrier_sync(tc::BAR_TURN + wg, 256);   // the other warpgroup has issued the main loop of tile i - 1
     const int it0 = i * nkb;             // ring position of this tile's first k-block
     for (int kb = 0; kb < nkb; ++kb) {
-      const int s = (it0 + kb) % STAGES;
-      tc::mbar_wait_nocall(&full[s], (uint32_t)((it0 + kb) / STAGES) & 1u);
-      const uint32_t a_addr = tc::smem_u32(base + (size_t)s * STAGE_BYTES);
+      const auto ps = PipeState<STAGES>::at(it0 + kb);
+      ring->wait(ps);
+      const uint32_t a_addr = tc::smem_u32(base + (size_t)ps.slot * STAGE_BYTES);
       const uint64_t ad0 = tc::smem_desc_k_sw128(a_addr), ad1 = tc::smem_desc_k_sw128(a_addr + 8 * 1024);   // rows 0-63 / 64-127
       const uint64_t bd = tc::smem_desc_k_sw128(a_addr + A_STAGE_BYTES);
       tc::wg_fence_acc(acc0);
@@ -283,17 +272,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       tc::wg_wait<1>();                  // k-block kb - 1 has completed: its stage may be refilled
       tc::wg_fence_acc(acc0);
       tc::wg_fence_acc(acc1);
-      if (kb > 0 && lane == 0) tc::mbar_arrive(&empty[(it0 + kb - 1) % STAGES]);
+      if (kb > 0 && lane == 0) ring->release(PipeState<STAGES>::at(it0 + kb - 1));
     }
-    if (i + 1 < n_local) tc::named_barrier_arrive(3 + (wg ^ 1), 256);
+    if (i + 1 < n_local) tc::named_barrier_arrive(tc::BAR_TURN + (wg ^ 1), 256);
     tc::wg_wait<0>();
     tc::wg_fence_acc(acc0);
     tc::wg_fence_acc(acc1);
-    if (lane == 0) tc::mbar_arrive(&empty[(it0 + nkb - 1) % STAGES]);
-    if (i > 0) tc::named_barrier_sync(5 + wg, 256);   // the other warpgroup has read tile i - 1 out of the fp32 tile
+    if (lane == 0) ring->release(PipeState<STAGES>::at(it0 + nkb - 1));
+    if (i > 0) tc::named_barrier_sync(tc::BAR_ACC + wg, 256);   // the other warpgroup has read tile i - 1 out of the fp32 tile
     stage_store<BN>(sAcc, 0, acc0);
     stage_store<BN>(sAcc, 64, acc1);
-    tc::named_barrier_sync(ebar, 128);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
     const bool pass_acc = i + 1 < n_local;   // after its last read of the fp32 tile this warpgroup hands it on (named_barrier_arrive)
 
     // ---------------- epilogue: thread = output row
@@ -314,7 +303,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
 #pragma unroll
         for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
       }
-      if (pass_acc) tc::named_barrier_arrive(5 + (wg ^ 1), 256);
+      if (pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
       if (m < p.M) {
         if (p.ss_in != nullptr) {   // fused out_norm: A is the raw residual stream, W carries the channel scale
 #pragma unroll
@@ -351,7 +340,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       for (int c = 0; c < BN / 32; ++c) {
         float v[32];
         stage_ld32<BN>(sAcc, row, c * 32, v);
-        if (c == BN / 32 - 1 && pass_acc) tc::named_barrier_arrive(5 + (wg ^ 1), 256);
+        if (c == BN / 32 - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
         if (!live) continue;
         const int n = n0 + c * 32;
         const int64_t b = m / ((int64_t)p.hc * p.wc);
@@ -395,7 +384,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
 #pragma unroll
           for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
         }
-        if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(5 + (wg ^ 1), 256);
+        if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
         if (EPI != TCE_GEGLU && p.ss_in != nullptr) {
           // fused RMSNorm row scale.  q and k are cosine-normalised afterwards (scale invariant): only v needs it.
           bool apply = true;
@@ -494,7 +483,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
         if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = (ss_acc[0] + ss_acc[1]) + (ss_acc[2] + ss_acc[3]);
       }
       tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
-      tc::named_barrier_sync(ebar, 128);
+      tc::named_barrier_sync(tc::BAR_WG + wg, 128);
       if (row == 0) {
         if constexpr (EPI == TCE_GEGLU) {
           tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
