@@ -70,18 +70,9 @@ constexpr size_t WS_SMEM = (size_t)WS_QBUF * TILE_BYTES + (size_t)WS_KV_STAGES *
 
 // tile -> image b, window (wi, wj), first head of the pair
 __device__ __forceinline__ void ws_window(const AttnParams& p, int tile, int& b, int& wi, int& wj, int& head0) {
-  const int hp = p.nh >> 1, nww = p.w >> 3, per_img = (p.h >> 3) * nww * hp;
-  b = tile / per_img;
-  int rem = tile - b * per_img;
-  const int win = rem / hp;
-  head0 = 2 * (rem - win * hp);
-  wi = win / nww;
-  wj = win - wi * nww;
-}
-// origin of quadrant q of window (wi, wj) in original coordinates (:274)
-__device__ __forceinline__ void ws_quad(const AttnParams& p, int wi, int wj, int q, int& r, int& c) {
-  r = (wi * 8 + (q >> 1) * 4 - p.shift + p.h) % p.h;
-  c = (wj * 8 + (q & 1) * 4 - p.shift + p.w) % p.w;
+  const int hp = p.nh >> 1, win = tile / hp;
+  head0 = 2 * (tile - win * hp);
+  tc::window_coords(win, p.h, p.w, b, wi, wj);
 }
 // tile -> image b, head, 128-query tile m (GLOBAL)
 __device__ __forceinline__ void ws_global(const AttnParams& p, int tile, int& b, int& head, int& m) {
@@ -95,15 +86,13 @@ template <int MODE, bool BOUNDED>
 __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_out,
                                                                 const AttnParams p) {
   constexpr int NK = MODE == MODE_WINDOW ? 64 : 128;   // keys per block seen by one warpgroup
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sQ = base;
+  uint8_t* sQ = tc::smem_1k();
   uint8_t* sKV = sQ + WS_QBUF * TILE_BYTES;                    // stage s: K at 2 s TILE_BYTES, V after it
   uint8_t* sO = sKV + WS_KV_STAGES * 2 * TILE_BYTES;
   WsBars* bars = reinterpret_cast<WsBars*>(sO + 2 * HALF_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nblk = MODE == MODE_WINDOW ? 1 : p.nblk;
-  const int n_local = (int)blockIdx.x < p.n_tiles ? (p.n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const int n_local = tc::tiles_owned(p.n_tiles);
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tm_in);
@@ -114,7 +103,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
   }
   __syncthreads();
   tc::pdl_wait();                              // programmatic launch: the qkv projection before us must be complete from here on
-  tc::pdl_launch_dependents();
+  KDB_PDL_TRIGGER();
 
   if (warp >= 8) {
     // ------------------------------------------------------------------ TMA producer
@@ -127,7 +116,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             int r, c;
-            ws_quad(p, wi, wj, q, r, c);
+            tc::quad_origin(wi, wj, q, p.h, p.w, p.shift, r, c);
             tc::tma_load_4d(dst + hd * HALF_BYTES + q * 2048, &tm_in, bar, (t * p.nh + head0 + hd) * DH, c, r, b);
           }
       };
@@ -206,79 +195,19 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
       tc::wg_wait<0>();
       tc::wg_fence_acc(s);
       if (j == nblk - 1 && lane == 0) bars->q.release(qs);   // every read of this Q tile is done
-      // ---- softmax in registers.  Key column 8 c + cq (+1); WINDOW: it lies in quadrant c / 2, and the seam mask keeps a query to keys
-      // on its own side of the wrapped row / column of the top / left windows.
-      auto key_ok = [&](int c) -> bool {
-        const int kq = c >> 1;
-        return (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-      };
-      if constexpr (!BOUNDED) {
-        float n0 = mx0, n1 = mx1;
-#pragma unroll
-        for (int c = 0; c < NK / 8; ++c) {
-          if (MODE == MODE_WINDOW && !key_ok(c)) s[4 * c] = s[4 * c + 1] = s[4 * c + 2] = s[4 * c + 3] = -INFINITY;
-          n0 = fmaxf(n0, fmaxf(s[4 * c], s[4 * c + 1]));
-          n1 = fmaxf(n1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
-        }
-        n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 1));
-        n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 2));
-        n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 1));
-        n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 2));
-        if (j > 0) {                           // the maximum grew: rescale what was accumulated against the old one
-          const float a0 = exp2f((mx0 - n0) * LOG2E), a1 = exp2f((mx1 - n1) * LOG2E);
-          l0 *= a0;
-          l1 *= a1;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            o[4 * c] *= a0;
-            o[4 * c + 1] *= a0;
-            o[4 * c + 2] *= a1;
-            o[4 * c + 3] *= a1;
-          }
-        }
-        mx0 = n0;
-        mx1 = n1;
-      }
-      const float mb0 = mx0 * LOG2E, mb1 = mx1 * LOG2E;
-      uint32_t pf[NK / 4];
-#pragma unroll
-      for (int i2 = 0; i2 < NK / 4; ++i2) {
-        const float mb = (i2 & 1) ? mb1 : mb0;
-        float p0 = exp2f(fmaf(s[2 * i2], LOG2E, -mb)), p1 = exp2f(fmaf(s[2 * i2 + 1], LOG2E, -mb));
-        if (BOUNDED && MODE == MODE_WINDOW && !key_ok(i2 >> 1)) p0 = p1 = 0.f;   // (bounded) zero probability instead of a -inf logit
-        pf[i2] = tc::pack_bf16x2(p0, p1);
-        float e0, e1;
-        tc::unpack_bf16x2(pf[i2], e0, e1);     // l accumulates exactly what the P V MMA sees
-        if (i2 & 1) l1 += e0 + e1;
-        else l0 += e0 + e1;
-      }
-      // ---- O += P V, 16 keys per step: rows 16 kk.. of V
-      tc::wg_fence_acc(o);
-      tc::wg_fence_acc(pf);
-      tc::wg_fence();
-      const uint64_t vdesc = tc::smem_desc_mn_sw128(v_addr, 1024, 1024);
-#pragma unroll
-      for (int kk = 0; kk < NK / 16; ++kk) {
-        const uint32_t a[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
-        tc::wgmma_64_rs<1>(o, a, vdesc + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
-      }
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(o);
+      // ---- softmax in registers and O += P V.  WINDOW: key column block c lies in quadrant c / 2.
+      auto key_ok = [&](int c) { return tc::seam_ok(quad, c >> 1, seam_r, seam_c); };
+      tc::softmax_pv<NK, BOUNDED>(s, key_ok, j > 0, mx0, mx1, l0, l1, o, tc::smem_desc_mn_sw128(v_addr, 1024, 1024));
       if (lane == 0) bars->kv.release(ks);
     }
     // ---- O / l -> bf16 staging tile (rows = this warpgroup's 64 queries) -> TMA store
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+    tc::softmax_normalize(o, l0, l1);
     if (t == 0) tc::tma_store_wait_read();    // the previous tile's store has read the staging tile
     tc::named_barrier_sync(tc::BAR_WG + wg, 128);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
-      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw, c) + cq * 2) = tc::pack_bf16x2(o[4 * c] * inv0, o[4 * c + 1] * inv0);
-      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw + 8, c) + cq * 2) = tc::pack_bf16x2(o[4 * c + 2] * inv1, o[4 * c + 3] * inv1);
+      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw, c) + cq * 2) = tc::pack_bf16x2(o[4 * c], o[4 * c + 1]);
+      *reinterpret_cast<uint32_t*>(sOw + tc::sw128_offset(rw + 8, c) + cq * 2) = tc::pack_bf16x2(o[4 * c + 2], o[4 * c + 3]);
     }
     tc::fence_proxy_async();                   // staging tile (generic-proxy writes) -> visible to the TMA engine
     tc::named_barrier_sync(tc::BAR_WG + wg, 128);
@@ -287,7 +216,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1) attn_ws_kernel(const __grid_con
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           int r, c;
-          ws_quad(p, wi, wj, q, r, c);
+          tc::quad_origin(wi, wj, q, p.h, p.w, p.shift, r, c);
           tc::tma_store_4d(&tm_out, sOw + q * 2048, head * DH, c, r, b);
         }
       } else {
@@ -308,8 +237,7 @@ struct Bars {
 template <bool BOUNDED>
 __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
                                                          const AttnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* base = tc::smem_1k();
   uint8_t* sQ = base;
   uint8_t* sK = base + TILE_BYTES;
   uint8_t* sV = base + 2 * TILE_BYTES;
@@ -343,7 +271,7 @@ __global__ void __launch_bounds__(160, 1) attn_na_kernel(const __grid_constant__
   tc::fence_proxy_async();
   __syncthreads();
   tc::pdl_wait();                              // programmatic launch: the qkv projection before us must be complete from here on
-  tc::pdl_launch_dependents();
+  KDB_PDL_TRIGGER();
 
   if (warp == 4) {
     if (tc::elect_one()) {
@@ -499,25 +427,15 @@ bool tc_attention_supported(int h, int w, int nh, int e, int attn_type, int attn
   return false;
 }
 
-template <typename K>
-static cudaError_t set_smem(K kernel, size_t smem) {
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-}
-
-// persistent WINDOW / GLOBAL launch: min(tiles, SMs) CTAs; programmatic dependent launch, so that barrier init overlaps the tail of the
-// qkv projection
+// persistent WINDOW / GLOBAL launch; programmatic dependent launch, so that barrier init overlaps the tail of the qkv projection
 template <int MODE>
-static cudaError_t launch_ws(cudaStream_t st, const CUtensorMap& tin, const CUtensorMap& tout, const AttnParams& p) {
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = set_smem(attn_ws_kernel<MODE, false>, WS_SMEM);
-    if (e == cudaSuccess) e = set_smem(attn_ws_kernel<MODE, true>, WS_SMEM);
-    if (e != cudaSuccess) return e;
-    attr = true;
-  }
-  const dim3 grid((unsigned)(p.n_tiles < num_sms() ? p.n_tiles : num_sms()));
-  if (p.bound != nullptr) return launch_pdl(attn_ws_kernel<MODE, true>, grid, dim3(WS_THREADS), WS_SMEM, st, tin, tout, p);
-  return launch_pdl(attn_ws_kernel<MODE, false>, grid, dim3(WS_THREADS), WS_SMEM, st, tin, tout, p);
+static int launch_ws(cudaStream_t st, const CUtensorMap& tin, const CUtensorMap& tout, const AttnParams& p) {
+  const bool bounded = p.bound != nullptr;
+  auto kernel = bounded ? attn_ws_kernel<MODE, true> : attn_ws_kernel<MODE, false>;
+  static bool opened[2] = {false, false};
+  if (int rc = set_smem_once(kernel, opened[bounded], (int)WS_SMEM)) return rc;
+  KDB_CUDA(launch_pdl(kernel, persistent_grid(p.n_tiles), dim3(WS_THREADS), WS_SMEM, st, tin, tout, p));
+  return 0;
 }
 
 int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh, int e, int attn_type, int attn_param, int shift,
@@ -534,31 +452,22 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
   int rc;
   if (attn_type == KDB_ATTN_SHIFTED_WINDOW) {
     KDB_REQUIRE(shift == 0 || shift == 4, KDB_ERR_UNSUPPORTED, "attention_tc: window shift must be 0 or window/2");
-    const uint64_t dims[4] = {F, (uint64_t)w, (uint64_t)h, (uint64_t)B}, dims_o[4] = {C, (uint64_t)w, (uint64_t)h, (uint64_t)B};
-    const uint64_t strides[3] = {F * 2, F * 2 * w, F * 2 * w * h}, strides_o[3] = {C * 2, C * 2 * w, C * 2 * w * h};
-    const uint32_t box[4] = {DH, 4, 4, 1};    // one quadrant of a window
-    if ((rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, box))) return rc;
-    if ((rc = make_tmap_bf16(&to, out, 4, dims_o, strides_o, box))) return rc;
+    if ((rc = make_tmap_tokens(&tm, qkv, F, B, h, w, DH, 4, 4))) return rc;     // one quadrant of a window
+    if ((rc = make_tmap_tokens(&to, out, C, B, h, w, DH, 4, 4))) return rc;
     p.nblk = 1;
     p.n_tiles = B * (h / 8) * (w / 8) * (nh / 2);
-    KDB_CUDA(launch_ws<MODE_WINDOW>(st, tm, to, p));
+    if ((rc = launch_ws<MODE_WINDOW>(st, tm, to, p))) return rc;
   } else if (attn_type == KDB_ATTN_NEIGHBORHOOD) {
-    static bool attr_n = false;
-    const uint64_t dims[4] = {F, (uint64_t)w, (uint64_t)h, (uint64_t)B};
-    const uint64_t strides[3] = {F * 2, F * 2 * w, F * 2 * w * h};
-    const uint32_t box_q[4] = {DH, NA_QW, NA_QH, 1}, box_kv[4] = {DH, NA_KW, NA_BLK_ROWS, 1};
-    if ((rc = make_tmap_bf16(&tm, qkv, 4, dims, strides, box_q))) return rc;
     CUtensorMap tkv;
-    if ((rc = make_tmap_bf16(&tkv, qkv, 4, dims, strides, box_kv))) return rc;
-    if (!attr_n) {
-      KDB_CUDA(set_smem(attn_na_kernel<false>, ATTN_NA_SMEM));
-      KDB_CUDA(set_smem(attn_na_kernel<true>, ATTN_NA_SMEM));
-      attr_n = true;
-    }
+    if ((rc = make_tmap_tokens(&tm, qkv, F, B, h, w, DH, NA_QW, NA_QH))) return rc;
+    if ((rc = make_tmap_tokens(&tkv, qkv, F, B, h, w, DH, NA_KW, NA_BLK_ROWS))) return rc;
+    const bool bounded = p.bound != nullptr;
+    auto kernel = bounded ? attn_na_kernel<true> : attn_na_kernel<false>;
+    static bool opened[2] = {false, false};
+    if ((rc = set_smem_once(kernel, opened[bounded], (int)ATTN_NA_SMEM))) return rc;
     p.nblk = 3;      // 14 halo rows = 5 + 5 + 4
     dim3 grid((unsigned)((h / NA_QH) * (w / NA_QW)), (unsigned)nh, (unsigned)B);
-    if (p.bound != nullptr) KDB_CUDA(launch_pdl(attn_na_kernel<true>, grid, dim3(160), ATTN_NA_SMEM, st, tm, tkv, p));
-    else KDB_CUDA(launch_pdl(attn_na_kernel<false>, grid, dim3(160), ATTN_NA_SMEM, st, tm, tkv, p));
+    KDB_CUDA(launch_pdl(kernel, grid, dim3(160), ATTN_NA_SMEM, st, tm, tkv, p));
   } else {
     const uint64_t T = (uint64_t)h * w;
     const uint64_t dims[3] = {F, T, (uint64_t)B}, dims_o[3] = {C, T, (uint64_t)B};
@@ -568,7 +477,7 @@ int launch_attention_tc(const bf16* qkv, bf16* out, int B, int h, int w, int nh,
     if ((rc = make_tmap_bf16(&to, out, 3, dims_o, strides_o, box_o))) return rc;
     p.nblk = (int)(T / ROWS);
     p.n_tiles = B * nh * p.nblk;
-    KDB_CUDA(launch_ws<MODE_GLOBAL>(st, tm, to, p));
+    if ((rc = launch_ws<MODE_GLOBAL>(st, tm, to, p))) return rc;
   }
   KDB_LAUNCH_CHECK(F_ATTN_TC, st);
   return 0;

@@ -54,33 +54,16 @@ struct AttnBlockParams {
   int h, w, shift, nwin;   // nwin = B (h / 8) (w / 8)
 };
 
-// window `win` of the rolled image -> image b, window row wi, window column wj
-__device__ __forceinline__ void ab_window(const AttnBlockParams& p, int win, int& b, int& wi, int& wj) {
-  const int nww = p.w >> 3, per_img = (p.h >> 3) * nww;
-  b = win / per_img;
-  const int rem = win - b * per_img;
-  wi = rem / nww;
-  wj = rem - wi * nww;
-}
-// origin of quadrant q of window (wi, wj) in original coordinates (:274)
-__device__ __forceinline__ void ab_quad(const AttnBlockParams& p, int wi, int wj, int q, int& r, int& c) {
-  r = (wi * 8 + (q >> 1) * 4 - p.shift + p.h) % p.h;
-  c = (wj * 8 + (q & 1) * 4 - p.shift + p.w) % p.w;
-}
-
 __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                           const __grid_constant__ CUtensorMap tmwq,
                                                                           const __grid_constant__ CUtensorMap tmwo, const AttnBlockParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sX = base;
+  uint8_t* sX = tc::smem_1k();
   uint8_t* sWQ = sX + AB_XBUF * AB_X_BYTES;
   uint8_t* sWO = sWQ + 2 * AB_WQKV_KB;
   uint8_t* sKV = sWO + AB_WO_BYTES;
   AttnBlockBars* bars = reinterpret_cast<AttnBlockBars*>(sKV + 4 * AB_KV_BYTES);
   const int pwarp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles = (p.nwin + 1) >> 1;
-  const int n_local = (int)blockIdx.x < n_tiles ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const int n_local = tc::tiles_owned((p.nwin + 1) >> 1);
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmx);
@@ -94,7 +77,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   // x and its row statistics come from the kernel before us; the folded Wqkv is rewritten by the fold kernel at the start of every
   // evaluation, so the weights are loaded after the wait as well
   tc::pdl_wait();
-  tc::pdl_launch_dependents();
+  KDB_PDL_TRIGGER();
 
   if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
@@ -114,11 +97,11 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
         uint64_t* bar = bars->x.acquire(xs, (uint32_t)nw * 2u * AB_KV_BYTES);
         for (int s = 0; s < nw; ++s) {
           int b, wi, wj;
-          ab_window(p, win0 + s, b, wi, wj);
+          tc::window_coords(win0 + s, p.h, p.w, b, wi, wj);
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             int r, c;
-            ab_quad(p, wi, wj, q, r, c);
+            tc::quad_origin(wi, wj, q, p.h, p.w, p.shift, r, c);
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb)
               tc::tma_load_4d(sX + (size_t)xs.slot * AB_X_BYTES + kb * A_STAGE_BYTES + s * AB_KV_BYTES + q * 2048, &tmx, bar, kb * BK, c, r, b);
@@ -143,7 +126,6 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
   const uint64_t vdesc = tc::smem_desc_mn_sw128(tc::smem_u32(sV), 1024, 1024);
   const float sqs[2] = {sqrtf(__ldg(p.qk_scale)), sqrtf(__ldg(p.qk_scale + 1))};
   const int T = p.h * p.w;
-  constexpr float LOG2E = 1.4426950408889634f;
 
   // [64 x 64] accumulator -> bf16 SW128 tile, rows = tokens (K-major B operand of S = Q K^T, MN-major B operand of O = P V)
   auto store_tile = [&](uint8_t* dst, const float (&a)[32]) {
@@ -201,8 +183,8 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     const int win = 2 * ((int)blockIdx.x + i * (int)gridDim.x) + wg;
     if (win >= p.nwin) continue;
     int b, wi, wj, qr, qc;
-    ab_window(p, win, b, wi, wj);
-    ab_quad(p, wi, wj, quad, qr, qc);
+    tc::window_coords(win, p.h, p.w, b, wi, wj);
+    tc::quad_origin(wi, wj, quad, p.h, p.w, p.shift, qr, qc);
     const int tok0 = (qr + lr) * p.w + qc + lc, tok1 = tok0 + 2 * p.w;
     const int64_t m0 = (int64_t)b * T + tok0, m1 = (int64_t)b * T + tok1;
     const float rstd0 = rsqrtf(__ldg(p.ss_in + m0 * SS_PARTS) / (float)AB_C + 1e-6f);
@@ -278,60 +260,14 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
       tc::wg_commit();
       tc::wg_wait<0>();
       tc::wg_fence_acc(s);
-      // ---- softmax in registers.  Key column 8 j + cq (+1) lies in quadrant j / 2; the seam mask (:300-315) keeps a query to keys
-      // on its own side of the wrapped row / column of the top / left windows.
-      float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int kq = j >> 1;
-        const bool ok = (!seam_r || ((kq >> 1) == (quad >> 1))) && (!seam_c || ((kq & 1) == (quad & 1)));
-        if (!ok) s[4 * j] = s[4 * j + 1] = s[4 * j + 2] = s[4 * j + 3] = -INFINITY;
-        mx0 = fmaxf(mx0, fmaxf(s[4 * j], s[4 * j + 1]));
-        mx1 = fmaxf(mx1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
-      }
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-      const float mb0 = mx0 * LOG2E, mb1 = mx1 * LOG2E;
-      uint32_t pf[16];
-      float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-      for (int i2 = 0; i2 < 16; ++i2) {
-        const float mb = (i2 & 1) ? mb1 : mb0;
-        pf[i2] = tc::pack_bf16x2(exp2f(fmaf(s[2 * i2], LOG2E, -mb)), exp2f(fmaf(s[2 * i2 + 1], LOG2E, -mb)));
-        float e0, e1;
-        tc::unpack_bf16x2(pf[i2], e0, e1);     // l accumulates exactly what the P V MMA sees
-        if (i2 & 1) l1 += e0 + e1;
-        else l0 += e0 + e1;
-      }
-      l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-      l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-      l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-      l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-      // ---- O = P V
+      // ---- softmax in registers (one key block, unbounded) and O = P V.  Key column block j lies in quadrant j / 2.
+      float mx0 = -INFINITY, mx1 = -INFINITY, l0 = 0.f, l1 = 0.f;
       float o[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) o[j] = 0.f;
-      tc::wg_fence_acc(o);
-      tc::wg_fence_acc(pf);
-      tc::wg_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {        // 16 keys per step: rows 16 kk.. of V
-        const uint32_t a[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
-        tc::wgmma_64_rs<1>(o, a, vdesc + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
-      }
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(o);
-      const float inv0 = __frcp_rn(l0), inv1 = __frcp_rn(l1);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        o[4 * j] *= inv0;
-        o[4 * j + 1] *= inv0;
-        o[4 * j + 2] *= inv1;
-        o[4 * j + 3] *= inv1;
-      }
+      auto key_ok = [&](int j) { return tc::seam_ok(quad, j >> 1, seam_r, seam_c); };
+      tc::softmax_pv<64, false>(s, key_ok, false, mx0, mx1, l0, l1, o, vdesc);
+      tc::softmax_normalize(o, l0, l1);
       uint32_t oh[16];
       to_afrag(o, oh);
 #pragma unroll
@@ -363,27 +299,10 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
     tc::wg_fence_acc(acc);
     // ---- epilogue: x_new = acc + x (residual from the X tile in shared memory), in place, then TMA store of this window
     uint8_t* xt = sX + (size_t)xs.slot * AB_X_BYTES;
-    float ss0 = 0.f, ss1 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      uint8_t* sub = xt + (j >> 3) * A_STAGE_BYTES;
-      uint32_t* p0 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0, j & 7) + cq * 2);
-      uint32_t* p1 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0 + 8, j & 7) + cq * 2);
-      const uint32_t x0 = *p0, x1 = *p1;
-      const float a0 = acc[4 * j] + __uint_as_float(x0 << 16), a1 = acc[4 * j + 1] + __uint_as_float(x0 & 0xffff0000u);
-      const float b0 = acc[4 * j + 2] + __uint_as_float(x1 << 16), b1 = acc[4 * j + 3] + __uint_as_float(x1 & 0xffff0000u);
-      ss0 = fmaf(a0, a0, fmaf(a1, a1, ss0));
-      ss1 = fmaf(b0, b0, fmaf(b1, b1, ss1));
-      *p0 = tc::pack_bf16x2(a0, a1);
-      *p1 = tc::pack_bf16x2(b0, b1);
-    }
-    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
-    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
-    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
-    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+    const float2 ss = tc::residual_add(xt, r0, cq, acc);
     if ((lane & 3) == 0) {
-      p.ss_out[m0 * SS_PARTS] = ss0;
-      p.ss_out[m1 * SS_PARTS] = ss1;
+      p.ss_out[m0 * SS_PARTS] = ss.x;
+      p.ss_out[m1 * SS_PARTS] = ss.y;
     }
     tc::fence_proxy_async();
     tc::named_barrier_sync(tc::BAR_WG + wg, 128);
@@ -391,7 +310,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) gemm_wg_attn_block_kernel(const
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         int r, c;
-        ab_quad(p, wi, wj, q, r, c);
+        tc::quad_origin(wi, wj, q, p.h, p.w, p.shift, r, c);
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) tc::tma_store_4d(&tmx, xt + kb * A_STAGE_BYTES + wg * AB_KV_BYTES + q * 2048, kb * BK, c, r, b);
       }
@@ -413,21 +332,13 @@ int launch_attn_block_impl(bf16* x, const bf16* w_qkv, const bf16* w_out, const 
                            int shift, const float* ss_in, float* ss_out, cudaStream_t st) {
   CUtensorMap tx, twq, two;
   int rc;
-  const uint64_t dims[4] = {(uint64_t)AB_C, (uint64_t)w, (uint64_t)h, (uint64_t)B};
-  const uint64_t strides[3] = {(uint64_t)AB_C * 2, (uint64_t)AB_C * 2 * w, (uint64_t)AB_C * 2 * w * h};
-  const uint32_t box[4] = {BK, 4, 4, 1};
-  if ((rc = make_tmap_bf16(&tx, x, 4, dims, strides, box))) return rc;
+  if ((rc = make_tmap_tokens(&tx, x, AB_C, B, h, w, BK, 4, 4))) return rc;
   if ((rc = tmap_2d(&twq, w_qkv, AB_C, 3 * AB_C, BK, 192))) return rc;
   if ((rc = tmap_2d(&two, w_out, AB_C, AB_C, BK, AB_C))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    KDB_CUDA(cudaFuncSetAttribute(gemm_wg_attn_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AB_SMEM));
-    attr_set = true;
-  }
+  static bool opened = false;
+  if ((rc = set_smem_once(gemm_wg_attn_block_kernel, opened, (int)AB_SMEM))) return rc;
   AttnBlockParams p{ss_in, ss_out, reinterpret_cast<const float4*>(rope), qk_scale, h, w, shift, B * (h / 8) * (w / 8)};
-  const int n_tiles = (p.nwin + 1) / 2;
-  KDB_CUDA(launch_pdl(gemm_wg_attn_block_kernel, dim3((unsigned)(n_tiles < num_sms() ? n_tiles : num_sms())), dim3(AB_THREADS), AB_SMEM, st,
-                      tx, twq, two, p));
+  KDB_CUDA(launch_pdl(gemm_wg_attn_block_kernel, persistent_grid((p.nwin + 1) / 2), dim3(AB_THREADS), AB_SMEM, st, tx, twq, two, p));
   KDB_LAUNCH_CHECK(F_GEMM_TC, st);
   return 0;
 }

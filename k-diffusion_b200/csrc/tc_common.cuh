@@ -14,11 +14,21 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its predecessor in the stream is
-// still running; pdl_wait() blocks until the predecessor has completed and its writes are visible.  pdl_launch_dependents()
-// tells the scheduler that the NEXT kernel's CTAs may be placed as soon as this grid's CTAs have all passed this point (or
-// exited) and resources free up.  Both are no-ops for ordinary launches.
+// still running; pdl_wait() blocks until the predecessor has completed and its writes are visible (KDB_PDL_TRIGGER, common.cuh,
+// lets the next kernel start).  A no-op for ordinary launches.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// ---------------------------------------------------------------- persistent kernels
+// The kernel's dynamic shared memory from its first 1024-byte boundary on (SWIZZLE_128B tiles need that alignment); the kernels
+// request 1 KiB more than their layout for it.
+__device__ __forceinline__ uint8_t* smem_1k() {
+  extern __shared__ uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+}
+// How many of `tiles` this CTA owns: a persistent CTA takes tiles blockIdx.x, + gridDim.x, ...
+__device__ __forceinline__ int tiles_owned(int tiles) {
+  return (int)blockIdx.x < tiles ? (tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+}
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -52,21 +62,9 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: a protocol bug traps after 2 s with a message instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const uint64_t t0 = globaltimer_ns();
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 63u) == 0 && globaltimer_ns() - t0 > 2000000000ull) {
-      printf("libkdb200: mbarrier wait timed out (block %d,%d,%d thread %d parity %u)\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-
-// mbar_wait without the message: a kernel whose function body contains a call (printf is one) gets every wgmma serialised by ptxas
-// (each one waited for before the next issues) and the caller-saved registers around the call spilled.  Still bounded: traps after 2 s.
+// Bounded wait: a protocol bug traps after 2 s instead of hanging the GPU.  No message: a kernel whose function body contains a call
+// (printf is one) gets every wgmma serialised by ptxas (each one waited for before the next issues) and the caller-saved registers
+// around the call spilled.
 __device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const uint64_t t0 = globaltimer_ns();
@@ -329,12 +327,140 @@ __device__ __forceinline__ void unpack_bf16x2(uint32_t v, float& lo, float& hi) 
   hi = __high2float(t);
 }
 
+// ---------------------------------------------------------------- shifted windows of 8x8 tokens (reference image_transformer_v2.py:253-337)
+// A window moves as four 4x4-token quadrant boxes; its rows are quadrant-major, then (row, column) inside the quadrant.
+// window `win` of a [B, h, w] token grid -> image b, window row wi, window column wj
+__device__ __forceinline__ void window_coords(int win, int h, int w, int& b, int& wi, int& wj) {
+  const int nww = w >> 3, per_img = (h >> 3) * nww;
+  b = win / per_img;
+  const int rem = win - b * per_img;
+  wi = rem / nww;
+  wj = rem - wi * nww;
+}
+// origin of quadrant q of window (wi, wj) in original coordinates: the roll of the shifted layers (:274)
+__device__ __forceinline__ void quad_origin(int wi, int wj, int q, int h, int w, int shift, int& r, int& c) {
+  r = (wi * 8 + (q >> 1) * 4 - shift + h) % h;
+  c = (wj * 8 + (q & 1) * 4 - shift + w) % w;
+}
+// seam mask (:300-315): in the top (seam_r) / left (seam_c) windows of a shifted layer a query of quadrant qq sees a key of quadrant kq
+// only on its own side of the wrapped row / column
+__device__ __forceinline__ bool seam_ok(int qq, int kq, bool seam_r, bool seam_c) {
+  return (!seam_r || ((kq >> 1) == (qq >> 1))) && (!seam_c || ((kq & 1) == (qq & 1)));
+}
+
+// ---------------------------------------------------------------- attention on a register score fragment
+// One key block of O = softmax(S) V for the 64 query rows of a warpgroup.  s: S [64 x NK] as a wgmma fragment (rows rw, rw + 8, column
+// pair 2 (t % 4) of every 8-column block c); key_ok(c): block c's keys are visible.  mx0 / mx1: the rows' maxima so far (BOUNDED: the
+// fixed shift exp(s - bound)); l0 / l1: this thread's part of the rows' sums of P; o += P V.  Without the bound, when `rescale` (a later
+// key block) l and o are rescaled from the old maximum to the new one.  P is rounded to bf16, the register A operand of the P V wgmma,
+// and l sums the rounded values.  vdesc: V [NK keys x 64] bf16, an MN-major SW128 operand.
+template <int NK, bool BOUNDED, typename KeyOk>
+__device__ __forceinline__ void softmax_pv(float (&s)[NK / 2], const KeyOk& key_ok, bool rescale, float& mx0, float& mx1, float& l0, float& l1,
+                                           float (&o)[32], uint64_t vdesc) {
+  constexpr float LOG2E = 1.4426950408889634f;
+  if constexpr (!BOUNDED) {
+    float n0 = mx0, n1 = mx1;
+#pragma unroll
+    for (int c = 0; c < NK / 8; ++c) {
+      if (!key_ok(c)) s[4 * c] = s[4 * c + 1] = s[4 * c + 2] = s[4 * c + 3] = -INFINITY;
+      n0 = fmaxf(n0, fmaxf(s[4 * c], s[4 * c + 1]));
+      n1 = fmaxf(n1, fmaxf(s[4 * c + 2], s[4 * c + 3]));
+    }
+    n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 1));
+    n0 = fmaxf(n0, __shfl_xor_sync(0xffffffffu, n0, 2));
+    n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 1));
+    n1 = fmaxf(n1, __shfl_xor_sync(0xffffffffu, n1, 2));
+    if (rescale) {                             // the maximum grew: rescale what was accumulated against the old one
+      const float a0 = exp2f((mx0 - n0) * LOG2E), a1 = exp2f((mx1 - n1) * LOG2E);
+      l0 *= a0;
+      l1 *= a1;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        o[4 * c] *= a0;
+        o[4 * c + 1] *= a0;
+        o[4 * c + 2] *= a1;
+        o[4 * c + 3] *= a1;
+      }
+    }
+    mx0 = n0;
+    mx1 = n1;
+  }
+  const float mb0 = mx0 * LOG2E, mb1 = mx1 * LOG2E;
+  uint32_t pf[NK / 4];
+#pragma unroll
+  for (int i2 = 0; i2 < NK / 4; ++i2) {
+    const float mb = (i2 & 1) ? mb1 : mb0;
+    float p0 = exp2f(fmaf(s[2 * i2], LOG2E, -mb)), p1 = exp2f(fmaf(s[2 * i2 + 1], LOG2E, -mb));
+    if (BOUNDED && !key_ok(i2 >> 1)) p0 = p1 = 0.f;   // (bounded) zero probability instead of a -inf logit
+    pf[i2] = pack_bf16x2(p0, p1);
+    float e0, e1;
+    unpack_bf16x2(pf[i2], e0, e1);             // l accumulates exactly what the P V MMA sees
+    if (i2 & 1) l1 += e0 + e1;
+    else l0 += e0 + e1;
+  }
+  // ---- O += P V, 16 keys per step: rows 16 kk.. of V
+  wg_fence_acc(o);
+  wg_fence_acc(pf);
+  wg_fence();
+#pragma unroll
+  for (int kk = 0; kk < NK / 16; ++kk) {
+    const uint32_t a[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
+    wgmma_64_rs<1>(o, a, vdesc + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
+  }
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(o);
+}
+// after the last key block: O / l, l summed over the quad that holds a row
+__device__ __forceinline__ void softmax_normalize(float (&o)[32], float l0, float l1) {
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = __frcp_rn(l0), inv1 = __frcp_rn(l1);
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    o[4 * c] *= inv0;
+    o[4 * c + 1] *= inv0;
+    o[4 * c + 2] *= inv1;
+    o[4 * c + 3] *= inv1;
+  }
+}
+
+// ---------------------------------------------------------------- residual epilogue of the fused kernels
+// x += acc in place, where acc is a thread's fragment of 64 rows x 128 columns (rows r, r + 8, column pair cq of every 8-column block)
+// and x a bf16 tile of 128 columns held as two [128 x 64] SW128 halves of 16 KiB.  Returns the two rows' sums of squares of the new x,
+// reduced over the quad.
+__device__ __forceinline__ float2 residual_add(uint8_t* xt, int r, int cq, const float (&acc)[64]) {
+  float ss0 = 0.f, ss1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    uint8_t* sub = xt + (j >> 3) * (128 * 128);
+    uint32_t* p0 = reinterpret_cast<uint32_t*>(sub + sw128_offset(r, j & 7) + cq * 2);
+    uint32_t* p1 = reinterpret_cast<uint32_t*>(sub + sw128_offset(r + 8, j & 7) + cq * 2);
+    const uint32_t x0 = *p0, x1 = *p1;
+    const float a0 = acc[4 * j] + __uint_as_float(x0 << 16), a1 = acc[4 * j + 1] + __uint_as_float(x0 & 0xffff0000u);
+    const float b0 = acc[4 * j + 2] + __uint_as_float(x1 << 16), b1 = acc[4 * j + 3] + __uint_as_float(x1 & 0xffff0000u);
+    ss0 = fmaf(a0, a0, fmaf(a1, a1, ss0));
+    ss1 = fmaf(b0, b0, fmaf(b1, b1, ss1));
+    *p0 = pack_bf16x2(a0, a1);
+    *p1 = pack_bf16x2(b0, b1);
+  }
+  ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
+  ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
+  ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
+  ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+  return make_float2(ss0, ss1);
+}
+
 }  // namespace tc
 
 // ---------------------------------------------------------------- host: tensor maps
 // 2-D..4-D bf16 tensor map with 128B swizzle; dims/strides innermost first (strides in bytes, for dims 1..rank-1).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box);
+// [B, h, w, C] bf16 tokens as the 4-D map (C, w, h, B) with box {box_c, box_w, box_h, 1}
+int make_tmap_tokens(CUtensorMap* out, const void* base, uint64_t C, int B, int h, int w, uint32_t box_c, uint32_t box_w, uint32_t box_h);
 
 // SM count of the current device: the grid of the persistent kernels
 inline int num_sms() {
@@ -345,6 +471,8 @@ inline int num_sms() {
   }();
   return n;
 }
+// grid of a persistent kernel over `tiles` tiles: min(tiles, SMs) CTAs
+inline dim3 persistent_grid(int64_t tiles) { return dim3((unsigned)(tiles < num_sms() ? tiles : num_sms())); }
 
 // ---------------------------------------------------------------- host: programmatic dependent launch
 // Launches `kernel` with programmatic stream serialization, so that its prologue overlaps the tail of the previous kernel in the

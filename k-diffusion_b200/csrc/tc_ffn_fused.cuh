@@ -52,16 +52,13 @@ struct FfnParams {
 __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmwu,
                                                                  const __grid_constant__ CUtensorMap tmwd, const __grid_constant__ CUtensorMap tmo,
                                                                  const FfnParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sX = base;
+  uint8_t* sX = tc::smem_1k();
   uint8_t* sWU = sX + FF_XBUF * FF_X_BYTES;
   uint8_t* sWD = sWU + FF_WU * FF_WU_BYTES;
   FfnBars* bars = reinterpret_cast<FfnBars*>(sWD + FF_WD * FF_WD_BYTES);
   const int pwarp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nc = p.nc;
-  const int m_tiles = (int)(p.M / BM);
-  const int n_local = (int)blockIdx.x < m_tiles ? (m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const int n_local = tc::tiles_owned((int)(p.M / BM));
 
   if (threadIdx.x == 0) {
     tc::tma_prefetch_desc(&tmx);
@@ -75,7 +72,7 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
   }
   __syncthreads();
   tc::pdl_wait();                    // x (and its row statistics) come from the kernel before us
-  tc::pdl_launch_dependents();
+  KDB_PDL_TRIGGER();
 
   if (pwarp >= 8) {
     // ------------------------------------------------------------------ TMA producer
@@ -198,28 +195,10 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
     ds.advance();
     // ---- final epilogue: out = acc2 + x (residual from the X tile in shared memory), in place, then TMA store of this half
     uint8_t* xt = sX + (size_t)xs.slot * FF_X_BYTES;
-    float ss0 = 0.f, ss1 = 0.f;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      uint8_t* sub = xt + (j >> 3) * SUB_TILE_BYTES;
-      const uint32_t in16 = (uint32_t)(cq * 2);              // byte offset of the column pair inside its 16-byte chunk
-      uint32_t* p0 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0, j & 7) + in16);
-      uint32_t* p1 = reinterpret_cast<uint32_t*>(sub + tc::sw128_offset(r0 + 8, j & 7) + in16);
-      const uint32_t x0 = *p0, x1 = *p1;
-      const float a0 = acc2[4 * j] + __uint_as_float(x0 << 16), a1 = acc2[4 * j + 1] + __uint_as_float(x0 & 0xffff0000u);
-      const float b0 = acc2[4 * j + 2] + __uint_as_float(x1 << 16), b1 = acc2[4 * j + 3] + __uint_as_float(x1 & 0xffff0000u);
-      ss0 = fmaf(a0, a0, fmaf(a1, a1, ss0));
-      ss1 = fmaf(b0, b0, fmaf(b1, b1, ss1));
-      *p0 = tc::pack_bf16x2(a0, a1);
-      *p1 = tc::pack_bf16x2(b0, b1);
-    }
-    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1);
-    ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
-    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1);
-    ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+    const float2 ss = tc::residual_add(xt, r0, cq, acc2);
     if (p.ss_out != nullptr && (lane & 3) == 0) {
-      p.ss_out[(m0 + r0) * SS_PARTS] = ss0;
-      p.ss_out[(m0 + r0 + 8) * SS_PARTS] = ss1;
+      p.ss_out[(m0 + r0) * SS_PARTS] = ss.x;
+      p.ss_out[(m0 + r0 + 8) * SS_PARTS] = ss.y;
     }
     tc::fence_proxy_async();
     tc::named_barrier_sync(tc::BAR_WG + wg, 128);
@@ -244,15 +223,10 @@ int launch_ffn_fused_impl(bf16* x, const bf16* w_up_il, const bf16* w_down, int6
   if ((rc = tmap_2d(&twu, w_up_il, FF_C, (uint64_t)2 * dff, BK, 128))) return rc;
   if ((rc = tmap_2d(&twd, w_down, (uint64_t)dff, FF_C, BK, FF_C))) return rc;
   if ((rc = tmap_2d(&to, x, FF_C, (uint64_t)M, 64, BM / 2))) return rc;     // each warpgroup stores its 64 rows
-  static bool attr_set = false;
-  if (!attr_set) {
-    KDB_CUDA(cudaFuncSetAttribute(ffn_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_SMEM));
-    attr_set = true;
-  }
+  static bool opened = false;
+  if ((rc = set_smem_once(ffn_fused_kernel, opened, (int)FF_SMEM))) return rc;
   FfnParams p{ss_in, ss_out, M, dff / FF_CH};
-  const int64_t m_tiles = M / BM;
-  KDB_CUDA(launch_pdl(ffn_fused_kernel, dim3((unsigned)(m_tiles < num_sms() ? m_tiles : num_sms())), dim3(FF_THREADS), FF_SMEM, st, tx, twu,
-                      twd, to, p));
+  KDB_CUDA(launch_pdl(ffn_fused_kernel, persistent_grid(M / BM), dim3(FF_THREADS), FF_SMEM, st, tx, twu, twd, to, p));
   KDB_LAUNCH_CHECK(F_GEMM_TC, st);
   return 0;
 }
