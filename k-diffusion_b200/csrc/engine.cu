@@ -425,14 +425,18 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
   const bool ffn = f.fold && f.stats && L.up_wf != nullptr && tc_ffn_fused_supported(M, C, L.dff) && !m->tapped(tag + ".geglu");
   if constexpr (std::is_same_v<T, bf16>) {
     T* xn = reinterpret_cast<T*>(f.ws.xn);
+    GemmEpi ge;
+    ge.mode = EPI_GEGLU;
+    GemmEpi gf = ge;
+    gf.ss_in = f.ws.rowss;
     if (ffn) {
       rc = launch_ffn_fused(x, L.up_wf, L.down_wb, M, C, L.dff, f.ws.rowss, f.ws.rowss, f.st);
       f.stats = true;
-    } else if (f.fold && f.stats && L.up_wf != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C, true)) {
-      rc = launch_gemm_tc_geglu(x, L.up_wf, gb, M, 2 * L.dff, C, f.st, f.ws.rowss);
-    } else if (L.up_wb_il != nullptr && tc_gemm_geglu_supported(M, 2 * L.dff, C)) {
+    } else if (f.fold && f.stats && L.up_wf != nullptr && tc_gemm_supported(M, 2 * L.dff, C, gf)) {
+      rc = launch_gemm_tc(x, L.up_wf, gb, M, 2 * L.dff, C, gf, f.st);
+    } else if (L.up_wb_il != nullptr && tc_gemm_supported(M, 2 * L.dff, C, ge)) {
       rc = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-      if (!rc) rc = launch_gemm_tc_geglu(xn, L.up_wb_il, gb, M, 2 * L.dff, C, f.st);
+      if (!rc) rc = launch_gemm_tc(xn, L.up_wb_il, gb, M, 2 * L.dff, C, ge, f.st);
     } else {
       rc = unfused();
     }
@@ -484,10 +488,10 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       r = launch_patch_in<T>(v, sigma, sd, m->patch_in_w, cur + (int64_t)B * h0 * w0 * C0, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
     return r;
   };
-  // patch_in: on the tensor core, which leaves the row statistics for the first fused RMSNorm, or the scalar kernel
+  // patch_in: on the tensor core, which leaves the row statistics for the first fused RMSNorm, or the scalar kernel (other patch
+  // geometries, where finalize made no patch_in_wb, and latents that start inside a 16-byte granule)
   if constexpr (kBf16) {
-    if (m->patch_in_wb != nullptr && tc_patch_in_supported(c.in_channels, c.patch_h, c.patch_w, C0, W) &&
-        (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    if (m->patch_in_wb != nullptr && tc_patch_in_supported(x, C0, W)) {
       f.stats = f.emit;
       rc = launch_patch_in_tc(x, sigma, sd, m->patch_in_wb, cur, B, H, W, C0, f.stats ? ws.rowss : nullptr, st);
     } else {
@@ -562,14 +566,23 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   // The tensor-core epilogue un-patches and applies the Karras combine; it reads x and writes out as float4, so a view that starts
   // inside a 16-byte granule (a storage offset, a caller's out= buffer) takes the scalar kernel.
   if constexpr (kBf16) {
-    const bool aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sd <= 0.f || (reinterpret_cast<uintptr_t>(x) & 15) == 0);
-    if (m->patch_out_wb != nullptr && aligned && tc_patch_out_supported(C0, c.out_channels, c.patch_h, c.patch_w, W)) {
-      if (f.stats && m->patch_out_wf != nullptr && C0 % 128 == 0 && C0 <= 128 * SS_PARTS)
-        return launch_patch_out_tc(cur, m->patch_out_wf, x, sigma, sd, out, B, H, W, C0, st, ws.rowss);
+    const int64_t M0 = (int64_t)B * h0 * w0;
+    GemmEpi pe;
+    pe.mode = EPI_PATCH_OUT;
+    pe.img = out;
+    pe.x_in = x;
+    pe.sigma = sigma;
+    pe.sigma_data = sd;
+    pe.H = H;
+    pe.W = W;
+    GemmEpi pf = pe;
+    pf.ss_in = ws.rowss;
+    if (f.stats && m->patch_out_wf != nullptr && tc_gemm_supported(M0, 64, C0, pf))
+      return launch_gemm_tc(cur, m->patch_out_wf, nullptr, M0, 64, C0, pf, st);
+    if (m->patch_out_wb != nullptr && tc_gemm_supported(M0, 64, C0, pe)) {
       bf16* xn = reinterpret_cast<bf16*>(ws.xn);
-      const int64_t M0 = (int64_t)B * h0 * w0;
       if ((rc = launch_rmsnorm<bf16>(cur, xn, m->out_norm, 0, M0, M0, C0, st))) return rc;
-      return launch_patch_out_tc(xn, m->patch_out_wb, x, sigma, sd, out, B, H, W, C0, st);
+      return launch_gemm_tc(xn, m->patch_out_wb, nullptr, M0, 64, C0, pe, st);
     }
   }
   if (tape)
@@ -786,7 +799,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   }
   m->patch_out_wb = nullptr;
   m->patch_out_wf = nullptr;
-  if (Np <= 64) {   // zero-padded bf16 patch_out weight [64, C0]
+  if (c.out_channels == 3 && c.patch_h == 4 && c.patch_w == 4) {   // zero-padded bf16 patch_out weight [64, C0] of the EPI_PATCH_OUT GEMM
     if ((rc = m->alloc(&m->patch_out_wb, (size_t)64 * C0))) return rc;
     KDB_CUDA(cudaMemsetAsync(m->patch_out_wb, 0, (size_t)64 * C0 * sizeof(bf16), st));
     if ((rc = launch_f32_to_bf16(m->patch_out_w, m->patch_out_wb, (int64_t)Np * C0, st))) return rc;

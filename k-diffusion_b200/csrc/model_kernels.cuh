@@ -6,10 +6,13 @@
 
 namespace kdb {
 
-enum GemmEpilogue { EPI_STORE = 0, EPI_RESID = 1, EPI_SPLIT_LERP = 2, EPI_QKV_ROPE = 3 };
+// The epilogue of a token-stream GEMM.  The values are gemm_wg_kernel's EPI template argument; the SIMT GEMM runs STORE, RESID and
+// SPLIT_LERP only.
+enum GemmEpilogue { EPI_STORE = 0, EPI_RESID = 1, EPI_GEGLU = 2, EPI_SPLIT_LERP = 3, EPI_QKV_ROPE = 4, EPI_PATCH_OUT = 5 };
 
 struct GemmEpi {
   int mode = EPI_STORE;
+  // EPI_GEGLU (tensor-core path only): the rows of W interleave 8 value / 8 gate rows; out[M, N/2] = value * gelu(gate)
   const void* resid = nullptr;   // EPI_RESID: [M,N] same type as out.  EPI_SPLIT_LERP: skip [B, 2hc, 2wc, C]
   const float* fac = nullptr;    // EPI_SPLIT_LERP: device scalar (TokenSplit.fac)
   int hc = 0, wc = 0, C = 0;     // EPI_SPLIT_LERP: coarse grid and fine channel count (N == 4*C)
@@ -20,12 +23,20 @@ struct GemmEpi {
   // TokenMerge folded into the A-operand load (tensor-core path only): A = fine tokens [B, 2*mhc, 2*mwc, mC], K = 4*mC in
   // (nh nw e) order, M = B*mhc*mwc.  mC == 0 -> A is a plain [M, K] matrix.
   int mhc = 0, mwc = 0, mC = 0;
-  // fused RMSNorm (tensor-core kernel only).  Consumer (EPI_STORE / EPI_QKV_ROPE): A is the raw residual stream, W
-  // already carries the channel scale, ss_in [M, 8] holds sum(x^2) per 128-channel block of every row and the epilogue scales
-  // the accumulator by 1/rms (q/k thirds of EPI_QKV_ROPE are scale invariant).  Producer (EPI_RESID / EPI_SPLIT_LERP): ss_out
-  // receives those sums for the rows written.
+  // fused RMSNorm (tensor-core kernel only).  Consumer (EPI_STORE / EPI_QKV_ROPE / EPI_GEGLU / EPI_PATCH_OUT): A is the raw
+  // residual stream, W already carries the channel scale, ss_in [M, 8] holds sum(x^2) per 128-channel block of every row and the
+  // epilogue scales the accumulator by 1/rms (q/k thirds of EPI_QKV_ROPE are scale invariant).  Producer (EPI_RESID /
+  // EPI_SPLIT_LERP, and EPI_STORE): ss_out receives those sums for the rows written.
   const float* ss_in = nullptr;
   float* ss_out = nullptr;
+  // EPI_PATCH_OUT (tensor-core path only): rows are the tokens [B, H/4, W/4], columns the 4x4 patches of 3 channels (48 of N = 64
+  // used).  The GEMM's bf16 output is unused: the epilogue un-patches to img, fp32 NCHW [B, 3, H, W], and with sigma_data > 0
+  // applies the Karras combine with x_in [B, 3, H, W] and sigma [B].
+  float* img = nullptr;
+  const float* x_in = nullptr;
+  const float* sigma = nullptr;
+  float sigma_data = 0.f;
+  int H = 0, W = 0;
 };
 
 // x [B,C,H,W] fp32 (* c_in(sigma) if sigma_data > 0) -> tokens [B, H/ph, W/pw, N]   (image_transformer_v2.py:586-595,723-724)

@@ -3,9 +3,11 @@
 // M edge by the tensor map).
 //
 // C[M,N] = A[M,K] W[N,K]^T for every nn.Linear on the token stream (reference image_transformer_v2.py:126-139).
-// Epilogues: plain store; +residual (out_proj / down_proj, :396,:493; residual tile prefetched by TMA while the main loop
-// runs); GEGLU (:89-95; rows of W interleaved 8 value / 8 gate); cosine-sim scaling + axial RoPE of q and k fused into the
-// qkv projection (:106-114,187-199,245-248; cos/sin from a per-layer table); TokenSplit scatter + lerp (:618-621).
+// Epilogues (GemmEpilogue): EPI_STORE; EPI_RESID, +residual (out_proj / down_proj, :396,:493; residual tile prefetched by TMA
+// while the main loop runs); EPI_GEGLU (:89-95; rows of W interleaved 8 value / 8 gate); EPI_SPLIT_LERP, TokenSplit scatter + lerp
+// (:618-621); EPI_QKV_ROPE, cosine-sim scaling + axial RoPE of q and k fused into the qkv projection (:106-114,187-199,245-248;
+// cos/sin from a per-layer table); EPI_PATCH_OUT, TokenSplitWithoutSkip 4x4 to fp32 NCHW + the Karras combine (:598-607,:758-760).
+// One descriptor (GemmEpi), one predicate (tc_gemm_supported) and one launcher (launch_gemm_tc) for all of them.
 #include "tc_common.cuh"
 #include "tc_kernels.cuh"
 
@@ -75,29 +77,13 @@ constexpr int SUB_TILE_BYTES = BM * 128;     // one [128 x 64] bf16 output sub-t
 constexpr int GEMM_THREADS = 384;            // warpgroups 0, 1: MMA + epilogue of alternate tiles, warpgroup 2: TMA producer (one warp)
 constexpr int GEMM_RING_BYTES = 96 * 1024;   // TMA ring: 3 stages of a 128-wide tile, 4 of a 64-wide one
 
-enum TcEpi { TCE_STORE = 0, TCE_RESID = 1, TCE_GEGLU = 2, TCE_SPLIT = 3, TCE_QKV = 4, TCE_PATCHOUT = 5 };
-
-struct TcParams {
+// The kernel's parameter block: the epilogue descriptor, the output and the shape, and what launch_gemm_tc derives from them.
+struct GemmArgs : GemmEpi {
   bf16* out;
-  const bf16* resid;     // SPLIT: skip [B, 2hc, 2wc, Cf]
-  const float* fac;
   int64_t M;
   int N, K;
-  int hc, wc, Cf;
-  // QKV
-  const float2* rope;    // float4 [nh][8][T] (cos, cos, sin, sin) of angle pairs, see rope_table_kernel
-  const float* qk_scale; // [nh]
-  int C, nh, T;
-  // PATCHOUT (4x4 patches, 3 output channels): un-patch to NCHW fp32 + Karras combine with the input latent
-  float* fout;
-  const float* x_in;
-  const float* sigma;
-  float sd;
-  int H, Wimg, th, tw;
-  const float* ss_in;    // fused RMSNorm (consumer): A = raw x, W carries the channel scale; [M, SS_PARTS] sums of squares of x
-  float* ss_out;         // RESID / SPLIT / STORE (producer): sums of squares of the rows written, for the next fused RMSNorm
-  int a_merge, mwc, mC;  // A operand gathered from fine tokens (TokenMerge): coarse grid width, fine channels
-  int box_w, box_h;      // 5-D TMA box of the merge gather: 128 rows = box_h x box_w coarse tokens
+  int box_w, box_h;      // 5-D TMA box of the merge gather (mC > 0): 128 rows = box_h x box_w coarse tokens
+  int th, tw;            // EPI_PATCH_OUT: token grid H / 4 x W / 4
 };
 
 __device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
@@ -137,7 +123,7 @@ bool quad_box(int wc, int* box_w, int* box_h) {
 // warpgroup the bf16 output staging tile (RESID: the residual tile is loaded into it and the epilogue adds in place), then the
 // barriers.  128-wide RESID / STORE / QKV: 96 + 64 + 2 x 32 KiB + 1 KiB of alignment = 225 KiB.
 template <int BN, int EPI> constexpr int out_bytes() {
-  return EPI == TCE_GEGLU ? SUB_TILE_BYTES : (EPI == TCE_SPLIT || EPI == TCE_PATCHOUT) ? 0 : (BN / 64) * SUB_TILE_BYTES;
+  return EPI == EPI_GEGLU ? SUB_TILE_BYTES : (EPI == EPI_SPLIT_LERP || EPI == EPI_PATCH_OUT) ? 0 : (BN / 64) * SUB_TILE_BYTES;
 }
 template <int BN, int EPI> constexpr size_t gemm_smem() { return 1024 + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>() + 128; }
 
@@ -179,13 +165,13 @@ __device__ __forceinline__ void stage_ld32(const float* s, int row, int col0, fl
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
                                                                   const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
-                                                                  const TcParams p) {
+                                                                  const GemmArgs p) {
   KDB_PDL_TRIGGER();
   constexpr int B_STAGE_BYTES = BN * BK * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   constexpr int STAGES = GEMM_RING_BYTES / STAGE_BYTES;
   constexpr int NSUB = BN / 64;
-  constexpr bool RES = EPI == TCE_RESID;
+  constexpr bool RES = EPI == EPI_RESID;
   uint8_t* base = tc::smem_1k();
   float* sAcc = reinterpret_cast<float*>(base + GEMM_RING_BYTES);
   auto* ring = reinterpret_cast<tc::TmaRing<STAGES>*>(base + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>());
@@ -219,7 +205,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           const auto ps = PipeState<STAGES>::at(it);
           uint64_t* bar = ring->acquire(ps, STAGE_BYTES);
           uint8_t* a = base + (size_t)ps.slot * STAGE_BYTES;
-          if (p.a_merge) {   // TokenMerge: k-block kb lives in quadrant (nh, nw) of the fine grid, channels e0..e0+63
+          if (p.mC > 0) {    // TokenMerge: k-block kb lives in quadrant (nh, nw) of the fine grid, channels e0..e0+63
             const int qd = (kb * BK) / p.mC, e0 = kb * BK - qd * p.mC;
             tc::tma_load_5d(a, &tma, bar, e0, qd & 1, p.box_h == 1 ? (int)(m0 % p.mwc) : 0, qd >> 1, (int)(m0 / p.mwc));
           } else {
@@ -297,7 +283,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       const float4* sp = reinterpret_cast<const float4*>(p.ss_in + (m < p.M ? m : 0) * SS_PARTS);
       rstd = rsqrtf(tc::rowss_sum(__ldg(sp), __ldg(sp + 1), p.K >> 7) / (float)p.K + 1e-6f);
     }
-    if constexpr (EPI == TCE_PATCHOUT) {
+    if constexpr (EPI == EPI_PATCH_OUT) {
       // TokenSplitWithoutSkip 4x4 + NCHW + Denoiser combine (reference :598-607,:758-760, layers.py:88-90).  Row m = token
       // (b, ty, tx); column n = (nh*4 + nw)*3 + c.  For fixed (c, nh) the 4 nw pixels are one float4.
       float v[64];
@@ -319,24 +305,24 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
         const int r = (int)(m - (int64_t)b * per);
         const int ty = r / p.tw, tx = r - ty * p.tw;
         float c_skip = 0.f, c_out = 1.f, c_in;
-        if (p.sd > 0.f) karras_scalings(__ldg(p.sigma + b), p.sd, c_skip, c_out, c_in);
+        if (p.sigma_data > 0.f) karras_scalings(__ldg(p.sigma + b), p.sigma_data, c_skip, c_out, c_in);
 #pragma unroll
         for (int c = 0; c < 3; ++c)
 #pragma unroll
           for (int nh = 0; nh < 4; ++nh) {
-            const int64_t o = (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.Wimg + tx * 4;
+            const int64_t o = (((int64_t)b * 3 + c) * p.H + (ty * 4 + nh)) * p.W + tx * 4;
             float4 y = make_float4(bf16_round(v[(nh * 4 + 0) * 3 + c]), bf16_round(v[(nh * 4 + 1) * 3 + c]), bf16_round(v[(nh * 4 + 2) * 3 + c]),
                                    bf16_round(v[(nh * 4 + 3) * 3 + c]));
-            if (p.sd > 0.f) {
+            if (p.sigma_data > 0.f) {
               const float4 xi = __ldg(reinterpret_cast<const float4*>(p.x_in + o));
               y = make_float4(y.x * c_out + xi.x * c_skip, y.y * c_out + xi.y * c_skip, y.z * c_out + xi.z * c_skip, y.w * c_out + xi.w * c_skip);
             }
-            *reinterpret_cast<float4*>(p.fout + o) = y;
+            *reinterpret_cast<float4*>(p.img + o) = y;
           }
       }
-    } else if constexpr (EPI == TCE_SPLIT) {
+    } else if constexpr (EPI == EPI_SPLIT_LERP) {
       // TokenSplit + torch.lerp(skip, x, fac) (reference :618-621): row m = (b, hy, wx) on the coarse grid; 32 columns inside one
-      // (nh, nw) quadrant (Cf % 32 == 0), scattered to the fine token
+      // (nh, nw) quadrant (C % 32 == 0), scattered to the fine token
       const bool live = m < p.M;
       const float facv = __ldg(p.fac);
       float ss = 0.f;
@@ -351,10 +337,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
         const int64_t b = m / ((int64_t)p.hc * p.wc);
         const int r = (int)(m - b * p.hc * p.wc);
         const int hy = r / p.wc, wx = r - hy * p.wc;
-        const int qd = n / p.Cf, e = n - qd * p.Cf;
+        const int qd = n / p.C, e = n - qd * p.C;
         fine = (b * (2 * p.hc) + (2 * hy + (qd >> 1))) * (2 * p.wc) + (2 * wx + (qd & 1));
-        const int64_t off = fine * p.Cf + e;
-        const uint4* sk = reinterpret_cast<const uint4*>(p.resid + off);
+        const int64_t off = fine * p.C + e;
+        const uint4* sk = reinterpret_cast<const uint4*>(static_cast<const bf16*>(p.resid) + off);
         uint4* dst = reinterpret_cast<uint4*>(p.out + off);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -374,8 +360,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           dst[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
         }
       }
-      // statistics of the new residual stream for the next fused RMSNorm (BN = 128 inside one quadrant: Cf % 128 == 0)
-      if (p.ss_out != nullptr && live) p.ss_out[fine * SS_PARTS + ((n0 % p.Cf) >> 7)] = ss;
+      // statistics of the new residual stream for the next fused RMSNorm (BN = 128 inside one quadrant: C % 128 == 0)
+      if (p.ss_out != nullptr && live) p.ss_out[fine * SS_PARTS + ((n0 % p.C) >> 7)] = ss;
     } else {
       if constexpr (RES) tc::mbar_wait_nocall(&resid_full[wg], (uint32_t)(i >> 1) & 1u);
       float ss_acc[4] = {0.f, 0.f, 0.f, 0.f};   // producer side: sum of squares of the row this thread writes
@@ -390,16 +376,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
         }
         if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
-        if (EPI != TCE_GEGLU && p.ss_in != nullptr) {
+        if (EPI != EPI_GEGLU && p.ss_in != nullptr) {
           // fused RMSNorm row scale.  q and k are cosine-normalised afterwards (scale invariant): only v needs it.
           bool apply = true;
-          if constexpr (EPI == TCE_QKV) apply = (n0 + g * 64) >= 2 * p.C;
+          if constexpr (EPI == EPI_QKV_ROPE) apply = (n0 + g * 64) >= 2 * p.C;
           if (apply) {
 #pragma unroll
             for (int k = 0; k < 64; ++k) v[k] *= rstd;
           }
         }
-        if constexpr (EPI == TCE_GEGLU) {
+        if constexpr (EPI == EPI_GEGLU) {
           // columns come as [8 value | 8 gate] groups (interleaved up_proj rows) -> 32 outputs = chunks 4g..4g+3 of the output sub-tile
           const tc::f32x2 r2 = tc::pk2(rstd, rstd), rh = tc::pk2(0.5f * rstd, 0.5f * rstd);     // the GELU's 0.5 rides on the value's row scale
 #pragma unroll
@@ -431,7 +417,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
               }
             }
           }
-          if constexpr (RES || EPI == TCE_STORE) {
+          if constexpr (RES || EPI == EPI_STORE) {
             if (p.ss_out != nullptr) {
 #pragma unroll
               for (int k = 0; k < 64; k += 4) {
@@ -442,14 +428,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
               }
             }
           }
-          if constexpr (EPI == TCE_QKV) {
+          if constexpr (EPI == EPI_QKV_ROPE) {
             const int n = n0 + g * 64;               // one head of q, k or v (feature order (t nh e), d_head 64)
             const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
             if (t3 < 2) {
               // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248).  Columns (2i, 2i+1) pair with (16+2i, 17+2i); the
               // table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4.
-              const int64_t tok = (m < p.M ? m : 0) % p.T;
-              const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T + tok;   // [head][i][token]
+              const int64_t tok = (m < p.M ? m : 0) % p.T_tokens;
+              const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T_tokens + tok;   // [head][i][token]
               tc::f32x2 P[32];
 #pragma unroll
               for (int k = 0; k < 32; ++k) P[k] = tc::pk2(v[2 * k], v[2 * k + 1]);
@@ -465,7 +451,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
               const tc::f32x2 sc2 = tc::pk2(sc, sc);
 #pragma unroll
               for (int k = 0; k < 8; ++k) {
-                const float4 cs = __ldg(tb + (int64_t)k * p.T);
+                const float4 cs = __ldg(tb + (int64_t)k * p.T_tokens);
                 const tc::f32x2 C = tc::pk2(cs.x, cs.y), S = tc::pk2(cs.z, cs.w);
                 const tc::f32x2 X1 = P[k], X2 = P[8 + k];
                 P[k] = tc::mul2(tc::fma2(X2, tc::neg2(S), tc::mul2(X1, C)), sc2);
@@ -484,13 +470,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
                            tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
         }
       }
-      if constexpr (RES || EPI == TCE_STORE) {
+      if constexpr (RES || EPI == EPI_STORE) {
         if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = (ss_acc[0] + ss_acc[1]) + (ss_acc[2] + ss_acc[3]);
       }
       tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
       tc::named_barrier_sync(tc::BAR_WG + wg, 128);
       if (row == 0) {
-        if constexpr (EPI == TCE_GEGLU) {
+        if constexpr (EPI == EPI_GEGLU) {
           tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
         } else {
 #pragma unroll
@@ -508,22 +494,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
 #include "tc_attn_block.cuh"
 
 template <int BN, int EPI>
-int launch_tc(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) {
+int launch_tc(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) {
   CUtensorMap ta, tb, tcm, tr;
   int rc;
-  if (p.a_merge) {
+  if (p.mC > 0) {
     if ((rc = tmap_quad(&ta, A, p.mC, p.mwc, (uint64_t)p.M / p.mwc, p.box_w, p.box_h))) return rc;
   } else {
     if ((rc = tmap_2d(&ta, A, (uint64_t)p.K, (uint64_t)p.M, BK, BM))) return rc;
   }
   if ((rc = tmap_2d(&tb, W, (uint64_t)p.K, (uint64_t)p.N, BK, BN))) return rc;
-  const uint64_t n_out = EPI == TCE_GEGLU ? (uint64_t)p.N / 2 : (uint64_t)p.N;
-  if (EPI != TCE_SPLIT && EPI != TCE_PATCHOUT) {
+  const uint64_t n_out = EPI == EPI_GEGLU ? (uint64_t)p.N / 2 : (uint64_t)p.N;
+  if (EPI != EPI_SPLIT_LERP && EPI != EPI_PATCH_OUT) {
     if ((rc = tmap_2d(&tcm, p.out, n_out, (uint64_t)p.M, 64, BM))) return rc;
   } else {
     tcm = ta;
   }
-  if (EPI == TCE_RESID) {
+  if (EPI == EPI_RESID) {
     if ((rc = tmap_2d(&tr, p.resid, (uint64_t)p.N, (uint64_t)p.M, 64, BM))) return rc;
   } else {
     tr = ta;
@@ -533,19 +519,58 @@ int launch_tc(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) 
   static bool opened = false;
   if ((rc = set_smem_once(gemm_wg_kernel<BN, EPI>, opened, (int)smem))) return rc;
   KDB_CUDA(launch_pdl(gemm_wg_kernel<BN, EPI>, persistent_grid(ceil_div(p.M, BM) * (p.N / BN)), dim3(GEMM_THREADS), smem, st, ta, tb, tcm, tr, p));
-  KDB_LAUNCH_CHECK(EPI == TCE_PATCHOUT ? F_PATCH_OUT : F_GEMM_TC, st);   // (the profiler's per-family bookkeeping only)
+  KDB_LAUNCH_CHECK(EPI == EPI_PATCH_OUT ? F_PATCH_OUT : F_GEMM_TC, st);   // (the profiler's per-family bookkeeping only)
   return 0;
 }
 
 // 128-wide tiles whenever N allows: they emit the per-128-channel row statistics of the fused RMSNorm
 template <int EPI>
-int dispatch_bn(const bf16* A, const bf16* W, const TcParams& p, cudaStream_t st) {
+int dispatch_bn(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) {
   if (p.N % 128 == 0) return launch_tc<128, EPI>(A, W, p, st);
   return launch_tc<64, EPI>(A, W, p, st);
 }
 
 bool shape_ok(int64_t M, int N, int K) {
   return M > 0 && M < (65535LL * BM) && N >= 64 && N % 64 == 0 && K >= 64 && K % 64 == 0;
+}
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// the epilogue of this mode and N writes one row-statistics slot per 128 output channels (128-wide tiles, at most SS_PARTS slots)
+bool rowss_fits(int N, const GemmEpi& epi) {
+  if (N % 128 != 0) return false;
+  if (epi.mode == EPI_RESID || epi.mode == EPI_STORE) return N <= 128 * SS_PARTS;   // (STORE: the TokenMerge projection)
+  if (epi.mode == EPI_SPLIT_LERP) return epi.C % 128 == 0 && epi.C <= 128 * SS_PARTS;
+  return false;
+}
+
+// Everything gemm_wg_kernel needs of the problem and its epilogue.
+bool gemm_fits(int64_t M, int N, int K, const GemmEpi& epi) {
+  if (!shape_ok(M, N, K)) return false;
+  if (epi.ss_in != nullptr) {   // fused RMSNorm consumer: 1/rms from the K / 128 slots of each row
+    if (K % 128 != 0 || K > 128 * SS_PARTS || epi.mC > 0 || epi.mode == EPI_RESID || epi.mode == EPI_SPLIT_LERP) return false;
+    if ((epi.mode == EPI_STORE || epi.mode == EPI_QKV_ROPE) && N % 128 != 0) return false;
+  }
+  if (epi.ss_out != nullptr && !rowss_fits(N, epi)) return false;
+  if (epi.mC > 0) {   // TokenMerge gather folded into the A loads: 128-wide tiles, plain store epilogue
+    int bw, bh;
+    if (epi.mode != EPI_STORE || N % 128 != 0 || epi.mC % 64 != 0 || K != 4 * epi.mC || M % epi.mwc != 0 || !quad_box(epi.mwc, &bw, &bh)) return false;
+  }
+  switch (epi.mode) {
+    case EPI_STORE:
+    case EPI_RESID:
+      return true;
+    case EPI_GEGLU:   // 128-wide tiles only
+      return N % 128 == 0;
+    case EPI_SPLIT_LERP:
+      return epi.C % 32 == 0 && N == 4 * epi.C;
+    case EPI_QKV_ROPE:
+      return N == 3 * epi.C && epi.C % 64 == 0 && epi.nh * 64 == epi.C && epi.rope != nullptr;
+    case EPI_PATCH_OUT:   // 48 of 64 columns used; float4 stores of img and loads of x_in
+      return N == 64 && epi.W % 4 == 0 && aligned16(epi.img) && (epi.sigma_data <= 0.f || aligned16(epi.x_in));
+    default:
+      return false;
+  }
 }
 
 }  // namespace
@@ -714,103 +739,48 @@ static bool g_tc_disabled = [] {
   return e != nullptr && e[0] == '1';
 }();
 
-bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi) {
-  if (g_tc_disabled || !shape_ok(M, N, K)) return false;
-  if (epi.ss_in != nullptr && (N % 128 != 0 || K % 128 != 0 || K > 128 * SS_PARTS || (epi.mode != EPI_STORE && epi.mode != EPI_QKV_ROPE) || epi.mC > 0))
-    return false;
-  if (epi.mC > 0) {   // TokenMerge gather folded into the A loads: 128-wide tiles, plain store epilogue
-    int bw, bh;
-    if (epi.mode != EPI_STORE || N % 128 != 0 || epi.mC % 64 != 0 || K != 4 * epi.mC || M % epi.mwc != 0 || !quad_box(epi.mwc, &bw, &bh)) return false;
-  }
-  if (epi.mode == EPI_SPLIT_LERP) return epi.C % 32 == 0 && N == 4 * epi.C;
-  if (epi.mode == EPI_QKV_ROPE) return N == 3 * epi.C && epi.C % 64 == 0 && epi.nh * 64 == epi.C && epi.rope != nullptr;
-  return epi.mode == EPI_STORE || epi.mode == EPI_RESID;
-}
+// KDB200_DISABLE_TC steers the engine's routes away from the tensor-core kernels; an explicit launch_gemm_tc (kdb_gemm_bf16) still runs
+bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi) { return !g_tc_disabled && gemm_fits(M, N, K, epi); }
 
 // true when the RESID / SPLIT / STORE GEMM of this shape runs on 128-wide tiles, which leave sum(x^2) of every row they write
-bool tc_gemm_emits_rowss(int64_t M, int N, int K, const GemmEpi& epi) {
-  if (!tc_gemm_supported(M, N, K, epi)) return false;
-  if (N % 128 != 0) return false;
-  if (epi.mode == EPI_RESID || epi.mode == EPI_STORE) return N <= 128 * SS_PARTS;   // (STORE: the TokenMerge projection)
-  if (epi.mode == EPI_SPLIT_LERP) return epi.C % 128 == 0 && epi.C <= 128 * SS_PARTS;
-  return false;
-}
+bool tc_gemm_emits_rowss(int64_t M, int N, int K, const GemmEpi& epi) { return tc_gemm_supported(M, N, K, epi) && rowss_fits(N, epi); }
 
 int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st) {
-  KDB_REQUIRE(shape_ok(M, N, K), KDB_ERR_BAD_SHAPE, "gemm_tc: unsupported shape M=%lld N=%d K=%d", (long long)M, N, K);
-  KDB_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0,
-              KDB_ERR_BAD_ARG, "gemm_tc: operands must be 16-byte aligned");
-  TcParams p{};
+  KDB_REQUIRE(aligned16(A) && aligned16(W) && aligned16(C), KDB_ERR_BAD_ARG, "gemm_tc: operands must be 16-byte aligned");
+  KDB_REQUIRE(gemm_fits(M, N, K, epi), KDB_ERR_UNSUPPORTED, "gemm_tc: epilogue %d does not support M=%lld N=%d K=%d with these options", epi.mode,
+              (long long)M, N, K);
+  GemmArgs p{};
+  static_cast<GemmEpi&>(p) = epi;
   p.out = C;
   p.M = M;
   p.N = N;
   p.K = K;
-  p.ss_in = epi.ss_in;
-  p.ss_out = epi.ss_out;
-  KDB_REQUIRE(epi.ss_in == nullptr || tc_gemm_supported(M, N, K, epi), KDB_ERR_UNSUPPORTED, "gemm_tc: fused-norm geometry not supported");
-  KDB_REQUIRE(epi.ss_out == nullptr || tc_gemm_emits_rowss(M, N, K, epi), KDB_ERR_UNSUPPORTED, "gemm_tc: this shape cannot emit row statistics");
+  p.th = epi.H / 4;
+  p.tw = epi.W / 4;
   if (epi.mC > 0) {
-    KDB_REQUIRE(tc_gemm_supported(M, N, K, epi), KDB_ERR_UNSUPPORTED, "gemm_tc: token-merge geometry not supported");
-    p.a_merge = 1;
-    p.mC = epi.mC;
-    p.mwc = epi.mwc;
     quad_box(epi.mwc, &p.box_w, &p.box_h);
-    return launch_tc<128, TCE_STORE>(A, W, p, st);
+    return launch_tc<128, EPI_STORE>(A, W, p, st);
   }
   switch (epi.mode) {
     case EPI_STORE:
-      return dispatch_bn<TCE_STORE>(A, W, p, st);
+      return dispatch_bn<EPI_STORE>(A, W, p, st);
     case EPI_RESID:
-      p.resid = static_cast<const bf16*>(epi.resid);
-      return dispatch_bn<TCE_RESID>(A, W, p, st);
+      return dispatch_bn<EPI_RESID>(A, W, p, st);
+    case EPI_GEGLU:
+      return launch_tc<128, EPI_GEGLU>(A, W, p, st);
     case EPI_SPLIT_LERP:
-      p.resid = static_cast<const bf16*>(epi.resid);
-      p.fac = epi.fac;
-      p.hc = epi.hc;
-      p.wc = epi.wc;
-      p.Cf = epi.C;
-      return dispatch_bn<TCE_SPLIT>(A, W, p, st);
+      return dispatch_bn<EPI_SPLIT_LERP>(A, W, p, st);
     case EPI_QKV_ROPE:
-      p.rope = epi.rope;
-      p.qk_scale = epi.qk_scale;
-      p.C = epi.C;
-      p.nh = epi.nh;
-      p.T = epi.T_tokens;
-      return dispatch_bn<TCE_QKV>(A, W, p, st);
+      return dispatch_bn<EPI_QKV_ROPE>(A, W, p, st);
+    case EPI_PATCH_OUT:
+      return launch_tc<64, EPI_PATCH_OUT>(A, W, p, st);
     default:
-      KDB_REQUIRE(false, KDB_ERR_BAD_ARG, "gemm_tc: bad epilogue");
+      return KDB_ERR_BAD_ARG;   // (not reached: gemm_fits accepts no other mode)
   }
 }
 
-// patch_out on the tensor core: tokens already normalised (xn bf16 [M, C0]), W zero-padded to [64, C0]
-bool tc_patch_out_supported(int C0, int Cout, int ph, int pw, int Wimg) {
-  return !g_tc_disabled && C0 % 64 == 0 && Cout == 3 && ph == 4 && pw == 4 && Wimg % 4 == 0;
-}
-
-int launch_patch_out_tc(const bf16* xn, const bf16* W_pad, const float* x_in, const float* sigma, float sigma_data, float* out, int B, int H,
-                        int Wimg, int C0, cudaStream_t st, const float* ss_in) {
-  KDB_REQUIRE(ss_in == nullptr || (C0 % 128 == 0 && C0 <= 128 * SS_PARTS), KDB_ERR_UNSUPPORTED, "patch_out_tc: fused norm needs C0 %% 128 == 0");
-  KDB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (sigma_data <= 0.f || (reinterpret_cast<uintptr_t>(x_in) & 15) == 0), KDB_ERR_BAD_ARG,
-              "patch_out_tc: x and out must be 16-byte aligned (float4 epilogue)");
-  TcParams p{};
-  p.ss_in = ss_in;
-  p.M = (int64_t)B * (H / 4) * (Wimg / 4);
-  p.N = 64;
-  p.K = C0;
-  p.fout = out;
-  p.x_in = x_in;
-  p.sigma = sigma;
-  p.sd = sigma_data;
-  p.H = H;
-  p.Wimg = Wimg;
-  p.th = H / 4;
-  p.tw = Wimg / 4;
-  KDB_REQUIRE(shape_ok(p.M, 64, C0), KDB_ERR_BAD_SHAPE, "patch_out_tc: unsupported shape");
-  return launch_tc<64, TCE_PATCHOUT>(xn, W_pad, p, st);
-}
-
-bool tc_patch_in_supported(int Cin, int ph, int pw, int C0, int Wimg) {
-  return !g_tc_disabled && Cin == 3 && ph == 4 && pw == 4 && C0 % 128 == 0 && C0 <= 128 * SS_PARTS && Wimg % 4 == 0;
+bool tc_patch_in_supported(const float* x, int C0, int Wimg) {
+  return !g_tc_disabled && C0 % 128 == 0 && C0 <= 128 * SS_PARTS && Wimg % 4 == 0 && aligned16(x);
 }
 
 int prepare_patch_in_weight(const float* W, bf16* out, int C0, cudaStream_t st) {
@@ -832,7 +802,8 @@ int launch_patch_in_tc(const float* x, const float* sigma, float sigma_data, con
   p.M = (int64_t)B * p.th * p.tw;
   p.N = C0;
   p.ss_out = ss_out;
-  KDB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, KDB_ERR_BAD_ARG, "patch_in_tc: input must be 16-byte aligned");
+  KDB_REQUIRE(tc_patch_in_supported(x, C0, Wimg), KDB_ERR_UNSUPPORTED,
+              "patch_in_tc: needs C0 %% 128 == 0, C0 <= %d, W %% 4 == 0 and a 16-byte aligned input (got C0=%d W=%d)", 128 * SS_PARTS, C0, Wimg);
   CUtensorMap tw, tcm;
   int rc;
   if ((rc = tmap_2d(&tw, W_perm, 64, (uint64_t)C0, 64, 128))) return rc;
@@ -842,11 +813,6 @@ int launch_patch_in_tc(const float* x, const float* sigma, float sigma_data, con
   patch_in_tc_kernel<<<dim3((unsigned)ceil_div(p.M, BM), (unsigned)(C0 / 128)), PATCH_IN_THREADS, PATCH_IN_SMEM, st>>>(tw, tcm, p);
   KDB_LAUNCH_CHECK(F_PATCH_IN, st);
   return 0;
-}
-
-bool tc_gemm_geglu_supported(int64_t M, int N2, int K, bool fused_norm) {
-  if (fused_norm && (K % 128 != 0 || K > 128 * SS_PARTS)) return false;
-  return !g_tc_disabled && shape_ok(M, N2, K) && N2 % 128 == 0;
 }
 
 __global__ void __launch_bounds__(256) fold_norm_weights_kernel(const FoldDesc* __restrict__ descs, const float* __restrict__ cond) {
@@ -873,17 +839,6 @@ int launch_fold_norm_weights(const FoldDesc* descs_dev, int n_desc, const float*
   fold_norm_weights_kernel<<<dim3(48, (unsigned)n_desc), 256, 0, st>>>(descs_dev, cond_row);
   KDB_LAUNCH_CHECK(F_FUSED_NORM, st);
   return 0;
-}
-
-int launch_gemm_tc_geglu(const bf16* A, const bf16* W_il, bf16* out, int64_t M, int N2, int K, cudaStream_t st, const float* ss_in) {
-  KDB_REQUIRE(tc_gemm_geglu_supported(M, N2, K, ss_in != nullptr), KDB_ERR_BAD_SHAPE, "gemm_tc_geglu: unsupported shape");
-  TcParams p{};
-  p.ss_in = ss_in;
-  p.out = out;
-  p.M = M;
-  p.N = N2;
-  p.K = K;
-  return launch_tc<128, TCE_GEGLU>(A, W_il, p, st);
 }
 
 bool tc_ffn_fused_supported(int64_t M, int C, int dff) {
@@ -924,9 +879,12 @@ extern "C" int kdb_gemm_bf16(const void* a, const void* w, void* c, int M, int N
 extern "C" int kdb_gemm_bf16_geglu(const void* a, const void* w_il, void* c, int M, int N2, int K, const float* ss_in, void* stream) {
   using namespace kdb;
   KDB_REQUIRE(a && w_il && c, KDB_ERR_BAD_ARG, "gemm_bf16_geglu: NULL operand");
-  KDB_REQUIRE(tc_gemm_geglu_supported(M, N2, K, ss_in != nullptr), KDB_ERR_UNSUPPORTED,
+  GemmEpi e;
+  e.mode = EPI_GEGLU;
+  e.ss_in = ss_in;
+  KDB_REQUIRE(tc_gemm_supported(M, N2, K, e), KDB_ERR_UNSUPPORTED,
               "gemm_bf16_geglu: needs N2 %% 128 == 0 and K %% 64 == 0 (K %% 128 == 0, K <= 1024 with ss_in); got M=%d N2=%d K=%d", M, N2, K);
-  return launch_gemm_tc_geglu(static_cast<const bf16*>(a), static_cast<const bf16*>(w_il), static_cast<bf16*>(c), M, N2, K, (cudaStream_t)stream, ss_in);
+  return launch_gemm_tc(static_cast<const bf16*>(a), static_cast<const bf16*>(w_il), static_cast<bf16*>(c), M, N2, K, e, (cudaStream_t)stream);
 }
 
 extern "C" int kdb_ffn_fused_bf16(void* x, const void* w_up_il, const void* w_down, int M, int d_ff, const float* ss_in, float* ss_out, void* stream) {

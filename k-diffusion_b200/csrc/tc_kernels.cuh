@@ -4,17 +4,16 @@
 
 namespace kdb {
 
-// C[M,N] = A[M,K] W[N,K]^T (+ epilogue), bf16 operands staged by TMA, fp32 accumulators in registers (wgmma).
+// C[M,N] = A[M,K] W[N,K]^T (+ the epilogue epi.mode), bf16 operands staged by TMA, fp32 accumulators in registers (wgmma).
+// tc_gemm_supported: the kernel runs this problem with this epilogue (false under KDB200_DISABLE_TC).  launch_gemm_tc refuses what the
+// kernel cannot run.  EPI_GEGLU: W rows interleaved 8 value / 8 gate, C [M, N/2].  EPI_PATCH_OUT: W = patch_out's weight zero-padded to
+// [64, K], C unused (the epilogue writes epi.img).
 bool tc_gemm_supported(int64_t M, int N, int K, const GemmEpi& epi);
 // Fused RMSNorm: a RESID / SPLIT_LERP GEMM with N % 128 == 0 can leave sum(x^2) of every row it writes ([rows, SS_PARTS] fp32, one slot per 128
-// channels) and a STORE / QKV_ROPE / GEGLU GEMM whose A operand is that x can apply 1/rms in its epilogue (GemmEpi::ss_out / ss_in).
+// channels) and a STORE / QKV_ROPE / GEGLU / PATCH_OUT GEMM whose A operand is that x can apply 1/rms in its epilogue (GemmEpi::ss_out / ss_in).
 constexpr int SS_PARTS = 8;
 bool tc_gemm_emits_rowss(int64_t M, int N, int K, const GemmEpi& epi);
 int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st);
-
-// up_proj with the GEGLU fused into the epilogue; W rows interleaved 8 value / 8 gate (engine.cu).
-bool tc_gemm_geglu_supported(int64_t M, int N2, int K, bool fused_norm = false);
-int launch_gemm_tc_geglu(const bf16* A, const bf16* W_il, bf16* out, int64_t M, int N2, int K, cudaStream_t st, const float* ss_in = nullptr);
 
 // The whole feed-forward block of a 128-wide level in one kernel (tc_ffn_fused.cuh): x <- x + down(value(x_n) * gelu(gate(x_n))), in place.
 // w_up_il carries the AdaRMSNorm channel scale (fold kernel) and the value / gate row interleave; ss_in = row statistics of x (required),
@@ -37,14 +36,8 @@ struct FoldDesc {
 };
 int launch_fold_norm_weights(const FoldDesc* descs_dev, int n_desc, const float* cond_row, cudaStream_t st);
 
-// patch_out (4x4 patches, 3 channels): xn bf16 [M, C0] x W_pad bf16 [64, C0] -> fp32 NCHW with the Karras combine fused.
-// ss_in != nullptr: xn is the RAW residual stream, W_pad carries out_norm.scale and the epilogue applies 1/rms per token.
-bool tc_patch_out_supported(int C0, int Cout, int ph, int pw, int Wimg);
-int launch_patch_out_tc(const bf16* xn, const bf16* W_pad, const float* x_in, const float* sigma, float sigma_data, float* out, int B, int H,
-                        int Wimg, int C0, cudaStream_t st, const float* ss_in = nullptr);
-
-// patch_in (4x4 patches of a 3-channel fp32 latent) on the tensor core; W_perm = prepare_patch_in_weight(patch_in.proj.weight)
-bool tc_patch_in_supported(int Cin, int ph, int pw, int C0, int Wimg);
+// patch_in (4x4 patches of a 3-channel fp32 latent x) on the tensor core; W_perm = prepare_patch_in_weight(patch_in.proj.weight)
+bool tc_patch_in_supported(const float* x, int C0, int Wimg);
 int prepare_patch_in_weight(const float* W, bf16* out_perm, int C0, cudaStream_t st);
 int launch_patch_in_tc(const float* x, const float* sigma, float sigma_data, const bf16* W_perm, bf16* out, int B, int H, int Wimg, int C0,
                        float* ss_out, cudaStream_t st);

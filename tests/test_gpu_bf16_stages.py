@@ -315,7 +315,7 @@ def ref_split(P, l, x, skip, nm=None, emu=False):
     if nm == "fac_swap":
         fac = 1.0 - fac
     skip = skip.to(dt)
-    if emu:           # the TCE_SPLIT epilogue's two-branch lerp
+    if emu:           # the EPI_SPLIT_LERP epilogue's two-branch lerp
         d = up - skip
         return bf(skip + fac * d if fac < 0.5 else up - d * (1.0 - fac))
     return torch.lerp(skip, up, fac)
