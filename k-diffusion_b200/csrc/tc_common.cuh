@@ -102,6 +102,11 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
                "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
@@ -325,6 +330,23 @@ __device__ __forceinline__ void unpack_bf16x2(uint32_t v, float& lo, float& hi) 
   __nv_bfloat162 t = *reinterpret_cast<__nv_bfloat162*>(&v);
   lo = __low2float(t);
   hi = __high2float(t);
+}
+
+// GEGLU on a wgmma accumulator fragment of 64 rows x 128 columns whose W rows interleave 8 value / 8 gate rows: 8-column block 2q holds
+// 8 value features, block 2q + 1 their gates, so a value and its gate sit in the same thread.  h0 / h1: 0.5 x the value scale of the
+// thread's rows r, r + 8 (the GELU's 0.5 rides on it); g0 / g1: their gate scale.  o[2q] / o[2q + 1]: hidden features 8q + cq, 8q + cq + 1
+// of row r / r + 8 as bf16x2 -- which is also the bf16 A fragment of k16 step q / 2 (wgmma_128_rs).
+__device__ __forceinline__ void geglu_fragment(const float (&acc)[64], f32x2 h0, f32x2 h1, f32x2 g0, f32x2 g1, uint32_t (&o)[16]) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const f32x2 v0 = mul2(pk2(acc[8 * q], acc[8 * q + 1]), h0), v1 = mul2(pk2(acc[8 * q + 2], acc[8 * q + 3]), h1);
+    const f32x2 q0 = mul2(pk2(acc[8 * q + 4], acc[8 * q + 5]), g0), q1 = mul2(pk2(acc[8 * q + 6], acc[8 * q + 7]), g1);
+    float o0, o1, o2, o3;
+    upk2(geglu2(v0, q0), o0, o1);
+    upk2(geglu2(v1, q1), o2, o3);
+    o[2 * q] = pack_bf16x2(o0, o1);
+    o[2 * q + 1] = pack_bf16x2(o2, o3);
+  }
 }
 
 // ---------------------------------------------------------------- shifted windows of 8x8 tokens (reference image_transformer_v2.py:253-337)

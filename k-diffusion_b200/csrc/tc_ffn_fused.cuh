@@ -137,18 +137,8 @@ __global__ void __launch_bounds__(FF_THREADS, 1) ffn_fused_kernel(const __grid_c
           if (lane == 0) bars->wd.release(ds);
           ds.advance();
         }
-        // ---- GEGLU(c - 1): 8-column block 2q = 8 value features, block 2q + 1 = their gates -> hidden block q (rows r0, r0 + 8)
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const tc::f32x2 v0 = tc::mul2(tc::pk2(acc1[8 * q], acc1[8 * q + 1]), h0), v1 = tc::mul2(tc::pk2(acc1[8 * q + 2], acc1[8 * q + 3]), h1);
-          const tc::f32x2 q0 = tc::mul2(tc::pk2(acc1[8 * q + 4], acc1[8 * q + 5]), g0), q1 = tc::mul2(tc::pk2(acc1[8 * q + 6], acc1[8 * q + 7]), g1);
-          float o0, o1, o2, o3;
-          tc::upk2(tc::geglu2(v0, q0), o0, o1);
-          tc::upk2(tc::geglu2(v1, q1), o2, o3);
-          // A fragment of k16 step q / 2: {block 2kk row r0, block 2kk row r0 + 8, block 2kk + 1 row r0, block 2kk + 1 row r0 + 8}
-          hreg[(q >> 1) * 4 + (q & 1) * 2 + 0] = tc::pack_bf16x2(o0, o1);
-          hreg[(q >> 1) * 4 + (q & 1) * 2 + 1] = tc::pack_bf16x2(o2, o3);
-        }
+        // ---- GEGLU(c - 1) -> hidden block q of rows r0, r0 + 8 = the A fragment of M2's k16 steps
+        tc::geglu_fragment(acc1, h0, h1, g0, g1, hreg);
       }
 #pragma unroll
       for (int j = 0; j < 64; ++j) acc1[j] = 0.f;

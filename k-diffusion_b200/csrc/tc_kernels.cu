@@ -1,6 +1,6 @@
 // tc_kernels.cu -- bf16 tensor-core GEMM for sm_90a: TMA (SWIZZLE_128B tiles) -> shared memory -> wgmma (fp32 accumulators in
-// registers) -> fp32 shared-memory tile -> fused epilogue (thread = output row) -> swizzled shared tile -> TMA store (clipped at the
-// M edge by the tensor map).
+// registers) -> fp32 shared-memory tile -> fused epilogue (thread = output row; GEGLU: on the accumulator fragments) -> swizzled
+// shared tile -> TMA store (clipped at the M edge by the tensor map).
 //
 // C[M,N] = A[M,K] W[N,K]^T for every nn.Linear on the token stream (reference image_transformer_v2.py:126-139).
 // Epilogues (GemmEpilogue): EPI_STORE; EPI_RESID, +residual (out_proj / down_proj, :396,:493; residual tile prefetched by TMA
@@ -75,14 +75,14 @@ constexpr int BM = 128, BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KiB
 constexpr int SUB_TILE_BYTES = BM * 128;     // one [128 x 64] bf16 output sub-tile
 constexpr int GEMM_THREADS = 384;            // warpgroups 0, 1: MMA + epilogue of alternate tiles, warpgroup 2: TMA producer (one warp)
-constexpr int GEMM_RING_BYTES = 96 * 1024;   // TMA ring: 3 stages of a 128-wide tile, 4 of a 64-wide one
 
 // The kernel's parameter block: the epilogue descriptor, the output and the shape, and what launch_gemm_tc derives from them.
 struct GemmArgs : GemmEpi {
   bf16* out;
   int64_t M;
   int N, K;
-  int box_w, box_h;      // 5-D TMA box of the merge gather (mC > 0): 128 rows = box_h x box_w coarse tokens
+  int box_w, box_h;      // 5-D TMA box of the merge gather (mC > 0) or of the split scatter (EPI_SPLIT_LERP, box_w > 0): 128 rows =
+                         // box_h x box_w coarse tokens
   int th, tw;            // EPI_PATCH_OUT: token grid H / 4 x W / 4
 };
 
@@ -119,13 +119,26 @@ bool quad_box(int wc, int* box_w, int* box_h) {
   return true;
 }
 
+// TMA coordinates in tmap_quad's view of the [128 x 64] box that holds coarse rows m0.. (m0 % 128 == 0) and columns n.. of quadrant
+// n / C: the same box for the merge's A loads (n = k, C = mC) and for the split's skip loads and output stores
+struct QuadCoord {
+  int e, nw, wx, nh, row;
+};
+__device__ __forceinline__ QuadCoord quad_coord(int64_t m0, int n, int C, int wc, int box_h) {
+  const int qd = n / C;
+  return QuadCoord{n - qd * C, qd & 1, box_h == 1 ? (int)(m0 % wc) : 0, qd >> 1, (int)(m0 / wc)};
+}
+
 // Shared memory of one GEMM CTA: the TMA ring, the fp32 accumulator tile (shared by the two warpgroups, in tile order), per
 // warpgroup the bf16 output staging tile (RESID: the residual tile is loaded into it and the epilogue adds in place), then the
-// barriers.  128-wide RESID / STORE / QKV: 96 + 64 + 2 x 32 KiB + 1 KiB of alignment = 225 KiB.
+// barriers.  128-wide RESID / STORE / QKV / SPLIT: 96 + 64 + 2 x 32 KiB + 1 KiB of alignment = 225 KiB.  GEGLU runs its epilogue on the
+// accumulator fragments and has no fp32 tile: its ring takes those 64 KiB, 6 stages of 32 KiB + 2 x 16 KiB + 1 KiB = 225 KiB.
 template <int BN, int EPI> constexpr int out_bytes() {
-  return EPI == EPI_GEGLU ? SUB_TILE_BYTES : (EPI == EPI_SPLIT_LERP || EPI == EPI_PATCH_OUT) ? 0 : (BN / 64) * SUB_TILE_BYTES;
+  return EPI == EPI_GEGLU ? SUB_TILE_BYTES : EPI == EPI_PATCH_OUT ? 0 : (BN / 64) * SUB_TILE_BYTES;
 }
-template <int BN, int EPI> constexpr size_t gemm_smem() { return 1024 + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>() + 128; }
+template <int BN, int EPI> constexpr int acc_bytes() { return EPI == EPI_GEGLU ? 0 : BM * BN * 4; }
+template <int EPI> constexpr int ring_bytes() { return EPI == EPI_GEGLU ? 192 * 1024 : 96 * 1024; }   // 96 KiB: 3 stages of 128-wide tiles, 4 of 64-wide
+template <int BN, int EPI> constexpr size_t gemm_smem() { return 1024 + ring_bytes<EPI>() + acc_bytes<BN, EPI>() + 2 * out_bytes<BN, EPI>() + 128; }
 
 // The fp32 accumulator tile is [128 rows x BN columns] with the 16-byte chunks of row r XOR-swizzled by r % 8: the fragment stores
 // (8 rows x 4 column pairs per warp) and the row reads (32 rows, one float4 each) both spread evenly over the banks.
@@ -161,7 +174,9 @@ __device__ __forceinline__ void stage_ld32(const float* s, int row, int col0, fl
 // releases the previous stage, and hands the MMA issue to the other warpgroup once its last k-block is issued (BAR_TURN: the two
 // main loops never interleave, which also keeps each ring stage at most one phase ahead of its waiter).  Its epilogue then
 // writes the accumulators to the fp32 tile in shared memory so that each thread owns one output row (fp32 arithmetic, one rounding
-// to bf16 at the pack, one TMA store per 64 columns), and hands the fp32 tile on once its rows are read (BAR_ACC).
+// to bf16 at the pack, one TMA store per 64 columns), and hands the fp32 tile on once its rows are read (BAR_ACC).  GEGLU works
+// element by element on value / gate pairs that share a thread: it runs on the accumulator fragments themselves and writes bf16
+// pairs straight into its staging tile, without the fp32 tile or BAR_ACC.
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
                                                                   const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
@@ -169,12 +184,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
   KDB_PDL_TRIGGER();
   constexpr int B_STAGE_BYTES = BN * BK * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr int STAGES = GEMM_RING_BYTES / STAGE_BYTES;
+  constexpr int RING_BYTES = ring_bytes<EPI>();
+  constexpr int STAGES = RING_BYTES / STAGE_BYTES;
   constexpr int NSUB = BN / 64;
   constexpr bool RES = EPI == EPI_RESID;
   uint8_t* base = tc::smem_1k();
-  float* sAcc = reinterpret_cast<float*>(base + GEMM_RING_BYTES);
-  auto* ring = reinterpret_cast<tc::TmaRing<STAGES>*>(base + GEMM_RING_BYTES + BM * BN * 4 + 2 * out_bytes<BN, EPI>());
+  float* sAcc = reinterpret_cast<float*>(base + RING_BYTES);
+  auto* ring = reinterpret_cast<tc::TmaRing<STAGES>*>(base + RING_BYTES + acc_bytes<BN, EPI>() + 2 * out_bytes<BN, EPI>());
   uint64_t* resid_full = reinterpret_cast<uint64_t*>(ring + 1);   // one per warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -206,8 +222,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           uint64_t* bar = ring->acquire(ps, STAGE_BYTES);
           uint8_t* a = base + (size_t)ps.slot * STAGE_BYTES;
           if (p.mC > 0) {    // TokenMerge: k-block kb lives in quadrant (nh, nw) of the fine grid, channels e0..e0+63
-            const int qd = (kb * BK) / p.mC, e0 = kb * BK - qd * p.mC;
-            tc::tma_load_5d(a, &tma, bar, e0, qd & 1, p.box_h == 1 ? (int)(m0 % p.mwc) : 0, qd >> 1, (int)(m0 / p.mwc));
+            const QuadCoord q = quad_coord(m0, kb * BK, p.mC, p.mwc, p.box_h);
+            tc::tma_load_5d(a, &tma, bar, q.e, q.nw, q.wx, q.nh, q.row);
           } else {
             tc::tma_load_2d(a, &tma, bar, kb * BK, (int)m0);
           }
@@ -221,16 +237,37 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
 
   const int wg = warp >> 2;
   const int row = threadIdx.x & 127;
-  uint8_t* sC = base + GEMM_RING_BYTES + BM * BN * 4 + wg * out_bytes<BN, EPI>();
+  uint8_t* sC = base + RING_BYTES + acc_bytes<BN, EPI>() + wg * out_bytes<BN, EPI>();
+  const int r0 = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);   // fragment rows r0, r0 + 8 (+ 64 in acc1), column pair cq
   for (int i = wg; i < n_local; i += 2) {
     const int t = (int)blockIdx.x + i * (int)gridDim.x;
     const int64_t m0 = (int64_t)(t / n_tiles) * BM;
     const int n0 = (t % n_tiles) * BN;
-    if constexpr (RES) {                 // the previous tile's store has finished reading sC (tma_store_wait_read below)
-      if (row == 0) {
+    // the residual / skip tile by TMA into sC; the previous tile's store has finished reading sC (tma_store_wait_read below)
+    if constexpr (RES || EPI == EPI_SPLIT_LERP) {
+      if (row == 0 && (RES || p.box_w > 0)) {
         tc::mbar_arrive_expect_tx(&resid_full[wg], NSUB * SUB_TILE_BYTES);
 #pragma unroll
-        for (int g = 0; g < NSUB; ++g) tc::tma_load_2d(sC + g * SUB_TILE_BYTES, &tmr, &resid_full[wg], n0 + g * 64, (int)m0);
+        for (int g = 0; g < NSUB; ++g) {
+          if constexpr (RES) {
+            tc::tma_load_2d(sC + g * SUB_TILE_BYTES, &tmr, &resid_full[wg], n0 + g * 64, (int)m0);
+          } else {
+            const QuadCoord q = quad_coord(m0, n0 + g * 64, p.C, p.wc, p.box_h);
+            tc::tma_load_5d(sC + g * SUB_TILE_BYTES, &tmr, &resid_full[wg], q.e, q.nw, q.wx, q.nh, q.row);
+          }
+        }
+      }
+    }
+    // GEGLU: 1/rms of the fragment rows r0, r0 + 8, 64 + r0, 72 + r0, loaded while the other warpgroup's main loop runs
+    float frag_rstd[4] = {1.f, 1.f, 1.f, 1.f};
+    if constexpr (EPI == EPI_GEGLU) {
+      if (p.ss_in != nullptr) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const int64_t m = m0 + r0 + 64 * (h >> 1) + 8 * (h & 1);
+          const float4* sp = reinterpret_cast<const float4*>(p.ss_in + (m < p.M ? m : 0) * SS_PARTS);
+          frag_rstd[h] = rsqrtf(tc::rowss_sum(__ldg(sp), __ldg(sp + 1), p.K >> 7) / (float)p.K + 1e-6f);
+        }
       }
     }
 
@@ -270,6 +307,32 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
     tc::wg_fence_acc(acc0);
     tc::wg_fence_acc(acc1);
     if (lane == 0) ring->release(PipeState<STAGES>::at(it0 + nkb - 1));
+
+    if constexpr (EPI == EPI_GEGLU) {
+      // ---------------- epilogue on the fragments: output column 8q + cq of row r = GEGLU of the pair in 8-column blocks 2q, 2q + 1
+      tc::named_barrier_sync(tc::BAR_WG + wg, 128);   // row 0 has seen the previous tile's store finish reading sC
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const float r_a = frag_rstd[2 * half], r_b = frag_rstd[2 * half + 1];
+        uint32_t o[16];
+        tc::geglu_fragment(half == 0 ? acc0 : acc1, tc::pk2(0.5f * r_a, 0.5f * r_a), tc::pk2(0.5f * r_b, 0.5f * r_b), tc::pk2(r_a, r_a),
+                           tc::pk2(r_b, r_b), o);
+        const int r = 64 * half + r0;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          *reinterpret_cast<uint32_t*>(sC + tc::sw128_offset(r, q) + 2 * cq) = o[2 * q];
+          *reinterpret_cast<uint32_t*>(sC + tc::sw128_offset(r + 8, q) + 2 * cq) = o[2 * q + 1];
+        }
+      }
+      tc::fence_proxy_async();
+      tc::named_barrier_sync(tc::BAR_WG + wg, 128);
+      if (row == 0) {
+        tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
+        tc::tma_store_commit();
+        tc::tma_store_wait_read();
+      }
+      continue;
+    }
     if (i > 0) tc::named_barrier_sync(tc::BAR_ACC + wg, 256);   // the other warpgroup has read tile i - 1 out of the fp32 tile
     stage_store<BN>(sAcc, 0, acc0);
     stage_store<BN>(sAcc, 64, acc1);
@@ -321,12 +384,70 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           }
       }
     } else if constexpr (EPI == EPI_SPLIT_LERP) {
-      // TokenSplit + torch.lerp(skip, x, fac) (reference :618-621): row m = (b, hy, wx) on the coarse grid; 32 columns inside one
-      // (nh, nw) quadrant (C % 32 == 0), scattered to the fine token
+      // TokenSplit + torch.lerp(skip, x, fac) (reference :618-621): row m = (b, hy, wx) on the coarse grid, column n = (quadrant
+      // (nh, nw), channel e), scattered to the fine token.  The lerp takes one of two forms by fac; sum(x^2) runs in column order.
       const bool live = m < p.M;
       const float facv = __ldg(p.fac);
       float ss = 0.f;
       int64_t fine = 0;
+      if (p.box_w > 0) {
+        // 64 columns of one quadrant x 128 coarse rows are one box of the quadrant maps: the skip tile arrived by TMA under the main
+        // loop, the lerp runs in place (each thread its own row), and the tile leaves by TMA store through the same box of `out`
+        tc::mbar_wait_nocall(&resid_full[wg], (uint32_t)(i >> 1) & 1u);
+#pragma unroll 1
+        for (int g = 0; g < NSUB; ++g) {
+          float v[64];
+          {
+            float t0[32], t1[32];
+            stage_ld32<BN>(sAcc, row, g * 64, t0);
+            stage_ld32<BN>(sAcc, row, g * 64 + 32, t1);
+#pragma unroll
+            for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
+          }
+          if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
+          uint8_t* cg = sC + g * SUB_TILE_BYTES;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            uint4* cp = reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j));
+            const uint4 r4 = *cp;
+            const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
+            uint32_t ow[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float lo = __uint_as_float(rw[q] << 16), hi = __uint_as_float(rw[q] & 0xffff0000u);
+              const float e0 = v[j * 8 + q * 2], e1 = v[j * 8 + q * 2 + 1];
+              const float d0 = e0 - lo, d1 = e1 - hi;
+              const float o0 = (facv < 0.5f) ? fmaf(facv, d0, lo) : e0 - d0 * (1.f - facv);
+              const float o1 = (facv < 0.5f) ? fmaf(facv, d1, hi) : e1 - d1 * (1.f - facv);
+              ss = fmaf(o0, o0, fmaf(o1, o1, ss));
+              ow[q] = tc::pack_bf16x2(o0, o1);
+            }
+            *cp = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+          }
+        }
+        if (p.ss_out != nullptr && live) {
+          const int64_t b = m / ((int64_t)p.hc * p.wc);
+          const int r = (int)(m - b * p.hc * p.wc);
+          const int hy = r / p.wc, wx = r - hy * p.wc, qd = n0 / p.C;
+          fine = (b * (2 * p.hc) + (2 * hy + (qd >> 1))) * (2 * p.wc) + (2 * wx + (qd & 1));
+          p.ss_out[fine * SS_PARTS + ((n0 % p.C) >> 7)] = ss;
+        }
+        tc::fence_proxy_async();
+        tc::named_barrier_sync(tc::BAR_WG + wg, 128);
+        if (row == 0) {
+#pragma unroll
+          for (int g = 0; g < NSUB; ++g) {
+            const QuadCoord q = quad_coord(m0, n0 + g * 64, p.C, p.wc, p.box_h);
+            tc::tma_store_5d(&tmc, sC + g * SUB_TILE_BYTES, q.e, q.nw, q.wx, q.nh, q.row);
+          }
+          tc::tma_store_commit();
+          tc::tma_store_wait_read();
+        }
+        continue;
+      }
+      // Coarse grids whose 128-row blocks are no box of the quadrant map (quad_box fails: wc >= 128 and not a multiple of 128, or
+      // wc < 128 and not a divisor of it) and C % 64 != 0: 32 columns inside one quadrant (C % 32 == 0) per step, per-thread global
+      // loads of the skip and stores of the output
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         float v[32];
@@ -376,7 +497,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
         }
         if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
-        if (EPI != EPI_GEGLU && p.ss_in != nullptr) {
+        if (p.ss_in != nullptr) {
           // fused RMSNorm row scale.  q and k are cosine-normalised afterwards (scale invariant): only v needs it.
           bool apply = true;
           if constexpr (EPI == EPI_QKV_ROPE) apply = (n0 + g * 64) >= 2 * p.C;
@@ -385,90 +506,70 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
             for (int k = 0; k < 64; ++k) v[k] *= rstd;
           }
         }
-        if constexpr (EPI == EPI_GEGLU) {
-          // columns come as [8 value | 8 gate] groups (interleaved up_proj rows) -> 32 outputs = chunks 4g..4g+3 of the output sub-tile
-          const tc::f32x2 r2 = tc::pk2(rstd, rstd), rh = tc::pk2(0.5f * rstd, 0.5f * rstd);     // the GELU's 0.5 rides on the value's row scale
+        uint8_t* cg = sC + g * SUB_TILE_BYTES;
+        if constexpr (RES) {
 #pragma unroll
-          for (int gg = 0; gg < 4; ++gg) {
-            uint32_t o[4];
+          for (int j = 0; j < 8; ++j) {      // this thread reads and then overwrites only its own row
+            const uint4 r4 = *reinterpret_cast<const uint4*>(cg + tc::sw128_offset(row, j));
+            const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              tc::f32x2 val = tc::pk2(v[gg * 16 + 2 * j], v[gg * 16 + 2 * j + 1]);
-              tc::f32x2 gate = tc::pk2(v[gg * 16 + 8 + 2 * j], v[gg * 16 + 8 + 2 * j + 1]);
-              val = tc::mul2(val, rh);
-              if (p.ss_in != nullptr) gate = tc::mul2(gate, r2);
-              float o0, o1;
-              tc::upk2(tc::geglu2(val, gate), o0, o1);
-              o[j] = tc::pack_bf16x2(o0, o1);
-            }
-            *reinterpret_cast<uint4*>(sC + tc::sw128_offset(row, g * 4 + gg)) = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-        } else {
-          uint8_t* cg = sC + g * SUB_TILE_BYTES;
-          if constexpr (RES) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {      // this thread reads and then overwrites only its own row
-              const uint4 r4 = *reinterpret_cast<const uint4*>(cg + tc::sw128_offset(row, j));
-              const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                v[j * 8 + q * 2] += __uint_as_float(rw[q] << 16);
-                v[j * 8 + q * 2 + 1] += __uint_as_float(rw[q] & 0xffff0000u);
-              }
+            for (int q = 0; q < 4; ++q) {
+              v[j * 8 + q * 2] += __uint_as_float(rw[q] << 16);
+              v[j * 8 + q * 2 + 1] += __uint_as_float(rw[q] & 0xffff0000u);
             }
           }
-          if constexpr (RES || EPI == EPI_STORE) {
-            if (p.ss_out != nullptr) {
-#pragma unroll
-              for (int k = 0; k < 64; k += 4) {
-                ss_acc[0] = fmaf(v[k], v[k], ss_acc[0]);
-                ss_acc[1] = fmaf(v[k + 1], v[k + 1], ss_acc[1]);
-                ss_acc[2] = fmaf(v[k + 2], v[k + 2], ss_acc[2]);
-                ss_acc[3] = fmaf(v[k + 3], v[k + 3], ss_acc[3]);
-              }
-            }
-          }
-          if constexpr (EPI == EPI_QKV_ROPE) {
-            const int n = n0 + g * 64;               // one head of q, k or v (feature order (t nh e), d_head 64)
-            const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
-            if (t3 < 2) {
-              // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248).  Columns (2i, 2i+1) pair with (16+2i, 17+2i); the
-              // table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4.
-              const int64_t tok = (m < p.M ? m : 0) % p.T_tokens;
-              const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T_tokens + tok;   // [head][i][token]
-              tc::f32x2 P[32];
-#pragma unroll
-              for (int k = 0; k < 32; ++k) P[k] = tc::pk2(v[2 * k], v[2 * k + 1]);
-              tc::f32x2 q0 = tc::mul2(P[0], P[0]), q1 = tc::mul2(P[1], P[1]), q2 = tc::mul2(P[2], P[2]), q3 = tc::mul2(P[3], P[3]);
-#pragma unroll
-              for (int k = 4; k < 32; k += 4) {
-                q0 = tc::fma2(P[k], P[k], q0);
-                q1 = tc::fma2(P[k + 1], P[k + 1], q1);
-                q2 = tc::fma2(P[k + 2], P[k + 2], q2);
-                q3 = tc::fma2(P[k + 3], P[k + 3], q3);
-              }
-              const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y)) + 1e-6f);
-              const tc::f32x2 sc2 = tc::pk2(sc, sc);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const float4 cs = __ldg(tb + (int64_t)k * p.T_tokens);
-                const tc::f32x2 C = tc::pk2(cs.x, cs.y), S = tc::pk2(cs.z, cs.w);
-                const tc::f32x2 X1 = P[k], X2 = P[8 + k];
-                P[k] = tc::mul2(tc::fma2(X2, tc::neg2(S), tc::mul2(X1, C)), sc2);
-                P[8 + k] = tc::mul2(tc::fma2(X1, S, tc::mul2(X2, C)), sc2);
-              }
-#pragma unroll
-              for (int k = 16; k < 32; ++k) P[k] = tc::mul2(P[k], sc2);
-#pragma unroll
-              for (int k = 0; k < 32; ++k) tc::upk2(P[k], v[2 * k], v[2 * k + 1]);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j)) =
-                make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
-                           tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
         }
+        if constexpr (RES || EPI == EPI_STORE) {
+          if (p.ss_out != nullptr) {
+#pragma unroll
+            for (int k = 0; k < 64; k += 4) {
+              ss_acc[0] = fmaf(v[k], v[k], ss_acc[0]);
+              ss_acc[1] = fmaf(v[k + 1], v[k + 1], ss_acc[1]);
+              ss_acc[2] = fmaf(v[k + 2], v[k + 2], ss_acc[2]);
+              ss_acc[3] = fmaf(v[k + 3], v[k + 3], ss_acc[3]);
+            }
+          }
+        }
+        if constexpr (EPI == EPI_QKV_ROPE) {
+          const int n = n0 + g * 64;               // one head of q, k or v (feature order (t nh e), d_head 64)
+          const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
+          if (t3 < 2) {
+            // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248).  Columns (2i, 2i+1) pair with (16+2i, 17+2i); the
+            // table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4.
+            const int64_t tok = (m < p.M ? m : 0) % p.T_tokens;
+            const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T_tokens + tok;   // [head][i][token]
+            tc::f32x2 P[32];
+#pragma unroll
+            for (int k = 0; k < 32; ++k) P[k] = tc::pk2(v[2 * k], v[2 * k + 1]);
+            tc::f32x2 q0 = tc::mul2(P[0], P[0]), q1 = tc::mul2(P[1], P[1]), q2 = tc::mul2(P[2], P[2]), q3 = tc::mul2(P[3], P[3]);
+#pragma unroll
+            for (int k = 4; k < 32; k += 4) {
+              q0 = tc::fma2(P[k], P[k], q0);
+              q1 = tc::fma2(P[k + 1], P[k + 1], q1);
+              q2 = tc::fma2(P[k + 2], P[k + 2], q2);
+              q3 = tc::fma2(P[k + 3], P[k + 3], q3);
+            }
+            const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y)) + 1e-6f);
+            const tc::f32x2 sc2 = tc::pk2(sc, sc);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              const float4 cs = __ldg(tb + (int64_t)k * p.T_tokens);
+              const tc::f32x2 C = tc::pk2(cs.x, cs.y), S = tc::pk2(cs.z, cs.w);
+              const tc::f32x2 X1 = P[k], X2 = P[8 + k];
+              P[k] = tc::mul2(tc::fma2(X2, tc::neg2(S), tc::mul2(X1, C)), sc2);
+              P[8 + k] = tc::mul2(tc::fma2(X1, S, tc::mul2(X2, C)), sc2);
+            }
+#pragma unroll
+            for (int k = 16; k < 32; ++k) P[k] = tc::mul2(P[k], sc2);
+#pragma unroll
+            for (int k = 0; k < 32; ++k) tc::upk2(P[k], v[2 * k], v[2 * k + 1]);
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint4*>(cg + tc::sw128_offset(row, j)) =
+              make_uint4(tc::pack_bf16x2(v[j * 8 + 0], v[j * 8 + 1]), tc::pack_bf16x2(v[j * 8 + 2], v[j * 8 + 3]),
+                         tc::pack_bf16x2(v[j * 8 + 4], v[j * 8 + 5]), tc::pack_bf16x2(v[j * 8 + 6], v[j * 8 + 7]));
       }
       if constexpr (RES || EPI == EPI_STORE) {
         if (p.ss_out != nullptr && m < p.M) p.ss_out[m * SS_PARTS + (n0 >> 7)] = (ss_acc[0] + ss_acc[1]) + (ss_acc[2] + ss_acc[3]);
@@ -476,12 +577,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
       tc::named_barrier_sync(tc::BAR_WG + wg, 128);
       if (row == 0) {
-        if constexpr (EPI == EPI_GEGLU) {
-          tc::tma_store_2d(&tmc, sC, n0 / 2, (int)m0);
-        } else {
 #pragma unroll
-          for (int g = 0; g < NSUB; ++g) tc::tma_store_2d(&tmc, sC + g * SUB_TILE_BYTES, n0 + g * 64, (int)m0);
-        }
+        for (int g = 0; g < NSUB; ++g) tc::tma_store_2d(&tmc, sC + g * SUB_TILE_BYTES, n0 + g * 64, (int)m0);
         tc::tma_store_commit();
         tc::tma_store_wait_read();             // sC stays alive until the bulk store has read it; the next tile re-fills it
       }
@@ -504,15 +601,20 @@ int launch_tc(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) 
   }
   if ((rc = tmap_2d(&tb, W, (uint64_t)p.K, (uint64_t)p.N, BK, BN))) return rc;
   const uint64_t n_out = EPI == EPI_GEGLU ? (uint64_t)p.N / 2 : (uint64_t)p.N;
-  if (EPI != EPI_SPLIT_LERP && EPI != EPI_PATCH_OUT) {
-    if ((rc = tmap_2d(&tcm, p.out, n_out, (uint64_t)p.M, 64, BM))) return rc;
+  if (EPI == EPI_SPLIT_LERP && p.box_w > 0) {   // skip and out: fine token tensors [B, 2 hc, 2 wc, C] in quadrant view
+    if ((rc = tmap_quad(&tcm, p.out, p.C, p.wc, (uint64_t)p.M / p.wc, p.box_w, p.box_h))) return rc;
+    if ((rc = tmap_quad(&tr, p.resid, p.C, p.wc, (uint64_t)p.M / p.wc, p.box_w, p.box_h))) return rc;
   } else {
-    tcm = ta;
-  }
-  if (EPI == EPI_RESID) {
-    if ((rc = tmap_2d(&tr, p.resid, (uint64_t)p.N, (uint64_t)p.M, 64, BM))) return rc;
-  } else {
-    tr = ta;
+    if (EPI != EPI_SPLIT_LERP && EPI != EPI_PATCH_OUT) {
+      if ((rc = tmap_2d(&tcm, p.out, n_out, (uint64_t)p.M, 64, BM))) return rc;
+    } else {
+      tcm = ta;
+    }
+    if (EPI == EPI_RESID) {
+      if ((rc = tmap_2d(&tr, p.resid, (uint64_t)p.N, (uint64_t)p.M, 64, BM))) return rc;
+    } else {
+      tr = ta;
+    }
   }
   constexpr size_t smem = gemm_smem<BN, EPI>();
   static_assert(smem <= 227 * 1024, "GEMM shared memory exceeds the 227 KiB opt-in limit");
@@ -761,6 +863,9 @@ int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int 
     quad_box(epi.mwc, &p.box_w, &p.box_h);
     return launch_tc<128, EPI_STORE>(A, W, p, st);
   }
+  // the split moves its skip and output tiles by TMA when a 128-row block is one box of the quadrant maps (else box_w stays 0).
+  // Each tile reads exactly the skip elements it writes, so `out` may alias `skip`.
+  if (epi.mode == EPI_SPLIT_LERP && epi.C % 64 == 0 && epi.wc > 0 && M % epi.wc == 0 && aligned16(epi.resid)) quad_box(epi.wc, &p.box_w, &p.box_h);
   switch (epi.mode) {
     case EPI_STORE:
       return dispatch_bn<EPI_STORE>(A, W, p, st);
