@@ -428,18 +428,83 @@ int launch_rope_table(const float* pos, const float* freqs, float2* out, int T_t
 // ------------------------------------------------------------------------------------------------
 // Generic attention: one warp per (batch, head, query); key set enumerated per attention type (KeySet, attn_sets.cuh).
 // ------------------------------------------------------------------------------------------------
+
+// The per-warp shared-memory slot: VECS vectors of e floats, then ARRS float arrays and one int array (the tokens) of n entries each,
+// n the most keys (or queries) one warp can have.  The launcher sizes it by floats(), the kernel carves it with the accessors.
+template <int VECS, int ARRS>
+struct AttnSlot {
+  __host__ __device__ static size_t floats(int e, int n) { return (size_t)VECS * e + (size_t)(ARRS + 1) * n; }
+  float* p;
+  int e, n;
+  __device__ AttnSlot(float* sm, int e_, int n_) : p(sm + (threadIdx.x >> 5) * floats(e_, n_)), e(e_), n(n_) {}
+  __device__ float* vec(int i) const { return p + i * e; }
+  __device__ float* arr(int i) const { return p + VECS * e + i * n; }
+  __device__ int* toks() const { return reinterpret_cast<int*>(arr(ARRS)); }
+};
+
+// q . k of the query qv (e floats, in shared memory) and the key row kp, fmaf in d order
+template <typename T>
+__device__ __forceinline__ float attn_dot(const float* qv, const T* kp, int e) {
+  float s = 0.f;
+  for (int d = 0; d < e; ++d) s = fmaf(qv[d], to_f(kp[d]), s);
+  return s;
+}
+
+// The key walk: for the lane's keys j = lane, lane + 32, ... < nk of ks, toks[j] = the key's token (-1: masked) and sc[j] = score(j, tok)
+// (-inf for a masked key, without a call).  -> the maximum score of the warp.
+template <typename Score>
+__device__ __forceinline__ float attn_scores(const KeySet& ks, int nk, float* sc, int* toks, Score score) {
+  float mx = -INFINITY;
+  for (int j0 = 0; j0 < nk; j0 += 32) {
+    const int j = j0 + (threadIdx.x & 31);
+    if (j < nk) {
+      const int tok = ks.token(j);
+      const float s = tok >= 0 ? score(j, tok) : -INFINITY;
+      sc[j] = s;
+      toks[j] = tok;
+      mx = fmaxf(mx, s);
+    }
+  }
+  return warp_max(mx);
+}
+
+// The softmax numerators in place of the lane's scores: p_j = exp(s_j - mx), 0 for a masked key.  -> sum_j p_j over the warp.
+__device__ __forceinline__ float attn_softmax(float* sc, const int* toks, int nk, float mx) {
+  float sum = 0.f;
+  for (int j = threadIdx.x & 31; j < nk; j += 32) {
+    const float p = (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
+    sc[j] = p;
+    sum += p;
+  }
+  return warp_sum(sum);
+}
+
+// sum_j w_j x(j, tok_j) over the n tokens of the slot in j order, one fmaf per token, masked tokens skipped.  x reads the row of tok_j
+// at the caller's dimension d; a second sum over the same tokens can ride in x.
+template <typename X>
+__device__ __forceinline__ float attn_wsum(const float* w, const int* toks, int n, X x) {
+  float acc = 0.f;
+  for (int j = 0; j < n; ++j) {
+    const int tok = toks[j];
+    if (tok >= 0) acc = fmaf(w[j], x(j, tok), acc);
+  }
+  return acc;
+}
+
+using AttnFwdSlot = AttnSlot<1, 1>;   // q | p | key tokens
+
 template <typename T>
 __global__ void __launch_bounds__(128) attn_generic_kernel(const T* __restrict__ qkv, T* __restrict__ out, int h, int w, int nh, int e,
                                                            int type, int param, int shift, int maxkeys) {
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int Ttok = h * w;
-  const int q = blockIdx.x * 4 + warp;
+  const int q = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int head = blockIdx.y;
   const int64_t b = blockIdx.z;
-  float* qv = sm + (size_t)warp * (e + 2 * maxkeys);
-  float* sc = qv + e;
-  int* toks = reinterpret_cast<int*>(sc + maxkeys);
+  const AttnFwdSlot slot(sm, e, maxkeys);
+  float *qv = slot.vec(0), *sc = slot.arr(0);
+  int* toks = slot.toks();
   if (q >= Ttok) return;
   const int64_t rs = 3LL * nh * e;                        // row stride of qkv
   const T* base = qkv + b * Ttok * rs;
@@ -449,46 +514,18 @@ __global__ void __launch_bounds__(128) attn_generic_kernel(const T* __restrict__
   KeySet ks;
   ks.init(type, h, w, param, shift, q);
   const int nk = ks.count();
-  float mx = -INFINITY;
-  for (int j0 = 0; j0 < nk; j0 += 32) {
-    const int j = j0 + lane;
-    if (j < nk) {
-      const int tok = ks.token(j);
-      float s = -INFINITY;
-      if (tok >= 0) {
-        const T* kp = base + (int64_t)tok * rs + (int64_t)(nh + head) * e;
-        s = 0.f;
-        for (int d = 0; d < e; ++d) s = fmaf(qv[d], to_f(kp[d]), s);
-      }
-      sc[j] = s;
-      toks[j] = tok;
-      mx = fmaxf(mx, s);
-    }
-  }
-  mx = warp_max(mx);
-  float sum = 0.f;
+  const T* kb = base + (int64_t)(nh + head) * e;
+  const float mx = attn_scores(ks, nk, sc, toks, [&](int, int tok) { return attn_dot(qv, kb + tok * rs, e); });
+  const float inv = 1.f / attn_softmax(sc, toks, nk, mx);
   __syncwarp();
-  for (int j = lane; j < nk; j += 32) {
-    const float p = (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
-    sc[j] = p;
-    sum += p;
-  }
-  sum = warp_sum(sum);
-  __syncwarp();
-  const float inv = 1.f / sum;
+  const T* vb = base + (int64_t)(2 * nh + head) * e;
   T* op = out + (b * Ttok + q) * (int64_t)nh * e + (int64_t)head * e;
-  for (int d = lane; d < e; d += 32) {
-    float acc = 0.f;
-    for (int j = 0; j < nk; ++j) {
-      const int tok = toks[j];
-      if (tok >= 0) acc = fmaf(sc[j], to_f(base[(int64_t)tok * rs + (int64_t)(2 * nh + head) * e + d]), acc);
-    }
-    op[d] = from_f<T>(acc * inv);
-  }
+  for (int d = lane; d < e; d += 32) op[d] = from_f<T>(attn_wsum(sc, toks, nk, [&](int, int tok) { return to_f(vb[tok * rs + d]); }) * inv);
 }
 
-// Launch geometry of the warp-per-query (or per-key) attention kernels: a grid of (query blocks of 4 warps, heads, images), the key set's
-// geometry checked, and per_warp floats of dynamic shared memory per warp within the budget the kernel is opened to on its first launch.
+// Launch of a warp-per-query (or per-key) attention kernel: a grid of (blocks of 4 warps, heads, images), the key set's geometry checked,
+// and a Slot of n keys (or queries) per warp within the budget the kernel is opened to on its first launch.  Every kernel takes its
+// pointers, then (h, w, nh, e, type, param, shift, n).
 constexpr int kAttnSmemMax = 200 * 1024;
 
 int check_attn_geometry(int h, int w, int type, int param) {
@@ -504,26 +541,30 @@ int check_attn_geometry(int h, int w, int type, int param) {
   return 0;
 }
 
-template <typename K>
-int attn_smem(K kernel, bool& opened, const char* what, int keys, size_t per_warp, size_t* smem) {
-  *smem = sizeof(float) * 4 * per_warp;
-  KDB_REQUIRE(*smem <= kAttnSmemMax, KDB_ERR_UNSUPPORTED, "%s: %d keys exceed the shared-memory budget", what, keys);
-  return set_smem_once(kernel, opened, kAttnSmemMax);
+template <typename Slot>
+int attn_smem(const char* what, int e, int n, size_t* smem) {
+  *smem = sizeof(float) * 4 * Slot::floats(e, n);
+  KDB_REQUIRE(*smem <= kAttnSmemMax, KDB_ERR_UNSUPPORTED, "%s: %d keys exceed the shared-memory budget", what, n);
+  return 0;
 }
 
-dim3 attn_grid(int B, int h, int w, int nh) { return dim3((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B); }
+template <typename Slot, auto kernel, typename... P>
+int launch_attn(const char* what, int n, int B, int h, int w, int nh, int e, int type, int param, int shift, cudaStream_t st, P... ptrs) {
+  static bool opened = false;
+  size_t smem;
+  int rc = check_attn_geometry(h, w, type, param);
+  if (rc || (rc = attn_smem<Slot>(what, e, n, &smem)) || (rc = set_smem_once(kernel, opened, kAttnSmemMax))) return rc;
+  kernel<<<dim3((unsigned)ceil_div(h * w, 4), (unsigned)nh, (unsigned)B), 128, smem, st>>>(ptrs..., h, w, nh, e, type, param, shift, n);
+  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
+  return 0;
+}
 
 template <typename T>
 int launch_attention_generic(const T* qkv, T* out, int B, int h, int w, int nh, int e, int attn_type, int attn_param, int shift,
                              cudaStream_t st) {
   const int maxkeys = KeySet::count(attn_type, h, w, attn_param);
-  static bool opened = false;
-  size_t smem;
-  int rc = check_attn_geometry(h, w, attn_type, attn_param);
-  if (rc || (rc = attn_smem(attn_generic_kernel<T>, opened, "attention_generic", maxkeys, e + 2 * maxkeys, &smem))) return rc;
-  attn_generic_kernel<T><<<attn_grid(B, h, w, nh), 128, smem, st>>>(qkv, out, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
-  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
-  return 0;
+  return launch_attn<AttnFwdSlot, attn_generic_kernel<T>>("attention_generic", maxkeys, B, h, w, nh, e, attn_type, attn_param, shift, st, qkv,
+                                                          out);
 }
 template int launch_attention_generic<float>(const float*, float*, int, int, int, int, int, int, int, int, cudaStream_t);
 template int launch_attention_generic<bf16>(const bf16*, bf16*, int, int, int, int, int, int, int, int, cudaStream_t);
@@ -702,19 +743,19 @@ int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, cons
 
 // Attention tangent, one warp per (batch, head, query), the key set of attn_generic_kernel:
 //   do_i = sum_j P_ij dv_j + sum_j P_ij dS_ij (v_j - o_i),   dS_ij = dq_i . k_j + q_i . dk_j
+using AttnJvpSlot = AttnSlot<2, 2>;   // q, dq | p, dS | key tokens
+
 __global__ void __launch_bounds__(128) attn_jvp_kernel(const float* __restrict__ qkv, const float* __restrict__ dqkv, float* __restrict__ dout,
                                                        int h, int w, int nh, int e, int type, int param, int shift, int maxkeys) {
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int Ttok = h * w;
-  const int q = blockIdx.x * 4 + warp;
+  const int q = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int head = blockIdx.y;
   const int64_t b = blockIdx.z;
-  float* qv = sm + (size_t)warp * (2 * e + 3 * maxkeys);
-  float* dqv = qv + e;
-  float* sc = dqv + e;
-  float* dsc = sc + maxkeys;
-  int* toks = reinterpret_cast<int*>(dsc + maxkeys);
+  const AttnJvpSlot slot(sm, e, maxkeys);
+  float *qv = slot.vec(0), *dqv = slot.vec(1), *sc = slot.arr(0), *dsc = slot.arr(1);
+  int* toks = slot.toks();
   if (q >= Ttok) return;
   const int64_t rs = 3LL * nh * e;
   const float* base = qkv + b * Ttok * rs;
@@ -727,53 +768,31 @@ __global__ void __launch_bounds__(128) attn_jvp_kernel(const float* __restrict__
   KeySet ks;
   ks.init(type, h, w, param, shift, q);
   const int nk = ks.count();
-  float mx = -INFINITY;
-  for (int j0 = 0; j0 < nk; j0 += 32) {
-    const int j = j0 + lane;
-    if (j < nk) {
-      const int tok = ks.token(j);
-      float s = -INFINITY, ds = 0.f;
-      if (tok >= 0) {
-        const float* kp = base + (int64_t)tok * rs + (int64_t)(nh + head) * e;
-        const float* dkp = dbase + (int64_t)tok * rs + (int64_t)(nh + head) * e;
-        s = 0.f;
-        for (int d = 0; d < e; ++d) {
-          s = fmaf(qv[d], kp[d], s);
-          ds = fmaf(dqv[d], kp[d], fmaf(qv[d], dkp[d], ds));
-        }
-      }
-      sc[j] = s;
-      dsc[j] = ds;
-      toks[j] = tok;
-      mx = fmaxf(mx, s);
+  const float *kb = base + (int64_t)(nh + head) * e, *dkb = dbase + (int64_t)(nh + head) * e;
+  const float mx = attn_scores(ks, nk, sc, toks, [&](int j, int tok) {   // s, and dS in the same loop over the key rows
+    const float *kp = kb + tok * rs, *dkp = dkb + tok * rs;
+    float s = 0.f, ds = 0.f;
+    for (int d = 0; d < e; ++d) {
+      s = fmaf(qv[d], kp[d], s);
+      ds = fmaf(dqv[d], kp[d], fmaf(qv[d], dkp[d], ds));
     }
-  }
-  mx = warp_max(mx);
-  float sum = 0.f, sds = 0.f;
+    dsc[j] = ds;
+    return s;
+  });
+  const float inv = 1.f / attn_softmax(sc, toks, nk, mx);
+  float sds = 0.f;
+  for (int j = lane; j < nk; j += 32) sds = fmaf(sc[j], toks[j] >= 0 ? dsc[j] : 0.f, sds);   // dS of a masked key: never written
+  const float psd = warp_sum(sds) * inv;   // sum_j P_j dS_j
   __syncwarp();
-  for (int j = lane; j < nk; j += 32) {
-    const float p = (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
-    sc[j] = p;
-    sum += p;
-    sds = fmaf(p, dsc[j], sds);
-  }
-  sum = warp_sum(sum);
-  sds = warp_sum(sds);
-  __syncwarp();
-  const float inv = 1.f / sum;
-  const float psd = sds * inv;   // sum_j P_j dS_j
+  const float *vb = base + (int64_t)(2 * nh + head) * e, *dvb = dbase + (int64_t)(2 * nh + head) * e;
   float* op = dout + (b * Ttok + q) * (int64_t)nh * e + (int64_t)head * e;
   for (int d = lane; d < e; d += 32) {
-    float o = 0.f, t = 0.f;
-    for (int j = 0; j < nk; ++j) {
-      const int tok = toks[j];
-      if (tok >= 0) {
-        const int64_t vo = (int64_t)tok * rs + (int64_t)(2 * nh + head) * e + d;
-        const float vv = base[vo];
-        o = fmaf(sc[j], vv, o);
-        t = fmaf(sc[j], fmaf(dsc[j], vv, dbase[vo]), t);
-      }
-    }
+    float o = 0.f;   // sum_j P_j v_j, in the pass of t
+    const float t = attn_wsum(sc, toks, nk, [&](int j, int tok) {
+      const float vv = vb[tok * rs + d];
+      o = fmaf(sc[j], vv, o);
+      return fmaf(dsc[j], vv, dvb[tok * rs + d]);
+    });
     op[d] = t * inv - (o * inv) * psd;
   }
 }
@@ -781,13 +800,7 @@ __global__ void __launch_bounds__(128) attn_jvp_kernel(const float* __restrict__
 int launch_attention_jvp(const float* qkv, const float* dqkv, float* dout, int B, int h, int w, int nh, int e, int attn_type, int attn_param,
                          int shift, cudaStream_t st) {
   const int maxkeys = KeySet::count(attn_type, h, w, attn_param);
-  static bool opened = false;
-  size_t smem;
-  int rc = check_attn_geometry(h, w, attn_type, attn_param);
-  if (rc || (rc = attn_smem(attn_jvp_kernel, opened, "attention_jvp", maxkeys, 2 * e + 3 * maxkeys, &smem))) return rc;
-  attn_jvp_kernel<<<attn_grid(B, h, w, nh), 128, smem, st>>>(qkv, dqkv, dout, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
-  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
-  return 0;
+  return launch_attn<AttnJvpSlot, attn_jvp_kernel>("attention_jvp", maxkeys, B, h, w, nh, e, attn_type, attn_param, shift, st, qkv, dqkv, dout);
 }
 
 // d(a gelu(g)) = da gelu(g) + a (Phi(g) + g phi(g)) dg, erf form
@@ -986,19 +999,21 @@ int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, cons
 // Attention VJP, query-centric pass: one warp per (batch, head, query i) over the key set of attn_generic_kernel.
 //   Delta_i = dO_i . O_i,  dS_ij = P_ij (dO_i . v_j - Delta_i),  dq_i = sum_j dS_ij k_j
 // It also leaves (row maximum, 1 / row sum, Delta_i) of query i in stats [B, nh, T, 3] for the key-centric pass.
+using AttnVjpQSlot = AttnSlot<2, 1>;    // q, dO | p, then dS | key tokens
+using AttnVjpKvSlot = AttnSlot<2, 2>;   // k, v | P, dS | query tokens
+
 __global__ void __launch_bounds__(128) attn_vjp_q_kernel(const float* __restrict__ qkv, const float* __restrict__ o, const float* __restrict__ dout,
                                                          float* __restrict__ dqkv, float* __restrict__ stats, int h, int w, int nh, int e,
                                                          int type, int param, int shift, int maxkeys) {
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int Ttok = h * w;
-  const int q = blockIdx.x * 4 + warp;
+  const int q = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int head = blockIdx.y;
   const int64_t b = blockIdx.z;
-  float* qv = sm + (size_t)warp * (2 * e + 2 * maxkeys);
-  float* dov = qv + e;
-  float* sc = dov + e;
-  int* toks = reinterpret_cast<int*>(sc + maxkeys);
+  const AttnVjpQSlot slot(sm, e, maxkeys);
+  float *qv = slot.vec(0), *dov = slot.vec(1), *sc = slot.arr(0);
+  int* toks = slot.toks();
   if (q >= Ttok) return;
   const int64_t rs = 3LL * nh * e;
   const float* base = qkv + b * Ttok * rs;
@@ -1014,24 +1029,9 @@ __global__ void __launch_bounds__(128) attn_vjp_q_kernel(const float* __restrict
   KeySet ks;
   ks.init(type, h, w, param, shift, q);
   const int nk = ks.count();
-  float mx = -INFINITY;
-  for (int j = lane; j < nk; j += 32) {
-    const int tok = ks.token(j);
-    float s = -INFINITY;
-    if (tok >= 0) {
-      const float* kp = base + (int64_t)tok * rs + (int64_t)(nh + head) * e;
-      s = 0.f;
-      for (int d = 0; d < e; ++d) s = fmaf(qv[d], kp[d], s);
-    }
-    sc[j] = s;
-    toks[j] = tok;
-    mx = fmaxf(mx, s);
-  }
-  mx = warp_max(mx);
-  float sum = 0.f;
-  for (int j = lane; j < nk; j += 32) sum += (toks[j] >= 0) ? expf(sc[j] - mx) : 0.f;
-  sum = warp_sum(sum);
-  const float inv = 1.f / sum;
+  const float* kb = base + (int64_t)(nh + head) * e;
+  const float mx = attn_scores(ks, nk, sc, toks, [&](int, int tok) { return attn_dot(qv, kb + tok * rs, e); });
+  const float inv = 1.f / attn_softmax(sc, toks, nk, mx);
   for (int j = lane; j < nk; j += 32) {
     const int tok = toks[j];
     float ds = 0.f;
@@ -1039,20 +1039,13 @@ __global__ void __launch_bounds__(128) attn_vjp_q_kernel(const float* __restrict
       const float* vp = base + (int64_t)tok * rs + (int64_t)(2 * nh + head) * e;
       float dp = 0.f;
       for (int d = 0; d < e; ++d) dp = fmaf(dov[d], vp[d], dp);
-      ds = expf(sc[j] - mx) * inv * (dp - delta);
+      ds = sc[j] * inv * (dp - delta);
     }
     sc[j] = ds;
   }
   __syncwarp();
   float* dq = dqkv + (b * Ttok + q) * rs + (int64_t)head * e;
-  for (int d = lane; d < e; d += 32) {
-    float acc = 0.f;
-    for (int j = 0; j < nk; ++j) {
-      const int tok = toks[j];
-      if (tok >= 0) acc = fmaf(sc[j], base[(int64_t)tok * rs + (int64_t)(nh + head) * e + d], acc);
-    }
-    dq[d] = acc;
-  }
+  for (int d = lane; d < e; d += 32) dq[d] = attn_wsum(sc, toks, nk, [&](int, int tok) { return kb[tok * rs + d]; });
   if (lane == 0) {
     float* st = stats + ((b * nh + head) * Ttok + q) * 3;
     st[0] = mx;
@@ -1067,16 +1060,14 @@ __global__ void __launch_bounds__(128) attn_vjp_kv_kernel(const float* __restric
                                                           float* __restrict__ dqkv, int h, int w, int nh, int e, int type, int param, int shift,
                                                           int maxq) {
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int Ttok = h * w;
-  const int kt = blockIdx.x * 4 + warp;
+  const int kt = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int head = blockIdx.y;
   const int64_t b = blockIdx.z;
-  float* kv = sm + (size_t)warp * (2 * e + 3 * maxq);
-  float* vv = kv + e;
-  float* pv = vv + e;
-  float* dsv = pv + maxq;
-  int* toks = reinterpret_cast<int*>(dsv + maxq);
+  const AttnVjpKvSlot slot(sm, e, maxq);
+  float *kv = slot.vec(0), *vv = slot.vec(1), *pv = slot.arr(0), *dsv = slot.arr(1);
+  int* toks = slot.toks();
   if (kt >= Ttok) return;
   const int64_t rs = 3LL * nh * e;
   const float* base = qkv + b * Ttok * rs;
@@ -1110,16 +1101,14 @@ __global__ void __launch_bounds__(128) attn_vjp_kv_kernel(const float* __restric
   __syncwarp();
   float* dk = dqkv + (b * Ttok + kt) * rs + (int64_t)(nh + head) * e;
   float* dvv = dk + (int64_t)nh * e;
+  const float* qb = base + (int64_t)head * e;
+  const float* dob = dout + b * Ttok * (int64_t)nh * e + (int64_t)head * e;
   for (int d = lane; d < e; d += 32) {
-    float ak = 0.f, av = 0.f;
-    for (int t = 0; t < nq; ++t) {
-      const int tok = toks[t];
-      if (tok >= 0) {
-        ak = fmaf(dsv[t], base[(int64_t)tok * rs + (int64_t)head * e + d], ak);
-        av = fmaf(pv[t], dout[(b * Ttok + tok) * (int64_t)nh * e + (int64_t)head * e + d], av);
-      }
-    }
-    dk[d] = ak;
+    float av = 0.f;   // sum_i P_ij dO_i, in the pass of dk
+    dk[d] = attn_wsum(dsv, toks, nq, [&](int t, int tok) {
+      av = fmaf(pv[t], dob[tok * (int64_t)nh * e + d], av);
+      return qb[tok * rs + d];
+    });
     dvv[d] = av;
   }
 }
@@ -1127,18 +1116,15 @@ __global__ void __launch_bounds__(128) attn_vjp_kv_kernel(const float* __restric
 int launch_attention_vjp(const float* qkv, const float* out, const float* dout, float* dqkv, float* stats, int B, int h, int w, int nh, int e,
                          int attn_type, int attn_param, int shift, cudaStream_t st) {
   const int maxkeys = KeySet::count(attn_type, h, w, attn_param), maxq = QuerySet::max_count(attn_type, h, w, attn_param);
-  static bool opened_q = false, opened_kv = false;
-  size_t smem_q, smem_kv;
+  // the key-centric slot is the larger (maxq >= maxkeys): a shape it cannot take is refused before the first launch
+  size_t smem_kv;
   int rc = check_attn_geometry(h, w, attn_type, attn_param);
-  if (rc || (rc = attn_smem(attn_vjp_q_kernel, opened_q, "attention_vjp", maxkeys, 2 * e + 2 * maxkeys, &smem_q)) ||
-      (rc = attn_smem(attn_vjp_kv_kernel, opened_kv, "attention_vjp", maxq, 2 * e + 3 * maxq, &smem_kv)))
+  if (rc || (rc = attn_smem<AttnVjpKvSlot>("attention_vjp", e, maxq, &smem_kv)) ||
+      (rc = launch_attn<AttnVjpQSlot, attn_vjp_q_kernel>("attention_vjp", maxkeys, B, h, w, nh, e, attn_type, attn_param, shift, st, qkv, out,
+                                                         dout, dqkv, stats)))
     return rc;
-  const dim3 grid = attn_grid(B, h, w, nh);
-  attn_vjp_q_kernel<<<grid, 128, smem_q, st>>>(qkv, out, dout, dqkv, stats, h, w, nh, e, attn_type, attn_param, shift, maxkeys);
-  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
-  attn_vjp_kv_kernel<<<grid, 128, smem_kv, st>>>(qkv, dout, stats, dqkv, h, w, nh, e, attn_type, attn_param, shift, maxq);
-  KDB_LAUNCH_CHECK(F_ATTN_GENERIC, st);
-  return 0;
+  return launch_attn<AttnVjpKvSlot, attn_vjp_kv_kernel>("attention_vjp", maxq, B, h, w, nh, e, attn_type, attn_param, shift, st, qkv, dout,
+                                                        stats, dqkv);
 }
 
 // da = dy gelu(g), dg = dy a (Phi(g) + g phi(g)), erf form; h [M, 2F] the primal up_proj output, dh [M, 2F]
