@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 13
+#define KDB_ABI_VERSION 14
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -133,7 +133,10 @@ int kdb_noise_brownian(float* out, const int64_t* seeds, int batch, int64_t per_
 #define KDB_MAX_LEVELS 8
 
 enum { KDB_ATTN_NONE = 0, KDB_ATTN_GLOBAL = 1, KDB_ATTN_NEIGHBORHOOD = 2, KDB_ATTN_SHIFTED_WINDOW = 3 };
-enum { KDB_PREC_FP32 = 0, KDB_PREC_BF16 = 1 };   /* arithmetic of the token stream / GEMM operands */
+/* arithmetic of the token stream / GEMM operands.  KDB_PREC_TF32 (the image_v1 U-Net only; every kdb_model_* entry point returns
+ * KDB_ERR_UNSUPPORTED for it): convolution and attention operands rounded to tf32, fp32 accumulation, fp32 activations, weights and
+ * outputs. */
+enum { KDB_PREC_FP32 = 0, KDB_PREC_BF16 = 1, KDB_PREC_TF32 = 2 };
 
 typedef struct KdbModelConfig {
   int32_t n_levels;                       /* len(levels); last level is the mid level       (:682-699) */
@@ -277,12 +280,15 @@ int64_t kdb_unet_cond_stride(const KdbUNet* m);
 int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, float* cond_out,
                           void* stream);
 
-/* Workspace of one forward in bytes; KDB_ERR_UNSUPPORTED for a precision other than KDB_PREC_FP32. */
+/* Workspace of one forward in bytes, the same at KDB_PREC_FP32 and KDB_PREC_TF32; KDB_ERR_UNSUPPORTED for any other precision. */
 int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int height, int width);
 
 /* One evaluation on x [B, in_channels, H, W] -> out of the same shape, as kdb_model_forward: sigma_data > 0 gives the
  * Karras-preconditioned denoiser, sigma_data <= 0 the raw inner model; cond rows with cond_batch_stride (0 = one shared row).
- * KDB_PREC_FP32 only (any other precision: KDB_ERR_UNSUPPORTED).  Every level but the innermost needs an even grid and every
+ * KDB_PREC_FP32: every kernel in fp32.  KDB_PREC_TF32: every convolution (the ResConvBlock 3x3 convs and 1x1 skip, qkv_proj and
+ * out_proj) on the tensor cores (kdb_unet_conv_tf32) with weights rounded to tf32 by finalize, and self-attention of d_head 64 on the
+ * tensor cores (kdb_attention at KDB_PREC_TF32; other head sizes keep the fp32 kernel); AdaGN, resampling, patch in / out and the
+ * conditioning stay fp32.  Any other precision: KDB_ERR_UNSUPPORTED.  Every level but the innermost needs an even grid and every
  * level at least 2x2.  Allocates nothing and synchronises nothing, so it can be captured into a CUDA graph; a workspace shorter
  * than kdb_unet_workspace_bytes returns KDB_ERR_WORKSPACE.  Deterministic (no atomics). */
 int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
@@ -333,7 +339,10 @@ int kdb_attn_block_bf16(void* x_bf16, const void* w_qkv_bf16, const void* w_out_
  * cosine-normalised and rotated.  attn_type/attn_param/shift as in KdbModelConfig (:523 for shift).
  * logit_bound (tensor-core path only, may be NULL): [n_heads] device floats, each in (0, 40], with |q . k| <= bound for that
  * head -- for cosine-similarity attention the layer's `scale` parameter (:106-114).  The kernels then use the bound as
- * softmax's fixed shift (one pass over the keys, no row maximum); NULL keeps the exact two-pass row-maximum kernels. */
+ * softmax's fixed shift (one pass over the keys, no row maximum); NULL keeps the exact two-pass row-maximum kernels.
+ * KDB_PREC_TF32 (fast 0, KDB_ATTN_GLOBAL, d_head 64, fp32 tensors, 1/sqrt(d_head) already in q): the image_v1 U-Net's attention
+ * (layers.py:181-200) on the tensor cores, q, k, v and the probabilities truncated to tf32, fp32 accumulation, running-maximum softmax;
+ * any other attention type, head size or `fast` at that precision is KDB_ERR_UNSUPPORTED. */
 int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch, int h, int w, int n_heads, int d_head,
                   int attn_type, int attn_param, int shift, const float* logit_bound, void* stream);
 
@@ -357,6 +366,13 @@ int kdb_attention_vjp(const float* qkv, const float* out, const float* dout, flo
  * with r2 NULL = r1 alone.  c1, c2 and rc1 must be multiples of 4; batch * h * w is at most 65535 * 64 (KDB_ERR_BAD_SHAPE). */
 int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1, int rc1,
                   const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
+
+/* The same convolution, arguments and layouts on the tensor cores (wgmma, the kernel kdb_unet_forward runs at KDB_PREC_TF32): the
+ * products take tf32 operands -- the low 13 mantissa bits of every input and weight element are ignored (truncation), so a caller
+ * wanting round-to-nearest weights rounds them first, as kdb_unet_finalize does -- and accumulate in fp32; bias and residual are added
+ * in fp32.  No grid-row limit on batch * h * w. */
+int kdb_unet_conv_tf32(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1,
+                       int rc1, const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "model_core.cuh"
+#include "unet_kernels.cuh"
 #include "tc_kernels.cuh"
 
 namespace kdb {
@@ -868,6 +869,10 @@ int kdb_model_conditioning(KdbModel* m, int rows, const float* sigma, const floa
 
 size_t kdb_model_workspace_bytes(const KdbModel* m, int precision, int batch, int height, int width) {
   if (!m || batch <= 0 || height <= 0 || width <= 0) return 0;
+  if (precision == KDB_PREC_TF32) {
+    set_error("model_workspace_bytes: the tf32 precision is built for the image_v1 U-Net only");
+    return 0;
+  }
   Workspace ws;
   Carver cv(nullptr, 1024);
   carve(m->cfg, precision, batch, height, width, cv, ws);
@@ -908,6 +913,7 @@ int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int wid
                       size_t workspace_bytes, void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward: model not finalized");
   KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward: NULL argument");
+  KDB_REQUIRE(precision != KDB_PREC_TF32, KDB_ERR_UNSUPPORTED, "forward: the tf32 precision is built for the image_v1 U-Net only");
   KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_BF16, KDB_ERR_BAD_ARG, "forward: bad precision %d", precision);
   int rc = check_image(m, "forward", height, width, sigma_data);
   if (rc) return rc;
@@ -968,6 +974,10 @@ int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch
                   int attn_param, int shift, const float* logit_bound, void* stream) {
   KDB_REQUIRE(qkv && out && batch > 0 && h > 0 && w > 0 && n_heads > 0 && d_head > 0, KDB_ERR_BAD_ARG, "attention: bad argument");
   cudaStream_t st = (cudaStream_t)stream;
+  if (precision == KDB_PREC_TF32) {   // the image_v1 U-Net's global attention on fp32 tensors (q pre-scaled), d_head 64
+    KDB_REQUIRE(attn_type == KDB_ATTN_GLOBAL && !fast, KDB_ERR_UNSUPPORTED, "attention: tf32 is built for global attention only");
+    return launch_unet_attn_tf32(static_cast<const float*>(qkv), static_cast<float*>(out), batch, h * w, n_heads, d_head, st);
+  }
   if (precision == KDB_PREC_FP32) {
     KDB_REQUIRE(!fast, KDB_ERR_UNSUPPORTED, "attention: tensor-core path is bf16 only");
     return launch_attention_generic<float>(static_cast<const float*>(qkv), static_cast<float*>(out), batch, h, w, n_heads, d_head,

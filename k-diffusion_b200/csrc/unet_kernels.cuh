@@ -24,6 +24,16 @@ struct ConvArgs {
   int B = 0, H = 0, W = 0, N = 0;
 };
 int launch_unet_conv(const ConvArgs& a, int ks, cudaStream_t st);
+// The same convolution on the tensor cores at KDB_PREC_TF32 (unet_tf32.cu): tf32 operands, fp32 accumulation.  w is expected rounded
+// to tf32 (launch_unet_round_tf32); activations are truncated to tf32 by the MMA.
+int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st);
+// Global self-attention at KDB_PREC_TF32 (unet_tf32.cu): qkv [B, T, 3 nh 64] fp32 in (t nh e) order with 1/sqrt(d_head) folded into q
+// -> out [B, T, nh 64] fp32; q, k, v and the softmax probabilities truncated to tf32, fp32 accumulation, running-maximum softmax.  Any
+// T >= 1.  unet_attn_tf32_supported: the head sizes it is built for (64); the engine keeps attn_generic for the others.
+bool unet_attn_tf32_supported(int d_head);
+int launch_unet_attn_tf32(const float* qkv, float* out, int B, int T, int nh, int d_head, cudaStream_t st);
+// dst[i] = src[i] rounded to the nearest tf32 value (ties away from zero), stored as fp32
+int launch_unet_round_tf32(const float* src, float* dst, int64_t n, cudaStream_t st);
 
 // AdaGN (layers.py:172-175), optionally followed by the erf GELU: out = [gelu](group_norm(x) * (1 + weight) + bias) with the
 // (weight, bias) pair read from the conditioning row of image b at cond + b * cond_bs + ada_off (C weights, then C biases).

@@ -16,10 +16,10 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 
-PREC_FP32, PREC_BF16 = 0, 1
+PREC_FP32, PREC_BF16, PREC_TF32 = 0, 1, 2
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 MAX_LEVELS = 8
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -94,6 +94,7 @@ SIGNATURES = {
     "kdb_attention_jvp": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_attention_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_conv": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_unet_conv_tf32": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
 }
 
 _lib = None
@@ -340,7 +341,7 @@ def noise_brownian(like, seeds, t_min, t_max, t0, t1, depth=24, out=None):
 _ATTN_CODE = {"none": ATTN_NONE, "global": ATTN_GLOBAL, "neighborhood": ATTN_NEIGHBORHOOD, "shifted-window": ATTN_SHIFTED_WINDOW}
 
 
-UNET_NO_DERIVATIVE = "the image_v1 U-Net engine has no derivative: only its fp32 forward is built (no JVP, VJP or autograd through x)"
+UNET_NO_DERIVATIVE = "the image_v1 U-Net engine has no derivative: only its forward is built (no JVP, VJP or autograd through x)"
 
 
 def unet_has_no_derivative(*args, **kwargs):
@@ -533,7 +534,7 @@ class Engine:
 
 
 class UNetEngine(Engine):
-    """The image_v1 U-Net on the exact fp32 path: the Engine calls where the sampler executor makes them; no derivatives."""
+    """The image_v1 U-Net at PREC_FP32 or PREC_TF32: the Engine calls where the sampler executor makes them; no derivatives."""
 
     _api = "unet"
 
@@ -650,11 +651,7 @@ def attention(qkv, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, fast
     return out
 
 
-@_on_device_of_first
-def unet_conv(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
-    """The U-Net engine's convolution (kdb_unet_conv): x1 [B,h,w,c1] and x2 [B,h,w,c2] token-major fp32 (their channel concatenation is
-    the input), w the tap-major weight [N, ksize*ksize, c1 + c2], bias [N], the residual [B,h,w,N] given as r1 (the first rc1 channels,
-    all N without r2) and r2 (the rest) -> out [B,h,w,N]."""
+def _unet_conv(fn, x1, w, ksize, x2, bias, r1, r2, out):
     require_cuda(x1, w, x2, bias, r1, r2, out)
     B, h, wd, c1 = x1.shape
     N = w.shape[0]
@@ -663,7 +660,33 @@ def unet_conv(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
     if out is None:
         out = torch.empty(B, h, wd, N, dtype=torch.float32, device=x1.device)
     x1, x2, w, bias, r1, r2 = (None if t is None else f32c(t) for t in (x1, x2, w, bias, r1, r2))
-    check(lib().kdb_unet_conv(ptr(x1), c1, ptr(x2), c2, ptr(w), ptr(bias), ptr(r1), rc1, ptr(r2), ptr(out), B, h, wd, N, ksize, stream()))
+    check(fn(ptr(x1), c1, ptr(x2), c2, ptr(w), ptr(bias), ptr(r1), rc1, ptr(r2), ptr(out), B, h, wd, N, ksize, stream()))
+    return out
+
+
+@_on_device_of_first
+def unet_conv(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
+    """The U-Net engine's convolution (kdb_unet_conv): x1 [B,h,w,c1] and x2 [B,h,w,c2] token-major fp32 (their channel concatenation is
+    the input), w the tap-major weight [N, ksize*ksize, c1 + c2], bias [N], the residual [B,h,w,N] given as r1 (the first rc1 channels,
+    all N without r2) and r2 (the rest) -> out [B,h,w,N]."""
+    return _unet_conv(lib().kdb_unet_conv, x1, w, ksize, x2, bias, r1, r2, out)
+
+
+@_on_device_of_first
+def unet_conv_tf32(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
+    """unet_conv on the tensor cores (kdb_unet_conv_tf32): the same arguments; the products take the inputs and w truncated to tf32 (round
+    w to tf32 first for round-to-nearest weights, as the engine does) and accumulate in fp32."""
+    return _unet_conv(lib().kdb_unet_conv_tf32, x1, w, ksize, x2, bias, r1, r2, out)
+
+
+@_on_device_of_first
+def unet_attention_tf32(qkv, h, w, n_heads, d_head=64):
+    """The U-Net engine's global attention at tf32 (kdb_attention with PREC_TF32): qkv [B, h*w, 3*n_heads*d_head] fp32 in (t nh e) order,
+    1/sqrt(d_head) already in q -> [B, h*w, n_heads*d_head] fp32.  q, k, v and the probabilities are truncated to tf32; d_head 64."""
+    require_cuda(qkv)
+    B = qkv.shape[0]
+    out = torch.empty(B, h * w, n_heads * d_head, dtype=torch.float32, device=qkv.device)
+    check(lib().kdb_attention(PREC_TF32, 0, ptr(f32c(qkv)), ptr(out), B, h, w, n_heads, d_head, ATTN_GLOBAL, 0, 0, None, stream()))
     return out
 
 

@@ -191,6 +191,8 @@ class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
 
     def resolved_precision(self):
         p = flags.resolve_precision(self.precision, self.patch_in.proj.weight.dtype)
+        if p == "tf32":
+            raise ValueError("the image_transformer_v2 engine runs at fp32 or bf16 (tf32 is built for the image_v1 U-Net only)")
         return _native.PREC_BF16 if p == "bf16" else _native.PREC_FP32
 
     def param_groups(self, *args, **kwargs):

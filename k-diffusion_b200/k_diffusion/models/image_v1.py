@@ -1,9 +1,10 @@
-"""image_v1 U-Net denoiser -- parameter container + native forward on the exact fp32 path.
+"""image_v1 U-Net denoiser -- parameter container + native forward, exact fp32 or with tf32 convolutions and attention.
 
 Constructor, forward signature and `state_dict()` layout follow the reference (k_diffusion/models/image_v1.py, layers.py:116-313),
 so reference checkpoints load unchanged; the forward pass itself is executed by libkdb200.so (kdb_unet_*).  The torch modules
-below only hold named parameters and buffers: none of their forward methods runs.  Inference only; fp32 only (a tensor-core
-route for the U-Net is not built).
+below only hold named parameters and buffers: none of their forward methods runs.  Inference only.  Precision: fp32 (the default,
+every kernel exact fp32) or, by set_precision("tf32") or KDB200_PRECISION=tf32, every convolution and the d_head-64 attention on the tensor cores with tf32
+operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True).
 """
 from types import SimpleNamespace
 
@@ -158,17 +159,17 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
         return eng
 
     def set_precision(self, precision):
-        """'fp32' or None/'auto' (both the exact fp32 path); the U-Net has no bf16 route."""
-        if precision not in (None, "auto", "fp32", "float32"):
-            raise ValueError(f"the image_v1 U-Net runs on the exact fp32 path only (got precision {precision!r})")
-        self.precision = None if precision in (None, "auto") else "fp32"
+        """'fp32' or None/'auto' (the exact fp32 path), or 'tf32' (tf32 convolutions and attention); the U-Net has no bf16 route."""
+        if precision not in (None, "auto", "fp32", "float32", "tf32"):
+            raise ValueError(f"the image_v1 U-Net runs at fp32 or tf32 (got precision {precision!r})")
+        self.precision = None if precision in (None, "auto") else "tf32" if precision == "tf32" else "fp32"
         return self
 
     def resolved_precision(self):
         p = flags.resolve_precision(self.precision, torch.float32)
-        if p != "fp32":
-            raise ValueError(f"the image_v1 U-Net runs on the exact fp32 path only (resolved precision {p!r})")
-        return _native.PREC_FP32
+        if p not in ("fp32", "tf32"):
+            raise ValueError(f"the image_v1 U-Net runs at fp32 or tf32 (resolved precision {p!r})")
+        return _native.PREC_TF32 if p == "tf32" else _native.PREC_FP32
 
     def param_groups(self, *args, **kwargs):
         raise NotImplementedError("training is out of scope for the H100 sampling path")
