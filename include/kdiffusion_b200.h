@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 14
+#define KDB_ABI_VERSION 15
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -127,7 +127,8 @@ int kdb_noise_brownian(float* out, const int64_t* seeds, int batch, int64_t per_
                        double t_min, double t_max, double t0, double t1, int depth, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * image_transformer_v2 denoiser engine (models/image_transformer_v2.py:667-762, layers.py:45-90)
+ * image_transformer_v2 denoiser engine (models/image_transformer_v2.py:667-762, layers.py:45-90), which also runs
+ * image_transformer_v1 (models/image_transformer_v1.py:280-344) as a one-level model with global attention
  * ------------------------------------------------------------------------------------------ */
 
 #define KDB_MAX_LEVELS 8
@@ -137,6 +138,15 @@ enum { KDB_ATTN_NONE = 0, KDB_ATTN_GLOBAL = 1, KDB_ATTN_NEIGHBORHOOD = 2, KDB_AT
  * KDB_ERR_UNSUPPORTED for it): convolution and attention operands rounded to tf32, fp32 accumulation, fp32 activations, weights and
  * outputs. */
 enum { KDB_PREC_FP32 = 0, KDB_PREC_BF16 = 1, KDB_PREC_TF32 = 2 };
+/* KdbModelConfig.family.  KDB_FAMILY_ITV1: image_transformer_v1 with n_levels 1, width = depth's d_model, d_ff, attn_type
+ * KDB_ATTN_GLOBAL, d_head 64, mapping_width = d_model, mapping_depth 2, mapping_d_ff = d_ff, mapping_cond_dim 0.  Its keys are v1's own
+ * ("blocks.<i>.self_attn.qk_norm.scale", "in_proj.weight", ...); kdb_model_finalize derives the engine's tables from them: qkv_proj
+ * with the q and k rows of each head permuted (new column j <- 2j, j + 32 <- 2j + 1), the cosine-sim scale exp(min(qk_norm.scale,
+ * ln 100)) with eps 64e-6 (QKNorm + SDPA's 1/sqrt(d_head)), the RoPE frequencies exp(freqs_h) | exp(freqs_w) over all 64 columns, and
+ * in_proj's columns / out_proj's rows reordered from v1's patch feature order (c i j) to the engine's (i j c).  Positions follow the
+ * image's aspect ratio W / H (v1's pixel_aspect_ratio = patch_h / patch_w).  The ".qkv" debug tap then holds q and k in the permuted
+ * column order. */
+enum { KDB_FAMILY_ITV2 = 0, KDB_FAMILY_ITV1 = 1 };
 
 typedef struct KdbModelConfig {
   int32_t n_levels;                       /* len(levels); last level is the mid level       (:682-699) */
@@ -151,6 +161,7 @@ typedef struct KdbModelConfig {
   int32_t attn_type[KDB_MAX_LEVELS];      /* KDB_ATTN_*                                                 */
   int32_t d_head[KDB_MAX_LEVELS];
   int32_t attn_param[KDB_MAX_LEVELS];     /* kernel_size (neighborhood) / window_size (shifted window)  */
+  int32_t family;                         /* KDB_FAMILY_*                                               */
 } KdbModelConfig;
 
 typedef struct KdbModel KdbModel;
@@ -159,7 +170,8 @@ int  kdb_model_create(const KdbModelConfig* cfg, KdbModel** out);
 void kdb_model_destroy(KdbModel* m);
 
 /* Bind one state-dict entry (fp32, contiguous, device) by its reference key name, e.g.
- * "down_levels.0.1.self_attn.qkv_proj.weight" (key list: SURVEY.md section 8b).  The pointer is
+ * "down_levels.0.1.self_attn.qkv_proj.weight" (key list: SURVEY.md section 8b), or for KDB_FAMILY_ITV1
+ * "blocks.3.self_attn.pos_emb.freqs_h".  The pointer is
  * borrowed: it must stay valid until the next kdb_model_finalize or destroy.  Replaces
  * nn.Module.load_state_dict for the engine (sample.py:44). */
 int kdb_model_set_tensor(KdbModel* m, const char* key, const float* data, const int64_t* shape, int ndim);

@@ -1,9 +1,11 @@
 // engine.cu -- host-side execution plan for the image_transformer_v2 denoiser
-// (reference: k_diffusion/models/image_transformer_v2.py:667-762 and layers.py:88-90).
+// (reference: k_diffusion/models/image_transformer_v2.py:667-762 and layers.py:88-90), and for image_transformer_v1
+// (image_transformer_v1.py:280-344), which runs as a one-level model with global attention through weights derived at finalize.
 //
 // The engine owns no activations: the caller passes one workspace; the plan carves it.  Weights are
 // borrowed device pointers keyed by the reference state-dict names; kdb_model_finalize builds the
-// derived tables (bf16 copies, concatenated AdaRMSNorm projection, position grids).
+// derived tables (bf16 copies, concatenated AdaRMSNorm projection, position grids, the QkRope tables).
+#include <algorithm>
 #include <cmath>
 #include <map>
 #include <string>
@@ -21,17 +23,18 @@ struct LayerPlan {
   int level = 0, attn_type = 0, attn_param = 0, shift = 0;
   int C = 0, dff = 0, nh = 0, e = 0;
   int ada_attn = -1, ada_ff = -1;   // offsets into a conditioning row
-  const float *attn_norm_w = nullptr, *qkv_w = nullptr, *scale = nullptr, *freqs = nullptr, *out_w = nullptr;
+  const float *attn_norm_w = nullptr, *qkv_w = nullptr, *out_w = nullptr;
+  QkRope qr;                         // cosine-sim + RoPE of q and k (freqs always, scale for v1: finalize's tables)
   const float *ff_norm_w = nullptr, *up_w = nullptr, *down_w = nullptr;
   bf16 *qkv_wb = nullptr, *out_wb = nullptr, *up_wb = nullptr, *down_wb = nullptr;
   bf16* up_wb_il = nullptr;          // up_proj rows interleaved (value/gate) for the fused GEGLU epilogue
-  bool bounded = false;              // every scale[h] in (0, KDB_ATTN_MAX_BOUND]: the scale is the attention kernels' fixed softmax shift
+  bool bounded = false;              // every qr.scale[h] in (0, KDB_ATTN_MAX_BOUND]: the scale is the attention kernels' fixed softmax shift
   bf16 *qkv_wf = nullptr, *up_wf = nullptr;   // per-evaluation copies with the AdaRMSNorm channel scale folded in (fused norm)
 };
 
 struct PosTables {
   std::vector<float*> pos;          // per level: [T_l, 2] (y, x)
-  std::vector<float2*> rope;        // per layer (KdbModel::layers): [T_l, nh, 16] (cos, sin) of the RoPE angles, or nullptr
+  std::vector<float2*> rope;        // per layer (KdbModel::layers): [T_l, nh, R/2] (cos, sin) of the RoPE angles, or nullptr
 };
 
 }  // namespace kdb
@@ -64,6 +67,42 @@ int make_bf16(KdbModel* m, const float* src, int64_t n, bf16** dst, cudaStream_t
   return launch_f32_to_bf16(src, *dst, n, st);
 }
 
+// the n floats at device pointer src, on the host
+int download(const float* src, size_t n, std::vector<float>& out, cudaStream_t st) {
+  out.resize(n);
+  KDB_CUDA(cudaMemcpyAsync(out.data(), src, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+  KDB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// a device copy of host floats, owned by the model
+int upload(KdbModel* m, const std::vector<float>& v, const float** out, cudaStream_t st) {
+  float* d = nullptr;
+  int rc = m->alloc(&d, v.size());
+  if (rc) return rc;
+  KDB_CUDA(cudaMemcpyAsync(d, v.data(), sizeof(float) * v.size(), cudaMemcpyHostToDevice, st));
+  KDB_CUDA(cudaStreamSynchronize(st));
+  *out = d;
+  return 0;
+}
+
+// an owned copy of the [rows, cols] matrix src whose row r (cols == 1: element r) is row perm(r) of src
+template <typename P>
+int permuted_rows(KdbModel* m, const float* src, int64_t rows, int64_t cols, P&& perm, const float** out, cudaStream_t st) {
+  std::vector<float> a, b((size_t)(rows * cols));
+  int rc = download(src, (size_t)(rows * cols), a, st);
+  if (rc) return rc;
+  for (int64_t r = 0; r < rows; ++r) std::copy_n(a.begin() + perm(r) * cols, cols, b.begin() + r * cols);
+  return upload(m, b, out, st);
+}
+
+// image_transformer_v1's patch feature order (c i j) (Patching / Unpatching, image_transformer_v1.py:223,242) -> the engine's (i j c)
+// (TokenMerge / TokenSplitWithoutSkip, image_transformer_v2.py:594,607): the (c i j) index of (i j c) feature n
+int64_t v1_patch_feature(int64_t n, int ch, int ph, int pw) {
+  const int64_t q = n / ch, c = n - q * ch;
+  return c * ph * pw + q;
+}
+
 // rows of up_proj [2F, C] reordered so that every 16-row group holds 8 value rows followed by the
 // 8 matching gate rows: lets a tensor-core epilogue that owns >= 16 consecutive columns apply GEGLU.
 __global__ void interleave_geglu_rows_kernel(const float* __restrict__ w, bf16* __restrict__ out, int F, int C) {
@@ -86,6 +125,10 @@ template <typename F>
 int for_each_layer(const KdbModelConfig& c, F&& f) {
   const int n = c.n_levels;
   int rc = 0;
+  if (c.family == KDB_FAMILY_ITV1) {   // image_transformer_v1.py:296: blocks.<i>, one level
+    for (int i = 0; i < c.depth[0] && rc == 0; ++i) rc = f("blocks." + std::to_string(i) + ".", 0, i);
+    return rc;
+  }
   for (int l = 0; l < n - 1; ++l)
     for (int i = 0; i < c.depth[l] && rc == 0; ++i) rc = f("down_levels." + std::to_string(l) + "." + std::to_string(i) + ".", l, i);
   for (int i = 0; i < c.depth[n - 1] && rc == 0; ++i) rc = f("mid_level." + std::to_string(i) + ".", n - 1, i);
@@ -112,19 +155,57 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
     const std::string a = prefix + "self_attn.";
     GET(a + "norm.linear.weight", &L.attn_norm_w, L.C, mw);
     GET(a + "qkv_proj.weight", &L.qkv_w, 3 * L.C, L.C);
-    GET(a + "scale", &L.scale, L.nh);
-    GET(a + "pos_emb.freqs", &L.freqs, L.nh, L.e / 8);
     GET(a + "out_proj.weight", &L.out_w, L.C, L.C);
     L.ada_attn = *ada_off;
     *ada_off += L.C;
-    {   // |q . k| <= scale_h after the cosine-similarity normalisation: usable as a fixed softmax shift while exp(-2 scale) stays normal
-      std::vector<float> hs((size_t)L.nh);
-      KDB_CUDA(cudaMemcpyAsync(hs.data(), L.scale, sizeof(float) * L.nh, cudaMemcpyDeviceToHost, st));
-      KDB_CUDA(cudaStreamSynchronize(st));
-      L.bounded = true;
-      for (float v : hs) L.bounded = L.bounded && v > 0.f && v <= KDB_ATTN_MAX_BOUND;
-    }
     int rc;
+    const int e = L.e, nh = L.nh;
+    std::vector<float> hs, tab((size_t)nh * (e / 2));   // the scale per head; a QkRope frequency table wide enough for R = e
+    if (c.family == KDB_FAMILY_ITV1) {
+      // QKNorm + SDPA (image_transformer_v1.py:108-128,163-169): q . k exp(0.5 s - 0.25 ln e)^2 e / sqrt(mean q^2 + eps)(mean k^2 + eps) / sqrt(e)
+      // = exp(s) q . k / sqrt((sum q^2 + e eps)(sum k^2 + e eps)), the cosine-sim logit with scale exp(min(s, ln 100)) (proj_'s clamp,
+      // :119-123) and eps e * 1e-6.  AxialRoPE (axial_rope.py:86-107) turns the pairs (2j, 2j+1) of all e columns by pos_y exp(freqs_h[j])
+      // (j < e/4) or pos_x exp(freqs_w[j - e/4]): half-split RoPE of R = e on q and k rows permuted within each head (new j <- old 2j,
+      // new j + e/2 <- old 2j + 1), which changes neither q . k nor the row norms.  v keeps its rows.
+      const float *s, *fh, *fw;
+      GET(a + "qk_norm.scale", &s, nh);
+      GET(a + "pos_emb.freqs_h", &fh, nh, e / 4);
+      GET(a + "pos_emb.freqs_w", &fw, nh, e / 4);
+      if ((rc = download(s, nh, hs, st))) return rc;
+      for (float& v : hs) v = std::exp(std::min(v, std::log(100.f)));
+      std::vector<float> y, x;
+      if ((rc = download(fh, (size_t)nh * (e / 4), y, st)) || (rc = download(fw, (size_t)nh * (e / 4), x, st))) return rc;
+      for (int h = 0; h < nh; ++h)
+        for (int j = 0; j < e / 4; ++j) {
+          tab[(size_t)h * (e / 2) + j] = std::exp(y[(size_t)h * (e / 4) + j]);
+          tab[(size_t)h * (e / 2) + e / 4 + j] = std::exp(x[(size_t)h * (e / 4) + j]);
+        }
+      const int64_t C = L.C;
+      auto perm = [C, e](int64_t r) {
+        if (r >= 2 * C) return r;
+        const int64_t base = r - r % e, j = r % e;
+        return base + (j < e / 2 ? 2 * j : 2 * (j - e / 2) + 1);
+      };
+      if ((rc = permuted_rows(m, L.qkv_w, 3 * C, C, perm, &L.qkv_w, st)) || (rc = upload(m, hs, &L.qr.scale, st))) return rc;
+      L.qr.eps = (float)e * 1e-6f;
+      L.qr.R = e;
+    } else {
+      // image_transformer_v2.py:106-114,187-199: cosine sim with eps 1e-6, and AxialRoPE(d_head // 2) whose freqs [nh, e/8] serve both axes
+      const float* f;
+      GET(a + "scale", &L.qr.scale, nh);
+      GET(a + "pos_emb.freqs", &f, nh, e / 8);
+      std::vector<float> fv;
+      if ((rc = download(L.qr.scale, nh, hs, st)) || (rc = download(f, (size_t)nh * (e / 8), fv, st))) return rc;
+      tab.resize((size_t)nh * (e / 4));
+      for (int h = 0; h < nh; ++h)
+        for (int j = 0; j < e / 4; ++j) tab[(size_t)h * (e / 4) + j] = fv[(size_t)h * (e / 8) + j % (e / 8)];
+      L.qr.eps = 1e-6f;
+      L.qr.R = e / 2;
+    }
+    if ((rc = upload(m, tab, &L.qr.freqs, st))) return rc;
+    // |q . k| <= scale_h after the cosine-similarity normalisation: usable as a fixed softmax shift while exp(-2 scale) stays normal
+    L.bounded = true;
+    for (float v : hs) L.bounded = L.bounded && v > 0.f && v <= KDB_ATTN_MAX_BOUND;
     if ((rc = make_bf16(m, L.qkv_w, 3LL * L.C * L.C, &L.qkv_wb, st))) return rc;
     if ((rc = make_bf16(m, L.out_w, (int64_t)L.C * L.C, &L.out_wb, st))) return rc;
     if ((rc = m->alloc(&L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
@@ -148,6 +229,7 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
 }
 
 int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
+  const KdbModelConfig& c = m->cfg;
   auto key = std::make_pair(h0, w0);
   auto it = m->pos_cache.find(key);
   if (it != m->pos_cache.end()) {
@@ -158,8 +240,10 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
   KDB_CUDA(cudaStreamIsCapturing(st, &cs));
   KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED,
               "first forward for a new token grid (%dx%d) must run outside CUDA-graph capture", h0, w0);
-  // axial_rope.py:31-68: cell centres in [-1,1] (short side scaled by the aspect ratio), (y, x) order
-  const double ar = (double)w0 / (double)h0;
+  // axial_rope.py:31-68: cell centres in [-1,1] (short side scaled by the aspect ratio), (y, x) order.  The aspect ratio is the token
+  // grid's for v2 (image_transformer_v2.py:725); v1 passes pixel_aspect_ratio = patch_h / patch_w (image_transformer_v1.py:224), which
+  // makes it the image's, W / H
+  const double ar = c.family == KDB_FAMILY_ITV1 ? (double)w0 * c.patch_w / ((double)h0 * c.patch_h) : (double)w0 / (double)h0;
   const double ys = ar > 1.0 ? 1.0 / ar : 1.0, xs = ar < 1.0 ? ar : 1.0;
   std::vector<double> cur((size_t)h0 * w0 * 2);
   for (int i = 0; i < h0; ++i)
@@ -197,9 +281,9 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
     const LayerPlan& L = m->layers[k];
     if (L.attn_type == KDB_ATTN_NONE || L.e != 64) continue;
     const int T_l = (h0 >> L.level) * (w0 >> L.level);
-    int rc = m->alloc(&pt.rope[k], (size_t)T_l * L.nh * 16);
+    int rc = m->alloc(&pt.rope[k], (size_t)T_l * L.nh * (L.qr.R / 2));
     if (rc) return rc;
-    if ((rc = launch_rope_table(pt.pos[L.level], L.freqs, pt.rope[k], T_l, L.nh, L.e / 8, st))) return rc;
+    if ((rc = launch_rope_table(pt.pos[L.level], L.qr.freqs, pt.rope[k], T_l, L.nh, L.qr.R / 4, st))) return rc;
   }
   KDB_CUDA(cudaStreamSynchronize(st));
   auto ins = m->pos_cache.emplace(key, std::move(pt));
@@ -328,8 +412,8 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
     if (!r) r = linear<T>(xn, WSel<T>::qkv(L), raw, Ma, 3 * C, C, GemmEpi{}, f.st);
     // the tangent reads the un-normalised primal q and k, so it runs before the primal launch
     if constexpr (std::is_same_v<T, float>)
-      if (!r && f.jvp) r = launch_qknorm_rope_jvp(raw, raw + M * 3 * C, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
-    return r ? r : launch_qknorm_rope<T>(raw, qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+      if (!r && f.jvp) r = launch_qknorm_rope_jvp(raw, raw + M * 3 * C, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
+    return r ? r : launch_qknorm_rope<T>(raw, qkv, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
   };
   int rc;
   if constexpr (std::is_same_v<T, bf16>) {
@@ -339,12 +423,14 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
     qe.nh = L.nh;
     qe.T_tokens = (int)Ttok;
     qe.rope = rope;
-    qe.qk_scale = L.scale;
+    qe.qk_scale = L.qr.scale;
+    qe.qk_eps = L.qr.eps;
+    qe.rope_r = L.qr.R;
     GemmEpi qf = qe;
     qf.ss_in = f.ws.rowss;
     if (f.fold && f.stats && tc_gemm_supported(M, 3 * C, C, qf)) {
       rc = launch_gemm_tc(x, L.qkv_wf, qkv, M, 3 * C, C, qf, f.st);
-      if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, qkv, pos, L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, f.st);
+      if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, qkv, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
     } else if (qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
       if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv_wb, qkv, M, 3 * C, C, qe, f.st);
     } else {
@@ -355,7 +441,7 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
   }
   if (rc || (rc = m->tap<T>(tag + ".qkv", qkv, Ma * 3 * C, f.st))) return rc;
   // q, k are normalised on every route above, so |q . k| <= scale: the attention kernels' fixed softmax shift when bounded
-  if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.scale : nullptr)))
+  if ((rc = attention_dispatch<T>(qkv, ao, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st, L.bounded ? L.qr.scale : nullptr)))
     return rc;
   if constexpr (std::is_same_v<T, float>)
     if (f.jvp && (rc = launch_attention_jvp(qkv, qkv + M * 3 * C, ao + M * C, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, f.st)))
@@ -395,7 +481,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
                        tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift);
     if constexpr (std::is_same_v<T, bf16>) {
       if (block) {
-        if ((rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st))) return rc;
+        if ((rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.qr.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st))) return rc;
         f.stats = true;
       }
     }
@@ -669,7 +755,7 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w) 
   if ((rc = launch_gemm_vjp(g, L.out_w, vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
   if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
-  if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.freqs, L.scale, M, (int)Ttok, L.nh, L.e, st))) return rc;
+  if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st))) return rc;
   if ((rc = launch_gemm_vjp(vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
   return launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, st);
 }
@@ -725,6 +811,10 @@ int kdb_model_create(const KdbModelConfig* cfg, KdbModel** out) {
   KDB_REQUIRE(cfg->patch_h >= 1 && cfg->patch_w >= 1 && cfg->in_channels >= 1 && cfg->out_channels >= 1, KDB_ERR_BAD_ARG,
               "model_create: bad patch/channels");
   KDB_REQUIRE(cfg->mapping_depth >= 0 && cfg->mapping_depth <= 8 && cfg->mapping_width >= 2, KDB_ERR_BAD_ARG, "model_create: bad mapping spec");
+  KDB_REQUIRE(cfg->family == KDB_FAMILY_ITV2 || cfg->family == KDB_FAMILY_ITV1, KDB_ERR_BAD_ARG, "model_create: unknown model family %d", cfg->family);
+  KDB_REQUIRE(cfg->family != KDB_FAMILY_ITV1 || (cfg->n_levels == 1 && cfg->attn_type[0] == KDB_ATTN_GLOBAL && cfg->d_head[0] == 64 &&
+                                                 cfg->mapping_width == cfg->width[0] && cfg->mapping_cond_dim == 0),
+              KDB_ERR_BAD_ARG, "model_create: image_transformer_v1 is one level of global attention, d_head 64, mapping width = width, no mapping_cond");
   for (int l = 0; l < cfg->n_levels; ++l) {
     KDB_REQUIRE(cfg->width[l] > 0 && cfg->depth[l] >= 0 && cfg->d_ff[l] > 0, KDB_ERR_BAD_ARG, "model_create: bad level %d", l);
     KDB_REQUIRE(cfg->attn_type[l] >= KDB_ATTN_NONE && cfg->attn_type[l] <= KDB_ATTN_SHIFTED_WINDOW, KDB_ERR_BAD_ARG,
@@ -788,10 +878,23 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     if ((rc = make_bf16(m, m->merge_w[l], 4LL * c.width[l] * c.width[l + 1], &m->merge_wb[l], st))) return rc;
     if ((rc = make_bf16(m, m->split_w[l], 4LL * c.width[l] * c.width[l + 1], &m->split_wb[l], st))) return rc;
   }
-  const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels;
-  GET("patch_in.proj.weight", &m->patch_in_w, C0, (int64_t)c.patch_h * c.patch_w * c.in_channels);
+  const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels, Ni = c.patch_h * c.patch_w * c.in_channels;
   GET("out_norm.scale", &m->out_norm, C0);
-  GET("patch_out.proj.weight", &m->patch_out_w, Np, C0);
+  if (c.family == KDB_FAMILY_ITV1) {   // in_proj / out_proj (image_transformer_v1.py:295,298) in the engine's patch feature order
+    const float *wi, *wo;
+    GET("in_proj.weight", &wi, C0, Ni);
+    GET("out_proj.weight", &wo, Np, C0);
+    std::vector<float> a, b((size_t)C0 * Ni);
+    if ((rc = download(wi, (size_t)C0 * Ni, a, st))) return rc;
+    for (int64_t r = 0; r < C0; ++r)
+      for (int64_t n = 0; n < Ni; ++n) b[r * Ni + n] = a[r * Ni + v1_patch_feature(n, c.in_channels, c.patch_h, c.patch_w)];
+    if ((rc = upload(m, b, &m->patch_in_w, st))) return rc;
+    auto perm = [&](int64_t r) { return v1_patch_feature(r, c.out_channels, c.patch_h, c.patch_w); };
+    if ((rc = permuted_rows(m, wo, Np, C0, perm, &m->patch_out_w, st))) return rc;
+  } else {
+    GET("patch_in.proj.weight", &m->patch_in_w, C0, Ni);
+    GET("patch_out.proj.weight", &m->patch_out_w, Np, C0);
+  }
 
   m->patch_in_wb = nullptr;
   if (c.in_channels == 3 && c.patch_h == 4 && c.patch_w == 4 && C0 % 128 == 0) {

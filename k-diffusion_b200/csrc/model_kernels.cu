@@ -41,27 +41,27 @@ __device__ __forceinline__ int64_t merge_source(int64_t i, int hc, int wc, int C
   return fine_offset(r / hc, hy, wx, q, e, hc, wc, Cf);
 }
 
-// Tangent of a row norm y = x r, r = rsqrt(ss / n + eps), ss = sum x^2 (RMSNorm: n = row width; cosine-sim: n = 1), along u with
-// sd = x . u: dy = r u - x r^3 sd / n.  The row sums are the caller's.
+// Tangent of a row norm y = x r, r = rsqrt(ss / n + eps), ss = sum x^2 (RMSNorm: n = row width; cosine-sim: n = 1, the layer's eps), along
+// u with sd = x . u: dy = r u - x r^3 sd / n.  The row sums are the caller's.
 struct NormTangent {
   float r, r3m;
-  __device__ NormTangent(float ss, float sd, float n) : r(rsqrtf(ss / n + kEps)), r3m(r * r * r * (sd / n)) {}
+  __device__ NormTangent(float ss, float sd, float n, float eps = kEps) : r(rsqrtf(ss / n + eps)), r3m(r * r * r * (sd / n)) {}
   __device__ float operator()(float x, float u) const { return r * u - x * r3m; }
 };
 
-// Axial RoPE of a head of e columns (AxialRoPE(d_head // 2)): column j < e/4 pairs with column j + e/4 and both turn by
-// theta_j = pos_y f_j (j < nf) or pos_x f_(j - nf), nf = e/8, f = the head's freqs; columns from e/2 on pass through.
+// Axial RoPE of the first R columns of a head (QkRope): column j < R/2 pairs with column j + R/2 and both turn by
+// theta_j = pos_y f_j (j < nf) or pos_x f_j (j >= nf), nf = R/4, f = the head's R/2 frequencies; columns from R on pass through.
 __device__ __forceinline__ void rope_sincos(float py, float px, const float* f, int j, int nf, float& s, float& c) {
-  sincosf((j < nf ? py : px) * f[j < nf ? j : j - nf], &s, &c);
+  sincosf((j < nf ? py : px) * f[j], &s, &c);
 }
 // column d of the rotated head v; INV: rotated by -theta (the transpose)
 template <bool INV>
-__device__ __forceinline__ float rope_rotate(const float* v, int d, int e, float py, float px, const float* f) {
-  const int dr = e / 4;
-  if (d >= 2 * dr) return v[d];
+__device__ __forceinline__ float rope_rotate(const float* v, int d, int R, float py, float px, const float* f) {
+  const int dr = R / 2;
+  if (d >= R) return v[d];
   const int j = d < dr ? d : d - dr;
   float s, c;
-  rope_sincos(py, px, f, j, e / 8, s, c);
+  rope_sincos(py, px, f, j, R / 4, s, c);
   const float x1 = v[j], x2 = v[j + dr];
   if constexpr (INV)
     return d < dr ? x1 * c + x2 * s : x2 * c - x1 * s;
@@ -352,8 +352,7 @@ template int launch_gemm_simt<bf16, bf16>(const bf16*, const bf16*, bf16*, int64
 // head).
 // ------------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, const float* __restrict__ pos,
-                                                          const float* __restrict__ freqs, const float* __restrict__ scale,
+__global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, const float* __restrict__ pos, const QkRope qr,
                                                           int64_t rows, int Ttok, int nh, int e) {
   extern __shared__ float sm[];   // [warps][2][e]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -363,7 +362,8 @@ __global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, 
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * 2 * e;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
-  const float sqs = sqrtf(scale[h]);
+  const float sqs = sqrtf(qr.scale[h]);
+  const float* f = qr.freqs + h * (qr.R / 2);
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
     const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
@@ -374,11 +374,11 @@ __global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, 
       ss = fmaf(f, f, ss);
     }
     ss = warp_sum(ss);
-    const float sc = sqs * rsqrtf(ss + kEps);
+    const float sc = sqs * rsqrtf(ss + qr.eps);
     // the reference rounds the scaled q/k back to the activation dtype before RoPE (:114)
     for (int d = lane; d < e; d += 32) buf[t * e + d] = to_f(from_f<T>(to_f(v[d]) * sc));
     __syncwarp();
-    for (int d = lane; d < e; d += 32) dst[off + d] = from_f<T>(rope_rotate<false>(buf + t * e, d, e, py, px, freqs + h * (e / 8)));
+    for (int d = lane; d < e; d += 32) dst[off + d] = from_f<T>(rope_rotate<false>(buf + t * e, d, qr.R, py, px, f));
     __syncwarp();
   }
   if (src != dst) {
@@ -387,21 +387,27 @@ __global__ void __launch_bounds__(128) qknorm_rope_kernel(const T* src, T* dst, 
   }
 }
 
+static int check_qk_rope(const char* what, const QkRope& qr, int e) {
+  KDB_REQUIRE(e % 8 == 0 && qr.R % 4 == 0 && qr.R > 0 && qr.R <= e, KDB_ERR_BAD_SHAPE,
+              "%s: d_head %d must be a multiple of 8 and the rotated width %d a multiple of 4, at most d_head", what, e, qr.R);
+  return 0;
+}
+
 template <typename T>
-int launch_qknorm_rope(const T* src, T* dst, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh, int e,
-                       cudaStream_t st) {
-  KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope: d_head %d must be a multiple of 8", e);
+int launch_qknorm_rope(const T* src, T* dst, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e, cudaStream_t st) {
+  if (int rc = check_qk_rope("qknorm_rope", qr, e)) return rc;
   const size_t smem = sizeof(float) * 4 * 2 * e;
-  qknorm_rope_kernel<T><<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(src, dst, pos, freqs, scale, rows, T_tokens, nh, e);
+  qknorm_rope_kernel<T><<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(src, dst, pos, qr, rows, T_tokens, nh, e);
   KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
   return 0;
 }
-template int launch_qknorm_rope<float>(const float*, float*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
-template int launch_qknorm_rope<bf16>(const bf16*, bf16*, const float*, const float*, const float*, int64_t, int, int, int, cudaStream_t);
+template int launch_qknorm_rope<float>(const float*, float*, const float*, const QkRope&, int64_t, int, int, int, cudaStream_t);
+template int launch_qknorm_rope<bf16>(const bf16*, bf16*, const float*, const QkRope&, int64_t, int, int, int, cudaStream_t);
 
 // RoPE table for the QKV epilogue: float4 [(head * nf + i) * T + token] = (cos t_2i, cos t_2i+1, sin t_2i, sin t_2i+1), i < nf.
 // Token-minor, so the 32 threads of an epilogue warp (32 consecutive tokens) read 512 contiguous bytes per load, and the
-// (cos, cos, sin, sin) order is what the packed-fp32 rotation consumes.  theta_j = pos_h * f_j (j < nf) or pos_w * f_{j-nf}.
+// (cos, cos, sin, sin) order is what the packed-fp32 rotation consumes.  theta_j = pos_h * f_j (j < nf) or pos_w * f_j (j >= nf),
+// f = the head's 2 nf frequencies (QkRope::freqs, nf = R/4).
 __global__ void __launch_bounds__(256) rope_table_kernel(const float* __restrict__ pos, const float* __restrict__ freqs,
                                                          float2* __restrict__ out, int T_tokens, int nh, int nf) {
   const int total = T_tokens * nh * 2 * nf;
@@ -411,7 +417,7 @@ __global__ void __launch_bounds__(256) rope_table_kernel(const float* __restrict
     const int j = (i / T_tokens) % (2 * nf);
     const int h = i / (T_tokens * 2 * nf);
     float s, c;
-    rope_sincos(pos[t * 2], pos[t * 2 + 1], freqs + h * nf, j, nf, s, c);
+    rope_sincos(pos[t * 2], pos[t * 2 + 1], freqs + h * 2 * nf, j, nf, s, c);
     const int64_t base = (((int64_t)h * nf + (j >> 1)) * T_tokens + t) * 4;
     o[base + (j & 1)] = c;
     o[base + 2 + (j & 1)] = s;
@@ -702,8 +708,7 @@ int launch_rmsnorm_jvp(const float* x, const float* dx, float* dy, const float* 
 
 // One warp per (token row, head) of the tangent rows; reads the un-normalised primal q, k of the same row.
 __global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __restrict__ qkv, float* __restrict__ dqkv,
-                                                              const float* __restrict__ pos, const float* __restrict__ freqs,
-                                                              const float* __restrict__ scale, int64_t rows, int Ttok, int nh, int e) {
+                                                              const float* __restrict__ pos, const QkRope qr, int64_t rows, int Ttok, int nh, int e) {
   extern __shared__ float sm[];   // [warps][2][e]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
@@ -712,7 +717,8 @@ __global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __res
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * 2 * e;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
-  const float sqs = sqrtf(scale[h]);
+  const float sqs = sqrtf(qr.scale[h]);
+  const float* f = qr.freqs + h * (qr.R / 2);
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
     const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
@@ -724,19 +730,19 @@ __global__ void __launch_bounds__(128) qknorm_rope_jvp_kernel(const float* __res
       sd = fmaf(v[d], dv[d], sd);
     }
     // the tangent of the cosine-sim scaling, then the primal's rotation
-    const NormTangent nt(warp_sum(ss), warp_sum(sd), 1.f);
+    const NormTangent nt(warp_sum(ss), warp_sum(sd), 1.f, qr.eps);
     for (int d = lane; d < e; d += 32) buf[t * e + d] = sqs * nt(v[d], dv[d]);
     __syncwarp();
-    for (int d = lane; d < e; d += 32) dv[d] = rope_rotate<false>(buf + t * e, d, e, py, px, freqs + h * (e / 8));
+    for (int d = lane; d < e; d += 32) dv[d] = rope_rotate<false>(buf + t * e, d, qr.R, py, px, f);
     __syncwarp();
   }
 }
 
-int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
-                           int nh, int e, cudaStream_t st) {
-  KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope_jvp: d_head %d must be a multiple of 8", e);
+int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
+                           cudaStream_t st) {
+  if (int rc = check_qk_rope("qknorm_rope_jvp", qr, e)) return rc;
   const size_t smem = sizeof(float) * 4 * 2 * e;
-  qknorm_rope_jvp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, freqs, scale, rows, T_tokens, nh, e);
+  qknorm_rope_jvp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, qr, rows, T_tokens, nh, e);
   KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
   return 0;
 }
@@ -958,8 +964,7 @@ int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* 
 // dq = sqrt(scale) (rho g - q rho^3 (q . g)), rho = rsqrt(sum q^2 + eps) of the un-normalised primal q in qkv.  One warp per
 // (token row, head).
 __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __restrict__ qkv, float* __restrict__ dqkv,
-                                                              const float* __restrict__ pos, const float* __restrict__ freqs,
-                                                              const float* __restrict__ scale, int64_t rows, int Ttok, int nh, int e) {
+                                                              const float* __restrict__ pos, const QkRope qr, int64_t rows, int Ttok, int nh, int e) {
   extern __shared__ float sm[];   // [warps][e]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
@@ -968,30 +973,31 @@ __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __res
   const int h = (int)(item - row * nh);
   float* buf = sm + (size_t)warp * e;
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
-  const float sqs = sqrtf(scale[h]);
+  const float sqs = sqrtf(qr.scale[h]);
+  const float* f = qr.freqs + h * (qr.R / 2);
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
     const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
     const float* v = qkv + off;
     float* dv = dqkv + off;
-    for (int d = lane; d < e; d += 32) buf[d] = rope_rotate<true>(dv, d, e, py, px, freqs + h * (e / 8));
+    for (int d = lane; d < e; d += 32) buf[d] = rope_rotate<true>(dv, d, qr.R, py, px, f);
     __syncwarp();
     float ss = 0.f, sg = 0.f;
     for (int d = lane; d < e; d += 32) {
       ss = fmaf(v[d], v[d], ss);
       sg = fmaf(v[d], buf[d], sg);
     }
-    const NormTangent nt(warp_sum(ss), warp_sum(sg), 1.f);
+    const NormTangent nt(warp_sum(ss), warp_sum(sg), 1.f, qr.eps);
     for (int d = lane; d < e; d += 32) dv[d] = sqs * nt(v[d], buf[d]);
     __syncwarp();
   }
 }
 
-int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
-                           int nh, int e, cudaStream_t st) {
-  KDB_REQUIRE(e % 8 == 0, KDB_ERR_BAD_SHAPE, "qknorm_rope_vjp: d_head %d must be a multiple of 8", e);
+int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
+                           cudaStream_t st) {
+  if (int rc = check_qk_rope("qknorm_rope_vjp", qr, e)) return rc;
   const size_t smem = sizeof(float) * 4 * e;
-  qknorm_rope_vjp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, freqs, scale, rows, T_tokens, nh, e);
+  qknorm_rope_vjp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, qr, rows, T_tokens, nh, e);
   KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
   return 0;
 }

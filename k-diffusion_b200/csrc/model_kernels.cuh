@@ -17,8 +17,10 @@ struct GemmEpi {
   const float* fac = nullptr;    // EPI_SPLIT_LERP: device scalar (TokenSplit.fac)
   int hc = 0, wc = 0, C = 0;     // EPI_SPLIT_LERP: coarse grid and fine channel count (N == 4*C)
   // EPI_QKV_ROPE (tensor-core path only): cosine-sim scaling + axial RoPE of the q and k thirds (N == 3*C, d_head 64)
-  const float2* rope = nullptr;  // launch_rope_table: float4 [nh][8][T_tokens] = (cos, cos, sin, sin) of the angle pairs
+  const float2* rope = nullptr;  // launch_rope_table: float4 [nh][rope_r / 4][T_tokens] = (cos, cos, sin, sin) of the angle pairs
   const float* qk_scale = nullptr;   // [nh]
+  float qk_eps = 1e-6f;          // QkRope::eps (image_transformer_v2's unless set)
+  int rope_r = 32;               // QkRope::R: 32 (image_transformer_v2) or 64 (image_transformer_v1, all of a head)
   int nh = 0, T_tokens = 0;
   // TokenMerge folded into the A-operand load (tensor-core path only): A = fine tokens [B, 2*mhc, 2*mwc, mC], K = 4*mC in
   // (nh nw e) order, M = B*mhc*mwc.  mC == 0 -> A is a plain [M, K] matrix.
@@ -54,11 +56,22 @@ int launch_rmsnorm(const T* x, T* y, const float* scale, int64_t scale_bstride, 
 template <typename T, typename TW>
 int launch_gemm_simt(const T* A, const TW* W, T* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st);
 
-// cosine-sim scaling of q,k and axial RoPE, qkv [rows, 3, nh, e] src -> dst (src == dst: in place; else v is copied through)
-// (image_transformer_v2.py:106-114,187-199,245-248).  pos [T,2] (y,x) for the level, freqs [nh, e/8], scale [nh]; rows = B*T
+// Cosine-sim scaling and axial RoPE of one layer's q and k heads of e columns (image_transformer_v2.py:106-114,187-199,245-248):
+//   q^ = sqrt(scale_h) q / sqrt(sum q^2 + eps), then column j < R/2 of q^ and column j + R/2 turn by theta_j = pos_y freqs[h, j]
+//   (j < R/4) or pos_x freqs[h, j] (j >= R/4); columns from R on pass through.
+// image_transformer_v2: R = e/2, freqs = (f, f) of its pos_emb.freqs f [nh, e/8], eps 1e-6.  image_transformer_v1 (QKNorm + the
+// interleaved AxialRoPE of all e columns) is the same map on q, k rows permuted by kdb_model_finalize: R = e, freqs = exp(freqs_h) |
+// exp(freqs_w), scale = exp(min(qk_norm.scale, ln 100)), eps = e * 1e-6.
+struct QkRope {
+  const float* freqs = nullptr;   // [nh, R/2]
+  const float* scale = nullptr;   // [nh]; |q^ . k^| <= scale_h
+  float eps = 0.f;
+  int R = 0;
+};
+
+// QkRope on qkv [rows, 3, nh, e] src -> dst (src == dst: in place; else v is copied through).  pos [T,2] (y,x) for the level; rows = B*T
 template <typename T>
-int launch_qknorm_rope(const T* src, T* dst, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens, int nh,
-                       int e, cudaStream_t st);
+int launch_qknorm_rope(const T* src, T* dst, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e, cudaStream_t st);
 
 // softmax(q k^T) v over the key set of attn_type (scale 1.0); qkv [B,h,w,3,nh,e] -> out [B,h,w,nh,e]
 template <typename T>
@@ -85,8 +98,8 @@ int launch_patch_out(const T* tokens, const float* norm_scale, const float* W, c
 int launch_rmsnorm_jvp(const float* x, const float* dx, float* dy, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
                        int64_t rows, int C, cudaStream_t st);
 // cosine-sim scale + RoPE of the tangent q, k (in place on dqkv [rows, 3, nh, e]); qkv holds the primal q, k BEFORE launch_qknorm_rope
-int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
-                           int nh, int e, cudaStream_t st);
+int launch_qknorm_rope_jvp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
+                           cudaStream_t st);
 // attention tangent over the key set of launch_attention_generic; qkv = the normalised, rotated primal, dqkv its tangent
 int launch_attention_jvp(const float* qkv, const float* dqkv, float* dout, int B, int h, int w, int nh, int e, int attn_type, int attn_param,
                          int shift, cudaStream_t st);
@@ -106,8 +119,8 @@ int launch_gemm_vjp(const float* dC, const float* W, float* out, int64_t M, int 
 int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
                        int64_t rows, int C, cudaStream_t st);
 // cosine-sim scale + RoPE, in place on the q, k thirds of dqkv [rows, 3, nh, e] (v passes through); qkv = the primal BEFORE launch_qknorm_rope
-int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, int64_t rows, int T_tokens,
-                           int nh, int e, cudaStream_t st);
+int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
+                           cudaStream_t st);
 // attention over the key set of launch_attention_generic: qkv the normalised, rotated primal, out its output, dout the output gradient
 // -> dqkv [B, T, 3, nh, e].  stats: scratch of B * nh * T * 3 floats (per-query softmax statistics handed from the query-centric pass
 // to the key-centric one)
@@ -145,7 +158,7 @@ struct CondWeights {
 int launch_conditioning(const CondWeights& w, int rows, const float* sigma, const float* aug, const int64_t* cls, const float* mcond,
                         float* out, int64_t out_stride, cudaStream_t st);
 
-// (cos, sin) table of the axial RoPE angles: out[t, h, j] for j < 2*nf: theta = (j < nf ? pos_y : pos_x)[t] * freqs[h, j % nf]
+// (cos, sin) table of the axial RoPE angles of QkRope with R = 4 nf: theta_j = (j < nf ? pos_y : pos_x)[t] * freqs[h, j], j < 2 nf
 int launch_rope_table(const float* pos, const float* freqs, float2* out, int T_tokens, int nh, int nf, cudaStream_t st);
 
 // dtype conversion helpers

@@ -186,7 +186,12 @@ __device__ __forceinline__ void stage_ld32(const float* s, int row, int col0, fl
 // to bf16 at the pack, one TMA store per 64 columns), and hands the fp32 tile on once its rows are read (BAR_ACC).  GEGLU works
 // element by element on value / gate pairs that share a thread: it runs on the accumulator fragments themselves and writes bf16
 // pairs straight into its staging tile, without the fp32 tile or BAR_ACC.
-template <int BN, int EPI>
+// ROPE_R: EPI_QKV_ROPE's rotated width R when it is not 32 (one value: image_transformer_v1 rotates all 64 columns of a head); the
+// other instantiations keep an empty pack, and with it their demangled names (gemm_wg_kernel<64, 5>, which profilers report).
+template <int... R> struct RopeWidth { static constexpr int value = 32; };
+template <int R> struct RopeWidth<R> { static constexpr int value = R; };
+
+template <int BN, int EPI, int... ROPE_R>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_constant__ CUtensorMap tma, const __grid_constant__ CUtensorMap tmb,
                                                                   const __grid_constant__ CUtensorMap tmc, const __grid_constant__ CUtensorMap tmr,
                                                                   const GemmArgs p) {
@@ -543,10 +548,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           const int n = n0 + g * 64;               // one head of q, k or v (feature order (t nh e), d_head 64)
           const int t3 = n / p.C, head = (n - t3 * p.C) >> 6;
           if (t3 < 2) {
-            // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248).  Columns (2i, 2i+1) pair with (16+2i, 17+2i); the
-            // table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4.
+            // cosine-sim scale + axial RoPE (reference :106-114,187-199,245-248; QkRope).  Columns (2i, 2i+1) pair with (R/2+2i,
+            // R/2+1+2i); the table holds (cos_2i, cos_2i+1, sin_2i, sin_2i+1) per float4, R/4 of them per head.
+            constexpr int RQ = RopeWidth<ROPE_R...>::value / 4;
+            static_assert(RQ * 4 <= 64 && RQ % 4 == 0, "rotated width must be a multiple of 16, at most d_head 64");
             const int64_t tok = (m < p.M ? m : 0) % p.T_tokens;
-            const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * 8 * p.T_tokens + tok;   // [head][i][token]
+            const float4* tb = reinterpret_cast<const float4*>(p.rope) + (int64_t)head * RQ * p.T_tokens + tok;   // [head][i][token]
             tc::f32x2 P[32];
 #pragma unroll
             for (int k = 0; k < 32; ++k) P[k] = tc::pk2(v[2 * k], v[2 * k + 1]);
@@ -558,18 +565,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
               q2 = tc::fma2(P[k + 2], P[k + 2], q2);
               q3 = tc::fma2(P[k + 3], P[k + 3], q3);
             }
-            const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y)) + 1e-6f);
+            const float sc = sqrtf(__ldg(p.qk_scale + head)) * rsqrtf(((q0.x + q0.y) + (q1.x + q1.y)) + ((q2.x + q2.y) + (q3.x + q3.y)) + p.qk_eps);
             const tc::f32x2 sc2 = tc::pk2(sc, sc);
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
+            for (int k = 0; k < RQ; ++k) {
               const float4 cs = __ldg(tb + (int64_t)k * p.T_tokens);
               const tc::f32x2 C = tc::pk2(cs.x, cs.y), S = tc::pk2(cs.z, cs.w);
-              const tc::f32x2 X1 = P[k], X2 = P[8 + k];
+              const tc::f32x2 X1 = P[k], X2 = P[RQ + k];
               P[k] = tc::mul2(tc::fma2(X2, tc::neg2(S), tc::mul2(X1, C)), sc2);
-              P[8 + k] = tc::mul2(tc::fma2(X1, S, tc::mul2(X2, C)), sc2);
+              P[RQ + k] = tc::mul2(tc::fma2(X1, S, tc::mul2(X2, C)), sc2);
             }
 #pragma unroll
-            for (int k = 16; k < 32; ++k) P[k] = tc::mul2(P[k], sc2);
+            for (int k = 2 * RQ; k < 32; ++k) P[k] = tc::mul2(P[k], sc2);
 #pragma unroll
             for (int k = 0; k < 32; ++k) tc::upk2(P[k], v[2 * k], v[2 * k + 1]);
           }
@@ -599,7 +606,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
 #include "tc_ffn_fused.cuh"
 #include "tc_attn_block.cuh"
 
-template <int BN, int EPI>
+template <int BN, int EPI, int... ROPE_R>
 int launch_tc(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) {
   CUtensorMap ta, tb, tcm, tr;
   int rc;
@@ -628,17 +635,17 @@ int launch_tc(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) 
   constexpr size_t smem = gemm_smem<BN, EPI>();
   static_assert(smem <= 227 * 1024, "GEMM shared memory exceeds the 227 KiB opt-in limit");
   static bool opened = false;
-  if ((rc = set_smem_once(gemm_wg_kernel<BN, EPI>, opened, (int)smem))) return rc;
-  KDB_CUDA(launch_pdl(gemm_wg_kernel<BN, EPI>, persistent_grid(ceil_div(p.M, BM) * (p.N / BN)), dim3(GEMM_THREADS), smem, st, ta, tb, tcm, tr, p));
+  if ((rc = set_smem_once(gemm_wg_kernel<BN, EPI, ROPE_R...>, opened, (int)smem))) return rc;
+  KDB_CUDA(launch_pdl(gemm_wg_kernel<BN, EPI, ROPE_R...>, persistent_grid(ceil_div(p.M, BM) * (p.N / BN)), dim3(GEMM_THREADS), smem, st, ta, tb, tcm, tr, p));
   KDB_LAUNCH_CHECK(EPI == EPI_PATCH_OUT ? F_PATCH_OUT : F_GEMM_TC, st);   // (the profiler's per-family bookkeeping only)
   return 0;
 }
 
 // 128-wide tiles whenever N allows: they emit the per-128-channel row statistics of the fused RMSNorm
-template <int EPI>
+template <int EPI, int... ROPE_R>
 int dispatch_bn(const bf16* A, const bf16* W, const GemmArgs& p, cudaStream_t st) {
-  if (p.N % 128 == 0) return launch_tc<128, EPI>(A, W, p, st);
-  return launch_tc<64, EPI>(A, W, p, st);
+  if (p.N % 128 == 0) return launch_tc<128, EPI, ROPE_R...>(A, W, p, st);
+  return launch_tc<64, EPI, ROPE_R...>(A, W, p, st);
 }
 
 bool shape_ok(int64_t M, int N, int K) {
@@ -676,7 +683,7 @@ bool gemm_fits(int64_t M, int N, int K, const GemmEpi& epi) {
     case EPI_SPLIT_LERP:
       return epi.C % 32 == 0 && N == 4 * epi.C;
     case EPI_QKV_ROPE:
-      return N == 3 * epi.C && epi.C % 64 == 0 && epi.nh * 64 == epi.C && epi.rope != nullptr;
+      return N == 3 * epi.C && epi.C % 64 == 0 && epi.nh * 64 == epi.C && epi.rope != nullptr && (epi.rope_r == 32 || epi.rope_r == 64);
     case EPI_PATCH_OUT:   // 48 of 64 columns used; float4 stores of img and loads of x_in
       return N == 64 && epi.W % 4 == 0 && aligned16(epi.img) && (epi.sigma_data <= 0.f || aligned16(epi.x_in));
     default:
@@ -885,7 +892,7 @@ int launch_gemm_tc(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int 
     case EPI_SPLIT_LERP:
       return dispatch_bn<EPI_SPLIT_LERP>(A, W, p, st);
     case EPI_QKV_ROPE:
-      return dispatch_bn<EPI_QKV_ROPE>(A, W, p, st);
+      return epi.rope_r == 64 ? dispatch_bn<EPI_QKV_ROPE, 64>(A, W, p, st) : dispatch_bn<EPI_QKV_ROPE>(A, W, p, st);
     case EPI_PATCH_OUT:
       return launch_tc<64, EPI_PATCH_OUT>(A, W, p, st);
     default:

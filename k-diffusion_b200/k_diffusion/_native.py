@@ -18,8 +18,9 @@ LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 
 PREC_FP32, PREC_BF16, PREC_TF32 = 0, 1, 2
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
+FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -30,7 +31,7 @@ class KdbModelConfig(ctypes.Structure):
         ("n_levels", _i32), ("in_channels", _i32), ("out_channels", _i32), ("patch_h", _i32), ("patch_w", _i32),
         ("mapping_width", _i32), ("mapping_depth", _i32), ("mapping_d_ff", _i32), ("num_classes", _i32), ("mapping_cond_dim", _i32),
         ("width", _i32 * MAX_LEVELS), ("depth", _i32 * MAX_LEVELS), ("d_ff", _i32 * MAX_LEVELS), ("attn_type", _i32 * MAX_LEVELS),
-        ("d_head", _i32 * MAX_LEVELS), ("attn_param", _i32 * MAX_LEVELS),
+        ("d_head", _i32 * MAX_LEVELS), ("attn_param", _i32 * MAX_LEVELS), ("family", _i32),
     ]
 
 
@@ -370,7 +371,7 @@ class EngineCache:
 
 
 class Engine:
-    """Owns one native model handle on one device: a KdbModel for an ImageTransformerDenoiserModelV2 (`_api` "model"), or, in the
+    """Owns one native model handle on one device: a KdbModel for an ImageTransformerDenoiserModelV2 or V1 (`_api` "model"), or, in the
     UNetEngine subclass, a KdbUNet for an ImageDenoiserModelV1 (`_api` "unet").  Both handles take the same calls (create, destroy,
     set_tensor, finalize, cond_stride, workspace_bytes, forward, debug_tap, tap_count) under kdb_<api>_*."""
 
@@ -396,6 +397,7 @@ class Engine:
         cfg.patch_h, cfg.patch_w = spec["patch_size"]
         cfg.mapping_width, cfg.mapping_depth, cfg.mapping_d_ff = spec["mapping_width"], spec["mapping_depth"], spec["mapping_d_ff"]
         cfg.num_classes, cfg.mapping_cond_dim = spec["num_classes"], spec["mapping_cond_dim"]
+        cfg.family = spec.get("family", FAMILY_ITV2)
         for i, lv in enumerate(levels):
             cfg.width[i], cfg.depth[i], cfg.d_ff[i] = lv["width"], lv["depth"], lv["d_ff"]
             cfg.attn_type[i] = _ATTN_CODE[lv["attn"]]

@@ -1,9 +1,10 @@
 """Config loading / model factory for the path in scope (reference: k_diffusion/config.py:23-231).
 
 Accepts the reference's JSON files, dicts, and `.safetensors` checkpoints carrying the config in
-their metadata.  `image_transformer_v2` and `image_v1` can be built; `image_transformer_v1` is out of scope.
+their metadata.  `image_transformer_v2`, `image_transformer_v1` and `image_v1` can be built.
 """
 import json
+import math
 from functools import partial
 from pathlib import Path
 
@@ -17,6 +18,7 @@ _V1_OPT_DEFAULTS = dict(type='adamw', lr=1e-4, betas=[0.95, 0.999], eps=1e-6, we
 # keys make_model needs that have no default: the reference fails on them later, in make_model (KeyError)
 _V1_REQUIRED = ('input_channels', 'input_size', 'mapping_out', 'depths', 'channels', 'self_attn_depths')
 _V2_OPT_DEFAULTS = dict(type='adamw', lr=5e-4, betas=[0.9, 0.99], eps=1e-8, weight_decay=1e-4)
+_ITV1_MODEL_DEFAULTS = dict(d_ff=0, augment_wrapper=False, skip_stages=0, has_variance=False)
 _COMMON_DEFAULTS = {
     'model': dict(sigma_data=1., dropout_rate=0., augment_prob=0., loss_config='karras', loss_weighting='karras', loss_scales=1),
     'dataset': dict(type='imagefolder', num_classes=0, cond_dropout_rate=0.1),
@@ -34,6 +36,17 @@ def _overlay(base, head):
     for k, v in head.items():
         out[k] = _overlay(base[k], v) if k in base else v
     return out
+
+
+def round_to_power_of_two(x, tol):
+    """The nearest multiple of 2**k to x for the largest k < ceil(log2 x) that lands within relative `tol` of x; x rounded to an integer
+    when none does (the d_ff default of image_transformer_v1 configs, reference config.py:11-20)."""
+    for k in range(math.ceil(math.log2(x)) - 1, -1, -1):
+        step = 2 ** k
+        candidate = round(x / step) * step
+        if abs(candidate - x) <= tol * abs(x):
+            return candidate
+    return round(x)
 
 
 def _read(path_or_dict):
@@ -55,8 +68,19 @@ def load_config(path_or_dict):
         if missing:
             raise ValueError(f'image_v1 config lacks {missing} (make_model needs them and they have no default)')
         return _overlay(_COMMON_DEFAULTS, _overlay({'model': _V1_MODEL_DEFAULTS, 'optimizer': _V1_OPT_DEFAULTS}, config))
+    if kind == 'image_transformer_v1':
+        config = _overlay({'model': _ITV1_MODEL_DEFAULTS, 'optimizer': _V2_OPT_DEFAULTS}, config)
+        m = config['model']
+        if m['augment_wrapper']:
+            raise ValueError('image_transformer_v1 with augment_wrapper: the wrapper passes mapping_cond, which the v1 model does not take')
+        if m['width'] % 64 != 0:
+            raise ValueError(f"image_transformer_v1 width {m['width']} is not a multiple of its d_head 64")
+        if not m['d_ff']:
+            m['d_ff'] = round_to_power_of_two(m['width'] * 8 / 3, tol=0.05)
+        return _overlay(_COMMON_DEFAULTS, config)
     if kind != 'image_transformer_v2':
-        raise ValueError(f'model type {kind!r} is out of scope for the H100 sampling path (image_transformer_v2 and image_v1 only)')
+        raise ValueError(f'model type {kind!r} is out of scope for the H100 sampling path (image_transformer_v2, image_transformer_v1 and '
+                         'image_v1 only)')
     config = _overlay({'model': _V2_MODEL_DEFAULTS, 'optimizer': _V2_OPT_DEFAULTS}, config)
     m = config['model']
     n = len(m['widths'])
@@ -97,6 +121,13 @@ def make_model(config):
             patch_size=m['patch_size'], dropout_rate=m['dropout_rate'], mapping_cond_dim=m['mapping_cond_dim'] + (9 if m['augment_wrapper'] else 0),
             unet_cond_dim=m['unet_cond_dim'], cross_cond_dim=m['cross_cond_dim'], skip_stages=m['skip_stages'], has_variance=m['has_variance'])
         return augmentation.KarrasAugmentWrapper(model) if m['augment_wrapper'] else model
+    if m['type'] == 'image_transformer_v1':
+        if m.get('augment_wrapper'):
+            raise ValueError('image_transformer_v1 with augment_wrapper: the wrapper passes mapping_cond, which the v1 model does not take')
+        return models.ImageTransformerDenoiserModelV1(
+            n_layers=m['depth'], d_model=m['width'], d_ff=m['d_ff'], in_features=m['input_channels'], out_features=m['input_channels'],
+            patch_size=m['patch_size'], num_classes=num_classes + 1 if num_classes else 0, dropout=m['dropout_rate'],
+            sigma_data=m['sigma_data'])
     if m['type'] != 'image_transformer_v2':
         raise ValueError(f'unsupported model type {m["type"]}')
     v2 = models.image_transformer_v2

@@ -127,44 +127,16 @@ def _level(spec, cond_width):
     return nn.ModuleList([_layer(spec, cond_width) for _ in range(spec.depth)])
 
 
-class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
-    def __init__(self, levels, mapping, in_channels, out_channels, patch_size, num_classes=0, mapping_cond_dim=0):
-        super().__init__()
-        levels = list(levels)
-        patch_size = tuple(patch_size) if not isinstance(patch_size, int) else (patch_size, patch_size)
-        self.num_classes = num_classes
-        self.levels, self.mapping_spec = levels, mapping
-        self.in_channels, self.out_channels, self.patch_size, self.mapping_cond_dim = in_channels, out_channels, patch_size, mapping_cond_dim
-        for spec in levels:
-            _attn_kind(spec.self_attn)           # raises ValueError on unsupported specs, like the reference (:693)
-        mw = mapping.width
-        w0 = levels[0].width
-        n_patch = patch_size[0] * patch_size[1]
+class TransformerEngineModel(_native.EngineCache, nn.Module):
+    """What the transformer models share on top of their parameters: the native engine (a KdbModel of `family`), the precision, and
+    the evaluation entry points (the raw model, the Karras-preconditioned denoiser, their JVP / VJP, torch.autograd through x).  A
+    subclass sets `levels`, `mapping_spec`, `in_channels`, `out_channels`, `patch_size`, `num_classes`, `mapping_cond_dim`,
+    `class_emb`, `mapping_cond_in_proj`, `precision`, `_engines` and the parameter tree whose state-dict keys the engine of its family
+    binds."""
 
-        self.patch_in = _Node(proj=_linear(w0, in_channels * n_patch))
-        self.time_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 1)))            # layers.FourierFeatures(1, mw)
-        self.time_in_proj = _linear(mw, mw)
-        self.aug_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 9)))             # layers.FourierFeatures(9, mw)
-        self.aug_in_proj = _linear(mw, mw)
-        self.class_emb = _Node(weight=torch.randn(num_classes, mw)) if num_classes else None
-        self.mapping_cond_in_proj = _linear(mw, mapping_cond_dim) if mapping_cond_dim else None
-        self.mapping = _Node(
-            in_norm=_Node(scale=torch.ones(mw)),
-            blocks=nn.ModuleList([
-                _Node(norm=_Node(scale=torch.ones(mw)), up_proj=_linear(mapping.d_ff * 2, mw), down_proj=_linear(mw, mapping.d_ff, zero=True))
-                for _ in range(mapping.depth)]),
-            out_norm=_Node(scale=torch.ones(mw)),
-        )
-        self.down_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
-        self.up_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
-        self.mid_level = _level(levels[-1], mw)
-        self.merges = nn.ModuleList([_Node(proj=_linear(b.width, a.width * 4)) for a, b in zip(levels[:-1], levels[1:])])
-        self.splits = nn.ModuleList([_Node(proj=_linear(a.width * 4, b.width), fac=torch.ones(1) * 0.5) for a, b in zip(levels[:-1], levels[1:])])
-        self.out_norm = _Node(scale=torch.ones(w0))
-        self.patch_out = _Node(proj=_linear(out_channels * n_patch, w0, zero=True))
-
-        self.precision = None        # None -> flags.resolve_precision ("auto" unless KDB200_PRECISION is set)
-        self._engines = {}
+    family = _native.FAMILY_ITV2
+    kind = "image_transformer_v2"
+    dtype_key = "patch_in.proj.weight"      # the parameter whose dtype picks the "auto" precision
 
     # ------------------------------------------------------------------ engine plumbing
     def engine_spec(self):
@@ -174,7 +146,7 @@ class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
             lv.append(dict(width=s.width, depth=s.depth, d_ff=s.d_ff, attn=kind, d_head=getattr(s.self_attn, "d_head", 0), attn_param=param))
         return dict(levels=lv, in_channels=self.in_channels, out_channels=self.out_channels, patch_size=self.patch_size,
                     mapping_width=self.mapping_spec.width, mapping_depth=self.mapping_spec.depth, mapping_d_ff=self.mapping_spec.d_ff,
-                    num_classes=self.num_classes, mapping_cond_dim=self.mapping_cond_dim)
+                    num_classes=self.num_classes, mapping_cond_dim=self.mapping_cond_dim, family=self.family)
 
     def engine(self):
         """Native engine with the current parameters bound (rebinds only after the parameters changed)."""
@@ -190,9 +162,9 @@ class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
         return self
 
     def resolved_precision(self):
-        p = flags.resolve_precision(self.precision, self.patch_in.proj.weight.dtype)
+        p = flags.resolve_precision(self.precision, self.get_parameter(self.dtype_key).dtype)
         if p == "tf32":
-            raise ValueError("the image_transformer_v2 engine runs at fp32 or bf16 (tf32 is built for the image_v1 U-Net only)")
+            raise ValueError(f"the {self.kind} engine runs at fp32 or bf16 (tf32 is built for the image_v1 U-Net only)")
         return _native.PREC_BF16 if p == "bf16" else _native.PREC_FP32
 
     def param_groups(self, *args, **kwargs):
@@ -247,10 +219,6 @@ class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
             return res if x.dtype == torch.float32 else tuple(r.to(x.dtype) for r in res)
         return res if x.dtype == torch.float32 else res.to(x.dtype)
 
-    def forward(self, x, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
-        """F(x, sigma): the raw inner model (reference :721-762)."""
-        return self._run(x, sigma, 0.0, aug_cond, class_cond, mapping_cond)
-
     def denoise(self, x, sigma, sigma_data, aug_cond=None, class_cond=None, mapping_cond=None, out=None):
         """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
         return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, out=out)
@@ -274,6 +242,50 @@ class ImageTransformerDenoiserModelV2(_native.EngineCache, nn.Module):
         """(D(x, sigma), u^T J_D(x)) of the Karras-preconditioned evaluation, u^T J_D = c_skip u + c_in J_F(c_in x)^T (c_out u), in one
         engine call.  Always runs on the exact fp32 path, whatever `set_precision` selected."""
         return self._run(x, sigma, float(sigma_data), aug_cond, class_cond, mapping_cond, cotangent=u)
+
+
+class ImageTransformerDenoiserModelV2(TransformerEngineModel):
+    def __init__(self, levels, mapping, in_channels, out_channels, patch_size, num_classes=0, mapping_cond_dim=0):
+        super().__init__()
+        levels = list(levels)
+        patch_size = tuple(patch_size) if not isinstance(patch_size, int) else (patch_size, patch_size)
+        self.num_classes = num_classes
+        self.levels, self.mapping_spec = levels, mapping
+        self.in_channels, self.out_channels, self.patch_size, self.mapping_cond_dim = in_channels, out_channels, patch_size, mapping_cond_dim
+        for spec in levels:
+            _attn_kind(spec.self_attn)           # raises ValueError on unsupported specs, like the reference (:693)
+        mw = mapping.width
+        w0 = levels[0].width
+        n_patch = patch_size[0] * patch_size[1]
+
+        self.patch_in = _Node(proj=_linear(w0, in_channels * n_patch))
+        self.time_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 1)))            # layers.FourierFeatures(1, mw)
+        self.time_in_proj = _linear(mw, mw)
+        self.aug_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 9)))             # layers.FourierFeatures(9, mw)
+        self.aug_in_proj = _linear(mw, mw)
+        self.class_emb = _Node(weight=torch.randn(num_classes, mw)) if num_classes else None
+        self.mapping_cond_in_proj = _linear(mw, mapping_cond_dim) if mapping_cond_dim else None
+        self.mapping = _Node(
+            in_norm=_Node(scale=torch.ones(mw)),
+            blocks=nn.ModuleList([
+                _Node(norm=_Node(scale=torch.ones(mw)), up_proj=_linear(mapping.d_ff * 2, mw), down_proj=_linear(mw, mapping.d_ff, zero=True))
+                for _ in range(mapping.depth)]),
+            out_norm=_Node(scale=torch.ones(mw)),
+        )
+        self.down_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
+        self.up_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
+        self.mid_level = _level(levels[-1], mw)
+        self.merges = nn.ModuleList([_Node(proj=_linear(b.width, a.width * 4)) for a, b in zip(levels[:-1], levels[1:])])
+        self.splits = nn.ModuleList([_Node(proj=_linear(a.width * 4, b.width), fac=torch.ones(1) * 0.5) for a, b in zip(levels[:-1], levels[1:])])
+        self.out_norm = _Node(scale=torch.ones(w0))
+        self.patch_out = _Node(proj=_linear(out_channels * n_patch, w0, zero=True))
+
+        self.precision = None        # None -> flags.resolve_precision ("auto" unless KDB200_PRECISION is set)
+        self._engines = {}
+
+    def forward(self, x, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
+        """F(x, sigma): the raw inner model (reference :721-762)."""
+        return self._run(x, sigma, 0.0, aug_cond, class_cond, mapping_cond)
 
 
 class _NativeEval(torch.autograd.Function):

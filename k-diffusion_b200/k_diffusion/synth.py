@@ -35,6 +35,11 @@ def synth_tensor(key, shape, seed=0):
         return torch.randn(shape, generator=g) * ZERO_INIT_STD
     if key.endswith("self_attn.scale"):
         return 5.0 + 10.0 * torch.rand(shape, generator=g)          # cosine-sim temperature, init 10
+    # image_transformer_v1 (reference models/image_transformer_v1.py:108-128, axial_rope.py:86-93)
+    if key.endswith("qk_norm.scale"):
+        return 2.5 + 2.8 * torch.rand(shape, generator=g)           # log temperature, init ln 10; above ln 100 = 4.61 is clamped
+    if key.endswith(("pos_emb.freqs_h", "pos_emb.freqs_w")):
+        return math.log(math.pi) + math.log(5.0) * torch.rand(shape, generator=g)   # log frequencies, init log-spaced pi .. 5 pi
     if key.endswith("fac"):
         return 0.3 + 0.4 * torch.rand(shape, generator=g)           # TokenSplit lerp factor, init 0.5
     if key.endswith(".scale"):
