@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 15
+#define KDB_ABI_VERSION 16
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -134,10 +134,10 @@ int kdb_noise_brownian(float* out, const int64_t* seeds, int batch, int64_t per_
 #define KDB_MAX_LEVELS 8
 
 enum { KDB_ATTN_NONE = 0, KDB_ATTN_GLOBAL = 1, KDB_ATTN_NEIGHBORHOOD = 2, KDB_ATTN_SHIFTED_WINDOW = 3 };
-/* arithmetic of the token stream / GEMM operands.  KDB_PREC_TF32 (the image_v1 U-Net only; every kdb_model_* entry point returns
- * KDB_ERR_UNSUPPORTED for it): convolution and attention operands rounded to tf32, fp32 accumulation, fp32 activations, weights and
- * outputs. */
-enum { KDB_PREC_FP32 = 0, KDB_PREC_BF16 = 1, KDB_PREC_TF32 = 2 };
+/* arithmetic of the token stream / GEMM operands.  KDB_PREC_TF32 and KDB_PREC_FP16 (the image_v1 U-Net only; every kdb_model_* entry
+ * point returns KDB_ERR_UNSUPPORTED for them): convolution and attention operands rounded to tf32 / fp16, fp32 accumulation, fp32
+ * activations and outputs.  fp16 rounding is to nearest even without saturation: an operand of magnitude >= 65520 becomes +-inf. */
+enum { KDB_PREC_FP32 = 0, KDB_PREC_BF16 = 1, KDB_PREC_TF32 = 2, KDB_PREC_FP16 = 3 };
 /* KdbModelConfig.family.  KDB_FAMILY_ITV1: image_transformer_v1 with n_levels 1, width = depth's d_model, d_ff, attn_type
  * KDB_ATTN_GLOBAL, d_head 64, mapping_width = d_model, mapping_depth 2, mapping_d_ff = d_ff, mapping_cond_dim 0.  Its keys are v1's own
  * ("blocks.<i>.self_attn.qk_norm.scale", "in_proj.weight", ...); kdb_model_finalize derives the engine's tables from them: qkv_proj
@@ -292,7 +292,8 @@ int64_t kdb_unet_cond_stride(const KdbUNet* m);
 int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, float* cond_out,
                           void* stream);
 
-/* Workspace of one forward in bytes, the same at KDB_PREC_FP32 and KDB_PREC_TF32; KDB_ERR_UNSUPPORTED for any other precision. */
+/* Workspace of one forward in bytes, the same at KDB_PREC_FP32, KDB_PREC_TF32 and KDB_PREC_FP16; KDB_ERR_UNSUPPORTED for any other
+ * precision. */
 int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int height, int width);
 
 /* One evaluation on x [B, in_channels, H, W] -> out of the same shape, as kdb_model_forward: sigma_data > 0 gives the
@@ -300,7 +301,8 @@ int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int
  * KDB_PREC_FP32: every kernel in fp32.  KDB_PREC_TF32: every convolution (the ResConvBlock 3x3 convs and 1x1 skip, qkv_proj and
  * out_proj) on the tensor cores (kdb_unet_conv_tf32) with weights rounded to tf32 by finalize, and self-attention of d_head 64 on the
  * tensor cores (kdb_attention at KDB_PREC_TF32; other head sizes keep the fp32 kernel); AdaGN, resampling, patch in / out and the
- * conditioning stay fp32.  Any other precision: KDB_ERR_UNSUPPORTED.  Every level but the innermost needs an even grid and every
+ * conditioning stay fp32.  KDB_PREC_FP16: the same with fp16 operands (kdb_unet_conv_fp16 on fp16 weight copies made by finalize,
+ * kdb_attention at KDB_PREC_FP16).  Any other precision: KDB_ERR_UNSUPPORTED.  Every level but the innermost needs an even grid and every
  * level at least 2x2.  Allocates nothing and synchronises nothing, so it can be captured into a CUDA graph; a workspace shorter
  * than kdb_unet_workspace_bytes returns KDB_ERR_WORKSPACE.  Deterministic (no atomics). */
 int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
@@ -354,7 +356,8 @@ int kdb_attn_block_bf16(void* x_bf16, const void* w_qkv_bf16, const void* w_out_
  * softmax's fixed shift (one pass over the keys, no row maximum); NULL keeps the exact two-pass row-maximum kernels.
  * KDB_PREC_TF32 (fast 0, KDB_ATTN_GLOBAL, d_head 64, fp32 tensors, 1/sqrt(d_head) already in q): the image_v1 U-Net's attention
  * (layers.py:181-200) on the tensor cores, q, k, v and the probabilities truncated to tf32, fp32 accumulation, running-maximum softmax;
- * any other attention type, head size or `fast` at that precision is KDB_ERR_UNSUPPORTED. */
+ * any other attention type, head size or `fast` at that precision is KDB_ERR_UNSUPPORTED.  KDB_PREC_FP16: the same with q, k, v and the
+ * probabilities rounded to fp16 (nearest even); scores, softmax and the sum l of the rounded probabilities stay fp32. */
 int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch, int h, int w, int n_heads, int d_head,
                   int attn_type, int attn_param, int shift, const float* logit_bound, void* stream);
 
@@ -384,6 +387,14 @@ int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const floa
  * wanting round-to-nearest weights rounds them first, as kdb_unet_finalize does -- and accumulate in fp32; bias and residual are added
  * in fp32.  No grid-row limit on batch * h * w. */
 int kdb_unet_conv_tf32(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1,
+                       int rc1, const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
+
+/* The same convolution and arguments with fp16 operands (wgmma, the kernel kdb_unet_forward runs at KDB_PREC_FP16).  w_tapmajor_f16 is
+ * the tap-major weight in fp16, [n_out, ksize*ksize, ld] with ld = c1 + c2 rounded up to a multiple of 8 (the padding channels are
+ * never read), as kdb_unet_finalize rounds it (nearest even).  The activations are rounded to the nearest fp16 (ties to even) inside
+ * the kernel, without saturation: an input of magnitude >= 65520 becomes +-inf there and reaches the outputs it feeds as inf or NaN.
+ * Products accumulate in fp32; bias and residual are added in fp32.  No grid-row limit on batch * h * w. */
+int kdb_unet_conv_fp16(const float* in1, int c1, const float* in2, int c2, const void* w_tapmajor_f16, const float* bias, const float* r1,
                        int rc1, const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
 
 #ifdef __cplusplus

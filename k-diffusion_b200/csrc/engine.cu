@@ -972,8 +972,8 @@ int kdb_model_conditioning(KdbModel* m, int rows, const float* sigma, const floa
 
 size_t kdb_model_workspace_bytes(const KdbModel* m, int precision, int batch, int height, int width) {
   if (!m || batch <= 0 || height <= 0 || width <= 0) return 0;
-  if (precision == KDB_PREC_TF32) {
-    set_error("model_workspace_bytes: the tf32 precision is built for the image_v1 U-Net only");
+  if (precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16) {
+    set_error("model_workspace_bytes: the tf32 and fp16 precisions are built for the image_v1 U-Net only");
     return 0;
   }
   Workspace ws;
@@ -1016,7 +1016,8 @@ int kdb_model_forward(KdbModel* m, int precision, int batch, int height, int wid
                       size_t workspace_bytes, void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward: model not finalized");
   KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward: NULL argument");
-  KDB_REQUIRE(precision != KDB_PREC_TF32, KDB_ERR_UNSUPPORTED, "forward: the tf32 precision is built for the image_v1 U-Net only");
+  KDB_REQUIRE(precision != KDB_PREC_TF32 && precision != KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
+              "forward: the tf32 and fp16 precisions are built for the image_v1 U-Net only");
   KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_BF16, KDB_ERR_BAD_ARG, "forward: bad precision %d", precision);
   int rc = check_image(m, "forward", height, width, sigma_data);
   if (rc) return rc;
@@ -1080,6 +1081,10 @@ int kdb_attention(int precision, int fast, const void* qkv, void* out, int batch
   if (precision == KDB_PREC_TF32) {   // the image_v1 U-Net's global attention on fp32 tensors (q pre-scaled), d_head 64
     KDB_REQUIRE(attn_type == KDB_ATTN_GLOBAL && !fast, KDB_ERR_UNSUPPORTED, "attention: tf32 is built for global attention only");
     return launch_unet_attn_tf32(static_cast<const float*>(qkv), static_cast<float*>(out), batch, h * w, n_heads, d_head, st);
+  }
+  if (precision == KDB_PREC_FP16) {   // the same at fp16
+    KDB_REQUIRE(attn_type == KDB_ATTN_GLOBAL && !fast, KDB_ERR_UNSUPPORTED, "attention: fp16 is built for global attention only");
+    return launch_unet_attn_fp16(static_cast<const float*>(qkv), static_cast<float*>(out), batch, h * w, n_heads, d_head, st);
   }
   if (precision == KDB_PREC_FP32) {
     KDB_REQUIRE(!fast, KDB_ERR_UNSUPPORTED, "attention: tensor-core path is bf16 only");

@@ -221,6 +221,17 @@ __device__ __forceinline__ void wgmma_128_rs(float (&d)[64], const uint32_t (&a)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 
+// the same with fp16 operands: A a m64k16 fp16 fragment (4 x f16x2, the lower k index in the low half), B fp16 K-major
+__device__ __forceinline__ void wgmma_128_rs_f16(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+
 // D[64 x 64] (+)= A[registers: m64k16 bf16 fragment] * B[smem]; TB = 1: B is MN-major (N contiguous)
 template <int TB>
 __device__ __forceinline__ void wgmma_64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
@@ -318,6 +329,10 @@ __device__ __forceinline__ f32x2 geglu2(f32x2 half_val, f32x2 gate) {
 // inside the swizzle atom is +2 on the descriptor.
 __device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+// 64B swizzle: K-major tile whose rows are 64 bytes (32 fp16) wide, 8-row groups 512 B apart; a K step of 16 fp16 = 32 B is +2.
+__device__ __forceinline__ uint64_t smem_desc_k_sw64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (32ull << 32) | (2ull << 62);
 }
 // MN-major operand tile (rows of the *K* index are 128 B = 64 bf16 of the MN index): 64-element MN atoms LBO apart, 8-row K groups SBO apart.
 __device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -495,6 +510,9 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
                    const uint32_t* box);
 // the same for fp32 elements (a 128-byte swizzle row is 32 of them); out-of-bounds box elements read as zeros
 int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box);
+// fp16 elements with a 64-byte swizzle (a 32-element row is one 64-byte swizzle row); out-of-bounds box elements read as zeros
+int make_tmap_f16_sw64(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                       const uint32_t* box);
 // [B, h, w, C] bf16 tokens as the 4-D map (C, w, h, B) with box {box_c, box_w, box_h, 1}
 int make_tmap_tokens(CUtensorMap* out, const void* base, uint64_t C, int B, int h, int w, uint32_t box_c, uint32_t box_w, uint32_t box_h);
 

@@ -31,7 +31,7 @@ static EncodeTiledFn encode_fn() {
 }
 
 static int make_tmap(CUtensorMap* out, CUtensorMapDataType type, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box) {
+                     const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = encode_fn();
   KDB_REQUIRE(fn != nullptr, KDB_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled not available from this driver");
   cuuint64_t gd[5];
@@ -44,8 +44,7 @@ static int make_tmap(CUtensorMap* out, CUtensorMapDataType type, const void* bas
     if (i > 0) gs[i - 1] = strides_bytes[i - 1];
   }
   CUresult r = fn(out, type, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   KDB_REQUIRE(r == CUDA_SUCCESS, KDB_ERR_BAD_ARG, "cuTensorMapEncodeTiled failed with CUresult %d (rank %d, dim0 %llu, box0 %u)", (int)r,
               rank, (unsigned long long)dims[0], box[0]);
   return 0;
@@ -57,6 +56,10 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 
 int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box);
+}
+
+int make_tmap_f16_sw64(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 int make_tmap_tokens(CUtensorMap* out, const void* base, uint64_t C, int B, int h, int w, uint32_t box_c, uint32_t box_w, uint32_t box_h) {

@@ -1,9 +1,10 @@
-// unet_engine.cu -- host-side execution plan of the image_v1 U-Net denoiser, on the exact fp32 path or with its convolutions at tf32
+// unet_engine.cu -- host-side execution plan of the image_v1 U-Net denoiser, on the exact fp32 path or with its convolutions and
+// attention at tf32 or fp16
 // (reference: k_diffusion/models/image_v1.py, layers.py:116-313, augmentation.py:92-104).
 //
 // Like the transformer engine, it owns no activations: the caller passes one workspace and the forward carves it.  Weights are
 // borrowed device pointers keyed by the state-dict names of ImageDenoiserModelV1; kdb_unet_finalize builds the derived tables
-// (tap-major convolution weights and their tf32-rounded copies, the attention scale folded into qkv_proj's q rows, the concatenated
+// (tap-major convolution weights and their tf32- and fp16-rounded copies, the attention scale folded into qkv_proj's q rows, the concatenated
 // AdaGN mappers).
 #include <algorithm>
 #include <cmath>
@@ -17,14 +18,21 @@ namespace {
 
 enum ModKind { M_RES = 0, M_ATTN, M_DOWN, M_UP, M_CONCAT };
 
+// the derived (owned) copies of one conv weight: tap-major fp32, and that rounded to tf32 and to fp16
+struct ConvW {
+  const float* f32 = nullptr;
+  const float* tf32 = nullptr;
+  const __half* f16 = nullptr;
+};
+
 // One module of the U-Net in execution order.  M_CONCAT starts a UBlock that receives the matching skip.
 struct UMod {
   int kind = M_RES, level = 0;
   std::string tap;
   int c_in = 0, c_mid = 0, c_out = 0;
   int groups1 = 1, groups2 = 1, ada1 = 0, ada2 = 0;
-  const float *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr, *skip_w = nullptr;   // derived (owned) weights
-  const float *w1_tf32 = nullptr, *w2_tf32 = nullptr, *skip_w_tf32 = nullptr;                  // ... rounded to tf32
+  ConvW w1, w2, skip_w;
+  const float *b1 = nullptr, *b2 = nullptr;   // derived (owned) biases
   const float *mapper1_w = nullptr, *mapper1_b = nullptr, *mapper2_w = nullptr, *mapper2_b = nullptr;
   bool to_skip = false;           // the last module of a DBlock writes the level's skip buffer
 };
@@ -44,18 +52,20 @@ using namespace kdb;
 namespace {
 
 // owned tap-major copy of a conv weight [N, C, ks, ks], the first scaled_rows output rows times scale, and that copy rounded to tf32
-int conv_weight(KdbUNet* m, const std::string& key, int N, int C, int ks, const float** out, const float** out_tf32, cudaStream_t st,
-                int scaled_rows = 0, float scale = 1.f) {
+// and to fp16
+int conv_weight(KdbUNet* m, const std::string& key, int N, int C, int ks, ConvW* out, cudaStream_t st, int scaled_rows = 0,
+                float scale = 1.f) {
   const float* src;
   GET(key, &src, N, C, ks, ks);
   const size_t n = (size_t)N * C * ks * ks;
   float *dst = nullptr, *dst_tf32 = nullptr;
+  __half* dst_f16 = nullptr;
   int rc = m->alloc(&dst, n);
-  if (rc || (rc = m->alloc(&dst_tf32, n)) || (rc = launch_unet_reorder_conv_weight(src, dst, N, C, ks, scaled_rows, scale, st)) ||
-      (rc = launch_unet_round_tf32(dst, dst_tf32, (int64_t)n, st)))
+  if (rc || (rc = m->alloc(&dst_tf32, n)) || (rc = m->alloc(&dst_f16, (size_t)N * ks * ks * f16_weight_ld(C))) ||
+      (rc = launch_unet_reorder_conv_weight(src, dst, N, C, ks, scaled_rows, scale, st)) ||
+      (rc = launch_unet_round_tf32(dst, dst_tf32, (int64_t)n, st)) || (rc = launch_unet_round_f16(dst, dst_f16, (int64_t)N * ks * ks, C, st)))
     return rc;
-  *out = dst;
-  *out_tf32 = dst_tf32;
+  *out = ConvW{dst, dst_tf32, dst_f16};
   return 0;
 }
 
@@ -82,12 +92,12 @@ int mapper(KdbUNet* m, const std::string& prefix, int C, const float** w, const 
 int plan_res(KdbUNet* m, const std::string& p, UMod& u, cudaStream_t st) {
   int rc;
   if ((rc = mapper(m, p + "main.0.", u.c_in, &u.mapper1_w, &u.mapper1_b, &u.ada1))) return rc;
-  if ((rc = conv_weight(m, p + "main.2.weight", u.c_mid, u.c_in, 3, &u.w1, &u.w1_tf32, st))) return rc;
+  if ((rc = conv_weight(m, p + "main.2.weight", u.c_mid, u.c_in, 3, &u.w1, st))) return rc;
   if ((rc = bias_copy(m, p + "main.2.bias", u.c_mid, &u.b1, st))) return rc;
   if ((rc = mapper(m, p + "main.4.", u.c_mid, &u.mapper2_w, &u.mapper2_b, &u.ada2))) return rc;
-  if ((rc = conv_weight(m, p + "main.6.weight", u.c_out, u.c_mid, 3, &u.w2, &u.w2_tf32, st))) return rc;
+  if ((rc = conv_weight(m, p + "main.6.weight", u.c_out, u.c_mid, 3, &u.w2, st))) return rc;
   if ((rc = bias_copy(m, p + "main.6.bias", u.c_out, &u.b2, st))) return rc;
-  if (u.c_in != u.c_out && (rc = conv_weight(m, p + "skip.weight", u.c_out, u.c_in, 1, &u.skip_w, &u.skip_w_tf32, st))) return rc;
+  if (u.c_in != u.c_out && (rc = conv_weight(m, p + "skip.weight", u.c_out, u.c_in, 1, &u.skip_w, st))) return rc;
   u.groups1 = std::max(1, u.c_in / 32);
   u.groups2 = std::max(1, u.c_mid / 32);
   return 0;
@@ -99,9 +109,9 @@ int plan_attn(KdbUNet* m, const std::string& p, UMod& u, cudaStream_t st) {
   const int C = u.c_out, nh = std::max(1, C / 64);
   const float scale = 1.f / std::sqrt((float)(C / nh));
   if ((rc = mapper(m, p + "norm_in.", C, &u.mapper1_w, &u.mapper1_b, &u.ada1))) return rc;
-  if ((rc = conv_weight(m, p + "qkv_proj.weight", 3 * C, C, 1, &u.w1, &u.w1_tf32, st, C, scale))) return rc;
+  if ((rc = conv_weight(m, p + "qkv_proj.weight", 3 * C, C, 1, &u.w1, st, C, scale))) return rc;
   if ((rc = bias_copy(m, p + "qkv_proj.bias", 3 * C, &u.b1, st, C, scale))) return rc;
-  if ((rc = conv_weight(m, p + "out_proj.weight", C, C, 1, &u.w2, &u.w2_tf32, st))) return rc;
+  if ((rc = conv_weight(m, p + "out_proj.weight", C, C, 1, &u.w2, st))) return rc;
   if ((rc = bias_copy(m, p + "out_proj.bias", C, &u.b2, st))) return rc;
   u.groups1 = std::max(1, C / 32);
   return 0;
@@ -183,13 +193,14 @@ struct Src {
   int c2 = 0;
 };
 
-// a convolution at the forward's precision: `w` the fp32 weight, `w_tf32` its rounded copy
-int conv(int prec, ConvArgs a, const float* w, const float* w_tf32, int ks, cudaStream_t st) {
+// a convolution at the forward's precision, on the copy of its weight made for that precision
+int conv(int prec, ConvArgs a, const ConvW& w, int ks, cudaStream_t st) {
+  if (prec == KDB_PREC_FP16) return launch_unet_conv_fp16(a, w.f16, ks, st);
   if (prec == KDB_PREC_TF32) {
-    a.w = w_tf32;
+    a.w = w.tf32;
     return launch_unet_conv_tf32(a, ks, st);
   }
-  a.w = w;
+  a.w = w.f32;
   return launch_unet_conv(a, ks, st);
 }
 
@@ -199,21 +210,21 @@ int run_res(int prec, const UMod& u, const Src& in, float* out, UWs& ws, int B, 
   ConvArgs a;
   a.B = B, a.H = h, a.W = w;
   a.in1 = ws.n1, a.c1 = u.c_in, a.bias = u.b1, a.out = ws.n2, a.N = u.c_mid;
-  if ((rc = conv(prec, a, u.w1, u.w1_tf32, 3, st))) return rc;
+  if ((rc = conv(prec, a, u.w1, 3, st))) return rc;
   if ((rc = launch_unet_adagn(ws.n2, u.c_mid, nullptr, 0, ws.n1, cond, cbs, u.ada2, u.groups2, true, B, h * w, st))) return rc;
   ConvArgs c2;
   c2.B = B, c2.H = h, c2.W = w;
-  if (u.skip_w != nullptr) {
+  if (u.skip_w.f32 != nullptr) {
     ConvArgs s;
     s.B = B, s.H = h, s.W = w;
     s.in1 = in.p1, s.c1 = in.c1, s.in2 = in.p2, s.c2 = in.c2, s.out = ws.s, s.N = u.c_out;
-    if ((rc = conv(prec, s, u.skip_w, u.skip_w_tf32, 1, st))) return rc;
+    if ((rc = conv(prec, s, u.skip_w, 1, st))) return rc;
     c2.r1 = ws.s, c2.rc1 = u.c_out;
   } else {
     c2.r1 = in.p1, c2.rc1 = in.c1, c2.r2 = in.p2;
   }
   c2.in1 = ws.n1, c2.c1 = u.c_mid, c2.bias = u.b2, c2.out = out, c2.N = u.c_out;
-  return conv(prec, c2, u.w2, u.w2_tf32, 3, st);
+  return conv(prec, c2, u.w2, 3, st);
 }
 
 int run_attn(int prec, const UMod& u, const float* x, float* out, UWs& ws, int B, int h, int w, const float* cond, int64_t cbs, cudaStream_t st) {
@@ -223,17 +234,20 @@ int run_attn(int prec, const UMod& u, const float* x, float* out, UWs& ws, int B
   ConvArgs q;
   q.B = B, q.H = h, q.W = w;
   q.in1 = ws.n1, q.c1 = C, q.bias = u.b1, q.out = ws.qkv, q.N = 3 * C;
-  if ((rc = conv(prec, q, u.w1, u.w1_tf32, 1, st))) return rc;
-  // at tf32 the tensor-core attention takes the head size it is built for (64, that of every reference config); others keep attn_generic
-  if (prec == KDB_PREC_TF32 && unet_attn_tf32_supported(C / nh))
+  if ((rc = conv(prec, q, u.w1, 1, st))) return rc;
+  // at tf32 and fp16 the tensor-core attention takes the head size it is built for (64, that of every reference config); others keep
+  // attn_generic
+  if (prec == KDB_PREC_TF32 && unet_attn_tc_supported(C / nh))
     rc = launch_unet_attn_tf32(ws.qkv, ws.ao, B, h * w, nh, C / nh, st);
+  else if (prec == KDB_PREC_FP16 && unet_attn_tc_supported(C / nh))
+    rc = launch_unet_attn_fp16(ws.qkv, ws.ao, B, h * w, nh, C / nh, st);
   else
     rc = launch_attention_generic<float>(ws.qkv, ws.ao, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st);
   if (rc) return rc;
   ConvArgs o;
   o.B = B, o.H = h, o.W = w;
   o.in1 = ws.ao, o.c1 = C, o.bias = u.b2, o.r1 = x, o.rc1 = C, o.out = out, o.N = C;
-  return conv(prec, o, u.w2, u.w2_tf32, 1, st);
+  return conv(prec, o, u.w2, 1, st);
 }
 
 int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cbs, float* out,
@@ -399,8 +413,8 @@ int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float*
 
 int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int height, int width) {
   KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "unet_workspace_bytes: bad argument");
-  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED,
-              "unet_workspace_bytes: the fp32 and tf32 paths are built (precision %d)", precision);
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
+              "unet_workspace_bytes: the fp32, tf32 and fp16 paths are built (precision %d)", precision);
   UWs ws;
   carve(m->cfg, batch, height, width, nullptr, ws);
   return (int64_t)ws.total;
@@ -410,8 +424,8 @@ int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width
                      const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_forward: model NULL or not finalized");
   KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward: NULL argument");
-  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED,
-              "unet_forward: the fp32 and tf32 paths are built (precision %d)", precision);
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
+              "unet_forward: the fp32, tf32 and fp16 paths are built (precision %d)", precision);
   const KdbUNetConfig& c = m->cfg;
   KDB_REQUIRE(height > 0 && width > 0 && height % c.patch_size == 0 && width % c.patch_size == 0, KDB_ERR_BAD_SHAPE,
               "unet_forward: %dx%d not divisible by the patch size %d", height, width, c.patch_size);
@@ -449,6 +463,14 @@ int kdb_unet_conv_tf32(const float* in1, int c1, const float* in2, int c2, const
   a.in1 = in1, a.c1 = c1, a.in2 = in2, a.c2 = c2, a.w = w_tapmajor, a.bias = bias, a.r1 = r1, a.rc1 = rc1, a.r2 = r2, a.out = out;
   a.B = batch, a.H = h, a.W = w, a.N = n_out;
   return launch_unet_conv_tf32(a, ksize, (cudaStream_t)stream);
+}
+
+int kdb_unet_conv_fp16(const float* in1, int c1, const float* in2, int c2, const void* w_tapmajor_f16, const float* bias, const float* r1,
+                       int rc1, const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream) {
+  ConvArgs a;
+  a.in1 = in1, a.c1 = c1, a.in2 = in2, a.c2 = c2, a.bias = bias, a.r1 = r1, a.rc1 = rc1, a.r2 = r2, a.out = out;
+  a.B = batch, a.H = h, a.W = w, a.N = n_out;
+  return launch_unet_conv_fp16(a, static_cast<const __half*>(w_tapmajor_f16), ksize, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -2,6 +2,8 @@
 // Activations are token-major: [B, H, W, C] fp32, channels contiguous (DESIGN.md section 3).  Every kernel is deterministic:
 // fixed reduction orders, no atomics.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace kdb {
@@ -27,13 +29,23 @@ int launch_unet_conv(const ConvArgs& a, int ks, cudaStream_t st);
 // The same convolution on the tensor cores at KDB_PREC_TF32 (unet_tf32.cu): tf32 operands, fp32 accumulation.  w is expected rounded
 // to tf32 (launch_unet_round_tf32); activations are truncated to tf32 by the MMA.
 int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st);
-// Global self-attention at KDB_PREC_TF32 (unet_tf32.cu): qkv [B, T, 3 nh 64] fp32 in (t nh e) order with 1/sqrt(d_head) folded into q
-// -> out [B, T, nh 64] fp32; q, k, v and the softmax probabilities truncated to tf32, fp32 accumulation, running-maximum softmax.  Any
-// T >= 1.  unet_attn_tf32_supported: the head sizes it is built for (64); the engine keeps attn_generic for the others.
-bool unet_attn_tf32_supported(int d_head);
+// ... at KDB_PREC_FP16 (unet_tf32.cu): fp16 operands, fp32 accumulation.  a.w is not read: w is the fp16 tap-major weight
+// [N, ks*ks, f16_weight_ld(c1 + c2)] (launch_unet_round_f16); activations are rounded to the nearest fp16 (ties to even) in registers.
+// An operand of magnitude >= 65520 becomes +-inf (no saturation).
+int launch_unet_conv_fp16(const ConvArgs& a, const __half* w, int ks, cudaStream_t st);
+// the row length of an fp16 weight of `channels` input channels: rounded up to 8 (16-byte rows for TMA; the padding is never read)
+int f16_weight_ld(int channels);
+// Global self-attention at KDB_PREC_TF32 / KDB_PREC_FP16 (unet_tf32.cu): qkv [B, T, 3 nh 64] fp32 in (t nh e) order with 1/sqrt(d_head)
+// folded into q -> out [B, T, nh 64] fp32; q, k, v and the softmax probabilities truncated to tf32 / rounded to fp16 (nearest even),
+// fp32 scores, softmax and accumulation, running-maximum softmax.  Any T >= 1.  unet_attn_tc_supported: the head sizes they are built
+// for (64); the engine keeps attn_generic for the others.
+bool unet_attn_tc_supported(int d_head);
 int launch_unet_attn_tf32(const float* qkv, float* out, int B, int T, int nh, int d_head, cudaStream_t st);
+int launch_unet_attn_fp16(const float* qkv, float* out, int B, int T, int nh, int d_head, cudaStream_t st);
 // dst[i] = src[i] rounded to the nearest tf32 value (ties away from zero), stored as fp32
 int launch_unet_round_tf32(const float* src, float* dst, int64_t n, cudaStream_t st);
+// src [rows, C] fp32 -> dst [rows, f16_weight_ld(C)] fp16, rounded to nearest even (+-inf past 65504), the padding zero
+int launch_unet_round_f16(const float* src, __half* dst, int64_t rows, int C, cudaStream_t st);
 
 // AdaGN (layers.py:172-175), optionally followed by the erf GELU: out = [gelu](group_norm(x) * (1 + weight) + bias) with the
 // (weight, bias) pair read from the conditioning row of image b at cond + b * cond_bs + ada_off (C weights, then C biases).

@@ -16,11 +16,11 @@ import torch
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = Path(os.environ.get("KDB200_LIB", _HERE / "_lib" / "libkdb200.so"))
 
-PREC_FP32, PREC_BF16, PREC_TF32 = 0, 1, 2
+PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -96,6 +96,7 @@ SIGNATURES = {
     "kdb_attention_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_conv": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_conv_tf32": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_unet_conv_fp16": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
 }
 
 _lib = None
@@ -536,7 +537,7 @@ class Engine:
 
 
 class UNetEngine(Engine):
-    """The image_v1 U-Net at PREC_FP32 or PREC_TF32: the Engine calls where the sampler executor makes them; no derivatives."""
+    """The image_v1 U-Net at PREC_FP32, PREC_TF32 or PREC_FP16: the Engine calls where the sampler executor makes them; no derivatives."""
 
     _api = "unet"
 
@@ -653,7 +654,7 @@ def attention(qkv, h, w, n_heads, d_head, attn_type, attn_param=0, shift=0, fast
     return out
 
 
-def _unet_conv(fn, x1, w, ksize, x2, bias, r1, r2, out):
+def _unet_conv(fn, x1, w, ksize, x2, bias, r1, r2, out, w_dtype=torch.float32):
     require_cuda(x1, w, x2, bias, r1, r2, out)
     B, h, wd, c1 = x1.shape
     N = w.shape[0]
@@ -661,7 +662,8 @@ def _unet_conv(fn, x1, w, ksize, x2, bias, r1, r2, out):
     rc1 = 0 if r1 is None else r1.shape[-1]
     if out is None:
         out = torch.empty(B, h, wd, N, dtype=torch.float32, device=x1.device)
-    x1, x2, w, bias, r1, r2 = (None if t is None else f32c(t) for t in (x1, x2, w, bias, r1, r2))
+    x1, x2, bias, r1, r2 = (None if t is None else f32c(t) for t in (x1, x2, bias, r1, r2))
+    w = w.to(w_dtype).contiguous()
     check(fn(ptr(x1), c1, ptr(x2), c2, ptr(w), ptr(bias), ptr(r1), rc1, ptr(r2), ptr(out), B, h, wd, N, ksize, stream()))
     return out
 
@@ -682,14 +684,37 @@ def unet_conv_tf32(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None)
 
 
 @_on_device_of_first
-def unet_attention_tf32(qkv, h, w, n_heads, d_head=64):
-    """The U-Net engine's global attention at tf32 (kdb_attention with PREC_TF32): qkv [B, h*w, 3*n_heads*d_head] fp32 in (t nh e) order,
-    1/sqrt(d_head) already in q -> [B, h*w, n_heads*d_head] fp32.  q, k, v and the probabilities are truncated to tf32; d_head 64."""
+def unet_conv_fp16(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None):
+    """unet_conv with fp16 operands (kdb_unet_conv_fp16): the same arguments; w (fp32 or fp16, tap-major [N, ksize*ksize, c1 + c2]) is
+    rounded to fp16 (nearest even, as the engine's finalize does) and padded to the kernel's row length, the inputs are rounded to fp16 in
+    the kernel; fp32 accumulation.  Rounding does not saturate: an operand of magnitude >= 65520 becomes inf."""
+    require_cuda(w)
+    ct = w.shape[-1]
+    w16 = torch.zeros(*w.shape[:-1], (ct + 7) // 8 * 8, dtype=torch.float16, device=w.device)
+    w16[..., :ct] = w
+    return _unet_conv(lib().kdb_unet_conv_fp16, x1, w16, ksize, x2, bias, r1, r2, out, w_dtype=torch.float16)
+
+
+def _unet_attention(precision, qkv, h, w, n_heads, d_head):
     require_cuda(qkv)
     B = qkv.shape[0]
     out = torch.empty(B, h * w, n_heads * d_head, dtype=torch.float32, device=qkv.device)
-    check(lib().kdb_attention(PREC_TF32, 0, ptr(f32c(qkv)), ptr(out), B, h, w, n_heads, d_head, ATTN_GLOBAL, 0, 0, None, stream()))
+    check(lib().kdb_attention(precision, 0, ptr(f32c(qkv)), ptr(out), B, h, w, n_heads, d_head, ATTN_GLOBAL, 0, 0, None, stream()))
     return out
+
+
+@_on_device_of_first
+def unet_attention_tf32(qkv, h, w, n_heads, d_head=64):
+    """The U-Net engine's global attention at tf32 (kdb_attention with PREC_TF32): qkv [B, h*w, 3*n_heads*d_head] fp32 in (t nh e) order,
+    1/sqrt(d_head) already in q -> [B, h*w, n_heads*d_head] fp32.  q, k, v and the probabilities are truncated to tf32; d_head 64."""
+    return _unet_attention(PREC_TF32, qkv, h, w, n_heads, d_head)
+
+
+@_on_device_of_first
+def unet_attention_fp16(qkv, h, w, n_heads, d_head=64):
+    """unet_attention_tf32 at fp16 (kdb_attention with PREC_FP16): q, k, v and the probabilities are rounded to fp16 (nearest even); the
+    scores, the softmax and its sum stay fp32."""
+    return _unet_attention(PREC_FP16, qkv, h, w, n_heads, d_head)
 
 
 def _fp32_attention_args(tensors, numels):

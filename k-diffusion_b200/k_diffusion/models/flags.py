@@ -3,13 +3,15 @@
 K_DIFFUSION_USE_COMPILE / K_DIFFUSION_USE_FLASH_2 are accepted and ignored: there is no
 torch.compile or flash-attn path here.  The only switch is the arithmetic of the token stream:
 
-    KDB200_PRECISION = auto | fp32 | bf16 | tf32      (default auto)
+    KDB200_PRECISION = auto | fp32 | bf16 | tf32 | fp16      (default auto)
 
 auto = bf16 when the call happens under torch.autocast(bfloat16) or the module's parameters are
 bf16 (what `accelerate` mixed precision does for the reference), fp32 otherwise -- sample.py never
 enables autocast, so the reference's inference default is true fp32 and so is ours.  tf32 (the image_v1
 U-Net only, never chosen by auto): convolution and attention operands rounded to tf32 with fp32 accumulation -- what the
-reference's Conv2d already computes on an H100, where torch.backends.cudnn.allow_tf32 is True by default.
+reference's Conv2d already computes on an H100, where torch.backends.cudnn.allow_tf32 is True by default.  fp16 (the image_v1
+U-Net only, never chosen by auto, not even for fp16 parameters or under autocast(float16)): the same operands rounded to fp16 --
+the 10 explicit significand bits of tf32, a narrower exponent range, twice the tensor-core rate.
 """
 import os
 
@@ -32,6 +34,8 @@ def resolve_precision(requested, param_dtype):
         return "bf16"
     if req == "tf32":
         return "tf32"
+    if req in ("fp16", "float16"):
+        return "fp16"
     if req != "auto":
         raise ValueError(f"unknown precision {req!r}")
     if param_dtype == torch.bfloat16:

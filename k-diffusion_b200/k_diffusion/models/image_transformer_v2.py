@@ -163,8 +163,8 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
 
     def resolved_precision(self):
         p = flags.resolve_precision(self.precision, self.get_parameter(self.dtype_key).dtype)
-        if p == "tf32":
-            raise ValueError(f"the {self.kind} engine runs at fp32 or bf16 (tf32 is built for the image_v1 U-Net only)")
+        if p in ("tf32", "fp16"):
+            raise ValueError(f"the {self.kind} engine runs at fp32 or bf16 ({p} is built for the image_v1 U-Net only)")
         return _native.PREC_BF16 if p == "bf16" else _native.PREC_FP32
 
     def param_groups(self, *args, **kwargs):

@@ -1,10 +1,11 @@
-"""image_v1 U-Net denoiser -- parameter container + native forward, exact fp32 or with tf32 convolutions and attention.
+"""image_v1 U-Net denoiser -- parameter container + native forward, exact fp32 or with tf32 or fp16 convolutions and attention.
 
 Constructor, forward signature and `state_dict()` layout follow the reference (k_diffusion/models/image_v1.py, layers.py:116-313),
 so reference checkpoints load unchanged; the forward pass itself is executed by libkdb200.so (kdb_unet_*).  The torch modules
 below only hold named parameters and buffers: none of their forward methods runs.  Inference only.  Precision: fp32 (the default,
 every kernel exact fp32) or, by set_precision("tf32") or KDB200_PRECISION=tf32, every convolution and the d_head-64 attention on the tensor cores with tf32
-operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True).
+operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True) -- or, by
+set_precision("fp16") or KDB200_PRECISION=fp16, the same with fp16 operands (same significand width, narrower exponent range).
 """
 from types import SimpleNamespace
 
@@ -158,18 +159,22 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
         eng.bind(dict(self.state_dict(keep_vars=True)))
         return eng
 
+    _PRECISIONS = {"fp32": "fp32", "float32": "fp32", "tf32": "tf32", "fp16": "fp16", "float16": "fp16"}
+
     def set_precision(self, precision):
-        """'fp32' or None/'auto' (the exact fp32 path), or 'tf32' (tf32 convolutions and attention); the U-Net has no bf16 route."""
-        if precision not in (None, "auto", "fp32", "float32", "tf32"):
-            raise ValueError(f"the image_v1 U-Net runs at fp32 or tf32 (got precision {precision!r})")
-        self.precision = None if precision in (None, "auto") else "tf32" if precision == "tf32" else "fp32"
+        """'fp32' or None/'auto' (the exact fp32 path), 'tf32' or 'fp16' (tf32 / fp16 convolutions and attention); the U-Net has no bf16
+        route."""
+        if precision not in (None, "auto") and precision not in self._PRECISIONS:
+            raise ValueError(f"the image_v1 U-Net runs at fp32, tf32 or fp16 (got precision {precision!r})")
+        self.precision = None if precision in (None, "auto") else self._PRECISIONS[precision]
         return self
 
     def resolved_precision(self):
         p = flags.resolve_precision(self.precision, torch.float32)
-        if p not in ("fp32", "tf32"):
-            raise ValueError(f"the image_v1 U-Net runs at fp32 or tf32 (resolved precision {p!r})")
-        return _native.PREC_TF32 if p == "tf32" else _native.PREC_FP32
+        codes = {"fp32": _native.PREC_FP32, "tf32": _native.PREC_TF32, "fp16": _native.PREC_FP16}
+        if p not in codes:
+            raise ValueError(f"the image_v1 U-Net runs at fp32, tf32 or fp16 (resolved precision {p!r})")
+        return codes[p]
 
     def param_groups(self, *args, **kwargs):
         raise NotImplementedError("training is out of scope for the H100 sampling path")

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """(GPU) Heun-50 on the image_v1 config_cifar10 U-Net: the native engine against torch eager of the same function.
 
-    python tools/unet_bench.py [--batch 256] [--steps 50] [--precision fp32|tf32] [--json out.json]
+    python tools/unet_bench.py [--batch 256] [--steps 50] [--precision fp32|tf32|fp16] [--json out.json]
 
 Native: images/s of one graph-captured sample_heun call (warm-up call first, then the timed call ends in a device synchronise),
 and the device time per kernel family of one eager denoiser evaluation (kdb_profile_*, stream gated so the launches run back to
@@ -10,7 +10,9 @@ functional model (oracle/unet_oracle.py) on the same card, the same Heun loop (o
 cuDNN / matmul TF32 off and, at --precision tf32, also on (torch's own default for cuDNN convolutions).  The convolution and
 attention FLOPs of one evaluation are computed from the shapes; over the profiled time of their kernel families they are reported as a
 share of the H100 SXM data-sheet dense TF32 rate (495 TFLOP/s) -- a share of a data-sheet figure, not a rate the card reached.
-Synthetic seeded weights.  The card's name, power limit and SM clock are read in the same call.
+--precision fp16 times, in one call, the fp16, tf32 and fp32 native routes alternating (two rounds), then torch eager with TF32 on and
+under autocast(float16); each leg reports images/s, the device time of one evaluation's convolutions, attention and AdaGN, and its
+sample's rel-L2 against the native fp32 sample.  Synthetic seeded weights.  The card's name, power limit and SM clock are read in the same call.
 """
 import argparse
 import json
@@ -45,6 +47,7 @@ def timed(fn):
 
 
 TF32_DATASHEET_FLOPS = 495e12          # H100 SXM, dense TF32, at up to 700 W
+FP16_DATASHEET_FLOPS = 989e12          # H100 SXM, dense FP16, at up to 700 W
 
 
 def eval_flops(sd, m, B):
@@ -80,11 +83,72 @@ def native_leg(den, model, precision, x, sigmas, B, nfe):
     return out, res
 
 
+def kernel_split(fams):
+    """ms per evaluation of the convolutions, the attention and AdaGN from kdb_profile's kernel families"""
+    ms = lambda names: round(sum(v["ms"] for f, v in fams.items() if f in names), 3)
+    return {"conv": ms({"unet_conv", "unet_conv_tf32", "unet_conv_fp16"}), "attention": ms({"attn_generic", "unet_attn_tf32", "unet_attn_fp16"}),
+            "adagn": ms({"unet_adagn"})}
+
+
+def torch_eager_leg(oden, x, sigmas, B, nfe, settings):
+    """torch eager Heun of the oracle's functional model: images/s, and the device time of one evaluation's convolutions (aten::conv2d,
+    which includes the depthwise resampling filters), attention (aten::scaled_dot_product_attention) and group norms (AdaGN) from
+    torch.profiler in a separate run"""
+    O.sample_heun(oden, x, sigmas[:3])                                              # warm-up of every shape
+    out, t = timed(lambda: O.sample_heun(oden, x, sigmas))
+    sig = torch.full([x.shape[0]], 2.0, device="cuda")
+    oden(x, sig)
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA, torch.profiler.ProfilerActivity.CPU]) as prof:
+        oden(x, sig)
+        torch.cuda.synchronize()
+    ops = {e.key: e.device_time_total / 1e3 for e in prof.key_averages()}
+    split = {"conv": ops.get("aten::conv2d", 0.0), "attention": ops.get("aten::scaled_dot_product_attention", 0.0),
+             "adagn": ops.get("aten::group_norm", 0.0)}
+    return out, {"images_per_s": B / t, "s_per_call": t, "ms_per_eval": 1e3 * t / nfe, "settings": settings,
+                 "kernels_ms_per_eval": {k: round(v, 3) for k, v in split.items()}}
+
+
+def fp16_comparison(den, model, sd, m, x, sigmas, B, nfe, conv_flops, attn_flops, rounds=2):
+    """--precision fp16: the fp16, tf32 and fp32 native routes, alternating for `rounds` rounds (the samples and kernel times of the last
+    round), then torch eager with TF32 on and under autocast(float16); every sample's rel-L2 against the native fp32 one"""
+    legs, samples = {}, {}
+    for _ in range(rounds):
+        for prec in ("fp16", "tf32", "fp32"):
+            samples[prec], r = native_leg(den, model, prec, x, sigmas, B, nfe)
+            legs.setdefault(prec, []).append(r)
+    ref = samples["fp32"]
+    rel = lambda s: float((s - ref).double().norm() / ref.double().norm())
+    res = {}
+    for prec, rs in legs.items():
+        r = dict(rs[-1])
+        r["images_per_s_each_round"] = [q["images_per_s"] for q in rs]
+        r["split_ms_per_eval"] = kernel_split(r["kernels_ms_per_eval"])
+        r["rel_l2_vs_native_fp32"] = rel(samples[prec])
+        res[f"native_{prec}"] = r
+    for prec, peak in (("fp16", FP16_DATASHEET_FLOPS), ("tf32", TF32_DATASHEET_FLOPS)):
+        sp = res[f"native_{prec}"]["split_ms_per_eval"]
+        res[f"native_{prec}"]["share_of_datasheet"] = {
+            "conv": conv_flops / (sp["conv"] * 1e-3) / peak, "attention": attn_flops / (sp["attention"] * 1e-3) / peak,
+            "note": f"FLOPs from the shapes over the profiled kernel time, divided by the {peak / 1e12:.0f} TFLOP/s dense data-sheet "
+                    "figure; not a reached rate"}
+    res["speedup_fp16_vs_tf32_each_round"] = [t["s_per_call"] / f["s_per_call"] for f, t in zip(legs["fp16"], legs["tf32"])]
+    sdc = {k: v.cuda() for k, v in U.strip_prefix(sd).items()}
+    oden = U.make_denoiser(sdc, m)
+    torch.backends.cudnn.allow_tf32 = True
+    torch.backends.cuda.matmul.allow_tf32 = True
+    out, res["torch_eager_tf32"] = torch_eager_leg(oden, x, sigmas, B, nfe, "cuDNN convolutions and matmuls, TF32 on")
+    res["torch_eager_tf32"]["rel_l2_vs_native_fp32"] = rel(out)
+    with torch.autocast("cuda", dtype=torch.float16):
+        out, res["torch_eager_autocast_fp16"] = torch_eager_leg(oden, x, sigmas, B, nfe, "autocast(float16), TF32 on")
+    res["torch_eager_autocast_fp16"]["rel_l2_vs_native_fp32"] = rel(out.float())
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--precision", choices=["fp32", "tf32"], default="fp32")
+    ap.add_argument("--precision", choices=["fp32", "tf32", "fp16"], default="fp32")
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     meta = json.loads((ROOT / "tests/golden/unet_configs.json").read_text())["cifar10"]
@@ -101,6 +165,15 @@ def main():
                                        f"{a.precision}"}
     conv_flops, attn_flops = eval_flops(U.strip_prefix(sd), m, a.batch)
     res["flops_per_eval"] = {"conv": conv_flops, "attention": attn_flops}
+
+    if a.precision == "fp16":
+        with torch.no_grad():
+            res.update(fp16_comparison(den, model, sd, m, x, sigmas, a.batch, nfe, conv_flops, attn_flops))
+        res["card_after"] = card()
+        print(json.dumps(res, indent=1))
+        if a.json:
+            Path(a.json).write_text(json.dumps(res, indent=1))
+        return
 
     with torch.no_grad():
         native, res["native"] = native_leg(den, model, a.precision, x, sigmas, a.batch, nfe)
