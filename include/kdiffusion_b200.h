@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 16
+#define KDB_ABI_VERSION 17
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -396,6 +396,35 @@ int kdb_unet_conv_tf32(const float* in1, int c1, const float* in2, int c2, const
  * Products accumulate in fp32; bias and residual are added in fp32.  No grid-row limit on batch * h * w. */
 int kdb_unet_conv_fp16(const float* in1, int c1, const float* in2, int c2, const void* w_tapmajor_f16, const float* bias, const float* r1,
                        int rc1, const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Sample scoring: KID and FID on extracted features (evaluation.py:93-161), fp32 FFMA products as the reference computes them with
+ * TF32 off.  Features are row-major fp32 [rows, d].  No atomics: two calls on the same inputs return the same bits.  Unlike the
+ * solver and forward calls these are not meant for CUDA-graph capture (kdb_mmd_sums copies its segment list from host memory).
+ * ------------------------------------------------------------------------------------------ */
+
+/* Squared MMD with the polynomial kernel k(a, b) = (a . b / d + 1)^3 of S segments in one call: segment s pairs rows
+ * [x_offsets_host[s], x_offsets_host[s + 1]) of x [m, d] with rows [y_offsets_host[s], y_offsets_host[s + 1]) of y [n, d] (kid's
+ * partitions, evaluation.py:114-123, or the leading batch entries of squared_mmd, :99-111).  out [S, 4] fp64 receives per segment the
+ * sum of k(x, x) off its diagonal, the same of k(y, y), the sum of k(x, y) and term_1 + term_2 - term_3 formed in fp64 (nan for a
+ * segment of fewer than 2 rows, as 0/0 in the reference).  Each kernel value is an fp32 dot product over d (fmaf in index order), then
+ * fp32 (dot / d + 1)^3; only the tiles on or above the diagonal of k(x, x) and k(y, y) are computed and the strict upper triangle counts
+ * twice; tile sums and their totals are fp64 in a fixed order.  Offsets are host arrays of S + 1 nondecreasing row indices within
+ * [0, m] / [0, n], 1 <= S <= 65535.  kdb_mmd_workspace_bytes returns the workspace the same segment list needs (or a negative
+ * KDB_ERR_*); a shorter one returns KDB_ERR_WORKSPACE.  Two launches whatever S is. */
+int64_t kdb_mmd_workspace_bytes(const int64_t* x_offsets_host, const int64_t* y_offsets_host, int n_segments);
+int kdb_mmd_sums(const float* x, int64_t m, const float* y, int64_t n, int d, const int64_t* x_offsets_host, const int64_t* y_offsets_host,
+                 int n_segments, double* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* out [batch, m, n] fp32 = (x . y^T / d + 1)^3 of x [batch, m, d] and y [batch, n, d] (evaluation.py:93-96), each element as
+ * kdb_mmd_sums computes it.  batch <= 65535 and ceil(m / 64) <= 65535. */
+int kdb_polynomial_kernel(const float* x, const float* y, float* out, int batch, int m, int n, int d, void* stream);
+
+/* mean [d] and cov [d, d] fp32 of x [n, d] (evaluation.py:151-155: x.mean(0) and torch.cov(x.T)): the column sums in fp64 in a fixed
+ * order, divided by n; then the upper-triangle 64x64 tiles of (x - mean)^T (x - mean) / (n - 1), with x - mean in fp32 and fmaf over the
+ * samples in order, each element written to (i, j) and (j, i), so cov is exactly symmetric (n = 1 gives nan, as torch.cov).
+ * 1 <= n <= INT32_MAX.  Two launches, no workspace. */
+int kdb_feature_mean_cov(const float* x, int64_t n, int d, float* mean, float* cov, void* stream);
 
 #ifdef __cplusplus
 }

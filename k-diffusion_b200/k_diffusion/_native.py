@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -97,6 +97,10 @@ SIGNATURES = {
     "kdb_unet_conv": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_conv_tf32": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_conv_fp16": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_mmd_workspace_bytes": (_i64, [ctypes.POINTER(_i64), ctypes.POINTER(_i64), _i32]),
+    "kdb_mmd_sums": (_i32, [_vp, _i64, _vp, _i64, _i32, ctypes.POINTER(_i64), ctypes.POINTER(_i64), _i32, _vp, _vp, _sz, _vp]),
+    "kdb_polynomial_kernel": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_feature_mean_cov": (_i32, [_vp, _i64, _i32, _vp, _vp, _vp]),
 }
 
 _lib = None
@@ -750,3 +754,58 @@ def attention_vjp(qkv, out, dout, h, w, n_heads, d_head, attn_type, attn_param=0
     check(lib().kdb_attention_vjp(ptr(qkv), ptr(out), ptr(dout), ptr(dqkv), ptr(stats), B, h, w, n_heads, d_head, code, attn_param, shift,
                                    stream()))
     return dqkv
+
+
+# ---------------------------------------------------------------------------------------------
+# sample scoring (KID / FID)
+# ---------------------------------------------------------------------------------------------
+
+def _features(*tensors):
+    for t in tensors:
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"features must be contiguous fp32 (got {t.dtype}, shape {tuple(t.shape)})")
+
+
+@_on_device_of_first
+def mmd_sums(x, y, x_offsets, y_offsets):
+    """x [m, d] and y [n, d] contiguous fp32; x_offsets / y_offsets: S + 1 row bounds each (host ints), segment s pairing rows
+    x_offsets[s]:x_offsets[s+1] of x with y_offsets[s]:y_offsets[s+1] of y -> [S, 4] float64 (k(x, x) off-diagonal sum, k(y, y)
+    off-diagonal sum, k(x, y) sum, squared MMD) with the polynomial kernel (kdb_mmd_sums)."""
+    require_cuda(x, y)
+    _features(x, y)
+    S = len(x_offsets) - 1
+    if len(y_offsets) != S + 1 or x.shape[1] != y.shape[1]:
+        raise ValueError(f"{len(x_offsets)} x bounds and {len(y_offsets)} y bounds; feature widths {x.shape[1]} and {y.shape[1]}")
+    xo = (_i64 * (S + 1))(*x_offsets)
+    yo = (_i64 * (S + 1))(*y_offsets)
+    need = int(lib().kdb_mmd_workspace_bytes(xo, yo, S))
+    if need < 0:
+        check(need)
+    ws = torch.empty(need, dtype=torch.uint8, device=x.device)
+    out = torch.empty(S, 4, dtype=torch.float64, device=x.device)
+    check(lib().kdb_mmd_sums(ptr(x), x.shape[0], ptr(y), y.shape[0], x.shape[1], xo, yo, S, ptr(out), ptr(ws), need, stream()))
+    return out
+
+
+@_on_device_of_first
+def polynomial_kernel(x, y):
+    """x [B, m, d] and y [B, n, d] contiguous fp32 -> [B, m, n] fp32 (x . y^T / d + 1)^3 (kdb_polynomial_kernel)."""
+    require_cuda(x, y)
+    _features(x, y)
+    B, m, d = x.shape
+    n = y.shape[1]
+    out = torch.empty(B, m, n, dtype=torch.float32, device=x.device)
+    check(lib().kdb_polynomial_kernel(ptr(x), ptr(y), ptr(out), B, m, n, d, stream()))
+    return out
+
+
+@_on_device_of_first
+def feature_mean_cov(x):
+    """x [n, d] contiguous fp32 -> (mean [d], cov [d, d]) fp32, x.mean(0) and torch.cov(x.T) (kdb_feature_mean_cov)."""
+    require_cuda(x)
+    _features(x)
+    n, d = x.shape
+    mean = torch.empty(d, dtype=torch.float32, device=x.device)
+    cov = torch.empty(d, d, dtype=torch.float32, device=x.device)
+    check(lib().kdb_feature_mean_cov(ptr(x), n, d, ptr(mean), ptr(cov), stream()))
+    return mean, cov

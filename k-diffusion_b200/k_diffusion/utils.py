@@ -1,4 +1,4 @@
-"""Small helpers on the sampling path (reference: k_diffusion/utils.py:43-48,82-85)."""
+"""Small helpers on the sampling path (reference: k_diffusion/utils.py:43-48,82-85,429-443)."""
 from contextlib import contextmanager
 
 
@@ -57,3 +57,21 @@ def eval_mode(model):
 
 def train_mode(model):
     return _mode(model, True)
+
+
+@contextmanager
+def tf32_mode(cudnn=None, matmul=None):
+    """Context manager (and decorator) setting whether cuDNN convolutions and CUDA matmuls may use TF32 (utils.py:429-443).  A flag
+    given as True or False is put back to its previous value on exit, also when the body raises; None leaves that flag alone."""
+    import torch
+    flags = [(torch.backends.cudnn, cudnn), (torch.backends.cuda.matmul, matmul)]
+    saved = [owner.allow_tf32 for owner, _ in flags]
+    try:
+        for owner, value in flags:
+            if value is not None:
+                owner.allow_tf32 = value
+        yield
+    finally:
+        for (owner, value), old in zip(flags, saved):
+            if value is not None:
+                owner.allow_tf32 = old
