@@ -143,39 +143,62 @@ __device__ __forceinline__ QuadCoord quad_coord(int64_t m0, int n, int C, int wc
 
 // Shared memory of one GEMM CTA: the TMA ring, the fp32 accumulator tile (shared by the two warpgroups, in tile order), per
 // warpgroup the bf16 output staging tile (RESID: the residual tile is loaded into it and the epilogue adds in place), then the
-// barriers.  128-wide RESID / STORE / QKV / SPLIT: 96 + 64 + 2 x 32 KiB + 1 KiB of alignment = 225 KiB.  GEGLU runs its epilogue on the
-// accumulator fragments and has no fp32 tile: its ring takes those 64 KiB, 6 stages of 32 KiB + 2 x 16 KiB + 1 KiB = 225 KiB.
+// barriers.  The fp32 tile holds 64 columns of the 128 x BN accumulators at a time (a 128-wide epilogue stages its second half once
+// every thread has read the first), so 128-wide RESID / STORE / QKV / SPLIT take 128 + 32 + 2 x 32 KiB + 1 KiB of alignment = 225 KiB:
+// 4 ring stages instead of the 3 a whole 64 KiB fp32 tile leaves room for.  GEGLU runs its epilogue on the accumulator fragments and
+// has no fp32 tile: 6 stages of 32 KiB + 2 x 16 KiB + 1 KiB = 225 KiB.
 template <int BN, int EPI> constexpr int out_bytes() {
   return EPI == EPI_GEGLU ? SUB_TILE_BYTES : EPI == EPI_PATCH_OUT ? 0 : (BN / 64) * SUB_TILE_BYTES;
 }
-template <int BN, int EPI> constexpr int acc_bytes() { return EPI == EPI_GEGLU ? 0 : BM * BN * 4; }
-template <int EPI> constexpr int ring_bytes() { return EPI == EPI_GEGLU ? 192 * 1024 : 96 * 1024; }   // 96 KiB: 3 stages of 128-wide tiles, 4 of 64-wide
+constexpr int ACC_COLS = 64;                 // columns of the fp32 accumulator tile
+template <int BN, int EPI> constexpr int acc_bytes() { return EPI == EPI_GEGLU ? 0 : BM * ACC_COLS * 4; }
+template <int EPI> constexpr int ring_bytes() { return EPI == EPI_GEGLU ? 192 * 1024 : 128 * 1024; }   // 128 KiB: 4 stages of 128-wide tiles, 5 of 64-wide
 template <int BN, int EPI> constexpr size_t gemm_smem() { return 1024 + ring_bytes<EPI>() + acc_bytes<BN, EPI>() + 2 * out_bytes<BN, EPI>() + 128; }
 
-// The fp32 accumulator tile is [128 rows x BN columns] with the 16-byte chunks of row r XOR-swizzled by r % 8: the fragment stores
+// The fp32 accumulator tile is [128 rows x 64 columns] with the 16-byte chunks of row r XOR-swizzled by r % 8: the fragment stores
 // (8 rows x 4 column pairs per warp) and the row reads (32 rows, one float4 each) both spread evenly over the banks.
-template <int BN> __device__ __forceinline__ int stage_off(int row, int chunk) { return row * BN + ((chunk ^ (row & 7)) << 2); }
-// accumulator fragment of rows [row0, row0 + 64) -> the fp32 tile
-template <int BN>
+__device__ __forceinline__ int stage_off(int row, int chunk) { return row * ACC_COLS + ((chunk ^ (row & 7)) << 2); }
+// columns [64 H, 64 H + 64) of the accumulator fragment of rows [row0, row0 + 64) -> the fp32 tile
+template <int BN, int H>
 __device__ __forceinline__ void stage_store(float* s, int row0, const float (&d)[BN / 2]) {
   const int t = threadIdx.x & 127;
   const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    *reinterpret_cast<float2*>(s + stage_off<BN>(r, 2 * j + (c >> 2)) + (c & 3)) = make_float2(d[4 * j], d[4 * j + 1]);
-    *reinterpret_cast<float2*>(s + stage_off<BN>(r + 8, 2 * j + (c >> 2)) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  for (int j = 0; j < ACC_COLS / 8; ++j) {
+    const int jd = H * (ACC_COLS / 8) + j;   // 8-column block of the fragment
+    *reinterpret_cast<float2*>(s + stage_off(r, 2 * j + (c >> 2)) + (c & 3)) = make_float2(d[4 * jd], d[4 * jd + 1]);
+    *reinterpret_cast<float2*>(s + stage_off(r + 8, 2 * j + (c >> 2)) + (c & 3)) = make_float2(d[4 * jd + 2], d[4 * jd + 3]);
   }
 }
-// 32 consecutive columns of one row of the fp32 tile
+// Columns 64..127 of a 128-wide tile replace columns 0..63 in the fp32 tile, once every thread of the warpgroup has read those
 template <int BN>
+__device__ __forceinline__ void stage_second_half(float* s, int wg, const float (&acc0)[BN / 2], const float (&acc1)[BN / 2]) {
+  if constexpr (BN == 128) {
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
+    stage_store<BN, 1>(s, 0, acc0);
+    stage_store<BN, 1>(s, 64, acc1);
+    tc::named_barrier_sync(tc::BAR_WG + wg, 128);
+  }
+}
+// 32 consecutive columns of one row of the fp32 tile; col0 is the column in the 128 x BN tile (the half it lies in is staged)
 __device__ __forceinline__ void stage_ld32(const float* s, int row, int col0, float (&v)[32]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float4 q = *reinterpret_cast<const float4*>(s + stage_off<BN>(row, (col0 >> 2) + i));
+    const float4 q = *reinterpret_cast<const float4*>(s + stage_off(row, ((col0 % ACC_COLS) >> 2) + i));
     v[4 * i] = q.x;
     v[4 * i + 1] = q.y;
     v[4 * i + 2] = q.z;
     v[4 * i + 3] = q.w;
+  }
+}
+__device__ __forceinline__ void stage_ld64(const float* s, int row, int col0, float (&v)[64]) {
+  float t0[32], t1[32];
+  stage_ld32(s, row, col0, t0);
+  stage_ld32(s, row, col0 + 32, t1);
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    v[k] = t0[k];
+    v[32 + k] = t1[k];
   }
 }
 
@@ -351,8 +374,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       continue;
     }
     if (i > 0) tc::named_barrier_sync(tc::BAR_ACC + wg, 256);   // the other warpgroup has read tile i - 1 out of the fp32 tile
-    stage_store<BN>(sAcc, 0, acc0);
-    stage_store<BN>(sAcc, 64, acc1);
+    stage_store<BN, 0>(sAcc, 0, acc0);
+    stage_store<BN, 0>(sAcc, 64, acc1);
     tc::named_barrier_sync(tc::BAR_WG + wg, 128);
     const bool pass_acc = i + 1 < n_local;   // after its last read of the fp32 tile this warpgroup hands it on (named_barrier_arrive)
 
@@ -369,8 +392,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       float v[64];
       {
         float t0[32], t1[32];
-        stage_ld32<BN>(sAcc, row, 0, t0);
-        stage_ld32<BN>(sAcc, row, 32, t1);
+        stage_ld32(sAcc, row, 0, t0);
+        stage_ld32(sAcc, row, 32, t1);
 #pragma unroll
         for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
       }
@@ -413,11 +436,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
         tc::mbar_wait_nocall(&resid_full[wg], (uint32_t)(i >> 1) & 1u);
 #pragma unroll 1
         for (int g = 0; g < NSUB; ++g) {
+          if (g == 1) stage_second_half<BN>(sAcc, wg, acc0, acc1);
           float v[64];
           {
             float t0[32], t1[32];
-            stage_ld32<BN>(sAcc, row, g * 64, t0);
-            stage_ld32<BN>(sAcc, row, g * 64 + 32, t1);
+            stage_ld32(sAcc, row, g * 64, t0);
+            stage_ld32(sAcc, row, g * 64 + 32, t1);
 #pragma unroll
             for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
           }
@@ -467,8 +491,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       // loads of the skip and stores of the output
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
+        if (c == 2) stage_second_half<BN>(sAcc, wg, acc0, acc1);
         float v[32];
-        stage_ld32<BN>(sAcc, row, c * 32, v);
+        stage_ld32(sAcc, row, c * 32, v);
         if (c == BN / 32 - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
         if (!live) continue;
         const int n = n0 + c * 32;
@@ -503,16 +528,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
     } else {
       if constexpr (RES) tc::mbar_wait_nocall(&resid_full[wg], (uint32_t)(i >> 1) & 1u);
       float ss_acc[4] = {0.f, 0.f, 0.f, 0.f};   // producer side: sum of squares of the row this thread writes
+      float v[64];
+      stage_ld64(sAcc, row, 0, v);
+      stage_second_half<BN>(sAcc, wg, acc0, acc1);   // the fragments are dead from here on
 #pragma unroll 1
       for (int g = 0; g < NSUB; ++g) {
-        float v[64];
-        {
-          float t0[32], t1[32];
-          stage_ld32<BN>(sAcc, row, g * 64, t0);
-          stage_ld32<BN>(sAcc, row, g * 64 + 32, t1);
-#pragma unroll
-          for (int k = 0; k < 32; ++k) { v[k] = t0[k]; v[32 + k] = t1[k]; }
-        }
+        if (g > 0) stage_ld64(sAcc, row, g * 64, v);
         if (g == NSUB - 1 && pass_acc) tc::named_barrier_arrive(tc::BAR_ACC + (wg ^ 1), 256);
         if (p.ss_in != nullptr) {
           // fused RMSNorm row scale.  q and k are cosine-normalised afterwards (scale invariant): only v needs it.

@@ -8,6 +8,10 @@ The library is the one k_diffusion._native loads: $KDB200_LIB if set, so two bui
 evaluation is enqueued behind a gate kernel (kernels back to back, as in a graph replay) with CUDA events around every launch; a
 launch's time is the median over --repeat evaluations.  Bound = max(FLOPs / 989 TFLOP/s, minimum bytes / 3.35 TB/s), the H100 SXM
 data-sheet figures (dense BF16, HBM3); minimum bytes = A + W + output, plus the residual / skip tensor of out / down / split.
+
+Operand stream = the A and W bytes the CTAs' TMA rings load from L2, from the tile shapes (every 128 x BN tile loads one A and one W
+k-block per 64-wide k-step), and the same over the launch's time in TB/s.  No L2 bandwidth is printed against it: none has been
+measured for this access pattern.
 """
 import argparse
 import json
@@ -49,6 +53,12 @@ def min_bytes(label, M, N, K):
     return 2 * (M * K + N * K + out + extra)
 
 
+def operand_bytes(M, N, K):
+    """A + W bytes the GEMM's rings load: 128 x BN tiles (BN = 128, or 64 when N % 128 != 0), a 128 x 64 A and a BN x 64 W k-block each"""
+    bn = 128 if N % 128 == 0 else 64
+    return -(-M // 128) * (N // bn) * (K // 64) * (128 + bn) * 64 * 2
+
+
 def bench(name, repeat):
     raw, batch = CONFIGS[name]
     cfg = K.config.load_config(raw())
@@ -81,10 +91,12 @@ def bench(name, repeat):
         us = sorted(ts)[len(ts) // 2] * 1e3
         flop, byts = 2.0 * macs, min_bytes(label, M, N, Kd)
         t_mma, t_hbm = flop / (PEAK_TFLOPS * 1e12) * 1e6, byts / (PEAK_TBS * 1e12) * 1e6
+        opnd = operand_bytes(M, N, Kd)
         rows.append(dict(label=label, M=M, N=N, K=Kd, us=round(us, 2), tflops=round(flop / us / 1e6, 1), gbs=round(byts / us / 1e3),
-                         bound_us=round(max(t_mma, t_hbm), 2), bound_by="MMA" if t_mma >= t_hbm else "HBM"))
+                         bound_us=round(max(t_mma, t_hbm), 2), bound_by="MMA" if t_mma >= t_hbm else "HBM",
+                         operand_mb=round(opnd / 1e6, 1), operand_tbs=round(opnd / us / 1e6, 2)))
     return dict(config=name, batch=batch, generic_gemm_us=round(sum(r["us"] for r in rows), 1),
-                bound_us=round(sum(r["bound_us"] for r in rows), 1), launches=rows)
+                bound_us=round(sum(r["bound_us"] for r in rows), 1), operand_mb=round(sum(r["operand_mb"] for r in rows), 1), launches=rows)
 
 
 def main():
@@ -97,10 +109,12 @@ def main():
     res = dict(gpu=gpu_info(), lib=str(_native.LIB_PATH), configs=[bench(c, a.repeat) for c in a.configs])
     print(json.dumps(res["gpu"]), res["lib"])
     for c in res["configs"]:
-        print(f"{c['config']} B={c['batch']}: generic GEMMs {c['generic_gemm_us']:.1f} us per evaluation (bound {c['bound_us']:.1f} us)")
+        print(f"{c['config']} B={c['batch']}: generic GEMMs {c['generic_gemm_us']:.1f} us per evaluation (bound {c['bound_us']:.1f} us); "
+              f"operand stream {c['operand_mb']:.0f} MB")
         for r in c["launches"]:
             print(f"  {r['label']:16s} {r['M']:6d} x {r['N']:5d} x {r['K']:5d}  {r['us']:8.2f} us  {r['tflops']:6.1f} TFLOP/s  "
-                  f"{r['gbs']:5d} GB/s  bound {r['bound_us']:6.2f} us ({r['bound_by']}, {r['bound_us'] / r['us']:5.1%})")
+                  f"{r['gbs']:5d} GB/s  bound {r['bound_us']:6.2f} us ({r['bound_by']}, {r['bound_us'] / r['us']:5.1%})  "
+                  f"operands {r['operand_mb']:6.1f} MB {r['operand_tbs']:5.2f} TB/s")
     if a.json:
         Path(a.json).write_text(json.dumps(res, indent=1))
 
