@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 17
+#define KDB_ABI_VERSION 18
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -109,6 +109,28 @@ int kdb_precond_scale_in(const float* x, const float* sigma, float sigma_data, f
                          int batch, int64_t per_sample, void* stream);
 int kdb_precond_combine(const float* f, const float* x, const float* sigma, float sigma_data, float* out,
                         int batch, int64_t per_sample, void* stream);
+
+/* The per-evaluation math of the external model wrappers (external.py:9-38, 87-177: VDenoiser, DiscreteEpsDDPMDenoiser,
+ * OpenAIDenoiser, CompVisDenoiser, DiscreteVDDPMDenoiser, CompVisVDenoiser); sigma is [B] fp32.  Every product and sum is
+ * rounded on its own (no FMA contraction), in the order the reference's torch expressions evaluate, so on the same GPU the
+ * result equals the reference's fp32 expression bit for bit.  With s2 = sigma^2 + sigma_data^2:
+ *   kdb_external_scale_in : out[b,...] = x[b,...] * c_in,   c_in = 1 / sqrt(s2)
+ *   kdb_external_combine  : kind KDB_EXTERNAL_EPS  out[b,...] = x[b,...] + f[b,...] * (-sigma[b])
+ *                           kind KDB_EXTERNAL_V    out[b,...] = f[b,...] * c_out + x[b,...] * c_skip,
+ *                                                  c_out = -sigma sigma_data / sqrt(s2), c_skip = (1 / s2) sigma_data^2
+ * `f` is the inner model's output as it stands: dtype KDB_DTYPE_F32 / F16 / BF16 (converted to fp32 exactly), each sample
+ * a contiguous run of per_sample elements, sample b starting at f + b * f_batch_stride elements (so the eps half of a
+ * learned-variance output, output[:, :C], is read in place).  Either of `f` and `x` may be NULL, which drops its term:
+ * the derivatives (g_eps = -sigma u, g_v = c_out u, g_x = c_skip u and the tangents) run on the same kernel. */
+#define KDB_EXTERNAL_EPS 0
+#define KDB_EXTERNAL_V   1
+#define KDB_DTYPE_F32    0
+#define KDB_DTYPE_F16    1
+#define KDB_DTYPE_BF16   2
+int kdb_external_scale_in(const float* x, const float* sigma, float sigma_data, float* out, int batch, int64_t per_sample,
+                          void* stream);
+int kdb_external_combine(int kind, const void* f, int f_dtype, int64_t f_batch_stride, const float* x, const float* sigma,
+                         float sigma_data, float* out, int batch, int64_t per_sample, void* stream);
 
 /* Counter-based standard-normal fill (Philox4x32-10 + Box-Muller): element i of sample b gets the
  * (seed[b], stream_id, i) variate, so results do not depend on how a batch is sharded across GPUs.

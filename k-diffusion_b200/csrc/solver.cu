@@ -5,12 +5,14 @@
 //
 // Reference semantics: k_diffusion/sampling.py:46-62 (to_d, ancestral step, default noise),
 // :65-114 (Brownian noise), :117-184 (euler / euler_ancestral / heun), :584-607 (dpmpp_2m),
-// k_diffusion/layers.py:70-74,88-90 (Denoiser scalings).
+// k_diffusion/layers.py:70-74,88-90 (Denoiser scalings), k_diffusion/external.py:9-38,87-177 (external model wrappers).
 #include <cmath>
 #include <cstdarg>
 #include <cstring>
 #include <atomic>
 #include <vector>
+
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 
@@ -205,6 +207,95 @@ __global__ void __launch_bounds__(256) precond_kernel(const float* __restrict__ 
         out[i] = x[i] * c_in;
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// External model wrappers (reference external.py:9-38, 87-177): scale-in and the eps / v combine around a foreign inner model.
+// torch evaluates the reference's expressions one rounded operation per kernel, so every product, sum, square root and
+// reciprocal here is an explicitly rounded intrinsic in the same order (nvcc would otherwise contract a*b + c into an FMA):
+//   s2 = sigma * sigma + sd^2        c_in = rcp(sqrt(s2))           (`1 / t` is reciprocal(t) * 1 in torch)
+//   eps: out = f * (-sigma) + x      v: out = f * c_out + x * c_skip, c_out = (-sigma * sd) / sqrt(s2), c_skip = rcp(s2) * sd^2
+// As out = f * cf + x * cx (cx = 1 for eps: x * 1 is exact), one kernel serves scale-in (no f), both combines and, with either
+// term dropped, their derivatives.
+// ------------------------------------------------------------------------------------------------
+enum ExtMode { EXT_SCALE_IN = 0, EXT_EPS = 1, EXT_V = 2 };
+
+__device__ __forceinline__ void external_coefs(int mode, float sigma, float sd, float& cf, float& cx) {
+  const float sd2 = __fmul_rn(sd, sd);
+  const float s2 = __fadd_rn(__fmul_rn(sigma, sigma), sd2);
+  if (mode == EXT_EPS) {
+    cf = -sigma;
+    cx = 1.f;
+  } else if (mode == EXT_V) {
+    cf = __fdiv_rn(__fmul_rn(-sigma, sd), __fsqrt_rn(s2));
+    cx = __fmul_rn(__frcp_rn(s2), sd2);
+  } else {
+    cf = 0.f;
+    cx = __frcp_rn(__fsqrt_rn(s2));
+  }
+}
+
+__device__ __forceinline__ float ext_f(float v) { return v; }
+__device__ __forceinline__ float ext_f(__half v) { return __half2float(v); }
+__device__ __forceinline__ float ext_f(bf16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float4 ext_load4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+template <typename T>
+__device__ __forceinline__ float4 ext_load4(const T* p) {         // four 16-bit values in one 8-byte load
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const T* h = reinterpret_cast<const T*>(&u);
+  return make_float4(ext_f(h[0]), ext_f(h[1]), ext_f(h[2]), ext_f(h[3]));
+}
+
+__device__ __forceinline__ float ext_apply(bool has_f, bool has_x, float f, float x, float cf, float cx) {
+  if (!has_f) return __fmul_rn(x, cx);
+  if (!has_x) return __fmul_rn(f, cf);
+  return __fadd_rn(__fmul_rn(f, cf), __fmul_rn(x, cx));
+}
+
+// blockIdx.y walks the samples (the per-sample coefficients are computed once per thread and sample), blockIdx.x the elements
+// of one sample: 4 per thread and step when VEC (per_sample, f's batch stride and every pointer allow 128-bit x / out access).
+template <typename TF, bool VEC>
+__global__ void __launch_bounds__(256) external_kernel(int mode, const TF* f, int64_t f_stride, const float* x,
+                                                       const float* __restrict__ sigma, float sd, float* out, int batch,
+                                                       int64_t per_sample) {
+  const bool has_f = f != nullptr, has_x = x != nullptr;
+  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    float cf, cx;
+    external_coefs(mode, __ldg(sigma + b), sd, cf, cx);
+    const TF* fb = has_f ? f + (int64_t)b * f_stride : nullptr;
+    const float* xb = has_x ? x + (int64_t)b * per_sample : nullptr;
+    float* ob = out + (int64_t)b * per_sample;
+    if constexpr (VEC) {
+      for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < per_sample / 4; i += (int64_t)gridDim.x * 256) {
+        const float4 fv = has_f ? ext_load4(fb + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 xv = has_x ? reinterpret_cast<const float4*>(xb)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        reinterpret_cast<float4*>(ob)[i] = make_float4(ext_apply(has_f, has_x, fv.x, xv.x, cf, cx), ext_apply(has_f, has_x, fv.y, xv.y, cf, cx),
+                                                       ext_apply(has_f, has_x, fv.z, xv.z, cf, cx), ext_apply(has_f, has_x, fv.w, xv.w, cf, cx));
+      }
+    } else {
+      for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < per_sample; i += (int64_t)gridDim.x * 256)
+        ob[i] = ext_apply(has_f, has_x, has_f ? ext_f(fb[i]) : 0.f, has_x ? xb[i] : 0.f, cf, cx);
+    }
+  }
+}
+
+template <typename TF>
+static int external_launch(int mode, const TF* f, int64_t f_stride, const float* x, const float* sigma, float sd, float* out, int batch,
+                           int64_t per_sample, cudaStream_t st) {
+  const auto al = [](const void* p, uintptr_t a) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
+  const bool vec = per_sample % 4 == 0 && f_stride % 4 == 0 && al(f, 4 * sizeof(TF)) && al(x, 16) && al(out, 16);
+  const int gy = batch < 65535 ? batch : 65535;
+  int64_t gx = ceil_div(vec ? per_sample / 4 : per_sample, 256);
+  const int64_t cap = (int64_t)kNumSMs * 8 / gy;                 // ~8 resident CTAs per SM over the whole grid
+  if (gx > cap) gx = cap;
+  if (gx < 1) gx = 1;
+  const dim3 grid((unsigned)gx, (unsigned)gy);
+  if (vec)
+    external_kernel<TF, true><<<grid, 256, 0, st>>>(mode, f, f_stride, x, sigma, sd, out, batch, per_sample);
+  else
+    external_kernel<TF, false><<<grid, 256, 0, st>>>(mode, f, f_stride, x, sigma, sd, out, batch, per_sample);
+  KDB_LAUNCH_CHECK(F_PRECOND, st);
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -552,6 +643,31 @@ int kdb_precond_combine(const float* f, const float* x, const float* sigma, floa
   precond_kernel<1><<<precond_grid(total), 256, 0, (cudaStream_t)stream>>>(f, x, sigma, sigma_data, out, per_sample, total);
   KDB_LAUNCH_CHECK(F_PRECOND, (cudaStream_t)stream);
   return 0;
+}
+
+int kdb_external_scale_in(const float* x, const float* sigma, float sigma_data, float* out, int batch, int64_t per_sample, void* stream) {
+  KDB_REQUIRE(x && sigma && out && batch > 0 && per_sample > 0, KDB_ERR_BAD_ARG, "external_scale_in: bad args");
+  return external_launch<float>(EXT_SCALE_IN, nullptr, 0, x, sigma, sigma_data, out, batch, per_sample, (cudaStream_t)stream);
+}
+
+int kdb_external_combine(int kind, const void* f, int f_dtype, int64_t f_batch_stride, const float* x, const float* sigma, float sigma_data,
+                         float* out, int batch, int64_t per_sample, void* stream) {
+  KDB_REQUIRE((f || x) && sigma && out && batch > 0 && per_sample > 0 && f_batch_stride >= 0, KDB_ERR_BAD_ARG,
+              "external_combine: bad args (f and x may not both be NULL)");
+  KDB_REQUIRE(kind == KDB_EXTERNAL_EPS || kind == KDB_EXTERNAL_V, KDB_ERR_BAD_ARG, "external_combine: kind %d is neither eps nor v", kind);
+  const int mode = kind == KDB_EXTERNAL_EPS ? EXT_EPS : EXT_V;
+  const cudaStream_t st = (cudaStream_t)stream;
+  switch (f_dtype) {
+    case KDB_DTYPE_F32:
+      return external_launch(mode, static_cast<const float*>(f), f_batch_stride, x, sigma, sigma_data, out, batch, per_sample, st);
+    case KDB_DTYPE_F16:
+      return external_launch(mode, static_cast<const __half*>(f), f_batch_stride, x, sigma, sigma_data, out, batch, per_sample, st);
+    case KDB_DTYPE_BF16:
+      return external_launch(mode, static_cast<const bf16*>(f), f_batch_stride, x, sigma, sigma_data, out, batch, per_sample, st);
+    default:
+      set_error("external_combine: f_dtype %d is not KDB_DTYPE_F32 / F16 / BF16", f_dtype);
+      return KDB_ERR_BAD_ARG;
+  }
 }
 
 int kdb_noise_normal(float* out, const int64_t* seeds, uint64_t stream_id, int batch, int64_t per_sample, void* stream) {

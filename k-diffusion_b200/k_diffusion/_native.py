@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -62,6 +62,8 @@ SIGNATURES = {
     "kdb_solver_to_d": (_i32, [_vp, _vp, _vp, _vp, _i32, _i64, _vp]),
     "kdb_precond_scale_in": (_i32, [_vp, _vp, _f32, _vp, _i32, _i64, _vp]),
     "kdb_precond_combine": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
+    "kdb_external_scale_in": (_i32, [_vp, _vp, _f32, _vp, _i32, _i64, _vp]),
+    "kdb_external_combine": (_i32, [_i32, _vp, _i32, _i64, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
     "kdb_noise_normal": (_i32, [_vp, _vp, _u64, _i32, _i64, _vp]),
     "kdb_noise_brownian": (_i32, [_vp, _vp, _i32, _i64, _f64, _f64, _f64, _f64, _i32, _vp]),
     "kdb_model_create": (_i32, [ctypes.POINTER(KdbModelConfig), ctypes.POINTER(_vp)]),
@@ -321,6 +323,60 @@ def precond_combine(f, x, sigma, sigma_data, out=None):
     require_cuda(f, x, sigma)
     out = _out_like(x, out)
     check(lib().kdb_precond_combine(ptr(f), ptr(x), ptr(sigma), sigma_data, ptr(out), x.shape[0], x[0].numel(), stream()))
+    return out
+
+
+EXTERNAL_EPS, EXTERNAL_V = 0, 1
+_EXT_DTYPE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+@_on_device_of_first
+def external_scale_in(x, sigma, sigma_data=1.0):
+    """x [B, ...] fp32 contiguous, sigma [B] fp32 -> x * c_in, c_in = 1 / sqrt(sigma^2 + sigma_data^2) rounded as the reference's
+    torch expression (external.py get_scalings)."""
+    require_cuda(x, sigma)
+    out = torch.empty_like(x)
+    B = x.shape[0]
+    check(lib().kdb_external_scale_in(ptr(x), ptr(sigma), float(sigma_data), ptr(out), B, x.numel() // B, stream()))
+    return out
+
+
+def _per_sample_stride(f, B):
+    """f's batch stride if each of its B samples is one contiguous run (a contiguous tensor, or a channel slice of one such as the
+    eps half of a learned-variance output), else None."""
+    shape, strides = f.shape, f.stride()
+    if f.ndim == 0 or shape[0] != B:
+        return None
+    run = 1
+    for d in range(f.ndim - 1, 0, -1):
+        if shape[d] != 1 and strides[d] != run:
+            return None
+        run *= shape[d]
+    return strides[0] if B > 1 else run
+
+
+def external_combine(kind, f, x, sigma, sigma_data=1.0):
+    """The output combine of an external wrapper: kind EXTERNAL_EPS -> x + f * (-sigma), EXTERNAL_V -> f * c_out + x * c_skip.
+    f (the inner model's output: fp32, fp16 or bf16, each sample contiguous, any batch stride) is read in place; either f or x
+    may be None, which drops its term.  x fp32 contiguous, sigma [B] fp32 -> fp32 [B, ...] of x's (or f's) shape."""
+    require_cuda(f, x, sigma)
+    like = x if x is not None else f
+    B = like.shape[0]
+    n = like.numel() // B
+    stride, code = 0, 0
+    if f is not None:
+        if f.dtype not in _EXT_DTYPE:
+            raise TypeError(f"the inner model returned {f.dtype}; the external wrappers take fp32, fp16 or bf16 outputs")
+        if x is not None and f.shape != x.shape:
+            raise ValueError(f"inner model output of shape {tuple(f.shape)} for an input of shape {tuple(x.shape)}")
+        stride = _per_sample_stride(f, B)
+        if stride is None:
+            f = f.contiguous()
+            stride = n
+        code = _EXT_DTYPE[f.dtype]
+    out = torch.empty(like.shape, dtype=torch.float32, device=like.device)
+    with device_of(like):
+        check(lib().kdb_external_combine(kind, ptr(f), code, stride, ptr(x), ptr(sigma), float(sigma_data), ptr(out), B, n, stream()))
     return out
 
 
