@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 18
+#define KDB_ABI_VERSION 19
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -109,6 +109,20 @@ int kdb_precond_scale_in(const float* x, const float* sigma, float sigma_data, f
                          int batch, int64_t per_sample, void* stream);
 int kdb_precond_combine(const float* f, const float* x, const float* sigma, float sigma_data, float* out,
                         int batch, int64_t per_sample, void* stream);
+
+/* Training losses with the Karras preconditioner, scales == 1 (layers.py:76-86 Denoiser.loss, :107-111 SimpleLossDenoiser.loss); x (the
+ * clean input), noise [B, ...], sigma [B], sigma_data > 0, per_sample elements per image.
+ *   kdb_loss_noised_input: out = (x + noise * sigma) * c_in(sigma), the inner model's input
+ *   kdb_denoiser_loss:     f = the inner model's output on it.  KDB_LOSS_DENOISER: loss[b] = mean((f - target)^2) * weight[b],
+ *                          target = (x - c_skip * (x + noise sigma)) / c_out.  KDB_LOSS_SIMPLE (weight unused): loss[b] = mean((eps - noise)^2),
+ *                          eps = ((x + noise sigma) - (f c_out + (x + noise sigma) c_skip)) / sigma.  cotangent (or NULL) receives d loss[b] / d f.
+ * One CTA per image, a fixed-order sum: two calls give the same bits. */
+#define KDB_LOSS_DENOISER 0
+#define KDB_LOSS_SIMPLE   1
+int kdb_loss_noised_input(const float* x, const float* noise, const float* sigma, float sigma_data, float* out,
+                          int batch, int64_t per_sample, void* stream);
+int kdb_denoiser_loss(int kind, const float* x, const float* noise, const float* sigma, const float* weight, float sigma_data,
+                      const float* f, float* loss, float* cotangent, int batch, int64_t per_sample, void* stream);
 
 /* The per-evaluation math of the external model wrappers (external.py:9-38, 87-177: VDenoiser, DiscreteEpsDDPMDenoiser,
  * OpenAIDenoiser, CompVisDenoiser, DiscreteVDDPMDenoiser, CompVisVDenoiser); sigma is [B] fp32.  Every product and sum is
@@ -261,6 +275,29 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
                           const float* cond, int64_t cond_batch_stride,
                           const float* cotangent, float* out, float* grad_x,
                           void* workspace, size_t workspace_bytes, void* stream);
+
+/* Parameter gradients (training) of an image_transformer_v2 model, fp32.  kdb_model_set_grad binds a gradient buffer [shape] fp32 on the
+ * device to the state-dict key of a parameter, as kdb_model_set_tensor binds weights (data == NULL unbinds the key); binding needs no
+ * finalize.  kdb_model_forward_train runs the raw model F (sigma_data 0) forward at fp32, bit for bit as kdb_model_forward, takes the
+ * cotangent u [B, C_out, H, W] on out = F(x, sigma) and OVERWRITES every bound gradient with u^T dF/dparam summed over the batch; grad_x
+ * (shape of x, or NULL) receives u^T dF/dx.  Unbound parameters are skipped.  The walk is that of kdb_model_forward_vjp with the weight
+ * gradients added, then the AdaRMSNorm projections and the mapping network (which is why the raw conditioning inputs are passed: sigma
+ * [B], aug_cond [B, 9] or NULL, class_cond [B] int64 when num_classes > 0, mapping_cond [B, mapping_cond_dim] when mapping_cond_dim > 0).
+ * cond holds one conditioning row per image (kdb_model_conditioning of those inputs; cond_batch_stride == kdb_model_cond_stride).  Bind the
+ * weights first: kdb_model_set_grad returns KDB_ERR_MISSING_KEY for a key that is no tensor set on the model, KDB_ERR_BAD_SHAPE for a shape
+ * other than that tensor's, and KDB_ERR_BAD_ARG for the buffers time_emb.weight, aug_emb.weight and *.pos_emb.freqs, which take no
+ * gradient; kdb_model_forward_train repeats these checks for every bound key (the weights may have been rebound since) and returns the
+ * same codes.  image_transformer_v1 handles return KDB_ERR_UNSUPPORTED.  The
+ * workspace is kdb_model_train_workspace_bytes(m, batch, height, width) bytes (the finalized model's size; negative KDB_ERR_* on bad
+ * arguments).  No atomics: every sum over tokens or images runs in an order fixed by the shapes, so two calls give the same bits.  Same
+ * stream and allocation rules as kdb_model_forward. */
+int     kdb_model_set_grad(KdbModel* m, const char* key, float* data, const int64_t* shape, int ndim);
+int64_t kdb_model_train_workspace_bytes(const KdbModel* m, int batch, int height, int width);
+int     kdb_model_forward_train(KdbModel* m, int batch, int height, int width,
+                                const float* x, const float* sigma, const float* aug_cond, const int64_t* class_cond,
+                                const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
+                                const float* cotangent, float* out, float* grad_x,
+                                void* workspace, size_t workspace_bytes, void* stream);
 
 /* Debug/parity tap: arm a copy of one intermediate of the NEXT forward into `out` (fp32, device).
  * name: "patch_in", "L<l>.down", "L<l>.merge", "mid", "L<l>.split", "L<l>.up", "layer<k>.xn1",

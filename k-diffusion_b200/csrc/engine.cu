@@ -10,6 +10,7 @@
 #include <map>
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include "model_core.cuh"
@@ -57,6 +58,7 @@ struct KdbModel : ModelCore {
   int ada_total = 0;
   CondWeights cw{};
   std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
+  std::unordered_map<std::string, TensorRef> grads;      // kdb_model_set_grad: gradient buffers by state-dict key (written, p is not const)
 };
 
 namespace {
@@ -690,10 +692,13 @@ struct VjpSpace {
   std::vector<float*> g;      // per level: gradient of the residual stream [B, T_l, C_l]
   float *qkv_raw = nullptr;   // the qkv projection of the half being differentiated, before cosine-sim + RoPE
   float *dqkv = nullptr, *dbuf = nullptr, *dh = nullptr, *stats = nullptr;
+  // kdb_model_forward_train only (carve_vjp with train): the AdaRMSNorm scale gradients [B, ada_total] (the layout of the conditioning
+  // rows), the mapping network's output gradient [B, mw], its MapLayout rows, out_norm's rstd per token [B T0], the reduction partials
+  float *dscale = nullptr, *dcond = nullptr, *map_keep = nullptr, *map_grad = nullptr, *rstd = nullptr, *part = nullptr;
   size_t total = 0;
 };
 
-void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Workspace& ws, VjpSpace& vs) {
+void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Workspace& ws, VjpSpace& vs, int ada_total = 0, bool train = false) {
   Carver cv(workspace, 1024);
   carve(c, KDB_PREC_FP32, B, H, W, cv, ws);
   cv.off = ws.total;
@@ -725,13 +730,32 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Wo
   vs.dbuf = take(md);
   vs.dh = take(mh);
   vs.stats = take(mst);
+  if (train) {
+    const MapLayout ml{c.mapping_width, c.mapping_d_ff, c.mapping_depth};
+    vs.dscale = take((size_t)B * ada_total);
+    vs.dcond = take((size_t)B * c.mapping_width);
+    vs.map_keep = take((size_t)B * ml.keep_floats());
+    vs.map_grad = take((size_t)B * ml.grad_floats());
+    vs.rstd = take((size_t)B * T0);
+    vs.part = take((size_t)kTrainPartFloats);
+  }
   vs.total = cv.total();
 }
+
+// What kdb_model_forward_train adds to the reverse walk: the bound gradient buffers.
+struct Train {
+  const KdbModel* m;
+  float* grad(const std::string& key) const {
+    auto it = m->grads.find(key);
+    return it == m->grads.end() ? nullptr : const_cast<float*>(it->second.p);
+  }
+};
 
 // Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
 // its activations from the tape with the forward's functions (ff_up, attn_activations; f is an fp32 forward of B images), runs the
 // backward kernels and adds the branch gradient to g.
-int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w) {
+// tr != nullptr: also the gradients of the layer's weights, head scales and (into vs.dscale) AdaRMSNorm scales.
+int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, const Train* tr = nullptr) {
   const LayerPlan& L = m->layers[k];
   const int64_t Ttok = (int64_t)h * w, M = (int64_t)f.B * Ttok;
   const int C = L.C, F = L.dff;
@@ -743,28 +767,45 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w) 
   int rc;
   // feed-forward half: x + down(geglu(up(norm(x))))
   const float* x = vs.tape[2 * k + 1];
+  const std::string ff = L.prefix + "ff.", sa = L.prefix + "self_attn.";
   if ((rc = ff_up<float>(m, f, k, x, h, w))) return rc;
+  if (tr) {   // down_proj's input, the GEGLU output
+    float* gb = reinterpret_cast<float*>(f.ws.gbuf);
+    if ((rc = launch_geglu<float>(hb, gb, M, F, st)) || (rc = launch_wgrad(g, C, gb, F, tr->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
+      return rc;
+  }
   if ((rc = launch_gemm_vjp(g, L.down_w, vs.dbuf, M, C, F, VJP_STORE, 0, 0, 0, st))) return rc;
   if ((rc = launch_geglu_vjp(hb, vs.dbuf, vs.dh, M, F, st))) return rc;
+  if (tr && (rc = launch_wgrad(vs.dh, 2 * F, xn, C, tr->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
   if ((rc = launch_gemm_vjp(vs.dh, L.up_w, xn, M, 2 * F, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_ff, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   if ((rc = launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, st))) return rc;
   if (L.attn_type == KDB_ATTN_NONE) return 0;
   // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
   x = vs.tape[2 * k];
   if ((rc = attn_activations<float>(m, f, k, x, h, w, vs.qkv_raw))) return rc;
+  if (tr && (rc = launch_wgrad(g, C, ao, C, tr->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
   if ((rc = launch_gemm_vjp(g, L.out_w, vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
   if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
-  if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st))) return rc;
+  // the attention's statistics are spent: vs.stats takes the per-(row, head) terms of the head scales' gradient
+  if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st, tr ? vs.stats : nullptr)))
+    return rc;
+  if (tr && ((rc = launch_colsum(vs.stats, M, L.nh, tr->grad(sa + "scale"), vs.part, st)) ||
+             (rc = launch_wgrad(vs.dqkv, 3 * C, xn, C, tr->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
+    return rc;
   if ((rc = launch_gemm_vjp(vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_attn, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   return launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, st);
 }
 
 // out = the fp32 forward (bit for bit: the same launches, plus the tape copies), then grad_x = u^T J(x) by a walk of the forward in
 // reverse: patch_out + out_norm + combine; each up level's layers then its split-lerp; the mid layers; each down level (innermost
 // first) its merge then its layers; patch_in.
+// tr != nullptr (kdb_model_forward_train): along the walk, the gradients of patch_out, out_norm, every layer, split and merge, patch_in, and
+// the AdaRMSNorm scales into vs.dscale; grad_x may then be nullptr.
 int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, const float* sigma, float sd, const float* cond, int64_t cond_bs,
-             float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st) {
+             float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st, const Train* tr = nullptr) {
   const PosTables* pt = nullptr;
   int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data(), &pt);
   if (rc) return rc;
@@ -772,31 +813,61 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
   const int n = c.n_levels, C0 = c.width[0];
   const int h0 = H / c.patch_h, w0 = W / c.patch_w;
   Fwd f{B, ws, st, cond, cond_bs, pt, false, false, false, false};
+  const int64_t M0 = (int64_t)B * h0 * w0;
+  float* part = vs.part;
+  // training: the backward also leaves out_norm's output gradient (ws.xn) and rstd; patch_out's weight gradient then reads its output
+  // gradient (the patch rows of u) and its input (the out-normed stream) in place
+  float* dnorm = tr ? reinterpret_cast<float*>(ws.xn) : nullptr;
   if ((rc = launch_patch_out_vjp(vs.tape.back(), m->out_norm, m->patch_out_w, u, sigma, sd, vs.g[0], B, c.out_channels, H, W, c.patch_h,
-                                 c.patch_w, C0, st)))
+                                 c.patch_w, C0, st, dnorm, tr ? vs.rstd : nullptr)))
+    return rc;
+  if (tr && ((rc = launch_wgrad_patch_out(u, vs.tape.back(), m->out_norm, vs.rstd, tr->grad("patch_out.proj.weight"), B, c.out_channels, H, W,
+                                          c.patch_h, c.patch_w, C0, part, st)) ||
+             (rc = launch_norm_scale_grad(vs.tape.back(), C0, dnorm, C0, tr->grad("out_norm.scale"), 0, M0, M0, C0, part, st))))
     return rc;
   int k = (int)m->layers.size();
   float* mg = reinterpret_cast<float*>(ws.mg);
   for (int l = 0; l < n - 1; ++l) {
     const int h = h0 >> l, w = w0 >> l;
     for (int i = 0; i < c.depth[l]; ++i)
-      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w))) return rc;
+      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w, tr))) return rc;
+    // the split's input, the coarse stream it read: the mid level's output or the next level's up stream, both intact since the forward
+    const float* coarse = reinterpret_cast<const float*>(l == n - 2 ? ws.xs[n - 1] : ws.xup[l + 1]);
+    const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
+    const std::string sp = "splits." + std::to_string(l) + ".";
+    if (tr) {   // d fac = sum (y - skip) dup with y = the split projection recomputed (vs.dbuf), skip = ws.xs[l]
+      if ((rc = launch_gemm_simt<float, float>(coarse, m->split_w[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{}, st)) ||
+          (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], tr->grad(sp + "fac"), B, h, w, c.width[l],
+                                      part, st)))
+        return rc;
+    }
     // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
     if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
+    if (tr && (rc = launch_wgrad(mg, 4 * c.width[l], coarse, c.width[l + 1], tr->grad(sp + "proj.weight"), Mc, 4 * c.width[l], c.width[l + 1],
+                                 part, st)))
+      return rc;
     if ((rc = launch_gemm_vjp(mg, m->split_w[l], vs.g[l + 1], (int64_t)B * (h / 2) * (w / 2), 4 * c.width[l], c.width[l + 1], VJP_STORE, 0, 0, 0,
                               st)))
       return rc;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
-    if ((rc = vjp_layer(m, f, vs, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1)))) return rc;
+    if ((rc = vjp_layer(m, f, vs, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1), tr))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     const int h = h0 >> l, w = w0 >> l;
+    if (tr && (rc = launch_wgrad_merge(vs.g[l + 1], reinterpret_cast<const float*>(ws.xs[l]), tr->grad("merges." + std::to_string(l) + ".proj.weight"),
+                                       (int64_t)B * (h / 2) * (w / 2), c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
+      return rc;
     // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added
     if ((rc = launch_gemm_vjp(vs.g[l + 1], m->merge_w[l], vs.g[l], (int64_t)B * (h / 2) * (w / 2), c.width[l + 1], 4 * c.width[l],
                               VJP_UNPATCH_ACC, h / 2, w / 2, c.width[l], st)))
       return rc;
     for (int i = 0; i < c.depth[l]; ++i)
-      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w))) return rc;
+      if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w, tr))) return rc;
+  }
+  if (tr) {   // patch_in's input: the patch rows of x
+    if ((rc = launch_wgrad_patch_in(vs.g[0], x, tr->grad("patch_in.proj.weight"), B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, part, st)))
+      return rc;
+    if (grad_x == nullptr) return 0;
   }
   return launch_patch_in_vjp(vs.g[0], m->patch_in_w, u, sigma, sd, grad_x, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
 }
@@ -1068,6 +1139,112 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
   KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_vjp: workspace %zu < required %zu", workspace_bytes, vs.total);
   return m->disarm_tap(
       vjp_impl(m, batch, height, width, x, cotangent, sigma, sigma_data, cond, cond_batch_stride, out, grad_x, ws, vs, (cudaStream_t)stream));
+}
+
+}  // extern "C"
+
+namespace {
+
+// A gradient buffer for `key` is refused unless the model has a tensor of that key and shape that is a parameter (not a buffer)
+int check_grad_key(const KdbModel* m, const std::string& k, const std::vector<int64_t>& shape) {
+  auto it = m->tensors.find(k);
+  KDB_REQUIRE(it != m->tensors.end(), KDB_ERR_MISSING_KEY, "gradient bound to '%s', which is no tensor of the model", k.c_str());
+  KDB_REQUIRE(it->second.shape == shape, KDB_ERR_BAD_SHAPE, "gradient of '%s' has the wrong shape", k.c_str());
+  const bool buffer = k == "time_emb.weight" || k == "aug_emb.weight" || (k.size() >= 13 && k.compare(k.size() - 13, 13, "pos_emb.freqs") == 0);
+  KDB_REQUIRE(!buffer, KDB_ERR_BAD_ARG, "'%s' is a buffer, not a parameter", k.c_str());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int kdb_model_set_grad(KdbModel* m, const char* key, float* data, const int64_t* shape, int ndim) {
+  KDB_REQUIRE(m && key && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "set_grad: bad argument");
+  if (data == nullptr) {
+    m->grads.erase(key);
+    return 0;
+  }
+  if (int rc = check_grad_key(m, key, std::vector<int64_t>(shape, shape + ndim))) return rc;
+  ModelCore::TensorRef& t = m->grads[key];
+  t.p = data;
+  t.shape.assign(shape, shape + ndim);
+  return 0;
+}
+
+int64_t kdb_model_train_workspace_bytes(const KdbModel* m, int batch, int height, int width) {
+  KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "train_workspace_bytes: bad argument");
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "train_workspace_bytes: model not finalized");
+  Workspace ws;
+  VjpSpace vs;
+  carve_vjp(m->cfg, batch, height, width, nullptr, ws, vs, m->ada_total, true);
+  return (int64_t)vs.total;
+}
+
+int kdb_model_forward_train(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, const float* aug_cond,
+                            const int64_t* class_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
+                            const float* cotangent, float* out, float* grad_x, void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward_train: model not finalized");
+  const KdbModelConfig& c = m->cfg;
+  KDB_REQUIRE(c.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED,
+              "forward_train: image_transformer_v1 runs on weights permuted and folded at finalize; its parameter gradients are not built");
+  KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_train: NULL argument");
+  KDB_REQUIRE(!(c.num_classes > 0 && class_cond == nullptr), KDB_ERR_BAD_ARG, "class_cond must be specified if num_classes > 0");
+  KDB_REQUIRE(!(c.mapping_cond_dim > 0 && mapping_cond == nullptr), KDB_ERR_BAD_ARG, "mapping_cond must be specified if mapping_cond_dim > 0");
+  KDB_REQUIRE(cond_batch_stride == kdb_model_cond_stride(m), KDB_ERR_BAD_ARG,
+              "forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
+              (long long)kdb_model_cond_stride(m));
+  int rc;
+  for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
+    if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
+  if ((rc = check_image(m, "forward_train", height, width, 0.f))) return rc;
+  Workspace ws;
+  VjpSpace vs;
+  carve_vjp(c, batch, height, width, workspace, ws, vs, m->ada_total, true);
+  KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_train: workspace %zu < required %zu", workspace_bytes, vs.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  const Train tr{m};
+  if ((rc = m->disarm_tap(vjp_impl(m, batch, height, width, x, cotangent, sigma, 0.f, cond, cond_batch_stride, out, grad_x, ws, vs, st, &tr))))
+    return rc;
+  // AdaRMSNorm: scale = 1 + cond W^T per image, so d W = sum_b dscale_b cond_b (cond: the last mw floats of the conditioning row) and the
+  // mapping network's output gets dscale W over every layer at once (ada_cat: the layers' W stacked in the order of the scales)
+  const int B = batch, mw = c.mapping_width, A = m->ada_total;
+  const float* cond_vec = cond + A;
+  float* part = vs.part;
+  for (const LayerPlan& L : m->layers) {
+    if (L.ada_attn >= 0 &&
+        (rc = launch_wgrad(vs.dscale + L.ada_attn, A, cond_vec, cond_batch_stride, tr.grad(L.prefix + "self_attn.norm.linear.weight"), B, L.C, mw,
+                           part, st)))
+      return rc;
+    if ((rc = launch_wgrad(vs.dscale + L.ada_ff, A, cond_vec, cond_batch_stride, tr.grad(L.prefix + "ff.norm.linear.weight"), B, L.C, mw, part, st)))
+      return rc;
+  }
+  if ((rc = launch_gemm_vjp(vs.dscale, m->ada_cat, vs.dcond, B, A, mw, VJP_STORE, 0, 0, 0, st)) ||
+      (rc = launch_mapping_backward(m->cw, B, sigma, aug_cond, class_cond, mapping_cond, vs.dcond, vs.map_keep, vs.map_grad, st)))
+    return rc;
+  // the mapping network's weights from the activations and gradients its backward left per row
+  const MapLayout ml{mw, c.mapping_d_ff, c.mapping_depth};
+  const int64_t K = ml.keep_floats(), G = ml.grad_floats();
+  const float *keep = vs.map_keep, *grad = vs.map_grad;
+  const int D = c.mapping_depth, F = c.mapping_d_ff;
+  if ((rc = launch_norm_scale_grad(keep + ml.r(D), K, vs.dcond, mw, tr.grad("mapping.out_norm.scale"), 0, B, B, mw, part, st))) return rc;
+  for (int l = 0; l < D; ++l) {
+    const std::string p = "mapping.blocks." + std::to_string(l) + ".";
+    if ((rc = launch_norm_scale_grad(keep + ml.r(l), K, grad + ml.dxn(l), G, tr.grad(p + "norm.scale"), 0, B, B, mw, part, st)) ||
+        (rc = launch_wgrad(grad + ml.dh(l), G, keep + ml.xn(l), K, tr.grad(p + "up_proj.weight"), B, 2 * F, mw, part, st)) ||
+        (rc = launch_wgrad(grad + ml.dr(l + 1), G, keep + ml.g(l), K, tr.grad(p + "down_proj.weight"), B, mw, F, part, st)))
+      return rc;
+  }
+  const float* demb = grad + ml.demb();
+  if ((rc = launch_norm_scale_grad(keep + ml.emb(), K, grad + ml.dr(0), G, tr.grad("mapping.in_norm.scale"), 0, B, B, mw, part, st)) ||
+      (rc = launch_wgrad(demb, G, keep + ml.ff_t(), K, tr.grad("time_in_proj.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_wgrad(demb, G, keep + ml.ff_a(), K, tr.grad("aug_in_proj.weight"), B, mw, mw, part, st)))
+    return rc;
+  if (c.mapping_cond_dim > 0 &&
+      (rc = launch_wgrad(demb, G, mapping_cond, c.mapping_cond_dim, tr.grad("mapping_cond_in_proj.weight"), B, mw, c.mapping_cond_dim, part, st)))
+    return rc;
+  if (c.num_classes > 0) return launch_class_emb_grad(demb, G, class_cond, tr.grad("class_emb.weight"), B, c.num_classes, mw, st);
+  return 0;
 }
 
 int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

@@ -17,30 +17,6 @@ constexpr float kEps = 1e-6f;   // RMSNorm / cosine-sim eps (image_transformer_v
 // grid of a grid-stride kernel of 256 threads over n elements
 static unsigned grid_stride_blocks(int64_t n) { return (unsigned)std::min<int64_t>(ceil_div(n, 256), kNumSMs * 16); }
 
-// NCHW offset of patch column n = (nh, nw, c) of token (ty, tx) of image b: channel c of pixel (ty ph + nh, tx pw + nw)
-__device__ __forceinline__ int64_t patch_pixel(int b, int ty, int tx, int n, int C, int H, int W, int ph, int pw) {
-  const int q = n / C, c = n - q * C;
-  const int nh = q / pw, nw = q - nh * pw;
-  return nchw_offset(b, c, ty * ph + nh, tx * pw + nw, C, H, W);
-}
-
-// TokenMerge / TokenSplit 2x2 order (image_transformer_v2.py:594,618): channel e of quadrant q = 2 nh + nw of coarse token (hy, wx)
-// of image b is channel e of fine token (2 hy + nh, 2 wx + nw) of [B, 2 hc, 2 wc, Cf]
-__device__ __forceinline__ int64_t fine_offset(int64_t b, int hy, int wx, int q, int e, int hc, int wc, int Cf) {
-  return ((b * (2 * hc) + (2 * hy + (q >> 1))) * (2 * wc) + (2 * wx + (q & 1))) * Cf + e;
-}
-// element i of a coarse [B, hc, wc, 4 Cf] tensor in that order -> offset of its fine element
-__device__ __forceinline__ int64_t merge_source(int64_t i, int hc, int wc, int Cf) {
-  const int e = (int)(i % Cf);
-  int64_t r = i / Cf;
-  const int q = (int)(r & 3);
-  r >>= 2;
-  const int wx = (int)(r % wc);
-  r /= wc;
-  const int hy = (int)(r % hc);
-  return fine_offset(r / hc, hy, wx, q, e, hc, wc, Cf);
-}
-
 // Tangent of a row norm y = x r, r = rsqrt(ss / n + eps), ss = sum x^2 (RMSNorm: n = row width; cosine-sim: n = 1, the layer's eps), along
 // u with sd = x . u: dy = r u - x r^3 sd / n.  The row sums are the caller's.
 struct NormTangent {
@@ -963,8 +939,10 @@ int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* 
 // In place on the q and k thirds of dqkv: g = R(theta)^T dq^ (rotate by -theta on the primal's column pairs), then
 // dq = sqrt(scale) (rho g - q rho^3 (q . g)), rho = rsqrt(sum q^2 + eps) of the un-normalised primal q in qkv.  One warp per
 // (token row, head).
+// dscale != nullptr: dscale[row, h] = (g_q . q rho_q + g_k . k rho_k) / (2 sqrt(scale)), the (row, head) term of d scale_h.
 __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __restrict__ qkv, float* __restrict__ dqkv,
-                                                              const float* __restrict__ pos, const QkRope qr, int64_t rows, int Ttok, int nh, int e) {
+                                                              const float* __restrict__ pos, const QkRope qr, int64_t rows, int Ttok, int nh, int e,
+                                                              float* __restrict__ dscale) {
   extern __shared__ float sm[];   // [warps][e]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp;
@@ -975,6 +953,7 @@ __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __res
   const float py = pos[(row % Ttok) * 2 + 0], px = pos[(row % Ttok) * 2 + 1];
   const float sqs = sqrtf(qr.scale[h]);
   const float* f = qr.freqs + h * (qr.R / 2);
+  float ds = 0.f;
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
     const int64_t off = (row * 3 + t) * (int64_t)nh * e + (int64_t)h * e;
@@ -987,17 +966,20 @@ __global__ void __launch_bounds__(128) qknorm_rope_vjp_kernel(const float* __res
       ss = fmaf(v[d], v[d], ss);
       sg = fmaf(v[d], buf[d], sg);
     }
-    const NormTangent nt(warp_sum(ss), warp_sum(sg), 1.f, qr.eps);
+    const float sgs = warp_sum(sg);
+    const NormTangent nt(warp_sum(ss), sgs, 1.f, qr.eps);
     for (int d = lane; d < e; d += 32) dv[d] = sqs * nt(v[d], buf[d]);
+    if (dscale != nullptr) ds = fmaf(sgs, nt.r, ds);
     __syncwarp();
   }
+  if (dscale != nullptr && lane == 0) dscale[item] = ds / (2.f * sqs);
 }
 
 int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
-                           cudaStream_t st) {
+                           cudaStream_t st, float* dscale_rows) {
   if (int rc = check_qk_rope("qknorm_rope_vjp", qr, e)) return rc;
   const size_t smem = sizeof(float) * 4 * e;
-  qknorm_rope_vjp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, qr, rows, T_tokens, nh, e);
+  qknorm_rope_vjp_kernel<<<(unsigned)ceil_div(rows * nh, 4), 128, smem, st>>>(qkv, dqkv, pos, qr, rows, T_tokens, nh, e, dscale_rows);
   KDB_LAUNCH_CHECK(F_QKNORM_ROPE, st);
   return 0;
 }
@@ -1180,7 +1162,7 @@ int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int
 __global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restrict__ tokens, const float* __restrict__ nscale,
                                                             const float* __restrict__ W, const float* __restrict__ u, const float* __restrict__ sigma,
                                                             float sd, float* __restrict__ dtokens, int Cout, int H, int Wd, int ph, int pw,
-                                                            int C0, int64_t tokens_total) {
+                                                            int C0, int64_t tokens_total, float* __restrict__ dnorm, float* __restrict__ rstd) {
   extern __shared__ float sm[];   // [warps][C0 + N]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t tok = (int64_t)blockIdx.x * 4 + warp;
@@ -1209,15 +1191,18 @@ __global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restr
   const NormTangent nt(warp_sum(ss), warp_sum(sdot), (float)C0);
   float* dr = dtokens + tok * C0;
   for (int c = lane; c < C0; c += 32) dr[c] = nt(xr[c], __ldg(nscale + c) * dn[c]);
+  if (dnorm != nullptr)
+    for (int c = lane; c < C0; c += 32) dnorm[tok * C0 + c] = dn[c];
+  if (rstd != nullptr && lane == 0) rstd[tok] = nt.r;
 }
 
 int launch_patch_out_vjp(const float* tokens, const float* norm_scale, const float* W, const float* u, const float* sigma, float sigma_data,
-                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st) {
+                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st, float* dnorm, float* rstd) {
   const int64_t tok = (int64_t)B * (H / ph) * (Wd / pw);
   const size_t smem = sizeof(float) * 4 * (size_t)(C0 + ph * pw * Cout);
   KDB_REQUIRE(smem <= 48 * 1024, KDB_ERR_UNSUPPORTED, "patch_out_vjp: width %d too large", C0);
   patch_out_vjp_kernel<<<(unsigned)ceil_div(tok, 4), 128, smem, st>>>(tokens, norm_scale, W, u, sigma, sigma_data, dtokens, Cout, H, Wd, ph, pw,
-                                                                      C0, tok);
+                                                                      C0, tok, dnorm, rstd);
   KDB_LAUNCH_CHECK(F_PATCH_OUT, st);
   return 0;
 }
@@ -1311,19 +1296,17 @@ __device__ __forceinline__ void block_rmsnorm(const float* x, float* y, const fl
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(256) conditioning_kernel(const CondWeights w, const float* __restrict__ sigma,
-                                                           const float* __restrict__ aug, const int64_t* __restrict__ cls,
-                                                           const float* __restrict__ mcond, float* __restrict__ out, int64_t out_stride) {
-  extern __shared__ float4 cond_sm4[];          // 16-byte aligned: block_matvec reads its input vector as float4
-  float* sm = reinterpret_cast<float*>(cond_sm4);
+// Where map_forward leaves each activation of one conditioning row.  The conditioning kernel aliases them onto a few shared-memory
+// vectors (every r[l] is one in-place stream, g[l] overwrites up[l]); the mapping backward gives each its own slot of a MapLayout row.
+struct MapBufs {
+  float *ff_t, *ff_a, *emb, *mc, *red, *cond;
+  float *r[9], *xn[8], *up[8], *g[8];
+};
+
+// FourierFeatures -> in-proj -> MappingNetwork of conditioning row `row` (image_transformer_v2.py:552-581,734-740): cond = b.cond
+__device__ void map_forward(const CondWeights& w, int row, const float* __restrict__ sigma, const float* __restrict__ aug,
+                            const int64_t* __restrict__ cls, const float* __restrict__ mcond, const MapBufs& b) {
   const int mw = w.mw, dff = w.dff;
-  float* ff = sm;              // [mw]   fourier features
-  float* emb = ff + mw;        // [mw]   summed embedding / residual stream
-  float* xn = emb + mw;        // [mw]
-  float* up = xn + mw;         // [2*dff]
-  float* red = up + 2 * dff;   // [32]
-  float* mc = red + 32;        // [mcond_dim]
-  const int row = blockIdx.x;
   const int half = mw / 2;
   const float two_pi = 6.283185307179586f;
 
@@ -1333,11 +1316,11 @@ __global__ void __launch_bounds__(256) conditioning_kernel(const CondWeights w, 
     const float f = (two_pi * c_noise) * __ldg(w.time_emb + j);
     float s, c;
     sincosf(f, &s, &c);
-    ff[j] = c;
-    ff[half + j] = s;
+    b.ff_t[j] = c;
+    b.ff_t[half + j] = s;
   }
   __syncthreads();
-  block_matvec(w.time_in, ff, emb, 0, mw, mw, false);
+  block_matvec(w.time_in, b.ff_t, b.emb, 0, mw, mw, false);
   __syncthreads();
   // augmentation embedding (zeros when aug_cond is None, :736-737)
   for (int j = threadIdx.x; j < half; j += blockDim.x) {
@@ -1346,35 +1329,60 @@ __global__ void __launch_bounds__(256) conditioning_kernel(const CondWeights w, 
       for (int k = 0; k < 9; ++k) f = fmaf(two_pi * aug[(int64_t)row * 9 + k], __ldg(w.aug_emb + j * 9 + k), f);
     float s, c;
     sincosf(f, &s, &c);
-    ff[j] = c;
-    ff[half + j] = s;
+    b.ff_a[j] = c;
+    b.ff_a[half + j] = s;
   }
   __syncthreads();
-  block_matvec(w.aug_in, ff, emb, 0, mw, mw, true);
+  block_matvec(w.aug_in, b.ff_a, b.emb, 0, mw, mw, true);
   __syncthreads();
   if (w.class_emb != nullptr) {
     const int64_t ci = cls[row];
-    for (int j = threadIdx.x; j < mw; j += blockDim.x) emb[j] += __ldg(w.class_emb + ci * mw + j);
+    for (int j = threadIdx.x; j < mw; j += blockDim.x) b.emb[j] += __ldg(w.class_emb + ci * mw + j);
   }
   if (w.mcond_in != nullptr) {
-    for (int j = threadIdx.x; j < w.mcond_dim; j += blockDim.x) mc[j] = mcond[(int64_t)row * w.mcond_dim + j];
+    for (int j = threadIdx.x; j < w.mcond_dim; j += blockDim.x) b.mc[j] = mcond[(int64_t)row * w.mcond_dim + j];
     __syncthreads();
-    block_matvec(w.mcond_in, mc, emb, 0, mw, w.mcond_dim, true);
+    block_matvec(w.mcond_in, b.mc, b.emb, 0, mw, w.mcond_dim, true);
   }
   __syncthreads();
 
   // MappingNetwork (:569-581)
-  block_rmsnorm(emb, emb, w.in_norm, mw, red);
+  block_rmsnorm(b.emb, b.r[0], w.in_norm, mw, b.red);
   for (int l = 0; l < w.depth; ++l) {
-    block_rmsnorm(emb, xn, w.blk_norm[l], mw, red);
-    block_matvec(w.blk_up[l], xn, up, 0, 2 * dff, mw, false);
+    block_rmsnorm(b.r[l], b.xn[l], w.blk_norm[l], mw, b.red);
+    block_matvec(w.blk_up[l], b.xn[l], b.up[l], 0, 2 * dff, mw, false);
     __syncthreads();
-    for (int i = threadIdx.x; i < dff; i += blockDim.x) up[i] = up[i] * gelu_erf(up[dff + i]);
+    for (int i = threadIdx.x; i < dff; i += blockDim.x) b.g[l][i] = b.up[l][i] * gelu_erf(b.up[l][dff + i]);
+    if (b.r[l + 1] != b.r[l])
+      for (int i = threadIdx.x; i < mw; i += blockDim.x) b.r[l + 1][i] = b.r[l][i];
     __syncthreads();
-    block_matvec(w.blk_down[l], up, emb, 0, mw, dff, true);
+    block_matvec(w.blk_down[l], b.g[l], b.r[l + 1], 0, mw, dff, true);
     __syncthreads();
   }
-  block_rmsnorm(emb, xn, w.out_norm, mw, red);
+  block_rmsnorm(b.r[w.depth], b.cond, w.out_norm, mw, b.red);
+}
+
+__global__ void __launch_bounds__(256) conditioning_kernel(const CondWeights w, const float* __restrict__ sigma,
+                                                           const float* __restrict__ aug, const int64_t* __restrict__ cls,
+                                                           const float* __restrict__ mcond, float* __restrict__ out, int64_t out_stride) {
+  extern __shared__ float4 cond_sm4[];          // 16-byte aligned: block_matvec reads its input vector as float4
+  float* sm = reinterpret_cast<float*>(cond_sm4);
+  const int mw = w.mw, dff = w.dff;
+  MapBufs b;
+  b.ff_t = b.ff_a = sm;        // [mw]   fourier features
+  b.emb = b.ff_t + mw;         // [mw]   summed embedding / residual stream
+  float* xn = b.emb + mw;      // [mw]
+  float* up = xn + mw;         // [2*dff]
+  b.red = up + 2 * dff;        // [32]
+  b.mc = b.red + 32;           // [mcond_dim]
+  b.cond = xn;
+  for (int l = 0; l <= 8; ++l) b.r[l] = b.emb;
+  for (int l = 0; l < 8; ++l) {
+    b.xn[l] = xn;
+    b.up[l] = b.g[l] = up;
+  }
+  const int row = blockIdx.x;
+  map_forward(w, row, sigma, aug, cls, mcond, b);
 
   // every AdaRMSNorm: scale = Linear(cond) + 1   (:166).  The CTAs of one row (gridDim.y) share the outputs; each repeats the
   // (short) mapping network so that no second launch or grid-wide hand-off is needed.
@@ -1392,6 +1400,92 @@ int launch_conditioning(const CondWeights& w, int rows, const float* sigma, cons
   const size_t smem = sizeof(float) * (size_t)(3 * w.mw + 2 * w.dff + 32 + w.mcond_dim);
   KDB_REQUIRE(smem <= 48 * 1024, KDB_ERR_UNSUPPORTED, "conditioning: mapping network too wide");
   conditioning_kernel<<<dim3((unsigned)rows, 4), 256, smem, st>>>(w, sigma, aug, cls, mcond, out, out_stride);
+  KDB_LAUNCH_CHECK(F_COND, st);
+  return 0;
+}
+
+// dx (+)= the input gradient of y = x * scale * rsqrt(mean(x^2) + eps) (block_rmsnorm) for the output gradient dy, vectors of n
+__device__ __forceinline__ void block_rmsnorm_vjp(const float* x, const float* dy, const float* __restrict__ scale, float* dx, int n, float* red,
+                                                  bool accumulate) {
+  float ss = 0.f, sd = 0.f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    ss = fmaf(x[i], x[i], ss);
+    sd = fmaf(x[i], __ldg(scale + i) * dy[i], sd);
+  }
+  ss = block_sum(ss, red);
+  sd = block_sum(sd, red);
+  const NormTangent nt(ss, sd, (float)n);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float v = nt(x[i], __ldg(scale + i) * dy[i]);
+    dx[i] = accumulate ? dx[i] + v : v;
+  }
+  __syncthreads();
+}
+
+// vout[k] = sum over o < n_rows of W[o, k] vin[o] for k < n_cols (the input gradient of block_matvec), o in order
+__device__ __forceinline__ void block_matvec_t(const float* __restrict__ W, const float* vin, float* vout, int n_rows, int n_cols) {
+  for (int k = threadIdx.x; k < n_cols; k += blockDim.x) {
+    float s = 0.f;
+    for (int o = 0; o < n_rows; ++o) s = fmaf(__ldg(W + (int64_t)o * n_cols + k), vin[o], s);
+    vout[k] = s;
+  }
+}
+
+// One CTA per conditioning row: map_forward into the row's MapLayout slots of keep, then the reverse walk out_norm, the blocks (last
+// first), in_norm, from dcond into the row of grad.
+__global__ void __launch_bounds__(256) mapping_backward_kernel(const CondWeights w, const MapLayout L, const float* __restrict__ sigma,
+                                                               const float* __restrict__ aug, const int64_t* __restrict__ cls,
+                                                               const float* __restrict__ mcond, const float* __restrict__ dcond,
+                                                               float* __restrict__ keep, float* __restrict__ grad) {
+  extern __shared__ float4 map_bwd_sm4[];
+  float* sm = reinterpret_cast<float*>(map_bwd_sm4);
+  const int mw = w.mw, dff = w.dff, D = w.depth;
+  const int row = blockIdx.x;
+  float* k = keep + (int64_t)row * L.keep_floats();
+  float* g = grad + (int64_t)row * L.grad_floats();
+  MapBufs b;
+  b.mc = sm;                                     // [mcond_dim], 16-byte aligned for block_matvec
+  b.red = sm + ((w.mcond_dim + 3) & ~3);         // [32]
+  float* dg = b.red + 32;                        // [dff]
+  b.ff_t = k + L.ff_t();
+  b.ff_a = k + L.ff_a();
+  b.emb = k + L.emb();
+  b.cond = g + L.demb();                         // the recomputed cond is not needed: scratch until demb is written
+  for (int l = 0; l <= D; ++l) b.r[l] = k + L.r(l);
+  for (int l = 0; l < D; ++l) {
+    b.xn[l] = k + L.xn(l);
+    b.up[l] = k + L.up(l);
+    b.g[l] = k + L.g(l);
+  }
+  map_forward(w, row, sigma, aug, cls, mcond, b);
+
+  block_rmsnorm_vjp(b.r[D], dcond + (int64_t)row * mw, w.out_norm, g + L.dr(D), mw, b.red, false);
+  for (int l = D - 1; l >= 0; --l) {
+    const float* dr1 = g + L.dr(l + 1);
+    float *dxn = g + L.dxn(l), *dh = g + L.dh(l), *dr = g + L.dr(l);
+    block_matvec_t(w.blk_down[l], dr1, dg, mw, dff);
+    __syncthreads();
+    for (int i = threadIdx.x; i < dff; i += blockDim.x) {   // GEGLU backward, as geglu_vjp_kernel
+      float gelu, slope;
+      gelu_erf_slope(b.up[l][dff + i], gelu, slope);
+      dh[i] = dg[i] * gelu;
+      dh[dff + i] = dg[i] * (b.up[l][i] * slope);
+    }
+    for (int i = threadIdx.x; i < mw; i += blockDim.x) dr[i] = dr1[i];   // the residual branch
+    __syncthreads();
+    block_matvec_t(w.blk_up[l], dh, dxn, 2 * dff, mw);
+    __syncthreads();
+    block_rmsnorm_vjp(b.r[l], dxn, w.blk_norm[l], dr, mw, b.red, true);
+  }
+  block_rmsnorm_vjp(b.emb, g + L.dr(0), w.in_norm, g + L.demb(), mw, b.red, false);
+}
+
+int launch_mapping_backward(const CondWeights& w, int rows, const float* sigma, const float* aug, const int64_t* cls, const float* mcond,
+                            const float* dcond, float* keep, float* grad, cudaStream_t st) {
+  KDB_REQUIRE(w.mw % 4 == 0 && w.dff % 2 == 0 && w.depth <= 8, KDB_ERR_UNSUPPORTED, "mapping backward: mapping width must be a multiple of 4, depth <= 8");
+  const size_t smem = sizeof(float) * (size_t)(((w.mcond_dim + 3) & ~3) + 32 + w.dff);
+  KDB_REQUIRE(smem <= 48 * 1024, KDB_ERR_UNSUPPORTED, "mapping backward: mapping network too wide");
+  mapping_backward_kernel<<<(unsigned)rows, 256, smem, st>>>(w, MapLayout{w.mw, w.dff, w.depth}, sigma, aug, cls, mcond, dcond, keep, grad);
   KDB_LAUNCH_CHECK(F_COND, st);
   return 0;
 }

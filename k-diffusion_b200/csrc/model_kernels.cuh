@@ -41,6 +41,30 @@ struct GemmEpi {
   int H = 0, W = 0;
 };
 
+// NCHW offset of patch column n = (nh, nw, c) of token (ty, tx) of image b: channel c of pixel (ty ph + nh, tx pw + nw)
+__device__ __forceinline__ int64_t patch_pixel(int b, int ty, int tx, int n, int C, int H, int W, int ph, int pw) {
+  const int q = n / C, c = n - q * C;
+  const int nh = q / pw, nw = q - nh * pw;
+  return nchw_offset(b, c, ty * ph + nh, tx * pw + nw, C, H, W);
+}
+
+// TokenMerge / TokenSplit 2x2 order (image_transformer_v2.py:594,618): channel e of quadrant q = 2 nh + nw of coarse token (hy, wx)
+// of image b is channel e of fine token (2 hy + nh, 2 wx + nw) of [B, 2 hc, 2 wc, Cf]
+__device__ __forceinline__ int64_t fine_offset(int64_t b, int hy, int wx, int q, int e, int hc, int wc, int Cf) {
+  return ((b * (2 * hc) + (2 * hy + (q >> 1))) * (2 * wc) + (2 * wx + (q & 1))) * Cf + e;
+}
+// element i of a coarse [B, hc, wc, 4 Cf] tensor in that order -> offset of its fine element
+__device__ __forceinline__ int64_t merge_source(int64_t i, int hc, int wc, int Cf) {
+  const int e = (int)(i % Cf);
+  int64_t r = i / Cf;
+  const int q = (int)(r & 3);
+  r >>= 2;
+  const int wx = (int)(r % wc);
+  r /= wc;
+  const int hy = (int)(r % hc);
+  return fine_offset(r / hc, hy, wx, q, e, hc, wc, Cf);
+}
+
 // x [B,C,H,W] fp32 (* c_in(sigma) if sigma_data > 0) -> tokens [B, H/ph, W/pw, N]   (image_transformer_v2.py:586-595,723-724)
 template <typename T>
 int launch_patch_in(const float* x, const float* sigma, float sigma_data, const float* W, T* out, int B, int C, int H, int Wd,
@@ -118,9 +142,10 @@ int launch_gemm_vjp(const float* dC, const float* W, float* out, int64_t M, int 
 // RMSNorm: dx += r (s dy) - x r^3 mean(x s dy), r = rsqrt(mean(x^2) + eps); scale rows as launch_rmsnorm
 int launch_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_batch,
                        int64_t rows, int C, cudaStream_t st);
-// cosine-sim scale + RoPE, in place on the q, k thirds of dqkv [rows, 3, nh, e] (v passes through); qkv = the primal BEFORE launch_qknorm_rope
+// cosine-sim scale + RoPE, in place on the q, k thirds of dqkv [rows, 3, nh, e] (v passes through); qkv = the primal BEFORE launch_qknorm_rope.
+// dscale_rows != nullptr: also [rows, nh] the contribution of each (row, head) to the gradient of the head's scale
 int launch_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const QkRope& qr, int64_t rows, int T_tokens, int nh, int e,
-                           cudaStream_t st);
+                           cudaStream_t st, float* dscale_rows = nullptr);
 // attention over the key set of launch_attention_generic: qkv the normalised, rotated primal, out its output, dout the output gradient
 // -> dqkv [B, T, 3, nh, e].  stats: scratch of B * nh * T * 3 floats (per-query softmax statistics handed from the query-centric pass
 // to the key-centric one)
@@ -131,8 +156,11 @@ int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int 
 // TokenSplit lerp: out [B, H/2, W/2, 4C] = patch2x2(fac dup) (then launch_gemm_vjp with the split weight), dup *= (1 - fac) in place
 int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int H, int Wd, int C, cudaStream_t st);
 // out_norm + patch_out + un-patch: dtokens = RMSNorm_vjp(tokens, patch(c_out u) W_po)  (c_out = 1 when sigma_data <= 0)
+// Where given, also dnorm [tokens, C0] the gradient of out_norm's output and rstd [tokens] each token's rsqrt(mean(x^2) + eps) as the
+// forward computes it
 int launch_patch_out_vjp(const float* tokens, const float* norm_scale, const float* W, const float* u, const float* sigma, float sigma_data,
-                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st);
+                         float* dtokens, int B, int Cout, int H, int Wd, int ph, int pw, int C0, cudaStream_t st, float* dnorm = nullptr,
+                         float* rstd = nullptr);
 // patch_in: grad_x = c_skip u + c_in unpatch(dtokens W_pi) (sigma_data > 0), else unpatch(dtokens W_pi)
 int launch_patch_in_vjp(const float* dtokens, const float* W, const float* u, const float* sigma, float sigma_data, float* grad_x, int B, int C,
                         int H, int Wd, int ph, int pw, int N, cudaStream_t st);
@@ -157,6 +185,60 @@ struct CondWeights {
 };
 int launch_conditioning(const CondWeights& w, int rows, const float* sigma, const float* aug, const int64_t* cls, const float* mcond,
                         float* out, int64_t out_stride, cudaStream_t st);
+
+// The mapping network's backward, one CTA per conditioning row (train_kernels.cu reduces what it leaves into the weight gradients).
+// Per row it recomputes the forward of launch_conditioning into `keep` and, from dcond [rows, mw] (the gradient of the mapping network's
+// output), writes the gradients of the activations into `grad`.  MapLayout gives the offsets of each vector in a row of either.
+struct MapLayout {
+  int mw, dff, depth;
+  // keep: Fourier features of sigma and of aug_cond, the summed embedding entering in_norm, the stream r[l] entering block l (r[depth]:
+  // entering out_norm), each block's normed input, up_proj output (value | gate) and GEGLU output
+  __host__ __device__ int ff_t() const { return 0; }
+  __host__ __device__ int ff_a() const { return mw; }
+  __host__ __device__ int emb() const { return 2 * mw; }
+  __host__ __device__ int r(int l) const { return 3 * mw + l * mw; }
+  __host__ __device__ int xn(int l) const { return r(depth + 1) + l * blk(); }
+  __host__ __device__ int up(int l) const { return xn(l) + mw; }
+  __host__ __device__ int g(int l) const { return up(l) + 2 * dff; }
+  __host__ __device__ int blk() const { return mw + 2 * dff + ((dff + 3) & ~3); }
+  __host__ __device__ int keep_floats() const { return xn(depth); }
+  // grad: d r[l] (l <= depth), d(normed input) and d(up_proj output) of block l, d(embedding entering in_norm)
+  __host__ __device__ int dr(int l) const { return l * mw; }
+  __host__ __device__ int dxn(int l) const { return (depth + 1) * mw + l * (mw + 2 * dff); }
+  __host__ __device__ int dh(int l) const { return dxn(l) + mw; }
+  __host__ __device__ int demb() const { return dxn(depth); }
+  __host__ __device__ int grad_floats() const { return demb() + mw; }
+};
+int launch_mapping_backward(const CondWeights& w, int rows, const float* sigma, const float* aug, const int64_t* cls, const float* mcond,
+                            const float* dcond, float* keep, float* grad, cudaStream_t st);
+
+// Parameter-gradient reductions (train_kernels.cu), fp32.  No atomics; every sum runs in an order fixed by the shapes alone, so two calls
+// give the same bits.  `part` is scratch of kTrainPartFloats floats (reduction partials).  A NULL output skips the launch.
+constexpr int64_t kTrainPartFloats = int64_t(1) << 22;
+// dW[N, K] = sum over the rows m < M of dY[m, n] X[m, k] (the weight gradient of Y = X W^T); dY and X rows ldy, ldx floats apart
+int launch_wgrad(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part, cudaStream_t st);
+// the same with X the TokenMerge gather of the fine tokens [B, 2hc, 2wc, Cf] (M = B hc wc coarse rows, K = 4 Cf) read in place
+int launch_wgrad_merge(const float* dY, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part, cudaStream_t st);
+// out[b * ldo + c] = sum over the rows r of image b of dy[r, c] x[r, c] rsqrt(mean(x_r^2) + eps): the gradient of an RMSNorm's channel scale
+// per image (rows_per_batch rows each; rows_per_batch == rows: one sum over all rows)
+int launch_norm_scale_grad(const float* x, int64_t ldx, const float* dy, int64_t ldy, float* out, int64_t ldo, int64_t rows_per_batch,
+                           int64_t rows, int C, float* part, cudaStream_t st);
+// out[c] = sum over r < rows of P[r, c]
+int launch_colsum(const float* P, int64_t rows, int C, float* out, float* part, cudaStream_t st);
+// the gradient of TokenSplit's fac: sum of (y - skip) dup, y [B, H/2, W/2, 4C] the split projection in TokenMerge order, skip and dup
+// (the gradient of the split's output) [B, H, W, C]
+int launch_split_fac_grad(const float* y, const float* skip, const float* dup, float* out, int B, int H, int Wd, int C, float* part,
+                          cudaStream_t st);
+// patch_in's weight gradient: dW [N, (nh nw c)] = sum over tokens of dtok[tok, n] times the patch row of the NCHW image x [B, C, H, W],
+// read in place
+int launch_wgrad_patch_in(const float* dtok, const float* x, float* dW, int B, int C, int H, int Wd, int ph, int pw, int N, float* part,
+                          cudaStream_t st);
+// patch_out's weight gradient: dW [(nh nw c), C0] = sum over tokens of the patch row of u [B, C, H, W] times out_norm's output, both read
+// in place (the output as tokens [B T, C0] * (scale * rstd), rstd from launch_patch_out_vjp)
+int launch_wgrad_patch_out(const float* u, const float* tokens, const float* scale, const float* rstd, float* dW, int B, int C, int H, int Wd,
+                           int ph, int pw, int C0, float* part, cudaStream_t st);
+// class_emb's gradient: out[k, :] = sum over the rows r with cls[r] == k of demb[r, :] (ld ldd), rows in order; every row k < n_classes written
+int launch_class_emb_grad(const float* demb, int64_t ldd, const int64_t* cls, float* out, int rows, int n_classes, int mw, cudaStream_t st);
 
 // (cos, sin) table of the axial RoPE angles of QkRope with R = 4 nf: theta_j = (j < nf ? pos_y : pos_x)[t] * freqs[h, j], j < 2 nf
 int launch_rope_table(const float* pos, const float* freqs, float2* out, int T_tokens, int nh, int nf, cudaStream_t st);

@@ -190,7 +190,7 @@ static int ew_launch(const EwParams& p, int n_in, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------------
 // Karras preconditioner around an opaque inner model
 // ------------------------------------------------------------------------------------------------
-template <int MODE>   // 0: x*c_in   1: f*c_out + x*c_skip   2: (x - f)/sigma
+template <int MODE>   // 0: x*c_in   1: f*c_out + x*c_skip   2: (x - f)/sigma   3: (x + f*sigma)*c_in (f: the noise of a training loss)
 __global__ void __launch_bounds__(256) precond_kernel(const float* __restrict__ f, const float* __restrict__ x,
                                                       const float* __restrict__ sigma, float sd, float* __restrict__ out,
                                                       int64_t per_sample, int64_t total) {
@@ -203,6 +203,8 @@ __global__ void __launch_bounds__(256) precond_kernel(const float* __restrict__ 
       karras_scalings(sigma[b], sd, c_skip, c_out, c_in);
       if constexpr (MODE == 1)
         out[i] = f[i] * c_out + x[i] * c_skip;
+      else if constexpr (MODE == 3)
+        out[i] = __fmul_rn(__fadd_rn(x[i], __fmul_rn(f[i], sigma[b])), c_in);
       else
         out[i] = x[i] * c_in;
     }
@@ -641,6 +643,57 @@ int kdb_precond_combine(const float* f, const float* x, const float* sigma, floa
   KDB_REQUIRE(f && x && sigma && out && batch > 0 && per_sample > 0, KDB_ERR_BAD_ARG, "precond_combine: bad args");
   const int64_t total = (int64_t)batch * per_sample;
   precond_kernel<1><<<precond_grid(total), 256, 0, (cudaStream_t)stream>>>(f, x, sigma, sigma_data, out, per_sample, total);
+  KDB_LAUNCH_CHECK(F_PRECOND, (cudaStream_t)stream);
+  return 0;
+}
+
+// The training losses of layers.py:76-86 (Denoiser, scales == 1) and :107-111 (SimpleLossDenoiser), one CTA per sample.  Each
+// product and sum is rounded on its own, in the order of the reference's expressions; the mean is a fixed-order block sum.
+__global__ void __launch_bounds__(256) denoiser_loss_kernel(int kind, const float* __restrict__ x, const float* __restrict__ noise,
+                                                            const float* __restrict__ sigma, const float* __restrict__ weight, float sd,
+                                                            const float* __restrict__ f, float* __restrict__ loss, float* __restrict__ cot,
+                                                            int64_t per_sample) {
+  __shared__ float red[8];
+  const int64_t b = blockIdx.x;
+  const float s = sigma[b];
+  float c_skip, c_out, c_in;
+  karras_scalings(s, sd, c_skip, c_out, c_in);
+  const float w = kind == KDB_LOSS_DENOISER ? weight[b] : 1.f;
+  const float inv_n = 1.f / (float)per_sample;
+  // d loss / d f = 2 r g / N with r the residual: g = w (Denoiser), -c_out / sigma (SimpleLossDenoiser: r = eps - noise)
+  const float g = kind == KDB_LOSS_DENOISER ? w : __fdiv_rn(-c_out, s);
+  float acc = 0.f;
+  for (int64_t i = threadIdx.x; i < per_sample; i += 256) {
+    const int64_t j = b * per_sample + i;
+    const float xn = __fadd_rn(x[j], __fmul_rn(noise[j], s));
+    float r;
+    if (kind == KDB_LOSS_DENOISER) {
+      r = __fsub_rn(f[j], __fdiv_rn(__fsub_rn(x[j], __fmul_rn(c_skip, xn)), c_out));
+    } else {
+      const float den = __fadd_rn(__fmul_rn(f[j], c_out), __fmul_rn(xn, c_skip));
+      r = __fsub_rn(__fdiv_rn(__fsub_rn(xn, den), s), noise[j]);
+    }
+    acc = __fadd_rn(acc, __fmul_rn(r, r));
+    if (cot != nullptr) cot[j] = __fmul_rn(__fmul_rn(2.f * g, r), inv_n);
+  }
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) loss[b] = __fmul_rn(__fdiv_rn(acc, (float)per_sample), w);
+}
+
+int kdb_loss_noised_input(const float* x, const float* noise, const float* sigma, float sigma_data, float* out, int batch, int64_t per_sample,
+                          void* stream) {
+  KDB_REQUIRE(x && noise && sigma && out && batch > 0 && per_sample > 0 && sigma_data > 0.f, KDB_ERR_BAD_ARG, "loss_noised_input: bad args");
+  const int64_t total = (int64_t)batch * per_sample;
+  precond_kernel<3><<<precond_grid(total), 256, 0, (cudaStream_t)stream>>>(noise, x, sigma, sigma_data, out, per_sample, total);
+  KDB_LAUNCH_CHECK(F_PRECOND, (cudaStream_t)stream);
+  return 0;
+}
+
+int kdb_denoiser_loss(int kind, const float* x, const float* noise, const float* sigma, const float* weight, float sigma_data, const float* f,
+                      float* loss, float* cotangent, int batch, int64_t per_sample, void* stream) {
+  KDB_REQUIRE(x && noise && sigma && f && loss && batch > 0 && per_sample > 0 && sigma_data > 0.f, KDB_ERR_BAD_ARG, "denoiser_loss: bad args");
+  KDB_REQUIRE(kind == KDB_LOSS_SIMPLE || (kind == KDB_LOSS_DENOISER && weight), KDB_ERR_BAD_ARG, "denoiser_loss: bad kind %d or NULL weight", kind);
+  denoiser_loss_kernel<<<(unsigned)batch, 256, 0, (cudaStream_t)stream>>>(kind, x, noise, sigma, weight, sigma_data, f, loss, cotangent, per_sample);
   KDB_LAUNCH_CHECK(F_PRECOND, (cudaStream_t)stream);
   return 0;
 }

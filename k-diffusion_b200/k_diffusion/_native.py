@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 18
+ABI_VERSION = 19
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -77,6 +77,11 @@ SIGNATURES = {
     "kdb_model_forward_jvp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "kdb_model_vjp_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
     "kdb_model_forward_vjp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_model_set_grad": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
+    "kdb_model_train_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
+    "kdb_model_forward_train": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_loss_noised_input": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
+    "kdb_denoiser_loss": (_i32, [_i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i32, _i64, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_model_tap_count": (_i64, [_vp]),
     "kdb_unet_create": (_i32, [ctypes.POINTER(KdbUNetConfig), ctypes.POINTER(_vp)]),
@@ -341,6 +346,29 @@ def external_scale_in(x, sigma, sigma_data=1.0):
     return out
 
 
+LOSS_DENOISER, LOSS_SIMPLE = 0, 1
+
+
+@_on_device_of_first
+def loss_noised_input(x, noise, sigma, sigma_data):
+    """(x + noise * sigma) * c_in(sigma): the inner model's input of a training loss (layers.py:79-81)"""
+    require_cuda(x, noise, sigma)
+    out = torch.empty_like(x)
+    check(lib().kdb_loss_noised_input(ptr(x), ptr(noise), ptr(sigma), float(sigma_data), ptr(out), x.shape[0], x[0].numel(), stream()))
+    return out
+
+
+@_on_device_of_first
+def denoiser_loss(x, noise, sigma, weight, sigma_data, f, kind):
+    """-> (loss [B], d loss[b] / d f): kdb_denoiser_loss (LOSS_DENOISER: layers.py:76-86 with scales == 1; LOSS_SIMPLE: :107-111)"""
+    require_cuda(x, noise, sigma, weight, f)
+    loss = torch.empty(x.shape[0], device=x.device, dtype=torch.float32)
+    cot = torch.empty_like(f)
+    check(lib().kdb_denoiser_loss(kind, ptr(x), ptr(noise), ptr(sigma), ptr(weight), float(sigma_data), ptr(f), ptr(loss), ptr(cot),
+                                  x.shape[0], x[0].numel(), stream()))
+    return loss, cot
+
+
 def _per_sample_stride(f, B):
     """f's batch stride if each of its B samples is one contiguous run (a contiguous tensor, or a channel slice of one such as the
     eps half of a learned-variance output), else None."""
@@ -446,6 +474,7 @@ class Engine:
         self._h = _vp()
         check(self._fn("create")(ctypes.byref(self.cfg), ctypes.byref(self._h)))
         self._sig, self._held, self._ws, self._stride, self.device = None, {}, None, None, None
+        self._grad_keys = set()
 
     @staticmethod
     def _config(spec):
@@ -586,6 +615,26 @@ class Engine:
             check(lib().kdb_model_forward_vjp(self._h, PREC_FP32, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
                                               ptr(u), ptr(out), ptr(out_grad), ptr(ws), ws.numel(), stream()))
         return out, out_grad
+
+    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None):
+        """Parameter gradients on the fp32 path: binds `grads` ({state-dict key: fp32 CUDA tensor of the parameter's shape}, every other
+        key unbound), then one kdb_model_forward_train: out = F(x) at fp32, every bound gradient = u^T dF/dparam, grad_x (if given) u^T dF/dx."""
+        B, _, H, W = x.shape
+        shape = (B, self.cfg.out_channels, H, W)
+        if tuple(u.shape) != shape:
+            raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {shape}")
+        out = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
+        for k in self._grad_keys - set(grads):
+            check(lib().kdb_model_set_grad(self._h, k.encode(), None, None, 0))
+        for k, g in grads.items():
+            dims = (_i64 * g.ndim)(*g.shape)
+            check(lib().kdb_model_set_grad(self._h, k.encode(), ptr(g), dims, g.ndim))
+        self._grad_keys = set(grads)
+        ws = self._reserve(lib().kdb_model_train_workspace_bytes(self._h, B, H, W), x.device)
+        with device_of(x):
+            check(lib().kdb_model_forward_train(self._h, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(class_cond), ptr(mapping_cond),
+                                                ptr(cond), self._stride, ptr(u), ptr(out), ptr(grad_x), ptr(ws), ws.numel(), stream()))
+        return out
 
     def arm_tap(self, name, capacity, device):
         buf = torch.empty(capacity, dtype=torch.float32, device=device)

@@ -34,7 +34,19 @@ class KarrasAugmentWrapper(nn.Module):
         return self.inner_model.param_groups(*args, **kwargs)
 
     # ------------------------------------------------------------------ native interface (Denoiser / sampler executor)
+    def _native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, mapping_cond=None, **kwargs):
+        if aug_cond is None:
+            aug_cond = input.new_zeros([input.shape[0], 9])
+        mapping_cond = aug_cond if mapping_cond is None else torch.cat([aug_cond, mapping_cond], dim=1)
+        return self.inner_model.native_loss(kind, input, noise, sigma, sigma_data, weight, mapping_cond=mapping_cond, **kwargs)
+
     def __getattr__(self, name):
+        if name == "native_loss":   # Denoiser.loss: the inner model's native loss with the wrapper's conditioning, where it has one
+            inner = self._modules["inner_model"]
+            if isinstance(inner, ImageDenoiserModelV1):
+                return _native.unet_has_no_derivative
+            if hasattr(inner, "native_loss"):
+                return self._native_loss
         if name in ("engine", "denoise", "levels", "resolved_precision", "_check_cond", "class_emb", "mapping_cond_in_proj",
                     "denoise_jvp", "denoise_vjp", "set_precision"):
             inner = self._modules["inner_model"]

@@ -10,7 +10,8 @@ class Denoiser(nn.Module):
 
     With an `ImageTransformerDenoiserModelV2` inside, the three scalings are folded into the
     engine's first and last kernels; any other `inner_model` is wrapped with two elementwise
-    kernels (scale-in, combine).  `loss` (training) is out of scope.
+    kernels (scale-in, combine).  `loss` trains an `ImageTransformerDenoiserModelV2` on the
+    native engine (fp32 parameter gradients) and any other inner model through torch autograd.
     """
 
     def __init__(self, inner_model, sigma_data=1., weighting='karras', scales=1):
@@ -36,8 +37,31 @@ class Denoiser(nn.Module):
         var = sigma ** 2 + self.sigma_data ** 2
         return self.sigma_data ** 2 / var, sigma * self.sigma_data / var ** 0.5, 1 / var ** 0.5
 
-    def loss(self, *args, **kwargs):
-        raise NotImplementedError('training losses are out of scope for the H100 sampling path')
+    _loss_kind = _native.LOSS_DENOISER
+
+    def _check_loss(self):
+        if self.scales != 1:
+            raise NotImplementedError('loss with scales != 1 weights the error by frequency through a DCT (dctorch), which is not built')
+
+    def loss(self, input, noise, sigma, **kwargs):
+        """Per-sample losses [B] (reference layers.py:76-86, scales == 1).  A native image_transformer_v2 inner model runs one fp32 engine
+        evaluation and one loss kernel, and its backward one native call that writes every parameter's gradient; image_transformer_v1 and
+        the image_v1 U-Net raise NotImplementedError.  Any other inner model runs the reference formula under torch autograd."""
+        self._check_loss()
+        native_loss = getattr(self.inner_model, 'native_loss', None)
+        if native_loss is not None:
+            return native_loss(self._loss_kind, input, noise, sigma, self.sigma_data, self.weighting(sigma), **kwargs)
+        if self.is_native():
+            raise NotImplementedError(f'{type(self.inner_model).__name__}: parameter gradients are built for image_transformer_v2 models only')
+        return self._torch_loss(input, noise, sigma, **kwargs)
+
+    def _torch_loss(self, input, noise, sigma, **kwargs):
+        c_skip, c_out, c_in = [utils.append_dims(x, input.ndim) for x in self.get_scalings(sigma)]
+        c_weight = self.weighting(sigma)
+        noised_input = input + noise * utils.append_dims(sigma, input.ndim)
+        model_output = self.inner_model(noised_input * c_in, sigma, **kwargs)
+        target = (input - c_skip * noised_input) / c_out
+        return ((model_output - target) ** 2).flatten(1).mean(1) * c_weight
 
     def is_native(self):
         return hasattr(self.inner_model, 'denoise') and hasattr(self.inner_model, 'engine')
@@ -85,11 +109,24 @@ class Denoiser(nn.Module):
 
 
 class DenoiserWithVariance(Denoiser):
-    """reference layers.py:93-101: differs from Denoiser in `loss` only (training, out of scope); sampling is identical."""
+    """reference layers.py:93-101: differs from Denoiser in `loss` only, which needs the inner model's learned variance; sampling is
+    identical."""
+
+    def loss(self, input, noise, sigma, **kwargs):
+        raise NotImplementedError('DenoiserWithVariance.loss needs the inner model\'s return_variance output, which is not built')
 
 
 class SimpleLossDenoiser(Denoiser):
     """L_simple with the Karras et al. preconditioner (reference layers.py:104-113): differs from Denoiser in `loss` only."""
+
+    _loss_kind = _native.LOSS_SIMPLE
+
+    def _torch_loss(self, input, noise, sigma, **kwargs):
+        c_skip, c_out, c_in = [utils.append_dims(x, input.ndim) for x in self.get_scalings(sigma)]
+        noised_input = input + noise * utils.append_dims(sigma, input.ndim)
+        denoised = self.inner_model(noised_input * c_in, sigma, **kwargs) * c_out + noised_input * c_skip
+        eps = (noised_input - denoised) / utils.append_dims(sigma, input.ndim)
+        return (eps - noise).pow(2).flatten(1).mean(1)
 
 
 class FourierFeatures(nn.Module):

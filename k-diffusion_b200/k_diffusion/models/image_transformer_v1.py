@@ -87,6 +87,10 @@ class ImageTransformerDenoiserModelV1(TransformerEngineModel):
         self.precision = None        # None -> flags.resolve_precision ("auto" unless KDB200_PRECISION is set)
         self._engines = {}
 
+    def param_groups(self, *args, **kwargs):
+        """Training image_transformer_v1 is not built (its parameters carry none of the reference's weight-decay / mapping tags)."""
+        raise NotImplementedError("image_transformer_v1: training is not built; parameter gradients exist for image_transformer_v2 only")
+
     def _check_cond(self, class_cond, mapping_cond):
         if mapping_cond is not None:
             raise TypeError("image_transformer_v1 takes no mapping_cond (reference forward(x, sigma, aug_cond=None, class_cond=None))")

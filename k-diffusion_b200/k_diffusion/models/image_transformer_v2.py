@@ -3,7 +3,8 @@
 Constructor signature, spec dataclasses and `state_dict()` layout follow the reference
 (k_diffusion/models/image_transformer_v2.py:626-706) so reference checkpoints load unchanged; the
 forward pass itself (:721-762) is executed by libkdb200.so.  This module holds no layer logic: it
-is a tree of named parameters whose names reproduce the reference keys.  Inference only.
+is a tree of named parameters whose names reproduce the reference keys.  Parameter gradients (training) come from the engine's fp32
+reverse walk through `Denoiser.loss`; `param_groups` returns the reference's optimizer groups.
 """
 import math
 from dataclasses import dataclass
@@ -74,6 +75,36 @@ class _Buffer:
         self.tensor = tensor
 
 
+# Param tags (reference :57-84): "wd" marks the weights that take weight decay, "mapping" the mapping network and the AdaRMSNorm
+# projections, which train at a scaled learning rate.
+def tag_param(param, tag):
+    if not hasattr(param, "_tags"):
+        param._tags = set([tag])
+    else:
+        param._tags.add(tag)
+    return param
+
+
+def tag_module(module, tag):
+    for param in module.parameters():
+        tag_param(param, tag)
+    return module
+
+
+def apply_wd(module):
+    for name, param in module.named_parameters():
+        if name.endswith("weight"):
+            tag_param(param, "wd")
+    return module
+
+
+def filter_params(function, module):
+    for param in module.parameters():
+        tags = getattr(param, "_tags", set())
+        if function(tags):
+            yield param
+
+
 def _linear(n_out, n_in, zero=False):
     """nn.Linear(bias=False) weight: U(-1/sqrt(in), 1/sqrt(in)), or zeros where the reference zero-inits."""
     w = torch.zeros(n_out, n_in)
@@ -102,6 +133,11 @@ def _attn_kind(spec):
     raise ValueError(f"unsupported self attention spec {spec}")
 
 
+def _ada_linear(width, cond_width):
+    """AdaRMSNorm's projection (reference :159-160)"""
+    return tag_module(apply_wd(_linear(width, cond_width, zero=True)), "mapping")
+
+
 def _layer(spec, cond_width):
     kind, _ = _attn_kind(spec.self_attn)
     parts = {}
@@ -109,16 +145,16 @@ def _layer(spec, cond_width):
         d_head = spec.self_attn.d_head
         n_heads = spec.width // d_head
         parts["self_attn"] = _Node(
-            norm=_Node(linear=_linear(spec.width, cond_width, zero=True)),
-            qkv_proj=_linear(spec.width * 3, spec.width),
+            norm=_Node(linear=_ada_linear(spec.width, cond_width)),
+            qkv_proj=apply_wd(_linear(spec.width * 3, spec.width)),
             scale=torch.full([n_heads], 10.0),
             pos_emb=_Node(freqs=_Buffer(_rope_freqs(d_head, n_heads))),
-            out_proj=_linear(spec.width, spec.width, zero=True),
+            out_proj=apply_wd(_linear(spec.width, spec.width, zero=True)),
         )
     parts["ff"] = _Node(
-        norm=_Node(linear=_linear(spec.width, cond_width, zero=True)),
-        up_proj=_linear(spec.d_ff * 2, spec.width),
-        down_proj=_linear(spec.width, spec.d_ff, zero=True),
+        norm=_Node(linear=_ada_linear(spec.width, cond_width)),
+        up_proj=apply_wd(_linear(spec.d_ff * 2, spec.width)),
+        down_proj=apply_wd(_linear(spec.width, spec.d_ff, zero=True)),
     )
     return _Node(**parts)
 
@@ -167,8 +203,39 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
             raise ValueError(f"the {self.kind} engine runs at fp32 or bf16 ({p} is built for the image_v1 U-Net only)")
         return _native.PREC_BF16 if p == "bf16" else _native.PREC_FP32
 
-    def param_groups(self, *args, **kwargs):
-        raise NotImplementedError("training is out of scope for the H100 sampling path")
+    def param_groups(self, base_lr=5e-4, mapping_lr_scale=1 / 3):
+        """The reference's four optimizer groups (:708-718): weight decay or not, mapping network (scaled learning rate) or not."""
+        wd = filter_params(lambda tags: "wd" in tags and "mapping" not in tags, self)
+        no_wd = filter_params(lambda tags: "wd" not in tags and "mapping" not in tags, self)
+        mapping_wd = filter_params(lambda tags: "wd" in tags and "mapping" in tags, self)
+        mapping_no_wd = filter_params(lambda tags: "wd" not in tags and "mapping" in tags, self)
+        return [
+            {"params": list(wd), "lr": base_lr},
+            {"params": list(no_wd), "lr": base_lr, "weight_decay": 0.0},
+            {"params": list(mapping_wd), "lr": base_lr * mapping_lr_scale},
+            {"params": list(mapping_no_wd), "lr": base_lr * mapping_lr_scale, "weight_decay": 0.0}
+        ]
+
+    def native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, class_cond=None, mapping_cond=None):
+        """Per-sample training losses [B] of the Karras-preconditioned denoiser around this model (`_native.LOSS_DENOISER`: reference
+        layers.py:76-86 with scales == 1 and per-sample `weight`; `LOSS_SIMPLE`: :107-111), with a grad_fn that reaches every parameter
+        requiring grad.  The forward is one fp32 engine evaluation and one loss kernel; the backward is one kdb_model_forward_train.
+        Always fp32, whatever `set_precision` selected."""
+        if self.family != _native.FAMILY_ITV2:
+            raise NotImplementedError(f"{self.kind}: parameter gradients are built for image_transformer_v2 models only")
+        for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
+            if t.requires_grad:
+                raise RuntimeError(f"the native loss differentiates the model's parameters only, but {name} requires grad")
+        _native.require_cuda(input, noise, sigma)
+        if self.training and any(s.dropout > 0 for s in self.levels):
+            raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
+        self._check_cond(class_cond, mapping_cond)
+        if input.ndim != 4 or noise.shape != input.shape:
+            raise ValueError(f"expected input and noise of one shape [B, C, H, W], got {tuple(input.shape)} and {tuple(noise.shape)}")
+        named = [(k, p) for k, p in self.named_parameters() if p.requires_grad]
+        keys = tuple(k for k, _ in named)
+        return _NativeLoss.apply(self, kind, input, noise, sigma, float(sigma_data), weight, aug_cond, class_cond, mapping_cond, keys,
+                                 *(p for _, p in named))
 
     # ------------------------------------------------------------------ forward
     def _check_cond(self, class_cond, mapping_cond):
@@ -258,27 +325,29 @@ class ImageTransformerDenoiserModelV2(TransformerEngineModel):
         w0 = levels[0].width
         n_patch = patch_size[0] * patch_size[1]
 
-        self.patch_in = _Node(proj=_linear(w0, in_channels * n_patch))
+        self.patch_in = _Node(proj=apply_wd(_linear(w0, in_channels * n_patch)))
         self.time_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 1)))            # layers.FourierFeatures(1, mw)
         self.time_in_proj = _linear(mw, mw)
         self.aug_emb = _Node(weight=_Buffer(torch.randn(mw // 2, 9)))             # layers.FourierFeatures(9, mw)
         self.aug_in_proj = _linear(mw, mw)
         self.class_emb = _Node(weight=torch.randn(num_classes, mw)) if num_classes else None
         self.mapping_cond_in_proj = _linear(mw, mapping_cond_dim) if mapping_cond_dim else None
-        self.mapping = _Node(
+        self.mapping = tag_module(_Node(
             in_norm=_Node(scale=torch.ones(mw)),
             blocks=nn.ModuleList([
-                _Node(norm=_Node(scale=torch.ones(mw)), up_proj=_linear(mapping.d_ff * 2, mw), down_proj=_linear(mw, mapping.d_ff, zero=True))
+                _Node(norm=_Node(scale=torch.ones(mw)), up_proj=apply_wd(_linear(mapping.d_ff * 2, mw)),
+                      down_proj=apply_wd(_linear(mw, mapping.d_ff, zero=True)))
                 for _ in range(mapping.depth)]),
             out_norm=_Node(scale=torch.ones(mw)),
-        )
+        ), "mapping")
         self.down_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
         self.up_levels = nn.ModuleList([_level(s, mw) for s in levels[:-1]])
         self.mid_level = _level(levels[-1], mw)
-        self.merges = nn.ModuleList([_Node(proj=_linear(b.width, a.width * 4)) for a, b in zip(levels[:-1], levels[1:])])
-        self.splits = nn.ModuleList([_Node(proj=_linear(a.width * 4, b.width), fac=torch.ones(1) * 0.5) for a, b in zip(levels[:-1], levels[1:])])
+        self.merges = nn.ModuleList([_Node(proj=apply_wd(_linear(b.width, a.width * 4))) for a, b in zip(levels[:-1], levels[1:])])
+        self.splits = nn.ModuleList([_Node(proj=apply_wd(_linear(a.width * 4, b.width)), fac=torch.ones(1) * 0.5)
+                                     for a, b in zip(levels[:-1], levels[1:])])
         self.out_norm = _Node(scale=torch.ones(w0))
-        self.patch_out = _Node(proj=_linear(out_channels * n_patch, w0, zero=True))
+        self.patch_out = _Node(proj=apply_wd(_linear(out_channels * n_patch, w0, zero=True)))
 
         self.precision = None        # None -> flags.resolve_precision ("auto" unless KDB200_PRECISION is set)
         self._engines = {}
@@ -320,3 +389,37 @@ def _autograd_eval(model, x, sigma, sigma_data, aug_cond, class_cond, mapping_co
     if out is not None:
         raise RuntimeError("out= cannot be used when x requires grad (the result must carry a grad_fn)")
     return _NativeEval.apply(x, model, sigma, sigma_data, aug_cond, class_cond, mapping_cond)
+
+
+class _NativeLoss(torch.autograd.Function):
+    """A training loss through the native engine with respect to the model's parameters (passed after `keys`, their state-dict names).
+    The forward saves the per-element cotangent d loss[b] / d F of the loss kernel; the backward scales it by the incoming gradient of
+    each sample's loss and makes one kdb_model_forward_train, which writes every parameter's gradient."""
+
+    @staticmethod
+    def forward(ctx, model, kind, x, noise, sigma, sigma_data, weight, aug_cond, class_cond, mapping_cond, keys, *params):
+        with torch.cuda.device(x.device):
+            x, noise = _native.f32c(x), _native.f32c(noise)
+            sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
+            w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
+            xin = _native.loss_noised_input(x, noise, sig, sigma_data)
+            eng, xin, sig, cond = model._inputs(xin, sig, aug_cond, class_cond, mapping_cond)
+            f = eng.forward(xin, sig, cond, eng.cond_stride, 0.0, _native.PREC_FP32)
+            loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
+        aug = None if aug_cond is None else _native.f32c(aug_cond)
+        cls = class_cond.to(torch.int64).contiguous() if class_cond is not None and model.class_emb is not None else None
+        mc = _native.f32c(mapping_cond) if mapping_cond is not None and model.mapping_cond_in_proj is not None else None
+        ctx.model, ctx.keys = model, keys
+        ctx.save_for_backward(xin, sig, cond, cot, aug, cls, mc)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        xin, sig, cond, cot, aug, cls, mc = ctx.saved_tensors
+        params = dict(ctx.model.named_parameters())
+        with torch.cuda.device(xin.device):
+            u = cot * _native.f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
+            grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
+            ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads)
+        return (None,) * 11 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)
