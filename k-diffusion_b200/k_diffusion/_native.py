@@ -435,8 +435,74 @@ UNET_NO_DERIVATIVE = "the image_v1 U-Net engine has no derivative: only its forw
 
 
 def unet_has_no_derivative(*args, **kwargs):
-    """What every derivative entry point of the U-Net does (the engine, the model and the augment wrapper's view of it)."""
+    """What every derivative entry point of the U-Net does (the engine, the model and the augment wrapper around it)."""
     raise NotImplementedError(UNET_NO_DERIVATIVE)
+
+
+def check_input(x, sigma, dropout):
+    """The checks of x and sigma every native model makes before evaluating; `dropout`: the model is in training mode with dropout."""
+    require_cuda(x, sigma)
+    if x.ndim != 4:
+        raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
+    if dropout:
+        raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
+
+
+def require_cond(class_cond, mapping_cond, class_needed, mapping_needed):
+    """The native front ends' refusal of a missing conditioning input the model needs (the reference's forwards raise the same)."""
+    if class_cond is None and class_needed:
+        raise ValueError("class_cond must be specified if num_classes > 0")
+    if mapping_cond is None and mapping_needed:
+        raise ValueError("mapping_cond must be specified if mapping_cond_dim > 0")
+
+
+class Evaluation:
+    """The answer of a native model's front end `native_eval(x, sigma, aug_cond, class_cond, mapping_cond, precision)`, which validates
+    those inputs: the bound engine, the precision code, x as fp32, sigma as [B] fp32 (None when the caller brings its own rows, as the
+    sampler does) and the conditioning exactly as the engine takes it (`takes_class` / `takes_mapping`: whether it takes class_cond /
+    mapping_cond; aug_cond is always taken)."""
+
+    def __init__(self, engine, precision, x, sigma, aug_cond, class_cond, mapping_cond, takes_class, takes_mapping):
+        self.engine, self.precision, self.dtype = engine, precision, x.dtype
+        self.x = f32c(x)
+        self.sigma = None
+        if sigma is not None:
+            self.sigma = f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else f32c(sigma)
+            if self.sigma.shape != (x.shape[0],):
+                raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
+        self._takes, self._uncond = (takes_class, takes_mapping), None
+        self.cond = self.cond_args(1, aug_cond, class_cond, mapping_cond)
+
+    def guide(self, uncond):
+        """Make this the evaluation of classifier-free guidance's doubled batch [uncond | cond]: class_cond rows of class `uncond` first."""
+        n = int(self.engine.cfg.num_classes)
+        if self._takes[0] and not torch.cuda.is_current_stream_capturing() and not 0 <= uncond < n:
+            raise IndexError(f"CFG unconditional class {uncond} outside class_emb ({n} rows)")
+        self._uncond = uncond
+        return self
+
+    def cond_args(self, reps=1, aug_cond=None, class_cond=None, mapping_cond=None):
+        """(aug_cond, class_cond, mapping_cond) as the engine takes them, None where it takes none, for `reps` evaluations stacked along
+        the batch.  The sampler passes its own copies of the inputs this evaluation was made with (a captured graph reads static ones)."""
+        class_cond = class_cond if self._takes[0] else None
+        if self._uncond is not None:
+            class_cond = torch.cat([torch.full_like(class_cond, self._uncond), class_cond])
+        args = (aug_cond, class_cond, mapping_cond if self._takes[1] else None)
+        return args if reps == 1 else tuple(None if t is None else t.repeat(reps, *([1] * (t.ndim - 1))) for t in args)
+
+    def conditioning(self):
+        return self.engine.conditioning(self.sigma, *self.cond)
+
+    def cast(self, res):
+        """An engine result (or a tuple of them) in x's dtype."""
+        if self.dtype == torch.float32:
+            return res
+        return tuple(r.to(self.dtype) for r in res) if isinstance(res, tuple) else res.to(self.dtype)
+
+    def forward(self, sigma_data, out=None):
+        """The raw model (sigma_data 0) or the Karras-preconditioned denoiser at this evaluation's precision, in x's dtype."""
+        return self.cast(self.engine.forward(self.x, self.sigma, self.conditioning(), self.engine.cond_stride, sigma_data, self.precision,
+                                             out=out))
 
 
 class EngineCache:
@@ -667,9 +733,7 @@ class UNetEngine(Engine):
         return x.shape[1]
 
     def conditioning(self, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
-        """-> [rows, cond_stride] fp32 table (mapping net + every AdaGN's (weight, bias))."""
-        if class_cond is not None:
-            raise TypeError("the image_v1 U-Net takes no class_cond")
+        """-> [rows, cond_stride] fp32 table (mapping net + every AdaGN's (weight, bias)); class_cond is refused by the model's front end."""
         require_cuda(sigma, aug_cond, mapping_cond)
         sigma = f32c(sigma)
         rows = sigma.numel()

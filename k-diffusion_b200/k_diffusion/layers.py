@@ -64,7 +64,8 @@ class Denoiser(nn.Module):
         return ((model_output - target) ** 2).flatten(1).mean(1) * c_weight
 
     def is_native(self):
-        return hasattr(self.inner_model, 'denoise') and hasattr(self.inner_model, 'engine')
+        """Whether the inner model has a native front end (`native_eval`), which the fused paths here and the samplers evaluate through."""
+        return getattr(self.inner_model, 'native_eval', None) is not None
 
     def forward(self, input, sigma, **kwargs):
         _native.require_cuda(input, sigma)

@@ -226,23 +226,17 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
             if t.requires_grad:
                 raise RuntimeError(f"the native loss differentiates the model's parameters only, but {name} requires grad")
-        _native.require_cuda(input, noise, sigma)
-        if self.training and any(s.dropout > 0 for s in self.levels):
-            raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
-        self._check_cond(class_cond, mapping_cond)
+        _native.require_cuda(noise)
         if input.ndim != 4 or noise.shape != input.shape:
             raise ValueError(f"expected input and noise of one shape [B, C, H, W], got {tuple(input.shape)} and {tuple(noise.shape)}")
+        ev = self.native_eval(input, sigma, aug_cond, class_cond, mapping_cond, precision=_native.PREC_FP32)
         named = [(k, p) for k, p in self.named_parameters() if p.requires_grad]
         keys = tuple(k for k, _ in named)
-        return _NativeLoss.apply(self, kind, input, noise, sigma, float(sigma_data), weight, aug_cond, class_cond, mapping_cond, keys,
-                                 *(p for _, p in named))
+        return _NativeLoss.apply(self, ev, kind, _native.f32c(noise), float(sigma_data), weight, keys, *(p for _, p in named))
 
     # ------------------------------------------------------------------ forward
     def _check_cond(self, class_cond, mapping_cond):
-        if class_cond is None and self.class_emb is not None:
-            raise ValueError("class_cond must be specified if num_classes > 0")
-        if mapping_cond is None and self.mapping_cond_in_proj is not None:
-            raise ValueError("mapping_cond must be specified if mapping_cond_dim > 0")
+        _native.require_cond(class_cond, mapping_cond, self.class_emb is not None, self.mapping_cond_in_proj is not None)
 
     def conditioning(self, sigma, aug_cond=None, class_cond=None, mapping_cond=None):
         """Conditioning table rows for `sigma` [rows] (mapping network + all AdaRMSNorm scales)."""
@@ -250,41 +244,32 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         return self.engine().conditioning(sigma, aug_cond, class_cond if self.class_emb is not None else None,
                                           mapping_cond if self.mapping_cond_in_proj is not None else None)
 
-    def _inputs(self, x, sigma, aug_cond, class_cond, mapping_cond):
-        """(engine, fp32 x, sigma [B], conditioning rows) of one evaluation; the caller has made x's device current."""
-        xin = _native.f32c(x)
-        sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
-        if sig.shape != (x.shape[0],):
-            raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
+    def native_eval(self, x, sigma=None, aug_cond=None, class_cond=None, mapping_cond=None, precision=None):
+        """The native front end: validates one evaluation's inputs and returns its `_native.Evaluation` (the bound engine, `precision`
+        or, when None, the resolved precision, and the engine's arguments).  Labels are range-checked here, outside stream capture,
+        because the conditioning kernel indexes class_emb with them (nn.Embedding raises on out-of-range labels, reference :735)."""
+        _native.check_input(x, sigma, self.training and any(s.dropout > 0 for s in self.levels))
+        self._check_cond(class_cond, mapping_cond)
         eng = self.engine()
         if self.class_emb is not None and not torch.cuda.is_current_stream_capturing():
-            eng.check_class_range(class_cond)           # nn.Embedding raises on out-of-range labels (reference :735)
-        cond = eng.conditioning(sig, aug_cond, class_cond if self.class_emb is not None else None,
-                                mapping_cond if self.mapping_cond_in_proj is not None else None)
-        return eng, xin, sig, cond
+            eng.check_class_range(class_cond)
+        return _native.Evaluation(eng, self.resolved_precision() if precision is None else precision, x, sigma, aug_cond, class_cond,
+                                  mapping_cond, self.class_emb is not None, self.mapping_cond_in_proj is not None)
 
     def _run(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out=None, tangent=None, cotangent=None):
-        _native.require_cuda(x, sigma, tangent, cotangent)
-        if x.ndim != 4:
-            raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
-        if self.training and any(s.dropout > 0 for s in self.levels):
-            raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
-        self._check_cond(class_cond, mapping_cond)
-        if tangent is None and cotangent is None and torch.is_grad_enabled() and x.requires_grad:
-            return _autograd_eval(self, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out)
-        with torch.cuda.device(x.device):
-            eng, xin, sig, cond = self._inputs(x, sigma, aug_cond, class_cond, mapping_cond)
-            if tangent is not None:
-                if tangent.shape != x.shape:
-                    raise ValueError(f"tangent must have the shape of x {tuple(x.shape)}, got {tuple(tangent.shape)}")
-                res = eng.forward_jvp(xin, _native.f32c(tangent), sig, cond, eng.cond_stride, sigma_data)
-            elif cotangent is not None:
-                res = eng.forward_vjp(xin, _native.f32c(cotangent), sig, cond, eng.cond_stride, sigma_data)
-            else:
-                res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
-        if tangent is not None or cotangent is not None:
-            return res if x.dtype == torch.float32 else tuple(r.to(x.dtype) for r in res)
-        return res if x.dtype == torch.float32 else res.to(x.dtype)
+        _native.require_cuda(tangent, cotangent)
+        derivative = tangent is not None or cotangent is not None
+        ev = self.native_eval(x, sigma, aug_cond, class_cond, mapping_cond, _native.PREC_FP32 if derivative else None)
+        if not derivative and torch.is_grad_enabled() and x.requires_grad:
+            return _autograd_eval(self, ev, x, sigma, sigma_data, aug_cond, mapping_cond, out)
+        eng = ev.engine
+        if tangent is not None:
+            if tangent.shape != x.shape:
+                raise ValueError(f"tangent must have the shape of x {tuple(x.shape)}, got {tuple(tangent.shape)}")
+            return ev.cast(eng.forward_jvp(ev.x, _native.f32c(tangent), ev.sigma, ev.conditioning(), eng.cond_stride, sigma_data))
+        if cotangent is not None:
+            return ev.cast(eng.forward_vjp(ev.x, _native.f32c(cotangent), ev.sigma, ev.conditioning(), eng.cond_stride, sigma_data))
+        return ev.forward(sigma_data, out)
 
     def denoise(self, x, sigma, sigma_data, aug_cond=None, class_cond=None, mapping_cond=None, out=None):
         """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
@@ -363,32 +348,30 @@ class _NativeEval(torch.autograd.Function):
     bf16 the gradient is therefore that of the fp32 function."""
 
     @staticmethod
-    def forward(ctx, x, model, sigma, sigma_data, aug_cond, class_cond, mapping_cond):
-        with torch.cuda.device(x.device):
-            eng, xin, sig, cond = model._inputs(x, sigma, aug_cond, class_cond, mapping_cond)
-            res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, model.resolved_precision())
+    def forward(ctx, x, model, ev, sigma_data):
+        cond = ev.conditioning()
+        res = ev.engine.forward(ev.x, ev.sigma, cond, ev.engine.cond_stride, sigma_data, ev.precision)
         ctx.model, ctx.sigma_data, ctx.dtype = model, sigma_data, x.dtype
-        ctx.save_for_backward(xin, sig, cond)
-        return res if x.dtype == torch.float32 else res.to(x.dtype)
+        ctx.save_for_backward(ev.x, ev.sigma, cond)
+        return ev.cast(res)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         xin, sig, cond = ctx.saved_tensors
-        with torch.cuda.device(xin.device):
-            eng = ctx.model.engine()
-            _, gx = eng.forward_vjp(xin, _native.f32c(grad_out), sig, cond, eng.cond_stride, ctx.sigma_data)
-        return gx.to(ctx.dtype), None, None, None, None, None, None
+        eng = ctx.model.engine()
+        _, gx = eng.forward_vjp(xin, _native.f32c(grad_out), sig, cond, eng.cond_stride, ctx.sigma_data)
+        return gx.to(ctx.dtype), None, None, None
 
 
-def _autograd_eval(model, x, sigma, sigma_data, aug_cond, class_cond, mapping_cond, out):
+def _autograd_eval(model, ev, x, sigma, sigma_data, aug_cond, mapping_cond, out):
     """An evaluation whose x requires grad: the gradient reaches x only, so other inputs that require grad are refused, not ignored."""
     for name, t in (("sigma", sigma), ("aug_cond", aug_cond), ("mapping_cond", mapping_cond)):
         if t is not None and t.requires_grad:
             raise RuntimeError(f"the native model is differentiable with respect to x only, but {name} requires grad")
     if out is not None:
         raise RuntimeError("out= cannot be used when x requires grad (the result must carry a grad_fn)")
-    return _NativeEval.apply(x, model, sigma, sigma_data, aug_cond, class_cond, mapping_cond)
+    return _NativeEval.apply(x, model, ev, sigma_data)
 
 
 class _NativeLoss(torch.autograd.Function):
@@ -397,20 +380,17 @@ class _NativeLoss(torch.autograd.Function):
     each sample's loss and makes one kdb_model_forward_train, which writes every parameter's gradient."""
 
     @staticmethod
-    def forward(ctx, model, kind, x, noise, sigma, sigma_data, weight, aug_cond, class_cond, mapping_cond, keys, *params):
-        with torch.cuda.device(x.device):
-            x, noise = _native.f32c(x), _native.f32c(noise)
-            sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
-            w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
-            xin = _native.loss_noised_input(x, noise, sig, sigma_data)
-            eng, xin, sig, cond = model._inputs(xin, sig, aug_cond, class_cond, mapping_cond)
-            f = eng.forward(xin, sig, cond, eng.cond_stride, 0.0, _native.PREC_FP32)
-            loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
-        aug = None if aug_cond is None else _native.f32c(aug_cond)
-        cls = class_cond.to(torch.int64).contiguous() if class_cond is not None and model.class_emb is not None else None
-        mc = _native.f32c(mapping_cond) if mapping_cond is not None and model.mapping_cond_in_proj is not None else None
+    def forward(ctx, model, ev, kind, noise, sigma_data, weight, keys, *params):
+        x, sig = ev.x, ev.sigma
+        w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
+        xin = _native.loss_noised_input(x, noise, sig, sigma_data)
+        cond = ev.conditioning()
+        f = ev.engine.forward(xin, sig, cond, ev.engine.cond_stride, 0.0, ev.precision)
+        loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
+        aug, cls, mc = ev.cond
         ctx.model, ctx.keys = model, keys
-        ctx.save_for_backward(xin, sig, cond, cot, aug, cls, mc)
+        ctx.save_for_backward(xin, sig, cond, cot, None if aug is None else _native.f32c(aug),
+                              None if cls is None else cls.to(torch.int64).contiguous(), None if mc is None else _native.f32c(mc))
         return loss
 
     @staticmethod
@@ -418,8 +398,7 @@ class _NativeLoss(torch.autograd.Function):
     def backward(ctx, grad_loss):
         xin, sig, cond, cot, aug, cls, mc = ctx.saved_tensors
         params = dict(ctx.model.named_parameters())
-        with torch.cuda.device(xin.device):
-            u = cot * _native.f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
-            grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
-            ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads)
-        return (None,) * 11 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)
+        u = cot * _native.f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
+        grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
+        ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads)
+        return (None,) * 7 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)

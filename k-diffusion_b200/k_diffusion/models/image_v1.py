@@ -7,8 +7,6 @@ every kernel exact fp32) or, by set_precision("tf32") or KDB200_PRECISION=tf32, 
 operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True) -- or, by
 set_precision("fp16") or KDB200_PRECISION=fp16, the same with fp16 operands (same significand width, narrower exponent range).
 """
-from types import SimpleNamespace
-
 import torch
 from torch import nn
 
@@ -141,11 +139,6 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
         self._engines = {}
 
     # ------------------------------------------------------------------ engine plumbing
-    @property
-    def levels(self):
-        """per-level dropout (what the sampler executor checks before running the inference-only engine)"""
-        return [SimpleNamespace(dropout=self.dropout_rate)] * len(self.depths)
-
     def engine_spec(self, augment):
         return dict(c_in=self.c_in, feats_in=self.feats_in, depths=self.depths, channels=self.channels, self_attn_depths=self.self_attn_depths,
                     mapping_cond_dim=self.mapping_cond_dim, augment=augment, patch_size=self.patch_size, skip_stages=self.u_net.skip_stages,
@@ -179,55 +172,30 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
     def param_groups(self, *args, **kwargs):
         raise NotImplementedError("training is out of scope for the H100 sampling path")
 
-    # ------------------------------------------------------------------ native interface of the bare model (no augment wrapper)
-    class_emb = None
-
-    @property
-    def mapping_cond_in_proj(self):
-        return True if self.mapping_cond_dim > 0 else None
-
-    def _check_cond(self, class_cond, mapping_cond):
-        self.check_cond(False, class_cond, mapping_cond)
-
-    def denoise(self, x, sigma, sigma_data, mapping_cond=None, out=None):
-        """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
-        return self.run(x, sigma, float(sigma_data), False, mapping_cond=mapping_cond, out=out)
-
-    denoise_jvp = denoise_vjp = _native.unet_has_no_derivative
-
-    # ------------------------------------------------------------------ forward
-    def user_mapping_cond_dim(self, augment):
-        return self.mapping_cond_dim - (9 if augment else 0)
-
-    def check_cond(self, augment, class_cond, mapping_cond):
-        if class_cond is not None:
-            raise TypeError("the image_v1 U-Net takes no class_cond")
-        if mapping_cond is not None and self.user_mapping_cond_dim(augment) <= 0:
-            raise ValueError("this model takes no mapping_cond")
-        if mapping_cond is None and augment and self.user_mapping_cond_dim(augment) > 0:
-            raise ValueError("mapping_cond must be specified if mapping_cond_dim > 0")
-
-    def run(self, x, sigma, sigma_data, augment, aug_cond=None, mapping_cond=None, out=None):
-        """One native evaluation: the raw model (sigma_data <= 0) or the Karras-preconditioned denoiser."""
-        _native.require_cuda(x, sigma)
-        if x.ndim != 4:
-            raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
-        if self.training and self.dropout_rate > 0:
-            raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
+    # ------------------------------------------------------------------ native front end
+    def native_eval(self, x, sigma=None, aug_cond=None, class_cond=None, mapping_cond=None, precision=None, augment=False):
+        """The native front end: validates one evaluation's inputs and returns its `_native.Evaluation` (the bound engine, `precision`
+        or, when None, the resolved precision, and the engine's arguments).  `augment`: the evaluation KarrasAugmentWrapper asks for,
+        whose engine forms mapping_cond = cat([aug_cond or zeros(B, 9), mapping_cond]) in its conditioning kernel."""
+        _native.check_input(x, sigma, self.training and self.dropout_rate > 0)
         if torch.is_grad_enabled() and x.requires_grad:
             _native.unet_has_no_derivative()
         if aug_cond is not None and not augment:
             raise TypeError("aug_cond needs the KarrasAugmentWrapper")
-        self.check_cond(augment, None, mapping_cond)
-        with torch.cuda.device(x.device):
-            xin = _native.f32c(x)
-            sig = _native.f32c(sigma).expand(x.shape[0]).contiguous() if sigma.numel() == 1 else _native.f32c(sigma)
-            if sig.shape != (x.shape[0],):
-                raise ValueError(f"sigma must have shape [{x.shape[0]}], got {tuple(sigma.shape)}")
-            eng = self.engine(augment)
-            cond = eng.conditioning(sig, aug_cond, None, mapping_cond)
-            res = eng.forward(xin, sig, cond, eng.cond_stride, sigma_data, self.resolved_precision(), out=out)
-        return res if x.dtype == torch.float32 else res.to(x.dtype)
+        if class_cond is not None:
+            raise TypeError("the image_v1 U-Net takes no class_cond")
+        user_mapping_cond_dim = self.mapping_cond_dim - (9 if augment else 0)
+        if mapping_cond is not None and user_mapping_cond_dim <= 0:
+            raise ValueError("this model takes no mapping_cond")
+        _native.require_cond(None, mapping_cond, False, augment and user_mapping_cond_dim > 0)
+        return _native.Evaluation(self.engine(augment), self.resolved_precision() if precision is None else precision, x, sigma, aug_cond,
+                                  None, mapping_cond, False, True)
+
+    def denoise(self, x, sigma, sigma_data, mapping_cond=None, out=None):
+        """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
+        return self.native_eval(x, sigma, mapping_cond=mapping_cond).forward(float(sigma_data), out)
+
+    denoise_jvp = denoise_vjp = _native.unet_has_no_derivative
 
     def forward(self, input, sigma, mapping_cond=None, unet_cond=None, cross_cond=None, cross_cond_padding=None, return_variance=False):
         """reference image_v1.py:135-157"""
@@ -235,4 +203,4 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
             raise NotImplementedError('unet_cond and cross-attention conditioning are not supported by the native image_v1 engine')
         if return_variance:
             raise NotImplementedError('the variance output is a training quantity; the native engine returns the denoised channels only')
-        return self.run(input, sigma, 0.0, False, mapping_cond=mapping_cond)
+        return self.native_eval(input, sigma, mapping_cond=mapping_cond).forward(0.0)

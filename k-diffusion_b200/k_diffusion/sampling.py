@@ -503,18 +503,11 @@ class _Evaluator:
         sig = torch.tensor(eval_sigmas, dtype=torch.float32, device=x.device)
         self.sigma_rows = sig[:, None].expand(len(eval_sigmas), self.B).contiguous()
         if self.native:
-            inner = base.inner_model
-            if x.ndim != 4:
-                raise ValueError(f"expected x of shape [B, C, H, W], got {tuple(x.shape)}")
-            if inner.training and any(s.dropout > 0 for s in inner.levels):       # same checks as the module's own forward
-                raise RuntimeError("dropout > 0 in training mode: the native path is inference only -- call model.eval()")
-            inner._check_cond(extra_args.get("class_cond"), extra_args.get("mapping_cond"))
-            self.inner, self.eng = inner, inner.engine()
-            if inner.class_emb is not None and not torch.cuda.is_current_stream_capturing():
-                self.eng.check_class_range(extra_args.get("class_cond"))          # once per sampler call, outside the loop
-                if self.cfg is not None and not 0 <= self.cfg.num_classes < int(self.eng.cfg.num_classes):
-                    raise IndexError(f"CFG unconditional class {self.cfg.num_classes} outside class_emb ({int(self.eng.cfg.num_classes)} rows)")
-            self.precision = inner.resolved_precision()
+            self.inner = base.inner_model
+            self.call = self.inner.native_eval(x, None, **extra_args)      # every check of the inputs, once per sampler call
+            if self.cfg is not None:
+                self.call.guide(self.cfg.num_classes)
+            self.eng, self.precision = self.call.engine, self.call.precision
             self.sigma_data = float(base.sigma_data)
             self.per_sample = any(extra_args.get(k) is not None for k in _NATIVE_KW)
             self._sig_rows, self.table = sig, None                               # conditioning table: built on first use
@@ -533,16 +526,11 @@ class _Evaluator:
         """The per-sample conditioning tensors a captured graph reads ((name, tensor) pairs, stable order)."""
         return [(k, self.extra_args[k]) for k in sorted(_NATIVE_KW) if self.native and self.extra_args.get(k) is not None]
 
-    def _cond_args(self, rows_per_eval, reps):
-        """aug / class / mapping conditioning tensors for `reps` evaluations (the doubled CFG batch included)."""
+    def _cond_args(self, reps):
+        """aug / class / mapping conditioning tensors for `reps` evaluations (the doubled CFG batch included), read from extra_args, which
+        a graph capture points at its static copies."""
         ea = self.extra_args
-        cc = ea.get("class_cond") if self.inner.class_emb is not None else None
-        if self.cfg is not None:
-            cc = torch.cat([torch.full_like(cc, self.cfg.num_classes), cc])
-        aug = ea.get("aug_cond")
-        mc = ea.get("mapping_cond") if self.inner.mapping_cond_in_proj is not None else None
-        rep_ = lambda t: None if t is None else (t if reps == 1 else t.repeat(reps, *([1] * (t.ndim - 1))))
-        return rep_(aug), rep_(cc), rep_(mc)
+        return self.call.cond_args(reps, ea.get("aug_cond"), ea.get("class_cond"), ea.get("mapping_cond"))
 
     def _per_sample_rows(self, k, rows):
         """Conditioning rows [rows, stride] of evaluation k.  All evaluations' rows come from ONE launch when they fit the
@@ -551,10 +539,10 @@ class _Evaluator:
         sig_rows = self.sigma_rows2 if self.cfg is not None else self.sigma_rows
         if self.n_evals * rows * stride * 4 <= _COND_TABLE_BYTES:
             if self.table is None:
-                aug, cc, mc = self._cond_args(rows, self.n_evals)
+                aug, cc, mc = self._cond_args(self.n_evals)
                 self.table = self.eng.conditioning(sig_rows.reshape(-1), aug, cc, mc)
             return self.table[k * rows:(k + 1) * rows]
-        aug, cc, mc = self._cond_args(rows, 1)
+        aug, cc, mc = self._cond_args(1)
         return self.eng.conditioning(sig_rows[k], aug, cc, mc)
 
     def __call__(self, k, x, out=None):
@@ -728,6 +716,30 @@ def _on_x_device(fn):
     return wrapper
 
 
+def _exec_op(op, T, ev, k, draw=None):
+    """Execute one plan op on the named buffers T; `k` indexes the next model evaluation and `draw(sigma_from, sigma_to)` makes the
+    noise of 'noise' ops.  Returns the number of model evaluations made (1 for 'eval', else 0)."""
+    kind = op[0]
+    if kind == 'eval':
+        T[op[1]] = ev(k, T[op[2]])
+        return 1
+    if kind == 'lin':
+        T[op[1]] = _lin_x([(T[n], c) for n, c in op[2]], keep_zero=True)
+    elif kind == 'euler':
+        T[op[1]] = _native.euler_step(T[op[2]], T[op[3]], op[4], noise=None if op[5] is None else T[op[5]], cn=op[6])
+    elif kind == 'heun':
+        T[op[1]] = _native.heun_correct(T[op[2]], T[op[3]], T[op[4]], T[op[5]], op[6], op[7])
+    elif kind == 'dpmpp_2m':
+        T[op[1]] = _native.dpmpp_2m_step(T[op[2]], T[op[3]], T[op[4]] if op[8] != 0 else None, *op[5:])
+    elif kind == 'noise':
+        T[op[1]] = _native.f32c(draw(op[2], op[3]))
+    elif kind == 'randn':
+        T[op[1]] = torch.randn_like(T['x'])
+    else:                    # 'keep': alias, evaluations always write fresh buffers
+        T[op[1]] = T[op[2]]
+    return 0
+
+
 def _sample_ops(name, model, x, sigmas, plan_fn, extra_args, callback, disable, params, noise_sampler=None, callback_extra=None, on_eval=None):
     """Run an op plan.  `plan_fn(sig)` builds it from the host copy of `sigmas` (or is the plan itself, a list);
     `callback_extra(st)` may add keys to the callback payload of a step; `on_eval()` runs after every model evaluation (like `callback`
@@ -738,37 +750,24 @@ def _sample_ops(name, model, x, sigmas, plan_fn, extra_args, callback, disable, 
     ours = isinstance(noise_sampler, (BrownianTreeNoiseSampler, PhiloxNoiseSampler))
     ev = _Evaluator(model, xw, extra_args, [s_ for st in plan for s_ in st['evals']])
 
+    def draw(sigma_from, sigma_to):      # our samplers take host floats (no sync); foreign callables get tensors like the reference
+        args = (sigma_from, sigma_to) if ours else (_scalar_like(sigmas, sigma_from), _scalar_like(sigmas, sigma_to))
+        return noise_sampler(*args)
+
     def body(xc):
         T = {'x': xc}
         k = 0
         for st in _progress(plan, disable):
             first = True
             for op in st['ops']:
-                kind = op[0]
-                if kind == 'eval':
-                    T[op[1]] = ev(k, T[op[2]])
-                    k += 1
+                k += _exec_op(op, T, ev, k, draw)
+                if op[0] == 'eval':
                     if on_eval is not None:
                         on_eval()
                     if first and callback is not None:
                         callback({'x': T[op[2]], 'i': st['i'], 'sigma': sigmas[st['i']], 'sigma_hat': _scalar_like(sigmas, st['sigma_hat']),
                                   'denoised': T[op[1]], **({} if callback_extra is None else callback_extra(st))})
                     first = False
-                elif kind == 'lin':
-                    T[op[1]] = _lin_x([(T[n], c) for n, c in op[2]], keep_zero=True)
-                elif kind == 'euler':
-                    T[op[1]] = _native.euler_step(T[op[2]], T[op[3]], op[4], noise=None if op[5] is None else T[op[5]], cn=op[6])
-                elif kind == 'heun':
-                    T[op[1]] = _native.heun_correct(T[op[2]], T[op[3]], T[op[4]], T[op[5]], op[6], op[7])
-                elif kind == 'dpmpp_2m':
-                    T[op[1]] = _native.dpmpp_2m_step(T[op[2]], T[op[3]], T[op[4]] if op[8] != 0 else None, *op[5:])
-                elif kind == 'noise':    # our samplers take host floats (no sync); foreign callables get tensors like the reference
-                    args = (op[2], op[3]) if ours else (_scalar_like(sigmas, op[2]), _scalar_like(sigmas, op[3]))
-                    T[op[1]] = _native.f32c(noise_sampler(*args))
-                elif kind == 'randn':
-                    T[op[1]] = torch.randn_like(T['x'])
-                else:                    # 'keep': alias, evaluations always write fresh buffers
-                    T[op[1]] = T[op[2]]
         return T['x']
 
     # a graph replays the same noise kernels every call: only legal without noise or with the Brownian tree
@@ -1041,17 +1040,11 @@ def sample_dpm_adaptive(model, x, sigma_min, sigma_max, extra_args=None, callbac
             lo_ops, _ = _dpm_step_ops(float(s), t_down, 2, 'lo', r1=1 / 3)
             ops = hi_ops[:3] + [lo_ops[3]] + hi_ops[3:]      # u1, den1, eps1 | lo | u2, den2, eps2, hi
         ev = _Evaluator(model, xc, extra_args, [_dpm_sigma(float(s))] + evals)
-        T = {'x': xc, 'den': ev(0, xc)}
-        on_eval()
-        ops = [_dpm_eps_op('eps', 'x', 'den', _dpm_sigma(float(s)))] + ops
-        k = 1
-        for op in ops:
+        T, k = {'x': xc}, 0
+        for op in [('eval', 'den', 'x'), _dpm_eps_op('eps', 'x', 'den', _dpm_sigma(float(s)))] + ops:
+            k += _exec_op(op, T, ev, k)
             if op[0] == 'eval':
-                T[op[1]] = ev(k, T[op[2]])
-                k += 1
                 on_eval()
-            else:
-                T[op[1]] = _native.lincomb([T[n_] for n_, _ in op[2]], [float(c) for _, c in op[2]])
         error = _native.dpm_error(T['lo'], T['hi'], x_prev, atol, rtol)
         accept = pid.propose_step(error)
         if accept:
