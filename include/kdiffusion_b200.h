@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 19
+#define KDB_ABI_VERSION 20
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -278,7 +278,8 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
 
 /* Parameter gradients (training) of an image_transformer_v2 model, fp32.  kdb_model_set_grad binds a gradient buffer [shape] fp32 on the
  * device to the state-dict key of a parameter, as kdb_model_set_tensor binds weights (data == NULL unbinds the key); binding needs no
- * finalize.  kdb_model_forward_train runs the raw model F (sigma_data 0) forward at fp32, bit for bit as kdb_model_forward, takes the
+ * finalize.  kdb_model_forward_train runs the raw model F (sigma_data 0) forward at the training precision (kdb_model_set_train_precision
+ * below; at the default KDB_PREC_FP32 bit for bit as kdb_model_forward), takes the
  * cotangent u [B, C_out, H, W] on out = F(x, sigma) and OVERWRITES every bound gradient with u^T dF/dparam summed over the batch; grad_x
  * (shape of x, or NULL) receives u^T dF/dx.  Unbound parameters are skipped.  The walk is that of kdb_model_forward_vjp with the weight
  * gradients added, then the AdaRMSNorm projections and the mapping network (which is why the raw conditioning inputs are passed: sigma
@@ -298,6 +299,22 @@ int     kdb_model_forward_train(KdbModel* m, int batch, int height, int width,
                                 const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
                                 const float* cotangent, float* out, float* grad_x,
                                 void* workspace, size_t workspace_bytes, void* stream);
+
+/* Training precision of an image_transformer_v2 handle: KDB_PREC_FP32 (the default, the exact path above) or KDB_PREC_TF32, any other value
+ * KDB_ERR_UNSUPPORTED, as is any value on an image_transformer_v1 handle (and KDB_PREC_TF32 when a level's width or d_ff is not a multiple
+ * of 4).  At KDB_PREC_TF32, kdb_model_finalize also builds two copies of every token-stream weight (qkv_proj, out_proj, up_proj, down_proj,
+ * merges.*.proj, splits.*.proj): one rounded to the nearest tf32 (ties away from zero) and its transpose rounded alike.  kdb_model_forward_train
+ * then runs each of those Linears, in the forward, in the input gradients and in the weight gradients, on the tensor cores with tf32 operands
+ * (activations and output gradients truncated to tf32, weights rounded) and fp32 accumulation; patch_in, patch_out, every norm, cosine-sim +
+ * RoPE, GEGLU, the attention, the mapping network and the conditioning stay exact fp32.  Still deterministic, no atomics.  The workspace of
+ * kdb_model_train_workspace_bytes is the same at both precisions.  A change of precision leaves the handle not finalized (KDB_ERR_NOT_FINAL
+ * until the next kdb_model_finalize).  kdb_model_forward, _jvp, _vjp and the sampler never read it.
+ * kdb_model_train_forward: the forward of kdb_model_forward_train without the reverse walk, at the handle's training precision: F(x), or with
+ * sigma_data > 0 the Karras-preconditioned D, bit for bit as kdb_model_forward_train's out (KDB_PREC_FP32: as kdb_model_forward at
+ * KDB_PREC_FP32).  Arguments, workspace (kdb_model_workspace_bytes at KDB_PREC_FP32) and rules as for kdb_model_forward. */
+int kdb_model_set_train_precision(KdbModel* m, int precision);
+int kdb_model_train_forward(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                            const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Debug/parity tap: arm a copy of one intermediate of the NEXT forward into `out` (fp32, device).
  * name: "patch_in", "L<l>.down", "L<l>.merge", "mid", "L<l>.split", "L<l>.up", "layer<k>.xn1",
@@ -376,6 +393,14 @@ int64_t kdb_unet_tap_count(const KdbUNet* m);
 /* ------------------------------------------------------------------------------------------
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)
  * ------------------------------------------------------------------------------------------ */
+
+/* The weight gradient of the tf32 training precision: dw[n, k] = sum over rows r < m of dy[r, n] x[r, k], dy and x truncated to tf32 (the
+ * low 13 mantissa bits cleared), products accumulated in fp32 on the tensor cores (mma.sync).  dy rows ldy floats apart (>= n) in both modes,
+ * x rows ldx (>= k); with merge_hc, merge_wc > 0, x is instead read in place as the TokenMerge 2x2 gather of contiguous fine tokens
+ * [m / (merge_hc merge_wc), 2 merge_hc, 2 merge_wc, k / 4] (ldx unused; m a multiple of merge_hc merge_wc, k of 4).  The rows are split into chunks fixed by (m, n, k) alone, each chunk's partial written to
+ * scratch (2^22 floats) and the partials summed in chunk order: no atomics, two calls give the same bits.  Every element of dw is written. */
+int kdb_wgrad_tf32(const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc, int merge_wc,
+                   float* scratch, void* stream);
 
 /* C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulate (wgmma), bf16 out. */
 int kdb_gemm_bf16(const void* a_bf16, const void* w_bf16, void* c_bf16, int M, int N, int K, void* stream);

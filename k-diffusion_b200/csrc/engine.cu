@@ -19,6 +19,13 @@
 
 namespace kdb {
 
+// The tf32 training precision's copies of a token-stream weight [N, K] (kdb_model_finalize, at KDB_PREC_TF32 only): w rounded to the
+// nearest tf32 (ties away from zero), the forward's B operand, and t = its transpose [K, N] rounded alike, the input gradient's
+struct Tf32W {
+  float* w = nullptr;
+  float* t = nullptr;
+};
+
 struct LayerPlan {
   std::string prefix;
   int level = 0, attn_type = 0, attn_param = 0, shift = 0;
@@ -31,6 +38,7 @@ struct LayerPlan {
   bf16* up_wb_il = nullptr;          // up_proj rows interleaved (value/gate) for the fused GEGLU epilogue
   bool bounded = false;              // every qr.scale[h] in (0, KDB_ATTN_MAX_BOUND]: the scale is the attention kernels' fixed softmax shift
   bf16 *qkv_wf = nullptr, *up_wf = nullptr;   // per-evaluation copies with the AdaRMSNorm channel scale folded in (fused norm)
+  Tf32W qkv_t, out_t, up_t, down_t;
 };
 
 struct PosTables {
@@ -59,6 +67,16 @@ struct KdbModel : ModelCore {
   CondWeights cw{};
   std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
   std::unordered_map<std::string, TensorRef> grads;      // kdb_model_set_grad: gradient buffers by state-dict key (written, p is not const)
+  int train_prec = KDB_PREC_FP32;                        // kdb_model_set_train_precision
+  std::vector<Tf32W> merge_t, split_t;
+  // The device buffers of the tf32 weight copies (pointer, floats), kept across finalizes instead of in `owned`: every finalize takes them
+  // in the same order (take_tf32), so the re-finalize after each optimizer step reuses them and allocates and frees nothing for them
+  std::vector<std::pair<float*, size_t>> tf32_bufs;
+  size_t tf32_next = 0;
+
+  ~KdbModel() {
+    for (auto& b : tf32_bufs) cudaFree(b.first);
+  }
 };
 
 namespace {
@@ -117,6 +135,55 @@ __global__ void interleave_geglu_rows_kernel(const float* __restrict__ w, bf16* 
     const int64_t src_row = (j < 8) ? (g * 8 + j) : ((int64_t)F + g * 8 + (j - 8));
     out[i] = __float2bfloat16_rn(w[src_row * C + c]);
   }
+}
+
+// dst [K, N] = src [N, K]^T rounded to the nearest tf32, ties away from zero (launch_unet_round_tf32's rounding), through 32 x 32 tiles
+__global__ void __launch_bounds__(256) round_tf32_transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int N, int K) {
+  __shared__ float t[32][33];
+  const int k0 = blockIdx.x * 32, n0 = blockIdx.y * 32, tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (int i = ty; i < 32; i += 8)
+    if (n0 + i < N && k0 + tx < K) t[i][tx] = src[(int64_t)(n0 + i) * K + k0 + tx];
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8)
+    if (k0 + i < K && n0 + tx < N) {
+      uint32_t r;
+      asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(t[tx][i]));
+      dst[(int64_t)(k0 + i) * N + n0 + tx] = __uint_as_float(r);
+    }
+}
+
+// the next tf32 copy buffer of n floats: the one the previous finalize took at this position when its size matches, else a new one
+int take_tf32(KdbModel* m, float** p, size_t n) {
+  auto& bufs = m->tf32_bufs;
+  const size_t i = m->tf32_next++;
+  if (i < bufs.size() && bufs[i].second == n) {
+    *p = bufs[i].first;
+    return 0;
+  }
+  if (i == bufs.size()) bufs.emplace_back(nullptr, 0);
+  cudaFree(bufs[i].first);
+  bufs[i] = {nullptr, 0};
+  void* q = nullptr;
+  KDB_CUDA(cudaMalloc(&q, n * sizeof(float) + 1024));
+  bufs[i] = {static_cast<float*>(q), n};
+  *p = bufs[i].first;
+  return 0;
+}
+
+// the buffers past those this finalize took (the model shrank, or the precision went back to fp32)
+void trim_tf32(KdbModel* m) {
+  for (size_t i = m->tf32_next; i < m->tf32_bufs.size(); ++i) cudaFree(m->tf32_bufs[i].first);
+  m->tf32_bufs.resize(std::min(m->tf32_next, m->tf32_bufs.size()));
+}
+
+// the tf32 copies of the weight [N, K] at src
+int make_tf32(KdbModel* m, const float* src, int N, int K, Tf32W* dst, cudaStream_t st) {
+  int rc;
+  if ((rc = take_tf32(m, &dst->w, (size_t)N * K)) || (rc = take_tf32(m, &dst->t, (size_t)N * K))) return rc;
+  if ((rc = launch_unet_round_tf32(src, dst->w, (int64_t)N * K, st))) return rc;
+  round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(K, 32), (unsigned)ceil_div(N, 32)), 256, 0, st>>>(src, dst->t, N, K);
+  KDB_LAUNCH_CHECK(F_CONVERT, st);
+  return 0;
 }
 
 // The layers in execution order, which is also the order of KdbModel::layers and of the conditioning row: down levels, mid, up levels
@@ -211,6 +278,9 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
     if ((rc = make_bf16(m, L.qkv_w, 3LL * L.C * L.C, &L.qkv_wb, st))) return rc;
     if ((rc = make_bf16(m, L.out_w, (int64_t)L.C * L.C, &L.out_wb, st))) return rc;
     if ((rc = m->alloc(&L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
+    if (m->train_prec == KDB_PREC_TF32 &&
+        ((rc = make_tf32(m, L.qkv_w, 3 * L.C, L.C, &L.qkv_t, st)) || (rc = make_tf32(m, L.out_w, L.C, L.C, &L.out_t, st))))
+      return rc;
   }
   const std::string f = prefix + "ff.";
   GET(f + "norm.linear.weight", &L.ff_norm_w, L.C, mw);
@@ -221,6 +291,9 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
   int rc;
   if ((rc = make_bf16(m, L.up_w, 2LL * L.dff * L.C, &L.up_wb, st))) return rc;
   if ((rc = make_bf16(m, L.down_w, (int64_t)L.C * L.dff, &L.down_wb, st))) return rc;
+  if (m->train_prec == KDB_PREC_TF32 &&
+      ((rc = make_tf32(m, L.up_w, 2 * L.dff, L.C, &L.up_t, st)) || (rc = make_tf32(m, L.down_w, L.C, L.dff, &L.down_t, st))))
+    return rc;
   if (L.dff % 8 == 0) {
     if ((rc = m->alloc(&L.up_wb_il, (size_t)2 * L.dff * L.C))) return rc;
     interleave_geglu_rows_kernel<<<kNumSMs * 4, 256, 0, st>>>(L.up_w, L.up_wb_il, L.dff, L.C);
@@ -373,6 +446,7 @@ struct Fwd {
   bool stats;               // ws.rowss holds the row statistics of the current residual stream
   bool jvp;                 // fp32 forward-mode derivative: images [B, 2B) of every token buffer carry the tangent of images [0, B)
   float* const* tape = nullptr;   // fp32 reverse mode: slot 2k / 2k+1 keep the residual stream entering layer k's attention / feed-forward half
+  bool tf32 = false;              // fp32 tokens, the tf32 training route: every token-stream Linear on the tensor cores (fwd_linear)
 
   // images held by the token buffers: linear launches and taps cover them all, nonlinear primal launches the first B
   int images() const { return jvp ? 2 * B : B; }
@@ -383,6 +457,25 @@ struct Fwd {
     e.ss_out = stats ? ws.rowss : nullptr;
   }
 };
+
+// The tf32 training route's token-stream Linear: out [M, N] = A [M, K] w^T (+ resid [M, N], which may be out) with tf32 operands and fp32
+// accumulation, the U-Net's 1x1 tensor-core convolution over M tokens.  w is a rounded copy: Tf32W::w for a forward Linear, Tf32W::t for
+// an input gradient dA = dC W.
+int linear_tf32(const float* A, const float* w, float* out, int64_t M, int N, int K, const float* resid, cudaStream_t st) {
+  KDB_REQUIRE(M <= INT32_MAX, KDB_ERR_BAD_SHAPE, "tf32 linear: %lld rows", (long long)M);
+  ConvArgs a;
+  a.in1 = A, a.c1 = K, a.w = w, a.r1 = resid, a.rc1 = resid ? N : 0, a.out = out;
+  a.B = 1, a.H = 1, a.W = (int)M, a.N = N;
+  return launch_unet_conv_tf32(a, 1, st, F_GEMM_TF32);
+}
+
+// A token-stream Linear of the forward (STORE or RESID): linear_tf32 on the copy wt on the tf32 route, else linear<T>
+template <typename T>
+int fwd_linear(const Fwd& f, const T* A, const typename WSel<T>::W* W, const Tf32W& wt, T* C, int64_t M, int N, int K, const GemmEpi& e) {
+  if constexpr (std::is_same_v<T, float>)
+    if (f.tf32) return linear_tf32(A, wt.w, C, M, N, K, e.mode == EPI_RESID ? static_cast<const float*>(e.resid) : nullptr, f.st);
+  return linear<T>(A, W, C, M, N, K, e, f.st);
+}
 
 // The attention half's activations from the residual stream x, up to the attention output in ws.ao: the qkv projection goes to raw,
 // the cosine-normalised and rotated q, k (with v) to ws.qkv.  The forward passes raw = ws.qkv and cosine-sim + RoPE runs in place (so
@@ -411,7 +504,7 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
   };
   auto unfused = [&] {
     int r = norm();
-    if (!r) r = linear<T>(xn, WSel<T>::qkv(L), raw, Ma, 3 * C, C, GemmEpi{}, f.st);
+    if (!r) r = fwd_linear<T>(f, xn, WSel<T>::qkv(L), L.qkv_t, raw, Ma, 3 * C, C, GemmEpi{});
     // the tangent reads the un-normalised primal q and k, so it runs before the primal launch
     if constexpr (std::is_same_v<T, float>)
       if (!r && f.jvp) r = launch_qknorm_rope_jvp(raw, raw + M * 3 * C, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
@@ -462,7 +555,7 @@ int ff_up(KdbModel* m, Fwd& f, int k, const T* x, int h, int w) {
   int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
   if constexpr (std::is_same_v<T, float>)
     if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-  return r ? r : linear<T>(xn, WSel<T>::up(L), reinterpret_cast<T*>(f.ws.hbuf), f.images() * Ttok, 2 * L.dff, C, GemmEpi{}, f.st);
+  return r ? r : fwd_linear<T>(f, xn, WSel<T>::up(L), L.up_t, reinterpret_cast<T*>(f.ws.hbuf), f.images() * Ttok, 2 * L.dff, C, GemmEpi{});
 }
 
 template <typename T>
@@ -493,7 +586,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
       e.mode = EPI_RESID;
       e.resid = x;
       f.produce(e, Ma, C, C);
-      if ((rc = linear<T>(reinterpret_cast<T*>(f.ws.ao), WSel<T>::out(L), x, Ma, C, C, e, f.st))) return rc;
+      if ((rc = fwd_linear<T>(f, reinterpret_cast<T*>(f.ws.ao), WSel<T>::out(L), L.out_t, x, Ma, C, C, e))) return rc;
     }
     if ((rc = m->tap<T>(tag + ".attn", x, Ma * C, f.st))) return rc;
   }
@@ -539,7 +632,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     e.mode = EPI_RESID;
     e.resid = x;
     f.produce(e, Ma, C, L.dff);
-    if ((rc = linear<T>(gb, WSel<T>::down(L), x, Ma, C, L.dff, e, f.st))) return rc;
+    if ((rc = fwd_linear<T>(f, gb, WSel<T>::down(L), L.down_t, x, Ma, C, L.dff, e))) return rc;
   }
   return m->tap<T>(tag + ".ff", x, Ma * C, f.st);
 }
@@ -550,10 +643,12 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
 // tape != nullptr (fp32 only): the residual stream entering every attention / feed-forward half and out_norm is copied to the tape
 // (slots 2k, 2k+1 of layer k, slot 2 * layers for out_norm) for the reverse walk of kdb_model_forward_vjp; the launches are unchanged.
 // pos_tables != nullptr: receives the position tables of this token grid.
+// tf32 (fp32 only): the tf32 training route, every token-stream Linear through linear_tf32 on finalize's copies; TokenSplit then stores
+// its projection to ws.mg and un-patches it with the lerp in launch_split_unpatch_lerp.
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
                  int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st, float* const* tape = nullptr,
-                 const PosTables** pos_tables = nullptr) {
+                 const PosTables** pos_tables = nullptr, bool tf32 = false) {
   constexpr bool kBf16 = std::is_same_v<T, bf16>;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
@@ -566,6 +661,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false, !kBf16 && v != nullptr};
   f.fold = f.emit && cond_bs == 0 && m->fold_descs != nullptr;
   f.tape = tape;
+  f.tf32 = tf32;
   if (f.fold && (rc = launch_fold_norm_weights(m->fold_descs, m->n_fold, cond, st))) return rc;
   const int Bt = f.images();
 
@@ -603,7 +699,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       T* mg = reinterpret_cast<T*>(ws.mg);
       f.stats = false;
       int r = launch_merge_gather<T>(cur, mg, Bt, h, w, c.width[l], st);
-      return r ? r : linear<T>(mg, WSel<T>::merge(m, l), nxt, Mc, N, K, GemmEpi{}, st);
+      return r ? r : fwd_linear<T>(f, mg, WSel<T>::merge(m, l), m->merge_t[l], nxt, Mc, N, K, GemmEpi{});
     };
     // TokenMerge: the 2x2 gather rides on the GEMM's TMA loads when the geometry allows, else a gather kernel and a plain GEMM
     if constexpr (kBf16) {
@@ -639,7 +735,16 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     e.wc = w;
     e.C = c.width[l];
     f.produce(e, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1]);
-    if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], e, st))) return rc;
+    if (tf32) {
+      if constexpr (!kBf16) {
+        float* y = reinterpret_cast<float*>(ws.mg);
+        if ((rc = linear_tf32(cur, m->split_t[l].w, y, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], nullptr, st)) ||
+            (rc = launch_split_unpatch_lerp(y, reinterpret_cast<const float*>(ws.xs[l]), m->split_fac[l], up, Bt, 2 * h, 2 * w, c.width[l], st)))
+          return rc;
+      }
+    } else if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], e, st))) {
+      return rc;
+    }
     h *= 2;
     w *= 2;
     if ((rc = m->tap<T>("L" + std::to_string(l) + ".split", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
@@ -751,6 +856,16 @@ struct Train {
   }
 };
 
+// The reverse walk's token-stream GEMMs: the input gradient dA [M, K] = dC [M, N] W [N, K] and the weight gradient dW [N, K] = dY^T X, on
+// the tf32 route on the tensor cores (linear_tf32 on the transposed copy, launch_wgrad_tf32), else exact fp32
+int input_grad(bool tf32, const float* dC, const float* W, const Tf32W& wt, float* out, int64_t M, int N, int K, cudaStream_t st) {
+  return tf32 ? linear_tf32(dC, wt.t, out, M, K, N, nullptr, st) : launch_gemm_vjp(dC, W, out, M, N, K, VJP_STORE, 0, 0, 0, st);
+}
+int weight_grad(bool tf32, const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part,
+                cudaStream_t st) {
+  return tf32 ? launch_wgrad_tf32(dY, ldy, X, ldx, dW, M, N, K, part, st) : launch_wgrad(dY, ldy, X, ldx, dW, M, N, K, part, st);
+}
+
 // Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
 // its activations from the tape with the forward's functions (ff_up, attn_activations; f is an fp32 forward of B images), runs the
 // backward kernels and adds the branch gradient to g.
@@ -771,30 +886,31 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
   if ((rc = ff_up<float>(m, f, k, x, h, w))) return rc;
   if (tr) {   // down_proj's input, the GEGLU output
     float* gb = reinterpret_cast<float*>(f.ws.gbuf);
-    if ((rc = launch_geglu<float>(hb, gb, M, F, st)) || (rc = launch_wgrad(g, C, gb, F, tr->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
+    if ((rc = launch_geglu<float>(hb, gb, M, F, st)) ||
+        (rc = weight_grad(f.tf32, g, C, gb, F, tr->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
       return rc;
   }
-  if ((rc = launch_gemm_vjp(g, L.down_w, vs.dbuf, M, C, F, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = input_grad(f.tf32, g, L.down_w, L.down_t, vs.dbuf, M, C, F, st))) return rc;
   if ((rc = launch_geglu_vjp(hb, vs.dbuf, vs.dh, M, F, st))) return rc;
-  if (tr && (rc = launch_wgrad(vs.dh, 2 * F, xn, C, tr->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
-  if ((rc = launch_gemm_vjp(vs.dh, L.up_w, xn, M, 2 * F, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if (tr && (rc = weight_grad(f.tf32, vs.dh, 2 * F, xn, C, tr->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
+  if ((rc = input_grad(f.tf32, vs.dh, L.up_w, L.up_t, xn, M, 2 * F, C, st))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_ff, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   if ((rc = launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, st))) return rc;
   if (L.attn_type == KDB_ATTN_NONE) return 0;
   // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
   x = vs.tape[2 * k];
   if ((rc = attn_activations<float>(m, f, k, x, h, w, vs.qkv_raw))) return rc;
-  if (tr && (rc = launch_wgrad(g, C, ao, C, tr->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
-  if ((rc = launch_gemm_vjp(g, L.out_w, vs.dbuf, M, C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if (tr && (rc = weight_grad(f.tf32, g, C, ao, C, tr->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
+  if ((rc = input_grad(f.tf32, g, L.out_w, L.out_t, vs.dbuf, M, C, C, st))) return rc;
   if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
   // the attention's statistics are spent: vs.stats takes the per-(row, head) terms of the head scales' gradient
   if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st, tr ? vs.stats : nullptr)))
     return rc;
   if (tr && ((rc = launch_colsum(vs.stats, M, L.nh, tr->grad(sa + "scale"), vs.part, st)) ||
-             (rc = launch_wgrad(vs.dqkv, 3 * C, xn, C, tr->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
+             (rc = weight_grad(f.tf32, vs.dqkv, 3 * C, xn, C, tr->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
     return rc;
-  if ((rc = launch_gemm_vjp(vs.dqkv, L.qkv_w, xn, M, 3 * C, C, VJP_STORE, 0, 0, 0, st))) return rc;
+  if ((rc = input_grad(f.tf32, vs.dqkv, L.qkv_w, L.qkv_t, xn, M, 3 * C, C, st))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_attn, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   return launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, st);
 }
@@ -803,16 +919,19 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
 // reverse: patch_out + out_norm + combine; each up level's layers then its split-lerp; the mid layers; each down level (innermost
 // first) its merge then its layers; patch_in.
 // tr != nullptr (kdb_model_forward_train): along the walk, the gradients of patch_out, out_norm, every layer, split and merge, patch_in, and
-// the AdaRMSNorm scales into vs.dscale; grad_x may then be nullptr.
+// the AdaRMSNorm scales into vs.dscale; grad_x may then be nullptr.  At the tf32 training precision the forward, the recomputes and every
+// token-stream input and weight gradient take the tf32 route.
 int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, const float* sigma, float sd, const float* cond, int64_t cond_bs,
              float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st, const Train* tr = nullptr) {
   const PosTables* pt = nullptr;
-  int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data(), &pt);
+  const bool tf32 = tr != nullptr && m->train_prec == KDB_PREC_TF32;
+  int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data(), &pt, tf32);
   if (rc) return rc;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, C0 = c.width[0];
   const int h0 = H / c.patch_h, w0 = W / c.patch_w;
   Fwd f{B, ws, st, cond, cond_bs, pt, false, false, false, false};
+  f.tf32 = tf32;
   const int64_t M0 = (int64_t)B * h0 * w0;
   float* part = vs.part;
   // training: the backward also leaves out_norm's output gradient (ws.xn) and rstd; patch_out's weight gradient then reads its output
@@ -836,31 +955,39 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
     const std::string sp = "splits." + std::to_string(l) + ".";
     if (tr) {   // d fac = sum (y - skip) dup with y = the split projection recomputed (vs.dbuf), skip = ws.xs[l]
-      if ((rc = launch_gemm_simt<float, float>(coarse, m->split_w[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{}, st)) ||
+      if ((rc = tf32 ? linear_tf32(coarse, m->split_t[l].w, vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], nullptr, st)
+                     : launch_gemm_simt<float, float>(coarse, m->split_w[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{}, st)) ||
           (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], tr->grad(sp + "fac"), B, h, w, c.width[l],
                                       part, st)))
         return rc;
     }
     // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
     if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
-    if (tr && (rc = launch_wgrad(mg, 4 * c.width[l], coarse, c.width[l + 1], tr->grad(sp + "proj.weight"), Mc, 4 * c.width[l], c.width[l + 1],
-                                 part, st)))
+    if (tr && (rc = weight_grad(tf32, mg, 4 * c.width[l], coarse, c.width[l + 1], tr->grad(sp + "proj.weight"), Mc, 4 * c.width[l],
+                                c.width[l + 1], part, st)))
       return rc;
-    if ((rc = launch_gemm_vjp(mg, m->split_w[l], vs.g[l + 1], (int64_t)B * (h / 2) * (w / 2), 4 * c.width[l], c.width[l + 1], VJP_STORE, 0, 0, 0,
-                              st)))
-      return rc;
+    if ((rc = input_grad(tf32, mg, m->split_w[l], m->split_t[l], vs.g[l + 1], Mc, 4 * c.width[l], c.width[l + 1], st))) return rc;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
     if ((rc = vjp_layer(m, f, vs, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1), tr))) return rc;
   for (int l = n - 2; l >= 0; --l) {
     const int h = h0 >> l, w = w0 >> l;
-    if (tr && (rc = launch_wgrad_merge(vs.g[l + 1], reinterpret_cast<const float*>(ws.xs[l]), tr->grad("merges." + std::to_string(l) + ".proj.weight"),
-                                       (int64_t)B * (h / 2) * (w / 2), c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
+    const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
+    float* dmw = tr ? tr->grad("merges." + std::to_string(l) + ".proj.weight") : nullptr;
+    const float* fine = reinterpret_cast<const float*>(ws.xs[l]);
+    if (dmw && (rc = tf32 ? launch_wgrad_tf32_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)
+                          : launch_wgrad_merge(vs.g[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
       return rc;
-    // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added
-    if ((rc = launch_gemm_vjp(vs.g[l + 1], m->merge_w[l], vs.g[l], (int64_t)B * (h / 2) * (w / 2), c.width[l + 1], 4 * c.width[l],
-                              VJP_UNPATCH_ACC, h / 2, w / 2, c.width[l], st)))
+    // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added; on the tf32 route the
+    // GEMM stores dnxt W to ws.mg and a scatter kernel adds it
+    if (tf32) {
+      if ((rc = linear_tf32(vs.g[l + 1], m->merge_t[l].t, mg, Mc, 4 * c.width[l], c.width[l + 1], nullptr, st)) ||
+          (rc = launch_merge_scatter_add(mg, vs.g[l], B, h, w, c.width[l], st)))
+        return rc;
+    } else if ((rc = launch_gemm_vjp(vs.g[l + 1], m->merge_w[l], vs.g[l], Mc, c.width[l + 1], 4 * c.width[l], VJP_UNPATCH_ACC, h / 2, w / 2,
+                                     c.width[l], st))) {
       return rc;
+    }
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w, tr))) return rc;
   }
@@ -917,6 +1044,9 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->split_fac.assign(n, nullptr);
   m->merge_wb.assign(n, nullptr);
   m->split_wb.assign(n, nullptr);
+  m->merge_t.assign(n, Tf32W{});
+  m->split_t.assign(n, Tf32W{});
+  m->tf32_next = 0;
   int ada = 0;
   int rc = for_each_layer(c, [&](const std::string& prefix, int level, int index) {
     m->layers.emplace_back();
@@ -948,7 +1078,11 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     GET("splits." + std::to_string(l) + ".fac", &m->split_fac[l], 1);
     if ((rc = make_bf16(m, m->merge_w[l], 4LL * c.width[l] * c.width[l + 1], &m->merge_wb[l], st))) return rc;
     if ((rc = make_bf16(m, m->split_w[l], 4LL * c.width[l] * c.width[l + 1], &m->split_wb[l], st))) return rc;
+    if (m->train_prec == KDB_PREC_TF32 && ((rc = make_tf32(m, m->merge_w[l], c.width[l + 1], 4 * c.width[l], &m->merge_t[l], st)) ||
+                                           (rc = make_tf32(m, m->split_w[l], 4 * c.width[l], c.width[l + 1], &m->split_t[l], st))))
+      return rc;
   }
+  trim_tf32(m);
   const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels, Ni = c.patch_h * c.patch_w * c.in_channels;
   GET("out_norm.scale", &m->out_norm, C0);
   if (c.family == KDB_FAMILY_ITV1) {   // in_proj / out_proj (image_transformer_v1.py:295,298) in the engine's patch feature order
@@ -1245,6 +1379,48 @@ int kdb_model_forward_train(KdbModel* m, int batch, int height, int width, const
     return rc;
   if (c.num_classes > 0) return launch_class_emb_grad(demb, G, class_cond, tr.grad("class_emb.weight"), B, c.num_classes, mw, st);
   return 0;
+}
+
+int kdb_model_set_train_precision(KdbModel* m, int precision) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "set_train_precision: NULL model");
+  const KdbModelConfig& c = m->cfg;
+  KDB_REQUIRE(c.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED, "set_train_precision: parameter gradients are built for image_transformer_v2 only");
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED,
+              "set_train_precision: training runs at fp32 or tf32 (precision %d)", precision);
+  if (precision == KDB_PREC_TF32)
+    for (int l = 0; l < c.n_levels; ++l)   // the tensor-core GEMM's TMA rows: 16-byte strides
+      KDB_REQUIRE(c.width[l] % 4 == 0 && c.d_ff[l] % 4 == 0, KDB_ERR_UNSUPPORTED,
+                  "set_train_precision: tf32 needs widths and d_ff that are multiples of 4 (level %d: %d, %d)", l, c.width[l], c.d_ff[l]);
+  if (precision != m->train_prec) m->finalized = false;   // the tf32 weight copies are finalize's
+  m->train_prec = precision;
+  return 0;
+}
+
+int kdb_model_train_forward(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, float sigma_data, const float* cond,
+                            int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "train_forward: model not finalized");
+  KDB_REQUIRE(m->cfg.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED, "train_forward: parameter gradients are built for image_transformer_v2 only");
+  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "train_forward: NULL argument");
+  int rc = check_image(m, "train_forward", height, width, sigma_data);
+  if (rc) return rc;
+  Workspace ws;
+  if ((rc = carve_checked(m, "train_forward", KDB_PREC_FP32, batch, height, width, workspace, workspace_bytes, ws))) return rc;
+  return m->disarm_tap(forward_impl<float>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
+                                           (cudaStream_t)stream, nullptr, nullptr, m->train_prec == KDB_PREC_TF32));
+}
+
+int kdb_wgrad_tf32(const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc, int merge_wc,
+                   float* scratch, void* stream) {
+  KDB_REQUIRE(dy && x && dw && scratch && m > 0 && n > 0 && k > 0, KDB_ERR_BAD_ARG, "wgrad_tf32: bad argument");
+  KDB_REQUIRE(ldy >= n, KDB_ERR_BAD_ARG, "wgrad_tf32: ldy %lld < n %d", (long long)ldy, n);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (merge_hc > 0 || merge_wc > 0) {
+    KDB_REQUIRE(merge_hc > 0 && merge_wc > 0 && k % 4 == 0 && m % ((int64_t)merge_hc * merge_wc) == 0, KDB_ERR_BAD_SHAPE,
+                "wgrad_tf32: merge geometry %dx%d with k %d, m %lld", merge_hc, merge_wc, k, (long long)m);
+    return launch_wgrad_tf32_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st);
+  }
+  KDB_REQUIRE(ldx >= k, KDB_ERR_BAD_ARG, "wgrad_tf32: ldx %lld < k %d", (long long)ldx, k);
+  return launch_wgrad_tf32(dy, ldy, x, ldx, dw, m, n, k, scratch, st);
 }
 
 int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

@@ -1157,6 +1157,44 @@ int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int
   return 0;
 }
 
+// TokenSplit after a plain projection y [B, H/2, W/2, (nh nw e)]: up = lerp(skip, unpatch2x2(y), fac), as gemm_simt_kernel's
+// EPI_SPLIT_LERP epilogue computes each element.  One thread per element, coarse index i in the TokenMerge order.
+__global__ void __launch_bounds__(256) split_unpatch_lerp_kernel(const float* __restrict__ y, const float* __restrict__ skip,
+                                                                 const float* __restrict__ fac, float* __restrict__ up, int H, int Wd, int C,
+                                                                 int64_t total) {
+  const float f = __ldg(fac);
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int64_t dst = merge_source(i, H / 2, Wd / 2, C);
+    up[dst] = lerp_like_torch(skip[dst], y[i], f);
+  }
+}
+
+int launch_split_unpatch_lerp(const float* y, const float* skip, const float* fac, float* up, int B, int H, int Wd, int C, cudaStream_t st) {
+  KDB_REQUIRE(H % 2 == 0 && Wd % 2 == 0, KDB_ERR_BAD_SHAPE, "token split: grid %dx%d not even", H, Wd);
+  const int64_t total = (int64_t)B * H * Wd * C;
+  split_unpatch_lerp_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(y, skip, fac, up, H, Wd, C, total);
+  KDB_LAUNCH_CHECK(F_MERGE_GATHER, st);
+  return 0;
+}
+
+// TokenMerge VJP after a plain input-gradient GEMM d [B, H/2, W/2, (nh nw e)]: dfine += unpatch2x2(d).  The map is a bijection, so each
+// fine element is read and written by one thread.
+__global__ void __launch_bounds__(256) merge_scatter_add_kernel(const float* __restrict__ d, float* __restrict__ dfine, int H, int Wd, int C,
+                                                                int64_t total) {
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
+    const int64_t dst = merge_source(i, H / 2, Wd / 2, C);
+    dfine[dst] += d[i];
+  }
+}
+
+int launch_merge_scatter_add(const float* d, float* dfine, int B, int H, int Wd, int C, cudaStream_t st) {
+  KDB_REQUIRE(H % 2 == 0 && Wd % 2 == 0, KDB_ERR_BAD_SHAPE, "token merge vjp: grid %dx%d not even", H, Wd);
+  const int64_t total = (int64_t)B * H * Wd * C;
+  merge_scatter_add_kernel<<<grid_stride_blocks(total), 256, 0, st>>>(d, dfine, H, Wd, C, total);
+  KDB_LAUNCH_CHECK(F_MERGE_GATHER, st);
+  return 0;
+}
+
 // patch_out + out_norm VJP: per token, dy = patch(c_out u) (c_out = 1 for the raw model), dxn = dy W_po, dt = RMSNorm_vjp(tokens, dxn)
 // written to dtokens.  One warp per token.
 __global__ void __launch_bounds__(128) patch_out_vjp_kernel(const float* __restrict__ tokens, const float* __restrict__ nscale,

@@ -155,6 +155,10 @@ int launch_attention_vjp(const float* qkv, const float* out, const float* dout, 
 int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int F, cudaStream_t st);
 // TokenSplit lerp: out [B, H/2, W/2, 4C] = patch2x2(fac dup) (then launch_gemm_vjp with the split weight), dup *= (1 - fac) in place
 int launch_split_vjp_gather(float* dup, float* out, const float* fac, int B, int H, int Wd, int C, cudaStream_t st);
+// The elementwise halves of TokenSplit and of the TokenMerge VJP around a plain [M, N] GEMM (the tf32 training route): H, Wd the fine grid, C
+// the fine channels.  up = lerp(skip, unpatch2x2(y), fac) with y [B, H/2, W/2, 4C]; dfine += unpatch2x2(d) with d [B, H/2, W/2, 4C].
+int launch_split_unpatch_lerp(const float* y, const float* skip, const float* fac, float* up, int B, int H, int Wd, int C, cudaStream_t st);
+int launch_merge_scatter_add(const float* d, float* dfine, int B, int H, int Wd, int C, cudaStream_t st);
 // out_norm + patch_out + un-patch: dtokens = RMSNorm_vjp(tokens, patch(c_out u) W_po)  (c_out = 1 when sigma_data <= 0)
 // Where given, also dnorm [tokens, C0] the gradient of out_norm's output and rstd [tokens] each token's rsqrt(mean(x^2) + eps) as the
 // forward computes it
@@ -219,6 +223,12 @@ constexpr int64_t kTrainPartFloats = int64_t(1) << 22;
 int launch_wgrad(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part, cudaStream_t st);
 // the same with X the TokenMerge gather of the fine tokens [B, 2hc, 2wc, Cf] (M = B hc wc coarse rows, K = 4 Cf) read in place
 int launch_wgrad_merge(const float* dY, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part, cudaStream_t st);
+// Both with tf32 operands on the tensor cores (mma.sync): dY and X truncated to tf32 (the low 13 mantissa bits cleared), fp32 accumulation,
+// the same row chunks and chunk-order sum as launch_wgrad
+int launch_wgrad_tf32(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part,
+                      cudaStream_t st);
+int launch_wgrad_tf32_merge(const float* dY, int64_t ldy, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part,
+                            cudaStream_t st);
 // out[b * ldo + c] = sum over the rows r of image b of dy[r, c] x[r, c] rsqrt(mean(x_r^2) + eps): the gradient of an RMSNorm's channel scale
 // per image (rows_per_batch rows each; rows_per_batch == rows: one sum over all rows)
 int launch_norm_scale_grad(const float* x, int64_t ldx, const float* dy, int64_t ldy, float* out, int64_t ldo, int64_t rows_per_batch,

@@ -28,7 +28,8 @@ struct ConvArgs {
 int launch_unet_conv(const ConvArgs& a, int ks, cudaStream_t st);
 // The same convolution on the tensor cores at KDB_PREC_TF32 (unet_tf32.cu): tf32 operands, fp32 accumulation.  w is expected rounded
 // to tf32 (launch_unet_round_tf32); activations are truncated to tf32 by the MMA.
-int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st);
+// family: the launch family it is counted under (kdb_launch_breakdown)
+int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st, int family = F_UNET_CONV_TF32);
 // ... at KDB_PREC_FP16 (unet_tf32.cu): fp16 operands, fp32 accumulation.  a.w is not read: w is the fp16 tap-major weight
 // [N, ks*ks, f16_weight_ld(c1 + c2)] (launch_unet_round_f16); activations are rounded to the nearest fp16 (ties to even) in registers.
 // An operand of magnitude >= 65520 becomes +-inf (no saturation).

@@ -576,8 +576,8 @@ int launch_attn_tc(const float* qkv, float* out, int B, int T, int nh, int d_hea
 
 int f16_weight_ld(int channels) { return (channels + 7) / 8 * 8; }
 
-int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st) {
-  return launch_conv_tc<Tf32Ops>(a, a.w, ks, st, "unet_conv_tf32", F_UNET_CONV_TF32);
+int launch_unet_conv_tf32(const ConvArgs& a, int ks, cudaStream_t st, int family) {
+  return launch_conv_tc<Tf32Ops>(a, a.w, ks, st, "unet_conv_tf32", family);
 }
 
 int launch_unet_conv_fp16(const ConvArgs& a, const __half* w, int ks, cudaStream_t st) {

@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 19
+ABI_VERSION = 20
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -80,6 +80,8 @@ SIGNATURES = {
     "kdb_model_set_grad": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
     "kdb_model_train_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
     "kdb_model_forward_train": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_model_set_train_precision": (_i32, [_vp, _i32]),
+    "kdb_model_train_forward": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_loss_noised_input": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
     "kdb_denoiser_loss": (_i32, [_i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i32, _i64, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
@@ -94,6 +96,7 @@ SIGNATURES = {
     "kdb_unet_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_unet_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_unet_tap_count": (_i64, [_vp]),
+    "kdb_wgrad_tf32": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16_geglu": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
@@ -702,6 +705,24 @@ class Engine:
                                                 ptr(cond), self._stride, ptr(u), ptr(out), ptr(grad_x), ptr(ws), ws.numel(), stream()))
         return out
 
+    def set_train_precision(self, precision):
+        """kdb_model_set_train_precision (PREC_FP32 or PREC_TF32); a change re-finalizes at the next bind, which builds or drops the tf32
+        weight copies."""
+        if precision != getattr(self, "_train_prec", PREC_FP32):
+            check(lib().kdb_model_set_train_precision(self._h, precision))
+            self._train_prec, self._sig = precision, None
+
+    def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, out=None):
+        """kdb_model_train_forward: the forward of forward_train at the training precision (x [B,C,H,W] fp32), bit for bit its `out`."""
+        B, _, H, W = x.shape
+        if out is None:
+            out = torch.empty(B, self.cfg.out_channels, H, W, device=x.device, dtype=torch.float32)
+        ws = self._workspace(PREC_FP32, B, H, W, x.device)
+        with device_of(x):
+            check(lib().kdb_model_train_forward(self._h, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride, ptr(out),
+                                                ptr(ws), ws.numel(), stream()))
+        return out
+
     def arm_tap(self, name, capacity, device):
         buf = torch.empty(capacity, dtype=torch.float32, device=device)
         check(self._fn("debug_tap")(self._h, name.encode(), ptr(buf), capacity))
@@ -760,6 +781,39 @@ def gemm_bf16(a, w):
     N = w.shape[0]
     out = torch.empty(M, N, dtype=torch.bfloat16, device=a.device)
     check(lib().kdb_gemm_bf16(ptr(a), ptr(w), ptr(out), M, N, K, stream()))
+    return out
+
+
+WGRAD_SCRATCH_FLOATS = 1 << 22
+
+
+@_on_device_of_first
+def wgrad_tf32(dy, x, n_rows=None, merge=None, out=None):
+    """kdb_wgrad_tf32: dW [N, K] = dy[:m]^T x[:m] with tf32 operands (truncated) and fp32 accumulation.  dy [m, N] and x [m, K] fp32
+    with unit column stride (any row stride); merge=(hc, wc): x is instead the fine tokens [B, 2hc, 2wc, Cf] read as the TokenMerge gather,
+    K = 4 Cf.  out: an [N, K] fp32 contiguous buffer to write (every element is written)."""
+    require_cuda(dy, x, out)
+    m = dy.shape[0] if n_rows is None else n_rows
+    N = dy.shape[1]
+    K = x.shape[-1] * 4 if merge else x.shape[1]
+    if dy.dtype != torch.float32 or x.dtype != torch.float32 or dy.ndim != 2 or x.ndim != (4 if merge else 2):
+        raise ValueError("wgrad_tf32: dy [m, N] and x [m, K] (merge: [B, 2hc, 2wc, Cf]) fp32")
+    if dy.stride(1) != 1 or (not merge and x.stride(1) != 1) or (merge and not x.is_contiguous()):
+        raise ValueError("wgrad_tf32: operands need contiguous rows (the merge gather: contiguous fine tokens)")
+    if not 0 < m <= dy.shape[0]:
+        raise ValueError(f"wgrad_tf32: {m} rows of a dy with {dy.shape[0]}")
+    if merge:
+        hc, wc = merge
+        if hc <= 0 or wc <= 0 or tuple(x.shape[1:3]) != (2 * hc, 2 * wc) or m % (hc * wc) or m // (hc * wc) > x.shape[0]:
+            raise ValueError(f"wgrad_tf32: fine tokens {tuple(x.shape)} do not hold the TokenMerge gather of {m} rows of a {hc}x{wc} grid")
+    elif m > x.shape[0]:
+        raise ValueError(f"wgrad_tf32: {m} rows of an x with {x.shape[0]}")
+    if out is not None and (tuple(out.shape) != (N, K) or out.dtype != torch.float32 or not out.is_contiguous()):
+        raise ValueError(f"wgrad_tf32: out must be a contiguous fp32 [{N}, {K}] tensor")
+    out = torch.empty(N, K, device=dy.device, dtype=torch.float32) if out is None else out
+    scratch = torch.empty(WGRAD_SCRATCH_FLOATS, device=dy.device, dtype=torch.float32)
+    hc, wc = merge if merge else (0, 0)
+    check(lib().kdb_wgrad_tf32(ptr(dy), dy.stride(0), ptr(x), 0 if merge else x.stride(0), ptr(out), m, N, K, hc, wc, ptr(scratch), stream()))
     return out
 
 

@@ -57,6 +57,11 @@ class KarrasAugmentWrapper(nn.Module):
         self.inner_model.set_precision(precision)
         return self
 
+    def set_train_precision(self, precision):
+        """The inner model's training precision (image_transformer_v2 only; the U-Net raises NotImplementedError)."""
+        self.inner_model.set_train_precision(precision)
+        return self
+
     def resolved_precision(self):
         return self.inner_model.resolved_precision()
 

@@ -3,8 +3,9 @@
 Constructor signature, spec dataclasses and `state_dict()` layout follow the reference
 (k_diffusion/models/image_transformer_v2.py:626-706) so reference checkpoints load unchanged; the
 forward pass itself (:721-762) is executed by libkdb200.so.  This module holds no layer logic: it
-is a tree of named parameters whose names reproduce the reference keys.  Parameter gradients (training) come from the engine's fp32
-reverse walk through `Denoiser.loss`; `param_groups` returns the reference's optimizer groups.
+is a tree of named parameters whose names reproduce the reference keys.  Parameter gradients (training) come from the engine's reverse
+walk through `Denoiser.loss`, at fp32 or, after `set_train_precision("tf32")`, with tf32 token-stream GEMMs; `param_groups` returns the
+reference's optimizer groups.
 """
 import math
 from dataclasses import dataclass
@@ -189,12 +190,27 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         eng = self._engines.get(None)
         if eng is None:
             eng = self._engines[None] = _native.Engine(self.engine_spec())
+        eng.set_train_precision(getattr(self, "train_precision", _native.PREC_FP32))
         eng.bind(dict(self.state_dict(keep_vars=True)))
         return eng
 
     def set_precision(self, precision):
         """'fp32' (exact path, parity gate), 'bf16' (tensor-core path) or None/'auto'."""
         self.precision = None if precision in (None, "auto") else precision
+        return self
+
+    _TRAIN_PRECISIONS = {None: _native.PREC_FP32, "fp32": _native.PREC_FP32, "float32": _native.PREC_FP32, "tf32": _native.PREC_TF32}
+
+    def set_train_precision(self, precision):
+        """The arithmetic of `Denoiser.loss` and its backward: 'fp32' / 'float32' / None (the default, exact fp32) or 'tf32' (every
+        token-stream Linear -- qkv, out, up, down, merge and split projections -- with tf32 operands and fp32 accumulation on the tensor
+        cores, in the loss's forward, its input gradients and its weight gradients; what an nn.Linear computes under
+        torch.backends.cuda.matmul.allow_tf32 = True).  Sampling, `jvp`, `vjp` and autograd through x are not affected."""
+        if self.family != _native.FAMILY_ITV2:
+            raise NotImplementedError(f"{self.kind}: parameter gradients are built for image_transformer_v2 models only")
+        if not (precision is None or isinstance(precision, str)) or precision not in self._TRAIN_PRECISIONS:
+            raise ValueError(f"training runs at 'fp32' or 'tf32' (got {precision!r})")
+        self.train_precision = self._TRAIN_PRECISIONS[precision]
         return self
 
     def resolved_precision(self):
@@ -219,8 +235,8 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
     def native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, class_cond=None, mapping_cond=None):
         """Per-sample training losses [B] of the Karras-preconditioned denoiser around this model (`_native.LOSS_DENOISER`: reference
         layers.py:76-86 with scales == 1 and per-sample `weight`; `LOSS_SIMPLE`: :107-111), with a grad_fn that reaches every parameter
-        requiring grad.  The forward is one fp32 engine evaluation and one loss kernel; the backward is one kdb_model_forward_train.
-        Always fp32, whatever `set_precision` selected."""
+        requiring grad.  The forward is one engine evaluation and one loss kernel; the backward is one kdb_model_forward_train.  The
+        arithmetic is `set_train_precision`'s (fp32 unless set), whatever `set_precision` selected."""
         if self.family != _native.FAMILY_ITV2:
             raise NotImplementedError(f"{self.kind}: parameter gradients are built for image_transformer_v2 models only")
         for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
@@ -385,7 +401,10 @@ class _NativeLoss(torch.autograd.Function):
         w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
         xin = _native.loss_noised_input(x, noise, sig, sigma_data)
         cond = ev.conditioning()
-        f = ev.engine.forward(xin, sig, cond, ev.engine.cond_stride, 0.0, ev.precision)
+        if getattr(model, "train_precision", _native.PREC_FP32) == _native.PREC_TF32:   # the forward of the tf32 training walk
+            f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0)
+        else:
+            f = ev.engine.forward(xin, sig, cond, ev.engine.cond_stride, 0.0, ev.precision)
         loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
         aug, cls, mc = ev.cond
         ctx.model, ctx.keys = model, keys

@@ -172,6 +172,9 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
     def param_groups(self, *args, **kwargs):
         raise NotImplementedError("training is out of scope for the H100 sampling path")
 
+    def set_train_precision(self, precision):
+        raise NotImplementedError("the image_v1 U-Net has no native training: only its forward is built")
+
     # ------------------------------------------------------------------ native front end
     def native_eval(self, x, sigma=None, aug_cond=None, class_cond=None, mapping_cond=None, precision=None, augment=False):
         """The native front end: validates one evaluation's inputs and returns its `_native.Evaluation` (the bound engine, `precision`
