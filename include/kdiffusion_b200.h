@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 20
+#define KDB_ABI_VERSION 21
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -276,44 +276,42 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
                           const float* cotangent, float* out, float* grad_x,
                           void* workspace, size_t workspace_bytes, void* stream);
 
-/* Parameter gradients (training) of an image_transformer_v2 model, fp32.  kdb_model_set_grad binds a gradient buffer [shape] fp32 on the
- * device to the state-dict key of a parameter, as kdb_model_set_tensor binds weights (data == NULL unbinds the key); binding needs no
- * finalize.  kdb_model_forward_train runs the raw model F (sigma_data 0) forward at the training precision (kdb_model_set_train_precision
- * below; at the default KDB_PREC_FP32 bit for bit as kdb_model_forward), takes the
- * cotangent u [B, C_out, H, W] on out = F(x, sigma) and OVERWRITES every bound gradient with u^T dF/dparam summed over the batch; grad_x
- * (shape of x, or NULL) receives u^T dF/dx.  Unbound parameters are skipped.  The walk is that of kdb_model_forward_vjp with the weight
- * gradients added, then the AdaRMSNorm projections and the mapping network (which is why the raw conditioning inputs are passed: sigma
- * [B], aug_cond [B, 9] or NULL, class_cond [B] int64 when num_classes > 0, mapping_cond [B, mapping_cond_dim] when mapping_cond_dim > 0).
- * cond holds one conditioning row per image (kdb_model_conditioning of those inputs; cond_batch_stride == kdb_model_cond_stride).  Bind the
- * weights first: kdb_model_set_grad returns KDB_ERR_MISSING_KEY for a key that is no tensor set on the model, KDB_ERR_BAD_SHAPE for a shape
- * other than that tensor's, and KDB_ERR_BAD_ARG for the buffers time_emb.weight, aug_emb.weight and *.pos_emb.freqs, which take no
- * gradient; kdb_model_forward_train repeats these checks for every bound key (the weights may have been rebound since) and returns the
- * same codes.  image_transformer_v1 handles return KDB_ERR_UNSUPPORTED.  The
- * workspace is kdb_model_train_workspace_bytes(m, batch, height, width) bytes (the finalized model's size; negative KDB_ERR_* on bad
- * arguments).  No atomics: every sum over tokens or images runs in an order fixed by the shapes, so two calls give the same bits.  Same
- * stream and allocation rules as kdb_model_forward. */
+/* Parameter gradients (training) of an image_transformer_v2 model.  kdb_model_set_grad binds a gradient buffer [shape] fp32 on the device to
+ * the state-dict key of a parameter, as kdb_model_set_tensor binds weights (data == NULL unbinds the key); binding needs no finalize.
+ * kdb_model_forward_train runs the raw model F (sigma_data 0) forward at the training precision `precision` (below; at KDB_PREC_FP32 bit for
+ * bit as kdb_model_forward), takes the cotangent u [B, C_out, H, W] on out = F(x, sigma) and OVERWRITES every bound gradient with u^T
+ * dF/dparam summed over the batch; grad_x (shape of x, or NULL) receives u^T dF/dx.  Unbound parameters are skipped.  The walk is that of
+ * kdb_model_forward_vjp with the weight gradients added, then the AdaRMSNorm projections and the mapping network (which is why the raw
+ * conditioning inputs are passed: sigma [B], aug_cond [B, 9] or NULL, class_cond [B] int64 when num_classes > 0, mapping_cond [B,
+ * mapping_cond_dim] when mapping_cond_dim > 0).  cond holds one conditioning row per image (kdb_model_conditioning of those inputs;
+ * cond_batch_stride == kdb_model_cond_stride).  Bind the weights first: kdb_model_set_grad returns KDB_ERR_MISSING_KEY for a key that is no
+ * tensor set on the model, KDB_ERR_BAD_SHAPE for a shape other than that tensor's, and KDB_ERR_BAD_ARG for the buffers time_emb.weight,
+ * aug_emb.weight and *.pos_emb.freqs, which take no gradient; kdb_model_forward_train repeats these checks for every bound key (the weights
+ * may have been rebound since) and returns the same codes.  The workspace is kdb_model_train_workspace_bytes(m, batch, height, width) bytes
+ * (the finalized model's size; negative KDB_ERR_* on bad arguments).  No atomics: every sum over tokens or images runs in an order fixed by
+ * the shapes, so two calls give the same bits.  Same stream and allocation rules as kdb_model_forward. */
 int     kdb_model_set_grad(KdbModel* m, const char* key, float* data, const int64_t* shape, int ndim);
 int64_t kdb_model_train_workspace_bytes(const KdbModel* m, int batch, int height, int width);
-int     kdb_model_forward_train(KdbModel* m, int batch, int height, int width,
+int     kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, int width,
                                 const float* x, const float* sigma, const float* aug_cond, const int64_t* class_cond,
                                 const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
                                 const float* cotangent, float* out, float* grad_x,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
-/* Training precision of an image_transformer_v2 handle: KDB_PREC_FP32 (the default, the exact path above) or KDB_PREC_TF32, any other value
- * KDB_ERR_UNSUPPORTED, as is any value on an image_transformer_v1 handle (and KDB_PREC_TF32 when a level's width or d_ff is not a multiple
- * of 4).  At KDB_PREC_TF32, kdb_model_finalize also builds two copies of every token-stream weight (qkv_proj, out_proj, up_proj, down_proj,
- * merges.*.proj, splits.*.proj): one rounded to the nearest tf32 (ties away from zero) and its transpose rounded alike.  kdb_model_forward_train
- * then runs each of those Linears, in the forward, in the input gradients and in the weight gradients, on the tensor cores with tf32 operands
- * (activations and output gradients truncated to tf32, weights rounded) and fp32 accumulation; patch_in, patch_out, every norm, cosine-sim +
- * RoPE, GEGLU, the attention, the mapping network and the conditioning stay exact fp32.  Still deterministic, no atomics.  The workspace of
- * kdb_model_train_workspace_bytes is the same at both precisions.  A change of precision leaves the handle not finalized (KDB_ERR_NOT_FINAL
- * until the next kdb_model_finalize).  kdb_model_forward, _jvp, _vjp and the sampler never read it.
- * kdb_model_train_forward: the forward of kdb_model_forward_train without the reverse walk, at the handle's training precision: F(x), or with
- * sigma_data > 0 the Karras-preconditioned D, bit for bit as kdb_model_forward_train's out (KDB_PREC_FP32: as kdb_model_forward at
+/* The training precision, `precision` of kdb_model_forward_train and kdb_model_train_forward: KDB_PREC_FP32 (the exact path above) or
+ * KDB_PREC_TF32.  Any other value returns KDB_ERR_UNSUPPORTED, as does any value on an image_transformer_v1 handle, and KDB_PREC_TF32 when a
+ * level's width or d_ff is not a multiple of 4; these checks come before the finalize check.  At KDB_PREC_TF32 each of the token-stream
+ * Linears (qkv_proj, out_proj, up_proj, down_proj, merges.*.proj, splits.*.proj) runs, in the forward, in the input gradients and in the weight
+ * gradients, on the tensor cores with tf32 operands (activations and output gradients truncated to tf32, weights rounded to the nearest tf32,
+ * ties away from zero) and fp32 accumulation; patch_in, patch_out, every norm, cosine-sim + RoPE, GEGLU, the attention, the mapping network and
+ * the conditioning stay exact fp32.  Still deterministic, no atomics.  The first KDB_PREC_TF32 call after a kdb_model_finalize builds two
+ * copies of every token-stream weight, one rounded and its transpose rounded alike, in memory the handle keeps until kdb_model_destroy; that
+ * call must run outside CUDA-graph capture (KDB_ERR_UNSUPPORTED otherwise).  The workspace of kdb_model_train_workspace_bytes is the same at
+ * both precisions.
+ * kdb_model_train_forward: the forward of kdb_model_forward_train without the reverse walk: F(x), or with sigma_data > 0 the
+ * Karras-preconditioned D, bit for bit as kdb_model_forward_train's out at the same precision (KDB_PREC_FP32: as kdb_model_forward at
  * KDB_PREC_FP32).  Arguments, workspace (kdb_model_workspace_bytes at KDB_PREC_FP32) and rules as for kdb_model_forward. */
-int kdb_model_set_train_precision(KdbModel* m, int precision);
-int kdb_model_train_forward(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+int kdb_model_train_forward(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
                             const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Debug/parity tap: arm a copy of one intermediate of the NEXT forward into `out` (fp32, device).

@@ -19,8 +19,8 @@
 
 namespace kdb {
 
-// The tf32 training precision's copies of a token-stream weight [N, K] (kdb_model_finalize, at KDB_PREC_TF32 only): w rounded to the
-// nearest tf32 (ties away from zero), the forward's B operand, and t = its transpose [K, N] rounded alike, the input gradient's
+// The tf32 training precision's copies of a token-stream weight [N, K] (ensure_tf32): w rounded to the nearest tf32 (ties away from
+// zero), the forward's B operand, and t = its transpose [K, N] rounded alike, the input gradient's
 struct Tf32W {
   float* w = nullptr;
   float* t = nullptr;
@@ -67,15 +67,15 @@ struct KdbModel : ModelCore {
   CondWeights cw{};
   std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
   std::unordered_map<std::string, TensorRef> grads;      // kdb_model_set_grad: gradient buffers by state-dict key (written, p is not const)
-  int train_prec = KDB_PREC_FP32;                        // kdb_model_set_train_precision
   std::vector<Tf32W> merge_t, split_t;
-  // The device buffers of the tf32 weight copies (pointer, floats), kept across finalizes instead of in `owned`: every finalize takes them
-  // in the same order (take_tf32), so the re-finalize after each optimizer step reuses them and allocates and frees nothing for them
-  std::vector<std::pair<float*, size_t>> tf32_bufs;
-  size_t tf32_next = 0;
+  // ensure_tf32's device memory, one allocation per Tf32W copy in the order of its list, kept across finalizes instead of in `owned`.
+  // Separate allocations, not one buffer: with one buffer, kdb_model_finalize's reallocation of the owned buffers took ~13 ms instead of
+  // ~5.5 ms per rebind on cfg1 (H100 80GB HBM3, 700 W), which made every tf32 training step that much slower
+  std::vector<float*> tf32_mem;
+  bool tf32_ready = false;   // the Tf32W copies are of the weights the last finalize read
 
   ~KdbModel() {
-    for (auto& b : tf32_bufs) cudaFree(b.first);
+    for (float* p : tf32_mem) cudaFree(p);
   }
 };
 
@@ -150,40 +150,6 @@ __global__ void __launch_bounds__(256) round_tf32_transpose_kernel(const float* 
       asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(t[tx][i]));
       dst[(int64_t)(k0 + i) * N + n0 + tx] = __uint_as_float(r);
     }
-}
-
-// the next tf32 copy buffer of n floats: the one the previous finalize took at this position when its size matches, else a new one
-int take_tf32(KdbModel* m, float** p, size_t n) {
-  auto& bufs = m->tf32_bufs;
-  const size_t i = m->tf32_next++;
-  if (i < bufs.size() && bufs[i].second == n) {
-    *p = bufs[i].first;
-    return 0;
-  }
-  if (i == bufs.size()) bufs.emplace_back(nullptr, 0);
-  cudaFree(bufs[i].first);
-  bufs[i] = {nullptr, 0};
-  void* q = nullptr;
-  KDB_CUDA(cudaMalloc(&q, n * sizeof(float) + 1024));
-  bufs[i] = {static_cast<float*>(q), n};
-  *p = bufs[i].first;
-  return 0;
-}
-
-// the buffers past those this finalize took (the model shrank, or the precision went back to fp32)
-void trim_tf32(KdbModel* m) {
-  for (size_t i = m->tf32_next; i < m->tf32_bufs.size(); ++i) cudaFree(m->tf32_bufs[i].first);
-  m->tf32_bufs.resize(std::min(m->tf32_next, m->tf32_bufs.size()));
-}
-
-// the tf32 copies of the weight [N, K] at src
-int make_tf32(KdbModel* m, const float* src, int N, int K, Tf32W* dst, cudaStream_t st) {
-  int rc;
-  if ((rc = take_tf32(m, &dst->w, (size_t)N * K)) || (rc = take_tf32(m, &dst->t, (size_t)N * K))) return rc;
-  if ((rc = launch_unet_round_tf32(src, dst->w, (int64_t)N * K, st))) return rc;
-  round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(K, 32), (unsigned)ceil_div(N, 32)), 256, 0, st>>>(src, dst->t, N, K);
-  KDB_LAUNCH_CHECK(F_CONVERT, st);
-  return 0;
 }
 
 // The layers in execution order, which is also the order of KdbModel::layers and of the conditioning row: down levels, mid, up levels
@@ -278,9 +244,6 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
     if ((rc = make_bf16(m, L.qkv_w, 3LL * L.C * L.C, &L.qkv_wb, st))) return rc;
     if ((rc = make_bf16(m, L.out_w, (int64_t)L.C * L.C, &L.out_wb, st))) return rc;
     if ((rc = m->alloc(&L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
-    if (m->train_prec == KDB_PREC_TF32 &&
-        ((rc = make_tf32(m, L.qkv_w, 3 * L.C, L.C, &L.qkv_t, st)) || (rc = make_tf32(m, L.out_w, L.C, L.C, &L.out_t, st))))
-      return rc;
   }
   const std::string f = prefix + "ff.";
   GET(f + "norm.linear.weight", &L.ff_norm_w, L.C, mw);
@@ -291,9 +254,6 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
   int rc;
   if ((rc = make_bf16(m, L.up_w, 2LL * L.dff * L.C, &L.up_wb, st))) return rc;
   if ((rc = make_bf16(m, L.down_w, (int64_t)L.C * L.dff, &L.down_wb, st))) return rc;
-  if (m->train_prec == KDB_PREC_TF32 &&
-      ((rc = make_tf32(m, L.up_w, 2 * L.dff, L.C, &L.up_t, st)) || (rc = make_tf32(m, L.down_w, L.C, L.dff, &L.down_t, st))))
-    return rc;
   if (L.dff % 8 == 0) {
     if ((rc = m->alloc(&L.up_wb_il, (size_t)2 * L.dff * L.C))) return rc;
     interleave_geglu_rows_kernel<<<kNumSMs * 4, 256, 0, st>>>(L.up_w, L.up_wb_il, L.dff, L.C);
@@ -363,6 +323,48 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
   KDB_CUDA(cudaStreamSynchronize(st));
   auto ins = m->pos_cache.emplace(key, std::move(pt));
   *out = &ins.first->second;
+  return 0;
+}
+
+// The tf32 training precision's weight copies, built by the first tf32 call after a finalize: the Tf32W of every layer's qkv, out, up and
+// down projection, then of every level's merge and split, in KdbModel::tf32_mem
+int ensure_tf32(KdbModel* m, cudaStream_t st) {
+  if (m->tf32_ready) return 0;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  KDB_CUDA(cudaStreamIsCapturing(st, &cs));
+  KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED,
+              "the first tf32 training call after a finalize builds the tf32 weight copies: it must run outside CUDA-graph capture");
+  struct Copy { const float* src; int N, K; Tf32W* dst; };
+  std::vector<Copy> copies;
+  for (LayerPlan& L : m->layers) {
+    if (L.attn_type != KDB_ATTN_NONE) {
+      copies.push_back({L.qkv_w, 3 * L.C, L.C, &L.qkv_t});
+      copies.push_back({L.out_w, L.C, L.C, &L.out_t});
+    }
+    copies.push_back({L.up_w, 2 * L.dff, L.C, &L.up_t});
+    copies.push_back({L.down_w, L.C, L.dff, &L.down_t});
+  }
+  const KdbModelConfig& c = m->cfg;
+  for (int l = 0; l < c.n_levels - 1; ++l) {
+    copies.push_back({m->merge_w[l], c.width[l + 1], 4 * c.width[l], &m->merge_t[l]});
+    copies.push_back({m->split_w[l], 4 * c.width[l], c.width[l + 1], &m->split_t[l]});
+  }
+  while (m->tf32_mem.size() < 2 * copies.size()) {   // once per handle: the shapes are the config's
+    const Copy& k = copies[m->tf32_mem.size() / 2];
+    void* p = nullptr;
+    KDB_CUDA(cudaMalloc(&p, sizeof(float) * k.N * k.K + 1024));
+    m->tf32_mem.push_back(static_cast<float*>(p));
+  }
+  for (size_t i = 0; i < copies.size(); ++i) {
+    copies[i].dst->w = m->tf32_mem[2 * i];
+    copies[i].dst->t = m->tf32_mem[2 * i + 1];
+  }
+  for (const Copy& k : copies) {
+    if (int rc = launch_unet_round_tf32(k.src, k.dst->w, (int64_t)k.N * k.K, st)) return rc;
+    round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(k.K, 32), (unsigned)ceil_div(k.N, 32)), 256, 0, st>>>(k.src, k.dst->t, k.N, k.K);
+    KDB_LAUNCH_CHECK(F_CONVERT, st);
+  }
+  m->tf32_ready = true;
   return 0;
 }
 
@@ -643,7 +645,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
 // tape != nullptr (fp32 only): the residual stream entering every attention / feed-forward half and out_norm is copied to the tape
 // (slots 2k, 2k+1 of layer k, slot 2 * layers for out_norm) for the reverse walk of kdb_model_forward_vjp; the launches are unchanged.
 // pos_tables != nullptr: receives the position tables of this token grid.
-// tf32 (fp32 only): the tf32 training route, every token-stream Linear through linear_tf32 on finalize's copies; TokenSplit then stores
+// tf32 (fp32 only): the tf32 training route, every token-stream Linear through linear_tf32 on ensure_tf32's copies; TokenSplit then stores
 // its projection to ws.mg and un-patches it with the lerp in launch_split_unpatch_lerp.
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
@@ -655,7 +657,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
   const int h0 = H / c.patch_h, w0 = W / c.patch_w;
   PosTables* pt = nullptr;
   int rc = ensure_pos(m, h0, w0, st, &pt);
-  if (rc) return rc;
+  if (rc || (tf32 && (rc = ensure_tf32(m, st)))) return rc;
   if (pos_tables) *pos_tables = pt;
   m->tap_count = 0;
   Fwd f{B, ws, st, cond, cond_bs, pt, kBf16 && m->fuse_norm, false, false, !kBf16 && v != nullptr};
@@ -847,9 +849,10 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Wo
   vs.total = cv.total();
 }
 
-// What kdb_model_forward_train adds to the reverse walk: the bound gradient buffers.
+// What kdb_model_forward_train adds to the reverse walk: the bound gradient buffers, and its precision.
 struct Train {
   const KdbModel* m;
+  bool tf32;   // KDB_PREC_TF32: the forward, the recomputes and every token-stream input and weight gradient take the tf32 route
   float* grad(const std::string& key) const {
     auto it = m->grads.find(key);
     return it == m->grads.end() ? nullptr : const_cast<float*>(it->second.p);
@@ -919,12 +922,11 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
 // reverse: patch_out + out_norm + combine; each up level's layers then its split-lerp; the mid layers; each down level (innermost
 // first) its merge then its layers; patch_in.
 // tr != nullptr (kdb_model_forward_train): along the walk, the gradients of patch_out, out_norm, every layer, split and merge, patch_in, and
-// the AdaRMSNorm scales into vs.dscale; grad_x may then be nullptr.  At the tf32 training precision the forward, the recomputes and every
-// token-stream input and weight gradient take the tf32 route.
+// the AdaRMSNorm scales into vs.dscale; grad_x may then be nullptr.
 int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, const float* sigma, float sd, const float* cond, int64_t cond_bs,
              float* out, float* grad_x, Workspace& ws, VjpSpace& vs, cudaStream_t st, const Train* tr = nullptr) {
   const PosTables* pt = nullptr;
-  const bool tf32 = tr != nullptr && m->train_prec == KDB_PREC_TF32;
+  const bool tf32 = tr != nullptr && tr->tf32;
   int rc = forward_impl<float>(m, B, H, W, x, nullptr, sigma, sd, cond, cond_bs, out, nullptr, ws, st, vs.tape.data(), &pt, tf32);
   if (rc) return rc;
   const KdbModelConfig& c = m->cfg;
@@ -955,8 +957,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
     const std::string sp = "splits." + std::to_string(l) + ".";
     if (tr) {   // d fac = sum (y - skip) dup with y = the split projection recomputed (vs.dbuf), skip = ws.xs[l]
-      if ((rc = tf32 ? linear_tf32(coarse, m->split_t[l].w, vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], nullptr, st)
-                     : launch_gemm_simt<float, float>(coarse, m->split_w[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{}, st)) ||
+      if ((rc = fwd_linear<float>(f, coarse, m->split_w[l], m->split_t[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{})) ||
           (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], tr->grad(sp + "fac"), B, h, w, c.width[l],
                                       part, st)))
         return rc;
@@ -1036,6 +1037,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->free_all();
   m->pos_cache.clear();
   m->finalized = false;
+  m->tf32_ready = false;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, mw = c.mapping_width;
   m->layers.clear();
@@ -1046,7 +1048,6 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->split_wb.assign(n, nullptr);
   m->merge_t.assign(n, Tf32W{});
   m->split_t.assign(n, Tf32W{});
-  m->tf32_next = 0;
   int ada = 0;
   int rc = for_each_layer(c, [&](const std::string& prefix, int level, int index) {
     m->layers.emplace_back();
@@ -1078,11 +1079,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     GET("splits." + std::to_string(l) + ".fac", &m->split_fac[l], 1);
     if ((rc = make_bf16(m, m->merge_w[l], 4LL * c.width[l] * c.width[l + 1], &m->merge_wb[l], st))) return rc;
     if ((rc = make_bf16(m, m->split_w[l], 4LL * c.width[l] * c.width[l + 1], &m->split_wb[l], st))) return rc;
-    if (m->train_prec == KDB_PREC_TF32 && ((rc = make_tf32(m, m->merge_w[l], c.width[l + 1], 4 * c.width[l], &m->merge_t[l], st)) ||
-                                           (rc = make_tf32(m, m->split_w[l], 4 * c.width[l], c.width[l + 1], &m->split_t[l], st))))
-      return rc;
   }
-  trim_tf32(m);
   const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels, Ni = c.patch_h * c.patch_w * c.in_channels;
   GET("out_norm.scale", &m->out_norm, C0);
   if (c.family == KDB_FAMILY_ITV1) {   // in_proj / out_proj (image_transformer_v1.py:295,298) in the engine's patch feature order
@@ -1289,6 +1286,22 @@ int check_grad_key(const KdbModel* m, const std::string& k, const std::vector<in
   return 0;
 }
 
+// The precision of the training calls: KDB_PREC_FP32 or KDB_PREC_TF32, on image_transformer_v2 handles.  It needs no finalize, so the
+// refusals come before the finalize check.
+int check_training_precision(const KdbModel* m, const char* what, int precision) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "%s: NULL model", what);
+  const KdbModelConfig& c = m->cfg;
+  KDB_REQUIRE(c.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED,
+              "%s: image_transformer_v1 runs on weights permuted and folded at finalize; its parameter gradients are not built", what);
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED, "%s: training runs at fp32 or tf32 (precision %d)",
+              what, precision);
+  if (precision == KDB_PREC_TF32)
+    for (int l = 0; l < c.n_levels; ++l)   // the tensor-core GEMM's TMA rows: 16-byte strides
+      KDB_REQUIRE(c.width[l] % 4 == 0 && c.d_ff[l] % 4 == 0, KDB_ERR_UNSUPPORTED,
+                  "%s: tf32 needs widths and d_ff that are multiples of 4 (level %d: %d, %d)", what, l, c.width[l], c.d_ff[l]);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1315,20 +1328,20 @@ int64_t kdb_model_train_workspace_bytes(const KdbModel* m, int batch, int height
   return (int64_t)vs.total;
 }
 
-int kdb_model_forward_train(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, const float* aug_cond,
-                            const int64_t* class_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
-                            const float* cotangent, float* out, float* grad_x, void* workspace, size_t workspace_bytes, void* stream) {
-  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "forward_train: model not finalized");
+int kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
+                            const float* aug_cond, const int64_t* class_cond, const float* mapping_cond, const float* cond,
+                            int64_t cond_batch_stride, const float* cotangent, float* out, float* grad_x, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  int rc = check_training_precision(m, "forward_train", precision);
+  if (rc) return rc;
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "forward_train: model not finalized");
   const KdbModelConfig& c = m->cfg;
-  KDB_REQUIRE(c.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED,
-              "forward_train: image_transformer_v1 runs on weights permuted and folded at finalize; its parameter gradients are not built");
   KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_train: NULL argument");
   KDB_REQUIRE(!(c.num_classes > 0 && class_cond == nullptr), KDB_ERR_BAD_ARG, "class_cond must be specified if num_classes > 0");
   KDB_REQUIRE(!(c.mapping_cond_dim > 0 && mapping_cond == nullptr), KDB_ERR_BAD_ARG, "mapping_cond must be specified if mapping_cond_dim > 0");
   KDB_REQUIRE(cond_batch_stride == kdb_model_cond_stride(m), KDB_ERR_BAD_ARG,
               "forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
               (long long)kdb_model_cond_stride(m));
-  int rc;
   for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
     if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
   if ((rc = check_image(m, "forward_train", height, width, 0.f))) return rc;
@@ -1337,7 +1350,7 @@ int kdb_model_forward_train(KdbModel* m, int batch, int height, int width, const
   carve_vjp(c, batch, height, width, workspace, ws, vs, m->ada_total, true);
   KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_train: workspace %zu < required %zu", workspace_bytes, vs.total);
   cudaStream_t st = (cudaStream_t)stream;
-  const Train tr{m};
+  const Train tr{m, precision == KDB_PREC_TF32};
   if ((rc = m->disarm_tap(vjp_impl(m, batch, height, width, x, cotangent, sigma, 0.f, cond, cond_batch_stride, out, grad_x, ws, vs, st, &tr))))
     return rc;
   // AdaRMSNorm: scale = 1 + cond W^T per image, so d W = sum_b dscale_b cond_b (cond: the last mw floats of the conditioning row) and the
@@ -1381,32 +1394,17 @@ int kdb_model_forward_train(KdbModel* m, int batch, int height, int width, const
   return 0;
 }
 
-int kdb_model_set_train_precision(KdbModel* m, int precision) {
-  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "set_train_precision: NULL model");
-  const KdbModelConfig& c = m->cfg;
-  KDB_REQUIRE(c.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED, "set_train_precision: parameter gradients are built for image_transformer_v2 only");
-  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED,
-              "set_train_precision: training runs at fp32 or tf32 (precision %d)", precision);
-  if (precision == KDB_PREC_TF32)
-    for (int l = 0; l < c.n_levels; ++l)   // the tensor-core GEMM's TMA rows: 16-byte strides
-      KDB_REQUIRE(c.width[l] % 4 == 0 && c.d_ff[l] % 4 == 0, KDB_ERR_UNSUPPORTED,
-                  "set_train_precision: tf32 needs widths and d_ff that are multiples of 4 (level %d: %d, %d)", l, c.width[l], c.d_ff[l]);
-  if (precision != m->train_prec) m->finalized = false;   // the tf32 weight copies are finalize's
-  m->train_prec = precision;
-  return 0;
-}
-
-int kdb_model_train_forward(KdbModel* m, int batch, int height, int width, const float* x, const float* sigma, float sigma_data, const float* cond,
-                            int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
-  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "train_forward: model not finalized");
-  KDB_REQUIRE(m->cfg.family == KDB_FAMILY_ITV2, KDB_ERR_UNSUPPORTED, "train_forward: parameter gradients are built for image_transformer_v2 only");
-  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "train_forward: NULL argument");
-  int rc = check_image(m, "train_forward", height, width, sigma_data);
+int kdb_model_train_forward(KdbModel* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                            const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_training_precision(m, "train_forward", precision);
   if (rc) return rc;
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "train_forward: model not finalized");
+  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "train_forward: NULL argument");
+  if ((rc = check_image(m, "train_forward", height, width, sigma_data))) return rc;
   Workspace ws;
   if ((rc = carve_checked(m, "train_forward", KDB_PREC_FP32, batch, height, width, workspace, workspace_bytes, ws))) return rc;
   return m->disarm_tap(forward_impl<float>(m, batch, height, width, x, nullptr, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, ws,
-                                           (cudaStream_t)stream, nullptr, nullptr, m->train_prec == KDB_PREC_TF32));
+                                           (cudaStream_t)stream, nullptr, nullptr, precision == KDB_PREC_TF32));
 }
 
 int kdb_wgrad_tf32(const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc, int merge_wc,

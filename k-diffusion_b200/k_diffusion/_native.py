@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 20
+ABI_VERSION = 21
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -79,9 +79,8 @@ SIGNATURES = {
     "kdb_model_forward_vjp": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "kdb_model_set_grad": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
     "kdb_model_train_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
-    "kdb_model_forward_train": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "kdb_model_set_train_precision": (_i32, [_vp, _i32]),
-    "kdb_model_train_forward": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
+    "kdb_model_forward_train": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_model_train_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_loss_noised_input": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
     "kdb_denoiser_loss": (_i32, [_i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i32, _i64, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
@@ -685,9 +684,10 @@ class Engine:
                                               ptr(u), ptr(out), ptr(out_grad), ptr(ws), ws.numel(), stream()))
         return out, out_grad
 
-    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None):
-        """Parameter gradients on the fp32 path: binds `grads` ({state-dict key: fp32 CUDA tensor of the parameter's shape}, every other
-        key unbound), then one kdb_model_forward_train: out = F(x) at fp32, every bound gradient = u^T dF/dparam, grad_x (if given) u^T dF/dx."""
+    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32):
+        """Parameter gradients at the training precision (PREC_FP32 or PREC_TF32): binds `grads` ({state-dict key: fp32 CUDA tensor of the
+        parameter's shape}, every other key unbound), then one kdb_model_forward_train: out = F(x), every bound gradient = u^T dF/dparam,
+        grad_x (if given) u^T dF/dx."""
         B, _, H, W = x.shape
         shape = (B, self.cfg.out_channels, H, W)
         if tuple(u.shape) != shape:
@@ -701,26 +701,20 @@ class Engine:
         self._grad_keys = set(grads)
         ws = self._reserve(lib().kdb_model_train_workspace_bytes(self._h, B, H, W), x.device)
         with device_of(x):
-            check(lib().kdb_model_forward_train(self._h, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(class_cond), ptr(mapping_cond),
-                                                ptr(cond), self._stride, ptr(u), ptr(out), ptr(grad_x), ptr(ws), ws.numel(), stream()))
+            check(lib().kdb_model_forward_train(self._h, precision, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(class_cond),
+                                                ptr(mapping_cond), ptr(cond), self._stride, ptr(u), ptr(out), ptr(grad_x), ptr(ws), ws.numel(),
+                                                stream()))
         return out
 
-    def set_train_precision(self, precision):
-        """kdb_model_set_train_precision (PREC_FP32 or PREC_TF32); a change re-finalizes at the next bind, which builds or drops the tf32
-        weight copies."""
-        if precision != getattr(self, "_train_prec", PREC_FP32):
-            check(lib().kdb_model_set_train_precision(self._h, precision))
-            self._train_prec, self._sig = precision, None
-
-    def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, out=None):
-        """kdb_model_train_forward: the forward of forward_train at the training precision (x [B,C,H,W] fp32), bit for bit its `out`."""
+    def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
+        """kdb_model_train_forward: the forward of forward_train at `precision` (x [B,C,H,W] fp32), bit for bit its `out`."""
         B, _, H, W = x.shape
         if out is None:
             out = torch.empty(B, self.cfg.out_channels, H, W, device=x.device, dtype=torch.float32)
         ws = self._workspace(PREC_FP32, B, H, W, x.device)
         with device_of(x):
-            check(lib().kdb_model_train_forward(self._h, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride, ptr(out),
-                                                ptr(ws), ws.numel(), stream()))
+            check(lib().kdb_model_train_forward(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
+                                                ptr(out), ptr(ws), ws.numel(), stream()))
         return out
 
     def arm_tap(self, name, capacity, device):

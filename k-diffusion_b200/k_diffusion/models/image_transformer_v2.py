@@ -190,7 +190,6 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         eng = self._engines.get(None)
         if eng is None:
             eng = self._engines[None] = _native.Engine(self.engine_spec())
-        eng.set_train_precision(getattr(self, "train_precision", _native.PREC_FP32))
         eng.bind(dict(self.state_dict(keep_vars=True)))
         return eng
 
@@ -236,7 +235,8 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         """Per-sample training losses [B] of the Karras-preconditioned denoiser around this model (`_native.LOSS_DENOISER`: reference
         layers.py:76-86 with scales == 1 and per-sample `weight`; `LOSS_SIMPLE`: :107-111), with a grad_fn that reaches every parameter
         requiring grad.  The forward is one engine evaluation and one loss kernel; the backward is one kdb_model_forward_train.  The
-        arithmetic is `set_train_precision`'s (fp32 unless set), whatever `set_precision` selected."""
+        arithmetic is `set_train_precision`'s when the loss is computed (fp32 unless set), for its backward too, whatever `set_precision`
+        selected."""
         if self.family != _native.FAMILY_ITV2:
             raise NotImplementedError(f"{self.kind}: parameter gradients are built for image_transformer_v2 models only")
         for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
@@ -393,7 +393,8 @@ def _autograd_eval(model, ev, x, sigma, sigma_data, aug_cond, mapping_cond, out)
 class _NativeLoss(torch.autograd.Function):
     """A training loss through the native engine with respect to the model's parameters (passed after `keys`, their state-dict names).
     The forward saves the per-element cotangent d loss[b] / d F of the loss kernel; the backward scales it by the incoming gradient of
-    each sample's loss and makes one kdb_model_forward_train, which writes every parameter's gradient."""
+    each sample's loss and makes one kdb_model_forward_train, which writes every parameter's gradient.  Both run at the model's training
+    precision as the forward found it."""
 
     @staticmethod
     def forward(ctx, model, ev, kind, noise, sigma_data, weight, keys, *params):
@@ -401,13 +402,11 @@ class _NativeLoss(torch.autograd.Function):
         w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
         xin = _native.loss_noised_input(x, noise, sig, sigma_data)
         cond = ev.conditioning()
-        if getattr(model, "train_precision", _native.PREC_FP32) == _native.PREC_TF32:   # the forward of the tf32 training walk
-            f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0)
-        else:
-            f = ev.engine.forward(xin, sig, cond, ev.engine.cond_stride, 0.0, ev.precision)
+        precision = getattr(model, "train_precision", _native.PREC_FP32)
+        f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
         loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
         aug, cls, mc = ev.cond
-        ctx.model, ctx.keys = model, keys
+        ctx.model, ctx.keys, ctx.precision = model, keys, precision
         ctx.save_for_backward(xin, sig, cond, cot, None if aug is None else _native.f32c(aug),
                               None if cls is None else cls.to(torch.int64).contiguous(), None if mc is None else _native.f32c(mc))
         return loss
@@ -419,5 +418,5 @@ class _NativeLoss(torch.autograd.Function):
         params = dict(ctx.model.named_parameters())
         u = cot * _native.f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
         grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
-        ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads)
+        ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads, precision=ctx.precision)
         return (None,) * 7 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)

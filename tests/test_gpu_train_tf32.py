@@ -95,23 +95,53 @@ def test_three_levels_with_augment_wrapper_tf32():
     check_against_restatement(cfg, sd, loss, got, x, noise, sigma, kw, gw)
 
 
-def test_loss_is_the_forward_of_the_training_walk():
-    """At tf32 the loss's F (kdb_model_train_forward) is bit for bit the out of kdb_model_forward_train, and not the fp32 forward"""
+def _walk_inputs(cfg, inner, seed):
+    """cuda inputs of one engine call on LEVELS3 through the augment wrapper: x, sigma, the conditioning rows and mapping_cond"""
+    x, noise, sigma, kw, gw = (t.cuda() if isinstance(t, torch.Tensor) else t for t in inputs(cfg, 2, seed))
+    mc = torch.cat([kw["aug_cond"].cuda(), kw["mapping_cond"].cuda()], 1)
+    return x, sigma, inner.engine().conditioning(sigma, None, None, mc), mc
+
+
+def test_train_forward_is_the_forward_of_the_training_walk():
+    """The loss's F (kdb_model_train_forward) is bit for bit the out of kdb_model_forward_train at the same precision: at tf32 not the fp32
+    forward, at fp32 the fp32 forward"""
     cfg, inner, sd, model = build(LEVELS3, wrap=True)
-    inner.set_train_precision("tf32")
-    x, noise, sigma, kw, gw = (t.cuda() if isinstance(t, torch.Tensor) else t for t in inputs(cfg, 2, 6))
-    kw = {k: v.cuda() for k, v in kw.items()}
+    x, sigma, cond, mc = _walk_inputs(cfg, inner, 6)
     eng = inner.engine()
-    mc = torch.cat([kw["aug_cond"], kw["mapping_cond"]], 1)
-    cond = eng.conditioning(sigma, None, None, mc)
-    f = eng.train_forward(x, sigma, cond, eng.cond_stride, 0.0)
-    out = eng.forward_train(x, torch.ones_like(x), sigma, None, None, mc, cond, {})
+    f = eng.train_forward(x, sigma, cond, eng.cond_stride, 0.0, _native.PREC_TF32)
+    out = eng.forward_train(x, torch.ones_like(x), sigma, None, None, mc, cond, {}, precision=_native.PREC_TF32)
     assert torch.equal(f, out)
     f32 = eng.forward(x, sigma, cond, eng.cond_stride, 0.0, _native.PREC_FP32)
     assert not torch.equal(f, f32) and (f - f32).norm() < 1e-2 * f32.norm()
+    assert torch.equal(eng.train_forward(x, sigma, cond, eng.cond_stride, 0.0, _native.PREC_FP32), f32)
     # the sampling forward ignores the training precision
-    inner.set_train_precision("fp32")
+    inner.set_train_precision("tf32")
     assert torch.equal(inner.engine().forward(x, sigma, cond, eng.cond_stride, 0.0, _native.PREC_FP32), f32)
+
+
+def test_alternating_precisions_on_one_engine():
+    """fp32 and tf32 training walks in turn on one engine, with no rebind between them: each bit for bit that of a fresh engine at its
+    precision (the first tf32 call after the finalize builds the tf32 copies, the fp32 calls leave them alone)"""
+    cfg, inner, sd, model = build(LEVELS3, wrap=True)
+    x, sigma, cond, mc = _walk_inputs(cfg, inner, 11)
+    u = torch.randn(x.shape, generator=torch.Generator().manual_seed(12)).cuda()
+    params = {k: p for k, p in inner.named_parameters() if p.requires_grad}
+
+    def walk(eng, precision):
+        grads = {k: torch.empty(p.shape, device="cuda") for k, p in params.items()}
+        return eng.forward_train(x, u, sigma, None, None, mc, cond, grads, precision=precision), grads
+
+    eng = inner.engine()
+    order = [_native.PREC_FP32, _native.PREC_TF32, _native.PREC_FP32, _native.PREC_TF32, _native.PREC_TF32, _native.PREC_FP32]
+    got = [walk(eng, p) for p in order]
+    want = {}
+    for p in (_native.PREC_FP32, _native.PREC_TF32):
+        fresh = _native.Engine(inner.engine_spec())
+        fresh.bind(dict(inner.state_dict(keep_vars=True)))
+        want[p] = walk(fresh, p)
+    assert not torch.equal(want[_native.PREC_FP32][0], want[_native.PREC_TF32][0])
+    for p, (out, grads) in zip(order, got):
+        assert torch.equal(out, want[p][0]) and all(torch.equal(g, want[p][1][k]) for k, g in grads.items()), p
 
 
 def test_two_calls_bit_identical_and_batch_is_sum_of_images_tf32():
@@ -165,6 +195,23 @@ def test_switching_back_to_fp32_gives_the_fp32_bits():
     assert torch.equal(l0, l1) and torch.equal(l0, l2)
     assert all(torch.equal(g0[k], g1[k]) and torch.equal(g0[k], g2[k]) for k in g0)
     assert not torch.equal(l0, lt) and any(not torch.equal(g0[k], gt[k]) for k in g0)
+
+
+def test_tf32_copies_follow_the_weights_after_an_update():
+    """An optimizer step updates the weights in place; the next loss re-finalizes the engine, and its tf32 copies are those of the updated
+    weights: the gradients equal, bit for bit, those of a fresh model built at the updated weights"""
+    cfg, inner, sd, model = build(CLASS)
+    inner.set_train_precision("tf32")
+    x, noise, sigma, kw, gw = inputs(cfg, 2, 9)
+    l0, _ = native_grads(model, inner, x, noise, sigma, kw, gw)
+    torch.optim.AdamW(inner.param_groups(1e-2), betas=(0.9, 0.95), eps=1e-6, weight_decay=1e-3).step()
+    l1, g1 = native_grads(model, inner, x, noise, sigma, kw, gw)
+    _, fresh, _, fresh_model = build(CLASS)
+    fresh.load_state_dict(inner.state_dict())
+    fresh.set_train_precision("tf32")
+    l2, g2 = native_grads(fresh_model, fresh, x, noise, sigma, kw, gw)
+    assert not torch.equal(l0, l1)
+    assert torch.equal(l1, l2) and all(torch.equal(g1[k], g2[k]) for k in g1)
 
 
 def test_cfg1_tf32_gradients():

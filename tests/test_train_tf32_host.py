@@ -134,24 +134,32 @@ def test_v1_and_unet_have_no_training_precision():
                 m.set_train_precision(p)
 
 
-def test_engine_entry_points_without_gpu():
-    """kdb_model_set_train_precision's refusals need no GPU: a bad value, the v1 family, widths the tensor-core GEMM cannot stream"""
+def test_training_calls_refuse_precisions_without_gpu():
+    """The training calls' refusals of a precision need no GPU and no finalize: a bad value, the v1 family, widths the tensor-core GEMM
+    cannot stream; a precision they accept meets the finalize check"""
     L = _native.lib()
+
+    def calls(h, precision):   # kdb_model_forward_train, then kdb_model_train_forward, with every other argument NULL or zero
+        yield L.kdb_model_forward_train(h, precision, 1, 16, 16, None, None, None, None, None, None, 0, None, None, None, None, 0, None)
+        yield L.kdb_model_train_forward(h, precision, 1, 16, 16, None, None, 0.0, None, 0, None, None, 0, None)
+
     _, inner, _ = model_of(CLASS)
     eng = _native.Engine(inner.engine_spec())
-    assert L.kdb_model_set_train_precision(eng._h, _native.PREC_TF32) == 0
-    assert L.kdb_model_set_train_precision(eng._h, _native.PREC_FP32) == 0
+    for good in (_native.PREC_TF32, _native.PREC_FP32):
+        assert tuple(calls(eng._h, good)) == (-6, -6)   # KDB_ERR_NOT_FINAL
     for bad in (_native.PREC_BF16, _native.PREC_FP16, 7):
-        assert L.kdb_model_set_train_precision(eng._h, bad) == -2   # KDB_ERR_UNSUPPORTED
+        assert tuple(calls(eng._h, bad)) == (-2, -2)   # KDB_ERR_UNSUPPORTED
     odd = inner.engine_spec()
     odd["levels"][0]["d_ff"] = 66
-    assert L.kdb_model_set_train_precision(_native.Engine(odd)._h, _native.PREC_TF32) == -2
-    assert b"multiples of 4" in L.kdb_last_error()
+    odd_eng = _native.Engine(odd)
+    for rc in calls(odd_eng._h, _native.PREC_TF32):
+        assert rc == -2 and b"multiples of 4" in L.kdb_last_error()
+    assert tuple(calls(odd_eng._h, _native.PREC_FP32)) == (-6, -6)
     v1 = K.config.make_model(K.config.load_config({"model": {"type": "image_transformer_v1", "input_channels": 1, "input_size": [8, 8],
                                                              "patch_size": [2, 2], "depth": 1, "width": 64, "d_ff": 128}}))
     v1eng = _native.Engine(v1.engine_spec())
-    assert L.kdb_model_set_train_precision(v1eng._h, _native.PREC_FP32) == -2
-    assert L.kdb_model_train_forward(eng._h, 1, 16, 16, None, None, 0.0, None, 0, None, None, 0, None) == -6   # KDB_ERR_NOT_FINAL
+    for p in (_native.PREC_FP32, _native.PREC_TF32):
+        assert tuple(calls(v1eng._h, p)) == (-2, -2)
 
 
 class _StubEngine:
@@ -168,12 +176,12 @@ class _StubEngine:
         self.log.append(("forward", precision))
         return torch.zeros_like(x)
 
-    def train_forward(self, x, sigma, cond, stride, sigma_data, out=None):
-        self.log.append(("train_forward", sigma_data))
+    def train_forward(self, x, sigma, cond, stride, sigma_data, precision, out=None):
+        self.log.append(("train_forward", sigma_data, precision))
         return torch.zeros_like(x)
 
-    def forward_train(self, x, u, sigma, aug, cls, mc, cond, grads, out=None, grad_x=None):
-        self.log.append("forward_train")
+    def forward_train(self, x, u, sigma, aug, cls, mc, cond, grads, out=None, grad_x=None, precision=_native.PREC_FP32):
+        self.log.append(("forward_train", precision))
         for g in grads.values():
             g.zero_()
         return torch.zeros_like(x)
@@ -183,7 +191,8 @@ class _StubEngine:
 
 
 @pytest.mark.parametrize("precision", ["fp32", "tf32"])
-def test_loss_calls_train_forward_only_at_tf32(monkeypatch, precision):
+def test_loss_runs_at_the_training_precision(monkeypatch, precision):
+    """The loss calls train_forward, then its backward forward_train, both at the model's training precision when the loss was computed"""
     monkeypatch.setattr(_native, "require_cuda", lambda *t: None)
     monkeypatch.setattr(torch.cuda, "is_current_stream_capturing", lambda: False)
     monkeypatch.setattr(_native, "loss_noised_input", lambda x, noise, sigma, sd: x + noise * sigma.view(-1, 1, 1, 1))
@@ -196,10 +205,11 @@ def test_loss_calls_train_forward_only_at_tf32(monkeypatch, precision):
     model = K.config.make_denoiser_wrapper(cfg)(inner)
     x = torch.randn(2, 1, 16, 16)
     loss = model.loss(x, torch.randn_like(x), torch.tensor([0.5, 2.0]), class_cond=torch.tensor([1, 2]))
+    inner.set_train_precision("fp32" if precision == "tf32" else "tf32")   # the backward keeps the forward's precision
     loss.sum().backward()
     calls = [c for c in log if c != "conditioning"]
-    want = ("train_forward", 0.0) if precision == "tf32" else ("forward", _native.PREC_FP32)
-    assert calls == [want, "forward_train"]
+    code = _native.PREC_TF32 if precision == "tf32" else _native.PREC_FP32
+    assert calls == [("train_forward", 0.0, code), ("forward_train", code)]
 
 
 def _inputs(B=2, seed=0):
