@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 21
+#define KDB_ABI_VERSION 22
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -507,6 +507,30 @@ int kdb_polynomial_kernel(const float* x, const float* y, float* out, int batch,
  * samples in order, each element written to (i, j) and (j, i), so cov is exactly symmetric (n = 1 gives nan, as torch.cov).
  * 1 <= n <= INT32_MAX.  Two launches, no workspace. */
 int kdb_feature_mean_cov(const float* x, int64_t n, int d, float* mean, float* cov, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Training loop: the EMA model update after each optimizer step (utils.py:88-104 ema_update)
+ * ------------------------------------------------------------------------------------------ */
+
+/* One segment of kdb_ema_update: n fp32 elements at src and dst (device, 4-byte aligned, not overlapping).
+ * KDB_EMA_LERP (a parameter): dst = torch.lerp(dst, src, weight); KDB_EMA_COPY (a buffer): dst = src. */
+#define KDB_EMA_LERP 0
+#define KDB_EMA_COPY 1
+typedef struct KdbEmaSeg {
+  const float* src;
+  float* dst;
+  int64_t n;
+  int32_t mode;
+} KdbEmaSeg;
+
+/* Every segment of the host table segs_host[0 .. n_segs) in one launch, weight = 1 - decay.  The lerp is torch's CUDA lerp_ with a scalar
+ * weight, |w| < 0.5 ? dst + w (src - dst) : src - (src - dst) (1 - w) in fp32, each branch one fused multiply-add: bit for bit lerp_ on the
+ * same GPU.  A segment of n = 0 is skipped; NULL src or dst with n > 0, a mode other than KDB_EMA_LERP / KDB_EMA_COPY or a pointer that
+ * is not 4-byte aligned return KDB_ERR_BAD_ARG before any CUDA call.  Grid-stride over all segments' elements, 128-bit loads and stores
+ * where src and dst are co-aligned (scalar head and tail), scalar otherwise; every element written once, no atomics.  The table is staged
+ * in a pinned host buffer the library reuses and copied to the device on `stream`, so the call is not capturable: under CUDA-graph capture
+ * it returns KDB_ERR_UNSUPPORTED.  The library's first call on a device, and a call with more segments than any before, allocates. */
+int kdb_ema_update(const KdbEmaSeg* segs_host, int n_segs, float weight, void* stream);
 
 #ifdef __cplusplus
 }

@@ -19,7 +19,7 @@ enum Family {
   F_QKNORM_ROPE, F_ATTN_GENERIC, F_ATTN_TC, F_GEGLU, F_MERGE_GATHER, F_CONVERT, F_FUSED_NORM,
   F_UNET_CONV, F_UNET_ADAGN, F_UNET_RESAMPLE, F_UNET_PATCH, F_UNET_COND, F_UNET_CONV_TF32, F_UNET_ATTN_TF32,
   F_UNET_CONV_FP16, F_UNET_ATTN_FP16, F_MMD_TILES, F_MMD_REDUCE, F_POLY_KERNEL, F_COL_MEAN, F_COV,
-  F_GEMM_TF32, F_WGRAD_TF32, F_COUNT
+  F_GEMM_TF32, F_WGRAD_TF32, F_EMA, F_COUNT
 };
 void count_launch(int family, cudaStream_t st);
 

@@ -28,7 +28,7 @@ static const char* kFamilyNames[F_COUNT] = {
     "qknorm_rope", "attn_generic", "attn_tc", "geglu", "merge_gather", "convert", "fused_norm",
     "unet_conv", "unet_adagn", "unet_resample", "unet_patch", "unet_cond", "unet_conv_tf32", "unet_attn_tf32",
     "unet_conv_fp16", "unet_attn_fp16", "mmd_tiles", "mmd_reduce", "poly_kernel", "col_mean", "cov",
-    "gemm_tf32", "wgrad_tf32"};
+    "gemm_tf32", "wgrad_tf32", "ema"};
 
 void set_error(const char* fmt, ...) {
   va_list ap;

@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 21
+ABI_VERSION = 22
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -41,6 +41,13 @@ class KdbUNetConfig(ctypes.Structure):
         ("augment_wrapper", _i32), ("skip_stages", _i32), ("has_variance", _i32),
         ("depth", _i32 * MAX_LEVELS), ("channels", _i32 * MAX_LEVELS), ("self_attn", _i32 * MAX_LEVELS),
     ]
+
+
+EMA_LERP, EMA_COPY = 0, 1
+
+
+class KdbEmaSeg(ctypes.Structure):
+    _fields_ = [("src", _vp), ("dst", _vp), ("n", _i64), ("mode", _i32)]
 
 
 # name -> (restype, argtypes); this table is also what tests/test_abi.py checks against the header.
@@ -110,6 +117,7 @@ SIGNATURES = {
     "kdb_mmd_sums": (_i32, [_vp, _i64, _vp, _i64, _i32, ctypes.POINTER(_i64), ctypes.POINTER(_i64), _i32, _vp, _vp, _sz, _vp]),
     "kdb_polynomial_kernel": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "kdb_feature_mean_cov": (_i32, [_vp, _i64, _i32, _vp, _vp, _vp]),
+    "kdb_ema_update": (_i32, [ctypes.POINTER(KdbEmaSeg), _i32, _f32, _vp]),
 }
 
 _lib = None
@@ -1026,3 +1034,18 @@ def feature_mean_cov(x):
     cov = torch.empty(d, d, dtype=torch.float32, device=x.device)
     check(lib().kdb_feature_mean_cov(ptr(x), n, d, ptr(mean), ptr(cov), stream()))
     return mean, cov
+
+
+# ---------------------------------------------------------------------------------------------
+# training loop
+# ---------------------------------------------------------------------------------------------
+
+@_on_device_of_first
+def ema_update(dsts, srcs, modes, weight):
+    """kdb_ema_update: dst <- torch.lerp(dst, src, weight) (EMA_LERP) or dst <- src (EMA_COPY) for every (dst, src, mode), contiguous fp32
+    tensors of equal size on one CUDA device, in one launch on the current stream."""
+    require_cuda(*dsts, *srcs)
+    table = (KdbEmaSeg * max(len(dsts), 1))()
+    for i, (d, s, m) in enumerate(zip(dsts, srcs, modes)):
+        table[i].src, table[i].dst, table[i].n, table[i].mode = s.data_ptr(), d.data_ptr(), d.numel(), m
+    check(lib().kdb_ema_update(table, len(dsts), weight, stream()))

@@ -1,5 +1,6 @@
 """Config loading / model factory for the path in scope (reference: k_diffusion/config.py:23-231).
 
+make_sample_density (config.py:234-268) builds the sigma sample density of train.py's step.
 Accepts the reference's JSON files, dicts, and `.safetensors` checkpoints carrying the config in
 their metadata.  `image_transformer_v2`, `image_transformer_v1` and `image_v1` can be built.
 """
@@ -8,7 +9,7 @@ import math
 from functools import partial
 from pathlib import Path
 
-from . import augmentation, layers, models
+from . import augmentation, layers, models, utils
 
 _V2_MODEL_DEFAULTS = dict(mapping_width=256, mapping_depth=2, mapping_d_ff=None, mapping_cond_dim=0, mapping_dropout_rate=0.,
                           d_ffs=None, self_attns=None, dropout_rate=None, augment_wrapper=False, skip_stages=0, has_variance=False)
@@ -154,3 +155,40 @@ def make_denoiser_wrapper(config):
             raise ValueError('Simple loss config does not support a variance output')
         return partial(layers.SimpleLossDenoiser, sigma_data=sigma_data)
     raise ValueError('Unknown loss config type')
+
+
+def _first(d, *keys):
+    """d[key] of the first of `keys` present; a KeyError naming the last when none is (the reference's 'mean' if 'mean' in d else d['loc'])."""
+    for k in keys[:-1]:
+        if k in d:
+            return d[k]
+    return d[keys[-1]]
+
+
+def make_sample_density(config):
+    """The sigma sample density of a model config (config['model'] of a loaded config; config.py:234-268): a function of (shape, device=,
+    dtype=) drawing training sigmas, one of utils.rand_* with the config's parameters bound.  `sigma_sample_density.type`: lognormal
+    (mean | loc, std | scale), loglogistic (loc = log sigma_data, scale = 0.5, min_value = 0, max_value = inf), loguniform (min_value |
+    sigma_min, max_value | sigma_max), v-diffusion or cosine (min_value = 1e-3, max_value = 1e3), split-lognormal (mean | loc, std_1 | scale_1,
+    std_2 | scale_2) or cosine-interpolated (min_value = min(sigma_min, 1e-3), max_value = max(sigma_max, 1e3), image_d = max(input_size),
+    noise_d_low = 32, noise_d_high = max(input_size)); any other type raises ValueError."""
+    sd = config['sigma_sample_density']
+    sigma_data = config['sigma_data']
+    kind = sd['type']
+    if kind == 'lognormal':
+        return partial(utils.rand_log_normal, loc=_first(sd, 'mean', 'loc'), scale=_first(sd, 'std', 'scale'))
+    if kind == 'loglogistic':
+        return partial(utils.rand_log_logistic, loc=sd['loc'] if 'loc' in sd else math.log(sigma_data), scale=sd.get('scale', 0.5), min_value=sd.get('min_value', 0.), max_value=sd.get('max_value', float('inf')))
+    if kind == 'loguniform':
+        return partial(utils.rand_log_uniform, min_value=sd['min_value'] if 'min_value' in sd else config['sigma_min'], max_value=sd['max_value'] if 'max_value' in sd else config['sigma_max'])
+    if kind in {'v-diffusion', 'cosine'}:
+        return partial(utils.rand_v_diffusion, sigma_data=sigma_data, min_value=sd.get('min_value', 1e-3), max_value=sd.get('max_value', 1e3))
+    if kind == 'split-lognormal':
+        return partial(utils.rand_split_log_normal, loc=_first(sd, 'mean', 'loc'), scale_1=_first(sd, 'std_1', 'scale_1'),
+                       scale_2=_first(sd, 'std_2', 'scale_2'))
+    if kind == 'cosine-interpolated':
+        size = max(config['input_size'])
+        return partial(utils.rand_cosine_interpolated, image_d=sd.get('image_d', size), noise_d_low=sd.get('noise_d_low', 32),
+                       noise_d_high=sd.get('noise_d_high', size), sigma_data=sigma_data,
+                       min_value=sd.get('min_value', min(config['sigma_min'], 1e-3)), max_value=sd.get('max_value', max(config['sigma_max'], 1e3)))
+    raise ValueError('Unknown sample density type')

@@ -1,4 +1,4 @@
-"""Backend switches (the reference's env flags live in models/flags.py:9-14).
+"""Backend switches (the reference's env flags live in models/flags.py:9-14) and the reference's activation checkpointing flag (:17-31).
 
 K_DIFFUSION_USE_COMPILE / K_DIFFUSION_USE_FLASH_2 are accepted and ignored: there is no
 torch.compile or flash-attn path here.  The only switch is the arithmetic of the token stream:
@@ -14,6 +14,8 @@ U-Net only, never chosen by auto, not even for fp16 parameters or under autocast
 the 10 explicit significand bits of tf32, a narrower exponent range, twice the tensor-core rate.
 """
 import os
+import threading
+from contextlib import contextmanager
 
 import torch
 
@@ -24,6 +26,27 @@ def get_use_compile():
 
 def get_use_flash_attention_2():
     return False
+
+
+state = threading.local()
+state.checkpointing = False
+
+
+@contextmanager
+def checkpointing(enable=True):
+    """Within the block, get_checkpointing() returns `enable` on this thread (models/flags.py:17-31), which the reference's models read to
+    recompute activations in their backward (torch.utils.checkpoint) instead of keeping them.  The native models ignore it: their backward
+    already keeps only the residual stream entering each attention and feed-forward half on a tape and recomputes every activation from it
+    (DESIGN section 3), so there is nothing more to drop."""
+    try:
+        old, state.checkpointing = get_checkpointing(), enable
+        yield
+    finally:
+        state.checkpointing = old
+
+
+def get_checkpointing():
+    return getattr(state, "checkpointing", False)
 
 
 def resolve_precision(requested, param_dtype):
