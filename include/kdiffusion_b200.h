@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 22
+#define KDB_ABI_VERSION 23
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -392,13 +392,40 @@ int64_t kdb_unet_tap_count(const KdbUNet* m);
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)
  * ------------------------------------------------------------------------------------------ */
 
-/* The weight gradient of the tf32 training precision: dw[n, k] = sum over rows r < m of dy[r, n] x[r, k], dy and x truncated to tf32 (the
- * low 13 mantissa bits cleared), products accumulated in fp32 on the tensor cores (mma.sync).  dy rows ldy floats apart (>= n) in both modes,
- * x rows ldx (>= k); with merge_hc, merge_wc > 0, x is instead read in place as the TokenMerge 2x2 gather of contiguous fine tokens
- * [m / (merge_hc merge_wc), 2 merge_hc, 2 merge_wc, k / 4] (ldx unused; m a multiple of merge_hc merge_wc, k of 4).  The rows are split into chunks fixed by (m, n, k) alone, each chunk's partial written to
- * scratch (2^22 floats) and the partials summed in chunk order: no atomics, two calls give the same bits.  Every element of dw is written. */
-int kdb_wgrad_tf32(const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc, int merge_wc,
-                   float* scratch, void* stream);
+/* The parameter-gradient reductions of kdb_model_forward_train (the launches it makes).  No atomics: every sum is split into chunks fixed
+ * by the shapes alone, each chunk summed in row order into scratch (caller scratch of 2^22 floats) and the partials summed in chunk order,
+ * so two calls on the same inputs give the same bits.  Every element of the output is written.  Arguments are checked before any launch.
+ *
+ * kdb_wgrad: the weight gradient of a Linear, dw[n, k] = sum over rows r < m of dy[r, n] x[r, k].  KDB_PREC_FP32: fp32 fmaf products and
+ * sums; KDB_PREC_TF32: dy and x truncated to tf32 (the low 13 mantissa bits cleared), products accumulated in fp32 on the tensor cores
+ * (mma.sync); other precisions KDB_ERR_UNSUPPORTED.  dy rows ldy floats apart (>= n) in both modes, x rows ldx (>= k); with merge_hc,
+ * merge_wc > 0, x is instead read in place as the TokenMerge 2x2 gather of contiguous fine tokens [m / (merge_hc merge_wc), 2 merge_hc,
+ * 2 merge_wc, k / 4] (ldx unused; m a multiple of merge_hc merge_wc, k of 4). */
+int kdb_wgrad(int precision, const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc,
+              int merge_wc, float* scratch, void* stream);
+/* patch_in's weight gradient, fp32: dw [n, patch_h patch_w channels] = sum over the tokens t of dtok[t, n] (contiguous, [batch T, n]) times
+ * the patch row of t in the NCHW image x [batch, channels, height, width], read in place, columns in the order (ph pw c). */
+int kdb_wgrad_patch_in(const float* dtok, const float* x, float* dw, int batch, int channels, int height, int width, int patch_h, int patch_w,
+                       int n, float* scratch, void* stream);
+/* patch_out's weight gradient, fp32: dw [patch_h patch_w channels, c0] = sum over the tokens t of the patch row of t in u [batch, channels,
+ * height, width] times out_norm's output tokens[t, :] * (scale * rstd[t]) (tokens [batch T, c0], scale [c0], rstd [batch T]). */
+int kdb_wgrad_patch_out(const float* u, const float* tokens, const float* scale, const float* rstd, float* dw, int batch, int channels,
+                        int height, int width, int patch_h, int patch_w, int c0, float* scratch, void* stream);
+/* An RMSNorm channel scale's gradient per image: out[b ldo + j] = sum over the rows r of image b of dy[r, j] x[r, j] rstd_r, rstd_r =
+ * rsqrt(mean_j x[r, j]^2 + 1e-6) recomputed in fp32; x rows ldx floats apart, dy rows ldy (both >= c); rows a multiple of rows_per_image
+ * (rows_per_image == rows: one sum over all rows, ldo unused; else ldo >= c).  KDB_ERR_BAD_SHAPE when (rows / rows_per_image) times
+ * ceil(rows_per_image / 64) times c exceeds 2^22. */
+int kdb_norm_scale_grad(const float* x, int64_t ldx, const float* dy, int64_t ldy, float* out, int64_t ldo, int64_t rows_per_image,
+                        int64_t rows, int c, float* scratch, void* stream);
+/* Column sums: out[j] = sum over r < rows of p[r, j], p contiguous [rows, c].  KDB_ERR_BAD_SHAPE when ceil(rows / 256) c exceeds 2^22. */
+int kdb_colsum(const float* p, int64_t rows, int c, float* out, float* scratch, void* stream);
+/* TokenSplit's fac gradient: out[0] = sum of (y - skip) dup over the elements of skip and dup [batch, height, width, c], y [batch, height / 2,
+ * width / 2, 4 c] the split projection in TokenMerge order (height and width even). */
+int kdb_split_fac_grad(const float* y, const float* skip, const float* dup, float* out, int batch, int height, int width, int c, float* scratch,
+                       void* stream);
+/* class_emb's gradient: out[j, :] = sum over the rows r < rows with cls[r] == j (int64, device) of demb[r, :] (rows ldd >= mw floats apart),
+ * rows in order, for every j < n_classes (zero where no row has that class; a class outside [0, n_classes) adds to nothing).  No scratch. */
+int kdb_class_emb_grad(const float* demb, int64_t ldd, const int64_t* cls, float* out, int rows, int n_classes, int mw, void* stream);
 
 /* C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulate (wgmma), bf16 out. */
 int kdb_gemm_bf16(const void* a_bf16, const void* w_bf16, void* c_bf16, int M, int N, int K, void* stream);

@@ -977,7 +977,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     float* dmw = tr ? tr->grad("merges." + std::to_string(l) + ".proj.weight") : nullptr;
     const float* fine = reinterpret_cast<const float*>(ws.xs[l]);
     if (dmw && (rc = tf32 ? launch_wgrad_tf32_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)
-                          : launch_wgrad_merge(vs.g[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
+                          : launch_wgrad_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
       return rc;
     // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added; on the tf32 route the
     // GEMM stores dnxt W to ws.mg and a scatter kernel adds it
@@ -1407,18 +1407,65 @@ int kdb_model_train_forward(KdbModel* m, int precision, int batch, int height, i
                                            (cudaStream_t)stream, nullptr, nullptr, precision == KDB_PREC_TF32));
 }
 
-int kdb_wgrad_tf32(const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc, int merge_wc,
-                   float* scratch, void* stream) {
-  KDB_REQUIRE(dy && x && dw && scratch && m > 0 && n > 0 && k > 0, KDB_ERR_BAD_ARG, "wgrad_tf32: bad argument");
-  KDB_REQUIRE(ldy >= n, KDB_ERR_BAD_ARG, "wgrad_tf32: ldy %lld < n %d", (long long)ldy, n);
+int kdb_wgrad(int precision, const float* dy, int64_t ldy, const float* x, int64_t ldx, float* dw, int64_t m, int n, int k, int merge_hc,
+              int merge_wc, float* scratch, void* stream) {
+  KDB_REQUIRE(dy && x && dw && scratch && m > 0 && n > 0 && k > 0, KDB_ERR_BAD_ARG, "wgrad: bad argument");
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED, "wgrad: precision %d is neither fp32 nor tf32",
+              precision);
+  KDB_REQUIRE(ldy >= n, KDB_ERR_BAD_ARG, "wgrad: ldy %lld < n %d", (long long)ldy, n);
+  const bool tf32 = precision == KDB_PREC_TF32;
   cudaStream_t st = (cudaStream_t)stream;
   if (merge_hc > 0 || merge_wc > 0) {
     KDB_REQUIRE(merge_hc > 0 && merge_wc > 0 && k % 4 == 0 && m % ((int64_t)merge_hc * merge_wc) == 0, KDB_ERR_BAD_SHAPE,
-                "wgrad_tf32: merge geometry %dx%d with k %d, m %lld", merge_hc, merge_wc, k, (long long)m);
-    return launch_wgrad_tf32_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st);
+                "wgrad: merge geometry %dx%d with k %d, m %lld", merge_hc, merge_wc, k, (long long)m);
+    return tf32 ? launch_wgrad_tf32_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st)
+                : launch_wgrad_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st);
   }
-  KDB_REQUIRE(ldx >= k, KDB_ERR_BAD_ARG, "wgrad_tf32: ldx %lld < k %d", (long long)ldx, k);
-  return launch_wgrad_tf32(dy, ldy, x, ldx, dw, m, n, k, scratch, st);
+  KDB_REQUIRE(ldx >= k, KDB_ERR_BAD_ARG, "wgrad: ldx %lld < k %d", (long long)ldx, k);
+  return weight_grad(tf32, dy, ldy, x, ldx, dw, m, n, k, scratch, st);
+}
+
+int kdb_wgrad_patch_in(const float* dtok, const float* x, float* dw, int batch, int channels, int height, int width, int patch_h, int patch_w,
+                       int n, float* scratch, void* stream) {
+  KDB_REQUIRE(dtok && x && dw && scratch && batch > 0 && channels > 0 && n > 0 && patch_h > 0 && patch_w > 0, KDB_ERR_BAD_ARG,
+              "wgrad_patch_in: bad argument");
+  KDB_REQUIRE(height > 0 && width > 0 && height % patch_h == 0 && width % patch_w == 0, KDB_ERR_BAD_SHAPE,
+              "wgrad_patch_in: %dx%d image in %dx%d patches", height, width, patch_h, patch_w);
+  return launch_wgrad_patch_in(dtok, x, dw, batch, channels, height, width, patch_h, patch_w, n, scratch, (cudaStream_t)stream);
+}
+
+int kdb_wgrad_patch_out(const float* u, const float* tokens, const float* scale, const float* rstd, float* dw, int batch, int channels,
+                        int height, int width, int patch_h, int patch_w, int c0, float* scratch, void* stream) {
+  KDB_REQUIRE(u && tokens && scale && rstd && dw && scratch && batch > 0 && channels > 0 && c0 > 0 && patch_h > 0 && patch_w > 0,
+              KDB_ERR_BAD_ARG, "wgrad_patch_out: bad argument");
+  KDB_REQUIRE(height > 0 && width > 0 && height % patch_h == 0 && width % patch_w == 0, KDB_ERR_BAD_SHAPE,
+              "wgrad_patch_out: %dx%d image in %dx%d patches", height, width, patch_h, patch_w);
+  return launch_wgrad_patch_out(u, tokens, scale, rstd, dw, batch, channels, height, width, patch_h, patch_w, c0, scratch, (cudaStream_t)stream);
+}
+
+int kdb_norm_scale_grad(const float* x, int64_t ldx, const float* dy, int64_t ldy, float* out, int64_t ldo, int64_t rows_per_image,
+                        int64_t rows, int c, float* scratch, void* stream) {
+  KDB_REQUIRE(x && dy && out && scratch && c > 0 && ldx >= c && ldy >= c, KDB_ERR_BAD_ARG, "norm_scale_grad: bad argument");
+  KDB_REQUIRE(rows_per_image == rows || ldo >= c, KDB_ERR_BAD_ARG, "norm_scale_grad: ldo %lld < c %d with several images", (long long)ldo, c);
+  return launch_norm_scale_grad(x, ldx, dy, ldy, out, ldo, rows_per_image, rows, c, scratch, (cudaStream_t)stream);
+}
+
+int kdb_colsum(const float* p, int64_t rows, int c, float* out, float* scratch, void* stream) {
+  KDB_REQUIRE(p && out && scratch && rows > 0 && c > 0, KDB_ERR_BAD_ARG, "colsum: bad argument");
+  return launch_colsum(p, rows, c, out, scratch, (cudaStream_t)stream);
+}
+
+int kdb_split_fac_grad(const float* y, const float* skip, const float* dup, float* out, int batch, int height, int width, int c, float* scratch,
+                       void* stream) {
+  KDB_REQUIRE(y && skip && dup && out && scratch && batch > 0 && c > 0, KDB_ERR_BAD_ARG, "split_fac_grad: bad argument");
+  KDB_REQUIRE(height >= 2 && width >= 2 && height % 2 == 0 && width % 2 == 0, KDB_ERR_BAD_SHAPE, "split_fac_grad: %dx%d fine grid", height,
+              width);
+  return launch_split_fac_grad(y, skip, dup, out, batch, height, width, c, scratch, (cudaStream_t)stream);
+}
+
+int kdb_class_emb_grad(const float* demb, int64_t ldd, const int64_t* cls, float* out, int rows, int n_classes, int mw, void* stream) {
+  KDB_REQUIRE(demb && cls && out && rows > 0 && n_classes > 0 && mw > 0 && ldd >= mw, KDB_ERR_BAD_ARG, "class_emb_grad: bad argument");
+  return launch_class_emb_grad(demb, ldd, cls, out, rows, n_classes, mw, (cudaStream_t)stream);
 }
 
 int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

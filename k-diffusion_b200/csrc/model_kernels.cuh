@@ -222,7 +222,8 @@ constexpr int64_t kTrainPartFloats = int64_t(1) << 22;
 // dW[N, K] = sum over the rows m < M of dY[m, n] X[m, k] (the weight gradient of Y = X W^T); dY and X rows ldy, ldx floats apart
 int launch_wgrad(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part, cudaStream_t st);
 // the same with X the TokenMerge gather of the fine tokens [B, 2hc, 2wc, Cf] (M = B hc wc coarse rows, K = 4 Cf) read in place
-int launch_wgrad_merge(const float* dY, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part, cudaStream_t st);
+int launch_wgrad_merge(const float* dY, int64_t ldy, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part,
+                       cudaStream_t st);
 // Both with tf32 operands on the tensor cores (mma.sync): dY and X truncated to tf32 (the low 13 mantissa bits cleared), fp32 accumulation,
 // the same row chunks and chunk-order sum as launch_wgrad
 int launch_wgrad_tf32(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part,

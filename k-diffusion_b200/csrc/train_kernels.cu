@@ -252,8 +252,9 @@ int launch_wgrad(const float* dY, int64_t ldy, const float* X, int64_t ldx, floa
   return wgrad<false>(Rows{dY, ldy}, Rows{X, ldx}, dW, M, N, K, part, st);
 }
 
-int launch_wgrad_merge(const float* dY, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part, cudaStream_t st) {
-  return wgrad<false>(Rows{dY, N}, MergeX{fine, hc, wc, Cf}, dW, M, N, 4 * Cf, part, st);
+int launch_wgrad_merge(const float* dY, int64_t ldy, const float* fine, float* dW, int64_t M, int N, int hc, int wc, int Cf, float* part,
+                       cudaStream_t st) {
+  return wgrad<false>(Rows{dY, ldy}, MergeX{fine, hc, wc, Cf}, dW, M, N, 4 * Cf, part, st);
 }
 
 int launch_wgrad_tf32(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part,

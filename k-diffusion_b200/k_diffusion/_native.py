@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 22
+ABI_VERSION = 23
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -102,7 +102,13 @@ SIGNATURES = {
     "kdb_unet_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_unet_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_unet_tap_count": (_i64, [_vp]),
-    "kdb_wgrad_tf32": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_wgrad": (_i32, [_i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_wgrad_patch_in": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_wgrad_patch_out": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_norm_scale_grad": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
+    "kdb_colsum": (_i32, [_vp, _i64, _i32, _vp, _vp, _vp]),
+    "kdb_split_fac_grad": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_class_emb_grad": (_i32, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16_geglu": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
@@ -789,33 +795,157 @@ def gemm_bf16(a, w):
 WGRAD_SCRATCH_FLOATS = 1 << 22
 
 
+def _scratch(t):
+    return torch.empty(WGRAD_SCRATCH_FLOATS, device=t.device, dtype=torch.float32)
+
+
+def _out(out, shape, like, name):
+    """out, checked to be a contiguous fp32 tensor of `shape`, or a new one (the entry points write every element)"""
+    if out is None:
+        return torch.empty(shape, device=like.device, dtype=torch.float32)
+    if tuple(out.shape) != tuple(shape) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError(f"{name}: out must be a contiguous fp32 {list(shape)} tensor")
+    return out
+
+
+def _fp32_rows(name, *ts):
+    """each a 2-D fp32 tensor with unit column stride (any row stride)"""
+    for t in ts:
+        if t.dtype != torch.float32 or t.ndim != 2 or t.stride(1) != 1:
+            raise ValueError(f"{name}: operands must be 2-D fp32 with contiguous rows, got {t.dtype} {tuple(t.shape)} strides {t.stride()}")
+
+
+def _fp32_contiguous(name, *ts):
+    for t in ts:
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"{name}: operands must be contiguous fp32, got {t.dtype} {tuple(t.shape)}")
+
+
 @_on_device_of_first
-def wgrad_tf32(dy, x, n_rows=None, merge=None, out=None):
-    """kdb_wgrad_tf32: dW [N, K] = dy[:m]^T x[:m] with tf32 operands (truncated) and fp32 accumulation.  dy [m, N] and x [m, K] fp32
-    with unit column stride (any row stride); merge=(hc, wc): x is instead the fine tokens [B, 2hc, 2wc, Cf] read as the TokenMerge gather,
-    K = 4 Cf.  out: an [N, K] fp32 contiguous buffer to write (every element is written)."""
+def wgrad(dy, x, precision=PREC_FP32, n_rows=None, merge=None, out=None):
+    """kdb_wgrad: dW [N, K] = dy[:m]^T x[:m], fp32 (PREC_FP32) or with tf32 operands (truncated) and fp32 accumulation (PREC_TF32).
+    dy [m, N] and x [m, K] fp32 with unit column stride (any row stride); merge=(hc, wc): x is instead the fine tokens [B, 2hc, 2wc, Cf] read
+    as the TokenMerge gather, K = 4 Cf.  out: an [N, K] fp32 contiguous buffer to write (every element is written)."""
     require_cuda(dy, x, out)
     m = dy.shape[0] if n_rows is None else n_rows
     N = dy.shape[1]
     K = x.shape[-1] * 4 if merge else x.shape[1]
     if dy.dtype != torch.float32 or x.dtype != torch.float32 or dy.ndim != 2 or x.ndim != (4 if merge else 2):
-        raise ValueError("wgrad_tf32: dy [m, N] and x [m, K] (merge: [B, 2hc, 2wc, Cf]) fp32")
+        raise ValueError("wgrad: dy [m, N] and x [m, K] (merge: [B, 2hc, 2wc, Cf]) fp32")
     if dy.stride(1) != 1 or (not merge and x.stride(1) != 1) or (merge and not x.is_contiguous()):
-        raise ValueError("wgrad_tf32: operands need contiguous rows (the merge gather: contiguous fine tokens)")
+        raise ValueError("wgrad: operands need contiguous rows (the merge gather: contiguous fine tokens)")
     if not 0 < m <= dy.shape[0]:
-        raise ValueError(f"wgrad_tf32: {m} rows of a dy with {dy.shape[0]}")
+        raise ValueError(f"wgrad: {m} rows of a dy with {dy.shape[0]}")
     if merge:
         hc, wc = merge
         if hc <= 0 or wc <= 0 or tuple(x.shape[1:3]) != (2 * hc, 2 * wc) or m % (hc * wc) or m // (hc * wc) > x.shape[0]:
-            raise ValueError(f"wgrad_tf32: fine tokens {tuple(x.shape)} do not hold the TokenMerge gather of {m} rows of a {hc}x{wc} grid")
+            raise ValueError(f"wgrad: fine tokens {tuple(x.shape)} do not hold the TokenMerge gather of {m} rows of a {hc}x{wc} grid")
     elif m > x.shape[0]:
-        raise ValueError(f"wgrad_tf32: {m} rows of an x with {x.shape[0]}")
-    if out is not None and (tuple(out.shape) != (N, K) or out.dtype != torch.float32 or not out.is_contiguous()):
-        raise ValueError(f"wgrad_tf32: out must be a contiguous fp32 [{N}, {K}] tensor")
-    out = torch.empty(N, K, device=dy.device, dtype=torch.float32) if out is None else out
-    scratch = torch.empty(WGRAD_SCRATCH_FLOATS, device=dy.device, dtype=torch.float32)
+        raise ValueError(f"wgrad: {m} rows of an x with {x.shape[0]}")
+    out = _out(out, (N, K), dy, "wgrad")
     hc, wc = merge if merge else (0, 0)
-    check(lib().kdb_wgrad_tf32(ptr(dy), dy.stride(0), ptr(x), 0 if merge else x.stride(0), ptr(out), m, N, K, hc, wc, ptr(scratch), stream()))
+    check(lib().kdb_wgrad(precision, ptr(dy), dy.stride(0), ptr(x), 0 if merge else x.stride(0), ptr(out), m, N, K, hc, wc, ptr(_scratch(dy)),
+                          stream()))
+    return out
+
+
+
+def wgrad_tf32(dy, x, n_rows=None, merge=None, out=None):
+    """wgrad at PREC_TF32: the tf32 training precision's weight gradient (kdb_wgrad with tf32 operands), same arguments"""
+    return wgrad(dy, x, PREC_TF32, n_rows=n_rows, merge=merge, out=out)
+
+
+@_on_device_of_first
+def wgrad_patch_in(dtok, x, patch, out=None):
+    """kdb_wgrad_patch_in: dW [N, ph pw C] = dtok^T P with P the patch rows (columns (ph pw c)) of the NCHW image x [B, C, H, W] and
+    dtok [B (H/ph) (W/pw), N] contiguous fp32"""
+    require_cuda(dtok, x, out)
+    _fp32_contiguous("wgrad_patch_in", dtok, x)
+    (ph, pw), (B, C, H, W) = patch, x.shape
+    if ph <= 0 or pw <= 0 or H % ph or W % pw or dtok.ndim != 2 or dtok.shape[0] != B * (H // ph) * (W // pw):
+        raise ValueError(f"wgrad_patch_in: dtok {tuple(dtok.shape)} is not one row per {ph}x{pw} patch of an image {tuple(x.shape)}")
+    N = dtok.shape[1]
+    out = _out(out, (N, ph * pw * C), dtok, "wgrad_patch_in")
+    check(lib().kdb_wgrad_patch_in(ptr(dtok), ptr(x), ptr(out), B, C, H, W, ph, pw, N, ptr(_scratch(x)), stream()))
+    return out
+
+
+@_on_device_of_first
+def wgrad_patch_out(u, tokens, scale, rstd, patch, out=None):
+    """kdb_wgrad_patch_out: dW [ph pw C, C0] = P^T (tokens * (scale * rstd)) with P the patch rows (columns (ph pw c)) of u [B, C, H, W],
+    tokens [B (H/ph) (W/pw), C0], scale [C0] and rstd [B (H/ph) (W/pw)], all contiguous fp32"""
+    require_cuda(u, tokens, scale, rstd, out)
+    _fp32_contiguous("wgrad_patch_out", u, tokens, scale, rstd)
+    (ph, pw), (B, C, H, W) = patch, u.shape
+    T = B * (H // ph) * (W // pw) if ph > 0 and pw > 0 else -1
+    if ph <= 0 or pw <= 0 or H % ph or W % pw or tokens.ndim != 2 or tokens.shape[0] != T or tuple(rstd.shape) != (T,) or \
+            tuple(scale.shape) != (tokens.shape[1],):
+        raise ValueError(f"wgrad_patch_out: tokens {tuple(tokens.shape)}, scale {tuple(scale.shape)} and rstd {tuple(rstd.shape)} do not match "
+                         f"{ph}x{pw} patches of {tuple(u.shape)}")
+    C0 = tokens.shape[1]
+    out = _out(out, (ph * pw * C, C0), u, "wgrad_patch_out")
+    check(lib().kdb_wgrad_patch_out(ptr(u), ptr(tokens), ptr(scale), ptr(rstd), ptr(out), B, C, H, W, ph, pw, C0, ptr(_scratch(u)), stream()))
+    return out
+
+
+@_on_device_of_first
+def norm_scale_grad(x, dy, rows_per_image=None, out=None, ldo=None):
+    """kdb_norm_scale_grad: the RMSNorm scale gradient per image, sum over each image's rows of dy * x * rsqrt(mean(x^2) + 1e-6); x and dy
+    [rows, C] fp32 with contiguous rows (any row stride), rows_per_image (default: all rows, one image).  -> [B, C], or written into out
+    (flat, contiguous) at out[b * ldo + c] (ldo default C)"""
+    require_cuda(x, dy, out)
+    _fp32_rows("norm_scale_grad", x, dy)
+    rows, C = x.shape
+    R = rows if rows_per_image is None else rows_per_image
+    if tuple(dy.shape) != (rows, C) or R <= 0 or rows % R:
+        raise ValueError(f"norm_scale_grad: x {tuple(x.shape)}, dy {tuple(dy.shape)} with {R} rows per image")
+    B, ldo = rows // R, C if ldo is None else ldo
+    if out is None:
+        out = torch.empty(B, C, device=x.device, dtype=torch.float32)
+        ldo = C
+    elif out.dtype != torch.float32 or not out.is_contiguous() or (B > 1 and ldo < C) or out.numel() < (B - 1) * ldo + C:
+        raise ValueError(f"norm_scale_grad: out {tuple(out.shape)} does not hold {B} images of {C} channels {ldo} apart")
+    check(lib().kdb_norm_scale_grad(ptr(x), x.stride(0), ptr(dy), dy.stride(0), ptr(out), ldo, R, rows, C, ptr(_scratch(x)), stream()))
+    return out
+
+
+@_on_device_of_first
+def colsum(p, out=None):
+    """kdb_colsum: the column sums [C] of p [rows, C] contiguous fp32"""
+    require_cuda(p, out)
+    _fp32_contiguous("colsum", p)
+    if p.ndim != 2:
+        raise ValueError(f"colsum: p must be [rows, C], got {tuple(p.shape)}")
+    out = _out(out, (p.shape[1],), p, "colsum")
+    check(lib().kdb_colsum(ptr(p), p.shape[0], p.shape[1], ptr(out), ptr(_scratch(p)), stream()))
+    return out
+
+
+@_on_device_of_first
+def split_fac_grad(y, skip, dup, out=None):
+    """kdb_split_fac_grad: TokenSplit's fac gradient [1], the sum of (y - skip) dup with y [B, H/2, W/2, 4C] in TokenMerge order and skip,
+    dup [B, H, W, C], all contiguous fp32"""
+    require_cuda(y, skip, dup, out)
+    _fp32_contiguous("split_fac_grad", y, skip, dup)
+    B, H, W, C = skip.shape
+    if tuple(dup.shape) != (B, H, W, C) or H % 2 or W % 2 or tuple(y.shape) != (B, H // 2, W // 2, 4 * C):
+        raise ValueError(f"split_fac_grad: y {tuple(y.shape)}, skip {tuple(skip.shape)}, dup {tuple(dup.shape)}")
+    out = _out(out, (1,), y, "split_fac_grad")
+    check(lib().kdb_split_fac_grad(ptr(y), ptr(skip), ptr(dup), ptr(out), B, H, W, C, ptr(_scratch(y)), stream()))
+    return out
+
+
+@_on_device_of_first
+def class_emb_grad(demb, cls, n_classes, out=None):
+    """kdb_class_emb_grad: [n_classes, mw], row j the sum of the rows of demb [rows, mw] (fp32, contiguous rows) whose class cls [rows]
+    (int64) is j"""
+    require_cuda(demb, cls, out)
+    _fp32_rows("class_emb_grad", demb)
+    rows, mw = demb.shape
+    if cls.dtype != torch.int64 or tuple(cls.shape) != (rows,) or not cls.is_contiguous():
+        raise ValueError(f"class_emb_grad: cls must be contiguous int64 [{rows}], got {cls.dtype} {tuple(cls.shape)}")
+    out = _out(out, (n_classes, mw), demb, "class_emb_grad")
+    check(lib().kdb_class_emb_grad(ptr(demb), demb.stride(0), ptr(cls), ptr(out), rows, n_classes, mw, stream()))
     return out
 
 

@@ -4,8 +4,8 @@ only; natten, dctorch and the other absent modules stubbed):
 
     K_DIFFUSION_REFERENCE=<checkout> python oracle/make_golden_train.py      # -> tests/golden/train.npz, tests/golden/train_meta.json
 
-For a class-conditional model (soft-min-snr, and the simple loss) and a three-level model (shifted-window, global and none levels,
-mapping_cond, aug_cond through KarrasAugmentWrapper) with synth.py weights: the per-sample losses of Denoiser.loss in float64 and fp32,
+For a class-conditional model (soft-min-snr, and the simple loss), a three-level model (shifted-window, global and none levels,
+mapping_cond, aug_cond through KarrasAugmentWrapper), cfg1 (the MNIST transformer) and the CIFAR-10 transformer, with synth.py weights: the per-sample losses of Denoiser.loss in float64 and fp32,
 and for every parameter the norm of its float64 gradient, its dot product with a fixed probe, and the relative L2 distance of the fp32
 gradient from the float64 one (the reference's own fp32 error).  Also the names of the four param_groups of those models and of cfg1.
 The inputs follow tests/test_train_host.py's recipe."""
@@ -34,6 +34,9 @@ LEVELS3 = {"model": {"type": "image_transformer_v2", "input_channels": 3, "input
                      "self_attns": [{"type": "shifted-window", "d_head": 16, "window_size": 4}, {"type": "global", "d_head": 16},
                                     {"type": "none"}]}}
 CASES = {"class": (CLASS, "karras", False), "class_simple": (CLASS, "simple", False), "levels3": (LEVELS3, "karras", True)}
+# the reference's own transformer configs: cfg1 (MNIST, tests/golden/cfg1_mnist_shapes.json) and the CIFAR-10 transformer, whose loaded
+# config and parameter shapes this script records in tests/golden/cifar10_transformer_shapes.json
+REF_CASES = {"cfg1": "cfg1_mnist_shapes.json", "cifar10": "cifar10_transformer_shapes.json"}
 
 
 def synth_sd(synth, shapes, seed=3):
@@ -72,7 +75,12 @@ def main():
     synth = G._load_synth()
     torch.set_num_threads(8)
     rec, meta = {}, {"param_groups": {}, "cases": {}}
-    for name, (cfg, loss_config, wrap) in CASES.items():
+    golden = ROOT / "tests" / "golden"
+    c10 = K.config.load_config(json.loads((G.REF / "configs" / "config_cifar10_transformer.json").read_text()))
+    shapes = {k: list(v.shape) for k, v in K.config.make_model(c10).state_dict().items()}
+    (golden / REF_CASES["cifar10"]).write_text(json.dumps(dict(config=c10, shapes=shapes), indent=1))
+    cases = dict(CASES, **{name: (json.loads((golden / f).read_text())["config"], "karras", False) for name, f in REF_CASES.items()})
+    for name, (cfg, loss_config, wrap) in cases.items():
         c = K.config.load_config(json.loads(json.dumps(cfg)))
         c["model"]["loss_config"] = loss_config
         inner = K.config.make_model(c)

@@ -107,6 +107,9 @@ def check_against_oracle(cfg, sd, got_loss, got, x, noise, sigma, kw, gw, simple
         assert err <= 8 * ref + 1e-6, f"{k}: rel-L2 {err:.3e} vs the fp32 distance {ref:.3e}"
 
 
+GOLDEN = Path(__file__).resolve().parent / "golden"
+
+
 @pytest.mark.parametrize("simple", [False, True])
 def test_class_conditional_gradients_match_float64(simple):
     cfg, inner, sd, model = build({"model": dict(CLASS["model"], loss_config="simple" if simple else "karras"), "dataset": CLASS["dataset"]})
@@ -178,11 +181,84 @@ def test_v1_training_call_is_unsupported():
         eng.forward_train(x, torch.randn_like(x), sig, None, None, None, cond, {})
 
 
-GOLDEN = Path(__file__).resolve().parent / "golden"
+# the reference's transformer configs: cfg1 (MNIST: d_head 64, patch 4 on a 7x7 grid, one level, no merges or splits), the CIFAR-10
+# transformer (two global levels of width 256 and 512) and cfg2 (the shifted-window Oxford Flowers model, window 8 at d_head 64)
+CFG1 = json.loads((GOLDEN / "cfg1_mnist_shapes.json").read_text())["config"]
+CIFAR10 = json.loads((GOLDEN / "cifar10_transformer_shapes.json").read_text())["config"]
+CFG2 = json.loads((GOLDEN / "cfg2_sw256_shapes.json").read_text())["config"]
+
+
+@pytest.mark.parametrize("B", [2, 5])
+def test_cfg1_gradients_match_float64(B):
+    """cfg1 at fp32 with the cond-dropout class 10 among the labels"""
+    cfg, inner, sd, model = build(CFG1)
+    x, noise, sigma, kw, gw = inputs(cfg, B, 20 + B, classes=[10, 3, 10, 0, 9][:B])
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+@pytest.mark.parametrize("wrap", [False, True], ids=["plain", "augment_wrapper"])
+def test_cifar10_transformer_gradients_match_float64(wrap):
+    spec = {"model": dict(CIFAR10["model"], mapping_cond_dim=9 if wrap else 0), "dataset": CIFAR10["dataset"]}
+    cfg, inner, sd, model = build(spec, wrap=wrap)
+    x, noise, sigma, kw, gw = inputs(cfg, 4, 30 + wrap, classes=[10, 2, 2, 7])
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+def test_cifar10_transformer_batch_of_16_is_the_sum_of_its_images():
+    """B = 16: level 0 holds 16 x 16 x 16 x 256 = 1,048,576 elements (TokenSplit's fac reduction loops past one pass of its grid) and
+    the AdaRMSNorm scale gradients fill 16 per-image slots"""
+    cfg, inner, sd, model = build(CIFAR10)
+    x, noise, sigma, kw, gw = inputs(cfg, 16, 32)
+    l1, g1 = native_grads(model, inner, x, noise, sigma, kw, gw)
+    parts = [native_grads(model, inner, x[i:i + 1], noise[i:i + 1], sigma[i:i + 1], {k: v[i:i + 1] for k, v in kw.items()}, gw[i:i + 1])
+             for i in range(16)]
+    assert torch.equal(l1, torch.cat([p[0] for p in parts]))
+    for k in g1:
+        s = sum(p[1][k] for p in parts)
+        assert (g1[k] - s).norm() <= 1e-5 * s.norm() + 1e-7, k
+
+
+@pytest.mark.parametrize("size,B", [(64, 2), (128, 1)])
+def test_cfg2_gradients_match_float64(size, B):
+    """cfg2 with its first level at 16x16 and 32x32 tokens (window 8)"""
+    cfg, inner, sd, model = build({"model": dict(CFG2["model"], input_size=[size, size]), "dataset": CFG2["dataset"]})
+    x, noise, sigma, kw, gw = inputs(cfg, B, 40 + size)
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+FROZEN = {"mapping": ("mapping.",), "class_emb": ("class_emb.",), "level": ("down_levels.0.",), "merges_splits": ("merges.", "splits.")}
+
+
+@pytest.mark.parametrize("frozen", sorted(FROZEN))
+def test_frozen_parameters_leave_the_other_gradients_unchanged(frozen):
+    """Only parameters that require grad are bound: a frozen subset keeps grad None, and every other gradient is bit for bit that of the
+    run with all parameters"""
+    cfg, inner, sd, model = build(CLASS)
+    x, noise, sigma, kw, gw = inputs(cfg, 3, 50, classes=[10, 4, 4])
+    _, full = native_grads(model, inner, x, noise, sigma, kw, gw)
+    names = [k for k, _ in inner.named_parameters() if k.startswith(FROZEN[frozen])]
+    assert names
+    params = dict(inner.named_parameters())
+    for k in names:
+        params[k].requires_grad_(False)
+    inner.zero_grad(set_to_none=True)
+    loss = model.loss(x.cuda(), noise.cuda(), sigma.cuda(), **{k: v.cuda() for k, v in kw.items()})
+    (loss * gw.cuda()).sum().backward()
+    for k, p in params.items():
+        if k in names:
+            assert p.grad is None, k
+        else:
+            assert torch.equal(p.grad.cpu(), full[k]), k
+
+
 # oracle/make_golden_train.py's cases: the three-level model there has a global middle level (the reference needs natten for neighborhood)
 FIXTURE_LEVELS3 = {"model": dict(LEVELS3["model"], self_attns=[LEVELS3["model"]["self_attns"][0], {"type": "global", "d_head": 16},
                                                                LEVELS3["model"]["self_attns"][2]])}
-FIXTURES = {"class": (CLASS, "karras", False), "class_simple": (CLASS, "simple", False), "levels3": (FIXTURE_LEVELS3, "karras", True)}
+FIXTURES = {"class": (CLASS, "karras", False), "class_simple": (CLASS, "simple", False), "levels3": (FIXTURE_LEVELS3, "karras", True),
+            "cfg1": (CFG1, "karras", False), "cifar10": (CIFAR10, "karras", False)}
 
 
 @pytest.mark.parametrize("case", sorted(FIXTURES))

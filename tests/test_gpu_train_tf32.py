@@ -1,11 +1,11 @@
-"""The tf32 training precision on the H100: kdb_wgrad_tf32 kernel by kernel against float64 sums of its truncated operands, and the whole
+"""The tf32 training precision on the H100: kdb_wgrad at tf32 (_native.wgrad_tf32) kernel by kernel against float64 sums of its truncated operands, and the whole
 model's parameter gradients at tf32 against the tf32 restatement of tests/test_train_tf32_host.py: within a multiple of the restatement's own
 fp32-vs-float64 distance, clearly closer to it than to exact arithmetic, with the properties tests/test_gpu_train.py pins at fp32."""
 import pytest
 import torch
 
 from oracle.make_golden_tf32 import tf32_trunc
-from test_gpu_train import CLASS, LEVELS3, build, inputs, native_grads
+from test_gpu_train import CIFAR10, CLASS, LEVELS3, build, inputs, native_grads
 from test_train_tf32_host import restated_grads
 
 import k_diffusion as K
@@ -222,5 +222,14 @@ def test_cfg1_tf32_gradients():
     cfg, inner, sd, model = build(spec)
     inner.set_train_precision("tf32")
     x, noise, sigma, kw, gw = inputs(cfg, 2, 8)
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    check_against_restatement(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+def test_cifar10_transformer_tf32_gradients():
+    """the CIFAR-10 transformer (two global levels of width 256 and 512, d_head 64) at tf32 against the restatement"""
+    cfg, inner, sd, model = build(CIFAR10)
+    inner.set_train_precision("tf32")
+    x, noise, sigma, kw, gw = inputs(cfg, 2, 13, classes=[10, 6])
     loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
     check_against_restatement(cfg, sd, loss, got, x, noise, sigma, kw, gw)

@@ -28,7 +28,10 @@ LEVELS3 = {"model": {"type": "image_transformer_v2", "input_channels": 3, "input
                      "mapping_cond_dim": 12, "sigma_data": 0.5,
                      "self_attns": [{"type": "shifted-window", "d_head": 16, "window_size": 4}, {"type": "global", "d_head": 16},
                                     {"type": "none"}]}}
-CASES = {"class": (CLASS, False), "class_simple": (CLASS, True), "levels3": (LEVELS3, False)}
+# the reference's transformer configs as recorded beside their parameter shapes: cfg1 (MNIST) and the CIFAR-10 transformer
+REF_CONFIGS = {"cfg1": "cfg1_mnist_shapes.json", "cifar10": "cifar10_transformer_shapes.json"}
+CASES = {"class": (CLASS, False), "class_simple": (CLASS, True), "levels3": (LEVELS3, False),
+         **{name: (json.loads((GOLDEN / f).read_text())["config"], False) for name, f in REF_CONFIGS.items()}}
 BUFFERS = ("pos_emb.freqs", "time_emb.weight", "aug_emb.weight")
 
 
@@ -74,12 +77,9 @@ def test_oracle_loss_and_gradients_match_the_reference(case):
         assert (g * probe).sum().item() == pytest.approx(w["probe"], rel=2e-5, abs=2e-5 * w["norm"]), k
 
 
-@pytest.mark.parametrize("case", ["class", "levels3", "cfg1"])
+@pytest.mark.parametrize("case", ["class", "levels3", "cfg1", "cifar10"])
 def test_param_groups_match_the_reference(case):
-    if case == "cfg1":
-        inner = K.config.make_model(K.config.load_config(json.loads((GOLDEN / "cfg1_mnist_shapes.json").read_text())["config"]))
-    else:
-        _, inner, _ = model_of(CASES[case][0])
+    _, inner, _ = model_of(CASES[case][0])
     groups = inner.param_groups(1e-3, 0.25)
     names = {id(p): k for k, p in inner.named_parameters()}
     assert [[names[id(p)] for p in g["params"]] for g in groups] == META["param_groups"][case]
@@ -186,3 +186,34 @@ def test_set_grad_checks_key_shape_and_buffers_without_gpu():
         assert b"buffer" in L.kdb_last_error()
     finally:
         L.kdb_model_destroy(h)
+
+
+def test_reduction_wrappers_refuse_mismatched_operands(cpu_native, monkeypatch):
+    """The C reductions take no operand extents: each wrapper checks them before the call, so a mismatch raises instead of reading or
+    writing out of bounds"""
+    from k_diffusion import _native
+    monkeypatch.setattr(_native, "lib", lambda: pytest.fail("reached the library"))
+    z = torch.zeros
+    bad = [
+        lambda: _native.wgrad(z(10, 4), z(9, 5)),                                           # fewer x rows than dy rows
+        lambda: _native.wgrad(z(10, 4), z(10, 5), out=z(5, 4)),
+        lambda: _native.wgrad(z(10, 4), z(10, 5).t().contiguous().t()),                     # x columns not contiguous
+        lambda: _native.wgrad_patch_in(z(2 * 7 * 7, 8), z(2, 1, 28, 28), (4, 3)),            # 28 is not a multiple of 3
+        lambda: _native.wgrad_patch_in(z(2 * 7 * 6, 8), z(2, 1, 28, 28), (4, 4)),            # one token row per patch
+        lambda: _native.wgrad_patch_out(z(1, 3, 8, 8), z(16, 32), z(32), z(15), (2, 2)),     # rstd per token
+        lambda: _native.wgrad_patch_out(z(1, 3, 8, 8), z(16, 32), z(31), z(16), (2, 2)),     # scale per channel
+        lambda: _native.norm_scale_grad(z(10, 8), z(10, 8), 3),                              # rows a multiple of the rows per image
+        lambda: _native.norm_scale_grad(z(10, 8), z(10, 9)),
+        lambda: _native.norm_scale_grad(z(10, 8), z(10, 8), 5, out=z(8 + 8), ldo=7),         # images overlap
+        lambda: _native.norm_scale_grad(z(10, 8), z(10, 8), 5, out=z(10 + 7), ldo=10),       # too short for two images 10 apart
+        lambda: _native.colsum(z(10, 4).t()),
+        lambda: _native.colsum(z(10, 4), out=z(5)),
+        lambda: _native.split_fac_grad(z(1, 2, 2, 12), z(1, 4, 4, 3), z(1, 4, 5, 3)),
+        lambda: _native.split_fac_grad(z(1, 2, 3, 12), z(1, 4, 5, 3), z(1, 4, 5, 3)),      # odd fine grid
+        lambda: _native.class_emb_grad(z(4, 8), torch.zeros(4, dtype=torch.int32), 11),
+        lambda: _native.class_emb_grad(z(4, 8), torch.zeros(3, dtype=torch.int64), 11),
+    ]
+    for i, call in enumerate(bad):
+        with pytest.raises(ValueError):
+            call()
+            pytest.fail(f"case {i} was accepted")
