@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 24
+#define KDB_ABI_VERSION 25
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -388,6 +388,27 @@ int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width
 int     kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity);
 int64_t kdb_unet_tap_count(const KdbUNet* m);
 
+/* Parameter gradients (training) of the U-Net, exact fp32, as kdb_model_set_grad / kdb_model_forward_train do for image_transformer_v2.
+ * kdb_unet_set_grad binds a gradient buffer [shape] fp32 on the device to the state-dict key of a parameter (data == NULL unbinds it):
+ * KDB_ERR_MISSING_KEY for a key that is no tensor set on the model, KDB_ERR_BAD_SHAPE for a shape other than that tensor's, KDB_ERR_BAD_ARG
+ * for the buffers timestep_embed.weight and *.kernel (the resampling filters), which take no gradient, and for the parameters of the DBlocks
+ * and UBlocks of the levels below skip_stages, which the forward never runs.
+ * kdb_unet_forward_train runs the raw model F (sigma_data 0) forward, bit for bit as kdb_unet_forward at KDB_PREC_FP32, takes the cotangent
+ * u [B, in_channels, H, W] on out = F(x, sigma) and OVERWRITES every bound gradient with u^T dF/dparam summed over the batch (proj_out's
+ * variance row of a has_variance model: exactly 0); unbound parameters are skipped.  sigma [B], aug_cond [B, 9] or NULL and mapping_cond are
+ * the raw conditioning inputs as for kdb_unet_conditioning, cond one conditioning row per image made from them (cond_batch_stride ==
+ * kdb_unet_cond_stride).  precision must be KDB_PREC_FP32 (KDB_ERR_UNSUPPORTED otherwise).  The bound keys are checked again, with
+ * kdb_unet_set_grad's codes.  The first call after a kdb_unet_finalize builds the input-gradient copy of every convolution weight (taps
+ * reversed, channels swapped) in memory the handle keeps until kdb_unet_destroy; that call must run outside CUDA-graph capture
+ * (KDB_ERR_UNSUPPORTED otherwise).  The workspace is kdb_unet_train_workspace_bytes(m, batch, height, width) bytes (finalized model; negative
+ * KDB_ERR_* on bad arguments); it holds the tape of every module's output.  No atomics: every sum runs in an order fixed by the shapes, so
+ * two calls give the same bits. */
+int     kdb_unet_set_grad(KdbUNet* m, const char* key, float* data, const int64_t* shape, int ndim);
+int64_t kdb_unet_train_workspace_bytes(const KdbUNet* m, int batch, int height, int width);
+int     kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
+                               const float* aug_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
+                               const float* cotangent, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)
  * ------------------------------------------------------------------------------------------ */
@@ -490,6 +511,27 @@ int kdb_attention_vjp(const float* qkv, const float* out, const float* dout, flo
  * with r2 NULL = r1 alone.  c1, c2 and rc1 must be multiples of 4; batch * h * w is at most 65535 * 64 (KDB_ERR_BAD_SHAPE). */
 int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const float* w_tapmajor, const float* bias, const float* r1, int rc1,
                   const float* r2, float* out, int batch, int h, int w, int n_out, int ksize, void* stream);
+
+/* The backward kernels of kdb_unet_forward_train (fp32, deterministic, every output element written; arguments checked before any launch).
+ * kdb_unet_conv_wgrad: the weight gradient of kdb_unet_conv in torch's layout, dw [n_out, c1 + c2, ksize, ksize] = sum over the pixels m of
+ *   dy[m, n] (contiguous [batch, h, w, n_out]) times the input [in1 | in2] at pixel m shifted by the tap, zero outside the grid.  scratch:
+ *   2^22 floats.
+ * kdb_unet_flip_conv_weight: the weight of the input-gradient convolution, out [c_in, ksize^2, n_out] with out[c, tap, n] = w[n, ksize^2 - 1
+ *   - tap, c] of a tap-major w [n_out, ksize^2, c_in]; kdb_unet_conv of dy with it is the input gradient (what kdb_unet_forward_train
+ *   builds for every convolution).
+ * kdb_unet_adagn_vjp: the backward of AdaGN (+ the erf GELU when gelu): x = [in1 | in2] [batch, hw, c1 + c2] the AdaGN input, dy its output
+ *   gradient, the (weight, bias) pair read at cond + b * cond_batch_stride + ada_off as the forward reads it.  Writes dx (+ add when add is
+ *   not NULL; add [batch, hw, c1 + c2] may alias neither output) to dx1 (c1 channels) and dx2 (c2), and the gradients of the weight and bias
+ *   rows to dcond + b * dcond_batch_stride + ada_off (c1 + c2 floats each).
+ * kdb_unet_resample_vjp: the adjoint of the 2x resampling of an h x w grid (h, w >= 2), reflect padding included: dout [batch, h/2, w/2, c]
+ *   (up = 0) or [batch, 2h, 2w, c] (up = 1) -> din [batch, h, w, c] (+ add when not NULL; add may be din). */
+int kdb_unet_conv_wgrad(const float* dy, int n_out, const float* in1, int c1, const float* in2, int c2, float* dw, int batch, int h, int w,
+                        int ksize, float* scratch, void* stream);
+int kdb_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, const float* dy, const float* add, float* dx1, float* dx2,
+                       const float* cond, int64_t cond_batch_stride, int ada_off, float* dcond, int64_t dcond_batch_stride, int groups, int gelu,
+                       int batch, int hw, void* stream);
+int kdb_unet_flip_conv_weight(const float* w_tapmajor, float* out, int n_out, int c_in, int ksize, void* stream);
+int kdb_unet_resample_vjp(const float* dout, const float* add, float* din, int batch, int h, int w, int c, int up, void* stream);
 
 /* The same convolution, arguments and layouts on the tensor cores (wgmma, the kernel kdb_unet_forward runs at KDB_PREC_TF32): the
  * products take tf32 operands -- the low 13 mantissa bits of every input and weight element are ignored (truncation), so a caller

@@ -6,6 +6,7 @@
 
 #include "model_kernels.cuh"
 #include "simt_tile.cuh"
+#include "unet_kernels.cuh"
 
 namespace kdb {
 
@@ -60,6 +61,20 @@ struct NormX {    // RMSNorm's output x * (scale * rstd) of rows x [M, K], rstd 
   const float *x, *scale, *rstd;
   int K;
   __device__ float operator()(int64_t m, int k) const { return x[m * K + k] * (__ldg(scale + k) * rstd[m]); }
+};
+
+struct TapX {     // the input [in1 | in2] of a ks x ks convolution (U-Net, token-major [B, H, W, c]) at pixel m shifted by the tap of column
+                  // k = (c, tap), torch's weight order; zero outside the grid
+  const float *p1, *p2;
+  int c1, c2, H, W, ks;
+  __device__ float operator()(int64_t m, int k) const {
+    const int kk = ks * ks, c = k / kk, tap = k - c * kk;
+    const int dy = tap / ks - ks / 2, dx = tap % ks - ks / 2;
+    const int r = (int)(m % ((int64_t)H * W)), y = r / W + dy, x = r % W + dx;
+    if (y < 0 || y >= H || x < 0 || x >= W) return 0.f;
+    const int64_t pix = m + (int64_t)dy * W + dx;
+    return c < c1 ? p1[pix * c1 + c] : p2[pix * c2 + (c - c1)];
+  }
 };
 
 // Chunk z of the rows: part[z, n, k] = sum over m in the chunk of dY[m, n] X(m, k), on the tile loop of simt_tile.cuh with (n, k) as
@@ -275,6 +290,11 @@ int launch_wgrad_patch_in(const float* dtok, const float* x, float* dW, int B, i
 int launch_wgrad_patch_out(const float* u, const float* tokens, const float* scale, const float* rstd, float* dW, int B, int C, int H, int Wd,
                            int ph, int pw, int C0, float* part, cudaStream_t st) {
   return wgrad<false>(PatchX{u, C, H, Wd, ph, pw}, NormX{tokens, scale, rstd, C0}, dW, (int64_t)B * (H / ph) * (Wd / pw), ph * pw * C, C0, part, st);
+}
+
+int launch_wgrad_conv(const float* dY, int N, const float* in1, int c1, const float* in2, int c2, float* dW, int B, int H, int W, int ks,
+                      float* part, cudaStream_t st) {
+  return wgrad<false>(Rows{dY, N}, TapX{in1, in2, c1, c2, H, W, ks}, dW, (int64_t)B * H * W, N, (c1 + c2) * ks * ks, part, st);
 }
 
 int launch_norm_scale_grad(const float* x, int64_t ldx, const float* dy, int64_t ldy, float* out, int64_t ldo, int64_t rows_per_batch,

@@ -31,7 +31,9 @@ struct UMod {
   std::string tap;
   int c_in = 0, c_mid = 0, c_out = 0;
   int groups1 = 1, groups2 = 1, ada1 = 0, ada2 = 0;
+  std::string prefix;             // state-dict prefix of a ResConvBlock or SelfAttention2d
   ConvW w1, w2, skip_w;
+  const float *w1t = nullptr, *w2t = nullptr, *skip_t = nullptr;   // the input-gradient weights (ensure_bwd)
   const float *b1 = nullptr, *b2 = nullptr;   // derived (owned) biases
   const float *mapper1_w = nullptr, *mapper1_b = nullptr, *mapper2_w = nullptr, *mapper2_b = nullptr;
   bool to_skip = false;           // the last module of a DBlock writes the level's skip buffer
@@ -45,6 +47,13 @@ struct KdbUNet : kdb::ModelCore {
   const float *proj_in_w = nullptr, *proj_in_b = nullptr, *proj_out_w = nullptr, *proj_out_b = nullptr;
   int ada_total = 0;
   kdb::UNetCondWeights cw{};
+  std::unordered_map<std::string, TensorRef> grads;   // kdb_unet_set_grad: gradient buffers by state-dict key
+  // ensure_bwd's flipped convolution weights, one allocation per weight in the order of mods, kept across finalizes instead of in `owned`
+  std::vector<float*> bwd_mem;
+  bool bwd_ready = false;
+  ~KdbUNet() {
+    for (float* p : bwd_mem) cudaFree(p);
+  }
 };
 
 using namespace kdb;
@@ -129,6 +138,7 @@ int plan_block(KdbUNet* m, const std::string& p, int level, const char* tag, int
     r.c_mid = c_mid;
     r.c_out = i < depth - 1 ? c_mid : c_out;
     r.tap = std::string(tag) + std::to_string(level) + "." + std::to_string(idx);
+    r.prefix = p + std::to_string(idx) + ".";
     if ((rc = plan_res(m, p + std::to_string(idx) + ".", r, st))) return rc;
     m->mods.push_back(r);
     ++idx;
@@ -138,6 +148,7 @@ int plan_block(KdbUNet* m, const std::string& p, int level, const char* tag, int
       a.level = level;
       a.c_in = a.c_mid = a.c_out = r.c_out;
       a.tap = std::string(tag) + std::to_string(level) + "." + std::to_string(idx);
+      a.prefix = p + std::to_string(idx) + ".";
       if ((rc = plan_attn(m, p + std::to_string(idx) + ".", a, st))) return rc;
       m->mods.push_back(a);
       ++idx;
@@ -250,19 +261,27 @@ int run_attn(int prec, const UMod& u, const float* x, float* out, UWs& ws, int B
   return conv(prec, o, u.w2, 1, st);
 }
 
+// tape != nullptr (training): patch_in writes tape[0] and module i (of m->mods) tape[i + 1], which a DBlock's last module's UBlock then reads
+// as its skip; the launches are those of tape == nullptr
 int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cbs, float* out,
-                 UWs& ws, cudaStream_t st) {
+                 UWs& ws, cudaStream_t st, float* const* tape = nullptr) {
   const KdbUNetConfig& c = m->cfg;
   const int s0 = c.skip_stages, C0 = c.channels[std::max(0, s0 - 1)];
   int h, w, rc;
   level_dims(c, H, W, s0, &h, &w);
-  if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, ws.x[0], B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
-  if ((rc = m->tap("patch_in", ws.x[0], (int64_t)B * h * w * C0, st))) return rc;
-  Src cur{ws.x[0], C0, nullptr, 0};
+  float* x0 = tape ? tape[0] : ws.x[0];
+  if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, x0, B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
+  if ((rc = m->tap("patch_in", x0, (int64_t)B * h * w * C0, st))) return rc;
+  Src cur{x0, C0, nullptr, 0};
   int cur_buf = 0;                         // index of the ping-pong buffer holding cur (-1: a skip buffer)
-  for (const UMod& u : m->mods) {
+  for (size_t i = 0; i < m->mods.size(); ++i) {
+    const UMod& u = m->mods[i];
     const int nb = cur_buf == 0 ? 1 : 0;
     float* dst = u.to_skip ? ws.skip[u.level] : ws.x[nb];
+    if (tape && u.kind != M_CONCAT) {
+      dst = tape[i + 1];
+      if (u.to_skip) ws.skip[u.level] = dst;
+    }
     int C = u.c_out;
     switch (u.kind) {
       case M_DOWN:
@@ -287,6 +306,310 @@ int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, cons
     cur_buf = u.to_skip ? -1 : nb;
   }
   return launch_unet_patch_out(cur.p1, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, cur.c1, st);
+}
+
+// ------------------------------------------------------------------------------------------------
+// training: the fp32 forward with a tape, then the reverse walk with every parameter's gradient
+// ------------------------------------------------------------------------------------------------
+
+// The training workspace: a forward's (UWs), the tape (patch_in's output, then every module's output: the input of the next), the stream
+// gradient in two ping-pong buffers, each level's skip gradient, the backward's scratch, the conditioning's gradients, the reduction partials.
+struct TWs {
+  UWs f;
+  std::vector<float*> tape;
+  float *g[2] = {}, *gskip[KDB_MAX_LEVELS] = {};
+  float *ga = nullptr, *gb = nullptr, *dqkv = nullptr, *stats = nullptr;
+  float *dss = nullptr, *dcond = nullptr, *dwcat = nullptr, *dbcat = nullptr, *U = nullptr, *xin = nullptr, *part = nullptr;
+  UNetMapGrad mg{};
+  size_t total = 0;
+};
+
+// the input (sources, grid) of every module of m->mods, as unet_forward with a tape feeds it (M_CONCAT: unused)
+struct ModIO {
+  Src in;
+  int h = 0, w = 0;
+};
+
+// The walk of unet_forward over the modules: fn(i, module, input, grid h, w, output channels)
+template <typename Fn>
+void walk(const KdbUNet* m, int H, int W, float* const* tape, Fn fn) {
+  const KdbUNetConfig& c = m->cfg;
+  int h, w;
+  level_dims(c, H, W, c.skip_stages, &h, &w);
+  Src cur{tape ? tape[0] : nullptr, c.channels[std::max(0, c.skip_stages - 1)], nullptr, 0};
+  float* skip[KDB_MAX_LEVELS] = {};
+  for (size_t i = 0; i < m->mods.size(); ++i) {
+    const UMod& u = m->mods[i];
+    if (u.kind == M_CONCAT) {
+      cur.p2 = skip[u.level], cur.c2 = c.channels[u.level];
+      continue;
+    }
+    const int h0 = h, w0 = w;
+    int C = u.c_out;
+    if (u.kind == M_DOWN) h /= 2, w /= 2, C = cur.c1;
+    if (u.kind == M_UP) h *= 2, w *= 2, C = cur.c1;
+    fn(i, u, cur, h0, w0, h, w, C);
+    float* dst = tape ? tape[i + 1] : nullptr;
+    if (u.to_skip) skip[u.level] = dst;
+    cur = Src{dst, C, nullptr, 0};
+  }
+}
+
+void carve_train(const KdbUNet* m, int B, int H, int W, void* workspace, TWs& t) {
+  const KdbUNetConfig& c = m->cfg;
+  carve(c, B, H, W, workspace, t.f);
+  Carver cv(workspace ? static_cast<char*>(workspace) + t.f.total : nullptr, 256);
+  auto take = [&](size_t floats) { return cv.take<float>(floats * sizeof(float)); };
+  const int s0 = c.skip_stages, mw = c.mapping_out, A = m->ada_total, p = c.patch_size;
+  const int Kin = c.in_channels * p * p, Kout = Kin + (c.has_variance ? 1 : 0);
+  int h, w;
+  level_dims(c, H, W, s0, &h, &w);
+  const size_t M0 = (size_t)B * h * w;
+  t.tape.assign(m->mods.size() + 1, nullptr);
+  t.tape[0] = take(M0 * c.channels[std::max(0, s0 - 1)]);
+  size_t elems = 0, stats = 0;
+  walk(m, H, W, nullptr, [&](size_t i, const UMod& u, const Src& in, int hi, int wi, int ho, int wo, int C) {
+    t.tape[i + 1] = take((size_t)B * ho * wo * C);
+    elems = std::max({elems, (size_t)B * hi * wi * (in.c1 + in.c2), (size_t)B * ho * wo * C, (size_t)B * hi * wi * 3 * u.c_out});
+    if (u.kind == M_ATTN) stats = std::max(stats, (size_t)B * hi * wi * std::max(1, u.c_out / 64) * 3);
+  });
+  t.g[0] = take(elems);
+  t.g[1] = take(elems);
+  for (int l = s0; l < c.n_levels - 1; ++l) {
+    int hl, wl;
+    level_dims(c, H, W, l, &hl, &wl);
+    t.gskip[l] = take((size_t)B * hl * wl * c.channels[l]);
+  }
+  t.ga = take(elems);
+  t.gb = take(elems);
+  t.dqkv = take(elems);
+  t.stats = take(stats);
+  t.dss = take((size_t)B * A);
+  t.dcond = take((size_t)B * mw);
+  t.dwcat = take((size_t)A * mw);
+  t.dbcat = take((size_t)A);
+  t.mg = UNetMapGrad{take((size_t)B * mw), take((size_t)B * mw), take((size_t)B * mw), take((size_t)B * mw), take((size_t)B * mw),
+                     take((size_t)B * std::max(1, c.mapping_cond_dim))};
+  t.U = take(M0 * Kout);
+  t.xin = take(M0 * Kin);
+  t.part = take((size_t)kTrainPartFloats);
+  t.total = t.f.total + cv.total();
+}
+
+// The input-gradient weights of every convolution (launch_unet_flip_conv_weight of its tap-major copy), built by the first training call after
+// a finalize into KdbUNet::bwd_mem, in the order of mods
+int ensure_bwd(KdbUNet* m, cudaStream_t st) {
+  if (m->bwd_ready) return 0;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  KDB_CUDA(cudaStreamIsCapturing(st, &cs));
+  KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED,
+              "the first training call after a finalize builds the input-gradient weights: it must run outside CUDA-graph capture");
+  struct Flip { const float* src; int N, C, ks; const float** dst; };
+  std::vector<Flip> flips;
+  for (UMod& u : m->mods) {
+    if (u.kind == M_RES) {
+      flips.push_back({u.w1.f32, u.c_mid, u.c_in, 3, &u.w1t});
+      flips.push_back({u.w2.f32, u.c_out, u.c_mid, 3, &u.w2t});
+      if (u.skip_w.f32 != nullptr) flips.push_back({u.skip_w.f32, u.c_out, u.c_in, 1, &u.skip_t});
+    } else if (u.kind == M_ATTN) {
+      flips.push_back({u.w1.f32, 3 * u.c_out, u.c_out, 1, &u.w1t});
+      flips.push_back({u.w2.f32, u.c_out, u.c_out, 1, &u.w2t});
+    }
+  }
+  while (m->bwd_mem.size() < flips.size()) {   // once per handle: the shapes are the config's
+    const Flip& f = flips[m->bwd_mem.size()];
+    void* p = nullptr;
+    KDB_CUDA(cudaMalloc(&p, sizeof(float) * f.N * f.C * f.ks * f.ks + 1024));
+    m->bwd_mem.push_back(static_cast<float*>(p));
+  }
+  for (size_t i = 0; i < flips.size(); ++i) {
+    const Flip& f = flips[i];
+    if (int rc = launch_unet_flip_conv_weight(f.src, m->bwd_mem[i], f.N, f.C, f.ks, st)) return rc;
+    *f.dst = m->bwd_mem[i];
+  }
+  KDB_CUDA(cudaStreamSynchronize(st));
+  m->bwd_ready = true;
+  return 0;
+}
+
+float* grad_of(const KdbUNet* m, const std::string& key) {
+  auto it = m->grads.find(key);
+  return it == m->grads.end() ? nullptr : const_cast<float*>(it->second.p);
+}
+
+int check_grad_key(const KdbUNet* m, const std::string& k, const std::vector<int64_t>& shape) {
+  auto it = m->tensors.find(k);
+  KDB_REQUIRE(it != m->tensors.end(), KDB_ERR_MISSING_KEY, "gradient bound to '%s', which is no tensor of the model", k.c_str());
+  KDB_REQUIRE(it->second.shape == shape, KDB_ERR_BAD_SHAPE, "gradient of '%s' has the wrong shape", k.c_str());
+  const bool buffer = k == "timestep_embed.weight" || (k.size() >= 7 && k.compare(k.size() - 7, 7, ".kernel") == 0);
+  KDB_REQUIRE(!buffer, KDB_ERR_BAD_ARG, "'%s' is a buffer, not a parameter", k.c_str());
+  const KdbUNetConfig& c = m->cfg;
+  for (int l = 0; l < c.skip_stages; ++l)   // the blocks of the levels below skip_stages, which the forward never runs
+    for (const std::string& p : {"u_net.d_blocks." + std::to_string(l) + ".", "u_net.u_blocks." + std::to_string(c.n_levels - 1 - l) + "."})
+      KDB_REQUIRE(k.compare(0, p.size(), p) != 0, KDB_ERR_BAD_ARG, "'%s' belongs to a block below skip_stages, which the forward never runs",
+                  k.c_str());
+  return 0;
+}
+
+ConvArgs conv_args(const float* in1, int c1, const float* in2, int c2, const float* w, const float* bias, float* out, int N, int B, int h, int wd) {
+  ConvArgs a;
+  a.in1 = in1, a.c1 = c1, a.in2 = in2, a.c2 = c2, a.w = w, a.bias = bias, a.out = out, a.N = N;
+  a.B = B, a.H = h, a.W = wd;
+  return a;
+}
+
+// ResConvBlock in reverse: g the gradient of its output [B, h, w, c_out]; writes that of its input, split as the input (out1: in.c1
+// channels, out2: in.c2), the gradients of its weights and (into t.dss) those of its AdaGN mappers' outputs.  Recomputes n1 = gelu(AdaGN1(x)),
+// h = conv1(n1) and n3 = gelu(AdaGN2(h)) with the forward's launches.
+int res_vjp(KdbUNet* m, const UMod& u, const Src& in, const float* g, float* out1, float* out2, TWs& t, int B, int h, int w, const float* cond,
+            int64_t cbs, cudaStream_t st) {
+  UWs& ws = t.f;
+  const int64_t M = (int64_t)B * h * w;
+  const int A = m->ada_total;
+  const std::string& p = u.prefix;
+  int rc;
+  if ((rc = launch_unet_adagn(in.p1, in.c1, in.p2, in.c2, ws.n1, cond, cbs, u.ada1, u.groups1, true, B, h * w, st)) ||
+      (rc = launch_unet_conv(conv_args(ws.n1, u.c_in, nullptr, 0, u.w1.f32, u.b1, ws.n2, u.c_mid, B, h, w), 3, st)) ||
+      (rc = launch_unet_adagn(ws.n2, u.c_mid, nullptr, 0, ws.qkv, cond, cbs, u.ada2, u.groups2, true, B, h * w, st)))
+    return rc;
+  // conv2: weight and bias gradients, then the gradient of n3 and through AdaGN2 + GELU that of h
+  if ((rc = launch_wgrad_conv(g, u.c_out, ws.qkv, u.c_mid, nullptr, 0, grad_of(m, p + "main.6.weight"), B, h, w, 3, t.part, st)) ||
+      (rc = launch_colsum(g, M, u.c_out, grad_of(m, p + "main.6.bias"), t.part, st)) ||
+      (rc = launch_unet_conv(conv_args(g, u.c_out, nullptr, 0, u.w2t, nullptr, t.ga, u.c_mid, B, h, w), 3, st)) ||
+      (rc = launch_unet_adagn_vjp(ws.n2, u.c_mid, nullptr, 0, t.ga, nullptr, t.gb, nullptr, cond, cbs, u.ada2, t.dss, A, u.groups2, true, B, h * w,
+                                  st)))
+    return rc;
+  // conv1, then the gradient of n1
+  if ((rc = launch_wgrad_conv(t.gb, u.c_mid, ws.n1, u.c_in, nullptr, 0, grad_of(m, p + "main.2.weight"), B, h, w, 3, t.part, st)) ||
+      (rc = launch_colsum(t.gb, M, u.c_mid, grad_of(m, p + "main.2.bias"), t.part, st)) ||
+      (rc = launch_unet_conv(conv_args(t.gb, u.c_mid, nullptr, 0, u.w1t, nullptr, t.ga, u.c_in, B, h, w), 3, st)))
+    return rc;
+  // the skip path's gradient (the 1x1 conv's input gradient, or g itself) is added by AdaGN1's backward
+  const float* add = g;
+  if (u.skip_t != nullptr) {
+    if ((rc = launch_wgrad_conv(g, u.c_out, in.p1, in.c1, in.p2, in.c2, grad_of(m, p + "skip.weight"), B, h, w, 1, t.part, st)) ||
+        (rc = launch_unet_conv(conv_args(g, u.c_out, nullptr, 0, u.skip_t, nullptr, t.gb, u.c_in, B, h, w), 1, st)))
+      return rc;
+    add = t.gb;
+  }
+  return launch_unet_adagn_vjp(in.p1, in.c1, in.p2, in.c2, t.ga, add, out1, out2, cond, cbs, u.ada1, t.dss, A, u.groups1, true, B, h * w, st);
+}
+
+// SelfAttention2d in reverse (x + out_proj(attn(qkv_proj(AdaGN(x))))), as res_vjp.  qkv_proj's q rows carry the folded softmax scale, so
+// the gradients of its unfolded weight and bias rows are those of the folded ones times the scale.
+int attn_vjp(KdbUNet* m, const UMod& u, const float* x, const float* g, float* out, TWs& t, int B, int h, int w, const float* cond, int64_t cbs,
+             cudaStream_t st) {
+  UWs& ws = t.f;
+  const int64_t M = (int64_t)B * h * w;
+  const int C = u.c_out, nh = std::max(1, C / 64);
+  const float scale = 1.f / std::sqrt((float)(C / nh));
+  const std::string& p = u.prefix;
+  float *dwq = grad_of(m, p + "qkv_proj.weight"), *dbq = grad_of(m, p + "qkv_proj.bias");
+  int rc;
+  if ((rc = launch_unet_adagn(x, C, nullptr, 0, ws.n1, cond, cbs, u.ada1, u.groups1, false, B, h * w, st)) ||
+      (rc = launch_unet_conv(conv_args(ws.n1, C, nullptr, 0, u.w1.f32, u.b1, ws.qkv, 3 * C, B, h, w), 1, st)) ||
+      (rc = launch_attention_generic<float>(ws.qkv, ws.ao, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st)))
+    return rc;
+  if ((rc = launch_wgrad_conv(g, C, ws.ao, C, nullptr, 0, grad_of(m, p + "out_proj.weight"), B, h, w, 1, t.part, st)) ||
+      (rc = launch_colsum(g, M, C, grad_of(m, p + "out_proj.bias"), t.part, st)) ||
+      (rc = launch_unet_conv(conv_args(g, C, nullptr, 0, u.w2t, nullptr, t.ga, C, B, h, w), 1, st)) ||
+      (rc = launch_attention_vjp(ws.qkv, ws.ao, t.ga, t.dqkv, t.stats, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st)))
+    return rc;
+  if ((rc = launch_wgrad_conv(t.dqkv, 3 * C, ws.n1, C, nullptr, 0, dwq, B, h, w, 1, t.part, st)) ||
+      (rc = launch_colsum(t.dqkv, M, 3 * C, dbq, t.part, st)) || (rc = launch_unet_scale(dwq, (int64_t)C * C, scale, st)) ||
+      (rc = launch_unet_scale(dbq, C, scale, st)) ||
+      (rc = launch_unet_conv(conv_args(t.dqkv, 3 * C, nullptr, 0, u.w1t, nullptr, t.ga, C, B, h, w), 1, st)))
+    return rc;
+  return launch_unet_adagn_vjp(x, C, nullptr, 0, t.ga, g, out, nullptr, cond, cbs, u.ada1, t.dss, m->ada_total, u.groups1, false, B, h * w, st);
+}
+
+// out = the fp32 forward of F (bit for bit unet_forward's launches, writing the tape), then u^T dF/dparam for every bound parameter by a
+// walk of the modules in reverse: proj_out, the UBlocks (innermost last), the DBlocks, proj_in; then the AdaGN mappers and the mapping network.
+int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sigma, const float* aug, const float* mcond, const float* cond,
+               int64_t cbs, const float* u, float* out, TWs& t, cudaStream_t st) {
+  const KdbUNetConfig& c = m->cfg;
+  int rc = ensure_bwd(m, st);
+  if (rc || (rc = unet_forward(m, KDB_PREC_FP32, B, H, W, x, sigma, 0.f, cond, cbs, out, t.f, st, t.tape.data()))) return rc;
+  const int s0 = c.skip_stages, C0 = c.channels[std::max(0, s0 - 1)], p = c.patch_size;
+  const int Kin = c.in_channels * p * p, Kout = Kin + (c.has_variance ? 1 : 0);
+  int h, w;
+  level_dims(c, H, W, s0, &h, &w);
+  const int64_t M0 = (int64_t)B * h * w;
+  float* part = t.part;
+  // proj_out + pixel_shuffle: U = the patch rows of u, with a zero column for the variance channel the output drops
+  if ((rc = launch_unet_unshuffle(u, t.U, B, c.in_channels, H, W, p, Kout, st)) ||
+      (rc = launch_wgrad(t.U, Kout, t.tape.back(), C0, grad_of(m, "proj_out.weight"), M0, Kout, C0, part, st)) ||
+      (rc = launch_colsum(t.U, M0, Kout, grad_of(m, "proj_out.bias"), part, st)) ||
+      (rc = launch_unet_proj_out_vjp(t.U, m->proj_out_w, t.g[0], M0, Kout, C0, st)))
+    return rc;
+  std::vector<ModIO> io(m->mods.size());
+  walk(m, H, W, t.tape.data(), [&](size_t i, const UMod&, const Src& in, int hi, int wi, int, int, int) { io[i] = ModIO{in, hi, wi}; });
+  int gi = 0;   // t.g[gi]: the gradient of the output of the module being reversed
+  for (size_t k = m->mods.size(); k-- > 0;) {
+    const UMod& mod = m->mods[k];
+    const ModIO& q = io[k];
+    float *g = t.g[gi], *gin = t.g[gi ^ 1];
+    switch (mod.kind) {
+      case M_CONCAT:
+        continue;
+      case M_DOWN:   // its input is the previous level's DBlock output, which the UBlock of that level also read: add that skip gradient
+        rc = launch_unet_resample_vjp(g, t.gskip[mod.level - 1], gin, B, q.h, q.w, q.in.c1, false, st);
+        break;
+      case M_UP:
+        rc = launch_unet_resample_vjp(g, nullptr, gin, B, q.h, q.w, q.in.c1, true, st);
+        break;
+      case M_RES:
+        rc = res_vjp(m, mod, q.in, g, gin, q.in.p2 ? t.gskip[mod.level] : nullptr, t, B, q.h, q.w, cond, cbs, st);
+        break;
+      default:
+        rc = attn_vjp(m, mod, q.in.p1, g, gin, t, B, q.h, q.w, cond, cbs, st);
+    }
+    if (rc) return rc;
+    gi ^= 1;
+  }
+  // proj_in: its input is the pixel_unshuffle of x (the caller's c_in-scaled input)
+  if ((rc = launch_unet_unshuffle(x, t.xin, B, c.in_channels, H, W, p, Kin, st)) ||
+      (rc = launch_wgrad(t.g[gi], C0, t.xin, Kin, grad_of(m, "proj_in.weight"), M0, C0, Kin, part, st)) ||
+      (rc = launch_colsum(t.g[gi], M0, C0, grad_of(m, "proj_in.bias"), part, st)))
+    return rc;
+  // the AdaGN mappers, concatenated as at finalize: one weight gradient over the B conditioning rows, scattered to the bound keys; then the
+  // gradient of the mapping network's output and its backward
+  const int A = m->ada_total, mw = c.mapping_out, mcd = c.mapping_cond_dim;
+  if ((rc = launch_wgrad(t.dss, A, cond + A, cbs, t.dwcat, B, A, mw, part, st)) || (rc = launch_colsum(t.dss, B, A, t.dbcat, part, st))) return rc;
+  for (const UMod& mod : m->mods) {
+    const int n_ada = mod.kind == M_RES ? 2 : (mod.kind == M_ATTN ? 1 : 0);
+    for (int i = 0; i < n_ada; ++i) {
+      const int off = i ? mod.ada2 : mod.ada1, C = i ? mod.c_mid : (mod.kind == M_RES ? mod.c_in : mod.c_out);
+      const std::string key = mod.prefix + (mod.kind == M_ATTN ? "norm_in." : i ? "main.4." : "main.0.");
+      if (float* dw = grad_of(m, key + "mapper.weight"))
+        KDB_CUDA(cudaMemcpyAsync(dw, t.dwcat + (size_t)off * mw, sizeof(float) * 2 * C * mw, cudaMemcpyDeviceToDevice, st));
+      if (float* db = grad_of(m, key + "mapper.bias"))
+        KDB_CUDA(cudaMemcpyAsync(db, t.dbcat + off, sizeof(float) * 2 * C, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  const UNetMapGrad& mg = t.mg;
+  if ((rc = launch_gemm_vjp(t.dss, m->cw.ada_w, t.dcond, B, A, mw, VJP_STORE, 0, 0, 0, st)) ||
+      (rc = launch_unet_mapping_vjp(m->cw, B, sigma, aug, mcond, t.dcond, mg, st)) ||
+      (rc = launch_wgrad(mg.dz1, mw, mg.a0, mw, grad_of(m, "mapping.2.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_colsum(mg.dz1, B, mw, grad_of(m, "mapping.2.bias"), part, st)) ||
+      (rc = launch_wgrad(mg.dz0, mw, mg.h0, mw, grad_of(m, "mapping.0.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_colsum(mg.dz0, B, mw, grad_of(m, "mapping.0.bias"), part, st)))
+    return rc;
+  return mcd > 0 ? launch_wgrad(mg.dh0, mw, mg.v, mcd, grad_of(m, "mapping_cond.weight"), B, mw, mcd, part, st) : 0;
+}
+
+// the grid checks of kdb_unet_forward and kdb_unet_forward_train
+int check_grid(const KdbUNetConfig& c, const char* what, int height, int width) {
+  KDB_REQUIRE(height > 0 && width > 0 && height % c.patch_size == 0 && width % c.patch_size == 0, KDB_ERR_BAD_SHAPE,
+              "%s: %dx%d not divisible by the patch size %d", what, height, width, c.patch_size);
+  for (int l = c.skip_stages; l < c.n_levels; ++l) {
+    int h, w;
+    level_dims(c, height, width, l, &h, &w);
+    const bool down_from = l < c.n_levels - 1;        // this grid is downsampled, and the upsample must restore it
+    KDB_REQUIRE(h >= 2 && w >= 2 && (!down_from || (h % 2 == 0 && w % 2 == 0)), KDB_ERR_BAD_SHAPE,
+                "%s: level %d grid %dx%d (every level but the innermost needs an even grid, every level >= 2x2)", what, l, h, w);
+  }
+  return 0;
 }
 
 }  // namespace
@@ -330,6 +653,7 @@ int kdb_unet_finalize(KdbUNet* m, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   m->free_all();
   m->finalized = false;
+  m->bwd_ready = false;
   m->mods.clear();
   m->ada_total = 0;
   const KdbUNetConfig& c = m->cfg;
@@ -427,19 +751,86 @@ int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width
   KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
               "unet_forward: the fp32, tf32 and fp16 paths are built (precision %d)", precision);
   const KdbUNetConfig& c = m->cfg;
-  KDB_REQUIRE(height > 0 && width > 0 && height % c.patch_size == 0 && width % c.patch_size == 0, KDB_ERR_BAD_SHAPE,
-              "unet_forward: %dx%d not divisible by the patch size %d", height, width, c.patch_size);
-  for (int l = c.skip_stages; l < c.n_levels; ++l) {
-    int h, w;
-    level_dims(c, height, width, l, &h, &w);
-    const bool down_from = l < c.n_levels - 1;        // this grid is downsampled, and the upsample must restore it
-    KDB_REQUIRE(h >= 2 && w >= 2 && (!down_from || (h % 2 == 0 && w % 2 == 0)), KDB_ERR_BAD_SHAPE,
-                "unet_forward: level %d grid %dx%d (every level but the innermost needs an even grid, every level >= 2x2)", l, h, w);
-  }
+  if (int rc = check_grid(c, "unet_forward", height, width)) return rc;
   UWs ws;
   carve(c, batch, height, width, workspace, ws);
   KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward: workspace %zu < required %zu", workspace_bytes, ws.total);
   return m->disarm_tap(unet_forward(m, precision, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream));
+}
+
+int kdb_unet_set_grad(KdbUNet* m, const char* key, float* data, const int64_t* shape, int ndim) {
+  KDB_REQUIRE(m && key && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "unet_set_grad: bad argument");
+  if (data == nullptr) {
+    m->grads.erase(key);
+    return 0;
+  }
+  if (int rc = check_grad_key(m, key, std::vector<int64_t>(shape, shape + ndim))) return rc;
+  ModelCore::TensorRef& t = m->grads[key];
+  t.p = data;
+  t.shape.assign(shape, shape + ndim);
+  return 0;
+}
+
+int64_t kdb_unet_train_workspace_bytes(const KdbUNet* m, int batch, int height, int width) {
+  KDB_REQUIRE(m && batch > 0 && height > 0 && width > 0, KDB_ERR_BAD_ARG, "unet_train_workspace_bytes: bad argument");
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "unet_train_workspace_bytes: model not finalized");
+  TWs t;
+  carve_train(m, batch, height, width, nullptr, t);
+  return (int64_t)t.total;
+}
+
+int kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, const float* aug_cond,
+                           const float* mapping_cond, const float* cond, int64_t cond_batch_stride, const float* cotangent, float* out,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_forward_train: NULL model");
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "unet_forward_train: U-Net training runs at fp32 (precision %d)", precision);
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "unet_forward_train: model not finalized");
+  KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward_train: NULL argument");
+  const KdbUNetConfig& c = m->cfg;
+  KDB_REQUIRE(!(aug_cond && !c.augment_wrapper), KDB_ERR_BAD_ARG, "unet_forward_train: aug_cond needs the augment wrapper");
+  KDB_REQUIRE(!(c.augment_wrapper && c.mapping_cond_dim > 9 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
+              "unet_forward_train: mapping_cond must be given (mapping_cond_dim %d)", c.mapping_cond_dim - 9);
+  KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG,
+              "unet_forward_train: the model takes no mapping_cond");
+  KDB_REQUIRE(cond_batch_stride == kdb_unet_cond_stride(m), KDB_ERR_BAD_ARG,
+              "unet_forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
+              (long long)kdb_unet_cond_stride(m));
+  int rc;
+  for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
+    if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
+  if ((rc = check_grid(c, "unet_forward_train", height, width))) return rc;
+  TWs t;
+  carve_train(m, batch, height, width, workspace, t);
+  KDB_REQUIRE(t.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward_train: workspace %zu < required %zu", workspace_bytes, t.total);
+  return m->disarm_tap(unet_train(m, batch, height, width, x, sigma, aug_cond, mapping_cond, cond, cond_batch_stride, cotangent, out, t,
+                                  (cudaStream_t)stream));
+}
+
+int kdb_unet_conv_wgrad(const float* dy, int n_out, const float* in1, int c1, const float* in2, int c2, float* dw, int batch, int h, int w, int ksize,
+                        float* scratch, void* stream) {
+  KDB_REQUIRE(dy && in1 && dw && scratch && n_out > 0 && c1 > 0 && c2 >= 0 && (c2 == 0 || in2) && batch > 0 && h > 0 && w > 0, KDB_ERR_BAD_ARG,
+              "unet_conv_wgrad: bad argument");
+  KDB_REQUIRE(ksize == 1 || ksize == 3, KDB_ERR_BAD_ARG, "unet_conv_wgrad: kernel size %d", ksize);
+  return launch_wgrad_conv(dy, n_out, in1, c1, in2, c2, dw, batch, h, w, ksize, scratch, (cudaStream_t)stream);
+}
+
+int kdb_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, const float* dy, const float* add, float* dx1, float* dx2,
+                       const float* cond, int64_t cond_batch_stride, int ada_off, float* dcond, int64_t dcond_batch_stride, int groups, int gelu,
+                       int batch, int hw, void* stream) {
+  KDB_REQUIRE(in1 && dy && dx1 && cond && dcond && c1 > 0 && c2 >= 0 && batch > 0 && hw > 0 && ada_off >= 0, KDB_ERR_BAD_ARG,
+              "unet_adagn_vjp: bad argument");
+  return launch_unet_adagn_vjp(in1, c1, in2, c2, dy, add, dx1, dx2, cond, cond_batch_stride, ada_off, dcond, dcond_batch_stride, groups, gelu != 0,
+                               batch, hw, (cudaStream_t)stream);
+}
+
+int kdb_unet_flip_conv_weight(const float* w_tapmajor, float* out, int n_out, int c_in, int ksize, void* stream) {
+  KDB_REQUIRE(w_tapmajor && out && n_out > 0 && c_in > 0 && (ksize == 1 || ksize == 3), KDB_ERR_BAD_ARG, "unet_flip_conv_weight: bad argument");
+  return launch_unet_flip_conv_weight(w_tapmajor, out, n_out, c_in, ksize, (cudaStream_t)stream);
+}
+
+int kdb_unet_resample_vjp(const float* dout, const float* add, float* din, int batch, int h, int w, int c, int up, void* stream) {
+  KDB_REQUIRE(dout && din && batch > 0 && c > 0, KDB_ERR_BAD_ARG, "unet_resample_vjp: bad argument");
+  return launch_unet_resample_vjp(dout, add, din, batch, h, w, c, up != 0, (cudaStream_t)stream);
 }
 
 int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

@@ -85,4 +85,38 @@ int launch_unet_conditioning(const UNetCondWeights& w, int rows, const float* si
 // torch conv weight [N, C, k, k] -> tap-major [N, k*k, C], times `scale` for rows n < scaled_rows (the folded attention scale)
 int launch_unet_reorder_conv_weight(const float* src, float* dst, int N, int C, int ks, int scaled_rows, float scale, cudaStream_t st);
 
+// Backward kernels of the U-Net's training (fp32, deterministic, one writer per output element).
+// The input gradient of a ks x ks convolution (zero padding ks / 2) is the convolution of its output gradient with the weight whose taps are
+// reversed and whose input and output channels are swapped: launch_unet_conv on dst [C, k*k, N] = flip(src [N, k*k, C]) (both tap-major).
+int launch_unet_flip_conv_weight(const float* src, float* dst, int N, int C, int ks, cudaStream_t st);
+// AdaGN (+ GELU) backward: x = [in1 | in2] the AdaGN input, dy [B, HW, c1 + c2] the gradient of its output (after the GELU when gelu), cond
+// rows as launch_adagn.  Writes dx (+ add [B, HW, c1 + c2] when add != NULL; add may alias neither output) split as the input was, to out1
+// (c1 channels) and out2 (c2), and d weight, d bias of the AdaGN's mapper output at dss + b * dss_bs + ada_off (C floats each, the layout of
+// the conditioning row).  Every element of out1, out2 and those dss rows is written.
+int launch_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, const float* dy, const float* add, float* out1, float* out2,
+                          const float* cond, int64_t cond_bs, int ada_off, float* dss, int64_t dss_bs, int groups, bool gelu, int B, int HW,
+                          cudaStream_t st);
+// Adjoint of launch_unet_resample for an input grid H x W: dout [B, H/2, W/2, C] (up = false) or [B, 2H, 2W, C] (up = true) ->
+// din [B, H, W, C] (+ add [B, H, W, C] when add != NULL; add may be din)
+int launch_unet_resample_vjp(const float* dout, const float* add, float* din, int B, int H, int W, int C, bool up, cudaStream_t st);
+// pixel_unshuffle: NCHW x [B, C, H, W] -> token rows out [B (H/p) (W/p), ld], column (c, i, j) (torch's order); columns C p p .. ld - 1 zero
+int launch_unet_unshuffle(const float* x, float* out, int B, int C, int H, int W, int p, int ld, cudaStream_t st);
+// proj_out's input gradient: out [M, K] = U [M, N] w [N, K]
+int launch_unet_proj_out_vjp(const float* U, const float* w, float* out, int64_t M, int N, int K, cudaStream_t st);
+// p[i] *= s for i < n (nothing for p == NULL)
+int launch_unet_scale(float* p, int64_t n, float s, cudaStream_t st);
+// The mapping network's backward (launch_unet_conditioning's h0 -> Linear, GELU, Linear, GELU), one CTA per row.  dcond [rows, mw] the
+// gradient of its output.  Per row: h0, a0 = gelu(z0) the second Linear's input, dz0, dz1 the gradients of the two Linears' outputs, dh0 that
+// of h0 ([rows, mw] each), and v [rows, mcond_dim] the mapping_cond vector (zeros where the conditioning kernel has none).
+struct UNetMapGrad {
+  float *h0, *a0, *dz0, *dz1, *dh0, *v;
+};
+int launch_unet_mapping_vjp(const UNetCondWeights& w, int rows, const float* sigma, const float* aug, const float* mcond, const float* dcond,
+                            const UNetMapGrad& out, cudaStream_t st);
+// The weight gradient of a ks x ks convolution (zero padding ks / 2) in torch's layout: dW [N, c1 + c2, ks, ks] = sum over the pixels m of
+// dY [m, n] times the input [in1 | in2] at pixel m shifted by the tap (zero outside the grid), read in place (train_kernels.cu; wgrad_kernel's
+// chunks and chunk-order sum, part: kTrainPartFloats floats)
+int launch_wgrad_conv(const float* dY, int N, const float* in1, int c1, const float* in2, int c2, float* dW, int B, int H, int W, int ks,
+                      float* part, cudaStream_t st);
+
 }  // namespace kdb

@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 24
+ABI_VERSION = 25
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -102,6 +102,13 @@ SIGNATURES = {
     "kdb_unet_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_unet_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_unet_tap_count": (_i64, [_vp]),
+    "kdb_unet_set_grad": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
+    "kdb_unet_train_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
+    "kdb_unet_forward_train": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_unet_conv_wgrad": (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_unet_adagn_vjp": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_unet_flip_conv_weight": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "kdb_unet_resample_vjp": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_wgrad": (_i32, [_i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_wgrad_patch_in": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_wgrad_patch_out": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
@@ -743,7 +750,8 @@ class Engine:
 
 
 class UNetEngine(Engine):
-    """The image_v1 U-Net at PREC_FP32, PREC_TF32 or PREC_FP16: the Engine calls where the sampler executor makes them; no derivatives."""
+    """The image_v1 U-Net at PREC_FP32, PREC_TF32 or PREC_FP16: the Engine calls where the sampler executor makes them, and the parameter
+    gradients of training at fp32 (forward_train); no derivative with respect to x."""
 
     _api = "unet"
 
@@ -776,6 +784,76 @@ class UNetEngine(Engine):
         return out
 
     forward_jvp = forward_vjp = unet_has_no_derivative
+
+    def train_workspace(self, B, H, W):
+        """kdb_unet_train_workspace_bytes: the workspace of forward_train for B images"""
+        need = int(lib().kdb_unet_train_workspace_bytes(self._h, B, H, W))
+        if need < 0:
+            check(need)
+        return need
+
+    def set_grad(self, grads):
+        """Binds `grads` ({state-dict key: fp32 CUDA tensor of the parameter's shape}) and unbinds every other key bound before."""
+        for k in self._grad_keys - set(grads):
+            check(lib().kdb_unet_set_grad(self._h, k.encode(), None, None, 0))
+        for k, g in grads.items():
+            dims = (_i64 * g.ndim)(*g.shape)
+            check(lib().kdb_unet_set_grad(self._h, k.encode(), ptr(g), dims, g.ndim))
+        self._grad_keys = set(grads)
+
+    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32):
+        """Parameter gradients at fp32 (kdb_unet_forward_train), with Engine.forward_train's arguments: binds `grads`, then out = F(x) and
+        every bound gradient = u^T dF/dparam.  The U-Net takes no class_cond and gives no grad_x."""
+        if class_cond is not None or grad_x is not None:
+            raise ValueError("the image_v1 U-Net takes no class_cond and its training call gives no gradient with respect to x")
+        B, C, H, W = x.shape
+        if tuple(u.shape) != (B, C, H, W):
+            raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {(B, C, H, W)}")
+        out = torch.empty_like(x) if out is None else out
+        self.set_grad(grads)
+        ws = self._reserve(self.train_workspace(B, H, W), x.device)
+        with device_of(x):
+            check(lib().kdb_unet_forward_train(self._h, precision, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(cond),
+                                               self._stride, ptr(u), ptr(out), ptr(ws), ws.numel(), stream()))
+        return out
+
+    def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
+        """The forward of forward_train: kdb_unet_forward at PREC_FP32 (the U-Net trains at fp32 only), bit for bit its `out`."""
+        if precision != PREC_FP32:
+            raise NotImplementedError("the image_v1 U-Net trains at fp32 only")
+        return self.forward(x, sigma, cond, cond_batch_stride, sigma_data, PREC_FP32, out=out)
+
+
+class NativeLoss(torch.autograd.Function):
+    """A training loss through a native engine with respect to the model's parameters (passed after `keys`, their state-dict names).
+    The forward saves the per-element cotangent d loss[b] / d F of the loss kernel; the backward scales it by the incoming gradient of
+    each sample's loss and makes one forward_train on the engine `engine()` returns (the model's, rebound to its current parameters), which
+    writes every parameter's gradient.  Both run at the model's training precision as the forward found it."""
+
+    @staticmethod
+    def forward(ctx, model, engine, ev, kind, noise, sigma_data, weight, keys, *params):
+        x, sig = ev.x, ev.sigma
+        w = None if weight is None else f32c(weight).expand(x.shape[0]).contiguous()
+        xin = loss_noised_input(x, noise, sig, sigma_data)
+        cond = ev.conditioning()
+        precision = getattr(model, "train_precision", PREC_FP32)
+        f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
+        loss, cot = denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
+        aug, cls, mc = ev.cond
+        ctx.model, ctx.engine, ctx.keys, ctx.precision = model, engine, keys, precision
+        ctx.save_for_backward(xin, sig, cond, cot, None if aug is None else f32c(aug),
+                              None if cls is None else cls.to(torch.int64).contiguous(), None if mc is None else f32c(mc))
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        xin, sig, cond, cot, aug, cls, mc = ctx.saved_tensors
+        params = dict(ctx.model.named_parameters())
+        u = cot * f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
+        grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
+        ctx.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads, precision=ctx.precision)
+        return (None,) * 8 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1054,6 +1132,68 @@ def unet_conv_fp16(x1, w, ksize, x2=None, bias=None, r1=None, r2=None, out=None)
     w16 = torch.zeros(*w.shape[:-1], (ct + 7) // 8 * 8, dtype=torch.float16, device=w.device)
     w16[..., :ct] = w
     return _unet_conv(lib().kdb_unet_conv_fp16, x1, w16, ksize, x2, bias, r1, r2, out, w_dtype=torch.float16)
+
+
+@_on_device_of_first
+def unet_conv_wgrad(dy, x1, ksize, x2=None, out=None):
+    """kdb_unet_conv_wgrad: the weight gradient [N, c1 + c2, ksize, ksize] of unet_conv, dy [B, h, w, N] and x1, x2 [B, h, w, c] token-major
+    fp32 contiguous"""
+    require_cuda(dy, x1, x2, out)
+    _fp32_contiguous("unet_conv_wgrad", *(t for t in (dy, x1, x2) if t is not None))
+    B, h, w, N = dy.shape
+    c2 = 0 if x2 is None else x2.shape[-1]
+    if x1.shape[:3] != dy.shape[:3] or (x2 is not None and x2.shape[:3] != dy.shape[:3]):
+        raise ValueError("unet_conv_wgrad: dy and the inputs must share [B, h, w]")
+    out = _out(out, (N, x1.shape[-1] + c2, ksize, ksize), dy, "unet_conv_wgrad")
+    check(lib().kdb_unet_conv_wgrad(ptr(dy), N, ptr(x1), x1.shape[-1], ptr(x2), c2, ptr(out), B, h, w, ksize, ptr(_scratch(dy)), stream()))
+    return out
+
+
+@_on_device_of_first
+def unet_adagn_vjp(x1, dy, cond, ada_off, groups, gelu, x2=None, add=None, dss=None):
+    """kdb_unet_adagn_vjp: x1 [B, h, w, c1] (and x2 [B, h, w, c2]) the AdaGN input, dy the gradient of its output, cond [B, stride] rows ->
+    (dx1, dx2 or None, dss [B, stride]: the mapper-output gradients at ada_off, the rest as passed in or NaN)"""
+    require_cuda(x1, dy, cond, x2, add, dss)
+    _fp32_contiguous("unet_adagn_vjp", *(t for t in (x1, dy, cond, x2, add, dss) if t is not None))
+    B, h, w, c1 = x1.shape
+    c2 = 0 if x2 is None else x2.shape[-1]
+    if tuple(dy.shape) != (B, h, w, c1 + c2) or (add is not None and add.shape != dy.shape) or cond.shape[0] != B:
+        raise ValueError("unet_adagn_vjp: operand shapes do not match")
+    if ada_off < 0 or ada_off + 2 * (c1 + c2) > cond.shape[1]:
+        raise ValueError("unet_adagn_vjp: the (weight, bias) pair lies outside the conditioning row")
+    dx1, dx2 = torch.empty_like(x1), None if x2 is None else torch.empty_like(x2)
+    dss = torch.full_like(cond, float("nan")) if dss is None else dss
+    check(lib().kdb_unet_adagn_vjp(ptr(x1), c1, ptr(x2), c2, ptr(dy), ptr(add), ptr(dx1), ptr(dx2), ptr(cond), cond.shape[1], ada_off, ptr(dss),
+                                   dss.shape[1], groups, int(gelu), B, h * w, stream()))
+    return dx1, dx2, dss
+
+
+@_on_device_of_first
+def unet_flip_conv_weight(w):
+    """kdb_unet_flip_conv_weight: tap-major w [N, ksize^2, C] fp32 -> the input-gradient convolution's weight [C, ksize^2, N]"""
+    require_cuda(w)
+    _fp32_contiguous("unet_flip_conv_weight", w)
+    N, kk, C = w.shape
+    if kk not in (1, 9):
+        raise ValueError(f"unet_flip_conv_weight: {kk} taps")
+    out = torch.empty(C, kk, N, device=w.device, dtype=torch.float32)
+    check(lib().kdb_unet_flip_conv_weight(ptr(w), ptr(out), N, C, 1 if kk == 1 else 3, stream()))
+    return out
+
+
+@_on_device_of_first
+def unet_resample_vjp(dout, h, w, up, add=None):
+    """kdb_unet_resample_vjp: the adjoint of the 2x down- (up = False) or upsampling of an h x w grid, dout [B, h', w', C] -> [B, h, w, C]"""
+    require_cuda(dout, add)
+    _fp32_contiguous("unet_resample_vjp", *(t for t in (dout, add) if t is not None))
+    B, ho, wo, C = dout.shape
+    if (ho, wo) != ((2 * h, 2 * w) if up else (h // 2, w // 2)):
+        raise ValueError(f"unet_resample_vjp: a {ho}x{wo} gradient is not the output grid of a {h}x{w} input")
+    din = torch.empty(B, h, w, C, device=dout.device, dtype=torch.float32)
+    if add is not None and tuple(add.shape) != tuple(din.shape):
+        raise ValueError("unet_resample_vjp: add must have the input's shape")
+    check(lib().kdb_unet_resample_vjp(ptr(dout), ptr(add), ptr(din), B, h, w, C, int(up), stream()))
+    return din
 
 
 def _unet_attention(precision, qkv, h, w, n_heads, d_head):

@@ -112,7 +112,8 @@ class KarrasAugmentWrapper(nn.Module):
         return self
 
     def set_train_precision(self, precision):
-        """The inner model's training precision (image_transformer_v2 only; the U-Net raises NotImplementedError)."""
+        """The inner model's training precision (image_transformer_v2 only; the U-Net, which trains at fp32 only, raises
+        NotImplementedError)."""
         self.inner_model.set_train_precision(precision)
         return self
 
@@ -123,7 +124,7 @@ class KarrasAugmentWrapper(nn.Module):
     def native_loss(self):
         """Denoiser.loss: the inner model's native loss with the wrapper's conditioning, where it has one."""
         if self.is_unet():
-            return _native.unet_has_no_derivative
+            return functools.partial(self.inner_model.native_loss, augment=True)
         return self._native_loss if hasattr(self.inner_model, "native_loss") else None
 
     def _native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, mapping_cond=None, **kwargs):

@@ -10,8 +10,9 @@ class Denoiser(nn.Module):
 
     With an `ImageTransformerDenoiserModelV2` inside, the three scalings are folded into the
     engine's first and last kernels; any other `inner_model` is wrapped with two elementwise
-    kernels (scale-in, combine).  `loss` trains an `ImageTransformerDenoiserModelV2` on the
-    native engine (fp32 parameter gradients) and any other inner model through torch autograd.
+    kernels (scale-in, combine).  `loss` trains an `ImageTransformerDenoiserModelV2` or an
+    `ImageDenoiserModelV1` U-Net on its native engine (parameter gradients) and any other inner
+    model through torch autograd.
     """
 
     def __init__(self, inner_model, sigma_data=1., weighting='karras', scales=1):
@@ -45,8 +46,9 @@ class Denoiser(nn.Module):
 
     def loss(self, input, noise, sigma, **kwargs):
         """Per-sample losses [B] (reference layers.py:76-86, scales == 1).  A native image_transformer_v2 inner model runs one fp32 engine
-        evaluation and one loss kernel, and its backward one native call that writes every parameter's gradient; image_transformer_v1 and
-        the image_v1 U-Net raise NotImplementedError.  Any other inner model runs the reference formula under torch autograd."""
+        evaluation and one loss kernel, and its backward one native call that writes every parameter's gradient; the image_v1 U-Net does the
+        same at exact fp32; image_transformer_v1 raises NotImplementedError.  Any other inner model runs the reference formula under torch
+        autograd."""
         self._check_loss()
         native_loss = getattr(self.inner_model, 'native_loss', None)
         if native_loss is not None:

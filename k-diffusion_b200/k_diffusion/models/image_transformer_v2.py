@@ -248,7 +248,8 @@ class TransformerEngineModel(_native.EngineCache, nn.Module):
         ev = self.native_eval(input, sigma, aug_cond, class_cond, mapping_cond, precision=_native.PREC_FP32)
         named = [(k, p) for k, p in self.named_parameters() if p.requires_grad]
         keys = tuple(k for k, _ in named)
-        return _NativeLoss.apply(self, ev, kind, _native.f32c(noise), float(sigma_data), weight, keys, *(p for _, p in named))
+        return _native.NativeLoss.apply(self, self.engine, ev, kind, _native.f32c(noise), float(sigma_data), weight, keys,
+                                        *(p for _, p in named))
 
     # ------------------------------------------------------------------ forward
     def _check_cond(self, class_cond, mapping_cond):
@@ -388,35 +389,3 @@ def _autograd_eval(model, ev, x, sigma, sigma_data, aug_cond, mapping_cond, out)
     if out is not None:
         raise RuntimeError("out= cannot be used when x requires grad (the result must carry a grad_fn)")
     return _NativeEval.apply(x, model, ev, sigma_data)
-
-
-class _NativeLoss(torch.autograd.Function):
-    """A training loss through the native engine with respect to the model's parameters (passed after `keys`, their state-dict names).
-    The forward saves the per-element cotangent d loss[b] / d F of the loss kernel; the backward scales it by the incoming gradient of
-    each sample's loss and makes one kdb_model_forward_train, which writes every parameter's gradient.  Both run at the model's training
-    precision as the forward found it."""
-
-    @staticmethod
-    def forward(ctx, model, ev, kind, noise, sigma_data, weight, keys, *params):
-        x, sig = ev.x, ev.sigma
-        w = None if weight is None else _native.f32c(weight).expand(x.shape[0]).contiguous()
-        xin = _native.loss_noised_input(x, noise, sig, sigma_data)
-        cond = ev.conditioning()
-        precision = getattr(model, "train_precision", _native.PREC_FP32)
-        f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
-        loss, cot = _native.denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
-        aug, cls, mc = ev.cond
-        ctx.model, ctx.keys, ctx.precision = model, keys, precision
-        ctx.save_for_backward(xin, sig, cond, cot, None if aug is None else _native.f32c(aug),
-                              None if cls is None else cls.to(torch.int64).contiguous(), None if mc is None else _native.f32c(mc))
-        return loss
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_loss):
-        xin, sig, cond, cot, aug, cls, mc = ctx.saved_tensors
-        params = dict(ctx.model.named_parameters())
-        u = cot * _native.f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
-        grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
-        ctx.model.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads, precision=ctx.precision)
-        return (None,) * 7 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)

@@ -2,7 +2,8 @@
 
 Constructor, forward signature and `state_dict()` layout follow the reference (k_diffusion/models/image_v1.py, layers.py:116-313),
 so reference checkpoints load unchanged; the forward pass itself is executed by libkdb200.so (kdb_unet_*).  The torch modules
-below only hold named parameters and buffers: none of their forward methods runs.  Inference only.  Precision: fp32 (the default,
+below only hold named parameters and buffers: none of their forward methods runs.  Parameter gradients (training) come from the engine's
+exact fp32 reverse walk through `Denoiser.loss`; `param_groups` returns the reference's optimizer groups.  Precision: fp32 (the default,
 every kernel exact fp32) or, by set_precision("tf32") or KDB200_PRECISION=tf32, every convolution and the d_head-64 attention on the tensor cores with tf32
 operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True) -- or, by
 set_precision("fp16") or KDB200_PRECISION=fp16, the same with fp16 operands (same significand width, narrower exponent range).
@@ -169,11 +170,46 @@ class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
             raise ValueError(f"the image_v1 U-Net runs at fp32, tf32 or fp16 (resolved precision {p!r})")
         return codes[p]
 
-    def param_groups(self, *args, **kwargs):
-        raise NotImplementedError("training is out of scope for the H100 sampling path")
+    def param_groups(self, base_lr=2e-4):
+        """The reference's two optimizer groups: weight decay for the weights of the mapping network (mapping_cond included) and of the U-Net
+        (the AdaGN mappers included), none for every other parameter."""
+        def decays(name):
+            return name.startswith(("mapping", "u_net")) and name.endswith(".weight")
+        named = list(self.named_parameters())
+        return [
+            {"params": [p for n, p in named if decays(n)], "lr": base_lr},
+            {"params": [p for n, p in named if not decays(n)], "lr": base_lr, "weight_decay": 0.0},
+        ]
 
     def set_train_precision(self, precision):
-        raise NotImplementedError("the image_v1 U-Net has no native training: only its forward is built")
+        """The U-Net trains at exact fp32 only, which `Denoiser.loss` always uses: there is no training precision to select."""
+        raise NotImplementedError("the image_v1 U-Net trains at exact fp32 only (its default): it has no tf32 training precision")
+
+    def _skipped_blocks(self):
+        """State-dict prefixes of the DBlocks and UBlocks of the levels below skip_stages, which the forward never runs (their parameters
+        get no gradient, as under torch autograd)"""
+        n = len(self.depths)
+        return tuple(p for i in range(self.u_net.skip_stages) for p in (f"u_net.d_blocks.{i}.", f"u_net.u_blocks.{n - 1 - i}."))
+
+    def native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, mapping_cond=None, augment=False):
+        """Per-sample training losses [B] of the Karras-preconditioned denoiser around this U-Net (`_native.LOSS_DENOISER` or `LOSS_SIMPLE`,
+        as for image_transformer_v2), with a grad_fn that reaches every parameter requiring grad.  The forward is one fp32 engine evaluation
+        and one loss kernel; the backward is one kdb_unet_forward_train, exact fp32.  `augment`: the loss KarrasAugmentWrapper asks for."""
+        for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
+            if t.requires_grad:
+                raise RuntimeError(f"the native loss differentiates the model's parameters only, but {name} requires grad")
+        if not (input.is_cuda and noise.is_cuda):
+            raise NotImplementedError("the image_v1 U-Net's loss runs on CUDA tensors only: there is no CPU U-Net")
+        _native.require_cuda(noise)
+        if input.ndim != 4 or noise.shape != input.shape:
+            raise ValueError(f"expected input and noise of one shape [B, C, H, W], got {tuple(input.shape)} and {tuple(noise.shape)}")
+        ev = self.native_eval(input, sigma, aug_cond, mapping_cond=mapping_cond, precision=_native.PREC_FP32, augment=augment)
+        # without mapping_cond, a model that forms no mapping_cond vector never uses mapping_cond.weight: no gradient, as under torch
+        unused = self._skipped_blocks() + (("mapping_cond.",) if mapping_cond is None and not augment else ())
+        named = [(k, p) for k, p in self.named_parameters() if p.requires_grad and not k.startswith(unused)]
+        keys = tuple(k for k, _ in named)
+        return _native.NativeLoss.apply(self, lambda: self.engine(augment), ev, kind, _native.f32c(noise), float(sigma_data), weight, keys,
+                                        *(p for _, p in named))
 
     # ------------------------------------------------------------------ native front end
     def native_eval(self, x, sigma=None, aug_cond=None, class_cond=None, mapping_cond=None, precision=None, augment=False):

@@ -9,6 +9,13 @@ torch.backends.cuda.matmul.allow_tf32 = True (what the reference's train.py:101 
     cfg2     the oxford_flowers shifted-window transformer at 64x64, B = 8, soft-min-snr
     cifar10  the reference's config_cifar10_transformer (32x32, patch 2, widths 256 / 512, depths 2 / 4, global attention), B = 128
              (dropout off: the native path trains without dropout)
+    mnist_unet    the reference's config_mnist image_v1 U-Net (28x28), B = 32, through KarrasAugmentWrapper (aug_cond zeros), dropout off
+    cifar10_unet  the reference's config_cifar10 image_v1 U-Net (32x32), B = 128, the same
+
+The U-Net cases have three legs: the native exact fp32 path (one kdb_unet_forward and one kdb_unet_forward_train per step) and the
+oracle's torch eager autograd with TF32 off and with torch.backends.cuda.matmul.allow_tf32 and torch.backends.cudnn.allow_tf32 on; their
+--profile splits a native step's GPU kernel time by kernel: unet_conv_kernel (the forward, the backward's recomputes and every input
+gradient), wgrad_kernel + segsum_kernel (weight and bias gradients), the attention VJP, the AdaGN backward, and the rest.
 
     python tools/train_bench.py [--iters 10] [--rounds 3] [--warmup 3] [--cases cfg1,cifar10] [--profile]
 
@@ -38,6 +45,9 @@ CIFAR10 = {"model": {"type": "image_transformer_v2", "input_channels": 3, "input
                      "loss_weighting": "soft-min-snr", "sigma_data": 0.5},
            "dataset": {"type": "cifar10", "num_classes": 10}}
 CASES = {"cfg1": ("cfg1_mnist_shapes.json", None, 32), "cfg2": ("cfg2_sw256_shapes.json", [64, 64], 8), "cifar10": (None, None, 128)}
+UNET_CASES = {"mnist_unet": ("mnist", 32), "cifar10_unet": ("cifar10", 128)}
+UNET_KERNELS = {"conv (forward, recompute, input gradients)": ("unet_conv_kernel",), "weight and bias gradients": ("wgrad_kernel", "segsum_kernel"),
+                "attention VJP": ("attn_vjp",), "AdaGN backward": ("unet_adagn_vjp_kernel",)}
 GEMM_KERNELS = ("gemm_simt_kernel", "gemm_vjp_kernel", "wgrad_kernel", "wgrad_tf32_kernel", "unet_conv_tc_kernel")
 BUFFERS = ("pos_emb.freqs", "time_emb.weight", "aug_emb.weight")
 
@@ -66,6 +76,9 @@ def main():
     args = ap.parse_args()
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     for name in args.cases.split(","):
+        if name in UNET_CASES:
+            print(json.dumps(unet_case(name, args, gpu)), flush=True)
+            continue
         fixture, size, B = CASES[name]
         cfg = json.loads((ROOT / "tests" / "golden" / fixture).read_text())["config"] if fixture else json.loads(json.dumps(CIFAR10))
         if size:
@@ -154,6 +167,92 @@ def main():
                 gemm += t if any(g in e.key for g in GEMM_KERNELS) else 0.0
             rec["native_fp32_gemm_share"] = gemm / total if total else None
         print(json.dumps(rec), flush=True)
+
+
+def timed_legs(legs, args):
+    for _ in range(args.warmup):
+        for leg in legs.values():
+            leg()
+    ms = {k: [] for k in legs}
+    for _ in range(args.rounds):
+        for k in legs:
+            ms[k].append([])
+        for _ in range(args.iters):
+            for k, leg in legs.items():
+                ms[k][-1].append(step_ms(leg))
+    return ms
+
+
+def unet_case(name, args, gpu):
+    from oracle import unet_oracle as U
+    ref, B = UNET_CASES[name]
+    cfg = json.loads((ROOT / "tests" / "golden" / "unet_configs.json").read_text())[ref]["config"]
+    cfg["model"]["dropout_rate"] = 0.0
+    cfg = K.config.load_config(cfg)
+    m = cfg["model"]
+    model = K.config.make_model(cfg)
+    inner = model.inner_model
+    sd = synth_sd({k: list(v.shape) for k, v in inner.state_dict().items()}, 3)
+    inner.load_state_dict(sd)
+    model = model.cuda().eval()
+    den = K.config.make_denoiser_wrapper(cfg)(model)
+    g = torch.Generator().manual_seed(0)
+    H, W = m["input_size"]
+    x = (torch.randn(B, m["input_channels"], H, W, generator=g) * 0.5).cuda()
+    noise = torch.randn(x.shape, generator=g).cuda()
+    sigma = torch.exp(torch.randn(B, generator=g) * 1.2 - 0.4).cuda()
+    opt = torch.optim.AdamW(inner.param_groups(1e-5), betas=(0.95, 0.999), eps=1e-6, weight_decay=1e-3)
+
+    def native():
+        opt.zero_grad(set_to_none=True)
+        den.loss(x, noise, sigma).mean().backward()
+        opt.step()
+
+    params = {k: v.cuda().requires_grad_(not k.endswith(("timestep_embed.weight", ".kernel"))) for k, v in sd.items()}
+    names = {id(p): k for k, p in inner.named_parameters()}
+    topt = torch.optim.AdamW([dict(g, params=[params[names[id(p)]] for p in g["params"]]) for g in inner.param_groups(1e-5)],
+                             betas=(0.95, 0.999), eps=1e-6, weight_decay=1e-3)
+    sdat = m["sigma_data"]
+
+    def oracle(tf32):
+        torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = tf32
+        topt.zero_grad(set_to_none=True)
+        c_skip, c_out, c_in = [c.view(-1, 1, 1, 1) for c in O.karras_scalings(sigma, sdat)]
+        noised = x + noise * sigma.view(-1, 1, 1, 1)
+        f = U.augment_forward(params, m, noised * c_in, sigma)
+        w = (sigma * sdat) ** 2 / (sigma ** 2 + sdat ** 2) ** 2
+        (((f - (x - c_skip * noised) / c_out) ** 2).flatten(1).mean(1) * w).mean().backward()
+        topt.step()
+        torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+
+    legs = {"native_fp32": native, "torch_eager_fp32": lambda: oracle(False), "torch_eager_tf32": lambda: oracle(True)}
+    ms = timed_legs(legs, args)
+
+    def refinalize():
+        with torch.no_grad():
+            next(inner.parameters()).add_(0.0)
+        inner.engine(True)
+    refinalize()
+    rec = dict(case=name, batch=B, size=[H, W], **{f"{k}_ms": stats(sum(v, [])) for k, v in ms.items()},
+               round_medians={k: [stats(r)["median"] for r in v] for k, v in ms.items()},
+               refinalize_ms=dict(fp32=stats([step_ms(refinalize) for _ in range(5)])["median"]), gpu=gpu)
+    if args.profile:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(3):
+                native()
+            torch.cuda.synchronize()
+        share = {k: 0.0 for k in UNET_KERNELS}
+        total = 0.0
+        for e in prof.key_averages():
+            t = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
+            total += t
+            for k, pats in UNET_KERNELS.items():
+                if any(p in e.key for p in pats):
+                    share[k] += t
+                    break
+        rec["native_fp32_kernel_share"] = {k: v / total for k, v in share.items()} if total else None
+    return rec
 
 
 if __name__ == "__main__":
