@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 25
+#define KDB_ABI_VERSION 26
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -524,7 +524,16 @@ int kdb_unet_conv(const float* in1, int c1, const float* in2, int c2, const floa
  *   not NULL; add [batch, hw, c1 + c2] may alias neither output) to dx1 (c1 channels) and dx2 (c2), and the gradients of the weight and bias
  *   rows to dcond + b * dcond_batch_stride + ada_off (c1 + c2 floats each).
  * kdb_unet_resample_vjp: the adjoint of the 2x resampling of an h x w grid (h, w >= 2), reflect padding included: dout [batch, h/2, w/2, c]
- *   (up = 0) or [batch, 2h, 2w, c] (up = 1) -> din [batch, h, w, c] (+ add when not NULL; add may be din). */
+ *   (up = 0) or [batch, 2h, 2w, c] (up = 1) -> din [batch, h, w, c] (+ add when not NULL; add may be din).
+ * kdb_unet_mapping_vjp: the mapping network's backward of a finalized U-Net, one row per image: sigma [rows], aug_cond and mapping_cond as
+ *   kdb_unet_conditioning takes them, dcond [rows, mapping_out] the gradient of the mapping network's output.  Writes, [rows, mapping_out]
+ *   each, h0 (Fourier features + the mapping_cond Linear), a0 (the second Linear's input), dz0 and dz1 (the gradients of the two Linears'
+ *   outputs) and dh0 (that of h0), and v [rows, mapping_cond_dim] (the mapping_cond vector, zeros where the model has none; v may be NULL
+ *   when mapping_cond_dim is 0).  It needs (6 mapping_out + mapping_cond_dim) floats of shared memory, at most 48 KiB: a wider model
+ *   returns KDB_ERR_UNSUPPORTED.
+ * kdb_unet_proj_out_vjp: proj_out's input gradient, out [rows, k] = u [rows, n] w [n, k].
+ * kdb_unet_unshuffle: pixel_unshuffle of an NCHW x [batch, c, h, w] (h, w multiples of p) to token rows out [batch (h/p) (w/p), ld], column
+ *   (c, i, j) in torch's order; columns c p p .. ld - 1 are zero. */
 int kdb_unet_conv_wgrad(const float* dy, int n_out, const float* in1, int c1, const float* in2, int c2, float* dw, int batch, int h, int w,
                         int ksize, float* scratch, void* stream);
 int kdb_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, const float* dy, const float* add, float* dx1, float* dx2,
@@ -532,6 +541,10 @@ int kdb_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, const
                        int batch, int hw, void* stream);
 int kdb_unet_flip_conv_weight(const float* w_tapmajor, float* out, int n_out, int c_in, int ksize, void* stream);
 int kdb_unet_resample_vjp(const float* dout, const float* add, float* din, int batch, int h, int w, int c, int up, void* stream);
+int kdb_unet_mapping_vjp(const KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, const float* dcond,
+                         float* h0, float* a0, float* dz0, float* dz1, float* dh0, float* v, void* stream);
+int kdb_unet_proj_out_vjp(const float* u, const float* w, float* out, int64_t rows, int n, int k, void* stream);
+int kdb_unet_unshuffle(const float* x, float* out, int batch, int c, int h, int w, int p, int ld, void* stream);
 
 /* The same convolution, arguments and layouts on the tensor cores (wgmma, the kernel kdb_unet_forward runs at KDB_PREC_TF32): the
  * products take tf32 operands -- the low 13 mantissa bits of every input and weight element are ignored (truncation), so a caller

@@ -612,6 +612,15 @@ int check_grid(const KdbUNetConfig& c, const char* what, int height, int width) 
   return 0;
 }
 
+// the aug_cond / mapping_cond checks of kdb_unet_conditioning, kdb_unet_forward_train and kdb_unet_mapping_vjp
+int check_conds(const KdbUNetConfig& c, const char* what, const float* aug_cond, const float* mapping_cond) {
+  KDB_REQUIRE(!(aug_cond && !c.augment_wrapper), KDB_ERR_BAD_ARG, "%s: aug_cond needs the augment wrapper", what);
+  KDB_REQUIRE(!(c.augment_wrapper && c.mapping_cond_dim > 9 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
+              "%s: mapping_cond must be given (mapping_cond_dim %d)", what, c.mapping_cond_dim - 9);
+  KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG, "%s: the model takes no mapping_cond", what);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -726,12 +735,7 @@ int kdb_unet_conditioning(KdbUNet* m, int rows, const float* sigma, const float*
                           void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_conditioning: model NULL or not finalized");
   KDB_REQUIRE(rows > 0 && sigma && cond_out, KDB_ERR_BAD_ARG, "unet_conditioning: bad arguments");
-  const KdbUNetConfig& c = m->cfg;
-  KDB_REQUIRE(!(aug_cond && !c.augment_wrapper), KDB_ERR_BAD_ARG, "unet_conditioning: aug_cond needs the augment wrapper");
-  KDB_REQUIRE(!(c.augment_wrapper && c.mapping_cond_dim > 9 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
-              "unet_conditioning: mapping_cond must be given (mapping_cond_dim %d)", c.mapping_cond_dim - 9);
-  KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG,
-              "unet_conditioning: the model takes no mapping_cond");
+  if (int rc = check_conds(m->cfg, "unet_conditioning", aug_cond, mapping_cond)) return rc;
   return launch_unet_conditioning(m->cw, rows, sigma, aug_cond, mapping_cond, cond_out, kdb_unet_cond_stride(m), (cudaStream_t)stream);
 }
 
@@ -787,15 +791,11 @@ int kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int
   KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "unet_forward_train: model not finalized");
   KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward_train: NULL argument");
   const KdbUNetConfig& c = m->cfg;
-  KDB_REQUIRE(!(aug_cond && !c.augment_wrapper), KDB_ERR_BAD_ARG, "unet_forward_train: aug_cond needs the augment wrapper");
-  KDB_REQUIRE(!(c.augment_wrapper && c.mapping_cond_dim > 9 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
-              "unet_forward_train: mapping_cond must be given (mapping_cond_dim %d)", c.mapping_cond_dim - 9);
-  KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG,
-              "unet_forward_train: the model takes no mapping_cond");
+  int rc;
+  if ((rc = check_conds(c, "unet_forward_train", aug_cond, mapping_cond))) return rc;
   KDB_REQUIRE(cond_batch_stride == kdb_unet_cond_stride(m), KDB_ERR_BAD_ARG,
               "unet_forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
               (long long)kdb_unet_cond_stride(m));
-  int rc;
   for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
     if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
   if ((rc = check_grid(c, "unet_forward_train", height, width))) return rc;
@@ -831,6 +831,26 @@ int kdb_unet_flip_conv_weight(const float* w_tapmajor, float* out, int n_out, in
 int kdb_unet_resample_vjp(const float* dout, const float* add, float* din, int batch, int h, int w, int c, int up, void* stream) {
   KDB_REQUIRE(dout && din && batch > 0 && c > 0, KDB_ERR_BAD_ARG, "unet_resample_vjp: bad argument");
   return launch_unet_resample_vjp(dout, add, din, batch, h, w, c, up != 0, (cudaStream_t)stream);
+}
+
+int kdb_unet_mapping_vjp(const KdbUNet* m, int rows, const float* sigma, const float* aug_cond, const float* mapping_cond, const float* dcond,
+                         float* h0, float* a0, float* dz0, float* dz1, float* dh0, float* v, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_mapping_vjp: model NULL or not finalized");
+  KDB_REQUIRE(rows > 0 && sigma && dcond && h0 && a0 && dz0 && dz1 && dh0 && (v || m->cfg.mapping_cond_dim == 0), KDB_ERR_BAD_ARG,
+              "unet_mapping_vjp: bad argument");
+  if (int rc = check_conds(m->cfg, "unet_mapping_vjp", aug_cond, mapping_cond)) return rc;
+  return launch_unet_mapping_vjp(m->cw, rows, sigma, aug_cond, mapping_cond, dcond, UNetMapGrad{h0, a0, dz0, dz1, dh0, v}, (cudaStream_t)stream);
+}
+
+int kdb_unet_proj_out_vjp(const float* u, const float* w, float* out, int64_t rows, int n, int k, void* stream) {
+  KDB_REQUIRE(u && w && out && rows > 0 && n > 0 && k > 0, KDB_ERR_BAD_ARG, "unet_proj_out_vjp: bad argument");
+  return launch_unet_proj_out_vjp(u, w, out, rows, n, k, (cudaStream_t)stream);
+}
+
+int kdb_unet_unshuffle(const float* x, float* out, int batch, int c, int h, int w, int p, int ld, void* stream) {
+  KDB_REQUIRE(x && out && batch > 0 && c > 0 && p > 0 && h > 0 && w > 0 && h % p == 0 && w % p == 0 && ld >= c * p * p, KDB_ERR_BAD_ARG,
+              "unet_unshuffle: bad argument");
+  return launch_unet_unshuffle(x, out, batch, c, h, w, p, ld, (cudaStream_t)stream);
 }
 
 int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

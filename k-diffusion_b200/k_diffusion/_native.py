@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 25
+ABI_VERSION = 26
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -109,6 +109,9 @@ SIGNATURES = {
     "kdb_unet_adagn_vjp": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_flip_conv_weight": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_unet_resample_vjp": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_unet_mapping_vjp": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "kdb_unet_proj_out_vjp": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp]),
+    "kdb_unet_unshuffle": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "kdb_wgrad": (_i32, [_i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_wgrad_patch_in": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_wgrad_patch_out": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
@@ -785,6 +788,25 @@ class UNetEngine(Engine):
 
     forward_jvp = forward_vjp = unet_has_no_derivative
 
+    def mapping_vjp(self, sigma, dcond, aug_cond=None, mapping_cond=None, out=None):
+        """kdb_unet_mapping_vjp: the mapping network's backward for sigma [rows] and dcond [rows, mapping_out] (the gradient of its output)
+        -> dict of h0, a0, dz0, dz1, dh0 [rows, mapping_out] and v [rows, mapping_cond_dim].  out: such a dict of buffers to write."""
+        require_cuda(sigma, dcond, aug_cond, mapping_cond)
+        rows, mw, mcd = sigma.numel(), self.cfg.mapping_out, self.cfg.mapping_cond_dim
+        _fp32_contiguous("unet_mapping_vjp", *(t for t in (sigma, dcond, aug_cond, mapping_cond) if t is not None))
+        user = mcd - (9 if self.cfg.augment_wrapper else 0)
+        if (tuple(dcond.shape) != (rows, mw) or (aug_cond is not None and tuple(aug_cond.shape) != (rows, 9))
+                or (mapping_cond is not None and tuple(mapping_cond.shape) != (rows, user))):
+            raise ValueError("unet_mapping_vjp: operand shapes do not match")
+        out = {} if out is None else out
+        res = {k: _out(out.get(k), (rows, mw), dcond, "unet_mapping_vjp") for k in ("h0", "a0", "dz0", "dz1", "dh0")}
+        res["v"] = _out(out.get("v"), (rows, mcd), dcond, "unet_mapping_vjp") if mcd else None
+        require_cuda(*res.values())
+        with device_of(sigma):
+            check(lib().kdb_unet_mapping_vjp(self._h, rows, ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(dcond),
+                                             *(ptr(res[k]) for k in ("h0", "a0", "dz0", "dz1", "dh0", "v")), stream()))
+        return res
+
     def train_workspace(self, B, H, W):
         """kdb_unet_train_workspace_bytes: the workspace of forward_train for B images"""
         need = int(lib().kdb_unet_train_workspace_bytes(self._h, B, H, W))
@@ -1150,18 +1172,22 @@ def unet_conv_wgrad(dy, x1, ksize, x2=None, out=None):
 
 
 @_on_device_of_first
-def unet_adagn_vjp(x1, dy, cond, ada_off, groups, gelu, x2=None, add=None, dss=None):
+def unet_adagn_vjp(x1, dy, cond, ada_off, groups, gelu, x2=None, add=None, dss=None, out=None):
     """kdb_unet_adagn_vjp: x1 [B, h, w, c1] (and x2 [B, h, w, c2]) the AdaGN input, dy the gradient of its output, cond [B, stride] rows ->
-    (dx1, dx2 or None, dss [B, stride]: the mapper-output gradients at ada_off, the rest as passed in or NaN)"""
+    (dx1, dx2 or None, dss [B, stride]: the mapper-output gradients at ada_off, the rest as passed in or NaN).  out: (dx1, dx2 or None)
+    buffers to write, of x1's and x2's shapes."""
     require_cuda(x1, dy, cond, x2, add, dss)
     _fp32_contiguous("unet_adagn_vjp", *(t for t in (x1, dy, cond, x2, add, dss) if t is not None))
     B, h, w, c1 = x1.shape
     c2 = 0 if x2 is None else x2.shape[-1]
     if tuple(dy.shape) != (B, h, w, c1 + c2) or (add is not None and add.shape != dy.shape) or cond.shape[0] != B:
         raise ValueError("unet_adagn_vjp: operand shapes do not match")
-    if ada_off < 0 or ada_off + 2 * (c1 + c2) > cond.shape[1]:
+    if ada_off < 0 or any(t is not None and (t.shape[0] != B or ada_off + 2 * (c1 + c2) > t.shape[1]) for t in (cond, dss)):
         raise ValueError("unet_adagn_vjp: the (weight, bias) pair lies outside the conditioning row")
-    dx1, dx2 = torch.empty_like(x1), None if x2 is None else torch.empty_like(x2)
+    o1, o2 = (None, None) if out is None else out
+    dx1 = _out(o1, x1.shape, x1, "unet_adagn_vjp")
+    dx2 = None if x2 is None else _out(o2, x2.shape, x2, "unet_adagn_vjp")
+    require_cuda(dx1, dx2)
     dss = torch.full_like(cond, float("nan")) if dss is None else dss
     check(lib().kdb_unet_adagn_vjp(ptr(x1), c1, ptr(x2), c2, ptr(dy), ptr(add), ptr(dx1), ptr(dx2), ptr(cond), cond.shape[1], ada_off, ptr(dss),
                                    dss.shape[1], groups, int(gelu), B, h * w, stream()))
@@ -1182,18 +1208,47 @@ def unet_flip_conv_weight(w):
 
 
 @_on_device_of_first
-def unet_resample_vjp(dout, h, w, up, add=None):
-    """kdb_unet_resample_vjp: the adjoint of the 2x down- (up = False) or upsampling of an h x w grid, dout [B, h', w', C] -> [B, h, w, C]"""
-    require_cuda(dout, add)
+def unet_resample_vjp(dout, h, w, up, add=None, out=None):
+    """kdb_unet_resample_vjp: the adjoint of the 2x down- (up = False) or upsampling of an h x w grid, dout [B, h', w', C] -> [B, h, w, C]
+    (+ add, which may be out itself)"""
+    require_cuda(dout, add, out)
     _fp32_contiguous("unet_resample_vjp", *(t for t in (dout, add) if t is not None))
     B, ho, wo, C = dout.shape
     if (ho, wo) != ((2 * h, 2 * w) if up else (h // 2, w // 2)):
         raise ValueError(f"unet_resample_vjp: a {ho}x{wo} gradient is not the output grid of a {h}x{w} input")
-    din = torch.empty(B, h, w, C, device=dout.device, dtype=torch.float32)
+    din = _out(out, (B, h, w, C), dout, "unet_resample_vjp")
     if add is not None and tuple(add.shape) != tuple(din.shape):
         raise ValueError("unet_resample_vjp: add must have the input's shape")
     check(lib().kdb_unet_resample_vjp(ptr(dout), ptr(add), ptr(din), B, h, w, C, int(up), stream()))
     return din
+
+
+@_on_device_of_first
+def unet_proj_out_vjp(u, w, out=None):
+    """kdb_unet_proj_out_vjp: proj_out's input gradient u [M, N] @ w [N, K] -> [M, K], u and w contiguous fp32"""
+    require_cuda(u, w, out)
+    _fp32_contiguous("unet_proj_out_vjp", u, w)
+    (M, N), K = u.shape, w.shape[-1]
+    if w.ndim != 2 or w.shape[0] != N:
+        raise ValueError(f"unet_proj_out_vjp: u {tuple(u.shape)} and w {tuple(w.shape)} do not chain")
+    out = _out(out, (M, K), u, "unet_proj_out_vjp")
+    check(lib().kdb_unet_proj_out_vjp(ptr(u), ptr(w), ptr(out), M, N, K, stream()))
+    return out
+
+
+@_on_device_of_first
+def unet_unshuffle(x, p, ld=None, out=None):
+    """kdb_unet_unshuffle: pixel_unshuffle of an NCHW x [B, C, H, W] fp32 -> token rows [B (H/p) (W/p), ld], column (c, i, j);
+    ld defaults to C p p, columns past it are zero"""
+    require_cuda(x, out)
+    _fp32_contiguous("unet_unshuffle", x)
+    B, C, H, W = x.shape
+    ld = C * p * p if ld is None else ld
+    if p < 1 or H % p or W % p or ld < C * p * p:
+        raise ValueError(f"unet_unshuffle: {H}x{W} by {p} into rows of {ld}")
+    out = _out(out, (B * (H // p) * (W // p), ld), x, "unet_unshuffle")
+    check(lib().kdb_unet_unshuffle(ptr(x), ptr(out), B, C, H, W, p, ld, stream()))
+    return out
 
 
 def _unet_attention(precision, qkv, h, w, n_heads, d_head):

@@ -104,6 +104,20 @@ CASES = [g + (e, nh, B, s) for i, g in enumerate(GEOMETRIES)
          for e, nh, B, s in [((8, 32, 64, 128)[i % 4], (1, 3)[i // 4 % 2], (1, 3)[i // 2 % 2], (10.0, 50.0)[i % 2])]]
 
 
+# The image_v1 U-Net's self-attention (layers.py:193-200): d_head = C / max(1, C / 64), so 36 (C < 64), 68 and 96 at the edge configs' widths,
+# with unnormalised gaussian q and k and the softmax scale 1 / sqrt(d_head) folded into q (s = 0 marks these), on its 7x7, 16x16 and 32x32 grids
+UNET_CASES = [("global", h, h, 0, 0, e, nh, B, 0.0) for (h, e, nh, B) in [(7, 36, 1, 3), (16, 68, 2, 2), (32, 96, 2, 1), (7, 96, 1, 2),
+                                                                           (16, 36, 1, 1), (32, 68, 1, 1)]]
+CASES += UNET_CASES
+
+
+def make_unet_qkv(B, T, nh, e, seed):
+    g = torch.Generator().manual_seed(seed)
+    t = torch.randn(B, T, 3, nh, e, generator=g, dtype=torch.float64)
+    t[:, :, 0] /= e ** 0.5
+    return t.float().reshape(B, T, 3 * nh * e)
+
+
 def _id(c):
     return f"{c[0]}-{c[1]}x{c[2]}-p{c[3]}-s{c[4]}-e{c[5]}-nh{c[6]}-B{c[7]}-scale{int(c[8])}"
 
@@ -117,7 +131,7 @@ def check_near_zero(got, want_scale, what):
 def test_derivatives_vs_float64_oracle(kind, h, w, param, shift, e, nh, B, s):
     T = h * w
     seed = h * 1000 + w * 10 + param + shift + e
-    qkv = make_qkv(B, T, nh, e, s, seed)
+    qkv = make_qkv(B, T, nh, e, s, seed) if s else make_unet_qkv(B, T, nh, e, seed)
     g = torch.Generator().manual_seed(seed + 1)
     dqkv = torch.randn(qkv.shape, generator=g)
     dout = torch.randn(B, T, nh * e, generator=g)
@@ -132,7 +146,7 @@ def test_derivatives_vs_float64_oracle(kind, h, w, param, shift, e, nh, B, s):
     dv_scale = float(thirds(want_g, nh, e)[2].abs().max())
     for name, got, want in zip(("dq", "dk", "dv"), thirds(gq, nh, e), thirds(want_g, nh, e)):
         if float(want.norm()) == 0:
-            check_near_zero(got, dv_scale * (s * e) ** 0.5, name)
+            check_near_zero(got, dv_scale * (max(s, 1.0) * e) ** 0.5, name)
         else:
             check_tangent(got, want, name)
 
@@ -184,12 +198,13 @@ def test_support_is_exactly_the_mask(kind, h, w, param, shift):
                                                   f"key {b} is seen by {allow[:, b].nonzero().flatten().tolist()}")
 
 
-def test_shared_memory_budget_edge():
-    """64x66 = 4224 tokens at d_head 64: 4 warps x (2 e + 3 T) floats = 200 KiB, the per-key pass's and the JVP's whole budget.  It runs and
-    matches; at 65x65 both entry points refuse with KDB_ERR_UNSUPPORTED and launch nothing."""
-    h, w, nh, e, s = 64, 66, 1, 64, 10.0
+def _budget_edge(h, w, e, refused, qkv_of):
+    """global attention on h x w tokens, the most the per-key pass (and the JVP) accepts at d_head e, runs and matches; on the grid
+    `refused`, one token more, both entry points refuse with KDB_ERR_UNSUPPORTED and launch nothing"""
+    nh = 1
     T = h * w
-    qkv = make_qkv(1, T, nh, e, s, 5)
+    assert 4 * 4 * (2 * e + 3 * T) <= 200 * 1024 < 4 * 4 * (2 * e + 3 * (T + 1)) and refused[0] * refused[1] == T + 1
+    qkv = qkv_of(T)
     g = torch.Generator().manual_seed(6)
     dqkv = torch.randn(qkv.shape, generator=g)
     dout = torch.randn(1, T, nh * e, generator=g)
@@ -203,7 +218,7 @@ def test_shared_memory_budget_edge():
     for name, got, want in zip(("dq", "dk", "dv"), thirds(gq, nh, e), thirds(want_g, nh, e)):
         check_tangent(got, want, name)
 
-    h = w = 65
+    h, w = refused
     T = h * w
     qkv = torch.zeros(1, T, 3 * nh * e, device=DEV)
     out, stats = torch.zeros(1, T, nh * e, device=DEV), torch.zeros(1, nh, T, 3, device=DEV)
@@ -217,3 +232,15 @@ def test_shared_memory_budget_edge():
     assert _native.launch_count() == n0
     with pytest.raises(RuntimeError, match="shared-memory"):
         _native.attention_jvp(qkv, qkv, h, w, nh, e, "global")
+
+
+def test_shared_memory_budget_edge():
+    """64x66 = 4224 tokens at d_head 64: 4 warps x (2 e + 3 T) floats = 200 KiB, the per-key pass's and the JVP's whole budget.  It runs and
+    matches; at 65x65 both entry points refuse with KDB_ERR_UNSUPPORTED and launch nothing."""
+    _budget_edge(64, 66, 64, (65, 65), lambda T: make_qkv(1, T, 1, 64, 10.0, 5))
+
+
+def test_shared_memory_budget_edge_at_unet_head_width():
+    """The same edge at d_head 96, the widest head of the U-Net's edge configs, on U-Net-style q and k: 22x191 = 4202 tokens fill the budget,
+    3x1401 = 4203 are refused"""
+    _budget_edge(22, 191, 96, (3, 1401), lambda T: make_unet_qkv(1, T, 1, 96, 5))

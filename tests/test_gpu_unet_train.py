@@ -67,12 +67,12 @@ def native_grads(model, inner, x, noise, sigma, kw, gw):
     return loss.detach().cpu(), {k: p.grad.detach().cpu().clone() for k, p in inner.named_parameters() if p.grad is not None}
 
 
-def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False):
-    """layers.py:76-86 (or :107-111) around the oracle's U-Net, autograd on the CPU"""
+def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False, device="cpu"):
+    """layers.py:76-86 (or :107-111) around the oracle's U-Net, autograd on `device` (losses and gradients returned on the CPU)"""
     m = cfg["model"]
-    params = {k: v.to(dtype).requires_grad_(not k.endswith(BUFFERS)) for k, v in sd.items()}
-    x, noise, sigma, gw = x.to(dtype), noise.to(dtype), sigma.to(dtype), gw.to(dtype)
-    kw = {k: v.to(dtype) for k, v in kw.items()}
+    params = {k: v.to(device, dtype).requires_grad_(not k.endswith(BUFFERS)) for k, v in sd.items()}
+    x, noise, sigma, gw = (t.to(device, dtype) for t in (x, noise, sigma, gw))
+    kw = {k: v.to(device, dtype) for k, v in kw.items()}
     sd_ = m["sigma_data"]
     c_skip, c_out, c_in = [c.view(-1, 1, 1, 1) for c in O.karras_scalings(sigma, sd_)]
     s4 = sigma.view(-1, 1, 1, 1)
@@ -86,15 +86,15 @@ def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False):
         w = (sigma * sd_) ** 2 / (sigma ** 2 + sd_ ** 2) ** 2 if m["loss_weighting"] == "soft-min-snr" else torch.ones_like(sigma)
         loss = ((f - (x - c_skip * noised) / c_out) ** 2).flatten(1).mean(1) * w
     (loss * gw).sum().backward()
-    return loss.detach(), {k: p.grad for k, p in params.items() if p.requires_grad and p.grad is not None}
+    return loss.detach().cpu(), {k: p.grad.cpu() for k, p in params.items() if p.requires_grad and p.grad is not None}
 
 
-def check_against_oracle(cfg, sd, got_loss, got, x, noise, sigma, kw, gw, simple=False, budget=None):
+def check_against_oracle(cfg, sd, got_loss, got, x, noise, sigma, kw, gw, simple=False, budget=None, device="cpu"):
     """Each native gradient within 8x the fp32-vs-float64 distance of the oracle's gradient, plus 1e-6 relative; exactly 0 where the
     float64 gradient is exactly 0.  The key rows of qkv_proj's bias are left out of the zero check: softmax does not change when one key
     bias is added to every score of a query, so their gradient is 0 only through cancellation, which fp32 leaves at rounding level."""
-    l64, g64 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float64, simple)
-    l32, g32 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float32, simple)
+    l64, g64 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float64, simple, device)
+    l32, g32 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float32, simple, device)
     assert torch.allclose(got_loss.double(), l64, rtol=1e-4, atol=0)
     assert set(got) == set(g64), set(got) ^ set(g64)
     for k, want in g64.items():
@@ -138,6 +138,49 @@ def test_reference_configs_gradients_match_float64(name):
     loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
     assert set(got) == {k for k, p in inner.named_parameters()}
     check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+@pytest.fixture(scope="module")
+def no_tf32():
+    """cuDNN convolutions and cuBLAS matmuls at full fp32 for the oracle on the GPU: under TF32 (operands rounded to 2^-11 instead of 2^-24)
+    its fp32-vs-float64 distance, and with it the gate, would loosen by three to four orders of magnitude"""
+    saved = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    yield
+    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = saved
+
+
+@pytest.mark.parametrize("name", ["mnist", "cifar10"])
+def test_reference_configs_at_the_training_batch_size(name, no_tf32):
+    """train.py's default batch of 64, where every level's weight gradients run several row chunks: every gradient within 8x the oracle's
+    fp32 distance (the oracle run on the GPU in float64 and fp32); every element of every gradient written through forward_train into NaN;
+    the batch equal to the float64 sum of eight batches of 8; two calls bit-identical"""
+    assert not torch.backends.cudnn.allow_tf32 and not torch.backends.cuda.matmul.allow_tf32
+    cfg, inner, sd, model = build(CONFIGS[name]["config"])
+    B = 64
+    x, noise, sigma, kw, gw = inputs(cfg, B, 15)
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    assert set(got) == {k for k, p in inner.named_parameters()}
+    check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw, device="cuda")
+
+    l2, again = native_grads(model, inner, x, noise, sigma, kw, gw)
+    assert torch.equal(loss, l2) and all(torch.equal(got[k], again[k]) for k in got), "two calls differ"
+
+    parts = [native_grads(model, inner, x[i:i + 8], noise[i:i + 8], sigma[i:i + 8], {k: v[i:i + 8] for k, v in kw.items()}, gw[i:i + 8])[1]
+             for i in range(0, B, 8)]
+    for k in got:
+        total = sum(p[k].double() for p in parts)
+        assert (got[k].double() - total).norm().item() <= 1e-5 * total.norm().item() + 1e-7, k
+
+    augment = cfg["model"].get("augment_wrapper", True)
+    kwc = {k: v.cuda() for k, v in kw.items()}
+    ev = inner.native_eval(x.cuda(), sigma.cuda(), kwc.get("aug_cond"), mapping_cond=kwc.get("mapping_cond"), precision=K._native.PREC_FP32,
+                           augment=augment)
+    grads = {k: torch.full_like(p, float("nan")) for k, p in inner.named_parameters()}
+    ev.engine.forward_train(ev.x, torch.randn_like(ev.x), ev.sigma, *ev.cond, ev.conditioning(), grads)
+    torch.cuda.synchronize()
+    for k, g in grads.items():
+        assert torch.isfinite(g).all(), f"{k}: {int((~torch.isfinite(g)).sum())} elements not written"
 
 
 def test_reference_init_leaves_only_proj_out_nonzero():
