@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 26
+#define KDB_ABI_VERSION 27
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -545,6 +545,58 @@ int kdb_unet_mapping_vjp(const KdbUNet* m, int rows, const float* sigma, const f
                          float* h0, float* a0, float* dz0, float* dz1, float* dh0, float* v, void* stream);
 int kdb_unet_proj_out_vjp(const float* u, const float* w, float* out, int64_t rows, int n, int k, void* stream);
 int kdb_unet_unshuffle(const float* x, float* out, int batch, int c, int h, int w, int p, int ld, void* stream);
+
+/* The reverse-mode kernels of kdb_model_forward_vjp / kdb_model_forward_train (fp32, deterministic: one writer per output element, no
+ * atomics, two calls give the same bits; arguments checked before any launch).  Each takes the primal input of one op and the gradient of
+ * its output, and writes (or, where named, adds to) the gradient of its input.
+ * kdb_gemm_vjp: the input gradient of C = A W^T, dA [m, k] = dc [m, n] w [n, k] (n, k multiples of 4).  epi 0 (VJP_STORE) writes it to
+ *   out [m, k]; epi 1 (VJP_UNPATCH_ACC) reads the rows as coarse tokens [m / (hc wc), hc, wc] and the columns as (nh nw e), e < cf (k = 4 cf),
+ *   and ADDS each element to the fine token out [m / (hc wc), 2 hc, 2 wc, cf] it came from (the TokenMerge VJP).  m above 65535 * 64 runs as
+ *   several launches of at most that many rows (of whole images for epi 1); one image of more rows is KDB_ERR_BAD_SHAPE.
+ * kdb_rmsnorm_vjp: ADDS the input gradient of y = x rsqrt(mean(x^2) + 1e-6) s to dx: dx += r (s dy) - x r^3 mean(x s dy), x, dy, dx
+ *   [rows, c]; the scale row of row i is scale + (i / rows_per_image) scale_bstride (scale_bstride 0: one shared row).
+ * kdb_qknorm_rope_vjp: in place on the q and k thirds of dqkv [rows, 3, n_heads, d_head] (v is left alone): the backward of the cosine-sim
+ *   scale and axial RoPE that kdb_model_forward applies to qkv (the primal before them, same layout), rows = batch t_tokens, pos [t_tokens, 2]
+ *   (y, x), freqs [n_heads, r / 2], scale [n_heads], eps as the forward's (r = d_head / 2 and eps 1e-6 for image_transformer_v2; r = d_head
+ *   for image_transformer_v1's layout).  dscale_rows (may be NULL): [rows, n_heads] the contribution of each (row, head) to the gradient of
+ *   that head's scale.  d_head a multiple of 8, r of 4, r <= d_head.
+ * kdb_geglu_vjp: h [m, 2f] = (value | gate) the up projection's output, dy [m, f] -> dh [m, 2f]: dy gelu(gate) | dy value gelu'(gate).
+ * kdb_split_vjp_gather: TokenSplit's lerp backward on a fine grid of batch x height x width x c (height, width even): out [batch, height / 2,
+ *   width / 2, 4 c] = fac dup gathered in TokenMerge order, and dup *= 1 - fac in place (fac: one device float).
+ * kdb_split_unpatch_lerp: up [batch, height, width, c] = torch.lerp(skip, unpatch2x2(y), fac), y [batch, height / 2, width / 2, 4 c].
+ * kdb_merge_scatter_add: dfine [batch, height, width, c] += unpatch2x2(d), d [batch, height / 2, width / 2, 4 c].
+ * kdb_patch_out_vjp: the backward of out_norm + patch_out: dtokens [T, c0] (T = batch (height / patch_h) (width / patch_w)) =
+ *   RMSNorm_vjp(tokens [T, c0], norm_scale [c0], patch(c_out u) w) with u [batch, channels, height, width] the output's gradient, w
+ *   [patch_h patch_w channels, c0] and c_out Karras's (sigma [batch]) when sigma_data > 0, 1 otherwise.  dnorm (may be NULL): [T, c0] the
+ *   gradient of out_norm's output; rstd (may be NULL): [T] each token's rsqrt(mean(x^2) + 1e-6).  It needs 4 (c0 + patch_h patch_w channels)
+ *   floats of shared memory, at most 48 KiB: more returns KDB_ERR_UNSUPPORTED.
+ * kdb_patch_in_vjp: grad_x [batch, channels, height, width] = unpatch(dtokens w) (dtokens [T, n], w [n, patch_h patch_w channels]); with
+ *   sigma_data > 0, c_skip u + c_in unpatch(dtokens w), Karras's scalings of sigma [batch] and u the output's gradient.
+ * kdb_model_mapping_vjp: the mapping network's backward of a finalized model, one row per image: sigma [rows], aug_cond, class_cond and
+ *   mapping_cond as kdb_model_conditioning takes them, dcond [rows, mapping_width] the gradient of the mapping network's output.  With mw =
+ *   mapping_width, D = mapping_depth, F = mapping_d_ff and F4 = F rounded up to a multiple of 4, each row of keep ((4 + D) mw + D (mw + 2 F +
+ *   F4) floats) receives the forward's activations: the Fourier features of sigma at 0 and of aug_cond at mw, the summed embedding entering
+ *   in_norm at 2 mw, the stream entering block l (l = D: out_norm) at (3 + l) mw, then per block l at (4 + D) mw + l (mw + 2 F + F4) its normed
+ *   input (mw), up_proj output (2 F) and GEGLU output (F).  Each row of grad ((D + 2) mw + D (mw + 2 F) floats) receives the gradients: of
+ *   the stream entering block l at l mw (l <= D), of block l's normed input at (D + 1) mw + l (mw + 2 F) and of its up_proj output
+ *   mw later, and of the summed embedding at (D + 1) mw + D (mw + 2 F).  D <= 8, mw a multiple of 4; a network whose (mapping_cond_dim
+ *   rounded up to 4) + 32 + F floats exceed 48 KiB of shared memory returns KDB_ERR_UNSUPPORTED. */
+int kdb_gemm_vjp(const float* dc, const float* w, float* out, int64_t m, int n, int k, int epi, int hc, int wc, int cf, void* stream);
+int kdb_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_image, int64_t rows,
+                    int c, void* stream);
+int kdb_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, float eps, int r, int64_t rows,
+                        int t_tokens, int n_heads, int d_head, float* dscale_rows, void* stream);
+int kdb_geglu_vjp(const float* h, const float* dy, float* dh, int64_t m, int f, void* stream);
+int kdb_split_vjp_gather(float* dup, float* out, const float* fac, int batch, int height, int width, int c, void* stream);
+int kdb_split_unpatch_lerp(const float* y, const float* skip, const float* fac, float* up, int batch, int height, int width, int c, void* stream);
+int kdb_merge_scatter_add(const float* d, float* dfine, int batch, int height, int width, int c, void* stream);
+int kdb_patch_out_vjp(const float* tokens, const float* norm_scale, const float* w, const float* u, const float* sigma, float sigma_data,
+                      float* dtokens, int batch, int channels, int height, int width, int patch_h, int patch_w, int c0, float* dnorm, float* rstd,
+                      void* stream);
+int kdb_patch_in_vjp(const float* dtokens, const float* w, const float* u, const float* sigma, float sigma_data, float* grad_x, int batch,
+                     int channels, int height, int width, int patch_h, int patch_w, int n, void* stream);
+int kdb_model_mapping_vjp(const KdbModel* m, int rows, const float* sigma, const float* aug_cond, const int64_t* class_cond,
+                          const float* mapping_cond, const float* dcond, float* keep, float* grad, void* stream);
 
 /* The same convolution, arguments and layouts on the tensor cores (wgmma, the kernel kdb_unet_forward runs at KDB_PREC_TF32): the
  * products take tf32 operands -- the low 13 mantissa bits of every input and weight element are ignored (truncation), so a caller

@@ -75,6 +75,14 @@ constexpr float kRsqrt2 = 0.70710678118654752440f;
 // erf GELU (image_transformer_v2.py:89-95, layers.py of image_v1) in the reference's association, 0.5 g (1 + erf(g / sqrt 2))
 __device__ __forceinline__ float gelu_erf(float g) { return 0.5f * g * (1.f + erff(g * kRsqrt2)); }
 
+// torch.lerp(self, end, w) in fp32 as ATen computes it (ATen/native/Lerp.h): |w| < 0.5 ? self + w (end - self) : end - (end - self) (1 - w),
+// each branch one fused multiply-add as nvcc contracts it in torch's kernel, written with explicit roundings so that no contraction here
+// can change it.  The TokenSplit lerps and the EMA update share it.
+__device__ __forceinline__ float lerp_torch(float self, float end, float w) {
+  const float d = __fsub_rn(end, self);
+  return fabsf(w) < 0.5f ? __fmaf_rn(w, d, self) : __fmaf_rn(-d, __fsub_rn(1.f, w), end);
+}
+
 // Karras preconditioner scalings (reference layers.py:70-74), fp32 like the reference.
 __device__ __forceinline__ void karras_scalings(float sigma, float sd, float& c_skip, float& c_out, float& c_in) {
   float s2 = sigma * sigma + sd * sd;

@@ -27,20 +27,13 @@ struct EmaSegDev {
   int head, tail, mode, vec;
 };
 
-// torch's lerp (ATen/native/Lerp.h) in fp32 with the weight's complement formed on the device as torch forms it, each branch one fused
-// multiply-add as nvcc contracts it in torch's kernel: |w| < 0.5 ? self + w (end - self) : end - (end - self) (1 - w)
-__device__ __forceinline__ float lerp_torch(float self, float end, float w, float one_minus_w) {
-  const float d = __fsub_rn(end, self);
-  return fabsf(w) < 0.5f ? __fmaf_rn(w, d, self) : __fmaf_rn(-d, one_minus_w, end);
-}
-
-__device__ __forceinline__ void ema_one(const EmaSegDev& s, int64_t i, float w, float omw) {
+// torch's lerp_ (lerp_torch, common.cuh)
+__device__ __forceinline__ void ema_one(const EmaSegDev& s, int64_t i, float w) {
   const float v = __ldg(s.src + i);
-  s.dst[i] = s.mode == KDB_EMA_COPY ? v : lerp_torch(s.dst[i], v, w, omw);
+  s.dst[i] = s.mode == KDB_EMA_COPY ? v : lerp_torch(s.dst[i], v, w);
 }
 
 __global__ void __launch_bounds__(kEmaThreads) ema_update_kernel(const EmaSegDev* __restrict__ segs, int n_segs, int64_t n_chunks, float w) {
-  const float omw = __fsub_rn(1.f, w);
   for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x) {
     int lo = 0, hi = n_segs - 1;   // the last segment whose chunk0 <= c (every segment has at least one chunk)
     while (lo < hi) {
@@ -50,8 +43,8 @@ __global__ void __launch_bounds__(kEmaThreads) ema_update_kernel(const EmaSegDev
     const EmaSegDev s = segs[lo];
     const int64_t k = c - s.chunk0;
     if (k == 0) {
-      if ((int)threadIdx.x < s.head) ema_one(s, threadIdx.x, w, omw);
-      if ((int)threadIdx.x < s.tail) ema_one(s, s.head + 4 * s.quads + threadIdx.x, w, omw);
+      if ((int)threadIdx.x < s.head) ema_one(s, threadIdx.x, w);
+      if ((int)threadIdx.x < s.tail) ema_one(s, s.head + 4 * s.quads + threadIdx.x, w);
     }
     const int64_t q0 = k * kEmaChunkQuads, q1 = std::min(s.quads, q0 + kEmaChunkQuads);
     const float* src = s.src + s.head;
@@ -72,17 +65,17 @@ __global__ void __launch_bounds__(kEmaThreads) ema_update_kernel(const EmaSegDev
         if (q >= q1) continue;
         float4 o = a[u];
         if (s.mode != KDB_EMA_COPY) {
-          o.x = lerp_torch(b[u].x, a[u].x, w, omw);
-          o.y = lerp_torch(b[u].y, a[u].y, w, omw);
-          o.z = lerp_torch(b[u].z, a[u].z, w, omw);
-          o.w = lerp_torch(b[u].w, a[u].w, w, omw);
+          o.x = lerp_torch(b[u].x, a[u].x, w);
+          o.y = lerp_torch(b[u].y, a[u].y, w);
+          o.z = lerp_torch(b[u].z, a[u].z, w);
+          o.w = lerp_torch(b[u].w, a[u].w, w);
         }
         reinterpret_cast<float4*>(dst)[q] = o;
       }
     } else {
       for (int64_t q = q0 + threadIdx.x; q < q1; q += kEmaThreads)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) ema_one(s, s.head + 4 * q + e, w, omw);
+        for (int e = 0; e < 4; ++e) ema_one(s, s.head + 4 * q + e, w);
     }
   }
 }

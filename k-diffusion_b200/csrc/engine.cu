@@ -1000,6 +1000,29 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
   return launch_patch_in_vjp(vs.g[0], m->patch_in_w, u, sigma, sd, grad_x, B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, st);
 }
 
+// the class_cond / mapping_cond checks of kdb_model_conditioning, kdb_model_forward_train and kdb_model_mapping_vjp (image_transformer_v2.py:729-732)
+int check_conds(const KdbModelConfig& c, const int64_t* class_cond, const float* mapping_cond) {
+  KDB_REQUIRE(!(c.num_classes > 0 && class_cond == nullptr), KDB_ERR_BAD_ARG, "class_cond must be specified if num_classes > 0");
+  KDB_REQUIRE(!(c.mapping_cond_dim > 0 && mapping_cond == nullptr), KDB_ERR_BAD_ARG, "mapping_cond must be specified if mapping_cond_dim > 0");
+  return 0;
+}
+
+// the fine grid of the TokenSplit / TokenMerge elementwise entry points
+int check_fine_grid(const char* what, int batch, int height, int width, int c) {
+  KDB_REQUIRE(batch > 0 && c > 0, KDB_ERR_BAD_ARG, "%s: bad argument", what);
+  KDB_REQUIRE(height >= 2 && width >= 2 && height % 2 == 0 && width % 2 == 0, KDB_ERR_BAD_SHAPE, "%s: %dx%d fine grid", what, height, width);
+  return 0;
+}
+
+// an NCHW image of batch x channels x height x width in patch_h x patch_w patches, and Karras's sigma where sigma_data > 0
+int check_patches(const char* what, int batch, int channels, int height, int width, int patch_h, int patch_w, float sigma_data,
+                  const float* sigma) {
+  KDB_REQUIRE(batch > 0 && channels > 0 && patch_h > 0 && patch_w > 0 && (sigma_data <= 0.f || sigma), KDB_ERR_BAD_ARG, "%s: bad argument", what);
+  KDB_REQUIRE(height > 0 && width > 0 && height % patch_h == 0 && width % patch_w == 0, KDB_ERR_BAD_SHAPE, "%s: %dx%d image in %dx%d patches",
+              what, height, width, patch_h, patch_w);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1164,10 +1187,7 @@ int kdb_model_conditioning(KdbModel* m, int rows, const float* sigma, const floa
                            const float* mapping_cond, float* cond_out, void* stream) {
   KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "conditioning: model not finalized");
   KDB_REQUIRE(rows > 0 && sigma && cond_out, KDB_ERR_BAD_ARG, "conditioning: bad arguments");
-  // image_transformer_v2.py:729-732
-  KDB_REQUIRE(!(m->cfg.num_classes > 0 && class_cond == nullptr), KDB_ERR_BAD_ARG, "class_cond must be specified if num_classes > 0");
-  KDB_REQUIRE(!(m->cfg.mapping_cond_dim > 0 && mapping_cond == nullptr), KDB_ERR_BAD_ARG,
-              "mapping_cond must be specified if mapping_cond_dim > 0");
+  if (int rc = check_conds(m->cfg, class_cond, mapping_cond)) return rc;
   return launch_conditioning(m->cw, rows, sigma, aug_cond, class_cond, mapping_cond, cond_out, kdb_model_cond_stride(m),
                              (cudaStream_t)stream);
 }
@@ -1337,8 +1357,7 @@ int kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, i
   KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "forward_train: model not finalized");
   const KdbModelConfig& c = m->cfg;
   KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_train: NULL argument");
-  KDB_REQUIRE(!(c.num_classes > 0 && class_cond == nullptr), KDB_ERR_BAD_ARG, "class_cond must be specified if num_classes > 0");
-  KDB_REQUIRE(!(c.mapping_cond_dim > 0 && mapping_cond == nullptr), KDB_ERR_BAD_ARG, "mapping_cond must be specified if mapping_cond_dim > 0");
+  if ((rc = check_conds(c, class_cond, mapping_cond))) return rc;
   KDB_REQUIRE(cond_batch_stride == kdb_model_cond_stride(m), KDB_ERR_BAD_ARG,
               "forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
               (long long)kdb_model_cond_stride(m));
@@ -1466,6 +1485,79 @@ int kdb_split_fac_grad(const float* y, const float* skip, const float* dup, floa
 int kdb_class_emb_grad(const float* demb, int64_t ldd, const int64_t* cls, float* out, int rows, int n_classes, int mw, void* stream) {
   KDB_REQUIRE(demb && cls && out && rows > 0 && n_classes > 0 && mw > 0 && ldd >= mw, KDB_ERR_BAD_ARG, "class_emb_grad: bad argument");
   return launch_class_emb_grad(demb, ldd, cls, out, rows, n_classes, mw, (cudaStream_t)stream);
+}
+
+int kdb_gemm_vjp(const float* dc, const float* w, float* out, int64_t m, int n, int k, int epi, int hc, int wc, int cf, void* stream) {
+  KDB_REQUIRE(dc && w && out && m > 0 && n > 0 && k > 0, KDB_ERR_BAD_ARG, "gemm_vjp: bad argument");
+  KDB_REQUIRE(epi == VJP_STORE || epi == VJP_UNPATCH_ACC, KDB_ERR_BAD_ARG, "gemm_vjp: bad epilogue %d", epi);
+  KDB_REQUIRE(epi == VJP_STORE || (hc > 0 && wc > 0 && cf > 0), KDB_ERR_BAD_ARG, "gemm_vjp: un-patch grid %dx%d of %d channels", hc, wc, cf);
+  return launch_gemm_vjp(dc, w, out, m, n, k, epi, hc, wc, cf, (cudaStream_t)stream);
+}
+
+int kdb_rmsnorm_vjp(const float* x, const float* dy, float* dx, const float* scale, int64_t scale_bstride, int64_t rows_per_image, int64_t rows,
+                    int c, void* stream) {
+  KDB_REQUIRE(x && dy && dx && scale && rows > 0 && c > 0 && rows_per_image > 0 && scale_bstride >= 0, KDB_ERR_BAD_ARG,
+              "rmsnorm_vjp: bad argument");
+  KDB_REQUIRE(ceil_div(rows, 8) <= INT32_MAX, KDB_ERR_BAD_SHAPE, "rmsnorm_vjp: %lld rows", (long long)rows);
+  return launch_rmsnorm_vjp(x, dy, dx, scale, scale_bstride, rows_per_image, rows, c, (cudaStream_t)stream);
+}
+
+int kdb_qknorm_rope_vjp(const float* qkv, float* dqkv, const float* pos, const float* freqs, const float* scale, float eps, int r, int64_t rows,
+                        int t_tokens, int n_heads, int d_head, float* dscale_rows, void* stream) {
+  KDB_REQUIRE(qkv && dqkv && pos && freqs && scale && rows > 0 && t_tokens > 0 && n_heads > 0 && eps >= 0.f, KDB_ERR_BAD_ARG,
+              "qknorm_rope_vjp: bad argument");
+  KDB_REQUIRE(rows % t_tokens == 0 && ceil_div(rows * n_heads, 4) <= INT32_MAX, KDB_ERR_BAD_SHAPE, "qknorm_rope_vjp: %lld rows of %d tokens",
+              (long long)rows, t_tokens);
+  QkRope qr;
+  qr.freqs = freqs, qr.scale = scale, qr.eps = eps, qr.R = r;
+  return launch_qknorm_rope_vjp(qkv, dqkv, pos, qr, rows, t_tokens, n_heads, d_head, (cudaStream_t)stream, dscale_rows);
+}
+
+int kdb_geglu_vjp(const float* h, const float* dy, float* dh, int64_t m, int f, void* stream) {
+  KDB_REQUIRE(h && dy && dh && m > 0 && f > 0, KDB_ERR_BAD_ARG, "geglu_vjp: bad argument");
+  return launch_geglu_vjp(h, dy, dh, m, f, (cudaStream_t)stream);
+}
+
+int kdb_split_vjp_gather(float* dup, float* out, const float* fac, int batch, int height, int width, int c, void* stream) {
+  KDB_REQUIRE(dup && out && fac, KDB_ERR_BAD_ARG, "split_vjp_gather: NULL argument");
+  if (int rc = check_fine_grid("split_vjp_gather", batch, height, width, c)) return rc;
+  return launch_split_vjp_gather(dup, out, fac, batch, height, width, c, (cudaStream_t)stream);
+}
+
+int kdb_split_unpatch_lerp(const float* y, const float* skip, const float* fac, float* up, int batch, int height, int width, int c, void* stream) {
+  KDB_REQUIRE(y && skip && fac && up, KDB_ERR_BAD_ARG, "split_unpatch_lerp: NULL argument");
+  if (int rc = check_fine_grid("split_unpatch_lerp", batch, height, width, c)) return rc;
+  return launch_split_unpatch_lerp(y, skip, fac, up, batch, height, width, c, (cudaStream_t)stream);
+}
+
+int kdb_merge_scatter_add(const float* d, float* dfine, int batch, int height, int width, int c, void* stream) {
+  KDB_REQUIRE(d && dfine, KDB_ERR_BAD_ARG, "merge_scatter_add: NULL argument");
+  if (int rc = check_fine_grid("merge_scatter_add", batch, height, width, c)) return rc;
+  return launch_merge_scatter_add(d, dfine, batch, height, width, c, (cudaStream_t)stream);
+}
+
+int kdb_patch_out_vjp(const float* tokens, const float* norm_scale, const float* w, const float* u, const float* sigma, float sigma_data,
+                      float* dtokens, int batch, int channels, int height, int width, int patch_h, int patch_w, int c0, float* dnorm, float* rstd,
+                      void* stream) {
+  KDB_REQUIRE(tokens && norm_scale && w && u && dtokens && c0 > 0, KDB_ERR_BAD_ARG, "patch_out_vjp: bad argument");
+  if (int rc = check_patches("patch_out_vjp", batch, channels, height, width, patch_h, patch_w, sigma_data, sigma)) return rc;
+  return launch_patch_out_vjp(tokens, norm_scale, w, u, sigma, sigma_data, dtokens, batch, channels, height, width, patch_h, patch_w, c0,
+                              (cudaStream_t)stream, dnorm, rstd);
+}
+
+int kdb_patch_in_vjp(const float* dtokens, const float* w, const float* u, const float* sigma, float sigma_data, float* grad_x, int batch,
+                     int channels, int height, int width, int patch_h, int patch_w, int n, void* stream) {
+  KDB_REQUIRE(dtokens && w && grad_x && n > 0 && (sigma_data <= 0.f || u), KDB_ERR_BAD_ARG, "patch_in_vjp: bad argument");
+  if (int rc = check_patches("patch_in_vjp", batch, channels, height, width, patch_h, patch_w, sigma_data, sigma)) return rc;
+  return launch_patch_in_vjp(dtokens, w, u, sigma, sigma_data, grad_x, batch, channels, height, width, patch_h, patch_w, n, (cudaStream_t)stream);
+}
+
+int kdb_model_mapping_vjp(const KdbModel* m, int rows, const float* sigma, const float* aug_cond, const int64_t* class_cond,
+                          const float* mapping_cond, const float* dcond, float* keep, float* grad, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "model_mapping_vjp: model NULL or not finalized");
+  KDB_REQUIRE(rows > 0 && sigma && dcond && keep && grad, KDB_ERR_BAD_ARG, "model_mapping_vjp: bad argument");
+  if (int rc = check_conds(m->cfg, class_cond, mapping_cond)) return rc;
+  return launch_mapping_backward(m->cw, rows, sigma, aug_cond, class_cond, mapping_cond, dcond, keep, grad, (cudaStream_t)stream);
 }
 
 int kdb_model_debug_tap(KdbModel* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

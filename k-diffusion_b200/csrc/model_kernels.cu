@@ -245,12 +245,6 @@ __device__ __forceinline__ void load4<bf16>(const bf16* p, bool ok, float (&v)[4
   } else { v[0] = v[1] = v[2] = v[3] = 0.f; }
 }
 
-__device__ __forceinline__ float lerp_like_torch(float start, float end, float w) {
-  // ATen lerp: w < 0.5 ? start + w (end - start) : end - (end - start)(1 - w)
-  const float d = end - start;
-  return (w < 0.5f) ? fmaf(w, d, start) : end - d * (1.f - w);
-}
-
 template <typename T, typename TW, int EPI>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(const T* __restrict__ A, const TW* __restrict__ W, T* __restrict__ Cout,
                                                         int64_t M, int N, int K, const T* __restrict__ resid,
@@ -280,7 +274,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const T* __restrict__ A,
       token_coords(m, hc, wc, b, hy, wx);
       const int q = n / Cf, e = n - q * Cf;
       const int64_t dst = fine_offset(b, hy, wx, q, e, hc, wc, Cf);
-      Cout[dst] = from_f<T>(lerp_like_torch(to_f(resid[dst]), acc, __ldg(fac)));
+      Cout[dst] = from_f<T>(lerp_torch(to_f(resid[dst]), acc, __ldg(fac)));
     }
   });
 }
@@ -1137,7 +1131,7 @@ int launch_geglu_vjp(const float* h, const float* dy, float* dh, int64_t M, int 
 }
 
 // TokenSplit VJP, elementwise part: dcur_patched = patch2x2(fac dup) -> out [B, H/2, W/2, (nh nw e)] (the TokenMerge gather order), and
-// dup <- (1 - fac) dup in place (the gradient the skip connection receives).  Same derivative on both branches of lerp_like_torch.
+// dup <- (1 - fac) dup in place (the gradient the skip connection receives).  Same derivative on both branches of lerp_torch.
 __global__ void __launch_bounds__(256) split_vjp_gather_kernel(float* __restrict__ dup, float* __restrict__ out, const float* __restrict__ fac,
                                                                int H, int Wd, int C, int64_t total) {
   const float f = __ldg(fac), g = 1.f - f;
@@ -1165,7 +1159,7 @@ __global__ void __launch_bounds__(256) split_unpatch_lerp_kernel(const float* __
   const float f = __ldg(fac);
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
     const int64_t dst = merge_source(i, H / 2, Wd / 2, C);
-    up[dst] = lerp_like_torch(skip[dst], y[i], f);
+    up[dst] = lerp_torch(skip[dst], y[i], f);
   }
 }
 

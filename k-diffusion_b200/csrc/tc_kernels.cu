@@ -425,7 +425,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
       }
     } else if constexpr (EPI == EPI_SPLIT_LERP) {
       // TokenSplit + torch.lerp(skip, x, fac) (reference :618-621): row m = (b, hy, wx) on the coarse grid, column n = (quadrant
-      // (nh, nw), channel e), scattered to the fine token.  The lerp takes one of two forms by fac; sum(x^2) runs in column order.
+      // (nh, nw), channel e), scattered to the fine token, the lerp torch's (lerp_torch); sum(x^2) runs in column order.
       const bool live = m < p.M;
       const float facv = __ldg(p.fac);
       float ss = 0.f;
@@ -457,9 +457,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
             for (int q = 0; q < 4; ++q) {
               const float lo = __uint_as_float(rw[q] << 16), hi = __uint_as_float(rw[q] & 0xffff0000u);
               const float e0 = v[j * 8 + q * 2], e1 = v[j * 8 + q * 2 + 1];
-              const float d0 = e0 - lo, d1 = e1 - hi;
-              const float o0 = (facv < 0.5f) ? fmaf(facv, d0, lo) : e0 - d0 * (1.f - facv);
-              const float o1 = (facv < 0.5f) ? fmaf(facv, d1, hi) : e1 - d1 * (1.f - facv);
+              const float o0 = lerp_torch(lo, e0, facv);
+              const float o1 = lerp_torch(hi, e1, facv);
               ss = fmaf(o0, o0, fmaf(o1, o1, ss));
               ow[q] = tc::pack_bf16x2(o0, o1);
             }
@@ -514,9 +513,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wg_kernel(const __grid_c
           for (int q = 0; q < 4; ++q) {
             const float lo = __uint_as_float(rw[q] << 16), hi = __uint_as_float(rw[q] & 0xffff0000u);   // bf16 -> fp32 is a shift / mask
             const float e0 = v[j * 8 + q * 2], e1 = v[j * 8 + q * 2 + 1];
-            const float d0 = e0 - lo, d1 = e1 - hi;
-            const float o0 = (facv < 0.5f) ? fmaf(facv, d0, lo) : e0 - d0 * (1.f - facv);
-            const float o1 = (facv < 0.5f) ? fmaf(facv, d1, hi) : e1 - d1 * (1.f - facv);
+            const float o0 = lerp_torch(lo, e0, facv);
+            const float o1 = lerp_torch(hi, e1, facv);
             ss = fmaf(o0, o0, fmaf(o1, o1, ss));
             ow[q] = tc::pack_bf16x2(o0, o1);
           }

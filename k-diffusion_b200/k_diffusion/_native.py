@@ -20,7 +20,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 26
+ABI_VERSION = 27
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -119,6 +119,16 @@ SIGNATURES = {
     "kdb_colsum": (_i32, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "kdb_split_fac_grad": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_class_emb_grad": (_i32, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "kdb_gemm_vjp": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_rmsnorm_vjp": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp]),
+    "kdb_qknorm_rope_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _f32, _i32, _i64, _i32, _i32, _i32, _vp, _vp]),
+    "kdb_geglu_vjp": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp]),
+    "kdb_split_vjp_gather": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_split_unpatch_lerp": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_merge_scatter_add": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_patch_out_vjp": (_i32, [_vp, _vp, _vp, _vp, _vp, _f32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "kdb_patch_in_vjp": (_i32, [_vp, _vp, _vp, _vp, _f32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "kdb_model_mapping_vjp": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "kdb_gemm_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "kdb_gemm_bf16_geglu": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "kdb_ffn_fused_bf16": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
@@ -732,6 +742,28 @@ class Engine:
                                                 stream()))
         return out
 
+    def mapping_vjp(self, sigma, dcond, aug_cond=None, class_cond=None, mapping_cond=None, out=None):
+        """kdb_model_mapping_vjp: the mapping network's backward for sigma [rows] and dcond [rows, mapping_width] (the gradient of its
+        output), conditioning as conditioning() takes it -> (keep [rows, keep floats], grad [rows, grad floats]), their rows laid out as
+        mapping_layout gives.  out: a (keep, grad) pair of buffers to write."""
+        require_cuda(sigma, dcond, aug_cond, class_cond, mapping_cond)
+        c = self.cfg
+        rows, L = sigma.numel(), mapping_layout(c.mapping_width, c.mapping_d_ff, c.mapping_depth)
+        _fp32_contiguous("model_mapping_vjp", *(t for t in (sigma, dcond, aug_cond, mapping_cond) if t is not None))
+        if (tuple(dcond.shape) != (rows, c.mapping_width) or (aug_cond is not None and tuple(aug_cond.shape) != (rows, 9))
+                or (mapping_cond is not None and tuple(mapping_cond.shape) != (rows, c.mapping_cond_dim))
+                or (class_cond is not None and (class_cond.dtype != torch.int64 or tuple(class_cond.shape) != (rows,)
+                                                or not class_cond.is_contiguous()))):
+            raise ValueError("model_mapping_vjp: operand shapes do not match")
+        keep, grad = (None, None) if out is None else out
+        keep = _out(keep, (rows, L["keep"]), dcond, "model_mapping_vjp")
+        grad = _out(grad, (rows, L["grad"]), dcond, "model_mapping_vjp")
+        require_cuda(keep, grad)
+        with device_of(sigma):
+            check(lib().kdb_model_mapping_vjp(self._h, rows, ptr(sigma), ptr(aug_cond), ptr(class_cond), ptr(mapping_cond), ptr(dcond), ptr(keep),
+                                              ptr(grad), stream()))
+        return keep, grad
+
     def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
         """kdb_model_train_forward: the forward of forward_train at `precision` (x [B,C,H,W] fp32), bit for bit its `out`."""
         B, _, H, W = x.shape
@@ -1049,6 +1081,195 @@ def class_emb_grad(demb, cls, n_classes, out=None):
     out = _out(out, (n_classes, mw), demb, "class_emb_grad")
     check(lib().kdb_class_emb_grad(ptr(demb), demb.stride(0), ptr(cls), ptr(out), rows, n_classes, mw, stream()))
     return out
+
+
+VJP_STORE, VJP_UNPATCH_ACC = 0, 1
+
+
+def _shaped(name, t, shape):
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name}: {tuple(t.shape)} where {list(shape)} is needed")
+
+
+@_on_device_of_first
+def gemm_vjp(dc, w, out=None, unpatch=None):
+    """kdb_gemm_vjp: the input gradient dA [M, K] = dc [M, N] w [N, K] of a Linear, contiguous fp32 (N, K multiples of 4).  unpatch=(hc, wc):
+    the rows are coarse tokens of hc x wc grids and dA is ADDED to out, the fine tokens [M / (hc wc), 2 hc, 2 wc, K / 4] (required), through
+    the TokenMerge un-patch."""
+    require_cuda(dc, w, out)
+    _fp32_contiguous("gemm_vjp", dc, w)
+    if dc.ndim != 2 or w.ndim != 2 or dc.shape[1] != w.shape[0]:
+        raise ValueError(f"gemm_vjp: dc {tuple(dc.shape)} and w {tuple(w.shape)} do not chain")
+    (M, N), K = dc.shape, w.shape[1]
+    hc, wc = unpatch or (0, 0)
+    if unpatch:
+        if out is None or hc <= 0 or wc <= 0 or K % 4 or M % (hc * wc):
+            raise ValueError(f"gemm_vjp: {M} x {K} does not un-patch onto {hc}x{wc} coarse grids, or no fine tokens to add to")
+        _fp32_contiguous("gemm_vjp", out)
+        _shaped("gemm_vjp", out, (M // (hc * wc), 2 * hc, 2 * wc, K // 4))
+    else:
+        out = _out(out, (M, K), dc, "gemm_vjp")
+    check(lib().kdb_gemm_vjp(ptr(dc), ptr(w), ptr(out), M, N, K, VJP_UNPATCH_ACC if unpatch else VJP_STORE, hc, wc, K // 4 if unpatch else 0,
+                             stream()))
+    return out
+
+
+@_on_device_of_first
+def rmsnorm_vjp(x, dy, scale, out, rows_per_image=None, scale_bstride=0):
+    """kdb_rmsnorm_vjp: ADDS the input gradient of an (Ada)RMSNorm to out (returned), x, dy and out [rows, C] contiguous fp32; the scale row
+    of image b (rows_per_image rows each, default all) starts at scale[b * scale_bstride] (0: one row shared by all)"""
+    require_cuda(x, dy, scale, out)
+    _fp32_contiguous("rmsnorm_vjp", x, dy, scale, out)
+    rows, C = x.shape
+    R = rows if rows_per_image is None else rows_per_image
+    _shaped("rmsnorm_vjp", dy, (rows, C))
+    _shaped("rmsnorm_vjp", out, (rows, C))
+    if R <= 0 or rows % R or scale_bstride < 0 or scale.numel() < (rows // R - 1) * scale_bstride + C:
+        raise ValueError(f"rmsnorm_vjp: {rows} rows of {R} per image, or a scale of {scale.numel()} floats for rows {scale_bstride} apart")
+    check(lib().kdb_rmsnorm_vjp(ptr(x), ptr(dy), ptr(out), ptr(scale), scale_bstride, R, rows, C, stream()))
+    return out
+
+
+@_on_device_of_first
+def qknorm_rope_vjp(qkv, dqkv, pos, freqs, scale, eps, r, dscale_rows=None):
+    """kdb_qknorm_rope_vjp: in place on the q and k thirds of dqkv [rows, 3, nh, e] (returned with dscale_rows), qkv the primal before the
+    cosine-sim scale and RoPE, pos [T, 2] (rows a multiple of T), freqs [nh, r / 2], scale [nh]; dscale_rows: None or an [rows, nh] buffer
+    for each (row, head)'s term of the head scale's gradient.  All contiguous fp32."""
+    require_cuda(qkv, dqkv, pos, freqs, scale, dscale_rows)
+    _fp32_contiguous("qknorm_rope_vjp", *(t for t in (qkv, dqkv, pos, freqs, scale, dscale_rows) if t is not None))
+    if qkv.ndim != 4 or qkv.shape[1] != 3 or pos.ndim != 2 or pos.shape[1] != 2:
+        raise ValueError(f"qknorm_rope_vjp: qkv {tuple(qkv.shape)} is no [rows, 3, nh, e], or pos {tuple(pos.shape)} no [T, 2]")
+    rows, _, nh, e = qkv.shape
+    T = pos.shape[0]
+    _shaped("qknorm_rope_vjp", dqkv, qkv.shape)
+    _shaped("qknorm_rope_vjp", freqs, (nh, r // 2))
+    _shaped("qknorm_rope_vjp", scale, (nh,))
+    if dscale_rows is not None:
+        _shaped("qknorm_rope_vjp", dscale_rows, (rows, nh))
+    if T <= 0 or rows % T:
+        raise ValueError(f"qknorm_rope_vjp: {rows} rows are no whole images of {T} tokens")
+    check(lib().kdb_qknorm_rope_vjp(ptr(qkv), ptr(dqkv), ptr(pos), ptr(freqs), ptr(scale), float(eps), r, rows, T, nh, e, ptr(dscale_rows),
+                                    stream()))
+    return dqkv, dscale_rows
+
+
+@_on_device_of_first
+def geglu_vjp(h, dy, out=None):
+    """kdb_geglu_vjp: h [M, 2F] (value | gate), dy [M, F] contiguous fp32 -> dh [M, 2F]"""
+    require_cuda(h, dy, out)
+    _fp32_contiguous("geglu_vjp", h, dy)
+    M, F = dy.shape
+    _shaped("geglu_vjp", h, (M, 2 * F))
+    out = _out(out, (M, 2 * F), h, "geglu_vjp")
+    check(lib().kdb_geglu_vjp(ptr(h), ptr(dy), ptr(out), M, F, stream()))
+    return out
+
+
+def _fine_and_coarse(name, fine, coarse, fac=None):
+    """fine [B, H, W, C] and coarse [B, H/2, W/2, 4C] contiguous fp32 (fac: one fp32 float) -> (B, H, W, C)"""
+    _fp32_contiguous(name, fine, coarse, *(() if fac is None else (fac,)))
+    if fine.ndim != 4 or fine.shape[1] % 2 or fine.shape[2] % 2 or (fac is not None and fac.numel() != 1):
+        raise ValueError(f"{name}: {tuple(fine.shape)} is no [B, H, W, C] with H and W even, or fac is not one float")
+    B, H, W, C = fine.shape
+    _shaped(name, coarse, (B, H // 2, W // 2, 4 * C))
+    return B, H, W, C
+
+
+@_on_device_of_first
+def split_vjp_gather(dup, fac, out=None):
+    """kdb_split_vjp_gather: TokenSplit's lerp backward, dup [B, H, W, C] -> out [B, H/2, W/2, 4C] = fac dup in TokenMerge order, and
+    dup *= 1 - fac IN PLACE; fac one fp32 float on the device"""
+    require_cuda(dup, fac, out)
+    B, H, W, C = dup.shape
+    out = _out(out, (B, H // 2, W // 2, 4 * C), dup, "split_vjp_gather")
+    _fine_and_coarse("split_vjp_gather", dup, out, fac)
+    check(lib().kdb_split_vjp_gather(ptr(dup), ptr(out), ptr(fac), B, H, W, C, stream()))
+    return out
+
+
+@_on_device_of_first
+def split_unpatch_lerp(y, skip, fac, out=None):
+    """kdb_split_unpatch_lerp: torch.lerp(skip, unpatch2x2(y), fac) -> [B, H, W, C], y [B, H/2, W/2, 4C], skip [B, H, W, C], fac one float"""
+    require_cuda(y, skip, fac, out)
+    B, H, W, C = _fine_and_coarse("split_unpatch_lerp", skip, y, fac)
+    out = _out(out, skip.shape, skip, "split_unpatch_lerp")
+    check(lib().kdb_split_unpatch_lerp(ptr(y), ptr(skip), ptr(fac), ptr(out), B, H, W, C, stream()))
+    return out
+
+
+@_on_device_of_first
+def merge_scatter_add(d, out):
+    """kdb_merge_scatter_add: out [B, H, W, C] += unpatch2x2(d), d [B, H/2, W/2, 4C]; returns out"""
+    require_cuda(d, out)
+    B, H, W, C = _fine_and_coarse("merge_scatter_add", out, d)
+    check(lib().kdb_merge_scatter_add(ptr(d), ptr(out), B, H, W, C, stream()))
+    return out
+
+
+def _patch_grid(name, size, patch, sigma, sigma_data):
+    (B, C, H, W), (ph, pw) = size, patch
+    if ph <= 0 or pw <= 0 or H % ph or W % pw:
+        raise ValueError(f"{name}: a {H}x{W} image in {ph}x{pw} patches")
+    if sigma_data > 0:
+        if sigma is None:
+            raise ValueError(f"{name}: sigma_data > 0 needs sigma")
+        _fp32_contiguous(name, sigma)
+        _shaped(name, sigma, (B,))
+    return B * (H // ph) * (W // pw)
+
+
+@_on_device_of_first
+def patch_out_vjp(tokens, norm_scale, w, u, patch, sigma=None, sigma_data=0.0, out=None, dnorm=None, rstd=None):
+    """kdb_patch_out_vjp: out_norm + patch_out's backward, tokens [T, C0], norm_scale [C0], w [ph pw C, C0], u [B, C, H, W] the output's
+    gradient (scaled by Karras's c_out of sigma [B] when sigma_data > 0) -> (dtokens [T, C0], dnorm, rstd): dnorm [T, C0] and rstd [T] are
+    written where given.  All contiguous fp32."""
+    require_cuda(tokens, norm_scale, w, u, sigma, out, dnorm, rstd)
+    _fp32_contiguous("patch_out_vjp", tokens, norm_scale, w, u, *(t for t in (dnorm, rstd) if t is not None))
+    T = _patch_grid("patch_out_vjp", u.shape, patch, sigma, sigma_data)
+    C0 = tokens.shape[-1]
+    _shaped("patch_out_vjp", tokens, (T, C0))
+    _shaped("patch_out_vjp", norm_scale, (C0,))
+    _shaped("patch_out_vjp", w, (patch[0] * patch[1] * u.shape[1], C0))
+    if dnorm is not None:
+        _shaped("patch_out_vjp", dnorm, (T, C0))
+    if rstd is not None:
+        _shaped("patch_out_vjp", rstd, (T,))
+    out = _out(out, (T, C0), tokens, "patch_out_vjp")
+    (B, C, H, W), (ph, pw) = u.shape, patch
+    check(lib().kdb_patch_out_vjp(ptr(tokens), ptr(norm_scale), ptr(w), ptr(u), ptr(sigma), float(sigma_data), ptr(out), B, C, H, W, ph, pw, C0,
+                                  ptr(dnorm), ptr(rstd), stream()))
+    return out, dnorm, rstd
+
+
+@_on_device_of_first
+def patch_in_vjp(dtokens, w, size, patch, u=None, sigma=None, sigma_data=0.0, out=None):
+    """kdb_patch_in_vjp: patch_in's backward to an image of size (B, C, H, W): unpatch(dtokens [T, N] w [N, ph pw C]), with sigma_data > 0
+    c_skip u + c_in unpatch(...) (u [B, C, H, W] the output's gradient, sigma [B]).  All contiguous fp32."""
+    require_cuda(dtokens, w, u, sigma, out)
+    _fp32_contiguous("patch_in_vjp", dtokens, w, *(() if u is None else (u,)))
+    T = _patch_grid("patch_in_vjp", size, patch, sigma, sigma_data)
+    N = dtokens.shape[-1]
+    _shaped("patch_in_vjp", dtokens, (T, N))
+    _shaped("patch_in_vjp", w, (N, patch[0] * patch[1] * size[1]))
+    if sigma_data > 0:
+        if u is None:
+            raise ValueError("patch_in_vjp: sigma_data > 0 needs u")
+        _shaped("patch_in_vjp", u, size)
+    out = _out(out, tuple(size), dtokens, "patch_in_vjp")
+    (B, C, H, W), (ph, pw) = size, patch
+    check(lib().kdb_patch_in_vjp(ptr(dtokens), ptr(w), ptr(u), ptr(sigma), float(sigma_data), ptr(out), B, C, H, W, ph, pw, N, stream()))
+    return out
+
+
+def mapping_layout(mw, dff, depth):
+    """The row layout of kdb_model_mapping_vjp's keep and grad (the header's formulas): their widths and each vector's offset"""
+    f4 = (dff + 3) // 4 * 4
+    blk = mw + 2 * dff + f4
+    xn = lambda l: (4 + depth) * mw + l * blk
+    dxn = lambda l: (depth + 1) * mw + l * (mw + 2 * dff)
+    return {"keep": xn(depth), "grad": dxn(depth) + mw, "ff_t": 0, "ff_a": mw, "emb": 2 * mw, "r": lambda l: (3 + l) * mw, "xn": xn,
+            "up": lambda l: xn(l) + mw, "g": lambda l: xn(l) + mw + 2 * dff, "dr": lambda l: l * mw, "dxn": dxn,
+            "dh": lambda l: dxn(l) + mw, "demb": dxn(depth)}
 
 
 def interleave_geglu_rows(w_up):

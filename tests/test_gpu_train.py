@@ -64,19 +64,21 @@ def native_grads(model, inner, x, noise, sigma, kw, gw):
     return loss.detach().cpu(), {k: p.grad.detach().cpu().clone() for k, p in inner.named_parameters()}
 
 
-def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False):
-    """layers.py:76-86 (or :107-111) around the oracle's model, autograd on the CPU"""
+def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False, device="cpu"):
+    """layers.py:76-86 (or :107-111) around the oracle's model, autograd on `device` (losses and gradients returned on the CPU)"""
     m = cfg["model"]
-    params = {k: v.to(dtype).requires_grad_(not k.endswith(("pos_emb.freqs", "time_emb.weight", "aug_emb.weight"))) for k, v in sd.items()}
-    x, noise, sigma, gw = x.to(dtype), noise.to(dtype), sigma.to(dtype), gw.to(dtype)
-    kw = {k: (v.to(dtype) if v.is_floating_point() else v) for k, v in kw.items()}
+    params = {k: v.to(device, dtype).requires_grad_(not k.endswith(("pos_emb.freqs", "time_emb.weight", "aug_emb.weight")))
+              for k, v in sd.items()}
+    x, noise, sigma, gw = (t.to(device, dtype) for t in (x, noise, sigma, gw))
+    kw = {k: (v.to(device, dtype) if v.is_floating_point() else v.to(device)) for k, v in kw.items()}
     if "aug_cond" in kw:   # the augment wrapper: mapping_cond = cat([aug_cond, mapping_cond])
         kw["mapping_cond"] = torch.cat([kw.pop("aug_cond"), kw["mapping_cond"]], 1)
     sd_ = m["sigma_data"]
     c_skip, c_out, c_in = [c.view(-1, 1, 1, 1) for c in O.karras_scalings(sigma, sd_)]
     s4 = sigma.view(-1, 1, 1, 1)
     noised = x + noise * s4
-    f = O.model_forward(params, m, noised * c_in, sigma, **kw)
+    with torch.device(device):   # the oracle's position tables and masks on the same device
+        f = O.model_forward(params, m, noised * c_in, sigma, **kw)
     if simple:
         den = f * c_out + noised * c_skip
         loss = (((noised - den) / s4 - noise) ** 2).flatten(1).mean(1)
@@ -84,14 +86,14 @@ def oracle_grads(cfg, sd, x, noise, sigma, kw, gw, dtype, simple=False):
         w = (sigma * sd_) ** 2 / (sigma ** 2 + sd_ ** 2) ** 2 if m["loss_weighting"] == "soft-min-snr" else torch.ones_like(sigma)
         loss = ((f - (x - c_skip * noised) / c_out) ** 2).flatten(1).mean(1) * w
     (loss * gw).sum().backward()
-    return loss.detach(), {k: p.grad for k, p in params.items() if p.requires_grad}
+    return loss.detach().cpu(), {k: p.grad.cpu() for k, p in params.items() if p.requires_grad}
 
 
-def check_against_oracle(cfg, sd, got_loss, got, x, noise, sigma, kw, gw, simple=False, budget=None):
+def check_against_oracle(cfg, sd, got_loss, got, x, noise, sigma, kw, gw, simple=False, budget=None, device="cpu"):
     """Each native gradient within 8x the fp32-vs-float64 distance of the oracle's gradient (budget: of the reference's, recorded in
     tests/golden/train_meta.json, where the inputs are the fixture's: the larger of the two), plus 1e-6 relative."""
-    l64, g64 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float64, simple)
-    l32, g32 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float32, simple)
+    l64, g64 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float64, simple, device)
+    l32, g32 = oracle_grads(cfg, sd, x, noise, sigma, kw, gw, torch.float32, simple, device)
     assert torch.allclose(got_loss.double(), l64, rtol=1e-5, atol=0)
     assert set(got) == set(g64)
     for k, want in g64.items():
@@ -227,6 +229,30 @@ def test_cfg2_gradients_match_float64(size, B):
     x, noise, sigma, kw, gw = inputs(cfg, B, 40 + size)
     loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
     check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw)
+
+
+@pytest.fixture(scope="module")
+def no_tf32():
+    """cuBLAS matmuls at full fp32 for the oracle on the GPU: under TF32 (operands rounded to 2^-11 instead of 2^-24) its fp32-vs-float64
+    distance, and with it the gate, would loosen by three to four orders of magnitude"""
+    saved = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    yield
+    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = saved
+
+
+@pytest.mark.parametrize("name", ["cfg1", "cifar10"])
+def test_reference_configs_at_the_training_batch_size(name, no_tf32):
+    """train.py's default batch of 64 (config_mnist_transformer: 3136 level-0 rows; config_cifar10_transformer: 16384 and 4096): every
+    gradient within 8x the oracle's fp32 distance, the oracle run on the GPU in float64 and fp32; two calls bit-identical"""
+    assert not torch.backends.cuda.matmul.allow_tf32
+    cfg, inner, sd, model = build({"cfg1": CFG1, "cifar10": CIFAR10}[name])
+    x, noise, sigma, kw, gw = inputs(cfg, 64, 60)
+    kw["class_cond"][:6] = 10   # cond-dropout rows among the labels
+    loss, got = native_grads(model, inner, x, noise, sigma, kw, gw)
+    check_against_oracle(cfg, sd, loss, got, x, noise, sigma, kw, gw, device="cuda")
+    l2, again = native_grads(model, inner, x, noise, sigma, kw, gw)
+    assert torch.equal(loss, l2) and all(torch.equal(got[k], again[k]) for k in got), "two calls differ"
 
 
 FROZEN = {"mapping": ("mapping.",), "class_emb": ("class_emb.",), "level": ("down_levels.0.",), "merges_splits": ("merges.", "splits.")}

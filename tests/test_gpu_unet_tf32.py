@@ -75,6 +75,11 @@ def tf32_oracle(monkeypatch, sd64):
 TF32_CASES = CONV_CASES + [
     (3, 7, 7, 36, 0, 68, 3, "r1"),            # 7x7 grids: two images and a padded row and column per M tile
     (2, 7, 7, 68, 36, 36, 1, 12),             # 7x7, two sources with c1 % 32 == 4 (a channel block holds both), residual split at 12
+    # the token-stream Linear of the transformer's tf32 training route (engine.cu linear_tf32: one 1 x M image, ksize 1): the cifar10
+    # transformer's level-0 qkv at B = 64, its level-1 residual form, and a ragged last pixel tile
+    (1, 1, 16384, 256, 0, 768, 1, None),
+    (1, 1, 4096, 512, 0, 512, 1, "r1"),
+    (1, 1, 3137, 256, 0, 256, 1, "r1"),
 ]
 
 
@@ -123,7 +128,8 @@ def test_conv_tf32_exact_on_dyadic_operands(case, with_bias):
 
 
 @pytest.mark.parametrize("case", [(3, 5, 9, 36, 0, 68, 3, 28), (2, 12, 20, 64, 32, 96, 3, None), (3, 6, 10, 20, 12, 36, 1, "r1"),
-                                  (2, 16, 16, 128, 128, 256, 3, None)],
+                                  (2, 16, 16, 128, 128, 256, 3, None), (1, 1, 16384, 256, 0, 768, 1, None), (1, 1, 4096, 512, 0, 512, 1, "r1"),
+                                  (1, 1, 3137, 256, 0, 256, 1, "r1")],
                          ids=lambda c: "B{}_{}x{}_c{}+{}_N{}_k{}_r{}".format(*c))
 def test_conv_tf32_random_operands_within_the_tf32_error_bound(case):
     """Inputs and weights both truncated to tf32 (relative error < 2^-10 each), fp32 accumulation of K products:

@@ -217,3 +217,87 @@ def test_reduction_wrappers_refuse_mismatched_operands(cpu_native, monkeypatch):
         with pytest.raises(ValueError):
             call()
             pytest.fail(f"case {i} was accepted")
+
+
+def test_vjp_wrappers_refuse_mismatched_operands(cpu_native, monkeypatch):
+    """The reverse-mode entry points take no operand extents either: each wrapper checks them before the call"""
+    from k_diffusion import _native
+    monkeypatch.setattr(_native, "lib", lambda: pytest.fail("reached the library"))
+    z = torch.zeros
+    bad = [
+        lambda: _native.gemm_vjp(z(10, 8), z(9, 4)),                                          # dc's columns are w's rows
+        lambda: _native.gemm_vjp(z(10, 8), z(8, 4), out=z(10, 5)),
+        lambda: _native.gemm_vjp(z(12, 8), z(8, 16), unpatch=(2, 3)),                          # un-patch needs the fine tokens
+        lambda: _native.gemm_vjp(z(12, 8), z(8, 16), out=z(2, 4, 6, 5), unpatch=(2, 3)),       # channels K / 4
+        lambda: _native.gemm_vjp(z(12, 8), z(8, 16), out=z(2, 4, 4, 4), unpatch=(2, 3)),       # fine grid 2hc x 2wc
+        lambda: _native.gemm_vjp(z(10, 8), z(8, 16), out=z(2, 4, 6, 4), unpatch=(2, 3)),       # whole images of hc wc rows
+        lambda: _native.rmsnorm_vjp(z(10, 8), z(10, 8), z(8), z(10, 7)),
+        lambda: _native.rmsnorm_vjp(z(10, 8), z(10, 8), z(8), z(10, 8), rows_per_image=3),     # whole images
+        lambda: _native.rmsnorm_vjp(z(10, 8), z(10, 8), z(8 + 7), z(10, 8), rows_per_image=5, scale_bstride=8),   # second scale row short
+        lambda: _native.qknorm_rope_vjp(z(12, 3, 2, 16), z(12, 3, 2, 16), z(5, 2), z(2, 4), z(2), 1e-6, 8),          # 12 rows of 5 tokens
+        lambda: _native.qknorm_rope_vjp(z(12, 3, 2, 16), z(12, 3, 2, 8), z(6, 2), z(2, 4), z(2), 1e-6, 8),
+        lambda: _native.qknorm_rope_vjp(z(12, 3, 2, 16), z(12, 3, 2, 16), z(6, 2), z(2, 8), z(2), 1e-6, 8),          # freqs [nh, r / 2]
+        lambda: _native.qknorm_rope_vjp(z(12, 3, 2, 16), z(12, 3, 2, 16), z(6, 2), z(2, 4), z(2), 1e-6, 8, z(12, 3)),
+        lambda: _native.geglu_vjp(z(6, 10), z(6, 4)),
+        lambda: _native.geglu_vjp(z(6, 8), z(6, 4), out=z(6, 4)),
+        lambda: _native.split_vjp_gather(z(1, 4, 5, 3), z(1)),                                # odd fine grid
+        lambda: _native.split_vjp_gather(z(1, 4, 4, 3), z(2)),                                # fac is one float
+        lambda: _native.split_vjp_gather(z(1, 4, 4, 3), z(1), out=z(1, 2, 2, 3)),
+        lambda: _native.split_unpatch_lerp(z(1, 2, 2, 12), z(1, 4, 4, 4), z(1)),
+        lambda: _native.split_unpatch_lerp(z(1, 2, 2, 12), z(1, 4, 4, 3), z(1), out=z(1, 4, 4, 4)),
+        lambda: _native.merge_scatter_add(z(1, 2, 3, 12), z(1, 4, 4, 3)),
+        lambda: _native.patch_out_vjp(z(16, 32), z(32), z(12, 32), z(1, 3, 8, 8), (2, 3)),    # 8 is no multiple of 3
+        lambda: _native.patch_out_vjp(z(15, 32), z(32), z(12, 32), z(1, 3, 8, 8), (2, 2)),    # one token per patch
+        lambda: _native.patch_out_vjp(z(16, 32), z(32), z(12, 31), z(1, 3, 8, 8), (2, 2)),
+        lambda: _native.patch_out_vjp(z(16, 32), z(32), z(12, 32), z(1, 3, 8, 8), (2, 2), sigma_data=0.5),   # Karras needs sigma
+        lambda: _native.patch_out_vjp(z(16, 32), z(32), z(12, 32), z(1, 3, 8, 8), (2, 2), rstd=z(15)),
+        lambda: _native.patch_in_vjp(z(16, 32), z(32, 12), (1, 3, 8, 8), (2, 2), sigma=z(1), sigma_data=0.5),   # Karras needs u
+        lambda: _native.patch_in_vjp(z(16, 32), z(32, 12), (1, 3, 8, 8), (2, 2), u=z(1, 3, 8, 8), sigma=z(2), sigma_data=0.5),
+        lambda: _native.patch_in_vjp(z(16, 32), z(32, 13), (1, 3, 8, 8), (2, 2)),
+        lambda: _native.patch_in_vjp(z(16, 32), z(32, 12), (1, 3, 8, 8), (2, 2), out=z(1, 3, 8, 9)),
+    ]
+    for i, call in enumerate(bad):
+        with pytest.raises(ValueError):
+            call()
+            pytest.fail(f"case {i} was accepted")
+
+
+def test_vjp_entry_points_refuse_bad_geometry_without_gpu():
+    """The C entry points check extents and geometry before any CUDA call, so host addresses suffice to see each refusal"""
+    from k_diffusion import _native
+    L = _native.lib()
+    p = _native.ptr(torch.zeros(4))
+    n0 = _native.launch_count()
+    refusals = [
+        (-4, L.kdb_gemm_vjp(p, p, p, 8, 6, 8, 0, 0, 0, 0, None)),                      # N not a multiple of 4
+        (-4, L.kdb_gemm_vjp(p, p, p, 12, 8, 16, 1, 2, 3, 3, None)),                    # un-patch with K != 4 Cf
+        (-4, L.kdb_gemm_vjp(p, p, p, 10, 8, 16, 1, 2, 3, 4, None)),                    # not whole images
+        (-4, L.kdb_gemm_vjp(p, p, p, 2048 * 2048, 4, 4, 1, 2048, 2048, 1, None)),      # one image past 65535 row tiles
+        (-1, L.kdb_gemm_vjp(p, p, p, 12, 8, 16, 2, 2, 3, 4, None)),                    # no such epilogue
+        (-1, L.kdb_gemm_vjp(p, p, p, 12, 8, 16, 1, 0, 3, 4, None)),
+        (-1, L.kdb_rmsnorm_vjp(p, p, p, p, -8, 5, 10, 8, None)),
+        (-1, L.kdb_rmsnorm_vjp(p, p, p, p, 8, 0, 10, 8, None)),
+        (-4, L.kdb_qknorm_rope_vjp(p, p, p, p, p, 1e-6, 8, 12, 5, 2, 16, None, None)),  # rows no multiple of the tokens
+        (-4, L.kdb_qknorm_rope_vjp(p, p, p, p, p, 1e-6, 32, 12, 6, 2, 16, None, None)), # rotated width past d_head
+        (-4, L.kdb_qknorm_rope_vjp(p, p, p, p, p, 1e-6, 8, 12, 6, 2, 12, None, None)),  # d_head not a multiple of 8
+        (-1, L.kdb_geglu_vjp(p, p, p, 4, 0, None)),
+        (-4, L.kdb_split_vjp_gather(p, p, p, 1, 4, 5, 3, None)),
+        (-4, L.kdb_split_unpatch_lerp(p, p, p, p, 1, 3, 4, 3, None)),
+        (-4, L.kdb_merge_scatter_add(p, p, 1, 0, 4, 3, None)),
+        (-4, L.kdb_patch_out_vjp(p, p, p, p, None, 0.0, p, 1, 3, 8, 9, 2, 2, 32, None, None, None)),
+        (-1, L.kdb_patch_out_vjp(p, p, p, p, None, 0.5, p, 1, 3, 8, 8, 2, 2, 32, None, None, None)),    # Karras without sigma
+        (-2, L.kdb_patch_out_vjp(p, p, p, p, None, 0.0, p, 1, 3, 8, 8, 4, 4, 3025, None, None, None)),  # past 48 KiB
+        (-4, L.kdb_patch_in_vjp(p, p, None, None, 0.0, p, 1, 3, 9, 8, 2, 2, 32, None)),
+        (-1, L.kdb_patch_in_vjp(p, p, None, p, 0.5, p, 1, 3, 8, 8, 2, 2, 32, None)),                     # Karras without u
+    ]
+    for i, (want, rc) in enumerate(refusals):
+        assert rc == want, (i, rc, L.kdb_last_error())
+    assert _native.launch_count() == n0
+    _, inner, _ = model_of(CLASS)
+    eng_cfg = _native.Engine._config(inner.engine_spec())
+    h = ctypes.c_void_p()
+    assert L.kdb_model_create(ctypes.byref(eng_cfg), ctypes.byref(h)) == 0
+    try:
+        assert L.kdb_model_mapping_vjp(h, 2, p, None, p, None, p, p, p, None) == -6      # KDB_ERR_NOT_FINAL
+    finally:
+        L.kdb_model_destroy(h)
