@@ -69,6 +69,8 @@ CASES = [
     (32, 16, 16, 8, "global", 0),               # the cfg2 middle-level shape
     (3, 16, 32, 3, "global", 0),                # S = 512, odd head count, 36 tiles
     (1, 32, 64, 1, "global", 0),                # S = 2048: 16 key blocks through the ring of stages
+    (16, 32, 32, 16, "global", 0),              # the cfg5 middle-level shape (512x512 model, widths 256/512/1024, batch 16)
+    (64, 16, 16, 8, "global", 0),               # the cfg3 middle-level shape (256x256 neighbourhood model, batch 64)
 ]
 
 

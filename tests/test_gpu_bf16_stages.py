@@ -13,6 +13,7 @@ Routes:
   per_sample  one conditioning row per image: the stand-alone RMSNorm writes xn = bf16(x * g * rstd); the qkv (QKV_ROPE epilogue)
               and GEGLU GEMMs read xn with bf16(W)
 """
+import copy
 import math
 import time
 
@@ -184,8 +185,13 @@ def _sdpa(q, k, v, allow, emu):
     return (p @ v) / p.sum(-1, keepdim=True)
 
 
-def _attend(q, k, v, L, shift, nm, emu):
-    """q, k, v [B, h, w, nh, e] -> [B, h, w, nh, e] (oracle global / shifted-window / neighbourhood attention, scale 1)"""
+NA_DENSE_MAX_T = 1024    # larger neighbourhood grids take the gathered [T, 49] reference: a dense [T, T] mask of 128 x 128 tokens is 1 GiB
+
+
+def _attend(q, k, v, L, shift, nm, emu, gathered=None):
+    """q, k, v [B, h, w, nh, e] -> [B, h, w, nh, e] (oracle global / shifted-window / neighbourhood attention, scale 1).
+    Neighbourhood attention over more than NA_DENSE_MAX_T tokens (or with gathered=True) gathers each query's 49 keys instead of
+    masking a dense [T, T] score matrix (test_gpu_attn_na.na_attention)."""
     B, h, w, nh, e = q.shape
     if L.kind == "shifted-window":
         ws = L.ws
@@ -196,6 +202,9 @@ def _attend(q, k, v, L, shift, nm, emu):
         o = _sdpa(win(q), win(k), win(v), O.shifted_window_allow(h // ws, w // ws, ws, shift), emu)
         o = o.reshape(B, nh, h // ws, w // ws, ws, ws, e).permute(0, 2, 4, 3, 5, 1, 6).reshape(B, h, w, nh, e)
         return torch.roll(o, shifts=(-shift, -shift), dims=(1, 2))
+    if L.kind == "neighborhood" and (gathered if gathered is not None else h * w > NA_DENSE_MAX_T):
+        from test_gpu_attn_na import na_attention
+        return na_attention(q, k, v, p_bf16=emu, nm="noclamp" if nm == "na_noclamp" else None)
     f = lambda t: t.reshape(B, h * w, nh, e).transpose(1, 2)
     allow = None
     if L.kind == "neighborhood":
@@ -507,6 +516,12 @@ def na_raw():
                       "depths": [2, 2, 2], "widths": [128, 256, 512], "sigma_data": 0.5, "sigma_min": 1e-2, "sigma_max": 160}}
 
 
+def bench_raw(name):
+    """bench.py's model config of a workload (cfg3 and cfg4: _NA_RAW at 256x256; cfg5: widths 256/512/1024 at 512x512)"""
+    import bench
+    return copy.deepcopy(bench.CONFIGS[name]["raw"])
+
+
 def latent(seed, B, H, W, sigma):
     g = torch.Generator().manual_seed(seed)
     return torch.randn(B, 3, H, W, generator=g) * (sigma * sigma + 0.25).sqrt().view(-1, 1, 1, 1)
@@ -524,9 +539,17 @@ CONFIGS = {
     "w384_64_b2": (wide_raw, 64, 64, [2.5, 40.0], (0, 1)),
     # the tensor-core neighbourhood kernel (32 x 32 tokens at level 0), the generic one at level 1
     "na_128_b2": (na_raw, 128, 128, [2.5, 40.0], (1, 2)),
+    # cfg3 / cfg4's model: the tensor-core neighbourhood kernel at 64 x 64 tokens with 2 heads and 32 x 32 with 4, the global kernel
+    # over 256 tokens with 8 heads; layers 1, 3 and 4 are one layer of each level
+    "cfg3_256_b2": (lambda: bench_raw("cfg3"), 256, 256, [2.5, 40.0], (1, 3, 4)),
+    # cfg5's model: a 256-wide level 0 (no fused 128-wide kernels), all 8 row-statistics slots at width 1024, neighbourhood attention
+    # at 128 x 128 tokens, global attention over 1024 tokens with 16 heads, merges with K = 1024 and 2048, a split with N = 2048 and a
+    # down projection with K = 3072
+    "cfg5_512_b2": (lambda: bench_raw("cfg5"), 512, 512, [2.5, 40.0], (1, 3, 4)),
 }
 ROUTES = [("cfg2_256_b2", "shared"), ("cfg2_256_b2", "per_sample"), ("cfg2_64_b3", "shared"), ("cfg2_64x1024_b1", "shared"),
-          ("w384_64_b2", "shared"), ("na_128_b2", "shared")]
+          ("w384_64_b2", "shared"), ("na_128_b2", "shared"), ("cfg3_256_b2", "shared"), ("cfg3_256_b2", "per_sample"),
+          ("cfg5_512_b2", "shared")]
 
 
 @pytest.mark.gpu
@@ -586,6 +609,36 @@ def test_bf16_stages_vs_fp32_reference(config, route):
           f"; {time.time() - t0:.1f} s")
     assert not W.failures, "\n".join(W.failures)
     assert not W.missed, "\n".join(W.missed)
+
+
+@pytest.mark.gpu
+@pytest.mark.timeout(900)
+@pytest.mark.parametrize("config,B", [("cfg3_256_b2", 64), ("cfg5_512_b2", 16)])
+def test_benchmark_batch_images_equal_single_image_runs(config, B):
+    """At the benchmark's batch (cfg3: 64, cfg5: 16) on the sampler's shared route (one conditioning row, stride 0), images 0, B/2
+    and B - 1 of the batch are bit for bit the same images run alone.  Every kernel on this route computes an image's rows from that
+    image only, in an order fixed by the shapes of one image (test_gpu_gemm_schedule.py and test_gpu_attn_persistent.py assert it
+    kernel by kernel); here it holds for the whole forward, where a tile schedule, statistics slot or workspace offset that
+    depended on the batch would show."""
+    from k_diffusion import _native as N_
+    raw_fn, H, Wd, _, _ = CONFIGS[config]
+    inner, P = make(raw_fn(), H, Wd)
+    inner = inner.to(DEV).eval().set_precision("bf16")
+    eng = inner.engine()
+    t0 = time.time()
+    sigma = torch.full([B], 2.5)
+    img, s_d = latent(13, B, H, Wd, sigma).to(DEV), sigma.to(DEV)
+    table = eng.conditioning(s_d[:1])
+    full = eng.forward(img, s_d, table, 0, P.sigma_data, N_.PREC_BF16).clone()
+    torch.cuda.synchronize()
+    assert bool(torch.isfinite(full).all())
+    for b in (0, B // 2, B - 1):
+        one = eng.forward(img[b:b + 1].contiguous(), s_d[b:b + 1], table, 0, P.sigma_data, N_.PREC_BF16)
+        torch.cuda.synchronize()
+        d = (full[b:b + 1] - one).abs()
+        assert torch.equal(full[b:b + 1].view(torch.int32), one.view(torch.int32)), \
+            f"image {b} of {B} differs from the same image alone: {int((d > 0).sum())} elements, max |diff| {float(d.max()):.3g}"
+    print(f"{config} B={B}: {time.time() - t0:.1f} s")
 
 
 @pytest.mark.gpu
@@ -680,3 +733,24 @@ def test_stage_tolerance_accepts_emulation_and_rejects_near_misses(route):
     assert not W.missed, "\n".join(W.missed)
     # every near-miss kind was exercised at least once
     assert {"attn", "ff", "merge", "split", "patch_in", "out", "qkv", "ao", "geglu"} <= set(W.worst)
+
+
+@pytest.mark.parametrize("emu", [False, True], ids=["fp32", "emulation"])
+@pytest.mark.parametrize("nm", [None, "na_noclamp"])
+def test_gathered_and_dense_neighbourhood_references_agree(nm, emu):
+    """na_128_b2's neighbourhood levels (32 x 32 tokens with 2 heads, 16 x 16 with 4) on the CPU: the gathered reference that the
+    larger grids of cfg3 and cfg5 take gives what the dense mask gives, for the stage reference, its emulation and its near miss."""
+    _, P = make(na_raw(), 128, 128)
+    dt = _dt(emu)
+    for L in (P.down[0][0], P.down[1][0]):
+        assert L.kind == "neighborhood"
+        h = 32 >> L.level
+        g = torch.Generator().manual_seed(L.k)
+        q, k, v = (torch.randn(2, h, h, L.nh, L.e, generator=g, dtype=dt) for _ in range(3))
+        q, k = (t / t.norm(dim=-1, keepdim=True) * 10 ** 0.5 for t in (q, k))     # the cosine-sim scale of a layer: |q . k| <= 10
+        dense = _attend(q, k, v, L, 0, nm, emu, gathered=False)
+        gathered = _attend(q, k, v, L, 0, nm, emu, gathered=True)
+        assert float((dense - gathered).abs().max()) < (1e-12 if emu else 1e-5), f"level {L.level}"
+    # the near miss is a different answer at this size
+    if nm is not None:
+        assert float((_attend(q, k, v, L, 0, None, emu) - dense).abs().max()) > 0.1

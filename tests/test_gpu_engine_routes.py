@@ -11,8 +11,12 @@ Cases:
   cfg1_<prec>       the class-conditional MNIST model, fp32 and bf16
   tap_<part>        cfg2 at 64x64 on the shared route with layer1.<part> armed: that 128-wide layer leaves its fused kernel
   x_off, out_off    x or out starting 4 bytes into its storage: the scalar patch_in / patch_out kernels
+
+Recording: `python tests/test_gpu_engine_routes.py OUT.json [CASE ...]` runs the named cases (default: those the golden file lacks) on
+the GPU and writes the golden file with them to OUT.json.
 """
 import json
+import sys
 
 import pytest
 import torch
@@ -77,3 +81,31 @@ def test_engine_route(case):
     want = json.loads((GOLDEN / "engine_routes.json").read_text())[case]
     got = route_families(case)
     assert got == want, f"{case}: launches\n  {got}\nexpected\n  {want}"
+
+
+# the benchmark's neighbourhood models: every attention layer runs on a tensor-core kernel (attn_na_kernel at the two neighbourhood
+# levels, attn_ws_kernel at the global level), none on attn_generic
+BENCH_NA = {"cfg3_256_b2": "cfg3", "cfg5_512_b2": "cfg5"}
+
+
+@pytest.mark.parametrize("case", [f"{c}/{r}" for c in BENCH_NA for r in ("shared", "per_sample")])
+def test_benchmark_na_models_route_every_attention_to_tensor_cores(case):
+    from test_gpu_bf16_stages import bench_raw
+    routes = json.loads((GOLDEN / "engine_routes.json").read_text())
+    assert case in routes, f"{case} is not recorded"
+    depths = bench_raw(BENCH_NA[case.split("/")[0]])["model"]["depths"]
+    n_attn = 2 * sum(depths[:-1]) + depths[-1]            # down and up layers of every outer level, then the middle level
+    seq = routes[case]
+    assert "attn_generic" not in seq
+    assert seq.count("attn_tc") == n_attn, f"{seq.count('attn_tc')} attn_tc launches, {n_attn} attention layers"
+
+
+if __name__ == "__main__":
+    golden = json.loads((GOLDEN / "engine_routes.json").read_text())
+    todo = sys.argv[2:] or [c for c in CASES if c not in golden]
+    for c in todo:
+        golden[c] = route_families(c)
+        print(c, len(golden[c]), "launches")
+    ordered = {c: golden[c] for c in CASES if c in golden}
+    with open(sys.argv[1], "w") as f:
+        f.write(json.dumps(ordered, indent=1) + "\n")
