@@ -10,7 +10,6 @@
 #include <map>
 #include <string>
 #include <type_traits>
-#include <unordered_map>
 #include <vector>
 
 #include "model_core.cuh"
@@ -66,17 +65,7 @@ struct KdbModel : ModelCore {
   int ada_total = 0;
   CondWeights cw{};
   std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
-  std::unordered_map<std::string, TensorRef> grads;      // kdb_model_set_grad: gradient buffers by state-dict key (written, p is not const)
   std::vector<Tf32W> merge_t, split_t;
-  // ensure_tf32's device memory, one allocation per Tf32W copy in the order of its list, kept across finalizes instead of in `owned`.
-  // Separate allocations, not one buffer: with one buffer, kdb_model_finalize's reallocation of the owned buffers took ~13 ms instead of
-  // ~5.5 ms per rebind on cfg1 (H100 80GB HBM3, 700 W), which made every tf32 training step that much slower
-  std::vector<float*> tf32_mem;
-  bool tf32_ready = false;   // the Tf32W copies are of the weights the last finalize read
-
-  ~KdbModel() {
-    for (float* p : tf32_mem) cudaFree(p);
-  }
 };
 
 namespace {
@@ -327,13 +316,9 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
 }
 
 // The tf32 training precision's weight copies, built by the first tf32 call after a finalize: the Tf32W of every layer's qkv, out, up and
-// down projection, then of every level's merge and split, in KdbModel::tf32_mem
+// down projection, then of every level's merge and split, in the model's kept allocations (w, t of each in turn)
 int ensure_tf32(KdbModel* m, cudaStream_t st) {
-  if (m->tf32_ready) return 0;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  KDB_CUDA(cudaStreamIsCapturing(st, &cs));
-  KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED,
-              "the first tf32 training call after a finalize builds the tf32 weight copies: it must run outside CUDA-graph capture");
+  if (m->kept_ready) return 0;
   struct Copy { const float* src; int N, K; Tf32W* dst; };
   std::vector<Copy> copies;
   for (LayerPlan& L : m->layers) {
@@ -349,22 +334,19 @@ int ensure_tf32(KdbModel* m, cudaStream_t st) {
     copies.push_back({m->merge_w[l], c.width[l + 1], 4 * c.width[l], &m->merge_t[l]});
     copies.push_back({m->split_w[l], 4 * c.width[l], c.width[l + 1], &m->split_t[l]});
   }
-  while (m->tf32_mem.size() < 2 * copies.size()) {   // once per handle: the shapes are the config's
-    const Copy& k = copies[m->tf32_mem.size() / 2];
-    void* p = nullptr;
-    KDB_CUDA(cudaMalloc(&p, sizeof(float) * k.N * k.K + 1024));
-    m->tf32_mem.push_back(static_cast<float*>(p));
-  }
+  std::vector<size_t> floats;
+  for (const Copy& k : copies) floats.insert(floats.end(), 2, (size_t)k.N * k.K);
+  if (int rc = m->keep(floats, "tf32 training call after a finalize builds the tf32 weight copies", st)) return rc;
   for (size_t i = 0; i < copies.size(); ++i) {
-    copies[i].dst->w = m->tf32_mem[2 * i];
-    copies[i].dst->t = m->tf32_mem[2 * i + 1];
+    copies[i].dst->w = m->kept[2 * i];
+    copies[i].dst->t = m->kept[2 * i + 1];
   }
   for (const Copy& k : copies) {
     if (int rc = launch_unet_round_tf32(k.src, k.dst->w, (int64_t)k.N * k.K, st)) return rc;
     round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(k.K, 32), (unsigned)ceil_div(k.N, 32)), 256, 0, st>>>(k.src, k.dst->t, k.N, k.K);
     KDB_LAUNCH_CHECK(F_CONVERT, st);
   }
-  m->tf32_ready = true;
+  m->kept_ready = true;
   return 0;
 }
 
@@ -849,14 +831,9 @@ void carve_vjp(const KdbModelConfig& c, int B, int H, int W, void* workspace, Wo
   vs.total = cv.total();
 }
 
-// What kdb_model_forward_train adds to the reverse walk: the bound gradient buffers, and its precision.
+// What kdb_model_forward_train adds to the reverse walk besides the model's bound gradient buffers: its precision.
 struct Train {
-  const KdbModel* m;
   bool tf32;   // KDB_PREC_TF32: the forward, the recomputes and every token-stream input and weight gradient take the tf32 route
-  float* grad(const std::string& key) const {
-    auto it = m->grads.find(key);
-    return it == m->grads.end() ? nullptr : const_cast<float*>(it->second.p);
-  }
 };
 
 // The reverse walk's token-stream GEMMs: the input gradient dA [M, K] = dC [M, N] W [N, K] and the weight gradient dW [N, K] = dY^T X, on
@@ -890,12 +867,12 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
   if (tr) {   // down_proj's input, the GEGLU output
     float* gb = reinterpret_cast<float*>(f.ws.gbuf);
     if ((rc = launch_geglu<float>(hb, gb, M, F, st)) ||
-        (rc = weight_grad(f.tf32, g, C, gb, F, tr->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
+        (rc = weight_grad(f.tf32, g, C, gb, F, m->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
       return rc;
   }
   if ((rc = input_grad(f.tf32, g, L.down_w, L.down_t, vs.dbuf, M, C, F, st))) return rc;
   if ((rc = launch_geglu_vjp(hb, vs.dbuf, vs.dh, M, F, st))) return rc;
-  if (tr && (rc = weight_grad(f.tf32, vs.dh, 2 * F, xn, C, tr->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
+  if (tr && (rc = weight_grad(f.tf32, vs.dh, 2 * F, xn, C, m->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
   if ((rc = input_grad(f.tf32, vs.dh, L.up_w, L.up_t, xn, M, 2 * F, C, st))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_ff, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   if ((rc = launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, st))) return rc;
@@ -903,15 +880,15 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
   // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
   x = vs.tape[2 * k];
   if ((rc = attn_activations<float>(m, f, k, x, h, w, vs.qkv_raw))) return rc;
-  if (tr && (rc = weight_grad(f.tf32, g, C, ao, C, tr->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
+  if (tr && (rc = weight_grad(f.tf32, g, C, ao, C, m->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
   if ((rc = input_grad(f.tf32, g, L.out_w, L.out_t, vs.dbuf, M, C, C, st))) return rc;
   if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
   // the attention's statistics are spent: vs.stats takes the per-(row, head) terms of the head scales' gradient
   if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st, tr ? vs.stats : nullptr)))
     return rc;
-  if (tr && ((rc = launch_colsum(vs.stats, M, L.nh, tr->grad(sa + "scale"), vs.part, st)) ||
-             (rc = weight_grad(f.tf32, vs.dqkv, 3 * C, xn, C, tr->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
+  if (tr && ((rc = launch_colsum(vs.stats, M, L.nh, m->grad(sa + "scale"), vs.part, st)) ||
+             (rc = weight_grad(f.tf32, vs.dqkv, 3 * C, xn, C, m->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
     return rc;
   if ((rc = input_grad(f.tf32, vs.dqkv, L.qkv_w, L.qkv_t, xn, M, 3 * C, C, st))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_attn, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
@@ -942,9 +919,9 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
   if ((rc = launch_patch_out_vjp(vs.tape.back(), m->out_norm, m->patch_out_w, u, sigma, sd, vs.g[0], B, c.out_channels, H, W, c.patch_h,
                                  c.patch_w, C0, st, dnorm, tr ? vs.rstd : nullptr)))
     return rc;
-  if (tr && ((rc = launch_wgrad_patch_out(u, vs.tape.back(), m->out_norm, vs.rstd, tr->grad("patch_out.proj.weight"), B, c.out_channels, H, W,
+  if (tr && ((rc = launch_wgrad_patch_out(u, vs.tape.back(), m->out_norm, vs.rstd, m->grad("patch_out.proj.weight"), B, c.out_channels, H, W,
                                           c.patch_h, c.patch_w, C0, part, st)) ||
-             (rc = launch_norm_scale_grad(vs.tape.back(), C0, dnorm, C0, tr->grad("out_norm.scale"), 0, M0, M0, C0, part, st))))
+             (rc = launch_norm_scale_grad(vs.tape.back(), C0, dnorm, C0, m->grad("out_norm.scale"), 0, M0, M0, C0, part, st))))
     return rc;
   int k = (int)m->layers.size();
   float* mg = reinterpret_cast<float*>(ws.mg);
@@ -958,13 +935,13 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     const std::string sp = "splits." + std::to_string(l) + ".";
     if (tr) {   // d fac = sum (y - skip) dup with y = the split projection recomputed (vs.dbuf), skip = ws.xs[l]
       if ((rc = fwd_linear<float>(f, coarse, m->split_w[l], m->split_t[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{})) ||
-          (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], tr->grad(sp + "fac"), B, h, w, c.width[l],
+          (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], m->grad(sp + "fac"), B, h, w, c.width[l],
                                       part, st)))
         return rc;
     }
     // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
     if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
-    if (tr && (rc = weight_grad(tf32, mg, 4 * c.width[l], coarse, c.width[l + 1], tr->grad(sp + "proj.weight"), Mc, 4 * c.width[l],
+    if (tr && (rc = weight_grad(tf32, mg, 4 * c.width[l], coarse, c.width[l + 1], m->grad(sp + "proj.weight"), Mc, 4 * c.width[l],
                                 c.width[l + 1], part, st)))
       return rc;
     if ((rc = input_grad(tf32, mg, m->split_w[l], m->split_t[l], vs.g[l + 1], Mc, 4 * c.width[l], c.width[l + 1], st))) return rc;
@@ -974,7 +951,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
   for (int l = n - 2; l >= 0; --l) {
     const int h = h0 >> l, w = w0 >> l;
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
-    float* dmw = tr ? tr->grad("merges." + std::to_string(l) + ".proj.weight") : nullptr;
+    float* dmw = tr ? m->grad("merges." + std::to_string(l) + ".proj.weight") : nullptr;
     const float* fine = reinterpret_cast<const float*>(ws.xs[l]);
     if (dmw && (rc = tf32 ? launch_wgrad_tf32_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)
                           : launch_wgrad_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
@@ -993,7 +970,7 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
       if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w, tr))) return rc;
   }
   if (tr) {   // patch_in's input: the patch rows of x
-    if ((rc = launch_wgrad_patch_in(vs.g[0], x, tr->grad("patch_in.proj.weight"), B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, part, st)))
+    if ((rc = launch_wgrad_patch_in(vs.g[0], x, m->grad("patch_in.proj.weight"), B, c.in_channels, H, W, c.patch_h, c.patch_w, C0, part, st)))
       return rc;
     if (grad_x == nullptr) return 0;
   }
@@ -1060,7 +1037,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   m->free_all();
   m->pos_cache.clear();
   m->finalized = false;
-  m->tf32_ready = false;
+  m->kept_ready = false;
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, mw = c.mapping_width;
   m->layers.clear();
@@ -1296,11 +1273,8 @@ int kdb_model_forward_vjp(KdbModel* m, int precision, int batch, int height, int
 
 namespace {
 
-// A gradient buffer for `key` is refused unless the model has a tensor of that key and shape that is a parameter (not a buffer)
-int check_grad_key(const KdbModel* m, const std::string& k, const std::vector<int64_t>& shape) {
-  auto it = m->tensors.find(k);
-  KDB_REQUIRE(it != m->tensors.end(), KDB_ERR_MISSING_KEY, "gradient bound to '%s', which is no tensor of the model", k.c_str());
-  KDB_REQUIRE(it->second.shape == shape, KDB_ERR_BAD_SHAPE, "gradient of '%s' has the wrong shape", k.c_str());
+// The transformer's refusal rule for a gradient buffer (check_grad): the tensors that are buffers, not parameters
+int check_grad_key(const KdbModel*, const std::string& k) {
   const bool buffer = k == "time_emb.weight" || k == "aug_emb.weight" || (k.size() >= 13 && k.compare(k.size() - 13, 13, "pos_emb.freqs") == 0);
   KDB_REQUIRE(!buffer, KDB_ERR_BAD_ARG, "'%s' is a buffer, not a parameter", k.c_str());
   return 0;
@@ -1327,16 +1301,7 @@ int check_training_precision(const KdbModel* m, const char* what, int precision)
 extern "C" {
 
 int kdb_model_set_grad(KdbModel* m, const char* key, float* data, const int64_t* shape, int ndim) {
-  KDB_REQUIRE(m && key && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "set_grad: bad argument");
-  if (data == nullptr) {
-    m->grads.erase(key);
-    return 0;
-  }
-  if (int rc = check_grad_key(m, key, std::vector<int64_t>(shape, shape + ndim))) return rc;
-  ModelCore::TensorRef& t = m->grads[key];
-  t.p = data;
-  t.shape.assign(shape, shape + ndim);
-  return 0;
+  return set_grad(m, "set_grad", key, data, shape, ndim, check_grad_key);
 }
 
 int64_t kdb_model_train_workspace_bytes(const KdbModel* m, int batch, int height, int width) {
@@ -1358,18 +1323,14 @@ int kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, i
   const KdbModelConfig& c = m->cfg;
   KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "forward_train: NULL argument");
   if ((rc = check_conds(c, class_cond, mapping_cond))) return rc;
-  KDB_REQUIRE(cond_batch_stride == kdb_model_cond_stride(m), KDB_ERR_BAD_ARG,
-              "forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
-              (long long)kdb_model_cond_stride(m));
-  for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
-    if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
+  if ((rc = check_train(m, "forward_train", cond_batch_stride, kdb_model_cond_stride(m), check_grad_key))) return rc;
   if ((rc = check_image(m, "forward_train", height, width, 0.f))) return rc;
   Workspace ws;
   VjpSpace vs;
   carve_vjp(c, batch, height, width, workspace, ws, vs, m->ada_total, true);
   KDB_REQUIRE(vs.total <= workspace_bytes, KDB_ERR_WORKSPACE, "forward_train: workspace %zu < required %zu", workspace_bytes, vs.total);
   cudaStream_t st = (cudaStream_t)stream;
-  const Train tr{m, precision == KDB_PREC_TF32};
+  const Train tr{precision == KDB_PREC_TF32};
   if ((rc = m->disarm_tap(vjp_impl(m, batch, height, width, x, cotangent, sigma, 0.f, cond, cond_batch_stride, out, grad_x, ws, vs, st, &tr))))
     return rc;
   // AdaRMSNorm: scale = 1 + cond W^T per image, so d W = sum_b dscale_b cond_b (cond: the last mw floats of the conditioning row) and the
@@ -1379,10 +1340,10 @@ int kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, i
   float* part = vs.part;
   for (const LayerPlan& L : m->layers) {
     if (L.ada_attn >= 0 &&
-        (rc = launch_wgrad(vs.dscale + L.ada_attn, A, cond_vec, cond_batch_stride, tr.grad(L.prefix + "self_attn.norm.linear.weight"), B, L.C, mw,
+        (rc = launch_wgrad(vs.dscale + L.ada_attn, A, cond_vec, cond_batch_stride, m->grad(L.prefix + "self_attn.norm.linear.weight"), B, L.C, mw,
                            part, st)))
       return rc;
-    if ((rc = launch_wgrad(vs.dscale + L.ada_ff, A, cond_vec, cond_batch_stride, tr.grad(L.prefix + "ff.norm.linear.weight"), B, L.C, mw, part, st)))
+    if ((rc = launch_wgrad(vs.dscale + L.ada_ff, A, cond_vec, cond_batch_stride, m->grad(L.prefix + "ff.norm.linear.weight"), B, L.C, mw, part, st)))
       return rc;
   }
   if ((rc = launch_gemm_vjp(vs.dscale, m->ada_cat, vs.dcond, B, A, mw, VJP_STORE, 0, 0, 0, st)) ||
@@ -1393,23 +1354,23 @@ int kdb_model_forward_train(KdbModel* m, int precision, int batch, int height, i
   const int64_t K = ml.keep_floats(), G = ml.grad_floats();
   const float *keep = vs.map_keep, *grad = vs.map_grad;
   const int D = c.mapping_depth, F = c.mapping_d_ff;
-  if ((rc = launch_norm_scale_grad(keep + ml.r(D), K, vs.dcond, mw, tr.grad("mapping.out_norm.scale"), 0, B, B, mw, part, st))) return rc;
+  if ((rc = launch_norm_scale_grad(keep + ml.r(D), K, vs.dcond, mw, m->grad("mapping.out_norm.scale"), 0, B, B, mw, part, st))) return rc;
   for (int l = 0; l < D; ++l) {
     const std::string p = "mapping.blocks." + std::to_string(l) + ".";
-    if ((rc = launch_norm_scale_grad(keep + ml.r(l), K, grad + ml.dxn(l), G, tr.grad(p + "norm.scale"), 0, B, B, mw, part, st)) ||
-        (rc = launch_wgrad(grad + ml.dh(l), G, keep + ml.xn(l), K, tr.grad(p + "up_proj.weight"), B, 2 * F, mw, part, st)) ||
-        (rc = launch_wgrad(grad + ml.dr(l + 1), G, keep + ml.g(l), K, tr.grad(p + "down_proj.weight"), B, mw, F, part, st)))
+    if ((rc = launch_norm_scale_grad(keep + ml.r(l), K, grad + ml.dxn(l), G, m->grad(p + "norm.scale"), 0, B, B, mw, part, st)) ||
+        (rc = launch_wgrad(grad + ml.dh(l), G, keep + ml.xn(l), K, m->grad(p + "up_proj.weight"), B, 2 * F, mw, part, st)) ||
+        (rc = launch_wgrad(grad + ml.dr(l + 1), G, keep + ml.g(l), K, m->grad(p + "down_proj.weight"), B, mw, F, part, st)))
       return rc;
   }
   const float* demb = grad + ml.demb();
-  if ((rc = launch_norm_scale_grad(keep + ml.emb(), K, grad + ml.dr(0), G, tr.grad("mapping.in_norm.scale"), 0, B, B, mw, part, st)) ||
-      (rc = launch_wgrad(demb, G, keep + ml.ff_t(), K, tr.grad("time_in_proj.weight"), B, mw, mw, part, st)) ||
-      (rc = launch_wgrad(demb, G, keep + ml.ff_a(), K, tr.grad("aug_in_proj.weight"), B, mw, mw, part, st)))
+  if ((rc = launch_norm_scale_grad(keep + ml.emb(), K, grad + ml.dr(0), G, m->grad("mapping.in_norm.scale"), 0, B, B, mw, part, st)) ||
+      (rc = launch_wgrad(demb, G, keep + ml.ff_t(), K, m->grad("time_in_proj.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_wgrad(demb, G, keep + ml.ff_a(), K, m->grad("aug_in_proj.weight"), B, mw, mw, part, st)))
     return rc;
   if (c.mapping_cond_dim > 0 &&
-      (rc = launch_wgrad(demb, G, mapping_cond, c.mapping_cond_dim, tr.grad("mapping_cond_in_proj.weight"), B, mw, c.mapping_cond_dim, part, st)))
+      (rc = launch_wgrad(demb, G, mapping_cond, c.mapping_cond_dim, m->grad("mapping_cond_in_proj.weight"), B, mw, c.mapping_cond_dim, part, st)))
     return rc;
-  if (c.num_classes > 0) return launch_class_emb_grad(demb, G, class_cond, tr.grad("class_emb.weight"), B, c.num_classes, mw, st);
+  if (c.num_classes > 0) return launch_class_emb_grad(demb, G, class_cond, m->grad("class_emb.weight"), B, c.num_classes, mw, st);
   return 0;
 }
 

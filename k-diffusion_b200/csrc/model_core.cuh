@@ -1,5 +1,6 @@
 // model_core.cuh -- host-side state every model engine shares (engine.cu, unet_engine.cu): the borrowed state-dict tensors and their
-// shape-checked lookup, owned device allocations, the debug tap, and the carver that lays out a caller's workspace.
+// shape-checked lookup, the bound gradient buffers, owned device allocations and the derived copies kept across finalizes, the debug
+// tap, and the carver that lays out a caller's workspace.
 #pragma once
 #include <initializer_list>
 #include <string>
@@ -16,14 +17,24 @@ struct ModelCore {
     std::vector<int64_t> shape;
   };
   std::unordered_map<std::string, TensorRef> tensors;
+  std::unordered_map<std::string, TensorRef> grads;   // kdb_*_set_grad: gradient buffers by state-dict key (written: p is not const)
   bool finalized = false;
   std::vector<void*> owned;
+  // The derived weight copies a training call builds (ensure_tf32, ensure_bwd), one allocation per copy in the order of its list, kept
+  // across finalizes instead of in `owned`.  Separate allocations, not one buffer: with one buffer, kdb_model_finalize's reallocation of
+  // the owned buffers took ~13 ms instead of ~5.5 ms per rebind on cfg1 (H100 80GB HBM3, 700 W), which made every tf32 training step
+  // that much slower
+  std::vector<float*> kept;
+  bool kept_ready = false;   // the kept copies are of the weights the last finalize read
   // debug tap: armed by kdb_*_debug_tap, filled by the forward's tap() at the stage of that name, disarmed when the forward returns
   std::string tap_name;
   float* tap_out = nullptr;
   int64_t tap_cap = 0, tap_count = 0;
 
-  ~ModelCore() { free_all(); }
+  ~ModelCore() {
+    free_all();
+    for (float* p : kept) cudaFree(p);
+  }
 
   // the registered tensor `key`, which must have shape `want`
   int get(const std::string& key, std::initializer_list<int64_t> want, const float** out) const {
@@ -56,6 +67,26 @@ struct ModelCore {
   void free_all() {
     for (void* p : owned) cudaFree(p);
     owned.clear();
+  }
+
+  // The first build of the kept copies after a finalize, whose allocations hold floats[i] floats each: refused under CUDA-graph capture
+  // (`what`: the call and what it builds), and `kept` grown to them once per handle (the shapes are the config's)
+  int keep(const std::vector<size_t>& floats, const char* what, cudaStream_t st) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    KDB_CUDA(cudaStreamIsCapturing(st, &cs));
+    KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED, "the first %s: it must run outside CUDA-graph capture", what);
+    while (kept.size() < floats.size()) {
+      void* p = nullptr;
+      KDB_CUDA(cudaMalloc(&p, sizeof(float) * floats[kept.size()] + 1024));
+      kept.push_back(static_cast<float*>(p));
+    }
+    return 0;
+  }
+
+  // the gradient buffer bound to `key`, or nullptr
+  float* grad(const std::string& key) const {
+    auto it = grads.find(key);
+    return it == grads.end() ? nullptr : const_cast<float*>(it->second.p);
   }
 
   // copies the n elements at p to the armed tap buffer as fp32 when `name` is the armed stage (tap_count < 0: the buffer is too short)
@@ -102,6 +133,42 @@ inline int arm_tap(ModelCore* m, const char* name, float* out, int64_t capacity)
   m->tap_out = out;
   m->tap_cap = capacity;
   m->tap_count = 0;
+  return 0;
+}
+
+// A gradient buffer for `k` is refused unless the model has a tensor of that key and shape, and then by the engine's `rule` (the tensors
+// that are no parameter its training call writes)
+template <typename M>
+int check_grad(const M* m, const std::string& k, const std::vector<int64_t>& shape, int (*rule)(const M*, const std::string&)) {
+  auto it = m->tensors.find(k);
+  KDB_REQUIRE(it != m->tensors.end(), KDB_ERR_MISSING_KEY, "gradient bound to '%s', which is no tensor of the model", k.c_str());
+  KDB_REQUIRE(it->second.shape == shape, KDB_ERR_BAD_SHAPE, "gradient of '%s' has the wrong shape", k.c_str());
+  return rule(m, k);
+}
+
+// the kdb_*_set_grad entry points of every engine (data == nullptr unbinds `key`)
+template <typename M>
+int set_grad(M* m, const char* what, const char* key, float* data, const int64_t* shape, int ndim, int (*rule)(const M*, const std::string&)) {
+  KDB_REQUIRE(m && key && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "%s: bad argument", what);
+  if (data == nullptr) {
+    m->grads.erase(key);
+    return 0;
+  }
+  std::vector<int64_t> dims(shape, shape + ndim);
+  if (int rc = check_grad(m, key, dims, rule)) return rc;
+  m->grads[key] = ModelCore::TensorRef{data, dims};
+  return 0;
+}
+
+// the binding checks of every kdb_*_forward_train: one conditioning row per image, and every bound gradient again (the weights may have
+// been rebound since the gradients were)
+template <typename M>
+int check_train(const M* m, const char* what, int64_t cond_batch_stride, int64_t cond_stride, int (*rule)(const M*, const std::string&)) {
+  KDB_REQUIRE(cond_batch_stride == cond_stride, KDB_ERR_BAD_ARG,
+              "%s: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", what, (long long)cond_batch_stride,
+              (long long)cond_stride);
+  for (const auto& kv : m->grads)
+    if (int rc = check_grad(m, kv.first, kv.second.shape, rule)) return rc;
   return 0;
 }
 

@@ -47,13 +47,6 @@ struct KdbUNet : kdb::ModelCore {
   const float *proj_in_w = nullptr, *proj_in_b = nullptr, *proj_out_w = nullptr, *proj_out_b = nullptr;
   int ada_total = 0;
   kdb::UNetCondWeights cw{};
-  std::unordered_map<std::string, TensorRef> grads;   // kdb_unet_set_grad: gradient buffers by state-dict key
-  // ensure_bwd's flipped convolution weights, one allocation per weight in the order of mods, kept across finalizes instead of in `owned`
-  std::vector<float*> bwd_mem;
-  bool bwd_ready = false;
-  ~KdbUNet() {
-    for (float* p : bwd_mem) cudaFree(p);
-  }
 };
 
 using namespace kdb;
@@ -261,6 +254,34 @@ int run_attn(int prec, const UMod& u, const float* x, float* out, UWs& ws, int B
   return conv(prec, o, u.w2, 1, st);
 }
 
+// The one walk over the modules in execution order: fn(i, module, input, grid h, w before it, h, w after it, output channels, out) runs or
+// sizes module i and sets out to the buffer it wrote (x0: patch_in's output).  walk makes that the next module's input, and a DBlock's
+// last module's output the skip its level's UBlock concatenates.  M_CONCAT takes no call.
+template <typename Fn>
+int walk(const KdbUNet* m, int H, int W, float* x0, Fn fn) {
+  const KdbUNetConfig& c = m->cfg;
+  int h, w;
+  level_dims(c, H, W, c.skip_stages, &h, &w);
+  Src cur{x0, c.channels[std::max(0, c.skip_stages - 1)], nullptr, 0};
+  float* skip[KDB_MAX_LEVELS] = {};
+  for (size_t i = 0; i < m->mods.size(); ++i) {
+    const UMod& u = m->mods[i];
+    if (u.kind == M_CONCAT) {
+      cur.p2 = skip[u.level], cur.c2 = c.channels[u.level];
+      continue;
+    }
+    const int h0 = h, w0 = w;
+    int C = u.c_out;
+    if (u.kind == M_DOWN) h /= 2, w /= 2, C = cur.c1;
+    if (u.kind == M_UP) h *= 2, w *= 2, C = cur.c1;
+    float* dst = nullptr;
+    if (int rc = fn(i, u, cur, h0, w0, h, w, C, dst)) return rc;
+    if (u.to_skip) skip[u.level] = dst;
+    cur = Src{dst, C, nullptr, 0};
+  }
+  return 0;
+}
+
 // tape != nullptr (training): patch_in writes tape[0] and module i (of m->mods) tape[i + 1], which a DBlock's last module's UBlock then reads
 // as its skip; the launches are those of tape == nullptr
 int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cbs, float* out,
@@ -269,43 +290,24 @@ int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, cons
   const int s0 = c.skip_stages, C0 = c.channels[std::max(0, s0 - 1)];
   int h, w, rc;
   level_dims(c, H, W, s0, &h, &w);
-  float* x0 = tape ? tape[0] : ws.x[0];
-  if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, x0, B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
-  if ((rc = m->tap("patch_in", x0, (int64_t)B * h * w * C0, st))) return rc;
-  Src cur{x0, C0, nullptr, 0};
-  int cur_buf = 0;                         // index of the ping-pong buffer holding cur (-1: a skip buffer)
-  for (size_t i = 0; i < m->mods.size(); ++i) {
-    const UMod& u = m->mods[i];
-    const int nb = cur_buf == 0 ? 1 : 0;
-    float* dst = u.to_skip ? ws.skip[u.level] : ws.x[nb];
-    if (tape && u.kind != M_CONCAT) {
-      dst = tape[i + 1];
-      if (u.to_skip) ws.skip[u.level] = dst;
-    }
-    int C = u.c_out;
-    switch (u.kind) {
-      case M_DOWN:
-        if ((rc = launch_unet_resample(cur.p1, dst, B, h, w, cur.c1, false, st))) return rc;
-        h /= 2, w /= 2, C = cur.c1;
-        break;
-      case M_UP:
-        if ((rc = launch_unet_resample(cur.p1, dst, B, h, w, cur.c1, true, st))) return rc;
-        h *= 2, w *= 2, C = cur.c1;
-        break;
-      case M_CONCAT:
-        cur.p2 = ws.skip[u.level], cur.c2 = c.channels[u.level];
-        continue;
-      case M_RES:
-        if ((rc = run_res(prec, u, cur, dst, ws, B, h, w, cond, cbs, st))) return rc;
-        break;
-      default:
-        if ((rc = run_attn(prec, u, cur.p1, dst, ws, B, h, w, cond, cbs, st))) return rc;
-    }
-    if ((rc = m->tap(u.tap, dst, (int64_t)B * h * w * C, st))) return rc;
-    cur = Src{dst, C, nullptr, 0};
-    cur_buf = u.to_skip ? -1 : nb;
-  }
-  return launch_unet_patch_out(cur.p1, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, cur.c1, st);
+  float* y = tape ? tape[0] : ws.x[0];   // patch_in's output, then each module's in turn
+  if ((rc = launch_unet_patch_in(x, sigma, sd, m->proj_in_w, m->proj_in_b, y, B, c.in_channels, H, W, c.patch_size, C0, st))) return rc;
+  if ((rc = m->tap("patch_in", y, (int64_t)B * h * w * C0, st))) return rc;
+  // without a tape, a module writes its level's skip buffer or the ping-pong buffer its input is not in
+  rc = walk(m, H, W, y, [&](size_t i, const UMod& u, const Src& in, int hi, int wi, int ho, int wo, int C, float*& dst) {
+    dst = tape ? tape[i + 1] : u.to_skip ? ws.skip[u.level] : ws.x[in.p1 == ws.x[0] ? 1 : 0];
+    int rc;
+    if (u.kind == M_DOWN || u.kind == M_UP)
+      rc = launch_unet_resample(in.p1, dst, B, hi, wi, in.c1, u.kind == M_UP, st);
+    else if (u.kind == M_RES)
+      rc = run_res(prec, u, in, dst, ws, B, hi, wi, cond, cbs, st);
+    else
+      rc = run_attn(prec, u, in.p1, dst, ws, B, hi, wi, cond, cbs, st);
+    y = dst;
+    return rc ? rc : m->tap(u.tap, dst, (int64_t)B * ho * wo * C, st);
+  });
+  if (rc) return rc;
+  return launch_unet_patch_out(y, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, C0, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -330,31 +332,6 @@ struct ModIO {
   int h = 0, w = 0;
 };
 
-// The walk of unet_forward over the modules: fn(i, module, input, grid h, w, output channels)
-template <typename Fn>
-void walk(const KdbUNet* m, int H, int W, float* const* tape, Fn fn) {
-  const KdbUNetConfig& c = m->cfg;
-  int h, w;
-  level_dims(c, H, W, c.skip_stages, &h, &w);
-  Src cur{tape ? tape[0] : nullptr, c.channels[std::max(0, c.skip_stages - 1)], nullptr, 0};
-  float* skip[KDB_MAX_LEVELS] = {};
-  for (size_t i = 0; i < m->mods.size(); ++i) {
-    const UMod& u = m->mods[i];
-    if (u.kind == M_CONCAT) {
-      cur.p2 = skip[u.level], cur.c2 = c.channels[u.level];
-      continue;
-    }
-    const int h0 = h, w0 = w;
-    int C = u.c_out;
-    if (u.kind == M_DOWN) h /= 2, w /= 2, C = cur.c1;
-    if (u.kind == M_UP) h *= 2, w *= 2, C = cur.c1;
-    fn(i, u, cur, h0, w0, h, w, C);
-    float* dst = tape ? tape[i + 1] : nullptr;
-    if (u.to_skip) skip[u.level] = dst;
-    cur = Src{dst, C, nullptr, 0};
-  }
-}
-
 void carve_train(const KdbUNet* m, int B, int H, int W, void* workspace, TWs& t) {
   const KdbUNetConfig& c = m->cfg;
   carve(c, B, H, W, workspace, t.f);
@@ -368,10 +345,11 @@ void carve_train(const KdbUNet* m, int B, int H, int W, void* workspace, TWs& t)
   t.tape.assign(m->mods.size() + 1, nullptr);
   t.tape[0] = take(M0 * c.channels[std::max(0, s0 - 1)]);
   size_t elems = 0, stats = 0;
-  walk(m, H, W, nullptr, [&](size_t i, const UMod& u, const Src& in, int hi, int wi, int ho, int wo, int C) {
-    t.tape[i + 1] = take((size_t)B * ho * wo * C);
+  walk(m, H, W, t.tape[0], [&](size_t i, const UMod& u, const Src& in, int hi, int wi, int ho, int wo, int C, float*& dst) {
+    dst = t.tape[i + 1] = take((size_t)B * ho * wo * C);
     elems = std::max({elems, (size_t)B * hi * wi * (in.c1 + in.c2), (size_t)B * ho * wo * C, (size_t)B * hi * wi * 3 * u.c_out});
     if (u.kind == M_ATTN) stats = std::max(stats, (size_t)B * hi * wi * std::max(1, u.c_out / 64) * 3);
+    return 0;
   });
   t.g[0] = take(elems);
   t.g[1] = take(elems);
@@ -397,13 +375,9 @@ void carve_train(const KdbUNet* m, int B, int H, int W, void* workspace, TWs& t)
 }
 
 // The input-gradient weights of every convolution (launch_unet_flip_conv_weight of its tap-major copy), built by the first training call after
-// a finalize into KdbUNet::bwd_mem, in the order of mods
+// a finalize into the model's kept allocations, in the order of mods
 int ensure_bwd(KdbUNet* m, cudaStream_t st) {
-  if (m->bwd_ready) return 0;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  KDB_CUDA(cudaStreamIsCapturing(st, &cs));
-  KDB_REQUIRE(cs == cudaStreamCaptureStatusNone, KDB_ERR_UNSUPPORTED,
-              "the first training call after a finalize builds the input-gradient weights: it must run outside CUDA-graph capture");
+  if (m->kept_ready) return 0;
   struct Flip { const float* src; int N, C, ks; const float** dst; };
   std::vector<Flip> flips;
   for (UMod& u : m->mods) {
@@ -416,31 +390,21 @@ int ensure_bwd(KdbUNet* m, cudaStream_t st) {
       flips.push_back({u.w2.f32, u.c_out, u.c_out, 1, &u.w2t});
     }
   }
-  while (m->bwd_mem.size() < flips.size()) {   // once per handle: the shapes are the config's
-    const Flip& f = flips[m->bwd_mem.size()];
-    void* p = nullptr;
-    KDB_CUDA(cudaMalloc(&p, sizeof(float) * f.N * f.C * f.ks * f.ks + 1024));
-    m->bwd_mem.push_back(static_cast<float*>(p));
-  }
+  std::vector<size_t> floats;
+  for (const Flip& f : flips) floats.push_back((size_t)f.N * f.C * f.ks * f.ks);
+  if (int rc = m->keep(floats, "training call after a finalize builds the input-gradient weights", st)) return rc;
   for (size_t i = 0; i < flips.size(); ++i) {
     const Flip& f = flips[i];
-    if (int rc = launch_unet_flip_conv_weight(f.src, m->bwd_mem[i], f.N, f.C, f.ks, st)) return rc;
-    *f.dst = m->bwd_mem[i];
+    if (int rc = launch_unet_flip_conv_weight(f.src, m->kept[i], f.N, f.C, f.ks, st)) return rc;
+    *f.dst = m->kept[i];
   }
   KDB_CUDA(cudaStreamSynchronize(st));
-  m->bwd_ready = true;
+  m->kept_ready = true;
   return 0;
 }
 
-float* grad_of(const KdbUNet* m, const std::string& key) {
-  auto it = m->grads.find(key);
-  return it == m->grads.end() ? nullptr : const_cast<float*>(it->second.p);
-}
-
-int check_grad_key(const KdbUNet* m, const std::string& k, const std::vector<int64_t>& shape) {
-  auto it = m->tensors.find(k);
-  KDB_REQUIRE(it != m->tensors.end(), KDB_ERR_MISSING_KEY, "gradient bound to '%s', which is no tensor of the model", k.c_str());
-  KDB_REQUIRE(it->second.shape == shape, KDB_ERR_BAD_SHAPE, "gradient of '%s' has the wrong shape", k.c_str());
+// The U-Net's refusal rule for a gradient buffer (check_grad): the buffers, and the blocks below skip_stages
+int check_grad_key(const KdbUNet* m, const std::string& k) {
   const bool buffer = k == "timestep_embed.weight" || (k.size() >= 7 && k.compare(k.size() - 7, 7, ".kernel") == 0);
   KDB_REQUIRE(!buffer, KDB_ERR_BAD_ARG, "'%s' is a buffer, not a parameter", k.c_str());
   const KdbUNetConfig& c = m->cfg;
@@ -473,21 +437,21 @@ int res_vjp(KdbUNet* m, const UMod& u, const Src& in, const float* g, float* out
       (rc = launch_unet_adagn(ws.n2, u.c_mid, nullptr, 0, ws.qkv, cond, cbs, u.ada2, u.groups2, true, B, h * w, st)))
     return rc;
   // conv2: weight and bias gradients, then the gradient of n3 and through AdaGN2 + GELU that of h
-  if ((rc = launch_wgrad_conv(g, u.c_out, ws.qkv, u.c_mid, nullptr, 0, grad_of(m, p + "main.6.weight"), B, h, w, 3, t.part, st)) ||
-      (rc = launch_colsum(g, M, u.c_out, grad_of(m, p + "main.6.bias"), t.part, st)) ||
+  if ((rc = launch_wgrad_conv(g, u.c_out, ws.qkv, u.c_mid, nullptr, 0, m->grad(p + "main.6.weight"), B, h, w, 3, t.part, st)) ||
+      (rc = launch_colsum(g, M, u.c_out, m->grad(p + "main.6.bias"), t.part, st)) ||
       (rc = launch_unet_conv(conv_args(g, u.c_out, nullptr, 0, u.w2t, nullptr, t.ga, u.c_mid, B, h, w), 3, st)) ||
       (rc = launch_unet_adagn_vjp(ws.n2, u.c_mid, nullptr, 0, t.ga, nullptr, t.gb, nullptr, cond, cbs, u.ada2, t.dss, A, u.groups2, true, B, h * w,
                                   st)))
     return rc;
   // conv1, then the gradient of n1
-  if ((rc = launch_wgrad_conv(t.gb, u.c_mid, ws.n1, u.c_in, nullptr, 0, grad_of(m, p + "main.2.weight"), B, h, w, 3, t.part, st)) ||
-      (rc = launch_colsum(t.gb, M, u.c_mid, grad_of(m, p + "main.2.bias"), t.part, st)) ||
+  if ((rc = launch_wgrad_conv(t.gb, u.c_mid, ws.n1, u.c_in, nullptr, 0, m->grad(p + "main.2.weight"), B, h, w, 3, t.part, st)) ||
+      (rc = launch_colsum(t.gb, M, u.c_mid, m->grad(p + "main.2.bias"), t.part, st)) ||
       (rc = launch_unet_conv(conv_args(t.gb, u.c_mid, nullptr, 0, u.w1t, nullptr, t.ga, u.c_in, B, h, w), 3, st)))
     return rc;
   // the skip path's gradient (the 1x1 conv's input gradient, or g itself) is added by AdaGN1's backward
   const float* add = g;
   if (u.skip_t != nullptr) {
-    if ((rc = launch_wgrad_conv(g, u.c_out, in.p1, in.c1, in.p2, in.c2, grad_of(m, p + "skip.weight"), B, h, w, 1, t.part, st)) ||
+    if ((rc = launch_wgrad_conv(g, u.c_out, in.p1, in.c1, in.p2, in.c2, m->grad(p + "skip.weight"), B, h, w, 1, t.part, st)) ||
         (rc = launch_unet_conv(conv_args(g, u.c_out, nullptr, 0, u.skip_t, nullptr, t.gb, u.c_in, B, h, w), 1, st)))
       return rc;
     add = t.gb;
@@ -504,14 +468,14 @@ int attn_vjp(KdbUNet* m, const UMod& u, const float* x, const float* g, float* o
   const int C = u.c_out, nh = std::max(1, C / 64);
   const float scale = 1.f / std::sqrt((float)(C / nh));
   const std::string& p = u.prefix;
-  float *dwq = grad_of(m, p + "qkv_proj.weight"), *dbq = grad_of(m, p + "qkv_proj.bias");
+  float *dwq = m->grad(p + "qkv_proj.weight"), *dbq = m->grad(p + "qkv_proj.bias");
   int rc;
   if ((rc = launch_unet_adagn(x, C, nullptr, 0, ws.n1, cond, cbs, u.ada1, u.groups1, false, B, h * w, st)) ||
       (rc = launch_unet_conv(conv_args(ws.n1, C, nullptr, 0, u.w1.f32, u.b1, ws.qkv, 3 * C, B, h, w), 1, st)) ||
       (rc = launch_attention_generic<float>(ws.qkv, ws.ao, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st)))
     return rc;
-  if ((rc = launch_wgrad_conv(g, C, ws.ao, C, nullptr, 0, grad_of(m, p + "out_proj.weight"), B, h, w, 1, t.part, st)) ||
-      (rc = launch_colsum(g, M, C, grad_of(m, p + "out_proj.bias"), t.part, st)) ||
+  if ((rc = launch_wgrad_conv(g, C, ws.ao, C, nullptr, 0, m->grad(p + "out_proj.weight"), B, h, w, 1, t.part, st)) ||
+      (rc = launch_colsum(g, M, C, m->grad(p + "out_proj.bias"), t.part, st)) ||
       (rc = launch_unet_conv(conv_args(g, C, nullptr, 0, u.w2t, nullptr, t.ga, C, B, h, w), 1, st)) ||
       (rc = launch_attention_vjp(ws.qkv, ws.ao, t.ga, t.dqkv, t.stats, B, h, w, nh, C / nh, KDB_ATTN_GLOBAL, 0, 0, st)))
     return rc;
@@ -538,12 +502,16 @@ int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sig
   float* part = t.part;
   // proj_out + pixel_shuffle: U = the patch rows of u, with a zero column for the variance channel the output drops
   if ((rc = launch_unet_unshuffle(u, t.U, B, c.in_channels, H, W, p, Kout, st)) ||
-      (rc = launch_wgrad(t.U, Kout, t.tape.back(), C0, grad_of(m, "proj_out.weight"), M0, Kout, C0, part, st)) ||
-      (rc = launch_colsum(t.U, M0, Kout, grad_of(m, "proj_out.bias"), part, st)) ||
+      (rc = launch_wgrad(t.U, Kout, t.tape.back(), C0, m->grad("proj_out.weight"), M0, Kout, C0, part, st)) ||
+      (rc = launch_colsum(t.U, M0, Kout, m->grad("proj_out.bias"), part, st)) ||
       (rc = launch_unet_proj_out_vjp(t.U, m->proj_out_w, t.g[0], M0, Kout, C0, st)))
     return rc;
   std::vector<ModIO> io(m->mods.size());
-  walk(m, H, W, t.tape.data(), [&](size_t i, const UMod&, const Src& in, int hi, int wi, int, int, int) { io[i] = ModIO{in, hi, wi}; });
+  walk(m, H, W, t.tape[0], [&](size_t i, const UMod&, const Src& in, int hi, int wi, int, int, int, float*& dst) {
+    io[i] = ModIO{in, hi, wi};
+    dst = t.tape[i + 1];
+    return 0;
+  });
   int gi = 0;   // t.g[gi]: the gradient of the output of the module being reversed
   for (size_t k = m->mods.size(); k-- > 0;) {
     const UMod& mod = m->mods[k];
@@ -569,8 +537,8 @@ int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sig
   }
   // proj_in: its input is the pixel_unshuffle of x (the caller's c_in-scaled input)
   if ((rc = launch_unet_unshuffle(x, t.xin, B, c.in_channels, H, W, p, Kin, st)) ||
-      (rc = launch_wgrad(t.g[gi], C0, t.xin, Kin, grad_of(m, "proj_in.weight"), M0, C0, Kin, part, st)) ||
-      (rc = launch_colsum(t.g[gi], M0, C0, grad_of(m, "proj_in.bias"), part, st)))
+      (rc = launch_wgrad(t.g[gi], C0, t.xin, Kin, m->grad("proj_in.weight"), M0, C0, Kin, part, st)) ||
+      (rc = launch_colsum(t.g[gi], M0, C0, m->grad("proj_in.bias"), part, st)))
     return rc;
   // the AdaGN mappers, concatenated as at finalize: one weight gradient over the B conditioning rows, scattered to the bound keys; then the
   // gradient of the mapping network's output and its backward
@@ -581,21 +549,21 @@ int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sig
     for (int i = 0; i < n_ada; ++i) {
       const int off = i ? mod.ada2 : mod.ada1, C = i ? mod.c_mid : (mod.kind == M_RES ? mod.c_in : mod.c_out);
       const std::string key = mod.prefix + (mod.kind == M_ATTN ? "norm_in." : i ? "main.4." : "main.0.");
-      if (float* dw = grad_of(m, key + "mapper.weight"))
+      if (float* dw = m->grad(key + "mapper.weight"))
         KDB_CUDA(cudaMemcpyAsync(dw, t.dwcat + (size_t)off * mw, sizeof(float) * 2 * C * mw, cudaMemcpyDeviceToDevice, st));
-      if (float* db = grad_of(m, key + "mapper.bias"))
+      if (float* db = m->grad(key + "mapper.bias"))
         KDB_CUDA(cudaMemcpyAsync(db, t.dbcat + off, sizeof(float) * 2 * C, cudaMemcpyDeviceToDevice, st));
     }
   }
   const UNetMapGrad& mg = t.mg;
   if ((rc = launch_gemm_vjp(t.dss, m->cw.ada_w, t.dcond, B, A, mw, VJP_STORE, 0, 0, 0, st)) ||
       (rc = launch_unet_mapping_vjp(m->cw, B, sigma, aug, mcond, t.dcond, mg, st)) ||
-      (rc = launch_wgrad(mg.dz1, mw, mg.a0, mw, grad_of(m, "mapping.2.weight"), B, mw, mw, part, st)) ||
-      (rc = launch_colsum(mg.dz1, B, mw, grad_of(m, "mapping.2.bias"), part, st)) ||
-      (rc = launch_wgrad(mg.dz0, mw, mg.h0, mw, grad_of(m, "mapping.0.weight"), B, mw, mw, part, st)) ||
-      (rc = launch_colsum(mg.dz0, B, mw, grad_of(m, "mapping.0.bias"), part, st)))
+      (rc = launch_wgrad(mg.dz1, mw, mg.a0, mw, m->grad("mapping.2.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_colsum(mg.dz1, B, mw, m->grad("mapping.2.bias"), part, st)) ||
+      (rc = launch_wgrad(mg.dz0, mw, mg.h0, mw, m->grad("mapping.0.weight"), B, mw, mw, part, st)) ||
+      (rc = launch_colsum(mg.dz0, B, mw, m->grad("mapping.0.bias"), part, st)))
     return rc;
-  return mcd > 0 ? launch_wgrad(mg.dh0, mw, mg.v, mcd, grad_of(m, "mapping_cond.weight"), B, mw, mcd, part, st) : 0;
+  return mcd > 0 ? launch_wgrad(mg.dh0, mw, mg.v, mcd, m->grad("mapping_cond.weight"), B, mw, mcd, part, st) : 0;
 }
 
 // the grid checks of kdb_unet_forward and kdb_unet_forward_train
@@ -662,7 +630,7 @@ int kdb_unet_finalize(KdbUNet* m, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   m->free_all();
   m->finalized = false;
-  m->bwd_ready = false;
+  m->kept_ready = false;
   m->mods.clear();
   m->ada_total = 0;
   const KdbUNetConfig& c = m->cfg;
@@ -763,16 +731,7 @@ int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width
 }
 
 int kdb_unet_set_grad(KdbUNet* m, const char* key, float* data, const int64_t* shape, int ndim) {
-  KDB_REQUIRE(m && key && ndim >= 0 && ndim <= 4 && (ndim == 0 || shape), KDB_ERR_BAD_ARG, "unet_set_grad: bad argument");
-  if (data == nullptr) {
-    m->grads.erase(key);
-    return 0;
-  }
-  if (int rc = check_grad_key(m, key, std::vector<int64_t>(shape, shape + ndim))) return rc;
-  ModelCore::TensorRef& t = m->grads[key];
-  t.p = data;
-  t.shape.assign(shape, shape + ndim);
-  return 0;
+  return set_grad(m, "unet_set_grad", key, data, shape, ndim, check_grad_key);
 }
 
 int64_t kdb_unet_train_workspace_bytes(const KdbUNet* m, int batch, int height, int width) {
@@ -793,11 +752,7 @@ int kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int
   const KdbUNetConfig& c = m->cfg;
   int rc;
   if ((rc = check_conds(c, "unet_forward_train", aug_cond, mapping_cond))) return rc;
-  KDB_REQUIRE(cond_batch_stride == kdb_unet_cond_stride(m), KDB_ERR_BAD_ARG,
-              "unet_forward_train: one conditioning row per image (cond_batch_stride %lld, the row stride is %lld)", (long long)cond_batch_stride,
-              (long long)kdb_unet_cond_stride(m));
-  for (const auto& kv : m->grads)   // again here: the weights may have been rebound since the gradients were
-    if ((rc = check_grad_key(m, kv.first, kv.second.shape))) return rc;
+  if ((rc = check_train(m, "unet_forward_train", cond_batch_stride, kdb_unet_cond_stride(m), check_grad_key))) return rc;
   if ((rc = check_grid(c, "unet_forward_train", height, width))) return rc;
   TWs t;
   carve_train(m, batch, height, width, workspace, t);

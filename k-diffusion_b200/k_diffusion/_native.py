@@ -566,7 +566,7 @@ class EngineCache:
 class Engine:
     """Owns one native model handle on one device: a KdbModel for an ImageTransformerDenoiserModelV2 or V1 (`_api` "model"), or, in the
     UNetEngine subclass, a KdbUNet for an ImageDenoiserModelV1 (`_api` "unet").  Both handles take the same calls (create, destroy,
-    set_tensor, finalize, cond_stride, workspace_bytes, forward, debug_tap, tap_count) under kdb_<api>_*."""
+    set_tensor, finalize, cond_stride, workspace_bytes, forward, set_grad, train_workspace_bytes, debug_tap, tap_count) under kdb_<api>_*."""
 
     _api = "model"
 
@@ -720,6 +720,22 @@ class Engine:
                                               ptr(u), ptr(out), ptr(out_grad), ptr(ws), ws.numel(), stream()))
         return out, out_grad
 
+    def train_workspace(self, B, H, W):
+        """kdb_<api>_train_workspace_bytes: the workspace of forward_train for B images"""
+        need = int(self._fn("train_workspace_bytes")(self._h, B, H, W))
+        if need < 0:
+            check(need)
+        return need
+
+    def set_grad(self, grads):
+        """Binds `grads` ({state-dict key: fp32 CUDA tensor of the parameter's shape}) and unbinds every other key bound before."""
+        for k in self._grad_keys - set(grads):
+            check(self._fn("set_grad")(self._h, k.encode(), None, None, 0))
+        for k, g in grads.items():
+            dims = (_i64 * g.ndim)(*g.shape)
+            check(self._fn("set_grad")(self._h, k.encode(), ptr(g), dims, g.ndim))
+        self._grad_keys = set(grads)
+
     def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32):
         """Parameter gradients at the training precision (PREC_FP32 or PREC_TF32): binds `grads` ({state-dict key: fp32 CUDA tensor of the
         parameter's shape}, every other key unbound), then one kdb_model_forward_train: out = F(x), every bound gradient = u^T dF/dparam,
@@ -729,13 +745,8 @@ class Engine:
         if tuple(u.shape) != shape:
             raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {shape}")
         out = torch.empty(shape, device=x.device, dtype=torch.float32) if out is None else out
-        for k in self._grad_keys - set(grads):
-            check(lib().kdb_model_set_grad(self._h, k.encode(), None, None, 0))
-        for k, g in grads.items():
-            dims = (_i64 * g.ndim)(*g.shape)
-            check(lib().kdb_model_set_grad(self._h, k.encode(), ptr(g), dims, g.ndim))
-        self._grad_keys = set(grads)
-        ws = self._reserve(lib().kdb_model_train_workspace_bytes(self._h, B, H, W), x.device)
+        self.set_grad(grads)
+        ws = self._reserve(self.train_workspace(B, H, W), x.device)
         with device_of(x):
             check(lib().kdb_model_forward_train(self._h, precision, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(class_cond),
                                                 ptr(mapping_cond), ptr(cond), self._stride, ptr(u), ptr(out), ptr(grad_x), ptr(ws), ws.numel(),
@@ -838,22 +849,6 @@ class UNetEngine(Engine):
             check(lib().kdb_unet_mapping_vjp(self._h, rows, ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(dcond),
                                              *(ptr(res[k]) for k in ("h0", "a0", "dz0", "dz1", "dh0", "v")), stream()))
         return res
-
-    def train_workspace(self, B, H, W):
-        """kdb_unet_train_workspace_bytes: the workspace of forward_train for B images"""
-        need = int(lib().kdb_unet_train_workspace_bytes(self._h, B, H, W))
-        if need < 0:
-            check(need)
-        return need
-
-    def set_grad(self, grads):
-        """Binds `grads` ({state-dict key: fp32 CUDA tensor of the parameter's shape}) and unbinds every other key bound before."""
-        for k in self._grad_keys - set(grads):
-            check(lib().kdb_unet_set_grad(self._h, k.encode(), None, None, 0))
-        for k, g in grads.items():
-            dims = (_i64 * g.ndim)(*g.shape)
-            check(lib().kdb_unet_set_grad(self._h, k.encode(), ptr(g), dims, g.ndim))
-        self._grad_keys = set(grads)
 
     def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32):
         """Parameter gradients at fp32 (kdb_unet_forward_train), with Engine.forward_train's arguments: binds `grads`, then out = F(x) and
