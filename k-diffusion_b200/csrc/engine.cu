@@ -25,19 +25,26 @@ struct Tf32W {
   float* t = nullptr;
 };
 
+// A token-stream Linear (qkv, out, up, down, merge, split): its fp32 weight w [N, K] and the weight's copy for each route, wb for bf16
+// sampling (bind, at finalize) and t for tf32 training (ensure_tf32).  lin_fwd, lin_dx and lin_dw pick the copy and the kernel.
+struct Lin {
+  const float* w = nullptr;
+  bf16* wb = nullptr;
+  Tf32W t;
+  int N = 0, K = 0;
+};
+
 struct LayerPlan {
   std::string prefix;
   int level = 0, attn_type = 0, attn_param = 0, shift = 0;
   int C = 0, dff = 0, nh = 0, e = 0;
   int ada_attn = -1, ada_ff = -1;   // offsets into a conditioning row
-  const float *attn_norm_w = nullptr, *qkv_w = nullptr, *out_w = nullptr;
+  const float *attn_norm_w = nullptr, *ff_norm_w = nullptr;
+  Lin qkv, out, up, down;
   QkRope qr;                         // cosine-sim + RoPE of q and k (freqs always, scale for v1: finalize's tables)
-  const float *ff_norm_w = nullptr, *up_w = nullptr, *down_w = nullptr;
-  bf16 *qkv_wb = nullptr, *out_wb = nullptr, *up_wb = nullptr, *down_wb = nullptr;
   bf16* up_wb_il = nullptr;          // up_proj rows interleaved (value/gate) for the fused GEGLU epilogue
   bool bounded = false;              // every qr.scale[h] in (0, KDB_ATTN_MAX_BOUND]: the scale is the attention kernels' fixed softmax shift
   bf16 *qkv_wf = nullptr, *up_wf = nullptr;   // per-evaluation copies with the AdaRMSNorm channel scale folded in (fused norm)
-  Tf32W qkv_t, out_t, up_t, down_t;
 };
 
 struct PosTables {
@@ -52,9 +59,9 @@ using namespace kdb;
 struct KdbModel : ModelCore {
   KdbModelConfig cfg{};
   std::vector<LayerPlan> layers;   // in execution order (for_each_layer)
-  std::vector<const float*> merge_w, split_w, split_fac;
+  std::vector<Lin> merge, split;   // per level l < n_levels - 1
+  std::vector<const float*> split_fac;
   const float *patch_in_w = nullptr, *out_norm = nullptr, *patch_out_w = nullptr;
-  std::vector<bf16*> merge_wb, split_wb;
   float* ada_cat = nullptr;
   FoldDesc* fold_descs = nullptr;   // device table for launch_fold_norm_weights
   int n_fold = 0;
@@ -65,7 +72,6 @@ struct KdbModel : ModelCore {
   int ada_total = 0;
   CondWeights cw{};
   std::map<std::pair<int, int>, PosTables> pos_cache;   // position tables per token grid, in owned allocations
-  std::vector<Tf32W> merge_t, split_t;
 };
 
 namespace {
@@ -103,6 +109,18 @@ int permuted_rows(KdbModel* m, const float* src, int64_t rows, int64_t cols, P&&
   if (rc) return rc;
   for (int64_t r = 0; r < rows; ++r) std::copy_n(a.begin() + perm(r) * cols, cols, b.begin() + r * cols);
   return upload(m, b, out, st);
+}
+
+// Binds the token-stream Linear `key` [N, K]: lin.w is the state-dict tensor (with `perm`, an owned copy whose row r is its row perm(r)),
+// lin.wb the bf16 copy of lin.w
+template <typename P = std::nullptr_t>
+int bind(KdbModel* m, Lin& lin, const std::string& key, int N, int K, cudaStream_t st, P perm = nullptr) {
+  GET(key, &lin.w, N, K);
+  lin.N = N;
+  lin.K = K;
+  if constexpr (!std::is_null_pointer_v<P>)
+    if (int rc = permuted_rows(m, lin.w, N, K, perm, &lin.w, st)) return rc;
+  return make_bf16(m, lin.w, (int64_t)N * K, &lin.wb, st);
 }
 
 // image_transformer_v1's patch feature order (c i j) (Patching / Unpatching, image_transformer_v1.py:223,242) -> the engine's (i j c)
@@ -178,8 +196,6 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
     L.shift = (L.attn_type == KDB_ATTN_SHIFTED_WINDOW && (index % 2 == 1)) ? L.attn_param / 2 : 0;
     const std::string a = prefix + "self_attn.";
     GET(a + "norm.linear.weight", &L.attn_norm_w, L.C, mw);
-    GET(a + "qkv_proj.weight", &L.qkv_w, 3 * L.C, L.C);
-    GET(a + "out_proj.weight", &L.out_w, L.C, L.C);
     L.ada_attn = *ada_off;
     *ada_off += L.C;
     int rc;
@@ -210,7 +226,7 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
         const int64_t base = r - r % e, j = r % e;
         return base + (j < e / 2 ? 2 * j : 2 * (j - e / 2) + 1);
       };
-      if ((rc = permuted_rows(m, L.qkv_w, 3 * C, C, perm, &L.qkv_w, st)) || (rc = upload(m, hs, &L.qr.scale, st))) return rc;
+      if ((rc = bind(m, L.qkv, a + "qkv_proj.weight", 3 * L.C, L.C, st, perm)) || (rc = upload(m, hs, &L.qr.scale, st))) return rc;
       L.qr.eps = (float)e * 1e-6f;
       L.qr.R = e;
     } else {
@@ -219,33 +235,30 @@ int plan_layer(KdbModel* m, LayerPlan& L, const std::string& prefix, int level, 
       GET(a + "scale", &L.qr.scale, nh);
       GET(a + "pos_emb.freqs", &f, nh, e / 8);
       std::vector<float> fv;
-      if ((rc = download(L.qr.scale, nh, hs, st)) || (rc = download(f, (size_t)nh * (e / 8), fv, st))) return rc;
+      if ((rc = bind(m, L.qkv, a + "qkv_proj.weight", 3 * L.C, L.C, st)) || (rc = download(L.qr.scale, nh, hs, st)) ||
+          (rc = download(f, (size_t)nh * (e / 8), fv, st)))
+        return rc;
       tab.resize((size_t)nh * (e / 4));
       for (int h = 0; h < nh; ++h)
         for (int j = 0; j < e / 4; ++j) tab[(size_t)h * (e / 4) + j] = fv[(size_t)h * (e / 8) + j % (e / 8)];
       L.qr.eps = 1e-6f;
       L.qr.R = e / 2;
     }
-    if ((rc = upload(m, tab, &L.qr.freqs, st))) return rc;
+    if ((rc = upload(m, tab, &L.qr.freqs, st)) || (rc = bind(m, L.out, a + "out_proj.weight", L.C, L.C, st))) return rc;
     // |q . k| <= scale_h after the cosine-similarity normalisation: usable as a fixed softmax shift while exp(-2 scale) stays normal
     L.bounded = true;
     for (float v : hs) L.bounded = L.bounded && v > 0.f && v <= KDB_ATTN_MAX_BOUND;
-    if ((rc = make_bf16(m, L.qkv_w, 3LL * L.C * L.C, &L.qkv_wb, st))) return rc;
-    if ((rc = make_bf16(m, L.out_w, (int64_t)L.C * L.C, &L.out_wb, st))) return rc;
     if ((rc = m->alloc(&L.qkv_wf, (size_t)3 * L.C * L.C))) return rc;
   }
   const std::string f = prefix + "ff.";
   GET(f + "norm.linear.weight", &L.ff_norm_w, L.C, mw);
-  GET(f + "up_proj.weight", &L.up_w, 2 * L.dff, L.C);
-  GET(f + "down_proj.weight", &L.down_w, L.C, L.dff);
   L.ada_ff = *ada_off;
   *ada_off += L.C;
   int rc;
-  if ((rc = make_bf16(m, L.up_w, 2LL * L.dff * L.C, &L.up_wb, st))) return rc;
-  if ((rc = make_bf16(m, L.down_w, (int64_t)L.C * L.dff, &L.down_wb, st))) return rc;
+  if ((rc = bind(m, L.up, f + "up_proj.weight", 2 * L.dff, L.C, st)) || (rc = bind(m, L.down, f + "down_proj.weight", L.C, L.dff, st))) return rc;
   if (L.dff % 8 == 0) {
     if ((rc = m->alloc(&L.up_wb_il, (size_t)2 * L.dff * L.C))) return rc;
-    interleave_geglu_rows_kernel<<<kNumSMs * 4, 256, 0, st>>>(L.up_w, L.up_wb_il, L.dff, L.C);
+    interleave_geglu_rows_kernel<<<kNumSMs * 4, 256, 0, st>>>(L.up.w, L.up_wb_il, L.dff, L.C);
     KDB_LAUNCH_CHECK(F_CONVERT, st);
     if ((rc = m->alloc(&L.up_wf, (size_t)2 * L.dff * L.C))) return rc;
   }
@@ -319,31 +332,19 @@ int ensure_pos(KdbModel* m, int h0, int w0, cudaStream_t st, PosTables** out) {
 // down projection, then of every level's merge and split, in the model's kept allocations (w, t of each in turn)
 int ensure_tf32(KdbModel* m, cudaStream_t st) {
   if (m->kept_ready) return 0;
-  struct Copy { const float* src; int N, K; Tf32W* dst; };
-  std::vector<Copy> copies;
+  std::vector<Lin*> lins;
   for (LayerPlan& L : m->layers) {
-    if (L.attn_type != KDB_ATTN_NONE) {
-      copies.push_back({L.qkv_w, 3 * L.C, L.C, &L.qkv_t});
-      copies.push_back({L.out_w, L.C, L.C, &L.out_t});
-    }
-    copies.push_back({L.up_w, 2 * L.dff, L.C, &L.up_t});
-    copies.push_back({L.down_w, L.C, L.dff, &L.down_t});
+    if (L.attn_type != KDB_ATTN_NONE) lins.insert(lins.end(), {&L.qkv, &L.out});
+    lins.insert(lins.end(), {&L.up, &L.down});
   }
-  const KdbModelConfig& c = m->cfg;
-  for (int l = 0; l < c.n_levels - 1; ++l) {
-    copies.push_back({m->merge_w[l], c.width[l + 1], 4 * c.width[l], &m->merge_t[l]});
-    copies.push_back({m->split_w[l], 4 * c.width[l], c.width[l + 1], &m->split_t[l]});
-  }
+  for (int l = 0; l < m->cfg.n_levels - 1; ++l) lins.insert(lins.end(), {&m->merge[l], &m->split[l]});
   std::vector<size_t> floats;
-  for (const Copy& k : copies) floats.insert(floats.end(), 2, (size_t)k.N * k.K);
+  for (const Lin* k : lins) floats.insert(floats.end(), 2, (size_t)k->N * k->K);
   if (int rc = m->keep(floats, "tf32 training call after a finalize builds the tf32 weight copies", st)) return rc;
-  for (size_t i = 0; i < copies.size(); ++i) {
-    copies[i].dst->w = m->kept[2 * i];
-    copies[i].dst->t = m->kept[2 * i + 1];
-  }
-  for (const Copy& k : copies) {
-    if (int rc = launch_unet_round_tf32(k.src, k.dst->w, (int64_t)k.N * k.K, st)) return rc;
-    round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(k.K, 32), (unsigned)ceil_div(k.N, 32)), 256, 0, st>>>(k.src, k.dst->t, k.N, k.K);
+  for (size_t i = 0; i < lins.size(); ++i) lins[i]->t = Tf32W{m->kept[2 * i], m->kept[2 * i + 1]};
+  for (const Lin* k : lins) {
+    if (int rc = launch_unet_round_tf32(k->w, k->t.w, (int64_t)k->N * k->K, st)) return rc;
+    round_tf32_transpose_kernel<<<dim3((unsigned)ceil_div(k->K, 32), (unsigned)ceil_div(k->N, 32)), 256, 0, st>>>(k->w, k->t.t, k->N, k->K);
     KDB_LAUNCH_CHECK(F_CONVERT, st);
   }
   m->kept_ready = true;
@@ -384,39 +385,6 @@ void carve(const KdbModelConfig& c, int prec, int B, int H, int W, Carver& cv, W
   ws.total = cv.total();
 }
 
-template <typename T> struct WSel;
-template <> struct WSel<float> {
-  typedef float W;
-  static const float* qkv(const LayerPlan& L) { return L.qkv_w; }
-  static const float* out(const LayerPlan& L) { return L.out_w; }
-  static const float* up(const LayerPlan& L) { return L.up_w; }
-  static const float* down(const LayerPlan& L) { return L.down_w; }
-  static const float* merge(const KdbModel* m, int l) { return m->merge_w[l]; }
-  static const float* split(const KdbModel* m, int l) { return m->split_w[l]; }
-};
-template <> struct WSel<bf16> {
-  typedef bf16 W;
-  static const bf16* qkv(const LayerPlan& L) { return L.qkv_wb; }
-  static const bf16* out(const LayerPlan& L) { return L.out_wb; }
-  static const bf16* up(const LayerPlan& L) { return L.up_wb; }
-  static const bf16* down(const LayerPlan& L) { return L.down_wb; }
-  static const bf16* merge(const KdbModel* m, int l) { return m->merge_wb[l]; }
-  static const bf16* split(const KdbModel* m, int l) { return m->split_wb[l]; }
-};
-
-// Linear dispatch: tensor-core kernel when the shape qualifies (bf16 only), SIMT otherwise.
-template <typename T>
-int linear(const T* A, const typename WSel<T>::W* W, T* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st);
-template <>
-int linear<float>(const float* A, const float* W, float* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st) {
-  return launch_gemm_simt<float, float>(A, W, C, M, N, K, epi, st);
-}
-template <>
-int linear<bf16>(const bf16* A, const bf16* W, bf16* C, int64_t M, int N, int K, const GemmEpi& epi, cudaStream_t st) {
-  if (tc_gemm_supported(M, N, K, epi)) return launch_gemm_tc(A, W, C, M, N, K, epi, st);
-  return launch_gemm_simt<bf16, bf16>(A, W, C, M, N, K, epi, st);
-}
-
 // One forward's state: its workspace, stream and conditioning rows, and what the fused RMSNorm may use.
 struct Fwd {
   int B;
@@ -430,7 +398,7 @@ struct Fwd {
   bool stats;               // ws.rowss holds the row statistics of the current residual stream
   bool jvp;                 // fp32 forward-mode derivative: images [B, 2B) of every token buffer carry the tangent of images [0, B)
   float* const* tape = nullptr;   // fp32 reverse mode: slot 2k / 2k+1 keep the residual stream entering layer k's attention / feed-forward half
-  bool tf32 = false;              // fp32 tokens, the tf32 training route: every token-stream Linear on the tensor cores (fwd_linear)
+  bool tf32 = false;              // fp32 tokens, the tf32 training route: every token-stream Linear on the tensor cores (lin_fwd, lin_dx)
 
   // images held by the token buffers: linear launches and taps cover them all, nonlinear primal launches the first B
   int images() const { return jvp ? 2 * B : B; }
@@ -453,12 +421,46 @@ int linear_tf32(const float* A, const float* w, float* out, int64_t M, int N, in
   return launch_unet_conv_tf32(a, 1, st, F_GEMM_TF32);
 }
 
-// A token-stream Linear of the forward (STORE or RESID): linear_tf32 on the copy wt on the tf32 route, else linear<T>
+// The forward of a token-stream Linear, C [M, N] = A [M, K] lin^T with the epilogue e (STORE, RESID or SPLIT_LERP): at bf16 the
+// tensor-core GEMM where it runs the problem, else the SIMT GEMM, on lin.wb; at fp32 the SIMT GEMM on lin.w; on the tf32 route
+// linear_tf32 on lin.t.w, which has no split epilogue: TokenSplit stores its projection to ws.mg and un-patches it with the lerp.
 template <typename T>
-int fwd_linear(const Fwd& f, const T* A, const typename WSel<T>::W* W, const Tf32W& wt, T* C, int64_t M, int N, int K, const GemmEpi& e) {
-  if constexpr (std::is_same_v<T, float>)
-    if (f.tf32) return linear_tf32(A, wt.w, C, M, N, K, e.mode == EPI_RESID ? static_cast<const float*>(e.resid) : nullptr, f.st);
-  return linear<T>(A, W, C, M, N, K, e, f.st);
+int lin_fwd(const Fwd& f, const T* A, const Lin& lin, T* C, int64_t M, const GemmEpi& e) {
+  const int N = lin.N, K = lin.K;
+  if constexpr (std::is_same_v<T, bf16>) {
+    if (tc_gemm_supported(M, N, K, e)) return launch_gemm_tc(A, lin.wb, C, M, N, K, e, f.st);
+    return launch_gemm_simt<bf16, bf16>(A, lin.wb, C, M, N, K, e, f.st);
+  } else {
+    if (!f.tf32) return launch_gemm_simt<float, float>(A, lin.w, C, M, N, K, e, f.st);
+    if (e.mode != EPI_SPLIT_LERP)
+      return linear_tf32(A, lin.t.w, C, M, N, K, e.mode == EPI_RESID ? static_cast<const float*>(e.resid) : nullptr, f.st);
+    float* y = reinterpret_cast<float*>(f.ws.mg);
+    int rc = linear_tf32(A, lin.t.w, y, M, N, K, nullptr, f.st);
+    return rc ? rc : launch_split_unpatch_lerp(y, static_cast<const float*>(e.resid), e.fac, C, f.images(), 2 * e.hc, 2 * e.wc, e.C, f.st);
+  }
+}
+
+// The input gradient of a token-stream Linear, dA [M, K] = dC [M, N] lin: exact fp32 (gemm_vjp on lin.w), or linear_tf32 on the
+// transposed copy lin.t.t on the tf32 route.  hc > 0: the Linear is a TokenMerge over an hc x wc coarse grid, and dA is un-patched 2x2 and
+// added to out, the fine stream's gradient; on the tf32 route dA goes to ws.mg and a scatter kernel adds it.
+int lin_dx(const Fwd& f, const float* dC, const Lin& lin, float* out, int64_t M, int hc = 0, int wc = 0) {
+  const int N = lin.N, K = lin.K;
+  if (!f.tf32) return launch_gemm_vjp(dC, lin.w, out, M, N, K, hc > 0 ? VJP_UNPATCH_ACC : VJP_STORE, hc, wc, hc > 0 ? K / 4 : 0, f.st);
+  if (hc == 0) return linear_tf32(dC, lin.t.t, out, M, K, N, nullptr, f.st);
+  float* d = reinterpret_cast<float*>(f.ws.mg);
+  int rc = linear_tf32(dC, lin.t.t, d, M, K, N, nullptr, f.st);
+  return rc ? rc : launch_merge_scatter_add(d, out, f.images(), 2 * hc, 2 * wc, K / 4, f.st);
+}
+
+// The weight gradient of a token-stream Linear, dW [N, K] = dY^T X over M rows: exact fp32 (wgrad), or tf32 operands on the tensor cores.
+// hc > 0: X is the fine stream of a TokenMerge over an hc x wc coarse grid, gathered 2x2 as the merge reads it (ldx unused).  The route
+// is a flag, not a Fwd: kdb_wgrad calls this outside any forward.
+int lin_dw(bool tf32, const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part, cudaStream_t st,
+           int hc = 0, int wc = 0) {
+  if (hc > 0)
+    return tf32 ? launch_wgrad_tf32_merge(dY, ldy, X, dW, M, N, hc, wc, K / 4, part, st)
+                : launch_wgrad_merge(dY, ldy, X, dW, M, N, hc, wc, K / 4, part, st);
+  return tf32 ? launch_wgrad_tf32(dY, ldy, X, ldx, dW, M, N, K, part, st) : launch_wgrad(dY, ldy, X, ldx, dW, M, N, K, part, st);
 }
 
 // The attention half's activations from the residual stream x, up to the attention output in ws.ao: the qkv projection goes to raw,
@@ -488,7 +490,7 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
   };
   auto unfused = [&] {
     int r = norm();
-    if (!r) r = fwd_linear<T>(f, xn, WSel<T>::qkv(L), L.qkv_t, raw, Ma, 3 * C, C, GemmEpi{});
+    if (!r) r = lin_fwd<T>(f, xn, L.qkv, raw, Ma, GemmEpi{});
     // the tangent reads the un-normalised primal q and k, so it runs before the primal launch
     if constexpr (std::is_same_v<T, float>)
       if (!r && f.jvp) r = launch_qknorm_rope_jvp(raw, raw + M * 3 * C, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
@@ -511,7 +513,7 @@ int attn_activations(KdbModel* m, Fwd& f, int k, const T* x, int h, int w, T* ra
       rc = launch_gemm_tc(x, L.qkv_wf, qkv, M, 3 * C, C, qf, f.st);
       if (!rc && qf.mode == EPI_STORE) rc = launch_qknorm_rope<T>(qkv, qkv, pos, L.qr, M, (int)Ttok, L.nh, L.e, f.st);
     } else if (qe.mode == EPI_QKV_ROPE && tc_gemm_supported(M, 3 * C, C, qe)) {
-      if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv_wb, qkv, M, 3 * C, C, qe, f.st);
+      if (!(rc = norm())) rc = launch_gemm_tc(xn, L.qkv.wb, qkv, M, 3 * C, C, qe, f.st);
     } else {
       rc = unfused();
     }
@@ -539,7 +541,7 @@ int ff_up(KdbModel* m, Fwd& f, int k, const T* x, int h, int w) {
   int r = launch_rmsnorm<T>(x, xn, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
   if constexpr (std::is_same_v<T, float>)
     if (!r && f.jvp) r = launch_rmsnorm_jvp(x, x + M * C, xn + M * C, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, f.st);
-  return r ? r : fwd_linear<T>(f, xn, WSel<T>::up(L), L.up_t, reinterpret_cast<T*>(f.ws.hbuf), f.images() * Ttok, 2 * L.dff, C, GemmEpi{});
+  return r ? r : lin_fwd<T>(f, xn, L.up, reinterpret_cast<T*>(f.ws.hbuf), f.images() * Ttok, GemmEpi{});
 }
 
 template <typename T>
@@ -560,7 +562,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
                        tc_attn_block_supported(h, w, C, L.nh, L.e, L.attn_type, L.attn_param, L.shift);
     if constexpr (std::is_same_v<T, bf16>) {
       if (block) {
-        if ((rc = launch_attn_block(x, L.qkv_wf, L.out_wb, rope, L.qr.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st))) return rc;
+        if ((rc = launch_attn_block(x, L.qkv_wf, L.out.wb, rope, L.qr.scale, f.B, h, w, L.shift, f.ws.rowss, f.ws.rowss, f.st))) return rc;
         f.stats = true;
       }
     }
@@ -570,7 +572,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
       e.mode = EPI_RESID;
       e.resid = x;
       f.produce(e, Ma, C, C);
-      if ((rc = fwd_linear<T>(f, reinterpret_cast<T*>(f.ws.ao), WSel<T>::out(L), L.out_t, x, Ma, C, C, e))) return rc;
+      if ((rc = lin_fwd<T>(f, reinterpret_cast<T*>(f.ws.ao), L.out, x, Ma, e))) return rc;
     }
     if ((rc = m->tap<T>(tag + ".attn", x, Ma * C, f.st))) return rc;
   }
@@ -596,7 +598,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     GemmEpi gf = ge;
     gf.ss_in = f.ws.rowss;
     if (ffn) {
-      rc = launch_ffn_fused(x, L.up_wf, L.down_wb, M, C, L.dff, f.ws.rowss, f.ws.rowss, f.st);
+      rc = launch_ffn_fused(x, L.up_wf, L.down.wb, M, C, L.dff, f.ws.rowss, f.ws.rowss, f.st);
       f.stats = true;
     } else if (f.fold && f.stats && L.up_wf != nullptr && tc_gemm_supported(M, 2 * L.dff, C, gf)) {
       rc = launch_gemm_tc(x, L.up_wf, gb, M, 2 * L.dff, C, gf, f.st);
@@ -616,7 +618,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
     e.mode = EPI_RESID;
     e.resid = x;
     f.produce(e, Ma, C, L.dff);
-    if ((rc = fwd_linear<T>(f, gb, WSel<T>::down(L), L.down_t, x, Ma, C, L.dff, e))) return rc;
+    if ((rc = lin_fwd<T>(f, gb, L.down, x, Ma, e))) return rc;
   }
   return m->tap<T>(tag + ".ff", x, Ma * C, f.st);
 }
@@ -627,8 +629,7 @@ int run_layer(KdbModel* m, Fwd& f, int k, T* x, int h, int w) {
 // tape != nullptr (fp32 only): the residual stream entering every attention / feed-forward half and out_norm is copied to the tape
 // (slots 2k, 2k+1 of layer k, slot 2 * layers for out_norm) for the reverse walk of kdb_model_forward_vjp; the launches are unchanged.
 // pos_tables != nullptr: receives the position tables of this token grid.
-// tf32 (fp32 only): the tf32 training route, every token-stream Linear through linear_tf32 on ensure_tf32's copies; TokenSplit then stores
-// its projection to ws.mg and un-patches it with the lerp in launch_split_unpatch_lerp.
+// tf32 (fp32 only): the tf32 training route, every token-stream Linear through linear_tf32 on ensure_tf32's copies (lin_fwd).
 template <typename T>
 int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* v, const float* sigma, float sd, const float* cond,
                  int64_t cond_bs, float* out, float* out_t, Workspace& ws, cudaStream_t st, float* const* tape = nullptr,
@@ -683,7 +684,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       T* mg = reinterpret_cast<T*>(ws.mg);
       f.stats = false;
       int r = launch_merge_gather<T>(cur, mg, Bt, h, w, c.width[l], st);
-      return r ? r : fwd_linear<T>(f, mg, WSel<T>::merge(m, l), m->merge_t[l], nxt, Mc, N, K, GemmEpi{});
+      return r ? r : lin_fwd<T>(f, mg, m->merge[l], nxt, Mc, GemmEpi{});
     };
     // TokenMerge: the 2x2 gather rides on the GEMM's TMA loads when the geometry allows, else a gather kernel and a plain GEMM
     if constexpr (kBf16) {
@@ -693,7 +694,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
       me.mwc = w / 2;
       if (tc_gemm_supported(Mc, N, K, me)) {
         f.produce(me, Mc, N, K);
-        rc = launch_gemm_tc(cur, m->merge_wb[l], nxt, Mc, N, K, me, st);
+        rc = launch_gemm_tc(cur, m->merge[l].wb, nxt, Mc, N, K, me, st);
       } else {
         rc = merge();
       }
@@ -719,16 +720,7 @@ int forward_impl(KdbModel* m, int B, int H, int W, const float* x, const float* 
     e.wc = w;
     e.C = c.width[l];
     f.produce(e, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1]);
-    if (tf32) {
-      if constexpr (!kBf16) {
-        float* y = reinterpret_cast<float*>(ws.mg);
-        if ((rc = linear_tf32(cur, m->split_t[l].w, y, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], nullptr, st)) ||
-            (rc = launch_split_unpatch_lerp(y, reinterpret_cast<const float*>(ws.xs[l]), m->split_fac[l], up, Bt, 2 * h, 2 * w, c.width[l], st)))
-          return rc;
-      }
-    } else if ((rc = linear<T>(cur, WSel<T>::split(m, l), up, (int64_t)Bt * h * w, 4 * c.width[l], c.width[l + 1], e, st))) {
-      return rc;
-    }
+    if ((rc = lin_fwd<T>(f, cur, m->split[l], up, (int64_t)Bt * h * w, e))) return rc;
     h *= 2;
     w *= 2;
     if ((rc = m->tap<T>("L" + std::to_string(l) + ".split", up, (int64_t)Bt * h * w * c.width[l], st))) return rc;
@@ -836,16 +828,6 @@ struct Train {
   bool tf32;   // KDB_PREC_TF32: the forward, the recomputes and every token-stream input and weight gradient take the tf32 route
 };
 
-// The reverse walk's token-stream GEMMs: the input gradient dA [M, K] = dC [M, N] W [N, K] and the weight gradient dW [N, K] = dY^T X, on
-// the tf32 route on the tensor cores (linear_tf32 on the transposed copy, launch_wgrad_tf32), else exact fp32
-int input_grad(bool tf32, const float* dC, const float* W, const Tf32W& wt, float* out, int64_t M, int N, int K, cudaStream_t st) {
-  return tf32 ? linear_tf32(dC, wt.t, out, M, K, N, nullptr, st) : launch_gemm_vjp(dC, W, out, M, N, K, VJP_STORE, 0, 0, 0, st);
-}
-int weight_grad(bool tf32, const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part,
-                cudaStream_t st) {
-  return tf32 ? launch_wgrad_tf32(dY, ldy, X, ldx, dW, M, N, K, part, st) : launch_wgrad(dY, ldy, X, ldx, dW, M, N, K, part, st);
-}
-
 // Layer k in reverse: g holds the gradient of the layer's output residual stream and receives that of its input.  Each half recomputes
 // its activations from the tape with the forward's functions (ff_up, attn_activations; f is an fp32 forward of B images), runs the
 // backward kernels and adds the branch gradient to g.
@@ -867,30 +849,30 @@ int vjp_layer(KdbModel* m, Fwd& f, VjpSpace& vs, int k, float* g, int h, int w, 
   if (tr) {   // down_proj's input, the GEGLU output
     float* gb = reinterpret_cast<float*>(f.ws.gbuf);
     if ((rc = launch_geglu<float>(hb, gb, M, F, st)) ||
-        (rc = weight_grad(f.tf32, g, C, gb, F, m->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
+        (rc = lin_dw(f.tf32, g, C, gb, F, m->grad(ff + "down_proj.weight"), M, C, F, vs.part, st)))
       return rc;
   }
-  if ((rc = input_grad(f.tf32, g, L.down_w, L.down_t, vs.dbuf, M, C, F, st))) return rc;
+  if ((rc = lin_dx(f, g, L.down, vs.dbuf, M))) return rc;
   if ((rc = launch_geglu_vjp(hb, vs.dbuf, vs.dh, M, F, st))) return rc;
-  if (tr && (rc = weight_grad(f.tf32, vs.dh, 2 * F, xn, C, m->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
-  if ((rc = input_grad(f.tf32, vs.dh, L.up_w, L.up_t, xn, M, 2 * F, C, st))) return rc;
+  if (tr && (rc = lin_dw(f.tf32, vs.dh, 2 * F, xn, C, m->grad(ff + "up_proj.weight"), M, 2 * F, C, vs.part, st))) return rc;
+  if ((rc = lin_dx(f, vs.dh, L.up, xn, M))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_ff, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   if ((rc = launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_ff, f.cond_bs, Ttok, M, C, st))) return rc;
   if (L.attn_type == KDB_ATTN_NONE) return 0;
   // attention half: x + out(attn(qknorm_rope(qkv(norm(x)))))
   x = vs.tape[2 * k];
   if ((rc = attn_activations<float>(m, f, k, x, h, w, vs.qkv_raw))) return rc;
-  if (tr && (rc = weight_grad(f.tf32, g, C, ao, C, m->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
-  if ((rc = input_grad(f.tf32, g, L.out_w, L.out_t, vs.dbuf, M, C, C, st))) return rc;
+  if (tr && (rc = lin_dw(f.tf32, g, C, ao, C, m->grad(sa + "out_proj.weight"), M, C, C, vs.part, st))) return rc;
+  if ((rc = lin_dx(f, g, L.out, vs.dbuf, M))) return rc;
   if ((rc = launch_attention_vjp(qkv, ao, vs.dbuf, vs.dqkv, vs.stats, f.B, h, w, L.nh, L.e, L.attn_type, L.attn_param, L.shift, st)))
     return rc;
   // the attention's statistics are spent: vs.stats takes the per-(row, head) terms of the head scales' gradient
   if ((rc = launch_qknorm_rope_vjp(vs.qkv_raw, vs.dqkv, f.pt->pos[L.level], L.qr, M, (int)Ttok, L.nh, L.e, st, tr ? vs.stats : nullptr)))
     return rc;
   if (tr && ((rc = launch_colsum(vs.stats, M, L.nh, m->grad(sa + "scale"), vs.part, st)) ||
-             (rc = weight_grad(f.tf32, vs.dqkv, 3 * C, xn, C, m->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
+             (rc = lin_dw(f.tf32, vs.dqkv, 3 * C, xn, C, m->grad(sa + "qkv_proj.weight"), M, 3 * C, C, vs.part, st))))
     return rc;
-  if ((rc = input_grad(f.tf32, vs.dqkv, L.qkv_w, L.qkv_t, xn, M, 3 * C, C, st))) return rc;
+  if ((rc = lin_dx(f, vs.dqkv, L.qkv, xn, M))) return rc;
   if (tr && (rc = launch_norm_scale_grad(x, C, xn, C, vs.dscale + L.ada_attn, m->ada_total, Ttok, M, C, vs.part, st))) return rc;
   return launch_rmsnorm_vjp(x, xn, g, f.cond + L.ada_attn, f.cond_bs, Ttok, M, C, st);
 }
@@ -934,17 +916,17 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
     const std::string sp = "splits." + std::to_string(l) + ".";
     if (tr) {   // d fac = sum (y - skip) dup with y = the split projection recomputed (vs.dbuf), skip = ws.xs[l]
-      if ((rc = fwd_linear<float>(f, coarse, m->split_w[l], m->split_t[l], vs.dbuf, Mc, 4 * c.width[l], c.width[l + 1], GemmEpi{})) ||
+      if ((rc = lin_fwd<float>(f, coarse, m->split[l], vs.dbuf, Mc, GemmEpi{})) ||
           (rc = launch_split_fac_grad(vs.dbuf, reinterpret_cast<const float*>(ws.xs[l]), vs.g[l], m->grad(sp + "fac"), B, h, w, c.width[l],
                                       part, st)))
         return rc;
     }
     // up = lerp(skip, unpatch(cur W^T), fac): the coarse stream gets patch2x2(fac dup) W, the skip keeps (1 - fac) dup in g[l]
     if ((rc = launch_split_vjp_gather(vs.g[l], mg, m->split_fac[l], B, h, w, c.width[l], st))) return rc;
-    if (tr && (rc = weight_grad(tf32, mg, 4 * c.width[l], coarse, c.width[l + 1], m->grad(sp + "proj.weight"), Mc, 4 * c.width[l],
-                                c.width[l + 1], part, st)))
+    if (tr && (rc = lin_dw(tf32, mg, 4 * c.width[l], coarse, c.width[l + 1], m->grad(sp + "proj.weight"), Mc, 4 * c.width[l], c.width[l + 1],
+                           part, st)))
       return rc;
-    if ((rc = input_grad(tf32, mg, m->split_w[l], m->split_t[l], vs.g[l + 1], Mc, 4 * c.width[l], c.width[l + 1], st))) return rc;
+    if ((rc = lin_dx(f, mg, m->split[l], vs.g[l + 1], Mc))) return rc;
   }
   for (int i = 0; i < c.depth[n - 1]; ++i)
     if ((rc = vjp_layer(m, f, vs, --k, vs.g[n - 1], h0 >> (n - 1), w0 >> (n - 1), tr))) return rc;
@@ -953,19 +935,10 @@ int vjp_impl(KdbModel* m, int B, int H, int W, const float* x, const float* u, c
     const int64_t Mc = (int64_t)B * (h / 2) * (w / 2);
     float* dmw = tr ? m->grad("merges." + std::to_string(l) + ".proj.weight") : nullptr;
     const float* fine = reinterpret_cast<const float*>(ws.xs[l]);
-    if (dmw && (rc = tf32 ? launch_wgrad_tf32_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)
-                          : launch_wgrad_merge(vs.g[l + 1], c.width[l + 1], fine, dmw, Mc, c.width[l + 1], h / 2, w / 2, c.width[l], part, st)))
+    if (dmw && (rc = lin_dw(tf32, vs.g[l + 1], c.width[l + 1], fine, c.width[l], dmw, Mc, c.width[l + 1], 4 * c.width[l], part, st, h / 2, w / 2)))
       return rc;
-    // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added; on the tf32 route the
-    // GEMM stores dnxt W to ws.mg and a scatter kernel adds it
-    if (tf32) {
-      if ((rc = linear_tf32(vs.g[l + 1], m->merge_t[l].t, mg, Mc, 4 * c.width[l], c.width[l + 1], nullptr, st)) ||
-          (rc = launch_merge_scatter_add(mg, vs.g[l], B, h, w, c.width[l], st)))
-        return rc;
-    } else if ((rc = launch_gemm_vjp(vs.g[l + 1], m->merge_w[l], vs.g[l], Mc, c.width[l + 1], 4 * c.width[l], VJP_UNPATCH_ACC, h / 2, w / 2,
-                                     c.width[l], st))) {
-      return rc;
-    }
+    // nxt = patch2x2(cur) W^T: the fine stream (already holding the skip gradient) gets unpatch2x2(dnxt W) added
+    if ((rc = lin_dx(f, vs.g[l + 1], m->merge[l], vs.g[l], Mc, h / 2, w / 2))) return rc;
     for (int i = 0; i < c.depth[l]; ++i)
       if ((rc = vjp_layer(m, f, vs, --k, vs.g[l], h, w, tr))) return rc;
   }
@@ -1041,13 +1014,9 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
   const KdbModelConfig& c = m->cfg;
   const int n = c.n_levels, mw = c.mapping_width;
   m->layers.clear();
-  m->merge_w.assign(n, nullptr);
-  m->split_w.assign(n, nullptr);
+  m->merge.assign(n, Lin{});
+  m->split.assign(n, Lin{});
   m->split_fac.assign(n, nullptr);
-  m->merge_wb.assign(n, nullptr);
-  m->split_wb.assign(n, nullptr);
-  m->merge_t.assign(n, Tf32W{});
-  m->split_t.assign(n, Tf32W{});
   int ada = 0;
   int rc = for_each_layer(c, [&](const std::string& prefix, int level, int index) {
     m->layers.emplace_back();
@@ -1060,7 +1029,7 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     std::vector<FoldDesc> descs;
     for (const LayerPlan& L : m->layers) {
       if (L.C % 8 != 0) continue;
-      if (L.qkv_wf != nullptr && L.ada_attn >= 0) descs.push_back(FoldDesc{L.qkv_wb, L.qkv_wf, 3 * L.C, L.C, L.ada_attn});
+      if (L.qkv_wf != nullptr && L.ada_attn >= 0) descs.push_back(FoldDesc{L.qkv.wb, L.qkv_wf, 3 * L.C, L.C, L.ada_attn});
       if (L.up_wf != nullptr && L.up_wb_il != nullptr) descs.push_back(FoldDesc{L.up_wb_il, L.up_wf, 2 * L.dff, L.C, L.ada_ff});
     }
     m->n_fold = (int)descs.size();
@@ -1074,11 +1043,10 @@ int kdb_model_finalize(KdbModel* m, void* stream) {
     m->fuse_norm = !(e != nullptr && e[0] == '1');
   }
   for (int l = 0; l < n - 1; ++l) {
-    GET("merges." + std::to_string(l) + ".proj.weight", &m->merge_w[l], c.width[l + 1], 4 * c.width[l]);
-    GET("splits." + std::to_string(l) + ".proj.weight", &m->split_w[l], 4 * c.width[l], c.width[l + 1]);
+    if ((rc = bind(m, m->merge[l], "merges." + std::to_string(l) + ".proj.weight", c.width[l + 1], 4 * c.width[l], st)) ||
+        (rc = bind(m, m->split[l], "splits." + std::to_string(l) + ".proj.weight", 4 * c.width[l], c.width[l + 1], st)))
+      return rc;
     GET("splits." + std::to_string(l) + ".fac", &m->split_fac[l], 1);
-    if ((rc = make_bf16(m, m->merge_w[l], 4LL * c.width[l] * c.width[l + 1], &m->merge_wb[l], st))) return rc;
-    if ((rc = make_bf16(m, m->split_w[l], 4LL * c.width[l] * c.width[l + 1], &m->split_wb[l], st))) return rc;
   }
   const int C0 = c.width[0], Np = c.patch_h * c.patch_w * c.out_channels, Ni = c.patch_h * c.patch_w * c.in_channels;
   GET("out_norm.scale", &m->out_norm, C0);
@@ -1393,16 +1361,12 @@ int kdb_wgrad(int precision, const float* dy, int64_t ldy, const float* x, int64
   KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32, KDB_ERR_UNSUPPORTED, "wgrad: precision %d is neither fp32 nor tf32",
               precision);
   KDB_REQUIRE(ldy >= n, KDB_ERR_BAD_ARG, "wgrad: ldy %lld < n %d", (long long)ldy, n);
-  const bool tf32 = precision == KDB_PREC_TF32;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (merge_hc > 0 || merge_wc > 0) {
+  if (merge_hc > 0 || merge_wc > 0)
     KDB_REQUIRE(merge_hc > 0 && merge_wc > 0 && k % 4 == 0 && m % ((int64_t)merge_hc * merge_wc) == 0, KDB_ERR_BAD_SHAPE,
                 "wgrad: merge geometry %dx%d with k %d, m %lld", merge_hc, merge_wc, k, (long long)m);
-    return tf32 ? launch_wgrad_tf32_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st)
-                : launch_wgrad_merge(dy, ldy, x, dw, m, n, merge_hc, merge_wc, k / 4, scratch, st);
-  }
-  KDB_REQUIRE(ldx >= k, KDB_ERR_BAD_ARG, "wgrad: ldx %lld < k %d", (long long)ldx, k);
-  return weight_grad(tf32, dy, ldy, x, ldx, dw, m, n, k, scratch, st);
+  else
+    KDB_REQUIRE(ldx >= k, KDB_ERR_BAD_ARG, "wgrad: ldx %lld < k %d", (long long)ldx, k);
+  return lin_dw(precision == KDB_PREC_TF32, dy, ldy, x, ldx, dw, m, n, k, scratch, (cudaStream_t)stream, merge_hc, merge_wc);
 }
 
 int kdb_wgrad_patch_in(const float* dtok, const float* x, float* dw, int batch, int channels, int height, int width, int patch_h, int patch_w,
