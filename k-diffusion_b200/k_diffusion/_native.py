@@ -10,6 +10,7 @@ import math
 import functools
 import os
 from pathlib import Path
+from typing import NamedTuple
 
 import torch
 
@@ -871,6 +872,30 @@ class UNetEngine(Engine):
         if precision != PREC_FP32:
             raise NotImplementedError("the image_v1 U-Net trains at fp32 only")
         return self.forward(x, sigma, cond, cond_batch_stride, sigma_data, PREC_FP32, out=out)
+
+
+class LossRequest(NamedTuple):
+    """What `Denoiser.loss` passes, as the keyword `loss_request`, through a DistributedDataParallel wrapper's forward to a native model
+    (see `NativeLossCall`), which then returns `request(self.native_loss, x, sigma, **conditioning)`: the training loss runs inside DDP's
+    forward, so DDP prepares its reducer, syncs its buffers and honours no_sync() as it does for a torch model.  A NamedTuple, so that
+    DDP's input mover carries it through with its tensors on the module's device."""
+    kind: int
+    noise: torch.Tensor
+    sigma_data: float
+    weight: object
+
+    def __call__(self, native_loss, input, sigma, **kwargs):
+        return native_loss(self.kind, input, self.noise, sigma, self.sigma_data, self.weight, **kwargs)
+
+
+class NativeLossCall:
+    """Base of the modules with a `native_loss` (the native models and KarrasAugmentWrapper): a call with the keyword `loss_request`
+    returns that request's native loss instead of running `forward`, whose signature stays the reference's."""
+
+    def __call__(self, *args, loss_request=None, **kwargs):
+        if loss_request is None:
+            return super().__call__(*args, **kwargs)
+        return loss_request(self.native_loss, *args, **kwargs)
 
 
 class NativeLoss(torch.autograd.Function):

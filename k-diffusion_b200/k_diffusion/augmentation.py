@@ -62,7 +62,7 @@ class KarrasAugmentationPipeline:
         return _native.augment(images, draws, self.a_prob, self.a_scale, self.a_aniso, self.a_trans, self.disable_all, with_mat)
 
 
-class KarrasAugmentWrapper(nn.Module):
+class KarrasAugmentWrapper(_native.NativeLossCall, nn.Module):
     """mapping_cond = cat([aug_cond or zeros(B, 9), mapping_cond]) for the inner model.
 
     Around a native ImageDenoiserModelV1 the concatenation happens inside the engine's conditioning kernel and the wrapper has the

@@ -48,11 +48,22 @@ class Denoiser(nn.Module):
         """Per-sample losses [B] (reference layers.py:76-86, scales == 1).  A native image_transformer_v2 inner model runs one fp32 engine
         evaluation and one loss kernel, and its backward one native call that writes every parameter's gradient; the image_v1 U-Net does the
         same at exact fp32; image_transformer_v1 raises NotImplementedError.  Any other inner model runs the reference formula under torch
-        autograd."""
+        autograd.
+
+        A native inner model wrapped in torch.nn.parallel.DistributedDataParallel (as Accelerate wraps it) runs its native loss inside
+        the wrapper's forward, called with the keyword `loss_request`; its backward writes every gradient at once, and DDP's reducer
+        averages them across the ranks (or, under no_sync(), leaves them to accumulate).  A model whose loss leaves some parameters
+        without a gradient -- a U-Net with skip_stages > 0, or mapping_cond.* when no mapping_cond is formed -- needs
+        find_unused_parameters=True, as under torch autograd."""
         self._check_loss()
-        native_loss = getattr(self.inner_model, 'native_loss', None)
+        inner = utils.unwrap_ddp(self.inner_model)
+        native_loss = getattr(inner, 'native_loss', None)
         if native_loss is not None:
-            return native_loss(self._loss_kind, input, noise, sigma, self.sigma_data, self.weighting(sigma), **kwargs)
+            request = _native.LossRequest(self._loss_kind, noise, self.sigma_data, self.weighting(sigma))
+            if inner is not self.inner_model:
+                # through DistributedDataParallel.forward, which prepares the reducer that all-reduces the backward's gradients
+                return self.inner_model(input, sigma, **kwargs, loss_request=request)
+            return request(native_loss, input, sigma, **kwargs)
         if self.is_native():
             raise NotImplementedError(f'{type(self.inner_model).__name__}: parameter gradients are built for image_transformer_v2 models only')
         return self._torch_loss(input, noise, sigma, **kwargs)
@@ -66,13 +77,14 @@ class Denoiser(nn.Module):
         return ((model_output - target) ** 2).flatten(1).mean(1) * c_weight
 
     def is_native(self):
-        """Whether the inner model has a native front end (`native_eval`), which the fused paths here and the samplers evaluate through."""
-        return getattr(self.inner_model, 'native_eval', None) is not None
+        """Whether the inner model, seen through a DistributedDataParallel wrapper, has a native front end (`native_eval`), which the
+        fused paths here and the samplers evaluate through."""
+        return getattr(utils.unwrap_ddp(self.inner_model), 'native_eval', None) is not None
 
     def forward(self, input, sigma, **kwargs):
         _native.require_cuda(input, sigma)
         if self.is_native():
-            return self.inner_model.denoise(input, sigma, self.sigma_data, **kwargs)
+            return utils.unwrap_ddp(self.inner_model).denoise(input, sigma, self.sigma_data, **kwargs)
         x = _native.f32c(input)
         sig = _native.f32c(sigma).expand(x.shape[0]).contiguous()
         f = self.inner_model(_native.precond_scale_in(x, sig, float(self.sigma_data)), sigma, **kwargs)
@@ -85,7 +97,7 @@ class Denoiser(nn.Module):
         inner(c_in x); the combine c_skip x + c_out f is linear, so one combine kernel serves the primal and the tangent."""
         _native.require_cuda(input, sigma, tangent)
         if self.is_native():
-            return self.inner_model.denoise_jvp(input, sigma, tangent, self.sigma_data, **kwargs)
+            return utils.unwrap_ddp(self.inner_model).denoise_jvp(input, sigma, tangent, self.sigma_data, **kwargs)
         x, t = _native.f32c(input), _native.f32c(tangent)
         sig = _native.f32c(sigma).expand(x.shape[0]).contiguous()
         sd = float(self.sigma_data)
@@ -101,7 +113,7 @@ class Denoiser(nn.Module):
         one combine kernel, as in `jvp`."""
         _native.require_cuda(input, sigma, cotangent)
         if self.is_native():
-            return self.inner_model.denoise_vjp(input, sigma, cotangent, self.sigma_data, **kwargs)
+            return utils.unwrap_ddp(self.inner_model).denoise_vjp(input, sigma, cotangent, self.sigma_data, **kwargs)
         x, u = _native.f32c(input), _native.f32c(cotangent)
         sig = _native.f32c(sigma).expand(x.shape[0]).contiguous()
         sd = float(self.sigma_data)

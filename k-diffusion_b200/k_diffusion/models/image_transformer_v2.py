@@ -164,7 +164,7 @@ def _level(spec, cond_width):
     return nn.ModuleList([_layer(spec, cond_width) for _ in range(spec.depth)])
 
 
-class TransformerEngineModel(_native.EngineCache, nn.Module):
+class TransformerEngineModel(_native.NativeLossCall, _native.EngineCache, nn.Module):
     """What the transformer models share on top of their parameters: the native engine (a KdbModel of `family`), the precision, and
     the evaluation entry points (the raw model, the Karras-preconditioned denoiser, their JVP / VJP, torch.autograd through x).  A
     subclass sets `levels`, `mapping_spec`, `in_channels`, `out_channels`, `patch_size`, `num_classes`, `mapping_cond_dim`,

@@ -110,7 +110,7 @@ class UNet(nn.Module):
         self.skip_stages = skip_stages
 
 
-class ImageDenoiserModelV1(_native.EngineCache, nn.Module):
+class ImageDenoiserModelV1(_native.NativeLossCall, _native.EngineCache, nn.Module):
     def __init__(self, c_in, feats_in, depths, channels, self_attn_depths, cross_attn_depths=None, mapping_cond_dim=0, unet_cond_dim=0,
                  cross_cond_dim=0, dropout_rate=0., patch_size=1, skip_stages=0, has_variance=False):
         super().__init__()

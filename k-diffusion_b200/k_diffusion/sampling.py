@@ -503,7 +503,7 @@ class _Evaluator:
         sig = torch.tensor(eval_sigmas, dtype=torch.float32, device=x.device)
         self.sigma_rows = sig[:, None].expand(len(eval_sigmas), self.B).contiguous()
         if self.native:
-            self.inner = base.inner_model
+            self.inner = utils.unwrap_ddp(base.inner_model)
             self.call = self.inner.native_eval(x, None, **extra_args)      # every check of the inputs, once per sampler call
             if self.cfg is not None:
                 self.call.guide(self.cfg.num_classes)

@@ -48,6 +48,12 @@ def n_params(module):
     return sum(p.numel() for p in module.parameters())
 
 
+def unwrap_ddp(model):
+    """`model.module` when `model` is a torch.nn.parallel.DistributedDataParallel wrapper (what Accelerate's `prepare` puts around a
+    model in a multi-process run), else `model`: the model whose native front end and native loss the package calls."""
+    return model.module if isinstance(model, torch.nn.parallel.DistributedDataParallel) else model
+
+
 @contextmanager
 def _mode(model, training):
     was = [m.training for m in model.modules()]
