@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define KDB_ABI_VERSION 27
+#define KDB_ABI_VERSION 28
 
 #define KDB_ERR_BAD_ARG      (-1)
 #define KDB_ERR_UNSUPPORTED  (-2)
@@ -123,6 +123,14 @@ int kdb_loss_noised_input(const float* x, const float* noise, const float* sigma
                           int batch, int64_t per_sample, void* stream);
 int kdb_denoiser_loss(int kind, const float* x, const float* noise, const float* sigma, const float* weight, float sigma_data,
                       const float* f, float* loss, float* cotangent, int batch, int64_t per_sample, void* stream);
+
+/* The training loss of a model with a learned variance (layers.py:93-101 DenoiserWithVariance.loss), with the arguments of
+ * kdb_denoiser_loss and logvar [B], the model's per-image log-variance (kdb_unet_forward_variance): with m = mean((f - target)^2),
+ * loss[b] = (m exp(-logvar[b]) + logvar[b]) / 2; cotangent (or NULL) receives d loss[b] / d f = (f - target) exp(-logvar[b]) / per_sample,
+ * dlogvar (or NULL) d loss[b] / d logvar[b] = (1 - m exp(-logvar[b])) / 2.  m, loss and dlogvar are formed in double and rounded once,
+ * since 1 - m exp(-logvar) cancels as the variance fits.  One CTA per image, a fixed-order sum: two calls give the same bits. */
+int kdb_variance_loss(const float* x, const float* noise, const float* sigma, float sigma_data, const float* f, const float* logvar, float* loss,
+                      float* cotangent, float* dlogvar, int batch, int64_t per_sample, void* stream);
 
 /* The per-evaluation math of the external model wrappers (external.py:9-38, 87-177: VDenoiser, DiscreteEpsDDPMDenoiser,
  * OpenAIDenoiser, CompVisDenoiser, DiscreteVDDPMDenoiser, CompVisVDenoiser); sigma is [B] fp32.  Every product and sum is
@@ -382,6 +390,13 @@ int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int
 int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
                      const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* kdb_unet_forward of a has_variance model (KDB_ERR_BAD_ARG for any other), whose `out` it writes bit for bit, plus the learned log-variance
+ * logvar [B] (image_v1.py:151-152, return_variance=True): proj_out's variance channel averaged over the (H/p) x (W/p) token grid, computed
+ * in fp32 from the features the forward's proj_out reads at every precision.  Same workspace. */
+int kdb_unet_forward_variance(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                              const float* cond, int64_t cond_batch_stride, float* out, float* logvar, void* workspace, size_t workspace_bytes,
+                              void* stream);
+
 /* Debug/parity tap of the NEXT forward, token-major [B, h, w, C] fp32: "patch_in", "d<l>.down", "d<l>.<i>", "u<l>.<i>",
  * "u<l>.up" -- level l, i the module index inside the reference's DBlock (1..) / UBlock (0..), i.e. the output of that
  * ResConvBlock or SelfAttention2d.  kdb_unet_tap_count: floats written (0 = not hit, < 0 = capacity too small). */
@@ -408,6 +423,13 @@ int64_t kdb_unet_train_workspace_bytes(const KdbUNet* m, int batch, int height, 
 int     kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
                                const float* aug_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
                                const float* cotangent, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* kdb_unet_forward_train of a has_variance model (KDB_ERR_BAD_ARG for any other) with the cotangent dlogvar [B] of its log-variance as
+ * well: every bound gradient = u^T dF/dparam + dlogvar^T dlogvar/dparam, which reaches proj_out's variance row and, through it, every
+ * parameter upstream.  Same arguments, checks, workspace and precision otherwise. */
+int     kdb_unet_forward_train_variance(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
+                                        const float* aug_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
+                                        const float* cotangent, const float* dlogvar, float* out, void* workspace, size_t workspace_bytes,
+                                        void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stand-alone kernels exposed for unit tests / profiling (same code the engine launches)

@@ -1399,6 +1399,11 @@ int kdb_colsum(const float* p, int64_t rows, int c, float* out, float* scratch, 
   return launch_colsum(p, rows, c, out, scratch, (cudaStream_t)stream);
 }
 
+int kdb_variance_loss(const float* x, const float* noise, const float* sigma, float sigma_data, const float* f, const float* logvar, float* loss,
+                      float* cotangent, float* dlogvar, int batch, int64_t per_sample, void* stream) {
+  return launch_variance_loss(x, noise, sigma, sigma_data, f, logvar, loss, cotangent, dlogvar, batch, per_sample, (cudaStream_t)stream);
+}
+
 int kdb_split_fac_grad(const float* y, const float* skip, const float* dup, float* out, int batch, int height, int width, int c, float* scratch,
                        void* stream) {
   KDB_REQUIRE(y && skip && dup && out && scratch && batch > 0 && c > 0, KDB_ERR_BAD_ARG, "split_fac_grad: bad argument");

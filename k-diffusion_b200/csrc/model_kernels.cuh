@@ -250,6 +250,11 @@ int launch_wgrad_patch_out(const float* u, const float* tokens, const float* sca
                            int ph, int pw, int C0, float* part, cudaStream_t st);
 // class_emb's gradient: out[k, :] = sum over the rows r with cls[r] == k of demb[r, :] (ld ldd), rows in order; every row k < n_classes written
 int launch_class_emb_grad(const float* demb, int64_t ldd, const int64_t* cls, float* out, int rows, int n_classes, int mw, cudaStream_t st);
+// DenoiserWithVariance's loss (layers.py:93-101), one CTA per image of n elements: with r = f - (x - c_skip xn) / c_out, xn = x + noise sigma,
+// and m = mean(r^2) (a fixed-order block sum in double), loss[b] = (m e^-lv + lv) / 2 and dlogvar[b] = (1 - m e^-lv) / 2 (or NULL) formed in
+// double and rounded once, cot = r e^-lv / n (or NULL); lv = logvar[b]
+int launch_variance_loss(const float* x, const float* noise, const float* sigma, float sigma_data, const float* f, const float* logvar, float* loss,
+                         float* cot, float* dlogvar, int B, int64_t n, cudaStream_t st);
 
 // (cos, sin) table of the axial RoPE angles of QkRope with R = 4 nf: theta_j = (j < nf ? pos_y : pos_x)[t] * freqs[h, j], j < 2 nf
 int launch_rope_table(const float* pos, const float* freqs, float2* out, int T_tokens, int nh, int nf, cudaStream_t st);

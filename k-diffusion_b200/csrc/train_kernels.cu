@@ -261,7 +261,58 @@ __global__ void __launch_bounds__(256) class_emb_grad_kernel(const float* __rest
   }
 }
 
+// block_sum's fixed order, in double
+__device__ __forceinline__ double block_sum_f64(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  double t = 0.0;
+  for (int i = 0; i < nw; ++i) t += red[i];
+  return t;
+}
+
+// The residual r as denoiser_loss_kernel forms it, in fp32.  Its squares are summed, and q = mean(r^2) e^-lv, the loss and d loss / d lv
+// formed, in double, each rounded to fp32 once: d loss / d lv = (1 - q) / 2 cancels as q nears 1 (where training drives logvar, and where a
+// batch's terms of both signs cancel again in proj_out's bias gradient), so fp32 rounding of the sum and of q would dominate its error.
+__global__ void __launch_bounds__(256) variance_loss_kernel(const float* __restrict__ x, const float* __restrict__ noise,
+                                                            const float* __restrict__ sigma, float sd, const float* __restrict__ f,
+                                                            const float* __restrict__ logvar, float* __restrict__ loss, float* __restrict__ cot,
+                                                            float* __restrict__ dlogvar, int64_t n) {
+  __shared__ double red[8];
+  const int64_t b = blockIdx.x;
+  const float s = sigma[b], lv = logvar[b];
+  float c_skip, c_out, c_in;
+  karras_scalings(s, sd, c_skip, c_out, c_in);
+  const double inv_var = exp(-(double)lv);
+  const float g = (float)(inv_var / (double)n);
+  double acc = 0.0;
+  for (int64_t i = threadIdx.x; i < n; i += 256) {
+    const int64_t j = b * n + i;
+    const float xn = __fadd_rn(x[j], __fmul_rn(noise[j], s));
+    const float r = __fsub_rn(f[j], __fdiv_rn(__fsub_rn(x[j], __fmul_rn(c_skip, xn)), c_out));
+    acc += (double)r * (double)r;
+    if (cot != nullptr) cot[j] = __fmul_rn(r, g);
+  }
+  acc = block_sum_f64(acc, red);
+  if (threadIdx.x == 0) {
+    const double q = acc / (double)n * inv_var;
+    loss[b] = (float)(0.5 * (q + (double)lv));
+    if (dlogvar != nullptr) dlogvar[b] = (float)(0.5 * (1.0 - q));
+  }
+}
+
 }  // namespace
+
+int launch_variance_loss(const float* x, const float* noise, const float* sigma, float sigma_data, const float* f, const float* logvar, float* loss,
+                         float* cot, float* dlogvar, int B, int64_t n, cudaStream_t st) {
+  KDB_REQUIRE(x && noise && sigma && f && logvar && loss && B > 0 && n > 0 && sigma_data > 0.f, KDB_ERR_BAD_ARG, "variance_loss: bad args");
+  variance_loss_kernel<<<(unsigned)B, 256, 0, st>>>(x, noise, sigma, sigma_data, f, logvar, loss, cot, dlogvar, n);
+  KDB_LAUNCH_CHECK(F_PRECOND, st);
+  return 0;
+}
 
 int launch_wgrad(const float* dY, int64_t ldy, const float* X, int64_t ldx, float* dW, int64_t M, int N, int K, float* part, cudaStream_t st) {
   return wgrad<false>(Rows{dY, ldy}, Rows{X, ldx}, dW, M, N, K, part, st);

@@ -283,9 +283,10 @@ int walk(const KdbUNet* m, int H, int W, float* x0, Fn fn) {
 }
 
 // tape != nullptr (training): patch_in writes tape[0] and module i (of m->mods) tape[i + 1], which a DBlock's last module's UBlock then reads
-// as its skip; the launches are those of tape == nullptr
+// as its skip; the launches are those of tape == nullptr.  logvar != nullptr (a has_variance model): the variance row's token mean per image
+// after patch_out, from the same features.
 int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, const float* sigma, float sd, const float* cond, int64_t cbs, float* out,
-                 UWs& ws, cudaStream_t st, float* const* tape = nullptr) {
+                 UWs& ws, cudaStream_t st, float* const* tape = nullptr, float* logvar = nullptr) {
   const KdbUNetConfig& c = m->cfg;
   const int s0 = c.skip_stages, C0 = c.channels[std::max(0, s0 - 1)];
   int h, w, rc;
@@ -306,8 +307,10 @@ int unet_forward(KdbUNet* m, int prec, int B, int H, int W, const float* x, cons
     y = dst;
     return rc ? rc : m->tap(u.tap, dst, (int64_t)B * ho * wo * C, st);
   });
-  if (rc) return rc;
-  return launch_unet_patch_out(y, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, C0, st);
+  if (rc || (rc = launch_unet_patch_out(y, m->proj_out_w, m->proj_out_b, x, sigma, sd, out, B, c.in_channels, H, W, c.patch_size, C0, st)))
+    return rc;
+  const int Kin = c.in_channels * c.patch_size * c.patch_size;
+  return logvar ? launch_unet_logvar(y, m->proj_out_w + (size_t)Kin * C0, m->proj_out_b + Kin, logvar, B, h * w, C0, st) : 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -487,10 +490,11 @@ int attn_vjp(KdbUNet* m, const UMod& u, const float* x, const float* g, float* o
   return launch_unet_adagn_vjp(x, C, nullptr, 0, t.ga, g, out, nullptr, cond, cbs, u.ada1, t.dss, m->ada_total, u.groups1, false, B, h * w, st);
 }
 
-// out = the fp32 forward of F (bit for bit unet_forward's launches, writing the tape), then u^T dF/dparam for every bound parameter by a
-// walk of the modules in reverse: proj_out, the UBlocks (innermost last), the DBlocks, proj_in; then the AdaGN mappers and the mapping network.
+// out = the fp32 forward of F (bit for bit unet_forward's launches, writing the tape), then u^T dF/dparam + dlogvar^T dlogvar/dparam for every
+// bound parameter by a walk of the modules in reverse: proj_out, the UBlocks (innermost last), the DBlocks, proj_in; then the AdaGN mappers and
+// the mapping network.  dlogvar == nullptr: the logvar term is absent.
 int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sigma, const float* aug, const float* mcond, const float* cond,
-               int64_t cbs, const float* u, float* out, TWs& t, cudaStream_t st) {
+               int64_t cbs, const float* u, const float* dlogvar, float* out, TWs& t, cudaStream_t st) {
   const KdbUNetConfig& c = m->cfg;
   int rc = ensure_bwd(m, st);
   if (rc || (rc = unet_forward(m, KDB_PREC_FP32, B, H, W, x, sigma, 0.f, cond, cbs, out, t.f, st, t.tape.data()))) return rc;
@@ -500,8 +504,9 @@ int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sig
   level_dims(c, H, W, s0, &h, &w);
   const int64_t M0 = (int64_t)B * h * w;
   float* part = t.part;
-  // proj_out + pixel_shuffle: U = the patch rows of u, with a zero column for the variance channel the output drops
-  if ((rc = launch_unet_unshuffle(u, t.U, B, c.in_channels, H, W, p, Kout, st)) ||
+  // proj_out + pixel_shuffle: U = the patch rows of u, with a column for the variance channel the output drops: dlogvar[b] / T on image b's
+  // T tokens (logvar[b] is their mean), or zero
+  if ((rc = launch_unet_unshuffle(u, t.U, B, c.in_channels, H, W, p, Kout, dlogvar, st)) ||
       (rc = launch_wgrad(t.U, Kout, t.tape.back(), C0, m->grad("proj_out.weight"), M0, Kout, C0, part, st)) ||
       (rc = launch_colsum(t.U, M0, Kout, m->grad("proj_out.bias"), part, st)) ||
       (rc = launch_unet_proj_out_vjp(t.U, m->proj_out_w, t.g[0], M0, Kout, C0, st)))
@@ -536,7 +541,7 @@ int unet_train(KdbUNet* m, int B, int H, int W, const float* x, const float* sig
     gi ^= 1;
   }
   // proj_in: its input is the pixel_unshuffle of x (the caller's c_in-scaled input)
-  if ((rc = launch_unet_unshuffle(x, t.xin, B, c.in_channels, H, W, p, Kin, st)) ||
+  if ((rc = launch_unet_unshuffle(x, t.xin, B, c.in_channels, H, W, p, Kin, nullptr, st)) ||
       (rc = launch_wgrad(t.g[gi], C0, t.xin, Kin, m->grad("proj_in.weight"), M0, C0, Kin, part, st)) ||
       (rc = launch_colsum(t.g[gi], M0, C0, m->grad("proj_in.bias"), part, st)))
     return rc;
@@ -587,6 +592,42 @@ int check_conds(const KdbUNetConfig& c, const char* what, const float* aug_cond,
               "%s: mapping_cond must be given (mapping_cond_dim %d)", what, c.mapping_cond_dim - 9);
   KDB_REQUIRE(!(mapping_cond && c.mapping_cond_dim == (c.augment_wrapper ? 9 : 0)), KDB_ERR_BAD_ARG, "%s: the model takes no mapping_cond", what);
   return 0;
+}
+
+// kdb_unet_forward and kdb_unet_forward_variance (logvar != nullptr); `what` names the entry point in errors
+int forward_entry(KdbUNet* m, const char* what, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                  const float* cond, int64_t cond_batch_stride, float* out, float* logvar, void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "%s: model NULL or not finalized", what);
+  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "%s: NULL argument", what);
+  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
+              "%s: the fp32, tf32 and fp16 paths are built (precision %d)", what, precision);
+  const KdbUNetConfig& c = m->cfg;
+  if (int rc = check_grid(c, what, height, width)) return rc;
+  UWs ws;
+  carve(c, batch, height, width, workspace, ws);
+  KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "%s: workspace %zu < required %zu", what, workspace_bytes, ws.total);
+  return m->disarm_tap(unet_forward(m, precision, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream,
+                                    nullptr, logvar));
+}
+
+// kdb_unet_forward_train and kdb_unet_forward_train_variance (dlogvar != nullptr)
+int train_entry(KdbUNet* m, const char* what, int precision, int batch, int height, int width, const float* x, const float* sigma, const float* aug_cond,
+                const float* mapping_cond, const float* cond, int64_t cond_batch_stride, const float* cotangent, const float* dlogvar, float* out,
+                void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "%s: NULL model", what);
+  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "%s: U-Net training runs at fp32 (precision %d)", what, precision);
+  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "%s: model not finalized", what);
+  KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "%s: NULL argument", what);
+  const KdbUNetConfig& c = m->cfg;
+  int rc;
+  if ((rc = check_conds(c, what, aug_cond, mapping_cond))) return rc;
+  if ((rc = check_train(m, what, cond_batch_stride, kdb_unet_cond_stride(m), check_grad_key))) return rc;
+  if ((rc = check_grid(c, what, height, width))) return rc;
+  TWs t;
+  carve_train(m, batch, height, width, workspace, t);
+  KDB_REQUIRE(t.total <= workspace_bytes, KDB_ERR_WORKSPACE, "%s: workspace %zu < required %zu", what, workspace_bytes, t.total);
+  return m->disarm_tap(unet_train(m, batch, height, width, x, sigma, aug_cond, mapping_cond, cond, cond_batch_stride, cotangent, dlogvar, out, t,
+                                  (cudaStream_t)stream));
 }
 
 }  // namespace
@@ -718,16 +759,17 @@ int64_t kdb_unet_workspace_bytes(const KdbUNet* m, int precision, int batch, int
 
 int kdb_unet_forward(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
                      const float* cond, int64_t cond_batch_stride, float* out, void* workspace, size_t workspace_bytes, void* stream) {
-  KDB_REQUIRE(m && m->finalized, KDB_ERR_NOT_FINAL, "unet_forward: model NULL or not finalized");
-  KDB_REQUIRE(x && sigma && cond && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward: NULL argument");
-  KDB_REQUIRE(precision == KDB_PREC_FP32 || precision == KDB_PREC_TF32 || precision == KDB_PREC_FP16, KDB_ERR_UNSUPPORTED,
-              "unet_forward: the fp32, tf32 and fp16 paths are built (precision %d)", precision);
-  const KdbUNetConfig& c = m->cfg;
-  if (int rc = check_grid(c, "unet_forward", height, width)) return rc;
-  UWs ws;
-  carve(c, batch, height, width, workspace, ws);
-  KDB_REQUIRE(ws.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward: workspace %zu < required %zu", workspace_bytes, ws.total);
-  return m->disarm_tap(unet_forward(m, precision, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, ws, (cudaStream_t)stream));
+  return forward_entry(m, "unet_forward", precision, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, nullptr, workspace,
+                       workspace_bytes, stream);
+}
+
+int kdb_unet_forward_variance(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, float sigma_data,
+                              const float* cond, int64_t cond_batch_stride, float* out, float* logvar, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  KDB_REQUIRE(m && m->cfg.has_variance, KDB_ERR_BAD_ARG, "unet_forward_variance: model NULL or without has_variance");
+  KDB_REQUIRE(logvar, KDB_ERR_BAD_ARG, "unet_forward_variance: NULL logvar");
+  return forward_entry(m, "unet_forward_variance", precision, batch, height, width, x, sigma, sigma_data, cond, cond_batch_stride, out, logvar,
+                       workspace, workspace_bytes, stream);
 }
 
 int kdb_unet_set_grad(KdbUNet* m, const char* key, float* data, const int64_t* shape, int ndim) {
@@ -745,20 +787,17 @@ int64_t kdb_unet_train_workspace_bytes(const KdbUNet* m, int batch, int height, 
 int kdb_unet_forward_train(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma, const float* aug_cond,
                            const float* mapping_cond, const float* cond, int64_t cond_batch_stride, const float* cotangent, float* out,
                            void* workspace, size_t workspace_bytes, void* stream) {
-  KDB_REQUIRE(m, KDB_ERR_BAD_ARG, "unet_forward_train: NULL model");
-  KDB_REQUIRE(precision == KDB_PREC_FP32, KDB_ERR_UNSUPPORTED, "unet_forward_train: U-Net training runs at fp32 (precision %d)", precision);
-  KDB_REQUIRE(m->finalized, KDB_ERR_NOT_FINAL, "unet_forward_train: model not finalized");
-  KDB_REQUIRE(x && sigma && cond && cotangent && out && workspace && batch > 0, KDB_ERR_BAD_ARG, "unet_forward_train: NULL argument");
-  const KdbUNetConfig& c = m->cfg;
-  int rc;
-  if ((rc = check_conds(c, "unet_forward_train", aug_cond, mapping_cond))) return rc;
-  if ((rc = check_train(m, "unet_forward_train", cond_batch_stride, kdb_unet_cond_stride(m), check_grad_key))) return rc;
-  if ((rc = check_grid(c, "unet_forward_train", height, width))) return rc;
-  TWs t;
-  carve_train(m, batch, height, width, workspace, t);
-  KDB_REQUIRE(t.total <= workspace_bytes, KDB_ERR_WORKSPACE, "unet_forward_train: workspace %zu < required %zu", workspace_bytes, t.total);
-  return m->disarm_tap(unet_train(m, batch, height, width, x, sigma, aug_cond, mapping_cond, cond, cond_batch_stride, cotangent, out, t,
-                                  (cudaStream_t)stream));
+  return train_entry(m, "unet_forward_train", precision, batch, height, width, x, sigma, aug_cond, mapping_cond, cond, cond_batch_stride, cotangent,
+                     nullptr, out, workspace, workspace_bytes, stream);
+}
+
+int kdb_unet_forward_train_variance(KdbUNet* m, int precision, int batch, int height, int width, const float* x, const float* sigma,
+                                    const float* aug_cond, const float* mapping_cond, const float* cond, int64_t cond_batch_stride,
+                                    const float* cotangent, const float* dlogvar, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+  KDB_REQUIRE(m && m->cfg.has_variance, KDB_ERR_BAD_ARG, "unet_forward_train_variance: model NULL or without has_variance");
+  KDB_REQUIRE(dlogvar, KDB_ERR_BAD_ARG, "unet_forward_train_variance: NULL dlogvar");
+  return train_entry(m, "unet_forward_train_variance", precision, batch, height, width, x, sigma, aug_cond, mapping_cond, cond, cond_batch_stride,
+                     cotangent, dlogvar, out, workspace, workspace_bytes, stream);
 }
 
 int kdb_unet_conv_wgrad(const float* dy, int n_out, const float* in1, int c1, const float* in2, int c2, float* dw, int batch, int h, int w, int ksize,
@@ -805,7 +844,7 @@ int kdb_unet_proj_out_vjp(const float* u, const float* w, float* out, int64_t ro
 int kdb_unet_unshuffle(const float* x, float* out, int batch, int c, int h, int w, int p, int ld, void* stream) {
   KDB_REQUIRE(x && out && batch > 0 && c > 0 && p > 0 && h > 0 && w > 0 && h % p == 0 && w % p == 0 && ld >= c * p * p, KDB_ERR_BAD_ARG,
               "unet_unshuffle: bad argument");
-  return launch_unet_unshuffle(x, out, batch, c, h, w, p, ld, (cudaStream_t)stream);
+  return launch_unet_unshuffle(x, out, batch, c, h, w, p, ld, nullptr, (cudaStream_t)stream);
 }
 
 int kdb_unet_debug_tap(KdbUNet* m, const char* name, float* out, int64_t capacity) { return arm_tap(m, name, out, capacity); }

@@ -199,6 +199,23 @@ __global__ void __launch_bounds__(256) unet_patch_out_kernel(const float* __rest
   }
 }
 
+// proj_out's variance row averaged over the token grid (image_v1.py:151-152), one CTA per image: each thread forms w_v . y[b, t] for the
+// tokens t = threadIdx.x (mod 256) in order, then a fixed-order block sum
+__global__ void __launch_bounds__(256) unet_logvar_kernel(const float* __restrict__ tok, const float* __restrict__ wv, const float* __restrict__ bv,
+                                                          float* __restrict__ logvar, int T, int K) {
+  __shared__ float red[8];
+  const int b = blockIdx.x;
+  float acc = 0.f;
+  for (int t = threadIdx.x; t < T; t += 256) {
+    const float* y = tok + ((int64_t)b * T + t) * K;
+    float d = 0.f;
+    for (int k = 0; k < K; ++k) d = fmaf(__ldg(wv + k), y[k], d);
+    acc = __fadd_rn(acc, d);
+  }
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) logvar[b] = __fadd_rn(__ldg(bv), __fdiv_rn(acc, (float)T));
+}
+
 // ------------------------------------------------------------------------------------------------
 // conditioning
 // ------------------------------------------------------------------------------------------------
@@ -413,9 +430,10 @@ __global__ void __launch_bounds__(256) unet_flip_kernel(const float* __restrict_
   }
 }
 
-// pixel_unshuffle of NCHW x [B, C, H, W] to token rows [B (H/p) (W/p), ld], column (c, i, j); columns C p p .. ld - 1 zero
+// pixel_unshuffle of NCHW x [B, C, H, W] to token rows [B (H/p) (W/p), ld], column (c, i, j); column C p p holds col[b] / (h w) when col is
+// given, every other column past C p p zero
 __global__ void __launch_bounds__(256) unet_unshuffle_kernel(const float* __restrict__ x, float* __restrict__ out, int B, int C, int H, int W, int p,
-                                                             int ld) {
+                                                             int ld, const float* __restrict__ col) {
   const int h = H / p, wd = W / p, K = C * p * p;
   const int64_t total = (int64_t)B * h * wd * ld;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -426,6 +444,8 @@ __global__ void __launch_bounds__(256) unet_unshuffle_kernel(const float* __rest
       token_coords(i / ld, h, wd, b, ty, tx);
       const int c = o / (p * p), r = o - c * p * p;
       v = x[nchw_offset(b, c, ty * p + r / p, tx * p + r % p, C, H, W)];
+    } else if (o == K && col != nullptr) {
+      v = __fdiv_rn(col[i / ld / ((int64_t)h * wd)], (float)(h * wd));
     }
     out[i] = v;
   }
@@ -560,6 +580,13 @@ int launch_unet_patch_out(const float* tokens, const float* w, const float* bias
   return 0;
 }
 
+int launch_unet_logvar(const float* tokens, const float* wv, const float* bv, float* logvar, int B, int T, int K, cudaStream_t st) {
+  KDB_REQUIRE(tokens && wv && bv && logvar && B > 0 && T > 0 && K > 0, KDB_ERR_BAD_ARG, "unet_logvar: bad arguments");
+  unet_logvar_kernel<<<(unsigned)B, 256, 0, st>>>(tokens, wv, bv, logvar, T, K);
+  KDB_LAUNCH_CHECK(F_UNET_PATCH, st);
+  return 0;
+}
+
 int launch_unet_conditioning(const UNetCondWeights& w, int rows, const float* sigma, const float* aug, const float* mcond, float* out,
                              int64_t out_stride, cudaStream_t st) {
   KDB_REQUIRE(w.mw % 2 == 0 && w.mw > 0, KDB_ERR_UNSUPPORTED, "unet_conditioning: mapping_out must be even");
@@ -606,8 +633,10 @@ int launch_unet_flip_conv_weight(const float* src, float* dst, int N, int C, int
   return 0;
 }
 
-int launch_unet_unshuffle(const float* x, float* out, int B, int C, int H, int W, int p, int ld, cudaStream_t st) {
-  unet_unshuffle_kernel<<<grid_for((int64_t)B * (H / p) * (W / p) * ld), 256, 0, st>>>(x, out, B, C, H, W, p, ld);
+int launch_unet_unshuffle(const float* x, float* out, int B, int C, int H, int W, int p, int ld, const float* col, cudaStream_t st) {
+  KDB_REQUIRE(col == nullptr || ld > C * p * p, KDB_ERR_BAD_ARG, "unet_unshuffle: no column %d for the per-image value in rows of %d", C * p * p,
+              ld);
+  unet_unshuffle_kernel<<<grid_for((int64_t)B * (H / p) * (W / p) * ld), 256, 0, st>>>(x, out, B, C, H, W, p, ld, col);
   KDB_LAUNCH_CHECK(F_UNET_PATCH, st);
   return 0;
 }

@@ -69,6 +69,9 @@ int launch_unet_patch_in(const float* x, const float* sigma, float sigma_data, c
 // out [B, Cout, H, W] NCHW.
 int launch_unet_patch_out(const float* tokens, const float* w, const float* bias, const float* x_in, const float* sigma, float sigma_data,
                           float* out, int B, int Cout, int H, int W, int p, int K, cudaStream_t st);
+// The learned log-variance of a has_variance model (image_v1.py:151-152): logvar[b] = bv[0] + (1/T) sum over t of wv . tokens[b, t], tokens
+// [B, T, K] (proj_out's input), wv [K] and bv proj_out's variance row and bias.  One CTA per image, a fixed-order sum.
+int launch_unet_logvar(const float* tokens, const float* wv, const float* bv, float* logvar, int B, int T, int K, cudaStream_t st);
 
 // Conditioning (image_v1.py:136-139, augmentation.py:97-104, and every AdaGN mapper, layers.py:173): per row
 //   cond = MappingNet(FourierFeatures(log(sigma) / 4) + mapping_cond_linear(v)),  v = [aug_cond or zeros(9), mapping_cond] with the
@@ -99,8 +102,9 @@ int launch_unet_adagn_vjp(const float* in1, int c1, const float* in2, int c2, co
 // Adjoint of launch_unet_resample for an input grid H x W: dout [B, H/2, W/2, C] (up = false) or [B, 2H, 2W, C] (up = true) ->
 // din [B, H, W, C] (+ add [B, H, W, C] when add != NULL; add may be din)
 int launch_unet_resample_vjp(const float* dout, const float* add, float* din, int B, int H, int W, int C, bool up, cudaStream_t st);
-// pixel_unshuffle: NCHW x [B, C, H, W] -> token rows out [B (H/p) (W/p), ld], column (c, i, j) (torch's order); columns C p p .. ld - 1 zero
-int launch_unet_unshuffle(const float* x, float* out, int B, int C, int H, int W, int p, int ld, cudaStream_t st);
+// pixel_unshuffle: NCHW x [B, C, H, W] -> token rows out [B (H/p) (W/p), ld], column (c, i, j) (torch's order); columns C p p .. ld - 1 zero,
+// except column C p p of image b's rows, which is col[b] / ((H/p) (W/p)) when col is given (the variance row's share of d logvar[b])
+int launch_unet_unshuffle(const float* x, float* out, int B, int C, int H, int W, int p, int ld, const float* col, cudaStream_t st);
 // proj_out's input gradient: out [M, K] = U [M, N] w [N, K]
 int launch_unet_proj_out_vjp(const float* U, const float* w, float* out, int64_t M, int N, int K, cudaStream_t st);
 // p[i] *= s for i < n (nothing for p == NULL)

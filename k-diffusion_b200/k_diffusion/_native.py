@@ -21,7 +21,7 @@ PREC_FP32, PREC_BF16, PREC_TF32, PREC_FP16 = 0, 1, 2, 3
 ATTN_NONE, ATTN_GLOBAL, ATTN_NEIGHBORHOOD, ATTN_SHIFTED_WINDOW = 0, 1, 2, 3
 FAMILY_ITV2, FAMILY_ITV1 = 0, 1
 MAX_LEVELS = 8
-ABI_VERSION = 27
+ABI_VERSION = 28
 
 _vp, _i32, _i64, _f32, _f64, _u64, _sz = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double,
                                            ctypes.c_uint64, ctypes.c_size_t)
@@ -91,6 +91,7 @@ SIGNATURES = {
     "kdb_model_train_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
     "kdb_loss_noised_input": (_i32, [_vp, _vp, _vp, _f32, _vp, _i32, _i64, _vp]),
     "kdb_denoiser_loss": (_i32, [_i32, _vp, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _i32, _i64, _vp]),
+    "kdb_variance_loss": (_i32, [_vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp]),
     "kdb_model_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_model_tap_count": (_i64, [_vp]),
     "kdb_unet_create": (_i32, [ctypes.POINTER(KdbUNetConfig), ctypes.POINTER(_vp)]),
@@ -101,11 +102,13 @@ SIGNATURES = {
     "kdb_unet_conditioning": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "kdb_unet_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32, _i32]),
     "kdb_unet_forward": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _sz, _vp]),
+    "kdb_unet_forward_variance": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
     "kdb_unet_debug_tap": (_i32, [_vp, ctypes.c_char_p, _vp, _i64]),
     "kdb_unet_tap_count": (_i64, [_vp]),
     "kdb_unet_set_grad": (_i32, [_vp, ctypes.c_char_p, _vp, ctypes.POINTER(_i64), _i32]),
     "kdb_unet_train_workspace_bytes": (_i64, [_vp, _i32, _i32, _i32]),
     "kdb_unet_forward_train": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "kdb_unet_forward_train_variance": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _sz, _vp]),
     "kdb_unet_conv_wgrad": (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "kdb_unet_adagn_vjp": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
     "kdb_unet_flip_conv_weight": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
@@ -386,6 +389,7 @@ def external_scale_in(x, sigma, sigma_data=1.0):
 
 
 LOSS_DENOISER, LOSS_SIMPLE = 0, 1
+LOSS_VARIANCE = 2     # DenoiserWithVariance.loss: kdb_variance_loss on the model's F and logvar (no kdb_denoiser_loss kind)
 
 
 @_on_device_of_first
@@ -406,6 +410,18 @@ def denoiser_loss(x, noise, sigma, weight, sigma_data, f, kind):
     check(lib().kdb_denoiser_loss(kind, ptr(x), ptr(noise), ptr(sigma), ptr(weight), float(sigma_data), ptr(f), ptr(loss), ptr(cot),
                                   x.shape[0], x[0].numel(), stream()))
     return loss, cot
+
+
+@_on_device_of_first
+def variance_loss(x, noise, sigma, sigma_data, f, logvar):
+    """-> (loss [B], d loss[b] / d f, d loss[b] / d logvar[b]): kdb_variance_loss (layers.py:93-101)"""
+    require_cuda(x, noise, sigma, f, logvar)
+    B = x.shape[0]
+    loss, dlogvar = (torch.empty(B, device=x.device, dtype=torch.float32) for _ in range(2))
+    cot = torch.empty_like(f)
+    check(lib().kdb_variance_loss(ptr(x), ptr(noise), ptr(sigma), float(sigma_data), ptr(f), ptr(logvar), ptr(loss), ptr(cot), ptr(dlogvar), B,
+                                  x[0].numel(), stream()))
+    return loss, cot, dlogvar
 
 
 def _per_sample_stride(f, B):
@@ -832,6 +848,17 @@ class UNetEngine(Engine):
 
     forward_jvp = forward_vjp = unet_has_no_derivative
 
+    def forward_variance(self, x, sigma, cond, cond_batch_stride, sigma_data, precision):
+        """kdb_unet_forward_variance: forward()'s output, bit for bit, and the has_variance model's log-variance [B] -> (out, logvar)"""
+        B, C, H, W = x.shape
+        out = torch.empty_like(x)
+        logvar = torch.empty(B, device=x.device, dtype=torch.float32)
+        ws = self._workspace(precision, B, H, W, x.device)
+        with device_of(x):
+            check(lib().kdb_unet_forward_variance(self._h, precision, B, H, W, ptr(x), ptr(sigma), float(sigma_data), ptr(cond), cond_batch_stride,
+                                                  ptr(out), ptr(logvar), ptr(ws), ws.numel(), stream()))
+        return out, logvar
+
     def mapping_vjp(self, sigma, dcond, aug_cond=None, mapping_cond=None, out=None):
         """kdb_unet_mapping_vjp: the mapping network's backward for sigma [rows] and dcond [rows, mapping_out] (the gradient of its output)
         -> dict of h0, a0, dz0, dz1, dh0 [rows, mapping_out] and v [rows, mapping_cond_dim].  out: such a dict of buffers to write."""
@@ -851,20 +878,28 @@ class UNetEngine(Engine):
                                              *(ptr(res[k]) for k in ("h0", "a0", "dz0", "dz1", "dh0", "v")), stream()))
         return res
 
-    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32):
+    def forward_train(self, x, u, sigma, aug_cond, class_cond, mapping_cond, cond, grads, out=None, grad_x=None, precision=PREC_FP32,
+                      dlogvar=None):
         """Parameter gradients at fp32 (kdb_unet_forward_train), with Engine.forward_train's arguments: binds `grads`, then out = F(x) and
-        every bound gradient = u^T dF/dparam.  The U-Net takes no class_cond and gives no grad_x."""
+        every bound gradient = u^T dF/dparam, plus dlogvar^T dlogvar/dparam when `dlogvar` [B] (the cotangent of a has_variance model's
+        log-variance) is given (kdb_unet_forward_train_variance).  The U-Net takes no class_cond and gives no grad_x."""
         if class_cond is not None or grad_x is not None:
             raise ValueError("the image_v1 U-Net takes no class_cond and its training call gives no gradient with respect to x")
         B, C, H, W = x.shape
         if tuple(u.shape) != (B, C, H, W):
             raise ValueError(f"cotangent shape {tuple(u.shape)} != output shape {(B, C, H, W)}")
+        if dlogvar is not None and tuple(dlogvar.shape) != (B,):
+            raise ValueError(f"dlogvar shape {tuple(dlogvar.shape)} != ({B},)")
         out = torch.empty_like(x) if out is None else out
         self.set_grad(grads)
         ws = self._reserve(self.train_workspace(B, H, W), x.device)
+        args = (ptr(x), ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(cond), self._stride, ptr(u))
         with device_of(x):
-            check(lib().kdb_unet_forward_train(self._h, precision, B, H, W, ptr(x), ptr(sigma), ptr(aug_cond), ptr(mapping_cond), ptr(cond),
-                                               self._stride, ptr(u), ptr(out), ptr(ws), ws.numel(), stream()))
+            if dlogvar is None:
+                check(lib().kdb_unet_forward_train(self._h, precision, B, H, W, *args, ptr(out), ptr(ws), ws.numel(), stream()))
+            else:
+                check(lib().kdb_unet_forward_train_variance(self._h, precision, B, H, W, *args, ptr(f32c(dlogvar)), ptr(out), ptr(ws), ws.numel(),
+                                                            stream()))
         return out
 
     def train_forward(self, x, sigma, cond, cond_batch_stride, sigma_data, precision, out=None):
@@ -900,33 +935,41 @@ class NativeLossCall:
 
 class NativeLoss(torch.autograd.Function):
     """A training loss through a native engine with respect to the model's parameters (passed after `keys`, their state-dict names).
-    The forward saves the per-element cotangent d loss[b] / d F of the loss kernel; the backward scales it by the incoming gradient of
-    each sample's loss and makes one forward_train on the engine `engine()` returns (the model's, rebound to its current parameters), which
-    writes every parameter's gradient.  Both run at the model's training precision as the forward found it."""
+    The forward saves the per-element cotangent d loss[b] / d F of the loss kernel (and, for LOSS_VARIANCE, d loss[b] / d logvar[b]); the
+    backward scales it by the incoming gradient of each sample's loss and makes one forward_train on the engine `engine()` returns (the
+    model's, rebound to its current parameters), which writes every parameter's gradient.  Both run at the model's training precision as the
+    forward found it."""
 
     @staticmethod
     def forward(ctx, model, engine, ev, kind, noise, sigma_data, weight, keys, *params):
         x, sig = ev.x, ev.sigma
-        w = None if weight is None else f32c(weight).expand(x.shape[0]).contiguous()
         xin = loss_noised_input(x, noise, sig, sigma_data)
         cond = ev.conditioning()
         precision = getattr(model, "train_precision", PREC_FP32)
-        f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
-        loss, cot = denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
+        dlogvar = None
+        if kind == LOSS_VARIANCE:
+            f, logvar = ev.engine.forward_variance(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
+            loss, cot, dlogvar = variance_loss(x, noise, sig, sigma_data, f, logvar)
+        else:
+            w = None if weight is None else f32c(weight).expand(x.shape[0]).contiguous()
+            f = ev.engine.train_forward(xin, sig, cond, ev.engine.cond_stride, 0.0, precision)
+            loss, cot = denoiser_loss(x, noise, sig, w, sigma_data, f, kind)
         aug, cls, mc = ev.cond
         ctx.model, ctx.engine, ctx.keys, ctx.precision = model, engine, keys, precision
-        ctx.save_for_backward(xin, sig, cond, cot, None if aug is None else f32c(aug),
+        ctx.save_for_backward(xin, sig, cond, cot, dlogvar, None if aug is None else f32c(aug),
                               None if cls is None else cls.to(torch.int64).contiguous(), None if mc is None else f32c(mc))
         return loss
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        xin, sig, cond, cot, aug, cls, mc = ctx.saved_tensors
+        xin, sig, cond, cot, dlogvar, aug, cls, mc = ctx.saved_tensors
         params = dict(ctx.model.named_parameters())
-        u = cot * f32c(grad_loss).view(-1, *([1] * (cot.ndim - 1)))
+        g = f32c(grad_loss)
+        u = cot * g.view(-1, *([1] * (cot.ndim - 1)))
         grads = {k: torch.empty(params[k].shape, device=xin.device, dtype=torch.float32) for k in ctx.keys}
-        ctx.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads, precision=ctx.precision)
+        extra = {} if dlogvar is None else {"dlogvar": dlogvar * g}
+        ctx.engine().forward_train(xin, u, sig, aug, cls, mc, cond, grads, precision=ctx.precision, **extra)
         return (None,) * 8 + tuple(grads[k].to(params[k].dtype) for k in ctx.keys)
 
 

@@ -77,9 +77,10 @@ class KarrasAugmentWrapper(_native.NativeLossCall, nn.Module):
 
     def forward(self, input, sigma, aug_cond=None, mapping_cond=None, **kwargs):
         if self.is_unet():
+            return_variance = kwargs.pop("return_variance", False)
             if kwargs:
                 return self.inner_model.forward(input, sigma, **kwargs)      # raises for the unsupported options
-            return self.native_eval(input, sigma, aug_cond, mapping_cond=mapping_cond).forward(0.0)
+            return self.inner_model.evaluate(return_variance, input, sigma, aug_cond, mapping_cond=mapping_cond, augment=True)
         return self.inner_model(input, sigma, mapping_cond=self._mapping_cond(input, aug_cond, mapping_cond), **kwargs)
 
     @staticmethod

@@ -125,10 +125,26 @@ class Denoiser(nn.Module):
 
 class DenoiserWithVariance(Denoiser):
     """reference layers.py:93-101: differs from Denoiser in `loss` only, which needs the inner model's learned variance; sampling is
-    identical."""
+    identical.
 
-    def loss(self, input, noise, sigma, **kwargs):
-        raise NotImplementedError('DenoiserWithVariance.loss needs the inner model\'s return_variance output, which is not built')
+    `loss` (scales and weighting are accepted and ignored, as in the reference) runs natively around an image_v1 U-Net with has_variance,
+    bare, in KarrasAugmentWrapper or in DistributedDataParallel: one fp32 engine evaluation that also forms logvar, one loss kernel, and a
+    backward that writes every parameter's gradient, proj_out's variance row included.  The transformers and a U-Net without has_variance
+    raise NotImplementedError; any other inner model runs the reference formula under torch autograd, called with return_variance=True."""
+
+    _loss_kind = _native.LOSS_VARIANCE
+
+    def _check_loss(self):
+        pass
+
+    def _torch_loss(self, input, noise, sigma, **kwargs):
+        c_skip, c_out, c_in = [utils.append_dims(x, input.ndim) for x in self.get_scalings(sigma)]
+        noised_input = input + noise * utils.append_dims(sigma, input.ndim)
+        model_output, logvar = self.inner_model(noised_input * c_in, sigma, return_variance=True, **kwargs)
+        logvar = utils.append_dims(logvar, model_output.ndim)
+        target = (input - c_skip * noised_input) / c_out
+        losses = ((model_output - target) ** 2 / logvar.exp() + logvar) / 2
+        return losses.flatten(1).mean(1)
 
 
 class SimpleLossDenoiser(Denoiser):

@@ -237,6 +237,9 @@ class TransformerEngineModel(_native.NativeLossCall, _native.EngineCache, nn.Mod
         requiring grad.  The forward is one engine evaluation and one loss kernel; the backward is one kdb_model_forward_train.  The
         arithmetic is `set_train_precision`'s when the loss is computed (fp32 unless set), for its backward too, whatever `set_precision`
         selected."""
+        if kind == _native.LOSS_VARIANCE:
+            raise NotImplementedError(f"{self.kind}: DenoiserWithVariance.loss needs the inner model's return_variance output, which the "
+                                      "transformers do not have")
         if self.family != _native.FAMILY_ITV2:
             raise NotImplementedError(f"{self.kind}: parameter gradients are built for image_transformer_v2 models only")
         for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):

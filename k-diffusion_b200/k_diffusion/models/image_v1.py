@@ -3,7 +3,7 @@
 Constructor, forward signature and `state_dict()` layout follow the reference (k_diffusion/models/image_v1.py, layers.py:116-313),
 so reference checkpoints load unchanged; the forward pass itself is executed by libkdb200.so (kdb_unet_*).  The torch modules
 below only hold named parameters and buffers: none of their forward methods runs.  Parameter gradients (training) come from the engine's
-exact fp32 reverse walk through `Denoiser.loss`; `param_groups` returns the reference's optimizer groups.  Precision: fp32 (the default,
+exact fp32 reverse walk through `Denoiser.loss` (and, for a has_variance model, `DenoiserWithVariance.loss`); `param_groups` returns the reference's optimizer groups.  Precision: fp32 (the default,
 every kernel exact fp32) or, by set_precision("tf32") or KDB200_PRECISION=tf32, every convolution and the d_head-64 attention on the tensor cores with tf32
 operands and fp32 accumulation -- the arithmetic the reference's Conv2d gets on an H100 (cudnn.allow_tf32 defaults to True) -- or, by
 set_precision("fp16") or KDB200_PRECISION=fp16, the same with fp16 operands (same significand width, narrower exponent range).
@@ -193,8 +193,12 @@ class ImageDenoiserModelV1(_native.NativeLossCall, _native.EngineCache, nn.Modul
 
     def native_loss(self, kind, input, noise, sigma, sigma_data, weight, aug_cond=None, mapping_cond=None, augment=False):
         """Per-sample training losses [B] of the Karras-preconditioned denoiser around this U-Net (`_native.LOSS_DENOISER` or `LOSS_SIMPLE`,
-        as for image_transformer_v2), with a grad_fn that reaches every parameter requiring grad.  The forward is one fp32 engine evaluation
-        and one loss kernel; the backward is one kdb_unet_forward_train, exact fp32.  `augment`: the loss KarrasAugmentWrapper asks for."""
+        as for image_transformer_v2, or `LOSS_VARIANCE`, DenoiserWithVariance's, for a has_variance model), with a grad_fn that reaches every
+        parameter requiring grad.  The forward is one fp32 engine evaluation and one loss kernel; the backward is one kdb_unet_forward_train
+        (kdb_unet_forward_train_variance for LOSS_VARIANCE), exact fp32.  `augment`: the loss KarrasAugmentWrapper asks for."""
+        if kind == _native.LOSS_VARIANCE and not self.has_variance:
+            raise NotImplementedError("DenoiserWithVariance.loss needs the inner model's return_variance output: this U-Net has no variance "
+                                      "channel (has_variance is false)")
         for name, t in (("input", input), ("noise", noise), ("sigma", sigma)):
             if t.requires_grad:
                 raise RuntimeError(f"the native loss differentiates the model's parameters only, but {name} requires grad")
@@ -230,6 +234,17 @@ class ImageDenoiserModelV1(_native.NativeLossCall, _native.EngineCache, nn.Modul
         return _native.Evaluation(self.engine(augment), self.resolved_precision() if precision is None else precision, x, sigma, aug_cond,
                                   None, mapping_cond, False, True)
 
+    def evaluate(self, return_variance, *args, **kwargs):
+        """The raw model's output, at the model's precision in x's dtype, of the evaluation native_eval(*args, **kwargs) makes; with
+        return_variance (a has_variance model only) the pair (output, logvar [B]), image_v1.py:150-156."""
+        if return_variance and not self.has_variance:
+            raise NotImplementedError('return_variance needs a model with has_variance: without one the reference returns the output alone, '
+                                      'which the native engine does not mimic')
+        ev = self.native_eval(*args, **kwargs)
+        if not return_variance:
+            return ev.forward(0.0)
+        return ev.cast(ev.engine.forward_variance(ev.x, ev.sigma, ev.conditioning(), ev.engine.cond_stride, 0.0, ev.precision))
+
     def denoise(self, x, sigma, sigma_data, mapping_cond=None, out=None):
         """Fused Karras-preconditioned evaluation c_skip x + c_out F(c_in x, sigma) (layers.py:88-90)."""
         return self.native_eval(x, sigma, mapping_cond=mapping_cond).forward(float(sigma_data), out)
@@ -240,6 +255,4 @@ class ImageDenoiserModelV1(_native.NativeLossCall, _native.EngineCache, nn.Modul
         """reference image_v1.py:135-157"""
         if unet_cond is not None or cross_cond is not None:
             raise NotImplementedError('unet_cond and cross-attention conditioning are not supported by the native image_v1 engine')
-        if return_variance:
-            raise NotImplementedError('the variance output is a training quantity; the native engine returns the denoised channels only')
-        return self.native_eval(input, sigma, mapping_cond=mapping_cond).forward(0.0)
+        return self.evaluate(return_variance, input, sigma, mapping_cond=mapping_cond)

@@ -11,6 +11,8 @@ torch.backends.cuda.matmul.allow_tf32 = True (what the reference's train.py:101 
              (dropout off: the native path trains without dropout)
     mnist_unet    the reference's config_mnist image_v1 U-Net (28x28), B = 32, through KarrasAugmentWrapper (aug_cond zeros), dropout off
     cifar10_unet  the reference's config_cifar10 image_v1 U-Net (32x32), B = 128, the same
+    cifar10_unet_variance  that U-Net with has_variance: true, B = 128: a DenoiserWithVariance step (kdb_unet_forward_variance,
+             kdb_variance_loss, kdb_unet_forward_train_variance) against a Denoiser step on the same model, timed alternately
 
 The U-Net cases have three legs: the native exact fp32 path (one kdb_unet_forward and one kdb_unet_forward_train per step) and the
 oracle's torch eager autograd with TF32 off and with torch.backends.cuda.matmul.allow_tf32 and torch.backends.cudnn.allow_tf32 on; their
@@ -76,6 +78,9 @@ def main():
     args = ap.parse_args()
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     for name in args.cases.split(","):
+        if name == "cifar10_unet_variance":
+            print(json.dumps(variance_case(args, gpu)), flush=True)
+            continue
         if name in UNET_CASES:
             print(json.dumps(unet_case(name, args, gpu)), flush=True)
             continue
@@ -253,6 +258,38 @@ def unet_case(name, args, gpu):
                     break
         rec["native_fp32_kernel_share"] = {k: v / total for k, v in share.items()} if total else None
     return rec
+
+
+def variance_case(args, gpu):
+    """The learned-variance loss's cost: the same has_variance U-Net and AdamW step behind DenoiserWithVariance and behind Denoiser"""
+    cfg = json.loads((ROOT / "tests" / "golden" / "unet_configs.json").read_text())["cifar10"]["config"]
+    cfg["model"].update(dropout_rate=0.0, has_variance=True)
+    cfg = K.config.load_config(cfg)
+    m, B = cfg["model"], 128
+    model = K.config.make_model(cfg)
+    inner = model.inner_model
+    inner.load_state_dict(synth_sd({k: list(v.shape) for k, v in inner.state_dict().items()}, 3))
+    model = model.cuda().eval()
+    g = torch.Generator().manual_seed(0)
+    H, W = m["input_size"]
+    x = (torch.randn(B, m["input_channels"], H, W, generator=g) * 0.5).cuda()
+    noise = torch.randn(x.shape, generator=g).cuda()
+    sigma = torch.exp(torch.randn(B, generator=g) * 1.2 - 0.4).cuda()
+    opt = torch.optim.AdamW(inner.param_groups(1e-5), betas=(0.95, 0.999), eps=1e-6, weight_decay=1e-3)
+
+    def leg(den):
+        def step():
+            opt.zero_grad(set_to_none=True)
+            den.loss(x, noise, sigma).mean().backward()
+            opt.step()
+        return step
+
+    variance = K.config.make_denoiser_wrapper(cfg)(model)
+    assert type(variance) is K.layers.DenoiserWithVariance
+    legs = {"variance": leg(variance), "denoiser": leg(K.layers.Denoiser(model, m["sigma_data"], weighting=m["loss_weighting"]))}
+    ms = timed_legs(legs, args)
+    return dict(case="cifar10_unet_variance", batch=B, size=[H, W], **{f"{k}_ms": stats(sum(v, [])) for k, v in ms.items()},
+                round_medians={k: [stats(r)["median"] for r in v] for k, v in ms.items()}, gpu=gpu)
 
 
 if __name__ == "__main__":
